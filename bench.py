@@ -1,16 +1,22 @@
-"""bench.py -- MU iterations/sec of the dense NMF hot path on B200 (BASELINE.json metric).
+"""bench.py -- MU iterations/sec of the dense NMF hot path on H100 (BASELINE.json metric).
 
     python bench.py [--gpus N --steps K --warmup W] [--impl reference|reference-cuda]
                     [--config cfg2|cfg1|cfg3|cfg4s|cfg5] [--beta B] [--precision auto|f32|f16|f16_split]
+                    [--dump-outputs DIR]
 
 A "step" is one `fit(V, beta, tol=-inf, max_iter=ITERS)` pass (the reference's own benchmark protocol,
 examples/benchmarks/benchmark.ipynb cell 4: loss evaluations every 10 iterations included) on one
-synthetic batch: V = rand(N, C) rounded to bf16-representable values, W0/H0 = |randn| (SURVEY 8d).
+synthetic batch: V = rand(N, C) rounded to bf16-representable values, W0/H0 = |randn|.
 
   value : ITERS * K * n_gpus / t   with V, W, H resident in HBM (one shard per GPU)
   e2e   : the same through the public API with HOST (pinned) tensors: the module and V live on the CPU,
           `fit` stages V/W/H through the GPU and copies the factors back, all inside the timed region
-  roofline / cpu_baseline / gpu_reference : see DESIGN.md section "Measurement"
+  roofline / cpu_baseline / gpu_reference : the fused contraction against the HBM and tensor-core bounds; the
+          reference on the host cores and on the same GPU
+
+--dump-outputs DIR writes the factors the last timed step returned (W.npy, H.npy, float32; a fixed, seeded row sample of a
+factor when the two together would exceed 64 MB) so that two builds can be compared output for output: the inputs
+depend only on the arguments.
 
 Configs (BASELINE.json `configs`): cfg1 256x512 R=16 beta=2 | cfg2 65536x4096 R=64 KL (the metric's config, default) |
 cfg3 NMFD 1025x8192 R=16 T=128 KL | cfg4s one 131072x8192 R=128 row shard (1/8) of the 8192 x 2^20 problem |
@@ -56,29 +62,8 @@ def load_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return dict(hbm=d["hbm_gbs"], tc=d["bf16_tflops"], tc_sustained=d["bf16_tflops_sustained"], src="measured")
-    return dict(hbm=6650.0, tc=1590.0, tc_sustained=1400.0, src="fallback")
-
-
-def ncu_traffic(precision, cfg_name):
-    """(bytes, source file): dram read+write bytes per launch of the fused contraction kernel from the newest committed
-    `ncu --set full` capture of this precision at cfg2.  It is a replayed constant, not measured in this run."""
-    if cfg_name not in ("cfg2", "cfg5"):
-        return None, None
-    for rnd in ("r2", "r1"):
-        rel = os.path.join("profiles", f"{rnd}_ncu_tc_contract_{precision}.txt")
-        try:
-            tot, launches = 0.0, 0
-            for ln in open(os.path.join(ROOT, rel)):
-                ln = ln.strip()
-                if ln.startswith("dram__bytes_read.sum") or ln.startswith("dram__bytes_write.sum"):
-                    val, unit = ln.split("=")[1].split()[:2]
-                    tot += float(val) * {"Mbyte": 1e6, "Gbyte": 1e9, "Kbyte": 1e3, "byte": 1.0}[unit]
-                    launches += ln.startswith("dram__bytes_read.sum")
-            if tot:
-                return tot / max(launches, 1), rel      # the capture may hold the W and the H launch: per-launch mean
-        except Exception:
-            continue
-    return None, None
+    # NVIDIA H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense FP16 -- a bound, not a measured rate
+    return dict(hbm=3350.0, tc=989.0, tc_sustained=989.0, src="data-sheet")
 
 
 def make_inputs(N, C, R, seed, floor=0.0):
@@ -106,7 +91,7 @@ def v_floor(beta):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -175,7 +160,7 @@ class ClockSampler:
         top = sm[len(sm) // 2:] if sm else []        # samples under load = upper half
         med = top[len(top) // 2] if top else None
         watts.sort()
-        wtop = watts[len(watts) // 2:] if watts else []     # board power under load (DESIGN.md 4.1: the cfg2 line sits at the cap)
+        wtop = watts[len(watts) // 2:] if watts else []     # board power under load (the cfg2 line sits at the cap)
         return {"sm_mhz": med, "sm_max_mhz": smax, "reasons": sorted(reasons), "samples": len(sm), "window": self.window,
                 "board_power_w": wtop[len(wtop) // 2] if wtop else None}
 
@@ -220,8 +205,8 @@ def timed_steps(fn, steps, warmup, world):
 
 
 def reference_module():
-    """The unmodified reference (baseline/_ref, pip-installed from /root/reference) or None."""
-    ref = os.path.join(ROOT, "baseline", "_ref")
+    """The unmodified reference (oracle/_ref, installed by build() from a reference source tree) or None."""
+    ref = os.path.join(ROOT, "oracle", "_ref")
     if os.path.isdir(os.path.join(ref, "torchnmf")):
         if ref not in sys.path:
             sys.path.insert(0, ref)
@@ -232,7 +217,7 @@ def reference_module():
 
 def cpu_reference_rate(kind, V, W0, H0, beta, iters, warm=True):
     """it/s of the reference's CPU path: one discarded fit(max_iter=1), then fit(tol=-inf, max_iter=iters) timed
-    (BASELINE.md section 4) on all host cores.  Falls back to the oracle port when baseline/_ref is absent."""
+    (BASELINE.md section 4) on all host cores.  Falls back to the oracle port when oracle/_ref is absent."""
     torch.set_num_threads(os.cpu_count())
     try:
         torch.set_flush_denormal(True)       # README.md:101-102 of the reference
@@ -260,7 +245,7 @@ def cpu_reference_rate(kind, V, W0, H0, beta, iters, warm=True):
 
 
 def gpu_reference_rate(kind, V_dev, W0, H0, beta, iters):
-    """it/s of the UNMODIFIED reference moved to the same B200 with .cuda() (cuBLAS + unfused ATen ops, fp32, the two
+    """it/s of the UNMODIFIED reference moved to the same GPU with .cuda() (cuBLAS + unfused ATen ops, fp32, the two
     autograd backward passes of nmf.py:52-92): the "library path on the same box" line (BASELINE.md section 4)."""
     rn = reference_module()
     if rn is None:
@@ -293,7 +278,7 @@ def config_inputs(cfg_name, beta, seed):
 
 
 def run_reference_arm(a, cfg_name, beta):
-    """`--impl reference`: the reference's own CPU implementation (baseline/_ref) on this box's host cores, rank 0 only.
+    """`--impl reference`: the reference's own CPU implementation (oracle/_ref) on this box's host cores, rank 0 only.
     Same protocol as the `cpu_baseline` of the main arm: a discarded 1-iteration fit, then K x fit(max_iter=ref_iters)."""
     kind, shape, _, desc = CONFIGS[cfg_name]
     if int(os.environ.get("RANK", "0")) != 0:
@@ -336,7 +321,7 @@ def run_reference_cuda_arm(a, cfg_name, beta):
         res = gpu_reference_rate(kind, V_dev, W0, H0, beta, a.iters)
     dt = time.perf_counter() - t0
     if not res or res.get("value") is None:
-        emit({"impl": "reference-cuda", "unavailable": (res or {}).get("unavailable", "baseline/_ref not installed")})
+        emit({"impl": "reference-cuda", "unavailable": (res or {}).get("unavailable", "oracle/_ref not installed")})
         return
     emit({"impl": "reference-cuda", "metric": "MU iterations/sec", "value": res["value"], "unit": "iter/s", "n_gpus": 1,
           "steps": a.steps, "warmup": 1, "ms_per_step": 1e3 * dt / a.steps, "higher_is_better": True, "scaling": "weak",
@@ -352,7 +337,7 @@ def workload_config(cfg_name, beta, world, iters, precision):
     if kind == "nmf":
         N, C, R = shape
         c.update({"N_per_gpu": N, "C": C, "R": R,
-                  "l2": "inputs larger than L2 (V shard >= 512 MiB)" if N * C * 2 > 126e6 else "inputs fit in L2"})
+                  "l2": "inputs larger than L2 (V shard >= 512 MiB)" if N * C * 2 > 50e6 else "inputs fit in L2"})
     else:
         B, C, L, R, T = shape
         c.update({"B": B, "C": C, "L": L, "R": R, "T": T,
@@ -381,7 +366,7 @@ def emit(line):
 
 
 def flops_per_iter(kind, shape, beta):
-    """Algorithmic FLOPs of one MU iteration of the algorithm actually run (SURVEY 8d)."""
+    """Algorithmic FLOPs of one MU iteration of the algorithm actually run."""
     if kind == "nmfd":
         B, C, L, R, T = shape
         return 4 * 2.0 * B * C * R * T * (L - T + 1) * (1.0 if beta == 1 else 1.5)
@@ -456,6 +441,22 @@ def cfg4_shard_rate(dev, rank, world, group, precision, iters=40):
     return out
 
 
+def dump_outputs(out_dir, arrays, budget=64 << 20):
+    """Save each array as out_dir/<name>.npy (float32).  When they exceed `budget` bytes together, every array is cut to
+    the same fixed, seeded sample of its leading-axis rows (sorted), so the files stay comparable between runs."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    host = {k: v.detach().float().cpu() for k, v in arrays.items()}
+    total = sum(t.numel() * 4 for t in host.values())
+    for name, t in host.items():
+        if total > budget and t.shape[0] > 1:
+            keep = max(1, int(t.shape[0] * budget / total))
+            g = torch.Generator().manual_seed(0)
+            idx = torch.randperm(t.shape[0], generator=g)[:keep].sort().values
+            t = t[idx]
+        np.save(os.path.join(out_dir, f"{name}.npy"), t.numpy().astype(np.float32))
+
+
 def main():
     _capture_stdout()
     ap = argparse.ArgumentParser()
@@ -472,6 +473,8 @@ def main():
     ap.add_argument("--no-gpu-reference", action="store_true")
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-extras", action="store_true", help="skip north_star_cfg4 / sharded_check")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the factors of the last timed step as DIR/<name>.npy")
     a = ap.parse_args()
     kind, shape, beta, desc = CONFIGS[a.config]
     if beta is None:
@@ -498,7 +501,7 @@ def main():
     peaks = load_peaks()
     group = dist.group.WORLD if world > 1 else None
     if kind == "nmfd" and world > 1:
-        group = None                     # NMFD: replicas only (DESIGN.md section 7)
+        group = None                     # NMFD: replicas only
 
     # ---------------- inputs: one full shard per rank (weak scaling) -----------------------------------
     V_cpu, W0, H0 = config_inputs(a.config, beta, 2 * rank)
@@ -535,6 +538,8 @@ def main():
     clocks = sampler.stop() if sampler else None
     precision = model.last_fit_precision
     value = a.iters * a.steps * world / (ms * 1e-3)
+    if a.dump_outputs and rank == 0:
+        dump_outputs(a.dump_outputs, {"W": model.W.data, "H": model.H.data})
 
     # ---------------- end to end through the public API with host buffers ------------------------------
     e2e = None
@@ -598,16 +603,15 @@ def main():
         ach_gb = v_bytes / t_dom / 1e9
         tensor = {"achieved": ach_tf, "peak": peaks["tc"], "unit": "TFLOP/s", "frac": ach_tf / peaks["tc"],
                   "algorithmic_flops_per_launch": flops_launch,
-                  "peak_source": f"{peaks['src']} MEASURED_PEAKS.json bf16 burst (f16 has the same tensor peak)"}
+                  "peak_source": f"{peaks['src']} bf16 (f16 has the same tensor peak)"}
         hbm = {"achieved": ach_gb, "peak": peaks["hbm"], "unit": "GB/s", "frac": ach_gb / peaks["hbm"],
                "algorithmic_bytes_per_launch": v_bytes,
-               "peak_source": f"{peaks['src']} MEASURED_PEAKS.json copy bandwidth (burst)"}
+               "peak_source": f"{peaks['src']} HBM bandwidth"}
         # the binding roofline is the one whose minimum time for this launch is larger (cfg2, R=64: HBM 82 us vs tensor
         # 41 us; at R=128 the two meet); the other one is reported next to it
         hbm_bound = v_bytes / (peaks["hbm"] * 1e9) >= flops_launch / (peaks["tc"] * 1e12) or precision == "f32"
-        traffic, traffic_src = ncu_traffic(precision, a.config)
         roof = dict(hbm if hbm_bound else tensor)
-        roof.update({"bound": "hbm" if hbm_bound else "tensor", "traffic": traffic, "traffic_source": traffic_src,
+        roof.update({"bound": "hbm" if hbm_bound else "tensor", "traffic": None, "traffic_source": None,
                      "kernel": f"fused {which_dom}-update contraction ({precision})", "kernel_ms": t_dom * 1e3,
                      "kernel_ms_w": times["w"] * 1e3, "kernel_ms_h": times["h"] * 1e3,
                      "tensor" if hbm_bound else "hbm": tensor if hbm_bound else hbm,
@@ -619,7 +623,7 @@ def main():
                 "frac": step_tf / peaks["tc_sustained"], "traffic": None, "traffic_source": None,
                 "kernel": "NMFD iteration (recon x2, wgrad, dgrad): step-level figure, the target is L2-resident",
                 "algorithmic_flops_per_iteration": fl_iter,
-                "peak_source": f"{peaks['src']} MEASURED_PEAKS.json bf16 sustained"}
+                "peak_source": f"{peaks['src']} bf16 sustained"}
 
     # ---------------- same-box baselines (rank 0, N=1 only) ------------------------------------------------------
     cpu = gpu_ref = None

@@ -1,5 +1,5 @@
 /*
- * nmf_b200.h -- C ABI of the B200-native multiplicative-update NMF engine (libnmf_b200.so).
+ * nmf_b200.h -- C ABI of the H100-native multiplicative-update NMF engine (libnmf_b200.so).
  *
  * This is the drop-in boundary for ONE hot path of yoyololicon/pytorch-NMF (torchnmf 0.3.5):
  * the body of BaseComponent.fit()'s iteration loop for dense targets
@@ -8,7 +8,7 @@
  *
  * i.e. reconstruct (nmf.py:691-693 NMF, :776-779 NMFD) + _double_backward_update (nmf.py:52-92)
  * + the KL denominators (nmf.py:122-131) + metrics.beta_div (metrics.py:60-96).  The reference has
- * no FFI: its seam is Python (SURVEY.md 8b).  The binding a maintainer adds on the reference side is
+ * no FFI: its seam is Python.  The binding a maintainer adds on the reference side is
  * the ctypes stub shown in INTEGRATION.md; the Python host side shipped here
  * (pytorch-nmf_b200/torchnmf_b200) is that stub plus the unchanged NMF/NMFD module surface.
  *
@@ -39,8 +39,8 @@ extern "C" {
 enum {
   NMFB200_PREC_AUTO      = -1, /* f16 tensor-core path when the rank allows it (R <= 128), else f32 */
   NMFB200_PREC_F32       = 0,  /* fused CUDA-core kernels, fp32 operands and accumulators (exact) */
-  NMFB200_PREC_F16       = 1,  /* tcgen05, fp16 operands, fp32 accumulate                         */
-  NMFB200_PREC_F16_SPLIT = 2   /* tcgen05, fp16 hi/lo split factors (~22-bit), fp16 ratio tile    */
+  NMFB200_PREC_F16       = 1,  /* wgmma, fp16 operands, fp32 accumulate                           */
+  NMFB200_PREC_F16_SPLIT = 2   /* wgmma, fp16 hi/lo split factors (~22-bit), fp16 ratio tile      */
 };
 
 /* error codes */
@@ -55,7 +55,7 @@ typedef struct nmfb200_ctx nmfb200_ctx;
 
 int         nmfb200_abi_version(void);
 const char* nmfb200_last_error(void);
-/* "src=<sha256/16 of csrc/* + this header> nvcc=<version> arch=sm_100a built=<date time>": which sources this binary is */
+/* "src=<sha256/16 of csrc/* + this header> nvcc=<version> arch=sm_90a built=<date time>": which sources this binary is */
 const char* nmfb200_build_info(void);
 /* number of kernels this library has launched in this process (bench.py's gpu_launches) */
 int64_t     nmfb200_launch_count(void);
@@ -115,7 +115,7 @@ int nmfb200_nmf_loss(nmfb200_ctx* ctx, const float* W, const float* H, double be
 int nmfb200_nmf_loss_prefetch_w(nmfb200_ctx* ctx, const float* W, const float* H, double beta,
                                 double* loss_dev, void* stream);
 
-/* Row-sharded W update (SURVEY.md 8e).  `partial` is a device fp32 buffer of
+/* Row-sharded W update.  `partial` is a device fp32 buffer of
  * nmfb200_nmf_w_partial_numel() elements receiving this shard's raw numerator (C*R), then either
  * colsum(H_local) (R, beta == 1) or the raw denominator (C*R).  The caller sum-all-reduces it and
  * passes the reduced buffer to _w_apply, which performs nmf.py:78-92 on every rank identically. */

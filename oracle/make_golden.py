@@ -1,13 +1,13 @@
 """Generate tests/golden/*.npz by running the REAL reference (torchnmf 0.3.5).
 
 TEST INFRASTRUCTURE ONLY (see oracle/mu_oracle.py header).  Run in the build container, where
-the reference is importable from /root/reference (read-only) or baseline/_ref:
+the reference is importable from oracle/_ref (oracle/build_ref.py):
 
     python oracle/make_golden.py            # small cases (seconds)
     python oracle/make_golden.py --cfg2     # + the 200-iteration 65536x4096 R=64 KL run (~10 min CPU)
 
-The GPU box has no reference; the fixtures written here are what travels.  Inputs are generated
-from fixed torch CPU seeds (SURVEY 8d): V = rand(N,C) rounded to bf16-representable values, so the
+The GPU tests do not import the reference; the fixtures written here are what they compare against.  Inputs are generated
+from fixed torch CPU seeds: V = rand(N,C) rounded to bf16-representable values, so the
 fp32 reference and the 16-bit-operand engine consume bit-identical data; W0/H0 = |randn|.
 """
 import argparse
@@ -20,7 +20,7 @@ import numpy as np
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-for cand in (os.path.join(ROOT, "baseline", "_ref"), "/root/reference"):
+for cand in (os.path.join(ROOT, "oracle", "_ref"),):
     if os.path.isdir(os.path.join(cand, "torchnmf")):
         sys.path.insert(0, cand)
         break
@@ -123,7 +123,7 @@ def save_cases(cases, fname):
 def cfg2_case(iters=200):
     """BASELINE.json configs[1]: V (65536, 4096), R = 64, beta = 1, 200 iterations from seeds 0/1.
     Only subsampled factor rows are stored (W rows ::8, H rows ::128); inputs are regenerated from
-    the seeds on the GPU box and verified against the float64 checksums stored here."""
+    the seeds on the GPU machine and verified against the float64 checksums stored here."""
     torch.set_num_threads(os.cpu_count())
     torch.set_flush_denormal(True)     # README.md:101-102
     N, C, R = 65536, 4096, 64

@@ -16,7 +16,7 @@ F.linear/F.conv1d) of the reference's autograd-derived update, written from the 
     torchnmf/constants.py:3  eps = float32 machine epsilon
 
 Parity status: PINNED.  ``oracle/make_golden.py`` runs the real reference (imported from
-/root/reference in the build container) from identical initial factors and stores its outputs
+oracle/_ref) from identical initial factors and stores its outputs
 under ``tests/golden/``; ``tests/test_oracle.py`` checks this restatement against those vectors
 (bit-exact for alpha == 0 on the build container's torch, <= 2e-6 relative otherwise).
 
@@ -105,7 +105,7 @@ def nmf_reconstruct(H, W):
 
 def nmf_w_contractions(V, W, H, beta):
     """Raw numerator / denominator of the W update before relu/eps/l1/l2 (linear in the rows of
-    V and H, so row shards can be summed -- SURVEY 8e).  Returns (num (C,R), den (C,R) or colsum(H) (1,R))."""
+    V and H, so row shards can be summed).  Returns (num (C,R), den (C,R) or colsum(H) (1,R))."""
     Pn, Pp = phi(V, nmf_reconstruct(H, W), beta)
     num = Pn.t() @ H
     den = H.sum(0, keepdim=True) if beta == 1 else Pp.t() @ H    # nmf.py:122-125

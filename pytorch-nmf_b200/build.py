@@ -1,8 +1,8 @@
-"""Build libnmf_b200.so (the C-ABI CUDA library) in-tree with nvcc for sm_100a.
+"""Build libnmf_b200.so (the C-ABI CUDA library) in-tree with nvcc for sm_90a.
 
     python pytorch-nmf_b200/build.py [--force] [--verbose]
 
-The output (pytorch-nmf_b200/lib/libnmf_b200.so) is git-ignored but travels to the GPU box.
+The output (pytorch-nmf_b200/lib/libnmf_b200.so) is git-ignored; build() rebuilds it when a source is newer.
 """
 import os
 import shutil
@@ -15,14 +15,9 @@ LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libnmf_b200.so")
 SOURCES = ["capi.cu", "simt_nmf.cu", "update.cu", "nmfd.cu", "tc_nmf.cu", "tc_nmfd.cu", "sparse_nmf.cu", "project.cu"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr",
 ]
-if os.environ.get("NMFB200_BUILD_TRACE"):       # tuning build (tools/tc_trace.py, tc_knock.py): separate library, loaded
-    NVCC_FLAGS += ["-DNMFB200_TRACE"]           # with NMFB200_LIB=<...>/lib/trace/libnmf_b200.so
-    LIBDIR = os.path.join(LIBDIR, "trace")
-    LIB = os.path.join(LIBDIR, "libnmf_b200.so")
-
 
 def _nvcc():
     for cand in (os.environ.get("NVCC"), shutil.which("nvcc"), "/usr/local/cuda/bin/nvcc"):
@@ -33,7 +28,7 @@ def _nvcc():
 
 def source_hash():
     """sha256 over every file the library is compiled from (csrc/*, include/nmf_b200.h), first 16 hex digits.  Compiled
-    into the library (nmfb200_build_info) so a test can prove the .so on the GPU box was built from these sources."""
+    into the library (nmfb200_build_info) so a test can prove the .so that runs was built from these sources."""
     import hashlib
     h = hashlib.sha256()
     files = sorted(os.path.join(CSRC, f) for f in os.listdir(CSRC)) + [os.path.join(HERE, "..", "include", "nmf_b200.h")]
@@ -53,7 +48,7 @@ def _stale():
 
 
 def build(force=False, verbose=False):
-    """Compile every CUDA source for sm_100a into one shared library.  Returns the library path."""
+    """Compile every CUDA source for sm_90a into one shared library.  Returns the library path."""
     if not force and not _stale():
         return LIB
     os.makedirs(LIBDIR, exist_ok=True)

@@ -1,4 +1,4 @@
-// Shared declarations for the libnmf_b200 kernels (sm_100a only).
+// Shared declarations for the libnmf_b200 kernels (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>

@@ -397,7 +397,7 @@ int nmfd_recon_phi(const NmfdShape& s, const float* V, const float* W, const flo
 int nmfd_wgrad_nsplit(const NmfdShape& s) {
   const WgradPlan p = wgrad_plan(s);
   const int64_t tiles = (int64_t)p.ntt * p.nrg * p.nog * ceil_div(s.C, p.mt);
-  int64_t ns = ceil_div(148 * 4, tiles);
+  int64_t ns = ceil_div(132 * 4, tiles);
   const int64_t nlines = (int64_t)s.B * s.J1() * s.J2();
   if (ns > nlines) ns = nlines;
   if (ns > 64) ns = 64;
@@ -424,7 +424,7 @@ int nmfd_wgrad(const NmfdShape& s, const float* G, const float* H, float* out, i
 int nmfd_dgrad_nsplit(const NmfdShape& s) {
   const dim3 g = slide_grid(s, false, row_tile(s.R), s.R, 1);
   const int64_t tiles = (int64_t)g.x * g.y * g.z;
-  int64_t ns = ceil_div(148 * 4, tiles);
+  int64_t ns = ceil_div(132 * 4, tiles);
   if (ns > s.C) ns = s.C;
   if (ns > 64) ns = 64;
   if (ns < 1) ns = 1;

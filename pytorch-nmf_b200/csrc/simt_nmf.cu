@@ -295,7 +295,7 @@ __global__ void __launch_bounds__(256) sum_partials_kernel(const double* __restr
 
 int loss_chunks(int64_t Mr, int64_t Nc) {
   int64_t rb = ceil_div(Mr, kTile), tiles = ceil_div(Nc, kTile);
-  int64_t want = ceil_div(148 * 4, rb);
+  int64_t want = ceil_div(132 * 4, rb);      // a few waves over the 132 SMs of an H100
   if (want < 1) want = 1;
   if (want > tiles) want = tiles;
   return (int)want;

@@ -1,24 +1,19 @@
-// Tensor-core path of the dense NMF factor update for sm_100a: tcgen05.mma + TMEM + TMA.
+// Tensor-core path of the dense NMF factor update for sm_90a: wgmma + TMA + mbarrier.
 //
-// One persistent, warp-specialised CTA per SM walks work items (128-row block of the row factor F,
-// chunk of 128-column tiles).  Per tile (FlashAttention-shaped, but with a ratio instead of softmax):
+// One persistent CTA per SM walks work items (128-row block of the row factor F, chunk of TN-column tiles of V).  Warpgroup 0
+// is the TMA producer (one thread): per item the F block, per tile the G tile [TN c][KW] and the V tile [128 m][TN c]
+// (fp16, SWIZZLE_128B) into a ring of NS stages.  Warpgroups 1 and 2 each own 64 rows of the item and, per 64-column step
+// of a tile (FlashAttention-shaped, with a ratio instead of softmax):
 //
-//   TMA      G tile [128 c][KW] and V tile [128 m][128 c] (fp16, SWIZZLE_128B) -> shared memory
-//   MMA-1    S[128 m][128 c]  = F_blk G_tile^T            tcgen05.mma SS, fp32 accumulators in TMEM
-//   ratio    P = V * rcp(S*c1 + c2)  (== V / (F G^T + eps), nmf.py:65); the CENTRED tile P - kappa -> fp16, written
-//            back to TMEM over S columns the writer has already read (256 threads per tile: two warpgroups, each all 128
-//            TMEM lanes x half the columns)
-//   MMA-2    O[128 m][KW]   += (P - kappa) G_tile          tcgen05.mma TS (A from TMEM, B = G tile MN-major)
-//            (numerator = O + kappa colsum(G), added in fp32 by the ratio stage)
+//   S[64 m][64 c]  = F_rows G_step^T            wgmma SS, fp32 accumulators in registers
+//   ratio          P = V * rcp(S*c1 + c2)  (== V / (F G^T + eps), nmf.py:65); the CENTRED tile P - kappa -> fp16, packed
+//                  straight into the A-operand fragment of the next wgmma (the accumulator and A layouts coincide)
+//   O[64 m][RP]   += (P - kappa) G_step         wgmma RS (A from registers, B = G tile MN-major)
+//                  (numerator = O + kappa colsum(G), added in fp32 by the ratio stage)
 //
 // so neither S = WH nor P = V/(WH) ever leaves the SM (nmf.py:376-378 materialises both in HBM).
 // F/G are fp16 copies of the factors scaled by a power of two; in split mode they carry hi|lo halves
-// (KW = 2*Rp) and S = Fhi Ghi + Flo Ghi + Fhi Glo, O = P [Ghi|Glo] recovers ~22-bit factors.
-//
-// Warp roles (512 threads): 0-3, 4-7 ratio warpgroups (left / right half of the tile's columns) | 8-11 epilogue (O -> fp32
-// partial numerators) | 12 TMA producer for V (the HBM stream, own ring) | 13 MMA issuer for S (one lane) | 14 TMA producer
-// for F/G (L2-resident factors) | 15 MMA issuer for O.  The control warps have the highest ids = highest issue priority.
-// S runs up to NS tiles ahead of O in the tensor pipe, across work-item boundaries.
+// (KW = 2*Rp) and S = Fhi Ghi + Flo Ghi + Fhi Glo, O = P Ghi + P Glo recovers ~22-bit factors.
 #include "tc_nmf.cuh"
 
 #include <cooperative_groups.h>
@@ -30,32 +25,22 @@
 #include <string>
 #include <vector>
 
-#include "sm100_ptx.cuh"
+#include "sm90_ptx.cuh"
 
 namespace nmfb200 {
 
 namespace {
 
-constexpr int kTileM = 128;          // rows of the row factor per work item (= TMEM lanes)
-constexpr uint32_t kTmemCols = 512;
-constexpr uint32_t kColS = 0;        // S/P stages: columns [TN i, TN i + TN); O accumulator follows at NS * TN
+constexpr int kTileM = 128;          // rows of the row factor per work item (two consumer warpgroups of 64 rows)
+constexpr int kStep = 64;            // columns of a tile per S / ratio / O step
+constexpr int kThreads = 384;        // warpgroup 0: TMA producer | warpgroups 1, 2: MMA + ratio stage
 
 // Compile-time configuration of the fused kernel.
 //   RP    padded rank (64 or 128);  SPLIT  hi|lo fp16 factors (KW = 2 RP operand columns)
-//   TN    tile width in columns of V (64 or 128): narrower tiles = deeper rings in the same shared memory
-//   NF / NG / NV  F blocks, G-tile ring, V-tile ring;  NS  S/P accumulator stages in TMEM (the S-MMA warp runs up to
-//   NS tiles ahead of the O-MMA warp)
-//   NRW   ratio warpgroups (each processes TN / NRW columns of every tile)
-//   NP    0: the ratio tile P is written over the S columns of its stage (the stage is free again when the O-MMA has
-//         consumed P).  > 0: P has NP buffers of TN / 2 columns of its own: an S stage is handed back as soon as the
-//         ratio warps have READ it, a P buffer when its O-MMA has completed -- two short rings instead of one long one.
-constexpr unsigned kEpiPaceNs = 100;     // pause between the epilogue's row stores (see the epilogue warpgroup)
-
-template <int RP_, bool SPLIT_, int TN_, int NF_, int NG_, int NV_, int NS_, int NRW_ = 2, int NP_ = 0>
+//   TN    tile width in columns of V (64 or 128)
+template <int RP_, bool SPLIT_, int TN_>
 struct Cfg {
-  static constexpr int RP = RP_, TN = TN_, NF = NF_, NG = NG_, NV = NV_, NS = NS_, NRW = NRW_, NP = NP_;
-  // 4 NRW ratio warps, then 4 epilogue warps, then 4 control warps (TMA V / MMA S / TMA F,G / MMA O)
-  static constexpr int kThreads = 128 + 128 * NRW_ + 128;
+  static constexpr int RP = RP_, TN = TN_;
   static constexpr bool SPLIT = SPLIT_;
   static constexpr int KW = RP_ * (SPLIT_ ? 2 : 1);
 };
@@ -73,38 +58,23 @@ struct TcKernelParams {
   int ef, eg;                 // which of exps[] belong to F and G
   double* loss_part;          // LOSS mode: [gridDim.x][2] = {sum v~ lg2(x), sum S~}
   const float* kappa;         // device scalar: centring constant of the ratio tile (typical P), 0 = off
-  int pf_dist;                // L2 prefetch distance of the V stream in tiles (0 = off)
-  long long* trace;           // tuning aid: per-tile event timestamps of CTA 0 ([tile][16]), or nullptr
-  int knock;                  // tuning build only (NMFB200_TC_KNOCK): bit mask of pipeline stages to skip
 };
 
-// Event timeline of CTA 0 (tools/tc_trace.py): compiled in only with -DNMFB200_TRACE (build.py: NMFB200_BUILD_TRACE=1);
-// the product build carries no trace code in the warp-specialised loops.
-#ifdef NMFB200_TRACE
-#define TC_TRACE(tile, k)                                                        \
-  do {                                                                         \
-    if (p.trace && blockIdx.x == 0 && (tile) < 256) p.trace[(tile) * 16 + (k)] = clock64(); \
-  } while (0)
-#define TC_KNOCK(bit) ((p.knock & (bit)) != 0)      // knock-out experiments (results invalid): which stage bounds the kernel?
-#else
-#define TC_TRACE(tile, k) do { } while (0)
-#define TC_KNOCK(bit) false
-#endif
-
-// shared memory: NF F blocks | NG G-tile ring | NV V-tile ring | mbarriers | tmem ptr | loss slots
-template <int KW, int TN, int NF, int NG, int NV, int NS, int NP = 0>
+// shared memory: F block | NS stages of (G tile, V tile) | mbarriers | loss slots.  As many stages as fit in the 227 KB
+// a block may opt into: the V stream is the HBM-bound one and wants as many tiles in flight as possible.
+template <int KW, int TN>
 struct SmemLayout {
   static constexpr int kFBytes = kTileM * KW * 2;
   static constexpr int kGBytes = TN * KW * 2;
   static constexpr int kVBytes = kTileM * TN * 2;
+  static constexpr int kStageBytes = kGBytes + kVBytes;
+  static constexpr int NS = (232448 - 1024 - 256 - kFBytes) / kStageBytes;
   static constexpr int kF = 0;
-  static constexpr int kG = kF + NF * kFBytes;
-  static constexpr int kV = kG + NG * kGBytes;
-  static constexpr int kBar = kV + NV * kVBytes;
-  static constexpr int kNumBars = 2 * NF + 2 * NG + 2 * NV + 2 * NS + 2 * (NP ? NP : NS) + 2;
-  static constexpr int kTmemPtr = kBar + 8 * kNumBars;
-  static constexpr int kLossSlots = kTmemPtr + 16;
-  static constexpr int kTotal = kLossSlots + 16 * 16;
+  static constexpr int kStage0 = kFBytes;
+  static constexpr int kBar = kStage0 + NS * kStageBytes;
+  static constexpr int kNumBars = 2 + 2 * NS;
+  static constexpr int kLossSlots = kBar + 8 * kNumBars;
+  static constexpr int kTotal = kLossSlots + 8 * 16;
 };
 
 // BM selects the phi stage (nmf.py:61-74): 0 = beta 1 (one centred ratio tile, one accumulator); otherwise two tiles
@@ -119,34 +89,17 @@ enum : int { kBmKL = 0, kBmIS = 1, kBm05 = 2, kBm15 = 3, kBmGen = 4, kBmEU = 5 }
 // tile it forms anyway (metrics.py:22 needs sum V lg(WH + eps) and sum WH at exactly the factors the next W update starts
 // from), so the loss evaluation of every 10th iteration costs one lg2 per element instead of a pass over V of its own.
 template <class C, int BM, bool LOSS, bool FOLD = false>
-__global__ void __launch_bounds__(C::kThreads, 1)
+__global__ void __launch_bounds__(kThreads, 1)
 tc_contract_kernel(const __grid_constant__ CUtensorMap tmF, const __grid_constant__ CUtensorMap tmG,
                    const __grid_constant__ CUtensorMap tmV, const TcKernelParams p) {
-  constexpr int RP = C::RP, KW = C::KW, TN = C::TN, NF = C::NF, NG = C::NG, NV = C::NV, NS = C::NS;
+  constexpr int RP = C::RP, KW = C::KW, TN = C::TN;
   constexpr bool SPLIT = C::SPLIT;
-  constexpr int NRW = C::NRW;
-  // Warp roles by warp id.  The warp scheduler of an SM sub-partition prefers the HIGHEST warp id among its eligible warps
-  // (B300_MICROARCH.md, "arbiter priority: hi-wid-first"), and the TMA producers / MMA issuers are short serial
-  // instruction streams on the critical path of every tile hand-off: they get the top four ids (one per sub-partition),
-  // the throughput-bound ratio warps the lowest.  (Round 1 had them at ids 0-3: a wake-up of an issuing warp took 500-900
-  // cycles while the ratio warps of its sub-partition were busy, profiles/r2_trace_*.txt.)
-  constexpr int kEpiWarp0 = 4 * NRW;              // first epilogue warp (ratio warps are 0 .. 4 NRW - 1)
-  constexpr int kCtl0 = 4 * NRW + 4;              // control warps: +0 TMA (V) | +1 MMA issuer S | +2 TMA (F, G) | +3 MMA issuer O
   constexpr bool TWO = BM != kBmKL && BM != kBmEU && !LOSS;     // LOSS kernels only need S, whatever the beta
   constexpr bool EU = BM == kBmEU;
-  // TMEM columns.  one-output: S/P stages [0, NS TN) | O [NS TN, NS TN + KW).
-  //               two-output: S/Pn stages [0, 256) | Pp stages [256, 384) | O_num [384, 448) | O_den [448, 512)
-  constexpr int NP = C::NP;
-  constexpr bool PSEP = NP > 0;                   // P in buffers of its own (one-output update kernels only)
-  constexpr int NPB = PSEP ? NP : NS;             // P-full / P-empty barriers
-  constexpr uint32_t kColPp = NS * TN;
-  constexpr uint32_t kColP = NS * TN;             // PSEP: P buffer b = columns [kColP + b TN/2, + TN/2)
-  constexpr uint32_t kColO = TWO ? 384 : (PSEP ? NS * TN + NP * (TN / 2) : NS * TN);
-  constexpr uint32_t kColO2 = 448;
-  using L = SmemLayout<KW, TN, NF, NG, NV, NS, NP>;
-  static_assert(TWO || (int)kColO + KW <= (int)kTmemCols, "TMEM budget");
-  static_assert(!PSEP || (!TWO && !LOSS) || LOSS, "separate P buffers: one-output kernels");
-  static_assert(!TWO || (!SPLIT && RP == 64 && TN == 128 && NS == 2), "two-output kernels: fast mode, R <= 64");
+  using L = SmemLayout<KW, TN>;
+  constexpr int NS = L::NS;
+  static_assert(NS >= 2, "shared memory: at least two stages");
+  static_assert(!TWO || (!SPLIT && RP == 64), "two-output kernels: fast mode, R <= 64");
   static_assert(TN == 64 || TN == 128, "tile width");
   static_assert(RP == 64 || RP == 128, "padded rank");
   static_assert(!FOLD || (!LOSS && BM == kBmKL), "loss folded into the update kernel: beta 1 only");
@@ -154,519 +107,152 @@ tc_contract_kernel(const __grid_constant__ CUtensorMap tmF, const __grid_constan
   const uint32_t raw32 = ptx::smem_u32(smem_raw);
   const uint32_t sbase = (raw32 + 1023u) & ~1023u;
   uint8_t* smem_al = smem_raw + (sbase - raw32);
-  const uint32_t sF = sbase + L::kF, sG = sbase + L::kG, sV = sbase + L::kV;
-  const uint32_t bar0 = sbase + L::kBar;
-  auto BAR = [&](int i) { return bar0 + 8u * i; };
-  constexpr int B_FFULL = 0, B_FEMPTY = NF, B_GFULL = 2 * NF, B_GEMPTY = B_GFULL + NG, B_VFULL = B_GEMPTY + NG,
-                B_VEMPTY = B_VFULL + NV, B_SFULL = B_VEMPTY + NV, B_SEMPTY = B_SFULL + NS, B_PFULL = B_SEMPTY + NS,
-                B_PEMPTY = B_PFULL + NPB, B_OFULL = B_PEMPTY + NPB, B_OEMPTY = B_OFULL + 1;
-  volatile uint32_t* tmem_ptr_smem = reinterpret_cast<volatile uint32_t*>(smem_al + L::kTmemPtr);
-  double* loss_slots = reinterpret_cast<double*>(smem_al + L::kLossSlots);      // [8 ratio warps][2]
+  const uint32_t sF = sbase + L::kF;
+  auto STAGE = [&](uint32_t s) { return sbase + L::kStage0 + s * (uint32_t)L::kStageBytes; };
+  auto BAR = [&](int i) { return sbase + L::kBar + 8u * i; };
+  constexpr int B_FFULL = 0, B_FEMPTY = 1, B_FULL = 2, B_EMPTY = 2 + NS;
+  double* loss_slots = reinterpret_cast<double*>(smem_al + L::kLossSlots);      // [8 consumer warps][2]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7;
 
-  if (warp == kCtl0 && lane == 0) {
+  if (threadIdx.x == 0) {
     ptx::prefetch_tmap(&tmF); ptx::prefetch_tmap(&tmG); ptx::prefetch_tmap(&tmV);
-    for (int i = 0; i < NF; ++i) { ptx::mbar_init(BAR(B_FFULL + i), 1); ptx::mbar_init(BAR(B_FEMPTY + i), 1); }
-    for (int i = 0; i < NG; ++i) { ptx::mbar_init(BAR(B_GFULL + i), 1); ptx::mbar_init(BAR(B_GEMPTY + i), 1); }
-    for (int i = 0; i < NV; ++i) { ptx::mbar_init(BAR(B_VFULL + i), 1); ptx::mbar_init(BAR(B_VEMPTY + i), 4 * NRW); }
-    for (int i = 0; i < NS; ++i) { ptx::mbar_init(BAR(B_SFULL + i), 1); ptx::mbar_init(BAR(B_SEMPTY + i), 4 * NRW); }
-    for (int i = 0; i < NPB; ++i) { ptx::mbar_init(BAR(B_PFULL + i), 4 * NRW); ptx::mbar_init(BAR(B_PEMPTY + i), 1); }
-    ptx::mbar_init(BAR(B_OFULL), 1);
-    ptx::mbar_init(BAR(B_OEMPTY), 4);
+    ptx::mbar_init(BAR(B_FFULL), 1);
+    ptx::mbar_init(BAR(B_FEMPTY), 8);               // one arrival per consumer warp
+    for (int i = 0; i < NS; ++i) { ptx::mbar_init(BAR(B_FULL + i), 1); ptx::mbar_init(BAR(B_EMPTY + i), 8); }
     ptx::fence_barrier_init();
     ptx::fence_proxy_async();
   }
-  if (warp == kCtl0 + 1) {
-    ptx::tmem_alloc(sbase + L::kTmemPtr, kTmemCols);
-    ptx::tmem_relinquish();
-  }
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem = *tmem_ptr_smem;
 
   const int total_items = p.row_blocks * p.nchunks;
 
-  if (warp == kCtl0) {
-    // =========================== TMA producer: V tiles (the HBM stream) =================================
-    // HBM latency under load (~3 us) times the per-SM share of the bandwidth is more than the shared-memory ring
-    // can hold in flight, so the stream is staged through L2: tile t + kPfDist is prefetched into L2 (no smem,
-    // no barrier) while tile t is copied L2 -> smem into the ring.
-    if (lane == 0) {
-      const int kPfDist = p.pf_dist;
-      int pf_item = blockIdx.x, pf_j = 0, pf_te = 0, pf_rb = 0;
-      bool pf_live = pf_item < total_items;
-      auto pf_load_item = [&]() {
-        pf_rb = pf_item % p.row_blocks;
-        const int chunk = pf_item / p.row_blocks;
-        pf_j = chunk * p.tiles_per_chunk;
-        pf_te = min(p.tiles, pf_j + p.tiles_per_chunk);
-      };
-      auto pf_issue_and_advance = [&]() {
-        if (!pf_live) return;
-        for (int vb = 0; vb < TN / 64; ++vb) ptx::tma_prefetch_l2_2d(&tmV, pf_j * TN + vb * 64, pf_rb * kTileM);
-        if (++pf_j >= pf_te) {
-          pf_item += gridDim.x;
-          pf_live = pf_item < total_items;
-          if (pf_live) pf_load_item();
-        }
-      };
-      if (pf_live) pf_load_item();
-      for (int k = 0; k < kPfDist; ++k) pf_issue_and_advance();
-      uint32_t t = 0;
-      for (int item = blockIdx.x; item < total_items; item += gridDim.x) {
-        const int rb = item % p.row_blocks, chunk = item / p.row_blocks;
-        const int tb = chunk * p.tiles_per_chunk;
-        const int te = min(p.tiles, tb + p.tiles_per_chunk);
-        for (int j = tb; j < te; ++j, ++t) {
-          const uint32_t s = t % NV, ph = (t / NV) & 1;
-          if (kPfDist > 0) pf_issue_and_advance();
-          ptx::mbar_wait(BAR(B_VEMPTY + s), ph ^ 1);
-          TC_TRACE(t, 7);
-          if (TC_KNOCK(32) && t >= (uint32_t)NV) { ptx::mbar_arrive(BAR(B_VFULL + s)); continue; }
-          ptx::mbar_expect_tx(BAR(B_VFULL + s), L::kVBytes);
-          for (int vb = 0; vb < TN / 64; ++vb)
-            ptx::tma_load_2d(&tmV, BAR(B_VFULL + s), sV + s * L::kVBytes + vb * (kTileM * 128), j * TN + vb * 64,
-                             rb * kTileM);
-        }
-      }
-    }
-  } else if (warp == kCtl0 + 2) {
-    // =========================== TMA producer: F blocks and G tiles (L2-resident factors) ================
-    if (lane == 0) {
+  if (wg == 0) {
+    // =========================== TMA producer =====================================================
+    if (threadIdx.x == 0) {
       uint32_t it = 0, t = 0;
       for (int item = blockIdx.x; item < total_items; item += gridDim.x, ++it) {
         const int rb = item % p.row_blocks, chunk = item / p.row_blocks;
         const int tb = chunk * p.tiles_per_chunk;
         const int te = min(p.tiles, tb + p.tiles_per_chunk);
-        const uint32_t fb = it % NF;
-        ptx::mbar_wait(BAR(B_FEMPTY + fb), ((it / NF) & 1) ^ 1);
-        ptx::mbar_expect_tx(BAR(B_FFULL + fb), L::kFBytes);
+        ptx::mbar_wait(BAR(B_FEMPTY), (it & 1) ^ 1);                 // both consumer warpgroups are done with the last F
+        ptx::mbar_expect_tx(BAR(B_FFULL), L::kFBytes);
         for (int kb = 0; kb < KW / 64; ++kb)
-          ptx::tma_load_2d(&tmF, BAR(B_FFULL + fb), sF + fb * L::kFBytes + kb * (kTileM * 128), kb * 64, rb * kTileM);
+          ptx::tma_load_2d(&tmF, BAR(B_FFULL), sF + kb * (kTileM * 128), kb * 64, rb * kTileM);
         for (int j = tb; j < te; ++j, ++t) {
-          const uint32_t s = t % NG, ph = (t / NG) & 1;
-          ptx::mbar_wait(BAR(B_GEMPTY + s), ph ^ 1);
-          TC_TRACE(t, 8);
-          ptx::mbar_expect_tx(BAR(B_GFULL + s), L::kGBytes);
+          const uint32_t s = t % NS, ph = (t / NS) & 1;
+          ptx::mbar_wait(BAR(B_EMPTY + s), ph ^ 1);
+          ptx::mbar_expect_tx(BAR(B_FULL + s), L::kStageBytes);
+          const uint32_t sG = STAGE(s), sV = sG + L::kGBytes;
           for (int kb = 0; kb < KW / 64; ++kb)
-            ptx::tma_load_2d(&tmG, BAR(B_GFULL + s), sG + s * L::kGBytes + kb * (TN * 128), kb * 64, j * TN);
+            ptx::tma_load_2d(&tmG, BAR(B_FULL + s), sG + kb * (TN * 128), kb * 64, j * TN);
+          for (int vb = 0; vb < TN / 64; ++vb)
+            ptx::tma_load_2d(&tmV, BAR(B_FULL + s), sV + vb * (kTileM * 128), j * TN + vb * 64, rb * kTileM);
         }
       }
     }
-  } else if (warp == kCtl0 + 1) {
-    // =========================== MMA issuer 1: S = F G^T =============================
-    // Two issuing warps share the tensor pipe.  An issuing warp is a latency-bound serial instruction stream (barrier
-    // polls, descriptor arithmetic in uniform registers, tcgen05.mma issue: measured ~780 cycles per S or O step), so
-    // one warp issuing both S and O produced one tile per ~1570 cycles and left the ratio warpgroups waiting for S.
-    // This warp runs ahead with the S-MMAs, across work-item boundaries, bounded by the G ring and by the NS
-    // accumulator stages (p_empty: the O-MMA of the tile NS earlier has consumed the stage); warp 3 issues the O-MMAs as
-    // ratio tiles complete.  Each loop is warp-uniform; one elected lane issues tcgen05.mma / commit.
-    {
-      constexpr uint32_t idescS = ptx::idesc_f16(kTileM, TN, 0, 0);
-      constexpr uint32_t descHi = ptx::smem_desc_hi_sw128(1024);
-      // S = sum over terms (F part, G part): fast: (0,0); split: (hi,hi), (lo,hi), (hi,lo)
-      constexpr int kTerms = SPLIT ? 3 : 1;
-      constexpr int termF[3] = {0, 1, 0}, termG[3] = {0, 0, 1};
-      uint32_t sg = 0, sg_ph = 0;                 // G stage / phase
-      uint32_t ss = 0, ss_ph = 0;                 // S stage / phase of its p_empty barrier
-      uint32_t ts = 0;                            // tile counter (trace only)
-      uint32_t it = 0;
-      for (int item = blockIdx.x; item < total_items; item += gridDim.x, ++it) {
-        const int tb = (item / p.row_blocks) * p.tiles_per_chunk;
-        const int n = min(p.tiles, tb + p.tiles_per_chunk) - tb;
-        const uint32_t f_s = it % NF;
-        if (lane == 0) ptx::mbar_wait(BAR(B_FFULL + f_s), (it / NF) & 1);       // F block of this item landed
-        __syncwarp();      // one poller; the warp is converged again before any elect.sync / tcgen05 issue
-        const uint32_t fbase = sF + f_s * L::kFBytes;
-        for (int j = 0; j < n; ++j) {
-          if (lane == 0) {
-            TC_TRACE(ts, 0);
-            ptx::mbar_wait(BAR(B_GFULL + sg), sg_ph);              // G tile landed
-            TC_TRACE(ts, 12);
-            // the stage is free: the O-MMA of the tile NS earlier consumed its P (alias layout) / the ratio warps have
-            // read the S of the tile NS earlier (P buffers of their own)
-            ptx::mbar_wait(BAR((PSEP && !LOSS ? B_SEMPTY : B_PEMPTY) + ss), ss_ph ^ 1);
-            TC_TRACE(ts, 1);
-          }
-          __syncwarp();
-          ptx::tc_fence_after();
-          const uint32_t gbase = sG + sg * L::kGBytes;
-          const uint32_t dS = tmem + kColS + ss * TN;
-          if (ptx::elect_one()) {
+    return;
+  }
+
+  // =========================== consumer warpgroups ===================================================
+  const int cw = wg - 1;                       // rows [64 cw, 64 cw + 64) of every item
+  const int cwarp = warp - 4;                  // consumer warp 0..7 (loss slots)
+  const int g8 = lane >> 2, c4 = lane & 3;
+  // accumulator fragment of wgmma m64nN: element (r0 + 8 h, 8 j + 2 c4 + e) sits in d[4 j + 2 h + e]
+  const int r0 = cw * 64 + (warp & 3) * 16 + g8;
+  const int ev = p.exps[0], ea = p.exps[p.ef], eb = p.exps[p.eg], ep = p.exps[3];
+  // update: x' = (S + eps) * 2^(v-p), so P~ = V~ / x' = P * 2^p (P ~ 1 maps to ~1: fp16-safe for any input scale)
+  // loss  : x  = S + eps in true scale
+  const float c1 = (LOSS || TWO) ? exp2f((float)(-ea - eb)) : exp2f((float)(ev - ea - eb - ep));
+  const float c2 = (LOSS || TWO) ? kEps : kEps * exp2f((float)(ev - ep));
+  // two-output kernels: Pn~ = V~ x^(beta-2) kn, Pp~ = x^(beta-1) kd with x = S + eps in true scale
+  const float kn = TWO ? exp2f((float)(p.exps[4] - ev)) : 0.f;
+  const float kd = TWO ? exp2f((float)p.exps[5]) : 0.f;
+  // The tile fed to the second MMA is the CENTRED ratio (P - kappa) 2^p with kappa = sum(V) / sum(W H^T) (-> 1 as the fit
+  // converges); kappa * colsum(G) is added back in fp32 by the ratio stage.  Tensor-core accumulation truncates, a
+  // one-signed bias that the scale-free direction (W a, H / a) of KL-NMF integrates over iterations; the centred sum is
+  // signed and small, and its fp16 rounding error is relative to |P - kappa| instead of |P|.
+  const float negpc = (LOSS || TWO || EU) ? 0.f : -(*p.kappa) * exp2f((float)ep);
+  // beta 2: P~ = (V - WH) 2^pe = v~ cv - s~ cs   (pe = exps[4], from mean(V)); loss: true scale (pe = 0)
+  const float eu_cv = EU ? exp2f((float)((LOSS ? 0 : p.exps[4]) - ev)) : 0.f;
+  // update: the tile is V - kappa WH with kappa = sum(V) / sum(WH) (the scale-matched residual; kappa -> 1 as the fit
+  // converges), so that far from convergence (WH >> V) the numerator is not a small difference of large sums
+  const float eu_cs = EU ? exp2f((float)((LOSS ? 0 : p.exps[4]) - ea - eb)) * (LOSS ? 1.f : *p.kappa) : 0.f;
+  const float vinv = exp2f(-(float)ev);
+  const float c1l = exp2f((float)(-ea - eb));            // FOLD: x = WH + eps in true scale (the LOSS kernel's c1 / c2)
+  const float oscale = exp2f(-(float)(p.exps[p.eg] + p.exps[(TWO || EU) ? 4 : 3]));      // O = sum (P 2^p) (G 2^eg)
+  const float oscale2 = TWO ? exp2f(-(float)(p.exps[p.eg] + p.exps[5])) : 0.f;
+  // S = sum over terms (F part, G part): fast: (0,0); split: (hi,hi), (lo,hi), (hi,lo)
+  constexpr int kTerms = SPLIT ? 3 : 1;
+  constexpr int termF[3] = {0, 1, 0}, termG[3] = {0, 0, 1};
+  double accA = 0.0, accB = 0.0;
+  uint32_t it = 0, t = 0;
+  for (int item = blockIdx.x; item < total_items; item += gridDim.x, ++it) {
+    const int rb = item % p.row_blocks, chunk = item / p.row_blocks;
+    const int tb = chunk * p.tiles_per_chunk;
+    const int n = min(p.tiles, tb + p.tiles_per_chunk) - tb;
+    float o[RP / 2], o2[TWO ? 32 : 1];
 #pragma unroll
-            for (int term = 0; term < kTerms; ++term) {
-              if (TC_KNOCK(16)) break;
-              // operand halves (hi / lo) are RP/64 sub-blocks of 64 columns each; a k-step is 32 B inside a sub-block
+    for (int i = 0; i < RP / 2; ++i) o[i] = 0.f;
 #pragma unroll
-              for (int ks = 0; ks < RP / 16; ++ks) {
-                const uint32_t alo = ptx::smem_desc_lo(fbase + (termF[term] * (RP / 64) + ks / 4) * (kTileM * 128), 16);
-                const uint32_t blo = ptx::smem_desc_lo(gbase + (termG[term] * (RP / 64) + ks / 4) * (TN * 128), 16);
-                ptx::mma_ss(dS, ptx::make_desc(alo + 2 * (ks % 4), descHi), ptx::make_desc(blo + 2 * (ks % 4), descHi),
-                            idescS, (term | ks) ? 1u : 0u);
-              }
-            }
-            ptx::mma_commit(BAR(B_SFULL + ss));
-            if (j == n - 1) ptx::mma_commit(BAR(B_FEMPTY + f_s));  // last S of the item: its F block is free
-            TC_TRACE(ts, 13);
+    for (int i = 0; i < (TWO ? 32 : 1); ++i) o2[i] = 0.f;
+    ptx::mbar_wait(BAR(B_FFULL), it & 1);
+    for (int j = 0; j < n; ++j, ++t) {
+      const uint32_t s = t % NS;
+      ptx::mbar_wait(BAR(B_FULL + s), (t / NS) & 1);
+      const uint32_t sG = STAGE(s), sV = sG + L::kGBytes;
+#pragma unroll 1
+      for (int st = 0; st < TN / kStep; ++st) {
+        // ---- S = F G^T over the 64 columns of this step
+        float sacc[32];
+        ptx::wgmma_fence();
+#pragma unroll
+        for (int term = 0; term < kTerms; ++term) {
+#pragma unroll
+          for (int ks = 0; ks < RP / 16; ++ks) {
+            const uint32_t fa = sF + (termF[term] * (RP / 64) + ks / 4) * (kTileM * 128) + cw * (64 * 128) + (ks % 4) * 32;
+            const uint32_t gb = sG + (termG[term] * (RP / 64) + ks / 4) * (TN * 128) + st * (kStep * 128) + (ks % 4) * 32;
+            ptx::wgmma_ss_m64n64(sacc, ptx::gmma_desc_sw128(fa, 16, 1024), ptx::gmma_desc_sw128(gb, 16, 1024),
+                                 (term | ks) ? 1u : 0u);
           }
-          __syncwarp();
-          if (++sg == NG) { sg = 0; sg_ph ^= 1; }
-          if (++ss == NS) { ss = 0; ss_ph ^= 1; }
-          ++ts;
         }
-      }
-    }
-  } else if (warp == kCtl0 + 3) {
-    // =========================== MMA issuer 2: O += P G =============================
-    {
-      constexpr uint32_t idescO = ptx::idesc_f16(kTileM, KW, 0, 1);
-      constexpr uint32_t descHi = ptx::smem_desc_hi_sw128(1024);
-      constexpr int NO = (PSEP && !LOSS) ? NP : NS;   // ring the O-MMAs walk: P buffers of their own, or the S/P stages
-      uint32_t og = 0, os = 0, os_ph = 0;         // G stage, P stage + p_full phase
-      uint32_t to = 0;                            // tile counter (trace only)
-      uint32_t it = 0;
-      for (int item = blockIdx.x; item < total_items; item += gridDim.x, ++it) {
-        const int tb = (item / p.row_blocks) * p.tiles_per_chunk;
-        const int n = min(p.tiles, tb + p.tiles_per_chunk) - tb;
-        for (int j = 0; j < n; ++j) {
-          const bool first = j == 0, last = j == n - 1;
-          if (lane == 0) {
-            TC_TRACE(to, 5);
-            ptx::mbar_wait(BAR(B_PFULL + os), os_ph);                              // ratio tile written
-            if (first && !LOSS) ptx::mbar_wait(BAR(B_OEMPTY), (it & 1) ^ 1);       // epilogue drained O (none in LOSS mode)
-            TC_TRACE(to, 6);
-          }
-          __syncwarp();
-          ptx::tc_fence_after();
-          if (LOSS) {
-            if (ptx::elect_one()) {                    // nothing to multiply: the ratio warpgroup consumed S, release
-              ptx::mbar_arrive(BAR(B_GEMPTY + og));
-              ptx::mbar_arrive(BAR(B_PEMPTY + os));
-            }
-          } else {
-            // B = G tile as [K = 16 c-rows][N = KW] MN-major: 8-row groups 1024 B apart, 64-wide column blocks
-            // (hi | lo, RP/64 blocks each) one sub-block (TN x 128 B) apart
-            const uint32_t blo = ptx::smem_desc_lo(sG + og * L::kGBytes, TN * 128);
-            const uint32_t aP = PSEP ? tmem + kColP + os * (TN / 2) : tmem + kColS + os * TN;
-            if (ptx::elect_one()) {
+        ptx::wgmma_commit();
+        ptx::wgmma_wait<0>();
+        ptx::fence_regs(sacc);
+        // ---- ratio stage on the accumulator fragment; V~ pairs from the swizzled V tile: byte (row, 16-byte chunk k)
+        //      of a 64-column sub-tile sits at row*128 + ((k ^ row%8) << 4), and row % 8 = g8 for both rows of a thread
+        const uint32_t vsub = sV + st * (kTileM * 128) + (uint32_t)c4 * 4u;
+        const int col0 = (tb + j) * TN + st * kStep + 2 * c4;      // global column of d[4 j + 2 h]
+        uint32_t pa[16], pp[TWO ? 16 : 1];
+        float la = 0.f, lb = 0.f;
 #pragma unroll
-              for (int ks = 0; ks < TN / 16; ++ks) {
-                if (TC_KNOCK(8)) break;
-                // P k-step ks was written by ratio warpgroup ks / kKsPerWg: at the start of that warpgroup's S columns
-                // (alias layout) or packed in k order into the P buffer
-                constexpr int kKsPerWg = TN / 16 / NRW;
-                ptx::mma_ts(tmem + kColO, aP + (PSEP ? ks * 8 : (ks / kKsPerWg) * (TN / NRW) + (ks % kKsPerWg) * 8),
-                            ptx::make_desc(blo + ks * 128, descHi), idescO, (first && ks == 0) ? 0u : 1u);
-                if (TWO)
-                  ptx::mma_ts(tmem + kColO2, tmem + kColPp + os * 64 + ks * 8, ptx::make_desc(blo + ks * 128, descHi),
-                              idescO, (first && ks == 0) ? 0u : 1u);
-                if (ks == 0) TC_TRACE(to, 15);
-              }
-              ptx::mma_commit(BAR(B_GEMPTY + og));     // G tile free (its S-MMA finished before the ratio tile existed)
-              ptx::mma_commit(BAR(B_PEMPTY + os));     // S/P stage free
-              if (last) ptx::mma_commit(BAR(B_OFULL));
-              TC_TRACE(to, 14);
-            }
-          }
-          __syncwarp();
-          if (++og == NG) og = 0;
-          if (++os == NO) { os = 0; os_ph ^= 1; }
-          ++to;
-        }
-      }
-    }
-  } else if (warp < kEpiWarp0) {
-    // =========================== ratio warpgroups =======================
-    // Every tile is split by COLUMNS between the NRW ratio warpgroups (each covers all 128 TMEM lanes): the time a tile
-    // spends in the ratio stage is what holds its S/P accumulator stage, and with NS = 3 stages that hold time -- not
-    // MUFU, shared-memory or HBM throughput -- set the tile period (knock-out timing, DESIGN.md 4.1).  Splitting a
-    // tile halves the hold; alternating whole tiles between the warpgroups did not.
-    const int g = warp >> 2;                   // this warpgroup handles columns [g TN / NRW, (g + 1) TN / NRW) of every tile
-    const int q = warp & 3;                    // TMEM lane quarter this warp may touch
-    const int row = q * 32 + lane;
-    const uint32_t lane_addr = (uint32_t)(q * 32) << 16;
-    const int ev = p.exps[0], ea = p.exps[p.ef], eb = p.exps[p.eg], ep = p.exps[3];
-    // update: x' = (S + eps) * 2^(v-p), so P~ = V~ / x' = P * 2^p (P ~ 1 maps to ~1: fp16-safe for any input scale)
-    // loss  : x  = S + eps in true scale
-    const float c1 = (LOSS || TWO) ? exp2f((float)(-ea - eb)) : exp2f((float)(ev - ea - eb - ep));
-    const float c2 = (LOSS || TWO) ? kEps : kEps * exp2f((float)(ev - ep));
-    // two-output kernels: Pn~ = V~ x^(beta-2) kn, Pp~ = x^(beta-1) kd with x = S + eps in true scale
-    const float kn = TWO ? exp2f((float)(p.exps[4] - ev)) : 0.f;
-    const float kd = TWO ? exp2f((float)p.exps[5]) : 0.f;
-    // The tile fed to MMA-2 is the CENTRED ratio (P - kappa) 2^p with kappa = sum(V) / sum(W H^T) (-> 1 as the fit
-    // converges); kappa * colsum(G) is added back in fp32 by the ratio stage.  Tensor-core accumulation truncates
-    // (measured: -4.7e-5 relative on this all-positive sum, profiles/README.md), a one-signed bias that the
-    // scale-free direction (W a, H / a) of KL-NMF integrates over iterations; the centred sum is signed and
-    // small, and its fp16 rounding error is relative to |P - kappa| instead of |P|.
-    const float negpc = (LOSS || TWO || EU) ? 0.f : -(*p.kappa) * exp2f((float)ep);
-    // beta 2: P~ = (V - WH) 2^pe = v~ cv - s~ cs   (pe = exps[4], from mean(V)); loss: true scale (pe = 0)
-    const float eu_cv = EU ? exp2f((float)((LOSS ? 0 : p.exps[4]) - ev)) : 0.f;
-    // update: the tile is V - kappa WH with kappa = sum(V) / sum(WH) (the scale-matched residual; kappa -> 1 as the fit
-    // converges), so that far from convergence (WH >> V) the numerator is not a small difference of large sums
-    const float eu_cs = EU ? exp2f((float)((LOSS ? 0 : p.exps[4]) - ea - eb)) * (LOSS ? 1.f : *p.kappa) : 0.f;
-    double accA = 0.0, accB = 0.0;
-    uint32_t t = 0;
-    const float vinv = exp2f(-(float)ev);
-    if constexpr (!LOSS && !TWO) {
-      // ---- update tiles of beta 1 / beta 2: ONE flat software pipeline over every (tile, 16-column chunk) of this CTA.
-      // The stage is bound by the FMA pipe of the four SM sub-partitions, not by latency (measured, tools/ubench/pipes.cu on
-      // the B200: FFMA 1.6, FFMA2 2.3, FMUL2 3.7, HFMA2 2.0, IMAD / LOP3 / PRMT 2.1, MUFU 8.0 cycles per warp instruction and
-      // sub-partition; four ratio warpgroups instead of two changed nothing).  Hence:
-      // * everything runs as packed fp32 pairs through FFMA2 (a product is an FFMA2 with a zero addend: FMUL2 is slower);
-      // * three quarters of the reciprocals are batched four elements to two MUFU ops (1/a = b rcp(a b): +3 FFMA2 per four
-      //   elements, -2 MUFU), which balances the XU pipe (640 cycles per tile) against the FMA pipe (~690);
-      // * addresses are formed once per tile (swizzled shared-memory offsets by one XOR with a constant per load), ring
-      //   positions are counted, not divided;
-      // * the TMEM load of S and the shared-memory load of V for chunk c + 1 are in flight while chunk c is computed, across
-      //   tile boundaries (the next tile's first chunk is requested before this tile's last chunk is computed).
-      // A "chunk" is CW columns of the tile: the unit of the load / compute software pipeline (the loads of chunk c + 1 are in
-      // flight while chunk c is computed).  32-column chunks (twice the lookahead, 126 registers) measured slower than 16
-      // (116 / 122 us vs 111 / 118 us per launch at cfg2): the stage is not waiting for its loads.
-      constexpr int CW = 16;                                    // tmem_ld16 / tmem_st8 below
-      constexpr int kChunks = TN / CW;
-      constexpr int kCpw = kChunks / NRW;                       // chunks per warpgroup and tile
-      static_assert(kCpw % 2 == 0 && kChunks % NRW == 0, "chunks per ratio warpgroup");
-      const int c_lo = g * kCpw;
-      uint32_t my_tiles = 0;
-      for (int item = blockIdx.x; item < total_items; item += gridDim.x) {
-        const int tb = (item / p.row_blocks) * p.tiles_per_chunk;
-        my_tiles += min(p.tiles, tb + p.tiles_per_chunk) - tb;
-      }
-      const uint64_t C1 = ptx::pk2(c1, c1), C2 = ptx::pk2(c2, c2), NEGPC = ptx::pk2(negpc, negpc), Z2 = ptx::pk2(0.f, 0.f);
-      const uint64_t EUCV = ptx::pk2(eu_cv, eu_cv), EUNCS = ptx::pk2(-eu_cs, -eu_cs);
-      // FOLD: x = WH + eps in true scale (the LOSS kernel's c1 / c2), sum v~ lg2 x and sum S~ of this thread and tile
-      const float c1l = exp2f((float)(-ea - eb));
-      const uint64_t C1L = ptx::pk2(c1l, c1l), C2L = ptx::pk2(kEps, kEps), ONE2 = ptx::pk2(1.f, 1.f);
-      float fold_a = 0.f;
-      uint64_t FOLD_B = Z2;
-      // this thread's row inside a 128-byte-swizzled V sub-tile: byte (row, 16-byte chunk k) sits at row*128 + ((k ^ row%8) << 4)
-      const uint32_t vrow = (uint32_t)row * 128u + ((uint32_t)(row & 7) << 4);
-      const uint32_t tS0 = tmem + lane_addr + kColS;            // TMEM address of this warp's lanes, stage 0, column 0
-      constexpr int NV4 = CW / 8;                               // 16-byte shared-memory loads per chunk
-      uint32_t sA[CW], sB[CW];
-      uint4 vA[NV4], vB[NV4];
-      auto load_chunk = [&](uint32_t tS, uint32_t vT, int c, uint32_t (&sr)[CW], uint4 (&vv)[NV4]) {
-        ptx::tmem_ld16(tS + c * CW, sr);
+        for (int jn = 0; jn < 8; ++jn) {
 #pragma unroll
-        for (int k = 0; k < NV4; ++k) {
-          if (TC_KNOCK(2)) { vv[k] = make_uint4(0x3c003c00u, 0x3c003c00u, 0x3c003c00u, 0x3c003c00u); continue; }
-          const int col16 = c * NV4 + k;                                           // 16-byte column group of the tile (8 fp16)
-          const uint32_t kx = (uint32_t)(col16 & 7) << 4;                          // compile-time per unrolled load
-          asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];"
-                       : "=r"(vv[k].x), "=r"(vv[k].y), "=r"(vv[k].z), "=r"(vv[k].w)
-                       : "r"((vT ^ kx) + (uint32_t)((col16 >> 3) * (kTileM * 128))));
-        }
-      };
-      auto compute_chunk = [&](uint32_t tS, uint32_t tP, int c, const uint32_t (&sr)[CW], const uint4 (&vv)[NV4]) {
-        const uint32_t* vw = reinterpret_cast<const uint32_t*>(vv);
-        uint32_t preg[CW / 2];
-#pragma unroll
-        for (int qd = 0; qd < CW / 4; ++qd) {                    // four consecutive columns: pairs a = (0, 1), b = (2, 3)
-          const float2 va = __half22float2(*reinterpret_cast<const __half2*>(&vw[2 * qd]));
-          const float2 vb = __half22float2(*reinterpret_cast<const __half2*>(&vw[2 * qd + 1]));
-          const uint64_t Va = ptx::pk2(va.x, va.y), Vb = ptx::pk2(vb.x, vb.y);
-          const uint64_t Sa = ptx::pk2(__uint_as_float(sr[4 * qd]), __uint_as_float(sr[4 * qd + 1]));
-          const uint64_t Sb = ptx::pk2(__uint_as_float(sr[4 * qd + 2]), __uint_as_float(sr[4 * qd + 3]));
-          uint64_t Pa, Pb;
-          if (EU) {
-            Pa = ptx::fma2(Sa, EUNCS, ptx::fma2(Va, EUCV, Z2));                       // nmf.py:62-63: V - kappa WH
-            Pb = ptx::fma2(Sb, EUNCS, ptx::fma2(Vb, EUCV, Z2));
-          } else {
-            const uint64_t Xa = ptx::fma2(Sa, C1, C2), Xb = ptx::fma2(Sb, C1, C2);   // (WH + eps) in the scale of V~ / P~
-            if constexpr (FOLD) {                                                    // metrics.py:22 on the same S tile
-              float l0, l1, l2, l3;
-              ptx::upk2(ptx::fma2(Sa, C1L, C2L), l0, l1);
-              ptx::upk2(ptx::fma2(Sb, C1L, C2L), l2, l3);
-              fold_a = fmaf(va.x, __log2f(l0), fold_a);
-              fold_a = fmaf(va.y, __log2f(l1), fold_a);
-              fold_a = fmaf(vb.x, __log2f(l2), fold_a);
-              fold_a = fmaf(vb.y, __log2f(l3), fold_a);
-              FOLD_B = ptx::fma2(Sa, ONE2, FOLD_B);
-              FOLD_B = ptx::fma2(Sb, ONE2, FOLD_B);
-            }
-            uint64_t Ra, Rb;                                                         // 1 / x of pair a, pair b
-            if ((qd & 3) != 0) {
-              // batched: 1 / x0 = x2 r0, 1 / x1 = x3 r1, 1 / x2 = x0 r0, 1 / x3 = x1 r1 with r = rcp(x_a x_b)
-              float m0, m1;
-              ptx::upk2(ptx::fma2(Xa, Xb, Z2), m0, m1);
-              const uint64_t Rr = ptx::pk2(TC_KNOCK(1) ? m0 : ptx::rcp_approx(m0), TC_KNOCK(1) ? m1 : ptx::rcp_approx(m1));
-              Ra = ptx::fma2(Rr, Xb, Z2);
-              Rb = ptx::fma2(Rr, Xa, Z2);
-            } else {
-              float x0, x1, x2, x3;
-              ptx::upk2(Xa, x0, x1);
-              ptx::upk2(Xb, x2, x3);
-              Ra = ptx::pk2(TC_KNOCK(1) ? x0 : ptx::rcp_approx(x0), TC_KNOCK(1) ? x1 : ptx::rcp_approx(x1));
-              Rb = ptx::pk2(TC_KNOCK(1) ? x2 : ptx::rcp_approx(x2), TC_KNOCK(1) ? x3 : ptx::rcp_approx(x3));
-            }
-            Pa = ptx::fma2(Va, Ra, NEGPC);                                           // nmf.py:65, centred
-            Pb = ptx::fma2(Vb, Rb, NEGPC);
-          }
-          float a0, a1, b0, b1;
-          ptx::upk2(Pa, a0, a1);
-          ptx::upk2(Pb, b0, b1);
-          preg[2 * qd] = ptx::pack_f16x2_sat(a0, a1);
-          preg[2 * qd + 1] = ptx::pack_f16x2_sat(b0, b1);
-        }
-        // P of warpgroup g goes over the S columns that warpgroup owns (and has already read): [g TN / NRW, ...), or into
-        // its k-ordered slice of the tile's own P buffer
-        const uint32_t dst = PSEP ? tP + c * (CW / 2) : tS + g * (TN / NRW) + (c - c_lo) * (CW / 2);
-        ptx::tmem_st8(dst, preg);
-      };
-      uint32_t st = 0, sv = 0, phS = 0, phV = 0;        // S stage and V slot of the tile being computed, phases of their full barriers
-      uint32_t pb = 0, phP = 0;                         // PSEP: P buffer of the tile being computed, phase of its empty barrier
-      uint32_t tS = tS0, vT = sV + vrow;
-      const uint32_t tP0 = tmem + lane_addr + kColP;
-      if (my_tiles > 0) {
-        if (q == 0 && lane == 0) TC_TRACE(0, 2);
-        ptx::mbar_wait(BAR(B_VFULL), 0);                            // V tile landed (TMA -> this thread)
-        ptx::mbar_wait(BAR(B_SFULL), 0);                            // S tile complete
-        if (q == 0 && lane == 0) TC_TRACE(0, 4);
-        ptx::tc_fence_after();
-        load_chunk(tS, vT, c_lo, sA, vA);
-      }
-      for (uint32_t tt = 0; tt < my_tiles; ++tt) {
-        const bool more = tt + 1 < my_tiles;
-        // ring positions of the next tile
-        uint32_t st1 = st + 1, phS1 = phS, sv1 = sv + 1, phV1 = phV;
-        if (st1 == NS) { st1 = 0; phS1 ^= 1; }
-        if (sv1 == NV) { sv1 = 0; phV1 ^= 1; }
-        const uint32_t tS1 = tS0 + st1 * TN, vT1 = sV + sv1 * L::kVBytes + vrow;
-        const uint32_t tP = tP0 + pb * (TN / 2);
-        if (PSEP) ptx::mbar_wait(BAR(B_PEMPTY + pb), phP ^ 1);      // the O-MMA of the tile NP earlier has consumed this buffer
-#pragma unroll
-        for (int cc = 0; cc < kCpw; cc += 2) {
-          const int c = c_lo + cc;
-          const bool lastpair = cc + 2 >= kCpw;
-          // The next tile's full barriers are TESTED a chunk of work before they are needed: a try_wait returns its answer
-          // after ~100 cycles even when the phase completed long ago (ncu source page: 15 % of the ratio warps' time sat on
-          // the two polls of every tile), and both ratio warps of a sub-partition reach them together.
-          bool okV = false, okS = false;
-          if (lastpair && more) {
-            okV = ptx::mbar_test_wait(BAR(B_VFULL + sv1), phV1);
-            okS = ptx::mbar_test_wait(BAR(B_SFULL + st1), phS1);
-          }
-          ptx::tc_wait_ld();
-          load_chunk(tS, vT, c + 1, sB, vB);
-          compute_chunk(tS, tP, c, sA, vA);
-          ptx::tc_wait_ld();
-          if (!lastpair) {
-            load_chunk(tS, vT, c + 2, sA, vA);
-          } else {
-            if (PSEP) {
-              // every S column of this tile is in registers (tcgen05.wait::ld above): hand the S stage back now, a chunk
-              // before the P tile is complete.  (Not the V slot: an ld.shared is only known to have landed once its
-              // result has been consumed.)
-              ptx::tc_fence_before();
-              __syncwarp();
-              if (lane == 0) ptx::mbar_arrive(BAR(B_SEMPTY + st));
-            }
-            if (more) {
-              if (g == 0 && q == 0 && lane == 0) TC_TRACE(tt + 1, 2);
-              if (!okV) ptx::mbar_wait(BAR(B_VFULL + sv1), phV1);
-              if (g == 0 && q == 0 && lane == 0) TC_TRACE(tt + 1, 3);
-              if (!okS) ptx::mbar_wait(BAR(B_SFULL + st1), phS1);
-              if (g == 0 && q == 0 && lane == 0) TC_TRACE(tt + 1, 4);
-              ptx::tc_fence_after();
-              load_chunk(tS1, vT1, c_lo, sA, vA);
-            }
-          }
-          compute_chunk(tS, tP, c + 1, sB, vB);
-        }
-        // hand the tile on: P complete (alias layout: this also frees the S stage once the O-MMA has run) + the V slot
-        if (lane == 0 && g == 0 && q == 0) TC_TRACE(tt, 10);
-        ptx::tc_wait_st();
-        ptx::tc_fence_before();
-        __syncwarp();                  // every lane's P stores are complete and fenced, its V reads have returned
-        if (lane == 0) {               // ONE arrival per warp (barrier counts = warps): 32x fewer mbarrier operations
-          ptx::mbar_arrive(BAR(B_PFULL + (PSEP ? pb : st)));
-          ptx::mbar_arrive(BAR(B_VEMPTY + sv));
-        }
-        if (lane == 0 && g == 0 && q == 0) TC_TRACE(tt, 9);
-        if (lane == 0 && g == NRW - 1 && q == 3) TC_TRACE(tt, 11);
-        st = st1; phS = phS1; sv = sv1; phV = phV1; tS = tS1; vT = vT1;
-        if (PSEP && ++pb == (uint32_t)NP) { pb = 0; phP ^= 1; }
-        if constexpr (FOLD) {                    // per-tile fp32 sums (TN / NRW elements per thread) into the double totals
-          float b0, b1;
-          ptx::upk2(FOLD_B, b0, b1);
-          accA += (double)fold_a;
-          accB += (double)(b0 + b1);
-          fold_a = 0.f;
-          FOLD_B = Z2;
-        }
-      }
-    } else {
-    for (int item = blockIdx.x; item < total_items; item += gridDim.x) {
-      const int chunk = item / p.row_blocks;
-      const int tb = chunk * p.tiles_per_chunk;
-      const int te = min(p.tiles, tb + p.tiles_per_chunk);
-      const int n = te - tb;
-      const bool row_ok = (item % p.row_blocks) * kTileM + row < p.Mr;
-      for (int j = 0; j < n; ++j) {
-        const uint32_t tt = t + j;
-        const uint32_t s = tt % NV, st = tt % NS;
-        if (q == 0 && lane == 0) TC_TRACE(tt, 2);
-        ptx::mbar_wait(BAR(B_VFULL + s), (tt / NV) & 1);              // V tile landed (TMA -> this thread)
-        if (q == 0 && lane == 0) TC_TRACE(tt, 3);
-        ptx::mbar_wait(BAR(B_SFULL + st), (tt / NS) & 1);       // S tile complete
-        if (q == 0 && lane == 0) TC_TRACE(tt, 4);
-        ptx::tc_fence_after();
-        const uint32_t vrow = sV + s * L::kVBytes + row * 128;
-        {
-#pragma unroll
-        for (int c4r = 0; c4r < TN / 32 / NRW; ++c4r) {
-          const int c4 = g * (TN / 32 / NRW) + c4r;
-          uint32_t sreg[32];
-          ptx::tmem_ld32(tmem + lane_addr + kColS + st * TN + c4 * 32, sreg);
-          uint4 vv[4];
-          const uint32_t vsub = vrow + (c4 >> 1) * (kTileM * 128);
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            if (TC_KNOCK(2)) { vv[k] = make_uint4(0x3c003c00u, 0x3c003c00u, 0x3c003c00u, 0x3c003c00u); continue; }
-            const uint32_t chunk16 = (uint32_t)((c4 & 1) * 4 + k) ^ (uint32_t)(row & 7);
-            asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];"
-                         : "=r"(vv[k].x), "=r"(vv[k].y), "=r"(vv[k].z), "=r"(vv[k].w)
-                         : "r"(vsub + (chunk16 << 4)));
-          }
-          ptx::tc_wait_ld();
-          const uint32_t* vw = reinterpret_cast<const uint32_t*>(vv);
-          if (LOSS && EU) {
-            float la = 0.f;                        // metrics.py:39: 0.5 sum (WH - V)^2 (zero-filled edges contribute 0)
-#pragma unroll
-            for (int i = 0; i < 16; ++i) {
-              const float2 vf = __half22float2(*reinterpret_cast<const __half2*>(&vw[i]));
-              const float d0 = fmaf(vf.x, eu_cv, -__uint_as_float(sreg[2 * i]) * eu_cs);
-              const float d1 = fmaf(vf.y, eu_cv, -__uint_as_float(sreg[2 * i + 1]) * eu_cs);
+          for (int h = 0; h < 2; ++h) {
+            const int row = r0 + 8 * h;
+            uint32_t vraw;
+            asm volatile("ld.shared.u32 %0, [%1];" : "=r"(vraw)
+                         : "r"(vsub + (uint32_t)row * 128u + ((uint32_t)(jn ^ g8) << 4)));
+            const float2 vf = __half22float2(*reinterpret_cast<const __half2*>(&vraw));
+            const float s0 = sacc[4 * jn + 2 * h], s1 = sacc[4 * jn + 2 * h + 1];
+            const int ai = (jn >> 1) * 4 + (jn & 1) * 2 + h;       // A fragment: k-step jn / 2, register (jn & 1) * 2 + h
+            if (LOSS && EU) {                      // metrics.py:39: 0.5 sum (WH - V)^2 (zero-filled edges contribute 0)
+              const float d0 = fmaf(vf.x, eu_cv, -s0 * eu_cs), d1 = fmaf(vf.y, eu_cv, -s1 * eu_cs);
               la = fmaf(d0, d0, la);
               la = fmaf(d1, d1, la);
-            }
-            accA += (double)la;
-          } else if (LOSS && BM == kBmKL) {
-            float la = 0.f, lb = 0.f;
-#pragma unroll
-            for (int i = 0; i < 16; ++i) {
-              const float2 vf = __half22float2(*reinterpret_cast<const __half2*>(&vw[i]));
-              const float s0 = __uint_as_float(sreg[2 * i]), s1 = __uint_as_float(sreg[2 * i + 1]);
+            } else if (LOSS && BM == kBmKL) {
               la = fmaf(vf.x, __log2f(fmaf(s0, c1, c2)), la);
               la = fmaf(vf.y, __log2f(fmaf(s1, c1, c2)), la);
               lb += s0 + s1;
-            }
-            accA += (double)la;
-            accB += (double)lb;
-          } else if (LOSS) {
-            // metrics.py:56-57 (beta 0) and :84-96 (generic): A = sum t x^(beta-1), B = sum x^beta (beta 0: sum ln x / ln 2).
-            // Out-of-range rows / columns are zero-filled operands (x = eps there) and must be masked out.
-            float la = 0.f, lb = 0.f;
-            const int col0 = (tb + j) * TN + c4 * 32;
-#pragma unroll
-            for (int i = 0; i < 16; ++i) {
-              const float2 vf = __half22float2(*reinterpret_cast<const __half2*>(&vw[i]));
+            } else if (LOSS) {
+              // metrics.py:56-57 (beta 0) and :84-96 (generic): A = sum t x^(beta-1), B = sum x^beta (beta 0: sum ln x / ln 2).
+              // Out-of-range rows / columns are zero-filled operands (x = eps there) and must be masked out.
+              const bool row_ok = rb * kTileM + row < p.Mr;
 #pragma unroll
               for (int e = 0; e < 2; ++e) {
-                const bool ok = row_ok && col0 + 2 * i + e < p.Nc;
-                const float x = fmaf(__uint_as_float(sreg[2 * i + e]), c1, c2);
+                const bool ok = row_ok && col0 + 8 * jn + e < p.Nc;
+                const float x = fmaf(e ? s1 : s0, c1, c2);
                 const float v = (e ? vf.y : vf.x) * vinv;
                 const float lx = __log2f(x);
                 float ta, tb2;
@@ -681,18 +267,11 @@ tc_contract_kernel(const __grid_constant__ CUtensorMap tmF, const __grid_constan
                 la += ok ? ta : 0.f;
                 lb += ok ? tb2 : 0.f;
               }
-            }
-            accA += (double)la;
-            accB += (double)lb;
-          } else if (TWO) {
-            uint32_t pn[16], pp[16];
-#pragma unroll
-            for (int i = 0; i < 16; ++i) {
-              const float2 vf = __half22float2(*reinterpret_cast<const __half2*>(&vw[i]));
+            } else if (TWO) {
               float fn[2], fp[2];
 #pragma unroll
               for (int e = 0; e < 2; ++e) {
-                const float x = fmaf(__uint_as_float(sreg[2 * i + e]), c1, c2);        // WH + eps, nmf.py:68,72
+                const float x = fmaf(e ? s1 : s0, c1, c2);          // WH + eps, nmf.py:68,72
                 if (BM == kBmIS) {                 // nmf.py:68-70
                   const float r = ptx::rcp_approx(x);
                   fp[e] = r; fn[e] = r * r;
@@ -707,144 +286,88 @@ tc_contract_kernel(const __grid_constant__ CUtensorMap tmF, const __grid_constan
                   fp[e] = exp2f(p.bm1 * l); fn[e] = exp2f(p.bm2 * l);
                 }
               }
-              pn[i] = ptx::pack_f16x2_sat(vf.x * fn[0] * kn, vf.y * fn[1] * kn);
-              pp[i] = ptx::pack_f16x2_sat(fp[0] * kd, fp[1] * kd);
+              pa[ai] = ptx::pack_f16x2_sat(vf.x * fn[0] * kn, vf.y * fn[1] * kn);
+              pp[TWO ? ai : 0] = ptx::pack_f16x2_sat(fp[0] * kd, fp[1] * kd);
+            } else if (EU) {
+              pa[ai] = ptx::pack_f16x2_sat(fmaf(s0, -eu_cs, vf.x * eu_cv), fmaf(s1, -eu_cs, vf.y * eu_cv));   // nmf.py:62-63
+            } else {
+              const float x0 = fmaf(s0, c1, c2), x1 = fmaf(s1, c1, c2);     // (WH + eps) in the scale of V~ / P~
+              if constexpr (FOLD) {                                          // metrics.py:22 on the same S tile
+                la = fmaf(vf.x, __log2f(fmaf(s0, c1l, kEps)), la);
+                la = fmaf(vf.y, __log2f(fmaf(s1, c1l, kEps)), la);
+                lb += s0 + s1;
+              }
+              pa[ai] = ptx::pack_f16x2_sat(fmaf(vf.x, ptx::rcp_approx(x0), negpc),    // nmf.py:65, centred
+                                           fmaf(vf.y, ptx::rcp_approx(x1), negpc));
             }
-            ptx::tmem_st16(tmem + lane_addr + kColS + st * TN + g * (TN / NRW) + c4r * 16, pn);   // own S columns, see above
-            ptx::tmem_st16(tmem + lane_addr + kColPp + st * 64 + c4 * 16, pp);
           }
         }
+        if (LOSS || FOLD) { accA += (double)la; accB += (double)lb; }
+        if constexpr (!LOSS) {
+          // ---- O += P G over the same 64 columns: B = G step as [K = 16 c-rows][N = RP] MN-major, 8-row groups 1024 B
+          //      apart, 64-wide column blocks one sub-block (TN x 128 B) apart; split: hi and lo halves into the same O
+          ptx::wgmma_fence();
+#pragma unroll
+          for (int kk = 0; kk < kStep / 16; ++kk) {
+            const uint32_t a[4] = {pa[4 * kk], pa[4 * kk + 1], pa[4 * kk + 2], pa[4 * kk + 3]};
+#pragma unroll
+            for (int half = 0; half < (SPLIT ? 2 : 1); ++half) {
+              const uint32_t gb = sG + half * (RP / 64) * (TN * 128) + st * (kStep * 128) + kk * (16 * 128);
+              const uint64_t db = ptx::gmma_desc_sw128(gb, TN * 128, 1024);
+              if constexpr (RP == 64) ptx::wgmma_rs_m64n64_tb(o, a, db);
+              else ptx::wgmma_rs_m64n128_tb(o, a, db);
+            }
+            if constexpr (TWO) {
+              const uint32_t a2[4] = {pp[4 * kk], pp[4 * kk + 1], pp[4 * kk + 2], pp[4 * kk + 3]};
+              const uint32_t gb = sG + st * (kStep * 128) + kk * (16 * 128);
+              ptx::wgmma_rs_m64n64_tb(o2, a2, ptx::gmma_desc_sw128(gb, TN * 128, 1024));
+            }
+          }
+          ptx::wgmma_commit();
+          ptx::wgmma_wait<0>();
+          ptx::fence_regs(o);
+          ptx::fence_regs(o2);
         }
-        if (!LOSS) ptx::tc_wait_st();
-        ptx::tc_fence_before();
-        __syncwarp();
-        if (lane == 0) {
-          ptx::mbar_arrive(BAR(B_PFULL + st));
-          ptx::mbar_arrive(BAR(B_VEMPTY + s));
-        }
-        if (q == 0 && lane == 0) TC_TRACE(tt, 9);
       }
-      t += n;
-    }
-    }   // LOSS and two-output kernels
-    if (LOSS || FOLD) {
-      for (int o = 16; o > 0; o >>= 1) {
-        accA += __shfl_xor_sync(0xffffffffu, accA, o);
-        accB += __shfl_xor_sync(0xffffffffu, accB, o);
-      }
-      if (lane == 0) { loss_slots[2 * warp] = accA; loss_slots[2 * warp + 1] = accB; }
-    }
-  } else if (warp >= kEpiWarp0 && warp < kCtl0 && !LOSS) {
-    // =========================== epilogue warpgroup =====================
-    const int q = warp & 3;
-    const int row = q * 32 + lane;
-    const uint32_t lane_addr = (uint32_t)(q * 32) << 16;
-    const float oscale = exp2f(-(float)(p.exps[p.eg] + p.exps[(TWO || EU) ? 4 : 3]));      // O = sum (P 2^p) (G 2^eg)
-    const float oscale2 = TWO ? exp2f(-(float)(p.exps[p.eg] + p.exps[5])) : 0.f;
-    uint32_t it = 0;
-    for (int item = blockIdx.x; item < total_items; item += gridDim.x, ++it) {
-      const int rb = item % p.row_blocks, chunk = item / p.row_blocks;
-      if (lane == 0) ptx::mbar_wait(BAR(B_OFULL), it & 1);      // one polling lane per warp
+      // every read of this stage has completed (wgmma.wait, ld.shared results consumed): hand it back
       __syncwarp();
-      ptx::tc_fence_after();
-      const int64_t grow = (int64_t)rb * kTileM + row;
-      float* dst = p.part + (int64_t)chunk * p.chunk_stride + grow * p.ldp;
-      if (TWO) {
-        // numerator then denominator accumulator (64 columns each); O is handed back after the last TMEM load
-        float* dst2 = p.part2 + (int64_t)chunk * p.chunk_stride + grow * p.ldp;
+      if (lane == 0) ptx::mbar_arrive(BAR(B_EMPTY + s));
+    }
+    __syncwarp();
+    if (lane == 0) ptx::mbar_arrive(BAR(B_FEMPTY));
+    if constexpr (!LOSS) {
+      // ---- epilogue: the item's partial numerators (and denominators) of its 64 rows
 #pragma unroll
-        for (int half = 0; half < 2; ++half) {
-          float o[64];
+      for (int h = 0; h < 2; ++h) {
+        const int64_t grow = (int64_t)rb * kTileM + r0 + 8 * h;
+        if (grow >= p.Mr) continue;
+        float* dst = p.part + (int64_t)chunk * p.chunk_stride + grow * p.ldp + 2 * c4;
 #pragma unroll
-          for (int c = 0; c < 2; ++c) {
-            uint32_t raw[32];
-            ptx::tmem_ld32(tmem + lane_addr + (half ? kColO2 : kColO) + c * 32, raw);
-            ptx::tc_wait_ld();
+        for (int jn = 0; jn < RP / 8; ++jn)
+          *reinterpret_cast<float2*>(dst + 8 * jn) = make_float2(o[4 * jn + 2 * h] * oscale, o[4 * jn + 2 * h + 1] * oscale);
+        if constexpr (TWO) {
+          float* dst2 = p.part2 + (int64_t)chunk * p.chunk_stride + grow * p.ldp + 2 * c4;
 #pragma unroll
-            for (int i = 0; i < 32; ++i) o[c * 32 + i] = __uint_as_float(raw[i]) * (half ? oscale2 : oscale);
-          }
-          if (half == 1) { ptx::tc_fence_before(); __syncwarp(); if (lane == 0) ptx::mbar_arrive(BAR(B_OEMPTY)); }
-          if (grow < p.Mr) {
-            float* d = half ? dst2 : dst;
-#pragma unroll
-            for (int i = 0; i < 64; i += 4) *reinterpret_cast<float4*>(d + i) = make_float4(o[i], o[i + 1], o[i + 2], o[i + 3]);
-          }
-        }
-        continue;
-      }
-      if (RP == 64) {
-        // whole O row (64 values) into registers, hand the accumulator back to the MMA warp, then store
-        float o[64];
-#pragma unroll
-        for (int c = 0; c < 2; ++c) {
-          uint32_t hi[32];
-          ptx::tmem_ld32(tmem + lane_addr + kColO + c * 32, hi);
-          if (SPLIT) {
-            uint32_t lo[32];
-            ptx::tmem_ld32(tmem + lane_addr + kColO + RP + c * 32, lo);
-            ptx::tc_wait_ld();
-#pragma unroll
-            for (int i = 0; i < 32; ++i) o[c * 32 + i] = (__uint_as_float(hi[i]) + __uint_as_float(lo[i])) * oscale;
-          } else {
-            ptx::tc_wait_ld();
-#pragma unroll
-            for (int i = 0; i < 32; ++i) o[c * 32 + i] = __uint_as_float(hi[i]) * oscale;
-          }
-        }
-        ptx::tc_fence_before();
-        __syncwarp();
-        if (lane == 0) ptx::mbar_arrive(BAR(B_OEMPTY));
-        // Each lane owns a row, so one store instruction touches 32 cache lines = 32 passes through the load/store unit
-        // that the ratio warps' shared-memory loads (and every other memory instruction of the SM) queue behind: issued
-        // back to back, the 64 stores of an item stopped the whole SM for ~2300 cycles at every item boundary (per-tile
-        // trace: 9 % of the launch).  Nothing waits for these stores (the next epilogue is 16 tiles away): pace them.
-        if (grow < p.Mr) {
-#pragma unroll
-          for (int i = 0; i < 64; i += 8) {          // 256-bit stores: half the instructions, half the passes
-            asm volatile("st.global.v8.f32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};"
-                         ::"l"(dst + i), "f"(o[i]), "f"(o[i + 1]), "f"(o[i + 2]), "f"(o[i + 3]), "f"(o[i + 4]), "f"(o[i + 5]),
-                           "f"(o[i + 6]), "f"(o[i + 7]) : "memory");
-            __nanosleep(kEpiPaceNs);
-          }
-        }
-        continue;
-      }
-#pragma unroll
-      for (int c = 0; c < RP / 32; ++c) {
-        uint32_t hi[32];
-        ptx::tmem_ld32(tmem + lane_addr + kColO + c * 32, hi);
-        float o[32];
-        if (SPLIT) {
-          uint32_t lo[32];
-          ptx::tmem_ld32(tmem + lane_addr + kColO + RP + c * 32, lo);
-          ptx::tc_wait_ld();
-#pragma unroll
-          for (int i = 0; i < 32; ++i) o[i] = (__uint_as_float(hi[i]) + __uint_as_float(lo[i])) * oscale;
-        } else {
-          ptx::tc_wait_ld();
-#pragma unroll
-          for (int i = 0; i < 32; ++i) o[i] = __uint_as_float(hi[i]) * oscale;
-        }
-        if (grow < p.Mr) {
-#pragma unroll
-          for (int i = 0; i < 32; i += 4)
-            *reinterpret_cast<float4*>(dst + c * 32 + i) = make_float4(o[i], o[i + 1], o[i + 2], o[i + 3]);
+          for (int jn = 0; jn < 8; ++jn)
+            *reinterpret_cast<float2*>(dst2 + 8 * jn) =
+                make_float2(o2[4 * jn + 2 * h] * oscale2, o2[4 * jn + 2 * h + 1] * oscale2);
         }
       }
-      ptx::tc_fence_before();
-      __syncwarp();
-      if (lane == 0) ptx::mbar_arrive(BAR(B_OEMPTY));
     }
   }
-
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == kCtl0 + 1) ptx::tmem_dealloc(tmem, kTmemCols);
-  if ((LOSS || FOLD) && threadIdx.x == (kCtl0 + 3) * 32) {          // fixed-order sum of the 8 ratio warps
-    double a = 0.0, b = 0.0;
-    for (int w = 0; w < 4 * NRW; ++w) { a += loss_slots[2 * w]; b += loss_slots[2 * w + 1]; }
-    p.loss_part[2 * blockIdx.x] = a;
-    p.loss_part[2 * blockIdx.x + 1] = b;
+  if constexpr (LOSS || FOLD) {
+    for (int off = 16; off > 0; off >>= 1) {
+      accA += __shfl_xor_sync(0xffffffffu, accA, off);
+      accB += __shfl_xor_sync(0xffffffffu, accB, off);
+    }
+    if (lane == 0) { loss_slots[2 * cwarp] = accA; loss_slots[2 * cwarp + 1] = accB; }
+    asm volatile("bar.sync 1, 256;" ::: "memory");           // the two consumer warpgroups only
+    if (threadIdx.x == 128) {                                 // fixed-order sum of the 8 consumer warps
+      double a = 0.0, b = 0.0;
+      for (int w = 0; w < 8; ++w) { a += loss_slots[2 * w]; b += loss_slots[2 * w + 1]; }
+      p.loss_part[2 * blockIdx.x] = a;
+      p.loss_part[2 * blockIdx.x + 1] = b;
+    }
   }
 }
 
@@ -1772,7 +1295,7 @@ struct TcState {
   int peer_world = 0, peer_rank = 0;
   unsigned int peer_iter = 0;
   int64_t peer_buf_floats = 0;
-  int device = 0, num_sms = 148;
+  int device = 0, num_sms = 132;
   int64_t N = 0, C = 0, R = 0;
   bool split = true;
   int Rp = 64;                      // padded rank: 64 or 128
@@ -1816,21 +1339,13 @@ struct TcState {
   cudaStream_t gstream = nullptr;   // capture / replay stream (the caller's may be the legacy default stream, which cannot capture)
   cudaEvent_t gev_in = nullptr, gev_out = nullptr;
   bool dirty_w = true, dirty_h = true, has_target = false;
-  // Environment knobs, read once in tc_create.  Product build: NMFB200_CENTER=0 (diagnostic: kappa centring off, see
-  // tools/bias_probe.py), NMFB200_GRAPH=1 (CUDA-graph replay of tc_iterate), NMFB200_TC_CHECK=1 (watchdog check after
-  // every tc_contract_only).  Tuning build (-DNMFB200_TRACE) only: NMFB200_TC_VARIANT, NMFB200_TC_PF, NMFB200_TC_KNOCK,
-  // NMFB200_TC_PARK, NMFB200_TC_TRACE=<file>.
+  // Environment knobs, read once in tc_create: NMFB200_CENTER=0 (diagnostic: kappa centring off), NMFB200_GRAPH=1
+  // (CUDA-graph replay of tc_iterate), NMFB200_TC_CHECK=1 (watchdog check after every tc_contract_only).
   int center = 1;
   bool use_graph = false, check_each = false;
-  int pf_dist = 0;                  // L2 prefetch distance of the V stream in tiles (measured: no gain; 0 = off)
-  int variant = 0;                  // pipeline configuration variant
-  int knock = 0;                    // knock-out mask (tools/tc_knock.py)
-  long long* trace = nullptr;       // event timestamps of CTA 0 (tools/tc_trace.py)
-  std::string trace_path;
   float* kappa = nullptr;           // device scalar
   float* zero = nullptr;            // device scalar 0 (kappa of an already complete numerator)
   int coop_blocks = 0;              // co-resident blocks of the fused tail kernel (cooperative launch), 0 = unavailable
-  bool psep = false;                // R <= 64 f16 kernel: P buffers of their own (NMFB200_TC_PSEP=1; staged, see DESIGN.md)
   bool fused_tail = false;          // ratio stage + operand refresh in one cooperative kernel (NMFB200_FUSED_TAIL=0: two kernels)
 };
 
@@ -1863,7 +1378,7 @@ void tc_destroy(TcState* s) {
   if (s->gev_out) cudaEventDestroy(s->gev_out);
   cudaFree(s->V16); cudaFree(s->Vt16); cudaFree(s->W16); cudaFree(s->H16); cudaFree(s->part); cudaFree(s->part2); cudaFree(s->gram); cudaFree(s->gram_part);
   cudaFree(s->colsum); cudaFree(s->cs_part); cudaFree(s->cs_super); cudaFree(s->ticket); cudaFree(s->absmax); cudaFree(s->exps);
-  cudaFree(s->vpart); cudaFree(s->vconst); cudaFree(s->vlossy); cudaFree(s->loss_part); cudaFree(s->vbeta); cudaFree(s->vbeta_part); cudaFree(s->kappa); cudaFree(s->zero); cudaFree(s->trace);
+  cudaFree(s->vpart); cudaFree(s->vconst); cudaFree(s->vlossy); cudaFree(s->loss_part); cudaFree(s->vbeta); cudaFree(s->vbeta_part); cudaFree(s->kappa); cudaFree(s->zero);
   delete s;
 }
 
@@ -1873,31 +1388,16 @@ int tc_create(TcState** out, int device, int64_t N, int64_t C, int64_t R, bool s
   s->device = device; s->N = N; s->C = C; s->R = R; s->split = split;
   s->Rp = R <= 64 ? 64 : 128;
   s->KW = split ? 2 * s->Rp : s->Rp;
-  s->TN = (split && s->Rp == 128) ? 64 : 128;   // 64-column tiles only where 128 do not fit (measured slower: MMA issue rate)
+  s->TN = (split && s->Rp == 128) ? 64 : 128;   // 64-column tiles where two 128-column stages do not fit next to the F block
   if (const char* e = getenv("NMFB200_CENTER")) s->center = atoi(e);
   s->use_graph = getenv("NMFB200_GRAPH") != nullptr;
   s->check_each = getenv("NMFB200_TC_CHECK") != nullptr;
-  if (const char* e = getenv("NMFB200_TC_PSEP")) s->psep = atoi(e) != 0;
-#ifdef NMFB200_TRACE
-  if (const char* e = getenv("NMFB200_TC_VARIANT")) s->variant = atoi(e);
-  if (const char* e = getenv("NMFB200_TC_PF")) s->pf_dist = atoi(e);
-  if (const char* e = getenv("NMFB200_TC_KNOCK")) s->knock = atoi(e);
-  {
-    const unsigned int park = getenv("NMFB200_TC_PARK") ? (unsigned)atoi(getenv("NMFB200_TC_PARK")) : 0u;   // default: parked polls; 2 = plain poll loop; > 2 = nanosleep(n) back-off
-    cudaMemcpyToSymbol(ptx::g_tune_park, &park, sizeof(park));
-  }
-  if (const char* e = getenv("NMFB200_TC_TRACE")) {
-    s->trace_path = e;
-    if (cudaMalloc(&s->trace, 256 * 16 * sizeof(long long)) != cudaSuccess) s->trace = nullptr;
-  }
-#endif
   s->ldc = round_up(C, 8);
   s->ldn = round_up(N, 8);
   cudaDeviceProp prop;
   NMF_CUDA_CHECK(cudaGetDeviceProperties(&prop, device));
   s->num_sms = prop.multiProcessorCount;
-  if (prop.major != 10) { delete s; set_error("the tensor-core path needs an sm_100 device"); return 1; }
-  if (s->variant == 1 && split && s->Rp == 64) s->TN = 64;
+  if (prop.major != 9) { delete s; set_error("the tensor-core path needs an sm_90 device"); return 1; }
   {
     int coop = 0, per_sm = 0;
     cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, device);
@@ -2128,7 +1628,7 @@ int ensure_synced(TcState* s, const float* W, const float* H, double beta, cudaS
 
 template <class C, int BM, bool LOSS, bool FOLD = false>
 int launch_contract_t(TcState* s, int which, double beta, cudaStream_t st) {
-  using L = SmemLayout<C::KW, C::TN, C::NF, C::NG, C::NV, C::NS, C::NP>;
+  using L = SmemLayout<C::KW, C::TN>;
   static_assert(L::kTotal + 1024 <= 232448, "shared memory budget (227 KB)");
   auto kern = tc_contract_kernel<C, BM, LOSS, FOLD>;
   if (!LOSS) s->w_pending = false;       // every update contraction overwrites the partial numerators
@@ -2151,51 +1651,27 @@ int launch_contract_t(TcState* s, int which, double beta, cudaStream_t st) {
   p.eg = which == 0 ? 2 : 1;
   p.loss_part = s->loss_part;
   p.kappa = s->kappa;
-  p.trace = s->trace;
-  p.knock = s->knock;
-  p.pf_dist = s->pf_dist;
-  if (s->trace) cudaMemsetAsync(s->trace, 0, 256 * 16 * sizeof(long long), st);
   const int items = pl.row_blocks * pl.nchunks;
   const int grid = items < s->num_sms ? items : s->num_sms;
   if (which == 0)
-    kern<<<grid, C::kThreads, smem, st>>>(s->tmWf, s->tmHg, s->tmVt, p);
+    kern<<<grid, kThreads, smem, st>>>(s->tmWf, s->tmHg, s->tmVt, p);
   else
-    kern<<<grid, C::kThreads, smem, st>>>(s->tmHf, s->tmWg, s->tmV, p);
+    kern<<<grid, kThreads, smem, st>>>(s->tmHf, s->tmWg, s->tmV, p);
   NMF_LAUNCH_CHECK();
   return grid;
 }
 
-// Kernel configurations <RP, SPLIT, TN, NF, NG, NV, NS> (224 KB of shared memory each).  Tuning notes in
-// profiles/README.md and DESIGN.md 4.1: the V ring must keep >= 3 tiles (>= 64 KB) in flight to cover HBM latency, the G
-// ring needs >= 4 stages (a G tile stays resident from its S-MMA to its O-MMA); deeper G rings (5, 6) changed nothing.
-using CfgFast64 = Cfg<64, false, 128, 2, 4, 4, 2, 2, 3>;   // F 2x16 | G 4x16 | V 4x32 KB ; TMEM S 2x128 + P 3x64 + O 64
-using CfgFast64A = Cfg<64, false, 128, 2, 4, 4, 3, 2>;     // round-1 layout (P over S, 3 stages): NMFB200_TC_PSEP=0, A/B only
-using CfgSplit64 = Cfg<64, true, 128, 1, 3, 3, 3>;       // F 32 | G 3x32 | V 3x32 KB     ; TMEM 3x128 + 128
-using CfgSplit64N = Cfg<64, true, 64, 1, 6, 6, 4>;       // (variant 1) 64-column tiles, deeper rings: slower
-using CfgFast128 = Cfg<128, false, 128, 1, 3, 3, 3>;     // F 32 | G 3x32 | V 3x32 KB     ; TMEM 3x128 + 128
-using CfgSplit128 = Cfg<128, true, 64, 1, 3, 4, 4>;      // F 64 | G 3x32 | V 4x16 KB     ; TMEM 4x64 + 256
-
-#ifdef NMFB200_TRACE    // tuning build: ring-depth experiments (NMFB200_TC_VARIANT = 4, 5, 6)
-using CfgFast64V4 = Cfg<64, false, 128, 1, 5, 4, 3>;
-using CfgFast64V5 = Cfg<64, false, 128, 1, 6, 3, 3>;
-using CfgFast64V6 = Cfg<64, false, 128, 1, 3, 5, 3>;
-#endif
-using CfgTwo64 = Cfg<64, false, 128, 2, 3, 4, 2>;        // beta != 1: F 2x16 | G 3x16 | V 4x32 KB ; TMEM 2x128 + 128 + 2x64
+// Kernel configurations <RP, SPLIT, TN>; the stage count follows from the shared-memory budget (SmemLayout::NS).
+using CfgFast64 = Cfg<64, false, 128>;       // F 16 KB | 4 stages x (G 16 + V 32 KB)
+using CfgSplit64 = Cfg<64, true, 128>;       // F 32 KB | 3 stages x (G 32 + V 32 KB)
+using CfgFast128 = Cfg<128, false, 128>;     // F 32 KB | 3 stages x (G 32 + V 32 KB)
+using CfgSplit128 = Cfg<128, true, 64>;      // F 64 KB | 3 stages x (G 32 + V 16 KB)
 
 // one-output kernels (beta 1: BM = kBmKL, beta 2: BM = kBmEU) over the configuration of this context
 template <int BM>
 int launch_contract_one(TcState* s, int which, double beta, cudaStream_t st) {
-#ifdef NMFB200_TRACE
-  if (s->Rp == 64 && BM == kBmKL && !s->split) {
-    if (s->variant == 4) return launch_contract_t<CfgFast64V4, BM, false>(s, which, beta, st);
-    if (s->variant == 5) return launch_contract_t<CfgFast64V5, BM, false>(s, which, beta, st);
-    if (s->variant == 6) return launch_contract_t<CfgFast64V6, BM, false>(s, which, beta, st);
-  }
-#endif
   if (s->Rp == 64) {
-    if (!s->split && !s->psep) return launch_contract_t<CfgFast64A, BM, false>(s, which, beta, st);
     if (!s->split) return launch_contract_t<CfgFast64, BM, false>(s, which, beta, st);
-    if (s->TN == 64) return launch_contract_t<CfgSplit64N, BM, false>(s, which, beta, st);
     return launch_contract_t<CfgSplit64, BM, false>(s, which, beta, st);
   }
   if (!s->split) return launch_contract_t<CfgFast128, BM, false>(s, which, beta, st);
@@ -2204,10 +1680,7 @@ int launch_contract_one(TcState* s, int which, double beta, cudaStream_t st) {
 
 // beta 1, W orientation, loss sums folded in (fast, non-split configurations)
 int launch_contract_w_fold(TcState* s, cudaStream_t st) {
-  if (s->Rp == 64) {
-    if (!s->psep) return launch_contract_t<CfgFast64A, kBmKL, false, true>(s, 0, 1.0, st);
-    return launch_contract_t<CfgFast64, kBmKL, false, true>(s, 0, 1.0, st);
-  }
+  if (s->Rp == 64) return launch_contract_t<CfgFast64, kBmKL, false, true>(s, 0, 1.0, st);
   return launch_contract_t<CfgFast128, kBmKL, false, true>(s, 0, 1.0, st);
 }
 
@@ -2215,7 +1688,6 @@ template <int BM>
 int launch_loss_bm(TcState* s, double beta, cudaStream_t st) {
   if (s->Rp == 64) {
     if (!s->split) return launch_contract_t<CfgFast64, BM, true>(s, 1, beta, st);
-    if (s->TN == 64) return launch_contract_t<CfgSplit64N, BM, true>(s, 1, beta, st);
     return launch_contract_t<CfgSplit64, BM, true>(s, 1, beta, st);
   }
   if (!s->split) return launch_contract_t<CfgFast128, BM, true>(s, 1, beta, st);
@@ -2226,10 +1698,10 @@ int launch_loss_bm(TcState* s, double beta, cudaStream_t st) {
 int launch_contract_two(TcState* s, int which, double beta, cudaStream_t st) {
   if (!s->part2) NMF_CUDA_CHECK(cudaMalloc(&s->part2, (size_t)s->part_floats * 4));
   int g;
-  if (beta == 0.0) g = launch_contract_t<CfgTwo64, kBmIS, false>(s, which, beta, st);
-  else if (beta == 0.5) g = launch_contract_t<CfgTwo64, kBm05, false>(s, which, beta, st);
-  else if (beta == 1.5) g = launch_contract_t<CfgTwo64, kBm15, false>(s, which, beta, st);
-  else g = launch_contract_t<CfgTwo64, kBmGen, false>(s, which, beta, st);
+  if (beta == 0.0) g = launch_contract_t<CfgFast64, kBmIS, false>(s, which, beta, st);
+  else if (beta == 0.5) g = launch_contract_t<CfgFast64, kBm05, false>(s, which, beta, st);
+  else if (beta == 1.5) g = launch_contract_t<CfgFast64, kBm15, false>(s, which, beta, st);
+  else g = launch_contract_t<CfgFast64, kBmGen, false>(s, which, beta, st);
   return g > 0 ? 0 : 2;
 }
 
@@ -2272,8 +1744,8 @@ int tc_iterate(TcState* s, float* W, float* H, double beta, double gamma, double
     s->gW = W; s->gH = H; s->gargs[0] = beta; s->gargs[1] = gamma; s->gargs[2] = l1; s->gargs[3] = l2;
   }
   // CUDA-graph replay of the iteration is opt-in (NMFB200_GRAPH=1): measured no gain at cfg2 -- the stream is never
-  // launch-bound (profiles/README.md) -- so the default keeps plain stream-ordered launches.
-  const bool use_graph = s->use_graph && s->trace == nullptr;
+  // launch-bound -- so the default keeps plain stream-ordered launches.
+  const bool use_graph = s->use_graph;
   cudaStream_t user = st;
   if (use_graph) {
     // run on an engine-owned stream, fenced against the caller's stream with events
@@ -2473,23 +1945,11 @@ int tc_contract_only(TcState* s, const float* W, const float* H, int which, doub
   if (rc == 0 && s->check_each) {
     if (tc_check_wait_abort(st) > 0) { set_error("mbarrier wait aborted (protocol bug)"); return 2; }
   }
-  if (rc == 0 && s->trace) {
-    std::vector<long long> h(256 * 16);
-    cudaMemcpyAsync(h.data(), s->trace, h.size() * sizeof(long long), cudaMemcpyDeviceToHost, st);
-    cudaStreamSynchronize(st);
-    if (FILE* f = fopen(s->trace_path.c_str(), "w")) {
-      for (int t = 0; t < 256; ++t) {
-        for (int k = 0; k < 16; ++k) fprintf(f, "%lld ", h[t * 16 + k]);
-        fprintf(f, "\n");
-      }
-      fclose(f);
-    }
-  }
   return rc;
 }
 
 bool tc_supports_loss_prefetch(const TcState* s, double beta) {
-  return beta == 1.0 && !s->split && s->trace == nullptr;
+  return beta == 1.0 && !s->split;
 }
 
 // The loss at the current factors from the W update's own contraction (beta 1): one pass over V yields both the loss sums and

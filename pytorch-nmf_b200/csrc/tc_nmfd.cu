@@ -1,4 +1,4 @@
-// NMFD (1-D convolutive NMF, nmf.py:776-779) on tcgen05 tensor cores for beta = 1: the three contractions of an update as
+// NMFD (1-D convolutive NMF, nmf.py:776-779) on Hopper tensor cores (wgmma) for beta = 1: the three contractions of an update as
 // im2col-free SLIDING GEMMs.
 //
 //   recon : S[c, l]     = sum_{r,t} W[c,r,t] H[r, l-t]           then the ratio epilogue  P~ = (V / (S + eps) - kappa) 2^p  (fp16)
@@ -9,11 +9,12 @@
 // matrix: row i of a 128 x 64 tile is the 64-element window of ONE fp16 vector (a padded row of H, or a row of P~) that
 // starts one element further than row i - 1 (recon, dgrad) or one element earlier (wgrad).  Nothing of that matrix ever
 // exists in global memory: per k-block the TMA warp bulk-copies the ~200-element source window into shared memory and
-// the eight producer warps write the 128 x 64 tile from it in the UMMA SWIZZLE_128B K-major layout (4-byte shared loads,
-// one byte-permute per word for odd shifts, 16-byte stores), 2 threads per row.  The MMA warp issues tcgen05.mma SS on
-// it exactly as on a TMA-written tile; accumulators live in TMEM; the epilogue warps read them back with tcgen05.ld.
+// the eight producer warps write the 128 x 64 tile from it in the SWIZZLE_128B K-major layout (4-byte shared loads,
+// one byte-permute per word for odd shifts, 16-byte stores), 2 threads per row.  The same eight warps then issue wgmma SS
+// on it exactly as on a TMA-written tile, 64 rows per warpgroup, with the accumulators in registers; after the k loop they
+// are staged through shared memory as fp32 rows for the epilogue warps.
 //
-// Precision design = the NMF kernel's (DESIGN.md 4.2): fp16 operands with power-of-two scales, fp32 accumulation, the
+// Precision design = the NMF kernel's: fp16 operands with power-of-two scales, fp32 accumulation, the
 // ratio tile centred on kappa = sum(V) / sum(WH) so that the K = 8192 ... 131200-term numerator sums are signed and small
 // (tensor-core accumulation truncates), kappa * colsum added back in fp32 by the ratio stage (apply_update).
 #include "tc_nmfd.cuh"
@@ -25,17 +26,17 @@
 #include <cstdlib>
 #include <string>
 
-#include "sm100_ptx.cuh"
+#include "sm90_ptx.cuh"
 
 namespace nmfb200 {
 
 namespace {
 
-constexpr int kM = 128;            // tile rows (TMEM lanes)
+constexpr int kM = 128;            // tile rows (two wgmma warpgroups of 64)
 constexpr int kKB = 64;            // k-block: 64 fp16 = one 128-byte swizzle row
 constexpr int kStages = 3;
 constexpr int kWinHalfs = 256;     // source window per k-block: 128 rows + 64 columns + alignment slack (512 bytes)
-constexpr int kThreads = 384;      // warp 0 TMA | warp 1 MMA | warps 2-3 idle | warps 4-11 producers (8-11 also epilogue)
+constexpr int kThreads = 384;      // warp 0 TMA | warps 1-3 idle | warps 4-11 producers + MMA (8-11 also epilogue)
 
 enum : int { kRecon = 0, kReconLoss = 1, kWgrad = 2, kDgrad = 3 };
 
@@ -53,6 +54,7 @@ struct NmfdTcParams {
   float* out;                     // wgrad: [nsplit][C][R][T]   dgrad: [nsplit][B][R][Lin]
   double* loss_part;              // recon loss: one partial per CTA
   int nsplit, kb_per_split;
+  int r_off;                      // dgrad: first component of this launch (components [r_off, r_off + 128))
 };
 
 struct Smem {
@@ -65,6 +67,9 @@ struct Smem {
   static constexpr int kTmemPtr = kBar + 8 * kNumBars;
   static constexpr int kRed = kTmemPtr + 16;
   static constexpr int kTotal = kRed + 8 * 16;
+  // after the k loop the accumulators are staged through [0, kWin) as fp32 rows of up to 128 columns
+  static constexpr int kAccPitch = 132;
+  static_assert(kM * kAccPitch * 4 <= kWin, "accumulator staging");
 };
 
 __device__ __forceinline__ void bulk_copy_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
@@ -76,9 +81,10 @@ __device__ __forceinline__ void bulk_copy_g2s(uint32_t dst, const void* src, uin
 // One kernel, four roles of the same pipeline (KIND):
 //   recon / recon-loss : grid (L tiles, C tiles, B);  plain = A = Wr16 tile (rows c), Toeplitz = B (rows l), N = 128
 //   wgrad              : grid (C tiles, R, nsplit);   plain = A = P16 tile (rows c),  Toeplitz = B (rows t), N = 128
-//   dgrad              : grid (Lin tiles, nsplit, B); Toeplitz = A (rows j), plain = B = Wf16 rows (c R + r), N = Rp16
+//   dgrad              : grid (Lin tiles, nsplit, B); Toeplitz = A (rows j), plain = B = Wf16 rows (c R + r_off + n), N = 128;
+//                        ranks above 128 take one launch per 128 components
 template <int KIND>
-__global__ void __launch_bounds__(kThreads, 2)
+__global__ void __launch_bounds__(kThreads, 1)
 tcnmfd_kernel(const __grid_constant__ CUtensorMap tmPlain, const NmfdTcParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   const uint32_t raw32 = ptx::smem_u32(smem_raw);
@@ -86,32 +92,22 @@ tcnmfd_kernel(const __grid_constant__ CUtensorMap tmPlain, const NmfdTcParams p)
   uint8_t* smem_al = smem_raw + (sbase - raw32);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   auto BAR = [&](int i) { return sbase + Smem::kBar + 8u * i; };
-  constexpr int B_WIN = 0, B_TILE = kStages, B_EMPTY = 2 * kStages, B_WREAD = 3 * kStages, B_ACC = 4 * kStages;
-  volatile uint32_t* tmem_ptr_smem = reinterpret_cast<volatile uint32_t*>(smem_al + Smem::kTmemPtr);
+  constexpr int B_WIN = 0, B_TILE = kStages, B_EMPTY = 2 * kStages, B_WREAD = 3 * kStages;
   constexpr bool RECON = KIND == kRecon || KIND == kReconLoss;
-  const int Rp16 = (p.R + 15) & ~15;
-  const uint32_t ncols = KIND == kDgrad ? (Rp16 <= 32 ? 32u : (Rp16 <= 64 ? 64u : (Rp16 <= 128 ? 128u : 256u))) : 128u;
+  const int Rb = min((p.R + 15) & ~15, 128);     // dgrad: B-tile rows loaded per k-block
 
   if (warp == 0 && lane == 0) {
     ptx::prefetch_tmap(&tmPlain);
     for (int i = 0; i < kStages; ++i) {
       ptx::mbar_init(BAR(B_WIN + i), 1);
       ptx::mbar_init(BAR(B_TILE + i), 8);        // one arrival per producer warp
-      ptx::mbar_init(BAR(B_EMPTY + i), 1);
+      ptx::mbar_init(BAR(B_EMPTY + i), 8);       // the MMAs of both warpgroups have completed
       ptx::mbar_init(BAR(B_WREAD + i), 8);       // the 8 producer warps have read the source window of this stage
     }
-    ptx::mbar_init(BAR(B_ACC), 1);
     ptx::fence_barrier_init();
     ptx::fence_proxy_async();
   }
-  if (warp == 1) {
-    ptx::tmem_alloc(sbase + Smem::kTmemPtr, ncols);
-    ptx::tmem_relinquish();
-  }
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem = *tmem_ptr_smem;
 
   // ---- what this CTA computes, as a list of k-blocks: (plain-tile coordinates, source vector, window start) -------------
   int nkb, kb0 = 0;
@@ -136,7 +132,7 @@ tcnmfd_kernel(const __grid_constant__ CUtensorMap tmPlain, const NmfdTcParams p)
       e0 = p.padl + lk * kKB;                               // row t reads H[l - t]: e0 - t
     } else {
       const int g = kb0 + kb, c = g / tkb, kk = g - c * tkb;
-      px = kk * kKB; py = c * p.R;
+      px = kk * kKB; py = c * p.R + p.r_off;
       src = p.P16 + ((int64_t)blockIdx.z * p.C + c) * p.Lq;
       e0 = blockIdx.x * kM + kk * kKB;                      // row j reads P[j + t]
     }
@@ -154,42 +150,23 @@ tcnmfd_kernel(const __grid_constant__ CUtensorMap tmPlain, const NmfdTcParams p)
         ptx::mbar_wait(BAR(B_WREAD + s), ph ^ 1);      // ... and every producer warp has read its source window
         int px, py, e0; const __half* src;
         kblock(kb, px, py, src, e0);
-        const uint32_t plain_bytes = KIND == kDgrad ? (uint32_t)Rp16 * kKB * 2 : (uint32_t)Smem::kTile;
+        const uint32_t plain_bytes = KIND == kDgrad ? (uint32_t)Rb * kKB * 2 : (uint32_t)Smem::kTile;
         ptx::mbar_expect_tx(BAR(B_WIN + s), plain_bytes + kWinHalfs * 2);
         ptx::tma_load_2d(&tmPlain, BAR(B_WIN + s), sbase + Smem::kPlain + s * Smem::kTile, px, py);
         bulk_copy_g2s(sbase + Smem::kWin + s * kWinHalfs * 2, src + win_begin(e0), kWinHalfs * 2, BAR(B_WIN + s));
       }
     }
-  } else if (warp == 1) {
-    // =========================== MMA issuer ==========================================================================
-    const uint32_t nmma = KIND == kDgrad ? (uint32_t)Rp16 : 128u;
-    const uint32_t idesc = ptx::idesc_f16(kM, (int)nmma, 0, 0);
-    constexpr uint32_t descHi = ptx::smem_desc_hi_sw128(1024);
-    for (int kb = 0; kb < nkb; ++kb) {
-      const int s = kb % kStages, ph = (kb / kStages) & 1;
-      if (lane == 0) {
-        ptx::mbar_wait(BAR(B_WIN + s), ph);       // plain tile landed (TMA -> this thread)
-        ptx::mbar_wait(BAR(B_TILE + s), ph);      // Toeplitz tile written by the 8 producer warps
-      }
-      __syncwarp();
-      ptx::tc_fence_after();
-      const uint32_t plain = sbase + Smem::kPlain + s * Smem::kTile, toep = sbase + Smem::kToep + s * Smem::kTile;
-      const uint32_t aBase = KIND == kDgrad ? toep : plain, bBase = KIND == kDgrad ? plain : toep;
-      if (ptx::elect_one()) {
-#pragma unroll
-        for (int ks = 0; ks < kKB / 16; ++ks) {
-          const uint32_t alo = ptx::smem_desc_lo(aBase, 16) + 2 * ks, blo = ptx::smem_desc_lo(bBase, 16) + 2 * ks;
-          ptx::mma_ss(tmem, ptx::make_desc(alo, descHi), ptx::make_desc(blo, descHi), idesc, (kb | ks) ? 1u : 0u);
-        }
-        ptx::mma_commit(BAR(B_EMPTY + s));
-        if (kb == nkb - 1) ptx::mma_commit(BAR(B_ACC));
-      }
-      __syncwarp();
-    }
   } else if (warp >= 4) {
     // =========================== Toeplitz producers: 8 warps, 2 threads per tile row ==================================
+    // Then each of the two warpgroups multiplies its 64 rows of the stage: acc[64 x 128] += A[rows] B^T (wgmma SS, the
+    // plain tile by TMA and the Toeplitz tile in the same SWIZZLE_128B K-major layout).  dgrad: N = 128 B-rows of which
+    // the first Rb were loaded; the columns beyond R are never stored.
     const int pt = threadIdx.x - 128;              // 0..255
     const int row = pt >> 1, half = pt & 1;        // this thread writes columns [32 half, 32 half + 32) of its row
+    const int mw = pt >> 7;                        // wgmma warpgroup: tile rows [64 mw, 64 mw + 64)
+    float acc[64];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
     for (int kb = 0; kb < nkb; ++kb) {
       const int s = kb % kStages, ph = (kb / kStages) & 1;
       int px, py, e0; const __half* src;
@@ -215,13 +192,40 @@ tcnmfd_kernel(const __grid_constant__ CUtensorMap tmPlain, const NmfdTcParams p)
       ptx::fence_proxy_async();                    // generic-proxy stores -> visible to the tensor core (async proxy)
       __syncwarp();
       if (lane == 0) { ptx::mbar_arrive(BAR(B_TILE + s)); ptx::mbar_arrive(BAR(B_WREAD + s)); }
+      ptx::mbar_wait(BAR(B_TILE + s), ph);                              // every row of the Toeplitz tile written
+      const uint32_t plain = sbase + Smem::kPlain + s * Smem::kTile, toep = sbase + Smem::kToep + s * Smem::kTile;
+      const uint32_t aBase = (KIND == kDgrad ? toep : plain) + mw * (64 * 128), bBase = KIND == kDgrad ? plain : toep;
+      ptx::wgmma_fence();
+#pragma unroll
+      for (int ks = 0; ks < kKB / 16; ++ks)
+        ptx::wgmma_ss_m64n128(acc, ptx::gmma_desc_sw128(aBase + ks * 32, 16, 1024), ptx::gmma_desc_sw128(bBase + ks * 32, 16, 1024), 1u);
+      ptx::wgmma_commit();
+      ptx::wgmma_wait<0>();
+      ptx::fence_regs(acc);
+      __syncwarp();
+      if (lane == 0) ptx::mbar_arrive(BAR(B_EMPTY + s));
     }
+    // stage the accumulators as fp32 rows (the k loop's tiles are no longer read by anyone once both warpgroups are here)
+    float* stg = reinterpret_cast<float*>(smem_al);
+    asm volatile("bar.sync 2, 256;" ::: "memory");
+    {
+      const int r0 = mw * 64 + (warp & 3) * 16 + (lane >> 2), c0 = 2 * (lane & 3);
+#pragma unroll
+      for (int jn = 0; jn < 16; ++jn)
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+          *reinterpret_cast<float2*>(stg + (r0 + 8 * h) * Smem::kAccPitch + 8 * jn + c0) =
+              make_float2(acc[4 * jn + 2 * h], acc[4 * jn + 2 * h + 1]);
+    }
+    asm volatile("bar.sync 2, 256;" ::: "memory");
     if (warp >= 8) {
-      // =========================== epilogue (warps 8-11 = TMEM lane quarters 0-3) =====================================
+      // =========================== epilogue (warps 8-11: one tile row per thread) =====================================
       const int q = warp & 3, r128 = q * 32 + lane;
-      const uint32_t lane_addr = (uint32_t)(q * 32) << 16;
-      ptx::mbar_wait(BAR(B_ACC), 0);
-      ptx::tc_fence_after();
+      const float* arow = stg + r128 * Smem::kAccPitch;
+      auto ld16 = [&](int j, uint32_t (&sr)[16]) {
+#pragma unroll
+        for (int i = 0; i < 16; ++i) sr[i] = __float_as_uint(arow[j * 16 + i]);
+      };
       const float sc = exp2f(-(float)(p.exps[KIND == kDgrad ? 0 : (RECON ? 0 : 2)] + p.exps[RECON ? 1 : (KIND == kWgrad ? 1 : 2)]));
       if (RECON) {
         const int c = blockIdx.y * kM + r128, b = blockIdx.z, l0 = blockIdx.x * kM;
@@ -233,8 +237,7 @@ tcnmfd_kernel(const __grid_constant__ CUtensorMap tmPlain, const NmfdTcParams p)
 #pragma unroll 1
         for (int j = 0; j < kM / 16; ++j) {
           uint32_t sr[16];
-          ptx::tmem_ld16(tmem + lane_addr + j * 16, sr);
-          ptx::tc_wait_ld();
+          ld16(j, sr);
           const int l = l0 + j * 16;
           float v[16];
 #pragma unroll
@@ -276,8 +279,7 @@ tcnmfd_kernel(const __grid_constant__ CUtensorMap tmPlain, const NmfdTcParams p)
 #pragma unroll 1
         for (int j = 0; j < kM / 16; ++j) {
           uint32_t sr[16];
-          ptx::tmem_ld16(tmem + lane_addr + j * 16, sr);
-          ptx::tc_wait_ld();
+          ld16(j, sr);
           if (c < p.C && j * 16 < p.T) {
             if (vec && j * 16 + 16 <= p.T) {
 #pragma unroll
@@ -294,14 +296,13 @@ tcnmfd_kernel(const __grid_constant__ CUtensorMap tmPlain, const NmfdTcParams p)
       } else {
         const int j = blockIdx.x * kM + r128, b = blockIdx.z;
 #pragma unroll 1
-        for (int jj = 0; jj < Rp16 / 16; ++jj) {
+        for (int jj = 0; jj < Rb / 16; ++jj) {
           uint32_t sr[16];
-          ptx::tmem_ld16(tmem + lane_addr + jj * 16, sr);
-          ptx::tc_wait_ld();
+          ld16(jj, sr);
           if (j < p.Lin) {
 #pragma unroll
             for (int i = 0; i < 16; ++i) {
-              const int r = jj * 16 + i;
+              const int r = p.r_off + jj * 16 + i;
               if (r < p.R) p.out[(((int64_t)blockIdx.y * p.B + b) * p.R + r) * p.Lin + j] = __uint_as_float(sr[i]) * sc;
             }
           }
@@ -309,287 +310,6 @@ tcnmfd_kernel(const __grid_constant__ CUtensorMap tmPlain, const NmfdTcParams p)
       }
     }
   }
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == 1) ptx::tmem_dealloc(tmem, ncols);
-}
-
-// ---- dgrad, second formulation: no Toeplitz tile is built at all ---------------------------------------------------------
-//   gH[r, 8q + s] = sum_c sum_u  P[c, 8q + u] * Ws[c, (r, s), u],      Ws[c, (r, s), u] = W[c, r, u - s]  (0 <= u - s < T)
-// With the output position split as j = 8q + s, the eight phases s move into the SMALL operand (eight shifted copies of W,
-// prepared once per update: N = (r, s) = 128 columns for 16 components), and the rows q of the big operand become windows
-// of P that start 8 elements = 16 BYTES apart: exactly the row pitch of a SWIZZLE_NONE K-major core matrix.  The A operand
-// of tcgen05.mma is therefore the raw fp16 row of P in shared memory, addressed by a descriptor whose core matrices overlap
-// (leading byte offset 16, stride byte offset 128): one 2.4 KB bulk copy per (c, 1024 output positions) instead of a
-// 128 x 64 tile per 64 shifts, and every MMA is a full-rate 128 x 128 x 16.  B = Ws tiles by TMA (SWIZZLE_128B).
-// grid (ceil(Lin / 2048), nsplit over c, B * ngroups);  2 accumulators (2 x 1024 output positions) share every B tile.
-constexpr int kD2Threads = 256;     // warp 0 TMA | warp 1 MMA | warps 4-7 epilogue
-constexpr int kD2Stages = 2;     // per CTA; two CTAs per SM (one in its epilogue while the other runs its main loop)
-constexpr int kD2Q = 2;             // q tiles (accumulators) per CTA
-
-struct Dgrad2Params {
-  int B, C, R, Lin, Lq, Tq, ngroups, nks;      // nks: 16-wide k-steps that carry shifts u <= T + 6
-  const __half* P16;
-  const int* exps;
-  float* out;                       // [nsplit][B][R][Lin]
-  int c_per_split;
-};
-
-__global__ void __launch_bounds__(kD2Threads, 2)
-tcnmfd_dgrad2_kernel(const __grid_constant__ CUtensorMap tmWs, const Dgrad2Params p) {
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  const uint32_t raw32 = ptx::smem_u32(smem_raw);
-  const uint32_t sbase = (raw32 + 1023u) & ~1023u;
-  uint8_t* smem_al = smem_raw + (sbase - raw32);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int nkk = p.Tq / kKB;                                   // B tiles (64 columns of u each) per c
-  const uint32_t seg_bytes = (uint32_t)(1024 + p.Tq) * 2;       // P[c][8 q0 .. 8 q0 + 1024 + Tq)
-  const uint32_t seg_pitch = (seg_bytes + 127u) & ~127u;
-  const uint32_t stage_bytes = (uint32_t)nkk * Smem::kTile + kD2Q * seg_pitch;
-  const uint32_t bar0 = sbase + kD2Stages * ((stage_bytes + 1023u) & ~1023u);
-  auto STAGE = [&](int s) { return sbase + (uint32_t)s * ((stage_bytes + 1023u) & ~1023u); };
-  auto BAR = [&](int i) { return bar0 + 8u * i; };
-  constexpr int B_FULL = 0, B_EMPTY = kD2Stages, B_ACC = 2 * kD2Stages;
-  volatile uint32_t* tmem_ptr_smem = reinterpret_cast<volatile uint32_t*>(smem_al + (bar0 - sbase) + 8 * (2 * kD2Stages + 1));
-  if (warp == 0 && lane == 0) {
-    ptx::prefetch_tmap(&tmWs);
-    for (int i = 0; i < kD2Stages; ++i) { ptx::mbar_init(BAR(B_FULL + i), 1); ptx::mbar_init(BAR(B_EMPTY + i), 1); }
-    ptx::mbar_init(BAR(B_ACC), 1);
-    ptx::fence_barrier_init();
-    ptx::fence_proxy_async();
-  }
-  if (warp == 1) {
-    ptx::tmem_alloc(bar0 + 8 * (2 * kD2Stages + 1), 256);
-    ptx::tmem_relinquish();
-  }
-  ptx::tc_fence_before();
-  __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem = *tmem_ptr_smem;
-  const int b = blockIdx.z / p.ngroups, grp = blockIdx.z - b * p.ngroups;
-  const int c0 = blockIdx.y * p.c_per_split, c1 = min(p.C, c0 + p.c_per_split);
-  const int nc = max(0, c1 - c0);
-  const int j0 = blockIdx.x * (kD2Q * 1024);                    // first output position of this CTA
-
-  if (warp == 0) {
-    if (lane == 0) {
-      for (int i = 0; i < nc; ++i) {
-        const int s = i % kD2Stages, ph = (i / kD2Stages) & 1, c = c0 + i;
-        ptx::mbar_wait(BAR(B_EMPTY + s), ph ^ 1);
-        ptx::mbar_expect_tx(BAR(B_FULL + s), (uint32_t)nkk * Smem::kTile + kD2Q * seg_bytes);
-        for (int kk = 0; kk < nkk; ++kk)
-          ptx::tma_load_2d(&tmWs, BAR(B_FULL + s), STAGE(s) + kk * Smem::kTile, kk * kKB, (c * p.ngroups + grp) * 128);
-        for (int qt = 0; qt < kD2Q; ++qt)
-          bulk_copy_g2s(STAGE(s) + nkk * Smem::kTile + qt * seg_pitch,
-                        p.P16 + ((int64_t)b * p.C + c) * p.Lq + j0 + qt * 1024, seg_bytes, BAR(B_FULL + s));
-      }
-    }
-  } else if (warp == 1) {
-    constexpr uint32_t idesc = ptx::idesc_f16(kM, 128, 0, 0);
-    constexpr uint32_t descHiB = ptx::smem_desc_hi_sw128(1024);
-    constexpr uint32_t descHiA = ((128u >> 4) & 0x3FFFu) | (1u << 14);      // SWIZZLE_NONE, stride byte offset 128 (8 rows x 16 B)
-    for (int i = 0; i < nc; ++i) {
-      const int s = i % kD2Stages, ph = (i / kD2Stages) & 1;
-      if (lane == 0) ptx::mbar_wait(BAR(B_FULL + s), ph);
-      __syncwarp();
-      ptx::tc_fence_after();
-      if (ptx::elect_one()) {
-        for (int qt = 0; qt < kD2Q; ++qt) {
-          const uint32_t seg = STAGE(s) + nkk * Smem::kTile + qt * seg_pitch;
-          for (int kst = 0; kst < p.nks; ++kst) {
-            const int kk = kst >> 2, ks = kst & 3;
-            // A: rows q = windows of the raw P row, 16 bytes apart; k-step = 16 elements = two core matrices 16 bytes apart
-            const uint32_t alo = ptx::smem_desc_lo(seg + (uint32_t)(kst * 16) * 2, 16);
-            const uint32_t blo = ptx::smem_desc_lo(STAGE(s) + kk * Smem::kTile, 16) + 2 * ks;
-            ptx::mma_ss(tmem + qt * 128, ptx::make_desc(alo, descHiA), ptx::make_desc(blo, descHiB), idesc, (i | kst) ? 1u : 0u);
-          }
-        }
-        ptx::mma_commit(BAR(B_EMPTY + s));
-        if (i == nc - 1) ptx::mma_commit(BAR(B_ACC));
-      }
-      __syncwarp();
-    }
-  } else if (warp >= 4) {
-    const int q = warp & 3, r128 = q * 32 + lane;
-    const uint32_t lane_addr = (uint32_t)(q * 32) << 16;
-    if (nc > 0) {
-      ptx::mbar_wait(BAR(B_ACC), 0);
-      ptx::tc_fence_after();
-    }
-    const float sc = exp2f(-(float)(p.exps[0] + p.exps[2]));
-    for (int qt = 0; qt < kD2Q; ++qt) {
-      const int j = j0 + qt * 1024 + 8 * r128;                   // this lane's 8 output positions
-#pragma unroll 1
-      for (int jj = 0; jj < 8; ++jj) {                            // 16 columns = 2 components x 8 phases
-        uint32_t sr[16];
-        if (nc > 0) { ptx::tmem_ld16(tmem + lane_addr + qt * 128 + jj * 16, sr); ptx::tc_wait_ld(); }
-        else {
-#pragma unroll
-          for (int i = 0; i < 16; ++i) sr[i] = 0u;
-        }
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int r = grp * 16 + jj * 2 + h;
-          if (r < p.R) {
-            float* dst = p.out + (((int64_t)blockIdx.y * p.B + b) * p.R + r) * p.Lin + j;
-#pragma unroll
-            for (int i = 0; i < 8; ++i)
-              if (j + i < p.Lin) dst[i] = __uint_as_float(sr[8 * h + i]) * sc;
-          }
-        }
-      }
-    }
-  }
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == 1) ptx::tmem_dealloc(tmem, 256);
-}
-
-// ---- recon, second formulation: the same eight-phase trick on the H side ---------------------------------------------------
-//   S[c, 8q + s] = sum_r sum_u  Wsh[(c, s), (r, u)] * H[r, 8q + u - A],      Wsh[(c, s), (r, u)] = W[c, r, s + A - u]
-// (A = T - 1 rounded up to 8, so that the window of H that row q reads starts 16-byte aligned).  M = 16 rows c x 8 phases s
-// from eight shifted copies of W (TMA, SWIZZLE_128B), N = 256 positions q = the raw padded fp16 row of H in shared memory
-// through an overlapping SWIZZLE_NONE descriptor (rows 16 bytes apart): no Toeplitz tile, every MMA a 128 x 256 x 16.
-// Epilogue: TMEM lane (c, s), column q  <->  S[c, 8q + s]; the eight phases of a row are neighbouring lanes, so the fp32
-// reads of V and the fp16 writes of the ratio tile coalesce across lanes.
-// grid (ceil(L / 2048), ceil(C / 16), B)
-constexpr int kR2N = 256;
-
-struct Recon2Params {
-  int B, C, L, R, Lp, padl, Lq, Tq, A8, nks;   // nks: 16-wide k-steps that carry shifts u <= A8 + 7
-  const __half* Hp16;
-  __half* P16out;
-  const float* V;
-  const int* exps;
-  const float* kappa;
-  double* loss_part;
-};
-
-template <bool LOSS>
-__global__ void __launch_bounds__(kD2Threads, 2)
-tcnmfd_recon2_kernel(const __grid_constant__ CUtensorMap tmWsh, const Recon2Params p) {
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  const uint32_t raw32 = ptx::smem_u32(smem_raw);
-  const uint32_t sbase = (raw32 + 1023u) & ~1023u;
-  uint8_t* smem_al = smem_raw + (sbase - raw32);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int nkk = p.Tq / kKB;
-  const uint32_t seg_bytes = (uint32_t)(8 * kR2N + p.Tq) * 2;
-  const uint32_t stage_pitch = ((uint32_t)nkk * Smem::kTile + seg_bytes + 1023u) & ~1023u;
-  const uint32_t bar0 = sbase + kD2Stages * stage_pitch;
-  auto STAGE = [&](int s) { return sbase + (uint32_t)s * stage_pitch; };
-  auto BAR = [&](int i) { return bar0 + 8u * i; };
-  constexpr int B_FULL = 0, B_EMPTY = kD2Stages, B_ACC = 2 * kD2Stages;
-  const uint32_t tptr = bar0 + 8 * (2 * kD2Stages + 1);
-  volatile uint32_t* tmem_ptr_smem = reinterpret_cast<volatile uint32_t*>(smem_al + (tptr - sbase));
-  double* red = reinterpret_cast<double*>(smem_al + (tptr - sbase) + 16);
-  if (warp == 0 && lane == 0) {
-    ptx::prefetch_tmap(&tmWsh);
-    for (int i = 0; i < kD2Stages; ++i) { ptx::mbar_init(BAR(B_FULL + i), 1); ptx::mbar_init(BAR(B_EMPTY + i), 1); }
-    ptx::mbar_init(BAR(B_ACC), 1);
-    ptx::fence_barrier_init();
-    ptx::fence_proxy_async();
-  }
-  if (warp == 1) {
-    ptx::tmem_alloc(tptr, kR2N);
-    ptx::tmem_relinquish();
-  }
-  ptx::tc_fence_before();
-  __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem = *tmem_ptr_smem;
-  const int b = blockIdx.z, cg = blockIdx.y, l0 = blockIdx.x * (8 * kR2N);
-
-  if (warp == 0) {
-    if (lane == 0) {
-      for (int r = 0; r < p.R; ++r) {
-        const int s = r % kD2Stages, ph = (r / kD2Stages) & 1;
-        ptx::mbar_wait(BAR(B_EMPTY + s), ph ^ 1);
-        ptx::mbar_expect_tx(BAR(B_FULL + s), (uint32_t)nkk * Smem::kTile + seg_bytes);
-        for (int kk = 0; kk < nkk; ++kk)
-          ptx::tma_load_2d(&tmWsh, BAR(B_FULL + s), STAGE(s) + kk * Smem::kTile, r * p.Tq + kk * kKB, cg * 128);
-        bulk_copy_g2s(STAGE(s) + nkk * Smem::kTile, p.Hp16 + ((int64_t)b * p.R + r) * p.Lp + p.padl - p.A8 + l0, seg_bytes,
-                      BAR(B_FULL + s));
-      }
-    }
-  } else if (warp == 1) {
-    constexpr uint32_t idesc = ptx::idesc_f16(kM, kR2N, 0, 0);
-    constexpr uint32_t descHiA = ptx::smem_desc_hi_sw128(1024);
-    constexpr uint32_t descHiB = ((128u >> 4) & 0x3FFFu) | (1u << 14);      // SWIZZLE_NONE, 8-row groups 128 bytes apart
-    for (int r = 0; r < p.R; ++r) {
-      const int s = r % kD2Stages, ph = (r / kD2Stages) & 1;
-      if (lane == 0) ptx::mbar_wait(BAR(B_FULL + s), ph);
-      __syncwarp();
-      ptx::tc_fence_after();
-      if (ptx::elect_one()) {
-        const uint32_t seg = STAGE(s) + nkk * Smem::kTile;
-        for (int kst = 0; kst < p.nks; ++kst) {
-          const int kk = kst >> 2, ks = kst & 3;
-          const uint32_t alo = ptx::smem_desc_lo(STAGE(s) + kk * Smem::kTile, 16) + 2 * ks;
-          const uint32_t blo = ptx::smem_desc_lo(seg + (uint32_t)(kst * 16) * 2, 16);
-          ptx::mma_ss(tmem, ptx::make_desc(alo, descHiA), ptx::make_desc(blo, descHiB), idesc, (r | kst) ? 1u : 0u);
-        }
-        ptx::mma_commit(BAR(B_EMPTY + s));
-        if (r == p.R - 1) ptx::mma_commit(BAR(B_ACC));
-      }
-      __syncwarp();
-    }
-  } else if (warp >= 4) {
-    const int q4 = warp & 3, m = q4 * 32 + lane;                 // TMEM lane = (c_local, s)
-    const uint32_t lane_addr = (uint32_t)(q4 * 32) << 16;
-    const int c = cg * 16 + (m >> 3), sph = m & 7;
-    const bool row_ok = c < p.C;
-    ptx::mbar_wait(BAR(B_ACC), 0);
-    ptx::tc_fence_after();
-    const float sc = exp2f(-(float)(p.exps[0] + p.exps[1]));
-    const float kap = *p.kappa, pscale = exp2f((float)p.exps[2]);
-    const float* vrow = p.V + ((int64_t)b * p.C + (row_ok ? c : 0)) * p.L;
-    __half* prow = p.P16out + ((int64_t)b * p.C + (row_ok ? c : 0)) * p.Lq;
-    double acc = 0.0;
-    // the 16 target values of chunk j + 1 are requested before chunk j is computed (one round trip per chunk, overlapped)
-    float v[16], vn[16];
-    auto load_v = [&](int j, float (&dst)[16]) {
-#pragma unroll
-      for (int i = 0; i < 16; ++i) {
-        const int l = l0 + 8 * (j * 16 + i) + sph;
-        dst[i] = (row_ok && l < p.L) ? __ldg(vrow + l) : 0.f;
-      }
-    };
-    load_v(0, vn);
-#pragma unroll 1
-    for (int j = 0; j < kR2N / 16; ++j) {
-      uint32_t sr[16];
-      ptx::tmem_ld16(tmem + lane_addr + j * 16, sr);
-#pragma unroll
-      for (int i = 0; i < 16; ++i) v[i] = vn[i];
-      if (j + 1 < kR2N / 16) load_v(j + 1, vn);
-      ptx::tc_wait_ld();
-      float a = 0.f;
-#pragma unroll
-      for (int i = 0; i < 16; ++i) {
-        const int l = l0 + 8 * (j * 16 + i) + sph;
-        const bool ok = row_ok && l < p.L;
-        const float x = fmaf(__uint_as_float(sr[i]), sc, kEps);
-        if (LOSS) {
-          if (ok) a += v[i] * (__logf(v[i] + kEps) - __logf(x)) - v[i] + (x - kEps);         // metrics.py:22
-        } else if (row_ok && l < p.Lq) {
-          const float pv = ok ? fmaf(v[i], ptx::rcp_approx(x), -kap) * pscale : 0.f;         // nmf.py:65, centred
-          prow[l] = __float2half_rn(fminf(pv, 65504.f));
-        }
-      }
-      acc += (double)a;
-    }
-    if (LOSS) {
-      for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
-      if (lane == 0) red[q4] = acc;
-      asm volatile("bar.sync 1, 128;");
-      if (q4 == 0 && lane == 0)
-        p.loss_part[((int64_t)blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x] = (red[0] + red[1]) + (red[2] + red[3]);
-    }
-  }
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == 1) ptx::tmem_dealloc(tmem, kR2N);
 }
 
 // ---- operand preparation --------------------------------------------------------------------------------------------------
@@ -662,79 +382,18 @@ fold_colsum_kernel(const FoldTail f) {
   }
 }
 
-// One pass over W (C, R, T), block c: every fp16 operand copy of this row, scaled by 2^eW (eW from the max of W), written
+// One pass over W (C, R, T), block c: both fp16 operand copies of this row, scaled by 2^eW (eW from the max of W), written
 // 16 bytes per thread and step, plus the row's per-component sums (-> colsum_W, nmf.py:128-131):
 //   Wr16[c][r Tp + tt]           = W[c, r, Tp - 1 - tt]        (recon: shifts reversed so that the H window ascends)
-//   Wf16[c][r Tp + tt]           = W[c, r, tt]                 (dgrad, Toeplitz-tile formulation)
-//   Ws16[(c, grp, r%16, s)][u]   = W[c, r, u - s]              (dgrad, eight shifted copies)
-//   Wsh16[(c, s)][r Tq + u]      = W[c, r, s + A8 - u]         (recon, eight shifted copies)
-//
-// The eight shifted copies dominate (cfg3: 100 MB per refresh).  Every 16-byte store gathers eight CONSECUTIVE shifts of one
-// component, so the lanes of a warp read W at addresses eight floats apart: from a dense shared-memory row that is an 8-way
-// bank conflict per load, and with per-element index arithmetic and bounds checks the kernel was instruction-bound on top
-// (36 us at cfg3, 2.8 TB/s).  Hence the row is staged scaled and DE-INTERLEAVED by shift residue:
-//     stage[r][t & 7][(t >> 3) + F]   for t in [-8 F, 8 (S - F)),  zero outside [0, T)
-// (S slots per residue class, F leading ones).  For a fixed copy index s (an unrolled loop) element k of a store then
-// sits at a compile-time class and a compile-time slot offset from the thread's base, consecutive lanes read consecutive
-// words, and out-of-range shifts read the zero margins: eight loads with immediate offsets, four packs, one store.  Stores
-// whose eight shifts all fall outside [0, T) are skipped: those bytes are zero from tc_nmfd_create on and nobody writes them.
-__device__ __forceinline__ void prep_w_shifted(const float* __restrict__ stage, int S, int F, int R, int T, int Tq, int A8,
-                                               int ngroups, int c, __half* __restrict__ Ws16, __half* __restrict__ Wsh16) {
-  const int NV = Tq >> 3;                                  // 16-byte stores per row of either copy
-  const unsigned int magic = 0xFFFFFFFFu / (unsigned)NV + 1u;     // j / NV == umulhi(j, magic) for the j below (< 2^16)
-  const int64_t rows = (int64_t)ngroups * 128;
-  auto pack8 = [](const float (&v)[8]) {
-    __half2 h[4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i) h[i] = __floats2half2_rn(v[2 * i], v[2 * i + 1]);
-    return *reinterpret_cast<const uint4*>(h);
-  };
-  // one item = one (component r, 8-shift group vec): its eight stores (the eight copies of one layout) share every address
-  // computation; inside, copy index and element index are compile-time, so a load is [base + class S + immediate].
-  // dgrad copies: Ws16[(c, grp, r % 16, SH)][u + k] = W[c, r, u + k - SH]
-  for (int j = threadIdx.x; j < R * NV; j += 256) {
-    const int r = (int)__umulhi((unsigned)j, magic), vec = j - r * NV, u = vec << 3;
-    const float* up = stage + (int64_t)r * 8 * S + F + vec;                     // ascending windows
-    __half* ws = Ws16 + ((int64_t)c * rows + (int64_t)(r >> 4) * 128 + (r & 15) * 8) * Tq + u;       // + SH Tq
-#pragma unroll
-    for (int SH = 0; SH < 8; ++SH) {
-      if (u + 7 - SH >= 0 && u - SH < T) {
-        float v[8];
-#pragma unroll
-        for (int k = 0; k < 8; ++k) v[k] = up[((k - SH) & 7) * S + ((k - SH) >> 3)];
-        *reinterpret_cast<uint4*>(ws + SH * Tq) = pack8(v);
-      }
-    }
-  }
-  // recon copies: Wsh16[(c, SH)][r Tq + u + k] = W[c, r, SH + A8 - u - k]
-  const int64_t wsh_step = (int64_t)R * Tq;
-  for (int j = threadIdx.x; j < R * NV; j += 256) {
-    const int r = (int)__umulhi((unsigned)j, magic), vec = j - r * NV, u = vec << 3;
-    const float* dn = stage + (int64_t)r * 8 * S + F + (A8 >> 3) - vec;         // descending windows
-    __half* wsh = Wsh16 + (int64_t)c * 8 * wsh_step + (int64_t)r * Tq + u;      // + SH R Tq
-#pragma unroll
-    for (int SH = 0; SH < 8; ++SH) {
-      if (SH + A8 - u >= 0 && SH + A8 - u - 7 < T) {
-        float v[8];
-#pragma unroll
-        for (int k = 0; k < 8; ++k) v[k] = dn[((SH - k) & 7) * S + ((SH - k) >> 3)];
-        *reinterpret_cast<uint4*>(wsh + SH * wsh_step) = pack8(v);
-      }
-    }
-  }
-}
-
+//   Wf16[c][r Tp + tt]           = W[c, r, tt]                 (dgrad)
 __global__ void __launch_bounds__(256, 8)     // 8 blocks per SM: the 1025 blocks of cfg3 run as one wave
-prep_w_kernel(const float* __restrict__ W, int C, int R, int T, int Tp, int Tq, int ngroups,
-              const unsigned int* __restrict__ absmax, int* __restrict__ exps, __half* __restrict__ Wr16,
-              __half* __restrict__ Wf16, __half* __restrict__ Ws16, __half* __restrict__ Wsh16, int A8,
-              float* __restrict__ cs_part, int use_smem, int S, int F) {
+prep_w_kernel(const float* __restrict__ W, int C, int R, int T, int Tp, const unsigned int* __restrict__ absmax,
+              int* __restrict__ exps, __half* __restrict__ Wr16, __half* __restrict__ Wf16, float* __restrict__ cs_part) {
   const int e = pow2_exp14(__uint_as_float(*absmax));
   if (blockIdx.x == 0 && threadIdx.x == 0) exps[0] = e;
   const float sc = exp2f((float)e);
   const int c = blockIdx.x;
   const float* Wg = W + (int64_t)c * R * T;
-  extern __shared__ float stage[];
   auto w_at = [&](int r, int t) { return (r < R && t >= 0 && t < T) ? Wg[r * T + t] * sc : 0.f; };
   auto pack8 = [&](const float (&v)[8]) {
     __half2 h[4];
@@ -742,55 +401,14 @@ prep_w_kernel(const float* __restrict__ W, int C, int R, int T, int Tp, int Tq, 
     for (int i = 0; i < 4; ++i) h[i] = __floats2half2_rn(v[2 * i], v[2 * i + 1]);
     return *reinterpret_cast<const uint4*>(h);
   };
-  // plain forward / reversed copies: only read by the Toeplitz-tile kernels (A/B switches, very long shifts)
   const int64_t rowlen = (int64_t)R * Tp;
-  for (int i8 = threadIdx.x; Wr16 != nullptr && i8 < R * Tp / 8; i8 += 256) {
+  for (int i8 = threadIdx.x; i8 < R * Tp / 8; i8 += 256) {
     const int i = i8 * 8, r = i / Tp, tt = i - r * Tp;
     float f[8], rv[8];
 #pragma unroll
     for (int k = 0; k < 8; ++k) { f[k] = w_at(r, tt + k); rv[k] = w_at(r, Tp - 1 - tt - k); }
     *reinterpret_cast<uint4*>(Wf16 + c * rowlen + i) = pack8(f);
     *reinterpret_cast<uint4*>(Wr16 + c * rowlen + i) = pack8(rv);
-  }
-  if (use_smem) {
-    for (int i = threadIdx.x; i < R * 8 * S; i += 256) stage[i] = 0.f;
-    __syncthreads();
-    // the row's R T values: eight independent loads in flight per thread before the first dependent shared-memory store
-    // (a loop of load -> store pairs paid the full memory latency R times per block and was what bounded this kernel)
-    const int RT = R * T;
-    const unsigned int magic_t = 0xFFFFFFFFu / (unsigned)T + 1u;          // i / T == umulhi(i, magic_t): R T < 2^16 here
-    for (int i0 = threadIdx.x; i0 < RT; i0 += 256 * 8) {
-      float x[8];
-#pragma unroll
-      for (int m = 0; m < 8; ++m) { const int i = i0 + m * 256; x[m] = i < RT ? Wg[i] : 0.f; }
-#pragma unroll
-      for (int m = 0; m < 8; ++m) {
-        const int i = i0 + m * 256;
-        if (i < RT) {
-          const int r = (int)__umulhi((unsigned)i, magic_t), t = i - r * T;
-          stage[(r * 8 + (t & 7)) * S + (t >> 3) + F] = x[m] * sc;
-        }
-      }
-    }
-    __syncthreads();
-    prep_w_shifted(stage, S, F, R, T, Tq, A8, ngroups, c, Ws16, Wsh16);
-  } else {                           // a row of W too long to stage: straight from global memory, every store written
-    const int64_t rows = (int64_t)ngroups * 128;
-    for (int i8 = threadIdx.x; i8 < rows * Tq / 8; i8 += 256) {
-      const int i = i8 * 8, n = i / Tq, u = i - n * Tq;
-      const int r = (n >> 7) * 16 + ((n & 127) >> 3), sh = n & 7;
-      float v[8];
-#pragma unroll
-      for (int k = 0; k < 8; ++k) v[k] = w_at(r, u + k - sh);
-      *reinterpret_cast<uint4*>(Ws16 + ((int64_t)c * rows + n) * Tq + u) = pack8(v);
-    }
-    for (int i8 = threadIdx.x; i8 < 8 * R * Tq / 8; i8 += 256) {
-      const int i = i8 * 8, sh = i / (R * Tq), ru = i - sh * (R * Tq), r = ru / Tq, u = ru - r * Tq;
-      float v[8];
-#pragma unroll
-      for (int k = 0; k < 8; ++k) v[k] = w_at(r, sh + A8 - u - k);
-      *reinterpret_cast<uint4*>(Wsh16 + ((int64_t)c * 8 + sh) * ((int64_t)R * Tq) + ru) = pack8(v);
-    }
   }
   // per-component sums of this row: warp w takes r = w, w + 8, ...; fixed order
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -875,15 +493,12 @@ int make_tmap2(CUtensorMap* m, const void* base, int64_t rows, int64_t cols, int
 struct TcNmfdState {
   NmfdShape d{};
   int Tp = 0, Lp = 0, padl = 0, Lq = 0, Cpad = 0;
-  __half *Wr16 = nullptr, *Wf16 = nullptr, *Hp16 = nullptr, *P16 = nullptr, *Ws16 = nullptr, *Wsh16 = nullptr;
-  int A8 = 0;                       // T - 1 rounded up to 8: alignment of the H window of the eight-phase recon
-  int Tq = 0, ngroups = 1, cps_h2 = 0, ws_h2 = 1;   // dgrad2: padded shift extent, 16-component groups, c per split, splits
+  __half *Wr16 = nullptr, *Wf16 = nullptr, *Hp16 = nullptr, *P16 = nullptr;
   float* part = nullptr;            // wgrad / dgrad split partials
   int64_t part_floats = 0;
   unsigned int* absmax = nullptr;   // [2]: max of W, max of H (float bits; written by absmax_kernel or by the ratio stage)
   float* colsum = nullptr;          // [2][R]: colsum_W | colsum_H
   float* cs_part = nullptr;         // per-row / per-block partial sums of the factor being refreshed
-  bool need_tile_copies = false;    // Wr16 / Wf16 are in use (see refresh)
   bool w_fresh = false, h_fresh = false;      // the fp16 copies / column sums of W, H match the fp32 factor
   bool aw_valid = false, ah_valid = false;    // absmax[0], absmax[1] hold the max of the current W, H
   int* exps = nullptr;              // {eW, eH, eP}
@@ -893,7 +508,7 @@ struct TcNmfdState {
   int loss_blocks = 0;
   int ws_w = 1, ws_h = 1;           // split counts of wgrad / dgrad
   int kbs_w = 0, kbs_h = 0;
-  CUtensorMap tmWr, tmWf, tmP, tmWs, tmWsh;
+  CUtensorMap tmWr, tmWf, tmP;
   bool attr_set = false;
 };
 
@@ -903,7 +518,7 @@ bool tc_nmfd_supported(const NmfdShape& d, double beta) {
 
 void tc_nmfd_destroy(TcNmfdState* s) {
   if (!s) return;
-  cudaFree(s->Wsh16); cudaFree(s->Ws16); cudaFree(s->Wr16); cudaFree(s->Wf16); cudaFree(s->Hp16); cudaFree(s->P16); cudaFree(s->part); cudaFree(s->absmax); cudaFree(s->colsum); cudaFree(s->cs_part);
+  cudaFree(s->Wr16); cudaFree(s->Wf16); cudaFree(s->Hp16); cudaFree(s->P16); cudaFree(s->part); cudaFree(s->absmax); cudaFree(s->colsum); cudaFree(s->cs_part);
   cudaFree(s->exps); cudaFree(s->kappa); cudaFree(s->vsum); cudaFree(s->loss_part);
   delete s;
 }
@@ -913,42 +528,27 @@ int tc_nmfd_create(TcNmfdState** out, const NmfdShape& d) {
   TcNmfdState* s = new TcNmfdState();
   s->d = d;
   s->Tp = (int)round_up(d.T, kKB);
-  s->padl = (int)round_up(s->Tp + 136, 8);                       // every window start >= 0 (padl >= A8 as well)
-  s->Lp = (int)round_up((int64_t)s->padl + round_up((int64_t)d.L, 8 * kR2N) + 256 + kWinHalfs + 136, 8);
-  s->A8 = (int)round_up(d.T - 1, 8);
-  s->Tq = (int)round_up(s->A8 + 8, kKB);                            // shifts u in [0, A8 + 7]; also covers dgrad's [0, T + 6]
-  s->ngroups = (int)ceil_div(d.R, 16);
-  s->Lq = (int)round_up(round_up((int64_t)d.L, 2048) + 1024 + s->Tq + kWinHalfs + 8, 8);
+  s->padl = (int)round_up(s->Tp + 136, 8);                       // every window start >= 0
+  s->Lp = (int)round_up((int64_t)s->padl + round_up((int64_t)d.L, 2048) + 256 + kWinHalfs + 136, 8);
+  s->Lq = (int)round_up(round_up((int64_t)d.L, 2048) + 1024 + s->Tp + kKB + kWinHalfs + 8, 8);
   s->Cpad = (int)round_up(d.C, kM);
   const int lkb = (int)ceil_div(d.L, kKB), tkb = s->Tp / kKB;
-  // split the K loops of wgrad / dgrad so that the grid is a few waves of 148 CTAs
+  // split the K loops of wgrad / dgrad so that the grid is a few waves of 132 CTAs
   const int64_t tiles_w = ceil_div(d.C, kM) * d.R, tiles_h = ceil_div(d.Lin, kM) * d.B;
   int64_t kb_w = (int64_t)d.B * lkb, kb_h = (int64_t)d.C * tkb;
-  s->ws_w = (int)std::max<int64_t>(1, std::min<int64_t>(kb_w / 8, ceil_div(148 * 4, tiles_w)));
-  s->ws_h = (int)std::max<int64_t>(1, std::min<int64_t>(kb_h / 8, ceil_div(148 * 4, tiles_h)));
+  s->ws_w = (int)std::max<int64_t>(1, std::min<int64_t>(kb_w / 8, ceil_div(132 * 4, tiles_w)));
+  s->ws_h = (int)std::max<int64_t>(1, std::min<int64_t>(kb_h / 8, ceil_div(132 * 4, tiles_h)));
   s->kbs_w = (int)ceil_div(kb_w, s->ws_w); s->ws_w = (int)ceil_div(kb_w, s->kbs_w);
   s->kbs_h = (int)ceil_div(kb_h, s->ws_h); s->ws_h = (int)ceil_div(kb_h, s->kbs_h);
-  {
-    const int64_t tiles = ceil_div(d.Lin, kD2Q * 1024) * d.B * s->ngroups;
-    int64_t ws = std::max<int64_t>(1, std::min<int64_t>(d.C / 4 > 0 ? d.C / 4 : 1, ceil_div(148, tiles)));
-    s->cps_h2 = (int)ceil_div(d.C, ws);
-    s->ws_h2 = (int)ceil_div(d.C, s->cps_h2);
-  }
-  const int hs = std::max(s->ws_h, s->ws_h2);
+  const int hs = s->ws_h;
   const int64_t pw = (int64_t)s->ws_w * d.C * d.R * d.T, ph = (int64_t)hs * d.B * d.R * d.Lin;
   s->part_floats = pw > ph ? pw : ph;
-  s->loss_blocks = (int)std::max<int64_t>(ceil_div(d.L, kM) * ceil_div(d.C, kM) * d.B, ceil_div(d.L, 8 * kR2N) * ceil_div(d.C, 16) * d.B);
+  s->loss_blocks = (int)(ceil_div(d.L, kM) * ceil_div(d.C, kM) * d.B);
   const size_t wbytes = (size_t)s->Cpad * d.R * s->Tp * 2, hbytes = (size_t)d.B * d.R * s->Lp * 2;
   const size_t pbytes = ((size_t)d.B * d.C + 1) * s->Lq * 2;
   cudaError_t e = cudaSuccess;
   if (e == cudaSuccess) e = cudaMalloc(&s->Wr16, wbytes);
   if (e == cudaSuccess) e = cudaMalloc(&s->Wf16, wbytes);
-  const size_t wshbytes = (size_t)s->Cpad * 8 * d.R * s->Tq * 2;
-  if (e == cudaSuccess) e = cudaMalloc(&s->Wsh16, wshbytes);
-  if (e == cudaSuccess) e = cudaMemset(s->Wsh16, 0, wshbytes);
-  const size_t wsbytes = (size_t)s->Cpad * s->ngroups * 128 * s->Tq * 2;
-  if (e == cudaSuccess) e = cudaMalloc(&s->Ws16, wsbytes);
-  if (e == cudaSuccess) e = cudaMemset(s->Ws16, 0, wsbytes);
   if (e == cudaSuccess) e = cudaMalloc(&s->Hp16, hbytes);
   if (e == cudaSuccess) e = cudaMalloc(&s->P16, pbytes);
   if (e == cudaSuccess) e = cudaMalloc(&s->part, (size_t)s->part_floats * 4);
@@ -973,21 +573,12 @@ int tc_nmfd_create(TcNmfdState** out, const NmfdShape& d) {
     set_error(std::string("tc_nmfd_create: ") + cudaGetErrorString(e));
     return 2;
   }
-  {
-    const int nkk = s->Tq / kKB;
-    const uint32_t st_r = (((uint32_t)nkk * Smem::kTile + (uint32_t)(8 * kR2N + s->Tq) * 2) + 1023u) & ~1023u;
-    const uint32_t st_d = (((uint32_t)nkk * Smem::kTile + kD2Q * ((((uint32_t)(1024 + s->Tq) * 2) + 127u) & ~127u)) + 1023u) & ~1023u;
-    const bool fits = kD2Stages * std::max(st_r, st_d) + 2048 <= 232448u;
-    s->need_tile_copies = !fits || getenv("NMFB200_NMFD_RECON1") != nullptr || getenv("NMFB200_NMFD_DGRAD1") != nullptr;
-  }
   int rc = 0;
   rc |= make_tmap2(&s->tmWr, s->Wr16, s->Cpad, (int64_t)d.R * s->Tp, (int64_t)d.R * s->Tp, kM);
-  // dgrad reads Wf16 as (C R) rows of Tp columns, Rp16 rows per tile
-  const int Rp16 = (d.R + 15) & ~15;
-  rc |= make_tmap2(&s->tmWf, s->Wf16, (int64_t)s->Cpad * d.R, s->Tp, s->Tp, Rp16);
+  // dgrad reads Wf16 as (C R) rows of Tp columns, up to 128 rows (components) per tile
+  const int Rb = (int)std::min<int64_t>((d.R + 15) & ~15, 128);
+  rc |= make_tmap2(&s->tmWf, s->Wf16, (int64_t)s->Cpad * d.R, s->Tp, s->Tp, Rb);
   rc |= make_tmap2(&s->tmP, s->P16, (int64_t)d.B * d.C, s->Lq, s->Lq, kM);
-  rc |= make_tmap2(&s->tmWs, s->Ws16, (int64_t)s->Cpad * s->ngroups * 128, s->Tq, s->Tq, 128);
-  rc |= make_tmap2(&s->tmWsh, s->Wsh16, (int64_t)s->Cpad * 8, (int64_t)d.R * s->Tq, (int64_t)d.R * s->Tq, 128);
   if (rc) { tc_nmfd_destroy(s); return 2; }
   *out = s;
   return 0;
@@ -1049,21 +640,7 @@ int refresh(TcNmfdState* s, const float* W, const float* H, cudaStream_t st) {
       NMF_LAUNCH_CHECK();
       s->aw_valid = true;
     }
-    // the reversed / forward copies are only read by the Toeplitz-tile kernels (A/B switches, or shifts too long for the
-    // eight-phase kernels' shared-memory stages)
-    const bool tile_copies = s->need_tile_copies;
-    // staging layout of prep_w_kernel: S slots per shift-residue class, F of them leading zeros (shifts down to A8 + 1 - Tq)
-    const int F = (s->Tq - s->A8) / 8 + 2, S = s->Tq / 8 + F;
-    const size_t wrow_bytes = (size_t)d.R * 8 * S * sizeof(float);
-    const int use_smem = (wrow_bytes <= 200 * 1024 && (int64_t)d.R * d.T < 65536) ? 1 : 0;
-    static size_t attr_bytes = 0;
-    if (use_smem && wrow_bytes > 48 * 1024 && wrow_bytes > attr_bytes) {
-      NMF_CUDA_CHECK(cudaFuncSetAttribute(prep_w_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wrow_bytes));
-      attr_bytes = wrow_bytes;
-    }
-    prep_w_kernel<<<d.C, 256, use_smem ? wrow_bytes : 0, st>>>(W, d.C, d.R, d.T, s->Tp, s->Tq, s->ngroups, s->absmax, s->exps,
-                                                               tile_copies ? s->Wr16 : nullptr, s->Wf16, s->Ws16, s->Wsh16,
-                                                               s->A8, s->cs_part, use_smem, S, F);
+    prep_w_kernel<<<d.C, 256, 0, st>>>(W, d.C, d.R, d.T, s->Tp, s->absmax, s->exps, s->Wr16, s->Wf16, s->cs_part);
     NMF_LAUNCH_CHECK();
     fold_colsum_kernel<<<d.R, 256, 0, st>>>(fold_tail_args(s, 0, d.C, 1, /*do_kappa=*/s->h_fresh));
     NMF_LAUNCH_CHECK();
@@ -1093,33 +670,6 @@ int tc_nmfd_recon(TcNmfdState* s, const float* V, const float* W, const float* H
                   cudaStream_t st) {
   int rc = refresh(s, W, H, st);
   if (rc) return rc;
-  static const bool v1 = getenv("NMFB200_NMFD_RECON1") != nullptr;      // A/B: the Toeplitz-tile formulation
-  const int nkk = s->Tq / kKB;
-  const uint32_t stage2 = (((uint32_t)nkk * Smem::kTile + (uint32_t)(8 * kR2N + s->Tq) * 2) + 1023u) & ~1023u;
-  const int smem2 = (int)(kD2Stages * stage2 + 8 * (2 * kD2Stages + 1) + 16 + 64 + 1024);
-  if (!v1 && smem2 <= 232448) {
-    const NmfdShape& d = s->d;
-    Recon2Params q{};
-    q.B = d.B; q.C = d.C; q.L = d.L; q.R = d.R; q.Lp = s->Lp; q.padl = s->padl; q.Lq = s->Lq; q.Tq = s->Tq; q.A8 = s->A8;
-    q.nks = (int)ceil_div(s->A8 + 8, 16);
-    q.Hp16 = s->Hp16; q.P16out = s->P16; q.V = V; q.exps = s->exps; q.kappa = s->kappa; q.loss_part = s->loss_part;
-    static int attr0 = 0, attr1 = 0;
-    int& attr = loss ? attr1 : attr0;
-    if (smem2 > attr) {
-      if (loss) NMF_CUDA_CHECK(cudaFuncSetAttribute(tcnmfd_recon2_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem2));
-      else NMF_CUDA_CHECK(cudaFuncSetAttribute(tcnmfd_recon2_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem2));
-      attr = smem2;
-    }
-    dim3 grid2((unsigned)ceil_div(d.L, 8 * kR2N), (unsigned)ceil_div(d.C, 16), (unsigned)d.B);
-    if (loss) {
-      tcnmfd_recon2_kernel<true><<<grid2, kD2Threads, smem2, st>>>(s->tmWsh, q);
-      NMF_LAUNCH_CHECK();
-      return sum_partials(s->loss_part, (int)(grid2.x * grid2.y * grid2.z), loss_dev, st);
-    }
-    tcnmfd_recon2_kernel<false><<<grid2, kD2Threads, smem2, st>>>(s->tmWsh, q);
-    NMF_LAUNCH_CHECK();
-    return 0;
-  }
   NmfdTcParams p = base_params(s, V);
   dim3 grid((unsigned)ceil_div(s->d.L, kM), (unsigned)ceil_div(s->d.C, kM), (unsigned)s->d.B);
   if (loss) {
@@ -1141,33 +691,11 @@ int tc_nmfd_wgrad(TcNmfdState* s, const float** part, int* nsplit, cudaStream_t 
 }
 
 int tc_nmfd_dgrad(TcNmfdState* s, const float** part, int* nsplit, cudaStream_t st) {
-  static const bool v1 = getenv("NMFB200_NMFD_DGRAD1") != nullptr;      // A/B: the Toeplitz-tile formulation
-  if (!v1) {
-    const NmfdShape& d = s->d;
-    Dgrad2Params q{};
-    q.B = d.B; q.C = d.C; q.R = d.R; q.Lin = d.Lin; q.Lq = s->Lq; q.Tq = s->Tq; q.ngroups = s->ngroups;
-    q.P16 = s->P16; q.exps = s->exps; q.out = s->part; q.c_per_split = s->cps_h2;
-    q.nks = (int)ceil_div(d.T + 7, 16);
-    const int nkk = s->Tq / kKB;
-    const uint32_t seg_pitch = (((uint32_t)(1024 + s->Tq) * 2) + 127u) & ~127u;
-    const uint32_t stage = (((uint32_t)nkk * Smem::kTile + kD2Q * seg_pitch) + 1023u) & ~1023u;
-    const int smem = (int)(kD2Stages * stage + 8 * (2 * kD2Stages + 1) + 16 + 1024);
-    if (smem > 232448) { set_error("nmfd dgrad: shift extent too large for the shared-memory stages"); return 1; }
-    static int attr_smem = 0;
-    if (smem > attr_smem) {
-      NMF_CUDA_CHECK(cudaFuncSetAttribute(tcnmfd_dgrad2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-      attr_smem = smem;
-    }
-    dim3 grid((unsigned)ceil_div(d.Lin, kD2Q * 1024), (unsigned)s->ws_h2, (unsigned)(d.B * s->ngroups));
-    tcnmfd_dgrad2_kernel<<<grid, kD2Threads, smem, st>>>(s->tmWs, q);
-    NMF_LAUNCH_CHECK();
-    *part = s->part; *nsplit = s->ws_h2;
-    return 0;
-  }
   NmfdTcParams p = base_params(s, nullptr);
   p.nsplit = s->ws_h; p.kb_per_split = s->kbs_h;
   dim3 grid((unsigned)ceil_div(s->d.Lin, kM), (unsigned)s->ws_h, (unsigned)s->d.B);
-  int rc = launch<kDgrad>(s, s->tmWf, grid, p, st);
+  int rc = 0;
+  for (p.r_off = 0; rc == 0 && p.r_off < s->d.R; p.r_off += 128) rc = launch<kDgrad>(s, s->tmWf, grid, p, st);
   *part = s->part; *nsplit = s->ws_h;
   return rc;
 }

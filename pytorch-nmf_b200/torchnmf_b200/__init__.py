@@ -1,5 +1,5 @@
-"""torchnmf_b200 -- B200-native (sm_100a) multiplicative-update NMF engine behind the
-torchnmf.nmf.NMF / NMFD module surface.  See DESIGN.md / INTEGRATION.md at the repo root."""
+"""torchnmf_b200 -- H100-native (sm_90a) multiplicative-update NMF engine behind the
+torchnmf.nmf.NMF / NMFD module surface.  See README.md / INTEGRATION.md at the repo root."""
 __version__ = "0.1.0"
 
 from . import constants, metrics, nmf, plca, trainer, utils  # noqa: F401

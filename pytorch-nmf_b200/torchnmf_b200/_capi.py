@@ -81,7 +81,7 @@ def load():
     lib = ctypes.CDLL(LIB_PATH)
     compat = bool(os.environ.get("NMFB200_LIB")) and bool(os.environ.get("NMFB200_LIB_COMPAT"))
     for name, (res, args) in SIGNATURES.items():
-        if compat and not hasattr(lib, name):       # A/B timing against an older build (tools/ only): newer symbols absent
+        if compat and not hasattr(lib, name):       # A/B timing against an older build: newer symbols absent
             continue
         fn = getattr(lib, name)          # AttributeError here == ABI mismatch
         fn.restype = res

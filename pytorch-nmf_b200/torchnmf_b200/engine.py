@@ -8,7 +8,7 @@ needs from its loop body:
     loss(beta) -> float            metrics.beta_div of the current reconstruction, nmf.py:360-361,:400-401
 
 `ShardedEngine` wraps any engine that also offers ``w_partial`` / ``w_apply`` / ``loss_tensor`` and
-inserts the one collective per iteration that the row-sharded layout needs (SURVEY.md 8e).
+inserts the one collective per iteration that the row-sharded layout needs.
 """
 import ctypes
 import os

@@ -1,4 +1,4 @@
-"""NMF / NMFD modules with the reference's surface and a B200-native `fit`.
+"""NMF / NMFD modules with the reference's surface and an H100-native `fit`.
 
 Mirrors the module surface of torchnmf 0.3.5 (`torchnmf/nmf.py`): `BaseComponent` (:173-292),
 `NMF` (:641-697), `NMFD` (:700-779) and `BaseComponent.fit` (:298-409).  Constructor arguments,
@@ -6,7 +6,7 @@ parameter shapes (`W (C,R[,T])`, `H (N,R)` / `(B,R,L_in)`), `forward`, `state_di
 `fit` signature / return value / exceptions are the reference's.  What differs is the inside of the
 iteration loop: instead of materialising `WH` and taking two autograd backward passes
 (`_double_backward_update`, :52-92), every update is one call into libnmf_b200.so, whose fused
-sm_100a kernels never write the (N x C) reconstruction or ratio matrices to HBM.
+sm_90a kernels never write the (N x C) reconstruction or ratio matrices to HBM.
 
 There is no CPU compute path: `fit` on CPU-resident modules copies V / W / H to the current CUDA
 device, runs there, and copies the factors back into the same Parameter storages ("host buffer"
@@ -189,7 +189,7 @@ class BaseComponent(torch.nn.Module):
         staged = False
         if self._engine_factory is None:
             if not torch.cuda.is_available():
-                raise RuntimeError("torchnmf_b200.fit needs a CUDA device (sm_100a); there is no CPU fallback")
+                raise RuntimeError("torchnmf_b200.fit needs a CUDA device (sm_90a); there is no CPU fallback")
             f32 = torch.float32
             on_gpu = W.device.type == "cuda"
             dev = W.device if on_gpu else torch.device("cuda", torch.cuda.current_device())

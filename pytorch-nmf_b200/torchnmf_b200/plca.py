@@ -1,4 +1,4 @@
-"""PLCA / SIPLCA / SIPLCA2 / SIPLCA3 with the reference's module surface (torchnmf/plca.py:28-625) and a B200-native `fit`.
+"""PLCA / SIPLCA / SIPLCA2 / SIPLCA3 with the reference's module surface (torchnmf/plca.py:28-625) and an H100-native `fit`.
 
     V (N, C) / sum(V)  ~=  H (N, R) diag(Z (R,)) W (C, R)^T,     W, H column-normalised, Z a distribution.
 
@@ -7,7 +7,7 @@ updates Z, W and H simultaneously from the three gradients.  Here the two big co
 
     dW[c, r] = sum_n P[n, c] (H Z)[n, r],      dHz[n, r] = sum_c P[n, c] W[c, r],      P = V / ((H Z) W^T + eps)
 
-are two launches of the fused tcgen05 KL contraction (`nmfb200_nmf_raw_terms` with the factor pair (W, H diag Z)): neither
+are two launches of the fused wgmma KL contraction (`nmfb200_nmf_raw_terms` with the factor pair (W, H diag Z)): neither
 WZH nor P reaches HBM.  dH = dHz * Z and dZ[r] = sum_n H[n, r] dHz[n, r] follow from them; everything after that is the
 reference's sequence of small factor-sized operations (plca.py:256-289).
 
@@ -123,14 +123,14 @@ class BaseComponent(torch.nn.Module):
         `(n_iter, norm)`).  Runs on the parameters' CUDA device; host-resident modules are staged like `NMF.fit`.
 
         precision: "f32" (default: the fused fp32 CUDA-core contraction, matches the reference to 1e-5 on the fixtures) |
-                   "f16" / "f16_split" (tcgen05 contraction: ~10x faster at large shapes; the EM recursion keeps the
+                   "f16" / "f16_split" (wgmma contraction: ~10x faster at large shapes; the EM recursion keeps the
                    fp16 operand rounding, measured 1.0-1.4e-3 relative after 30-50 iterations on the fixtures of
                    tests/golden/reference_next.npz -- outside the 1e-3 bar, hence opt-in)."""
         assert torch.all(V >= 0.), "Target should be non-negative."                         # plca.py:236
         W, H, Z = self.W, self.H, self.Z
         assert W is not None and H is not None and Z is not None, "fit() needs W, H and Z"
         if not torch.cuda.is_available():
-            raise RuntimeError("torchnmf_b200.PLCA.fit needs a CUDA device (sm_100a); there is no CPU fallback")
+            raise RuntimeError("torchnmf_b200.PLCA.fit needs a CUDA device (sm_90a); there is no CPU fallback")
         f32 = torch.float32
         on_gpu = W.device.type == "cuda"
         dev = W.device if on_gpu else torch.device("cuda", torch.cuda.current_device())

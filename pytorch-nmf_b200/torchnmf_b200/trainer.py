@@ -11,8 +11,8 @@ Two ways to obtain the two gradient terms `neg = relu(d<WH, V (WH+eps)^(beta-2)>
 
 * generic: two vector-Jacobian products through whatever graph the closure built (torch.autograd.grad) -- any
   composition of modules, CPU or GPU; this is the reference's algorithm.
-* fused (B200): when the prediction is the plain reconstruction of ONE `torchnmf_b200.NMF` module on a CUDA device and `p`
-  is that module's W or H, both terms come from ONE launch of the fused tcgen05 contraction
+* fused (GPU): when the prediction is the plain reconstruction of ONE `torchnmf_b200.NMF` module on a CUDA device and `p`
+  is that module's W or H, both terms come from ONE launch of the fused wgmma contraction
   (`nmfb200_nmf_raw_terms`): neither WH nor the ratio matrices are materialised by the update.  The closure may
   return the module itself instead of its output (`return V, model`) to skip the forward pass as well.  The
   convolutive modules (`NMFD`, `NMF2D`, `NMF3D`) take the same route through `nmfb200_nmfd_raw_terms` (the sliding
@@ -205,7 +205,7 @@ def _project_slices_(p, dim, k1, k2):
         _engine.hoyer_project_(p, dim, k1, k2)
         return
     if not (p.is_cuda or torch.cuda.is_available()):
-        raise RuntimeError("SparsityProj needs a CUDA device (sm_100a) for the projection; there is no CPU fallback")
+        raise RuntimeError("SparsityProj needs a CUDA device (sm_90a) for the projection; there is no CPU fallback")
     dev = p.device if p.is_cuda else torch.device("cuda", torch.cuda.current_device())
     tmp = p.detach().to(dev, torch.float32).contiguous()
     _engine.hoyer_project_(tmp, dim, torch.as_tensor(k1).to(dev), torch.as_tensor(k2).to(dev))

@@ -1,11 +1,11 @@
-"""GPU parity tests (run with `-m gpu` on the B200 box).  Everything goes through the public module
-surface -> ctypes -> libnmf_b200.so C ABI -> sm_100a kernels; the CPU oracle / reference-generated
+"""GPU parity tests (run with `-m gpu` on an H100).  Everything goes through the public module
+surface -> ctypes -> libnmf_b200.so C ABI -> sm_90a kernels; the CPU oracle / reference-generated
 golden vectors are only the checker.
 
 Tolerances (floating-point path, stated per the task contract):
   * precision="f32" (fused CUDA-core kernels, fp32 everywhere): rtol 2e-4, atol 1e-6 * max|x| after
     <= 50 iterations -- only summation order and libm-vs-CUDA pow/log differ from the reference.
-  * precision="f16" / "f16_split" (tcgen05): rtol 1e-3, atol 1e-5 * max|x| (BASELINE.json north_star).
+  * precision="f16" / "f16_split" (wgmma): rtol 1e-3, atol 1e-5 * max|x| (BASELINE.json north_star).
 """
 import math
 
@@ -157,7 +157,7 @@ def test_kl_update_preserves_marginals_and_decreases_loss(precision):
     eng.close()
 
 
-# ---- tensor-core (tcgen05) path -------------------------------------------------------------------------
+# ---- tensor-core (wgmma) path ---------------------------------------------------------------------------
 TC_RTOL, TC_ATOL_REL = 1e-3, 1e-5     # north_star: rtol 1e-3 (atol = 1e-5 * max|x| for near-zero entries)
 
 

@@ -136,6 +136,24 @@ def test_nmfd_tensor_core_fit_is_bitwise_repeatable():
         assert torch.equal(W, outs[0][0]) and torch.equal(H, outs[0][1])
 
 
+@pytest.mark.parametrize("R", [16, 160])
+def test_nmfd_tensor_core_ranks_above_128_match_oracle(R):
+    """The tensor-core NMFD path runs the H update's contraction in slices of 128 components: a rank above 128 takes two
+    slices and must land on the CPU oracle like a rank that fits in one."""
+    from oracle import mu_oracle as orc
+    torch.manual_seed(5)
+    V = torch.rand(1, 64, 300)
+    W0 = torch.rand(64, R, 9) + 0.1
+    H0 = torch.rand(1, R, 292) + 0.1
+    W, H, _, _ = orc.fit(V, W0, H0, beta=1, tol=float("-inf"), max_iter=5, kind="nmfd")
+    m = NMFD(W=W0, H=H0).cuda()
+    m.fit(V.cuda(), 1, float("-inf"), 5, precision="f16")
+    assert m.last_fit_precision == "f16"
+    for got, want in ((m.W.data.cpu(), W), (m.H.data.cpu(), H)):
+        err = ((got - want).abs() / (RTOL * want.abs() + ATOL_REL * float(want.abs().max()))).max().item()
+        assert err <= 1.0, f"R={R}: {err:.2f} x tolerance"
+
+
 # ---- the loss folded into the W update's contraction pass (nmfb200_nmf_loss_prefetch_w) -----------------------------------
 def _kl_engine(N, C, R):
     from torchnmf_b200 import engine as _engine

@@ -1,7 +1,7 @@
 """Pin the CPU oracle (oracle/mu_oracle.py) against outputs of the real reference.
 
 The fixtures in tests/golden/reference_small.npz were produced by oracle/make_golden.py, which
-imports torchnmf 0.3.5 from /root/reference and runs `fit` from identical initial factors.
+imports torchnmf 0.3.5 (oracle/_ref) and runs `fit` from identical initial factors.
 """
 import math
 
@@ -77,7 +77,7 @@ def test_nmfd_reconstruct_matches_definition():
 
 
 def test_sharded_w_contractions_sum_to_full():
-    # SURVEY 8e: row shards of (V, H) give partial numerators that add up (before relu/eps/l1/l2).
+    # row shards of (V, H) give partial numerators that add up (before relu/eps/l1/l2).
     torch.manual_seed(0)
     V = torch.rand(64, 30); W = torch.rand(30, 5); H = torch.rand(64, 5)
     for beta in (0.5, 1, 2):

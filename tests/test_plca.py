@@ -1,4 +1,4 @@
-"""The PLCA family (SURVEY.md section 8 row f2): `plca.PLCA` and the shift-invariant `SIPLCA` / `SIPLCA2` / `SIPLCA3`
+"""The PLCA family: `plca.PLCA` and the shift-invariant `SIPLCA` / `SIPLCA2` / `SIPLCA3`
 (reference: torchnmf/plca.py:193-625).
 
 Fixtures: tests/golden/reference_next.npz (PLCA) and tests/golden/reference_plca.npz (SIPLCA*), written by
@@ -164,7 +164,7 @@ def test_betamu_convolutive_fused_path_matches_reference(name, return_module):
 
 @pytest.mark.gpu
 def test_siplca_tensor_core_option():
-    """precision="f16": the beta = 1 tcgen05 sliding GEMMs of NMFD under the EM step (opt-in, like PLCA's: the EM recursion
+    """precision="f16": the beta = 1 wgmma sliding GEMMs of NMFD under the EM step (opt-in, like PLCA's: the EM recursion
     keeps the fp16 operand rounding, so the bar here is 3e-3)."""
     c = _case("siplca_tc")
     m = SIPLCA(W=_t(c, "W0"), H=_t(c, "H0"), Z=_t(c, "Z0")).cuda()

@@ -1,4 +1,4 @@
-"""World-size-2 gloo test of the row-sharded fit protocol (SURVEY.md 8e) on CPU.
+"""World-size-2 gloo test of the row-sharded fit protocol on CPU.
 
 Each rank owns a row shard of V and H and a replica of W; `ShardedEngine` inserts one sum-all-reduce
 per W update and one scalar all-reduce per loss evaluation.  The result must equal the unsharded fit
