@@ -80,7 +80,8 @@ __device__ __forceinline__ void bulk_copy_g2s(uint32_t dst, const void* src, uin
 
 // One kernel, four roles of the same pipeline (KIND):
 //   recon / recon-loss : grid (L tiles, C tiles, B);  plain = A = Wr16 tile (rows c), Toeplitz = B (rows l), N = 128
-//   wgrad              : grid (C tiles, R, nsplit);   plain = A = P16 tile (rows c),  Toeplitz = B (rows t), N = 128
+//   wgrad              : grid (C tiles, R x shift blocks, nsplit);  plain = A = P16 tile (rows c),  Toeplitz = B (rows t of
+//                        one block of 128 shifts), N = 128
 //   dgrad              : grid (Lin tiles, nsplit, B); Toeplitz = A (rows j), plain = B = Wf16 rows (c R + r_off + n), N = 128;
 //                        ranks above 128 take one launch per 128 components
 template <int KIND>
@@ -115,6 +116,7 @@ tcnmfd_kernel(const __grid_constant__ CUtensorMap tmPlain, const NmfdTcParams p)
   else { kb0 = (KIND == kWgrad ? blockIdx.z : blockIdx.y) * p.kb_per_split; nkb = p.kb_per_split; }
   const int lkb = (p.L + kKB - 1) / kKB;                    // wgrad: k-blocks per batch element
   const int tkb = p.Tp / kKB;
+  const int ntb = (p.T + kM - 1) / kM;                      // wgrad: blocks of 128 shifts (blockIdx.y = r ntb + tb)
   if (KIND == kWgrad) nkb = max(0, min(nkb, p.B * lkb - kb0));
   if (KIND == kDgrad) nkb = max(0, min(nkb, p.C * tkb - kb0));
   // per k-block: returns the plain tile's TMA coordinates (x = column, y = row), the source row pointer and the index of the
@@ -128,8 +130,8 @@ tcnmfd_kernel(const __grid_constant__ CUtensorMap tmPlain, const NmfdTcParams p)
     } else if (KIND == kWgrad) {
       const int g = kb0 + kb, b = g / lkb, lk = g - b * lkb;
       px = lk * kKB; py = b * p.C + blockIdx.x * kM;
-      src = p.Hp16 + ((int64_t)b * p.R + blockIdx.y) * p.Lp;
-      e0 = p.padl + lk * kKB;                               // row t reads H[l - t]: e0 - t
+      src = p.Hp16 + ((int64_t)b * p.R + blockIdx.y / ntb) * p.Lp;
+      e0 = p.padl + lk * kKB - (blockIdx.y % ntb) * kM;     // row i reads H[l - t] of shift t = 128 tb + i: e0 - i
     } else {
       const int g = kb0 + kb, c = g / tkb, kk = g - c * tkb;
       px = kk * kKB; py = c * p.R + p.r_off;
@@ -273,15 +275,15 @@ tcnmfd_kernel(const __grid_constant__ CUtensorMap tmPlain, const NmfdTcParams p)
             p.loss_part[((int64_t)blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x] = (red[0] + red[1]) + (red[2] + red[3]);
         }
       } else if (KIND == kWgrad) {
-        const int c = blockIdx.x * kM + r128, r = blockIdx.y;
-        float* dst = p.out + (((int64_t)blockIdx.z * p.C + (c < p.C ? c : 0)) * p.R + r) * p.T;    // [split][C][R][T]
+        const int c = blockIdx.x * kM + r128, r = blockIdx.y / ntb, t0 = (blockIdx.y % ntb) * kM;
+        float* dst = p.out + (((int64_t)blockIdx.z * p.C + (c < p.C ? c : 0)) * p.R + r) * p.T + t0;  // [split][C][R][T]
         const bool vec = (p.T & 3) == 0;
 #pragma unroll 1
         for (int j = 0; j < kM / 16; ++j) {
           uint32_t sr[16];
           ld16(j, sr);
-          if (c < p.C && j * 16 < p.T) {
-            if (vec && j * 16 + 16 <= p.T) {
+          if (c < p.C && t0 + j * 16 < p.T) {
+            if (vec && t0 + j * 16 + 16 <= p.T) {
 #pragma unroll
               for (int i = 0; i < 16; i += 4)
                 *reinterpret_cast<float4*>(dst + j * 16 + i) = make_float4(__uint_as_float(sr[i]) * sc, __uint_as_float(sr[i + 1]) * sc,
@@ -289,7 +291,7 @@ tcnmfd_kernel(const __grid_constant__ CUtensorMap tmPlain, const NmfdTcParams p)
             } else {
 #pragma unroll
               for (int i = 0; i < 16; ++i)
-                if (j * 16 + i < p.T) dst[j * 16 + i] = __uint_as_float(sr[i]) * sc;
+                if (t0 + j * 16 + i < p.T) dst[j * 16 + i] = __uint_as_float(sr[i]) * sc;
             }
           }
         }
@@ -513,7 +515,8 @@ struct TcNmfdState {
 };
 
 bool tc_nmfd_supported(const NmfdShape& d, double beta) {
-  return beta == 1.0 && d.R >= 1 && d.R <= 256 && d.T >= 1 && d.L >= d.T;
+  // wgrad's grid.y = R x blocks of 128 shifts
+  return beta == 1.0 && d.R >= 1 && d.R <= 256 && d.T >= 1 && d.L >= d.T && (int64_t)d.R * ceil_div(d.T, kM) <= 65535;
 }
 
 void tc_nmfd_destroy(TcNmfdState* s) {
@@ -534,7 +537,7 @@ int tc_nmfd_create(TcNmfdState** out, const NmfdShape& d) {
   s->Cpad = (int)round_up(d.C, kM);
   const int lkb = (int)ceil_div(d.L, kKB), tkb = s->Tp / kKB;
   // split the K loops of wgrad / dgrad so that the grid is a few waves of 132 CTAs
-  const int64_t tiles_w = ceil_div(d.C, kM) * d.R, tiles_h = ceil_div(d.Lin, kM) * d.B;
+  const int64_t tiles_w = ceil_div(d.C, kM) * d.R * ceil_div(d.T, kM), tiles_h = ceil_div(d.Lin, kM) * d.B;
   int64_t kb_w = (int64_t)d.B * lkb, kb_h = (int64_t)d.C * tkb;
   s->ws_w = (int)std::max<int64_t>(1, std::min<int64_t>(kb_w / 8, ceil_div(132 * 4, tiles_w)));
   s->ws_h = (int)std::max<int64_t>(1, std::min<int64_t>(kb_h / 8, ceil_div(132 * 4, tiles_h)));
@@ -684,7 +687,8 @@ int tc_nmfd_recon(TcNmfdState* s, const float* V, const float* W, const float* H
 int tc_nmfd_wgrad(TcNmfdState* s, const float** part, int* nsplit, cudaStream_t st) {
   NmfdTcParams p = base_params(s, nullptr);
   p.nsplit = s->ws_w; p.kb_per_split = s->kbs_w;
-  dim3 grid((unsigned)ceil_div(s->d.C, kM), (unsigned)s->d.R, (unsigned)s->ws_w);
+  // one CTA per (128 rows c, component r, block of 128 shifts t, split): the Toeplitz tile holds 128 shifts
+  dim3 grid((unsigned)ceil_div(s->d.C, kM), (unsigned)(s->d.R * ceil_div(s->d.T, kM)), (unsigned)s->ws_w);
   int rc = launch<kWgrad>(s, s->tmP, grid, p, st);
   *part = s->part; *nsplit = s->ws_w;
   return rc;
