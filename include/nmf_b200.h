@@ -194,6 +194,25 @@ int nmfb200_nmfd_raw_terms(nmfb200_ctx* ctx, const float* W, const float* H, int
  * path and refreshes only what it knows changed): refresh both at the next call. */
 int nmfb200_nmfd_sync_factors(nmfb200_ctx* ctx);
 
+/* ---- tile plans of the fp32 CUDA-core kernels (host only: no device work, no allocation) -------- */
+
+/* What a context of these sizes runs on the fp32 kernels, from the library's own planners.  `out` receives
+ * NMFB200_NMF_PLAN_LEN values (n must be at least that):
+ *   [0] chunks of the W update's contraction over the N rows    [1] chunks of the H update's over the C columns
+ *   [2] 64-wide tiles per chunk, W update                       [3] the same, H update (the last chunks may be short or empty)
+ *   [4] register blocks RB of the contraction (rank <= 16 RB)   [5] chunks of the loss pass   [6] its tiles per chunk
+ *   [7] blocks of the column sum over N rows (the W update's KL denominator)   [8] over C rows (the H update's) */
+#define NMFB200_NMF_PLAN_LEN 9
+int nmfb200_nmf_plan(int64_t N, int64_t C, int64_t R, int64_t* out, int n);
+/* The same for an NMFD / NMF2D / NMF3D context (arguments as nmfb200_nmfnd_create), NMFB200_NMFD_PLAN_LEN values:
+ *   [0] recon row tile MT (channels)   [1..3] recon grid x, y, z
+ *   [4] dgrad row tile MT (components)   [5] dgrad splits of C   [6..8] dgrad grid x, y, z
+ *   [9..15] wgrad plan mt, tp, nr, no, ntt, nrg, nog   [16] wgrad splits of the lines
+ *   [17], [18] 1 if the W / H ratio stage takes the four-elements-per-thread kernel, else 0 */
+#define NMFB200_NMFD_PLAN_LEN 19
+int nmfb200_nmfd_plan(int64_t B, int64_t C, int ndim, const int64_t* vdims, int64_t R, const int64_t* kdims,
+                      int64_t* out, int n);
+
 /* ---- sparseness-constrained NMF (Hoyer 2004) --------------------------------------------- */
 
 /* Replaces torchnmf.nmf._proj_func (nmf.py:21-49) and the Python loops that call it once per component

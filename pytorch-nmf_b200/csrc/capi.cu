@@ -228,6 +228,21 @@ int nmfb200_precision_for_beta(const nmfb200_ctx* ctx, double beta) {
   return (beta == 1.0 || beta == 2.0) ? ctx->precision : NMFB200_PREC_F16;
 }
 
+int nmfb200_nmf_plan(int64_t N, int64_t C, int64_t R, int64_t* out, int n) {
+  if (!out || n < NMFB200_NMF_PLAN_LEN) return fail(NMFB200_ERR_INVALID, "plan buffer too small");
+  if (N < 1 || C < 1 || R < 1) return fail(NMFB200_ERR_INVALID, "N, C, R must be positive");
+  if (R > 256) return fail(NMFB200_ERR_INVALID, "rank > 256 is not supported");
+  const int nch_w = chunks_for(C, N), nch_h = chunks_for(N, C);
+  SimtNmfPlan pw, ph;
+  simt_nmf_plan(C, N, (int)R, nch_w, &pw);          // W update: F = W (C rows), contracted over the N rows of V
+  simt_nmf_plan(N, C, (int)R, nch_h, &ph);          // H update, and the loss (F = H)
+  const int64_t v[NMFB200_NMF_PLAN_LEN] = {nch_w, nch_h, pw.tiles_per_chunk, ph.tiles_per_chunk, ph.rb, ph.loss_chunks,
+                                           ph.loss_tiles_per_chunk, colsum_scratch_floats(N, 1, 1),
+                                           colsum_scratch_floats(C, 1, 1)};
+  for (int i = 0; i < NMFB200_NMF_PLAN_LEN; ++i) out[i] = v[i];
+  return 0;
+}
+
 int nmfb200_nmf_set_target(nmfb200_ctx* ctx, const float* V, int64_t ldv, void* stream) {
   CTX_GUARD(ctx, 0);
   if (!V || ldv < ctx->C) return fail(NMFB200_ERR_INVALID, "bad target pointer / leading dimension");
@@ -577,10 +592,8 @@ int nmfb200_nmf_contract_only(nmfb200_ctx* ctx, const float* W, const float* H, 
 
 // One context type serves NMFD (one sliding axis) and NMF2D / NMF3D (the last axis slides, the outer ones are loops):
 // vdims / kdims hold the target's and the kernel's sizes over the ndim convolved axes.
-static int nmfd_create_impl(nmfb200_ctx** out, int device, int64_t B, int64_t C, int ndim, const int64_t* vdims,
-                            int64_t R, const int64_t* kdims, int precision) {
-  if (!out) return fail(NMFB200_ERR_INVALID, "out is null");
-  *out = nullptr;
+// The context's shape from the create arguments (validated): the outer axes right-aligned, X2 / T2 innermost of them.
+static int nmfd_shape_of(int64_t B, int64_t C, int ndim, const int64_t* vdims, int64_t R, const int64_t* kdims, NmfdShape* d) {
   if (ndim < 1 || ndim > 3 || !vdims || !kdims) return fail(NMFB200_ERR_INVALID, "1 to 3 convolved axes are supported");
   int64_t X[3] = {1, 1, 1}, K[3] = {1, 1, 1};            // right-aligned: X[2] / K[2] is the last (sliding) axis
   for (int i = 0; i < ndim; ++i) { X[3 - ndim + i] = vdims[i]; K[3 - ndim + i] = kdims[i]; }
@@ -589,11 +602,32 @@ static int nmfd_create_impl(nmfb200_ctx** out, int device, int64_t B, int64_t C,
   for (int i = 0; i < 3; ++i)
     if (K[i] < 1 || X[i] < K[i]) return fail(NMFB200_ERR_INVALID, "bad NMFD sizes");
   if (R > 256) return fail(NMFB200_ERR_INVALID, "rank > 256 is not supported");
-  if (precision != NMFB200_PREC_AUTO && precision != NMFB200_PREC_F32 && precision != NMFB200_PREC_F16)
-    return fail(NMFB200_ERR_INVALID, "NMFD precision must be auto, f32 or f16");
   if (B * C * X[0] * X[1] * L > (int64_t)1 << 40 || X[0] * X[1] * L > (int64_t)1 << 30 || K[0] * K[1] * T > (int64_t)1 << 24)
     return fail(NMFB200_ERR_INVALID, "NMFD target too large");
-  const bool one_d = X[0] == 1 && X[1] == 1;
+  *d = NmfdShape{(int)B, (int)C, (int)L, (int)R, (int)T, (int)(L - T + 1)};
+  d->X1 = (int)X[0]; d->X2 = (int)X[1]; d->T1 = (int)K[0]; d->T2 = (int)K[1];
+  return 0;
+}
+
+// The ratio stage's view of one NMFD factor (which = 0: W, 1: H): rows of R components x `inner` elements, one partial slab
+// per split.
+static ApplyArgs nmfd_apply_shape(const NmfdShape& d, int which, int nsplit) {
+  const int64_t inner = which == 0 ? d.w_inner() : d.h_inner();
+  ApplyArgs a{};
+  a.numel = (int64_t)(which == 0 ? d.C : d.B) * d.R * inner; a.R = d.R; a.inner = inner; a.rowlen = (int64_t)d.R * inner;
+  a.chunk_stride = a.numel; a.ldp = a.rowlen; a.nchunks = nsplit; a.out_scale = nullptr; a.absmax_bits = nullptr;
+  return a;
+}
+
+static int nmfd_create_impl(nmfb200_ctx** out, int device, int64_t B, int64_t C, int ndim, const int64_t* vdims,
+                            int64_t R, const int64_t* kdims, int precision) {
+  if (!out) return fail(NMFB200_ERR_INVALID, "out is null");
+  *out = nullptr;
+  NmfdShape shape;
+  if (int rc = nmfd_shape_of(B, C, ndim, vdims, R, kdims, &shape)) return rc;
+  if (precision != NMFB200_PREC_AUTO && precision != NMFB200_PREC_F32 && precision != NMFB200_PREC_F16)
+    return fail(NMFB200_ERR_INVALID, "NMFD precision must be auto, f32 or f16");
+  const bool one_d = shape.one_d();
   if (!one_d && precision == NMFB200_PREC_F16)
     return fail(NMFB200_ERR_INVALID, "NMF2D / NMF3D run on the fp32 kernels (precision auto or f32)");
   DeviceGuard guard(device);
@@ -602,8 +636,7 @@ static int nmfd_create_impl(nmfb200_ctx** out, int device, int64_t B, int64_t C,
   if (!c) return fail(NMFB200_ERR_INVALID, "out of host memory");
   c->kind = 1; c->device = device; c->precision = precision == NMFB200_PREC_F32 ? NMFB200_PREC_F32 : NMFB200_PREC_F16; c->R = R;
   c->auto_mode = precision == NMFB200_PREC_AUTO;
-  c->d = NmfdShape{(int)B, (int)C, (int)L, (int)R, (int)T, (int)(L - T + 1)};
-  c->d.X1 = (int)X[0]; c->d.X2 = (int)X[1]; c->d.T1 = (int)K[0]; c->d.T2 = (int)K[1];
+  c->d = shape;
   c->dgrad_nsplit = nmfd_dgrad_nsplit(c->d);
   c->wgrad_nsplit = nmfd_wgrad_nsplit(c->d);
   int64_t pf = (int64_t)c->wgrad_nsplit * C * R * c->d.w_inner();
@@ -696,10 +729,7 @@ static int nmfd_phi(nmfb200_ctx* c, const float* W, const float* H, double beta,
 static int nmfd_terms(nmfb200_ctx* ctx, const float* W, const float* H, int which, double beta, ApplyArgs& a, bool* tc,
                       cudaStream_t st) {
   const NmfdShape& d = ctx->d;
-  const int64_t inner = which == 0 ? d.w_inner() : d.h_inner();
-  a = ApplyArgs{};
-  a.numel = (int64_t)(which == 0 ? d.C : d.B) * d.R * inner; a.R = d.R; a.inner = inner; a.rowlen = (int64_t)d.R * inner;
-  a.chunk_stride = a.numel; a.ldp = a.rowlen; a.out_scale = nullptr; a.absmax_bits = nullptr;
+  a = nmfd_apply_shape(d, which, 1);
   *tc = nmfd_use_tc(ctx, beta);
   if (*tc) {
     int rc = nmfd_tc_recon(ctx, W, H, false, nullptr, st);
@@ -728,6 +758,23 @@ static int nmfd_terms(nmfb200_ctx* ctx, const float* W, const float* H, int whic
   }
   if (rc) return rc;
   a.num = ctx->num; a.den = beta == 1.0 ? nullptr : ctx->den; a.nchunks = nsplit; a.kl_den = kl;
+  return 0;
+}
+
+int nmfb200_nmfd_plan(int64_t B, int64_t C, int ndim, const int64_t* vdims, int64_t R, const int64_t* kdims, int64_t* out,
+                      int n) {
+  if (!out || n < NMFB200_NMFD_PLAN_LEN) return fail(NMFB200_ERR_INVALID, "plan buffer too small");
+  NmfdShape d;
+  if (int rc = nmfd_shape_of(B, C, ndim, vdims, R, kdims, &d)) return rc;
+  NmfdPlan p;
+  nmfd_plan(d, &p);
+  const WgradPlan& w = p.wgrad;
+  const int64_t v[NMFB200_NMFD_PLAN_LEN] = {
+      p.recon_mt, p.recon_grid.x, p.recon_grid.y, p.recon_grid.z,
+      p.dgrad_mt, p.dgrad_nsplit, p.dgrad_grid.x, p.dgrad_grid.y, p.dgrad_grid.z,
+      w.mt, w.tp, w.nr, w.no, w.ntt, w.nrg, w.nog, p.wgrad_nsplit,
+      apply_update_vec4_shape(nmfd_apply_shape(d, 0, p.wgrad_nsplit)), apply_update_vec4_shape(nmfd_apply_shape(d, 1, p.dgrad_nsplit))};
+  for (int i = 0; i < NMFB200_NMFD_PLAN_LEN; ++i) out[i] = v[i];
   return 0;
 }
 

@@ -64,6 +64,10 @@ int simt_nmf_loss(const float* V, int64_t ldv, const float* F, const float* G, i
                   int R, double beta, double* block_partials, int max_blocks, double* loss_dev,
                   cudaStream_t st);
 int simt_nmf_max_blocks(int64_t Mr, int64_t Nc);
+// The tile plan of simt_nmf_contract (Mr rows, Nc contracted columns, `nchunks` chunks) and of simt_nmf_loss: the register
+// blocks RB of 16 components, the 64-column tiles per chunk (the last chunks may be short or empty) and the loss's chunks.
+struct SimtNmfPlan { int rb; int64_t tiles_per_chunk; int loss_chunks; int64_t loss_tiles_per_chunk; };
+void simt_nmf_plan(int64_t Mr, int64_t Nc, int R, int nchunks, SimtNmfPlan* p);
 
 // update.cu --------------------------------------------------------------------------------
 // nmf.py:78-92 on a flattened parameter of `numel` elements whose rank index is
@@ -80,6 +84,8 @@ struct ApplyArgs {
   const float* kappa_vec;     // [R]
 };
 int apply_update(const ApplyArgs& a, cudaStream_t st);
+// whether apply_update takes its four-elements-per-thread kernel for this shape (16-byte aligned buffers provided)
+bool apply_update_vec4_shape(const ApplyArgs& a);
 // num_out[i] (and den_out[i] when a.den) = what the ratio stage would read for element i: summed partials + centring term
 int raw_sum(const ApplyArgs& a, float* num_out, float* den_out, cudaStream_t st);
 // sums[r] = sum over all other dims of x viewed as (outer, R, inner); deterministic two-stage.
@@ -138,5 +144,11 @@ int nmfd_wgrad_nsplit(const NmfdShape& s);
 // out[split][b,r,j] = sum_{c in split, t} W[c,r,t] G[b,c,j+t]   (j, t multi-indices)
 int nmfd_dgrad(const NmfdShape& s, const float* G, const float* W, float* out, int nsplit, cudaStream_t st);
 int nmfd_dgrad_nsplit(const NmfdShape& s);
+// wgrad's block plan (nmfd.cu): row tile MT of channels, TP = roundup(min(T, 64), 4) offsets of NR components for NO outer
+// kernel offsets per block; NTT x NRG x NOG column blocks
+struct WgradPlan { int mt, tp, nr, no, ntt, nrg, nog; };
+// what nmfd_recon_phi / nmfd_dgrad / nmfd_wgrad launch for this shape, with the splits the library uses
+struct NmfdPlan { int recon_mt; dim3 recon_grid; int dgrad_mt, dgrad_nsplit; dim3 dgrad_grid; WgradPlan wgrad; int wgrad_nsplit; };
+void nmfd_plan(const NmfdShape& s, NmfdPlan* p);
 
 }  // namespace nmfb200

@@ -221,7 +221,6 @@ nmfd_slide_kernel(NmfdShape s, SlideArgs a) {
 // A block owns MT channels x NCOL columns.  A column is (outer offset, component, offset t): TP = roundup(T, 4) <= 64 offsets
 // of NR components (their H windows are staged once per line) for each of NO outer offsets (each with its own G tile).
 // grid (t tiles * r groups * outer-offset groups, c tiles, nsplit), 256 threads.
-struct WgradPlan { int mt, tp, nr, no, ntt, nrg, nog; };
 
 template <int MT>
 __global__ void __launch_bounds__(256)
@@ -429,6 +428,16 @@ int nmfd_dgrad_nsplit(const NmfdShape& s) {
   if (ns > 64) ns = 64;
   if (ns < 1) ns = 1;
   return (int)ns;
+}
+
+void nmfd_plan(const NmfdShape& s, NmfdPlan* p) {
+  p->recon_mt = row_tile(s.C);
+  p->recon_grid = slide_grid(s, true, p->recon_mt, s.C, 1);
+  p->dgrad_mt = row_tile(s.R);
+  p->dgrad_nsplit = nmfd_dgrad_nsplit(s);
+  p->dgrad_grid = slide_grid(s, false, p->dgrad_mt, s.R, p->dgrad_nsplit);
+  p->wgrad = wgrad_plan(s);
+  p->wgrad_nsplit = nmfd_wgrad_nsplit(s);
 }
 
 int nmfd_dgrad(const NmfdShape& s, const float* G, const float* W, float* out, int nsplit, cudaStream_t st) {

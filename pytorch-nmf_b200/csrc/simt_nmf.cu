@@ -15,6 +15,14 @@ namespace {
 constexpr int kTile = 64;   // rows per CTA and columns per tile
 constexpr int kLd = 68;     // padded shared-memory pitch (floats): float4-aligned, conflict-free
 
+// 64-column tiles per chunk of the contracted dimension; the last chunks may be short or hold no tile at all
+__host__ __device__ inline int64_t chunk_tiles(int64_t Nc, int nchunks) {
+  return ((Nc + kTile - 1) / kTile + nchunks - 1) / nchunks;
+}
+
+// register blocks of 16 components per thread row of the contraction kernel (Rp = 16 RB >= R)
+inline int contract_rb(int R) { return R <= 16 ? 1 : R <= 32 ? 2 : R <= 64 ? 4 : R <= 128 ? 8 : 16; }
+
 template <int MODE>
 __device__ __forceinline__ void phi(float v, float s, float bm2, float bm1, float& pn, float& pp) {
   if (MODE == kKL) {
@@ -53,7 +61,7 @@ simt_contract_kernel(const float* __restrict__ V, int64_t ldv, const float* __re
   const int64_t m0 = (int64_t)blockIdx.x * kTile;
   const int chunk = blockIdx.y;
   const int64_t tiles_total = (Nc + kTile - 1) / kTile;
-  const int64_t tpc = (tiles_total + nchunks - 1) / nchunks;
+  const int64_t tpc = chunk_tiles(Nc, nchunks);
   const int64_t tile_begin = chunk * tpc;
   const int64_t tile_end = min(tiles_total, tile_begin + tpc);
 
@@ -238,7 +246,7 @@ simt_loss_kernel(const float* __restrict__ V, int64_t ldv, const float* __restri
   const int64_t m0 = (int64_t)blockIdx.x * kTile;
   const int chunk = blockIdx.y;
   const int64_t tiles_total = (Nc + kTile - 1) / kTile;
-  const int64_t tpc = (tiles_total + nchunks - 1) / nchunks;
+  const int64_t tpc = chunk_tiles(Nc, nchunks);
   const int64_t tile_begin = chunk * tpc;
   const int64_t tile_end = min(tiles_total, tile_begin + tpc);
   for (int idx = tid; idx < kTile * Rp; idx += 256) {
@@ -305,6 +313,13 @@ int loss_chunks(int64_t Mr, int64_t Nc) {
 
 int simt_nmf_max_blocks(int64_t Mr, int64_t Nc) { return (int)(ceil_div(Mr, kTile) * loss_chunks(Mr, Nc)); }
 
+void simt_nmf_plan(int64_t Mr, int64_t Nc, int R, int nchunks, SimtNmfPlan* p) {
+  p->rb = contract_rb(R);
+  p->tiles_per_chunk = chunk_tiles(Nc, nchunks);
+  p->loss_chunks = loss_chunks(Mr, Nc);
+  p->loss_tiles_per_chunk = chunk_tiles(Nc, p->loss_chunks);
+}
+
 int sum_partials(const double* p, int n, double* out, cudaStream_t st) {
   sum_partials_kernel<<<1, 256, 0, st>>>(p, n, out);
   NMF_LAUNCH_CHECK();
@@ -321,11 +336,13 @@ int simt_nmf_contract(const float* V, int64_t ldv, int trans, const float* F, co
 #define NMF_RB(RBV)                                                                                       \
   return launch_contract_rb<RBV>(trans, mode, grid, st, V, ldv, F, G, Mr, Nc, R, bm2, bm1, nchunks, num, den, \
                                  ldp, chunk_stride)
-  if (R <= 16) NMF_RB(1);
-  if (R <= 32) NMF_RB(2);
-  if (R <= 64) NMF_RB(4);
-  if (R <= 128) NMF_RB(8);
-  NMF_RB(16);
+  switch (contract_rb(R)) {
+    case 1: NMF_RB(1);
+    case 2: NMF_RB(2);
+    case 4: NMF_RB(4);
+    case 8: NMF_RB(8);
+    default: NMF_RB(16);
+  }
 #undef NMF_RB
 }
 

@@ -221,11 +221,14 @@ apply_update_vec4_kernel(ApplyArgs a) {
 
 static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
+bool apply_update_vec4_shape(const ApplyArgs& a) {
+  return a.inner % 4 == 0 && a.rowlen % 4 == 0 && a.ldp % 4 == 0 && a.numel % 4 == 0 &&
+         (a.nchunks == 1 || a.chunk_stride % 4 == 0);
+}
+
 int apply_update(const ApplyArgs& a, cudaStream_t st) {
   if (a.numel <= 0) return 0;
-  const bool vec4 = a.inner % 4 == 0 && a.rowlen % 4 == 0 && a.ldp % 4 == 0 && a.numel % 4 == 0 &&
-                    (a.nchunks == 1 || a.chunk_stride % 4 == 0) && aligned16(a.param) && aligned16(a.num) &&
-                    (!a.den || aligned16(a.den));
+  const bool vec4 = apply_update_vec4_shape(a) && aligned16(a.param) && aligned16(a.num) && (!a.den || aligned16(a.den));
   if (vec4)
     apply_update_vec4_kernel<<<(unsigned)ceil_div(a.numel / 4, 256), 256, 0, st>>>(a);
   else

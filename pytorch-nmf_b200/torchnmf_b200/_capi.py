@@ -60,7 +60,10 @@ SIGNATURES = {
     "nmfb200_nmfd_raw_terms": (_int, [_vp, _vp, _vp, _int, _dbl, _vp, _vp]),
     "nmfb200_nmfd_sync_factors": (_int, [_vp]),
     "nmfb200_hoyer_project": (_int, [_int, _vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp]),
+    "nmfb200_nmf_plan": (_int, [_i64, _i64, _i64, _c.POINTER(_i64), _int]),
+    "nmfb200_nmfd_plan": (_int, [_i64, _i64, _int, _c.POINTER(_i64), _i64, _c.POINTER(_i64), _c.POINTER(_i64), _int]),
 }
+NMF_PLAN_LEN, NMFD_PLAN_LEN = 9, 19         # include/nmf_b200.h
 
 _lib = None
 
@@ -107,3 +110,22 @@ def build_info():
 
 def launch_count():
     return int(load().nmfb200_launch_count())
+
+
+def nmf_plan(N, C, R):
+    """The fp32 kernels' tile plan of an (N, C) rank-R NMF context (nmfb200_nmf_plan), as a dict; no device needed."""
+    out = (_i64 * NMF_PLAN_LEN)()
+    check(load().nmfb200_nmf_plan(N, C, R, out, NMF_PLAN_LEN))
+    keys = ("nch_w", "nch_h", "tpc_w", "tpc_h", "rb", "loss_chunks", "loss_tpc", "colsum_blocks_n", "colsum_blocks_c")
+    return dict(zip(keys, out))
+
+
+def nmfd_plan(B, C, vdims, R, kdims):
+    """The fp32 kernels' tile plan of an NMFD / NMF2D / NMF3D context (nmfb200_nmfd_plan), as a dict; no device needed."""
+    nd = len(vdims)
+    out = (_i64 * NMFD_PLAN_LEN)()
+    check(load().nmfb200_nmfd_plan(B, C, nd, (_i64 * nd)(*vdims), R, (_i64 * nd)(*kdims), out, NMFD_PLAN_LEN))
+    v = list(out)
+    return {"recon_mt": v[0], "recon_grid": tuple(v[1:4]), "dgrad_mt": v[4], "dgrad_nsplit": v[5],
+            "dgrad_grid": tuple(v[6:9]), "wgrad": dict(zip(("mt", "tp", "nr", "no", "ntt", "nrg", "nog"), v[9:16])),
+            "wgrad_nsplit": v[16], "vec4_w": bool(v[17]), "vec4_h": bool(v[18])}
