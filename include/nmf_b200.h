@@ -126,7 +126,10 @@ int nmfb200_nmf_w_partial(nmfb200_ctx* ctx, const float* W, const float* H, doub
  * touching either: `out` receives the numerator relu-free (rows*R: the first backward pass of nmf.py:76-78 /
  * trainer.py:91-93), then colsum(other factor) (R, beta == 1: nmf.py:122-131) or the raw denominator (rows*R: the second
  * backward pass, nmf.py:82 / trainer.py:95-96).  This is what torchnmf.trainer.BetaMu.step (trainer.py:36-121) and
- * torchnmf.plca (plca.py:252-253: the simultaneous W / H / Z updates from ONE V / (W Z H) ratio) are built from. */
+ * torchnmf.plca (plca.py:252-253: the simultaneous W / H / Z updates from ONE V / (W Z H) ratio) are built from.
+ * A sparse target (nmfb200_nmf_set_target_sparse) serves beta 1 and 2 with the same layout, from the same kernels as its
+ * update: the numerator at the non-zeros only, the beta-2 denominator F (other^T other); any other beta returns
+ * NMFB200_ERR_INVALID. */
 int64_t nmfb200_nmf_raw_terms_numel(const nmfb200_ctx* ctx, int which, double beta);
 int nmfb200_nmf_raw_terms(nmfb200_ctx* ctx, const float* W, const float* H, int which, double beta,
                           float* out, void* stream);
@@ -204,6 +207,13 @@ int nmfb200_nmfd_sync_factors(nmfb200_ctx* ctx);
  *   [7] blocks of the column sum over N rows (the W update's KL denominator)   [8] over C rows (the H update's) */
 #define NMFB200_NMF_PLAN_LEN 9
 int nmfb200_nmf_plan(int64_t N, int64_t C, int64_t R, int64_t* out, int n);
+/* The same for the sparse-target kernels of an (N, C) rank-R context, NMFB200_SPARSE_PLAN_LEN values:
+ *   [0] rank floats per lane of the warp-per-row kernels (1, 2, 4, 8)   [1] Gram passes of 4096 (a, b) pairs
+ *   [2] Gram rows per block over the N rows of H (a multiple of 32)   [3] its blocks (at most 128, the last may be short)
+ *   [4], [5] the same over the C rows of W   [6] blocks (8 rows each) over N: the H update's gathers and the loss's partials
+ *   [7] over C: the W update's */
+#define NMFB200_SPARSE_PLAN_LEN 8
+int nmfb200_nmf_sparse_plan(int64_t N, int64_t C, int64_t R, int64_t* out, int n);
 /* The same for an NMFD / NMF2D / NMF3D context (arguments as nmfb200_nmfnd_create), NMFB200_NMFD_PLAN_LEN values:
  *   [0] recon row tile MT (channels)   [1..3] recon grid x, y, z
  *   [4] dgrad row tile MT (components)   [5] dgrad splits of C   [6..8] dgrad grid x, y, z

@@ -243,6 +243,20 @@ int nmfb200_nmf_plan(int64_t N, int64_t C, int64_t R, int64_t* out, int n) {
   return 0;
 }
 
+int nmfb200_nmf_sparse_plan(int64_t N, int64_t C, int64_t R, int64_t* out, int n) {
+  if (!out || n < NMFB200_SPARSE_PLAN_LEN) return fail(NMFB200_ERR_INVALID, "plan buffer too small");
+  if (N < 1 || C < 1 || R < 1) return fail(NMFB200_ERR_INVALID, "N, C, R must be positive");
+  if (R > 256) return fail(NMFB200_ERR_INVALID, "rank > 256 is not supported");
+  int64_t rpb_n, rpb_c;
+  int nb_n, nb_c;
+  sparse_gram_plan(N, &rpb_n, &nb_n);               // H^T H: the W update's beta-2 denominator, the beta-2 loss
+  sparse_gram_plan(C, &rpb_c, &nb_c);               // W^T W: the H update's, the loss
+  const int64_t v[NMFB200_SPARSE_PLAN_LEN] = {sparse_rpl((int)R), sparse_gram_passes((int)R), rpb_n, nb_n, rpb_c, nb_c,
+                                              sparse_gather_blocks(N), sparse_gather_blocks(C)};
+  for (int i = 0; i < NMFB200_SPARSE_PLAN_LEN; ++i) out[i] = v[i];
+  return 0;
+}
+
 int nmfb200_nmf_set_target(nmfb200_ctx* ctx, const float* V, int64_t ldv, void* stream) {
   CTX_GUARD(ctx, 0);
   if (!V || ldv < ctx->C) return fail(NMFB200_ERR_INVALID, "bad target pointer / leading dimension");
@@ -295,7 +309,7 @@ int nmfb200_nmf_set_target_sparse(nmfb200_ctx* ctx, int64_t nnz, const int64_t* 
   if (!ctx->sp_gram) {
     const int64_t R = ctx->R;
     NMF_CUDA_CHECK(cudaMalloc(&ctx->sp_gram, (size_t)(2 * R * R + sparse_gram_part_floats((int)R)) * sizeof(float)));
-    NMF_CUDA_CHECK(cudaMalloc(&ctx->sp_loss_part, (size_t)sparse_loss_blocks(ctx->N) * sizeof(double)));
+    NMF_CUDA_CHECK(cudaMalloc(&ctx->sp_loss_part, (size_t)sparse_gather_blocks(ctx->N) * sizeof(double)));
   }
   ctx->sp_crow = crow; ctx->sp_col = col; ctx->sp_val = val; ctx->sp_ccol = ccol; ctx->sp_row = row; ctx->sp_val_t = val_t;
   ctx->sp_vnorm_kl = v_norm_kl; ctx->sp_vnorm_eu = v_norm_eu;
@@ -304,34 +318,43 @@ int nmfb200_nmf_set_target_sparse(nmfb200_ctx* ctx, int64_t nnz, const int64_t* 
 }
 
 namespace {
-// one factor update on the compressed form whose segments are that factor's rows (which = 0: W over CSC, 1: H over CSR)
-int sparse_update(nmfb200_ctx* ctx, int which, float* F, const float* other, double beta, double gamma, double l1_reg,
-                  double l2_reg, cudaStream_t st) {
+// Raw terms of one factor's update on the compressed form whose segments are that factor's rows (which = 0: W over CSC,
+// 1: H over CSR): the numerator (rows x R) into `num`; into `den` the colsum of the other factor (R, beta 1) or the raw
+// denominator F (other^T other) (rows x R, beta 2).  Shared by the update and nmfb200_nmf_raw_terms.
+int sparse_terms(nmfb200_ctx* ctx, int which, const float* F, const float* other, double beta, float* num, float* den,
+                 cudaStream_t st) {
   if (beta != 1.0 && beta != 2.0) return fail(NMFB200_ERR_INVALID, "sparse targets: beta must be 1 or 2 (densify the target for other beta)");
   const int R = (int)ctx->R;
   const int64_t rows = which == 0 ? ctx->C : ctx->N, orows = which == 0 ? ctx->N : ctx->C;
   const int64_t* ptr = which == 0 ? ctx->sp_ccol : ctx->sp_crow;
   const int64_t* idx = which == 0 ? ctx->sp_row : ctx->sp_col;
   const float* val = which == 0 ? ctx->sp_val_t : ctx->sp_val;
-  int rc = sparse_numerator(ptr, idx, val, F, other, R, rows, beta, ctx->num, st);
+  int rc = sparse_numerator(ptr, idx, val, F, other, R, rows, beta, num, st);
   if (rc) return rc;
-  float* kl = nullptr;
-  if (beta == 1.0) {
-    kl = ctx->colsum + (1 - which) * R;                        // colsum of the OTHER factor, nmf.py:122-131
-    rc = factor_colsum(other, orows, R, 1, ctx->cs_scratch, ctx->cs_scratch_floats, kl, st);
-  } else {
-    rc = ensure_den(ctx);
+  if (beta == 1.0)                                             // colsum of the OTHER factor, nmf.py:122-131
+    return factor_colsum(other, orows, R, 1, ctx->cs_scratch, ctx->cs_scratch_floats, den, st);
+  float* G = ctx->sp_gram + (1 - which) * R * R;               // Gram matrix of the other factor
+  rc = sparse_gram(other, orows, R, ctx->sp_gram + 2 * R * R, G, st);
+  if (rc) return rc;
+  return sparse_rows_times_gram(F, G, rows, R, den, st);       // nmf.py:609
+}
+
+// one factor update: sparse_terms into the context's scratch, then the ratio stage
+int sparse_update(nmfb200_ctx* ctx, int which, float* F, const float* other, double beta, double gamma, double l1_reg,
+                  double l2_reg, cudaStream_t st) {
+  const int R = (int)ctx->R;
+  const int64_t rows = which == 0 ? ctx->C : ctx->N;
+  if (beta == 2.0) {
+    int rc = ensure_den(ctx);
     if (rc) return rc;
-    float* G = ctx->sp_gram + (1 - which) * R * R;             // Gram matrix of the other factor
-    rc = sparse_gram(other, orows, R, ctx->sp_gram + 2 * R * R, G, st);
-    if (rc) return rc;
-    rc = sparse_rows_times_gram(F, G, rows, R, ctx->den, st);  // nmf.py:609
   }
+  float* den = beta == 1.0 ? ctx->colsum + (1 - which) * R : ctx->den;
+  int rc = sparse_terms(ctx, which, F, other, beta, ctx->num, den, st);
   if (rc) return rc;
   ApplyArgs a{};
   a.param = F; a.numel = rows * R; a.R = R; a.inner = 1; a.rowlen = R;
-  a.num = ctx->num; a.den = beta == 1.0 ? nullptr : ctx->den; a.nchunks = 1; a.chunk_stride = 0;
-  a.ldp = R; a.kl_den = kl; a.out_scale = nullptr;
+  a.num = ctx->num; a.den = beta == 1.0 ? nullptr : den; a.nchunks = 1; a.chunk_stride = 0;
+  a.ldp = R; a.kl_den = beta == 1.0 ? den : nullptr; a.out_scale = nullptr;
   a.gamma = (float)gamma; a.l1 = (float)l1_reg; a.l2 = (float)l2_reg; a.absmax_bits = nullptr;
   return apply_update(a, st);
 }
@@ -500,14 +523,14 @@ int nmfb200_nmf_raw_terms(nmfb200_ctx* ctx, const float* W, const float* H, int 
                           void* stream) {
   CTX_GUARD(ctx, 0);
   if (!ctx->has_target) return fail(NMFB200_ERR_STATE, "set_target has not been called");
-  if (ctx->sparse) return fail(NMFB200_ERR_STATE, "not available for a sparse target");
   if (!W || !H || !out || (which != 0 && which != 1)) return fail(NMFB200_ERR_INVALID, "bad argument");
   cudaStream_t st = (cudaStream_t)stream;
+  const int64_t rows = which == 0 ? ctx->C : ctx->N;
+  const int64_t RR = rows * ctx->R;
+  if (ctx->sparse) return sparse_terms(ctx, which, which == 0 ? W : H, which == 0 ? H : W, beta, out, out + RR, st);
   if (use_tc(ctx, beta) && tc_supports_partial(ctx->tc, beta)) return tc_raw_terms(ctx->tc, which, W, H, beta, out, st);
   int rc = which == 0 ? simt_contract_w(ctx, W, H, beta, st) : simt_contract_h(ctx, W, H, beta, st);
   if (rc) return rc;
-  const int64_t rows = which == 0 ? ctx->C : ctx->N;
-  const int64_t RR = rows * ctx->R;
   const int nch = which == 0 ? ctx->nch_w : ctx->nch_h;
   rc = reduce_chunks(ctx->num, nch, RR, rows, (int)ctx->R, ctx->R, out, st);
   if (rc) return rc;

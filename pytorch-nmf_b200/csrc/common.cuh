@@ -117,7 +117,12 @@ int sparse_rows_times_gram(const float* F, const float* G, int64_t rows, int R, 
 int sparse_loss(const int64_t* crow, const int64_t* col, const float* val, const float* H, const float* W, int R, int64_t N,
                 double beta, const float* pos_a, const float* pos_b, double v_norm, double* loss_part, double* loss_dev,
                 cudaStream_t st);
-int sparse_loss_blocks(int64_t N);
+// launch plans (host only): rank floats per lane; blocks over nseg segments / rows (the loss: N, its partials); Gram rows per
+// block and blocks over `rows` rows; Gram passes of 4096 pairs
+int sparse_rpl(int R);
+int64_t sparse_gather_blocks(int64_t nseg);
+void sparse_gram_plan(int64_t rows, int64_t* rpb, int* nb);
+int sparse_gram_passes(int R);
 
 // nmfd.cu ----------------------------------------------------------------------------------
 // L, T, Lin are the sizes along the LAST (contiguous) axis; NMF2D / NMF3D (nmf.py:782-942) add up to two outer axes of the

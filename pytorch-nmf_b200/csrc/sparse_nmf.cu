@@ -17,6 +17,7 @@ namespace nmfb200 {
 namespace {
 
 enum SpMode : int { kSpKL = 0, kSpEU = 1, kSpKLLoss = 2, kSpEULoss = 3 };
+constexpr int kSpGramPass = 256 * 16;                 // Gram pairs per pass of sp_gram_part_kernel (16 per thread)
 
 template <int RPL, int MODE>
 __global__ void __launch_bounds__(256)
@@ -91,7 +92,7 @@ sp_gram_part_kernel(const float* __restrict__ F, int64_t rows, int R, int64_t rp
   const int64_t r0 = (int64_t)blockIdx.x * rpb, r1 = min(rows, r0 + rpb);
   const int npairs = R * R;
   float acc[16];                                      // R <= 64: 4096 / 256; larger ranks loop below
-  for (int base = 0; base < npairs; base += 256 * 16) {
+  for (int base = 0; base < npairs; base += kSpGramPass) {
 #pragma unroll
     for (int k = 0; k < 16; ++k) acc[k] = 0.f;
     for (int64_t rr = r0; rr < r1; rr += 32) {
@@ -155,11 +156,30 @@ __global__ void sp_loss_final_kernel(const double* __restrict__ neg_part, int np
   *out = v_norm + scale * pos - neg;
 }
 
+}  // namespace
+
+// Launch plans, shared by the launchers below and by nmfb200_nmf_sparse_plan.
+// Rank floats per lane of the warp-per-segment kernels: 1, 2, 4 or 8 (R <= 32, 64, 128, 256).
+int sparse_rpl(int R) {
+  const int rpl = (R + 31) / 32;
+  return rpl <= 1 ? 1 : rpl <= 2 ? 2 : rpl <= 4 ? 4 : 8;
+}
+// Blocks of the warp-per-segment kernels (8 warps each) over nseg segments or rows.
+int64_t sparse_gather_blocks(int64_t nseg) { return ceil_div(nseg, 8); }
+// Gram of a rows x R factor: at most 128 blocks of rpb rows (a multiple of the 32-row slab), the last one possibly short.
+void sparse_gram_plan(int64_t rows, int64_t* rpb, int* nb) {
+  *rpb = round_up(ceil_div(rows, 128), 32);
+  *nb = (int)ceil_div(rows, *rpb);
+}
+int sparse_gram_passes(int R) { return (int)ceil_div((int64_t)R * R, kSpGramPass); }
+
+namespace {
+
 template <int MODE>
 int launch_gather(const int64_t* ptr, const int64_t* idx, const float* val, const float* Fs, const float* Fo, int R,
                   int64_t nseg, float* out, double* loss_part, cudaStream_t st) {
-  const unsigned grid = (unsigned)ceil_div(nseg, 8);
-  const int rpl = (R + 31) / 32;
+  const unsigned grid = (unsigned)sparse_gather_blocks(nseg);
+  const int rpl = sparse_rpl(R);
   if (rpl <= 1) sp_gather_kernel<1, MODE><<<grid, 256, 0, st>>>(ptr, idx, val, Fs, Fo, R, nseg, out, loss_part);
   else if (rpl <= 2) sp_gather_kernel<2, MODE><<<grid, 256, 0, st>>>(ptr, idx, val, Fs, Fo, R, nseg, out, loss_part);
   else if (rpl <= 4) sp_gather_kernel<4, MODE><<<grid, 256, 0, st>>>(ptr, idx, val, Fs, Fo, R, nseg, out, loss_part);
@@ -171,7 +191,6 @@ int launch_gather(const int64_t* ptr, const int64_t* idx, const float* val, cons
 }  // namespace
 
 int64_t sparse_gram_part_floats(int R) { return (int64_t)128 * R * R; }
-int sparse_loss_blocks(int64_t N) { return (int)ceil_div(N, 8); }
 
 // raw numerator of one factor update: out (nseg x R); ptr / idx / val = the compressed form whose segments are that factor's rows
 int sparse_numerator(const int64_t* ptr, const int64_t* idx, const float* val, const float* Fself, const float* Fother,
@@ -181,8 +200,9 @@ int sparse_numerator(const int64_t* ptr, const int64_t* idx, const float* val, c
 }
 
 int sparse_gram(const float* F, int64_t rows, int R, float* part, float* out, cudaStream_t st) {
-  const int64_t rpb = round_up(ceil_div(rows, 128), 32);
-  const int nb = (int)ceil_div(rows, rpb);
+  int64_t rpb;
+  int nb;
+  sparse_gram_plan(rows, &rpb, &nb);
   sp_gram_part_kernel<<<nb, 256, 32 * R * sizeof(float), st>>>(F, rows, R, rpb, part);
   NMF_LAUNCH_CHECK();
   sp_gram_sum_kernel<<<(unsigned)ceil_div(R * R, 256), 256, 0, st>>>(part, nb, R * R, out);
@@ -191,8 +211,8 @@ int sparse_gram(const float* F, int64_t rows, int R, float* part, float* out, cu
 }
 
 int sparse_rows_times_gram(const float* F, const float* G, int64_t rows, int R, float* out, cudaStream_t st) {
-  const unsigned grid = (unsigned)ceil_div(rows, 8);
-  const int rpl = (R + 31) / 32;
+  const unsigned grid = (unsigned)sparse_gather_blocks(rows);
+  const int rpl = sparse_rpl(R);
   if (rpl <= 1) sp_rows_times_gram_kernel<1><<<grid, 256, 0, st>>>(F, G, rows, R, out);
   else if (rpl <= 2) sp_rows_times_gram_kernel<2><<<grid, 256, 0, st>>>(F, G, rows, R, out);
   else if (rpl <= 4) sp_rows_times_gram_kernel<4><<<grid, 256, 0, st>>>(F, G, rows, R, out);
@@ -209,7 +229,7 @@ int sparse_loss(const int64_t* crow, const int64_t* col, const float* val, const
   int rc = beta == 1.0 ? launch_gather<kSpKLLoss>(crow, col, val, H, W, R, N, nullptr, loss_part, st)
                        : launch_gather<kSpEULoss>(crow, col, val, H, W, R, N, nullptr, loss_part, st);
   if (rc) return rc;
-  sp_loss_final_kernel<<<1, 32, 0, st>>>(loss_part, sparse_loss_blocks(N), pos_a, pos_b, beta == 1.0 ? R : R * R,
+  sp_loss_final_kernel<<<1, 32, 0, st>>>(loss_part, (int)sparse_gather_blocks(N), pos_a, pos_b, beta == 1.0 ? R : R * R,
                                          beta == 1.0 ? 1.0 : 0.5, v_norm, loss_dev);
   NMF_LAUNCH_CHECK();
   return 0;

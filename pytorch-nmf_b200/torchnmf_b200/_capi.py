@@ -62,8 +62,9 @@ SIGNATURES = {
     "nmfb200_hoyer_project": (_int, [_int, _vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp]),
     "nmfb200_nmf_plan": (_int, [_i64, _i64, _i64, _c.POINTER(_i64), _int]),
     "nmfb200_nmfd_plan": (_int, [_i64, _i64, _int, _c.POINTER(_i64), _i64, _c.POINTER(_i64), _c.POINTER(_i64), _int]),
+    "nmfb200_nmf_sparse_plan": (_int, [_i64, _i64, _i64, _c.POINTER(_i64), _int]),
 }
-NMF_PLAN_LEN, NMFD_PLAN_LEN = 9, 19         # include/nmf_b200.h
+NMF_PLAN_LEN, NMFD_PLAN_LEN, SPARSE_PLAN_LEN = 9, 19, 8         # include/nmf_b200.h
 
 _lib = None
 
@@ -117,6 +118,15 @@ def nmf_plan(N, C, R):
     out = (_i64 * NMF_PLAN_LEN)()
     check(load().nmfb200_nmf_plan(N, C, R, out, NMF_PLAN_LEN))
     keys = ("nch_w", "nch_h", "tpc_w", "tpc_h", "rb", "loss_chunks", "loss_tpc", "colsum_blocks_n", "colsum_blocks_c")
+    return dict(zip(keys, out))
+
+
+def sparse_plan(N, C, R):
+    """The sparse-target kernels' launch plan of an (N, C) rank-R context (nmfb200_nmf_sparse_plan), as a dict; no device
+    needed.  Gram plans: `rpb_n` / `nb_n` over the N rows of H, `rpb_c` / `nb_c` over the C rows of W."""
+    out = (_i64 * SPARSE_PLAN_LEN)()
+    check(load().nmfb200_nmf_sparse_plan(N, C, R, out, SPARSE_PLAN_LEN))
+    keys = ("rpl", "gram_passes", "rpb_n", "nb_n", "rpb_c", "nb_c", "gather_blocks_n", "gather_blocks_c")
     return dict(zip(keys, out))
 
 

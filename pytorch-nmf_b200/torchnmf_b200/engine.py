@@ -305,6 +305,7 @@ class CudaSparseNmfEngine(_CudaEngine):
         R = W.shape[1]
         assert W.shape == (C, R) and H.shape == (N, R)
         self.W, self.H = W, H
+        self.N, self.C, self.R = N, C, R
         vals = V.values().to(torch.float32).contiguous()
         rows, cols = V.indices()[0].contiguous(), V.indices()[1].contiguous()      # coalesced: sorted by (row, col)
         nnz = int(vals.numel())
@@ -359,6 +360,9 @@ class CudaSparseNmfEngine(_CudaEngine):
         _capi.check(self._lib.nmfb200_nmf_loss(self._ctx, _ptr(self.W), _ptr(self.H), beta, _ptr(self._loss),
                                                _stream(self.device)))
         return self._loss
+
+    # the same call and layout as the dense target's; beta 1 and 2 only (the terms of the sparse update, nmf.py:603-638)
+    raw_terms = CudaNmfEngine.raw_terms
 
 
 class CudaNmfdEngine(_CudaEngine):
