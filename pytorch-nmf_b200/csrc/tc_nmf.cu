@@ -381,22 +381,11 @@ __device__ __forceinline__ int pow2_exp_for(float mx) {
   return 14 - e;
 }
 
-// What the last stage of a factor refresh publishes (one thread): the operand exponent of this factor, kappa =
-// sum(V) / sum(W H^T) = sum(V) / <colsum W, colsum H> (the typical P = V / (WH)), the ratio-tile exponent exps[3] with
-// kappa 2^p in [2^-4, 2^-3) (P - kappa is fp16-exact down to 2^-20 kappa, and a ratio has to exceed 5e5 kappa before the
-// saturating pack clips it), and the exponents of the beta != 1 tiles.
-__device__ __forceinline__ void publish_scales(int a, int which, int* __restrict__ exps, unsigned int* __restrict__ absmax_next,
-                                               float dot, const double* __restrict__ vconst, float* __restrict__ kappa,
-                                               int center, float bm1, float bm2, double cells) {
-  exps[1 + which] = a;
-  *absmax_next = 0u;
-  const float ptyp = (float)(vconst[0] / (double)dot);
-  int e = 0;
-  const bool ok = ptyp > 0.f && isfinite(ptyp);
-  if (ok) { frexpf(ptyp, &e); e = -3 - e; }     // ptyp * 2^e in [2^-4, 2^-3)
-  exps[3] = e;
-  *kappa = (ok && center) ? ptyp : 0.f;
-  // beta != 1: typical x = mean(WH), typical Pn = mean(V) x^(beta-2), Pp = x^(beta-1) -> both tiles near 2^0
+// The exponents of the beta != 1 tiles, exps[4] and exps[5]: typical x = mean(WH), typical Pn = mean(V) x^(beta-2),
+// Pp = x^(beta-1) -> both tiles near 2^0.  They depend on beta, so a contraction at another beta than the one they were
+// published for republishes them first (republish_beta_kernel).
+__device__ __forceinline__ void publish_beta_exps(int* __restrict__ exps, float dot, const double* __restrict__ vconst,
+                                                  float bm1, float bm2, double cells) {
   const float xbar = (float)((double)dot / cells), vbar = (float)(vconst[0] / cells);
   int en = 0, ed = 0;
   if (xbar > 0.f && isfinite(xbar)) {
@@ -407,6 +396,30 @@ __device__ __forceinline__ void publish_scales(int a, int which, int* __restrict
   }
   exps[4] = en;
   exps[5] = ed;
+}
+
+// What the last stage of a factor refresh publishes (one thread): the operand exponent of this factor, kappa =
+// sum(V) / sum(W H^T) = sum(V) / <colsum W, colsum H> (the typical P = V / (WH)) with the dot product itself in kappa[1],
+// the ratio-tile exponent exps[3] with kappa 2^p in [2^-4, 2^-3) (P - kappa is fp16-exact down to 2^-20 kappa, and a
+// ratio has to exceed 5e5 kappa before the saturating pack clips it), and the exponents of the beta != 1 tiles.
+__device__ __forceinline__ void publish_scales(int a, int which, int* __restrict__ exps, unsigned int* __restrict__ absmax_next,
+                                               float dot, const double* __restrict__ vconst, float* __restrict__ kappa,
+                                               int center, float bm1, float bm2, double cells) {
+  exps[1 + which] = a;
+  *absmax_next = 0u;
+  const float ptyp = (float)(vconst[0] / (double)dot);
+  int e = 0;
+  const bool ok = ptyp > 0.f && isfinite(ptyp);
+  if (ok) { frexpf(ptyp, &e); e = -3 - e; }     // ptyp * 2^e in [2^-4, 2^-3)
+  exps[3] = e;
+  kappa[0] = (ok && center) ? ptyp : 0.f;
+  kappa[1] = dot;
+  publish_beta_exps(exps, dot, vconst, bm1, bm2, cells);
+}
+
+__global__ void republish_beta_kernel(int* __restrict__ exps, const float* __restrict__ kappa,
+                                      const double* __restrict__ vconst, float bm1, float bm2, double cells) {
+  if (threadIdx.x == 0 && blockIdx.x == 0) publish_beta_exps(exps, kappa[1], vconst, bm1, bm2, cells);
 }
 
 __global__ void set_vexp_kernel(const float* __restrict__ minmax, int* __restrict__ exps) {
@@ -1343,8 +1356,9 @@ struct TcState {
   // (CUDA-graph replay of tc_iterate), NMFB200_TC_CHECK=1 (watchdog check after every tc_contract_only).
   int center = 1;
   bool use_graph = false, check_each = false;
-  float* kappa = nullptr;           // device scalar
-  float* zero = nullptr;            // device scalar 0 (kappa of an already complete numerator)
+  float* kappa = nullptr;           // device [2]: kappa, <colsum W, colsum H> it was derived from
+  double exps_beta = 1.0;           // the beta exps[4] / exps[5] were last published for
+  float* zero = nullptr;           // device scalar 0 (kappa of an already complete numerator)
   int coop_blocks = 0;              // co-resident blocks of the fused tail kernel (cooperative launch), 0 = unavailable
   bool fused_tail = false;          // ratio stage + operand refresh in one cooperative kernel (NMFB200_FUSED_TAIL=0: two kernels)
 };
@@ -1432,12 +1446,12 @@ int tc_create(TcState** out, int device, int64_t N, int64_t C, int64_t R, bool s
   if (e == cudaSuccess) e = cudaMalloc(&s->vconst, 2 * sizeof(double));
   if (e == cudaSuccess) e = cudaMalloc(&s->vlossy, sizeof(unsigned long long));
   if (e == cudaSuccess) e = cudaMalloc(&s->loss_part, (size_t)s->num_sms * 2 * sizeof(double));
-  if (e == cudaSuccess) e = cudaMalloc(&s->kappa, sizeof(float));
+  if (e == cudaSuccess) e = cudaMalloc(&s->kappa, 2 * sizeof(float));
   if (e == cudaSuccess) e = cudaMalloc(&s->zero, sizeof(float));
   if (e == cudaSuccess) e = cudaMemset(s->zero, 0, sizeof(float));
   if (e == cudaSuccess) e = cudaMalloc(&s->vbeta, sizeof(double));
   if (e == cudaSuccess) e = cudaMalloc(&s->vbeta_part, 1024 * sizeof(double));
-  if (e == cudaSuccess) e = cudaMemset(s->kappa, 0, sizeof(float));
+  if (e == cudaSuccess) e = cudaMemset(s->kappa, 0, 2 * sizeof(float));
   if (e == cudaSuccess) e = cudaMemset(s->W16, 0, (size_t)C * s->KW * 2);
   if (e == cudaSuccess) e = cudaMemset(s->H16, 0, (size_t)N * s->KW * 2);
   if (e == cudaSuccess) e = cudaMemset(s->exps, 0, 8 * sizeof(int));
@@ -1542,6 +1556,7 @@ int apply_and_finish(TcState* s, int which, float* param, bool apply, const Plan
     a.npeers = s->peer_world; a.flags = reinterpret_cast<const unsigned int*>(s->peer_block);
     a.flag_target = s->peer_iter; a.peer_err = s->peer_err;
   }
+  s->exps_beta = beta;                 // both branches below end in publish_scales at this beta
   if ((s->R & 3) == 0 && !(apply && beta == 2.0 && !reduced) && s->fused_tail) {
     // one cooperative launch: ratio stage, grid barrier, operand copy + scalars
     const int lanes = (int)s->R >> 2, rows_per_pass = 256 / lanes;
@@ -1705,7 +1720,20 @@ int launch_contract_two(TcState* s, int which, double beta, cudaStream_t st) {
   return g > 0 ? 0 : 2;
 }
 
+// The update kernels of beta != 1 scale their tiles by exps[4] / exps[5], which the last refresh published for ITS beta (an
+// update of W at beta 1 followed by one of H at beta 2 is legal): republish them for this beta from the stored dot product.
+// A stream launch, so it is captured with the rest of an iteration.
+int sync_beta_exps(TcState* s, double beta, cudaStream_t st) {
+  if (beta == 1.0 || s->exps_beta == beta) return 0;
+  republish_beta_kernel<<<1, 32, 0, st>>>(s->exps, s->kappa, s->vconst, (float)(beta - 1.0), (float)(beta - 2.0),
+                                          (double)s->N * (double)s->C);
+  NMF_LAUNCH_CHECK();
+  s->exps_beta = beta;
+  return 0;
+}
+
 int launch_contract(TcState* s, int which, double beta, cudaStream_t st) {
+  if (int rc = sync_beta_exps(s, beta, st)) return rc;
   if (beta == 2.0) return launch_contract_one<kBmEU>(s, which, beta, st) > 0 ? 0 : 2;
   if (beta != 1.0) return launch_contract_two(s, which, beta, st);
   return launch_contract_one<kBmKL>(s, which, beta, st) > 0 ? 0 : 2;
@@ -1765,6 +1793,8 @@ int tc_iterate(TcState* s, float* W, float* H, double beta, double gamma, double
     const int key = (int)((s->upd[0] & 1u) * 2u + (s->upd[1] & 1u));
     if (use_graph && s->gwarm && s->gexec[key]) {
       s->w_pending = false;                          // the replayed iteration runs its own W contraction
+      rc = sync_beta_exps(s, beta, st);              // a call between two replays may have published another beta
+      if (rc) return rc;
       NMF_CUDA_CHECK(cudaGraphLaunch(s->gexec[key], st));
       s->upd[0]++; s->upd[1]++;
       count_launch(s->gkernels);

@@ -511,7 +511,6 @@ struct TcNmfdState {
   int ws_w = 1, ws_h = 1;           // split counts of wgrad / dgrad
   int kbs_w = 0, kbs_h = 0;
   CUtensorMap tmWr, tmWf, tmP;
-  bool attr_set = false;
 };
 
 bool tc_nmfd_supported(const NmfdShape& d, double beta) {
@@ -603,11 +602,13 @@ namespace {
 template <int KIND>
 int launch(TcNmfdState* s, const CUtensorMap& tm, dim3 grid, NmfdTcParams& p, cudaStream_t st) {
   auto kern = tcnmfd_kernel<KIND>;
-  static bool attr = false;
+  static unsigned long long attr_set_mask = 0;      // per device (one bit each): the attribute is per-device state
   const int smem = Smem::kTotal + 1024;
-  if (!attr) {
+  int dev = 0;
+  NMF_CUDA_CHECK(cudaGetDevice(&dev));              // the caller has selected the context's device
+  if (!((attr_set_mask >> (dev & 63)) & 1ull)) {
     NMF_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    attr = true;
+    attr_set_mask |= 1ull << (dev & 63);
   }
   kern<<<grid, kThreads, smem, st>>>(tm, p);
   NMF_LAUNCH_CHECK();

@@ -36,6 +36,7 @@ ulp):
     4 sigma, and is the whole difference where a sum has a single flagged term.
   * the fp32 chunk sums and the kappa colsum addition: u ((nchunks + 1) A + |kappa colsum|).
 """
+import json
 import math
 
 import torch
@@ -304,3 +305,97 @@ class NmfdModel:
         # logf / fp32 per-16-element partial sums: a few ulp of each term
         bar = rel_s * (V.sum() + x.sum()) + 64 * U * terms
         return float(val), float(bar), float(terms)
+
+# ---- bars and plans shared by the term tests (tests/test_gpu_tc_terms.py) and the call sequences (tests/sequence_cases.py) ----
+RTOL64 = {"f16": 1.25e-3, "f16_split": 2.5e-4}            # the bars of tests/test_gpu_tc_terms.py (its docstring)
+LOSS_RELS = {"f16": 2.0 ** -11, "f16_split": 2.0 ** -20}
+# The model bar must stay below the float64 bar, so that a kernel within the model bar of the model passes the float64 bar
+# by construction (tests/test_tc_model.py checks that on the CPU).  It is not 5x below it everywhere: the split mode's is
+# dominated by the truncation of S over up to 24 k-steps of 3 x 128 products (2 x 195 ulp = 4.6e-5 relative), the
+# sliding GEMMs' by the possible one-ulp steps of the ratio tile in sums with few terms.  Each case reports the ratio.
+# What the model bar can see is checked directly instead: on STRUCT_CASES each of the three split terms, dropped, misses
+# the model by more than twice the bar (tests/test_tc_model.py).
+TIGHTER = 1.0
+
+
+def cdiv(a, b):
+    return -(-a // b)
+
+
+def plan(Mr, Nc, num_sms, TN):
+    """make_plan (csrc/tc_nmf.cu): (row blocks, tiles, chunks, tiles per chunk)."""
+    rb, tiles = cdiv(Mr, 128), cdiv(Nc, TN)
+    best, best_eff = 1, -1.0
+    for nch in range(1, min(tiles, 64) + 1):
+        tpc = cdiv(tiles, nch)
+        if tpc * TN < 512 and nch > 1:
+            break
+        if cdiv(tiles, tpc) != nch:
+            continue
+        items = rb * nch
+        eff = items / (cdiv(items, num_sms) * num_sms)
+        if eff > best_eff + 0.03:
+            best_eff, best = eff, nch
+        if best_eff >= 0.97:
+            break
+    return rb, tiles, best, cdiv(tiles, best)
+
+
+def tn(prec, R):
+    return 64 if (prec == "f16_split" and R > 64) else 128
+
+
+def _report(**kw):
+    print("TCTERMS " + json.dumps(kw))
+
+
+def check_terms(tag, got, model, bar, exact, rtol64):
+    """got / model / bar / exact: float64 on one device.  Asserts both bars and the tightness of the model bar."""
+    got, model, bar, exact = (t.double().cpu() for t in (got, model, bar, exact))
+    scale = exact.abs()
+    tight = float((bar / scale).max())
+    e_model = float(((got - model).abs() / bar).max())
+    e64 = float(((got - exact).abs() / scale).max())
+    _report(case=tag, model_err_over_bar=e_model, err64=e64, bar64=rtol64, model_bar_rel=tight)
+    assert tight * TIGHTER < rtol64, f"{tag}: the model bar ({tight:.2e} relative) is not below {rtol64:.1e}"
+    assert e_model <= 1.0, f"{tag}: {e_model:.2f} x the model bar"
+    assert e64 <= rtol64, f"{tag}: relative error {e64:.2e} against float64 > {rtol64:.1e}"
+    return max(e_model, e64 / rtol64)
+
+
+def check_loss(tag, got, model, exact, prec, beta):
+    val, bar, terms = model
+    g = max(1.0, abs(beta), abs(beta - 1))
+    bar64 = (LOSS_RELS[prec] * g + 2.0 ** -12) * terms
+    e_model, e64 = abs(got - val) / bar, abs(got - exact) / bar64
+    _report(case=tag, model_err_over_bar=e_model, err64_over_bar=e64, model_bar_rel=bar / terms, bar64_rel=bar64 / terms)
+    assert bar * TIGHTER < bar64, f"{tag}: model bar {bar:.3e} not below {bar64:.3e}"
+    assert e_model <= 1.0, f"{tag}: {got!r} vs model {val!r}: {e_model:.2f} x the model bar"
+    assert e64 <= 1.0, f"{tag}: {got!r} vs float64 {exact!r}: {e64:.2f} x the bar"
+    return max(e_model, e64)
+
+
+def nmfd_splits(B, C, L, R, T):
+    """tc_nmfd_create (csrc/tc_nmfd.cu): (ws_w, k-blocks per split, last split's), then the same for dgrad."""
+    Tp, Lin = cdiv(T, 64) * 64, L - T + 1
+    tiles_w, tiles_h = cdiv(C, 128) * R * cdiv(T, 128), cdiv(Lin, 128) * B
+    kb_w, kb_h = B * cdiv(L, 64), C * (Tp // 64)
+    out = []
+    for kb, tiles in ((kb_w, tiles_w), (kb_h, tiles_h)):
+        ws = max(1, min(kb // 8, cdiv(132 * 4, tiles)))
+        kbs = cdiv(kb, ws)
+        ws = cdiv(kb, kbs)
+        out += [ws, kbs, kb - (ws - 1) * kbs]
+    return out
+
+
+def nmfd_rtol64(case, V, W, H):
+    """The f16 bar, widened where the W numerator is a single-term sum (L = T): there the ratio tile's fp16 rounding,
+    up to 2^-11 |P - kappa| relative to P, is not averaged over any other term, and the kernel's tile may sit one fp16 ulp
+    (another 2^-11 |P - kappa|) from the exactly rounded one."""
+    B, C, L, R, T = case
+    if L != T:
+        return RTOL64["f16"]
+    m = NmfdModel(V, W, H, rounding=False)
+    P = m.V / (m.S + EPS)
+    return RTOL64["f16"] + 2.0 ** -10 * float(((P - m.kappa) / P).abs().max())

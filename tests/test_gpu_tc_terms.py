@@ -27,27 +27,14 @@ import pytest
 import torch
 
 import tc_model as tcm
+from tc_model import LOSS_RELS, RTOL64, TIGHTER, cdiv, nmfd_rtol64  # noqa: F401  (shared with the sequence harness)
+from tc_model import check_loss as _check_loss, check_terms as _check_terms, nmfd_splits as _nmfd_splits, plan as _plan, tn as _tn
 from oracle import mu_oracle as orc
 from oracle_engine import OracleNmfEngine, OracleNmfdEngine
 from torchnmf_b200 import NMFD
 from torchnmf_b200.engine import CudaNmfdEngine, CudaNmfEngine
 
 pytestmark = pytest.mark.gpu
-
-RTOL64 = {"f16": 1.25e-3, "f16_split": 2.5e-4}            # see the module docstring
-LOSS_RELS = {"f16": 2.0 ** -11, "f16_split": 2.0 ** -20}
-# The model bar must stay below the float64 bar, so that a kernel within the model bar of the model passes the float64 bar
-# by construction (tests/test_tc_model.py checks that on the CPU).  It is not 5x below it everywhere: the split mode's is
-# dominated by the truncation of S over up to 24 k-steps of 3 x 128 products (2 x 195 ulp = 4.6e-5 relative), the
-# sliding GEMMs' by the possible one-ulp steps of the ratio tile in sums with few terms.  Each case reports the ratio.
-# What the model bar can see is checked directly instead: on STRUCT_CASES each of the three split terms, dropped, misses
-# the model by more than twice the bar (tests/test_tc_model.py).
-TIGHTER = 1.0
-
-
-def cdiv(a, b):
-    return -(-a // b)
-
 
 # ---- NMF cases: every configuration <RP, SPLIT, TN> meets every edge -------------------------------------------------------
 # N and C each run through the residues 1, 63, 64, 65, 127, 0 mod 128: rows of F mod 128 in {1, 64, 65, 127, 0} and
@@ -73,29 +60,6 @@ NMF_CASES = _nmf_cases()
 # (fast mode: a split-mode model bar over 4161-term sums is not 5x tighter than the split mode's float64 bar)
 CHUNK_CASES = [("f16", 4161, 200, 20), ("f16", 200, 4161, 20), ("f16", 200, 2113, 100), ("f16", 2113, 200, 100)]
 TWO_BETAS = [0, 0.5, 1.5, 3, -1]
-
-
-def _plan(Mr, Nc, num_sms, TN):
-    """make_plan (csrc/tc_nmf.cu): (row blocks, tiles, chunks, tiles per chunk)."""
-    rb, tiles = cdiv(Mr, 128), cdiv(Nc, TN)
-    best, best_eff = 1, -1.0
-    for nch in range(1, min(tiles, 64) + 1):
-        tpc = cdiv(tiles, nch)
-        if tpc * TN < 512 and nch > 1:
-            break
-        if cdiv(tiles, tpc) != nch:
-            continue
-        items = rb * nch
-        eff = items / (cdiv(items, num_sms) * num_sms)
-        if eff > best_eff + 0.03:
-            best_eff, best = eff, nch
-        if best_eff >= 0.97:
-            break
-    return rb, tiles, best, cdiv(tiles, best)
-
-
-def _tn(prec, R):
-    return 64 if (prec == "f16_split" and R > 64) else 128
 
 
 def _data(N, C, R, seed, vmin=0.0, fmin=0.1):
@@ -137,34 +101,6 @@ def _structured_data(N, C, R, seed):
 STRUCT_CASES = [("f16_split", N, C, R) for N, C, R in
                 [(257, 192, 1), (319, 321, 8), (384, 447, 63), (321, 256, 64), (257, 192, 65), (383, 257, 100),
                  (320, 511, 127), (321, 256, 128)]]
-
-
-def _report(**kw):
-    print("TCTERMS " + json.dumps(kw))
-
-
-def _check_terms(tag, got, model, bar, exact, rtol64):
-    """got / model / bar / exact: float64 on one device.  Asserts both bars and the tightness of the model bar."""
-    got, model, bar, exact = (t.double().cpu() for t in (got, model, bar, exact))
-    scale = exact.abs()
-    tight = float((bar / scale).max())
-    e_model = float(((got - model).abs() / bar).max())
-    e64 = float(((got - exact).abs() / scale).max())
-    _report(case=tag, model_err_over_bar=e_model, err64=e64, bar64=rtol64, model_bar_rel=tight)
-    assert tight * TIGHTER < rtol64, f"{tag}: the model bar ({tight:.2e} relative) is not below {rtol64:.1e}"
-    assert e_model <= 1.0, f"{tag}: {e_model:.2f} x the model bar"
-    assert e64 <= rtol64, f"{tag}: relative error {e64:.2e} against float64 > {rtol64:.1e}"
-
-
-def _check_loss(tag, got, model, exact, prec, beta):
-    val, bar, terms = model
-    g = max(1.0, abs(beta), abs(beta - 1))
-    bar64 = (LOSS_RELS[prec] * g + 2.0 ** -12) * terms
-    e_model, e64 = abs(got - val) / bar, abs(got - exact) / bar64
-    _report(case=tag, model_err_over_bar=e_model, err64_over_bar=e64, model_bar_rel=bar / terms, bar64_rel=bar64 / terms)
-    assert bar * TIGHTER < bar64, f"{tag}: model bar {bar:.3e} not below {bar64:.3e}"
-    assert e_model <= 1.0, f"{tag}: {got!r} vs model {val!r}: {e_model:.2f} x the model bar"
-    assert e64 <= 1.0, f"{tag}: {got!r} vs float64 {exact!r}: {e64:.2f} x the bar"
 
 
 def _engine(prec, V, W, H):
@@ -319,20 +255,6 @@ NMFD_CASES = [
 ]
 
 
-def _nmfd_splits(B, C, L, R, T):
-    """tc_nmfd_create (csrc/tc_nmfd.cu): (ws_w, k-blocks per split, last split's), then the same for dgrad."""
-    Tp, Lin = cdiv(T, 64) * 64, L - T + 1
-    tiles_w, tiles_h = cdiv(C, 128) * R * cdiv(T, 128), cdiv(Lin, 128) * B
-    kb_w, kb_h = B * cdiv(L, 64), C * (Tp // 64)
-    out = []
-    for kb, tiles in ((kb_w, tiles_w), (kb_h, tiles_h)):
-        ws = max(1, min(kb // 8, cdiv(132 * 4, tiles)))
-        kbs = cdiv(kb, ws)
-        ws = cdiv(kb, kbs)
-        out += [ws, kbs, kb - (ws - 1) * kbs]
-    return out
-
-
 def _nmfd_data(B, C, L, R, T, seed):
     # a target bounded away from zero: where a sum has a single term (L = T) the centred numerator (P - kappa) G + kappa G
     # is only good to u kappa / P relative, which a V near zero would turn into the bar of the case
@@ -341,18 +263,6 @@ def _nmfd_data(B, C, L, R, T, seed):
     W = torch.rand(C, R, T, generator=g) + 0.1
     H = torch.rand(B, R, L - T + 1, generator=g) + 0.1
     return V, W, H
-
-
-def nmfd_rtol64(case, V, W, H):
-    """The f16 bar, widened where the W numerator is a single-term sum (L = T): there the ratio tile's fp16 rounding,
-    up to 2^-11 |P - kappa| relative to P, is not averaged over any other term, and the kernel's tile may sit one fp16 ulp
-    (another 2^-11 |P - kappa|) from the exactly rounded one."""
-    B, C, L, R, T = case
-    if L != T:
-        return RTOL64["f16"]
-    m = tcm.NmfdModel(V, W, H, rounding=False)
-    P = m.V / (m.S + tcm.EPS)
-    return RTOL64["f16"] + 2.0 ** -10 * float(((P - m.kappa) / P).abs().max())
 
 
 @pytest.mark.parametrize("case", NMFD_CASES, ids=_id)
