@@ -215,13 +215,23 @@ int nmfb200_nmf_plan(int64_t N, int64_t C, int64_t R, int64_t* out, int n);
 #define NMFB200_SPARSE_PLAN_LEN 8
 int nmfb200_nmf_sparse_plan(int64_t N, int64_t C, int64_t R, int64_t* out, int n);
 /* The same for an NMFD / NMF2D / NMF3D context (arguments as nmfb200_nmfnd_create), NMFB200_NMFD_PLAN_LEN values:
- *   [0] recon row tile MT (channels)   [1..3] recon grid x, y, z
- *   [4] dgrad row tile MT (components)   [5] dgrad splits of C   [6..8] dgrad grid x, y, z
+ *   [0] recon row tile MT (channels)   [1..3] recon grid x, y, z of one launch
+ *   [4] dgrad row tile MT (components)   [5] dgrad splits of C   [6..8] dgrad grid x, y, z of one launch
+ *   (z = batch elements per launch, at most 65535: a larger batch takes ceil(B / z) launches)
  *   [9..15] wgrad plan mt, tp, nr, no, ntt, nrg, nog   [16] wgrad splits of the lines
  *   [17], [18] 1 if the W / H ratio stage takes the four-elements-per-thread kernel, else 0 */
 #define NMFB200_NMFD_PLAN_LEN 19
 int nmfb200_nmfd_plan(int64_t B, int64_t C, int ndim, const int64_t* vdims, int64_t R, const int64_t* kdims,
                       int64_t* out, int n);
+/* What the tensor-core (beta 1) kernels of an NMFD context (arguments as nmfb200_nmfd_create) launch, from the planner
+ * those launches use; NMFB200_ERR_INVALID, naming the limit, for a shape that create rejects with precision f16 (and runs on
+ * the fp32 kernels with precision auto).  NMFB200_NMFD_TC_PLAN_LEN values:
+ *   [0..2] prep_w grid   [3..5] prep_h grid   [6..8] recon grid of one launch   [9..11] wgrad grid
+ *   [12..14] dgrad grid of one launch   [15] batch elements per recon / dgrad launch (grid z)   [16] launches (batch slices)
+ *   [17] dgrad launches per slice (blocks of 128 components)   [18] recon-loss partials
+ *   [19] wgrad splits   [20] wgrad k-blocks per split   [21] dgrad splits   [22] dgrad k-blocks per split */
+#define NMFB200_NMFD_TC_PLAN_LEN 23
+int nmfb200_nmfd_tc_plan(int64_t B, int64_t C, int64_t L, int64_t R, int64_t T, int64_t* out, int n);
 
 /* ---- sparseness-constrained NMF (Hoyer 2004) --------------------------------------------- */
 

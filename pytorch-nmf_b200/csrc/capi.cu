@@ -627,8 +627,20 @@ static int nmfd_shape_of(int64_t B, int64_t C, int ndim, const int64_t* vdims, i
   if (R > 256) return fail(NMFB200_ERR_INVALID, "rank > 256 is not supported");
   if (B * C * X[0] * X[1] * L > (int64_t)1 << 40 || X[0] * X[1] * L > (int64_t)1 << 30 || K[0] * K[1] * T > (int64_t)1 << 24)
     return fail(NMFB200_ERR_INVALID, "NMFD target too large");
+  // every size below is narrowed to int, and the kernels count in int: bound what they derive from it
+  if (C > kMaxGridYZ * 64)
+    return fail(NMFB200_ERR_INVALID, "NMFD supports at most 65535 x 64 = 4194240 channels (grid.y of the reconstruction)");
+  if (B * (X[0] - K[0] + 1) * (X[1] - K[1] + 1) > INT32_MAX)
+    return fail(NMFB200_ERR_INVALID, "NMFD batch x outer activation lines must be below 2^31 (the W gradient's line index)");
+  if ((C > R ? C : R) * K[0] * K[1] > INT32_MAX)
+    return fail(NMFB200_ERR_INVALID, "NMFD channels (or rank) x outer kernel offsets must be below 2^31 (the contraction index)");
   *d = NmfdShape{(int)B, (int)C, (int)L, (int)R, (int)T, (int)(L - T + 1)};
   d->X1 = (int)X[0]; d->X2 = (int)X[1]; d->T1 = (int)K[0]; d->T2 = (int)K[1];
+  NmfdPlan p;
+  nmfd_plan(*d, &p);
+  if (!grid_fits(p.recon_grid) || !grid_fits(p.dgrad_grid) || !grid_fits(p.wgrad_grid))
+    return fail(NMFB200_ERR_INVALID, "an NMFD grid of the fp32 kernels passes the CUDA grid limits");
+  if (nmfd_max_blocks(*d) > INT32_MAX) return fail(NMFB200_ERR_INVALID, "NMFD loss partials must number below 2^31");
   return 0;
 }
 
@@ -653,6 +665,9 @@ static int nmfd_create_impl(nmfb200_ctx** out, int device, int64_t B, int64_t C,
   const bool one_d = shape.one_d();
   if (!one_d && precision == NMFB200_PREC_F16)
     return fail(NMFB200_ERR_INVALID, "NMF2D / NMF3D run on the fp32 kernels (precision auto or f32)");
+  TcNmfdPlan tc_plan;
+  const char* tc_limit = one_d ? tc_nmfd_plan(shape, &tc_plan) : "";
+  if (precision == NMFB200_PREC_F16 && tc_limit) return fail(NMFB200_ERR_INVALID, tc_limit);
   DeviceGuard guard(device);
   if (!guard.ok) return fail(NMFB200_ERR_CUDA, "cannot select the requested device");
   nmfb200_ctx* c = new (std::nothrow) nmfb200_ctx();
@@ -668,7 +683,7 @@ static int nmfd_create_impl(nmfb200_ctx** out, int device, int64_t B, int64_t C,
   c->part_floats = pf;
   int64_t cs1 = colsum_scratch_floats(C, (int)R, c->d.w_inner()), cs2 = colsum_scratch_floats(B, (int)R, c->d.h_inner());
   c->cs_scratch_floats = cs1 > cs2 ? cs1 : cs2;
-  c->loss_max_blocks = nmfd_max_blocks(c->d);
+  c->loss_max_blocks = (int)nmfd_max_blocks(c->d);         // bounded by nmfd_shape_of
   cudaError_t e = cudaSuccess;
   if (e == cudaSuccess) e = cudaMalloc(&c->num, pf * sizeof(float));
   if (e == cudaSuccess) e = cudaMalloc(&c->colsum, 2 * R * sizeof(float));
@@ -680,7 +695,7 @@ static int nmfd_create_impl(nmfb200_ctx** out, int device, int64_t B, int64_t C,
     free_ctx(c);
     return fail(NMFB200_ERR_CUDA, std::string("cudaMalloc: ") + cudaGetErrorString(e));
   }
-  if (c->precision != NMFB200_PREC_F32 && one_d) {       // the tensor-core kernels cover the one-axis case
+  if (c->precision != NMFB200_PREC_F32 && !tc_limit) {    // the tensor-core kernels cover the one-axis case
     cudaDeviceProp prop;
     if (cudaGetDeviceProperties(&prop, device) == cudaSuccess && prop.major == 9) {
       int rc = tc_nmfd_create(&c->tcd, c->d);          // beta = 1 runs as wgmma sliding GEMMs (tc_nmfd.cu)
@@ -798,6 +813,20 @@ int nmfb200_nmfd_plan(int64_t B, int64_t C, int ndim, const int64_t* vdims, int6
       w.mt, w.tp, w.nr, w.no, w.ntt, w.nrg, w.nog, p.wgrad_nsplit,
       apply_update_vec4_shape(nmfd_apply_shape(d, 0, p.wgrad_nsplit)), apply_update_vec4_shape(nmfd_apply_shape(d, 1, p.dgrad_nsplit))};
   for (int i = 0; i < NMFB200_NMFD_PLAN_LEN; ++i) out[i] = v[i];
+  return 0;
+}
+
+int nmfb200_nmfd_tc_plan(int64_t B, int64_t C, int64_t L, int64_t R, int64_t T, int64_t* out, int n) {
+  if (!out || n < NMFB200_NMFD_TC_PLAN_LEN) return fail(NMFB200_ERR_INVALID, "plan buffer too small");
+  NmfdShape d;
+  if (int rc = nmfd_shape_of(B, C, 1, &L, R, &T, &d)) return rc;
+  TcNmfdPlan p;
+  if (const char* why = tc_nmfd_plan(d, &p)) return fail(NMFB200_ERR_INVALID, why);
+  const int64_t v[NMFB200_NMFD_TC_PLAN_LEN] = {
+      p.prep_w.x, p.prep_w.y, p.prep_w.z, p.prep_h.x, p.prep_h.y, p.prep_h.z, p.recon.x, p.recon.y, p.recon.z,
+      p.wgrad.x, p.wgrad.y, p.wgrad.z, p.dgrad.x, p.dgrad.y, p.dgrad.z, p.bslice, p.slices, p.dgrad_rblocks,
+      p.loss_blocks, p.ws_w, p.kbs_w, p.ws_h, p.kbs_h};
+  for (int i = 0; i < NMFB200_NMFD_TC_PLAN_LEN; ++i) out[i] = v[i];
   return 0;
 }
 

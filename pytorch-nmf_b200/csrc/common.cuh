@@ -46,6 +46,15 @@ int64_t launch_counter();
 static inline int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
 static inline int64_t round_up(int64_t a, int64_t b) { return ceil_div(a, b) * b; }
 
+// CUDA's grid limits: x up to 2^31 - 1 blocks, y and z up to 65535
+constexpr int64_t kMaxGridX = 0x7fffffff;
+constexpr int64_t kMaxGridYZ = 65535;
+// a launch's grid as planned on the host, before it is narrowed to dim3
+struct Grid3 { int64_t x, y, z; };
+static inline bool grid_fits(const Grid3& g) {
+  return g.x >= 1 && g.x <= kMaxGridX && g.y >= 1 && g.y <= kMaxGridYZ && g.z >= 1 && g.z <= kMaxGridYZ;
+}
+
 // ------------------------------------------------------------------------------------------
 // Launch wrappers implemented in the .cu files (all asynchronous on `st`, return 0 / error code)
 // ------------------------------------------------------------------------------------------
@@ -142,7 +151,10 @@ struct NmfdShape {
 int nmfd_recon_phi(const NmfdShape& s, const float* V, const float* W, const float* H, double beta,
                    float* Pn, float* Pp, double* loss_blocks, int max_blocks, double* loss_dev,
                    cudaStream_t st);
-int nmfd_max_blocks(const NmfdShape& s);
+// batch elements per launch of the kernels that put the batch on grid.z (fp32 recon / dgrad, tensor-core recon / dgrad)
+static inline int64_t nmfd_batch_slice(int64_t B) { return B < kMaxGridYZ ? B : kMaxGridYZ; }
+// loss partials of nmfd_recon_phi: one per block of all its launches
+int64_t nmfd_max_blocks(const NmfdShape& s);
 // out[c,r,t] = sum_{b,x} G[b,c,x] H[b,r,x-t]   (x, t multi-indices over up to three axes)
 int nmfd_wgrad(const NmfdShape& s, const float* G, const float* H, float* out, int nsplit, cudaStream_t st);   // out[split][C,R,T]
 int nmfd_wgrad_nsplit(const NmfdShape& s);
@@ -153,7 +165,12 @@ int nmfd_dgrad_nsplit(const NmfdShape& s);
 // kernel offsets per block; NTT x NRG x NOG column blocks
 struct WgradPlan { int mt, tp, nr, no, ntt, nrg, nog; };
 // what nmfd_recon_phi / nmfd_dgrad / nmfd_wgrad launch for this shape, with the splits the library uses
-struct NmfdPlan { int recon_mt; dim3 recon_grid; int dgrad_mt, dgrad_nsplit; dim3 dgrad_grid; WgradPlan wgrad; int wgrad_nsplit; };
+// (recon and dgrad grids are per launch: batches beyond grid.z take ceil(B / z) launches)
+struct NmfdPlan {
+  int recon_mt; Grid3 recon_grid; int dgrad_mt, dgrad_nsplit; Grid3 dgrad_grid; WgradPlan wgrad; int wgrad_nsplit;
+  Grid3 wgrad_grid;
+};
+Grid3 wgrad_grid(const NmfdShape& s, const WgradPlan& p, int nsplit);
 void nmfd_plan(const NmfdShape& s, NmfdPlan* p);
 
 }  // namespace nmfb200

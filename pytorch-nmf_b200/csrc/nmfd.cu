@@ -69,7 +69,8 @@ struct Geo {
 // ---- recon (FWD) and dgrad (!FWD): out[m, pos] = sum_{k, t} A[m, k, t] X[k, pos -/+ t] ---------------------------------------
 //   FWD : m = c, k = r, X = H, shift -t, zero outside H; the epilogue applies phi against V (or reduces the loss)
 //   !FWD: m = r, k = c in this block's split, X = G, shift +t; the epilogue writes the partial sums of this split
-// grid (line tiles * line groups, row tiles * nsplit, B), 256 threads
+// grid (line tiles * line groups, row tiles * nsplit, batch elements [b0, b0 + gridDim.z)), 256 threads: batches beyond the
+// 65535 of grid.z take several launches
 struct SlideArgs {
   const float* A;            // W
   const float* X;            // H (FWD) or G
@@ -78,6 +79,7 @@ struct SlideArgs {
   int nsplit;                // !FWD: splits of k
   const float* V; float beta; float* Pn; float* Pp; double* block_partials;     // FWD epilogue
   float* out;                // !FWD: [split][B][R][h_inner]
+  int b0;                    // first batch element of this launch
 };
 
 template <int MT, bool FWD, int MODE, bool LOSS>
@@ -99,7 +101,7 @@ nmfd_slide_kernel(NmfdShape s, SlideArgs a) {
   const int mtiles = (a.M + MT - 1) / MT;
   const int split = blockIdx.y / mtiles;
   const int m0 = (blockIdx.y - split * mtiles) * MT;
-  const int b = blockIdx.z;
+  const int b = a.b0 + blockIdx.z;
   const int kps = (a.K + a.nsplit - 1) / a.nsplit;
   const int kbeg = split * kps, kend = min(a.K, kbeg + kps);
   const int J1 = s.J1(), J2 = s.J2();
@@ -199,7 +201,7 @@ nmfd_slide_kernel(NmfdShape s, SlideArgs a) {
     if (LOSS) {
       const double tot = block_sum_d((double)local, red);
       if (tid == 0)
-        a.block_partials[((int64_t)blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x] = tot;
+        a.block_partials[((int64_t)b * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x] = tot;
     }
   } else {
     const int64_t HI = s.h_inner();
@@ -251,11 +253,12 @@ nmfd_wgrad_kernel(NmfdShape s, const float* __restrict__ Gm, const float* __rest
     for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
 
   // the lines are split over blockIdx.z: more blocks than the output tiles alone give, and shorter fp32 sums
-  const int nlines = s.B * J1 * J2, lps = (nlines + nsplit - 1) / nsplit;
-  const int line0 = blockIdx.z * lps, line1 = min(nlines, line0 + lps);
+  // 64-bit: create admits up to 2^31 - 1 lines, and the rounded-up split end may pass that
+  const int64_t nlines = (int64_t)s.B * J1 * J2, lps = (nlines + nsplit - 1) / nsplit;
+  const int64_t line0 = blockIdx.z * lps, line1 = min(nlines, line0 + lps);
   out += (int64_t)blockIdx.z * s.C * s.R * s.w_inner();
-  for (int bo = line0; bo < line1; ++bo) {                // every H line (b, j1, j2) meets the G lines (b, j1 + t1, j2 + t2)
-    const int b = bo / (J1 * J2), jo = bo - b * (J1 * J2);
+  for (int64_t bo = line0; bo < line1; ++bo) {            // every H line (b, j1, j2) meets the G lines (b, j1 + t1, j2 + t2)
+    const int b = (int)(bo / (J1 * J2)), jo = (int)(bo - (int64_t)b * (J1 * J2));
     const int j1 = jo / J2, j2 = jo - j1 * J2;
     const float* Hb = H + ((int64_t)b * s.R * J1 * J2 + jo) * s.Lin;           // + r * J1 * J2 * Lin per component
     const float* Gb = Gm + (int64_t)b * s.C * VI;
@@ -337,12 +340,15 @@ inline WgradPlan wgrad_plan(const NmfdShape& s) {
   return p;
 }
 
-dim3 slide_grid(const NmfdShape& s, bool fwd, int mt, int M, int nsplit) {
+// grid of one launch of the sliding kernel; z = the batch elements per launch (nmfd_batch_slice)
+Grid3 slide_grid(const NmfdShape& s, bool fwd, int mt, int M, int nsplit) {
   const int64_t out_lines = fwd ? (int64_t)s.X1 * s.X2 : (int64_t)s.J1() * s.J2();
   const int64_t lout = fwd ? s.L : s.Lin;
-  return dim3((unsigned)(ceil_div(lout, kLT) * ceil_div(out_lines, xt_of(mt))), (unsigned)(ceil_div(M, mt) * nsplit),
-              (unsigned)s.B);
+  return Grid3{ceil_div(lout, kLT) * ceil_div(out_lines, xt_of(mt)), ceil_div(M, mt) * nsplit, nmfd_batch_slice(s.B)};
 }
+
+dim3 dim3_of(const Grid3& g) { return dim3((unsigned)g.x, (unsigned)g.y, (unsigned)g.z); }
+
 
 template <int MT, bool FWD>
 void launch_slide(const NmfdShape& s, const SlideArgs& a, int mode, bool loss, dim3 grid, cudaStream_t st) {
@@ -370,25 +376,37 @@ void dispatch_slide(int mt, const NmfdShape& s, const SlideArgs& a, int mode, bo
   }
 }
 
+// one launch of the sliding kernel per slice of at most kMaxGridYZ batch elements
+template <bool FWD>
+int launch_slices(int mt, const NmfdShape& s, SlideArgs a, int mode, bool loss, const Grid3& g, cudaStream_t st) {
+  for (int64_t b0 = 0; b0 < s.B; b0 += g.z) {
+    a.b0 = (int)b0;
+    dim3 grid = dim3_of(g);
+    grid.z = (unsigned)std::min<int64_t>(g.z, s.B - b0);
+    dispatch_slide<FWD>(mt, s, a, mode, loss, grid, st);
+    NMF_LAUNCH_CHECK();
+  }
+  return 0;
+}
+
 }  // namespace
 
-int nmfd_max_blocks(const NmfdShape& s) {
-  const dim3 g = slide_grid(s, true, row_tile(s.C), s.C, 1);
-  return (int)((int64_t)g.x * g.y * g.z);
+int64_t nmfd_max_blocks(const NmfdShape& s) {
+  const Grid3 g = slide_grid(s, true, row_tile(s.C), s.C, 1);
+  return g.x * g.y * s.B;
 }
 
 int nmfd_recon_phi(const NmfdShape& s, const float* V, const float* W, const float* H, double beta, float* Pn,
                    float* Pp, double* loss_blocks, int max_blocks, double* loss_dev, cudaStream_t st) {
   const int mt = row_tile(s.C);
-  const dim3 grid = slide_grid(s, true, mt, s.C, 1);
-  const int nblocks = (int)((int64_t)grid.x * grid.y * grid.z);
+  const Grid3 grid = slide_grid(s, true, mt, s.C, 1);
+  const int nblocks = (int)nmfd_max_blocks(s);          // create bounds it (nmfd_shape_of)
   const bool loss = loss_blocks != nullptr;
   if (loss && nblocks > max_blocks) { set_error("nmfd loss: partial buffer too small"); return 1; }
   SlideArgs a{};
   a.A = W; a.X = H; a.M = s.C; a.K = s.R; a.sm = (int64_t)s.R * s.w_inner(); a.sk = s.w_inner(); a.nsplit = 1;
   a.V = V; a.beta = (float)beta; a.Pn = Pn; a.Pp = Pp; a.block_partials = loss_blocks; a.out = nullptr;
-  dispatch_slide<true>(mt, s, a, beta_mode(beta), loss, grid, st);
-  NMF_LAUNCH_CHECK();
+  if (int rc = launch_slices<true>(mt, s, a, beta_mode(beta), loss, grid, st)) return rc;
   if (loss) return sum_partials(loss_blocks, nblocks, loss_dev, st);
   return 0;
 }
@@ -408,7 +426,7 @@ int nmfd_wgrad(const NmfdShape& s, const float* G, const float* H, float* out, i
   const WgradPlan p = wgrad_plan(s);
   const int ncol = 4 * (256 / (p.mt / 4));
   if (p.nr * (p.tp + kTK) > (ncol / 4) * (4 + kTK)) { set_error("nmfd_wgrad: internal tile plan exceeds shared memory"); return 1; }
-  dim3 grid((unsigned)((int64_t)p.ntt * p.nrg * p.nog), (unsigned)ceil_div(s.C, p.mt), (unsigned)nsplit);
+  const dim3 grid = dim3_of(wgrad_grid(s, p, nsplit));
   switch (p.mt) {
     case 4: nmfd_wgrad_kernel<4><<<grid, 256, 0, st>>>(s, G, H, out, nsplit, p); break;
     case 8: nmfd_wgrad_kernel<8><<<grid, 256, 0, st>>>(s, G, H, out, nsplit, p); break;
@@ -421,13 +439,17 @@ int nmfd_wgrad(const NmfdShape& s, const float* G, const float* H, float* out, i
 }
 
 int nmfd_dgrad_nsplit(const NmfdShape& s) {
-  const dim3 g = slide_grid(s, false, row_tile(s.R), s.R, 1);
-  const int64_t tiles = (int64_t)g.x * g.y * g.z;
+  const Grid3 g = slide_grid(s, false, row_tile(s.R), s.R, 1);
+  const int64_t tiles = g.x * g.y * s.B;
   int64_t ns = ceil_div(132 * 4, tiles);
   if (ns > s.C) ns = s.C;
   if (ns > 64) ns = 64;
   if (ns < 1) ns = 1;
   return (int)ns;
+}
+
+Grid3 wgrad_grid(const NmfdShape& s, const WgradPlan& p, int nsplit) {
+  return Grid3{(int64_t)p.ntt * p.nrg * p.nog, ceil_div(s.C, p.mt), nsplit};
 }
 
 void nmfd_plan(const NmfdShape& s, NmfdPlan* p) {
@@ -438,18 +460,17 @@ void nmfd_plan(const NmfdShape& s, NmfdPlan* p) {
   p->dgrad_grid = slide_grid(s, false, p->dgrad_mt, s.R, p->dgrad_nsplit);
   p->wgrad = wgrad_plan(s);
   p->wgrad_nsplit = nmfd_wgrad_nsplit(s);
+  p->wgrad_grid = wgrad_grid(s, p->wgrad, p->wgrad_nsplit);
 }
 
 int nmfd_dgrad(const NmfdShape& s, const float* G, const float* W, float* out, int nsplit, cudaStream_t st) {
   if (s.R > 256) { set_error("nmfd_dgrad: rank must be <= 256"); return 1; }
   const int mt = row_tile(s.R);
-  const dim3 grid = slide_grid(s, false, mt, s.R, nsplit);
+  const Grid3 grid = slide_grid(s, false, mt, s.R, nsplit);
   SlideArgs a{};
   a.A = W; a.X = G; a.M = s.R; a.K = s.C; a.sm = s.w_inner(); a.sk = (int64_t)s.R * s.w_inner(); a.nsplit = nsplit;
   a.out = out;
-  dispatch_slide<false>(mt, s, a, 0, false, grid, st);
-  NMF_LAUNCH_CHECK();
-  return 0;
+  return launch_slices<false>(mt, s, a, 0, false, grid, st);
 }
 
 }  // namespace nmfb200

@@ -55,6 +55,7 @@ struct NmfdTcParams {
   double* loss_part;              // recon loss: one partial per CTA
   int nsplit, kb_per_split;
   int r_off;                      // dgrad: first component of this launch (components [r_off, r_off + 128))
+  int b0;                         // recon / dgrad: first batch element of this launch (batch b0 + blockIdx.z)
 };
 
 struct Smem {
@@ -79,10 +80,10 @@ __device__ __forceinline__ void bulk_copy_g2s(uint32_t dst, const void* src, uin
 }
 
 // One kernel, four roles of the same pipeline (KIND):
-//   recon / recon-loss : grid (L tiles, C tiles, B);  plain = A = Wr16 tile (rows c), Toeplitz = B (rows l), N = 128
+//   recon / recon-loss : grid (L tiles, C tiles, batch slice);  plain = A = Wr16 tile (rows c), Toeplitz = B (rows l), N = 128
 //   wgrad              : grid (C tiles, R x shift blocks, nsplit);  plain = A = P16 tile (rows c),  Toeplitz = B (rows t of
 //                        one block of 128 shifts), N = 128
-//   dgrad              : grid (Lin tiles, nsplit, B); Toeplitz = A (rows j), plain = B = Wf16 rows (c R + r_off + n), N = 128;
+//   dgrad              : grid (Lin tiles, nsplit, batch slice); Toeplitz = A (rows j), plain = B = Wf16 rows (c R + r_off + n), N = 128;
 //                        ranks above 128 take one launch per 128 components
 template <int KIND>
 __global__ void __launch_bounds__(kThreads, 1)
@@ -96,6 +97,7 @@ tcnmfd_kernel(const __grid_constant__ CUtensorMap tmPlain, const NmfdTcParams p)
   constexpr int B_WIN = 0, B_TILE = kStages, B_EMPTY = 2 * kStages, B_WREAD = 3 * kStages;
   constexpr bool RECON = KIND == kRecon || KIND == kReconLoss;
   const int Rb = min((p.R + 15) & ~15, 128);     // dgrad: B-tile rows loaded per k-block
+  const int bz = p.b0 + blockIdx.z;               // recon / dgrad: batch element
 
   if (warp == 0 && lane == 0) {
     ptx::prefetch_tmap(&tmPlain);
@@ -125,7 +127,7 @@ tcnmfd_kernel(const __grid_constant__ CUtensorMap tmPlain, const NmfdTcParams p)
     if (RECON) {
       const int r = kb / tkb, kk = kb - r * tkb;            // k = reversed shift t' in [64 kk, 64 kk + 64)
       px = r * p.Tp + kk * kKB; py = blockIdx.y * kM;
-      src = p.Hp16 + ((int64_t)blockIdx.z * p.R + r) * p.Lp;
+      src = p.Hp16 + ((int64_t)bz * p.R + r) * p.Lp;
       e0 = p.padl + blockIdx.x * kM - p.Tp + 1 + kk * kKB;  // H index l - t = l - (Tp - 1 - t')
     } else if (KIND == kWgrad) {
       const int g = kb0 + kb, b = g / lkb, lk = g - b * lkb;
@@ -135,7 +137,7 @@ tcnmfd_kernel(const __grid_constant__ CUtensorMap tmPlain, const NmfdTcParams p)
     } else {
       const int g = kb0 + kb, c = g / tkb, kk = g - c * tkb;
       px = kk * kKB; py = c * p.R + p.r_off;
-      src = p.P16 + ((int64_t)blockIdx.z * p.C + c) * p.Lq;
+      src = p.P16 + ((int64_t)bz * p.C + c) * p.Lq;
       e0 = blockIdx.x * kM + kk * kKB;                      // row j reads P[j + t]
     }
   };
@@ -230,7 +232,7 @@ tcnmfd_kernel(const __grid_constant__ CUtensorMap tmPlain, const NmfdTcParams p)
       };
       const float sc = exp2f(-(float)(p.exps[KIND == kDgrad ? 0 : (RECON ? 0 : 2)] + p.exps[RECON ? 1 : (KIND == kWgrad ? 1 : 2)]));
       if (RECON) {
-        const int c = blockIdx.y * kM + r128, b = blockIdx.z, l0 = blockIdx.x * kM;
+        const int c = blockIdx.y * kM + r128, b = bz, l0 = blockIdx.x * kM;
         const bool row_ok = c < p.C;
         const float kap = *p.kappa, pscale = exp2f((float)p.exps[2]);
         const float* vrow = p.V + ((int64_t)b * p.C + (row_ok ? c : 0)) * p.L;
@@ -272,7 +274,7 @@ tcnmfd_kernel(const __grid_constant__ CUtensorMap tmPlain, const NmfdTcParams p)
           if (lane == 0) red[q] = acc;
           asm volatile("bar.sync 1, 128;");
           if (q == 0 && lane == 0)
-            p.loss_part[((int64_t)blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x] = (red[0] + red[1]) + (red[2] + red[3]);
+            p.loss_part[((int64_t)b * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x] = (red[0] + red[1]) + (red[2] + red[3]);
         }
       } else if (KIND == kWgrad) {
         const int c = blockIdx.x * kM + r128, r = blockIdx.y / ntb, t0 = (blockIdx.y % ntb) * kM;
@@ -296,7 +298,7 @@ tcnmfd_kernel(const __grid_constant__ CUtensorMap tmPlain, const NmfdTcParams p)
           }
         }
       } else {
-        const int j = blockIdx.x * kM + r128, b = blockIdx.z;
+        const int j = blockIdx.x * kM + r128, b = bz;
 #pragma unroll 1
         for (int jj = 0; jj < Rb / 16; ++jj) {
           uint32_t sr[16];
@@ -423,16 +425,17 @@ prep_w_kernel(const float* __restrict__ W, int C, int R, int T, int Tp, const un
 }
 
 // H (B, R, Lin) fp32 -> Hp16 (B R rows x Lp): H[b,r,j] 2^eH at column padl + j (margins stay zero), 2048 elements per
-// block, + the block's partial sum (-> colsum_H, nmf.py:122-125).  grid (chunks, B R)
+// block, + the block's partial sum (-> colsum_H, nmf.py:122-125).  One-dimensional grid of B R nch blocks, block
+// (row, chunk) = row nch + chunk: B R alone may pass the 65535 of grid.y
 __global__ void __launch_bounds__(256)
-prep_h_kernel(const float* __restrict__ H, int Lin, int Lp, int padl, const unsigned int* __restrict__ absmax,
+prep_h_kernel(const float* __restrict__ H, int Lin, int Lp, int padl, int nch, const unsigned int* __restrict__ absmax,
               int* __restrict__ exps, __half* __restrict__ Hp16, float* __restrict__ cs_part) {
   __shared__ float sh[8];
   const int e = pow2_exp14(__uint_as_float(*absmax));
-  if (blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0) exps[1] = e;
+  if (blockIdx.x == 0 && threadIdx.x == 0) exps[1] = e;
   const float sc = exp2f((float)e);
-  const int64_t row = blockIdx.y;
-  const int j = blockIdx.x * 2048 + threadIdx.x * 8;
+  const int64_t row = blockIdx.x / nch;
+  const int j = (int)(blockIdx.x - row * nch) * 2048 + threadIdx.x * 8;
   float a = 0.f;
   if (j < Lin) {
     float v[8];
@@ -449,7 +452,7 @@ prep_h_kernel(const float* __restrict__ H, int Lin, int Lp, int padl, const unsi
   if (threadIdx.x == 0) {
     float t = 0.f;
     for (int i = 0; i < 8; ++i) t += sh[i];
-    cs_part[row * gridDim.x + blockIdx.x] = t;
+    cs_part[blockIdx.x] = t;
   }
 }
 
@@ -494,6 +497,7 @@ int make_tmap2(CUtensorMap* m, const void* base, int64_t rows, int64_t cols, int
 
 struct TcNmfdState {
   NmfdShape d{};
+  TcNmfdPlan plan{};
   int Tp = 0, Lp = 0, padl = 0, Lq = 0, Cpad = 0;
   __half *Wr16 = nullptr, *Wf16 = nullptr, *Hp16 = nullptr, *P16 = nullptr;
   float* part = nullptr;            // wgrad / dgrad split partials
@@ -513,9 +517,47 @@ struct TcNmfdState {
   CUtensorMap tmWr, tmWf, tmP;
 };
 
+const char* tc_nmfd_plan(const NmfdShape& d, TcNmfdPlan* p) {
+  *p = TcNmfdPlan{};
+  if (d.R < 1 || d.R > 256 || d.T < 1 || d.L < d.T) return "the tensor-core NMFD path needs 1 <= R <= 256 and 1 <= T <= L";
+  p->Tp = round_up(d.T, kKB);
+  p->padl = round_up(p->Tp + 136, 8);                       // every window start >= 0
+  p->Lp = round_up(p->padl + round_up(d.L, 2048) + 256 + kWinHalfs + 136, 8);
+  p->Lq = round_up(round_up(d.L, 2048) + 1024 + p->Tp + kKB + kWinHalfs + 8, 8);
+  p->Cpad = round_up(d.C, kM);
+  const int64_t lkb = ceil_div(d.L, kKB), tkb = p->Tp / kKB;
+  // split the K loops of wgrad / dgrad so that the grid is a few waves of 132 CTAs
+  const int64_t tiles_w = ceil_div(d.C, kM) * d.R * ceil_div(d.T, kM), tiles_h = ceil_div(d.Lin, kM) * d.B;
+  const int64_t kb_w = (int64_t)d.B * lkb, kb_h = (int64_t)d.C * tkb;
+  p->ws_w = std::max<int64_t>(1, std::min<int64_t>(kb_w / 8, ceil_div(132 * 4, tiles_w)));
+  p->ws_h = std::max<int64_t>(1, std::min<int64_t>(kb_h / 8, ceil_div(132 * 4, tiles_h)));
+  p->kbs_w = ceil_div(kb_w, p->ws_w); p->ws_w = ceil_div(kb_w, p->kbs_w);
+  p->kbs_h = ceil_div(kb_h, p->ws_h); p->ws_h = ceil_div(kb_h, p->kbs_h);
+  p->nch = ceil_div(d.Lin, 2048);
+  p->bslice = nmfd_batch_slice(d.B);
+  p->slices = ceil_div(d.B, p->bslice);
+  p->dgrad_rblocks = ceil_div(d.R, kM);
+  p->prep_w = Grid3{d.C, 1, 1};
+  p->prep_h = Grid3{(int64_t)d.B * d.R * p->nch, 1, 1};
+  p->recon = Grid3{ceil_div(d.L, kM), ceil_div(d.C, kM), p->bslice};
+  p->wgrad = Grid3{ceil_div(d.C, kM), (int64_t)d.R * ceil_div(d.T, kM), p->ws_w};
+  p->dgrad = Grid3{ceil_div(d.Lin, kM), p->ws_h, p->bslice};
+  p->loss_blocks = p->recon.x * p->recon.y * d.B;
+  if (!grid_fits(p->wgrad)) return "the tensor-core NMFD wgrad grid needs R ceil(T / 128) <= 65535";
+  for (const Grid3* g : {&p->prep_w, &p->prep_h, &p->recon, &p->dgrad})
+    if (!grid_fits(*g)) return "a tensor-core NMFD grid passes the CUDA grid limits";
+  // 32-bit quantities of the kernels: the TMA row coordinate b C + c of the ratio tile, the global k-block indices of
+  // wgrad / dgrad, the loss partial count (sum_partials), the row pitches
+  if ((int64_t)d.B * d.C + kM > INT32_MAX) return "the tensor-core NMFD path needs B C < 2^31 - 128 (TMA row coordinate)";
+  if (kb_w > INT32_MAX || kb_h > INT32_MAX || p->loss_blocks > INT32_MAX || p->Lp > INT32_MAX || p->Lq > INT32_MAX ||
+      p->Cpad * d.R > INT32_MAX)
+    return "a tensor-core NMFD block or k-block count passes 2^31 - 1";
+  return nullptr;
+}
+
 bool tc_nmfd_supported(const NmfdShape& d, double beta) {
-  // wgrad's grid.y = R x blocks of 128 shifts
-  return beta == 1.0 && d.R >= 1 && d.R <= 256 && d.T >= 1 && d.L >= d.T && (int64_t)d.R * ceil_div(d.T, kM) <= 65535;
+  TcNmfdPlan p;
+  return beta == 1.0 && tc_nmfd_plan(d, &p) == nullptr;
 }
 
 void tc_nmfd_destroy(TcNmfdState* s) {
@@ -527,25 +569,17 @@ void tc_nmfd_destroy(TcNmfdState* s) {
 
 int tc_nmfd_create(TcNmfdState** out, const NmfdShape& d) {
   *out = nullptr;
+  TcNmfdPlan plan;
+  if (const char* why = tc_nmfd_plan(d, &plan)) { set_error(why); return 1; }
   TcNmfdState* s = new TcNmfdState();
   s->d = d;
-  s->Tp = (int)round_up(d.T, kKB);
-  s->padl = (int)round_up(s->Tp + 136, 8);                       // every window start >= 0
-  s->Lp = (int)round_up((int64_t)s->padl + round_up((int64_t)d.L, 2048) + 256 + kWinHalfs + 136, 8);
-  s->Lq = (int)round_up(round_up((int64_t)d.L, 2048) + 1024 + s->Tp + kKB + kWinHalfs + 8, 8);
-  s->Cpad = (int)round_up(d.C, kM);
-  const int lkb = (int)ceil_div(d.L, kKB), tkb = s->Tp / kKB;
-  // split the K loops of wgrad / dgrad so that the grid is a few waves of 132 CTAs
-  const int64_t tiles_w = ceil_div(d.C, kM) * d.R * ceil_div(d.T, kM), tiles_h = ceil_div(d.Lin, kM) * d.B;
-  int64_t kb_w = (int64_t)d.B * lkb, kb_h = (int64_t)d.C * tkb;
-  s->ws_w = (int)std::max<int64_t>(1, std::min<int64_t>(kb_w / 8, ceil_div(132 * 4, tiles_w)));
-  s->ws_h = (int)std::max<int64_t>(1, std::min<int64_t>(kb_h / 8, ceil_div(132 * 4, tiles_h)));
-  s->kbs_w = (int)ceil_div(kb_w, s->ws_w); s->ws_w = (int)ceil_div(kb_w, s->kbs_w);
-  s->kbs_h = (int)ceil_div(kb_h, s->ws_h); s->ws_h = (int)ceil_div(kb_h, s->kbs_h);
-  const int hs = s->ws_h;
-  const int64_t pw = (int64_t)s->ws_w * d.C * d.R * d.T, ph = (int64_t)hs * d.B * d.R * d.Lin;
+  s->plan = plan;
+  const TcNmfdPlan& pl = s->plan;
+  s->Tp = (int)pl.Tp; s->padl = (int)pl.padl; s->Lp = (int)pl.Lp; s->Lq = (int)pl.Lq; s->Cpad = (int)pl.Cpad;
+  s->ws_w = (int)pl.ws_w; s->kbs_w = (int)pl.kbs_w; s->ws_h = (int)pl.ws_h; s->kbs_h = (int)pl.kbs_h;
+  const int64_t pw = (int64_t)s->ws_w * d.C * d.R * d.T, ph = (int64_t)s->ws_h * d.B * d.R * d.Lin;
   s->part_floats = pw > ph ? pw : ph;
-  s->loss_blocks = (int)(ceil_div(d.L, kM) * ceil_div(d.C, kM) * d.B);
+  s->loss_blocks = (int)pl.loss_blocks;
   const size_t wbytes = (size_t)s->Cpad * d.R * s->Tp * 2, hbytes = (size_t)d.B * d.R * s->Lp * 2;
   const size_t pbytes = ((size_t)d.B * d.C + 1) * s->Lq * 2;
   cudaError_t e = cudaSuccess;
@@ -557,7 +591,7 @@ int tc_nmfd_create(TcNmfdState** out, const NmfdShape& d) {
   if (e == cudaSuccess) e = cudaMalloc(&s->absmax, 2 * sizeof(unsigned int));
   if (e == cudaSuccess) e = cudaMalloc(&s->colsum, 2 * (size_t)d.R * sizeof(float));
   {
-    const int64_t np = std::max<int64_t>((int64_t)d.C * d.R, (int64_t)d.B * d.R * ceil_div(d.Lin, 2048));
+    const int64_t np = std::max<int64_t>((int64_t)d.C * d.R, pl.prep_h.x);
     if (e == cudaSuccess) e = cudaMalloc(&s->cs_part, (size_t)np * sizeof(float));
   }
   if (e == cudaSuccess) e = cudaMalloc(&s->exps, 8 * sizeof(int));          // [0..3] exponents, [4..5] fold tickets
@@ -599,8 +633,10 @@ int tc_nmfd_set_target(TcNmfdState* s, const float* V, double* vsum_host, cudaSt
 
 namespace {
 
+dim3 dim3_of(const Grid3& g) { return dim3((unsigned)g.x, (unsigned)g.y, (unsigned)g.z); }
+
 template <int KIND>
-int launch(TcNmfdState* s, const CUtensorMap& tm, dim3 grid, NmfdTcParams& p, cudaStream_t st) {
+int launch(TcNmfdState* s, const CUtensorMap& tm, dim3 grid, const NmfdTcParams& p, cudaStream_t st) {
   auto kern = tcnmfd_kernel<KIND>;
   static unsigned long long attr_set_mask = 0;      // per device (one bit each): the attribute is per-device state
   const int smem = Smem::kTotal + 1024;
@@ -612,6 +648,18 @@ int launch(TcNmfdState* s, const CUtensorMap& tm, dim3 grid, NmfdTcParams& p, cu
   }
   kern<<<grid, kThreads, smem, st>>>(tm, p);
   NMF_LAUNCH_CHECK();
+  return 0;
+}
+
+// recon / dgrad: one launch per slice of at most plan.bslice batch elements (grid.z), batch offset b0
+template <int KIND>
+int launch_slices(TcNmfdState* s, const CUtensorMap& tm, const Grid3& g, NmfdTcParams p, cudaStream_t st) {
+  for (int64_t b0 = 0; b0 < s->d.B; b0 += g.z) {
+    p.b0 = (int)b0;
+    dim3 grid = dim3_of(g);
+    grid.z = (unsigned)std::min<int64_t>(g.z, s->d.B - b0);
+    if (int rc = launch<KIND>(s, tm, grid, p, st)) return rc;
+  }
   return 0;
 }
 
@@ -644,7 +692,7 @@ int refresh(TcNmfdState* s, const float* W, const float* H, cudaStream_t st) {
       NMF_LAUNCH_CHECK();
       s->aw_valid = true;
     }
-    prep_w_kernel<<<d.C, 256, 0, st>>>(W, d.C, d.R, d.T, s->Tp, s->absmax, s->exps, s->Wr16, s->Wf16, s->cs_part);
+    prep_w_kernel<<<(unsigned)s->plan.prep_w.x, 256, 0, st>>>(W, d.C, d.R, d.T, s->Tp, s->absmax, s->exps, s->Wr16, s->Wf16, s->cs_part);
     NMF_LAUNCH_CHECK();
     fold_colsum_kernel<<<d.R, 256, 0, st>>>(fold_tail_args(s, 0, d.C, 1, /*do_kappa=*/s->h_fresh));
     NMF_LAUNCH_CHECK();
@@ -657,9 +705,9 @@ int refresh(TcNmfdState* s, const float* W, const float* H, cudaStream_t st) {
       NMF_LAUNCH_CHECK();
       s->ah_valid = true;
     }
-    const int nch = (int)ceil_div(d.Lin, 2048);
-    dim3 gh((unsigned)nch, (unsigned)(d.B * d.R));
-    prep_h_kernel<<<gh, 256, 0, st>>>(H, d.Lin, s->Lp, s->padl, s->absmax + 1, s->exps, s->Hp16, s->cs_part);
+    const int nch = (int)s->plan.nch;
+    prep_h_kernel<<<(unsigned)s->plan.prep_h.x, 256, 0, st>>>(H, d.Lin, s->Lp, s->padl, nch, s->absmax + 1, s->exps, s->Hp16,
+                                                              s->cs_part);
     NMF_LAUNCH_CHECK();
     fold_colsum_kernel<<<d.R, 256, 0, st>>>(fold_tail_args(s, 1, d.B, nch, /*do_kappa=*/1));
     NMF_LAUNCH_CHECK();
@@ -675,13 +723,12 @@ int tc_nmfd_recon(TcNmfdState* s, const float* V, const float* W, const float* H
   int rc = refresh(s, W, H, st);
   if (rc) return rc;
   NmfdTcParams p = base_params(s, V);
-  dim3 grid((unsigned)ceil_div(s->d.L, kM), (unsigned)ceil_div(s->d.C, kM), (unsigned)s->d.B);
   if (loss) {
-    rc = launch<kReconLoss>(s, s->tmWr, grid, p, st);
+    rc = launch_slices<kReconLoss>(s, s->tmWr, s->plan.recon, p, st);
     if (rc) return rc;
-    return sum_partials(s->loss_part, (int)(grid.x * grid.y * grid.z), loss_dev, st);
+    return sum_partials(s->loss_part, s->loss_blocks, loss_dev, st);
   }
-  return launch<kRecon>(s, s->tmWr, grid, p, st);
+  return launch_slices<kRecon>(s, s->tmWr, s->plan.recon, p, st);
 }
 
 // numerator partials of the W update from the P16 written by the last recon: [*nsplit][C][R][T] fp32
@@ -689,8 +736,7 @@ int tc_nmfd_wgrad(TcNmfdState* s, const float** part, int* nsplit, cudaStream_t 
   NmfdTcParams p = base_params(s, nullptr);
   p.nsplit = s->ws_w; p.kb_per_split = s->kbs_w;
   // one CTA per (128 rows c, component r, block of 128 shifts t, split): the Toeplitz tile holds 128 shifts
-  dim3 grid((unsigned)ceil_div(s->d.C, kM), (unsigned)(s->d.R * ceil_div(s->d.T, kM)), (unsigned)s->ws_w);
-  int rc = launch<kWgrad>(s, s->tmP, grid, p, st);
+  int rc = launch<kWgrad>(s, s->tmP, dim3_of(s->plan.wgrad), p, st);
   *part = s->part; *nsplit = s->ws_w;
   return rc;
 }
@@ -698,9 +744,8 @@ int tc_nmfd_wgrad(TcNmfdState* s, const float** part, int* nsplit, cudaStream_t 
 int tc_nmfd_dgrad(TcNmfdState* s, const float** part, int* nsplit, cudaStream_t st) {
   NmfdTcParams p = base_params(s, nullptr);
   p.nsplit = s->ws_h; p.kb_per_split = s->kbs_h;
-  dim3 grid((unsigned)ceil_div(s->d.Lin, kM), (unsigned)s->ws_h, (unsigned)s->d.B);
   int rc = 0;
-  for (p.r_off = 0; rc == 0 && p.r_off < s->d.R; p.r_off += 128) rc = launch<kDgrad>(s, s->tmWf, grid, p, st);
+  for (p.r_off = 0; rc == 0 && p.r_off < s->d.R; p.r_off += 128) rc = launch_slices<kDgrad>(s, s->tmWf, s->plan.dgrad, p, st);
   *part = s->part; *nsplit = s->ws_h;
   return rc;
 }

@@ -7,6 +7,19 @@ namespace nmfb200 {
 
 struct TcNmfdState;
 
+// What the tensor-core path launches for a shape, computed in 64 bits before anything is narrowed: the grids of the operand
+// preparation and contraction kernels (recon and dgrad grids per launch: batches beyond grid.z take `slices` launches of at
+// most `bslice` elements each, dgrad one launch per 128 components), split counts and buffer pitches.
+struct TcNmfdPlan {
+  int64_t Tp, padl, Lp, Lq, Cpad;
+  int64_t ws_w, kbs_w, ws_h, kbs_h;       // split-K of wgrad / dgrad: splits, k-blocks per split
+  int64_t loss_blocks;                    // recon-loss partials (one per CTA of all slices)
+  int64_t nch;                            // 2048-element chunks per H row (prep_h)
+  Grid3 prep_w, prep_h, recon, wgrad, dgrad;
+  int64_t bslice, slices, dgrad_rblocks;
+};
+// nullptr if every grid and every count the kernels hold in 32 bits fits, else the limit the shape crosses
+const char* tc_nmfd_plan(const NmfdShape& d, TcNmfdPlan* p);
 bool tc_nmfd_supported(const NmfdShape& d, double beta);
 int tc_nmfd_create(TcNmfdState** out, const NmfdShape& d);
 void tc_nmfd_destroy(TcNmfdState* s);

@@ -63,8 +63,9 @@ SIGNATURES = {
     "nmfb200_nmf_plan": (_int, [_i64, _i64, _i64, _c.POINTER(_i64), _int]),
     "nmfb200_nmfd_plan": (_int, [_i64, _i64, _int, _c.POINTER(_i64), _i64, _c.POINTER(_i64), _c.POINTER(_i64), _int]),
     "nmfb200_nmf_sparse_plan": (_int, [_i64, _i64, _i64, _c.POINTER(_i64), _int]),
+    "nmfb200_nmfd_tc_plan": (_int, [_i64, _i64, _i64, _i64, _i64, _c.POINTER(_i64), _int]),
 }
-NMF_PLAN_LEN, NMFD_PLAN_LEN, SPARSE_PLAN_LEN = 9, 19, 8         # include/nmf_b200.h
+NMF_PLAN_LEN, NMFD_PLAN_LEN, SPARSE_PLAN_LEN, NMFD_TC_PLAN_LEN = 9, 19, 8, 23         # include/nmf_b200.h
 
 _lib = None
 
@@ -139,3 +140,14 @@ def nmfd_plan(B, C, vdims, R, kdims):
     return {"recon_mt": v[0], "recon_grid": tuple(v[1:4]), "dgrad_mt": v[4], "dgrad_nsplit": v[5],
             "dgrad_grid": tuple(v[6:9]), "wgrad": dict(zip(("mt", "tp", "nr", "no", "ntt", "nrg", "nog"), v[9:16])),
             "wgrad_nsplit": v[16], "vec4_w": bool(v[17]), "vec4_h": bool(v[18])}
+
+
+def nmfd_tc_plan(B, C, L, R, T):
+    """The tensor-core NMFD kernels' launch plan (nmfb200_nmfd_tc_plan), as a dict; no device needed.  Raises NmfB200Error
+    naming the limit for a shape the tensor-core path does not take."""
+    out = (_i64 * NMFD_TC_PLAN_LEN)()
+    check(load().nmfb200_nmfd_tc_plan(B, C, L, R, T, out, NMFD_TC_PLAN_LEN))
+    v = list(out)
+    return {"prep_w": tuple(v[0:3]), "prep_h": tuple(v[3:6]), "recon": tuple(v[6:9]), "wgrad": tuple(v[9:12]),
+            "dgrad": tuple(v[12:15]), "bslice": v[15], "slices": v[16], "dgrad_rblocks": v[17], "loss_blocks": v[18],
+            "ws_w": v[19], "kbs_w": v[20], "ws_h": v[21], "kbs_h": v[22]}
