@@ -12,8 +12,7 @@ namespace nmfb200 {
 static thread_local std::string g_err;
 static std::atomic<int64_t> g_launches{0};
 void set_error(const std::string& msg) { g_err = msg; }
-void count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
-int64_t launch_counter() { return g_launches.load(); }
+void count_launch() { g_launches.fetch_add(1, std::memory_order_relaxed); }
 }  // namespace nmfb200
 
 using namespace nmfb200;
@@ -110,17 +109,27 @@ void free_ctx(nmfb200_ctx* c) {
   delete c;
 }
 
-// CUDA-core contraction of one NMF factor update into c->num / c->den (chunked partials).
-int simt_contract_w(nmfb200_ctx* c, const float* W, const float* H, double beta, cudaStream_t st) {
-  // F = W (C rows), G = H (N rows), Vm = V^T
+// CUDA-core contraction of one NMF factor update (which = 0: W, 1: H) into c->num / c->den (chunked partials).
+int simt_contract(nmfb200_ctx* c, int which, const float* W, const float* H, double beta, cudaStream_t st) {
   if (beta != 1.0) { int e = ensure_den(c); if (e) return e; }
-  return simt_nmf_contract(c->V, c->ldv, /*trans=*/1, W, H, c->C, c->N, (int)c->R, beta, c->nch_w, c->num,
-                           c->den, c->R, c->C * c->R, st);
+  // W update: F = W (C rows), G = H (N rows), Vm = V^T;  H update: F = H (N rows), G = W (C rows), Vm = V
+  const float* F = which == 0 ? W : H;
+  const float* G = which == 0 ? H : W;
+  const int64_t rows = which == 0 ? c->C : c->N, cols = which == 0 ? c->N : c->C;
+  return simt_nmf_contract(c->V, c->ldv, /*trans=*/which == 0 ? 1 : 0, F, G, rows, cols, (int)c->R, beta,
+                           which == 0 ? c->nch_w : c->nch_h, c->num, c->den, c->R, rows * c->R, st);
 }
-int simt_contract_h(nmfb200_ctx* c, const float* W, const float* H, double beta, cudaStream_t st) {
-  if (beta != 1.0) { int e = ensure_den(c); if (e) return e; }
-  return simt_nmf_contract(c->V, c->ldv, /*trans=*/0, H, W, c->N, c->C, (int)c->R, beta, c->nch_h, c->num,
-                           c->den, c->R, c->N * c->R, st);
+
+// The ratio stage's view of one NMF factor (which = 0: W, 1: H) of R components: numerators summed over `nchunks` partial
+// slabs, and `den` = the column sums of the other factor (beta 1) or the raw denominators in the numerators' layout.
+ApplyArgs nmf_apply_args(const nmfb200_ctx* c, int which, float* param, double beta, const float* num, const float* den,
+                         int nchunks, int64_t chunk_stride, double gamma, double l1, double l2) {
+  ApplyArgs a{};
+  a.param = param; a.numel = (which == 0 ? c->C : c->N) * c->R; a.R = (int)c->R; a.inner = 1; a.rowlen = c->R;
+  a.num = num; a.den = beta == 1.0 ? nullptr : den; a.nchunks = nchunks; a.chunk_stride = chunk_stride;
+  a.ldp = c->R; a.kl_den = beta == 1.0 ? den : nullptr; a.out_scale = nullptr;
+  a.gamma = (float)gamma; a.l1 = (float)l1; a.l2 = (float)l2; a.absmax_bits = nullptr;
+  return a;
 }
 
 bool use_tc(const nmfb200_ctx* c, double beta) {
@@ -342,21 +351,56 @@ int sparse_terms(nmfb200_ctx* ctx, int which, const float* F, const float* other
 // one factor update: sparse_terms into the context's scratch, then the ratio stage
 int sparse_update(nmfb200_ctx* ctx, int which, float* F, const float* other, double beta, double gamma, double l1_reg,
                   double l2_reg, cudaStream_t st) {
-  const int R = (int)ctx->R;
-  const int64_t rows = which == 0 ? ctx->C : ctx->N;
   if (beta == 2.0) {
     int rc = ensure_den(ctx);
     if (rc) return rc;
   }
-  float* den = beta == 1.0 ? ctx->colsum + (1 - which) * R : ctx->den;
+  float* den = beta == 1.0 ? ctx->colsum + (1 - which) * ctx->R : ctx->den;
   int rc = sparse_terms(ctx, which, F, other, beta, ctx->num, den, st);
   if (rc) return rc;
-  ApplyArgs a{};
-  a.param = F; a.numel = rows * R; a.R = R; a.inner = 1; a.rowlen = R;
-  a.num = ctx->num; a.den = beta == 1.0 ? nullptr : den; a.nchunks = 1; a.chunk_stride = 0;
-  a.ldp = R; a.kl_den = beta == 1.0 ? den : nullptr; a.out_scale = nullptr;
-  a.gamma = (float)gamma; a.l1 = (float)l1_reg; a.l2 = (float)l2_reg; a.absmax_bits = nullptr;
-  return apply_update(a, st);
+  return apply_update(nmf_apply_args(ctx, which, F, beta, ctx->num, den, 1, 0, gamma, l1_reg, l2_reg), st);
+}
+
+// One factor update (which = 0: param = W, 1: param = H) on the kernels that serve this context and beta: sparse-target,
+// tensor-core or fp32.  No device guard: the entry points select the context's device.
+int nmf_update(nmfb200_ctx* ctx, int which, float* param, const float* W, const float* H, double beta, double gamma,
+               double l1_reg, double l2_reg, cudaStream_t st) {
+  const float* other = which == 0 ? H : W;
+  if (ctx->sparse) return sparse_update(ctx, which, param, other, beta, gamma, l1_reg, l2_reg, st);
+  if (use_tc(ctx, beta)) return tc_update(ctx->tc, which, param, W, H, beta, gamma, l1_reg, l2_reg, st);
+  int rc = simt_contract(ctx, which, W, H, beta, st);
+  if (rc) return rc;
+  float* den = ctx->den;
+  if (beta == 1.0) {      // nmf.py:122-131: the KL denominator is the column sum of the OTHER factor
+    den = ctx->colsum + (1 - which) * ctx->R;
+    rc = factor_colsum(other, which == 0 ? ctx->N : ctx->C, (int)ctx->R, 1, ctx->cs_scratch, ctx->cs_scratch_floats, den, st);
+    if (rc) return rc;
+  }
+  const int64_t rows = which == 0 ? ctx->C : ctx->N;
+  rc = apply_update(nmf_apply_args(ctx, which, param, beta, ctx->num, den, which == 0 ? ctx->nch_w : ctx->nch_h,
+                                   rows * ctx->R, gamma, l1_reg, l2_reg), st);
+  if (rc) return rc;
+  if (ctx->tc) tc_mark_dirty(ctx->tc, which == 0, which == 1);
+  return 0;
+}
+
+// The raw terms of one factor's update (which = 0: W, 1: H) into `out`, nmfb200_nmf_raw_terms_numel floats.
+int nmf_raw_terms(nmfb200_ctx* ctx, const float* W, const float* H, int which, double beta, float* out, cudaStream_t st) {
+  const int64_t rows = which == 0 ? ctx->C : ctx->N;
+  const int64_t RR = rows * ctx->R;
+  if (ctx->sparse) return sparse_terms(ctx, which, which == 0 ? W : H, which == 0 ? H : W, beta, out, out + RR, st);
+  if (use_tc(ctx, beta) && tc_supports_partial(ctx->tc, beta)) return tc_raw_terms(ctx->tc, which, W, H, beta, out, st);
+  int rc = simt_contract(ctx, which, W, H, beta, st);
+  if (rc) return rc;
+  const int nch = which == 0 ? ctx->nch_w : ctx->nch_h;
+  rc = reduce_chunks(ctx->num, nch, RR, rows, (int)ctx->R, ctx->R, out, st);
+  if (rc) return rc;
+  if (beta == 1.0) {      // nmf.py:122-131: the KL denominator is the column sum of the OTHER factor
+    const float* other = which == 0 ? H : W;
+    return factor_colsum(other, which == 0 ? ctx->N : ctx->C, (int)ctx->R, 1, ctx->cs_scratch, ctx->cs_scratch_floats,
+                         out + RR, st);
+  }
+  return reduce_chunks(ctx->den, nch, RR, rows, (int)ctx->R, ctx->R, out + RR, st);
 }
 
 int sparse_loss_ctx(nmfb200_ctx* ctx, const float* W, const float* H, double beta, double* loss_dev, cudaStream_t st) {
@@ -404,26 +448,7 @@ int nmfb200_nmf_update_w(nmfb200_ctx* ctx, float* W, const float* H, double beta
   CTX_GUARD(ctx, 0);
   if (!ctx->has_target) return fail(NMFB200_ERR_STATE, "set_target has not been called");
   if (!W || !H) return fail(NMFB200_ERR_INVALID, "null factor pointer");
-  cudaStream_t st = (cudaStream_t)stream;
-  if (ctx->sparse) return sparse_update(ctx, 0, W, H, beta, gamma, l1_reg, l2_reg, st);
-  if (use_tc(ctx, beta)) return tc_update_w(ctx->tc, W, H, beta, gamma, l1_reg, l2_reg, st);
-  int rc = simt_contract_w(ctx, W, H, beta, st);
-  if (rc) return rc;
-  float* kl = nullptr;
-  if (beta == 1.0) {
-    kl = ctx->colsum + ctx->R;
-    rc = factor_colsum(H, ctx->N, (int)ctx->R, 1, ctx->cs_scratch, ctx->cs_scratch_floats, kl, st);
-    if (rc) return rc;
-  }
-  ApplyArgs a{};
-  a.param = W; a.numel = ctx->C * ctx->R; a.R = (int)ctx->R; a.inner = 1; a.rowlen = ctx->R;
-  a.num = ctx->num; a.den = beta == 1.0 ? nullptr : ctx->den; a.nchunks = ctx->nch_w;
-  a.chunk_stride = ctx->C * ctx->R; a.ldp = ctx->R; a.kl_den = kl; a.out_scale = nullptr;
-  a.gamma = (float)gamma; a.l1 = (float)l1_reg; a.l2 = (float)l2_reg; a.absmax_bits = nullptr;
-  rc = apply_update(a, st);
-  if (rc) return rc;
-  if (ctx->tc) tc_mark_dirty(ctx->tc, true, false);
-  return 0;
+  return nmf_update(ctx, 0, W, W, H, beta, gamma, l1_reg, l2_reg, (cudaStream_t)stream);
 }
 
 int nmfb200_nmf_update_h(nmfb200_ctx* ctx, const float* W, float* H, double beta, double gamma, double l1_reg,
@@ -431,26 +456,7 @@ int nmfb200_nmf_update_h(nmfb200_ctx* ctx, const float* W, float* H, double beta
   CTX_GUARD(ctx, 0);
   if (!ctx->has_target) return fail(NMFB200_ERR_STATE, "set_target has not been called");
   if (!W || !H) return fail(NMFB200_ERR_INVALID, "null factor pointer");
-  cudaStream_t st = (cudaStream_t)stream;
-  if (ctx->sparse) return sparse_update(ctx, 1, H, W, beta, gamma, l1_reg, l2_reg, st);
-  if (use_tc(ctx, beta)) return tc_update_h(ctx->tc, W, H, beta, gamma, l1_reg, l2_reg, st);
-  int rc = simt_contract_h(ctx, W, H, beta, st);
-  if (rc) return rc;
-  float* kl = nullptr;
-  if (beta == 1.0) {
-    kl = ctx->colsum;
-    rc = factor_colsum(W, ctx->C, (int)ctx->R, 1, ctx->cs_scratch, ctx->cs_scratch_floats, kl, st);
-    if (rc) return rc;
-  }
-  ApplyArgs a{};
-  a.param = H; a.numel = ctx->N * ctx->R; a.R = (int)ctx->R; a.inner = 1; a.rowlen = ctx->R;
-  a.num = ctx->num; a.den = beta == 1.0 ? nullptr : ctx->den; a.nchunks = ctx->nch_h;
-  a.chunk_stride = ctx->N * ctx->R; a.ldp = ctx->R; a.kl_den = kl; a.out_scale = nullptr;
-  a.gamma = (float)gamma; a.l1 = (float)l1_reg; a.l2 = (float)l2_reg; a.absmax_bits = nullptr;
-  rc = apply_update(a, st);
-  if (rc) return rc;
-  if (ctx->tc) tc_mark_dirty(ctx->tc, false, true);
-  return 0;
+  return nmf_update(ctx, 1, H, W, H, beta, gamma, l1_reg, l2_reg, (cudaStream_t)stream);
 }
 
 int nmfb200_nmf_iterate(nmfb200_ctx* ctx, float* W, float* H, double beta, double gamma, double l1_reg,
@@ -458,11 +464,11 @@ int nmfb200_nmf_iterate(nmfb200_ctx* ctx, float* W, float* H, double beta, doubl
   CTX_GUARD(ctx, 0);
   if (!ctx->has_target) return fail(NMFB200_ERR_STATE, "set_target has not been called");
   if (!W || !H || n_iter < 0) return fail(NMFB200_ERR_INVALID, "bad argument");
-  if (use_tc(ctx, beta)) return tc_iterate(ctx->tc, W, H, beta, gamma, l1_reg, l2_reg, n_iter, (cudaStream_t)stream);
+  cudaStream_t st = (cudaStream_t)stream;
   for (int i = 0; i < n_iter; ++i) {
-    int rc = nmfb200_nmf_update_w(ctx, W, H, beta, gamma, l1_reg, l2_reg, stream);
+    int rc = nmf_update(ctx, 0, W, W, H, beta, gamma, l1_reg, l2_reg, st);
     if (rc) return rc;
-    rc = nmfb200_nmf_update_h(ctx, W, H, beta, gamma, l1_reg, l2_reg, stream);
+    rc = nmf_update(ctx, 1, H, W, H, beta, gamma, l1_reg, l2_reg, st);
     if (rc) return rc;
   }
   return 0;
@@ -475,7 +481,7 @@ int nmfb200_nmf_loss(nmfb200_ctx* ctx, const float* W, const float* H, double be
   if (!W || !H || !loss_dev) return fail(NMFB200_ERR_INVALID, "null pointer");
   cudaStream_t st = (cudaStream_t)stream;
   if (ctx->sparse) return sparse_loss_ctx(ctx, W, H, beta, loss_dev, st);
-  if (use_tc(ctx, beta) && tc_supports_loss(ctx->tc, beta)) return tc_loss(ctx->tc, W, H, beta, loss_dev, st);
+  if (use_tc(ctx, beta)) return tc_loss(ctx->tc, W, H, beta, loss_dev, st);
   return simt_nmf_loss(ctx->V, ctx->ldv, H, W, ctx->N, ctx->C, (int)ctx->R, beta, ctx->loss_blocks,
                        ctx->loss_max_blocks, loss_dev, st);
 }
@@ -485,14 +491,13 @@ int nmfb200_nmf_loss_prefetch_w(nmfb200_ctx* ctx, const float* W, const float* H
   CTX_GUARD(ctx, 0);
   if (!ctx->has_target) return fail(NMFB200_ERR_STATE, "set_target has not been called");
   if (!W || !H || !loss_dev) return fail(NMFB200_ERR_INVALID, "null pointer");
-  if (!ctx->sparse && use_tc(ctx, beta) && tc_supports_loss(ctx->tc, beta))
+  if (!ctx->sparse && use_tc(ctx, beta))
     return tc_loss_prefetch_w(ctx->tc, W, H, beta, loss_dev, (cudaStream_t)stream);
   return nmfb200_nmf_loss(ctx, W, H, beta, loss_dev, stream);
 }
 
 int64_t nmfb200_nmf_w_partial_numel(const nmfb200_ctx* ctx, double beta) {
-  if (!ctx || ctx->kind != 0) return -1;
-  return beta == 1.0 ? ctx->C * ctx->R + ctx->R : 2 * ctx->C * ctx->R;
+  return nmfb200_nmf_raw_terms_numel(ctx, 0, beta);
 }
 
 int nmfb200_nmf_w_partial(nmfb200_ctx* ctx, const float* W, const float* H, double beta, float* partial,
@@ -501,16 +506,7 @@ int nmfb200_nmf_w_partial(nmfb200_ctx* ctx, const float* W, const float* H, doub
   if (!ctx->has_target) return fail(NMFB200_ERR_STATE, "set_target has not been called");
   if (ctx->sparse) return fail(NMFB200_ERR_STATE, "not available for a sparse target");
   if (!W || !H || !partial) return fail(NMFB200_ERR_INVALID, "null pointer");
-  cudaStream_t st = (cudaStream_t)stream;
-  if (use_tc(ctx, beta) && tc_supports_partial(ctx->tc, beta)) return tc_w_partial(ctx->tc, W, H, beta, partial, st);
-  int rc = simt_contract_w(ctx, W, H, beta, st);
-  if (rc) return rc;
-  const int64_t CR = ctx->C * ctx->R;
-  rc = reduce_chunks(ctx->num, ctx->nch_w, CR, ctx->C, (int)ctx->R, ctx->R, partial, st);
-  if (rc) return rc;
-  if (beta == 1.0)
-    return factor_colsum(H, ctx->N, (int)ctx->R, 1, ctx->cs_scratch, ctx->cs_scratch_floats, partial + CR, st);
-  return reduce_chunks(ctx->den, ctx->nch_w, CR, ctx->C, (int)ctx->R, ctx->R, partial + CR, st);
+  return nmf_raw_terms(ctx, W, H, 0, beta, partial, (cudaStream_t)stream);
 }
 
 int64_t nmfb200_nmf_raw_terms_numel(const nmfb200_ctx* ctx, int which, double beta) {
@@ -524,22 +520,7 @@ int nmfb200_nmf_raw_terms(nmfb200_ctx* ctx, const float* W, const float* H, int 
   CTX_GUARD(ctx, 0);
   if (!ctx->has_target) return fail(NMFB200_ERR_STATE, "set_target has not been called");
   if (!W || !H || !out || (which != 0 && which != 1)) return fail(NMFB200_ERR_INVALID, "bad argument");
-  cudaStream_t st = (cudaStream_t)stream;
-  const int64_t rows = which == 0 ? ctx->C : ctx->N;
-  const int64_t RR = rows * ctx->R;
-  if (ctx->sparse) return sparse_terms(ctx, which, which == 0 ? W : H, which == 0 ? H : W, beta, out, out + RR, st);
-  if (use_tc(ctx, beta) && tc_supports_partial(ctx->tc, beta)) return tc_raw_terms(ctx->tc, which, W, H, beta, out, st);
-  int rc = which == 0 ? simt_contract_w(ctx, W, H, beta, st) : simt_contract_h(ctx, W, H, beta, st);
-  if (rc) return rc;
-  const int nch = which == 0 ? ctx->nch_w : ctx->nch_h;
-  rc = reduce_chunks(ctx->num, nch, RR, rows, (int)ctx->R, ctx->R, out, st);
-  if (rc) return rc;
-  if (beta == 1.0) {      // nmf.py:122-131: the KL denominator is the column sum of the OTHER factor
-    const float* other = which == 0 ? H : W;
-    return factor_colsum(other, which == 0 ? ctx->N : ctx->C, (int)ctx->R, 1, ctx->cs_scratch, ctx->cs_scratch_floats,
-                         out + RR, st);
-  }
-  return reduce_chunks(ctx->den, nch, RR, rows, (int)ctx->R, ctx->R, out + RR, st);
+  return nmf_raw_terms(ctx, W, H, which, beta, out, (cudaStream_t)stream);
 }
 
 /* ---- row-sharded W update over peer memory (NVLink, one process per GPU) ---------------------- */
@@ -588,13 +569,7 @@ int nmfb200_nmf_w_apply(nmfb200_ctx* ctx, float* W, const float* reduced, double
   if (!W || !reduced) return fail(NMFB200_ERR_INVALID, "null pointer");
   cudaStream_t st = (cudaStream_t)stream;
   if (use_tc(ctx, beta)) return tc_w_apply(ctx->tc, W, reduced, beta, gamma, l1_reg, l2_reg, st);
-  const int64_t CR = ctx->C * ctx->R;
-  ApplyArgs a{};
-  a.param = W; a.numel = CR; a.R = (int)ctx->R; a.inner = 1; a.rowlen = ctx->R;
-  a.num = reduced; a.den = beta == 1.0 ? nullptr : reduced + CR; a.nchunks = 1; a.chunk_stride = 0;
-  a.ldp = ctx->R; a.kl_den = beta == 1.0 ? reduced + CR : nullptr; a.out_scale = nullptr;
-  a.gamma = (float)gamma; a.l1 = (float)l1_reg; a.l2 = (float)l2_reg; a.absmax_bits = nullptr;
-  int rc = apply_update(a, st);
+  int rc = apply_update(nmf_apply_args(ctx, 0, W, beta, reduced, reduced + ctx->C * ctx->R, 1, 0, gamma, l1_reg, l2_reg), st);
   if (rc) return rc;
   if (ctx->tc) tc_mark_dirty(ctx->tc, true, false);
   return 0;
@@ -608,7 +583,7 @@ int nmfb200_nmf_contract_only(nmfb200_ctx* ctx, const float* W, const float* H, 
   if (!W || !H) return fail(NMFB200_ERR_INVALID, "null factor pointer");
   cudaStream_t st = (cudaStream_t)stream;
   if (use_tc(ctx, beta)) return tc_contract_only(ctx->tc, W, H, which, beta, st);
-  return which == 0 ? simt_contract_w(ctx, W, H, beta, st) : simt_contract_h(ctx, W, H, beta, st);
+  return simt_contract(ctx, which, W, H, beta, st);
 }
 
 /* ---- NMFD ------------------------------------------------------------------------------------ */

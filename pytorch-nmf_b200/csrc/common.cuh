@@ -21,8 +21,7 @@ inline BetaMode beta_mode(double beta) {
 }
 
 void set_error(const std::string& msg);
-void count_launch(int n = 1);
-int64_t launch_counter();
+void count_launch();
 
 #define NMF_CUDA_CHECK(expr)                                                              \
   do {                                                                                    \

@@ -20,7 +20,6 @@
 #include <cuda.h>
 #include <cudaTypedefs.h>
 
-#include <cstdlib>
 #include <cstring>
 #include <string>
 #include <vector>
@@ -404,7 +403,7 @@ __device__ __forceinline__ void publish_beta_exps(int* __restrict__ exps, float 
 // ratio has to exceed 5e5 kappa before the saturating pack clips it), and the exponents of the beta != 1 tiles.
 __device__ __forceinline__ void publish_scales(int a, int which, int* __restrict__ exps, unsigned int* __restrict__ absmax_next,
                                                float dot, const double* __restrict__ vconst, float* __restrict__ kappa,
-                                               int center, float bm1, float bm2, double cells) {
+                                               float bm1, float bm2, double cells) {
   exps[1 + which] = a;
   *absmax_next = 0u;
   const float ptyp = (float)(vconst[0] / (double)dot);
@@ -412,7 +411,7 @@ __device__ __forceinline__ void publish_scales(int a, int which, int* __restrict
   const bool ok = ptyp > 0.f && isfinite(ptyp);
   if (ok) { frexpf(ptyp, &e); e = -3 - e; }     // ptyp * 2^e in [2^-4, 2^-3)
   exps[3] = e;
-  kappa[0] = (ok && center) ? ptyp : 0.f;
+  kappa[0] = ok ? ptyp : 0.f;
   kappa[1] = dot;
   publish_beta_exps(exps, dot, vconst, bm1, bm2, cells);
 }
@@ -548,72 +547,6 @@ tc_apply_kernel(TcApplyArgs a) {
   sh[rg][r] = cs;
   __syncthreads();
   if (threadIdx.x < 128) a.cs_part[(int64_t)blockIdx.x * 128 + r] = sh[0][r] + sh[1][r];
-  for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-  if ((threadIdx.x & 31) == 0 && mx > 0.f) atomicMax(a.absmax, __float_as_uint(mx));
-}
-
-// Vectorised variant for R % 4 == 0: one thread owns 4 consecutive rank lanes (float4) of a row; a 256-thread block
-// covers 256 / (R/4) rows per pass.  Same outputs as tc_apply_kernel.
-__global__ void __launch_bounds__(256)
-tc_apply_vec4_kernel(TcApplyArgs a) {
-  __shared__ float4 sh[256];
-  const int lanes = a.R >> 2;                    // threads per row
-  const int rows_per_pass = 256 / lanes;
-  const int rl = threadIdx.x / lanes, q = threadIdx.x - rl * lanes;      // row slot, rank quad
-  const int64_t row0 = (int64_t)blockIdx.x * a.rpb;
-  const int64_t row1 = min(a.rows, row0 + a.rpb);
-  float4 cs = make_float4(0.f, 0.f, 0.f, 0.f);
-  float mx = 0.f;
-  if (rl < rows_per_pass) {
-    float4 kd = make_float4(1.f, 1.f, 1.f, 1.f);
-    float kap = 0.f;
-    if (a.apply && !a.den) { kd = *reinterpret_cast<const float4*>(a.kl_den + 4 * q); kap = *a.kappa; }
-    for (int64_t row = row0 + rl; row < row1; row += rows_per_pass) {
-      float4* pp = reinterpret_cast<float4*>(a.param + row * a.R) + q;
-      float4 v = *pp;
-      if (a.apply) {
-        float4 num = make_float4(0.f, 0.f, 0.f, 0.f);
-        for (int ch = 0; ch < a.nchunks; ++ch) {
-          const float4 t = *(reinterpret_cast<const float4*>(a.num + ch * a.chunk_stride + row * a.Rp) + q);
-          num.x += t.x; num.y += t.y; num.z += t.z; num.w += t.w;
-        }
-        float4 dsum = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (a.den) {
-          for (int ch = 0; ch < a.nchunks; ++ch) {
-            const float4 t = *(reinterpret_cast<const float4*>(a.den + ch * a.chunk_stride + row * a.Rp) + q);
-            dsum.x += t.x; dsum.y += t.y; dsum.z += t.z; dsum.w += t.w;
-          }
-        }
-        float vv[4] = {v.x, v.y, v.z, v.w}, nn[4] = {num.x, num.y, num.z, num.w}, dd[4] = {kd.x, kd.y, kd.z, kd.w};
-        const float ds[4] = {dsum.x, dsum.y, dsum.z, dsum.w};
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const float n = a.den ? nn[i] : fmaf(kap, dd[i], nn[i]);  // beta == 1: the kernel accumulated sum (P - kappa) G
-          const float neg = fmaxf(n, 0.f) + kEps;                   // nmf.py:78
-          float pos = a.den ? fmaxf(ds[i], 0.f) + kEps : dd[i];     // nmf.py:83 | nmf.py:368-369 / :381-382
-          if (a.l1 > 0.f) pos += a.l1;                              // nmf.py:85-86
-          if (a.l2 > 0.f) pos = fmaf(a.l2, vv[i], pos);             // nmf.py:87-88
-          float mult = neg / pos;                                   // nmf.py:89
-          if (a.gamma != 1.0f) mult = powf(mult, a.gamma);          // nmf.py:90-91
-          vv[i] *= mult;                                            // nmf.py:92
-        }
-        v = make_float4(vv[0], vv[1], vv[2], vv[3]);
-        *pp = v;
-      }
-      cs.x += v.x; cs.y += v.y; cs.z += v.z; cs.w += v.w;
-      mx = fmaxf(fmaxf(mx, fmaxf(v.x, v.y)), fmaxf(v.z, v.w));
-    }
-  }
-  sh[threadIdx.x] = cs;
-  __syncthreads();
-  if (threadIdx.x < lanes) {
-    float4 t = make_float4(0.f, 0.f, 0.f, 0.f);
-    for (int k = 0; k < rows_per_pass; ++k) {
-      const float4 u = sh[k * lanes + threadIdx.x];
-      t.x += u.x; t.y += u.y; t.z += u.z; t.w += u.w;
-    }
-    *(reinterpret_cast<float4*>(a.cs_part + (int64_t)blockIdx.x * 128) + threadIdx.x) = t;
-  }
   for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
   if ((threadIdx.x & 31) == 0 && mx > 0.f) atomicMax(a.absmax, __float_as_uint(mx));
 }
@@ -842,7 +775,7 @@ tc_finish_kernel(const float* __restrict__ x, int64_t rows, int R, __half* __res
                  const unsigned int* __restrict__ absmax, unsigned int* __restrict__ absmax_next,
                  int* __restrict__ exps, int which, const float* __restrict__ cs_part, int cs_blocks,
                  float* __restrict__ colsum /* [2][R] */, const double* __restrict__ vconst,
-                 float* __restrict__ kappa, int center, float* __restrict__ cs_super, unsigned int* __restrict__ ticket,
+                 float* __restrict__ kappa, float* __restrict__ cs_super, unsigned int* __restrict__ ticket,
                  float bm1, float bm2, double cells) {
   const int a = pow2_exp_for(__uint_as_float(*absmax));
   const float sc = exp2f((float)a);
@@ -921,22 +854,23 @@ tc_finish_kernel(const float* __restrict__ x, int64_t rows, int R, __half* __res
         *ticket = 0u;
         float dot = 0.f;
         for (int k = 0; k < 128; ++k) dot += prod[k];
-        publish_scales(a, which, exps, absmax_next, dot, vconst, kappa, center, bm1, bm2, cells);
+        publish_scales(a, which, exps, absmax_next, dot, vconst, kappa, bm1, bm2, cells);
       }
     }
   }
 }
 
 // ---- ratio stage + operand refresh in ONE cooperative kernel (R % 4 == 0; beta != 2) ------------------------------------
-// Phase 1 = tc_apply_vec4_kernel (nmf.py:78-92 in place, per-block column sums, global max); grid barrier; phase 2 = the
-// fp16 operand copy with the exponent from that max (rows re-read from L2), while block 0 folds the column sums in fixed
-// order and publishes colsum / kappa / exponents.  Replaces two launches, one pass over the factor and the ticket
-// protocol of tc_finish_kernel; the W side also gets 2 x #SM blocks instead of rows / 64.
+// Phase 1 = the ratio stage with one thread per 4 consecutive rank lanes (float4) of a row (nmf.py:78-92 in place,
+// per-block column sums, global max); grid barrier; phase 2 = the fp16 operand copy with the exponent from that max (rows
+// re-read from L2), while block 0 folds the column sums in fixed order and publishes colsum / kappa / exponents.  Replaces
+// two launches, one pass over the factor and the ticket protocol of tc_finish_kernel; the W side also gets 2 x #SM blocks
+// instead of rows / 64.
 struct TcFinishArgs {
   __half* out; int KW, Rp;
   unsigned int* absmax; unsigned int* absmax_next;
   int* exps; int which;
-  float* colsum; const double* vconst; float* kappa; int center;
+  float* colsum; const double* vconst; float* kappa;
   float bm1, bm2; double cells;
 };
 
@@ -1111,7 +1045,7 @@ tc_apply_finish_kernel(TcApplyArgs a, TcFinishArgs f) {
     if (threadIdx.x == 0) {
       float dot = 0.f;
       for (int k = 0; k < 128; ++k) dot += prod[k];
-      publish_scales(ae, f.which, f.exps, f.absmax_next, dot, f.vconst, f.kappa, f.center, f.bm1, f.bm2, f.cells);
+      publish_scales(ae, f.which, f.exps, f.absmax_next, dot, f.vconst, f.kappa, f.bm1, f.bm2, f.cells);
     }
   }
 }
@@ -1343,34 +1277,16 @@ struct TcState {
   CUtensorMap tmWg, tmHg;           // factors as the column factor G: box 64 x TN
   Plan plan_w, plan_h;
   uint32_t upd[2] = {0, 0};         // per-factor update counter (selects the absmax slot)
-  // one MU iteration (W update + H update) captured as a CUDA graph, per absmax-slot parity pair
-  cudaGraphExec_t gexec[4] = {nullptr, nullptr, nullptr, nullptr};
-  int gkernels = 0;                 // kernels per captured iteration (for the launch counter)
-  const float* gW = nullptr; const float* gH = nullptr;
-  double gargs[4] = {0, 0, 0, 0};   // beta, gamma, l1, l2 the graphs were captured with
-  bool gwarm = false;               // one eager iteration has run with these arguments
-  cudaStream_t gstream = nullptr;   // capture / replay stream (the caller's may be the legacy default stream, which cannot capture)
-  cudaEvent_t gev_in = nullptr, gev_out = nullptr;
   bool dirty_w = true, dirty_h = true, has_target = false;
-  // Environment knobs, read once in tc_create: NMFB200_CENTER=0 (diagnostic: kappa centring off), NMFB200_GRAPH=1
-  // (CUDA-graph replay of tc_iterate), NMFB200_TC_CHECK=1 (watchdog check after every tc_contract_only).
-  int center = 1;
-  bool use_graph = false, check_each = false;
   float* kappa = nullptr;           // device [2]: kappa, <colsum W, colsum H> it was derived from
   double exps_beta = 1.0;           // the beta exps[4] / exps[5] were last published for
   float* zero = nullptr;           // device scalar 0 (kappa of an already complete numerator)
   int coop_blocks = 0;              // co-resident blocks of the fused tail kernel (cooperative launch), 0 = unavailable
-  bool fused_tail = false;          // ratio stage + operand refresh in one cooperative kernel (NMFB200_FUSED_TAIL=0: two kernels)
 };
 
 bool tc_shape_supported(int64_t N, int64_t C, int64_t R) {
   // the conversion kernel walks 64-row slabs on gridDim.y (<= 65535): taller targets take the fp32 kernels
   return R >= 1 && R <= 128 && N >= 1 && C >= 1 && N <= 65535ll * 64 && C < (1ll << 31);
-}
-
-static void drop_graphs(TcState* s) {
-  for (auto& g : s->gexec) { if (g) cudaGraphExecDestroy(g); g = nullptr; }
-  s->gwarm = false;
 }
 
 void tc_peer_release(TcState* s) {
@@ -1386,10 +1302,6 @@ void tc_peer_release(TcState* s) {
 void tc_destroy(TcState* s) {
   if (!s) return;      // the caller (capi.cu: free_ctx) has selected s->device
   tc_peer_release(s);
-  drop_graphs(s);
-  if (s->gstream) cudaStreamDestroy(s->gstream);
-  if (s->gev_in) cudaEventDestroy(s->gev_in);
-  if (s->gev_out) cudaEventDestroy(s->gev_out);
   cudaFree(s->V16); cudaFree(s->Vt16); cudaFree(s->W16); cudaFree(s->H16); cudaFree(s->part); cudaFree(s->part2); cudaFree(s->gram); cudaFree(s->gram_part);
   cudaFree(s->colsum); cudaFree(s->cs_part); cudaFree(s->cs_super); cudaFree(s->ticket); cudaFree(s->absmax); cudaFree(s->exps);
   cudaFree(s->vpart); cudaFree(s->vconst); cudaFree(s->vlossy); cudaFree(s->loss_part); cudaFree(s->vbeta); cudaFree(s->vbeta_part); cudaFree(s->kappa); cudaFree(s->zero);
@@ -1403,9 +1315,6 @@ int tc_create(TcState** out, int device, int64_t N, int64_t C, int64_t R, bool s
   s->Rp = R <= 64 ? 64 : 128;
   s->KW = split ? 2 * s->Rp : s->Rp;
   s->TN = (split && s->Rp == 128) ? 64 : 128;   // 64-column tiles where two 128-column stages do not fit next to the F block
-  if (const char* e = getenv("NMFB200_CENTER")) s->center = atoi(e);
-  s->use_graph = getenv("NMFB200_GRAPH") != nullptr;
-  s->check_each = getenv("NMFB200_TC_CHECK") != nullptr;
   s->ldc = round_up(C, 8);
   s->ldn = round_up(N, 8);
   cudaDeviceProp prop;
@@ -1421,8 +1330,6 @@ int tc_create(TcState** out, int device, int64_t N, int64_t C, int64_t R, bool s
       s->coop_blocks = per_sm * s->num_sms;
       if (s->coop_blocks > 1024) s->coop_blocks = 1024;      // cs_part capacity
     }
-    const char* e = getenv("NMFB200_FUSED_TAIL");
-    s->fused_tail = s->coop_blocks > 0 && !(e && atoi(e) == 0);
   }
   s->plan_w = make_plan(C, N, s->num_sms, s->TN);
   s->plan_h = make_plan(N, C, s->num_sms, s->TN);
@@ -1481,7 +1388,6 @@ bool tc_supports_beta(const TcState* s, double beta) {
   // other beta: two-output kernel (rank <= 64)
   return s->Rp == 64 && s->TN == 128;
 }
-bool tc_supports_loss(const TcState* s, double beta) { return tc_supports_beta(s, beta); }
 bool tc_supports_partial(const TcState* s, double beta) { return beta != 2.0 && tc_supports_beta(s, beta); }
 
 int tc_set_target(TcState* s, const float* V, int64_t ldv, const float* minmax_dev, cudaStream_t st) {
@@ -1497,7 +1403,6 @@ int tc_set_target(TcState* s, const float* V, int64_t ldv, const float* minmax_d
   NMF_LAUNCH_CHECK();
   s->has_target = true;
   s->Vsrc = V; s->ldv = ldv; s->vbeta_for = 1.0;
-  drop_graphs(s);
   s->dirty_w = s->dirty_h = true;      // exps[3] depends on sum(V)
   return 0;
 }
@@ -1548,7 +1453,7 @@ int apply_and_finish(TcState* s, int which, float* param, bool apply, const Plan
   a.gamma = (float)gamma; a.l1 = (float)l1; a.l2 = (float)l2;
   a.cs_part = s->cs_part; a.absmax = slot; a.apply = apply ? 1 : 0; a.kappa = reduced ? s->zero : s->kappa;
   if (peer) {
-    if (!((s->R & 3) == 0 && s->fused_tail)) { set_error("internal: peer W update needs the fused ratio-stage kernel"); return 1; }
+    if (!((s->R & 3) == 0 && s->coop_blocks > 0)) { set_error("internal: peer W update needs the fused ratio-stage kernel"); return 1; }
     // the ranks' slots of THIS rank's block for this iteration's parity (every rank pushed its packed partial into them)
     for (int p = 0; p < s->peer_world; ++p)
       a.peers[p] = reinterpret_cast<const float*>(s->peer_block) + 64 +
@@ -1557,7 +1462,7 @@ int apply_and_finish(TcState* s, int which, float* param, bool apply, const Plan
     a.flag_target = s->peer_iter; a.peer_err = s->peer_err;
   }
   s->exps_beta = beta;                 // both branches below end in publish_scales at this beta
-  if ((s->R & 3) == 0 && !(apply && beta == 2.0 && !reduced) && s->fused_tail) {
+  if ((s->R & 3) == 0 && s->coop_blocks > 0 && !(apply && beta == 2.0 && !reduced)) {
     // one cooperative launch: ratio stage, grid barrier, operand copy + scalars
     const int lanes = (int)s->R >> 2, rows_per_pass = 256 / lanes;
     int64_t g = ceil_div(rows, rows_per_pass);
@@ -1567,7 +1472,7 @@ int apply_and_finish(TcState* s, int which, float* param, bool apply, const Plan
     TcFinishArgs f{};
     f.out = which == 0 ? s->W16 : s->H16; f.KW = s->KW; f.Rp = s->Rp; f.absmax = slot; f.absmax_next = next;
     f.exps = s->exps; f.which = which; f.colsum = s->colsum; f.vconst = s->vconst; f.kappa = s->kappa;
-    f.center = s->center; f.bm1 = (float)(beta - 1.0); f.bm2 = (float)(beta - 2.0);
+    f.bm1 = (float)(beta - 1.0); f.bm2 = (float)(beta - 2.0);
     f.cells = (double)s->N * (double)s->C;
     void* args[2] = {&a, &f};
     const void* fn = s->split ? (const void*)tc_apply_finish_kernel<true> : (const void*)tc_apply_finish_kernel<false>;
@@ -1604,8 +1509,6 @@ int apply_and_finish(TcState* s, int which, float* param, bool apply, const Plan
       }
       tc_apply_eu_kernel<8><<<blocks, 256, eu_smem, st>>>(a, s->gram);
     }
-  } else if ((s->R & 3) == 0) {
-    tc_apply_vec4_kernel<<<blocks, 256, 0, st>>>(a);
   } else {
     tc_apply_kernel<<<blocks, 256, 0, st>>>(a);
   }
@@ -1614,11 +1517,11 @@ int apply_and_finish(TcState* s, int which, float* param, bool apply, const Plan
   const unsigned grid = (unsigned)ceil_div((s->R & 7) == 0 ? rows * (s->R >> 3) : rows * s->R, 256);
   if (s->split)
     tc_finish_kernel<true><<<grid, 256, 0, st>>>(param, rows, (int)s->R, out, s->KW, s->Rp, slot, next, s->exps, which,
-                                                 s->cs_part, blocks, s->colsum, s->vconst, s->kappa, s->center, s->cs_super, s->ticket,
+                                                 s->cs_part, blocks, s->colsum, s->vconst, s->kappa, s->cs_super, s->ticket,
                                                  (float)(beta - 1.0), (float)(beta - 2.0), (double)s->N * (double)s->C);
   else
     tc_finish_kernel<false><<<grid, 256, 0, st>>>(param, rows, (int)s->R, out, s->KW, s->Rp, slot, next, s->exps, which,
-                                                  s->cs_part, blocks, s->colsum, s->vconst, s->kappa, s->center, s->cs_super, s->ticket,
+                                                  s->cs_part, blocks, s->colsum, s->vconst, s->kappa, s->cs_super, s->ticket,
                                                  (float)(beta - 1.0), (float)(beta - 2.0), (double)s->N * (double)s->C);
   NMF_LAUNCH_CHECK();
   return 0;
@@ -1626,7 +1529,6 @@ int apply_and_finish(TcState* s, int which, float* param, bool apply, const Plan
 
 int ensure_synced(TcState* s, const float* W, const float* H, double beta, cudaStream_t st) {
   if (!s->has_target) { set_error("tensor-core path: set_target has not been called"); return 3; }
-  const bool both = s->dirty_w && s->dirty_h;
   if (s->dirty_w) {
     int rc = apply_and_finish(s, 0, const_cast<float*>(W), false, nullptr, beta, 1, 0, 0, st);
     if (rc) return rc;
@@ -1637,7 +1539,6 @@ int ensure_synced(TcState* s, const float* W, const float* H, double beta, cudaS
     if (rc) return rc;
     s->dirty_h = false;
   }
-  (void)both;   // the second refresh recomputes exps[3] with both column sums valid
   return 0;
 }
 
@@ -1722,7 +1623,6 @@ int launch_contract_two(TcState* s, int which, double beta, cudaStream_t st) {
 
 // The update kernels of beta != 1 scale their tiles by exps[4] / exps[5], which the last refresh published for ITS beta (an
 // update of W at beta 1 followed by one of H at beta 2 is legal): republish them for this beta from the stored dot product.
-// A stream launch, so it is captured with the rest of an iteration.
 int sync_beta_exps(TcState* s, double beta, cudaStream_t st) {
   if (beta == 1.0 || s->exps_beta == beta) return 0;
   republish_beta_kernel<<<1, 32, 0, st>>>(s->exps, s->kappa, s->vconst, (float)(beta - 1.0), (float)(beta - 2.0),
@@ -1741,92 +1641,19 @@ int launch_contract(TcState* s, int which, double beta, cudaStream_t st) {
 
 }  // namespace
 
-int tc_update_w(TcState* s, float* W, const float* H, double beta, double gamma, double l1, double l2,
-                cudaStream_t st) {
-  // tc_loss_prefetch_w already ran this contraction on these very factors (its numerators are still in `part`)
-  const bool reuse = s->w_pending && !s->dirty_w && !s->dirty_h && beta == 1.0;
+int tc_update(TcState* s, int which, float* param, const float* W, const float* H, double beta, double gamma, double l1,
+              double l2, cudaStream_t st) {
+  // tc_loss_prefetch_w already ran the W contraction on these very factors (its numerators are still in `part`)
+  const bool reuse = which == 0 && s->w_pending && !s->dirty_w && !s->dirty_h && beta == 1.0;
   s->w_pending = false;
   int rc = ensure_synced(s, W, H, beta, st);
   if (rc) return rc;
   if (!reuse) {
-    rc = launch_contract(s, 0, beta, st);
+    rc = launch_contract(s, which, beta, st);
     if (rc) return rc;
   }
-  return apply_and_finish(s, 0, W, true, &s->plan_w, beta, gamma, l1, l2, st, nullptr, H);
-}
-
-int tc_update_h(TcState* s, const float* W, float* H, double beta, double gamma, double l1, double l2,
-                cudaStream_t st) {
-  int rc = ensure_synced(s, W, H, beta, st);
-  if (rc) return rc;
-  rc = launch_contract(s, 1, beta, st);
-  if (rc) return rc;
-  return apply_and_finish(s, 1, H, true, &s->plan_h, beta, gamma, l1, l2, st, nullptr, W);
-}
-
-int tc_iterate(TcState* s, float* W, float* H, double beta, double gamma, double l1, double l2, int n_iter,
-               cudaStream_t st) {
-  if (n_iter <= 0) return 0;
-  if (s->gW != W || s->gH != H || s->gargs[0] != beta || s->gargs[1] != gamma || s->gargs[2] != l1 || s->gargs[3] != l2) {
-    drop_graphs(s);
-    s->gW = W; s->gH = H; s->gargs[0] = beta; s->gargs[1] = gamma; s->gargs[2] = l1; s->gargs[3] = l2;
-  }
-  // CUDA-graph replay of the iteration is opt-in (NMFB200_GRAPH=1): measured no gain at cfg2 -- the stream is never
-  // launch-bound -- so the default keeps plain stream-ordered launches.
-  const bool use_graph = s->use_graph;
-  cudaStream_t user = st;
-  if (use_graph) {
-    // run on an engine-owned stream, fenced against the caller's stream with events
-    if (!s->gstream) {
-      NMF_CUDA_CHECK(cudaStreamCreateWithFlags(&s->gstream, cudaStreamNonBlocking));
-      NMF_CUDA_CHECK(cudaEventCreateWithFlags(&s->gev_in, cudaEventDisableTiming));
-      NMF_CUDA_CHECK(cudaEventCreateWithFlags(&s->gev_out, cudaEventDisableTiming));
-    }
-    NMF_CUDA_CHECK(cudaEventRecord(s->gev_in, user));
-    NMF_CUDA_CHECK(cudaStreamWaitEvent(s->gstream, s->gev_in, 0));
-    st = s->gstream;
-  }
-  int rc = ensure_synced(s, W, H, beta, st);        // graphs assume clean operand copies
-  if (rc) return rc;
-  if (beta != 1.0 && !s->part2) NMF_CUDA_CHECK(cudaMalloc(&s->part2, (size_t)s->part_floats * 4));
-  for (int i = 0; i < n_iter; ++i) {
-    const int key = (int)((s->upd[0] & 1u) * 2u + (s->upd[1] & 1u));
-    if (use_graph && s->gwarm && s->gexec[key]) {
-      s->w_pending = false;                          // the replayed iteration runs its own W contraction
-      rc = sync_beta_exps(s, beta, st);              // a call between two replays may have published another beta
-      if (rc) return rc;
-      NMF_CUDA_CHECK(cudaGraphLaunch(s->gexec[key], st));
-      s->upd[0]++; s->upd[1]++;
-      count_launch(s->gkernels);
-      continue;
-    }
-    const bool capture = use_graph && s->gwarm;      // the first iteration runs eagerly (lazy module loads, attributes)
-    cudaGraph_t graph = nullptr;
-    const int64_t before = launch_counter();
-    if (capture) NMF_CUDA_CHECK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-    rc = tc_update_w(s, W, H, beta, gamma, l1, l2, st);
-    if (rc == 0) rc = tc_update_h(s, W, H, beta, gamma, l1, l2, st);
-    if (capture) {
-      cudaError_t e = cudaStreamEndCapture(st, &graph);
-      if (rc == 0 && e != cudaSuccess) { set_error(std::string("cudaStreamEndCapture: ") + cudaGetErrorString(e)); rc = 2; }
-      if (rc == 0) {
-        e = cudaGraphInstantiate(&s->gexec[key], graph, 0);
-        if (e != cudaSuccess) { set_error(std::string("cudaGraphInstantiate: ") + cudaGetErrorString(e)); rc = 2; }
-      }
-      if (graph) cudaGraphDestroy(graph);
-      if (rc) { drop_graphs(s); return rc; }
-      s->gkernels = (int)(launch_counter() - before);
-      NMF_CUDA_CHECK(cudaGraphLaunch(s->gexec[key], st));      // capture records, it does not execute
-    } else {
-      if (rc) return rc;
-      s->gwarm = true;
-    }
-  }
-  if (use_graph) {
-    NMF_CUDA_CHECK(cudaEventRecord(s->gev_out, s->gstream));
-    NMF_CUDA_CHECK(cudaStreamWaitEvent(user, s->gev_out, 0));
-  }
-  return 0;
+  return apply_and_finish(s, which, param, true, which == 0 ? &s->plan_w : &s->plan_h, beta, gamma, l1, l2, st, nullptr,
+                          which == 0 ? H : W);
 }
 
 // Raw update terms of one factor (which = 0: W, 1: H) in one dense buffer: numerator (rows x R; chunk sums, + kappa
@@ -1848,10 +1675,6 @@ int tc_raw_terms(TcState* s, int which, const float* W, const float* H, double b
   return 0;
 }
 
-int tc_w_partial(TcState* s, const float* W, const float* H, double beta, float* partial, cudaStream_t st) {
-  return tc_raw_terms(s, 0, W, H, beta, partial, st);
-}
-
 // Sharded W update, second half: nmf.py:78-92 on the all-reduced buffer with the tensor-core path's own ratio-stage
 // kernels, which also rebuild W16 / colsum(W) / exponents (no separate resync pass).
 int tc_w_apply(TcState* s, float* W, const float* reduced, double beta, double gamma, double l1, double l2,
@@ -1869,7 +1692,7 @@ int tc_w_apply(TcState* s, float* W, const float* reduced, double beta, double g
 // between; slots alternate by iteration parity (a rank can be at most one W update ahead of the slowest: its next push needs
 // every rank's counter of the update in between, which that rank publishes after it has read the previous slots).
 bool tc_peer_supported(const TcState* s, double beta) {
-  return (s->R & 3) == 0 && s->fused_tail && tc_supports_partial(s, beta);
+  return (s->R & 3) == 0 && s->coop_blocks > 0 && tc_supports_partial(s, beta);
 }
 
 int tc_peer_alloc(TcState* s, void* handle_out) {
@@ -1971,11 +1794,7 @@ int tc_check_wait_abort(cudaStream_t st) {
 int tc_contract_only(TcState* s, const float* W, const float* H, int which, double beta, cudaStream_t st) {
   int rc = ensure_synced(s, W, H, beta, st);
   if (rc) return rc;
-  rc = launch_contract(s, which, beta, st);
-  if (rc == 0 && s->check_each) {
-    if (tc_check_wait_abort(st) > 0) { set_error("mbarrier wait aborted (protocol bug)"); return 2; }
-  }
-  return rc;
+  return launch_contract(s, which, beta, st);
 }
 
 bool tc_supports_loss_prefetch(const TcState* s, double beta) {
@@ -1983,7 +1802,7 @@ bool tc_supports_loss_prefetch(const TcState* s, double beta) {
 }
 
 // The loss at the current factors from the W update's own contraction (beta 1): one pass over V yields both the loss sums and
-// the partial numerators; the next tc_update_w on unchanged factors skips its contraction.
+// the partial numerators; the next W update (tc_update) on unchanged factors skips its contraction.
 int tc_loss_prefetch_w(TcState* s, const float* W, const float* H, double beta, double* loss_dev, cudaStream_t st) {
   if (!tc_supports_loss_prefetch(s, beta)) return tc_loss(s, W, H, beta, loss_dev, st);
   int rc = ensure_synced(s, W, H, beta, st);

@@ -1,4 +1,4 @@
-// Tensor-core (tcgen05 / TMEM / TMA) path of the dense NMF update -- interface used by capi.cu.
+// Tensor-core (wgmma / TMA) path of the dense NMF update -- interface used by capi.cu.
 #pragma once
 #include "common.cuh"
 
@@ -6,12 +6,11 @@ namespace nmfb200 {
 
 struct TcState;
 
-// shapes the tcgen05 kernels accept (rank padded to 64 or 128 columns)
+// shapes the wgmma kernels accept (rank padded to 64 or 128 columns)
 bool tc_shape_supported(int64_t N, int64_t C, int64_t R);
 int tc_create(TcState** out, int device, int64_t N, int64_t C, int64_t R, bool split);
 void tc_destroy(TcState* s);
 bool tc_supports_beta(const TcState* s, double beta);
-bool tc_supports_loss(const TcState* s, double beta);
 // row-sharded partials: beta 2 keeps the fp32 contraction (its numerator needs the Gram matrix of the global H)
 bool tc_supports_partial(const TcState* s, double beta);
 // minmax_dev: device float[2] = {min(V), max(V)} already queued on `st`
@@ -22,14 +21,10 @@ int tc_target_lossy(TcState* s, unsigned long long* count, cudaStream_t st);
 int tc_target_sum(TcState* s, double* vsum, cudaStream_t st);
 // the fp32 factor changed outside the tensor-core path: operand copies must be rebuilt before use
 void tc_mark_dirty(TcState* s, bool w, bool h);
-int tc_update_w(TcState* s, float* W, const float* H, double beta, double gamma, double l1, double l2,
-                cudaStream_t st);
-int tc_update_h(TcState* s, const float* W, float* H, double beta, double gamma, double l1, double l2,
-                cudaStream_t st);
-int tc_iterate(TcState* s, float* W, float* H, double beta, double gamma, double l1, double l2, int n_iter,
-               cudaStream_t st);
-int tc_w_partial(TcState* s, const float* W, const float* H, double beta, float* partial, cudaStream_t st);
-// the same for either factor (which = 0: W, 1: H): [numerator rows x R | colsum(other) R (beta 1) or denominator rows x R]
+// one factor update in place (which = 0: param = W, 1: param = H)
+int tc_update(TcState* s, int which, float* param, const float* W, const float* H, double beta, double gamma, double l1,
+              double l2, cudaStream_t st);
+// raw terms of either factor's update (which = 0: W, 1: H): [numerator rows x R | colsum(other) R (beta 1) or denominator rows x R]
 int tc_raw_terms(TcState* s, int which, const float* W, const float* H, double beta, float* out, cudaStream_t st);
 int tc_w_apply(TcState* s, float* W, const float* reduced, double beta, double gamma, double l1, double l2,
                cudaStream_t st);
@@ -48,7 +43,7 @@ int tc_contract_only(TcState* s, const float* W, const float* H, int which, doub
 // debugging / health: report (and clear) a recorded mbarrier wait abort; synchronises the stream
 int tc_check_wait_abort(cudaStream_t st);
 int tc_loss(TcState* s, const float* W, const float* H, double beta, double* loss_dev, cudaStream_t st);
-// the same value out of the W update's own contraction pass (beta 1, non-split); the next tc_update_w on unchanged factors
+// the same value out of the W update's own contraction pass (beta 1, non-split); the next W update on unchanged factors
 // reuses the partial numerators.  Falls back to tc_loss where the fold is not built.
 int tc_loss_prefetch_w(TcState* s, const float* W, const float* H, double beta, double* loss_dev, cudaStream_t st);
 

@@ -84,15 +84,10 @@ def load():
             f"{LIB_PATH} not found: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
             "(needs nvcc). torchnmf_b200 has no CPU fallback.")
     lib = ctypes.CDLL(LIB_PATH)
-    compat = bool(os.environ.get("NMFB200_LIB")) and bool(os.environ.get("NMFB200_LIB_COMPAT"))
     for name, (res, args) in SIGNATURES.items():
-        if compat and not hasattr(lib, name):       # A/B timing against an older build: newer symbols absent
-            continue
         fn = getattr(lib, name)          # AttributeError here == ABI mismatch
         fn.restype = res
         fn.argtypes = args
-    if compat and not hasattr(lib, "nmfb200_ctx_check_health"):
-        lib.nmfb200_ctx_check_health = lambda ctx, stream: lib.nmfb200_check_health(stream)
     if lib.nmfb200_abi_version() != 1:
         raise NmfB200Error("libnmf_b200.so ABI version mismatch")
     _lib = lib

@@ -2,8 +2,8 @@
 
 TEST INFRASTRUCTURE ONLY.  `fit()`, `BetaMu.step`, PLCA and the sharded fit keep a context alive for hundreds of calls, and
 the workspace cache hands contexts from one fit to the next, so every call after the first runs on state left behind by
-earlier ones: the fp16 operand copies and their exponents, kappa, the dirty flags, the prefetched W numerators, captured
-graphs, the cached V-only loss term, the AUTO mode's tensor-core switch.  A harness run drives one context through a
+earlier ones: the fp16 operand copies and their exponents, kappa, the dirty flags, the prefetched W numerators, the cached
+V-only loss term, the AUTO mode's tensor-core switch.  A harness run drives one context through a
 sequence of steps; before every step it reads the factors back, and it checks that step's output against a float64
 evaluation of that one step FROM THOSE FACTORS.  Errors do not build up, so the per-call bars of the term tests apply
 unchanged (tests/tc_model.py, tests/f32_cases.py).
@@ -12,7 +12,7 @@ A step is a tuple (op, *args):
     ("update_w" | "update_h", beta, gamma, l1, l2)     one factor update
     ("raw", which, beta)                              the raw terms of one update (`raw_terms`)
     ("loss", beta) / ("prefetch", beta)               the loss pass / the loss folded into the next W update's contraction
-    ("iterate", beta, gamma, l1, l2)                  iterate(1): one W and one H update in one call (graph replay if on)
+    ("iterate", beta, gamma, l1, l2)                  iterate(1): one W and one H update in one call
     ("rescale", f)                                    W *= f and H /= f in place (W H unchanged), then sync()
     ("shard", beta, gamma, l1, l2)                    w_partial, that buffer as the "all-reduced" sum into w_apply
     ("target", name)                                  set_target of another target of the sequence on the same context
@@ -28,7 +28,7 @@ import torch
 
 TRANSITIONS = [
     "prefetch reused", "prefetch dropped", "dirty from the fp32 path", "beta change without refresh",
-    "graph captured", "graph replayed", "graph dropped", "tc_off flipped", "sparse to dense",
+    "tc_off flipped", "sparse to dense",
     "NMFD refresh after an fp32 update",
 ]
 SCALES = [-16, -12, 0, 12, 20]
@@ -42,7 +42,6 @@ class Seq:
     precision: str
     steps: list
     targets: dict = field(default_factory=dict)      # name -> (scale exponent, heavy-tailed)
-    graph: bool = False           # NMFB200_GRAPH=1 when the context is created
     tc: bool = True               # runs on the tensor cores at all (the scale sweep applies)
 
 
@@ -58,7 +57,7 @@ FIT_STEPS = [
     UW(1), UH(1), ("loss", 1), ("prefetch", 1), UW(1),                 # prefetch reused
     ("prefetch", 1), UH(1), UW(1),                                     # dropped: the H contraction overwrote it
     ("raw", 0, 1), ("raw", 1, 1), ("prefetch", 1), ("raw", 0, 1), UW(1),
-    # graphs (fit-graph): eager, capture of both absmax parities, replay; a new gamma drops them all
+    # iterations across both absmax parities, then with a new gamma and new l1
     ("iterate", 1, 1.0, 0.0, 0.0), ("iterate", 1, 1.0, 0.0, 0.0), ("iterate", 1, 1.0, 0.0, 0.0), ("iterate", 1, 1.0, 0.0, 0.0),
     ("iterate", 1, G8, 0.0, 0.0), ("iterate", 1, G8, 0.0, 0.0), ("iterate", 1, G8, 0.0, 0.0), ("iterate", 1, G8, 0.0, 0.0),
     ("iterate", 1, G8, 1e-3, 0.0), ("iterate", 1, G8, 1e-3, 0.0),
@@ -104,7 +103,6 @@ def sequences():
     return [
         Seq("fit-f16", "nmf", (300, 260, 40), "f16", FIT_STEPS),
         Seq("fit-split", "nmf", (300, 260, 40), "f16_split", FIT_STEPS),
-        Seq("fit-graph", "nmf", (300, 260, 40), "f16", FIT_STEPS, graph=True),
         Seq("mixed-f16", "nmf", (300, 260, 40), "f16", MIXED_STEPS),
         Seq("mixed-split", "nmf", (300, 260, 40), "f16_split", MIXED_STEPS),
         Seq("paths-r100", "nmf", (300, 260, 100), "f16", PATH_STEPS),
@@ -150,8 +148,6 @@ def simulate(seq):
     w_pending = False
     dirty = {"w": True, "h": True}
     exps_beta = None
-    gkey, gwarm, gcapt = None, False, set()
-    upd = [0, 0]
     nmfd_fp32_since_tc = False
     out = []
 
@@ -204,7 +200,6 @@ def simulate(seq):
                 ev.append("tc_off flipped")
             tc_off = new_off
             dirty["w"] = dirty["h"] = True
-            gkey, gwarm, gcapt = None, False, set()
         elif plan.path == "f32":
             writes = op in ("update_w", "update_h", "iterate") or (op == "raw" and seq.kind == "nmfd")
             if writes and has_tc and not tc_off and not sparse:
@@ -218,7 +213,6 @@ def simulate(seq):
             if op == "shard" and use_tc(beta):      # beta 2: w_apply's ratio stage republishes W at this beta
                 dirty["w"] = False
                 exps_beta = beta
-                upd[0] += 1
         elif op in ("update_w", "update_h"):
             if reuse:
                 plan.reuse = True
@@ -226,29 +220,13 @@ def simulate(seq):
             else:
                 contraction(beta, ev)
             exps_beta = beta
-            upd[0 if op == "update_w" else 1] += 1
         elif op == "iterate":
-            args = tuple(st[1:])
-            if gkey != args:
-                if gcapt:
-                    ev.append("graph dropped")
-                gkey, gwarm, gcapt = args, False, set()
             contraction(beta, ev)
-            key = (upd[0] % 2, upd[1] % 2)
-            if seq.graph and gwarm and key in gcapt:
-                ev.append("graph replayed")
-            elif seq.graph and gwarm:
-                ev.append("graph captured")
-                gcapt.add(key)
-            gwarm = True
             exps_beta = beta
-            upd[0] += 1
-            upd[1] += 1
         elif op == "shard":
             contraction(beta, ev)
             dirty["w"] = False
             exps_beta = beta
-            upd[0] += 1
         elif op == "raw" or seq.kind == "nmfd":
             contraction(beta, ev)
         else:                                       # the loss pass: refreshes what is dirty, reads no beta exponent

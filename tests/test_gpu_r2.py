@@ -154,6 +154,33 @@ def test_nmfd_tensor_core_ranks_above_128_match_oracle(R):
         assert err <= 1.0, f"R={R}: {err:.2f} x tolerance"
 
 
+@pytest.mark.parametrize("precision,R,beta", [(p, 40, b) for p in ("f16", "f16_split", "f32") for b in (1, 2, 0.5)]
+                         + [("f16", 13, 1)])
+def test_iterate_is_k_times_update_w_then_update_h(precision, R, beta):
+    """nmfb200_nmf_iterate(k) gives the bits of k x (update_w; update_h) on a second fresh context, on every path: the
+    tensor cores with the fused cooperative ratio stage (R % 4 == 0, beta != 2), with the two-launch one (R = 13, and the
+    beta 2 pair) and the fp32 kernels."""
+    from torchnmf_b200 import engine as _engine
+    k = 4                                   # both absmax parities of each factor
+    V, W0, H0 = _inputs((300, 260), (260, R), (300, R))
+    V = V.cuda()
+    _engine.release_workspaces()            # two new contexts, no state from earlier tests
+    a = _engine.CudaNmfEngine(V, W0.cuda(), H0.cuda(), precision)
+    b = _engine.CudaNmfEngine(V, W0.cuda(), H0.cuda(), precision)
+    try:
+        if precision != "f32":
+            assert a.precision_for(beta) != "f32", "the tensor-core path does not serve this case"
+        a.iterate(k, beta, 1.0, 0.0, 0.0)
+        for _ in range(k):
+            b.update_w(beta, 1.0, 0.0, 0.0)
+            b.update_h(beta, 1.0, 0.0, 0.0)
+        assert torch.equal(a.W, b.W) and torch.equal(a.H, b.H)
+    finally:
+        a.close()
+        b.close()
+        _engine.release_workspaces()
+
+
 # ---- the loss folded into the W update's contraction pass (nmfb200_nmf_loss_prefetch_w) -----------------------------------
 def _kl_engine(N, C, R):
     from torchnmf_b200 import engine as _engine

@@ -306,15 +306,6 @@ def _set_target_fn(seq, targets, chk):
     return set_target
 
 
-def _graph_launches(run_step):
-    """(output, number of cudaGraphLaunch calls) of one step, from a torch.profiler trace of the runtime API."""
-    from torch.profiler import ProfilerActivity, profile
-    with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
-        out = run_step()
-        torch.cuda.synchronize()
-    return out, sum(1 for ev in prof.events() if ev.name == "cudaGraphLaunch")
-
-
 def _check_launches(seq, plans, launches):
     """A W update at beta 1 on a valid prefetch launches one kernel fewer (its contraction) than one on clean operand copies
     without a prefetch; every other W update launches at least as many.  Both counts come from this context, whatever its
@@ -333,27 +324,18 @@ def _check_launches(seq, plans, launches):
             assert n >= plain[0], f"{seq.name}: a W update launched {n} kernels: it skipped its contraction"
 
 
-def _run(seq, scale=0, unbalanced=0, monkeypatch=None):
+def _run(seq, scale=0, unbalanced=0):
     targets, W, H = sc.fitted_data(seq, scale, unbalanced)
     chk = Checker(seq, scale)
     V = targets["V"].cuda()
     chk.V_dev = V
     chk.V = (V.to_dense() if V.is_sparse else V).double()
-    if seq.graph:
-        E.release_workspaces()                  # the graph switch is read when a context is created
-        monkeypatch.setenv("NMFB200_GRAPH", "1")
     eng = _make(seq, V, W.cuda(), H.cuda())
-    if seq.graph:
-        monkeypatch.delenv("NMFB200_GRAPH")
-    plans, launches, graph_calls = [], [], []
+    plans, launches = [], []
 
     def measure(plan, run_step):
         n0 = _capi.launch_count()
-        if seq.graph and plan.step[0] == "iterate":
-            out, g = _graph_launches(run_step)
-            graph_calls.append((plan, g))
-        else:
-            out = run_step()
+        out = run_step()
         launches.append(_capi.launch_count() - n0)
         plans.append(plan)
         return out
@@ -361,13 +343,7 @@ def _run(seq, scale=0, unbalanced=0, monkeypatch=None):
         eng, res = sc.run(seq, eng, chk, _set_target_fn(seq, targets, chk), measure)
     finally:
         eng.close()
-        if seq.graph:
-            E.release_workspaces()              # no later test may pick up a context with graph replay on
     _check_launches(seq, plans, launches)
-    # the graphs the host-side state machine expects: captured (and launched once) or replayed, else none at all
-    for plan, g in graph_calls:
-        want = 1 if ("graph captured" in plan.events or "graph replayed" in plan.events) else 0
-        assert g == want, f"{seq.name}: {plan.step} made {g} graph launches, expected {want} ({plan.events})"
     _report(seq=seq.name, scale=scale, unbalanced=unbalanced, steps=len(res), worst_err_over_bar=chk.worst)
     return res
 
@@ -377,18 +353,18 @@ TC_SEQS = [s for s in sc.sequences() if s.tc]
 
 @pytest.mark.parametrize("scale", sc.SCALES, ids=sc.scale_tag)
 @pytest.mark.parametrize("name", [s.name for s in TC_SEQS])
-def test_tensor_core_sequence(name, scale, monkeypatch):
-    _run(sc.by_name(name), scale, monkeypatch=monkeypatch)
+def test_tensor_core_sequence(name, scale):
+    _run(sc.by_name(name), scale)
 
 
 @pytest.mark.parametrize("name", ["fit-f16", "fit-split", "mixed-f16"])
-def test_unbalanced_factors(name, monkeypatch):
+def test_unbalanced_factors(name):
     """W 2^8 and H 2^-8: the operand exponents differ by 16, the product is unchanged."""
-    _run(sc.by_name(name), 0, unbalanced=8, monkeypatch=monkeypatch)
+    _run(sc.by_name(name), 0, unbalanced=8)
 
 
-def test_sparse_then_dense_on_one_context(monkeypatch):
-    _run(sc.by_name("sparse"), 0, monkeypatch=monkeypatch)
+def test_sparse_then_dense_on_one_context():
+    _run(sc.by_name("sparse"), 0)
 
 
 @pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs two GPUs in one process")
