@@ -38,7 +38,7 @@ extern "C" {
 /* arithmetic mode of the contraction kernels */
 enum {
   NMFB200_PREC_AUTO      = -1, /* f16 tensor-core path when the rank allows it (R <= 128), else f32 */
-  NMFB200_PREC_F32       = 0,  /* fused CUDA-core kernels, fp32 operands and accumulators (exact) */
+  NMFB200_PREC_F32       = 0,  /* fused CUDA-core kernels, fp32 operands and accumulators (exact), any rank */
   NMFB200_PREC_F16       = 1,  /* wgmma, fp16 operands, fp32 accumulate                           */
   NMFB200_PREC_F16_SPLIT = 2   /* wgmma, fp16 hi/lo split factors (~22-bit), fp16 ratio tile      */
 };
@@ -70,7 +70,9 @@ int nmfb200_ctx_check_health(nmfb200_ctx* ctx, void* stream);
 /* ---- dense NMF ------------------------------------------------------------------------- */
 
 /* Allocate the engine workspace for an (N,C) target of rank R on CUDA device `device`.
- * Mirrors the sizes fixed by NMF.__init__ (nmf.py:679-689). */
+ * Mirrors the sizes fixed by NMF.__init__ (nmf.py:679-689).  Any rank 1 <= R <= 65535 x 256 runs on the fp32 kernels
+ * (above 256 components in blocks of 256, each recomputing the reconstruction tile); the tensor-core precisions need
+ * R <= 128, and a sparse target (nmfb200_nmf_set_target_sparse) R <= 256. */
 int nmfb200_nmf_create(nmfb200_ctx** out, int device, int64_t N, int64_t C, int64_t R, int precision);
 void nmfb200_destroy(nmfb200_ctx* ctx);
 /* which NMFB200_PREC_* the context resolved to */
@@ -139,7 +141,8 @@ int nmfb200_nmf_w_apply(nmfb200_ctx* ctx, float* W, const float* reduced,
  * compressed forms -- CSR (crow[N+1], col[nnz], val[nnz]) and CSC = CSR of V^T (ccol[C+1], row[nnz], val_t[nnz]) -- int64
  * indices, fp32 values, device pointers borrowed until the next set_target*.  v_norm_kl / v_norm_eu: `_get_V_norm` nmf.py:161-170
  * for beta 1 / 2.  update_w / update_h / iterate / loss then evaluate the update terms at the non-zeros only (one warp per row
- * or column, fp32) and never form the dense product; any other beta returns NMFB200_ERR_INVALID (densify the target). */
+ * or column, fp32) and never form the dense product; any other beta returns NMFB200_ERR_INVALID (densify the target), as
+ * does a context of rank R > 256. */
 int nmfb200_nmf_set_target_sparse(nmfb200_ctx* ctx, int64_t nnz, const int64_t* crow, const int64_t* col, const float* val,
                                   const int64_t* ccol, const int64_t* row, const float* val_t,
                                   double v_norm_kl, double v_norm_eu, void* stream);
@@ -202,7 +205,8 @@ int nmfb200_nmfd_sync_factors(nmfb200_ctx* ctx);
  * NMFB200_NMF_PLAN_LEN values (n must be at least that):
  *   [0] chunks of the W update's contraction over the N rows    [1] chunks of the H update's over the C columns
  *   [2] 64-wide tiles per chunk, W update                       [3] the same, H update (the last chunks may be short or empty)
- *   [4] register blocks RB of the contraction (rank <= 16 RB)   [5] chunks of the loss pass   [6] its tiles per chunk
+ *   [4] register blocks RB of the contraction (rank <= 16 RB up to 256; above, 16 RB = 256 components per rank block,
+ *       ceil(R / 256) blocks on grid z)   [5] chunks of the loss pass   [6] its tiles per chunk
  *   [7] blocks of the column sum over N rows (the W update's KL denominator)   [8] over C rows (the H update's) */
 #define NMFB200_NMF_PLAN_LEN 9
 int nmfb200_nmf_plan(int64_t N, int64_t C, int64_t R, int64_t* out, int n);

@@ -84,8 +84,15 @@ struct DeviceGuard {
   DeviceGuard _dev_guard((ctx)->device);                                            \
   if (!_dev_guard.ok) return fail(NMFB200_ERR_CUDA, "cannot select the context's device");
 
-int chunks_for(int64_t rows, int64_t cols) {
-  int64_t rb = ceil_div(rows, 64), tiles = ceil_div(cols, 64);
+// Chunks of the contracted dimension of the fp32 contraction.  Above rank 256 the grid already holds one CTA per rank block
+// (simt_rank_blocks) for every row block and chunk: counting them keeps the nch x rows x R partial slabs from growing with
+// the blocks.
+// rank blocks of 256 components ride on grid z of the contraction and grid y of the column sum
+constexpr int64_t kMaxRank = kMaxGridYZ * 256;
+constexpr const char* kMaxRankMsg = "rank must be at most 65535 x 256 = 16776960";
+
+int chunks_for(int64_t rows, int64_t cols, int64_t R) {
+  int64_t rb = ceil_div(rows, 64) * simt_rank_blocks((int)R), tiles = ceil_div(cols, 64);
   int64_t want = ceil_div(132 * 4, rb);      // a few waves over the 132 SMs of an H100
   if (want > tiles) want = tiles;
   if (want > 32) want = 32;
@@ -178,7 +185,7 @@ int nmfb200_nmf_create(nmfb200_ctx** out, int device, int64_t N, int64_t C, int6
   if (!out) return fail(NMFB200_ERR_INVALID, "out is null");
   *out = nullptr;
   if (N < 1 || C < 1 || R < 1) return fail(NMFB200_ERR_INVALID, "N, C, R must be positive");
-  if (R > 256) return fail(NMFB200_ERR_INVALID, "rank > 256 is not supported");
+  if (R > kMaxRank) return fail(NMFB200_ERR_INVALID, kMaxRankMsg);
   if (precision < NMFB200_PREC_AUTO || precision > NMFB200_PREC_F16_SPLIT)
     return fail(NMFB200_ERR_INVALID, "unknown precision mode");
   DeviceGuard guard(device);
@@ -196,8 +203,8 @@ int nmfb200_nmf_create(nmfb200_ctx** out, int device, int64_t N, int64_t C, int6
   }
   c->precision = resolved;
   c->auto_mode = precision == NMFB200_PREC_AUTO;
-  c->nch_w = chunks_for(C, N);
-  c->nch_h = chunks_for(N, C);
+  c->nch_w = chunks_for(C, N, R);
+  c->nch_h = chunks_for(N, C, R);
   int64_t pf = (int64_t)c->nch_w * C * R;
   if ((int64_t)c->nch_h * N * R > pf) pf = (int64_t)c->nch_h * N * R;
   c->part_floats = pf;
@@ -240,8 +247,8 @@ int nmfb200_precision_for_beta(const nmfb200_ctx* ctx, double beta) {
 int nmfb200_nmf_plan(int64_t N, int64_t C, int64_t R, int64_t* out, int n) {
   if (!out || n < NMFB200_NMF_PLAN_LEN) return fail(NMFB200_ERR_INVALID, "plan buffer too small");
   if (N < 1 || C < 1 || R < 1) return fail(NMFB200_ERR_INVALID, "N, C, R must be positive");
-  if (R > 256) return fail(NMFB200_ERR_INVALID, "rank > 256 is not supported");
-  const int nch_w = chunks_for(C, N), nch_h = chunks_for(N, C);
+  if (R > kMaxRank) return fail(NMFB200_ERR_INVALID, kMaxRankMsg);
+  const int nch_w = chunks_for(C, N, R), nch_h = chunks_for(N, C, R);
   SimtNmfPlan pw, ph;
   simt_nmf_plan(C, N, (int)R, nch_w, &pw);          // W update: F = W (C rows), contracted over the N rows of V
   simt_nmf_plan(N, C, (int)R, nch_h, &ph);          // H update, and the loss (F = H)
@@ -255,7 +262,7 @@ int nmfb200_nmf_plan(int64_t N, int64_t C, int64_t R, int64_t* out, int n) {
 int nmfb200_nmf_sparse_plan(int64_t N, int64_t C, int64_t R, int64_t* out, int n) {
   if (!out || n < NMFB200_SPARSE_PLAN_LEN) return fail(NMFB200_ERR_INVALID, "plan buffer too small");
   if (N < 1 || C < 1 || R < 1) return fail(NMFB200_ERR_INVALID, "N, C, R must be positive");
-  if (R > 256) return fail(NMFB200_ERR_INVALID, "rank > 256 is not supported");
+  if (R > 256) return fail(NMFB200_ERR_INVALID, "rank > 256 is not supported by the sparse-target kernels (densify the target)");
   int64_t rpb_n, rpb_c;
   int nb_n, nb_c;
   sparse_gram_plan(N, &rpb_n, &nb_n);               // H^T H: the W update's beta-2 denominator, the beta-2 loss
@@ -315,6 +322,8 @@ int nmfb200_nmf_set_target_sparse(nmfb200_ctx* ctx, int64_t nnz, const int64_t* 
   (void)stream;
   if (nnz < 0 || !crow || !ccol || (nnz > 0 && (!col || !val || !row || !val_t)))
     return fail(NMFB200_ERR_INVALID, "bad compressed sparse target");
+  if (ctx->R > 256)
+    return fail(NMFB200_ERR_INVALID, "rank > 256 is not supported by the sparse-target kernels (densify the target)");
   if (!ctx->sp_gram) {
     const int64_t R = ctx->R;
     NMF_CUDA_CHECK(cudaMalloc(&ctx->sp_gram, (size_t)(2 * R * R + sparse_gram_part_floats((int)R)) * sizeof(float)));

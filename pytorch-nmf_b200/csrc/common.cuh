@@ -63,7 +63,7 @@ static inline bool grid_fits(const Grid3& g) {
 //   S = F G^T (Mr x Nc),  (Pn, Pp) = phi_beta(Vm, S)          [nmf.py:61-74]
 //   num[ch][m][r] = sum_{c in chunk ch} Pn[m,c] G[c,r]          [nmf.py:77]
 //   den[ch][m][r] = sum_{c in chunk ch} Pp[m,c] G[c,r]          [nmf.py:82, beta != 1 only]
-// Vm[m,c] = V[m*ldv + c] (trans = 0) or V[c*ldv + m] (trans = 1).
+// Vm[m,c] = V[m*ldv + c] (trans = 0) or V[c*ldv + m] (trans = 1).  Any rank R >= 1.
 int simt_nmf_contract(const float* V, int64_t ldv, int trans, const float* F, const float* G,
                       int64_t Mr, int64_t Nc, int R, double beta, int nchunks,
                       float* num, float* den, int64_t ldp, int64_t chunk_stride, cudaStream_t st);
@@ -72,6 +72,8 @@ int simt_nmf_loss(const float* V, int64_t ldv, const float* F, const float* G, i
                   int R, double beta, double* block_partials, int max_blocks, double* loss_dev,
                   cudaStream_t st);
 int simt_nmf_max_blocks(int64_t Mr, int64_t Nc);
+// Output blocks of 256 components of simt_nmf_contract (grid z): 1 up to rank 256, each block recomputes S over all ranks.
+int simt_rank_blocks(int R);
 // The tile plan of simt_nmf_contract (Mr rows, Nc contracted columns, `nchunks` chunks) and of simt_nmf_loss: the register
 // blocks RB of 16 components, the 64-column tiles per chunk (the last chunks may be short or empty) and the loss's chunks.
 struct SimtNmfPlan { int rb; int64_t tiles_per_chunk; int loss_chunks; int64_t loss_tiles_per_chunk; };

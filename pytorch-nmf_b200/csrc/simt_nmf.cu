@@ -6,6 +6,12 @@
 //   GEMM-2   num += Pn G_tile, den += Pp G_tile   (registers)                   nmf.py:77,82
 // so the (N x C) reconstruction and ratio matrices never exist in global memory.  The H update uses
 // (F,G,V) = (H,W,V); the W update uses (W,H,V^T) by reading V through a transposed tile load.
+//
+// Ranks above 256 (RB = 16, Rp = 256): S sums over rank chunks of 256 components staged one after another through the same
+// Fs / Gs buffers, and each CTA accumulates num / den for one output block of 256 components (blockIdx.z).  Its own chunk
+// runs last, so its G slice is still in Gs for GEMM-2.  S is recomputed once per output block: with nb = ceil(R / 256)
+// blocks the contraction does (nb + 1) / 2 (KL) or (nb + 2) / 3 (two outputs) times the minimal FLOPs.  With one block
+// (R <= 256) the kernel is the single-chunk kernel it always was: grid z = 1, F loaded once per CTA.
 #include "common.cuh"
 
 namespace nmfb200 {
@@ -22,6 +28,29 @@ __host__ __device__ inline int64_t chunk_tiles(int64_t Nc, int nchunks) {
 
 // register blocks of 16 components per thread row of the contraction kernel (Rp = 16 RB >= R)
 inline int contract_rb(int R) { return R <= 16 ? 1 : R <= 32 ? 2 : R <= 64 ? 4 : R <= 128 ? 8 : 16; }
+
+// GEMM-1 over `klen` components of the staged chunk: s[i][j] += Fs[r][4 ty + i] Gs[r][4 tx + j], r ascending
+__device__ __forceinline__ void gemm1(const float* Fs, const float* Gs, int klen, int tx, int ty, float (&s)[4][4]) {
+#pragma unroll 4
+  for (int r = 0; r < klen; ++r) {
+    float4 a = *reinterpret_cast<const float4*>(&Fs[r * kLd + 4 * ty]);
+    float4 b = *reinterpret_cast<const float4*>(&Gs[r * kLd + 4 * tx]);
+    float av[4] = {a.x, a.y, a.z, a.w}, bv[4] = {b.x, b.y, b.z, b.w};
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+      for (int j = 0; j < 4; ++j) s[i][j] = fmaf(av[i], bv[j], s[i][j]);
+  }
+}
+
+// components [k0, k0 + Rp) of `rows` consecutive rows of X (R columns) from row x0, transposed into Xs[r][row] (zero outside)
+__device__ __forceinline__ void stage_chunk(float* Xs, const float* __restrict__ X, int64_t x0, int64_t nx, int R, int k0,
+                                            int Rp, int tid) {
+  for (int idx = tid; idx < kTile * Rp; idx += 256) {
+    int row = idx / Rp, r = idx - row * Rp;
+    Xs[r * kLd + row] = (x0 + row < nx && k0 + r < R) ? X[(x0 + row) * R + k0 + r] : 0.f;
+  }
+}
 
 template <int MODE>
 __device__ __forceinline__ void phi(float v, float s, float bm2, float bm1, float& pn, float& pp) {
@@ -64,12 +93,12 @@ simt_contract_kernel(const float* __restrict__ V, int64_t ldv, const float* __re
   const int64_t tpc = chunk_tiles(Nc, nchunks);
   const int64_t tile_begin = chunk * tpc;
   const int64_t tile_end = min(tiles_total, tile_begin + tpc);
+  // rank blocks (R > 256 only: RB = 16): nb chunks of S's sum, this CTA's output block ob
+  const int nb = RB == 16 ? (int)gridDim.z : 1;
+  const int ob = RB == 16 ? (int)blockIdx.z : 0;
+  const bool multi = nb > 1;
 
-  for (int idx = tid; idx < kTile * Rp; idx += 256) {
-    int row = idx / Rp, r = idx - row * Rp;
-    float val = (m0 + row < Mr && r < R) ? F[(m0 + row) * R + r] : 0.f;
-    Fs[r * kLd + row] = val;
-  }
+  if (!multi) stage_chunk(Fs, F, m0, Mr, R, 0, Rp, tid);
 
   float accn[4][RB], accd[4][RB];
 #pragma unroll
@@ -79,41 +108,36 @@ simt_contract_kernel(const float* __restrict__ V, int64_t ldv, const float* __re
 
   for (int64_t tile = tile_begin; tile < tile_end; ++tile) {
     const int64_t c0 = tile * kTile;
-    __syncthreads();
-    for (int idx = tid; idx < kTile * Rp; idx += 256) {
-      int col = idx / Rp, r = idx - col * Rp;
-      float val = (c0 + col < Nc && r < R) ? G[(c0 + col) * R + r] : 0.f;
-      Gs[r * kLd + col] = val;
-    }
-    for (int idx = tid; idx < kTile * kTile; idx += 256) {
-      int a = idx >> 6, b = idx & 63;
-      int row, col;
-      float val = 0.f;
-      if (!TRANS) {
-        row = a; col = b;
-        if (m0 + row < Mr && c0 + col < Nc) val = V[(m0 + row) * ldv + c0 + col];
-      } else {
-        col = a; row = b;
-        if (m0 + row < Mr && c0 + col < Nc) val = V[(c0 + col) * ldv + m0 + row];
-      }
-      Ps[row * kLd + col] = val;
-    }
-    __syncthreads();
-
     float s[4][4];
 #pragma unroll
     for (int i = 0; i < 4; ++i)
 #pragma unroll
       for (int j = 0; j < 4; ++j) s[i][j] = 0.f;
-#pragma unroll 4
-    for (int r = 0; r < Rp; ++r) {
-      float4 a = *reinterpret_cast<const float4*>(&Fs[r * kLd + 4 * ty]);
-      float4 b = *reinterpret_cast<const float4*>(&Gs[r * kLd + 4 * tx]);
-      float av[4] = {a.x, a.y, a.z, a.w}, bv[4] = {b.x, b.y, b.z, b.w};
-#pragma unroll
-      for (int i = 0; i < 4; ++i)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) s[i][j] = fmaf(av[i], bv[j], s[i][j]);
+    for (int t = 0; t < nb; ++t) {
+      const int k0 = multi ? (ob + 1 + t) % nb * Rp : 0;     // the own block last: its G slice stays in Gs for GEMM-2
+      __syncthreads();
+      if (multi) stage_chunk(Fs, F, m0, Mr, R, k0, Rp, tid);
+      stage_chunk(Gs, G, c0, Nc, R, k0, Rp, tid);
+      if (t == 0) {
+        for (int idx = tid; idx < kTile * kTile; idx += 256) {
+          int a = idx >> 6, b = idx & 63;
+          int row, col;
+          float val = 0.f;
+          if (!TRANS) {
+            row = a; col = b;
+            if (m0 + row < Mr && c0 + col < Nc) val = V[(m0 + row) * ldv + c0 + col];
+          } else {
+            col = a; row = b;
+            if (m0 + row < Mr && c0 + col < Nc) val = V[(c0 + col) * ldv + m0 + row];
+          }
+          Ps[row * kLd + col] = val;
+        }
+      }
+      __syncthreads();
+      if (multi)
+        gemm1(Fs, Gs, min(Rp, (R - k0 + 15) & ~15), tx, ty, s);   // the chunk's components, zero-padded to 16
+      else
+        gemm1(Fs, Gs, Rp, tx, ty, s);
     }
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
@@ -154,7 +178,7 @@ simt_contract_kernel(const float* __restrict__ V, int64_t ldv, const float* __re
     if (row >= Mr) continue;
 #pragma unroll
     for (int k = 0; k < RB; ++k) {
-      int r = tx + 16 * k;
+      int r = ob * Rp + tx + 16 * k;
       if (r < R) {
         num[chunk * chunk_stride + row * ldp + r] = accn[i][k];
         if (kTwo) den[chunk * chunk_stride + row * ldp + r] = accd[i][k];
@@ -249,33 +273,23 @@ simt_loss_kernel(const float* __restrict__ V, int64_t ldv, const float* __restri
   const int64_t tpc = chunk_tiles(Nc, nchunks);
   const int64_t tile_begin = chunk * tpc;
   const int64_t tile_end = min(tiles_total, tile_begin + tpc);
-  for (int idx = tid; idx < kTile * Rp; idx += 256) {
-    int row = idx / Rp, r = idx - row * Rp;
-    Fs[r * kLd + row] = (m0 + row < Mr && r < R) ? F[(m0 + row) * R + r] : 0.f;
-  }
+  // Rp: the staged chunk width, round_up(R, 16) up to 256; above that S sums over rank chunks of 256 (F re-staged per chunk)
+  const bool multi = R > Rp;
+  if (!multi) stage_chunk(Fs, F, m0, Mr, R, 0, Rp, tid);
   double acc = 0.0;
   for (int64_t tile = tile_begin; tile < tile_end; ++tile) {
     const int64_t c0 = tile * kTile;
-    __syncthreads();
-    for (int idx = tid; idx < kTile * Rp; idx += 256) {
-      int col = idx / Rp, r = idx - col * Rp;
-      Gs[r * kLd + col] = (c0 + col < Nc && r < R) ? G[(c0 + col) * R + r] : 0.f;
-    }
-    __syncthreads();
     float s[4][4];
 #pragma unroll
     for (int i = 0; i < 4; ++i)
 #pragma unroll
       for (int j = 0; j < 4; ++j) s[i][j] = 0.f;
-#pragma unroll 4
-    for (int r = 0; r < Rp; ++r) {
-      float4 a = *reinterpret_cast<const float4*>(&Fs[r * kLd + 4 * ty]);
-      float4 b = *reinterpret_cast<const float4*>(&Gs[r * kLd + 4 * tx]);
-      float av[4] = {a.x, a.y, a.z, a.w}, bv[4] = {b.x, b.y, b.z, b.w};
-#pragma unroll
-      for (int i = 0; i < 4; ++i)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) s[i][j] = fmaf(av[i], bv[j], s[i][j]);
+    for (int k0 = 0; k0 < R; k0 += Rp) {
+      __syncthreads();
+      if (multi) stage_chunk(Fs, F, m0, Mr, R, k0, Rp, tid);
+      stage_chunk(Gs, G, c0, Nc, R, k0, Rp, tid);
+      __syncthreads();
+      gemm1(Fs, Gs, min(Rp, (R - k0 + 15) & ~15), tx, ty, s);
     }
     float local = 0.f;
 #pragma unroll
@@ -311,6 +325,8 @@ int loss_chunks(int64_t Mr, int64_t Nc) {
 
 }  // namespace
 
+int simt_rank_blocks(int R) { return (int)ceil_div(R, 256); }
+
 int simt_nmf_max_blocks(int64_t Mr, int64_t Nc) { return (int)(ceil_div(Mr, kTile) * loss_chunks(Mr, Nc)); }
 
 void simt_nmf_plan(int64_t Mr, int64_t Nc, int R, int nchunks, SimtNmfPlan* p) {
@@ -329,10 +345,10 @@ int sum_partials(const double* p, int n, double* out, cudaStream_t st) {
 int simt_nmf_contract(const float* V, int64_t ldv, int trans, const float* F, const float* G, int64_t Mr,
                       int64_t Nc, int R, double beta, int nchunks, float* num, float* den, int64_t ldp,
                       int64_t chunk_stride, cudaStream_t st) {
-  if (R < 1 || R > 256) { set_error("simt_nmf_contract: rank must be in [1, 256]"); return 1; }
+  if (R < 1) { set_error("simt_nmf_contract: rank must be positive"); return 1; }
   int mode = beta_mode(beta);
   float bm2 = (float)(beta - 2.0), bm1 = (float)(beta - 1.0);
-  dim3 grid((unsigned)ceil_div(Mr, kTile), (unsigned)nchunks);
+  dim3 grid((unsigned)ceil_div(Mr, kTile), (unsigned)nchunks, (unsigned)simt_rank_blocks(R));
 #define NMF_RB(RBV)                                                                                       \
   return launch_contract_rb<RBV>(trans, mode, grid, st, V, ldv, F, G, Mr, Nc, R, bm2, bm1, nchunks, num, den, \
                                  ldp, chunk_stride)
@@ -348,12 +364,12 @@ int simt_nmf_contract(const float* V, int64_t ldv, int trans, const float* F, co
 
 int simt_nmf_loss(const float* V, int64_t ldv, const float* F, const float* G, int64_t Mr, int64_t Nc, int R,
                   double beta, double* block_partials, int max_blocks, double* loss_dev, cudaStream_t st) {
-  if (R < 1 || R > 256) { set_error("simt_nmf_loss: rank must be in [1, 256]"); return 1; }
+  if (R < 1) { set_error("simt_nmf_loss: rank must be positive"); return 1; }
   int nchunks = loss_chunks(Mr, Nc);
   dim3 grid((unsigned)ceil_div(Mr, kTile), (unsigned)nchunks);
   int nblocks = (int)(grid.x * grid.y);
   if (nblocks > max_blocks) { set_error("simt_nmf_loss: partial buffer too small"); return 1; }
-  int Rp = (int)round_up(R, 16);
+  int Rp = (int)round_up(R < 256 ? R : 256, 16);
   size_t smem = (size_t)2 * Rp * kLd * sizeof(float);
   int mode = beta_mode(beta);
 #define NMF_LOSS(M)                                                                                     \

@@ -70,25 +70,27 @@ raw_sum_kernel(ApplyArgs a, float* __restrict__ num_out, float* __restrict__ den
   }
 }
 
-// stage 1 for inner == 1: x is (outer, R) row-major; block b sums a row slab.
+// stage 1 for inner == 1: x is (outer, R) row-major; block (b, y) sums a row slab of components [256 y, 256 y + 256).
 __global__ void __launch_bounds__(256)
 colsum_rows_kernel(const float* __restrict__ x, int64_t outer, int R, int64_t rows_per_block,
                    float* __restrict__ partial) {
   __shared__ float sh[256];
   const int tid = threadIdx.x;
-  const int ng = 256 / R > 0 ? 256 / R : 1;      // row groups (R <= 256)
-  const int g = tid / R, r = tid - g * R;
+  const int r0 = blockIdx.y * 256;
+  const int Rb = min(R - r0, 256);               // this block's components
+  const int ng = 256 / Rb > 0 ? 256 / Rb : 1;    // row groups
+  const int g = tid / Rb, r = tid - g * Rb;
   const int64_t row0 = (int64_t)blockIdx.x * rows_per_block;
   const int64_t row1 = min(outer, row0 + rows_per_block);
   float acc = 0.f;
   if (g < ng)
-    for (int64_t row = row0 + g; row < row1; row += ng) acc += x[row * R + r];
+    for (int64_t row = row0 + g; row < row1; row += ng) acc += x[row * R + r0 + r];
   sh[tid] = acc;
   __syncthreads();
-  if (tid < R) {
+  if (tid < Rb) {
     float t = 0.f;
-    for (int k = 0; k < ng; ++k) t += sh[k * R + tid];
-    partial[(int64_t)blockIdx.x * R + tid] = t;
+    for (int k = 0; k < ng; ++k) t += sh[k * Rb + tid];
+    partial[(int64_t)blockIdx.x * R + r0 + tid] = t;
   }
 }
 
@@ -254,14 +256,13 @@ int64_t colsum_scratch_floats(int64_t outer, int R, int64_t inner) { return cols
 
 int factor_colsum(const float* x, int64_t outer, int R, int64_t inner, float* scratch, int64_t scratch_floats,
                   float* sums, cudaStream_t st) {
-  if (R > 256) { set_error("factor_colsum: rank must be <= 256"); return 1; }
   const int64_t nb = colsum_blocks(outer, inner);
   if (nb * R > scratch_floats) { set_error("factor_colsum: scratch too small"); return 1; }
   if (inner > 1) {
     colsum_runs_kernel<<<(unsigned)(outer * R), 256, 0, st>>>(x, inner, scratch);
   } else {
     const int64_t rpb = ceil_div(outer, nb);
-    colsum_rows_kernel<<<(unsigned)nb, 256, 0, st>>>(x, outer, R, rpb, scratch);
+    colsum_rows_kernel<<<dim3((unsigned)nb, (unsigned)ceil_div(R, 256)), 256, 0, st>>>(x, outer, R, rpb, scratch);
   }
   NMF_LAUNCH_CHECK();
   colsum_final_kernel<<<(unsigned)ceil_div(R, 64), 64, 0, st>>>(scratch, nb, R, sums);

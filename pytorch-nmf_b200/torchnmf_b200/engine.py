@@ -49,7 +49,11 @@ def _workspace_bytes(key):
     """Upper estimate of the device memory a cached context of this key holds."""
     if key[0] == "nmf":                   # ("nmf", device, N, C, R, precision): V16 + Vt16 + split partials + fp32 scratch
         _, _, N, C, R = key[:5]
-        return 4 * N * C + 64 * (N + C) * max(R, 64)
+        est = 4 * N * C + 64 * (N + C) * max(R, 64)
+        if R > 256:                       # fp32 only: the chunked num / den partial slabs of the larger update
+            p = _capi.nmf_plan(N, C, R)
+            est += 8 * R * max(p["nch_w"] * C, p["nch_h"] * N)
+        return est
     if key[0] == "nmfd":                  # ("nmfd", device, B, C, X, R, K, precision): ratio tiles + shifted operand copies
         _, _, B, C, X, R, K = key[:7]
         nx, nk = 1, 1

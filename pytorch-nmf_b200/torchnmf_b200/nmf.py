@@ -194,8 +194,9 @@ class BaseComponent(torch.nn.Module):
             on_gpu = W.device.type == "cuda"
             dev = W.device if on_gpu else torch.device("cuda", torch.cuda.current_device())
             Vd = V.to(dev, non_blocking=True)
+            # the sparse-target kernels cover ranks up to 256; above, the target is densified like for other betas
             use_sparse_kernels = (sparse_kernels and sparse_target and beta in (1, 2) and group is None
-                                  and self._sparse_kernels)
+                                  and self._sparse_kernels and W.shape[1] <= 256)
             if not use_sparse_kernels:
                 Vd = (Vd.to_dense() if sparse_target else Vd).to(f32).contiguous()
             if on_gpu and W.dtype == f32 and H.dtype == f32:

@@ -86,7 +86,7 @@ class _FusedTerms:
                 and W.device == V.device and H.device == V.device and H.dim() == W.dim()
                 and W.data.is_contiguous() and H.data.is_contiguous()):
             return None
-        if W.shape[1] != H.shape[1] or W.shape[1] > 256:
+        if W.shape[1] != H.shape[1] or (nd and W.shape[1] > 256):     # the convolutive kernels stop at rank 256
             return None
         want = (H.shape[0], W.shape[0]) + tuple(j + k - 1 for j, k in zip(H.shape[2:], W.shape[2:]))
         if tuple(V.shape) != want:
