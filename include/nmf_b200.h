@@ -243,8 +243,14 @@ int nmfb200_nmfd_tc_plan(int64_t B, int64_t C, int64_t L, int64_t R, int64_t T, 
  * x[:, j, :] of the fp32 device tensor x viewed as (outer, D, inner) is replaced IN PLACE by the closest non-negative
  * vector with L1 norm k1[j] and squared L2 norm k2[j] (k1, k2: D device floats).  The reference's data-dependent loop
  * (one host synchronisation per round and slice) runs on the device, one block per slice, one launch for all D slices.
- * zeroed_ws: D * outer * inner bytes of device scratch.  Context-free: runs on CUDA device `device`, the caller's
- * current device is restored. */
+ * zeroed_ws: D * outer * inner bytes of device scratch, any contents (cleared in the first round).  Context-free: runs on
+ * CUDA device `device`, the caller's current device is restored.
+ * Degenerate slices, as the reference's arithmetic has them: where the surviving support is uniform after fp32 rounding
+ * (a constant slice, survivors that all tie, or one element whose shifted value x + (k1 - x) rounds exactly to k1)
+ * w.w = 0 and the quadratic gives 0 / 0, so the slice becomes NaN, as in the reference; a one-element slice whose shift
+ * does not round exactly keeps w != 0 and a finite result.  Where a round zeroes every coordinate the reference divides by zero (ZeroDivisionError); the kernel stops
+ * and leaves the slice at zero.  fp32 rounding decides which of the two a near-uniform slice meets: float64 and fp32 can
+ * differ there. */
 int nmfb200_hoyer_project(int device, float* x, int64_t outer, int64_t D, int64_t inner, const float* k1, const float* k2,
                           void* zeroed_ws, void* stream);
 
