@@ -14,7 +14,8 @@
  *
  * Conventions
  *   - plain C: pointers, sizes, doubles.  No torch / C++ types.
- *   - all matrix pointers are DEVICE pointers to fp32, row-major, reference layout:
+ *   - all matrix pointers are DEVICE pointers to fp32, row-major, reference layout, except that a dense target V may also
+ *     hold fp16 or bf16 elements (nmfb200_*_set_target_typed: read where they are, no fp32 copy):
  *       NMF : V (N,C)   W (C,R)   H (N,R)            V ~= H @ W^T            (nmf.py:659-662)
  *       NMFD: V (B,C,L) W (C,R,T) H (B,R,L-T+1)      V ~= conv1d(H, flip(W)) (nmf.py:743-750)
  *   - `stream` is a cudaStream_t passed as void* (0 = legacy default stream).  Every call is
@@ -41,6 +42,15 @@ enum {
   NMFB200_PREC_F32       = 0,  /* fused CUDA-core kernels, fp32 operands and accumulators (exact), any rank */
   NMFB200_PREC_F16       = 1,  /* wgmma, fp16 operands, fp32 accumulate                           */
   NMFB200_PREC_F16_SPLIT = 2   /* wgmma, fp16 hi/lo split factors (~22-bit), fp16 ratio tile      */
+};
+
+/* element type of a dense target V (nmfb200_nmf_set_target_typed / nmfb200_nmfd_set_target_typed).  The kernels convert
+ * each element to fp32 where they load it; fp16 and bf16 values are exact in fp32, so a half-precision target gives the
+ * results, bit for bit, of the same values registered as fp32. */
+enum {
+  NMFB200_DTYPE_F32  = 0,
+  NMFB200_DTYPE_F16  = 1,      /* IEEE binary16 (__half)        */
+  NMFB200_DTYPE_BF16 = 2       /* bfloat16 (__nv_bfloat16)      */
 };
 
 /* error codes */
@@ -85,6 +95,11 @@ int nmfb200_precision_for_beta(const nmfb200_ctx* ctx, double beta);
  * operand copies and the V-only loss terms.  Replaces nothing in the reference: V is simply the
  * argument of fit() (nmf.py:299).  Asynchronous. */
 int nmfb200_nmf_set_target(nmfb200_ctx* ctx, const float* V, int64_t ldv, void* stream);
+/* The same for a target of element type `dtype` (NMFB200_DTYPE_*); nmfb200_nmf_set_target is the NMFB200_DTYPE_F32 case.
+ * V stays borrowed: every later call of this context (update_*, iterate, loss, loss_prefetch_w, raw_terms, w_partial,
+ * contract_only, update_w_peer, target_minmax) reads it.  NMFB200_ERR_INVALID for an unknown dtype or a V not aligned to
+ * its element size (2 bytes for fp16 / bf16, 4 for fp32); no other alignment is required. */
+int nmfb200_nmf_set_target_typed(nmfb200_ctx* ctx, const void* V, int64_t ldv, int dtype, void* stream);
 /* min / max of the registered target (fit()'s validation, nmf.py:329-336).  Synchronises. */
 int nmfb200_target_minmax(nmfb200_ctx* ctx, float* vmin, float* vmax, void* stream);
 
@@ -181,6 +196,9 @@ int nmfb200_nmfd_create(nmfb200_ctx** out, int device, int64_t B, int64_t C, int
 int nmfb200_nmfnd_create(nmfb200_ctx** out, int device, int64_t B, int64_t C, int ndim, const int64_t* vdims,
                          int64_t R, const int64_t* kdims, int precision);
 int nmfb200_nmfd_set_target(nmfb200_ctx* ctx, const float* V, void* stream);
+/* The same for a contiguous target of element type `dtype` (NMFB200_DTYPE_*), with the checks of
+ * nmfb200_nmf_set_target_typed; nmfb200_nmfd_set_target is the NMFB200_DTYPE_F32 case. */
+int nmfb200_nmfd_set_target_typed(nmfb200_ctx* ctx, const void* V, int dtype, void* stream);
 int nmfb200_nmfd_update_w(nmfb200_ctx* ctx, float* W, const float* H,
                           double beta, double gamma, double l1_reg, double l2_reg, void* stream);
 int nmfb200_nmfd_update_h(nmfb200_ctx* ctx, const float* W, float* H,

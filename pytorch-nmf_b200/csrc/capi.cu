@@ -25,7 +25,8 @@ struct nmfb200_ctx {
   bool tc_off = false;      // AUTO found the target outside the fp16 operand range: fp32 CUDA-core kernels instead
   int64_t N = 0, C = 0, R = 0;
   NmfdShape d{};
-  const float* V = nullptr;
+  const void* V = nullptr;        // the dense target, borrowed: vdtype (NMFB200_DTYPE_*) elements
+  int vdtype = NMFB200_DTYPE_F32;
   int64_t ldv = 0;
   bool has_target = false;
   // chunked partial numerators / denominators of the CUDA-core path
@@ -123,7 +124,7 @@ int simt_contract(nmfb200_ctx* c, int which, const float* W, const float* H, dou
   const float* F = which == 0 ? W : H;
   const float* G = which == 0 ? H : W;
   const int64_t rows = which == 0 ? c->C : c->N, cols = which == 0 ? c->N : c->C;
-  return simt_nmf_contract(c->V, c->ldv, /*trans=*/which == 0 ? 1 : 0, F, G, rows, cols, (int)c->R, beta,
+  return simt_nmf_contract(c->V, c->vdtype, c->ldv, /*trans=*/which == 0 ? 1 : 0, F, G, rows, cols, (int)c->R, beta,
                            which == 0 ? c->nch_w : c->nch_h, c->num, c->den, c->R, rows * c->R, st);
 }
 
@@ -141,6 +142,19 @@ ApplyArgs nmf_apply_args(const nmfb200_ctx* c, int which, float* param, double b
 
 bool use_tc(const nmfb200_ctx* c, double beta) {
   return c->tc != nullptr && !c->tc_off && tc_supports_beta(c->tc, beta);
+}
+
+// What every dense set_target checks of the target's element type and pointer (the kernels load single elements: element
+// alignment is all they need).
+int check_target(const void* V, int dtype) {
+  if (!V) return fail(NMFB200_ERR_INVALID, "null target");
+  if (dtype != NMFB200_DTYPE_F32 && dtype != NMFB200_DTYPE_F16 && dtype != NMFB200_DTYPE_BF16)
+    return fail(NMFB200_ERR_INVALID, "unknown target dtype " + std::to_string(dtype) +
+                                         " (NMFB200_DTYPE_F32 = 0, NMFB200_DTYPE_F16 = 1, NMFB200_DTYPE_BF16 = 2)");
+  const int size = vdtype_size(dtype);
+  if (reinterpret_cast<uintptr_t>(V) % size)
+    return fail(NMFB200_ERR_INVALID, "target pointer is not aligned to its element size (" + std::to_string(size) + " bytes)");
+  return 0;
 }
 
 }  // namespace
@@ -274,15 +288,20 @@ int nmfb200_nmf_sparse_plan(int64_t N, int64_t C, int64_t R, int64_t* out, int n
 }
 
 int nmfb200_nmf_set_target(nmfb200_ctx* ctx, const float* V, int64_t ldv, void* stream) {
+  return nmfb200_nmf_set_target_typed(ctx, V, ldv, NMFB200_DTYPE_F32, stream);
+}
+
+int nmfb200_nmf_set_target_typed(nmfb200_ctx* ctx, const void* V, int64_t ldv, int dtype, void* stream) {
   CTX_GUARD(ctx, 0);
   if (!V || ldv < ctx->C) return fail(NMFB200_ERR_INVALID, "bad target pointer / leading dimension");
+  if (int rc = check_target(V, dtype)) return rc;
   cudaStream_t st = (cudaStream_t)stream;
-  ctx->V = V; ctx->ldv = ldv; ctx->has_target = true; ctx->sparse = false;
-  int rc = matrix_minmax(V, ctx->N, ctx->C, ldv, ctx->mm_scratch, ctx->mm_scratch + 2048, st);
+  ctx->V = V; ctx->vdtype = dtype; ctx->ldv = ldv; ctx->has_target = true; ctx->sparse = false;
+  int rc = matrix_minmax(V, dtype, ctx->N, ctx->C, ldv, ctx->mm_scratch, ctx->mm_scratch + 2048, st);
   if (rc) return rc;
   ctx->tc_off = false;
   if (ctx->tc) {
-    rc = tc_set_target(ctx->tc, V, ldv, ctx->mm_scratch + 2048, st);
+    rc = tc_set_target(ctx->tc, V, dtype, ldv, ctx->mm_scratch + 2048, st);
     if (rc) return rc;
     if (ctx->auto_mode) {
       // AUTO is conservative: the fp16 copy of V carries ONE power-of-two scale (max -> 2^14), so positive entries below
@@ -491,7 +510,7 @@ int nmfb200_nmf_loss(nmfb200_ctx* ctx, const float* W, const float* H, double be
   cudaStream_t st = (cudaStream_t)stream;
   if (ctx->sparse) return sparse_loss_ctx(ctx, W, H, beta, loss_dev, st);
   if (use_tc(ctx, beta)) return tc_loss(ctx->tc, W, H, beta, loss_dev, st);
-  return simt_nmf_loss(ctx->V, ctx->ldv, H, W, ctx->N, ctx->C, (int)ctx->R, beta, ctx->loss_blocks,
+  return simt_nmf_loss(ctx->V, ctx->vdtype, ctx->ldv, H, W, ctx->N, ctx->C, (int)ctx->R, beta, ctx->loss_blocks,
                        ctx->loss_max_blocks, loss_dev, st);
 }
 
@@ -704,17 +723,21 @@ int nmfb200_nmfnd_create(nmfb200_ctx** out, int device, int64_t B, int64_t C, in
 }
 
 int nmfb200_nmfd_set_target(nmfb200_ctx* ctx, const float* V, void* stream) {
+  return nmfb200_nmfd_set_target_typed(ctx, V, NMFB200_DTYPE_F32, stream);
+}
+
+int nmfb200_nmfd_set_target_typed(nmfb200_ctx* ctx, const void* V, int dtype, void* stream) {
   CTX_GUARD(ctx, 1);
-  if (!V) return fail(NMFB200_ERR_INVALID, "null target");
-  ctx->V = V; ctx->has_target = true;
+  if (int rc = check_target(V, dtype)) return rc;
+  ctx->V = V; ctx->vdtype = dtype; ctx->has_target = true;
   cudaStream_t st = (cudaStream_t)stream;
   const int64_t vin = ctx->d.v_inner();
-  int rc = matrix_minmax(V, (int64_t)ctx->d.B * ctx->d.C, vin, vin, ctx->mm_scratch, ctx->mm_scratch + 2048, st);
+  int rc = matrix_minmax(V, dtype, (int64_t)ctx->d.B * ctx->d.C, vin, vin, ctx->mm_scratch, ctx->mm_scratch + 2048, st);
   if (rc) return rc;
   ctx->tc_off = false;
   if (ctx->tcd) {
     double vsum = 0.0;
-    rc = tc_nmfd_set_target(ctx->tcd, V, &vsum, st);       // synchronises: sum(V) for kappa
+    rc = tc_nmfd_set_target(ctx->tcd, V, dtype, &vsum, st);       // synchronises: sum(V) for kappa
     if (rc) return rc;
     tc_nmfd_mark_dirty(ctx->tcd);                         // a new fit: the factors may be anything
     if (ctx->auto_mode) {                                 // same conservative rule as the NMF path: heavy-tailed targets stay fp32
@@ -733,7 +756,7 @@ static bool nmfd_use_tc(const nmfb200_ctx* c, double beta) {
   return c->tcd != nullptr && !c->tc_off && tc_nmfd_supported(c->d, beta);
 }
 static int nmfd_tc_recon(nmfb200_ctx* c, const float* W, const float* H, bool loss, double* loss_dev, cudaStream_t st) {
-  return tc_nmfd_recon(c->tcd, c->V, W, H, loss, loss_dev, st);
+  return tc_nmfd_recon(c->tcd, c->V, c->vdtype, W, H, loss, loss_dev, st);
 }
 
 static int nmfd_phi(nmfb200_ctx* c, const float* W, const float* H, double beta, cudaStream_t st) {
@@ -742,7 +765,7 @@ static int nmfd_phi(nmfb200_ctx* c, const float* W, const float* H, double beta,
     int e = ensure_den(c);
     if (e) return e;
   }
-  return nmfd_recon_phi(c->d, c->V, W, H, beta, c->Pn, c->Pp, nullptr, 0, nullptr, st);
+  return nmfd_recon_phi(c->d, c->V, c->vdtype, W, H, beta, c->Pn, c->Pp, nullptr, 0, nullptr, st);
 }
 
 // Both backward passes of one factor (which = 0: W, 1: H) from the current factors, described as the ratio stage's input:
@@ -875,7 +898,7 @@ int nmfb200_nmfd_loss(nmfb200_ctx* ctx, const float* W, const float* H, double b
   if (!ctx->has_target) return fail(NMFB200_ERR_STATE, "set_target has not been called");
   if (!W || !H || !loss_dev) return fail(NMFB200_ERR_INVALID, "null pointer");
   if (nmfd_use_tc(ctx, beta)) return nmfd_tc_recon(ctx, W, H, true, loss_dev, (cudaStream_t)stream);
-  return nmfd_recon_phi(ctx->d, ctx->V, W, H, beta, nullptr, nullptr, ctx->loss_blocks, ctx->loss_max_blocks,
+  return nmfd_recon_phi(ctx->d, ctx->V, ctx->vdtype, W, H, beta, nullptr, nullptr, ctx->loss_blocks, ctx->loss_max_blocks,
                         loss_dev, (cudaStream_t)stream);
 }
 

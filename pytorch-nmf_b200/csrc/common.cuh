@@ -2,14 +2,37 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
+#include <cuda_bf16.h>
 #include <stdint.h>
 #include <stdio.h>
 #include <string>
+#include <type_traits>
 
 namespace nmfb200 {
 
 // torchnmf/constants.py:3 -- float32 machine epsilon, 2^-23
 constexpr float kEps = 1.1920928955078125e-07f;
+
+// Element type of the dense target V (include/nmf_b200.h: NMFB200_DTYPE_*).  Every kernel that reads V takes it as a
+// template parameter TV and converts each element with to_f32 where it loads it.  fp16 and bf16 values are exact in fp32,
+// so everything after the load computes what it computes on an fp32 copy of the same values.
+enum VDtype : int { kVF32 = 0, kVF16 = 1, kVBF16 = 2 };
+__device__ __forceinline__ float to_f32(float v) { return v; }
+__device__ __forceinline__ float to_f32(__half v) { return __half2float(v); }
+// bf16 is the upper half of an fp32 word: the same bits as __bfloat162float, written as the integer shift because that form
+// leaves the fp32 CUDA-core contraction's register allocation as it is for fp32 (no extra spill in its beta != 0, 1, 2 kernels)
+__device__ __forceinline__ float to_f32(__nv_bfloat16 v) { return __uint_as_float((unsigned)__bfloat16_as_ushort(v) << 16); }
+static inline int vdtype_size(int dtype) { return dtype == kVF32 ? 4 : 2; }
+// Host dispatch: f(p) with p = V as `const float*`, `const __half*` or `const __nv_bfloat16*` per `dtype` (validated by the
+// caller: capi.cu's set_target); vtype_t<decltype(p)> is the element type.
+template <class P>
+using vtype_t = std::remove_cv_t<std::remove_pointer_t<P>>;
+template <class F>
+int with_vtype(const void* V, int dtype, F&& f) {
+  if (dtype == kVF16) return f(static_cast<const __half*>(V));
+  if (dtype == kVBF16) return f(static_cast<const __nv_bfloat16*>(V));
+  return f(static_cast<const float*>(V));
+}
 
 // beta-divergence branch of nmf.py:61-74 / metrics.py:60-96
 enum BetaMode : int { kKL = 0, kEU = 1, kIS = 2, kGeneric = 3 };
@@ -63,12 +86,12 @@ static inline bool grid_fits(const Grid3& g) {
 //   S = F G^T (Mr x Nc),  (Pn, Pp) = phi_beta(Vm, S)          [nmf.py:61-74]
 //   num[ch][m][r] = sum_{c in chunk ch} Pn[m,c] G[c,r]          [nmf.py:77]
 //   den[ch][m][r] = sum_{c in chunk ch} Pp[m,c] G[c,r]          [nmf.py:82, beta != 1 only]
-// Vm[m,c] = V[m*ldv + c] (trans = 0) or V[c*ldv + m] (trans = 1).  Any rank R >= 1.
-int simt_nmf_contract(const float* V, int64_t ldv, int trans, const float* F, const float* G,
+// Vm[m,c] = V[m*ldv + c] (trans = 0) or V[c*ldv + m] (trans = 1), elements of type `vdtype` (VDtype).  Any rank R >= 1.
+int simt_nmf_contract(const void* V, int vdtype, int64_t ldv, int trans, const float* F, const float* G,
                       int64_t Mr, int64_t Nc, int R, double beta, int nchunks,
                       float* num, float* den, int64_t ldp, int64_t chunk_stride, cudaStream_t st);
 // beta_div(F G^T, Vm) accumulated into block partials then *loss_dev (double).  v_const is unused here.
-int simt_nmf_loss(const float* V, int64_t ldv, const float* F, const float* G, int64_t Mr, int64_t Nc,
+int simt_nmf_loss(const void* V, int vdtype, int64_t ldv, const float* F, const float* G, int64_t Mr, int64_t Nc,
                   int R, double beta, double* block_partials, int max_blocks, double* loss_dev,
                   cudaStream_t st);
 int simt_nmf_max_blocks(int64_t Mr, int64_t Nc);
@@ -105,8 +128,8 @@ int64_t colsum_scratch_floats(int64_t outer, int R, int64_t inner);
 // dst[i] = sum_ch src[ch*stride + i]   (chunk reduction for the sharded partial buffers)
 int reduce_chunks(const float* src, int nchunks, int64_t chunk_stride, int64_t rows, int R, int64_t ldp,
                   float* dst, cudaStream_t st);
-// min / max of a strided fp32 matrix (fit()'s validation), results in mm[0..1]
-int matrix_minmax(const float* V, int64_t rows, int64_t cols, int64_t ld, float* scratch2048, float* mm,
+// min / max of a strided matrix of `vdtype` elements (fit()'s validation), results in mm[0..1]
+int matrix_minmax(const void* V, int vdtype, int64_t rows, int64_t cols, int64_t ld, float* scratch2048, float* mm,
                   cudaStream_t st);
 // *out = sum of n doubles in fixed order (single block)
 int sum_partials(const double* p, int n, double* out, cudaStream_t st);
@@ -149,7 +172,7 @@ struct NmfdShape {
 };
 // WH = conv(H, W); writes Pn (and Pp when beta != 1) (B,C,L) or, when loss_blocks != nullptr,
 // reduces beta_div(WH, V) instead.
-int nmfd_recon_phi(const NmfdShape& s, const float* V, const float* W, const float* H, double beta,
+int nmfd_recon_phi(const NmfdShape& s, const void* V, int vdtype, const float* W, const float* H, double beta,
                    float* Pn, float* Pp, double* loss_blocks, int max_blocks, double* loss_dev,
                    cudaStream_t st);
 // batch elements per launch of the kernels that put the batch on grid.z (fp32 recon / dgrad, tensor-core recon / dgrad)

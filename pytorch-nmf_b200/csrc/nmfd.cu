@@ -77,12 +77,12 @@ struct SlideArgs {
   int M, K;                  // rows of the output, size of the reduced dimension
   int64_t sm, sk;            // strides of A over m and k (elements); the offset (t1, t2, t) is contiguous
   int nsplit;                // !FWD: splits of k
-  const float* V; float beta; float* Pn; float* Pp; double* block_partials;     // FWD epilogue
+  const void* V; float beta; float* Pn; float* Pp; double* block_partials;      // FWD epilogue (V: TV elements)
   float* out;                // !FWD: [split][B][R][h_inner]
   int b0;                    // first batch element of this launch
 };
 
-template <int MT, bool FWD, int MODE, bool LOSS>
+template <int MT, bool FWD, int MODE, bool LOSS, typename TV>
 __global__ void __launch_bounds__(256)
 nmfd_slide_kernel(NmfdShape s, SlideArgs a) {
   using G = Geo<MT>;
@@ -186,7 +186,7 @@ nmfd_slide_kernel(NmfdShape s, SlideArgs a) {
         const int l = l0 + 4 * lt + j;
         if (c < s.C && l < s.L && o < OUT) {
           const int64_t off = (((int64_t)b * s.C + c) * OUT + o) * s.L + l;
-          const float v = a.V[off];
+          const float v = to_f32(static_cast<const TV*>(a.V)[off]);
           if (LOSS) {
             local += loss_term_d<MODE>(v, acc[i][j], a.beta);
           } else {
@@ -350,12 +350,13 @@ Grid3 slide_grid(const NmfdShape& s, bool fwd, int mt, int M, int nsplit) {
 dim3 dim3_of(const Grid3& g) { return dim3((unsigned)g.x, (unsigned)g.y, (unsigned)g.z); }
 
 
-template <int MT, bool FWD>
+// TV: the target's element type (FWD only; the dgrad pass reads no V and always takes float)
+template <int MT, bool FWD, typename TV>
 void launch_slide(const NmfdShape& s, const SlideArgs& a, int mode, bool loss, dim3 grid, cudaStream_t st) {
-  if (!FWD) { nmfd_slide_kernel<MT, false, kKL, false><<<grid, 256, 0, st>>>(s, a); return; }
-#define NMFD_GO(M)                                                              \
-  if (loss) nmfd_slide_kernel<MT, true, M, true><<<grid, 256, 0, st>>>(s, a);   \
-  else nmfd_slide_kernel<MT, true, M, false><<<grid, 256, 0, st>>>(s, a);
+  if (!FWD) { nmfd_slide_kernel<MT, false, kKL, false, float><<<grid, 256, 0, st>>>(s, a); return; }
+#define NMFD_GO(M)                                                                  \
+  if (loss) nmfd_slide_kernel<MT, true, M, true, TV><<<grid, 256, 0, st>>>(s, a);   \
+  else nmfd_slide_kernel<MT, true, M, false, TV><<<grid, 256, 0, st>>>(s, a);
   switch (mode) {
     case kKL: NMFD_GO(kKL); break;
     case kEU: NMFD_GO(kEU); break;
@@ -365,25 +366,25 @@ void launch_slide(const NmfdShape& s, const SlideArgs& a, int mode, bool loss, d
 #undef NMFD_GO
 }
 
-template <bool FWD>
+template <bool FWD, typename TV>
 void dispatch_slide(int mt, const NmfdShape& s, const SlideArgs& a, int mode, bool loss, dim3 grid, cudaStream_t st) {
   switch (mt) {
-    case 4: launch_slide<4, FWD>(s, a, mode, loss, grid, st); break;
-    case 8: launch_slide<8, FWD>(s, a, mode, loss, grid, st); break;
-    case 16: launch_slide<16, FWD>(s, a, mode, loss, grid, st); break;
-    case 32: launch_slide<32, FWD>(s, a, mode, loss, grid, st); break;
-    default: launch_slide<64, FWD>(s, a, mode, loss, grid, st); break;
+    case 4: launch_slide<4, FWD, TV>(s, a, mode, loss, grid, st); break;
+    case 8: launch_slide<8, FWD, TV>(s, a, mode, loss, grid, st); break;
+    case 16: launch_slide<16, FWD, TV>(s, a, mode, loss, grid, st); break;
+    case 32: launch_slide<32, FWD, TV>(s, a, mode, loss, grid, st); break;
+    default: launch_slide<64, FWD, TV>(s, a, mode, loss, grid, st); break;
   }
 }
 
 // one launch of the sliding kernel per slice of at most kMaxGridYZ batch elements
-template <bool FWD>
+template <bool FWD, typename TV = float>
 int launch_slices(int mt, const NmfdShape& s, SlideArgs a, int mode, bool loss, const Grid3& g, cudaStream_t st) {
   for (int64_t b0 = 0; b0 < s.B; b0 += g.z) {
     a.b0 = (int)b0;
     dim3 grid = dim3_of(g);
     grid.z = (unsigned)std::min<int64_t>(g.z, s.B - b0);
-    dispatch_slide<FWD>(mt, s, a, mode, loss, grid, st);
+    dispatch_slide<FWD, TV>(mt, s, a, mode, loss, grid, st);
     NMF_LAUNCH_CHECK();
   }
   return 0;
@@ -396,7 +397,7 @@ int64_t nmfd_max_blocks(const NmfdShape& s) {
   return g.x * g.y * s.B;
 }
 
-int nmfd_recon_phi(const NmfdShape& s, const float* V, const float* W, const float* H, double beta, float* Pn,
+int nmfd_recon_phi(const NmfdShape& s, const void* V, int vdtype, const float* W, const float* H, double beta, float* Pn,
                    float* Pp, double* loss_blocks, int max_blocks, double* loss_dev, cudaStream_t st) {
   const int mt = row_tile(s.C);
   const Grid3 grid = slide_grid(s, true, mt, s.C, 1);
@@ -406,7 +407,10 @@ int nmfd_recon_phi(const NmfdShape& s, const float* V, const float* W, const flo
   SlideArgs a{};
   a.A = W; a.X = H; a.M = s.C; a.K = s.R; a.sm = (int64_t)s.R * s.w_inner(); a.sk = s.w_inner(); a.nsplit = 1;
   a.V = V; a.beta = (float)beta; a.Pn = Pn; a.Pp = Pp; a.block_partials = loss_blocks; a.out = nullptr;
-  if (int rc = launch_slices<true>(mt, s, a, beta_mode(beta), loss, grid, st)) return rc;
+  if (int rc = with_vtype(V, vdtype, [&](auto Vt) {
+        return launch_slices<true, vtype_t<decltype(Vt)>>(mt, s, a, beta_mode(beta), loss, grid, st);
+      }))
+    return rc;
   if (loss) return sum_partials(loss_blocks, nblocks, loss_dev, st);
   return 0;
 }

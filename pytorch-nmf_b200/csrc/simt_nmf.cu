@@ -71,9 +71,9 @@ __device__ __forceinline__ void phi(float v, float s, float bm2, float bm1, floa
   }
 }
 
-template <int RB, bool TRANS, int MODE>
+template <int RB, bool TRANS, int MODE, typename TV>
 __global__ void __launch_bounds__(256)
-simt_contract_kernel(const float* __restrict__ V, int64_t ldv, const float* __restrict__ F,
+simt_contract_kernel(const TV* __restrict__ V, int64_t ldv, const float* __restrict__ F,
                      const float* __restrict__ G, int64_t Mr, int64_t Nc, int R, float bm2, float bm1,
                      int nchunks, float* __restrict__ num, float* __restrict__ den, int64_t ldp,
                      int64_t chunk_stride) {
@@ -125,10 +125,10 @@ simt_contract_kernel(const float* __restrict__ V, int64_t ldv, const float* __re
           float val = 0.f;
           if (!TRANS) {
             row = a; col = b;
-            if (m0 + row < Mr && c0 + col < Nc) val = V[(m0 + row) * ldv + c0 + col];
+            if (m0 + row < Mr && c0 + col < Nc) val = to_f32(V[(m0 + row) * ldv + c0 + col]);
           } else {
             col = a; row = b;
-            if (m0 + row < Mr && c0 + col < Nc) val = V[(c0 + col) * ldv + m0 + row];
+            if (m0 + row < Mr && c0 + col < Nc) val = to_f32(V[(c0 + col) * ldv + m0 + row]);
           }
           Ps[row * kLd + col] = val;
         }
@@ -187,13 +187,13 @@ simt_contract_kernel(const float* __restrict__ V, int64_t ldv, const float* __re
   }
 }
 
-template <int RB, bool TRANS>
-int launch_contract_mode(int mode, dim3 grid, size_t smem, cudaStream_t st, const float* V, int64_t ldv,
+template <int RB, bool TRANS, typename TV>
+int launch_contract_mode(int mode, dim3 grid, size_t smem, cudaStream_t st, const TV* V, int64_t ldv,
                          const float* F, const float* G, int64_t Mr, int64_t Nc, int R, float bm2, float bm1,
                          int nchunks, float* num, float* den, int64_t ldp, int64_t chunk_stride) {
 #define NMF_LAUNCH_MODE(M)                                                                              \
   {                                                                                                     \
-    auto kern = simt_contract_kernel<RB, TRANS, M>;                                                     \
+    auto kern = simt_contract_kernel<RB, TRANS, M, TV>;                                                 \
     NMF_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
     kern<<<grid, 256, smem, st>>>(V, ldv, F, G, Mr, Nc, R, bm2, bm1, nchunks, num, den, ldp,            \
                                   chunk_stride);                                                        \
@@ -209,17 +209,17 @@ int launch_contract_mode(int mode, dim3 grid, size_t smem, cudaStream_t st, cons
   return 0;
 }
 
-template <int RB>
-int launch_contract_rb(int trans, int mode, dim3 grid, cudaStream_t st, const float* V, int64_t ldv,
+template <int RB, typename TV>
+int launch_contract_rb(int trans, int mode, dim3 grid, cudaStream_t st, const TV* V, int64_t ldv,
                        const float* F, const float* G, int64_t Mr, int64_t Nc, int R, float bm2, float bm1,
                        int nchunks, float* num, float* den, int64_t ldp, int64_t chunk_stride) {
   const int Rp = 16 * RB;
   size_t smem = (size_t)(2 * Rp + kTile * (mode == kKL ? 1 : 2)) * kLd * sizeof(float);
   if (trans)
-    return launch_contract_mode<RB, true>(mode, grid, smem, st, V, ldv, F, G, Mr, Nc, R, bm2, bm1, nchunks,
-                                          num, den, ldp, chunk_stride);
-  return launch_contract_mode<RB, false>(mode, grid, smem, st, V, ldv, F, G, Mr, Nc, R, bm2, bm1, nchunks, num,
-                                         den, ldp, chunk_stride);
+    return launch_contract_mode<RB, true, TV>(mode, grid, smem, st, V, ldv, F, G, Mr, Nc, R, bm2, bm1, nchunks,
+                                              num, den, ldp, chunk_stride);
+  return launch_contract_mode<RB, false, TV>(mode, grid, smem, st, V, ldv, F, G, Mr, Nc, R, bm2, bm1, nchunks, num,
+                                             den, ldp, chunk_stride);
 }
 
 // ---- loss ------------------------------------------------------------------------------------
@@ -256,9 +256,9 @@ __device__ __forceinline__ double block_reduce_sum(double v, double* sh) {
   return t;   // valid in warp 0
 }
 
-template <int MODE>
+template <int MODE, typename TV>
 __global__ void __launch_bounds__(256)
-simt_loss_kernel(const float* __restrict__ V, int64_t ldv, const float* __restrict__ F,
+simt_loss_kernel(const TV* __restrict__ V, int64_t ldv, const float* __restrict__ F,
                  const float* __restrict__ G, int64_t Mr, int64_t Nc, int R, int Rp, float beta, int nchunks,
                  double* __restrict__ block_partials) {
   extern __shared__ __align__(16) float smem[];
@@ -298,7 +298,7 @@ simt_loss_kernel(const float* __restrict__ V, int64_t ldv, const float* __restri
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
         int64_t col = c0 + 4 * tx + j;
-        if (row < Mr && col < Nc) local += loss_term<MODE>(V[row * ldv + col], s[i][j], beta);
+        if (row < Mr && col < Nc) local += loss_term<MODE>(to_f32(V[row * ldv + col]), s[i][j], beta);
       }
     }
     acc += (double)local;
@@ -342,27 +342,31 @@ int sum_partials(const double* p, int n, double* out, cudaStream_t st) {
   return 0;
 }
 
-int simt_nmf_contract(const float* V, int64_t ldv, int trans, const float* F, const float* G, int64_t Mr,
+int simt_nmf_contract(const void* V, int vdtype, int64_t ldv, int trans, const float* F, const float* G, int64_t Mr,
                       int64_t Nc, int R, double beta, int nchunks, float* num, float* den, int64_t ldp,
                       int64_t chunk_stride, cudaStream_t st) {
   if (R < 1) { set_error("simt_nmf_contract: rank must be positive"); return 1; }
   int mode = beta_mode(beta);
   float bm2 = (float)(beta - 2.0), bm1 = (float)(beta - 1.0);
   dim3 grid((unsigned)ceil_div(Mr, kTile), (unsigned)nchunks, (unsigned)simt_rank_blocks(R));
-#define NMF_RB(RBV)                                                                                       \
-  return launch_contract_rb<RBV>(trans, mode, grid, st, V, ldv, F, G, Mr, Nc, R, bm2, bm1, nchunks, num, den, \
-                                 ldp, chunk_stride)
-  switch (contract_rb(R)) {
-    case 1: NMF_RB(1);
-    case 2: NMF_RB(2);
-    case 4: NMF_RB(4);
-    case 8: NMF_RB(8);
-    default: NMF_RB(16);
-  }
+  const int rb = contract_rb(R);
+  return with_vtype(V, vdtype, [&](auto Vt) {
+    using TV = vtype_t<decltype(Vt)>;
+#define NMF_RB(RBV)                                                                                            \
+  return launch_contract_rb<RBV, TV>(trans, mode, grid, st, Vt, ldv, F, G, Mr, Nc, R, bm2, bm1, nchunks, num, den, \
+                                     ldp, chunk_stride)
+    switch (rb) {
+      case 1: NMF_RB(1);
+      case 2: NMF_RB(2);
+      case 4: NMF_RB(4);
+      case 8: NMF_RB(8);
+      default: NMF_RB(16);
+    }
 #undef NMF_RB
+  });
 }
 
-int simt_nmf_loss(const float* V, int64_t ldv, const float* F, const float* G, int64_t Mr, int64_t Nc, int R,
+int simt_nmf_loss(const void* V, int vdtype, int64_t ldv, const float* F, const float* G, int64_t Mr, int64_t Nc, int R,
                   double beta, double* block_partials, int max_blocks, double* loss_dev, cudaStream_t st) {
   if (R < 1) { set_error("simt_nmf_loss: rank must be positive"); return 1; }
   int nchunks = loss_chunks(Mr, Nc);
@@ -372,20 +376,25 @@ int simt_nmf_loss(const float* V, int64_t ldv, const float* F, const float* G, i
   int Rp = (int)round_up(R < 256 ? R : 256, 16);
   size_t smem = (size_t)2 * Rp * kLd * sizeof(float);
   int mode = beta_mode(beta);
+  int rc = with_vtype(V, vdtype, [&](auto Vt) {
+    using TV = vtype_t<decltype(Vt)>;
 #define NMF_LOSS(M)                                                                                     \
   {                                                                                                     \
-    auto kern = simt_loss_kernel<M>;                                                                    \
+    auto kern = simt_loss_kernel<M, TV>;                                                                \
     NMF_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-    kern<<<grid, 256, smem, st>>>(V, ldv, F, G, Mr, Nc, R, Rp, (float)beta, nchunks, block_partials);   \
+    kern<<<grid, 256, smem, st>>>(Vt, ldv, F, G, Mr, Nc, R, Rp, (float)beta, nchunks, block_partials);  \
   }
-  switch (mode) {
-    case kKL: NMF_LOSS(kKL); break;
-    case kEU: NMF_LOSS(kEU); break;
-    case kIS: NMF_LOSS(kIS); break;
-    default: NMF_LOSS(kGeneric); break;
-  }
+    switch (mode) {
+      case kKL: NMF_LOSS(kKL); break;
+      case kEU: NMF_LOSS(kEU); break;
+      case kIS: NMF_LOSS(kIS); break;
+      default: NMF_LOSS(kGeneric); break;
+    }
 #undef NMF_LOSS
-  NMF_LAUNCH_CHECK();
+    NMF_LAUNCH_CHECK();
+    return 0;
+  });
+  if (rc) return rc;
   return sum_partials(block_partials, nblocks, loss_dev, st);
 }
 

@@ -438,10 +438,11 @@ __device__ __forceinline__ double block_sum256(double v, double* sh) {
   return t;     // valid in warp 0
 }
 
-// V (N x C fp32, ld) -> V16 (N x ldc) and Vt16 (C x ldn), both scaled by 2^exps[0]; 64x64 tiles.
+// V (N x C fp32 / fp16 / bf16, ld) -> V16 (N x ldc) and Vt16 (C x ldn), both scaled by 2^exps[0]; 64x64 tiles.
 // Also per-block partial sums of V and V*log(V+eps) (the V-only terms of metrics.kl_div, metrics.py:22).
+template <typename TV>
 __global__ void __launch_bounds__(256)
-v_to_f16_kernel(const float* __restrict__ V, int64_t ldv, int N, int C, __half* __restrict__ V16, int64_t ldc,
+v_to_f16_kernel(const TV* __restrict__ V, int64_t ldv, int N, int C, __half* __restrict__ V16, int64_t ldc,
                 __half* __restrict__ Vt16, int64_t ldn, const int* __restrict__ exps, double* __restrict__ vpart,
                 unsigned long long* __restrict__ lossy) {
   __shared__ float tile[64][65];
@@ -453,7 +454,7 @@ v_to_f16_kernel(const float* __restrict__ V, int64_t ldv, int N, int C, __half* 
   for (int idx = threadIdx.x; idx < 64 * 64; idx += 256) {
     int r = idx >> 6, c = idx & 63;
     const bool in = n0 + r < N && c0 + c < C;
-    const float raw = in ? V[(int64_t)(n0 + r) * ldv + c0 + c] : 0.f;
+    const float raw = in ? to_f32(V[(int64_t)(n0 + r) * ldv + c0 + c]) : 0.f;
     const float v = raw * sc;
     tile[r][c] = v;
     if (in) {
@@ -1153,15 +1154,16 @@ __global__ void tc_loss_final_beta_kernel(const double* __restrict__ part, int n
 }
 
 // V-only loss term: beta == 0: sum ln(V + eps); else sum t^beta with t = V (+ eps if beta < 0).  Two-level, fixed order.
+template <typename TV>
 __global__ void __launch_bounds__(256)
-v_beta_term_kernel(const float* __restrict__ V, int64_t rows, int64_t cols, int64_t ld, float beta,
+v_beta_term_kernel(const TV* __restrict__ V, int64_t rows, int64_t cols, int64_t ld, float beta,
                    double* __restrict__ blockpart) {
   __shared__ double red[8];
   double acc = 0.0;
   const int64_t total = rows * cols;
   for (int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x; i < total; i += (int64_t)gridDim.x * 256) {
     const int64_t r = i / cols, c = i - r * cols;
-    const float v = V[r * ld + c];
+    const float v = to_f32(V[r * ld + c]);
     acc += (double)(beta == 0.f ? logf(v + kEps) : powf(beta < 0.f ? v + kEps : v, beta));
   }
   const double t = block_sum256(acc, red);
@@ -1267,7 +1269,8 @@ struct TcState {
   unsigned long long* vlossy = nullptr;   // positive target entries the scaled fp16 copy cannot hold at full precision
   double* loss_part = nullptr;      // [num_sms][2]
   bool w_pending = false;           // tc_loss_prefetch_w: the W update's partial numerators of the CURRENT factors are in `part`
-  const float* Vsrc = nullptr;      // the registered fp32 target (borrowed) for the V-only loss terms
+  const void* Vsrc = nullptr;       // the registered target (borrowed, VDtype vdtype) for the V-only loss terms
+  int vdtype = kVF32;
   int64_t ldv = 0;
   double* vbeta = nullptr;          // device: V-only loss term of beta `vbeta_for`
   double* vbeta_part = nullptr;     // [1024]
@@ -1390,19 +1393,23 @@ bool tc_supports_beta(const TcState* s, double beta) {
 }
 bool tc_supports_partial(const TcState* s, double beta) { return beta != 2.0 && tc_supports_beta(s, beta); }
 
-int tc_set_target(TcState* s, const float* V, int64_t ldv, const float* minmax_dev, cudaStream_t st) {
+int tc_set_target(TcState* s, const void* V, int vdtype, int64_t ldv, const float* minmax_dev, cudaStream_t st) {
   s->w_pending = false;
   set_vexp_kernel<<<1, 32, 0, st>>>(minmax_dev, s->exps);
   NMF_LAUNCH_CHECK();
   dim3 grid((unsigned)ceil_div(s->C, 64), (unsigned)ceil_div(s->N, 64));
   NMF_CUDA_CHECK(cudaMemsetAsync(s->vlossy, 0, sizeof(unsigned long long), st));
-  v_to_f16_kernel<<<grid, 256, 0, st>>>(V, ldv, (int)s->N, (int)s->C, s->V16, s->ldc, s->Vt16, s->ldn, s->exps,
-                                        s->vpart, s->vlossy);
-  NMF_LAUNCH_CHECK();
+  int rc = with_vtype(V, vdtype, [&](auto Vt) {
+    v_to_f16_kernel<<<grid, 256, 0, st>>>(Vt, ldv, (int)s->N, (int)s->C, s->V16, s->ldc, s->Vt16, s->ldn, s->exps,
+                                          s->vpart, s->vlossy);
+    NMF_LAUNCH_CHECK();
+    return 0;
+  });
+  if (rc) return rc;
   reduce_vconst_kernel<<<1, 256, 0, st>>>(s->vpart, s->vblocks, s->vconst);
   NMF_LAUNCH_CHECK();
   s->has_target = true;
-  s->Vsrc = V; s->ldv = ldv; s->vbeta_for = 1.0;
+  s->Vsrc = V; s->vdtype = vdtype; s->ldv = ldv; s->vbeta_for = 1.0;
   s->dirty_w = s->dirty_h = true;      // exps[3] depends on sum(V)
   return 0;
 }
@@ -1827,8 +1834,12 @@ int tc_loss(TcState* s, const float* W, const float* H, double beta, double* los
     return 0;
   }
   if (beta != 2.0 && s->vbeta_for != beta) {      // V-only term of this beta, once per (target, beta)
-    v_beta_term_kernel<<<1024, 256, 0, st>>>(s->Vsrc, s->N, s->C, s->ldv, (float)beta, s->vbeta_part);
-    NMF_LAUNCH_CHECK();
+    rc = with_vtype(s->Vsrc, s->vdtype, [&](auto Vt) {
+      v_beta_term_kernel<<<1024, 256, 0, st>>>(Vt, s->N, s->C, s->ldv, (float)beta, s->vbeta_part);
+      NMF_LAUNCH_CHECK();
+      return 0;
+    });
+    if (rc) return rc;
     sum_blocks_kernel<<<1, 256, 0, st>>>(s->vbeta_part, 1024, s->vbeta);
     NMF_LAUNCH_CHECK();
     s->vbeta_for = beta;

@@ -13,8 +13,9 @@ void tc_destroy(TcState* s);
 bool tc_supports_beta(const TcState* s, double beta);
 // row-sharded partials: beta 2 keeps the fp32 contraction (its numerator needs the Gram matrix of the global H)
 bool tc_supports_partial(const TcState* s, double beta);
-// minmax_dev: device float[2] = {min(V), max(V)} already queued on `st`
-int tc_set_target(TcState* s, const float* V, int64_t ldv, const float* minmax_dev, cudaStream_t st);
+// V: `vdtype` (VDtype) elements, borrowed until the next call; minmax_dev: device float[2] = {min(V), max(V)} already
+// queued on `st`
+int tc_set_target(TcState* s, const void* V, int vdtype, int64_t ldv, const float* minmax_dev, cudaStream_t st);
 // number of positive target entries that the scaled fp16 copy holds only as subnormals / zero (synchronises `st`)
 int tc_target_lossy(TcState* s, unsigned long long* count, cudaStream_t st);
 // sum of the registered target (synchronises `st`)

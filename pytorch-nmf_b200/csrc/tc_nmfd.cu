@@ -48,7 +48,7 @@ struct NmfdTcParams {
   const __half* Hp16;             // [B*R][Lp]
   const __half* P16;              // [B*C][Lq]      (wgrad / dgrad source)
   __half* P16out;                 // recon output
-  const float* V;                 // [B][C][L] fp32
+  const float* V;                 // [B][C][L] of TV elements: the kernel reads it as const TV* (TV: its template parameter)
   const int* exps;                // {eW, eH, eP}: power-of-two exponents of W16, Hp16, P16
   const float* kappa;             // device scalar
   float* out;                     // wgrad: [nsplit][C][R][T]   dgrad: [nsplit][B][R][Lin]
@@ -85,7 +85,8 @@ __device__ __forceinline__ void bulk_copy_g2s(uint32_t dst, const void* src, uin
 //                        one block of 128 shifts), N = 128
 //   dgrad              : grid (Lin tiles, nsplit, batch slice); Toeplitz = A (rows j), plain = B = Wf16 rows (c R + r_off + n), N = 128;
 //                        ranks above 128 take one launch per 128 components
-template <int KIND>
+// TV: the target's element type (recon / recon-loss only; wgrad and dgrad read no V and take float)
+template <int KIND, typename TV>
 __global__ void __launch_bounds__(kThreads, 1)
 tcnmfd_kernel(const __grid_constant__ CUtensorMap tmPlain, const NmfdTcParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -235,7 +236,7 @@ tcnmfd_kernel(const __grid_constant__ CUtensorMap tmPlain, const NmfdTcParams p)
         const int c = blockIdx.y * kM + r128, b = bz, l0 = blockIdx.x * kM;
         const bool row_ok = c < p.C;
         const float kap = *p.kappa, pscale = exp2f((float)p.exps[2]);
-        const float* vrow = p.V + ((int64_t)b * p.C + (row_ok ? c : 0)) * p.L;
+        const TV* vrow = reinterpret_cast<const TV*>(p.V) + ((int64_t)b * p.C + (row_ok ? c : 0)) * p.L;
         __half* prow = p.P16out + ((int64_t)b * p.C + (row_ok ? c : 0)) * p.Lq;
         double acc = 0.0;
 #pragma unroll 1
@@ -245,7 +246,7 @@ tcnmfd_kernel(const __grid_constant__ CUtensorMap tmPlain, const NmfdTcParams p)
           const int l = l0 + j * 16;
           float v[16];
 #pragma unroll
-          for (int i = 0; i < 16; ++i) v[i] = (row_ok && l + i < p.L) ? vrow[l + i] : 0.f;
+          for (int i = 0; i < 16; ++i) v[i] = (row_ok && l + i < p.L) ? to_f32(vrow[l + i]) : 0.f;
           if (KIND == kReconLoss) {
             float a = 0.f;
 #pragma unroll
@@ -456,11 +457,12 @@ prep_h_kernel(const float* __restrict__ H, int Lin, int Lp, int padl, int nch, c
   }
 }
 
+template <typename TV>
 __global__ void __launch_bounds__(256)
-vsum_kernel(const float* __restrict__ V, int64_t n, double* __restrict__ part) {
+vsum_kernel(const TV* __restrict__ V, int64_t n, double* __restrict__ part) {
   __shared__ double sh[8];
   double a = 0.0;
-  for (int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x; i < n; i += (int64_t)gridDim.x * 256) a += (double)V[i];
+  for (int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x; i < n; i += (int64_t)gridDim.x * 256) a += (double)to_f32(V[i]);
   for (int o = 16; o > 0; o >>= 1) a += __shfl_xor_sync(0xffffffffu, a, o);
   if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = a;
   __syncthreads();
@@ -620,11 +622,15 @@ int tc_nmfd_create(TcNmfdState** out, const NmfdShape& d) {
   return 0;
 }
 
-int tc_nmfd_set_target(TcNmfdState* s, const float* V, double* vsum_host, cudaStream_t st) {
+int tc_nmfd_set_target(TcNmfdState* s, const void* V, int vdtype, double* vsum_host, cudaStream_t st) {
   const int64_t n = (int64_t)s->d.B * s->d.C * s->d.L;
-  vsum_kernel<<<256, 256, 0, st>>>(V, n, s->vsum + 1);
-  NMF_LAUNCH_CHECK();
-  int rc = sum_partials(s->vsum + 1, 256, s->vsum, st);
+  int rc = with_vtype(V, vdtype, [&](auto Vt) {
+    vsum_kernel<<<256, 256, 0, st>>>(Vt, n, s->vsum + 1);
+    NMF_LAUNCH_CHECK();
+    return 0;
+  });
+  if (rc) return rc;
+  rc = sum_partials(s->vsum + 1, 256, s->vsum, st);
   if (rc) return rc;
   NMF_CUDA_CHECK(cudaMemcpyAsync(vsum_host, s->vsum, sizeof(double), cudaMemcpyDeviceToHost, st));
   NMF_CUDA_CHECK(cudaStreamSynchronize(st));
@@ -635,9 +641,9 @@ namespace {
 
 dim3 dim3_of(const Grid3& g) { return dim3((unsigned)g.x, (unsigned)g.y, (unsigned)g.z); }
 
-template <int KIND>
+template <int KIND, typename TV = float>
 int launch(TcNmfdState* s, const CUtensorMap& tm, dim3 grid, const NmfdTcParams& p, cudaStream_t st) {
-  auto kern = tcnmfd_kernel<KIND>;
+  auto kern = tcnmfd_kernel<KIND, TV>;
   static unsigned long long attr_set_mask = 0;      // per device (one bit each): the attribute is per-device state
   const int smem = Smem::kTotal + 1024;
   int dev = 0;
@@ -652,22 +658,23 @@ int launch(TcNmfdState* s, const CUtensorMap& tm, dim3 grid, const NmfdTcParams&
 }
 
 // recon / dgrad: one launch per slice of at most plan.bslice batch elements (grid.z), batch offset b0
-template <int KIND>
+template <int KIND, typename TV = float>
 int launch_slices(TcNmfdState* s, const CUtensorMap& tm, const Grid3& g, NmfdTcParams p, cudaStream_t st) {
   for (int64_t b0 = 0; b0 < s->d.B; b0 += g.z) {
     p.b0 = (int)b0;
     dim3 grid = dim3_of(g);
     grid.z = (unsigned)std::min<int64_t>(g.z, s->d.B - b0);
-    if (int rc = launch<KIND>(s, tm, grid, p, st)) return rc;
+    if (int rc = launch<KIND, TV>(s, tm, grid, p, st)) return rc;
   }
   return 0;
 }
 
-NmfdTcParams base_params(TcNmfdState* s, const float* V) {
+NmfdTcParams base_params(TcNmfdState* s, const void* V) {
   NmfdTcParams p{};
   p.B = s->d.B; p.C = s->d.C; p.L = s->d.L; p.R = s->d.R; p.T = s->d.T; p.Lin = s->d.Lin; p.Tp = s->Tp;
   p.Lp = s->Lp; p.padl = s->padl; p.Lq = s->Lq;
-  p.Hp16 = s->Hp16; p.P16 = s->P16; p.P16out = s->P16; p.V = V; p.exps = s->exps; p.kappa = s->kappa;
+  p.Hp16 = s->Hp16; p.P16 = s->P16; p.P16out = s->P16; p.exps = s->exps; p.kappa = s->kappa;
+  p.V = static_cast<const float*>(V);
   p.out = s->part; p.loss_part = s->loss_part; p.nsplit = 1; p.kb_per_split = 0;
   return p;
 }
@@ -718,17 +725,18 @@ int refresh(TcNmfdState* s, const float* W, const float* H, cudaStream_t st) {
 
 }  // namespace
 
-int tc_nmfd_recon(TcNmfdState* s, const float* V, const float* W, const float* H, bool loss, double* loss_dev,
+int tc_nmfd_recon(TcNmfdState* s, const void* V, int vdtype, const float* W, const float* H, bool loss, double* loss_dev,
                   cudaStream_t st) {
   int rc = refresh(s, W, H, st);
   if (rc) return rc;
-  NmfdTcParams p = base_params(s, V);
-  if (loss) {
-    rc = launch_slices<kReconLoss>(s, s->tmWr, s->plan.recon, p, st);
-    if (rc) return rc;
-    return sum_partials(s->loss_part, s->loss_blocks, loss_dev, st);
-  }
-  return launch_slices<kRecon>(s, s->tmWr, s->plan.recon, p, st);
+  const NmfdTcParams p = base_params(s, V);
+  rc = with_vtype(V, vdtype, [&](auto Vt) {
+    using TV = vtype_t<decltype(Vt)>;
+    return loss ? launch_slices<kReconLoss, TV>(s, s->tmWr, s->plan.recon, p, st)
+                : launch_slices<kRecon, TV>(s, s->tmWr, s->plan.recon, p, st);
+  });
+  if (rc || !loss) return rc;
+  return sum_partials(s->loss_part, s->loss_blocks, loss_dev, st);
 }
 
 // numerator partials of the W update from the P16 written by the last recon: [*nsplit][C][R][T] fp32

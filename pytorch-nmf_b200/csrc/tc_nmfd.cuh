@@ -23,12 +23,12 @@ const char* tc_nmfd_plan(const NmfdShape& d, TcNmfdPlan* p);
 bool tc_nmfd_supported(const NmfdShape& d, double beta);
 int tc_nmfd_create(TcNmfdState** out, const NmfdShape& d);
 void tc_nmfd_destroy(TcNmfdState* s);
-// sum(V) for the centring constant kappa (also returned to the host: synchronises `st`)
-int tc_nmfd_set_target(TcNmfdState* s, const float* V, double* vsum_host, cudaStream_t st);
+// sum(V) for the centring constant kappa (also returned to the host: synchronises `st`); V holds `vdtype` (VDtype) elements
+int tc_nmfd_set_target(TcNmfdState* s, const void* V, int vdtype, double* vsum_host, cudaStream_t st);
 // brings the fp16 operand copies / column sums / kappa up to date with whichever factor changed since the last call, then
 // either writes the centred ratio tile (V / (WH + eps) - kappa) 2^p for the following wgrad / dgrad, or (loss) reduces
 // metrics.kl_div
-int tc_nmfd_recon(TcNmfdState* s, const float* V, const float* W, const float* H, bool loss, double* loss_dev,
+int tc_nmfd_recon(TcNmfdState* s, const void* V, int vdtype, const float* W, const float* H, bool loss, double* loss_dev,
                   cudaStream_t st);
 // split-K partial numerators from the ratio tile of the last recon: W side [nsplit][C][R][T], H side [nsplit][B][R][Lin]
 // (without the kappa * colsum term, which the ratio stage adds: ApplyArgs::kappa / kappa_vec)

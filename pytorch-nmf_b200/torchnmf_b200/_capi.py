@@ -7,12 +7,18 @@ There is NO fallback: if the library is missing or fails to load, every product 
 import ctypes
 import os
 
+import torch
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("NMFB200_LIB") or os.path.join(os.path.dirname(_HERE), "lib", "libnmf_b200.so")   # override: tuning builds
 
 PREC_AUTO, PREC_F32, PREC_F16, PREC_F16_SPLIT = -1, 0, 1, 2
 PRECISIONS = {"auto": PREC_AUTO, "f32": PREC_F32, "f16": PREC_F16, "f16_split": PREC_F16_SPLIT}
 PRECISION_NAMES = {v: k for k, v in PRECISIONS.items()}
+
+# element types a dense target may have (NMFB200_DTYPE_*); the factors are always fp32
+DTYPE_F32, DTYPE_F16, DTYPE_BF16 = 0, 1, 2
+DTYPES = {torch.float32: DTYPE_F32, torch.float16: DTYPE_F16, torch.bfloat16: DTYPE_BF16}
 
 _c = ctypes
 _vp, _i64, _dbl, _int = _c.c_void_p, _c.c_int64, _c.c_double, _c.c_int
@@ -30,6 +36,7 @@ SIGNATURES = {
     "nmfb200_precision": (_int, [_vp]),
     "nmfb200_precision_for_beta": (_int, [_vp, _dbl]),
     "nmfb200_nmf_set_target": (_int, [_vp, _vp, _i64, _vp]),
+    "nmfb200_nmf_set_target_typed": (_int, [_vp, _vp, _i64, _int, _vp]),
     "nmfb200_target_minmax": (_int, [_vp, _c.POINTER(_c.c_float), _c.POINTER(_c.c_float), _vp]),
     "nmfb200_nmf_sync_factors": (_int, [_vp, _vp, _vp, _vp]),
     "nmfb200_nmf_update_w": (_int, [_vp, _vp, _vp, _dbl, _dbl, _dbl, _dbl, _vp]),
@@ -53,6 +60,7 @@ SIGNATURES = {
     "nmfb200_nmfd_create": (_int, [_c.POINTER(_vp), _int, _i64, _i64, _i64, _i64, _i64, _int]),
     "nmfb200_nmfnd_create": (_int, [_c.POINTER(_vp), _int, _i64, _i64, _int, _c.POINTER(_i64), _i64, _c.POINTER(_i64), _int]),
     "nmfb200_nmfd_set_target": (_int, [_vp, _vp, _vp]),
+    "nmfb200_nmfd_set_target_typed": (_int, [_vp, _vp, _int, _vp]),
     "nmfb200_nmfd_update_w": (_int, [_vp, _vp, _vp, _dbl, _dbl, _dbl, _dbl, _vp]),
     "nmfb200_nmfd_update_h": (_int, [_vp, _vp, _vp, _dbl, _dbl, _dbl, _dbl, _vp]),
     "nmfb200_nmfd_loss": (_int, [_vp, _vp, _vp, _dbl, _vp, _vp]),

@@ -35,6 +35,18 @@ def _check_f32_cuda(t, name, device):
         raise ValueError(f"{name} must be contiguous")
 
 
+def _check_target(V, device, strided_rows=False):
+    """A dense target as the kernels read it: fp32, fp16 or bf16 (converted exactly where each element is loaded, so a
+    half-precision V gives the results of V.float() without an fp32 copy) on the engine's device, contiguous -- or, for
+    `strided_rows` (NMF), rows of unit column stride at a row stride >= the column count."""
+    if V.dtype not in _capi.DTYPES:
+        raise TypeError(f"V must be float32, float16 or bfloat16 (got {V.dtype})")
+    if V.device != device:
+        raise ValueError(f"V is on {V.device}, expected {device}")
+    if not (V.is_contiguous() or (strided_rows and V.stride(1) == 1 and V.stride(0) >= V.shape[1])):
+        raise ValueError("V must be contiguous" + (" or have unit column stride" if strided_rows else ""))
+
+
 # Engine workspaces (the fp16 operand copies of V are the size of V) are kept across fit() calls of the same
 # shape instead of being cudaMalloc'ed / cudaFree'd every time.  The memory is cudaMalloc'ed by the library, i.e. invisible
 # to torch's caching allocator, so the cache is bounded by BYTES (estimated from the shapes): at most
@@ -184,13 +196,15 @@ class _CudaEngine:
 
 
 class CudaNmfEngine(_CudaEngine):
-    """Dense NMF on one GPU: V (N,C), W (C,R), H (N,R), all fp32 CUDA tensors (W, H updated in place)."""
+    """Dense NMF on one GPU: V (N,C) fp32, fp16 or bf16 (rows may be strided), W (C,R) and H (N,R) fp32, all CUDA tensors
+    (W, H updated in place)."""
     kind = "nmf"
 
     def __init__(self, V, W, H, precision="auto"):
         super().__init__()
         self.device = W.device
-        for t, n in ((V, "V"), (W, "W"), (H, "H")):
+        _check_target(V, self.device, strided_rows=True)
+        for t, n in ((W, "W"), (H, "H")):
             _check_f32_cuda(t, n, self.device)
         N, C = V.shape
         R = W.shape[1]
@@ -201,7 +215,8 @@ class CudaNmfEngine(_CudaEngine):
         self._acquire(("nmf", dev_index, N, C, R, precision),
                       lambda ref: self._lib.nmfb200_nmf_create(ref, dev_index, N, C, R, _capi.PRECISIONS[precision]))
         self._loss = torch.zeros(1, dtype=torch.float64, device=self.device)
-        _capi.check(self._lib.nmfb200_nmf_set_target(self._ctx, _ptr(V), V.stride(0), _stream(self.device)))
+        _capi.check(self._lib.nmfb200_nmf_set_target_typed(self._ctx, _ptr(V), V.stride(0), _capi.DTYPES[V.dtype],
+                                                           _stream(self.device)))
         self.sync()
 
     def sync(self):
@@ -367,13 +382,15 @@ class CudaSparseNmfEngine(_CudaEngine):
 
 
 class CudaNmfdEngine(_CudaEngine):
-    """NMFD / NMF2D / NMF3D on one GPU: V (B,C,*X), W (C,R,*K), H (B,R,*(X-K+1)) over one to three convolved axes."""
+    """NMFD / NMF2D / NMF3D on one GPU: V (B,C,*X), W (C,R,*K), H (B,R,*(X-K+1)) over one to three convolved axes; V
+    contiguous fp32, fp16 or bf16, W and H contiguous fp32."""
     kind = "nmfd"
 
     def __init__(self, V, W, H, precision="auto"):
         super().__init__()
         self.device = W.device
-        for t, n in ((V, "V"), (W, "W"), (H, "H")):
+        _check_target(V, self.device)
+        for t, n in ((W, "W"), (H, "H")):
             _check_f32_cuda(t, n, self.device)
         B, C, *X = V.shape
         _, R, *K = W.shape
@@ -393,7 +410,7 @@ class CudaNmfdEngine(_CudaEngine):
                                                                 _capi.PRECISIONS[precision])
         self._acquire(("nmfd", dev_index, B, C, tuple(X), R, tuple(K), precision), create)
         self._loss = torch.zeros(1, dtype=torch.float64, device=self.device)
-        _capi.check(self._lib.nmfb200_nmfd_set_target(self._ctx, _ptr(V), _stream(self.device)))
+        _capi.check(self._lib.nmfb200_nmfd_set_target_typed(self._ctx, _ptr(V), _capi.DTYPES[V.dtype], _stream(self.device)))
 
     def sync(self):
         _capi.check(self._lib.nmfb200_nmfd_sync_factors(self._ctx))

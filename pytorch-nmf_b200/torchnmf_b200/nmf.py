@@ -162,10 +162,12 @@ class BaseComponent(torch.nn.Module):
     _engine_factory = None
     _sparse_targets = False       # NMF only (nmf.py:603-638); the convolutive models raise, as in the reference
     _sparse_kernels = True        # beta 1 / 2 on a sparse target: the library's sparse kernels (False: densify)
+    _strided_target = False       # the engine reads a row-strided (unit column stride) half-precision target as it is
 
     def _open_engine(self, V, beta, precision, group, sparse_kernels):
         """Shared entry of `fit` / `sparse_fit`: validation that needs no device pass, placement of V / W / H on the CUDA
-        device (host buffers and other dtypes are staged through fp32 device copies) and the engine for this target.
+        device (host buffers are copied there; a dense bf16 / fp16 target keeps its dtype, other target and factor dtypes are
+        staged through fp32 device copies) and the engine for this target.
         Returns (engine, W, H, Wd, Hd, staged): W / H the Parameters, Wd / Hd the fp32 device tensors the engine updates."""
         sparse_target = V.is_sparse
         if sparse_target and not self._sparse_targets:
@@ -197,7 +199,12 @@ class BaseComponent(torch.nn.Module):
             # the sparse-target kernels cover ranks up to 256; above, the target is densified like for other betas
             use_sparse_kernels = (sparse_kernels and sparse_target and beta in (1, 2) and group is None
                                   and self._sparse_kernels and W.shape[1] <= 256)
-            if not use_sparse_kernels:
+            if not sparse_target and Vd.dtype in (torch.float16, torch.bfloat16):
+                # the kernels convert each element exactly where they load it: the fit is bit for bit that of V.float(),
+                # without the fp32 copy (4 bytes per element of V)
+                if not (self._strided_target and Vd.stride(-1) == 1 and Vd.stride(0) >= Vd.shape[1]):
+                    Vd = Vd.contiguous()
+            elif not use_sparse_kernels:
                 Vd = (Vd.to_dense() if sparse_target else Vd).to(f32).contiguous()
             if on_gpu and W.dtype == f32 and H.dtype == f32:
                 Wd, Hd = W.data, H.data                       # updated in place, like param.data in the reference
@@ -232,8 +239,10 @@ class BaseComponent(torch.nn.Module):
                    (rows of V <-> rows of H) and W is replicated; one all-reduce per W update.
 
         dtype: the kernels keep fp32 master factors and fp32 accumulators.  The reference computes in the module's
-        dtype (nmf.py:214-218); here a float64 / half module (or target) is staged through fp32 copies and the result
-        is written back into the same Parameter storages in their own dtype.
+        dtype (nmf.py:214-218).  Here a dense bfloat16 / float16 target is read as it is, with no fp32 copy (NMF also
+        takes a row-strided view), and gives exactly the fit of `V.float()`; a float64 target is staged through an fp32
+        copy.  A float64 / half module is staged through fp32 copies and the result is written back into the same
+        Parameter storages in their own dtype.
         """
         eng, W, H, Wd, Hd, staged = self._open_engine(V, beta, precision, group, sparse_kernels=True)
 
@@ -392,6 +401,7 @@ class NMF(BaseComponent):
     """Non-negative matrix factorisation  V (N,C) ~= H (N,R) @ W (C,R)^T   (reference: nmf.py:641-697)."""
     _engine_cls = _engine.CudaNmfEngine
     _sparse_targets = True
+    _strided_target = True
 
     def __init__(self, Vshape=None, rank=None, **kwargs):
         if isinstance(Vshape, _Iterable):
