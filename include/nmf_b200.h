@@ -145,7 +145,8 @@ int nmfb200_nmf_w_partial(nmfb200_ctx* ctx, const float* W, const float* H, doub
  * torchnmf.plca (plca.py:252-253: the simultaneous W / H / Z updates from ONE V / (W Z H) ratio) are built from.
  * A sparse target (nmfb200_nmf_set_target_sparse) serves beta 1 and 2 with the same layout, from the same kernels as its
  * update: the numerator at the non-zeros only, the beta-2 denominator F (other^T other); any other beta returns
- * NMFB200_ERR_INVALID. */
+ * NMFB200_ERR_INVALID.  One set by nmfb200_nmf_set_target_sparse_any_beta also serves every other beta > 0 (2*rows*R floats:
+ * the numerator at the non-zeros, the V-free denominator equal bit for bit to a dense fp32 context's). */
 int64_t nmfb200_nmf_raw_terms_numel(const nmfb200_ctx* ctx, int which, double beta);
 int nmfb200_nmf_raw_terms(nmfb200_ctx* ctx, const float* W, const float* H, int which, double beta,
                           float* out, void* stream);
@@ -161,6 +162,18 @@ int nmfb200_nmf_w_apply(nmfb200_ctx* ctx, float* W, const float* reduced,
 int nmfb200_nmf_set_target_sparse(nmfb200_ctx* ctx, int64_t nnz, const int64_t* crow, const int64_t* col, const float* val,
                                   const int64_t* ccol, const int64_t* row, const float* val_t,
                                   double v_norm_kl, double v_norm_eu, void* stream);
+/* The same registration (same arguments and meaning, same refusals), on a context that then serves every beta > 0 without
+ * densifying V.  Beta 1 and 2 run exactly the kernels above.  Any other beta (x = w_c . h_n + eps, nmf.py:621-636):
+ *   numerators at the non-zeros only (num_H[n,:] = sum_{c in row n} v x^(beta-2) W[c,:], the W side over the columns);
+ *   denominators over all N x C cells but V-free (den_H[n,:] = sum_c x^(beta-1) W[c,:]): the fp32 contraction without the V
+ *   tile and the numerator GEMM, on the dense fp32 plan, so they equal a dense fp32 context's bit for bit;
+ *   loss = V_norm + sum_all x^beta / beta - sum_nnz v x^(beta-1) / (beta-1), V_norm = sum_nnz v^beta / (beta (beta-1)) taken
+ *   in the loss launch itself (v_norm_kl / v_norm_eu serve beta 1 / 2 only).
+ * Device memory stays O(nnz + (N + C) R).  beta <= 0 returns NMFB200_ERR_INVALID.  Every other set_target* on the context
+ * turns this off again. */
+int nmfb200_nmf_set_target_sparse_any_beta(nmfb200_ctx* ctx, int64_t nnz, const int64_t* crow, const int64_t* col,
+                                           const float* val, const int64_t* ccol, const int64_t* row, const float* val_t,
+                                           double v_norm_kl, double v_norm_eu, void* stream);
 
 /* Row-sharded W update over PEER MEMORY (ranks of one NVLink domain, one process per GPU, 2..8 ranks) -- the fused form of
  * w_partial -> all-reduce -> w_apply above, without a collective library call on the data path:

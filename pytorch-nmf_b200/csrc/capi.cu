@@ -42,6 +42,8 @@ struct nmfb200_ctx {
   float* mm_scratch = nullptr;    // 2048 + 2
   // sparse target (beta 1 / 2): borrowed CSR (rows of V) and CSC (= CSR of V^T) forms, V_norm of nmf.py:161-170
   bool sparse = false;
+  bool sp_any_beta = false;       // set by nmfb200_nmf_set_target_sparse_any_beta, reset by every other set_target
+  float* sp_den = nullptr;        // max(N, C) x R: the reduced V-free denominator of an update at beta != 1, 2
   const int64_t *sp_crow = nullptr, *sp_col = nullptr, *sp_ccol = nullptr, *sp_row = nullptr;
   const float *sp_val = nullptr, *sp_val_t = nullptr;
   double sp_vnorm_kl = 0.0, sp_vnorm_eu = 0.0;
@@ -113,7 +115,7 @@ void free_ctx(nmfb200_ctx* c) {
   if (c->tcd) tc_nmfd_destroy(c->tcd);
   cudaFree(c->num); cudaFree(c->den); cudaFree(c->colsum); cudaFree(c->cs_scratch);
   cudaFree(c->loss_blocks); cudaFree(c->mm_scratch); cudaFree(c->Pn); cudaFree(c->Pp);
-  cudaFree(c->sp_gram); cudaFree(c->sp_loss_part);
+  cudaFree(c->sp_gram); cudaFree(c->sp_loss_part); cudaFree(c->sp_den);
   delete c;
 }
 
@@ -296,7 +298,7 @@ int nmfb200_nmf_set_target_typed(nmfb200_ctx* ctx, const void* V, int64_t ldv, i
   if (!V || ldv < ctx->C) return fail(NMFB200_ERR_INVALID, "bad target pointer / leading dimension");
   if (int rc = check_target(V, dtype)) return rc;
   cudaStream_t st = (cudaStream_t)stream;
-  ctx->V = V; ctx->vdtype = dtype; ctx->ldv = ldv; ctx->has_target = true; ctx->sparse = false;
+  ctx->V = V; ctx->vdtype = dtype; ctx->ldv = ldv; ctx->has_target = true; ctx->sparse = false; ctx->sp_any_beta = false;
   int rc = matrix_minmax(V, dtype, ctx->N, ctx->C, ldv, ctx->mm_scratch, ctx->mm_scratch + 2048, st);
   if (rc) return rc;
   ctx->tc_off = false;
@@ -351,6 +353,21 @@ int nmfb200_nmf_set_target_sparse(nmfb200_ctx* ctx, int64_t nnz, const int64_t* 
   ctx->sp_crow = crow; ctx->sp_col = col; ctx->sp_val = val; ctx->sp_ccol = ccol; ctx->sp_row = row; ctx->sp_val_t = val_t;
   ctx->sp_vnorm_kl = v_norm_kl; ctx->sp_vnorm_eu = v_norm_eu;
   ctx->sparse = true; ctx->has_target = true; ctx->V = nullptr; ctx->tc_off = true;      // the dense kernels are out of play
+  ctx->sp_any_beta = false;
+  return 0;
+}
+
+int nmfb200_nmf_set_target_sparse_any_beta(nmfb200_ctx* ctx, int64_t nnz, const int64_t* crow, const int64_t* col,
+                                           const float* val, const int64_t* ccol, const int64_t* row, const float* val_t,
+                                           double v_norm_kl, double v_norm_eu, void* stream) {
+  int rc = nmfb200_nmf_set_target_sparse(ctx, nnz, crow, col, val, ccol, row, val_t, v_norm_kl, v_norm_eu, stream);
+  if (rc) return rc;
+  DeviceGuard guard(ctx->device);
+  if (!guard.ok) return fail(NMFB200_ERR_CUDA, "cannot select the context's device");
+  if ((rc = ensure_den(ctx))) return rc;
+  if (!ctx->sp_den)
+    NMF_CUDA_CHECK(cudaMalloc(&ctx->sp_den, (size_t)(ctx->N > ctx->C ? ctx->N : ctx->C) * ctx->R * sizeof(float)));
+  ctx->sp_any_beta = true;
   return 0;
 }
 
@@ -358,9 +375,18 @@ namespace {
 // Raw terms of one factor's update on the compressed form whose segments are that factor's rows (which = 0: W over CSC,
 // 1: H over CSR): the numerator (rows x R) into `num`; into `den` the colsum of the other factor (R, beta 1) or the raw
 // denominator F (other^T other) (rows x R, beta 2).  Shared by the update and nmfb200_nmf_raw_terms.
+// beta 1 and 2 run on every sparse context; any other beta > 0 only on one set by nmfb200_nmf_set_target_sparse_any_beta
+int check_sparse_beta(const nmfb200_ctx* ctx, double beta) {
+  if (beta == 1.0 || beta == 2.0) return 0;
+  if (!ctx->sp_any_beta)
+    return fail(NMFB200_ERR_INVALID, "sparse targets: beta must be 1 or 2 (densify the target for other beta)");
+  if (!(beta > 0.0)) return fail(NMFB200_ERR_INVALID, "sparse targets: beta must be positive");
+  return 0;
+}
+
 int sparse_terms(nmfb200_ctx* ctx, int which, const float* F, const float* other, double beta, float* num, float* den,
                  cudaStream_t st) {
-  if (beta != 1.0 && beta != 2.0) return fail(NMFB200_ERR_INVALID, "sparse targets: beta must be 1 or 2 (densify the target for other beta)");
+  if (int rc = check_sparse_beta(ctx, beta)) return rc;
   const int R = (int)ctx->R;
   const int64_t rows = which == 0 ? ctx->C : ctx->N, orows = which == 0 ? ctx->N : ctx->C;
   const int64_t* ptr = which == 0 ? ctx->sp_ccol : ctx->sp_crow;
@@ -368,6 +394,12 @@ int sparse_terms(nmfb200_ctx* ctx, int which, const float* F, const float* other
   const float* val = which == 0 ? ctx->sp_val_t : ctx->sp_val;
   int rc = sparse_numerator(ptr, idx, val, F, other, R, rows, beta, num, st);
   if (rc) return rc;
+  if (beta != 1.0 && beta != 2.0) {     // the V-free denominator on the dense fp32 plan, its chunks summed as the dense path does
+    const int nch = which == 0 ? ctx->nch_w : ctx->nch_h;
+    rc = simt_nmf_contract_den(F, other, rows, orows, R, beta, nch, ctx->den, ctx->R, rows * ctx->R, st);
+    if (rc) return rc;
+    return reduce_chunks(ctx->den, nch, rows * ctx->R, rows, R, ctx->R, den, st);
+  }
   if (beta == 1.0)                                             // colsum of the OTHER factor, nmf.py:122-131
     return factor_colsum(other, orows, R, 1, ctx->cs_scratch, ctx->cs_scratch_floats, den, st);
   float* G = ctx->sp_gram + (1 - which) * R * R;               // Gram matrix of the other factor
@@ -383,7 +415,8 @@ int sparse_update(nmfb200_ctx* ctx, int which, float* F, const float* other, dou
     int rc = ensure_den(ctx);
     if (rc) return rc;
   }
-  float* den = beta == 1.0 ? ctx->colsum + (1 - which) * ctx->R : ctx->den;
+  // beta 1: colsum; beta 2: the raw denominator; other beta: the chunk partials live in ctx->den, their sum goes to sp_den
+  float* den = beta == 1.0 ? ctx->colsum + (1 - which) * ctx->R : beta == 2.0 ? ctx->den : ctx->sp_den;
   int rc = sparse_terms(ctx, which, F, other, beta, ctx->num, den, st);
   if (rc) return rc;
   return apply_update(nmf_apply_args(ctx, which, F, beta, ctx->num, den, 1, 0, gamma, l1_reg, l2_reg), st);
@@ -432,8 +465,15 @@ int nmf_raw_terms(nmfb200_ctx* ctx, const float* W, const float* H, int which, d
 }
 
 int sparse_loss_ctx(nmfb200_ctx* ctx, const float* W, const float* H, double beta, double* loss_dev, cudaStream_t st) {
-  if (beta != 1.0 && beta != 2.0) return fail(NMFB200_ERR_INVALID, "sparse targets: beta must be 1 or 2");
+  if (int rc = check_sparse_beta(ctx, beta)) return rc;
   const int R = (int)ctx->R;
+  if (beta != 1.0 && beta != 2.0) {     // pos = sum x^beta over every cell without V, then V_norm - neg at the non-zeros
+    int npos = 0;
+    int rc = simt_nmf_pow_sum(H, W, ctx->N, ctx->C, R, beta, ctx->loss_blocks, ctx->loss_max_blocks, &npos, st);
+    if (rc) return rc;
+    return sparse_beta_loss(ctx->sp_crow, ctx->sp_col, ctx->sp_val, H, W, R, ctx->N, beta, ctx->loss_blocks, npos,
+                            ctx->sp_loss_part, loss_dev, st);
+  }
   const float *pa, *pb;
   int rc;
   if (beta == 1.0) {

@@ -95,6 +95,14 @@ int simt_nmf_loss(const void* V, int vdtype, int64_t ldv, const float* F, const 
                   int R, double beta, double* block_partials, int max_blocks, double* loss_dev,
                   cudaStream_t st);
 int simt_nmf_max_blocks(int64_t Mr, int64_t Nc);
+// The V-free pieces of a sparse target's update and loss at beta != 1, 2 (nmf.py:621-636):
+//   den[ch][m][r] = sum_{c in chunk ch} (S[m,c] + eps)^(beta-1) G[c,r]: simt_nmf_contract's denominator at this beta, bit for
+//   bit (same grid, chunks and arithmetic), without reading V; R <= 256.
+int simt_nmf_contract_den(const float* F, const float* G, int64_t Mr, int64_t Nc, int R, double beta, int nchunks,
+                          float* den, int64_t ldp, int64_t chunk_stride, cudaStream_t st);
+//   block_partials[*nblocks] of sum over every cell of (S + eps)^beta (fp32 terms, double block sums), on simt_nmf_loss's plan.
+int simt_nmf_pow_sum(const float* F, const float* G, int64_t Mr, int64_t Nc, int R, double beta, double* block_partials,
+                     int max_blocks, int* nblocks, cudaStream_t st);
 // Output blocks of 256 components of simt_nmf_contract (grid z): 1 up to rank 256, each block recomputes S over all ranks.
 int simt_rank_blocks(int R);
 // The tile plan of simt_nmf_contract (Mr rows, Nc contracted columns, `nchunks` chunks) and of simt_nmf_loss: the register
@@ -141,7 +149,8 @@ int hoyer_project(float* x, int64_t outer, int D, int64_t inner, const float* k1
                   unsigned char* zeroed_ws, cudaStream_t st);
 
 // sparse_nmf.cu ----------------------------------------------------------------------------
-// Sparse-target NMF for beta 1 and 2 (nmf.py:603-638): update terms at the non-zeros of V only, one warp per compressed segment.
+// Sparse-target NMF (nmf.py:603-638): update terms at the non-zeros of V only, one warp per compressed segment.  The numerator
+// of any beta > 0; the denominators of beta 1 (factor_colsum) and 2 (Gram) are below, of other beta simt_nmf_contract_den.
 int sparse_numerator(const int64_t* ptr, const int64_t* idx, const float* val, const float* Fself, const float* Fother,
                      int R, int64_t nseg, double beta, float* out, cudaStream_t st);
 int sparse_gram(const float* F, int64_t rows, int R, float* part, float* out, cudaStream_t st);          // out = F^T F (R x R)
@@ -150,6 +159,11 @@ int sparse_rows_times_gram(const float* F, const float* G, int64_t rows, int R, 
 int sparse_loss(const int64_t* crow, const int64_t* col, const float* val, const float* H, const float* W, int R, int64_t N,
                 double beta, const float* pos_a, const float* pos_b, double v_norm, double* loss_part, double* loss_dev,
                 cudaStream_t st);
+// beta != 1, 2 (the numerator: sparse_numerator): loss_dev = V_norm - neg from the gather over the CSR form + (sum of the npos
+// V-free pos_part from simt_nmf_pow_sum) / beta
+int sparse_beta_loss(const int64_t* crow, const int64_t* col, const float* val, const float* H, const float* W, int R,
+                     int64_t N, double beta, const double* pos_part, int npos, double* loss_part, double* loss_dev,
+                     cudaStream_t st);
 // launch plans (host only): rank floats per lane; blocks over nseg segments / rows (the loss: N, its partials); Gram rows per
 // block and blocks over `rows` rows; Gram passes of 4096 pairs
 int sparse_rpl(int R);

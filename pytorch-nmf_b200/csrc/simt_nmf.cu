@@ -12,6 +12,10 @@
 // runs last, so its G slice is still in Gs for GEMM-2.  S is recomputed once per output block: with nb = ceil(R / 256)
 // blocks the contraction does (nb + 1) / 2 (KL) or (nb + 2) / 3 (two outputs) times the minimal FLOPs.  With one block
 // (R <= 256) the kernel is the single-chunk kernel it always was: grid z = 1, F loaded once per CTA.
+//
+// kVFree (sparse targets at beta != 1, 2): the contraction forms only den += (S+eps)^(beta-1) G_tile and reads no V, with
+// kGeneric's plan, staging and arithmetic, so its den partials equal kGeneric's bit for bit whatever V holds; the loss sums
+// (S+eps)^beta over every cell, again without V.
 #include "common.cuh"
 
 namespace nmfb200 {
@@ -19,6 +23,7 @@ namespace nmfb200 {
 namespace {
 
 constexpr int kTile = 64;   // rows per CTA and columns per tile
+constexpr int kVFree = 4;   // MODE of the V-free kernels, beside BetaMode's kKL ... kGeneric
 constexpr int kLd = 68;     // padded shared-memory pitch (floats): float4-aligned, conflict-free
 
 // 64-column tiles per chunk of the contracted dimension; the last chunks may be short or hold no tile at all
@@ -78,12 +83,14 @@ simt_contract_kernel(const TV* __restrict__ V, int64_t ldv, const float* __restr
                      int nchunks, float* __restrict__ num, float* __restrict__ den, int64_t ldp,
                      int64_t chunk_stride) {
   constexpr int Rp = 16 * RB;
+  constexpr bool kDenOnly = (MODE == kVFree);
+  constexpr bool kNum = !kDenOnly;
   constexpr bool kTwo = (MODE != kKL);
   extern __shared__ __align__(16) float smem[];
   float* Fs = smem;                 // [Rp][kLd]  Fs[r][row]
   float* Gs = Fs + Rp * kLd;        // [Rp][kLd]  Gs[r][col]
   float* Ps = Gs + Rp * kLd;        // [64][kLd]  V tile, then Pn in place
-  float* Qs = Ps + kTile * kLd;     // [64][kLd]  Pp (kTwo only)
+  float* Qs = kDenOnly ? Ps : Ps + kTile * kLd;     // [64][kLd]  Pp (kTwo only; kVFree: in Ps's place)
 
   const int tid = threadIdx.x;
   const int tx = tid & 15, ty = tid >> 4;
@@ -118,7 +125,7 @@ simt_contract_kernel(const TV* __restrict__ V, int64_t ldv, const float* __restr
       __syncthreads();
       if (multi) stage_chunk(Fs, F, m0, Mr, R, k0, Rp, tid);
       stage_chunk(Gs, G, c0, Nc, R, k0, Rp, tid);
-      if (t == 0) {
+      if (kNum && t == 0) {
         for (int idx = tid; idx < kTile * kTile; idx += 256) {
           int a = idx >> 6, b = idx & 63;
           int row, col;
@@ -141,6 +148,16 @@ simt_contract_kernel(const TV* __restrict__ V, int64_t ldv, const float* __restr
     }
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
+      if (kDenOnly) {
+        float pp[4];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          float x = s[i][j] + kEps;        // phi<kGeneric>'s pp
+          pp[j] = powf(x, bm1);
+        }
+        *reinterpret_cast<float4*>(&Qs[(4 * ty + i) * kLd + 4 * tx]) = make_float4(pp[0], pp[1], pp[2], pp[3]);
+        continue;
+      }
       float4 v4 = *reinterpret_cast<const float4*>(&Ps[(4 * ty + i) * kLd + 4 * tx]);
       float vv[4] = {v4.x, v4.y, v4.z, v4.w}, pn[4], pp[4];
 #pragma unroll
@@ -156,7 +173,7 @@ simt_contract_kernel(const TV* __restrict__ V, int64_t ldv, const float* __restr
       float4 p[4], q[4];
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
-        p[i] = *reinterpret_cast<const float4*>(&Ps[(4 * ty + i) * kLd + c]);
+        if (kNum) p[i] = *reinterpret_cast<const float4*>(&Ps[(4 * ty + i) * kLd + c]);
         if (kTwo) q[i] = *reinterpret_cast<const float4*>(&Qs[(4 * ty + i) * kLd + c]);
       }
 #pragma unroll
@@ -164,7 +181,8 @@ simt_contract_kernel(const TV* __restrict__ V, int64_t ldv, const float* __restr
         float4 g = *reinterpret_cast<const float4*>(&Gs[(tx + 16 * k) * kLd + c]);
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
-          accn[i][k] = fmaf(p[i].x, g.x, fmaf(p[i].y, g.y, fmaf(p[i].z, g.z, fmaf(p[i].w, g.w, accn[i][k]))));
+          if (kNum)
+            accn[i][k] = fmaf(p[i].x, g.x, fmaf(p[i].y, g.y, fmaf(p[i].z, g.z, fmaf(p[i].w, g.w, accn[i][k]))));
           if (kTwo)
             accd[i][k] = fmaf(q[i].x, g.x, fmaf(q[i].y, g.y, fmaf(q[i].z, g.z, fmaf(q[i].w, g.w, accd[i][k]))));
         }
@@ -180,7 +198,7 @@ simt_contract_kernel(const TV* __restrict__ V, int64_t ldv, const float* __restr
     for (int k = 0; k < RB; ++k) {
       int r = ob * Rp + tx + 16 * k;
       if (r < R) {
-        num[chunk * chunk_stride + row * ldp + r] = accn[i][k];
+        if (kNum) num[chunk * chunk_stride + row * ldp + r] = accn[i][k];
         if (kTwo) den[chunk * chunk_stride + row * ldp + r] = accd[i][k];
       }
     }
@@ -298,7 +316,10 @@ simt_loss_kernel(const TV* __restrict__ V, int64_t ldv, const float* __restrict_
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
         int64_t col = c0 + 4 * tx + j;
-        if (row < Mr && col < Nc) local += loss_term<MODE>(to_f32(V[row * ldv + col]), s[i][j], beta);
+        if (row < Mr && col < Nc) {
+          if (MODE == kVFree) local += powf(s[i][j] + kEps, beta);       // nmf.py:635-636, before the division by beta
+          else local += loss_term<MODE>(to_f32(V[row * ldv + col]), s[i][j], beta);
+        }
       }
     }
     acc += (double)local;
@@ -396,6 +417,47 @@ int simt_nmf_loss(const void* V, int vdtype, int64_t ldv, const float* F, const 
   });
   if (rc) return rc;
   return sum_partials(block_partials, nblocks, loss_dev, st);
+}
+
+int simt_nmf_contract_den(const float* F, const float* G, int64_t Mr, int64_t Nc, int R, double beta, int nchunks,
+                          float* den, int64_t ldp, int64_t chunk_stride, cudaStream_t st) {
+  if (R < 1 || R > 256) { set_error("simt_nmf_contract_den: rank must be in [1, 256]"); return 1; }
+  const float bm1 = (float)(beta - 1.0);
+  const dim3 grid((unsigned)ceil_div(Mr, kTile), (unsigned)nchunks, 1u);
+  const int Rp = 16 * contract_rb(R);
+  const size_t smem = (size_t)(2 * Rp + kTile) * kLd * sizeof(float);     // Fs, Gs and the Pp tile
+#define NMF_DEN(RBV)                                                                                                 \
+  {                                                                                                                  \
+    auto kern = simt_contract_kernel<RBV, false, kVFree, float>;                                                     \
+    NMF_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));              \
+    kern<<<grid, 256, smem, st>>>(nullptr, 0, F, G, Mr, Nc, R, 0.f, bm1, nchunks, nullptr, den, ldp, chunk_stride); \
+  } break
+  switch (contract_rb(R)) {
+    case 1: NMF_DEN(1);
+    case 2: NMF_DEN(2);
+    case 4: NMF_DEN(4);
+    case 8: NMF_DEN(8);
+    default: NMF_DEN(16);
+  }
+#undef NMF_DEN
+  NMF_LAUNCH_CHECK();
+  return 0;
+}
+
+int simt_nmf_pow_sum(const float* F, const float* G, int64_t Mr, int64_t Nc, int R, double beta, double* block_partials,
+                     int max_blocks, int* nblocks, cudaStream_t st) {
+  if (R < 1) { set_error("simt_nmf_pow_sum: rank must be positive"); return 1; }
+  const int nchunks = loss_chunks(Mr, Nc);
+  const dim3 grid((unsigned)ceil_div(Mr, kTile), (unsigned)nchunks);
+  *nblocks = (int)(grid.x * grid.y);
+  if (*nblocks > max_blocks) { set_error("simt_nmf_pow_sum: partial buffer too small"); return 1; }
+  const int Rp = (int)round_up(R < 256 ? R : 256, 16);
+  const size_t smem = (size_t)2 * Rp * kLd * sizeof(float);
+  auto kern = simt_loss_kernel<kVFree, float>;
+  NMF_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  kern<<<grid, 256, smem, st>>>(nullptr, 0, F, G, Mr, Nc, R, Rp, (float)beta, nchunks, block_partials);
+  NMF_LAUNCH_CHECK();
+  return 0;
 }
 
 }  // namespace nmfb200

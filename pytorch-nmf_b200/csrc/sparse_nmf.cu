@@ -1,11 +1,16 @@
-// Sparse-target NMF (reference: nmf.py:603-638 `_nmf_sp_recon_beta_pos_neg`, :95-119 `_sp_double_backward_update`), beta 1 and 2:
-// the update terms touch WH only at the non-zeros of V (SDDMM) and never form the dense N x C product.
+// Sparse-target NMF (reference: nmf.py:603-638 `_nmf_sp_recon_beta_pos_neg`, :95-119 `_sp_double_backward_update`): the
+// numerators touch WH only at the non-zeros of V (SDDMM), and no kernel forms the dense N x C product.
 //
 //   beta 1:  num_H[n,:] = sum_{c in row n} v / (w_c . h_n + eps) * W[c,:]      den = colsum(W)                 nmf.py:617-619
 //            num_W[c,:] = sum_{n in col c} v / (w_c . h_n + eps) * H[n,:]      den = colsum(H)
 //            loss = V_norm + colsum(W) . colsum(H) - sum_nnz v log(w_c . h_n + eps)
 //   beta 2:  num_H = V W, den_H = H (W^T W);  num_W = V^T H, den_W = W (H^T H)                                 nmf.py:608-611
 //            loss = V_norm + 0.5 sum (H^T H o W^T W) - sum_nnz v (w_c . h_n)
+//   other beta > 0 (x = w_c . h_n + eps):                                                                  nmf.py:621-636
+//            num_H[n,:] = sum_{c in row n} v x^(beta-2) W[c,:]                den_H[n,:] = sum_c x^(beta-1) W[c,:] (all cells)
+//            loss = V_norm + sum_all x^beta / beta - sum_nnz v x^(beta-1) / (beta-1),  V_norm = sum_nnz v^beta / (beta (beta-1))
+//            The gathers here give the numerators and V_norm - neg; the V-free denominators and sum x^beta come from the fp32
+//            contraction and loss kernels (simt_nmf.cu, kVFree), which never read V.
 //
 // One warp owns one segment -- a row of the CSR form (H update) or a column of the CSC form (W update) -- keeps its own factor
 // row in registers, gathers the other factor's rows of its non-zeros (rank floats each, coalesced) and accumulates in fp32 in
@@ -16,14 +21,15 @@ namespace nmfb200 {
 
 namespace {
 
-enum SpMode : int { kSpKL = 0, kSpEU = 1, kSpKLLoss = 2, kSpEULoss = 3 };
+enum SpMode : int { kSpKL = 0, kSpEU = 1, kSpKLLoss = 2, kSpEULoss = 3, kSpBeta = 4, kSpBetaLoss = 5 };
 constexpr int kSpGramPass = 256 * 16;                 // Gram pairs per pass of sp_gram_part_kernel (16 per thread)
 
+// pa, pb, ca, cb: the beta constants of kSpBeta / kSpBetaLoss (unused by the other modes)
 template <int RPL, int MODE>
-__global__ void __launch_bounds__(256)
-sp_gather_kernel(const int64_t* __restrict__ ptr, const int64_t* __restrict__ idx, const float* __restrict__ val,
-                 const float* __restrict__ Fs, const float* __restrict__ Fo, int R, int64_t nseg, float* __restrict__ out,
-                 double* __restrict__ loss_part) {
+__device__ __forceinline__ void
+sp_gather(const int64_t* __restrict__ ptr, const int64_t* __restrict__ idx, const float* __restrict__ val,
+          const float* __restrict__ Fs, const float* __restrict__ Fo, int R, int64_t nseg, float* __restrict__ out,
+          double* __restrict__ loss_part, float pa, float pb, double ca, double cb) {
   const int lane = threadIdx.x & 31;
   const int64_t seg = (int64_t)blockIdx.x * 8 + (threadIdx.x >> 5);
   double lacc = 0.0;
@@ -59,13 +65,20 @@ sp_gather_kernel(const int64_t* __restrict__ ptr, const int64_t* __restrict__ id
       } else if (MODE == kSpEU) {
 #pragma unroll
         for (int k = 0; k < RPL; ++k) acc[k] = fmaf(v, w[k], acc[k]);
+      } else if (MODE == kSpBeta) {
+        const float ratio = v * powf(dot + kEps, pa);                 // pa = beta - 2: phi<kGeneric>'s pn at a stored entry
+#pragma unroll
+        for (int k = 0; k < RPL; ++k) acc[k] = fmaf(ratio, w[k], acc[k]);
+      } else if (MODE == kSpBetaLoss) {
+        // pa = beta, pb = beta - 1, ca = 1 / (beta (beta - 1)), cb = 1 / (beta - 1): V_norm's and neg's terms of this entry
+        lacc += (double)powf(v, pa) * ca - (double)(v * powf(dot + kEps, pb)) * cb;
       } else if (MODE == kSpKLLoss) {
         lacc += (double)(v * logf(dot + kEps));                      // nmf.py:619
       } else {
         lacc += (double)(v * dot);                                   // nmf.py:610
       }
     }
-    if (MODE == kSpKL || MODE == kSpEU) {
+    if (MODE == kSpKL || MODE == kSpEU || MODE == kSpBeta) {
 #pragma unroll
       for (int k = 0; k < RPL; ++k) {
         const int r = lane + 32 * k;
@@ -73,7 +86,7 @@ sp_gather_kernel(const int64_t* __restrict__ ptr, const int64_t* __restrict__ id
       }
     }
   }
-  if (MODE == kSpKLLoss || MODE == kSpEULoss) {
+  if (MODE == kSpKLLoss || MODE == kSpEULoss || MODE == kSpBetaLoss) {
     __shared__ double sh[8];
     if (lane == 0) sh[threadIdx.x >> 5] = lacc;       // every lane holds the same sum
     __syncthreads();
@@ -83,6 +96,23 @@ sp_gather_kernel(const int64_t* __restrict__ ptr, const int64_t* __restrict__ id
       loss_part[blockIdx.x] = t;
     }
   }
+}
+
+template <int RPL, int MODE>
+__global__ void __launch_bounds__(256)
+sp_gather_kernel(const int64_t* __restrict__ ptr, const int64_t* __restrict__ idx, const float* __restrict__ val,
+                 const float* __restrict__ Fs, const float* __restrict__ Fo, int R, int64_t nseg, float* __restrict__ out,
+                 double* __restrict__ loss_part) {
+  sp_gather<RPL, MODE>(ptr, idx, val, Fs, Fo, R, nseg, out, loss_part, 0.f, 0.f, 0.0, 0.0);
+}
+
+// the modes of beta != 1, 2, with their constants
+template <int RPL, int MODE>
+__global__ void __launch_bounds__(256)
+sp_gather_beta_kernel(const int64_t* __restrict__ ptr, const int64_t* __restrict__ idx, const float* __restrict__ val,
+                      const float* __restrict__ Fs, const float* __restrict__ Fo, int R, int64_t nseg, float* __restrict__ out,
+                      double* __restrict__ loss_part, float pa, float pb, double ca, double cb) {
+  sp_gather<RPL, MODE>(ptr, idx, val, Fs, Fo, R, nseg, out, loss_part, pa, pb, ca, cb);
 }
 
 // Gram matrix G = F^T F (R x R) of a (rows x R) factor: per-block slabs, then a fixed-order sum over the blocks
@@ -146,6 +176,25 @@ sp_rows_times_gram_kernel(const float* __restrict__ F, const float* __restrict__
   for (int k = 0; k < RPL; ++k) { const int r = lane + 32 * k; if (r < R) out[row * R + r] = acc[k]; }
 }
 
+// loss = (v_norm - neg) + pos / beta at beta != 1, 2: the gather's partials and the V-free sum x^beta's, each summed in a fixed
+// order (one block, strided per thread, then a fixed tree)
+__global__ void __launch_bounds__(256)
+sp_beta_loss_final_kernel(const double* __restrict__ vn_neg_part, int nvn, const double* __restrict__ pos_part, int npos,
+                          double beta, double* __restrict__ out) {
+  __shared__ double sa[256], sb[256];
+  double a = 0.0, b = 0.0;
+  for (int i = threadIdx.x; i < nvn; i += 256) a += vn_neg_part[i];
+  for (int i = threadIdx.x; i < npos; i += 256) b += pos_part[i];
+  sa[threadIdx.x] = a;
+  sb[threadIdx.x] = b;
+  __syncthreads();
+  for (int o = 128; o > 0; o >>= 1) {
+    if (threadIdx.x < o) { sa[threadIdx.x] += sa[threadIdx.x + o]; sb[threadIdx.x] += sb[threadIdx.x + o]; }
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) *out = sa[0] + sb[0] / beta;                 // nmf.py:635: pos /= beta
+}
+
 // loss = v_norm + pos - neg:  beta 1: pos = colsum(W) . colsum(H);  beta 2: pos = 0.5 sum(GW o GH)
 __global__ void sp_loss_final_kernel(const double* __restrict__ neg_part, int nparts, const float* __restrict__ a,
                                      const float* __restrict__ b, int n, double scale, double v_norm, double* __restrict__ out) {
@@ -177,13 +226,23 @@ namespace {
 
 template <int MODE>
 int launch_gather(const int64_t* ptr, const int64_t* idx, const float* val, const float* Fs, const float* Fo, int R,
-                  int64_t nseg, float* out, double* loss_part, cudaStream_t st) {
+                  int64_t nseg, float* out, double* loss_part, cudaStream_t st, float pa = 0.f, float pb = 0.f,
+                  double ca = 0.0, double cb = 0.0) {
   const unsigned grid = (unsigned)sparse_gather_blocks(nseg);
   const int rpl = sparse_rpl(R);
-  if (rpl <= 1) sp_gather_kernel<1, MODE><<<grid, 256, 0, st>>>(ptr, idx, val, Fs, Fo, R, nseg, out, loss_part);
-  else if (rpl <= 2) sp_gather_kernel<2, MODE><<<grid, 256, 0, st>>>(ptr, idx, val, Fs, Fo, R, nseg, out, loss_part);
-  else if (rpl <= 4) sp_gather_kernel<4, MODE><<<grid, 256, 0, st>>>(ptr, idx, val, Fs, Fo, R, nseg, out, loss_part);
-  else sp_gather_kernel<8, MODE><<<grid, 256, 0, st>>>(ptr, idx, val, Fs, Fo, R, nseg, out, loss_part);
+#define NMF_GATHER(RPLV)                                                                                           \
+  do {                                                                                                             \
+    if constexpr (MODE == kSpBeta || MODE == kSpBetaLoss)                                                          \
+      sp_gather_beta_kernel<RPLV, MODE><<<grid, 256, 0, st>>>(ptr, idx, val, Fs, Fo, R, nseg, out, loss_part, pa, pb, \
+                                                              ca, cb);                                             \
+    else                                                                                                           \
+      sp_gather_kernel<RPLV, MODE><<<grid, 256, 0, st>>>(ptr, idx, val, Fs, Fo, R, nseg, out, loss_part);           \
+  } while (0)
+  if (rpl <= 1) NMF_GATHER(1);
+  else if (rpl <= 2) NMF_GATHER(2);
+  else if (rpl <= 4) NMF_GATHER(4);
+  else NMF_GATHER(8);
+#undef NMF_GATHER
   NMF_LAUNCH_CHECK();
   return 0;
 }
@@ -196,7 +255,8 @@ int64_t sparse_gram_part_floats(int R) { return (int64_t)128 * R * R; }
 int sparse_numerator(const int64_t* ptr, const int64_t* idx, const float* val, const float* Fself, const float* Fother,
                      int R, int64_t nseg, double beta, float* out, cudaStream_t st) {
   if (beta == 1.0) return launch_gather<kSpKL>(ptr, idx, val, Fself, Fother, R, nseg, out, nullptr, st);
-  return launch_gather<kSpEU>(ptr, idx, val, Fself, Fother, R, nseg, out, nullptr, st);
+  if (beta == 2.0) return launch_gather<kSpEU>(ptr, idx, val, Fself, Fother, R, nseg, out, nullptr, st);
+  return launch_gather<kSpBeta>(ptr, idx, val, Fself, Fother, R, nseg, out, nullptr, st, (float)(beta - 2.0));
 }
 
 int sparse_gram(const float* F, int64_t rows, int R, float* part, float* out, cudaStream_t st) {
@@ -231,6 +291,17 @@ int sparse_loss(const int64_t* crow, const int64_t* col, const float* val, const
   if (rc) return rc;
   sp_loss_final_kernel<<<1, 32, 0, st>>>(loss_part, (int)sparse_gather_blocks(N), pos_a, pos_b, beta == 1.0 ? R : R * R,
                                          beta == 1.0 ? 1.0 : 0.5, v_norm, loss_dev);
+  NMF_LAUNCH_CHECK();
+  return 0;
+}
+
+int sparse_beta_loss(const int64_t* crow, const int64_t* col, const float* val, const float* H, const float* W, int R,
+                     int64_t N, double beta, const double* pos_part, int npos, double* loss_part, double* loss_dev,
+                     cudaStream_t st) {
+  int rc = launch_gather<kSpBetaLoss>(crow, col, val, H, W, R, N, nullptr, loss_part, st, (float)beta, (float)(beta - 1.0),
+                                      1.0 / (beta * (beta - 1.0)), 1.0 / (beta - 1.0));
+  if (rc) return rc;
+  sp_beta_loss_final_kernel<<<1, 256, 0, st>>>(loss_part, (int)sparse_gather_blocks(N), pos_part, npos, beta, loss_dev);
   NMF_LAUNCH_CHECK();
   return 0;
 }

@@ -310,6 +310,7 @@ class CudaSparseNmfEngine(_CudaEngine):
     its CSR and CSC forms are built here with torch (data-format plumbing) and the update terms are evaluated at the non-zeros
     only by the library (include/nmf_b200.h: nmfb200_nmf_set_target_sparse)."""
     kind = "nmf"
+    _set_target = "nmfb200_nmf_set_target_sparse"
 
     def __init__(self, V, W, H, precision="auto"):
         super().__init__()
@@ -343,7 +344,7 @@ class CudaSparseNmfEngine(_CudaEngine):
         self._acquire(("nmf", dev_index, N, C, R, "f32"),
                       lambda ref: self._lib.nmfb200_nmf_create(ref, dev_index, N, C, R, _capi.PRECISIONS["f32"]))
         self._loss = torch.zeros(1, dtype=torch.float64, device=self.device)
-        _capi.check(self._lib.nmfb200_nmf_set_target_sparse(
+        _capi.check(getattr(self._lib, self._set_target)(
             self._ctx, nnz, _ptr(self._crow), _ptr(self._col), _ptr(self._val), _ptr(self._ccol), _ptr(self._row),
             _ptr(self._val_t), self._vnorm_kl, self._vnorm_eu, _stream(self.device)))
 
@@ -379,6 +380,13 @@ class CudaSparseNmfEngine(_CudaEngine):
 
     # the same call and layout as the dense target's; beta 1 and 2 only (the terms of the sparse update, nmf.py:603-638)
     raw_terms = CudaNmfEngine.raw_terms
+
+
+class CudaSparseAnyBetaEngine(CudaSparseNmfEngine):
+    """NMF on a sparse target at every beta > 0, without densifying it (include/nmf_b200.h:
+    nmfb200_nmf_set_target_sparse_any_beta): beta 1 and 2 as CudaSparseNmfEngine; any other beta takes its numerators at the
+    non-zeros and its denominators and loss from V-free dense contractions, so the device holds O(nnz + (N + C) R)."""
+    _set_target = "nmfb200_nmf_set_target_sparse_any_beta"
 
 
 class CudaNmfdEngine(_CudaEngine):

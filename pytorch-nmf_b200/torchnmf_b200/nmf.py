@@ -13,7 +13,8 @@ device, runs there, and copies the factors back into the same Parameter storages
 mode, the `e2e` number of bench.py).  Without a CUDA device or without the built library it raises.
 
 `NMF2D` (:782-865) and `NMF3D` (:868-942) run the NMFD contractions with the last axis sliding and the outer axes as loops.
-Sparse targets are accepted by `NMF` (beta 1 / 2: the library's sparse kernels; other beta: densified on the device).
+Sparse targets are accepted by `NMF` and run on the library's sparse kernels at every beta > 0 up to rank 256 (densified on the
+device above that rank, for sharded fits and for `sparse_fit`).
 `sparse_fit` (:411-599, Hoyer's sparseness-constrained projected gradient) runs on the same engine: gradients from the fused
 raw-terms launch, line-search losses from the fused loss launch, every component projected by ONE
 `nmfb200_hoyer_project` launch.  `trainer.BetaMu` / `SparsityProj` and `plca.*` live in their own modules.
@@ -73,6 +74,15 @@ def _proj_func(s, k1, k2):
     out = s.detach().clone().reshape(1, 1, -1)
     _engine.hoyer_project_(out, 1, [float(k1)], [float(k2)])
     return out.view(s.shape)
+
+
+def _sparse_engine_cls(sparse_kernels, beta, rank, group):
+    """The engine of a sparse target, or None when the target is densified on the device: the sparse kernels serve rank <= 256
+    on one device (`group is None`); beta 1 and 2 take their own gathers and Gram / column sums, every other beta > 0 the
+    engine whose denominators and loss are V-free dense contractions."""
+    if not sparse_kernels or group is not None or rank > 256 or not beta > 0:
+        return None
+    return _engine.CudaSparseNmfEngine if beta in (1, 2) else _engine.CudaSparseAnyBetaEngine
 
 
 class _NullBar:
@@ -161,7 +171,7 @@ class BaseComponent(torch.nn.Module):
     # can be tested on a GPU-less box.  Deliberately NOT a parameter of `fit`: its signature stays the reference's.
     _engine_factory = None
     _sparse_targets = False       # NMF only (nmf.py:603-638); the convolutive models raise, as in the reference
-    _sparse_kernels = True        # beta 1 / 2 on a sparse target: the library's sparse kernels (False: densify)
+    _sparse_kernels = True        # a sparse target on the library's sparse kernels (False: densify)
     _strided_target = False       # the engine reads a row-strided (unit column stride) half-precision target as it is
 
     def _open_engine(self, V, beta, precision, group, sparse_kernels):
@@ -174,10 +184,11 @@ class BaseComponent(torch.nn.Module):
             raise NotImplementedError                      # nmf.py:294-295: only NMF derives the sparse update
         if sparse_target:
             # The reference's sparse derivation (nmf.py:95-119, :603-638: SDDMM at the non-zeros) is the same update as the
-            # dense one on V.to_dense() -- its own tests/test_nmf_sparse.py:8-37 asserts exactly that.  beta 1 and 2 run on
-            # the library's sparse kernels (update terms at the non-zeros only, engine.CudaSparseNmfEngine); for any other
-            # beta the reference itself forms WH densely (nmf.py:621-627), and so does this path: the target is densified
-            # ON THE DEVICE and takes the fused dense kernels (memory = the dense size).  `sparse_kernels=False` forces that.
+            # dense one on V.to_dense() -- its own tests/test_nmf_sparse.py:8-37 asserts exactly that.  The library's sparse
+            # kernels take it at every beta > 0 (_sparse_engine_cls): the numerators at the non-zeros only, and for beta
+            # != 1, 2 the denominators and the loss's sum (WH + eps)^beta from dense contractions that never read V, so the
+            # device holds O(nnz + (N + C) R), not N x C.  Ranks above 256, sharded fits and `sparse_kernels=False` densify
+            # the target ON THE DEVICE and take the fused dense kernels (memory = the dense size).
             V = V.coalesce()
             assert torch.all(V.values() >= 0.), "Target should be non-negative."            # nmf.py:329-330
             if beta <= 0:                                                                    # nmf.py:332-336
@@ -196,9 +207,9 @@ class BaseComponent(torch.nn.Module):
             on_gpu = W.device.type == "cuda"
             dev = W.device if on_gpu else torch.device("cuda", torch.cuda.current_device())
             Vd = V.to(dev, non_blocking=True)
-            # the sparse-target kernels cover ranks up to 256; above, the target is densified like for other betas
-            use_sparse_kernels = (sparse_kernels and sparse_target and beta in (1, 2) and group is None
-                                  and self._sparse_kernels and W.shape[1] <= 256)
+            sparse_cls = (_sparse_engine_cls(sparse_kernels and self._sparse_kernels, beta, W.shape[1], group)
+                          if sparse_target else None)
+            use_sparse_kernels = sparse_cls is not None
             if not sparse_target and Vd.dtype in (torch.float16, torch.bfloat16):
                 # the kernels convert each element exactly where they load it: the fit is bit for bit that of V.float(),
                 # without the fp32 copy (4 bytes per element of V)
@@ -214,8 +225,7 @@ class BaseComponent(torch.nn.Module):
                 Hd = H.data.to(dev, f32, non_blocking=True).contiguous()
             if not Wd.is_contiguous() or not Hd.is_contiguous():
                 raise ValueError("W and H must be contiguous")
-            eng = (_engine.CudaSparseNmfEngine(Vd.coalesce(), Wd, Hd) if use_sparse_kernels
-                   else self._build_engine(Vd, Wd, Hd, precision))
+            eng = sparse_cls(Vd.coalesce(), Wd, Hd) if use_sparse_kernels else self._build_engine(Vd, Wd, Hd, precision)
         else:
             Wd, Hd = W.data, H.data
             eng = self._engine_factory(V.to_dense() if (sparse_target and not sparse_kernels) else V, Wd, Hd)
@@ -243,6 +253,11 @@ class BaseComponent(torch.nn.Module):
         takes a row-strided view), and gives exactly the fit of `V.float()`; a float64 target is staged through an fp32
         copy.  A float64 / half module is staged through fp32 copies and the result is written back into the same
         Parameter storages in their own dtype.
+
+        sparse V (NMF, a COO tensor): fitted without densifying it at every beta > 0 up to rank 256 -- the update terms at
+        the stored entries only and, for beta != 1, 2, the denominators and the loss's sum (WH + eps)^beta from dense
+        contractions that never read V, so the device holds O(nnz + (N + C) R).  Above rank 256 or with `group`, the
+        target is densified on the device.
         """
         eng, W, H, Wd, Hd, staged = self._open_engine(V, beta, precision, group, sparse_kernels=True)
 
