@@ -205,7 +205,10 @@ int nmfb200_nmfd_create(nmfb200_ctx** out, int device, int64_t B, int64_t C, int
 /* NMF2D / NMF3D (nmf.py:782-865, :868-942: conv2d / conv3d with flipped kernels and full padding): the same context type
  * with ndim = 2 or 3 convolved axes.  vdims = the target's sizes over those axes, kdims = kernel_size; V (B,C,*vdims),
  * W (C,R,*kdims), H (B,R,*(vdims - kdims + 1)), all contiguous.  ndim = 1 is nmfb200_nmfd_create.  Every nmfb200_nmfd_*
- * call below serves these contexts; they run on the fp32 kernels (precision auto or f32). */
+ * call below serves these contexts.  With ndim 2 or 3, precision auto or f32 runs the fp32 kernels; NMFB200_PREC_F16 runs
+ * beta 1 on the tensor-core sliding GEMMs of NMFD, over the outer axes too (R <= 256 and the limits of
+ * nmfb200_nmfnd_tc_plan, whose message create returns otherwise), and every other beta on the fp32 kernels, as an NMFD
+ * context at f16 does (nmfb200_precision_for_beta says which). */
 int nmfb200_nmfnd_create(nmfb200_ctx** out, int device, int64_t B, int64_t C, int ndim, const int64_t* vdims,
                          int64_t R, const int64_t* kdims, int precision);
 int nmfb200_nmfd_set_target(nmfb200_ctx* ctx, const float* V, void* stream);
@@ -266,6 +269,16 @@ int nmfb200_nmfd_plan(int64_t B, int64_t C, int ndim, const int64_t* vdims, int6
  *   [19] wgrad splits   [20] wgrad k-blocks per split   [21] dgrad splits   [22] dgrad k-blocks per split */
 #define NMFB200_NMFD_TC_PLAN_LEN 23
 int nmfb200_nmfd_tc_plan(int64_t B, int64_t C, int64_t L, int64_t R, int64_t T, int64_t* out, int n);
+/* The same for an NMFD / NMF2D / NMF3D context (arguments as nmfb200_nmfnd_create): NMFB200_ERR_INVALID, naming the limit,
+ * for a shape that create rejects with precision f16.  NMFB200_NMFND_TC_PLAN_LEN values: [0..22] as above, where recon's
+ * grid z and [15], [16] count target lines (b, x1, x2) and [18] partials over all of them, then
+ *   [23] activation lines (b, j1, j2) per dgrad launch (grid z)   [24] dgrad launches (line slices)
+ *   [25] Tp (T rounded up to 64)   [26] H copy left margin   [27] H copy row pitch   [28] ratio tile row pitch
+ *   [29] C rounded up to 128   [30] 2048-element chunks per H row (prep_h)
+ * For ndim = 1 (or all outer sizes 1) [0..22] are nmfb200_nmfd_tc_plan's. */
+#define NMFB200_NMFND_TC_PLAN_LEN 31
+int nmfb200_nmfnd_tc_plan(int64_t B, int64_t C, int ndim, const int64_t* vdims, int64_t R, const int64_t* kdims,
+                          int64_t* out, int n);
 
 /* ---- sparseness-constrained NMF (Hoyer 2004) --------------------------------------------- */
 

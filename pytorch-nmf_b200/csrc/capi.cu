@@ -705,11 +705,10 @@ static int nmfd_create_impl(nmfb200_ctx** out, int device, int64_t B, int64_t C,
   if (int rc = nmfd_shape_of(B, C, ndim, vdims, R, kdims, &shape)) return rc;
   if (precision != NMFB200_PREC_AUTO && precision != NMFB200_PREC_F32 && precision != NMFB200_PREC_F16)
     return fail(NMFB200_ERR_INVALID, "NMFD precision must be auto, f32 or f16");
+  // NMF2D / NMF3D take the tensor-core kernels only when asked for (f16); auto keeps them on the fp32 kernels
   const bool one_d = shape.one_d();
-  if (!one_d && precision == NMFB200_PREC_F16)
-    return fail(NMFB200_ERR_INVALID, "NMF2D / NMF3D run on the fp32 kernels (precision auto or f32)");
   TcNmfdPlan tc_plan;
-  const char* tc_limit = one_d ? tc_nmfd_plan(shape, &tc_plan) : "";
+  const char* tc_limit = (one_d || precision == NMFB200_PREC_F16) ? tc_nmfd_plan(shape, &tc_plan) : "";
   if (precision == NMFB200_PREC_F16 && tc_limit) return fail(NMFB200_ERR_INVALID, tc_limit);
   DeviceGuard guard(device);
   if (!guard.ok) return fail(NMFB200_ERR_CUDA, "cannot select the requested device");
@@ -738,7 +737,7 @@ static int nmfd_create_impl(nmfb200_ctx** out, int device, int64_t B, int64_t C,
     free_ctx(c);
     return fail(NMFB200_ERR_CUDA, std::string("cudaMalloc: ") + cudaGetErrorString(e));
   }
-  if (c->precision != NMFB200_PREC_F32 && !tc_limit) {    // the tensor-core kernels cover the one-axis case
+  if (c->precision != NMFB200_PREC_F32 && !tc_limit) {    // NMFD at auto / f16, NMF2D / NMF3D at f16
     cudaDeviceProp prop;
     if (cudaGetDeviceProperties(&prop, device) == cudaSuccess && prop.major == 9) {
       int rc = tc_nmfd_create(&c->tcd, c->d);          // beta = 1 runs as wgmma sliding GEMMs (tc_nmfd.cu)
@@ -784,7 +783,7 @@ int nmfb200_nmfd_set_target_typed(nmfb200_ctx* ctx, const void* V, int dtype, vo
       float mm[2] = {0.f, 0.f};
       NMF_CUDA_CHECK(cudaMemcpyAsync(mm, ctx->mm_scratch + 2048, sizeof(mm), cudaMemcpyDeviceToHost, st));
       NMF_CUDA_CHECK(cudaStreamSynchronize(st));
-      const double mean = vsum / ((double)ctx->d.B * ctx->d.C * ctx->d.L);
+      const double mean = vsum / ((double)ctx->d.B * ctx->d.C * ctx->d.v_inner());
       ctx->tc_off = !(mean > 0.0) || (double)mm[1] > 64.0 * mean;
     }
   }
@@ -874,6 +873,21 @@ int nmfb200_nmfd_tc_plan(int64_t B, int64_t C, int64_t L, int64_t R, int64_t T, 
       p.wgrad.x, p.wgrad.y, p.wgrad.z, p.dgrad.x, p.dgrad.y, p.dgrad.z, p.bslice, p.slices, p.dgrad_rblocks,
       p.loss_blocks, p.ws_w, p.kbs_w, p.ws_h, p.kbs_h};
   for (int i = 0; i < NMFB200_NMFD_TC_PLAN_LEN; ++i) out[i] = v[i];
+  return 0;
+}
+
+int nmfb200_nmfnd_tc_plan(int64_t B, int64_t C, int ndim, const int64_t* vdims, int64_t R, const int64_t* kdims,
+                          int64_t* out, int n) {
+  if (!out || n < NMFB200_NMFND_TC_PLAN_LEN) return fail(NMFB200_ERR_INVALID, "plan buffer too small");
+  NmfdShape d;
+  if (int rc = nmfd_shape_of(B, C, ndim, vdims, R, kdims, &d)) return rc;
+  TcNmfdPlan p;
+  if (const char* why = tc_nmfd_plan(d, &p)) return fail(NMFB200_ERR_INVALID, why);
+  const int64_t v[NMFB200_NMFND_TC_PLAN_LEN] = {
+      p.prep_w.x, p.prep_w.y, p.prep_w.z, p.prep_h.x, p.prep_h.y, p.prep_h.z, p.recon.x, p.recon.y, p.recon.z,
+      p.wgrad.x, p.wgrad.y, p.wgrad.z, p.dgrad.x, p.dgrad.y, p.dgrad.z, p.bslice, p.slices, p.dgrad_rblocks,
+      p.loss_blocks, p.ws_w, p.kbs_w, p.ws_h, p.kbs_h, p.hslice, p.hslices, p.Tp, p.padl, p.Lp, p.Lq, p.Cpad, p.nch};
+  for (int i = 0; i < NMFB200_NMFND_TC_PLAN_LEN; ++i) out[i] = v[i];
   return 0;
 }
 

@@ -55,8 +55,15 @@ struct NmfdTcParams {
   double* loss_part;              // recon loss: one partial per CTA
   int nsplit, kb_per_split;
   int r_off;                      // dgrad: first component of this launch (components [r_off, r_off + 128))
-  int b0;                         // recon / dgrad: first batch element of this launch (batch b0 + blockIdx.z)
+  int b0;                         // recon / dgrad: first batch element of this launch (batch b0 + blockIdx.z); ND: first line
 };
+// NMF2D / NMF3D (the ND kernels): the outer axes of the target (X1, X2), of the kernel (T1, T2) and of H (J1, J2).  A
+// separate type, so that the NMFD kernels keep their parameter block (and code) as they are.
+struct NmfdNdParams : NmfdTcParams {
+  int X1, X2, T1, T2, J1, J2;
+};
+template <bool ND>
+using TcParams = std::conditional_t<ND, NmfdNdParams, NmfdTcParams>;
 
 struct Smem {
   static constexpr int kTile = kM * kKB * 2;                 // 16 KB
@@ -86,9 +93,19 @@ __device__ __forceinline__ void bulk_copy_g2s(uint32_t dst, const void* src, uin
 //   dgrad              : grid (Lin tiles, nsplit, batch slice); Toeplitz = A (rows j), plain = B = Wf16 rows (c R + r_off + n), N = 128;
 //                        ranks above 128 take one launch per 128 components
 // TV: the target's element type (recon / recon-loss only; wgrad and dgrad read no V and take float)
-template <int KIND, typename TV>
+// ND: NMF2D / NMF3D, the outer axes as further k-block and grid dimensions (csrc/nmfd.cu for the maths; (t1, t2) outer
+// kernel offsets, (x1, x2) target lines, (j1, j2) activation lines; the last axis slides as above):
+//   recon / recon-loss : grid.z = target lines (b, x1, x2); k-blocks (r, t1, t2, kk) over the valid offsets only,
+//                        0 <= x - t < J per outer axis; source Hp16 row (b, r, x1 - t1, x2 - t2), plain Wr16 column
+//                        ((r T1 + t1) T2 + t2) Tp + 64 kk
+//   wgrad              : grid.y = (r, t1, t2) x shift blocks; k-blocks (b, j1, j2, l-block); plain P16 line
+//                        (b, j1 + t1, j2 + t2), source H row (b, r, j1, j2)
+//   dgrad              : grid.z = activation lines (b, j1, j2); k-blocks (c, t1, t2, kk); source P16 line
+//                        (b, j1 + t1, j2 + t2) channel c, plain Wf16 rows c R + r_off + n, columns (t1 T2 + t2) Tp + 64 kk
+// P16 is line-major (row (line X1X2-index) C + c), so 128 channels of one line are one TMA box.  ND = false is the 1-D kernel.
+template <int KIND, typename TV, bool ND>
 __global__ void __launch_bounds__(kThreads, 1)
-tcnmfd_kernel(const __grid_constant__ CUtensorMap tmPlain, const NmfdTcParams p) {
+tcnmfd_kernel(const __grid_constant__ CUtensorMap tmPlain, const TcParams<ND> p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   const uint32_t raw32 = ptx::smem_u32(smem_raw);
   const uint32_t sbase = (raw32 + 1023u) & ~1023u;
@@ -115,17 +132,62 @@ tcnmfd_kernel(const __grid_constant__ CUtensorMap tmPlain, const NmfdTcParams p)
 
   // ---- what this CTA computes, as a list of k-blocks: (plain-tile coordinates, source vector, window start) -------------
   int nkb, kb0 = 0;
+  // ND: this CTA's line (recon: target line (lb, o1, o2); dgrad: activation line) and, for recon, its valid outer offsets
+  // t1 in [t1lo, t1lo + n1), t2 in [t2lo, t2lo + n2): the TMA warp and the producers count the same k-blocks
+  int lb = 0, o1 = 0, o2 = 0, t1lo = 0, n1 = 1, t2lo = 0, n2 = 1;
+  if constexpr (ND) {
+    if (RECON || KIND == kDgrad) {
+      const int O1 = RECON ? p.X1 : p.J1, O2 = RECON ? p.X2 : p.J2;
+      lb = bz / (O1 * O2);
+      const int o12 = bz - lb * (O1 * O2);
+      o1 = o12 / O2; o2 = o12 - o1 * O2;
+    }
+    if (RECON) {
+      t1lo = max(0, o1 - p.J1 + 1); n1 = min(p.T1 - 1, o1) - t1lo + 1;
+      t2lo = max(0, o2 - p.J2 + 1); n2 = min(p.T2 - 1, o2) - t2lo + 1;
+    }
+  }
   if (RECON) nkb = p.R * (p.Tp / kKB);
   else { kb0 = (KIND == kWgrad ? blockIdx.z : blockIdx.y) * p.kb_per_split; nkb = p.kb_per_split; }
-  const int lkb = (p.L + kKB - 1) / kKB;                    // wgrad: k-blocks per batch element
+  const int lkb = (p.L + kKB - 1) / kKB;                    // wgrad: k-blocks per batch element (ND: per activation line)
   const int tkb = p.Tp / kKB;
   const int ntb = (p.T + kM - 1) / kM;                      // wgrad: blocks of 128 shifts (blockIdx.y = r ntb + tb)
-  if (KIND == kWgrad) nkb = max(0, min(nkb, p.B * lkb - kb0));
-  if (KIND == kDgrad) nkb = max(0, min(nkb, p.C * tkb - kb0));
+  if constexpr (ND) {
+    if (RECON) nkb *= n1 * n2;
+    if (KIND == kWgrad) nkb = max(0, min(nkb, p.B * p.J1 * p.J2 * lkb - kb0));
+    if (KIND == kDgrad) nkb = max(0, min(nkb, p.C * p.T1 * p.T2 * tkb - kb0));
+  } else {
+    if (KIND == kWgrad) nkb = max(0, min(nkb, p.B * lkb - kb0));
+    if (KIND == kDgrad) nkb = max(0, min(nkb, p.C * tkb - kb0));
+  }
   // per k-block: returns the plain tile's TMA coordinates (x = column, y = row), the source row pointer and the index of the
   // source element that row 0 / column 0 of the Toeplitz tile reads; `dir` is the step of that index from row to row
   auto kblock = [&](int kb, int& px, int& py, const __half*& src, int& e0) {
-    if (RECON) {
+    if constexpr (ND) {
+      if (RECON) {
+        const int nper = n1 * n2 * tkb, r = kb / nper, rem = kb - r * nper;
+        const int a = rem / tkb, kk = rem - a * tkb, i1 = a / n2;
+        const int t1 = t1lo + i1, t2 = t2lo + (a - i1 * n2);
+        px = ((r * p.T1 + t1) * p.T2 + t2) * p.Tp + kk * kKB; py = blockIdx.y * kM;
+        src = p.Hp16 + ((((int64_t)lb * p.R + r) * p.J1 + (o1 - t1)) * p.J2 + (o2 - t2)) * p.Lp;
+        e0 = p.padl + blockIdx.x * kM - p.Tp + 1 + kk * kKB;
+      } else if (KIND == kWgrad) {
+        const int J12 = p.J1 * p.J2, T12 = p.T1 * p.T2;
+        const int g = kb0 + kb, ln = g / lkb, lk = g - ln * lkb;          // ln: activation line (b, j1, j2)
+        const int b = ln / J12, j12 = ln - b * J12, j1 = j12 / p.J2, j2 = j12 - j1 * p.J2;
+        const int rw = blockIdx.y / ntb, r = rw / T12, t12 = rw - r * T12, t1 = t12 / p.T2, t2 = t12 - t1 * p.T2;
+        px = lk * kKB; py = ((b * p.X1 + j1 + t1) * p.X2 + j2 + t2) * p.C + blockIdx.x * kM;
+        src = p.Hp16 + (((int64_t)b * p.R + r) * J12 + j12) * p.Lp;
+        e0 = p.padl + lk * kKB - (blockIdx.y % ntb) * kM;
+      } else {
+        const int T12 = p.T1 * p.T2;
+        const int g = kb0 + kb, a = g / tkb, kk = g - a * tkb, c = a / T12, t12 = a - c * T12;
+        const int t1 = t12 / p.T2, t2 = t12 - t1 * p.T2;
+        px = t12 * p.Tp + kk * kKB; py = c * p.R + p.r_off;
+        src = p.P16 + ((((int64_t)lb * p.X1 + o1 + t1) * p.X2 + o2 + t2) * p.C + c) * p.Lq;
+        e0 = blockIdx.x * kM + kk * kKB;
+      }
+    } else if (RECON) {
       const int r = kb / tkb, kk = kb - r * tkb;            // k = reversed shift t' in [64 kk, 64 kk + 64)
       px = r * p.Tp + kk * kKB; py = blockIdx.y * kM;
       src = p.Hp16 + ((int64_t)bz * p.R + r) * p.Lp;
@@ -237,6 +299,8 @@ tcnmfd_kernel(const __grid_constant__ CUtensorMap tmPlain, const NmfdTcParams p)
         const bool row_ok = c < p.C;
         const float kap = *p.kappa, pscale = exp2f((float)p.exps[2]);
         const TV* vrow = reinterpret_cast<const TV*>(p.V) + ((int64_t)b * p.C + (row_ok ? c : 0)) * p.L;
+        if constexpr (ND)          // V (B, C, X1, X2, L): line (lb, o1, o2) of channel c
+          vrow = reinterpret_cast<const TV*>(p.V) + (((int64_t)lb * p.C + (row_ok ? c : 0)) * (p.X1 * p.X2) + o1 * p.X2 + o2) * p.L;
         __half* prow = p.P16out + ((int64_t)b * p.C + (row_ok ? c : 0)) * p.Lq;
         double acc = 0.0;
 #pragma unroll 1
@@ -280,6 +344,8 @@ tcnmfd_kernel(const __grid_constant__ CUtensorMap tmPlain, const NmfdTcParams p)
       } else if (KIND == kWgrad) {
         const int c = blockIdx.x * kM + r128, r = blockIdx.y / ntb, t0 = (blockIdx.y % ntb) * kM;
         float* dst = p.out + (((int64_t)blockIdx.z * p.C + (c < p.C ? c : 0)) * p.R + r) * p.T + t0;  // [split][C][R][T]
+        if constexpr (ND)          // [split][C][R T1 T2][T], r = (r, t1, t2)
+          dst = p.out + (((int64_t)blockIdx.z * p.C + (c < p.C ? c : 0)) * (p.R * p.T1 * p.T2) + r) * p.T + t0;
         const bool vec = (p.T & 3) == 0;
 #pragma unroll 1
         for (int j = 0; j < kM / 16; ++j) {
@@ -308,7 +374,13 @@ tcnmfd_kernel(const __grid_constant__ CUtensorMap tmPlain, const NmfdTcParams p)
 #pragma unroll
             for (int i = 0; i < 16; ++i) {
               const int r = p.r_off + jj * 16 + i;
-              if (r < p.R) p.out[(((int64_t)blockIdx.y * p.B + b) * p.R + r) * p.Lin + j] = __uint_as_float(sr[i]) * sc;
+              if (r < p.R) {
+                if constexpr (ND)        // [split][B][R][J1 J2][Lin]
+                  p.out[((((int64_t)blockIdx.y * p.B + lb) * p.R + r) * (p.J1 * p.J2) + o1 * p.J2 + o2) * p.Lin + j] =
+                      __uint_as_float(sr[i]) * sc;
+                else
+                  p.out[(((int64_t)blockIdx.y * p.B + b) * p.R + r) * p.Lin + j] = __uint_as_float(sr[i]) * sc;
+              }
             }
           }
         }
@@ -388,7 +460,8 @@ fold_colsum_kernel(const FoldTail f) {
 }
 
 // One pass over W (C, R, T), block c: both fp16 operand copies of this row, scaled by 2^eW (eW from the max of W), written
-// 16 bytes per thread and step, plus the row's per-component sums (-> colsum_W, nmf.py:128-131):
+// 16 bytes per thread and step, plus the row's per-component sums (-> colsum_W, nmf.py:128-131).  NMF2D / NMF3D pass
+// R T1 T2 as R: each (r, t1, t2) is one row of T taps, and the fold sums the T1 T2 partials of each component.
 //   Wr16[c][r Tp + tt]           = W[c, r, Tp - 1 - tt]        (recon: shifts reversed so that the H window ascends)
 //   Wf16[c][r Tp + tt]           = W[c, r, tt]                 (dgrad)
 __global__ void __launch_bounds__(256, 8)     // 8 blocks per SM: the 1025 blocks of cfg3 run as one wave
@@ -427,7 +500,7 @@ prep_w_kernel(const float* __restrict__ W, int C, int R, int T, int Tp, const un
 
 // H (B, R, Lin) fp32 -> Hp16 (B R rows x Lp): H[b,r,j] 2^eH at column padl + j (margins stay zero), 2048 elements per
 // block, + the block's partial sum (-> colsum_H, nmf.py:122-125).  One-dimensional grid of B R nch blocks, block
-// (row, chunk) = row nch + chunk: B R alone may pass the 65535 of grid.y
+// (row, chunk) = row nch + chunk: B R alone may pass the 65535 of grid.y.  NMF2D / NMF3D: B R J1 J2 rows (b, r, j1, j2)
 __global__ void __launch_bounds__(256)
 prep_h_kernel(const float* __restrict__ H, int Lin, int Lp, int padl, int nch, const unsigned int* __restrict__ absmax,
               int* __restrict__ exps, __half* __restrict__ Hp16, float* __restrict__ cs_part) {
@@ -522,6 +595,8 @@ struct TcNmfdState {
 const char* tc_nmfd_plan(const NmfdShape& d, TcNmfdPlan* p) {
   *p = TcNmfdPlan{};
   if (d.R < 1 || d.R > 256 || d.T < 1 || d.L < d.T) return "the tensor-core NMFD path needs 1 <= R <= 256 and 1 <= T <= L";
+  // outer axes (NMF2D / NMF3D; all 1 for NMFD): target lines X12 = X1 X2, kernel offsets T12, activation lines J12
+  const int64_t X12 = (int64_t)d.X1 * d.X2, T12 = (int64_t)d.T1 * d.T2, J12 = (int64_t)d.J1() * d.J2();
   p->Tp = round_up(d.T, kKB);
   p->padl = round_up(p->Tp + 136, 8);                       // every window start >= 0
   p->Lp = round_up(p->padl + round_up(d.L, 2048) + 256 + kWinHalfs + 136, 8);
@@ -529,31 +604,47 @@ const char* tc_nmfd_plan(const NmfdShape& d, TcNmfdPlan* p) {
   p->Cpad = round_up(d.C, kM);
   const int64_t lkb = ceil_div(d.L, kKB), tkb = p->Tp / kKB;
   // split the K loops of wgrad / dgrad so that the grid is a few waves of 132 CTAs
-  const int64_t tiles_w = ceil_div(d.C, kM) * d.R * ceil_div(d.T, kM), tiles_h = ceil_div(d.Lin, kM) * d.B;
-  const int64_t kb_w = (int64_t)d.B * lkb, kb_h = (int64_t)d.C * tkb;
+  const int64_t tiles_w = ceil_div(d.C, kM) * d.R * T12 * ceil_div(d.T, kM), tiles_h = ceil_div(d.Lin, kM) * d.B * J12;
+  const int64_t kb_w = (int64_t)d.B * J12 * lkb, kb_h = (int64_t)d.C * T12 * tkb;
   p->ws_w = std::max<int64_t>(1, std::min<int64_t>(kb_w / 8, ceil_div(132 * 4, tiles_w)));
   p->ws_h = std::max<int64_t>(1, std::min<int64_t>(kb_h / 8, ceil_div(132 * 4, tiles_h)));
   p->kbs_w = ceil_div(kb_w, p->ws_w); p->ws_w = ceil_div(kb_w, p->kbs_w);
   p->kbs_h = ceil_div(kb_h, p->ws_h); p->ws_h = ceil_div(kb_h, p->kbs_h);
   p->nch = ceil_div(d.Lin, 2048);
-  p->bslice = nmfd_batch_slice(d.B);
-  p->slices = ceil_div(d.B, p->bslice);
+  p->bslice = nmfd_batch_slice((int64_t)d.B * X12);          // recon: one CTA row per target line (b, x1, x2)
+  p->slices = ceil_div((int64_t)d.B * X12, p->bslice);
+  p->hslice = nmfd_batch_slice((int64_t)d.B * J12);          // dgrad: per activation line (b, j1, j2)
+  p->hslices = ceil_div((int64_t)d.B * J12, p->hslice);
   p->dgrad_rblocks = ceil_div(d.R, kM);
   p->prep_w = Grid3{d.C, 1, 1};
-  p->prep_h = Grid3{(int64_t)d.B * d.R * p->nch, 1, 1};
+  p->prep_h = Grid3{(int64_t)d.B * d.R * J12 * p->nch, 1, 1};
   p->recon = Grid3{ceil_div(d.L, kM), ceil_div(d.C, kM), p->bslice};
-  p->wgrad = Grid3{ceil_div(d.C, kM), (int64_t)d.R * ceil_div(d.T, kM), p->ws_w};
-  p->dgrad = Grid3{ceil_div(d.Lin, kM), p->ws_h, p->bslice};
-  p->loss_blocks = p->recon.x * p->recon.y * d.B;
-  if (!grid_fits(p->wgrad)) return "the tensor-core NMFD wgrad grid needs R ceil(T / 128) <= 65535";
+  p->wgrad = Grid3{ceil_div(d.C, kM), (int64_t)d.R * T12 * ceil_div(d.T, kM), p->ws_w};
+  p->dgrad = Grid3{ceil_div(d.Lin, kM), p->ws_h, p->hslice};
+  p->loss_blocks = p->recon.x * p->recon.y * d.B * X12;
+  if (!grid_fits(p->wgrad))
+    return d.one_d() ? "the tensor-core NMFD wgrad grid needs R ceil(T / 128) <= 65535"
+                     : "the tensor-core NMFD wgrad grid needs R T1 T2 ceil(T / 128) <= 65535";
   for (const Grid3* g : {&p->prep_w, &p->prep_h, &p->recon, &p->dgrad})
     if (!grid_fits(*g)) return "a tensor-core NMFD grid passes the CUDA grid limits";
   // 32-bit quantities of the kernels: the TMA row coordinate b C + c of the ratio tile, the global k-block indices of
   // wgrad / dgrad, the loss partial count (sum_partials), the row pitches
-  if ((int64_t)d.B * d.C + kM > INT32_MAX) return "the tensor-core NMFD path needs B C < 2^31 - 128 (TMA row coordinate)";
-  if (kb_w > INT32_MAX || kb_h > INT32_MAX || p->loss_blocks > INT32_MAX || p->Lp > INT32_MAX || p->Lq > INT32_MAX ||
-      p->Cpad * d.R > INT32_MAX)
-    return "a tensor-core NMFD block or k-block count passes 2^31 - 1";
+  if (d.one_d()) {
+    if ((int64_t)d.B * d.C + kM > INT32_MAX) return "the tensor-core NMFD path needs B C < 2^31 - 128 (TMA row coordinate)";
+    if (kb_w > INT32_MAX || kb_h > INT32_MAX || p->loss_blocks > INT32_MAX || p->Lp > INT32_MAX || p->Lq > INT32_MAX ||
+        p->Cpad * d.R > INT32_MAX)
+      return "a tensor-core NMFD block or k-block count passes 2^31 - 1";
+    return nullptr;
+  }
+  if ((int64_t)d.B * X12 * d.C + kM > INT32_MAX)
+    return "the tensor-core NMF2D / NMF3D path needs B X1 X2 C < 2^31 - 128 (TMA row coordinate of the ratio tile)";
+  if (kb_w > INT32_MAX) return "the tensor-core NMF2D / NMF3D path needs B J1 J2 ceil(L / 64) < 2^31 (wgrad k-blocks)";
+  if (kb_h > INT32_MAX) return "the tensor-core NMF2D / NMF3D path needs C T1 T2 Tp / 64 < 2^31 (dgrad k-blocks)";
+  if ((int64_t)d.R * T12 * p->Tp > INT32_MAX)
+    return "the tensor-core NMF2D / NMF3D path needs R T1 T2 Tp < 2^31 (kernel copy pitch, recon k-blocks)";
+  if (p->Cpad * d.R > INT32_MAX) return "the tensor-core NMF2D / NMF3D path needs ceil(C / 128) 128 R < 2^31 (dgrad rows)";
+  if (p->loss_blocks > INT32_MAX) return "the tensor-core NMF2D / NMF3D path needs fewer than 2^31 recon-loss partials";
+  if (p->Lp > INT32_MAX || p->Lq > INT32_MAX) return "the tensor-core NMF2D / NMF3D path needs row pitches below 2^31";
   return nullptr;
 }
 
@@ -579,11 +670,12 @@ int tc_nmfd_create(TcNmfdState** out, const NmfdShape& d) {
   const TcNmfdPlan& pl = s->plan;
   s->Tp = (int)pl.Tp; s->padl = (int)pl.padl; s->Lp = (int)pl.Lp; s->Lq = (int)pl.Lq; s->Cpad = (int)pl.Cpad;
   s->ws_w = (int)pl.ws_w; s->kbs_w = (int)pl.kbs_w; s->ws_h = (int)pl.ws_h; s->kbs_h = (int)pl.kbs_h;
-  const int64_t pw = (int64_t)s->ws_w * d.C * d.R * d.T, ph = (int64_t)s->ws_h * d.B * d.R * d.Lin;
+  const int64_t X12 = (int64_t)d.X1 * d.X2, T12 = (int64_t)d.T1 * d.T2, J12 = (int64_t)d.J1() * d.J2();
+  const int64_t pw = (int64_t)s->ws_w * d.C * d.R * d.w_inner(), ph = (int64_t)s->ws_h * d.B * d.R * d.h_inner();
   s->part_floats = pw > ph ? pw : ph;
   s->loss_blocks = (int)pl.loss_blocks;
-  const size_t wbytes = (size_t)s->Cpad * d.R * s->Tp * 2, hbytes = (size_t)d.B * d.R * s->Lp * 2;
-  const size_t pbytes = ((size_t)d.B * d.C + 1) * s->Lq * 2;
+  const size_t wbytes = (size_t)s->Cpad * d.R * T12 * s->Tp * 2, hbytes = (size_t)d.B * d.R * J12 * s->Lp * 2;
+  const size_t pbytes = ((size_t)d.B * X12 * d.C + 1) * s->Lq * 2;
   cudaError_t e = cudaSuccess;
   if (e == cudaSuccess) e = cudaMalloc(&s->Wr16, wbytes);
   if (e == cudaSuccess) e = cudaMalloc(&s->Wf16, wbytes);
@@ -593,7 +685,7 @@ int tc_nmfd_create(TcNmfdState** out, const NmfdShape& d) {
   if (e == cudaSuccess) e = cudaMalloc(&s->absmax, 2 * sizeof(unsigned int));
   if (e == cudaSuccess) e = cudaMalloc(&s->colsum, 2 * (size_t)d.R * sizeof(float));
   {
-    const int64_t np = std::max<int64_t>((int64_t)d.C * d.R, pl.prep_h.x);
+    const int64_t np = std::max<int64_t>((int64_t)d.C * d.R * T12, pl.prep_h.x);
     if (e == cudaSuccess) e = cudaMalloc(&s->cs_part, (size_t)np * sizeof(float));
   }
   if (e == cudaSuccess) e = cudaMalloc(&s->exps, 8 * sizeof(int));          // [0..3] exponents, [4..5] fold tickets
@@ -612,18 +704,18 @@ int tc_nmfd_create(TcNmfdState** out, const NmfdShape& d) {
     return 2;
   }
   int rc = 0;
-  rc |= make_tmap2(&s->tmWr, s->Wr16, s->Cpad, (int64_t)d.R * s->Tp, (int64_t)d.R * s->Tp, kM);
-  // dgrad reads Wf16 as (C R) rows of Tp columns, up to 128 rows (components) per tile
+  rc |= make_tmap2(&s->tmWr, s->Wr16, s->Cpad, (int64_t)d.R * T12 * s->Tp, (int64_t)d.R * T12 * s->Tp, kM);
+  // dgrad reads Wf16 as (C R) rows of T1 T2 Tp columns, up to 128 rows (components) per tile
   const int Rb = (int)std::min<int64_t>((d.R + 15) & ~15, 128);
-  rc |= make_tmap2(&s->tmWf, s->Wf16, (int64_t)s->Cpad * d.R, s->Tp, s->Tp, Rb);
-  rc |= make_tmap2(&s->tmP, s->P16, (int64_t)d.B * d.C, s->Lq, s->Lq, kM);
+  rc |= make_tmap2(&s->tmWf, s->Wf16, (int64_t)s->Cpad * d.R, T12 * s->Tp, T12 * s->Tp, Rb);
+  rc |= make_tmap2(&s->tmP, s->P16, (int64_t)d.B * X12 * d.C, s->Lq, s->Lq, kM);
   if (rc) { tc_nmfd_destroy(s); return 2; }
   *out = s;
   return 0;
 }
 
 int tc_nmfd_set_target(TcNmfdState* s, const void* V, int vdtype, double* vsum_host, cudaStream_t st) {
-  const int64_t n = (int64_t)s->d.B * s->d.C * s->d.L;
+  const int64_t n = (int64_t)s->d.B * s->d.C * s->d.v_inner();
   int rc = with_vtype(V, vdtype, [&](auto Vt) {
     vsum_kernel<<<256, 256, 0, st>>>(Vt, n, s->vsum + 1);
     NMF_LAUNCH_CHECK();
@@ -641,9 +733,10 @@ namespace {
 
 dim3 dim3_of(const Grid3& g) { return dim3((unsigned)g.x, (unsigned)g.y, (unsigned)g.z); }
 
-template <int KIND, typename TV = float>
-int launch(TcNmfdState* s, const CUtensorMap& tm, dim3 grid, const NmfdTcParams& p, cudaStream_t st) {
-  auto kern = tcnmfd_kernel<KIND, TV>;
+template <int KIND, typename TV = float, bool ND = false>
+int launch(TcNmfdState* s, const CUtensorMap& tm, dim3 grid, const NmfdNdParams& pnd, cudaStream_t st) {
+  auto kern = tcnmfd_kernel<KIND, TV, ND>;
+  const TcParams<ND>& p = pnd;                      // NMFD: the NmfdTcParams part only
   static unsigned long long attr_set_mask = 0;      // per device (one bit each): the attribute is per-device state
   const int smem = Smem::kTotal + 1024;
   int dev = 0;
@@ -657,21 +750,23 @@ int launch(TcNmfdState* s, const CUtensorMap& tm, dim3 grid, const NmfdTcParams&
   return 0;
 }
 
-// recon / dgrad: one launch per slice of at most plan.bslice batch elements (grid.z), batch offset b0
-template <int KIND, typename TV = float>
-int launch_slices(TcNmfdState* s, const CUtensorMap& tm, const Grid3& g, NmfdTcParams p, cudaStream_t st) {
-  for (int64_t b0 = 0; b0 < s->d.B; b0 += g.z) {
+// recon / dgrad: one launch per slice of at most g.z of the `lines` batch elements (NMF2D / NMF3D: target or activation
+// lines) on grid.z, offset b0
+template <int KIND, typename TV = float, bool ND = false>
+int launch_slices(TcNmfdState* s, const CUtensorMap& tm, const Grid3& g, int64_t lines, NmfdNdParams p, cudaStream_t st) {
+  for (int64_t b0 = 0; b0 < lines; b0 += g.z) {
     p.b0 = (int)b0;
     dim3 grid = dim3_of(g);
-    grid.z = (unsigned)std::min<int64_t>(g.z, s->d.B - b0);
-    if (int rc = launch<KIND, TV>(s, tm, grid, p, st)) return rc;
+    grid.z = (unsigned)std::min<int64_t>(g.z, lines - b0);
+    if (int rc = launch<KIND, TV, ND>(s, tm, grid, p, st)) return rc;
   }
   return 0;
 }
 
-NmfdTcParams base_params(TcNmfdState* s, const void* V) {
-  NmfdTcParams p{};
+NmfdNdParams base_params(TcNmfdState* s, const void* V) {
+  NmfdNdParams p{};
   p.B = s->d.B; p.C = s->d.C; p.L = s->d.L; p.R = s->d.R; p.T = s->d.T; p.Lin = s->d.Lin; p.Tp = s->Tp;
+  p.X1 = s->d.X1; p.X2 = s->d.X2; p.T1 = s->d.T1; p.T2 = s->d.T2; p.J1 = s->d.J1(); p.J2 = s->d.J2();
   p.Lp = s->Lp; p.padl = s->padl; p.Lq = s->Lq;
   p.Hp16 = s->Hp16; p.P16 = s->P16; p.P16out = s->P16; p.exps = s->exps; p.kappa = s->kappa;
   p.V = static_cast<const float*>(V);
@@ -692,23 +787,26 @@ FoldTail fold_tail_args(TcNmfdState* s, int which, int outer, int inner, int do_
 // bring the fp16 operand copies, column sums (and with them kappa) up to date with the fp32 factors: only what changed
 int refresh(TcNmfdState* s, const float* W, const float* H, cudaStream_t st) {
   const NmfdShape& d = s->d;
+  const int T12 = d.T1 * d.T2, J12 = d.J1() * d.J2();       // 1 for NMFD
   if (!s->w_fresh) {
     if (!s->aw_valid) {
       NMF_CUDA_CHECK(cudaMemsetAsync(s->absmax, 0, sizeof(unsigned int), st));
-      absmax_kernel<<<256, 256, 0, st>>>(W, (int64_t)d.C * d.R * d.T, s->absmax);
+      absmax_kernel<<<256, 256, 0, st>>>(W, (int64_t)d.C * d.R * d.w_inner(), s->absmax);
       NMF_LAUNCH_CHECK();
       s->aw_valid = true;
     }
-    prep_w_kernel<<<(unsigned)s->plan.prep_w.x, 256, 0, st>>>(W, d.C, d.R, d.T, s->Tp, s->absmax, s->exps, s->Wr16, s->Wf16, s->cs_part);
+    // rows (r, t1, t2) of T taps; the fold sums each component's T1 T2 row partials of every channel
+    prep_w_kernel<<<(unsigned)s->plan.prep_w.x, 256, 0, st>>>(W, d.C, d.R * T12, d.T, s->Tp, s->absmax, s->exps, s->Wr16,
+                                                              s->Wf16, s->cs_part);
     NMF_LAUNCH_CHECK();
-    fold_colsum_kernel<<<d.R, 256, 0, st>>>(fold_tail_args(s, 0, d.C, 1, /*do_kappa=*/s->h_fresh));
+    fold_colsum_kernel<<<d.R, 256, 0, st>>>(fold_tail_args(s, 0, d.C, T12, /*do_kappa=*/s->h_fresh));
     NMF_LAUNCH_CHECK();
     s->w_fresh = true;
   }
   if (!s->h_fresh) {
     if (!s->ah_valid) {
       NMF_CUDA_CHECK(cudaMemsetAsync(s->absmax + 1, 0, sizeof(unsigned int), st));
-      absmax_kernel<<<256, 256, 0, st>>>(H, (int64_t)d.B * d.R * d.Lin, s->absmax + 1);
+      absmax_kernel<<<256, 256, 0, st>>>(H, (int64_t)d.B * d.R * d.h_inner(), s->absmax + 1);
       NMF_LAUNCH_CHECK();
       s->ah_valid = true;
     }
@@ -716,7 +814,7 @@ int refresh(TcNmfdState* s, const float* W, const float* H, cudaStream_t st) {
     prep_h_kernel<<<(unsigned)s->plan.prep_h.x, 256, 0, st>>>(H, d.Lin, s->Lp, s->padl, nch, s->absmax + 1, s->exps, s->Hp16,
                                                               s->cs_part);
     NMF_LAUNCH_CHECK();
-    fold_colsum_kernel<<<d.R, 256, 0, st>>>(fold_tail_args(s, 1, d.B, nch, /*do_kappa=*/1));
+    fold_colsum_kernel<<<d.R, 256, 0, st>>>(fold_tail_args(s, 1, d.B, J12 * nch, /*do_kappa=*/1));
     NMF_LAUNCH_CHECK();
     s->h_fresh = true;
   }
@@ -729,11 +827,16 @@ int tc_nmfd_recon(TcNmfdState* s, const void* V, int vdtype, const float* W, con
                   cudaStream_t st) {
   int rc = refresh(s, W, H, st);
   if (rc) return rc;
-  const NmfdTcParams p = base_params(s, V);
+  const NmfdNdParams p = base_params(s, V);
+  const int64_t lines = (int64_t)s->d.B * s->d.X1 * s->d.X2;
+  const bool nd = !s->d.one_d();
   rc = with_vtype(V, vdtype, [&](auto Vt) {
     using TV = vtype_t<decltype(Vt)>;
-    return loss ? launch_slices<kReconLoss, TV>(s, s->tmWr, s->plan.recon, p, st)
-                : launch_slices<kRecon, TV>(s, s->tmWr, s->plan.recon, p, st);
+    if (nd)
+      return loss ? launch_slices<kReconLoss, TV, true>(s, s->tmWr, s->plan.recon, lines, p, st)
+                  : launch_slices<kRecon, TV, true>(s, s->tmWr, s->plan.recon, lines, p, st);
+    return loss ? launch_slices<kReconLoss, TV>(s, s->tmWr, s->plan.recon, lines, p, st)
+                : launch_slices<kRecon, TV>(s, s->tmWr, s->plan.recon, lines, p, st);
   });
   if (rc || !loss) return rc;
   return sum_partials(s->loss_part, s->loss_blocks, loss_dev, st);
@@ -741,19 +844,25 @@ int tc_nmfd_recon(TcNmfdState* s, const void* V, int vdtype, const float* W, con
 
 // numerator partials of the W update from the P16 written by the last recon: [*nsplit][C][R][T] fp32
 int tc_nmfd_wgrad(TcNmfdState* s, const float** part, int* nsplit, cudaStream_t st) {
-  NmfdTcParams p = base_params(s, nullptr);
+  NmfdNdParams p = base_params(s, nullptr);
   p.nsplit = s->ws_w; p.kb_per_split = s->kbs_w;
   // one CTA per (128 rows c, component r, block of 128 shifts t, split): the Toeplitz tile holds 128 shifts
-  int rc = launch<kWgrad>(s, s->tmP, dim3_of(s->plan.wgrad), p, st);
+  // (NMF2D / NMF3D: per (r, t1, t2)); W side [nsplit][C][R][T1][T2][T]
+  const int rc = s->d.one_d() ? launch<kWgrad>(s, s->tmP, dim3_of(s->plan.wgrad), p, st)
+                              : launch<kWgrad, float, true>(s, s->tmP, dim3_of(s->plan.wgrad), p, st);
   *part = s->part; *nsplit = s->ws_w;
   return rc;
 }
 
 int tc_nmfd_dgrad(TcNmfdState* s, const float** part, int* nsplit, cudaStream_t st) {
-  NmfdTcParams p = base_params(s, nullptr);
+  NmfdNdParams p = base_params(s, nullptr);
   p.nsplit = s->ws_h; p.kb_per_split = s->kbs_h;
+  const int64_t lines = (int64_t)s->d.B * s->d.J1() * s->d.J2();
+  const bool nd = !s->d.one_d();
   int rc = 0;
-  for (p.r_off = 0; rc == 0 && p.r_off < s->d.R; p.r_off += 128) rc = launch_slices<kDgrad>(s, s->tmWf, s->plan.dgrad, p, st);
+  for (p.r_off = 0; rc == 0 && p.r_off < s->d.R; p.r_off += 128)
+    rc = nd ? launch_slices<kDgrad, float, true>(s, s->tmWf, s->plan.dgrad, lines, p, st)
+            : launch_slices<kDgrad>(s, s->tmWf, s->plan.dgrad, lines, p, st);
   *part = s->part; *nsplit = s->ws_h;
   return rc;
 }

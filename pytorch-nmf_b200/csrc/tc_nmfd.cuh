@@ -1,5 +1,5 @@
-// NMFD on tcgen05 tensor cores (beta = 1): sliding GEMMs with a Toeplitz operand built in shared memory -- interface used by
-// capi.cu.  See tc_nmfd.cu.
+// NMFD, NMF2D and NMF3D on wgmma tensor cores (beta = 1): sliding GEMMs with a Toeplitz operand built in shared memory --
+// interface used by capi.cu.  See tc_nmfd.cu.
 #pragma once
 #include "common.cuh"
 
@@ -9,7 +9,9 @@ struct TcNmfdState;
 
 // What the tensor-core path launches for a shape, computed in 64 bits before anything is narrowed: the grids of the operand
 // preparation and contraction kernels (recon and dgrad grids per launch: batches beyond grid.z take `slices` launches of at
-// most `bslice` elements each, dgrad one launch per 128 components), split counts and buffer pitches.
+// most `bslice` elements each, dgrad one launch per 128 components), split counts and buffer pitches.  NMF2D / NMF3D
+// (NmfdShape with outer axes): recon's grid.z runs over the B X1 X2 target lines, dgrad's over the B J1 J2 activation lines
+// (`hslices` launches of at most `hslice`); for NMFD both are the batch.
 struct TcNmfdPlan {
   int64_t Tp, padl, Lp, Lq, Cpad;
   int64_t ws_w, kbs_w, ws_h, kbs_h;       // split-K of wgrad / dgrad: splits, k-blocks per split
@@ -17,6 +19,7 @@ struct TcNmfdPlan {
   int64_t nch;                            // 2048-element chunks per H row (prep_h)
   Grid3 prep_w, prep_h, recon, wgrad, dgrad;
   int64_t bslice, slices, dgrad_rblocks;
+  int64_t hslice, hslices;
 };
 // nullptr if every grid and every count the kernels hold in 32 bits fits, else the limit the shape crosses
 const char* tc_nmfd_plan(const NmfdShape& d, TcNmfdPlan* p);

@@ -73,8 +73,10 @@ SIGNATURES = {
     "nmfb200_nmfd_plan": (_int, [_i64, _i64, _int, _c.POINTER(_i64), _i64, _c.POINTER(_i64), _c.POINTER(_i64), _int]),
     "nmfb200_nmf_sparse_plan": (_int, [_i64, _i64, _i64, _c.POINTER(_i64), _int]),
     "nmfb200_nmfd_tc_plan": (_int, [_i64, _i64, _i64, _i64, _i64, _c.POINTER(_i64), _int]),
+    "nmfb200_nmfnd_tc_plan": (_int, [_i64, _i64, _int, _c.POINTER(_i64), _i64, _c.POINTER(_i64), _c.POINTER(_i64), _int]),
 }
 NMF_PLAN_LEN, NMFD_PLAN_LEN, SPARSE_PLAN_LEN, NMFD_TC_PLAN_LEN = 9, 19, 8, 23         # include/nmf_b200.h
+NMFND_TC_PLAN_LEN = 31
 
 _lib = None
 
@@ -155,3 +157,17 @@ def nmfd_tc_plan(B, C, L, R, T):
     return {"prep_w": tuple(v[0:3]), "prep_h": tuple(v[3:6]), "recon": tuple(v[6:9]), "wgrad": tuple(v[9:12]),
             "dgrad": tuple(v[12:15]), "bslice": v[15], "slices": v[16], "dgrad_rblocks": v[17], "loss_blocks": v[18],
             "ws_w": v[19], "kbs_w": v[20], "ws_h": v[21], "kbs_h": v[22]}
+
+
+def nmfnd_tc_plan(B, C, vdims, R, kdims):
+    """The tensor-core kernels' launch plan of an NMFD / NMF2D / NMF3D context (nmfb200_nmfnd_tc_plan), as a dict; no
+    device needed.  `bslice` / `slices` count target lines (b, x1, x2) per recon launch, `hslice` / `hslices` activation
+    lines (b, j1, j2) per dgrad launch.  Raises NmfB200Error naming the limit for a shape the f16 path does not take."""
+    nd = len(vdims)
+    out = (_i64 * NMFND_TC_PLAN_LEN)()
+    check(load().nmfb200_nmfnd_tc_plan(B, C, nd, (_i64 * nd)(*vdims), R, (_i64 * nd)(*kdims), out, NMFND_TC_PLAN_LEN))
+    v = list(out)
+    return {"prep_w": tuple(v[0:3]), "prep_h": tuple(v[3:6]), "recon": tuple(v[6:9]), "wgrad": tuple(v[9:12]),
+            "dgrad": tuple(v[12:15]), "bslice": v[15], "slices": v[16], "dgrad_rblocks": v[17], "loss_blocks": v[18],
+            "ws_w": v[19], "kbs_w": v[20], "ws_h": v[21], "kbs_h": v[22], "hslice": v[23], "hslices": v[24],
+            "Tp": v[25], "padl": v[26], "Lp": v[27], "Lq": v[28], "Cpad": v[29], "nch": v[30]}

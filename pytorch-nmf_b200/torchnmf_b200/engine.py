@@ -73,7 +73,14 @@ def _workspace_bytes(key):
             nx *= x
         for k in K:
             nk *= k
-        return 12 * B * C * nx + 64 * C * R * nk + 64 * B * R * nx
+        est = 12 * B * C * nx + 64 * C * R * nk + 64 * B * R * nx
+        if len(X) > 1 and key[7] == "f16":   # NMF2D / NMF3D fp16 copies: ratio tile lines, W (twice), H lines
+            p = _capi.nmfnd_tc_plan(B, C, X, R, K)
+            lines, klines, hlines = nx // X[-1], nk // K[-1], B * R
+            for x, k in zip(X[:-1], K[:-1]):
+                hlines *= x - k + 1
+            est += 2 * p["Lq"] * B * C * lines + 4 * p["Cpad"] * R * klines * p["Tp"] + 2 * p["Lp"] * hlines
+        return est
     return 0
 
 
@@ -411,8 +418,7 @@ class CudaNmfdEngine(_CudaEngine):
             create = lambda ref: self._lib.nmfb200_nmfd_create(ref, dev_index, B, C, X[0], R, K[0],
                                                                _capi.PRECISIONS[precision])
         else:
-            if precision not in ("auto", "f32"):
-                raise ValueError("NMF2D / NMF3D run on the fp32 kernels: precision must be 'auto' or 'f32'")
+            # "f16": beta 1 on the tensor-core sliding GEMMs; "auto" stays on the fp32 kernels for NMF2D / NMF3D
             vd, kd = (ctypes.c_int64 * nd)(*X), (ctypes.c_int64 * nd)(*K)
             create = lambda ref: self._lib.nmfb200_nmfnd_create(ref, dev_index, B, C, nd, vd, R, kd,
                                                                 _capi.PRECISIONS[precision])

@@ -244,7 +244,9 @@ class BaseComponent(torch.nn.Module):
         `BaseComponent.fit` in the reference (nmf.py:298-409).  Keyword-only extras:
 
         precision: "auto" | "f32" | "f16" | "f16_split" -- arithmetic of the contraction kernels ("auto": fp16
-                   tensor-core operands where the target fits their range, fp32 CUDA cores otherwise)
+                   tensor-core operands where the target fits their range, fp32 CUDA cores otherwise).  NMF2D / NMF3D:
+                   "auto" and "f32" run the fp32 kernels; "f16" runs beta 1 on the tensor-core sliding GEMMs (rank <= 256)
+                   and other betas on the fp32 kernels.  `last_fit_precision` reports what ran.
         group:     a torch.distributed process group; V and H are then this rank's ROW shard
                    (rows of V <-> rows of H) and W is replicated; one all-reduce per W update.
 

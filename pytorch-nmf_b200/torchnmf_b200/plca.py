@@ -125,7 +125,8 @@ class BaseComponent(torch.nn.Module):
         precision: "f32" (default: the fused fp32 CUDA-core contraction, matches the reference to 1e-5 on the fixtures) |
                    "f16" / "f16_split" (wgmma contraction: ~10x faster at large shapes; the EM recursion keeps the
                    fp16 operand rounding, measured 1.0-1.4e-3 relative after 30-50 iterations on the fixtures of
-                   tests/golden/reference_next.npz -- outside the 1e-3 bar, hence opt-in)."""
+                   tests/golden/reference_next.npz -- outside the 1e-3 bar, hence opt-in).  SIPLCA2 / SIPLCA3 at "f16"
+                   run the tensor-core sliding GEMMs of NMFD with the outer axes (rank <= 256)."""
         assert torch.all(V >= 0.), "Target should be non-negative."                         # plca.py:236
         W, H, Z = self.W, self.H, self.Z
         assert W is not None and H is not None and Z is not None, "fit() needs W, H and Z"
