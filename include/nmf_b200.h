@@ -229,6 +229,17 @@ int nmfb200_nmfd_loss(nmfb200_ctx* ctx, const float* W, const float* H, double b
 int64_t nmfb200_nmfd_raw_terms_numel(const nmfb200_ctx* ctx, int which, double beta);
 int nmfb200_nmfd_raw_terms(nmfb200_ctx* ctx, const float* W, const float* H, int which, double beta,
                            float* out, void* stream);
+/* Batch-sharded W update of an NMFD / NMF2D / NMF3D context, the counterpart of nmfb200_nmf_w_partial / _w_apply: every
+ * rank holds a shard of V and H along the batch axis and a replica of W.  _w_partial writes this shard's W terms,
+ * exactly nmfb200_nmfd_raw_terms(which = 0): the raw numerator (C*R*prod(kdims)), then colsum(H_local) (R, beta == 1) or
+ * the raw denominator (C*R*prod(kdims)); _w_partial_numel (-1 for a null or non-NMFD context) is its length.  The caller
+ * sum-all-reduces the buffer and passes it to _w_apply, which runs the ratio stage nmf.py:78-92 on it, identically on
+ * every rank, and leaves the tensor-core state as nmfb200_nmfd_update_w does.  On one rank the pair is
+ * nmfb200_nmfd_update_w bit for bit. */
+int64_t nmfb200_nmfd_w_partial_numel(const nmfb200_ctx* ctx, double beta);
+int nmfb200_nmfd_w_partial(nmfb200_ctx* ctx, const float* W, const float* H, double beta, float* partial, void* stream);
+int nmfb200_nmfd_w_apply(nmfb200_ctx* ctx, float* W, const float* reduced, double beta, double gamma, double l1_reg,
+                         double l2_reg, void* stream);
 /* The caller changed W and / or H in place since the last call (the library keeps fp16 operand copies on the tensor-core
  * path and refreshes only what it knows changed): refresh both at the next call. */
 int nmfb200_nmfd_sync_factors(nmfb200_ctx* ctx);

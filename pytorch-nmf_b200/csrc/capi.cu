@@ -946,6 +946,31 @@ int nmfb200_nmfd_raw_terms(nmfb200_ctx* ctx, const float* W, const float* H, int
   return 0;
 }
 
+int64_t nmfb200_nmfd_w_partial_numel(const nmfb200_ctx* ctx, double beta) {
+  return nmfb200_nmfd_raw_terms_numel(ctx, 0, beta);
+}
+
+// the W terms of this rank's batch shard: the sum of the shards' terms is the whole batch's
+int nmfb200_nmfd_w_partial(nmfb200_ctx* ctx, const float* W, const float* H, double beta, float* partial, void* stream) {
+  return nmfb200_nmfd_raw_terms(ctx, W, H, 0, beta, partial, stream);
+}
+
+// nmfd_update's ratio stage on the summed terms: one slab, the centring term already folded in by raw_sum
+int nmfb200_nmfd_w_apply(nmfb200_ctx* ctx, float* W, const float* reduced, double beta, double gamma, double l1_reg,
+                         double l2_reg, void* stream) {
+  CTX_GUARD(ctx, 1);
+  if (!ctx->has_target) return fail(NMFB200_ERR_STATE, "set_target has not been called");
+  if (!W || !reduced) return fail(NMFB200_ERR_INVALID, "null pointer");
+  cudaStream_t st = (cudaStream_t)stream;
+  ApplyArgs a = nmfd_apply_shape(ctx->d, 0, 1);
+  a.param = W; a.num = reduced; a.gamma = (float)gamma; a.l1 = (float)l1_reg; a.l2 = (float)l2_reg;
+  if (beta == 1.0) a.kl_den = reduced + a.numel;
+  else a.den = reduced + a.numel;
+  if (nmfd_use_tc(ctx, beta)) a.absmax_bits = tc_nmfd_begin_update(ctx->tcd, 0, st);    // as nmfd_update leaves the state
+  else if (ctx->tcd) tc_nmfd_mark_dirty(ctx->tcd);
+  return apply_update(a, st);
+}
+
 int nmfb200_nmfd_loss(nmfb200_ctx* ctx, const float* W, const float* H, double beta, double* loss_dev,
                       void* stream) {
   CTX_GUARD(ctx, 1);

@@ -67,6 +67,9 @@ SIGNATURES = {
     "nmfb200_nmfd_loss": (_int, [_vp, _vp, _vp, _dbl, _vp, _vp]),
     "nmfb200_nmfd_raw_terms_numel": (_i64, [_vp, _int, _dbl]),
     "nmfb200_nmfd_raw_terms": (_int, [_vp, _vp, _vp, _int, _dbl, _vp, _vp]),
+    "nmfb200_nmfd_w_partial_numel": (_i64, [_vp, _dbl]),
+    "nmfb200_nmfd_w_partial": (_int, [_vp, _vp, _vp, _dbl, _vp, _vp]),
+    "nmfb200_nmfd_w_apply": (_int, [_vp, _vp, _vp, _dbl, _dbl, _dbl, _dbl, _vp]),
     "nmfb200_nmfd_sync_factors": (_int, [_vp]),
     "nmfb200_hoyer_project": (_int, [_int, _vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp]),
     "nmfb200_nmf_plan": (_int, [_i64, _i64, _i64, _c.POINTER(_i64), _int]),

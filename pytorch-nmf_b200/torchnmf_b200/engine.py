@@ -1,4 +1,4 @@
-"""Host-side engines: thin owners of an ``nmfb200_ctx`` plus the row-sharded W update.
+"""Host-side engines: thin owners of an ``nmfb200_ctx`` plus the sharded W update.
 
 An engine exposes exactly the operations ``BaseComponent.fit`` (nmf.py:366-407 in the reference)
 needs from its loop body:
@@ -453,14 +453,30 @@ class CudaNmfdEngine(_CudaEngine):
                                                 _stream(self.device)))
         return self._loss
 
+    # --- pieces of the batch-sharded W update -----------------------------------------------
+    def w_partial(self, beta):
+        n = int(self._lib.nmfb200_nmfd_w_partial_numel(self._ctx, beta))
+        buf = self._wbuf
+        if buf is None or buf.numel() != n:           # one buffer per engine, reused every iteration
+            buf = self._wbuf = torch.empty(n, dtype=torch.float32, device=self.device)
+        _capi.check(self._lib.nmfb200_nmfd_w_partial(self._ctx, _ptr(self.W), _ptr(self.H), beta, _ptr(buf),
+                                                     _stream(self.device)))
+        return buf
+
+    def w_apply(self, reduced, beta, gamma, l1_reg, l2_reg):
+        _capi.check(self._lib.nmfb200_nmfd_w_apply(self._ctx, _ptr(self.W), _ptr(reduced), beta, gamma, l1_reg,
+                                                   l2_reg, _stream(self.device)))
+
 
 class ShardedEngine:
-    """Row-sharded NMF over a process group: every rank holds V[n_g,:], H[n_g,:] and a replica of W.
+    """Sharded fit over a process group: every rank holds a shard of V and H and a replica of W -- NMF shards the rows
+    (V[n_g,:], H[n_g,:]), NMFD / NMF2D / NMF3D the batch axis (V[b_g], H[b_g]).
 
     H update and phi stage are local.  The W update is `local raw contraction -> ONE sum-all-reduce ->
     identical ratio stage on every rank` (relu/eps/l1/l2/gamma are applied after the reduction because
     they are not linear).  The loss is one more scalar all-reduce every 10th iteration, and min/max
-    for validation one at entry.  No V or H data ever moves.
+    for validation one at entry.  No V or H data ever moves.  NMF's W update may run over peer memory instead
+    (`_peer_ready`); the convolutive models always take the all-reduce.
     """
 
     def __init__(self, local, group=None):
@@ -498,6 +514,20 @@ class ShardedEngine:
     def _reduce_device(self):
         dev = getattr(self.local, "device", None)
         return dev if dev is not None else torch.device("cpu")
+
+    def check_same_sizes(self, names, sizes):
+        """Collective: raise ValueError on every rank unless every rank passed the same `sizes` (ints; `names` label them
+        in the message), so the W all-reduce never sums buffers of different lengths.  One MIN and one MAX all-reduce."""
+        lo = torch.tensor(sizes, dtype=torch.int64, device=self._reduce_device())
+        hi = lo.clone()
+        self._dist.all_reduce(lo, op=self._dist.ReduceOp.MIN, group=self.group)
+        self._dist.all_reduce(hi, op=self._dist.ReduceOp.MAX, group=self.group)
+        lo, hi = lo.tolist(), hi.tolist()
+        if lo != hi:
+            differ = ", ".join(f"{n} from {a} to {b}" for n, a, b in zip(names, lo, hi) if a != b)
+            mine = ", ".join(f"{n}={s}" for n, s in zip(names, sizes))
+            raise ValueError(f"sharded fit: every rank must have the same sizes past the batch axis, but across ranks {differ} "
+                             f"(this rank: {mine})")
 
     def _peer_ready(self, beta):
         """Collective, once per (engine, beta): may the W update run over peer memory?  Every rank must answer the same, so

@@ -230,9 +230,17 @@ class BaseComponent(torch.nn.Module):
             Wd, Hd = W.data, H.data
             eng = self._engine_factory(V.to_dense() if (sparse_target and not sparse_kernels) else V, Wd, Hd)
         if group is not None:
-            if eng.kind != "nmf":
-                raise NotImplementedError("row sharding is implemented for NMF only (NMFD: replicas only)")
             eng = _engine.ShardedEngine(eng, group)
+            if eng.kind == "nmfd":
+                # batch shards: the W terms' length depends on everything but B (ndim 1 to 3, padded with zeros to 3)
+                nd = V.dim() - 2
+                names = ["ndim", "C", "R"] + [f"kernel_size[{i}]" for i in range(3)] + [f"V.shape[{i + 2}]" for i in range(3)]
+                pad = [0] * (3 - nd)
+                try:
+                    eng.check_same_sizes(names, [nd, V.shape[1], W.shape[1], *W.shape[2:], *pad, *V.shape[2:], *pad])
+                except ValueError:
+                    eng.close()
+                    raise
         return eng, W, H, Wd, Hd, staged
 
     @torch.no_grad()
@@ -247,8 +255,11 @@ class BaseComponent(torch.nn.Module):
                    tensor-core operands where the target fits their range, fp32 CUDA cores otherwise).  NMF2D / NMF3D:
                    "auto" and "f32" run the fp32 kernels; "f16" runs beta 1 on the tensor-core sliding GEMMs (rank <= 256)
                    and other betas on the fp32 kernels.  `last_fit_precision` reports what ran.
-        group:     a torch.distributed process group; V and H are then this rank's ROW shard
-                   (rows of V <-> rows of H) and W is replicated; one all-reduce per W update.
+        group:     a torch.distributed process group; V and H are then this rank's shard and W is replicated, identical
+                   on every rank at entry; one all-reduce per W update.  NMF shards the rows (rows of V <-> rows of H);
+                   NMFD / NMF2D / NMF3D shard the batch axis (V (B_local,C,*X) <-> H (B_local,R,...)), and every rank
+                   must have the same C, R, kernel size and sizes past the batch axis (ValueError otherwise).  Shards may
+                   be uneven.  Each rank resolves precision="auto" from its own shard.
 
         dtype: the kernels keep fp32 master factors and fp32 accumulators.  The reference computes in the module's
         dtype (nmf.py:214-218).  Here a dense bfloat16 / float16 target is read as it is, with no fp32 copy (NMF also
