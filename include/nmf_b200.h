@@ -15,9 +15,12 @@
  * Conventions
  *   - plain C: pointers, sizes, doubles.  No torch / C++ types.
  *   - all matrix pointers are DEVICE pointers to fp32, row-major, reference layout, except that a dense target V may also
- *     hold fp16 or bf16 elements (nmfb200_*_set_target_typed: read where they are, no fp32 copy):
+ *     hold fp16 or bf16 elements (nmfb200_nmf_set_target / nmfb200_nmfd_set_target: read where they are, no fp32 copy):
  *       NMF : V (N,C)   W (C,R)   H (N,R)            V ~= H @ W^T            (nmf.py:659-662)
  *       NMFD: V (B,C,L) W (C,R,T) H (B,R,L-T+1)      V ~= conv1d(H, flip(W)) (nmf.py:743-750)
+ *   - a context holds one model, NMF or NMFD (NMF2D / NMF3D included), fixed by its create call.  The nmfb200_nmf_* and
+ *     nmfb200_nmfd_* calls take only contexts of their model (NMFB200_ERR_INVALID, "wrong context kind", otherwise); the
+ *     calls without a model in their name serve both.
  *   - `stream` is a cudaStream_t passed as void* (0 = legacy default stream).  Every call is
  *     asynchronous on that stream unless documented as synchronising.
  *   - W / H are the caller's storages (the nn.Parameter .data of the reference); updates are
@@ -34,7 +37,9 @@
 extern "C" {
 #endif
 
-#define NMFB200_ABI_VERSION 1
+/* 2: the update / loss / raw-terms / W-apply / sync calls serve both models under one name, and both dense set_target
+ * calls take the target's element type */
+#define NMFB200_ABI_VERSION 2
 
 /* arithmetic mode of the contraction kernels */
 enum {
@@ -44,9 +49,9 @@ enum {
   NMFB200_PREC_F16_SPLIT = 2   /* wgmma, fp16 hi/lo split factors (~22-bit), fp16 ratio tile      */
 };
 
-/* element type of a dense target V (nmfb200_nmf_set_target_typed / nmfb200_nmfd_set_target_typed).  The kernels convert
- * each element to fp32 where they load it; fp16 and bf16 values are exact in fp32, so a half-precision target gives the
- * results, bit for bit, of the same values registered as fp32. */
+/* element type of a dense target V (nmfb200_nmf_set_target / nmfb200_nmfd_set_target).  The kernels convert each element
+ * to fp32 where they load it; fp16 and bf16 values are exact in fp32, so a half-precision target gives the results, bit for
+ * bit, of the same values registered as fp32. */
 enum {
   NMFB200_DTYPE_F32  = 0,
   NMFB200_DTYPE_F16  = 1,      /* IEEE binary16 (__half)        */
@@ -70,11 +75,9 @@ const char* nmfb200_build_info(void);
 /* number of kernels this library has launched in this process (bench.py's gpu_launches) */
 int64_t     nmfb200_launch_count(void);
 
-/* Synchronises `stream` and reports whether any kernel of this library aborted an internal wait (a protocol
- * bug or a wedged device): 0 = healthy, non-zero = the results since the last check are invalid. */
-int nmfb200_check_health(void* stream);
-/* Same, on the context's device (the plain form looks at whichever device is current); the caller's current device is
- * left unchanged, as it is by every entry point that takes a context. */
+/* Synchronises `stream` and reports whether any kernel of this library aborted an internal wait (a protocol bug or a
+ * wedged device), on the context's device: 0 = healthy, non-zero = the results since the last check are invalid.  The
+ * caller's current device is left unchanged, as it is by every entry point that takes a context. */
 int nmfb200_ctx_check_health(nmfb200_ctx* ctx, void* stream);
 
 /* ---- dense NMF ------------------------------------------------------------------------- */
@@ -91,67 +94,27 @@ int nmfb200_precision(const nmfb200_ctx* ctx);
  * rank <= 64 and beta == 1 for rank <= 128; everything else runs the fp32 kernels) */
 int nmfb200_precision_for_beta(const nmfb200_ctx* ctx, double beta);
 
-/* Register the target V (device fp32, leading dimension ldv >= C).  Builds the engine-private
- * operand copies and the V-only loss terms.  Replaces nothing in the reference: V is simply the
- * argument of fit() (nmf.py:299).  Asynchronous. */
-int nmfb200_nmf_set_target(nmfb200_ctx* ctx, const float* V, int64_t ldv, void* stream);
-/* The same for a target of element type `dtype` (NMFB200_DTYPE_*); nmfb200_nmf_set_target is the NMFB200_DTYPE_F32 case.
- * V stays borrowed: every later call of this context (update_*, iterate, loss, loss_prefetch_w, raw_terms, w_partial,
- * contract_only, update_w_peer, target_minmax) reads it.  NMFB200_ERR_INVALID for an unknown dtype or a V not aligned to
- * its element size (2 bytes for fp16 / bf16, 4 for fp32); no other alignment is required. */
-int nmfb200_nmf_set_target_typed(nmfb200_ctx* ctx, const void* V, int64_t ldv, int dtype, void* stream);
+/* Register the target V: device elements of type `dtype` (NMFB200_DTYPE_*), leading dimension ldv >= C.  Builds the
+ * engine-private operand copies and the V-only loss terms.  Replaces nothing in the reference: V is simply the argument of
+ * fit() (nmf.py:299).  V stays borrowed: every later call of this context (update_*, iterate, loss, loss_prefetch_w,
+ * raw_terms, contract_only, update_w_peer, target_minmax) reads it.  NMFB200_ERR_INVALID for an unknown dtype or a V not
+ * aligned to its element size (2 bytes for fp16 / bf16, 4 for fp32); no other alignment is required.  Asynchronous. */
+int nmfb200_nmf_set_target(nmfb200_ctx* ctx, const void* V, int64_t ldv, int dtype, void* stream);
 /* min / max of the registered target (fit()'s validation, nmf.py:329-336).  Synchronises. */
 int nmfb200_target_minmax(nmfb200_ctx* ctx, float* vmin, float* vmax, void* stream);
 
-/* Tell the engine the fp32 factors changed outside its own update calls (fit() entry,
- * load_state_dict, a frozen factor): rebuilds operand copies and column sums.  Asynchronous. */
-int nmfb200_nmf_sync_factors(nmfb200_ctx* ctx, const float* W, const float* H, void* stream);
-
-/* One W update, nmf.py:367-378:  W <- W * ((relu(Pn^T H)+eps) / den)^gamma  in place.
- * l1_reg / l2_reg as computed at nmf.py:348-349; gamma as nmf.py:341-346. */
-int nmfb200_nmf_update_w(nmfb200_ctx* ctx, float* W, const float* H,
-                         double beta, double gamma, double l1_reg, double l2_reg, void* stream);
-/* One H update with the current (already updated) W, nmf.py:380-391. */
-int nmfb200_nmf_update_h(nmfb200_ctx* ctx, const float* W, float* H,
-                         double beta, double gamma, double l1_reg, double l2_reg, void* stream);
 /* n_iter consecutive MU iterations with both factors trainable: exactly n_iter x (update_w; update_h), i.e.
  * nmf.py:366-391 repeated, in one host call. */
 int nmfb200_nmf_iterate(nmfb200_ctx* ctx, float* W, float* H, double beta, double gamma, double l1_reg,
                         double l2_reg, int n_iter, void* stream);
-/* beta_div(H W^T, V, beta) (metrics.py:60-96) accumulated into the DEVICE double *loss_dev
- * (one element, overwritten).  Row shards add: the sum over ranks is the global divergence. */
-int nmfb200_nmf_loss(nmfb200_ctx* ctx, const float* W, const float* H, double beta,
-                     double* loss_dev, void* stream);
-/* The same value, evaluated at the factors the NEXT W update starts from (nmf.py:393-402 runs right before nmf.py:367 of the
+/* nmfb200_loss, evaluated at the factors the NEXT W update starts from (nmf.py:393-402 runs right before nmf.py:367 of the
  * following iteration): on the tensor-core path for beta == 1 the loss sums come out of the W update's own contraction pass
  * (one lg2 per element on the S tile that pass forms anyway, instead of a pass over V of its own), and the next
- * nmfb200_nmf_update_w / nmfb200_nmf_iterate on UNCHANGED factors with the same beta skips its contraction.  Any other
+ * nmfb200_update_w / nmfb200_nmf_iterate on UNCHANGED factors with the same beta skips its contraction.  Any other
  * call in between (or a stop of the fit) simply discards the prefetched numerators.  Elsewhere: identical to
- * nmfb200_nmf_loss. */
+ * nmfb200_loss. */
 int nmfb200_nmf_loss_prefetch_w(nmfb200_ctx* ctx, const float* W, const float* H, double beta,
                                 double* loss_dev, void* stream);
-
-/* Row-sharded W update.  `partial` is a device fp32 buffer of
- * nmfb200_nmf_w_partial_numel() elements receiving this shard's raw numerator (C*R), then either
- * colsum(H_local) (R, beta == 1) or the raw denominator (C*R).  The caller sum-all-reduces it and
- * passes the reduced buffer to _w_apply, which performs nmf.py:78-92 on every rank identically. */
-int64_t nmfb200_nmf_w_partial_numel(const nmfb200_ctx* ctx, double beta);
-int nmfb200_nmf_w_partial(nmfb200_ctx* ctx, const float* W, const float* H, double beta,
-                          float* partial, void* stream);
-/* Raw terms of the multiplicative update of ONE factor (which = 0: W, 1: H), computed from the current W and H without
- * touching either: `out` receives the numerator relu-free (rows*R: the first backward pass of nmf.py:76-78 /
- * trainer.py:91-93), then colsum(other factor) (R, beta == 1: nmf.py:122-131) or the raw denominator (rows*R: the second
- * backward pass, nmf.py:82 / trainer.py:95-96).  This is what torchnmf.trainer.BetaMu.step (trainer.py:36-121) and
- * torchnmf.plca (plca.py:252-253: the simultaneous W / H / Z updates from ONE V / (W Z H) ratio) are built from.
- * A sparse target (nmfb200_nmf_set_target_sparse) serves beta 1 and 2 with the same layout, from the same kernels as its
- * update: the numerator at the non-zeros only, the beta-2 denominator F (other^T other); any other beta returns
- * NMFB200_ERR_INVALID.  One set by nmfb200_nmf_set_target_sparse_any_beta also serves every other beta > 0 (2*rows*R floats:
- * the numerator at the non-zeros, the V-free denominator equal bit for bit to a dense fp32 context's). */
-int64_t nmfb200_nmf_raw_terms_numel(const nmfb200_ctx* ctx, int which, double beta);
-int nmfb200_nmf_raw_terms(nmfb200_ctx* ctx, const float* W, const float* H, int which, double beta,
-                          float* out, void* stream);
-int nmfb200_nmf_w_apply(nmfb200_ctx* ctx, float* W, const float* reduced,
-                        double beta, double gamma, double l1_reg, double l2_reg, void* stream);
 
 /* Sparse target for beta 1 and beta 2 (nmf.py:603-638 `_nmf_sp_recon_beta_pos_neg`, :95-119): registers V (N x C) in both
  * compressed forms -- CSR (crow[N+1], col[nnz], val[nnz]) and CSC = CSR of V^T (ccol[C+1], row[nnz], val_t[nnz]) -- int64
@@ -176,7 +139,7 @@ int nmfb200_nmf_set_target_sparse_any_beta(nmfb200_ctx* ctx, int64_t nnz, const 
                                            double v_norm_kl, double v_norm_eu, void* stream);
 
 /* Row-sharded W update over PEER MEMORY (ranks of one NVLink domain, one process per GPU, 2..8 ranks) -- the fused form of
- * w_partial -> all-reduce -> w_apply above, without a collective library call on the data path:
+ * raw_terms(which = 0) -> all-reduce -> w_apply below, without a collective library call on the data path:
  *   local contraction -> a pack kernel that pushes this rank's partial [C*R | R] into its slot of EVERY rank's exchange block
  *   (posted NVLink writes) and publishes its iteration counter -> ONE ratio-stage kernel per rank that waits for all counters,
  *   sums the slots of its own block in rank order (the replicas of W stay bit-identical) and applies nmf.py:78-92.
@@ -197,52 +160,63 @@ int nmfb200_nmf_update_w_peer(nmfb200_ctx* ctx, float* W, const float* H,
 int nmfb200_nmf_contract_only(nmfb200_ctx* ctx, const float* W, const float* H, int which, double beta,
                               void* stream);
 
-/* ---- NMFD (1-D convolutive NMF) ---------------------------------------------------------- */
+/* ---- NMFD (1-D convolutive NMF), NMF2D, NMF3D ------------------------------------------------ */
 
-/* Sizes as NMFD.__init__ (nmf.py:762-774): V (B,C,L), W (C,R,T), H (B,R,L-T+1). */
-int nmfb200_nmfd_create(nmfb200_ctx** out, int device, int64_t B, int64_t C, int64_t L,
-                        int64_t R, int64_t T, int precision);
-/* NMF2D / NMF3D (nmf.py:782-865, :868-942: conv2d / conv3d with flipped kernels and full padding): the same context type
- * with ndim = 2 or 3 convolved axes.  vdims = the target's sizes over those axes, kdims = kernel_size; V (B,C,*vdims),
- * W (C,R,*kdims), H (B,R,*(vdims - kdims + 1)), all contiguous.  ndim = 1 is nmfb200_nmfd_create.  Every nmfb200_nmfd_*
- * call below serves these contexts.  With ndim 2 or 3, precision auto or f32 runs the fp32 kernels; NMFB200_PREC_F16 runs
- * beta 1 on the tensor-core sliding GEMMs of NMFD, over the outer axes too (R <= 256 and the limits of
- * nmfb200_nmfnd_tc_plan, whose message create returns otherwise), and every other beta on the fp32 kernels, as an NMFD
- * context at f16 does (nmfb200_precision_for_beta says which). */
+/* Sizes as NMFD.__init__ (nmf.py:762-774) with ndim = 1: V (B,C,L), W (C,R,T), H (B,R,L-T+1), vdims = {L}, kdims = {T}.
+ * NMF2D / NMF3D (nmf.py:782-865, :868-942: conv2d / conv3d with flipped kernels and full padding) are the same context type
+ * with ndim = 2 or 3 convolved axes: vdims = the target's sizes over those axes, kdims = kernel_size; V (B,C,*vdims),
+ * W (C,R,*kdims), H (B,R,*(vdims - kdims + 1)), all contiguous.  Every NMFD call serves all three.  With ndim 2 or 3,
+ * precision auto or f32 runs the fp32 kernels; NMFB200_PREC_F16 runs beta 1 on the tensor-core sliding GEMMs of NMFD, over
+ * the outer axes too (R <= 256 and the limits of nmfb200_nmfnd_tc_plan, whose message create returns otherwise), and every
+ * other beta on the fp32 kernels, as an NMFD context at f16 does (nmfb200_precision_for_beta says which). */
 int nmfb200_nmfnd_create(nmfb200_ctx** out, int device, int64_t B, int64_t C, int ndim, const int64_t* vdims,
                          int64_t R, const int64_t* kdims, int precision);
-int nmfb200_nmfd_set_target(nmfb200_ctx* ctx, const float* V, void* stream);
-/* The same for a contiguous target of element type `dtype` (NMFB200_DTYPE_*), with the checks of
- * nmfb200_nmf_set_target_typed; nmfb200_nmfd_set_target is the NMFB200_DTYPE_F32 case. */
-int nmfb200_nmfd_set_target_typed(nmfb200_ctx* ctx, const void* V, int dtype, void* stream);
-int nmfb200_nmfd_update_w(nmfb200_ctx* ctx, float* W, const float* H,
-                          double beta, double gamma, double l1_reg, double l2_reg, void* stream);
-int nmfb200_nmfd_update_h(nmfb200_ctx* ctx, const float* W, float* H,
-                          double beta, double gamma, double l1_reg, double l2_reg, void* stream);
-int nmfb200_nmfd_loss(nmfb200_ctx* ctx, const float* W, const float* H, double beta,
-                      double* loss_dev, void* stream);
-/* The convolutive counterpart of nmfb200_nmf_raw_terms: both backward passes of ONE factor (which = 0: W, 1: H) through
- * the conv1d / conv2d / conv3d reconstruction (nmf.py:776-779, :862-865, :938-942) from the current W and H, neither
- * touched.  `out` = raw numerator (the factor's numel), then colsum(other factor) (R, beta == 1) or the raw denominator
- * (numel).  With W := W * Z this is one EM step's gradients of torchnmf.plca.SIPLCA / SIPLCA2 / SIPLCA3
- * (plca.py:252-253 with the reconstructions :453-455, :534-537, :621-625), and BetaMu.step for the convolutive modules. */
-int64_t nmfb200_nmfd_raw_terms_numel(const nmfb200_ctx* ctx, int which, double beta);
-int nmfb200_nmfd_raw_terms(nmfb200_ctx* ctx, const float* W, const float* H, int which, double beta,
-                           float* out, void* stream);
-/* Batch-sharded W update of an NMFD / NMF2D / NMF3D context, the counterpart of nmfb200_nmf_w_partial / _w_apply: every
- * rank holds a shard of V and H along the batch axis and a replica of W.  _w_partial writes this shard's W terms,
- * exactly nmfb200_nmfd_raw_terms(which = 0): the raw numerator (C*R*prod(kdims)), then colsum(H_local) (R, beta == 1) or
- * the raw denominator (C*R*prod(kdims)); _w_partial_numel (-1 for a null or non-NMFD context) is its length.  The caller
- * sum-all-reduces the buffer and passes it to _w_apply, which runs the ratio stage nmf.py:78-92 on it, identically on
- * every rank, and leaves the tensor-core state as nmfb200_nmfd_update_w does.  On one rank the pair is
- * nmfb200_nmfd_update_w bit for bit. */
-int64_t nmfb200_nmfd_w_partial_numel(const nmfb200_ctx* ctx, double beta);
-int nmfb200_nmfd_w_partial(nmfb200_ctx* ctx, const float* W, const float* H, double beta, float* partial, void* stream);
-int nmfb200_nmfd_w_apply(nmfb200_ctx* ctx, float* W, const float* reduced, double beta, double gamma, double l1_reg,
-                         double l2_reg, void* stream);
-/* The caller changed W and / or H in place since the last call (the library keeps fp16 operand copies on the tensor-core
- * path and refreshes only what it knows changed): refresh both at the next call. */
-int nmfb200_nmfd_sync_factors(nmfb200_ctx* ctx);
+/* Register a contiguous target of element type `dtype` (NMFB200_DTYPE_*), with the checks of nmfb200_nmf_set_target. */
+int nmfb200_nmfd_set_target(nmfb200_ctx* ctx, const void* V, int dtype, void* stream);
+
+/* ---- both models ------------------------------------------------------------------------- */
+
+/* Every call below takes a context of either model and runs that model's kernels.  update_w, update_h, loss, raw_terms and
+ * w_apply return NMFB200_ERR_STATE before the context's set_target*. */
+
+/* Tell the engine the fp32 factors changed outside its own update calls (fit() entry, load_state_dict, a frozen factor,
+ * a line search's trial factors): the tensor-core path keeps fp16 operand copies and refreshes only what it knows changed,
+ * so both are rebuilt at the next call.  No device work. */
+int nmfb200_sync_factors(nmfb200_ctx* ctx);
+
+/* One W update, nmf.py:367-378:  W <- W * ((relu(Pn^T H)+eps) / den)^gamma  in place.
+ * l1_reg / l2_reg as computed at nmf.py:348-349; gamma as nmf.py:341-346. */
+int nmfb200_update_w(nmfb200_ctx* ctx, float* W, const float* H,
+                     double beta, double gamma, double l1_reg, double l2_reg, void* stream);
+/* One H update with the current (already updated) W, nmf.py:380-391. */
+int nmfb200_update_h(nmfb200_ctx* ctx, const float* W, float* H,
+                     double beta, double gamma, double l1_reg, double l2_reg, void* stream);
+/* beta_div of the reconstruction against V (metrics.py:60-96) accumulated into the DEVICE double *loss_dev
+ * (one element, overwritten).  Row / batch shards add: the sum over ranks is the global divergence. */
+int nmfb200_loss(nmfb200_ctx* ctx, const float* W, const float* H, double beta, double* loss_dev, void* stream);
+
+/* Raw terms of the multiplicative update of ONE factor (which = 0: W, 1: H), computed from the current W and H without
+ * touching either: `out` receives the numerator relu-free (the factor's numel: the first backward pass of nmf.py:76-78 /
+ * trainer.py:91-93), then colsum(other factor) (R, beta == 1: nmf.py:122-131) or the raw denominator (the factor's numel:
+ * the second backward pass, nmf.py:82 / trainer.py:95-96); raw_terms_numel (-1 for a null context or a `which` other than
+ * 0 and 1) is its length.  This is what torchnmf.trainer.BetaMu.step (trainer.py:36-121) and torchnmf.plca (plca.py:252-253:
+ * the simultaneous W / H / Z updates from ONE V / (W Z H) ratio) are built from.
+ *   NMFD / NMF2D / NMF3D: both backward passes through the conv1d / conv2d / conv3d reconstruction (nmf.py:776-779,
+ *   :862-865, :938-942).  With W := W * Z this is one EM step's gradients of torchnmf.plca.SIPLCA / SIPLCA2 / SIPLCA3
+ *   (plca.py:252-253 with the reconstructions :453-455, :534-537, :621-625).
+ *   A sparse target (nmfb200_nmf_set_target_sparse) serves beta 1 and 2 with the same layout, from the same kernels as its
+ *   update: the numerator at the non-zeros only, the beta-2 denominator F (other^T other); any other beta returns
+ *   NMFB200_ERR_INVALID.  One set by nmfb200_nmf_set_target_sparse_any_beta also serves every other beta > 0 (2*rows*R
+ *   floats: the numerator at the non-zeros, the V-free denominator equal bit for bit to a dense fp32 context's).
+ * Sharded W update: every rank holds a shard of V and H (NMF: rows, the convolutive models: the batch axis) and a replica
+ * of W.  raw_terms(which = 0) writes this shard's W terms; the caller sum-all-reduces the buffer and passes it to w_apply,
+ * which runs the ratio stage nmf.py:78-92 on it, identically on every rank, and leaves the tensor-core state as update_w
+ * does.  On one rank the pair is update_w bit for bit.  A sparse context gets its W terms too, in the layout and from the
+ * kernels above. */
+int64_t nmfb200_raw_terms_numel(const nmfb200_ctx* ctx, int which, double beta);
+int nmfb200_raw_terms(nmfb200_ctx* ctx, const float* W, const float* H, int which, double beta, float* out, void* stream);
+int nmfb200_w_apply(nmfb200_ctx* ctx, float* W, const float* reduced, double beta, double gamma, double l1_reg,
+                    double l2_reg, void* stream);
 
 /* ---- tile plans of the fp32 CUDA-core kernels (host only: no device work, no allocation) -------- */
 
@@ -271,22 +245,17 @@ int nmfb200_nmf_sparse_plan(int64_t N, int64_t C, int64_t R, int64_t* out, int n
 #define NMFB200_NMFD_PLAN_LEN 19
 int nmfb200_nmfd_plan(int64_t B, int64_t C, int ndim, const int64_t* vdims, int64_t R, const int64_t* kdims,
                       int64_t* out, int n);
-/* What the tensor-core (beta 1) kernels of an NMFD context (arguments as nmfb200_nmfd_create) launch, from the planner
- * those launches use; NMFB200_ERR_INVALID, naming the limit, for a shape that create rejects with precision f16 (and runs on
- * the fp32 kernels with precision auto).  NMFB200_NMFD_TC_PLAN_LEN values:
+/* What the tensor-core (beta 1) kernels of an NMFD / NMF2D / NMF3D context (arguments as nmfb200_nmfnd_create) launch, from
+ * the planner those launches use; NMFB200_ERR_INVALID, naming the limit, for a shape that create rejects with precision f16
+ * (and NMFD runs on the fp32 kernels with precision auto).  NMFB200_NMFND_TC_PLAN_LEN values:
  *   [0..2] prep_w grid   [3..5] prep_h grid   [6..8] recon grid of one launch   [9..11] wgrad grid
- *   [12..14] dgrad grid of one launch   [15] batch elements per recon / dgrad launch (grid z)   [16] launches (batch slices)
- *   [17] dgrad launches per slice (blocks of 128 components)   [18] recon-loss partials
- *   [19] wgrad splits   [20] wgrad k-blocks per split   [21] dgrad splits   [22] dgrad k-blocks per split */
-#define NMFB200_NMFD_TC_PLAN_LEN 23
-int nmfb200_nmfd_tc_plan(int64_t B, int64_t C, int64_t L, int64_t R, int64_t T, int64_t* out, int n);
-/* The same for an NMFD / NMF2D / NMF3D context (arguments as nmfb200_nmfnd_create): NMFB200_ERR_INVALID, naming the limit,
- * for a shape that create rejects with precision f16.  NMFB200_NMFND_TC_PLAN_LEN values: [0..22] as above, where recon's
- * grid z and [15], [16] count target lines (b, x1, x2) and [18] partials over all of them, then
+ *   [12..14] dgrad grid of one launch   [15] target lines (b, x1, x2) per recon launch (grid z)   [16] recon launches
+ *   (line slices)   [17] dgrad launches per slice (blocks of 128 components)   [18] recon-loss partials over all lines
+ *   [19] wgrad splits   [20] wgrad k-blocks per split   [21] dgrad splits   [22] dgrad k-blocks per split
  *   [23] activation lines (b, j1, j2) per dgrad launch (grid z)   [24] dgrad launches (line slices)
  *   [25] Tp (T rounded up to 64)   [26] H copy left margin   [27] H copy row pitch   [28] ratio tile row pitch
  *   [29] C rounded up to 128   [30] 2048-element chunks per H row (prep_h)
- * For ndim = 1 (or all outer sizes 1) [0..22] are nmfb200_nmfd_tc_plan's. */
+ * Whatever the number of axes, a shape whose outer sizes are all 1 plans as its one-axis NMFD shape. */
 #define NMFB200_NMFND_TC_PLAN_LEN 31
 int nmfb200_nmfnd_tc_plan(int64_t B, int64_t C, int ndim, const int64_t* vdims, int64_t R, const int64_t* kdims,
                           int64_t* out, int n);

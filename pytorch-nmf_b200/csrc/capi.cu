@@ -39,7 +39,7 @@ struct nmfb200_ctx {
   int64_t cs_scratch_floats = 0;
   double* loss_blocks = nullptr;
   int loss_max_blocks = 0;
-  float* mm_scratch = nullptr;    // 2048 + 2
+  float* mm_scratch = nullptr;    // kMmFloats: matrix_minmax's partials, then the target's min / max
   // sparse target (beta 1 / 2): borrowed CSR (rows of V) and CSC (= CSR of V^T) forms, V_norm of nmf.py:161-170
   bool sparse = false;
   bool sp_any_beta = false;       // set by nmfb200_nmf_set_target_sparse_any_beta, reset by every other set_target
@@ -81,11 +81,20 @@ struct DeviceGuard {
   DeviceGuard& operator=(const DeviceGuard&) = delete;
 };
 
+// want_kind: 0 = NMF, 1 = NMFD, kAnyKind for the calls that serve both
+constexpr int kAnyKind = -1;
 #define CTX_GUARD(ctx, want_kind)                                                   \
   if (!(ctx)) return fail(NMFB200_ERR_INVALID, "null context");                     \
-  if ((ctx)->kind != (want_kind)) return fail(NMFB200_ERR_INVALID, "wrong context kind"); \
+  if ((want_kind) != kAnyKind && (ctx)->kind != (want_kind))                        \
+    return fail(NMFB200_ERR_INVALID, "wrong context kind");                         \
   DeviceGuard _dev_guard((ctx)->device);                                            \
   if (!_dev_guard.ok) return fail(NMFB200_ERR_CUDA, "cannot select the context's device");
+#define TARGET_GUARD(ctx) \
+  if (!(ctx)->has_target) return fail(NMFB200_ERR_STATE, "set_target has not been called");
+
+// mm_scratch: kMmPartials per-block partials of matrix_minmax, then the target's min / max
+constexpr int kMmPartials = 2048;
+constexpr int kMmFloats = kMmPartials + 2;
 
 // Chunks of the contracted dimension of the fp32 contraction.  Above rank 256 the grid already holds one CTA per rank block
 // (simt_rank_blocks) for every row block and chunk: counting them keeps the nch x rows x R partial slabs from growing with
@@ -117,6 +126,22 @@ void free_ctx(nmfb200_ctx* c) {
   cudaFree(c->loss_blocks); cudaFree(c->mm_scratch); cudaFree(c->Pn); cudaFree(c->Pp);
   cudaFree(c->sp_gram); cudaFree(c->sp_loss_part); cudaFree(c->sp_den);
   delete c;
+}
+
+// The create-time workspace of both kinds, sized from c->part_floats, R, cs_scratch_floats and loss_max_blocks, plus
+// `pn_floats` for NMFD's ratio tile (0: none).  On failure frees `c` and returns the error.
+int alloc_workspace(nmfb200_ctx* c, int64_t pn_floats) {
+  cudaError_t e = cudaMalloc(&c->num, c->part_floats * sizeof(float));
+  if (e == cudaSuccess) e = cudaMalloc(&c->colsum, 2 * c->R * sizeof(float));
+  if (e == cudaSuccess) e = cudaMalloc(&c->cs_scratch, c->cs_scratch_floats * sizeof(float));
+  if (e == cudaSuccess) e = cudaMalloc(&c->loss_blocks, (size_t)c->loss_max_blocks * sizeof(double));
+  if (e == cudaSuccess) e = cudaMalloc(&c->mm_scratch, kMmFloats * sizeof(float));
+  if (e == cudaSuccess && pn_floats) e = cudaMalloc(&c->Pn, pn_floats * sizeof(float));
+  if (e != cudaSuccess) {
+    free_ctx(c);
+    return fail(NMFB200_ERR_CUDA, std::string("cudaMalloc: ") + cudaGetErrorString(e));
+  }
+  return 0;
 }
 
 // CUDA-core contraction of one NMF factor update (which = 0: W, 1: H) into c->num / c->den (chunked partials).
@@ -159,6 +184,29 @@ int check_target(const void* V, int dtype) {
   return 0;
 }
 
+// AUTO keeps heavy-tailed targets (max / mean > 64: spectrogram-like, lognormal, ...) off the tensor cores.  Measured on the
+// lognormal fixtures of tests/golden/reference_r2.npz (30 iterations, tolerance rtol 1e-3): f16 34x, f16_split 2x, f32 0.1x
+// of the tolerance -- MU on such targets converges slowly and keeps the per-update operand rounding instead of averaging it
+// out as it does on well-conditioned data (uniform-like targets: 0.17x after 200 iterations).  `vsum` is the sum of the
+// target's `cells` elements; the max comes from set_target's matrix_minmax.  Synchronises.
+int auto_off_if_heavy_tailed(nmfb200_ctx* ctx, double vsum, double cells, cudaStream_t st) {
+  float mm[2] = {0.f, 0.f};
+  NMF_CUDA_CHECK(cudaMemcpyAsync(mm, ctx->mm_scratch + kMmPartials, sizeof(mm), cudaMemcpyDeviceToHost, st));
+  NMF_CUDA_CHECK(cudaStreamSynchronize(st));
+  const double mean = vsum / cells;
+  ctx->tc_off = !(mean > 0.0) || (double)mm[1] > 64.0 * mean;
+  return 0;
+}
+
+// Synchronises `stream` and reports whether a kernel of this library aborted an internal wait (on the current device).
+int check_health(void* stream) {
+  int rc = tc_check_wait_abort((cudaStream_t)stream);
+  if (rc == 0) rc = tc_nmfd_check_wait_abort();
+  if (rc > 0) return fail(NMFB200_ERR_STATE, "a kernel aborted an internal barrier wait; results are invalid");
+  if (rc < 0) return fail(NMFB200_ERR_CUDA, std::string("stream synchronize: ") + cudaGetErrorString(cudaGetLastError()));
+  return 0;
+}
+
 }  // namespace
 
 extern "C" {
@@ -186,15 +234,7 @@ int nmfb200_ctx_check_health(nmfb200_ctx* ctx, void* stream) {
                                                "'s buffer; results are invalid");
     if (pr < 0) return fail(NMFB200_ERR_CUDA, "stream synchronize failed");
   }
-  return nmfb200_check_health(stream);
-}
-
-int nmfb200_check_health(void* stream) {
-  int rc = tc_check_wait_abort((cudaStream_t)stream);
-  if (rc == 0) rc = tc_nmfd_check_wait_abort();
-  if (rc > 0) return fail(NMFB200_ERR_STATE, "a kernel aborted an internal barrier wait; results are invalid");
-  if (rc < 0) return fail(NMFB200_ERR_CUDA, std::string("stream synchronize: ") + cudaGetErrorString(cudaGetLastError()));
-  return 0;
+  return check_health(stream);
 }
 
 int nmfb200_nmf_create(nmfb200_ctx** out, int device, int64_t N, int64_t C, int64_t R, int precision) {
@@ -224,19 +264,9 @@ int nmfb200_nmf_create(nmfb200_ctx** out, int device, int64_t N, int64_t C, int6
   int64_t pf = (int64_t)c->nch_w * C * R;
   if ((int64_t)c->nch_h * N * R > pf) pf = (int64_t)c->nch_h * N * R;
   c->part_floats = pf;
-  int64_t csf = colsum_scratch_floats(N > C ? N : C, (int)R, 1);
-  c->cs_scratch_floats = csf;
+  c->cs_scratch_floats = colsum_scratch_floats(N > C ? N : C, (int)R, 1);
   c->loss_max_blocks = simt_nmf_max_blocks(N, C);
-  cudaError_t e = cudaSuccess;
-  if (e == cudaSuccess) e = cudaMalloc(&c->num, pf * sizeof(float));
-  if (e == cudaSuccess) e = cudaMalloc(&c->colsum, 2 * R * sizeof(float));
-  if (e == cudaSuccess) e = cudaMalloc(&c->cs_scratch, csf * sizeof(float));
-  if (e == cudaSuccess) e = cudaMalloc(&c->loss_blocks, (size_t)c->loss_max_blocks * sizeof(double));
-  if (e == cudaSuccess) e = cudaMalloc(&c->mm_scratch, 2050 * sizeof(float));
-  if (e != cudaSuccess) {
-    free_ctx(c);
-    return fail(NMFB200_ERR_CUDA, std::string("cudaMalloc: ") + cudaGetErrorString(e));
-  }
+  if (int rc = alloc_workspace(c, 0)) return rc;
   if (resolved != NMFB200_PREC_F32) {
     int rc = tc_create(&c->tc, device, N, C, R, resolved == NMFB200_PREC_F16_SPLIT);
     if (rc) { free_ctx(c); return rc; }
@@ -289,21 +319,18 @@ int nmfb200_nmf_sparse_plan(int64_t N, int64_t C, int64_t R, int64_t* out, int n
   return 0;
 }
 
-int nmfb200_nmf_set_target(nmfb200_ctx* ctx, const float* V, int64_t ldv, void* stream) {
-  return nmfb200_nmf_set_target_typed(ctx, V, ldv, NMFB200_DTYPE_F32, stream);
-}
-
-int nmfb200_nmf_set_target_typed(nmfb200_ctx* ctx, const void* V, int64_t ldv, int dtype, void* stream) {
+int nmfb200_nmf_set_target(nmfb200_ctx* ctx, const void* V, int64_t ldv, int dtype, void* stream) {
   CTX_GUARD(ctx, 0);
   if (!V || ldv < ctx->C) return fail(NMFB200_ERR_INVALID, "bad target pointer / leading dimension");
   if (int rc = check_target(V, dtype)) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   ctx->V = V; ctx->vdtype = dtype; ctx->ldv = ldv; ctx->has_target = true; ctx->sparse = false; ctx->sp_any_beta = false;
-  int rc = matrix_minmax(V, dtype, ctx->N, ctx->C, ldv, ctx->mm_scratch, ctx->mm_scratch + 2048, st);
+  float* minmax = ctx->mm_scratch + kMmPartials;
+  int rc = matrix_minmax(V, dtype, ctx->N, ctx->C, ldv, ctx->mm_scratch, minmax, st);
   if (rc) return rc;
   ctx->tc_off = false;
   if (ctx->tc) {
-    rc = tc_set_target(ctx->tc, V, dtype, ldv, ctx->mm_scratch + 2048, st);
+    rc = tc_set_target(ctx->tc, V, dtype, ldv, minmax, st);
     if (rc) return rc;
     if (ctx->auto_mode) {
       // AUTO is conservative: the fp16 copy of V carries ONE power-of-two scale (max -> 2^14), so positive entries below
@@ -315,19 +342,11 @@ int nmfb200_nmf_set_target_typed(nmfb200_ctx* ctx, const void* V, int64_t ldv, i
       if (rc) return rc;
       // a handful of tiny entries in a 10^8-cell matrix carry no structure; a quiet row / band (>= 1e-6 of the cells) does
       ctx->tc_off = (double)lossy > 1e-6 * (double)ctx->N * (double)ctx->C;
-      // ... and for heavy-tailed targets (max / mean > 64: spectrogram-like, lognormal, ...).  Measured on the lognormal
-      // fixtures of tests/golden/reference_r2.npz (30 iterations, tolerance rtol 1e-3): f16 34x, f16_split 2x, f32 0.1x of
-      // the tolerance -- MU on such targets converges slowly and keeps the per-update operand rounding instead of
-      // averaging it out as it does on well-conditioned data (uniform-like targets: 0.17x after 200 iterations).
-      if (!ctx->tc_off) {
+      if (!ctx->tc_off) {       // ... and for heavy-tailed targets
         double vsum = 0.0;
-        float mm[2] = {0.f, 0.f};
         rc = tc_target_sum(ctx->tc, &vsum, st);
         if (rc) return rc;
-        NMF_CUDA_CHECK(cudaMemcpyAsync(mm, ctx->mm_scratch + 2048, sizeof(mm), cudaMemcpyDeviceToHost, st));
-        NMF_CUDA_CHECK(cudaStreamSynchronize(st));
-        const double mean = vsum / ((double)ctx->N * (double)ctx->C);
-        ctx->tc_off = !(mean > 0.0) || (double)mm[1] > 64.0 * mean;
+        return auto_off_if_heavy_tailed(ctx, vsum, (double)ctx->N * (double)ctx->C, st);
       }
     }
   }
@@ -374,7 +393,7 @@ int nmfb200_nmf_set_target_sparse_any_beta(nmfb200_ctx* ctx, int64_t nnz, const 
 namespace {
 // Raw terms of one factor's update on the compressed form whose segments are that factor's rows (which = 0: W over CSC,
 // 1: H over CSR): the numerator (rows x R) into `num`; into `den` the colsum of the other factor (R, beta 1) or the raw
-// denominator F (other^T other) (rows x R, beta 2).  Shared by the update and nmfb200_nmf_raw_terms.
+// denominator F (other^T other) (rows x R, beta 2).  Shared by the update and nmfb200_raw_terms.
 // beta 1 and 2 run on every sparse context; any other beta > 0 only on one set by nmfb200_nmf_set_target_sparse_any_beta
 int check_sparse_beta(const nmfb200_ctx* ctx, double beta) {
   if (beta == 1.0 || beta == 2.0) return 0;
@@ -445,7 +464,7 @@ int nmf_update(nmfb200_ctx* ctx, int which, float* param, const float* W, const 
   return 0;
 }
 
-// The raw terms of one factor's update (which = 0: W, 1: H) into `out`, nmfb200_nmf_raw_terms_numel floats.
+// The raw terms of one factor's update (which = 0: W, 1: H) into `out`, nmfb200_raw_terms_numel floats.
 int nmf_raw_terms(nmfb200_ctx* ctx, const float* W, const float* H, int which, double beta, float* out, cudaStream_t st) {
   const int64_t rows = which == 0 ? ctx->C : ctx->N;
   const int64_t RR = rows * ctx->R;
@@ -495,42 +514,19 @@ int nmfb200_target_minmax(nmfb200_ctx* ctx, float* vmin, float* vmax, void* stre
   if (!ctx) return fail(NMFB200_ERR_INVALID, "null context");
   DeviceGuard guard(ctx->device);
   if (!guard.ok) return fail(NMFB200_ERR_CUDA, "cannot select the context's device");
-  if (!ctx->has_target) return fail(NMFB200_ERR_STATE, "set_target has not been called");
+  TARGET_GUARD(ctx);
   float mm[2];
-  NMF_CUDA_CHECK(cudaMemcpyAsync(mm, ctx->mm_scratch + 2048, sizeof(mm), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
+  NMF_CUDA_CHECK(cudaMemcpyAsync(mm, ctx->mm_scratch + kMmPartials, sizeof(mm), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
   NMF_CUDA_CHECK(cudaStreamSynchronize((cudaStream_t)stream));
   if (vmin) *vmin = mm[0];
   if (vmax) *vmax = mm[1];
   return 0;
 }
 
-int nmfb200_nmf_sync_factors(nmfb200_ctx* ctx, const float* W, const float* H, void* stream) {
-  CTX_GUARD(ctx, 0);
-  if (!W || !H) return fail(NMFB200_ERR_INVALID, "null factor pointer");
-  if (ctx->tc) tc_mark_dirty(ctx->tc, true, true);
-  return 0;   // operand copies are rebuilt lazily; the CUDA-core path reads the fp32 factors directly
-}
-
-int nmfb200_nmf_update_w(nmfb200_ctx* ctx, float* W, const float* H, double beta, double gamma, double l1_reg,
-                         double l2_reg, void* stream) {
-  CTX_GUARD(ctx, 0);
-  if (!ctx->has_target) return fail(NMFB200_ERR_STATE, "set_target has not been called");
-  if (!W || !H) return fail(NMFB200_ERR_INVALID, "null factor pointer");
-  return nmf_update(ctx, 0, W, W, H, beta, gamma, l1_reg, l2_reg, (cudaStream_t)stream);
-}
-
-int nmfb200_nmf_update_h(nmfb200_ctx* ctx, const float* W, float* H, double beta, double gamma, double l1_reg,
-                         double l2_reg, void* stream) {
-  CTX_GUARD(ctx, 0);
-  if (!ctx->has_target) return fail(NMFB200_ERR_STATE, "set_target has not been called");
-  if (!W || !H) return fail(NMFB200_ERR_INVALID, "null factor pointer");
-  return nmf_update(ctx, 1, H, W, H, beta, gamma, l1_reg, l2_reg, (cudaStream_t)stream);
-}
-
 int nmfb200_nmf_iterate(nmfb200_ctx* ctx, float* W, float* H, double beta, double gamma, double l1_reg,
                         double l2_reg, int n_iter, void* stream) {
   CTX_GUARD(ctx, 0);
-  if (!ctx->has_target) return fail(NMFB200_ERR_STATE, "set_target has not been called");
+  TARGET_GUARD(ctx);
   if (!W || !H || n_iter < 0) return fail(NMFB200_ERR_INVALID, "bad argument");
   cudaStream_t st = (cudaStream_t)stream;
   for (int i = 0; i < n_iter; ++i) {
@@ -542,53 +538,14 @@ int nmfb200_nmf_iterate(nmfb200_ctx* ctx, float* W, float* H, double beta, doubl
   return 0;
 }
 
-int nmfb200_nmf_loss(nmfb200_ctx* ctx, const float* W, const float* H, double beta, double* loss_dev,
-                     void* stream) {
-  CTX_GUARD(ctx, 0);
-  if (!ctx->has_target) return fail(NMFB200_ERR_STATE, "set_target has not been called");
-  if (!W || !H || !loss_dev) return fail(NMFB200_ERR_INVALID, "null pointer");
-  cudaStream_t st = (cudaStream_t)stream;
-  if (ctx->sparse) return sparse_loss_ctx(ctx, W, H, beta, loss_dev, st);
-  if (use_tc(ctx, beta)) return tc_loss(ctx->tc, W, H, beta, loss_dev, st);
-  return simt_nmf_loss(ctx->V, ctx->vdtype, ctx->ldv, H, W, ctx->N, ctx->C, (int)ctx->R, beta, ctx->loss_blocks,
-                       ctx->loss_max_blocks, loss_dev, st);
-}
-
 int nmfb200_nmf_loss_prefetch_w(nmfb200_ctx* ctx, const float* W, const float* H, double beta, double* loss_dev,
                                 void* stream) {
   CTX_GUARD(ctx, 0);
-  if (!ctx->has_target) return fail(NMFB200_ERR_STATE, "set_target has not been called");
+  TARGET_GUARD(ctx);
   if (!W || !H || !loss_dev) return fail(NMFB200_ERR_INVALID, "null pointer");
   if (!ctx->sparse && use_tc(ctx, beta))
     return tc_loss_prefetch_w(ctx->tc, W, H, beta, loss_dev, (cudaStream_t)stream);
-  return nmfb200_nmf_loss(ctx, W, H, beta, loss_dev, stream);
-}
-
-int64_t nmfb200_nmf_w_partial_numel(const nmfb200_ctx* ctx, double beta) {
-  return nmfb200_nmf_raw_terms_numel(ctx, 0, beta);
-}
-
-int nmfb200_nmf_w_partial(nmfb200_ctx* ctx, const float* W, const float* H, double beta, float* partial,
-                          void* stream) {
-  CTX_GUARD(ctx, 0);
-  if (!ctx->has_target) return fail(NMFB200_ERR_STATE, "set_target has not been called");
-  if (ctx->sparse) return fail(NMFB200_ERR_STATE, "not available for a sparse target");
-  if (!W || !H || !partial) return fail(NMFB200_ERR_INVALID, "null pointer");
-  return nmf_raw_terms(ctx, W, H, 0, beta, partial, (cudaStream_t)stream);
-}
-
-int64_t nmfb200_nmf_raw_terms_numel(const nmfb200_ctx* ctx, int which, double beta) {
-  if (!ctx || ctx->kind != 0 || (which != 0 && which != 1)) return -1;
-  const int64_t rows = which == 0 ? ctx->C : ctx->N;
-  return beta == 1.0 ? rows * ctx->R + ctx->R : 2 * rows * ctx->R;
-}
-
-int nmfb200_nmf_raw_terms(nmfb200_ctx* ctx, const float* W, const float* H, int which, double beta, float* out,
-                          void* stream) {
-  CTX_GUARD(ctx, 0);
-  if (!ctx->has_target) return fail(NMFB200_ERR_STATE, "set_target has not been called");
-  if (!W || !H || !out || (which != 0 && which != 1)) return fail(NMFB200_ERR_INVALID, "bad argument");
-  return nmf_raw_terms(ctx, W, H, which, beta, out, (cudaStream_t)stream);
+  return nmfb200_loss(ctx, W, H, beta, loss_dev, stream);
 }
 
 /* ---- row-sharded W update over peer memory (NVLink, one process per GPU) ---------------------- */
@@ -625,28 +582,16 @@ int nmfb200_nmf_peer_release(nmfb200_ctx* ctx) {
 int nmfb200_nmf_update_w_peer(nmfb200_ctx* ctx, float* W, const float* H, double beta, double gamma, double l1_reg,
                               double l2_reg, void* stream) {
   CTX_GUARD(ctx, 0);
-  if (!ctx->has_target) return fail(NMFB200_ERR_STATE, "set_target has not been called");
+  TARGET_GUARD(ctx);
   if (!W || !H) return fail(NMFB200_ERR_INVALID, "null factor pointer");
   if (!nmfb200_nmf_peer_supported(ctx, beta)) return fail(NMFB200_ERR_STATE, "peer-memory W update is not available for this context / beta");
   return tc_update_w_peer(ctx->tc, W, H, beta, gamma, l1_reg, l2_reg, (cudaStream_t)stream);
 }
 
-int nmfb200_nmf_w_apply(nmfb200_ctx* ctx, float* W, const float* reduced, double beta, double gamma,
-                        double l1_reg, double l2_reg, void* stream) {
-  CTX_GUARD(ctx, 0);
-  if (!W || !reduced) return fail(NMFB200_ERR_INVALID, "null pointer");
-  cudaStream_t st = (cudaStream_t)stream;
-  if (use_tc(ctx, beta)) return tc_w_apply(ctx->tc, W, reduced, beta, gamma, l1_reg, l2_reg, st);
-  int rc = apply_update(nmf_apply_args(ctx, 0, W, beta, reduced, reduced + ctx->C * ctx->R, 1, 0, gamma, l1_reg, l2_reg), st);
-  if (rc) return rc;
-  if (ctx->tc) tc_mark_dirty(ctx->tc, true, false);
-  return 0;
-}
-
 int nmfb200_nmf_contract_only(nmfb200_ctx* ctx, const float* W, const float* H, int which, double beta,
                               void* stream) {
   CTX_GUARD(ctx, 0);
-  if (!ctx->has_target) return fail(NMFB200_ERR_STATE, "set_target has not been called");
+  TARGET_GUARD(ctx);
   if (ctx->sparse) return fail(NMFB200_ERR_STATE, "not available for a sparse target");
   if (!W || !H) return fail(NMFB200_ERR_INVALID, "null factor pointer");
   cudaStream_t st = (cudaStream_t)stream;
@@ -697,8 +642,8 @@ static ApplyArgs nmfd_apply_shape(const NmfdShape& d, int which, int nsplit) {
   return a;
 }
 
-static int nmfd_create_impl(nmfb200_ctx** out, int device, int64_t B, int64_t C, int ndim, const int64_t* vdims,
-                            int64_t R, const int64_t* kdims, int precision) {
+int nmfb200_nmfnd_create(nmfb200_ctx** out, int device, int64_t B, int64_t C, int ndim, const int64_t* vdims,
+                         int64_t R, const int64_t* kdims, int precision) {
   if (!out) return fail(NMFB200_ERR_INVALID, "out is null");
   *out = nullptr;
   NmfdShape shape;
@@ -726,17 +671,7 @@ static int nmfd_create_impl(nmfb200_ctx** out, int device, int64_t B, int64_t C,
   int64_t cs1 = colsum_scratch_floats(C, (int)R, c->d.w_inner()), cs2 = colsum_scratch_floats(B, (int)R, c->d.h_inner());
   c->cs_scratch_floats = cs1 > cs2 ? cs1 : cs2;
   c->loss_max_blocks = (int)nmfd_max_blocks(c->d);         // bounded by nmfd_shape_of
-  cudaError_t e = cudaSuccess;
-  if (e == cudaSuccess) e = cudaMalloc(&c->num, pf * sizeof(float));
-  if (e == cudaSuccess) e = cudaMalloc(&c->colsum, 2 * R * sizeof(float));
-  if (e == cudaSuccess) e = cudaMalloc(&c->cs_scratch, c->cs_scratch_floats * sizeof(float));
-  if (e == cudaSuccess) e = cudaMalloc(&c->loss_blocks, (size_t)c->loss_max_blocks * sizeof(double));
-  if (e == cudaSuccess) e = cudaMalloc(&c->mm_scratch, 2050 * sizeof(float));
-  if (e == cudaSuccess) e = cudaMalloc(&c->Pn, (size_t)B * C * c->d.v_inner() * sizeof(float));
-  if (e != cudaSuccess) {
-    free_ctx(c);
-    return fail(NMFB200_ERR_CUDA, std::string("cudaMalloc: ") + cudaGetErrorString(e));
-  }
+  if (int rc = alloc_workspace(c, B * C * c->d.v_inner())) return rc;
   if (c->precision != NMFB200_PREC_F32 && !tc_limit) {    // NMFD at auto / f16, NMF2D / NMF3D at f16
     cudaDeviceProp prop;
     if (cudaGetDeviceProperties(&prop, device) == cudaSuccess && prop.major == 9) {
@@ -751,27 +686,13 @@ static int nmfd_create_impl(nmfb200_ctx** out, int device, int64_t B, int64_t C,
   return 0;
 }
 
-int nmfb200_nmfd_create(nmfb200_ctx** out, int device, int64_t B, int64_t C, int64_t L, int64_t R, int64_t T,
-                        int precision) {
-  return nmfd_create_impl(out, device, B, C, 1, &L, R, &T, precision);
-}
-
-int nmfb200_nmfnd_create(nmfb200_ctx** out, int device, int64_t B, int64_t C, int ndim, const int64_t* vdims,
-                         int64_t R, const int64_t* kdims, int precision) {
-  return nmfd_create_impl(out, device, B, C, ndim, vdims, R, kdims, precision);
-}
-
-int nmfb200_nmfd_set_target(nmfb200_ctx* ctx, const float* V, void* stream) {
-  return nmfb200_nmfd_set_target_typed(ctx, V, NMFB200_DTYPE_F32, stream);
-}
-
-int nmfb200_nmfd_set_target_typed(nmfb200_ctx* ctx, const void* V, int dtype, void* stream) {
+int nmfb200_nmfd_set_target(nmfb200_ctx* ctx, const void* V, int dtype, void* stream) {
   CTX_GUARD(ctx, 1);
   if (int rc = check_target(V, dtype)) return rc;
   ctx->V = V; ctx->vdtype = dtype; ctx->has_target = true;
   cudaStream_t st = (cudaStream_t)stream;
   const int64_t vin = ctx->d.v_inner();
-  int rc = matrix_minmax(V, dtype, (int64_t)ctx->d.B * ctx->d.C, vin, vin, ctx->mm_scratch, ctx->mm_scratch + 2048, st);
+  int rc = matrix_minmax(V, dtype, (int64_t)ctx->d.B * ctx->d.C, vin, vin, ctx->mm_scratch, ctx->mm_scratch + kMmPartials, st);
   if (rc) return rc;
   ctx->tc_off = false;
   if (ctx->tcd) {
@@ -779,13 +700,8 @@ int nmfb200_nmfd_set_target_typed(nmfb200_ctx* ctx, const void* V, int dtype, vo
     rc = tc_nmfd_set_target(ctx->tcd, V, dtype, &vsum, st);       // synchronises: sum(V) for kappa
     if (rc) return rc;
     tc_nmfd_mark_dirty(ctx->tcd);                         // a new fit: the factors may be anything
-    if (ctx->auto_mode) {                                 // same conservative rule as the NMF path: heavy-tailed targets stay fp32
-      float mm[2] = {0.f, 0.f};
-      NMF_CUDA_CHECK(cudaMemcpyAsync(mm, ctx->mm_scratch + 2048, sizeof(mm), cudaMemcpyDeviceToHost, st));
-      NMF_CUDA_CHECK(cudaStreamSynchronize(st));
-      const double mean = vsum / ((double)ctx->d.B * ctx->d.C * ctx->d.v_inner());
-      ctx->tc_off = !(mean > 0.0) || (double)mm[1] > 64.0 * mean;
-    }
+    if (ctx->auto_mode)                                   // same conservative rule as the NMF path: heavy-tailed targets stay fp32
+      return auto_off_if_heavy_tailed(ctx, vsum, (double)ctx->d.B * ctx->d.C * ctx->d.v_inner(), st);
   }
   return 0;
 }
@@ -793,9 +709,6 @@ int nmfb200_nmfd_set_target_typed(nmfb200_ctx* ctx, const void* V, int dtype, vo
 // beta = 1 on tensor cores: both column-sum vectors (KL denominators, nmf.py:122-131, and kappa), then the recon pass
 static bool nmfd_use_tc(const nmfb200_ctx* c, double beta) {
   return c->tcd != nullptr && !c->tc_off && tc_nmfd_supported(c->d, beta);
-}
-static int nmfd_tc_recon(nmfb200_ctx* c, const float* W, const float* H, bool loss, double* loss_dev, cudaStream_t st) {
-  return tc_nmfd_recon(c->tcd, c->V, c->vdtype, W, H, loss, loss_dev, st);
 }
 
 static int nmfd_phi(nmfb200_ctx* c, const float* W, const float* H, double beta, cudaStream_t st) {
@@ -809,14 +722,14 @@ static int nmfd_phi(nmfb200_ctx* c, const float* W, const float* H, double beta,
 
 // Both backward passes of one factor (which = 0: W, 1: H) from the current factors, described as the ratio stage's input:
 // split partial numerators (+ denominators for beta != 1), the KL column sums, the centring term of the tensor-core path.
-// Shared by the update (nmf.py:367-391) and by nmfb200_nmfd_raw_terms.  `tc` reports which path produced the terms.
+// Shared by the update (nmf.py:367-391) and by nmfd_raw_terms.  `tc` reports which path produced the terms.
 static int nmfd_terms(nmfb200_ctx* ctx, const float* W, const float* H, int which, double beta, ApplyArgs& a, bool* tc,
                       cudaStream_t st) {
   const NmfdShape& d = ctx->d;
   a = nmfd_apply_shape(d, which, 1);
   *tc = nmfd_use_tc(ctx, beta);
   if (*tc) {
-    int rc = nmfd_tc_recon(ctx, W, H, false, nullptr, st);
+    int rc = tc_nmfd_recon(ctx->tcd, ctx->V, ctx->vdtype, W, H, false, nullptr, st);
     if (rc) return rc;
     const float* part; int nsplit;
     rc = which == 0 ? tc_nmfd_wgrad(ctx->tcd, &part, &nsplit, st) : tc_nmfd_dgrad(ctx->tcd, &part, &nsplit, st);
@@ -862,20 +775,6 @@ int nmfb200_nmfd_plan(int64_t B, int64_t C, int ndim, const int64_t* vdims, int6
   return 0;
 }
 
-int nmfb200_nmfd_tc_plan(int64_t B, int64_t C, int64_t L, int64_t R, int64_t T, int64_t* out, int n) {
-  if (!out || n < NMFB200_NMFD_TC_PLAN_LEN) return fail(NMFB200_ERR_INVALID, "plan buffer too small");
-  NmfdShape d;
-  if (int rc = nmfd_shape_of(B, C, 1, &L, R, &T, &d)) return rc;
-  TcNmfdPlan p;
-  if (const char* why = tc_nmfd_plan(d, &p)) return fail(NMFB200_ERR_INVALID, why);
-  const int64_t v[NMFB200_NMFD_TC_PLAN_LEN] = {
-      p.prep_w.x, p.prep_w.y, p.prep_w.z, p.prep_h.x, p.prep_h.y, p.prep_h.z, p.recon.x, p.recon.y, p.recon.z,
-      p.wgrad.x, p.wgrad.y, p.wgrad.z, p.dgrad.x, p.dgrad.y, p.dgrad.z, p.bslice, p.slices, p.dgrad_rblocks,
-      p.loss_blocks, p.ws_w, p.kbs_w, p.ws_h, p.kbs_h};
-  for (int i = 0; i < NMFB200_NMFD_TC_PLAN_LEN; ++i) out[i] = v[i];
-  return 0;
-}
-
 int nmfb200_nmfnd_tc_plan(int64_t B, int64_t C, int ndim, const int64_t* vdims, int64_t R, const int64_t* kdims,
                           int64_t* out, int n) {
   if (!out || n < NMFB200_NMFND_TC_PLAN_LEN) return fail(NMFB200_ERR_INVALID, "plan buffer too small");
@@ -901,41 +800,10 @@ static int nmfd_update(nmfb200_ctx* ctx, const float* W, const float* H, int whi
   return apply_update(a, st);
 }
 
-int nmfb200_nmfd_update_w(nmfb200_ctx* ctx, float* W, const float* H, double beta, double gamma, double l1_reg,
-                          double l2_reg, void* stream) {
-  CTX_GUARD(ctx, 1);
-  if (!ctx->has_target) return fail(NMFB200_ERR_STATE, "set_target has not been called");
-  if (!W || !H) return fail(NMFB200_ERR_INVALID, "null factor pointer");
-  return nmfd_update(ctx, W, H, 0, W, beta, gamma, l1_reg, l2_reg, (cudaStream_t)stream);
-}
-
-int nmfb200_nmfd_update_h(nmfb200_ctx* ctx, const float* W, float* H, double beta, double gamma, double l1_reg,
-                          double l2_reg, void* stream) {
-  CTX_GUARD(ctx, 1);
-  if (!ctx->has_target) return fail(NMFB200_ERR_STATE, "set_target has not been called");
-  if (!W || !H) return fail(NMFB200_ERR_INVALID, "null factor pointer");
-  return nmfd_update(ctx, W, H, 1, H, beta, gamma, l1_reg, l2_reg, (cudaStream_t)stream);
-}
-
-int nmfb200_nmfd_sync_factors(nmfb200_ctx* ctx) {
-  CTX_GUARD(ctx, 1);
-  if (ctx->tcd) tc_nmfd_mark_dirty(ctx->tcd);
-  return 0;
-}
-
-int64_t nmfb200_nmfd_raw_terms_numel(const nmfb200_ctx* ctx, int which, double beta) {
-  if (!ctx || ctx->kind != 1 || (which != 0 && which != 1)) return -1;
-  const NmfdShape& d = ctx->d;
-  const int64_t n = (int64_t)(which == 0 ? d.C : d.B) * d.R * (which == 0 ? d.w_inner() : d.h_inner());
-  return beta == 1.0 ? n + d.R : 2 * n;
-}
-
-int nmfb200_nmfd_raw_terms(nmfb200_ctx* ctx, const float* W, const float* H, int which, double beta, float* out,
-                           void* stream) {
-  CTX_GUARD(ctx, 1);
-  if (!ctx->has_target) return fail(NMFB200_ERR_STATE, "set_target has not been called");
-  if (!W || !H || !out || (which != 0 && which != 1)) return fail(NMFB200_ERR_INVALID, "bad argument");
-  cudaStream_t st = (cudaStream_t)stream;
+// The raw terms of one factor's update (which = 0: W, 1: H) into `out`, nmfb200_raw_terms_numel floats: the split partials
+// summed with the centring term folded in (raw_sum), then the KL column sums at beta 1.
+static int nmfd_raw_terms(nmfb200_ctx* ctx, const float* W, const float* H, int which, double beta, float* out,
+                          cudaStream_t st) {
   ApplyArgs a; bool tc;
   int rc = nmfd_terms(ctx, W, H, which, beta, a, &tc, st);
   if (rc) return rc;
@@ -946,39 +814,91 @@ int nmfb200_nmfd_raw_terms(nmfb200_ctx* ctx, const float* W, const float* H, int
   return 0;
 }
 
-int64_t nmfb200_nmfd_w_partial_numel(const nmfb200_ctx* ctx, double beta) {
-  return nmfb200_nmfd_raw_terms_numel(ctx, 0, beta);
+/* ---- both kinds: the arguments are checked once, then the context's own kernels run ------------------------ */
+
+int nmfb200_sync_factors(nmfb200_ctx* ctx) {
+  CTX_GUARD(ctx, kAnyKind);
+  // operand copies are rebuilt lazily; the CUDA-core paths read the fp32 factors directly
+  if (ctx->tc) tc_mark_dirty(ctx->tc, true, true);
+  if (ctx->tcd) tc_nmfd_mark_dirty(ctx->tcd);
+  return 0;
 }
 
-// the W terms of this rank's batch shard: the sum of the shards' terms is the whole batch's
-int nmfb200_nmfd_w_partial(nmfb200_ctx* ctx, const float* W, const float* H, double beta, float* partial, void* stream) {
-  return nmfb200_nmfd_raw_terms(ctx, W, H, 0, beta, partial, stream);
+// update_w / update_h: one factor update (which = 0: param = W, 1: param = H)
+static int update_factor(nmfb200_ctx* ctx, int which, float* param, const float* W, const float* H, double beta,
+                         double gamma, double l1_reg, double l2_reg, void* stream) {
+  CTX_GUARD(ctx, kAnyKind);
+  TARGET_GUARD(ctx);
+  if (!W || !H) return fail(NMFB200_ERR_INVALID, "null factor pointer");
+  cudaStream_t st = (cudaStream_t)stream;
+  if (ctx->kind == 0) return nmf_update(ctx, which, param, W, H, beta, gamma, l1_reg, l2_reg, st);
+  return nmfd_update(ctx, W, H, which, param, beta, gamma, l1_reg, l2_reg, st);
 }
 
-// nmfd_update's ratio stage on the summed terms: one slab, the centring term already folded in by raw_sum
-int nmfb200_nmfd_w_apply(nmfb200_ctx* ctx, float* W, const float* reduced, double beta, double gamma, double l1_reg,
-                         double l2_reg, void* stream) {
-  CTX_GUARD(ctx, 1);
-  if (!ctx->has_target) return fail(NMFB200_ERR_STATE, "set_target has not been called");
+int nmfb200_update_w(nmfb200_ctx* ctx, float* W, const float* H, double beta, double gamma, double l1_reg, double l2_reg,
+                     void* stream) {
+  return update_factor(ctx, 0, W, W, H, beta, gamma, l1_reg, l2_reg, stream);
+}
+
+int nmfb200_update_h(nmfb200_ctx* ctx, const float* W, float* H, double beta, double gamma, double l1_reg, double l2_reg,
+                     void* stream) {
+  return update_factor(ctx, 1, H, W, H, beta, gamma, l1_reg, l2_reg, stream);
+}
+
+int nmfb200_loss(nmfb200_ctx* ctx, const float* W, const float* H, double beta, double* loss_dev, void* stream) {
+  CTX_GUARD(ctx, kAnyKind);
+  TARGET_GUARD(ctx);
+  if (!W || !H || !loss_dev) return fail(NMFB200_ERR_INVALID, "null pointer");
+  cudaStream_t st = (cudaStream_t)stream;
+  if (ctx->kind == 1) {
+    if (nmfd_use_tc(ctx, beta)) return tc_nmfd_recon(ctx->tcd, ctx->V, ctx->vdtype, W, H, true, loss_dev, st);
+    return nmfd_recon_phi(ctx->d, ctx->V, ctx->vdtype, W, H, beta, nullptr, nullptr, ctx->loss_blocks, ctx->loss_max_blocks,
+                          loss_dev, st);
+  }
+  if (ctx->sparse) return sparse_loss_ctx(ctx, W, H, beta, loss_dev, st);
+  if (use_tc(ctx, beta)) return tc_loss(ctx->tc, W, H, beta, loss_dev, st);
+  return simt_nmf_loss(ctx->V, ctx->vdtype, ctx->ldv, H, W, ctx->N, ctx->C, (int)ctx->R, beta, ctx->loss_blocks,
+                       ctx->loss_max_blocks, loss_dev, st);
+}
+
+int64_t nmfb200_raw_terms_numel(const nmfb200_ctx* ctx, int which, double beta) {
+  if (!ctx || (which != 0 && which != 1)) return -1;
+  const NmfdShape& d = ctx->d;
+  const int64_t n = ctx->kind == 0 ? (which == 0 ? ctx->C : ctx->N) * ctx->R
+                                   : (int64_t)(which == 0 ? d.C : d.B) * d.R * (which == 0 ? d.w_inner() : d.h_inner());
+  return beta == 1.0 ? n + ctx->R : 2 * n;
+}
+
+int nmfb200_raw_terms(nmfb200_ctx* ctx, const float* W, const float* H, int which, double beta, float* out, void* stream) {
+  CTX_GUARD(ctx, kAnyKind);
+  TARGET_GUARD(ctx);
+  if (!W || !H || !out || (which != 0 && which != 1)) return fail(NMFB200_ERR_INVALID, "bad argument");
+  cudaStream_t st = (cudaStream_t)stream;
+  if (ctx->kind == 0) return nmf_raw_terms(ctx, W, H, which, beta, out, st);
+  return nmfd_raw_terms(ctx, W, H, which, beta, out, st);
+}
+
+// The update's ratio stage on summed raw W terms: one slab, leaving the tensor-core state as update_w does
+int nmfb200_w_apply(nmfb200_ctx* ctx, float* W, const float* reduced, double beta, double gamma, double l1_reg,
+                    double l2_reg, void* stream) {
+  CTX_GUARD(ctx, kAnyKind);
+  TARGET_GUARD(ctx);
   if (!W || !reduced) return fail(NMFB200_ERR_INVALID, "null pointer");
   cudaStream_t st = (cudaStream_t)stream;
-  ApplyArgs a = nmfd_apply_shape(ctx->d, 0, 1);
+  if (ctx->kind == 0) {
+    if (use_tc(ctx, beta)) return tc_w_apply(ctx->tc, W, reduced, beta, gamma, l1_reg, l2_reg, st);
+    int rc = apply_update(nmf_apply_args(ctx, 0, W, beta, reduced, reduced + ctx->C * ctx->R, 1, 0, gamma, l1_reg, l2_reg), st);
+    if (rc) return rc;
+    if (ctx->tc) tc_mark_dirty(ctx->tc, true, false);
+    return 0;
+  }
+  ApplyArgs a = nmfd_apply_shape(ctx->d, 0, 1);     // the centring term is already folded in by raw_sum
   a.param = W; a.num = reduced; a.gamma = (float)gamma; a.l1 = (float)l1_reg; a.l2 = (float)l2_reg;
   if (beta == 1.0) a.kl_den = reduced + a.numel;
   else a.den = reduced + a.numel;
-  if (nmfd_use_tc(ctx, beta)) a.absmax_bits = tc_nmfd_begin_update(ctx->tcd, 0, st);    // as nmfd_update leaves the state
+  if (nmfd_use_tc(ctx, beta)) a.absmax_bits = tc_nmfd_begin_update(ctx->tcd, 0, st);
   else if (ctx->tcd) tc_nmfd_mark_dirty(ctx->tcd);
   return apply_update(a, st);
-}
-
-int nmfb200_nmfd_loss(nmfb200_ctx* ctx, const float* W, const float* H, double beta, double* loss_dev,
-                      void* stream) {
-  CTX_GUARD(ctx, 1);
-  if (!ctx->has_target) return fail(NMFB200_ERR_STATE, "set_target has not been called");
-  if (!W || !H || !loss_dev) return fail(NMFB200_ERR_INVALID, "null pointer");
-  if (nmfd_use_tc(ctx, beta)) return nmfd_tc_recon(ctx, W, H, true, loss_dev, (cudaStream_t)stream);
-  return nmfd_recon_phi(ctx->d, ctx->V, ctx->vdtype, W, H, beta, nullptr, nullptr, ctx->loss_blocks, ctx->loss_max_blocks,
-                        loss_dev, (cudaStream_t)stream);
 }
 
 int nmfb200_hoyer_project(int device, float* x, int64_t outer, int64_t D, int64_t inner, const float* k1, const float* k2,

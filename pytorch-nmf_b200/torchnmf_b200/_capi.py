@@ -29,26 +29,15 @@ SIGNATURES = {
     "nmfb200_last_error": (_c.c_char_p, []),
     "nmfb200_build_info": (_c.c_char_p, []),
     "nmfb200_launch_count": (_i64, []),
-    "nmfb200_check_health": (_int, [_vp]),
     "nmfb200_ctx_check_health": (_int, [_vp, _vp]),
     "nmfb200_nmf_create": (_int, [_c.POINTER(_vp), _int, _i64, _i64, _i64, _int]),
     "nmfb200_destroy": (None, [_vp]),
     "nmfb200_precision": (_int, [_vp]),
     "nmfb200_precision_for_beta": (_int, [_vp, _dbl]),
-    "nmfb200_nmf_set_target": (_int, [_vp, _vp, _i64, _vp]),
-    "nmfb200_nmf_set_target_typed": (_int, [_vp, _vp, _i64, _int, _vp]),
+    "nmfb200_nmf_set_target": (_int, [_vp, _vp, _i64, _int, _vp]),
     "nmfb200_target_minmax": (_int, [_vp, _c.POINTER(_c.c_float), _c.POINTER(_c.c_float), _vp]),
-    "nmfb200_nmf_sync_factors": (_int, [_vp, _vp, _vp, _vp]),
-    "nmfb200_nmf_update_w": (_int, [_vp, _vp, _vp, _dbl, _dbl, _dbl, _dbl, _vp]),
-    "nmfb200_nmf_update_h": (_int, [_vp, _vp, _vp, _dbl, _dbl, _dbl, _dbl, _vp]),
     "nmfb200_nmf_iterate": (_int, [_vp, _vp, _vp, _dbl, _dbl, _dbl, _dbl, _int, _vp]),
-    "nmfb200_nmf_loss": (_int, [_vp, _vp, _vp, _dbl, _vp, _vp]),
     "nmfb200_nmf_loss_prefetch_w": (_int, [_vp, _vp, _vp, _dbl, _vp, _vp]),
-    "nmfb200_nmf_w_partial_numel": (_i64, [_vp, _dbl]),
-    "nmfb200_nmf_w_partial": (_int, [_vp, _vp, _vp, _dbl, _vp, _vp]),
-    "nmfb200_nmf_raw_terms_numel": (_i64, [_vp, _int, _dbl]),
-    "nmfb200_nmf_raw_terms": (_int, [_vp, _vp, _vp, _int, _dbl, _vp, _vp]),
-    "nmfb200_nmf_w_apply": (_int, [_vp, _vp, _vp, _dbl, _dbl, _dbl, _dbl, _vp]),
     "nmfb200_nmf_contract_only": (_int, [_vp, _vp, _vp, _int, _dbl, _vp]),
     "nmfb200_nmf_set_target_sparse": (_int, [_vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _dbl, _dbl, _vp]),
     "nmfb200_nmf_set_target_sparse_any_beta": (_int, [_vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _dbl, _dbl, _vp]),
@@ -58,28 +47,22 @@ SIGNATURES = {
     "nmfb200_nmf_peer_world": (_int, [_vp]),
     "nmfb200_nmf_peer_release": (_int, [_vp]),
     "nmfb200_nmf_update_w_peer": (_int, [_vp, _vp, _vp, _dbl, _dbl, _dbl, _dbl, _vp]),
-    "nmfb200_nmfd_create": (_int, [_c.POINTER(_vp), _int, _i64, _i64, _i64, _i64, _i64, _int]),
     "nmfb200_nmfnd_create": (_int, [_c.POINTER(_vp), _int, _i64, _i64, _int, _c.POINTER(_i64), _i64, _c.POINTER(_i64), _int]),
-    "nmfb200_nmfd_set_target": (_int, [_vp, _vp, _vp]),
-    "nmfb200_nmfd_set_target_typed": (_int, [_vp, _vp, _int, _vp]),
-    "nmfb200_nmfd_update_w": (_int, [_vp, _vp, _vp, _dbl, _dbl, _dbl, _dbl, _vp]),
-    "nmfb200_nmfd_update_h": (_int, [_vp, _vp, _vp, _dbl, _dbl, _dbl, _dbl, _vp]),
-    "nmfb200_nmfd_loss": (_int, [_vp, _vp, _vp, _dbl, _vp, _vp]),
-    "nmfb200_nmfd_raw_terms_numel": (_i64, [_vp, _int, _dbl]),
-    "nmfb200_nmfd_raw_terms": (_int, [_vp, _vp, _vp, _int, _dbl, _vp, _vp]),
-    "nmfb200_nmfd_w_partial_numel": (_i64, [_vp, _dbl]),
-    "nmfb200_nmfd_w_partial": (_int, [_vp, _vp, _vp, _dbl, _vp, _vp]),
-    "nmfb200_nmfd_w_apply": (_int, [_vp, _vp, _vp, _dbl, _dbl, _dbl, _dbl, _vp]),
-    "nmfb200_nmfd_sync_factors": (_int, [_vp]),
+    "nmfb200_nmfd_set_target": (_int, [_vp, _vp, _int, _vp]),
+    "nmfb200_sync_factors": (_int, [_vp]),
+    "nmfb200_update_w": (_int, [_vp, _vp, _vp, _dbl, _dbl, _dbl, _dbl, _vp]),
+    "nmfb200_update_h": (_int, [_vp, _vp, _vp, _dbl, _dbl, _dbl, _dbl, _vp]),
+    "nmfb200_loss": (_int, [_vp, _vp, _vp, _dbl, _vp, _vp]),
+    "nmfb200_raw_terms_numel": (_i64, [_vp, _int, _dbl]),
+    "nmfb200_raw_terms": (_int, [_vp, _vp, _vp, _int, _dbl, _vp, _vp]),
+    "nmfb200_w_apply": (_int, [_vp, _vp, _vp, _dbl, _dbl, _dbl, _dbl, _vp]),
     "nmfb200_hoyer_project": (_int, [_int, _vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp]),
     "nmfb200_nmf_plan": (_int, [_i64, _i64, _i64, _c.POINTER(_i64), _int]),
     "nmfb200_nmfd_plan": (_int, [_i64, _i64, _int, _c.POINTER(_i64), _i64, _c.POINTER(_i64), _c.POINTER(_i64), _int]),
     "nmfb200_nmf_sparse_plan": (_int, [_i64, _i64, _i64, _c.POINTER(_i64), _int]),
-    "nmfb200_nmfd_tc_plan": (_int, [_i64, _i64, _i64, _i64, _i64, _c.POINTER(_i64), _int]),
     "nmfb200_nmfnd_tc_plan": (_int, [_i64, _i64, _int, _c.POINTER(_i64), _i64, _c.POINTER(_i64), _c.POINTER(_i64), _int]),
 }
-NMF_PLAN_LEN, NMFD_PLAN_LEN, SPARSE_PLAN_LEN, NMFD_TC_PLAN_LEN = 9, 19, 8, 23         # include/nmf_b200.h
-NMFND_TC_PLAN_LEN = 31
+NMF_PLAN_LEN, NMFD_PLAN_LEN, SPARSE_PLAN_LEN, NMFND_TC_PLAN_LEN = 9, 19, 8, 31         # include/nmf_b200.h
 
 _lib = None
 
@@ -102,7 +85,7 @@ def load():
         fn = getattr(lib, name)          # AttributeError here == ABI mismatch
         fn.restype = res
         fn.argtypes = args
-    if lib.nmfb200_abi_version() != 1:
+    if lib.nmfb200_abi_version() != 2:
         raise NmfB200Error("libnmf_b200.so ABI version mismatch")
     _lib = lib
     return lib
@@ -149,17 +132,6 @@ def nmfd_plan(B, C, vdims, R, kdims):
     return {"recon_mt": v[0], "recon_grid": tuple(v[1:4]), "dgrad_mt": v[4], "dgrad_nsplit": v[5],
             "dgrad_grid": tuple(v[6:9]), "wgrad": dict(zip(("mt", "tp", "nr", "no", "ntt", "nrg", "nog"), v[9:16])),
             "wgrad_nsplit": v[16], "vec4_w": bool(v[17]), "vec4_h": bool(v[18])}
-
-
-def nmfd_tc_plan(B, C, L, R, T):
-    """The tensor-core NMFD kernels' launch plan (nmfb200_nmfd_tc_plan), as a dict; no device needed.  Raises NmfB200Error
-    naming the limit for a shape the tensor-core path does not take."""
-    out = (_i64 * NMFD_TC_PLAN_LEN)()
-    check(load().nmfb200_nmfd_tc_plan(B, C, L, R, T, out, NMFD_TC_PLAN_LEN))
-    v = list(out)
-    return {"prep_w": tuple(v[0:3]), "prep_h": tuple(v[3:6]), "recon": tuple(v[6:9]), "wgrad": tuple(v[9:12]),
-            "dgrad": tuple(v[12:15]), "bslice": v[15], "slices": v[16], "dgrad_rblocks": v[17], "loss_blocks": v[18],
-            "ws_w": v[19], "kbs_w": v[20], "ws_h": v[21], "kbs_h": v[22]}
 
 
 def nmfnd_tc_plan(B, C, vdims, R, kdims):

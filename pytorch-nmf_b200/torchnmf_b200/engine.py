@@ -185,6 +185,49 @@ class _CudaEngine:
         """Raise if a kernel of the library aborted an internal wait since the last check (synchronises)."""
         _capi.check(self._lib.nmfb200_ctx_check_health(self._ctx, _stream(self.device)))
 
+    def sync(self):
+        _capi.check(self._lib.nmfb200_sync_factors(self._ctx))
+
+    def update_w(self, beta, gamma, l1_reg, l2_reg):
+        _capi.check(self._lib.nmfb200_update_w(self._ctx, _ptr(self.W), _ptr(self.H), beta, gamma, l1_reg, l2_reg,
+                                               _stream(self.device)))
+
+    def update_h(self, beta, gamma, l1_reg, l2_reg):
+        _capi.check(self._lib.nmfb200_update_h(self._ctx, _ptr(self.W), _ptr(self.H), beta, gamma, l1_reg, l2_reg,
+                                               _stream(self.device)))
+
+    def loss_tensor(self, beta):
+        _capi.check(self._lib.nmfb200_loss(self._ctx, _ptr(self.W), _ptr(self.H), beta, _ptr(self._loss),
+                                           _stream(self.device)))
+        return self._loss
+
+    def raw_terms(self, which, beta):
+        """(numerator, denominator) of the update of W (which=0) or H (which=1) from the CURRENT factors, untouched: the
+        numerator in the factor's shape; the denominator (R,) for beta == 1 (the column sums of the other factor), else in
+        the factor's shape.  What BetaMu.step and PLCA.fit are built from (include/nmf_b200.h: nmfb200_raw_terms)."""
+        f = self.W if which == 0 else self.H
+        n = int(self._lib.nmfb200_raw_terms_numel(self._ctx, int(which), float(beta)))
+        buf = torch.empty(n, dtype=torch.float32, device=self.device)
+        _capi.check(self._lib.nmfb200_raw_terms(self._ctx, _ptr(self.W), _ptr(self.H), int(which), float(beta), _ptr(buf),
+                                                _stream(self.device)))
+        num, den = buf[:f.numel()].view(f.shape), buf[f.numel():]
+        return num, (den if beta == 1 else den.view(f.shape))
+
+    # --- pieces of the sharded W update (ShardedEngine) ---------------------------------------
+    def w_partial(self, beta):
+        """This shard's raw W terms, raw_terms(0)'s layout flat, in one buffer per engine reused every iteration."""
+        n = int(self._lib.nmfb200_raw_terms_numel(self._ctx, 0, beta))
+        buf = self._wbuf
+        if buf is None or buf.numel() != n:
+            buf = self._wbuf = torch.empty(n, dtype=torch.float32, device=self.device)
+        _capi.check(self._lib.nmfb200_raw_terms(self._ctx, _ptr(self.W), _ptr(self.H), 0, beta, _ptr(buf),
+                                                _stream(self.device)))
+        return buf
+
+    def w_apply(self, reduced, beta, gamma, l1_reg, l2_reg):
+        _capi.check(self._lib.nmfb200_w_apply(self._ctx, _ptr(self.W), _ptr(reduced), beta, gamma, l1_reg, l2_reg,
+                                              _stream(self.device)))
+
     # ---- what sparse_fit (nmf.py:411-599) needs beyond the MU updates ----
     def project(self, x, dim, k1, k2):
         """Hoyer projection of every slice of x along `dim`, in place (one launch)."""
@@ -222,30 +265,14 @@ class CudaNmfEngine(_CudaEngine):
         self._acquire(("nmf", dev_index, N, C, R, precision),
                       lambda ref: self._lib.nmfb200_nmf_create(ref, dev_index, N, C, R, _capi.PRECISIONS[precision]))
         self._loss = torch.zeros(1, dtype=torch.float64, device=self.device)
-        _capi.check(self._lib.nmfb200_nmf_set_target_typed(self._ctx, _ptr(V), V.stride(0), _capi.DTYPES[V.dtype],
-                                                           _stream(self.device)))
+        _capi.check(self._lib.nmfb200_nmf_set_target(self._ctx, _ptr(V), V.stride(0), _capi.DTYPES[V.dtype],
+                                                     _stream(self.device)))
         self.sync()
-
-    def sync(self):
-        _capi.check(self._lib.nmfb200_nmf_sync_factors(self._ctx, _ptr(self.W), _ptr(self.H), _stream(self.device)))
-
-    def update_w(self, beta, gamma, l1_reg, l2_reg):
-        _capi.check(self._lib.nmfb200_nmf_update_w(self._ctx, _ptr(self.W), _ptr(self.H), beta, gamma, l1_reg,
-                                                   l2_reg, _stream(self.device)))
-
-    def update_h(self, beta, gamma, l1_reg, l2_reg):
-        _capi.check(self._lib.nmfb200_nmf_update_h(self._ctx, _ptr(self.W), _ptr(self.H), beta, gamma, l1_reg,
-                                                   l2_reg, _stream(self.device)))
 
     def iterate(self, n_iter, beta, gamma, l1_reg, l2_reg):
         """n_iter x (update_w; update_h) in one call."""
         _capi.check(self._lib.nmfb200_nmf_iterate(self._ctx, _ptr(self.W), _ptr(self.H), beta, gamma, l1_reg, l2_reg,
                                                   int(n_iter), _stream(self.device)))
-
-    def loss_tensor(self, beta):
-        _capi.check(self._lib.nmfb200_nmf_loss(self._ctx, _ptr(self.W), _ptr(self.H), beta, _ptr(self._loss),
-                                               _stream(self.device)))
-        return self._loss
 
     def loss_prefetch_w(self, beta):
         """The loss at the current factors, taken out of the NEXT W update's contraction pass where the library can fold it
@@ -260,29 +287,6 @@ class CudaNmfEngine(_CudaEngine):
         """bench.py: launch only the fused contraction kernel (0 = W update's, 1 = H update's)."""
         _capi.check(self._lib.nmfb200_nmf_contract_only(self._ctx, _ptr(self.W), _ptr(self.H), which, beta,
                                                         _stream(self.device)))
-
-    # --- pieces of the row-sharded W update -------------------------------------------------
-    def w_partial(self, beta):
-        n = int(self._lib.nmfb200_nmf_w_partial_numel(self._ctx, beta))
-        buf = self._wbuf
-        if buf is None or buf.numel() != n:           # one buffer per engine, reused every iteration
-            buf = self._wbuf = torch.empty(n, dtype=torch.float32, device=self.device)
-        _capi.check(self._lib.nmfb200_nmf_w_partial(self._ctx, _ptr(self.W), _ptr(self.H), beta, _ptr(buf),
-                                                    _stream(self.device)))
-        return buf
-
-    def raw_terms(self, which, beta):
-        """(numerator, denominator) of the update of W (which=0) or H (which=1) from the CURRENT factors, untouched:
-        numerator (rows, R); denominator (R,) for beta == 1 (the column sums of the other factor) else (rows, R).
-        What BetaMu.step and PLCA.fit are built from (include/nmf_b200.h: nmfb200_nmf_raw_terms)."""
-        n = int(self._lib.nmfb200_nmf_raw_terms_numel(self._ctx, int(which), float(beta)))
-        buf = torch.empty(n, dtype=torch.float32, device=self.device)
-        _capi.check(self._lib.nmfb200_nmf_raw_terms(self._ctx, _ptr(self.W), _ptr(self.H), int(which), float(beta),
-                                                    _ptr(buf), _stream(self.device)))
-        rows = self.C if which == 0 else self.N
-        num = buf[:rows * self.R].view(rows, self.R)
-        den = buf[rows * self.R:]
-        return num, (den if beta == 1 else den.view(rows, self.R))
 
     # ---- row-sharded W update over peer memory (include/nmf_b200.h: nmfb200_nmf_peer_*) ----
     def peer_supported(self, beta):
@@ -306,10 +310,6 @@ class CudaNmfEngine(_CudaEngine):
     def update_w_peer(self, beta, gamma, l1_reg, l2_reg):
         _capi.check(self._lib.nmfb200_nmf_update_w_peer(self._ctx, _ptr(self.W), _ptr(self.H), beta, gamma, l1_reg,
                                                         l2_reg, _stream(self.device)))
-
-    def w_apply(self, reduced, beta, gamma, l1_reg, l2_reg):
-        _capi.check(self._lib.nmfb200_nmf_w_apply(self._ctx, _ptr(self.W), _ptr(reduced), beta, gamma, l1_reg,
-                                                  l2_reg, _stream(self.device)))
 
 
 class CudaSparseNmfEngine(_CudaEngine):
@@ -365,28 +365,7 @@ class CudaSparseNmfEngine(_CudaEngine):
     def minmax(self):
         return (min(self._vmin, 0.0) if self._has_zeros else self._vmin), self._vmax
 
-    def sync(self):
-        pass
-
-    def update_w(self, beta, gamma, l1_reg, l2_reg):
-        _capi.check(self._lib.nmfb200_nmf_update_w(self._ctx, _ptr(self.W), _ptr(self.H), beta, gamma, l1_reg,
-                                                   l2_reg, _stream(self.device)))
-
-    def update_h(self, beta, gamma, l1_reg, l2_reg):
-        _capi.check(self._lib.nmfb200_nmf_update_h(self._ctx, _ptr(self.W), _ptr(self.H), beta, gamma, l1_reg,
-                                                   l2_reg, _stream(self.device)))
-
-    def iterate(self, n_iter, beta, gamma, l1_reg, l2_reg):
-        _capi.check(self._lib.nmfb200_nmf_iterate(self._ctx, _ptr(self.W), _ptr(self.H), beta, gamma, l1_reg, l2_reg,
-                                                  int(n_iter), _stream(self.device)))
-
-    def loss_tensor(self, beta):
-        _capi.check(self._lib.nmfb200_nmf_loss(self._ctx, _ptr(self.W), _ptr(self.H), beta, _ptr(self._loss),
-                                               _stream(self.device)))
-        return self._loss
-
-    # the same call and layout as the dense target's; beta 1 and 2 only (the terms of the sparse update, nmf.py:603-638)
-    raw_terms = CudaNmfEngine.raw_terms
+    iterate = CudaNmfEngine.iterate
 
 
 class CudaSparseAnyBetaEngine(CudaSparseNmfEngine):
@@ -414,58 +393,13 @@ class CudaNmfdEngine(_CudaEngine):
         assert W.shape == (C, R, *K) and H.shape == (B, R, *(x - k + 1 for x, k in zip(X, K)))
         self.V, self.W, self.H = V, W, H
         dev_index = self.device.index if self.device.index is not None else torch.cuda.current_device()
-        if nd == 1:
-            create = lambda ref: self._lib.nmfb200_nmfd_create(ref, dev_index, B, C, X[0], R, K[0],
-                                                               _capi.PRECISIONS[precision])
-        else:
-            # "f16": beta 1 on the tensor-core sliding GEMMs; "auto" stays on the fp32 kernels for NMF2D / NMF3D
-            vd, kd = (ctypes.c_int64 * nd)(*X), (ctypes.c_int64 * nd)(*K)
-            create = lambda ref: self._lib.nmfb200_nmfnd_create(ref, dev_index, B, C, nd, vd, R, kd,
-                                                                _capi.PRECISIONS[precision])
-        self._acquire(("nmfd", dev_index, B, C, tuple(X), R, tuple(K), precision), create)
+        # "f16": beta 1 on the tensor-core sliding GEMMs; "auto" stays on the fp32 kernels for NMF2D / NMF3D
+        vd, kd = (ctypes.c_int64 * nd)(*X), (ctypes.c_int64 * nd)(*K)
+        self._acquire(("nmfd", dev_index, B, C, tuple(X), R, tuple(K), precision),
+                      lambda ref: self._lib.nmfb200_nmfnd_create(ref, dev_index, B, C, nd, vd, R, kd,
+                                                                 _capi.PRECISIONS[precision]))
         self._loss = torch.zeros(1, dtype=torch.float64, device=self.device)
-        _capi.check(self._lib.nmfb200_nmfd_set_target_typed(self._ctx, _ptr(V), _capi.DTYPES[V.dtype], _stream(self.device)))
-
-    def sync(self):
-        _capi.check(self._lib.nmfb200_nmfd_sync_factors(self._ctx))
-
-    def raw_terms(self, which, beta):
-        """(numerator, denominator) of the update of W (which=0) or H (which=1) from the CURRENT factors, untouched, in
-        the factor's own shape; the denominator is (R,) for beta == 1 (include/nmf_b200.h: nmfb200_nmfd_raw_terms)."""
-        f = self.W if which == 0 else self.H
-        n = int(self._lib.nmfb200_nmfd_raw_terms_numel(self._ctx, int(which), float(beta)))
-        buf = torch.empty(n, dtype=torch.float32, device=self.device)
-        _capi.check(self._lib.nmfb200_nmfd_raw_terms(self._ctx, _ptr(self.W), _ptr(self.H), int(which), float(beta),
-                                                     _ptr(buf), _stream(self.device)))
-        num, den = buf[:f.numel()].view(f.shape), buf[f.numel():]
-        return num, (den if beta == 1 else den.view(f.shape))
-
-    def update_w(self, beta, gamma, l1_reg, l2_reg):
-        _capi.check(self._lib.nmfb200_nmfd_update_w(self._ctx, _ptr(self.W), _ptr(self.H), beta, gamma, l1_reg,
-                                                    l2_reg, _stream(self.device)))
-
-    def update_h(self, beta, gamma, l1_reg, l2_reg):
-        _capi.check(self._lib.nmfb200_nmfd_update_h(self._ctx, _ptr(self.W), _ptr(self.H), beta, gamma, l1_reg,
-                                                    l2_reg, _stream(self.device)))
-
-    def loss_tensor(self, beta):
-        _capi.check(self._lib.nmfb200_nmfd_loss(self._ctx, _ptr(self.W), _ptr(self.H), beta, _ptr(self._loss),
-                                                _stream(self.device)))
-        return self._loss
-
-    # --- pieces of the batch-sharded W update -----------------------------------------------
-    def w_partial(self, beta):
-        n = int(self._lib.nmfb200_nmfd_w_partial_numel(self._ctx, beta))
-        buf = self._wbuf
-        if buf is None or buf.numel() != n:           # one buffer per engine, reused every iteration
-            buf = self._wbuf = torch.empty(n, dtype=torch.float32, device=self.device)
-        _capi.check(self._lib.nmfb200_nmfd_w_partial(self._ctx, _ptr(self.W), _ptr(self.H), beta, _ptr(buf),
-                                                     _stream(self.device)))
-        return buf
-
-    def w_apply(self, reduced, beta, gamma, l1_reg, l2_reg):
-        _capi.check(self._lib.nmfb200_nmfd_w_apply(self._ctx, _ptr(self.W), _ptr(reduced), beta, gamma, l1_reg,
-                                                   l2_reg, _stream(self.device)))
+        _capi.check(self._lib.nmfb200_nmfd_set_target(self._ctx, _ptr(V), _capi.DTYPES[V.dtype], _stream(self.device)))
 
 
 class ShardedEngine:

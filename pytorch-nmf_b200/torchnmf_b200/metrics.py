@@ -1,6 +1,6 @@
 """Divergences of the reference's `torchnmf.metrics` surface (metrics.py:6-96): plain differentiable torch expressions,
 used by user code and by the generic (autograd) path of `trainer.BetaMu`.  `fit` never calls these: its loss comes from
-the fused kernels (`nmfb200_nmf_loss`).
+the fused kernels (`nmfb200_loss`).
 """
 import torch
 

@@ -343,7 +343,7 @@ class BaseComponent(torch.nn.Module):
         (nmf.py:503-511), a constrained one a projected-gradient step with a halving line search (:513-538), and H is
         re-normalised to unit component norms after its update (:588).  No stop rule: `max_iter` iterations are run.
 
-        On the engine: the gradient is `positive - negative` of ONE fused raw-terms launch (`nmfb200_*_raw_terms`), every
+        On the engine: the gradient is `positive - negative` of ONE fused raw-terms launch (`nmfb200_raw_terms`), every
         line-search loss one fused loss launch on the trial factor, and the per-component Python loop around `_proj_func`
         (nmf.py:519-522: R x rounds x 7 ATen launches and one `.item()` per round) is one `nmfb200_hoyer_project` launch.
 

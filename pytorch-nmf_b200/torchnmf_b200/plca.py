@@ -7,13 +7,13 @@ updates Z, W and H simultaneously from the three gradients.  Here the two big co
 
     dW[c, r] = sum_n P[n, c] (H Z)[n, r],      dHz[n, r] = sum_c P[n, c] W[c, r],      P = V / ((H Z) W^T + eps)
 
-are two launches of the fused wgmma KL contraction (`nmfb200_nmf_raw_terms` with the factor pair (W, H diag Z)): neither
+are two launches of the fused wgmma KL contraction (`nmfb200_raw_terms` with the factor pair (W, H diag Z)): neither
 WZH nor P reaches HBM.  dH = dHz * Z and dZ[r] = sum_n H[n, r] dHz[n, r] follow from them; everything after that is the
 reference's sequence of small factor-sized operations (plca.py:256-289).
 
 The shift-invariant models (plca.py:376-625) are the same EM step around the convolutive reconstruction
 `sum_{r,t} W[c,r,t] Z[r] H[b,r,x-t]`: the factor pair handed to the library is (W, H Z) as well, and the two gradients are
-the sliding contractions of `nmfb200_nmfd_raw_terms` (wgrad and dgrad of the ratio tile; csrc/nmfd.cu, csrc/tc_nmfd.cu).
+the sliding contractions of `nmfb200_raw_terms` (wgrad and dgrad of the ratio tile; csrc/nmfd.cu, csrc/tc_nmfd.cu).
 """
 import math
 from collections.abc import Iterable as _Iterable

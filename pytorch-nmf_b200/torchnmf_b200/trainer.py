@@ -13,9 +13,9 @@ Two ways to obtain the two gradient terms `neg = relu(d<WH, V (WH+eps)^(beta-2)>
   composition of modules, CPU or GPU; this is the reference's algorithm.
 * fused (GPU): when the prediction is the plain reconstruction of ONE `torchnmf_b200.NMF` module on a CUDA device and `p`
   is that module's W or H, both terms come from ONE launch of the fused wgmma contraction
-  (`nmfb200_nmf_raw_terms`): neither WH nor the ratio matrices are materialised by the update.  The closure may
+  (`nmfb200_raw_terms`): neither WH nor the ratio matrices are materialised by the update.  The closure may
   return the module itself instead of its output (`return V, model`) to skip the forward pass as well.  The
-  convolutive modules (`NMFD`, `NMF2D`, `NMF3D`) take the same route through `nmfb200_nmfd_raw_terms` (the sliding
+  convolutive modules (`NMFD`, `NMF2D`, `NMF3D`) take the same route through `nmfb200_raw_terms` (the sliding
   contractions of csrc/nmfd.cu / csrc/tc_nmfd.cu instead of two passes through cuDNN's convolution backward).
 
 `SparsityProj` (trainer.py:124-190): Hoyer's projected-gradient step around a loss closure.  The gradient is the

@@ -276,7 +276,7 @@ def nmfd_device_bytes(case, prec):
     b = 2 * 4 * B * C * L
     b += 4 * max(p["wgrad_nsplit"] * nw, p["dgrad_nsplit"] * nh)
     if prec == "f16":
-        tp, q = _tc_pitches(L, T), _capi.nmfd_tc_plan(B, C, L, R, T)
+        tp, q = _tc_pitches(L, T), _capi.nmfnd_tc_plan(B, C, [L], R, [T])
         b += 2 * (B * C + 1) * tp[1] + 2 * B * R * tp[0] + 2 * 2 * cdiv(C, 128) * 128 * R * cdiv(T, 64) * 64
         b += 4 * max(q["ws_w"] * nw, q["ws_h"] * nh)
     b += 4 * 3 * (2 * nw + 2 * nh)                        # factors, copies, raw terms

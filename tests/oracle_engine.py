@@ -60,7 +60,7 @@ class OracleNmfEngine(_OracleEngine):
     def update_h(self, beta, gamma, l1, l2):
         self.H.copy_(orc.nmf_update_h(self.V, self.W, self.H, beta, gamma, l1, l2))
 
-    # sharded pieces: same buffer layout as nmfb200_nmf_w_partial (include/nmf_b200.h)
+    # sharded pieces: same buffer layout as nmfb200_raw_terms(which = 0) (include/nmf_b200.h)
     def w_partial(self, beta):
         num, den = orc.nmf_w_contractions(self.V, self.W, self.H, beta)
         return torch.cat([num.reshape(-1), den.reshape(-1)]).contiguous()

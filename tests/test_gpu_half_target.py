@@ -244,7 +244,7 @@ def test_no_fp32_copy():
     release_workspaces()
 
 
-def test_c_abi_rejects_bad_targets():
+def test_set_target_rejects_bad_dtypes_and_alignment():
     lib = _capi.load()
     V16 = _target((64, 48), torch.bfloat16, 26)
     W0, H0 = _factors([(48, 8), (64, 8)], 27)
@@ -252,11 +252,11 @@ def test_c_abi_rejects_bad_targets():
     st = _engine._stream(V16.device)
     p = V16.data_ptr()
     try:
-        assert lib.nmfb200_nmf_set_target_typed(eng._ctx, ctypes.c_void_p(p), 48, 3, st) == 1      # NMFB200_ERR_INVALID
+        assert lib.nmfb200_nmf_set_target(eng._ctx, ctypes.c_void_p(p), 48, 3, st) == 1      # NMFB200_ERR_INVALID
         assert b"unknown target dtype 3" in lib.nmfb200_last_error()
-        assert lib.nmfb200_nmf_set_target_typed(eng._ctx, ctypes.c_void_p(p + 1), 48, _capi.DTYPE_BF16, st) == 1
+        assert lib.nmfb200_nmf_set_target(eng._ctx, ctypes.c_void_p(p + 1), 48, _capi.DTYPE_BF16, st) == 1
         assert b"not aligned to its element size (2 bytes)" in lib.nmfb200_last_error()
-        assert lib.nmfb200_nmf_set_target_typed(eng._ctx, ctypes.c_void_p(p + 2), 48, _capi.DTYPE_F32, st) == 1
+        assert lib.nmfb200_nmf_set_target(eng._ctx, ctypes.c_void_p(p + 2), 48, _capi.DTYPE_F32, st) == 1
         assert b"not aligned to its element size (4 bytes)" in lib.nmfb200_last_error()
         assert eng.minmax() == (float(V16.min()), float(V16.max()))     # the registered target is unchanged
     finally:
@@ -265,9 +265,9 @@ def test_c_abi_rejects_bad_targets():
     Wd, Hd = _factors([(8, 4, 5), (1, 4, 36)], 29)
     eng = CudaNmfdEngine(Vd, Wd.cuda(), Hd.cuda(), "f32")
     try:
-        assert lib.nmfb200_nmfd_set_target_typed(eng._ctx, ctypes.c_void_p(Vd.data_ptr()), 3, st) == 1
+        assert lib.nmfb200_nmfd_set_target(eng._ctx, ctypes.c_void_p(Vd.data_ptr()), 3, st) == 1
         assert b"unknown target dtype 3" in lib.nmfb200_last_error()
-        assert lib.nmfb200_nmfd_set_target_typed(eng._ctx, ctypes.c_void_p(Vd.data_ptr() + 1), _capi.DTYPE_F16, st) == 1
+        assert lib.nmfb200_nmfd_set_target(eng._ctx, ctypes.c_void_p(Vd.data_ptr() + 1), _capi.DTYPE_F16, st) == 1
         assert b"not aligned to its element size (2 bytes)" in lib.nmfb200_last_error()
     finally:
         eng.close()

@@ -225,7 +225,7 @@ def test_target_minmax_is_exact_and_nan_sticky(where):
 
 
 @pytest.mark.parametrize("nan_pad", [False, True])
-def test_target_minmax_ignores_the_padding_of_a_strided_target(nan_pad):
+def test_minmax_of_a_strided_target_ignores_its_padding(nan_pad):
     """nmfb200_nmf_set_target with ldv > C: the padding columns (NaN, -Inf, +Inf) must not reach the min / max."""
     g = torch.Generator().manual_seed(10)
     N, C, ldv = 1500, 1111, 1200
@@ -235,7 +235,8 @@ def test_target_minmax_ignores_the_padding_of_a_strided_target(nan_pad):
     V = Vp[:, :C].contiguous()
     eng = CudaNmfEngine(V.cuda(), torch.rand(C, 3, generator=g).cuda(), torch.rand(N, 3, generator=g).cuda(), "f32")
     Vpd = Vp.cuda()
-    _capi.check(eng._lib.nmfb200_nmf_set_target(eng._ctx, ctypes.c_void_p(Vpd.data_ptr()), ldv, _engine._stream(Vpd.device)))
+    _capi.check(eng._lib.nmfb200_nmf_set_target(eng._ctx, ctypes.c_void_p(Vpd.data_ptr()), ldv, _capi.DTYPE_F32,
+                                                 _engine._stream(Vpd.device)))
     got = eng.minmax()
     eng.close()
     release_workspaces()

@@ -180,7 +180,7 @@ def _nmfd_term_bars(case, prec, beta, want, which):
     if prec == "f16":
         # the f16 bar, plus what the fp32 accumulation of one split truncates (tests/tc_model.py): a sum of ~10^6 centred
         # terms on the tensor cores is not held to 1.25e-3 by the float64 bar alone
-        tcp = _capi.nmfd_tc_plan(B, C, L, R, T)
+        tcp = _capi.nmfnd_tc_plan(B, C, [L], R, [T])
         trunc = lc.nmfd_tc_trunc(tcp["kbs_w"] if which == 0 else tcp["kbs_h"]) * want[2][which][0]
         return lc.F16_BAR + trunc / want[which][0].abs(), lc.F16_BAR
     plan = _capi.nmfd_plan(B, C, [L], R, [T])
@@ -189,7 +189,7 @@ def _nmfd_term_bars(case, prec, beta, want, which):
 
 
 @pytest.mark.parametrize("name,prec,beta", _nmfd_runs())
-def test_nmfd_past_2p31(name, prec, beta):
+def test_nmfd_terms_and_updates_past_2p31(name, prec, beta):
     """The loss, the raw terms of both factors, then one W update and one H update, every entry."""
     case = lc.NMFD_BIG[name]
     B, C, L, R, T = lc.nmfd_dims(case)
@@ -243,7 +243,9 @@ def _create_error(kind, shape, prec):
     if kind == "nmf":
         rc = lib.nmfb200_nmf_create(ctypes.byref(ctx), 0, *shape, _capi.PRECISIONS[prec])
     else:
-        rc = lib.nmfb200_nmfd_create(ctypes.byref(ctx), 0, *shape, _capi.PRECISIONS[prec])
+        B, C, L, R, T = shape
+        rc = lib.nmfb200_nmfnd_create(ctypes.byref(ctx), 0, B, C, 1, (ctypes.c_int64 * 1)(L), R, (ctypes.c_int64 * 1)(T),
+                                      _capi.PRECISIONS[prec])
     if rc == 0:
         lib.nmfb200_destroy(ctx)
         return 0, ""
@@ -261,7 +263,23 @@ def _grid_data(kind, shape, seed):
     return tuple((torch.rand(*d, generator=g) + 0.5).cuda() for d in dims)
 
 
-@pytest.mark.parametrize("name,kind,shape,prec,expected", lc.GRID_CASES, ids=[c[0] for c in lc.GRID_CASES])
+def _nmfd_refused(case):
+    return case[1] == "nmfd" and case[4] != "runs"
+
+
+NMFD_REFUSED = [c for c in lc.GRID_CASES if _nmfd_refused(c)]
+
+
+@pytest.mark.parametrize("name,kind,shape,prec,expected", NMFD_REFUSED, ids=[c[0] for c in NMFD_REFUSED])
+def test_nmfnd_create_refuses_past_the_grid_limit(name, kind, shape, prec, expected):
+    rc, msg = _create_error(kind, shape, prec)
+    assert rc == 1 and expected[1] in msg, (rc, msg)
+
+
+GRID_CASES = [c for c in lc.GRID_CASES if not _nmfd_refused(c)]
+
+
+@pytest.mark.parametrize("name,kind,shape,prec,expected", GRID_CASES, ids=[c[0] for c in GRID_CASES])
 def test_grid_limit(name, kind, shape, prec, expected):
     _cleanup()
     if expected != "runs":
@@ -312,6 +330,6 @@ def test_grid_limit(name, kind, shape, prec, expected):
 
 
 @pytest.mark.parametrize("name,shape,prec,words", lc.REJECT_CASES, ids=[c[0] for c in lc.REJECT_CASES])
-def test_create_rejects_past_the_narrowing_bounds(name, shape, prec, words):
+def test_nmfnd_create_rejects_past_the_narrowing_bounds(name, shape, prec, words):
     rc, msg = _create_error("nmfd", shape, prec)
     assert rc == 1 and words in msg, (rc, msg)

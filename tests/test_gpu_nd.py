@@ -1,6 +1,6 @@
 """GPU parity of NMF2D / NMF3D (reference nmf.py:782-942) against reference-generated goldens
 (tests/golden/reference_nd.npz, written by `python oracle/make_golden.py --nd` from the real torchnmf 0.3.5) and against the
-oracle on seeded shapes.  Module surface -> ctypes -> C ABI (nmfb200_nmfnd_create + the nmfb200_nmfd_* calls)."""
+oracle on seeded shapes.  Module surface -> ctypes -> C ABI (nmfb200_nmfnd_create + the calls that serve every context)."""
 import pytest
 import torch
 

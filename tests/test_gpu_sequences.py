@@ -299,7 +299,7 @@ def _set_target_fn(seq, targets, chk):
             assert eng._ctx.value == ctx, "the workspace cache did not hand the sparse context on"
             return eng
         lib = _capi.load()
-        _capi.check(lib.nmfb200_nmf_set_target(eng._ctx, ctypes.c_void_p(V.data_ptr()), V.stride(0),
+        _capi.check(lib.nmfb200_nmf_set_target(eng._ctx, ctypes.c_void_p(V.data_ptr()), V.stride(0), _capi.DTYPE_F32,
                                                ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)))
         eng.V = V
         return eng
@@ -352,9 +352,15 @@ TC_SEQS = [s for s in sc.sequences() if s.tc]
 
 
 @pytest.mark.parametrize("scale", sc.SCALES, ids=sc.scale_tag)
-@pytest.mark.parametrize("name", [s.name for s in TC_SEQS])
+@pytest.mark.parametrize("name", [s.name for s in TC_SEQS if s.name != "target"])
 def test_tensor_core_sequence(name, scale):
     _run(sc.by_name(name), scale)
+
+
+@pytest.mark.parametrize("scale", sc.SCALES, ids=sc.scale_tag)
+def test_tensor_core_sequence_with_a_new_dense_target(scale):
+    """The "target" sequence: nmfb200_nmf_set_target registers a new fp32 target on a live tensor-core context."""
+    _run(sc.by_name("target"), scale)
 
 
 @pytest.mark.parametrize("name", ["fit-f16", "fit-split", "mixed-f16"])

@@ -1,5 +1,5 @@
 """Batch-sharded NMFD / NMF2D / NMF3D fits on the H100: V and H split along the batch axis, W replicated, one all-reduce of
-the W terms (nmfb200_nmfd_w_partial) before the ratio stage (nmfb200_nmfd_w_apply).
+the W terms (nmfb200_raw_terms(which = 0)) before the ratio stage (nmfb200_w_apply).
 
 (a) A one-rank group is the unsharded fit bit for bit: the partial folds the split slabs (and the tensor-core path's
     centring term) in the order the ratio stage does, the one-rank all-reduce is the identity, and the ratio stage on one
@@ -126,7 +126,7 @@ def test_two_gpus_nccl(tmp_path, name, beta):
 # ---- (d) the C ABI -----------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("name,beta,l1,l2", [("nmfd_f16", 1, 0.0, 0.0), ("nmfd_f32", 0.5, 0.0, 0.0),
                                              ("nmf2d_f16", 1, 0.05, 0.05), ("nmf3d_f32", 2, 0.05, 0.05)])
-def test_w_partial_is_raw_terms_and_w_apply_is_update_w(name, beta, l1, l2):
+def test_w_partial_is_w_raw_terms_and_w_apply_is_update_w(name, beta, l1, l2):
     from torchnmf_b200.engine import CudaNmfdEngine
     from torchnmf_b200.nmf import _gamma
     _, V, W0, H0, prec = _case(name)
@@ -134,7 +134,6 @@ def test_w_partial_is_raw_terms_and_w_apply_is_update_w(name, beta, l1, l2):
     a, b = (CudaNmfdEngine(V, W0.cuda(), H0.cuda(), prec) for _ in range(2))
     try:
         lib = a._lib
-        assert lib.nmfb200_nmfd_w_partial_numel(a._ctx, beta) == lib.nmfb200_nmfd_raw_terms_numel(a._ctx, 0, beta)
         assert a.precision_for(beta) == ("f16" if _uses_tc(name, beta) else "f32")
         for _ in range(3):           # later rounds start from a ratio stage's tensor-core state: w_apply must leave it right
             num, den = a.raw_terms(0, beta)
@@ -153,7 +152,7 @@ def test_w_partial_is_raw_terms_and_w_apply_is_update_w(name, beta, l1, l2):
         b.close()
 
 
-def test_w_partial_and_w_apply_refusals():
+def test_raw_terms_and_w_apply_refusals():
     from torchnmf_b200 import _capi
     lib = _capi.load()
     vp, st = ctypes.c_void_p, ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
@@ -162,34 +161,34 @@ def test_w_partial_and_w_apply_refusals():
     V = torch.rand(2, 8, 40, device="cuda")
     buf = torch.empty(2 * W.numel(), device="cuda")
     w, h, v, p = vp(W.data_ptr()), vp(H.data_ptr()), vp(V.data_ptr()), vp(buf.data_ptr())
-    assert lib.nmfb200_nmfd_w_partial_numel(None, 1.0) == -1
-    assert lib.nmfb200_nmfd_w_partial(None, w, h, 1.0, p, st) == ERR_INVALID
-    assert lib.nmfb200_nmfd_w_apply(None, w, p, 1.0, 1.0, 0.0, 0.0, st) == ERR_INVALID
+    assert lib.nmfb200_raw_terms_numel(None, 0, 1.0) == -1
+    assert lib.nmfb200_raw_terms(None, w, h, 0, 1.0, p, st) == ERR_INVALID
+    assert lib.nmfb200_w_apply(None, w, p, 1.0, 1.0, 0.0, 0.0, st) == ERR_INVALID
 
     nmf = vp()
     _capi.check(lib.nmfb200_nmf_create(ctypes.byref(nmf), 0, 64, 32, 4, _capi.PREC_F32))
-    try:
-        assert lib.nmfb200_nmfd_w_partial_numel(nmf, 1.0) == -1
-        assert lib.nmfb200_nmfd_w_partial(nmf, w, h, 1.0, p, st) == ERR_INVALID
-        assert lib.nmfb200_nmfd_w_apply(nmf, w, p, 1.0, 1.0, 0.0, 0.0, st) == ERR_INVALID
+    try:        # an NMF context takes the same calls: W terms of C * R (+ R at beta 1), and no ratio stage before a target
+        assert lib.nmfb200_raw_terms_numel(nmf, 0, 1.0) == 32 * 4 + 4
+        assert lib.nmfb200_w_apply(nmf, w, p, 1.0, 1.0, 0.0, 0.0, st) == ERR_STATE
     finally:
         lib.nmfb200_destroy(nmf)
 
     ctx = vp()
-    _capi.check(lib.nmfb200_nmfd_create(ctypes.byref(ctx), 0, 2, 8, 40, 4, 5, _capi.PREC_F32))
+    _capi.check(lib.nmfb200_nmfnd_create(ctypes.byref(ctx), 0, 2, 8, 1, (ctypes.c_int64 * 1)(40), 4,
+                                         (ctypes.c_int64 * 1)(5), _capi.PREC_F32))
     try:
-        assert lib.nmfb200_nmfd_w_partial_numel(ctx, 1.0) == W.numel() + 4
-        assert lib.nmfb200_nmfd_w_partial_numel(ctx, 0.5) == 2 * W.numel()
-        assert lib.nmfb200_nmfd_w_partial(ctx, w, h, 1.0, p, st) == ERR_STATE          # before set_target
-        assert lib.nmfb200_nmfd_w_apply(ctx, w, p, 1.0, 1.0, 0.0, 0.0, st) == ERR_STATE
-        _capi.check(lib.nmfb200_nmfd_set_target(ctx, v, st))
-        assert lib.nmfb200_nmfd_w_partial(ctx, None, h, 1.0, p, st) == ERR_INVALID
-        assert lib.nmfb200_nmfd_w_partial(ctx, w, None, 1.0, p, st) == ERR_INVALID
-        assert lib.nmfb200_nmfd_w_partial(ctx, w, h, 1.0, None, st) == ERR_INVALID
-        assert lib.nmfb200_nmfd_w_apply(ctx, None, p, 1.0, 1.0, 0.0, 0.0, st) == ERR_INVALID
-        assert lib.nmfb200_nmfd_w_apply(ctx, w, None, 1.0, 1.0, 0.0, 0.0, st) == ERR_INVALID
-        assert lib.nmfb200_nmfd_w_partial(ctx, w, h, 1.0, p, st) == 0
-        assert lib.nmfb200_nmfd_w_apply(ctx, w, p, 1.0, 1.0, 0.0, 0.0, st) == 0
+        assert lib.nmfb200_raw_terms_numel(ctx, 0, 1.0) == W.numel() + 4
+        assert lib.nmfb200_raw_terms_numel(ctx, 0, 0.5) == 2 * W.numel()
+        assert lib.nmfb200_raw_terms(ctx, w, h, 0, 1.0, p, st) == ERR_STATE          # before set_target
+        assert lib.nmfb200_w_apply(ctx, w, p, 1.0, 1.0, 0.0, 0.0, st) == ERR_STATE
+        _capi.check(lib.nmfb200_nmfd_set_target(ctx, v, _capi.DTYPE_F32, st))
+        assert lib.nmfb200_raw_terms(ctx, None, h, 0, 1.0, p, st) == ERR_INVALID
+        assert lib.nmfb200_raw_terms(ctx, w, None, 0, 1.0, p, st) == ERR_INVALID
+        assert lib.nmfb200_raw_terms(ctx, w, h, 0, 1.0, None, st) == ERR_INVALID
+        assert lib.nmfb200_w_apply(ctx, None, p, 1.0, 1.0, 0.0, 0.0, st) == ERR_INVALID
+        assert lib.nmfb200_w_apply(ctx, w, None, 1.0, 1.0, 0.0, 0.0, st) == ERR_INVALID
+        assert lib.nmfb200_raw_terms(ctx, w, h, 0, 1.0, p, st) == 0
+        assert lib.nmfb200_w_apply(ctx, w, p, 1.0, 1.0, 0.0, 0.0, st) == 0
         torch.cuda.synchronize()
         assert torch.isfinite(W).all() and (W > 0).all()
     finally:

@@ -55,10 +55,10 @@ def _poison(eng, beta):
 
 
 def _raw_terms_into_nan(eng, which, beta):
-    n = int(eng._lib.nmfb200_nmf_raw_terms_numel(eng._ctx, which, float(beta)))
+    n = int(eng._lib.nmfb200_raw_terms_numel(eng._ctx, which, float(beta)))
     buf = torch.full((n,), float("nan"), dtype=torch.float32, device=eng.device)
-    _capi.check(eng._lib.nmfb200_nmf_raw_terms(eng._ctx, _ptr(eng.W), _ptr(eng.H), which, float(beta), _ptr(buf),
-                                               _stream(eng.device)))
+    _capi.check(eng._lib.nmfb200_raw_terms(eng._ctx, _ptr(eng.W), _ptr(eng.H), which, float(beta), _ptr(buf),
+                                           _stream(eng.device)))
     rows = eng.C if which == 0 else eng.N
     return buf[:rows * eng.R].view(rows, eng.R), buf[rows * eng.R:].view(rows, eng.R)
 
@@ -78,7 +78,7 @@ def _check_bar(tag, got, want, bar):
 
 @pytest.mark.parametrize("beta", sb.BETAS)
 @pytest.mark.parametrize("case", sb.SPARSE_BETA, ids=_id)
-def test_raw_terms_numerators_in_bar_denominators_equal_dense(case, beta):
+def test_sparse_raw_terms_numerators_in_bar_denominators_equal_dense(case, beta):
     N, C, R, _ = case
     data = sb.sparse_bar_data(case, seed=N + C + R)
     eng = _engine_of(case, *data)

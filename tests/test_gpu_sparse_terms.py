@@ -57,10 +57,10 @@ def _poison(eng):
 
 def _raw_terms_into_nan(eng, which, beta):
     """raw_terms through the ABI into a NaN-filled buffer: an entry the kernels do not write stays NaN."""
-    n = int(eng._lib.nmfb200_nmf_raw_terms_numel(eng._ctx, which, float(beta)))
+    n = int(eng._lib.nmfb200_raw_terms_numel(eng._ctx, which, float(beta)))
     buf = torch.full((n,), float("nan"), dtype=torch.float32, device=eng.device)
-    _capi.check(eng._lib.nmfb200_nmf_raw_terms(eng._ctx, _ptr(eng.W), _ptr(eng.H), which, float(beta), _ptr(buf),
-                                               _stream(eng.device)))
+    _capi.check(eng._lib.nmfb200_raw_terms(eng._ctx, _ptr(eng.W), _ptr(eng.H), which, float(beta), _ptr(buf),
+                                           _stream(eng.device)))
     rows = eng.C if which == 0 else eng.N
     num, den = buf[:rows * eng.R].view(rows, eng.R), buf[rows * eng.R:]
     return num, (den if beta == 1 else den.view(rows, eng.R))
@@ -90,7 +90,7 @@ def _dev64(rows, cols, vals, W, H):
 # ---- (a) exact ------------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("beta", [2, 1])
 @pytest.mark.parametrize("case", sc.SPARSE_EXACT, ids=_id)
-def test_sparse_raw_terms_exact(case, beta):
+def test_sparse_raw_terms_exact_at_every_plan(case, beta):
     data, Q = _exact(case, beta, seed=sum(case[:3]) + beta)
     eng = _engine(case, *data)
     d64 = _dev64(*data)

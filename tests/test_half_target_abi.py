@@ -1,5 +1,5 @@
-"""The C ABI of half-precision targets, without a GPU: the dtype enum of include/nmf_b200.h, the two typed set_target entry
-points in the library and in the ctypes binding, and the host side's dtype map."""
+"""The C ABI of half-precision targets, without a GPU: the dtype enum of include/nmf_b200.h, the two dense set_target entry
+points (both take the dtype) in the library and in the ctypes binding, and the host side's dtype map."""
 import ctypes
 import os
 import re
@@ -21,16 +21,16 @@ def test_header_dtype_enum():
     assert _capi.DTYPES == {torch.float32: 0, torch.float16: 1, torch.bfloat16: 2}
 
 
-def test_typed_set_target_symbols_and_argtypes():
-    assert _capi.SIGNATURES["nmfb200_nmf_set_target_typed"] == (_int, [_vp, _vp, _i64, _int, _vp])
-    assert _capi.SIGNATURES["nmfb200_nmfd_set_target_typed"] == (_int, [_vp, _vp, _int, _vp])
+def test_set_target_symbols_and_argtypes():
+    assert _capi.SIGNATURES["nmfb200_nmf_set_target"] == (_int, [_vp, _vp, _i64, _int, _vp])
+    assert _capi.SIGNATURES["nmfb200_nmfd_set_target"] == (_int, [_vp, _vp, _int, _vp])
     lib = _capi.load()
-    for name in ("nmfb200_nmf_set_target_typed", "nmfb200_nmfd_set_target_typed"):
+    for name in ("nmfb200_nmf_set_target", "nmfb200_nmfd_set_target"):
         fn = getattr(lib, name)
         assert fn.restype is _int and fn.argtypes == _capi.SIGNATURES[name][1]
-    assert lib.nmfb200_nmf_set_target_typed(None, None, 1, 0, None) == 1
+    assert lib.nmfb200_nmf_set_target(None, None, 1, 0, None) == 1
     assert b"null context" in lib.nmfb200_last_error()
-    assert lib.nmfb200_nmfd_set_target_typed(None, None, 0, None) == 1
+    assert lib.nmfb200_nmfd_set_target(None, None, 0, None) == 1
 
 
 def test_engine_target_checks():

@@ -79,7 +79,7 @@ def test_high_rank_exact_bounds(case):
     assert fc.loss_bound(R * f * f, f * f) < fc.EXACT_LOSS
 
 
-def test_sparse_and_convolutive_plans_keep_the_rank_cap():
+def test_sparse_and_convolutive_plans_cap_the_rank():
     with pytest.raises(_capi.NmfB200Error, match="256"):
         _capi.sparse_plan(5, 6, 257)
     with pytest.raises(_capi.NmfB200Error, match="256"):
@@ -87,7 +87,7 @@ def test_sparse_and_convolutive_plans_keep_the_rank_cap():
     with pytest.raises(_capi.NmfB200Error, match="256"):
         _capi.nmfd_plan(1, 3, [7, 70], 257, [3, 8])
     with pytest.raises(_capi.NmfB200Error, match="256"):
-        _capi.nmfd_tc_plan(1, 4, 100, 257, 4)
+        _capi.nmfnd_tc_plan(1, 4, [100], 257, [4])
     _capi.nmfd_plan(1, 4, [100], 256, [4])
 
 

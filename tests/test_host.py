@@ -76,7 +76,7 @@ def test_forward_accepts_external_factors_and_autograd():
 
 
 # ---- the C-ABI library ---------------------------------------------------------------------------
-def test_library_exports_every_declared_symbol():
+def test_library_exports_every_declared_symbol_at_abi_2():
     header = open(os.path.join(ROOT, "include", "nmf_b200.h")).read()
     declared = set(re.findall(r"\b(nmfb200_[a-z0-9_]+)\s*\(", header))
     declared.discard("nmfb200_ctx")
@@ -84,7 +84,7 @@ def test_library_exports_every_declared_symbol():
     lib = ctypes.CDLL(_capi.LIB_PATH)
     for name in declared:
         assert hasattr(lib, name), name
-    assert _capi.load().nmfb200_abi_version() == 1
+    assert _capi.load().nmfb200_abi_version() == 2
 
 
 def test_library_was_built_from_these_sources():
@@ -99,14 +99,26 @@ def test_library_was_built_from_these_sources():
     assert "arch=sm_90a" in info and "nvcc=12." in info
 
 
-def test_library_rejects_bad_arguments_without_gpu_work():
+def test_library_refuses_bad_arguments_without_gpu_work():
     lib = _capi.load()
     ctx = ctypes.c_void_p()
     assert lib.nmfb200_nmf_create(None, 0, 4, 4, 2, 0) != 0
     assert lib.nmfb200_nmf_create(ctypes.byref(ctx), 0, 0, 4, 2, 0) != 0
     assert b"positive" in lib.nmfb200_last_error()
     assert lib.nmfb200_nmf_create(ctypes.byref(ctx), 0, 4, 4, 2, 77) != 0
-    assert lib.nmfb200_nmf_w_partial_numel(None, 1.0) == -1
+    assert lib.nmfb200_raw_terms_numel(None, 0, 1.0) == -1
+    # the calls that serve both kinds refuse a null context before touching a device
+    refusals = {
+        "sync_factors": lambda: lib.nmfb200_sync_factors(None),
+        "update_w": lambda: lib.nmfb200_update_w(None, None, None, 1.0, 1.0, 0.0, 0.0, None),
+        "update_h": lambda: lib.nmfb200_update_h(None, None, None, 1.0, 1.0, 0.0, 0.0, None),
+        "loss": lambda: lib.nmfb200_loss(None, None, None, 1.0, None, None),
+        "raw_terms": lambda: lib.nmfb200_raw_terms(None, None, None, 0, 1.0, None, None),
+        "w_apply": lambda: lib.nmfb200_w_apply(None, None, None, 1.0, 1.0, 0.0, 0.0, None),
+    }
+    for name, call in refusals.items():
+        assert call() == 1, name                                                  # NMFB200_ERR_INVALID
+        assert b"null context" in lib.nmfb200_last_error(), name
 
 
 @pytest.mark.skipif(torch.cuda.is_available(), reason="checks the loud failure on a CUDA-less host")

@@ -1,7 +1,7 @@
 """Host checks of the limit cases (tests/limit_cases.py) and of the launch plans at the CUDA grid limits; no GPU.
 
   * Every big case really crosses element 2^31 where it says, and every grid case sits where it says.
-  * The plan queries (nmfb200_nmfd_plan, nmfb200_nmfd_tc_plan) either reject a shape or report grids with x <= 2^31 - 1 and
+  * The plan queries (nmfb200_nmfd_plan, nmfb200_nmfnd_tc_plan) either reject a shape or report grids with x <= 2^31 - 1 and
     y, z <= 65535, and counts the library holds in 32 bits that fit, for every case and a sweep around each bound.
   * The float64 references taken in blocks (as the GPU tests take them) equal the one-block references, on scaled-down
     copies of the big cases with the same structure, and the GPU tests check every row, the crossing rows included.
@@ -41,7 +41,7 @@ def _nmfd_plan_ok(B, C, L, R, T):
 
 def _tc_plan_ok(B, C, L, R, T):
     try:
-        p = _capi.nmfd_tc_plan(B, C, L, R, T)
+        p = _capi.nmfnd_tc_plan(B, C, [L], R, [T])
     except _capi.NmfB200Error as e:
         return None, str(e)
     for k in ("prep_w", "prep_h", "recon", "wgrad", "dgrad"):
@@ -81,7 +81,7 @@ def test_nmf_big_case_crosses_2p31(name):
 
 
 @pytest.mark.parametrize("name", list(lc.NMFD_BIG))
-def test_nmfd_big_case_crosses_2p31(name):
+def test_nmfd_big_case_crosses_2p31_in_both_plans(name):
     case = lc.NMFD_BIG[name]
     B, C, L, R, T = lc.nmfd_dims(case)
     assert B >= 2 and C == 1025 and (R, T) == (16, 16) and B * C * L > lc.ELEM
@@ -128,7 +128,7 @@ def _sweep():
 PREP_H_X = [(512, 1, 2 ** 25 - 2048, 256, 1), (512, 1, 2 ** 25, 256, 1), (1024, 1, 2 ** 25, 256, 1)]
 
 
-def test_prep_h_grid_at_its_limit():
+def test_tc_prep_h_grid_at_its_limit():
     (ok, why), (over, why_over), (over2, _) = (_tc_plan_ok(*s) for s in PREP_H_X)
     assert ok is not None, why
     assert ok["prep_h"][0] == 2 ** 31 - 2 ** 17
@@ -137,7 +137,7 @@ def test_prep_h_grid_at_its_limit():
         assert _nmfd_plan_ok(B, C, L, R, T) is not None            # the fp32 kernels take them: only prep_h rejects
 
 
-def test_plan_queries_report_launchable_grids_or_reject():
+def test_plan_queries_report_launchable_grids_or_refuse():
     fp32_rejected = tc_rejected = 0
     for B, C, L, R, T in _sweep():
         p = _nmfd_plan_ok(B, C, L, R, T)
@@ -151,27 +151,25 @@ def test_plan_queries_report_launchable_grids_or_reject():
     assert fp32_rejected and tc_rejected
 
 
-def test_plan_queries_name_the_limit():
+def test_plan_queries_name_their_limit():
     msg = {}
     for name, shape, prec, words in lc.REJECT_CASES:
         try:
-            (_capi.nmfd_tc_plan if prec == "f16" else lambda *a: _capi.nmfd_plan(a[0], a[1], [a[2]], a[3], [a[4]]))(*shape)
+            B, C, L, R, T = shape
+            (_capi.nmfnd_tc_plan if prec == "f16" else _capi.nmfd_plan)(B, C, [L], R, [T])
         except _capi.NmfB200Error as e:
             msg[name] = str(e)
         assert words in msg.get(name, ""), (name, msg.get(name))
     for name, kind, shape, prec, expected in lc.GRID_CASES:
         if kind == "nmfd" and expected != "runs":
             with pytest.raises(_capi.NmfB200Error, match=expected[1].replace("(", r"\(").replace(")", r"\)")):
-                if prec == "f16":
-                    _capi.nmfd_tc_plan(*shape)
-                else:
-                    B, C, L, R, T = shape
-                    _capi.nmfd_plan(B, C, [L], R, [T])
+                B, C, L, R, T = shape
+                (_capi.nmfnd_tc_plan if prec == "f16" else _capi.nmfd_plan)(B, C, [L], R, [T])
 
 
-def test_batch_slices_cover_the_batch():
+def test_tc_batch_slices_cover_the_batch():
     for B in (1, 65534, 65535, 65536, 131070, 131071, 2 ** 20 + 3):
-        p = _capi.nmfd_tc_plan(B, 1, 4, 2, 2)
+        p = _capi.nmfnd_tc_plan(B, 1, [4], 2, [2])
         assert p["bslice"] == min(B, 65535) and p["slices"] == lc.cdiv(B, 65535)
         assert p["prep_h"] == (B * 2, 1, 1)
 
@@ -265,10 +263,11 @@ def test_nmf_wrapped_index_moves_an_entry_past_its_bar(name):
             assert moved > 1.0, (name, prec, beta, moved)
 
 
-def test_nmfd_wrapped_index_moves_an_entry_past_its_bar():
+def test_nmfd_wrapped_line_moves_an_entry_past_its_bar():
     """Against the f16 bar plus the accumulation term the GPU test adds, with the full case's k-blocks per split."""
     big = lc.NMFD_BIG["nmfd_long"]
-    tcp = _capi.nmfd_tc_plan(*lc.nmfd_dims(big))
+    B, C, L, R, T = lc.nmfd_dims(big)
+    tcp = _capi.nmfnd_tc_plan(B, C, [L], R, [T])
     case = lc.scaled(big, "nmfd", SCALE)
     V, W, H = lc.nmfd_data(case, "cpu")
     want = lc.nmfd_terms_ref(V, W, H, 1, kappa=lc.nmfd_kappa(V, W, H))

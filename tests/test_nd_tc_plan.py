@@ -40,14 +40,13 @@ def test_plan_matches_restatement_on_more_shapes(shape):
 
 @pytest.mark.parametrize("case", [(1, 1, 200, 1, 200), (3, 43, 400, 2, 3), (1, 24, 96, 256, 8), (70000, 3, 50, 4, 5)],
                          ids=str)
-def test_one_axis_plan_is_the_nmfd_plan(case):
-    """ndim 1 (and NMF2D shapes whose outer axes are all 1) plan exactly what nmfb200_nmfd_tc_plan plans."""
+def test_outer_axes_of_size_one_plan_as_one_axis(case):
+    """NMF2D / NMF3D shapes whose outer axes are all 1 plan exactly what their one-axis NMFD shape plans."""
     B, C, L, R, T = case
-    a = _capi.nmfd_tc_plan(*case)
-    for vd, kd in (((L,), (T,)), ((1, L), (1, T)), ((1, 1, L), (1, 1, T))):
-        b = _capi.nmfnd_tc_plan(B, C, vd, R, kd)
-        assert all(a[k] == b[k] for k in a)
-        assert (b["hslice"], b["hslices"]) == (b["bslice"], b["slices"])
+    a = _capi.nmfnd_tc_plan(B, C, (L,), R, (T,))
+    assert (a["hslice"], a["hslices"]) == (a["bslice"], a["slices"])
+    for vd, kd in (((1, L), (1, T)), ((1, 1, L), (1, 1, T))):
+        assert _capi.nmfnd_tc_plan(B, C, vd, R, kd) == a
 
 
 ND = "the tensor-core NMF2D / NMF3D path needs "

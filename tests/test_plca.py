@@ -6,7 +6,7 @@ Fixtures: tests/golden/reference_next.npz (PLCA) and tests/golden/reference_plca
 
 CPU tests: the closed-form oracle (oracle/plca_oracle.py) against those fixtures -- this is what pins it -- and the module
 surface (constructors, shapes, normalisation, reconstruct).  GPU tests: `fit` through the C ABI
-(`nmfb200_nmf_raw_terms` / `nmfb200_nmfd_raw_terms`) against the same fixtures at rtol 1e-3.
+(`nmfb200_raw_terms`) against the same fixtures at rtol 1e-3.
 """
 import os
 
@@ -151,7 +151,7 @@ def test_siplca_fit_matches_reference(name):
 @pytest.mark.parametrize("return_module", [False, True])
 @pytest.mark.parametrize("name", BETAMU_ND)
 def test_betamu_convolutive_fused_path_matches_reference(name, return_module):
-    """BetaMu.step over an NMFD / NMF2D / NMF3D leaf takes both terms from nmfb200_nmfd_raw_terms (trainer.py:36-121)."""
+    """BetaMu.step over an NMFD / NMF2D / NMF3D leaf takes both terms from nmfb200_raw_terms (trainer.py:36-121)."""
     c = _case(name)
     m, paths = _run_betamu(c, "cuda", return_module)
     assert set(paths) == {"fused"}, paths

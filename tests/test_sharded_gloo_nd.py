@@ -26,7 +26,7 @@ BOUNDS = [0, 3, B]          # uneven shards: 3 + 2 batch elements
 
 
 class ShardableOracleNmfdEngine(OracleNmfdEngine):
-    """The oracle NMFD engine plus the batch-sharded W update, in the buffer layout of nmfb200_nmfd_w_partial."""
+    """The oracle NMFD engine plus the batch-sharded W update, in the buffer layout of nmfb200_raw_terms(which = 0)."""
 
     def w_partial(self, beta):
         num, den = self.raw_terms(0, beta)

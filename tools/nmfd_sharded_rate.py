@@ -8,7 +8,7 @@ precision "auto" and at beta 0.5 precision "f32".  Per workload and rank, one JS
   * sharded_it_s / unsharded_it_s: a timed `fit` of --iters iterations (tol -inf) after a --warmup fit, host clock around a
     device synchronise, with and without `group`; the two alternate, --rounds times each;
   * allreduce_ms: CUDA events around --reps sum-all-reduces, over the same group, of a buffer as long as the W terms
-    (nmfb200_nmfd_w_partial_numel), i.e. the device time of the W update's exchange;
+    (nmfb200_raw_terms_numel(which = 0)), i.e. the device time of the W update's exchange;
   * allreduce_bytes_per_iter: the bytes each rank contributes per iteration (the W terms, plus the 8-byte loss every 10th
     iteration).
 Rank 0 first prints the card's name, power limit and maximum SM clock.  With --nproc_per_node 1 the group has one rank:
@@ -102,7 +102,7 @@ def main():
                 rec.setdefault("sharded_it_s" if sharded else "unsharded_it_s", []).append(round(rate, 2))
                 rec["ran" if sharded else "ran_unsharded"] = m.last_fit_precision
         eng = CudaNmfdEngine(V, W0.clone(), H0.clone(), prec)
-        n = int(eng._lib.nmfb200_nmfd_w_partial_numel(eng._ctx, beta))
+        n = int(eng._lib.nmfb200_raw_terms_numel(eng._ctx, 0, beta))
         eng.close()
         dist.barrier(group)
         rec["allreduce_ms"] = round(allreduce_ms(n, a.reps, group), 4)
