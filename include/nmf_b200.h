@@ -218,6 +218,19 @@ int nmfb200_raw_terms(nmfb200_ctx* ctx, const float* W, const float* H, int whic
 int nmfb200_w_apply(nmfb200_ctx* ctx, float* W, const float* reduced, double beta, double gamma, double l1_reg,
                     double l2_reg, void* stream);
 
+/* Fit only the observed cells of a dense target.  M: a DEVICE array of uint8 in V's shape, contiguous (NMF: N x C whatever
+ * V's ldv; the convolutive models: V's layout), non-zero = observed; borrowed like V.  Valid after nmfb200_nmf_set_target /
+ * nmfb200_nmfd_set_target (NMFB200_ERR_STATE before), NMFB200_ERR_INVALID on a sparse context.  A null M, or any later
+ * set_target*, clears the mask (contexts are reused between fits).  While a mask is set the loss is
+ * beta_div(WH[M], V[M]) -- the missing cells dropped, not zeroed -- and every update is nmf.py:78-92 applied to the two
+ * backward passes of that loss: num = (M * v x^(beta-2)) G, den = (M * x^(beta-1)) G, so at beta 1 den = M G instead of the
+ * column sums of G.  The kernels select, they never multiply by the mask: V is not read at a missing cell, so a NaN, Inf or
+ * negative value there gives the bits a zero gives.  update_w, update_h, nmf_iterate, loss, nmf_loss_prefetch_w (= loss),
+ * raw_terms (raw_terms_numel: 2 x the factor's numel at every beta), w_apply, contract_only and target_minmax (observed
+ * cells only) follow it; they run on the fp32 CUDA-core kernels (precision_for_beta reports NMFB200_PREC_F32,
+ * nmf_peer_supported 0) and leave the tensor-core operand copies marked stale.  Asynchronous. */
+int nmfb200_set_mask(nmfb200_ctx* ctx, const uint8_t* M, void* stream);
+
 /* ---- tile plans of the fp32 CUDA-core kernels (host only: no device work, no allocation) -------- */
 
 /* What a context of these sizes runs on the fp32 kernels, from the library's own planners.  `out` receives

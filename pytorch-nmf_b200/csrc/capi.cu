@@ -29,6 +29,9 @@ struct nmfb200_ctx {
   int vdtype = NMFB200_DTYPE_F32;
   int64_t ldv = 0;
   bool has_target = false;
+  // nmfb200_set_mask: the observed cells (uint8, V's shape, contiguous), borrowed; cleared by every set_target*.  While set,
+  // every pass runs the masked fp32 kernels and beta 1 takes its denominators from the contraction, not the column sums.
+  const uint8_t* mask = nullptr;
   // chunked partial numerators / denominators of the CUDA-core path
   float* num = nullptr;
   float* den = nullptr;
@@ -146,14 +149,18 @@ int alloc_workspace(nmfb200_ctx* c, int64_t pn_floats) {
 
 // CUDA-core contraction of one NMF factor update (which = 0: W, 1: H) into c->num / c->den (chunked partials).
 int simt_contract(nmfb200_ctx* c, int which, const float* W, const float* H, double beta, cudaStream_t st) {
-  if (beta != 1.0) { int e = ensure_den(c); if (e) return e; }
+  if (beta != 1.0 || c->mask) { int e = ensure_den(c); if (e) return e; }
   // W update: F = W (C rows), G = H (N rows), Vm = V^T;  H update: F = H (N rows), G = W (C rows), Vm = V
   const float* F = which == 0 ? W : H;
   const float* G = which == 0 ? H : W;
   const int64_t rows = which == 0 ? c->C : c->N, cols = which == 0 ? c->N : c->C;
   return simt_nmf_contract(c->V, c->vdtype, c->ldv, /*trans=*/which == 0 ? 1 : 0, F, G, rows, cols, (int)c->R, beta,
-                           which == 0 ? c->nch_w : c->nch_h, c->num, c->den, c->R, rows * c->R, st);
+                           which == 0 ? c->nch_w : c->nch_h, c->num, c->den, c->R, rows * c->R, c->mask, c->C, st);
 }
+
+// beta 1 without a mask: the denominator is the column sum of the other factor (nmf.py:122-131).  A masked fit takes it
+// from the second backward pass, M G, like every other beta.
+bool kl_colsum(const nmfb200_ctx* c, double beta) { return beta == 1.0 && !c->mask; }
 
 // The ratio stage's view of one NMF factor (which = 0: W, 1: H) of R components: numerators summed over `nchunks` partial
 // slabs, and `den` = the column sums of the other factor (beta 1) or the raw denominators in the numerators' layout.
@@ -161,14 +168,15 @@ ApplyArgs nmf_apply_args(const nmfb200_ctx* c, int which, float* param, double b
                          int nchunks, int64_t chunk_stride, double gamma, double l1, double l2) {
   ApplyArgs a{};
   a.param = param; a.numel = (which == 0 ? c->C : c->N) * c->R; a.R = (int)c->R; a.inner = 1; a.rowlen = c->R;
-  a.num = num; a.den = beta == 1.0 ? nullptr : den; a.nchunks = nchunks; a.chunk_stride = chunk_stride;
-  a.ldp = c->R; a.kl_den = beta == 1.0 ? den : nullptr; a.out_scale = nullptr;
+  const bool kl = kl_colsum(c, beta);
+  a.num = num; a.den = kl ? nullptr : den; a.nchunks = nchunks; a.chunk_stride = chunk_stride;
+  a.ldp = c->R; a.kl_den = kl ? den : nullptr; a.out_scale = nullptr;
   a.gamma = (float)gamma; a.l1 = (float)l1; a.l2 = (float)l2; a.absmax_bits = nullptr;
   return a;
 }
 
 bool use_tc(const nmfb200_ctx* c, double beta) {
-  return c->tc != nullptr && !c->tc_off && tc_supports_beta(c->tc, beta);
+  return c->tc != nullptr && !c->tc_off && !c->mask && tc_supports_beta(c->tc, beta);
 }
 
 // What every dense set_target checks of the target's element type and pointer (the kernels load single elements: element
@@ -284,6 +292,7 @@ int nmfb200_precision(const nmfb200_ctx* ctx) {
 
 int nmfb200_precision_for_beta(const nmfb200_ctx* ctx, double beta) {
   if (!ctx) return -100;
+  if (ctx->mask) return NMFB200_PREC_F32;
   if (ctx->kind == 1) return (ctx->tcd && !ctx->tc_off && tc_nmfd_supported(ctx->d, beta)) ? NMFB200_PREC_F16 : NMFB200_PREC_F32;
   if (ctx->kind != 0 || !use_tc(ctx, beta)) return NMFB200_PREC_F32;
   // beta != 1 kernels read only the hi halves of the operand copies
@@ -325,6 +334,7 @@ int nmfb200_nmf_set_target(nmfb200_ctx* ctx, const void* V, int64_t ldv, int dty
   if (int rc = check_target(V, dtype)) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   ctx->V = V; ctx->vdtype = dtype; ctx->ldv = ldv; ctx->has_target = true; ctx->sparse = false; ctx->sp_any_beta = false;
+  ctx->mask = nullptr;
   float* minmax = ctx->mm_scratch + kMmPartials;
   int rc = matrix_minmax(V, dtype, ctx->N, ctx->C, ldv, ctx->mm_scratch, minmax, st);
   if (rc) return rc;
@@ -372,6 +382,7 @@ int nmfb200_nmf_set_target_sparse(nmfb200_ctx* ctx, int64_t nnz, const int64_t* 
   ctx->sp_crow = crow; ctx->sp_col = col; ctx->sp_val = val; ctx->sp_ccol = ccol; ctx->sp_row = row; ctx->sp_val_t = val_t;
   ctx->sp_vnorm_kl = v_norm_kl; ctx->sp_vnorm_eu = v_norm_eu;
   ctx->sparse = true; ctx->has_target = true; ctx->V = nullptr; ctx->tc_off = true;      // the dense kernels are out of play
+  ctx->mask = nullptr;
   ctx->sp_any_beta = false;
   return 0;
 }
@@ -451,7 +462,7 @@ int nmf_update(nmfb200_ctx* ctx, int which, float* param, const float* W, const 
   int rc = simt_contract(ctx, which, W, H, beta, st);
   if (rc) return rc;
   float* den = ctx->den;
-  if (beta == 1.0) {      // nmf.py:122-131: the KL denominator is the column sum of the OTHER factor
+  if (kl_colsum(ctx, beta)) {      // nmf.py:122-131: the KL denominator is the column sum of the OTHER factor
     den = ctx->colsum + (1 - which) * ctx->R;
     rc = factor_colsum(other, which == 0 ? ctx->N : ctx->C, (int)ctx->R, 1, ctx->cs_scratch, ctx->cs_scratch_floats, den, st);
     if (rc) return rc;
@@ -475,7 +486,7 @@ int nmf_raw_terms(nmfb200_ctx* ctx, const float* W, const float* H, int which, d
   const int nch = which == 0 ? ctx->nch_w : ctx->nch_h;
   rc = reduce_chunks(ctx->num, nch, RR, rows, (int)ctx->R, ctx->R, out, st);
   if (rc) return rc;
-  if (beta == 1.0) {      // nmf.py:122-131: the KL denominator is the column sum of the OTHER factor
+  if (kl_colsum(ctx, beta)) {      // nmf.py:122-131: the KL denominator is the column sum of the OTHER factor
     const float* other = which == 0 ? H : W;
     return factor_colsum(other, which == 0 ? ctx->N : ctx->C, (int)ctx->R, 1, ctx->cs_scratch, ctx->cs_scratch_floats,
                          out + RR, st);
@@ -551,7 +562,7 @@ int nmfb200_nmf_loss_prefetch_w(nmfb200_ctx* ctx, const float* W, const float* H
 /* ---- row-sharded W update over peer memory (NVLink, one process per GPU) ---------------------- */
 
 int nmfb200_nmf_peer_supported(const nmfb200_ctx* ctx, double beta) {
-  if (!ctx || ctx->kind != 0 || !ctx->tc || ctx->tc_off || !ctx->has_target) return 0;
+  if (!ctx || ctx->kind != 0 || !ctx->tc || ctx->tc_off || !ctx->has_target || ctx->mask) return 0;
   return (tc_supports_beta(ctx->tc, beta) && tc_peer_supported(ctx->tc, beta)) ? 1 : 0;
 }
 
@@ -689,7 +700,7 @@ int nmfb200_nmfnd_create(nmfb200_ctx** out, int device, int64_t B, int64_t C, in
 int nmfb200_nmfd_set_target(nmfb200_ctx* ctx, const void* V, int dtype, void* stream) {
   CTX_GUARD(ctx, 1);
   if (int rc = check_target(V, dtype)) return rc;
-  ctx->V = V; ctx->vdtype = dtype; ctx->has_target = true;
+  ctx->V = V; ctx->vdtype = dtype; ctx->has_target = true; ctx->mask = nullptr;
   cudaStream_t st = (cudaStream_t)stream;
   const int64_t vin = ctx->d.v_inner();
   int rc = matrix_minmax(V, dtype, (int64_t)ctx->d.B * ctx->d.C, vin, vin, ctx->mm_scratch, ctx->mm_scratch + kMmPartials, st);
@@ -708,16 +719,16 @@ int nmfb200_nmfd_set_target(nmfb200_ctx* ctx, const void* V, int dtype, void* st
 
 // beta = 1 on tensor cores: both column-sum vectors (KL denominators, nmf.py:122-131, and kappa), then the recon pass
 static bool nmfd_use_tc(const nmfb200_ctx* c, double beta) {
-  return c->tcd != nullptr && !c->tc_off && tc_nmfd_supported(c->d, beta);
+  return c->tcd != nullptr && !c->tc_off && !c->mask && tc_nmfd_supported(c->d, beta);
 }
 
 static int nmfd_phi(nmfb200_ctx* c, const float* W, const float* H, double beta, cudaStream_t st) {
-  if (beta != 1.0) {
+  if (beta != 1.0 || c->mask) {
     if (!c->Pp) NMF_CUDA_CHECK(cudaMalloc(&c->Pp, (size_t)c->d.B * c->d.C * c->d.v_inner() * sizeof(float)));
     int e = ensure_den(c);
     if (e) return e;
   }
-  return nmfd_recon_phi(c->d, c->V, c->vdtype, W, H, beta, c->Pn, c->Pp, nullptr, 0, nullptr, st);
+  return nmfd_recon_phi(c->d, c->V, c->vdtype, W, H, beta, c->Pn, c->Pp, nullptr, 0, nullptr, st, c->mask);
 }
 
 // Both backward passes of one factor (which = 0: W, 1: H) from the current factors, described as the ratio stage's input:
@@ -746,7 +757,8 @@ static int nmfd_terms(nmfb200_ctx* ctx, const float* W, const float* H, int whic
   rc = which == 0 ? nmfd_wgrad(d, ctx->Pn, H, ctx->num, nsplit, st) : nmfd_dgrad(d, ctx->Pn, W, ctx->num, nsplit, st);
   if (rc) return rc;
   float* kl = nullptr;
-  if (beta == 1.0) {                                     // nmf.py:122-131: column sums of the OTHER factor
+  const bool colsum = kl_colsum(ctx, beta);
+  if (colsum) {                                          // nmf.py:122-131: column sums of the OTHER factor
     kl = ctx->colsum + (which == 0 ? d.R : 0);
     rc = which == 0 ? factor_colsum(H, d.B, d.R, d.h_inner(), ctx->cs_scratch, ctx->cs_scratch_floats, kl, st)
                     : factor_colsum(W, d.C, d.R, d.w_inner(), ctx->cs_scratch, ctx->cs_scratch_floats, kl, st);
@@ -754,7 +766,7 @@ static int nmfd_terms(nmfb200_ctx* ctx, const float* W, const float* H, int whic
     rc = which == 0 ? nmfd_wgrad(d, ctx->Pp, H, ctx->den, nsplit, st) : nmfd_dgrad(d, ctx->Pp, W, ctx->den, nsplit, st);
   }
   if (rc) return rc;
-  a.num = ctx->num; a.den = beta == 1.0 ? nullptr : ctx->den; a.nchunks = nsplit; a.kl_den = kl;
+  a.num = ctx->num; a.den = colsum ? nullptr : ctx->den; a.nchunks = nsplit; a.kl_den = kl;
   return 0;
 }
 
@@ -809,7 +821,7 @@ static int nmfd_raw_terms(nmfb200_ctx* ctx, const float* W, const float* H, int 
   if (rc) return rc;
   rc = raw_sum(a, out, a.den ? out + a.numel : nullptr, st);
   if (rc) return rc;
-  if (beta == 1.0)
+  if (a.kl_den)
     NMF_CUDA_CHECK(cudaMemcpyAsync(out + a.numel, a.kl_den, (size_t)ctx->d.R * sizeof(float), cudaMemcpyDeviceToDevice, st));
   return 0;
 }
@@ -853,12 +865,12 @@ int nmfb200_loss(nmfb200_ctx* ctx, const float* W, const float* H, double beta, 
   if (ctx->kind == 1) {
     if (nmfd_use_tc(ctx, beta)) return tc_nmfd_recon(ctx->tcd, ctx->V, ctx->vdtype, W, H, true, loss_dev, st);
     return nmfd_recon_phi(ctx->d, ctx->V, ctx->vdtype, W, H, beta, nullptr, nullptr, ctx->loss_blocks, ctx->loss_max_blocks,
-                          loss_dev, st);
+                          loss_dev, st, ctx->mask);
   }
   if (ctx->sparse) return sparse_loss_ctx(ctx, W, H, beta, loss_dev, st);
   if (use_tc(ctx, beta)) return tc_loss(ctx->tc, W, H, beta, loss_dev, st);
   return simt_nmf_loss(ctx->V, ctx->vdtype, ctx->ldv, H, W, ctx->N, ctx->C, (int)ctx->R, beta, ctx->loss_blocks,
-                       ctx->loss_max_blocks, loss_dev, st);
+                       ctx->loss_max_blocks, loss_dev, ctx->mask, ctx->C, st);
 }
 
 int64_t nmfb200_raw_terms_numel(const nmfb200_ctx* ctx, int which, double beta) {
@@ -866,7 +878,7 @@ int64_t nmfb200_raw_terms_numel(const nmfb200_ctx* ctx, int which, double beta) 
   const NmfdShape& d = ctx->d;
   const int64_t n = ctx->kind == 0 ? (which == 0 ? ctx->C : ctx->N) * ctx->R
                                    : (int64_t)(which == 0 ? d.C : d.B) * d.R * (which == 0 ? d.w_inner() : d.h_inner());
-  return beta == 1.0 ? n + ctx->R : 2 * n;
+  return kl_colsum(ctx, beta) ? n + ctx->R : 2 * n;
 }
 
 int nmfb200_raw_terms(nmfb200_ctx* ctx, const float* W, const float* H, int which, double beta, float* out, void* stream) {
@@ -894,11 +906,26 @@ int nmfb200_w_apply(nmfb200_ctx* ctx, float* W, const float* reduced, double bet
   }
   ApplyArgs a = nmfd_apply_shape(ctx->d, 0, 1);     // the centring term is already folded in by raw_sum
   a.param = W; a.num = reduced; a.gamma = (float)gamma; a.l1 = (float)l1_reg; a.l2 = (float)l2_reg;
-  if (beta == 1.0) a.kl_den = reduced + a.numel;
+  if (kl_colsum(ctx, beta)) a.kl_den = reduced + a.numel;
   else a.den = reduced + a.numel;
   if (nmfd_use_tc(ctx, beta)) a.absmax_bits = tc_nmfd_begin_update(ctx->tcd, 0, st);
   else if (ctx->tcd) tc_nmfd_mark_dirty(ctx->tcd);
   return apply_update(a, st);
+}
+
+int nmfb200_set_mask(nmfb200_ctx* ctx, const uint8_t* M, void* stream) {
+  CTX_GUARD(ctx, kAnyKind);
+  TARGET_GUARD(ctx);
+  if (ctx->sparse) return fail(NMFB200_ERR_INVALID, "a mask needs a dense target (set_target or nmfd_set_target)");
+  cudaStream_t st = (cudaStream_t)stream;
+  ctx->mask = M;
+  // the tensor-core paths are bypassed while a mask is set: their operand copies are rebuilt on their next use
+  if (ctx->tc) tc_mark_dirty(ctx->tc, true, true);
+  if (ctx->tcd) tc_nmfd_mark_dirty(ctx->tcd);
+  float* minmax = ctx->mm_scratch + kMmPartials;          // target_minmax: the observed cells only, or all of V again
+  if (ctx->kind == 0) return matrix_minmax(ctx->V, ctx->vdtype, ctx->N, ctx->C, ctx->ldv, ctx->mm_scratch, minmax, st, M);
+  const int64_t vin = ctx->d.v_inner();
+  return matrix_minmax(ctx->V, ctx->vdtype, (int64_t)ctx->d.B * ctx->d.C, vin, vin, ctx->mm_scratch, minmax, st, M);
 }
 
 int nmfb200_hoyer_project(int device, float* x, int64_t outer, int64_t D, int64_t inner, const float* k1, const float* k2,

@@ -87,13 +87,17 @@ static inline bool grid_fits(const Grid3& g) {
 //   num[ch][m][r] = sum_{c in chunk ch} Pn[m,c] G[c,r]          [nmf.py:77]
 //   den[ch][m][r] = sum_{c in chunk ch} Pp[m,c] G[c,r]          [nmf.py:82, beta != 1 only]
 // Vm[m,c] = V[m*ldv + c] (trans = 0) or V[c*ldv + m] (trans = 1), elements of type `vdtype` (VDtype).  Any rank R >= 1.
+// M (optional, uint8, read like V with pitch ldm): a fit on the observed cells only -- Pn = Pp = 0 where M is 0, V is not
+// read there, and den is always formed (beta 1: Pp = M).  M == nullptr runs the unmasked kernels.
 int simt_nmf_contract(const void* V, int vdtype, int64_t ldv, int trans, const float* F, const float* G,
                       int64_t Mr, int64_t Nc, int R, double beta, int nchunks,
-                      float* num, float* den, int64_t ldp, int64_t chunk_stride, cudaStream_t st);
-// beta_div(F G^T, Vm) accumulated into block partials then *loss_dev (double).  v_const is unused here.
+                      float* num, float* den, int64_t ldp, int64_t chunk_stride, const uint8_t* M, int64_t ldm,
+                      cudaStream_t st);
+// beta_div(F G^T, Vm) accumulated into block partials then *loss_dev (double); over the cells where M (optional, pitch
+// ldm, not transposed) is set.
 int simt_nmf_loss(const void* V, int vdtype, int64_t ldv, const float* F, const float* G, int64_t Mr, int64_t Nc,
-                  int R, double beta, double* block_partials, int max_blocks, double* loss_dev,
-                  cudaStream_t st);
+                  int R, double beta, double* block_partials, int max_blocks, double* loss_dev, const uint8_t* M,
+                  int64_t ldm, cudaStream_t st);
 int simt_nmf_max_blocks(int64_t Mr, int64_t Nc);
 // The V-free pieces of a sparse target's update and loss at beta != 1, 2 (nmf.py:621-636):
 //   den[ch][m][r] = sum_{c in chunk ch} (S[m,c] + eps)^(beta-1) G[c,r]: simt_nmf_contract's denominator at this beta, bit for
@@ -136,9 +140,10 @@ int64_t colsum_scratch_floats(int64_t outer, int R, int64_t inner);
 // dst[i] = sum_ch src[ch*stride + i]   (chunk reduction for the sharded partial buffers)
 int reduce_chunks(const float* src, int nchunks, int64_t chunk_stride, int64_t rows, int R, int64_t ldp,
                   float* dst, cudaStream_t st);
-// min / max of a strided matrix of `vdtype` elements (fit()'s validation), results in mm[0..1]
+// min / max of a strided matrix of `vdtype` elements (fit()'s validation), results in mm[0..1]; with M (optional, contiguous
+// rows x cols uint8) over the cells where M is set only (none: +inf / -inf)
 int matrix_minmax(const void* V, int vdtype, int64_t rows, int64_t cols, int64_t ld, float* scratch2048, float* mm,
-                  cudaStream_t st);
+                  cudaStream_t st, const uint8_t* M = nullptr);
 // *out = sum of n doubles in fixed order (single block)
 int sum_partials(const double* p, int n, double* out, cudaStream_t st);
 
@@ -185,10 +190,11 @@ struct NmfdShape {
   __host__ __device__ bool one_d() const { return X1 == 1 && X2 == 1 && T1 == 1 && T2 == 1; }
 };
 // WH = conv(H, W); writes Pn (and Pp when beta != 1) (B,C,L) or, when loss_blocks != nullptr,
-// reduces beta_div(WH, V) instead.
+// reduces beta_div(WH, V) instead.  M (optional, uint8 in V's layout): Pn = Pp = 0 at the missing cells and V is not read
+// there, Pp is written at every beta (beta 1: Pp = M as 0 / 1), and the loss skips them.
 int nmfd_recon_phi(const NmfdShape& s, const void* V, int vdtype, const float* W, const float* H, double beta,
                    float* Pn, float* Pp, double* loss_blocks, int max_blocks, double* loss_dev,
-                   cudaStream_t st);
+                   cudaStream_t st, const uint8_t* M = nullptr);
 // batch elements per launch of the kernels that put the batch on grid.z (fp32 recon / dgrad, tensor-core recon / dgrad)
 static inline int64_t nmfd_batch_slice(int64_t B) { return B < kMaxGridYZ ? B : kMaxGridYZ; }
 // loss partials of nmfd_recon_phi: one per block of all its launches

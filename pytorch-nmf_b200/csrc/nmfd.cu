@@ -78,11 +78,14 @@ struct SlideArgs {
   int64_t sm, sk;            // strides of A over m and k (elements); the offset (t1, t2, t) is contiguous
   int nsplit;                // !FWD: splits of k
   const void* V; float beta; float* Pn; float* Pp; double* block_partials;      // FWD epilogue (V: TV elements)
+  const uint8_t* mask;       // FWD, MASK: the observed cells (V's layout)
   float* out;                // !FWD: [split][B][R][h_inner]
   int b0;                    // first batch element of this launch
 };
 
-template <int MT, bool FWD, int MODE, bool LOSS, typename TV>
+// MASK (FWD only): a fit on the observed cells -- at a missing cell V is not read, Pn = Pp = 0 and the loss adds nothing;
+// Pp is written at every beta (beta 1: the mask as 0 / 1), so wgrad / dgrad of Pp give the denominators
+template <int MT, bool FWD, int MODE, bool LOSS, typename TV, bool MASK = false>
 __global__ void __launch_bounds__(256)
 nmfd_slide_kernel(NmfdShape s, SlideArgs a) {
   using G = Geo<MT>;
@@ -186,6 +189,10 @@ nmfd_slide_kernel(NmfdShape s, SlideArgs a) {
         const int l = l0 + 4 * lt + j;
         if (c < s.C && l < s.L && o < OUT) {
           const int64_t off = (((int64_t)b * s.C + c) * OUT + o) * s.L + l;
+          if (MASK && !a.mask[off]) {
+            if (!LOSS) { a.Pn[off] = 0.f; a.Pp[off] = 0.f; }
+            continue;
+          }
           const float v = to_f32(static_cast<const TV*>(a.V)[off]);
           if (LOSS) {
             local += loss_term_d<MODE>(v, acc[i][j], a.beta);
@@ -194,6 +201,7 @@ nmfd_slide_kernel(NmfdShape s, SlideArgs a) {
             phi_d<MODE>(v, acc[i][j], bm2, bm1, pn, pp);
             a.Pn[off] = pn;
             if (MODE != kKL) a.Pp[off] = pp;
+            else if (MASK) a.Pp[off] = 1.f;
           }
         }
       }
@@ -354,14 +362,23 @@ dim3 dim3_of(const Grid3& g) { return dim3((unsigned)g.x, (unsigned)g.y, (unsign
 template <int MT, bool FWD, typename TV>
 void launch_slide(const NmfdShape& s, const SlideArgs& a, int mode, bool loss, dim3 grid, cudaStream_t st) {
   if (!FWD) { nmfd_slide_kernel<MT, false, kKL, false, float><<<grid, 256, 0, st>>>(s, a); return; }
-#define NMFD_GO(M)                                                                  \
-  if (loss) nmfd_slide_kernel<MT, true, M, true, TV><<<grid, 256, 0, st>>>(s, a);   \
-  else nmfd_slide_kernel<MT, true, M, false, TV><<<grid, 256, 0, st>>>(s, a);
-  switch (mode) {
-    case kKL: NMFD_GO(kKL); break;
-    case kEU: NMFD_GO(kEU); break;
-    case kIS: NMFD_GO(kIS); break;
-    default: NMFD_GO(kGeneric); break;
+#define NMFD_GO(M, MK)                                                                  \
+  if (loss) nmfd_slide_kernel<MT, true, M, true, TV, MK><<<grid, 256, 0, st>>>(s, a);   \
+  else nmfd_slide_kernel<MT, true, M, false, TV, MK><<<grid, 256, 0, st>>>(s, a);
+  if (a.mask) {
+    switch (mode) {
+      case kKL: NMFD_GO(kKL, true); break;
+      case kEU: NMFD_GO(kEU, true); break;
+      case kIS: NMFD_GO(kIS, true); break;
+      default: NMFD_GO(kGeneric, true); break;
+    }
+  } else {
+    switch (mode) {
+      case kKL: NMFD_GO(kKL, false); break;
+      case kEU: NMFD_GO(kEU, false); break;
+      case kIS: NMFD_GO(kIS, false); break;
+      default: NMFD_GO(kGeneric, false); break;
+    }
   }
 #undef NMFD_GO
 }
@@ -398,7 +415,7 @@ int64_t nmfd_max_blocks(const NmfdShape& s) {
 }
 
 int nmfd_recon_phi(const NmfdShape& s, const void* V, int vdtype, const float* W, const float* H, double beta, float* Pn,
-                   float* Pp, double* loss_blocks, int max_blocks, double* loss_dev, cudaStream_t st) {
+                   float* Pp, double* loss_blocks, int max_blocks, double* loss_dev, cudaStream_t st, const uint8_t* M) {
   const int mt = row_tile(s.C);
   const Grid3 grid = slide_grid(s, true, mt, s.C, 1);
   const int nblocks = (int)nmfd_max_blocks(s);          // create bounds it (nmfd_shape_of)
@@ -406,7 +423,7 @@ int nmfd_recon_phi(const NmfdShape& s, const void* V, int vdtype, const float* W
   if (loss && nblocks > max_blocks) { set_error("nmfd loss: partial buffer too small"); return 1; }
   SlideArgs a{};
   a.A = W; a.X = H; a.M = s.C; a.K = s.R; a.sm = (int64_t)s.R * s.w_inner(); a.sk = s.w_inner(); a.nsplit = 1;
-  a.V = V; a.beta = (float)beta; a.Pn = Pn; a.Pp = Pp; a.block_partials = loss_blocks; a.out = nullptr;
+  a.V = V; a.beta = (float)beta; a.Pn = Pn; a.Pp = Pp; a.block_partials = loss_blocks; a.out = nullptr; a.mask = M;
   if (int rc = with_vtype(V, vdtype, [&](auto Vt) {
         return launch_slices<true, vtype_t<decltype(Vt)>>(mt, s, a, beta_mode(beta), loss, grid, st);
       }))

@@ -56,6 +56,7 @@ SIGNATURES = {
     "nmfb200_raw_terms_numel": (_i64, [_vp, _int, _dbl]),
     "nmfb200_raw_terms": (_int, [_vp, _vp, _vp, _int, _dbl, _vp, _vp]),
     "nmfb200_w_apply": (_int, [_vp, _vp, _vp, _dbl, _dbl, _dbl, _dbl, _vp]),
+    "nmfb200_set_mask": (_int, [_vp, _vp, _vp]),
     "nmfb200_hoyer_project": (_int, [_int, _vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp]),
     "nmfb200_nmf_plan": (_int, [_i64, _i64, _i64, _c.POINTER(_i64), _int]),
     "nmfb200_nmfd_plan": (_int, [_i64, _i64, _int, _c.POINTER(_i64), _i64, _c.POINTER(_i64), _c.POINTER(_i64), _int]),

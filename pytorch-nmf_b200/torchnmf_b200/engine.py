@@ -133,6 +133,7 @@ class _CudaEngine:
         self._loss = None
         self._key = None
         self._wbuf = None
+        self._mask = None
 
     def _acquire(self, key, create):
         """Take a cached context for `key` or create one with `create(ctx_ref)`."""
@@ -170,6 +171,18 @@ class _CudaEngine:
         """Arithmetic the contraction kernels use for this beta ("f32" when the tensor-core path does not cover it)."""
         return _capi.PRECISION_NAMES[self._lib.nmfb200_precision_for_beta(self._ctx, float(beta))]
 
+    def set_mask(self, M):
+        """Fit only the observed cells of V from now on (include/nmf_b200.h: nmfb200_set_mask): M is a contiguous bool or
+        uint8 tensor of V's shape on the engine's device, read in place (True = observed); None clears the mask.  The engine
+        keeps a reference to M while it is set.  minmax() then covers the observed cells only."""
+        if M is not None:
+            if M.dtype not in (torch.bool, torch.uint8) or M.device != self.device or not M.is_contiguous():
+                raise ValueError("the mask must be a contiguous bool tensor on the engine's device")
+            if tuple(M.shape) != tuple(self.V.shape):
+                raise ValueError(f"the mask's shape {tuple(M.shape)} does not match V's {tuple(self.V.shape)}")
+        self._mask = M
+        _capi.check(self._lib.nmfb200_set_mask(self._ctx, _ptr(M) if M is not None else None, _stream(self.device)))
+
     def minmax(self):
         vmin, vmax = ctypes.c_float(), ctypes.c_float()
         _capi.check(self._lib.nmfb200_target_minmax(self._ctx, ctypes.byref(vmin), ctypes.byref(vmax),
@@ -203,15 +216,16 @@ class _CudaEngine:
 
     def raw_terms(self, which, beta):
         """(numerator, denominator) of the update of W (which=0) or H (which=1) from the CURRENT factors, untouched: the
-        numerator in the factor's shape; the denominator (R,) for beta == 1 (the column sums of the other factor), else in
-        the factor's shape.  What BetaMu.step and PLCA.fit are built from (include/nmf_b200.h: nmfb200_raw_terms)."""
+        numerator in the factor's shape; the denominator (R,) for beta == 1 without a mask (the column sums of the other
+        factor), else in the factor's shape.  What BetaMu.step and PLCA.fit are built from (include/nmf_b200.h:
+        nmfb200_raw_terms)."""
         f = self.W if which == 0 else self.H
         n = int(self._lib.nmfb200_raw_terms_numel(self._ctx, int(which), float(beta)))
         buf = torch.empty(n, dtype=torch.float32, device=self.device)
         _capi.check(self._lib.nmfb200_raw_terms(self._ctx, _ptr(self.W), _ptr(self.H), int(which), float(beta), _ptr(buf),
                                                 _stream(self.device)))
         num, den = buf[:f.numel()].view(f.shape), buf[f.numel():]
-        return num, (den if beta == 1 else den.view(f.shape))
+        return num, (den if beta == 1 and self._mask is None else den.view(f.shape))
 
     # --- pieces of the sharded W update (ShardedEngine) ---------------------------------------
     def w_partial(self, beta):
@@ -435,6 +449,10 @@ class ShardedEngine:
 
     def sync(self):
         self.local.sync()
+
+    def set_mask(self, M):
+        """This rank's shard of the mask (the rows / batch elements of its V shard)."""
+        self.local.set_mask(M)
 
     def minmax(self):
         vmin, vmax = self.local.minmax()

@@ -174,10 +174,11 @@ class BaseComponent(torch.nn.Module):
     _sparse_kernels = True        # a sparse target on the library's sparse kernels (False: densify)
     _strided_target = False       # the engine reads a row-strided (unit column stride) half-precision target as it is
 
-    def _open_engine(self, V, beta, precision, group, sparse_kernels):
+    def _open_engine(self, V, beta, precision, group, sparse_kernels, mask=None):
         """Shared entry of `fit` / `sparse_fit`: validation that needs no device pass, placement of V / W / H on the CUDA
         device (host buffers are copied there; a dense bf16 / fp16 target keeps its dtype, other target and factor dtypes are
-        staged through fp32 device copies) and the engine for this target.
+        staged through fp32 device copies) and the engine for this target, with `mask` (validated by `_check_mask`) set on
+        it: moved to the engine's device and made contiguous, read there in place as one byte per cell.
         Returns (engine, W, H, Wd, Hd, staged): W / H the Parameters, Wd / Hd the fp32 device tensors the engine updates."""
         sparse_target = V.is_sparse
         if sparse_target and not self._sparse_targets:
@@ -226,9 +227,11 @@ class BaseComponent(torch.nn.Module):
             if not Wd.is_contiguous() or not Hd.is_contiguous():
                 raise ValueError("W and H must be contiguous")
             eng = sparse_cls(Vd.coalesce(), Wd, Hd) if use_sparse_kernels else self._build_engine(Vd, Wd, Hd, precision)
+            Md = mask.to(dev).contiguous() if mask is not None else None
         else:
             Wd, Hd = W.data, H.data
             eng = self._engine_factory(V.to_dense() if (sparse_target and not sparse_kernels) else V, Wd, Hd)
+            Md = mask
         if group is not None:
             eng = _engine.ShardedEngine(eng, group)
             if eng.kind == "nmfd":
@@ -241,11 +244,29 @@ class BaseComponent(torch.nn.Module):
                 except ValueError:
                     eng.close()
                     raise
+        if Md is not None:
+            try:
+                eng.set_mask(Md)
+            except Exception:
+                eng.close()
+                raise
         return eng, W, H, Wd, Hd, staged
+
+    @staticmethod
+    def _check_mask(V, mask, precision):
+        """fit()'s checks of a mask that need no device pass."""
+        if not isinstance(mask, Tensor) or mask.dtype != torch.bool:
+            raise ValueError(f"mask must be a torch.bool tensor (got {getattr(mask, 'dtype', type(mask))})")
+        if V.is_sparse:
+            raise ValueError("mask: a masked fit needs a dense target")
+        if tuple(mask.shape) != tuple(V.shape):
+            raise ValueError(f"mask shape {tuple(mask.shape)} does not match the target's {tuple(V.shape)}")
+        if precision in ("f16", "f16_split"):
+            raise ValueError(f"mask: masked fits run on the fp32 kernels; precision must be 'auto' or 'f32' (got {precision!r})")
 
     @torch.no_grad()
     def fit(self, V, beta=1, tol=1e-4, max_iter=200, verbose=False, alpha=0, l1_ratio=0, *,
-            precision="auto", group=None):
+            precision="auto", group=None, **options):
         """Learn the model for `V` by minimising the beta-divergence with multiplicative updates.
 
         Positional arguments, defaults, return value (`n_iter`) and exceptions are those of
@@ -271,11 +292,30 @@ class BaseComponent(torch.nn.Module):
         the stored entries only and, for beta != 1, 2, the denominators and the loss's sum (WH + eps)^beta from dense
         contractions that never read V, so the device holds O(nnz + (N + C) R).  Above rank 256 or with `group`, the
         target is densified on the device.
+
+        mask:      (keyword-only, default None; taken through **options so the named parameters stay the reference's
+                   plus `precision` and `group`) a torch.bool tensor of V's shape, True where V is observed: the fit minimises beta_div(WH[mask],
+                   V[mask]) -- the missing cells are dropped, not zeroed -- with every update the reference's ratio
+                   (nmf.py:78-92) of the two backward passes of that loss, i.e. what `trainer.BetaMu` does with the closure
+                   `(V[mask], model()[mask])`.  At beta 1 the denominator is therefore mask-weighted, not the column sums.
+                   The missing cells of V are never read into arithmetic (NaN there is fine), and the non-negativity and
+                   beta <= 0 checks look at the observed cells only.  A row or column with no observed cell leaves its row of
+                   H or W unchanged when alpha = 0.  Dense targets only (any dtype or row stride V may have), on the fp32
+                   kernels: precision "auto" resolves to "f32", "f16" / "f16_split" raise ValueError.  With `group`, each
+                   rank passes the mask shard of its V shard.
         """
-        eng, W, H, Wd, Hd, staged = self._open_engine(V, beta, precision, group, sparse_kernels=True)
+        mask = options.pop("mask", None)
+        if options:
+            raise TypeError(f"fit() got an unexpected keyword argument {next(iter(options))!r}")
+        if mask is not None:
+            self._check_mask(V, mask, precision)
+            precision = "f32"
+        eng, W, H, Wd, Hd, staged = self._open_engine(V, beta, precision, group, sparse_kernels=True, mask=mask)
 
         try:
             vmin, vmax = eng.minmax()
+            if mask is not None and vmin > vmax:                                           # +inf / -inf: nothing seen
+                raise ValueError("mask: no cell of the target is observed")
             assert vmin >= 0., "Target should be non-negative."                            # nmf.py:329-330
             if vmin == 0 and beta <= 0:                                                    # nmf.py:332-336
                 raise ValueError("When beta <= 0 and V contains zeros, the training process may diverge. "
