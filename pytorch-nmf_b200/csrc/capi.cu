@@ -36,7 +36,7 @@ struct nmfb200_ctx {
   float* num = nullptr;
   float* den = nullptr;
   int64_t part_floats = 0;
-  int nch_w = 1, nch_h = 1;
+  int nslab[2] = {1, 1};          // partial slabs of the W / H terms: contraction chunks (NMF), wgrad / dgrad splits (NMFD)
   float* colsum = nullptr;        // [2][R]: 0 = colsum(W), 1 = colsum(H)
   float* cs_scratch = nullptr;
   int64_t cs_scratch_floats = 0;
@@ -55,8 +55,6 @@ struct nmfb200_ctx {
   // NMFD
   float* Pn = nullptr;
   float* Pp = nullptr;
-  int wgrad_nsplit = 1;
-  int dgrad_nsplit = 1;
   // tensor-core path state (tc_nmf.cu / tc_nmfd.cu)
   TcState* tc = nullptr;
   TcNmfdState* tcd = nullptr;
@@ -147,36 +145,40 @@ int alloc_workspace(nmfb200_ctx* c, int64_t pn_floats) {
   return 0;
 }
 
-// CUDA-core contraction of one NMF factor update (which = 0: W, 1: H) into c->num / c->den (chunked partials).
-int simt_contract(nmfb200_ctx* c, int which, const float* W, const float* H, double beta, cudaStream_t st) {
-  if (beta != 1.0 || c->mask) { int e = ensure_den(c); if (e) return e; }
-  // W update: F = W (C rows), G = H (N rows), Vm = V^T;  H update: F = H (N rows), G = W (C rows), Vm = V
-  const float* F = which == 0 ? W : H;
-  const float* G = which == 0 ? H : W;
-  const int64_t rows = which == 0 ? c->C : c->N, cols = which == 0 ? c->N : c->C;
-  return simt_nmf_contract(c->V, c->vdtype, c->ldv, /*trans=*/which == 0 ? 1 : 0, F, G, rows, cols, (int)c->R, beta,
-                           which == 0 ? c->nch_w : c->nch_h, c->num, c->den, c->R, rows * c->R, c->mask, c->C, st);
-}
-
 // beta 1 without a mask: the denominator is the column sum of the other factor (nmf.py:122-131).  A masked fit takes it
 // from the second backward pass, M G, like every other beta.
 bool kl_colsum(const nmfb200_ctx* c, double beta) { return beta == 1.0 && !c->mask; }
 
-// The ratio stage's view of one NMF factor (which = 0: W, 1: H) of R components: numerators summed over `nchunks` partial
-// slabs, and `den` = the column sums of the other factor (beta 1) or the raw denominators in the numerators' layout.
-ApplyArgs nmf_apply_args(const nmfb200_ctx* c, int which, float* param, double beta, const float* num, const float* den,
-                         int nchunks, int64_t chunk_stride, double gamma, double l1, double l2) {
-  ApplyArgs a{};
-  a.param = param; a.numel = (which == 0 ? c->C : c->N) * c->R; a.R = (int)c->R; a.inner = 1; a.rowlen = c->R;
-  const bool kl = kl_colsum(c, beta);
-  a.num = num; a.den = kl ? nullptr : den; a.nchunks = nchunks; a.chunk_stride = chunk_stride;
-  a.ldp = c->R; a.kl_den = kl ? den : nullptr; a.out_scale = nullptr;
-  a.gamma = (float)gamma; a.l1 = (float)l1; a.l2 = (float)l2; a.absmax_bits = nullptr;
-  return a;
+// Whether the context's own tensor-core kernels (c->tc: NMF, c->tcd: NMFD / NMF2D / NMF3D) serve this beta.
+bool use_tc(const nmfb200_ctx* c, double beta) {
+  if (c->tc_off || c->mask) return false;
+  if (c->tc) return tc_supports_beta(c->tc, beta);
+  return c->tcd != nullptr && tc_nmfd_supported(c->d, beta);
 }
 
-bool use_tc(const nmfb200_ctx* c, double beta) {
-  return c->tc != nullptr && !c->tc_off && !c->mask && tc_supports_beta(c->tc, beta);
+// A pass outside the tensor-core state changed W (w) and / or H (h), or read them: NMF rebuilds the operand copies of the
+// changed factors on their next use, NMFD everything it derived from either.
+void mark_stale(nmfb200_ctx* c, bool w, bool h) {
+  if (c->tc) tc_mark_dirty(c->tc, w, h);
+  if (c->tcd) tc_nmfd_mark_dirty(c->tcd);
+}
+
+// One factor (which = 0: W, 1: H) and the other one: `rows` rows of R components x `inner` elements.  NMF: W is C x R and
+// H is N x R; NMFD / NMF2D / NMF3D: W is C x R x w_inner and H is B x R x h_inner.
+struct FactorDims { int64_t rows, inner, other_rows, other_inner; };
+FactorDims factor_dims(const nmfb200_ctx* c, int which) {
+  const NmfdShape& d = c->d;
+  const FactorDims w = c->kind == 0 ? FactorDims{c->C, 1, c->N, 1} : FactorDims{d.C, d.w_inner(), d.B, d.h_inner()};
+  return which == 0 ? w : FactorDims{w.other_rows, w.other_inner, w.rows, w.inner};
+}
+
+// The ratio stage's view of one factor's terms: its rows x R x inner elements, summed over `nchunks` slabs of that layout.
+ApplyArgs factor_view(const nmfb200_ctx* c, int which, int nchunks) {
+  const FactorDims f = factor_dims(c, which);
+  ApplyArgs a{};
+  a.R = (int)c->R; a.inner = f.inner; a.rowlen = c->R * f.inner; a.ldp = a.rowlen;
+  a.numel = f.rows * a.rowlen; a.chunk_stride = a.numel; a.nchunks = nchunks;
+  return a;
 }
 
 // What every dense set_target checks of the target's element type and pointer (the kernels load single elements: element
@@ -267,10 +269,10 @@ int nmfb200_nmf_create(nmfb200_ctx** out, int device, int64_t N, int64_t C, int6
   }
   c->precision = resolved;
   c->auto_mode = precision == NMFB200_PREC_AUTO;
-  c->nch_w = chunks_for(C, N, R);
-  c->nch_h = chunks_for(N, C, R);
-  int64_t pf = (int64_t)c->nch_w * C * R;
-  if ((int64_t)c->nch_h * N * R > pf) pf = (int64_t)c->nch_h * N * R;
+  c->nslab[0] = chunks_for(C, N, R);
+  c->nslab[1] = chunks_for(N, C, R);
+  int64_t pf = (int64_t)c->nslab[0] * C * R;
+  if ((int64_t)c->nslab[1] * N * R > pf) pf = (int64_t)c->nslab[1] * N * R;
   c->part_floats = pf;
   c->cs_scratch_floats = colsum_scratch_floats(N > C ? N : C, (int)R, 1);
   c->loss_max_blocks = simt_nmf_max_blocks(N, C);
@@ -292,11 +294,9 @@ int nmfb200_precision(const nmfb200_ctx* ctx) {
 
 int nmfb200_precision_for_beta(const nmfb200_ctx* ctx, double beta) {
   if (!ctx) return -100;
-  if (ctx->mask) return NMFB200_PREC_F32;
-  if (ctx->kind == 1) return (ctx->tcd && !ctx->tc_off && tc_nmfd_supported(ctx->d, beta)) ? NMFB200_PREC_F16 : NMFB200_PREC_F32;
-  if (ctx->kind != 0 || !use_tc(ctx, beta)) return NMFB200_PREC_F32;
-  // beta != 1 kernels read only the hi halves of the operand copies
-  return (beta == 1.0 || beta == 2.0) ? ctx->precision : NMFB200_PREC_F16;
+  if (!use_tc(ctx, beta)) return NMFB200_PREC_F32;
+  // NMF's beta != 1, 2 kernels read only the hi halves of the operand copies
+  return (ctx->tc && (beta == 1.0 || beta == 2.0)) ? ctx->precision : NMFB200_PREC_F16;
 }
 
 int nmfb200_nmf_plan(int64_t N, int64_t C, int64_t R, int64_t* out, int n) {
@@ -401,10 +401,154 @@ int nmfb200_nmf_set_target_sparse_any_beta(nmfb200_ctx* ctx, int64_t nnz, const 
   return 0;
 }
 
+/* ---- NMFD ------------------------------------------------------------------------------------ */
+
+// One context type serves NMFD (one sliding axis) and NMF2D / NMF3D (the last axis slides, the outer ones are loops):
+// vdims / kdims hold the target's and the kernel's sizes over the ndim convolved axes.
+// The context's shape from the create arguments (validated): the outer axes right-aligned, X2 / T2 innermost of them.
+static int nmfd_shape_of(int64_t B, int64_t C, int ndim, const int64_t* vdims, int64_t R, const int64_t* kdims, NmfdShape* d) {
+  if (ndim < 1 || ndim > 3 || !vdims || !kdims) return fail(NMFB200_ERR_INVALID, "1 to 3 convolved axes are supported");
+  int64_t X[3] = {1, 1, 1}, K[3] = {1, 1, 1};            // right-aligned: X[2] / K[2] is the last (sliding) axis
+  for (int i = 0; i < ndim; ++i) { X[3 - ndim + i] = vdims[i]; K[3 - ndim + i] = kdims[i]; }
+  const int64_t L = X[2], T = K[2];
+  if (B < 1 || C < 1 || R < 1) return fail(NMFB200_ERR_INVALID, "bad NMFD sizes");
+  for (int i = 0; i < 3; ++i)
+    if (K[i] < 1 || X[i] < K[i]) return fail(NMFB200_ERR_INVALID, "bad NMFD sizes");
+  if (R > 256) return fail(NMFB200_ERR_INVALID, "rank > 256 is not supported");
+  if (B * C * X[0] * X[1] * L > (int64_t)1 << 40 || X[0] * X[1] * L > (int64_t)1 << 30 || K[0] * K[1] * T > (int64_t)1 << 24)
+    return fail(NMFB200_ERR_INVALID, "NMFD target too large");
+  // every size below is narrowed to int, and the kernels count in int: bound what they derive from it
+  if (C > kMaxGridYZ * 64)
+    return fail(NMFB200_ERR_INVALID, "NMFD supports at most 65535 x 64 = 4194240 channels (grid.y of the reconstruction)");
+  if (B * (X[0] - K[0] + 1) * (X[1] - K[1] + 1) > INT32_MAX)
+    return fail(NMFB200_ERR_INVALID, "NMFD batch x outer activation lines must be below 2^31 (the W gradient's line index)");
+  if ((C > R ? C : R) * K[0] * K[1] > INT32_MAX)
+    return fail(NMFB200_ERR_INVALID, "NMFD channels (or rank) x outer kernel offsets must be below 2^31 (the contraction index)");
+  *d = NmfdShape{(int)B, (int)C, (int)L, (int)R, (int)T, (int)(L - T + 1)};
+  d->X1 = (int)X[0]; d->X2 = (int)X[1]; d->T1 = (int)K[0]; d->T2 = (int)K[1];
+  NmfdPlan p;
+  nmfd_plan(*d, &p);
+  if (!grid_fits(p.recon_grid) || !grid_fits(p.dgrad_grid) || !grid_fits(p.wgrad_grid))
+    return fail(NMFB200_ERR_INVALID, "an NMFD grid of the fp32 kernels passes the CUDA grid limits");
+  if (nmfd_max_blocks(*d) > INT32_MAX) return fail(NMFB200_ERR_INVALID, "NMFD loss partials must number below 2^31");
+  return 0;
+}
+
+int nmfb200_nmfnd_create(nmfb200_ctx** out, int device, int64_t B, int64_t C, int ndim, const int64_t* vdims,
+                         int64_t R, const int64_t* kdims, int precision) {
+  if (!out) return fail(NMFB200_ERR_INVALID, "out is null");
+  *out = nullptr;
+  NmfdShape shape;
+  if (int rc = nmfd_shape_of(B, C, ndim, vdims, R, kdims, &shape)) return rc;
+  if (precision != NMFB200_PREC_AUTO && precision != NMFB200_PREC_F32 && precision != NMFB200_PREC_F16)
+    return fail(NMFB200_ERR_INVALID, "NMFD precision must be auto, f32 or f16");
+  // NMF2D / NMF3D take the tensor-core kernels only when asked for (f16); auto keeps them on the fp32 kernels
+  const bool one_d = shape.one_d();
+  TcNmfdPlan tc_plan;
+  const char* tc_limit = (one_d || precision == NMFB200_PREC_F16) ? tc_nmfd_plan(shape, &tc_plan) : "";
+  if (precision == NMFB200_PREC_F16 && tc_limit) return fail(NMFB200_ERR_INVALID, tc_limit);
+  DeviceGuard guard(device);
+  if (!guard.ok) return fail(NMFB200_ERR_CUDA, "cannot select the requested device");
+  nmfb200_ctx* c = new (std::nothrow) nmfb200_ctx();
+  if (!c) return fail(NMFB200_ERR_INVALID, "out of host memory");
+  c->kind = 1; c->device = device; c->precision = precision == NMFB200_PREC_F32 ? NMFB200_PREC_F32 : NMFB200_PREC_F16; c->R = R;
+  c->auto_mode = precision == NMFB200_PREC_AUTO;
+  c->d = shape;
+  c->nslab[0] = nmfd_wgrad_nsplit(c->d);
+  c->nslab[1] = nmfd_dgrad_nsplit(c->d);
+  int64_t pf = (int64_t)c->nslab[0] * C * R * c->d.w_inner();
+  int64_t hf = (int64_t)c->nslab[1] * B * R * c->d.h_inner();
+  if (hf > pf) pf = hf;
+  c->part_floats = pf;
+  int64_t cs1 = colsum_scratch_floats(C, (int)R, c->d.w_inner()), cs2 = colsum_scratch_floats(B, (int)R, c->d.h_inner());
+  c->cs_scratch_floats = cs1 > cs2 ? cs1 : cs2;
+  c->loss_max_blocks = (int)nmfd_max_blocks(c->d);         // bounded by nmfd_shape_of
+  if (int rc = alloc_workspace(c, B * C * c->d.v_inner())) return rc;
+  if (c->precision != NMFB200_PREC_F32 && !tc_limit) {    // NMFD at auto / f16, NMF2D / NMF3D at f16
+    cudaDeviceProp prop;
+    if (cudaGetDeviceProperties(&prop, device) == cudaSuccess && prop.major == 9) {
+      int rc = tc_nmfd_create(&c->tcd, c->d);          // beta = 1 runs as wgmma sliding GEMMs (tc_nmfd.cu)
+      if (rc) { free_ctx(c); return rc; }
+    } else if (precision == NMFB200_PREC_F16) {
+      free_ctx(c);
+      return fail(NMFB200_ERR_INVALID, "the tensor-core NMFD path needs an sm_90 device");
+    }
+  }
+  *out = c;
+  return 0;
+}
+
+int nmfb200_nmfd_set_target(nmfb200_ctx* ctx, const void* V, int dtype, void* stream) {
+  CTX_GUARD(ctx, 1);
+  if (int rc = check_target(V, dtype)) return rc;
+  ctx->V = V; ctx->vdtype = dtype; ctx->has_target = true; ctx->mask = nullptr;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int64_t vin = ctx->d.v_inner();
+  int rc = matrix_minmax(V, dtype, (int64_t)ctx->d.B * ctx->d.C, vin, vin, ctx->mm_scratch, ctx->mm_scratch + kMmPartials, st);
+  if (rc) return rc;
+  ctx->tc_off = false;
+  if (ctx->tcd) {
+    double vsum = 0.0;
+    rc = tc_nmfd_set_target(ctx->tcd, V, dtype, &vsum, st);       // synchronises: sum(V) for kappa
+    if (rc) return rc;
+    tc_nmfd_mark_dirty(ctx->tcd);                         // a new fit: the factors may be anything
+    if (ctx->auto_mode)                                   // same conservative rule as the NMF path: heavy-tailed targets stay fp32
+      return auto_off_if_heavy_tailed(ctx, vsum, (double)ctx->d.B * ctx->d.C * ctx->d.v_inner(), st);
+  }
+  return 0;
+}
+
+int nmfb200_nmfd_plan(int64_t B, int64_t C, int ndim, const int64_t* vdims, int64_t R, const int64_t* kdims, int64_t* out,
+                      int n) {
+  if (!out || n < NMFB200_NMFD_PLAN_LEN) return fail(NMFB200_ERR_INVALID, "plan buffer too small");
+  NmfdShape d;
+  if (int rc = nmfd_shape_of(B, C, ndim, vdims, R, kdims, &d)) return rc;
+  NmfdPlan p;
+  nmfd_plan(d, &p);
+  const WgradPlan& w = p.wgrad;
+  nmfb200_ctx c;                      // the shape alone, for the ratio stage's views of W and H
+  c.kind = 1; c.R = R; c.d = d;
+  const int64_t v[NMFB200_NMFD_PLAN_LEN] = {
+      p.recon_mt, p.recon_grid.x, p.recon_grid.y, p.recon_grid.z,
+      p.dgrad_mt, p.dgrad_nsplit, p.dgrad_grid.x, p.dgrad_grid.y, p.dgrad_grid.z,
+      w.mt, w.tp, w.nr, w.no, w.ntt, w.nrg, w.nog, p.wgrad_nsplit,
+      apply_update_vec4_shape(factor_view(&c, 0, p.wgrad_nsplit)), apply_update_vec4_shape(factor_view(&c, 1, p.dgrad_nsplit))};
+  for (int i = 0; i < NMFB200_NMFD_PLAN_LEN; ++i) out[i] = v[i];
+  return 0;
+}
+
+int nmfb200_nmfnd_tc_plan(int64_t B, int64_t C, int ndim, const int64_t* vdims, int64_t R, const int64_t* kdims,
+                          int64_t* out, int n) {
+  if (!out || n < NMFB200_NMFND_TC_PLAN_LEN) return fail(NMFB200_ERR_INVALID, "plan buffer too small");
+  NmfdShape d;
+  if (int rc = nmfd_shape_of(B, C, ndim, vdims, R, kdims, &d)) return rc;
+  TcNmfdPlan p;
+  if (const char* why = tc_nmfd_plan(d, &p)) return fail(NMFB200_ERR_INVALID, why);
+  const int64_t v[NMFB200_NMFND_TC_PLAN_LEN] = {
+      p.prep_w.x, p.prep_w.y, p.prep_w.z, p.prep_h.x, p.prep_h.y, p.prep_h.z, p.recon.x, p.recon.y, p.recon.z,
+      p.wgrad.x, p.wgrad.y, p.wgrad.z, p.dgrad.x, p.dgrad.y, p.dgrad.z, p.bslice, p.slices, p.dgrad_rblocks,
+      p.loss_blocks, p.ws_w, p.kbs_w, p.ws_h, p.kbs_h, p.hslice, p.hslices, p.Tp, p.padl, p.Lp, p.Lq, p.Cpad, p.nch};
+  for (int i = 0; i < NMFB200_NMFND_TC_PLAN_LEN; ++i) out[i] = v[i];
+  return 0;
+}
+
+/* ---- both kinds: the mask, and the terms of one factor update that every CUDA-core path runs on ------------ */
+
+int nmfb200_set_mask(nmfb200_ctx* ctx, const uint8_t* M, void* stream) {
+  CTX_GUARD(ctx, kAnyKind);
+  TARGET_GUARD(ctx);
+  if (ctx->sparse) return fail(NMFB200_ERR_INVALID, "a mask needs a dense target (set_target or nmfd_set_target)");
+  cudaStream_t st = (cudaStream_t)stream;
+  ctx->mask = M;
+  // the tensor-core paths are bypassed while a mask is set: their operand copies are rebuilt on their next use
+  mark_stale(ctx, true, true);
+  float* minmax = ctx->mm_scratch + kMmPartials;          // target_minmax: the observed cells only, or all of V again
+  if (ctx->kind == 0) return matrix_minmax(ctx->V, ctx->vdtype, ctx->N, ctx->C, ctx->ldv, ctx->mm_scratch, minmax, st, M);
+  const int64_t vin = ctx->d.v_inner();
+  return matrix_minmax(ctx->V, ctx->vdtype, (int64_t)ctx->d.B * ctx->d.C, vin, vin, ctx->mm_scratch, minmax, st, M);
+}
+
 namespace {
-// Raw terms of one factor's update on the compressed form whose segments are that factor's rows (which = 0: W over CSC,
-// 1: H over CSR): the numerator (rows x R) into `num`; into `den` the colsum of the other factor (R, beta 1) or the raw
-// denominator F (other^T other) (rows x R, beta 2).  Shared by the update and nmfb200_raw_terms.
 // beta 1 and 2 run on every sparse context; any other beta > 0 only on one set by nmfb200_nmf_set_target_sparse_any_beta
 int check_sparse_beta(const nmfb200_ctx* ctx, double beta) {
   if (beta == 1.0 || beta == 2.0) return 0;
@@ -414,84 +558,119 @@ int check_sparse_beta(const nmfb200_ctx* ctx, double beta) {
   return 0;
 }
 
+// The terms of one factor's update on the compressed form whose segments are that factor's rows (which = 0: W over CSC,
+// 1: H over CSR), all in final form: the numerator (rows x R) into `num`; into `den` the colsum of the other factor (R, beta
+// 1), the raw denominator F (other^T other) (rows x R, beta 2) or, at any other beta, the V-free denominator's chunk sum.
 int sparse_terms(nmfb200_ctx* ctx, int which, const float* F, const float* other, double beta, float* num, float* den,
                  cudaStream_t st) {
   if (int rc = check_sparse_beta(ctx, beta)) return rc;
   const int R = (int)ctx->R;
-  const int64_t rows = which == 0 ? ctx->C : ctx->N, orows = which == 0 ? ctx->N : ctx->C;
+  const FactorDims f = factor_dims(ctx, which);
   const int64_t* ptr = which == 0 ? ctx->sp_ccol : ctx->sp_crow;
   const int64_t* idx = which == 0 ? ctx->sp_row : ctx->sp_col;
   const float* val = which == 0 ? ctx->sp_val_t : ctx->sp_val;
-  int rc = sparse_numerator(ptr, idx, val, F, other, R, rows, beta, num, st);
+  int rc = sparse_numerator(ptr, idx, val, F, other, R, f.rows, beta, num, st);
   if (rc) return rc;
   if (beta != 1.0 && beta != 2.0) {     // the V-free denominator on the dense fp32 plan, its chunks summed as the dense path does
-    const int nch = which == 0 ? ctx->nch_w : ctx->nch_h;
-    rc = simt_nmf_contract_den(F, other, rows, orows, R, beta, nch, ctx->den, ctx->R, rows * ctx->R, st);
+    ApplyArgs chunks = factor_view(ctx, which, ctx->nslab[which]);
+    chunks.num = ctx->den;
+    rc = simt_nmf_contract_den(F, other, f.rows, f.other_rows, R, beta, chunks.nchunks, ctx->den, ctx->R, chunks.numel, st);
     if (rc) return rc;
-    return reduce_chunks(ctx->den, nch, rows * ctx->R, rows, R, ctx->R, den, st);
+    return raw_sum(chunks, den, nullptr, st);
   }
   if (beta == 1.0)                                             // colsum of the OTHER factor, nmf.py:122-131
-    return factor_colsum(other, orows, R, 1, ctx->cs_scratch, ctx->cs_scratch_floats, den, st);
+    return factor_colsum(other, f.other_rows, R, 1, ctx->cs_scratch, ctx->cs_scratch_floats, den, st);
   float* G = ctx->sp_gram + (1 - which) * R * R;               // Gram matrix of the other factor
-  rc = sparse_gram(other, orows, R, ctx->sp_gram + 2 * R * R, G, st);
+  rc = sparse_gram(other, f.other_rows, R, ctx->sp_gram + 2 * R * R, G, st);
   if (rc) return rc;
-  return sparse_rows_times_gram(F, G, rows, R, den, st);       // nmf.py:609
+  return sparse_rows_times_gram(F, G, f.rows, R, den, st);     // nmf.py:609
 }
 
-// one factor update: sparse_terms into the context's scratch, then the ratio stage
-int sparse_update(nmfb200_ctx* ctx, int which, float* F, const float* other, double beta, double gamma, double l1_reg,
-                  double l2_reg, cudaStream_t st) {
-  if (beta == 2.0) {
-    int rc = ensure_den(ctx);
-    if (rc) return rc;
-  }
-  // beta 1: colsum; beta 2: the raw denominator; other beta: the chunk partials live in ctx->den, their sum goes to sp_den
-  float* den = beta == 1.0 ? ctx->colsum + (1 - which) * ctx->R : beta == 2.0 ? ctx->den : ctx->sp_den;
-  int rc = sparse_terms(ctx, which, F, other, beta, ctx->num, den, st);
-  if (rc) return rc;
-  return apply_update(nmf_apply_args(ctx, which, F, beta, ctx->num, den, 1, 0, gamma, l1_reg, l2_reg), st);
+// CUDA-core contraction of one NMF factor update (which = 0: W, 1: H) into c->num / c->den (chunked partials).
+int simt_contract(nmfb200_ctx* c, int which, const float* W, const float* H, double beta, cudaStream_t st) {
+  if (beta != 1.0 || c->mask) { int e = ensure_den(c); if (e) return e; }
+  // W update: F = W (C rows), G = H (N rows), Vm = V^T;  H update: F = H (N rows), G = W (C rows), Vm = V
+  const float* fac[2] = {W, H};
+  const FactorDims f = factor_dims(c, which);
+  return simt_nmf_contract(c->V, c->vdtype, c->ldv, /*trans=*/which == 0, fac[which], fac[1 - which], f.rows, f.other_rows,
+                           (int)c->R, beta, c->nslab[which], c->num, c->den, c->R, f.rows * c->R, c->mask, c->C, st);
 }
 
-// One factor update (which = 0: param = W, 1: param = H) on the kernels that serve this context and beta: sparse-target,
-// tensor-core or fp32.  No device guard: the entry points select the context's device.
-int nmf_update(nmfb200_ctx* ctx, int which, float* param, const float* W, const float* H, double beta, double gamma,
-               double l1_reg, double l2_reg, cudaStream_t st) {
-  const float* other = which == 0 ? H : W;
-  if (ctx->sparse) return sparse_update(ctx, which, param, other, beta, gamma, l1_reg, l2_reg, st);
-  if (use_tc(ctx, beta)) return tc_update(ctx->tc, which, param, W, H, beta, gamma, l1_reg, l2_reg, st);
-  int rc = simt_contract(ctx, which, W, H, beta, st);
-  if (rc) return rc;
-  float* den = ctx->den;
-  if (kl_colsum(ctx, beta)) {      // nmf.py:122-131: the KL denominator is the column sum of the OTHER factor
-    den = ctx->colsum + (1 - which) * ctx->R;
-    rc = factor_colsum(other, which == 0 ? ctx->N : ctx->C, (int)ctx->R, 1, ctx->cs_scratch, ctx->cs_scratch_floats, den, st);
-    if (rc) return rc;
+// The same for NMFD / NMF2D / NMF3D: the ratio tiles Pn (and Pp), then their backward passes (wgrad for W, dgrad for H) into
+// c->num and, unless the column sums serve, c->den (split partials).
+int nmfd_contract(nmfb200_ctx* c, int which, const float* W, const float* H, double beta, cudaStream_t st) {
+  const bool den = !kl_colsum(c, beta);
+  if (den) {
+    if (!c->Pp) NMF_CUDA_CHECK(cudaMalloc(&c->Pp, (size_t)c->d.B * c->d.C * c->d.v_inner() * sizeof(float)));
+    int e = ensure_den(c);
+    if (e) return e;
   }
-  const int64_t rows = which == 0 ? ctx->C : ctx->N;
-  rc = apply_update(nmf_apply_args(ctx, which, param, beta, ctx->num, den, which == 0 ? ctx->nch_w : ctx->nch_h,
-                                   rows * ctx->R, gamma, l1_reg, l2_reg), st);
+  int rc = nmfd_recon_phi(c->d, c->V, c->vdtype, W, H, beta, c->Pn, c->Pp, nullptr, 0, nullptr, st, c->mask);
+  auto grad = [&](const float* P, float* out) {
+    return which == 0 ? nmfd_wgrad(c->d, P, H, out, c->nslab[0], st) : nmfd_dgrad(c->d, P, W, out, c->nslab[1], st);
+  };
+  if (rc == 0) rc = grad(c->Pn, c->num);
+  if (rc == 0 && den) rc = grad(c->Pp, c->den);
+  return rc;
+}
+
+// Both backward passes of one factor (which = 0: W, 1: H) from the current factors, described as the ratio stage's input
+// (nmf.py:367-391): partial slabs of numerators and, but for unmasked beta 1, denominators; at unmasked beta 1 the column
+// sums of the other factor (nmf.py:122-131) as kl_den; on the NMFD tensor cores the centring term kappa / kappa_vec, with
+// `*tc` set.  Terms the kernels leave in final form -- the sparse numerator and denominator, the column sums -- go straight
+// to `out` ([numerator | denominator], nmfb200_raw_terms' layout) or, when it is null, to the context's scratch.  Serves
+// every path but the NMF tensor-core leaf (tc_update, tc_raw_terms).
+int factor_terms(nmfb200_ctx* c, int which, const float* W, const float* H, double beta, float* out, ApplyArgs& a,
+                 bool* tc, cudaStream_t st) {
+  a = factor_view(c, which, 1);
+  const float* fac[2] = {W, H};
+  const bool kl = kl_colsum(c, beta);
+  // where the final-form terms go without `out`: c->colsum is [colsum(W) | colsum(H)], the sparse raw denominator lives in
+  // c->den at beta 2 and in c->sp_den at other beta (whose c->den holds the chunks)
+  if (c->sparse && beta == 2.0 && !out) { int e = ensure_den(c); if (e) return e; }
+  float* num_out = out ? out : c->num;
+  float* den_out = out ? out + a.numel : kl ? c->colsum + (1 - which) * c->R : beta == 2.0 ? c->den : c->sp_den;
+  *tc = c->tcd && use_tc(c, beta);
+  if (*tc) {                  // NMFD beta 1: the recon pass also brings both column sums and kappa up to date
+    int rc = tc_nmfd_recon(c->tcd, c->V, c->vdtype, W, H, false, nullptr, st);
+    if (rc) return rc;
+    const float* part; int nsplit;
+    rc = which == 0 ? tc_nmfd_wgrad(c->tcd, &part, &nsplit, st) : tc_nmfd_dgrad(c->tcd, &part, &nsplit, st);
+    if (rc) return rc;
+    const float* cs = tc_nmfd_colsum(c->tcd) + (1 - which) * c->R;
+    a.num = part; a.nchunks = nsplit; a.kl_den = cs; a.kappa = tc_nmfd_kappa(c->tcd); a.kappa_vec = cs;
+    return 0;
+  }
+  if (c->sparse) {
+    a.num = num_out;
+    if (kl) a.kl_den = den_out;
+    else a.den = den_out;
+    return sparse_terms(c, which, fac[which], fac[1 - which], beta, num_out, den_out, st);
+  }
+  int rc = c->kind == 0 ? simt_contract(c, which, W, H, beta, st) : nmfd_contract(c, which, W, H, beta, st);
   if (rc) return rc;
-  if (ctx->tc) tc_mark_dirty(ctx->tc, which == 0, which == 1);
+  a.num = c->num; a.nchunks = c->nslab[which];
+  if (!kl) { a.den = c->den; return 0; }
+  a.kl_den = den_out;
+  const FactorDims f = factor_dims(c, which);
+  return factor_colsum(fac[1 - which], f.other_rows, (int)c->R, f.other_inner, c->cs_scratch, c->cs_scratch_floats, den_out,
+                       st);
+}
+
+// One factor update (which = 0: param = W, 1: param = H) on the kernels that serve this context and beta.  No device guard:
+// the entry points select the context's device.
+int update_factor(nmfb200_ctx* ctx, int which, float* param, const float* W, const float* H, double beta, double gamma,
+                  double l1_reg, double l2_reg, cudaStream_t st) {
+  if (ctx->tc && use_tc(ctx, beta)) return tc_update(ctx->tc, which, param, W, H, beta, gamma, l1_reg, l2_reg, st);
+  ApplyArgs a; bool tc;
+  int rc = factor_terms(ctx, which, W, H, beta, nullptr, a, &tc, st);
+  if (rc) return rc;
+  a.param = param; a.gamma = (float)gamma; a.l1 = (float)l1_reg; a.l2 = (float)l2_reg;
+  if (tc) a.absmax_bits = tc_nmfd_begin_update(ctx->tcd, which, st);
+  rc = apply_update(a, st);
+  if (rc) return rc;
+  if (!tc) mark_stale(ctx, which == 0, which == 1);
   return 0;
-}
-
-// The raw terms of one factor's update (which = 0: W, 1: H) into `out`, nmfb200_raw_terms_numel floats.
-int nmf_raw_terms(nmfb200_ctx* ctx, const float* W, const float* H, int which, double beta, float* out, cudaStream_t st) {
-  const int64_t rows = which == 0 ? ctx->C : ctx->N;
-  const int64_t RR = rows * ctx->R;
-  if (ctx->sparse) return sparse_terms(ctx, which, which == 0 ? W : H, which == 0 ? H : W, beta, out, out + RR, st);
-  if (use_tc(ctx, beta) && tc_supports_partial(ctx->tc, beta)) return tc_raw_terms(ctx->tc, which, W, H, beta, out, st);
-  int rc = simt_contract(ctx, which, W, H, beta, st);
-  if (rc) return rc;
-  const int nch = which == 0 ? ctx->nch_w : ctx->nch_h;
-  rc = reduce_chunks(ctx->num, nch, RR, rows, (int)ctx->R, ctx->R, out, st);
-  if (rc) return rc;
-  if (kl_colsum(ctx, beta)) {      // nmf.py:122-131: the KL denominator is the column sum of the OTHER factor
-    const float* other = which == 0 ? H : W;
-    return factor_colsum(other, which == 0 ? ctx->N : ctx->C, (int)ctx->R, 1, ctx->cs_scratch, ctx->cs_scratch_floats,
-                         out + RR, st);
-  }
-  return reduce_chunks(ctx->den, nch, RR, rows, (int)ctx->R, ctx->R, out + RR, st);
 }
 
 int sparse_loss_ctx(nmfb200_ctx* ctx, const float* W, const float* H, double beta, double* loss_dev, cudaStream_t st) {
@@ -541,9 +720,9 @@ int nmfb200_nmf_iterate(nmfb200_ctx* ctx, float* W, float* H, double beta, doubl
   if (!W || !H || n_iter < 0) return fail(NMFB200_ERR_INVALID, "bad argument");
   cudaStream_t st = (cudaStream_t)stream;
   for (int i = 0; i < n_iter; ++i) {
-    int rc = nmf_update(ctx, 0, W, W, H, beta, gamma, l1_reg, l2_reg, st);
+    int rc = update_factor(ctx, 0, W, W, H, beta, gamma, l1_reg, l2_reg, st);
     if (rc) return rc;
-    rc = nmf_update(ctx, 1, H, W, H, beta, gamma, l1_reg, l2_reg, st);
+    rc = update_factor(ctx, 1, H, W, H, beta, gamma, l1_reg, l2_reg, st);
     if (rc) return rc;
   }
   return 0;
@@ -562,8 +741,8 @@ int nmfb200_nmf_loss_prefetch_w(nmfb200_ctx* ctx, const float* W, const float* H
 /* ---- row-sharded W update over peer memory (NVLink, one process per GPU) ---------------------- */
 
 int nmfb200_nmf_peer_supported(const nmfb200_ctx* ctx, double beta) {
-  if (!ctx || ctx->kind != 0 || !ctx->tc || ctx->tc_off || !ctx->has_target || ctx->mask) return 0;
-  return (tc_supports_beta(ctx->tc, beta) && tc_peer_supported(ctx->tc, beta)) ? 1 : 0;
+  if (!ctx || ctx->kind != 0 || !ctx->has_target || !use_tc(ctx, beta)) return 0;
+  return tc_peer_supported(ctx->tc, beta) ? 1 : 0;
 }
 
 int nmfb200_nmf_peer_alloc(nmfb200_ctx* ctx, void* ipc_handle_out) {
@@ -610,251 +789,32 @@ int nmfb200_nmf_contract_only(nmfb200_ctx* ctx, const float* W, const float* H, 
   return simt_contract(ctx, which, W, H, beta, st);
 }
 
-/* ---- NMFD ------------------------------------------------------------------------------------ */
-
-// One context type serves NMFD (one sliding axis) and NMF2D / NMF3D (the last axis slides, the outer ones are loops):
-// vdims / kdims hold the target's and the kernel's sizes over the ndim convolved axes.
-// The context's shape from the create arguments (validated): the outer axes right-aligned, X2 / T2 innermost of them.
-static int nmfd_shape_of(int64_t B, int64_t C, int ndim, const int64_t* vdims, int64_t R, const int64_t* kdims, NmfdShape* d) {
-  if (ndim < 1 || ndim > 3 || !vdims || !kdims) return fail(NMFB200_ERR_INVALID, "1 to 3 convolved axes are supported");
-  int64_t X[3] = {1, 1, 1}, K[3] = {1, 1, 1};            // right-aligned: X[2] / K[2] is the last (sliding) axis
-  for (int i = 0; i < ndim; ++i) { X[3 - ndim + i] = vdims[i]; K[3 - ndim + i] = kdims[i]; }
-  const int64_t L = X[2], T = K[2];
-  if (B < 1 || C < 1 || R < 1) return fail(NMFB200_ERR_INVALID, "bad NMFD sizes");
-  for (int i = 0; i < 3; ++i)
-    if (K[i] < 1 || X[i] < K[i]) return fail(NMFB200_ERR_INVALID, "bad NMFD sizes");
-  if (R > 256) return fail(NMFB200_ERR_INVALID, "rank > 256 is not supported");
-  if (B * C * X[0] * X[1] * L > (int64_t)1 << 40 || X[0] * X[1] * L > (int64_t)1 << 30 || K[0] * K[1] * T > (int64_t)1 << 24)
-    return fail(NMFB200_ERR_INVALID, "NMFD target too large");
-  // every size below is narrowed to int, and the kernels count in int: bound what they derive from it
-  if (C > kMaxGridYZ * 64)
-    return fail(NMFB200_ERR_INVALID, "NMFD supports at most 65535 x 64 = 4194240 channels (grid.y of the reconstruction)");
-  if (B * (X[0] - K[0] + 1) * (X[1] - K[1] + 1) > INT32_MAX)
-    return fail(NMFB200_ERR_INVALID, "NMFD batch x outer activation lines must be below 2^31 (the W gradient's line index)");
-  if ((C > R ? C : R) * K[0] * K[1] > INT32_MAX)
-    return fail(NMFB200_ERR_INVALID, "NMFD channels (or rank) x outer kernel offsets must be below 2^31 (the contraction index)");
-  *d = NmfdShape{(int)B, (int)C, (int)L, (int)R, (int)T, (int)(L - T + 1)};
-  d->X1 = (int)X[0]; d->X2 = (int)X[1]; d->T1 = (int)K[0]; d->T2 = (int)K[1];
-  NmfdPlan p;
-  nmfd_plan(*d, &p);
-  if (!grid_fits(p.recon_grid) || !grid_fits(p.dgrad_grid) || !grid_fits(p.wgrad_grid))
-    return fail(NMFB200_ERR_INVALID, "an NMFD grid of the fp32 kernels passes the CUDA grid limits");
-  if (nmfd_max_blocks(*d) > INT32_MAX) return fail(NMFB200_ERR_INVALID, "NMFD loss partials must number below 2^31");
-  return 0;
-}
-
-// The ratio stage's view of one NMFD factor (which = 0: W, 1: H): rows of R components x `inner` elements, one partial slab
-// per split.
-static ApplyArgs nmfd_apply_shape(const NmfdShape& d, int which, int nsplit) {
-  const int64_t inner = which == 0 ? d.w_inner() : d.h_inner();
-  ApplyArgs a{};
-  a.numel = (int64_t)(which == 0 ? d.C : d.B) * d.R * inner; a.R = d.R; a.inner = inner; a.rowlen = (int64_t)d.R * inner;
-  a.chunk_stride = a.numel; a.ldp = a.rowlen; a.nchunks = nsplit; a.out_scale = nullptr; a.absmax_bits = nullptr;
-  return a;
-}
-
-int nmfb200_nmfnd_create(nmfb200_ctx** out, int device, int64_t B, int64_t C, int ndim, const int64_t* vdims,
-                         int64_t R, const int64_t* kdims, int precision) {
-  if (!out) return fail(NMFB200_ERR_INVALID, "out is null");
-  *out = nullptr;
-  NmfdShape shape;
-  if (int rc = nmfd_shape_of(B, C, ndim, vdims, R, kdims, &shape)) return rc;
-  if (precision != NMFB200_PREC_AUTO && precision != NMFB200_PREC_F32 && precision != NMFB200_PREC_F16)
-    return fail(NMFB200_ERR_INVALID, "NMFD precision must be auto, f32 or f16");
-  // NMF2D / NMF3D take the tensor-core kernels only when asked for (f16); auto keeps them on the fp32 kernels
-  const bool one_d = shape.one_d();
-  TcNmfdPlan tc_plan;
-  const char* tc_limit = (one_d || precision == NMFB200_PREC_F16) ? tc_nmfd_plan(shape, &tc_plan) : "";
-  if (precision == NMFB200_PREC_F16 && tc_limit) return fail(NMFB200_ERR_INVALID, tc_limit);
-  DeviceGuard guard(device);
-  if (!guard.ok) return fail(NMFB200_ERR_CUDA, "cannot select the requested device");
-  nmfb200_ctx* c = new (std::nothrow) nmfb200_ctx();
-  if (!c) return fail(NMFB200_ERR_INVALID, "out of host memory");
-  c->kind = 1; c->device = device; c->precision = precision == NMFB200_PREC_F32 ? NMFB200_PREC_F32 : NMFB200_PREC_F16; c->R = R;
-  c->auto_mode = precision == NMFB200_PREC_AUTO;
-  c->d = shape;
-  c->dgrad_nsplit = nmfd_dgrad_nsplit(c->d);
-  c->wgrad_nsplit = nmfd_wgrad_nsplit(c->d);
-  int64_t pf = (int64_t)c->wgrad_nsplit * C * R * c->d.w_inner();
-  int64_t hf = (int64_t)c->dgrad_nsplit * B * R * c->d.h_inner();
-  if (hf > pf) pf = hf;
-  c->part_floats = pf;
-  int64_t cs1 = colsum_scratch_floats(C, (int)R, c->d.w_inner()), cs2 = colsum_scratch_floats(B, (int)R, c->d.h_inner());
-  c->cs_scratch_floats = cs1 > cs2 ? cs1 : cs2;
-  c->loss_max_blocks = (int)nmfd_max_blocks(c->d);         // bounded by nmfd_shape_of
-  if (int rc = alloc_workspace(c, B * C * c->d.v_inner())) return rc;
-  if (c->precision != NMFB200_PREC_F32 && !tc_limit) {    // NMFD at auto / f16, NMF2D / NMF3D at f16
-    cudaDeviceProp prop;
-    if (cudaGetDeviceProperties(&prop, device) == cudaSuccess && prop.major == 9) {
-      int rc = tc_nmfd_create(&c->tcd, c->d);          // beta = 1 runs as wgmma sliding GEMMs (tc_nmfd.cu)
-      if (rc) { free_ctx(c); return rc; }
-    } else if (precision == NMFB200_PREC_F16) {
-      free_ctx(c);
-      return fail(NMFB200_ERR_INVALID, "the tensor-core NMFD path needs an sm_90 device");
-    }
-  }
-  *out = c;
-  return 0;
-}
-
-int nmfb200_nmfd_set_target(nmfb200_ctx* ctx, const void* V, int dtype, void* stream) {
-  CTX_GUARD(ctx, 1);
-  if (int rc = check_target(V, dtype)) return rc;
-  ctx->V = V; ctx->vdtype = dtype; ctx->has_target = true; ctx->mask = nullptr;
-  cudaStream_t st = (cudaStream_t)stream;
-  const int64_t vin = ctx->d.v_inner();
-  int rc = matrix_minmax(V, dtype, (int64_t)ctx->d.B * ctx->d.C, vin, vin, ctx->mm_scratch, ctx->mm_scratch + kMmPartials, st);
-  if (rc) return rc;
-  ctx->tc_off = false;
-  if (ctx->tcd) {
-    double vsum = 0.0;
-    rc = tc_nmfd_set_target(ctx->tcd, V, dtype, &vsum, st);       // synchronises: sum(V) for kappa
-    if (rc) return rc;
-    tc_nmfd_mark_dirty(ctx->tcd);                         // a new fit: the factors may be anything
-    if (ctx->auto_mode)                                   // same conservative rule as the NMF path: heavy-tailed targets stay fp32
-      return auto_off_if_heavy_tailed(ctx, vsum, (double)ctx->d.B * ctx->d.C * ctx->d.v_inner(), st);
-  }
-  return 0;
-}
-
-// beta = 1 on tensor cores: both column-sum vectors (KL denominators, nmf.py:122-131, and kappa), then the recon pass
-static bool nmfd_use_tc(const nmfb200_ctx* c, double beta) {
-  return c->tcd != nullptr && !c->tc_off && !c->mask && tc_nmfd_supported(c->d, beta);
-}
-
-static int nmfd_phi(nmfb200_ctx* c, const float* W, const float* H, double beta, cudaStream_t st) {
-  if (beta != 1.0 || c->mask) {
-    if (!c->Pp) NMF_CUDA_CHECK(cudaMalloc(&c->Pp, (size_t)c->d.B * c->d.C * c->d.v_inner() * sizeof(float)));
-    int e = ensure_den(c);
-    if (e) return e;
-  }
-  return nmfd_recon_phi(c->d, c->V, c->vdtype, W, H, beta, c->Pn, c->Pp, nullptr, 0, nullptr, st, c->mask);
-}
-
-// Both backward passes of one factor (which = 0: W, 1: H) from the current factors, described as the ratio stage's input:
-// split partial numerators (+ denominators for beta != 1), the KL column sums, the centring term of the tensor-core path.
-// Shared by the update (nmf.py:367-391) and by nmfd_raw_terms.  `tc` reports which path produced the terms.
-static int nmfd_terms(nmfb200_ctx* ctx, const float* W, const float* H, int which, double beta, ApplyArgs& a, bool* tc,
-                      cudaStream_t st) {
-  const NmfdShape& d = ctx->d;
-  a = nmfd_apply_shape(d, which, 1);
-  *tc = nmfd_use_tc(ctx, beta);
-  if (*tc) {
-    int rc = tc_nmfd_recon(ctx->tcd, ctx->V, ctx->vdtype, W, H, false, nullptr, st);
-    if (rc) return rc;
-    const float* part; int nsplit;
-    rc = which == 0 ? tc_nmfd_wgrad(ctx->tcd, &part, &nsplit, st) : tc_nmfd_dgrad(ctx->tcd, &part, &nsplit, st);
-    if (rc) return rc;
-    a.num = part; a.den = nullptr; a.nchunks = nsplit;
-    const float* cs = tc_nmfd_colsum(ctx->tcd) + (which == 0 ? d.R : 0);       // [colsum_W | colsum_H]
-    a.kl_den = cs; a.kappa = tc_nmfd_kappa(ctx->tcd); a.kappa_vec = cs;
-    return 0;
-  }
-  if (ctx->tcd) tc_nmfd_mark_dirty(ctx->tcd);            // this pass bypasses the tensor-core state
-  int rc = nmfd_phi(ctx, W, H, beta, st);
-  if (rc) return rc;
-  const int nsplit = which == 0 ? ctx->wgrad_nsplit : ctx->dgrad_nsplit;
-  rc = which == 0 ? nmfd_wgrad(d, ctx->Pn, H, ctx->num, nsplit, st) : nmfd_dgrad(d, ctx->Pn, W, ctx->num, nsplit, st);
-  if (rc) return rc;
-  float* kl = nullptr;
-  const bool colsum = kl_colsum(ctx, beta);
-  if (colsum) {                                          // nmf.py:122-131: column sums of the OTHER factor
-    kl = ctx->colsum + (which == 0 ? d.R : 0);
-    rc = which == 0 ? factor_colsum(H, d.B, d.R, d.h_inner(), ctx->cs_scratch, ctx->cs_scratch_floats, kl, st)
-                    : factor_colsum(W, d.C, d.R, d.w_inner(), ctx->cs_scratch, ctx->cs_scratch_floats, kl, st);
-  } else {
-    rc = which == 0 ? nmfd_wgrad(d, ctx->Pp, H, ctx->den, nsplit, st) : nmfd_dgrad(d, ctx->Pp, W, ctx->den, nsplit, st);
-  }
-  if (rc) return rc;
-  a.num = ctx->num; a.den = colsum ? nullptr : ctx->den; a.nchunks = nsplit; a.kl_den = kl;
-  return 0;
-}
-
-int nmfb200_nmfd_plan(int64_t B, int64_t C, int ndim, const int64_t* vdims, int64_t R, const int64_t* kdims, int64_t* out,
-                      int n) {
-  if (!out || n < NMFB200_NMFD_PLAN_LEN) return fail(NMFB200_ERR_INVALID, "plan buffer too small");
-  NmfdShape d;
-  if (int rc = nmfd_shape_of(B, C, ndim, vdims, R, kdims, &d)) return rc;
-  NmfdPlan p;
-  nmfd_plan(d, &p);
-  const WgradPlan& w = p.wgrad;
-  const int64_t v[NMFB200_NMFD_PLAN_LEN] = {
-      p.recon_mt, p.recon_grid.x, p.recon_grid.y, p.recon_grid.z,
-      p.dgrad_mt, p.dgrad_nsplit, p.dgrad_grid.x, p.dgrad_grid.y, p.dgrad_grid.z,
-      w.mt, w.tp, w.nr, w.no, w.ntt, w.nrg, w.nog, p.wgrad_nsplit,
-      apply_update_vec4_shape(nmfd_apply_shape(d, 0, p.wgrad_nsplit)), apply_update_vec4_shape(nmfd_apply_shape(d, 1, p.dgrad_nsplit))};
-  for (int i = 0; i < NMFB200_NMFD_PLAN_LEN; ++i) out[i] = v[i];
-  return 0;
-}
-
-int nmfb200_nmfnd_tc_plan(int64_t B, int64_t C, int ndim, const int64_t* vdims, int64_t R, const int64_t* kdims,
-                          int64_t* out, int n) {
-  if (!out || n < NMFB200_NMFND_TC_PLAN_LEN) return fail(NMFB200_ERR_INVALID, "plan buffer too small");
-  NmfdShape d;
-  if (int rc = nmfd_shape_of(B, C, ndim, vdims, R, kdims, &d)) return rc;
-  TcNmfdPlan p;
-  if (const char* why = tc_nmfd_plan(d, &p)) return fail(NMFB200_ERR_INVALID, why);
-  const int64_t v[NMFB200_NMFND_TC_PLAN_LEN] = {
-      p.prep_w.x, p.prep_w.y, p.prep_w.z, p.prep_h.x, p.prep_h.y, p.prep_h.z, p.recon.x, p.recon.y, p.recon.z,
-      p.wgrad.x, p.wgrad.y, p.wgrad.z, p.dgrad.x, p.dgrad.y, p.dgrad.z, p.bslice, p.slices, p.dgrad_rblocks,
-      p.loss_blocks, p.ws_w, p.kbs_w, p.ws_h, p.kbs_h, p.hslice, p.hslices, p.Tp, p.padl, p.Lp, p.Lq, p.Cpad, p.nch};
-  for (int i = 0; i < NMFB200_NMFND_TC_PLAN_LEN; ++i) out[i] = v[i];
-  return 0;
-}
-
-static int nmfd_update(nmfb200_ctx* ctx, const float* W, const float* H, int which, float* param, double beta, double gamma,
-                       double l1_reg, double l2_reg, cudaStream_t st) {
-  ApplyArgs a; bool tc;
-  int rc = nmfd_terms(ctx, W, H, which, beta, a, &tc, st);
-  if (rc) return rc;
-  a.param = param; a.gamma = (float)gamma; a.l1 = (float)l1_reg; a.l2 = (float)l2_reg;
-  if (tc) a.absmax_bits = tc_nmfd_begin_update(ctx->tcd, which, st);
-  return apply_update(a, st);
-}
-
-// The raw terms of one factor's update (which = 0: W, 1: H) into `out`, nmfb200_raw_terms_numel floats: the split partials
-// summed with the centring term folded in (raw_sum), then the KL column sums at beta 1.
-static int nmfd_raw_terms(nmfb200_ctx* ctx, const float* W, const float* H, int which, double beta, float* out,
-                          cudaStream_t st) {
-  ApplyArgs a; bool tc;
-  int rc = nmfd_terms(ctx, W, H, which, beta, a, &tc, st);
-  if (rc) return rc;
-  rc = raw_sum(a, out, a.den ? out + a.numel : nullptr, st);
-  if (rc) return rc;
-  if (a.kl_den)
-    NMF_CUDA_CHECK(cudaMemcpyAsync(out + a.numel, a.kl_den, (size_t)ctx->d.R * sizeof(float), cudaMemcpyDeviceToDevice, st));
-  return 0;
-}
-
 /* ---- both kinds: the arguments are checked once, then the context's own kernels run ------------------------ */
 
 int nmfb200_sync_factors(nmfb200_ctx* ctx) {
   CTX_GUARD(ctx, kAnyKind);
   // operand copies are rebuilt lazily; the CUDA-core paths read the fp32 factors directly
-  if (ctx->tc) tc_mark_dirty(ctx->tc, true, true);
-  if (ctx->tcd) tc_nmfd_mark_dirty(ctx->tcd);
+  mark_stale(ctx, true, true);
   return 0;
 }
 
 // update_w / update_h: one factor update (which = 0: param = W, 1: param = H)
-static int update_factor(nmfb200_ctx* ctx, int which, float* param, const float* W, const float* H, double beta,
-                         double gamma, double l1_reg, double l2_reg, void* stream) {
+static int checked_update(nmfb200_ctx* ctx, int which, float* param, const float* W, const float* H, double beta,
+                          double gamma, double l1_reg, double l2_reg, void* stream) {
   CTX_GUARD(ctx, kAnyKind);
   TARGET_GUARD(ctx);
   if (!W || !H) return fail(NMFB200_ERR_INVALID, "null factor pointer");
-  cudaStream_t st = (cudaStream_t)stream;
-  if (ctx->kind == 0) return nmf_update(ctx, which, param, W, H, beta, gamma, l1_reg, l2_reg, st);
-  return nmfd_update(ctx, W, H, which, param, beta, gamma, l1_reg, l2_reg, st);
+  return update_factor(ctx, which, param, W, H, beta, gamma, l1_reg, l2_reg, (cudaStream_t)stream);
 }
 
 int nmfb200_update_w(nmfb200_ctx* ctx, float* W, const float* H, double beta, double gamma, double l1_reg, double l2_reg,
                      void* stream) {
-  return update_factor(ctx, 0, W, W, H, beta, gamma, l1_reg, l2_reg, stream);
+  return checked_update(ctx, 0, W, W, H, beta, gamma, l1_reg, l2_reg, stream);
 }
 
 int nmfb200_update_h(nmfb200_ctx* ctx, const float* W, float* H, double beta, double gamma, double l1_reg, double l2_reg,
                      void* stream) {
-  return update_factor(ctx, 1, H, W, H, beta, gamma, l1_reg, l2_reg, stream);
+  return checked_update(ctx, 1, H, W, H, beta, gamma, l1_reg, l2_reg, stream);
 }
 
 int nmfb200_loss(nmfb200_ctx* ctx, const float* W, const float* H, double beta, double* loss_dev, void* stream) {
@@ -863,7 +823,7 @@ int nmfb200_loss(nmfb200_ctx* ctx, const float* W, const float* H, double beta, 
   if (!W || !H || !loss_dev) return fail(NMFB200_ERR_INVALID, "null pointer");
   cudaStream_t st = (cudaStream_t)stream;
   if (ctx->kind == 1) {
-    if (nmfd_use_tc(ctx, beta)) return tc_nmfd_recon(ctx->tcd, ctx->V, ctx->vdtype, W, H, true, loss_dev, st);
+    if (use_tc(ctx, beta)) return tc_nmfd_recon(ctx->tcd, ctx->V, ctx->vdtype, W, H, true, loss_dev, st);
     return nmfd_recon_phi(ctx->d, ctx->V, ctx->vdtype, W, H, beta, nullptr, nullptr, ctx->loss_blocks, ctx->loss_max_blocks,
                           loss_dev, st, ctx->mask);
   }
@@ -875,19 +835,28 @@ int nmfb200_loss(nmfb200_ctx* ctx, const float* W, const float* H, double beta, 
 
 int64_t nmfb200_raw_terms_numel(const nmfb200_ctx* ctx, int which, double beta) {
   if (!ctx || (which != 0 && which != 1)) return -1;
-  const NmfdShape& d = ctx->d;
-  const int64_t n = ctx->kind == 0 ? (which == 0 ? ctx->C : ctx->N) * ctx->R
-                                   : (int64_t)(which == 0 ? d.C : d.B) * d.R * (which == 0 ? d.w_inner() : d.h_inner());
+  const int64_t n = factor_view(ctx, which, 1).numel;
   return kl_colsum(ctx, beta) ? n + ctx->R : 2 * n;
 }
 
+// The raw terms of one factor's update (which = 0: W, 1: H) into `out`, nmfb200_raw_terms_numel floats: the partial slabs
+// summed with the centring term folded in (raw_sum), then the KL column sums at beta 1.
 int nmfb200_raw_terms(nmfb200_ctx* ctx, const float* W, const float* H, int which, double beta, float* out, void* stream) {
   CTX_GUARD(ctx, kAnyKind);
   TARGET_GUARD(ctx);
   if (!W || !H || !out || (which != 0 && which != 1)) return fail(NMFB200_ERR_INVALID, "bad argument");
   cudaStream_t st = (cudaStream_t)stream;
-  if (ctx->kind == 0) return nmf_raw_terms(ctx, W, H, which, beta, out, st);
-  return nmfd_raw_terms(ctx, W, H, which, beta, out, st);
+  if (ctx->tc && use_tc(ctx, beta) && tc_supports_partial(ctx->tc, beta))
+    return tc_raw_terms(ctx->tc, which, W, H, beta, out, st);
+  ApplyArgs a; bool tc;
+  int rc = factor_terms(ctx, which, W, H, beta, out, a, &tc, st);
+  if (rc) return rc;
+  float* den_out = out + a.numel;
+  if (a.num != out && (rc = raw_sum(a, out, den_out, st))) return rc;        // not already in final form
+  if (a.kl_den && a.kl_den != den_out)                  // the NMFD tensor cores keep their column sums
+    NMF_CUDA_CHECK(cudaMemcpyAsync(den_out, a.kl_den, (size_t)ctx->R * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  if (!tc) mark_stale(ctx, false, false);               // no factor changed: NMF's operand copies stay valid
+  return 0;
 }
 
 // The update's ratio stage on summed raw W terms: one slab, leaving the tensor-core state as update_w does
@@ -897,35 +866,17 @@ int nmfb200_w_apply(nmfb200_ctx* ctx, float* W, const float* reduced, double bet
   TARGET_GUARD(ctx);
   if (!W || !reduced) return fail(NMFB200_ERR_INVALID, "null pointer");
   cudaStream_t st = (cudaStream_t)stream;
-  if (ctx->kind == 0) {
-    if (use_tc(ctx, beta)) return tc_w_apply(ctx->tc, W, reduced, beta, gamma, l1_reg, l2_reg, st);
-    int rc = apply_update(nmf_apply_args(ctx, 0, W, beta, reduced, reduced + ctx->C * ctx->R, 1, 0, gamma, l1_reg, l2_reg), st);
-    if (rc) return rc;
-    if (ctx->tc) tc_mark_dirty(ctx->tc, true, false);
-    return 0;
-  }
-  ApplyArgs a = nmfd_apply_shape(ctx->d, 0, 1);     // the centring term is already folded in by raw_sum
+  if (ctx->tc && use_tc(ctx, beta)) return tc_w_apply(ctx->tc, W, reduced, beta, gamma, l1_reg, l2_reg, st);
+  ApplyArgs a = factor_view(ctx, 0, 1);     // an NMFD centring term is already folded in by raw_sum
   a.param = W; a.num = reduced; a.gamma = (float)gamma; a.l1 = (float)l1_reg; a.l2 = (float)l2_reg;
   if (kl_colsum(ctx, beta)) a.kl_den = reduced + a.numel;
   else a.den = reduced + a.numel;
-  if (nmfd_use_tc(ctx, beta)) a.absmax_bits = tc_nmfd_begin_update(ctx->tcd, 0, st);
-  else if (ctx->tcd) tc_nmfd_mark_dirty(ctx->tcd);
-  return apply_update(a, st);
-}
-
-int nmfb200_set_mask(nmfb200_ctx* ctx, const uint8_t* M, void* stream) {
-  CTX_GUARD(ctx, kAnyKind);
-  TARGET_GUARD(ctx);
-  if (ctx->sparse) return fail(NMFB200_ERR_INVALID, "a mask needs a dense target (set_target or nmfd_set_target)");
-  cudaStream_t st = (cudaStream_t)stream;
-  ctx->mask = M;
-  // the tensor-core paths are bypassed while a mask is set: their operand copies are rebuilt on their next use
-  if (ctx->tc) tc_mark_dirty(ctx->tc, true, true);
-  if (ctx->tcd) tc_nmfd_mark_dirty(ctx->tcd);
-  float* minmax = ctx->mm_scratch + kMmPartials;          // target_minmax: the observed cells only, or all of V again
-  if (ctx->kind == 0) return matrix_minmax(ctx->V, ctx->vdtype, ctx->N, ctx->C, ctx->ldv, ctx->mm_scratch, minmax, st, M);
-  const int64_t vin = ctx->d.v_inner();
-  return matrix_minmax(ctx->V, ctx->vdtype, (int64_t)ctx->d.B * ctx->d.C, vin, vin, ctx->mm_scratch, minmax, st, M);
+  const bool tc = use_tc(ctx, beta);        // here: the NMFD tensor cores
+  if (tc) a.absmax_bits = tc_nmfd_begin_update(ctx->tcd, 0, st);
+  int rc = apply_update(a, st);
+  if (rc) return rc;
+  if (!tc) mark_stale(ctx, true, false);
+  return 0;
 }
 
 int nmfb200_hoyer_project(int device, float* x, int64_t outer, int64_t D, int64_t inner, const float* k1, const float* k2,

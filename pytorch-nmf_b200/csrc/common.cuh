@@ -137,9 +137,6 @@ int raw_sum(const ApplyArgs& a, float* num_out, float* den_out, cudaStream_t st)
 int factor_colsum(const float* x, int64_t outer, int R, int64_t inner, float* scratch, int64_t scratch_floats,
                   float* sums, cudaStream_t st);
 int64_t colsum_scratch_floats(int64_t outer, int R, int64_t inner);
-// dst[i] = sum_ch src[ch*stride + i]   (chunk reduction for the sharded partial buffers)
-int reduce_chunks(const float* src, int nchunks, int64_t chunk_stride, int64_t rows, int R, int64_t ldp,
-                  float* dst, cudaStream_t st);
 // min / max of a strided matrix of `vdtype` elements (fit()'s validation), results in mm[0..1]; with M (optional, contiguous
 // rows x cols uint8) over the cells where M is set only (none: +inf / -inf)
 int matrix_minmax(const void* V, int vdtype, int64_t rows, int64_t cols, int64_t ld, float* scratch2048, float* mm,

@@ -166,4 +166,9 @@ __device__ __forceinline__ uint32_t pack_f16x2_sat(float lo, float hi) {
 }
 
 }  // namespace ptx
+
+// Host side (tc_nmf.cu): the TMA descriptor of a 2-D fp16 row-major tensor (rows x cols, row pitch ld elements), box 64
+// cols x box_rows rows, SWIZZLE_128B.
+int make_tmap(CUtensorMap* m, const void* base, int64_t rows, int64_t cols, int64_t ld, int box_rows);
+
 }  // namespace nmfb200

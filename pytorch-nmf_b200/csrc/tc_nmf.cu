@@ -1169,43 +1169,8 @@ v_beta_term_kernel(const TV* __restrict__ V, int64_t rows, int64_t cols, int64_t
   const double t = block_sum256(acc, red);
   if (threadIdx.x == 0) blockpart[blockIdx.x] = t;
 }
-__global__ void __launch_bounds__(256)
-sum_blocks_kernel(const double* __restrict__ blockpart, int n, double* __restrict__ out) {
-  __shared__ double red[8];
-  double acc = 0.0;
-  for (int i = threadIdx.x; i < n; i += 256) acc += blockpart[i];
-  const double t = block_sum256(acc, red);
-  if (threadIdx.x == 0) *out = t;
-}
 
 // ---- host side --------------------------------------------------------------------------------------
-
-PFN_cuTensorMapEncodeTiled_v12000 get_encode_fn() {
-  static PFN_cuTensorMapEncodeTiled_v12000 fn = nullptr;
-  if (fn) return fn;
-  void* ptr = nullptr;
-  cudaDriverEntryPointQueryResult qres;
-  if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres) != cudaSuccess ||
-      qres != cudaDriverEntryPointSuccess)
-    return nullptr;
-  fn = reinterpret_cast<PFN_cuTensorMapEncodeTiled_v12000>(ptr);
-  return fn;
-}
-
-// 2-D fp16 row-major tensor (rows x cols, row pitch ld elements), box 64 cols x box_rows rows, SWIZZLE_128B
-int make_tmap(CUtensorMap* m, const void* base, int64_t rows, int64_t cols, int64_t ld, int box_rows) {
-  auto fn = get_encode_fn();
-  if (!fn) { set_error("cuTensorMapEncodeTiled entry point not available"); return 2; }
-  cuuint64_t gdim[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  cuuint64_t gstr[1] = {(cuuint64_t)ld * 2};
-  cuuint32_t box[2] = {64, (cuuint32_t)box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(base), gdim, gstr, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled failed with code " + std::to_string((int)r)); return 2; }
-  return 0;
-}
 
 struct Plan { int row_blocks, tiles, nchunks, tpc; };
 
@@ -1232,6 +1197,32 @@ Plan make_plan(int64_t Mr, int64_t Nc, int num_sms, int TN) {
 }
 
 }  // namespace
+
+static PFN_cuTensorMapEncodeTiled_v12000 get_encode_fn() {
+  static PFN_cuTensorMapEncodeTiled_v12000 fn = nullptr;
+  if (fn) return fn;
+  void* ptr = nullptr;
+  cudaDriverEntryPointQueryResult qres;
+  if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres) != cudaSuccess ||
+      qres != cudaDriverEntryPointSuccess)
+    return nullptr;
+  fn = reinterpret_cast<PFN_cuTensorMapEncodeTiled_v12000>(ptr);
+  return fn;
+}
+
+int make_tmap(CUtensorMap* m, const void* base, int64_t rows, int64_t cols, int64_t ld, int box_rows) {
+  auto fn = get_encode_fn();
+  if (!fn) { set_error("cuTensorMapEncodeTiled entry point not available"); return 2; }
+  cuuint64_t gdim[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
+  cuuint64_t gstr[1] = {(cuuint64_t)ld * 2};
+  cuuint32_t box[2] = {64, (cuuint32_t)box_rows};
+  cuuint32_t estr[2] = {1, 1};
+  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(base), gdim, gstr, box, estr,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled failed with code " + std::to_string((int)r)); return 2; }
+  return 0;
+}
 
 struct TcState {
   // ---- row-sharded W update over peer memory (tc_peer_*): one cudaMalloc block per rank, shared by CUDA IPC:
@@ -1840,8 +1831,8 @@ int tc_loss(TcState* s, const float* W, const float* H, double beta, double* los
       return 0;
     });
     if (rc) return rc;
-    sum_blocks_kernel<<<1, 256, 0, st>>>(s->vbeta_part, 1024, s->vbeta);
-    NMF_LAUNCH_CHECK();
+    rc = sum_partials(s->vbeta_part, 1024, s->vbeta, st);
+    if (rc) return rc;
     s->vbeta_for = beta;
   }
   int grid = beta == 2.0 ? launch_loss_bm<kBmEU>(s, beta, st)

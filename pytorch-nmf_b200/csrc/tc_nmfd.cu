@@ -20,11 +20,9 @@
 #include "tc_nmfd.cuh"
 
 #include <cuda.h>
-#include <cudaTypedefs.h>
 
 #include <algorithm>
 #include <cstdlib>
-#include <string>
 
 #include "sm90_ptx.cuh"
 
@@ -542,32 +540,6 @@ vsum_kernel(const TV* __restrict__ V, int64_t n, double* __restrict__ part) {
   if (threadIdx.x == 0) { double t = 0.0; for (int i = 0; i < 8; ++i) t += sh[i]; part[blockIdx.x] = t; }
 }
 
-PFN_cuTensorMapEncodeTiled_v12000 encode_fn() {
-  static PFN_cuTensorMapEncodeTiled_v12000 fn = nullptr;
-  if (fn) return fn;
-  void* ptr = nullptr;
-  cudaDriverEntryPointQueryResult qres;
-  if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres) != cudaSuccess ||
-      qres != cudaDriverEntryPointSuccess)
-    return nullptr;
-  fn = reinterpret_cast<PFN_cuTensorMapEncodeTiled_v12000>(ptr);
-  return fn;
-}
-
-int make_tmap2(CUtensorMap* m, const void* base, int64_t rows, int64_t cols, int64_t ld, int box_rows) {
-  auto fn = encode_fn();
-  if (!fn) { set_error("cuTensorMapEncodeTiled entry point not available"); return 2; }
-  cuuint64_t gdim[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  cuuint64_t gstr[1] = {(cuuint64_t)ld * 2};
-  cuuint32_t box[2] = {64, (cuuint32_t)box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(base), gdim, gstr, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled (nmfd) failed with code " + std::to_string((int)r)); return 2; }
-  return 0;
-}
-
 }  // namespace
 
 struct TcNmfdState {
@@ -704,11 +676,11 @@ int tc_nmfd_create(TcNmfdState** out, const NmfdShape& d) {
     return 2;
   }
   int rc = 0;
-  rc |= make_tmap2(&s->tmWr, s->Wr16, s->Cpad, (int64_t)d.R * T12 * s->Tp, (int64_t)d.R * T12 * s->Tp, kM);
+  rc |= make_tmap(&s->tmWr, s->Wr16, s->Cpad, (int64_t)d.R * T12 * s->Tp, (int64_t)d.R * T12 * s->Tp, kM);
   // dgrad reads Wf16 as (C R) rows of T1 T2 Tp columns, up to 128 rows (components) per tile
   const int Rb = (int)std::min<int64_t>((d.R + 15) & ~15, 128);
-  rc |= make_tmap2(&s->tmWf, s->Wf16, (int64_t)s->Cpad * d.R, T12 * s->Tp, T12 * s->Tp, Rb);
-  rc |= make_tmap2(&s->tmP, s->P16, (int64_t)d.B * X12 * d.C, s->Lq, s->Lq, kM);
+  rc |= make_tmap(&s->tmWf, s->Wf16, (int64_t)s->Cpad * d.R, T12 * s->Tp, T12 * s->Tp, Rb);
+  rc |= make_tmap(&s->tmP, s->P16, (int64_t)d.B * X12 * d.C, s->Lq, s->Lq, kM);
   if (rc) { tc_nmfd_destroy(s); return 2; }
   *out = s;
   return 0;

@@ -119,18 +119,6 @@ __global__ void colsum_final_kernel(const float* __restrict__ partial, int64_t n
   sums[r] = t;
 }
 
-__global__ void __launch_bounds__(256)
-reduce_chunks_kernel(const float* __restrict__ src, int nchunks, int64_t chunk_stride, int64_t rows, int R,
-                     int64_t ldp, float* __restrict__ dst) {
-  const int64_t idx = (int64_t)blockIdx.x * 256 + threadIdx.x;
-  if (idx >= rows * R) return;
-  const int64_t row = idx / R;
-  const int r = (int)(idx - row * R);
-  float t = 0.f;
-  for (int ch = 0; ch < nchunks; ++ch) t += src[ch * chunk_stride + row * ldp + r];
-  dst[idx] = t;
-}
-
 __device__ __forceinline__ float nan_min(float a, float b) { return (a != a || b != b) ? NAN : fminf(a, b); }
 __device__ __forceinline__ float nan_max(float a, float b) { return (a != a || b != b) ? NAN : fmaxf(a, b); }
 
@@ -270,14 +258,6 @@ int factor_colsum(const float* x, int64_t outer, int R, int64_t inner, float* sc
   }
   NMF_LAUNCH_CHECK();
   colsum_final_kernel<<<(unsigned)ceil_div(R, 64), 64, 0, st>>>(scratch, nb, R, sums);
-  NMF_LAUNCH_CHECK();
-  return 0;
-}
-
-int reduce_chunks(const float* src, int nchunks, int64_t chunk_stride, int64_t rows, int R, int64_t ldp,
-                  float* dst, cudaStream_t st) {
-  reduce_chunks_kernel<<<(unsigned)ceil_div(rows * R, 256), 256, 0, st>>>(src, nchunks, chunk_stride, rows, R,
-                                                                         ldp, dst);
   NMF_LAUNCH_CHECK();
   return 0;
 }

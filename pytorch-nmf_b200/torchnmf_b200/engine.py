@@ -220,23 +220,24 @@ class _CudaEngine:
         factor), else in the factor's shape.  What BetaMu.step and PLCA.fit are built from (include/nmf_b200.h:
         nmfb200_raw_terms)."""
         f = self.W if which == 0 else self.H
-        n = int(self._lib.nmfb200_raw_terms_numel(self._ctx, int(which), float(beta)))
-        buf = torch.empty(n, dtype=torch.float32, device=self.device)
-        _capi.check(self._lib.nmfb200_raw_terms(self._ctx, _ptr(self.W), _ptr(self.H), int(which), float(beta), _ptr(buf),
-                                                _stream(self.device)))
+        buf = self._raw_terms_into(which, beta, None)
         num, den = buf[:f.numel()].view(f.shape), buf[f.numel():]
         return num, (den if beta == 1 and self._mask is None else den.view(f.shape))
+
+    def _raw_terms_into(self, which, beta, buf):
+        """nmfb200_raw_terms flat into `buf`, or into a new buffer when `buf` is None or of another size; returns it."""
+        n = int(self._lib.nmfb200_raw_terms_numel(self._ctx, int(which), float(beta)))
+        if buf is None or buf.numel() != n:
+            buf = torch.empty(n, dtype=torch.float32, device=self.device)
+        _capi.check(self._lib.nmfb200_raw_terms(self._ctx, _ptr(self.W), _ptr(self.H), int(which), float(beta), _ptr(buf),
+                                                _stream(self.device)))
+        return buf
 
     # --- pieces of the sharded W update (ShardedEngine) ---------------------------------------
     def w_partial(self, beta):
         """This shard's raw W terms, raw_terms(0)'s layout flat, in one buffer per engine reused every iteration."""
-        n = int(self._lib.nmfb200_raw_terms_numel(self._ctx, 0, beta))
-        buf = self._wbuf
-        if buf is None or buf.numel() != n:
-            buf = self._wbuf = torch.empty(n, dtype=torch.float32, device=self.device)
-        _capi.check(self._lib.nmfb200_raw_terms(self._ctx, _ptr(self.W), _ptr(self.H), 0, beta, _ptr(buf),
-                                                _stream(self.device)))
-        return buf
+        self._wbuf = self._raw_terms_into(0, beta, self._wbuf)
+        return self._wbuf
 
     def w_apply(self, reduced, beta, gamma, l1_reg, l2_reg):
         _capi.check(self._lib.nmfb200_w_apply(self._ctx, _ptr(self.W), _ptr(reduced), beta, gamma, l1_reg, l2_reg,
