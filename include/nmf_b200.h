@@ -137,6 +137,22 @@ int nmfb200_nmf_set_target_sparse(nmfb200_ctx* ctx, int64_t nnz, const int64_t* 
 int nmfb200_nmf_set_target_sparse_any_beta(nmfb200_ctx* ctx, int64_t nnz, const int64_t* crow, const int64_t* col,
                                            const float* val, const int64_t* ccol, const int64_t* row, const float* val_t,
                                            double v_norm_kl, double v_norm_eu, void* stream);
+/* Fit only the OBSERVED cells of V, listed as sparse entries: the nnz stored entries of the two compressed forms (layout and
+ * borrowing as nmfb200_nmf_set_target_sparse) are exactly the observed cells, each once, and val / val_t hold V's value
+ * there (zeros allowed: an observed zero is a cell of the loss, not a missing one).  No v_norm: the loss takes V's terms per
+ * cell.  From then on the context fits beta_div(WH[obs], V[obs]) at every beta, as nmfb200_set_mask does on a dense target,
+ * with every update nmf.py:78-92 applied to the two backward passes of that loss (x = w_c . h_n):
+ *   num_H[n,:] = sum_{c observed in row n} v a(x) W[c,:]      den_H[n,:] = sum_{c observed in row n} b(x) W[c,:]
+ *   (beta 2: a = 1, b = x; beta 1: a = 1 / (x + eps), b = 1; other: a = (x + eps)^(beta-2), b = (x + eps)^(beta-1)),
+ * the W side over the columns; both from ONE gather per row or column (one warp each, fp32, in stored order: no atomics),
+ * O(nnz R) per update, no dense product, Gram matrix or column sum.  update_w, update_h, nmf_iterate, loss,
+ * nmf_loss_prefetch_w (= loss), raw_terms (raw_terms_numel: 2 x the factor's numel at every beta), w_apply and
+ * target_minmax (the observed values; +inf / -inf when nnz == 0) follow it.  precision_for_beta reports NMFB200_PREC_F32,
+ * nmf_peer_supported 0; contract_only returns NMFB200_ERR_STATE and set_mask NMFB200_ERR_INVALID, as on a sparse context;
+ * a context of rank R > 256 returns NMFB200_ERR_INVALID.  Any other set_target* turns the mode off again.  Asynchronous. */
+int nmfb200_nmf_set_target_observed(nmfb200_ctx* ctx, int64_t nnz, const int64_t* crow, const int64_t* col,
+                                    const float* val, const int64_t* ccol, const int64_t* row, const float* val_t,
+                                    void* stream);
 
 /* Row-sharded W update over PEER MEMORY (ranks of one NVLink domain, one process per GPU, 2..8 ranks) -- the fused form of
  * raw_terms(which = 0) -> all-reduce -> w_apply below, without a collective library call on the data path:
@@ -246,7 +262,9 @@ int nmfb200_nmf_plan(int64_t N, int64_t C, int64_t R, int64_t* out, int n);
  *   [0] rank floats per lane of the warp-per-row kernels (1, 2, 4, 8)   [1] Gram passes of 4096 (a, b) pairs
  *   [2] Gram rows per block over the N rows of H (a multiple of 32)   [3] its blocks (at most 128, the last may be short)
  *   [4], [5] the same over the C rows of W   [6] blocks (8 rows each) over N: the H update's gathers and the loss's partials
- *   [7] over C: the W update's */
+ *   [7] over C: the W update's
+ * An observed-cell context (nmfb200_nmf_set_target_observed) runs its terms and loss gathers on [0], [6] and [7] and
+ * launches no Gram kernel. */
 #define NMFB200_SPARSE_PLAN_LEN 8
 int nmfb200_nmf_sparse_plan(int64_t N, int64_t C, int64_t R, int64_t* out, int n);
 /* The same for an NMFD / NMF2D / NMF3D context (arguments as nmfb200_nmfnd_create), NMFB200_NMFD_PLAN_LEN values:

@@ -46,6 +46,9 @@ struct nmfb200_ctx {
   // sparse target (beta 1 / 2): borrowed CSR (rows of V) and CSC (= CSR of V^T) forms, V_norm of nmf.py:161-170
   bool sparse = false;
   bool sp_any_beta = false;       // set by nmfb200_nmf_set_target_sparse_any_beta, reset by every other set_target
+  // set by nmfb200_nmf_set_target_observed, reset by every other set_target: the compressed forms hold the observed cells of
+  // a masked fit, and every beta fits beta_div(WH[obs], V[obs]) on the observed-cell gathers
+  bool observed = false;
   float* sp_den = nullptr;        // max(N, C) x R: the reduced V-free denominator of an update at beta != 1, 2
   const int64_t *sp_crow = nullptr, *sp_col = nullptr, *sp_ccol = nullptr, *sp_row = nullptr;
   const float *sp_val = nullptr, *sp_val_t = nullptr;
@@ -147,7 +150,7 @@ int alloc_workspace(nmfb200_ctx* c, int64_t pn_floats) {
 
 // beta 1 without a mask: the denominator is the column sum of the other factor (nmf.py:122-131).  A masked fit takes it
 // from the second backward pass, M G, like every other beta.
-bool kl_colsum(const nmfb200_ctx* c, double beta) { return beta == 1.0 && !c->mask; }
+bool kl_colsum(const nmfb200_ctx* c, double beta) { return beta == 1.0 && !c->mask && !c->observed; }
 
 // Whether the context's own tensor-core kernels (c->tc: NMF, c->tcd: NMFD / NMF2D / NMF3D) serve this beta.
 bool use_tc(const nmfb200_ctx* c, double beta) {
@@ -334,7 +337,7 @@ int nmfb200_nmf_set_target(nmfb200_ctx* ctx, const void* V, int64_t ldv, int dty
   if (int rc = check_target(V, dtype)) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   ctx->V = V; ctx->vdtype = dtype; ctx->ldv = ldv; ctx->has_target = true; ctx->sparse = false; ctx->sp_any_beta = false;
-  ctx->mask = nullptr;
+  ctx->observed = false; ctx->mask = nullptr;
   float* minmax = ctx->mm_scratch + kMmPartials;
   int rc = matrix_minmax(V, dtype, ctx->N, ctx->C, ldv, ctx->mm_scratch, minmax, st);
   if (rc) return rc;
@@ -384,6 +387,7 @@ int nmfb200_nmf_set_target_sparse(nmfb200_ctx* ctx, int64_t nnz, const int64_t* 
   ctx->sparse = true; ctx->has_target = true; ctx->V = nullptr; ctx->tc_off = true;      // the dense kernels are out of play
   ctx->mask = nullptr;
   ctx->sp_any_beta = false;
+  ctx->observed = false;
   return 0;
 }
 
@@ -399,6 +403,20 @@ int nmfb200_nmf_set_target_sparse_any_beta(nmfb200_ctx* ctx, int64_t nnz, const 
     NMF_CUDA_CHECK(cudaMalloc(&ctx->sp_den, (size_t)(ctx->N > ctx->C ? ctx->N : ctx->C) * ctx->R * sizeof(float)));
   ctx->sp_any_beta = true;
   return 0;
+}
+
+int nmfb200_nmf_set_target_observed(nmfb200_ctx* ctx, int64_t nnz, const int64_t* crow, const int64_t* col,
+                                    const float* val, const int64_t* ccol, const int64_t* row, const float* val_t,
+                                    void* stream) {
+  int rc = nmfb200_nmf_set_target_sparse(ctx, nnz, crow, col, val, ccol, row, val_t, 0.0, 0.0, stream);
+  if (rc) return rc;
+  DeviceGuard guard(ctx->device);
+  if (!guard.ok) return fail(NMFB200_ERR_CUDA, "cannot select the context's device");
+  if ((rc = ensure_den(ctx))) return rc;                  // the denominator of an update outside raw_terms
+  ctx->observed = true;
+  // target_minmax: the observed values (none: +inf / -inf)
+  return matrix_minmax(val, NMFB200_DTYPE_F32, 1, nnz, nnz, ctx->mm_scratch, ctx->mm_scratch + kMmPartials,
+                       (cudaStream_t)stream);
 }
 
 /* ---- NMFD ------------------------------------------------------------------------------------ */
@@ -549,9 +567,10 @@ int nmfb200_set_mask(nmfb200_ctx* ctx, const uint8_t* M, void* stream) {
 }
 
 namespace {
-// beta 1 and 2 run on every sparse context; any other beta > 0 only on one set by nmfb200_nmf_set_target_sparse_any_beta
+// beta 1 and 2 run on every sparse context; any other beta > 0 only on one set by nmfb200_nmf_set_target_sparse_any_beta,
+// every beta on one set by nmfb200_nmf_set_target_observed
 int check_sparse_beta(const nmfb200_ctx* ctx, double beta) {
-  if (beta == 1.0 || beta == 2.0) return 0;
+  if (beta == 1.0 || beta == 2.0 || ctx->observed) return 0;
   if (!ctx->sp_any_beta)
     return fail(NMFB200_ERR_INVALID, "sparse targets: beta must be 1 or 2 (densify the target for other beta)");
   if (!(beta > 0.0)) return fail(NMFB200_ERR_INVALID, "sparse targets: beta must be positive");
@@ -561,6 +580,7 @@ int check_sparse_beta(const nmfb200_ctx* ctx, double beta) {
 // The terms of one factor's update on the compressed form whose segments are that factor's rows (which = 0: W over CSC,
 // 1: H over CSR), all in final form: the numerator (rows x R) into `num`; into `den` the colsum of the other factor (R, beta
 // 1), the raw denominator F (other^T other) (rows x R, beta 2) or, at any other beta, the V-free denominator's chunk sum.
+// Observed cells: both from one gather at every beta.
 int sparse_terms(nmfb200_ctx* ctx, int which, const float* F, const float* other, double beta, float* num, float* den,
                  cudaStream_t st) {
   if (int rc = check_sparse_beta(ctx, beta)) return rc;
@@ -569,6 +589,7 @@ int sparse_terms(nmfb200_ctx* ctx, int which, const float* F, const float* other
   const int64_t* ptr = which == 0 ? ctx->sp_ccol : ctx->sp_crow;
   const int64_t* idx = which == 0 ? ctx->sp_row : ctx->sp_col;
   const float* val = which == 0 ? ctx->sp_val_t : ctx->sp_val;
+  if (ctx->observed) return observed_terms(ptr, idx, val, F, other, R, f.rows, beta, num, den, st);
   int rc = sparse_numerator(ptr, idx, val, F, other, R, f.rows, beta, num, st);
   if (rc) return rc;
   if (beta != 1.0 && beta != 2.0) {     // the V-free denominator on the dense fp32 plan, its chunks summed as the dense path does
@@ -626,10 +647,11 @@ int factor_terms(nmfb200_ctx* c, int which, const float* W, const float* H, doub
   const float* fac[2] = {W, H};
   const bool kl = kl_colsum(c, beta);
   // where the final-form terms go without `out`: c->colsum is [colsum(W) | colsum(H)], the sparse raw denominator lives in
-  // c->den at beta 2 and in c->sp_den at other beta (whose c->den holds the chunks)
+  // c->den at beta 2 and on observed cells, and in c->sp_den at other beta (whose c->den holds the chunks)
   if (c->sparse && beta == 2.0 && !out) { int e = ensure_den(c); if (e) return e; }
   float* num_out = out ? out : c->num;
-  float* den_out = out ? out + a.numel : kl ? c->colsum + (1 - which) * c->R : beta == 2.0 ? c->den : c->sp_den;
+  float* den_out = out ? out + a.numel
+                 : kl ? c->colsum + (1 - which) * c->R : (beta == 2.0 || c->observed) ? c->den : c->sp_den;
   *tc = c->tcd && use_tc(c, beta);
   if (*tc) {                  // NMFD beta 1: the recon pass also brings both column sums and kappa up to date
     int rc = tc_nmfd_recon(c->tcd, c->V, c->vdtype, W, H, false, nullptr, st);
@@ -676,6 +698,8 @@ int update_factor(nmfb200_ctx* ctx, int which, float* param, const float* W, con
 int sparse_loss_ctx(nmfb200_ctx* ctx, const float* W, const float* H, double beta, double* loss_dev, cudaStream_t st) {
   if (int rc = check_sparse_beta(ctx, beta)) return rc;
   const int R = (int)ctx->R;
+  if (ctx->observed)                    // every cell's term at the observed cells, nothing elsewhere
+    return observed_loss(ctx->sp_crow, ctx->sp_col, ctx->sp_val, H, W, R, ctx->N, beta, ctx->sp_loss_part, loss_dev, st);
   if (beta != 1.0 && beta != 2.0) {     // pos = sum x^beta over every cell without V, then V_norm - neg at the non-zeros
     int npos = 0;
     int rc = simt_nmf_pow_sum(H, W, ctx->N, ctx->C, R, beta, ctx->loss_blocks, ctx->loss_max_blocks, &npos, st);

@@ -43,6 +43,26 @@ inline BetaMode beta_mode(double beta) {
   return kGeneric;
 }
 
+// one cell's term of metrics.beta_div (metrics.py:60-96): v the target, s the reconstruction, in fp32; shared by the dense
+// loss kernels (simt_nmf.cu) and the observed-cell gathers (sparse_nmf.cu)
+template <int MODE>
+__device__ __forceinline__ float loss_term(float v, float s, float beta) {
+  if (MODE == kKL) {               // metrics.py:22
+    return v * (logf(v + kEps) - logf(s + kEps)) - v + s;
+  } else if (MODE == kEU) {        // metrics.py:39
+    float d = s - v;
+    return 0.5f * d * d;
+  } else if (MODE == kIS) {        // metrics.py:56-57
+    float te = v + kEps, xe = s + kEps;
+    return te / xe - logf(te) + logf(xe) - 1.0f;
+  } else {                         // metrics.py:84-96
+    float x = s + kEps;
+    float t = beta < 0.f ? v + kEps : v;
+    float bm = beta - 1.0f;
+    return (powf(t, beta) + bm * powf(x, beta) - beta * t * powf(x, bm)) / (beta * bm);
+  }
+}
+
 void set_error(const std::string& msg);
 void count_launch();
 
@@ -166,6 +186,13 @@ int sparse_loss(const int64_t* crow, const int64_t* col, const float* val, const
 int sparse_beta_loss(const int64_t* crow, const int64_t* col, const float* val, const float* H, const float* W, int R,
                      int64_t N, double beta, const double* pos_part, int npos, double* loss_part, double* loss_dev,
                      cudaStream_t st);
+// Observed cells of a masked fit (the stored entries, zeros included), every beta: both raw terms of one factor's update in one
+// gather per segment (num, den: nseg x R), and loss_dev = beta_div(WH[obs], V[obs]) over the CSR form (loss_part: one double
+// per gather block over the N rows)
+int observed_terms(const int64_t* ptr, const int64_t* idx, const float* val, const float* Fself, const float* Fother, int R,
+                   int64_t nseg, double beta, float* num, float* den, cudaStream_t st);
+int observed_loss(const int64_t* crow, const int64_t* col, const float* val, const float* H, const float* W, int R, int64_t N,
+                  double beta, double* loss_part, double* loss_dev, cudaStream_t st);
 // launch plans (host only): rank floats per lane; blocks over nseg segments / rows (the loss: N, its partials); Gram rows per
 // block and blocks over `rows` rows; Gram passes of 4096 pairs
 int sparse_rpl(int R);

@@ -265,24 +265,6 @@ int launch_contract_rb(int trans, int mode, dim3 grid, cudaStream_t st, const TV
 
 // ---- loss ------------------------------------------------------------------------------------
 
-template <int MODE>
-__device__ __forceinline__ float loss_term(float v, float s, float beta) {
-  if (MODE == kKL) {               // metrics.py:22
-    return v * (logf(v + kEps) - logf(s + kEps)) - v + s;
-  } else if (MODE == kEU) {        // metrics.py:39
-    float d = s - v;
-    return 0.5f * d * d;
-  } else if (MODE == kIS) {        // metrics.py:56-57
-    float te = v + kEps, xe = s + kEps;
-    return te / xe - logf(te) + logf(xe) - 1.0f;
-  } else {                         // metrics.py:84-96
-    float x = s + kEps;
-    float t = beta < 0.f ? v + kEps : v;
-    float bm = beta - 1.0f;
-    return (powf(t, beta) + bm * powf(x, beta) - beta * t * powf(x, bm)) / (beta * bm);
-  }
-}
-
 __device__ __forceinline__ double block_reduce_sum(double v, double* sh) {
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   int w = threadIdx.x >> 5, l = threadIdx.x & 31;

@@ -15,31 +15,62 @@
 // One warp owns one segment -- a row of the CSR form (H update) or a column of the CSC form (W update) -- keeps its own factor
 // row in registers, gathers the other factor's rows of its non-zeros (rank floats each, coalesced) and accumulates in fp32 in
 // the order of the stored indices: deterministic, no atomics.
+//
+// Observed cells (nmfb200_nmf_set_target_observed): the stored entries are the observed cells of a masked fit, zeros
+// included, and the loss is beta_div(WH[obs], V[obs]) at every beta.  Both backward passes of that loss are sums over the
+// observed cells only, so ONE gather per segment forms both terms, with x = w_j . f_s and a(x), b(x) of nmf.py:61-74:
+//   num[s,:] = sum_j v a(x) w_j      den[s,:] = sum_j b(x) w_j
+//   beta 2: a = 1, b = x;  beta 1: a = 1 / (x + eps), b = 1;  beta 0: a = 1 / (x + eps)^2, b = 1 / (x + eps);
+//   other:  b = (x + eps)^(beta - 1) from one powf, a = b / (x + eps)
+// and the loss gather sums metrics.beta_div's per-cell term (loss_term) at each stored entry, in double.
 #include "common.cuh"
 
 namespace nmfb200 {
 
 namespace {
 
-enum SpMode : int { kSpKL = 0, kSpEU = 1, kSpKLLoss = 2, kSpEULoss = 3, kSpBeta = 4, kSpBetaLoss = 5 };
+enum SpMode : int { kSpKL = 0, kSpEU = 1, kSpKLLoss = 2, kSpEULoss = 3, kSpBeta = 4, kSpBetaLoss = 5, kSpObsTerms = 6,
+                    kSpObsLoss = 7 };
 constexpr int kSpGramPass = 256 * 16;                 // Gram pairs per pass of sp_gram_part_kernel (16 per thread)
 
-// pa, pb, ca, cb: the beta constants of kSpBeta / kSpBetaLoss (unused by the other modes)
-template <int RPL, int MODE>
+// a(x) and b(x) of an observed cell at beta mode BM (BetaMode), x = w_j . f_s; bm1 = beta - 1 (kGeneric only)
+template <int BM>
+__device__ __forceinline__ void obs_phi(float x, float bm1, float& a, float& b) {
+  if (BM == kEU) {
+    a = 1.f;
+    b = x;                                                // nmf.py:62-63 (no eps)
+  } else if (BM == kKL) {
+    a = 1.0f / (x + kEps);                                // nmf.py:65; den: the observed cells' rows of the other factor
+    b = 1.f;
+  } else if (BM == kIS) {
+    const float r = 1.0f / (x + kEps);                    // nmf.py:68-70
+    a = r * r;
+    b = r;
+  } else {
+    const float xe = x + kEps;                            // nmf.py:72-74
+    b = powf(xe, bm1);
+    a = b / xe;
+  }
+}
+
+// pa, pb, ca, cb: the beta constants of kSpBeta / kSpBetaLoss (unused by the other modes); kSpObsTerms: pa = beta - 1,
+// den_out the denominator (nseg x R); kSpObsLoss: pa = beta.  BM: the beta mode of the two observed-cell modes.
+template <int RPL, int MODE, int BM = kKL>
 __device__ __forceinline__ void
 sp_gather(const int64_t* __restrict__ ptr, const int64_t* __restrict__ idx, const float* __restrict__ val,
           const float* __restrict__ Fs, const float* __restrict__ Fo, int R, int64_t nseg, float* __restrict__ out,
-          double* __restrict__ loss_part, float pa, float pb, double ca, double cb) {
+          float* __restrict__ den_out, double* __restrict__ loss_part, float pa, float pb, double ca, double cb) {
   const int lane = threadIdx.x & 31;
   const int64_t seg = (int64_t)blockIdx.x * 8 + (threadIdx.x >> 5);
   double lacc = 0.0;
   if (seg < nseg) {
-    float hs[RPL], acc[RPL];
+    float hs[RPL], acc[RPL], dacc[RPL];
 #pragma unroll
     for (int k = 0; k < RPL; ++k) {
       const int r = lane + 32 * k;
       hs[k] = r < R ? Fs[seg * R + r] : 0.f;
       acc[k] = 0.f;
+      dacc[k] = 0.f;
     }
     const int64_t e0 = ptr[seg], e1 = ptr[seg + 1];
     for (int64_t e = e0; e < e1; ++e) {
@@ -72,21 +103,33 @@ sp_gather(const int64_t* __restrict__ ptr, const int64_t* __restrict__ idx, cons
       } else if (MODE == kSpBetaLoss) {
         // pa = beta, pb = beta - 1, ca = 1 / (beta (beta - 1)), cb = 1 / (beta - 1): V_norm's and neg's terms of this entry
         lacc += (double)powf(v, pa) * ca - (double)(v * powf(dot + kEps, pb)) * cb;
+      } else if (MODE == kSpObsTerms) {
+        float a, b;
+        obs_phi<BM>(dot, pa, a, b);
+        const float ratio = v * a;
+#pragma unroll
+        for (int k = 0; k < RPL; ++k) {
+          acc[k] = fmaf(ratio, w[k], acc[k]);
+          dacc[k] = fmaf(b, w[k], dacc[k]);
+        }
+      } else if (MODE == kSpObsLoss) {
+        lacc += (double)loss_term<BM>(v, dot, pa);                   // metrics.py:60-96 at this cell
       } else if (MODE == kSpKLLoss) {
         lacc += (double)(v * logf(dot + kEps));                      // nmf.py:619
       } else {
         lacc += (double)(v * dot);                                   // nmf.py:610
       }
     }
-    if (MODE == kSpKL || MODE == kSpEU || MODE == kSpBeta) {
+    if (MODE == kSpKL || MODE == kSpEU || MODE == kSpBeta || MODE == kSpObsTerms) {
 #pragma unroll
       for (int k = 0; k < RPL; ++k) {
         const int r = lane + 32 * k;
         if (r < R) out[seg * R + r] = acc[k];
+        if (MODE == kSpObsTerms && r < R) den_out[seg * R + r] = dacc[k];
       }
     }
   }
-  if (MODE == kSpKLLoss || MODE == kSpEULoss || MODE == kSpBetaLoss) {
+  if (MODE == kSpKLLoss || MODE == kSpEULoss || MODE == kSpBetaLoss || MODE == kSpObsLoss) {
     __shared__ double sh[8];
     if (lane == 0) sh[threadIdx.x >> 5] = lacc;       // every lane holds the same sum
     __syncthreads();
@@ -103,7 +146,7 @@ __global__ void __launch_bounds__(256)
 sp_gather_kernel(const int64_t* __restrict__ ptr, const int64_t* __restrict__ idx, const float* __restrict__ val,
                  const float* __restrict__ Fs, const float* __restrict__ Fo, int R, int64_t nseg, float* __restrict__ out,
                  double* __restrict__ loss_part) {
-  sp_gather<RPL, MODE>(ptr, idx, val, Fs, Fo, R, nseg, out, loss_part, 0.f, 0.f, 0.0, 0.0);
+  sp_gather<RPL, MODE>(ptr, idx, val, Fs, Fo, R, nseg, out, nullptr, loss_part, 0.f, 0.f, 0.0, 0.0);
 }
 
 // the modes of beta != 1, 2, with their constants
@@ -112,7 +155,16 @@ __global__ void __launch_bounds__(256)
 sp_gather_beta_kernel(const int64_t* __restrict__ ptr, const int64_t* __restrict__ idx, const float* __restrict__ val,
                       const float* __restrict__ Fs, const float* __restrict__ Fo, int R, int64_t nseg, float* __restrict__ out,
                       double* __restrict__ loss_part, float pa, float pb, double ca, double cb) {
-  sp_gather<RPL, MODE>(ptr, idx, val, Fs, Fo, R, nseg, out, loss_part, pa, pb, ca, cb);
+  sp_gather<RPL, MODE>(ptr, idx, val, Fs, Fo, R, nseg, out, nullptr, loss_part, pa, pb, ca, cb);
+}
+
+// the observed-cell modes (kSpObsTerms, kSpObsLoss) at beta mode BM; pa as sp_gather's
+template <int RPL, int MODE, int BM>
+__global__ void __launch_bounds__(256)
+sp_gather_obs_kernel(const int64_t* __restrict__ ptr, const int64_t* __restrict__ idx, const float* __restrict__ val,
+                     const float* __restrict__ Fs, const float* __restrict__ Fo, int R, int64_t nseg, float* __restrict__ num,
+                     float* __restrict__ den, double* __restrict__ loss_part, float pa) {
+  sp_gather<RPL, MODE, BM>(ptr, idx, val, Fs, Fo, R, nseg, num, den, loss_part, pa, 0.f, 0.0, 0.0);
 }
 
 // Gram matrix G = F^T F (R x R) of a (rows x R) factor: per-block slabs, then a fixed-order sum over the blocks
@@ -247,6 +299,30 @@ int launch_gather(const int64_t* ptr, const int64_t* idx, const float* val, cons
   return 0;
 }
 
+// The observed-cell gathers: MODE kSpObsTerms or kSpObsLoss, on the plan of launch_gather
+template <int MODE>
+int launch_observed(const int64_t* ptr, const int64_t* idx, const float* val, const float* Fs, const float* Fo, int R,
+                    int64_t nseg, double beta, float* num, float* den, double* loss_part, cudaStream_t st) {
+  const unsigned grid = (unsigned)sparse_gather_blocks(nseg);
+  const int rpl = sparse_rpl(R);
+  const float pa = (float)(MODE == kSpObsTerms ? beta - 1.0 : beta);
+  auto go = [&](auto bm) {
+    constexpr int BM = decltype(bm)::value;
+    if (rpl <= 1) sp_gather_obs_kernel<1, MODE, BM><<<grid, 256, 0, st>>>(ptr, idx, val, Fs, Fo, R, nseg, num, den, loss_part, pa);
+    else if (rpl <= 2) sp_gather_obs_kernel<2, MODE, BM><<<grid, 256, 0, st>>>(ptr, idx, val, Fs, Fo, R, nseg, num, den, loss_part, pa);
+    else if (rpl <= 4) sp_gather_obs_kernel<4, MODE, BM><<<grid, 256, 0, st>>>(ptr, idx, val, Fs, Fo, R, nseg, num, den, loss_part, pa);
+    else sp_gather_obs_kernel<8, MODE, BM><<<grid, 256, 0, st>>>(ptr, idx, val, Fs, Fo, R, nseg, num, den, loss_part, pa);
+  };
+  switch (beta_mode(beta)) {
+    case kKL: go(std::integral_constant<int, kKL>{}); break;
+    case kEU: go(std::integral_constant<int, kEU>{}); break;
+    case kIS: go(std::integral_constant<int, kIS>{}); break;
+    default: go(std::integral_constant<int, kGeneric>{}); break;
+  }
+  NMF_LAUNCH_CHECK();
+  return 0;
+}
+
 }  // namespace
 
 int64_t sparse_gram_part_floats(int R) { return (int64_t)128 * R * R; }
@@ -302,6 +378,25 @@ int sparse_beta_loss(const int64_t* crow, const int64_t* col, const float* val, 
                                       1.0 / (beta * (beta - 1.0)), 1.0 / (beta - 1.0));
   if (rc) return rc;
   sp_beta_loss_final_kernel<<<1, 256, 0, st>>>(loss_part, (int)sparse_gather_blocks(N), pos_part, npos, beta, loss_dev);
+  NMF_LAUNCH_CHECK();
+  return 0;
+}
+
+// Observed cells: both raw terms of one factor's update (num, den: nseg x R) over the compressed form whose segments are that
+// factor's rows
+int observed_terms(const int64_t* ptr, const int64_t* idx, const float* val, const float* Fself, const float* Fother, int R,
+                   int64_t nseg, double beta, float* num, float* den, cudaStream_t st) {
+  return launch_observed<kSpObsTerms>(ptr, idx, val, Fself, Fother, R, nseg, beta, num, den, nullptr, st);
+}
+
+// Observed cells: loss_dev = sum over the stored entries of metrics.beta_div's term, one partial per block over the CSR rows,
+// then a fixed-order sum
+int observed_loss(const int64_t* crow, const int64_t* col, const float* val, const float* H, const float* W, int R, int64_t N,
+                  double beta, double* loss_part, double* loss_dev, cudaStream_t st) {
+  int rc = launch_observed<kSpObsLoss>(crow, col, val, H, W, R, N, beta, nullptr, nullptr, loss_part, st);
+  if (rc) return rc;
+  // no V-free part: npos = 0, and the divisor 1 leaves the gather's sum as it is (at every beta, 0 included)
+  sp_beta_loss_final_kernel<<<1, 256, 0, st>>>(loss_part, (int)sparse_gather_blocks(N), nullptr, 0, 1.0, loss_dev);
   NMF_LAUNCH_CHECK();
   return 0;
 }

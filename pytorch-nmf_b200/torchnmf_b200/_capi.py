@@ -41,6 +41,7 @@ SIGNATURES = {
     "nmfb200_nmf_contract_only": (_int, [_vp, _vp, _vp, _int, _dbl, _vp]),
     "nmfb200_nmf_set_target_sparse": (_int, [_vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _dbl, _dbl, _vp]),
     "nmfb200_nmf_set_target_sparse_any_beta": (_int, [_vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _dbl, _dbl, _vp]),
+    "nmfb200_nmf_set_target_observed": (_int, [_vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "nmfb200_nmf_peer_supported": (_int, [_vp, _dbl]),
     "nmfb200_nmf_peer_alloc": (_int, [_vp, _vp]),
     "nmfb200_nmf_peer_connect": (_int, [_vp, _int, _int, _vp]),

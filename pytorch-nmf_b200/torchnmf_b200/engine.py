@@ -327,6 +327,20 @@ class CudaNmfEngine(_CudaEngine):
                                                         l2_reg, _stream(self.device)))
 
 
+def _compressed_forms(V):
+    """Both compressed forms of a coalesced sparse COO tensor V (N,C) on the device, built with torch (data-format plumbing):
+    (crow, col, val) = CSR, (ccol, row, val_t) = CSC, int64 indices and fp32 values, all contiguous."""
+    N, C = V.shape
+    vals = V.values().to(torch.float32).contiguous()
+    rows, cols = V.indices()[0].contiguous(), V.indices()[1].contiguous()          # coalesced: sorted by (row, col)
+    crow = torch.zeros(N + 1, dtype=torch.int64, device=vals.device)
+    crow[1:] = torch.cumsum(torch.bincount(rows, minlength=N), 0)
+    order = torch.argsort(cols * N + rows)                                         # the same entries sorted by (col, row)
+    ccol = torch.zeros(C + 1, dtype=torch.int64, device=vals.device)
+    ccol[1:] = torch.cumsum(torch.bincount(cols, minlength=C), 0)
+    return crow, cols, vals, ccol, rows[order].contiguous(), vals[order].contiguous()
+
+
 class CudaSparseNmfEngine(_CudaEngine):
     """NMF on a sparse target, beta 1 or 2 (reference: nmf.py:603-638): V is a coalesced sparse COO tensor (N,C) on the device;
     its CSR and CSC forms are built here with torch (data-format plumbing) and the update terms are evaluated at the non-zeros
@@ -345,16 +359,9 @@ class CudaSparseNmfEngine(_CudaEngine):
         assert W.shape == (C, R) and H.shape == (N, R)
         self.W, self.H = W, H
         self.N, self.C, self.R = N, C, R
-        vals = V.values().to(torch.float32).contiguous()
-        rows, cols = V.indices()[0].contiguous(), V.indices()[1].contiguous()      # coalesced: sorted by (row, col)
+        self._crow, self._col, self._val, self._ccol, self._row, self._val_t = _compressed_forms(V)
+        vals = self._val
         nnz = int(vals.numel())
-        self._crow = torch.zeros(N + 1, dtype=torch.int64, device=self.device)
-        self._crow[1:] = torch.cumsum(torch.bincount(rows, minlength=N), 0)
-        order = torch.argsort(cols * N + rows)                                     # the same entries sorted by (col, row)
-        self._ccol = torch.zeros(C + 1, dtype=torch.int64, device=self.device)
-        self._ccol[1:] = torch.cumsum(torch.bincount(cols, minlength=C), 0)
-        self._col, self._val = cols, vals
-        self._row, self._val_t = rows[order].contiguous(), vals[order].contiguous()
         v64 = vals.double()
         pos = v64[v64 > 0]
         self._vnorm_kl = float((pos * pos.log()).sum() - v64.sum())                # nmf.py:166-167 (0 log 0 = 0)
@@ -388,6 +395,42 @@ class CudaSparseAnyBetaEngine(CudaSparseNmfEngine):
     nmfb200_nmf_set_target_sparse_any_beta): beta 1 and 2 as CudaSparseNmfEngine; any other beta takes its numerators at the
     non-zeros and its denominators and loss from V-free dense contractions, so the device holds O(nnz + (N + C) R)."""
     _set_target = "nmfb200_nmf_set_target_sparse_any_beta"
+
+
+class CudaObservedNmfEngine(_CudaEngine):
+    """NMF on the observed cells of a masked fit (include/nmf_b200.h: nmfb200_nmf_set_target_observed), rank <= 256: O is a
+    coalesced fp32 sparse COO tensor (N,C) on the device whose stored entries are exactly the observed cells, explicit zeros
+    included, with V's values there.  The fit minimises beta_div(WH[obs], V[obs]) at every beta; every update and the loss
+    touch the observed cells only, O(observed x R) per update."""
+    kind = "nmf"
+
+    def __init__(self, O, W, H, precision="auto"):
+        super().__init__()
+        self.device = W.device
+        for t, n in ((W, "W"), (H, "H")):
+            _check_f32_cuda(t, n, self.device)
+        assert O.is_sparse and O.is_coalesced() and O.device == W.device
+        N, C = O.shape
+        R = W.shape[1]
+        assert W.shape == (C, R) and H.shape == (N, R)
+        self.W, self.H = W, H
+        self.N, self.C, self.R = N, C, R
+        self._crow, self._col, self._val, self._ccol, self._row, self._val_t = _compressed_forms(O)
+        dev_index = self.device.index if self.device.index is not None else torch.cuda.current_device()
+        self._acquire(("nmf", dev_index, N, C, R, "f32"),
+                      lambda ref: self._lib.nmfb200_nmf_create(ref, dev_index, N, C, R, _capi.PRECISIONS["f32"]))
+        self._loss = torch.zeros(1, dtype=torch.float64, device=self.device)
+        _capi.check(self._lib.nmfb200_nmf_set_target_observed(
+            self._ctx, int(self._val.numel()), _ptr(self._crow), _ptr(self._col), _ptr(self._val), _ptr(self._ccol),
+            _ptr(self._row), _ptr(self._val_t), _stream(self.device)))
+
+    def raw_terms(self, which, beta):
+        """(numerator, denominator) of the update of W (which=0) or H (which=1), both in the factor's shape at every beta."""
+        f = self.W if which == 0 else self.H
+        buf = self._raw_terms_into(which, beta, None)
+        return buf[:f.numel()].view(f.shape), buf[f.numel():].view(f.shape)
+
+    iterate = CudaNmfEngine.iterate
 
 
 class CudaNmfdEngine(_CudaEngine):

@@ -85,6 +85,30 @@ def _sparse_engine_cls(sparse_kernels, beta, rank, group):
     return _engine.CudaSparseNmfEngine if beta in (1, 2) else _engine.CudaSparseAnyBetaEngine
 
 
+def _observed_cells(V, M, device):
+    """The observed set of a sparse mask M on `device`: a coalesced fp32 sparse COO tensor of V's shape whose stored entries
+    are exactly the cells where M stores True (each once, explicit zeros kept), holding V's value there -- a dense V's element,
+    gathered at those cells only, or a sparse V's stored value (0 where V stores nothing).  Linear indices row * C + col in
+    int64, so N * C beyond 2^31 is fine."""
+    N, C = V.shape
+    M = M.to(device)
+    idx, keep = M._indices(), M._values()                      # uncoalesced masks too: duplicates collapse in unique()
+    lin = torch.unique(idx[0][keep] * C + idx[1][keep])        # sorted: the COO tensor is coalesced as built
+    rows, cols = lin // C, lin % C
+    if V.is_sparse:
+        Vc = V.coalesce()
+        vlin = (Vc.indices()[0] * C + Vc.indices()[1]).to(device)
+        vvals = Vc.values().to(device, torch.float32)
+        vals = torch.zeros(lin.numel(), dtype=torch.float32, device=device)
+        if vlin.numel():
+            pos = torch.searchsorted(vlin, lin).clamp_(max=vlin.numel() - 1)
+            hit = vlin[pos] == lin
+            vals = torch.where(hit, vvals[pos], vals)
+    else:
+        vals = V[rows.to(V.device), cols.to(V.device)].to(device, torch.float32)
+    return torch.sparse_coo_tensor(torch.stack([rows, cols]), vals, (N, C), is_coalesced=True, check_invariants=False)
+
+
 class _NullBar:
     def __init__(self, *a, **k): pass
     def __enter__(self): return self
@@ -180,7 +204,8 @@ class BaseComponent(torch.nn.Module):
         staged through fp32 device copies) and the engine for this target, with `mask` (validated by `_check_mask`) set on
         it: moved to the engine's device and made contiguous, read there in place as one byte per cell.
         Returns (engine, W, H, Wd, Hd, staged): W / H the Parameters, Wd / Hd the fp32 device tensors the engine updates."""
-        sparse_target = V.is_sparse
+        observed = mask is not None and mask.is_sparse       # a sparse mask: the observed-cell kernels (NMF, _check_mask)
+        sparse_target = V.is_sparse and not observed
         if sparse_target and not self._sparse_targets:
             raise NotImplementedError                      # nmf.py:294-295: only NMF derives the sparse update
         if sparse_target:
@@ -207,17 +232,31 @@ class BaseComponent(torch.nn.Module):
             f32 = torch.float32
             on_gpu = W.device.type == "cuda"
             dev = W.device if on_gpu else torch.device("cuda", torch.cuda.current_device())
-            Vd = V.to(dev, non_blocking=True)
-            sparse_cls = (_sparse_engine_cls(sparse_kernels and self._sparse_kernels, beta, W.shape[1], group)
-                          if sparse_target else None)
+            if observed:
+                # the observed cells up to rank 256 (sharded or not); above it, scattered into a dense fp32 V and a dense
+                # mask on the device, for the dense masked kernels
+                O = _observed_cells(V, mask, dev)
+                if W.shape[1] <= 256:
+                    Vd, sparse_cls, mask = O, _engine.CudaObservedNmfEngine, None
+                else:
+                    rows, cols = O.indices()
+                    Vd = torch.zeros(O.shape, dtype=f32, device=dev)
+                    Vd[rows, cols] = O.values()
+                    mask = torch.zeros(O.shape, dtype=torch.bool, device=dev)
+                    mask[rows, cols] = True
+                    sparse_cls = None
+            else:
+                Vd = V.to(dev, non_blocking=True)
+                sparse_cls = (_sparse_engine_cls(sparse_kernels and self._sparse_kernels, beta, W.shape[1], group)
+                              if sparse_target else None)
+                if not sparse_target and Vd.dtype in (torch.float16, torch.bfloat16):
+                    # the kernels convert each element exactly where they load it: the fit is bit for bit that of V.float(),
+                    # without the fp32 copy (4 bytes per element of V)
+                    if not (self._strided_target and Vd.stride(-1) == 1 and Vd.stride(0) >= Vd.shape[1]):
+                        Vd = Vd.contiguous()
+                elif sparse_cls is None:
+                    Vd = (Vd.to_dense() if sparse_target else Vd).to(f32).contiguous()
             use_sparse_kernels = sparse_cls is not None
-            if not sparse_target and Vd.dtype in (torch.float16, torch.bfloat16):
-                # the kernels convert each element exactly where they load it: the fit is bit for bit that of V.float(),
-                # without the fp32 copy (4 bytes per element of V)
-                if not (self._strided_target and Vd.stride(-1) == 1 and Vd.stride(0) >= Vd.shape[1]):
-                    Vd = Vd.contiguous()
-            elif not use_sparse_kernels:
-                Vd = (Vd.to_dense() if sparse_target else Vd).to(f32).contiguous()
             if on_gpu and W.dtype == f32 and H.dtype == f32:
                 Wd, Hd = W.data, H.data                       # updated in place, like param.data in the reference
             else:
@@ -230,8 +269,11 @@ class BaseComponent(torch.nn.Module):
             Md = mask.to(dev).contiguous() if mask is not None else None
         else:
             Wd, Hd = W.data, H.data
-            eng = self._engine_factory(V.to_dense() if (sparse_target and not sparse_kernels) else V, Wd, Hd)
-            Md = mask
+            if observed:
+                eng, Md = self._engine_factory(_observed_cells(V, mask, W.device), Wd, Hd), None
+            else:
+                eng = self._engine_factory(V.to_dense() if (sparse_target and not sparse_kernels) else V, Wd, Hd)
+                Md = mask
         if group is not None:
             eng = _engine.ShardedEngine(eng, group)
             if eng.kind == "nmfd":
@@ -252,12 +294,15 @@ class BaseComponent(torch.nn.Module):
                 raise
         return eng, W, H, Wd, Hd, staged
 
-    @staticmethod
-    def _check_mask(V, mask, precision):
+    @classmethod
+    def _check_mask(cls, V, mask, precision):
         """fit()'s checks of a mask that need no device pass."""
         if not isinstance(mask, Tensor) or mask.dtype != torch.bool:
             raise ValueError(f"mask must be a torch.bool tensor (got {getattr(mask, 'dtype', type(mask))})")
-        if V.is_sparse:
+        if mask.is_sparse:
+            if not cls._sparse_targets:
+                raise ValueError(f"mask: a sparse mask is supported by NMF only (got {cls.__name__}); pass a dense mask")
+        elif V.is_sparse:
             raise ValueError("mask: a masked fit needs a dense target")
         if tuple(mask.shape) != tuple(V.shape):
             raise ValueError(f"mask shape {tuple(mask.shape)} does not match the target's {tuple(V.shape)}")
@@ -303,6 +348,13 @@ class BaseComponent(torch.nn.Module):
                    H or W unchanged when alpha = 0.  Dense targets only (any dtype or row stride V may have), on the fp32
                    kernels: precision "auto" resolves to "f32", "f16" / "f16_split" raise ValueError.  With `group`, each
                    rank passes the mask shard of its V shard.
+                   NMF also takes a sparse COO torch.bool mask: the observed cells are the coordinates where it stores True
+                   (a coordinate listed twice counts once; stored False entries are not observed), and V -- dense of any
+                   dtype or row stride, or sparse COO (0 where it stores nothing; its entries outside the mask are ignored)
+                   -- is read at those cells only.  The objective is the same; up to rank 256 every update and the loss
+                   run on the observed cells alone, O(observed x R) per update and O(observed + (N + C) R) memory, for
+                   matrix completion where few cells are observed.  Above rank 256 the observed values and the mask are
+                   densified on the device.  With `group`, each rank passes the row shards of V and of the mask.
         """
         mask = options.pop("mask", None)
         if options:
