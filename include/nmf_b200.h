@@ -153,6 +153,16 @@ int nmfb200_nmf_set_target_sparse_any_beta(nmfb200_ctx* ctx, int64_t nnz, const 
 int nmfb200_nmf_set_target_observed(nmfb200_ctx* ctx, int64_t nnz, const int64_t* crow, const int64_t* col,
                                     const float* val, const int64_t* ccol, const int64_t* row, const float* val_t,
                                     void* stream);
+/* The same as nmfb200_nmf_set_target_observed, plus one fp32 weight per stored entry: wt in the order of val (CSR), wt_t in
+ * the order of val_t (CSC), device pointers borrowed like the rest (null only when nnz == 0, else NMFB200_ERR_INVALID).  The
+ * context then fits sum_obs w d_beta(v | x): each entry's terms in both gathers are multiplied by its weight,
+ *   num_H[n,:] = sum_c (w v) a(x) W[c,:]      den_H[n,:] = sum_c (w b(x)) W[c,:]      loss = sum_obs w loss_term,
+ * so at beta 1 den = the weighted rows of the other factor.  The weights should be positive and finite (an entry of weight 0
+ * is better left out).  Everything else -- the calls that follow it, the refusals, what turns it off -- is
+ * nmfb200_nmf_set_target_observed's.  Asynchronous. */
+int nmfb200_nmf_set_target_observed_weighted(nmfb200_ctx* ctx, int64_t nnz, const int64_t* crow, const int64_t* col,
+                                             const float* val, const int64_t* ccol, const int64_t* row, const float* val_t,
+                                             const float* wt, const float* wt_t, void* stream);
 
 /* Row-sharded W update over PEER MEMORY (ranks of one NVLink domain, one process per GPU, 2..8 ranks) -- the fused form of
  * raw_terms(which = 0) -> all-reduce -> w_apply below, without a collective library call on the data path:
@@ -246,6 +256,19 @@ int nmfb200_w_apply(nmfb200_ctx* ctx, float* W, const float* reduced, double bet
  * cells only) follow it; they run on the fp32 CUDA-core kernels (precision_for_beta reports NMFB200_PREC_F32,
  * nmf_peer_supported 0) and leave the tensor-core operand copies marked stale.  Asynchronous. */
 int nmfb200_set_mask(nmfb200_ctx* ctx, const uint8_t* M, void* stream);
+
+/* Fit a dense target with per-cell weights.  Wt: a DEVICE array of fp32 in V's shape, contiguous (NMF: N x C whatever V's
+ * ldv; the convolutive models: V's layout), borrowed like V; every weight finite and >= 0 (not checked here).  Same contract
+ * as nmfb200_set_mask: valid after a dense set_target (NMFB200_ERR_STATE before), NMFB200_ERR_INVALID on a sparse or
+ * observed-cell context; a null Wt, or any later set_target*, clears it; set_mask and set_weight replace each other.  While
+ * a weight is set the loss is sum_{w > 0} w d_beta(v | x), and every update is nmf.py:78-92 applied to the two backward
+ * passes of that loss: num = (w v x^(beta-2)) G, den = (w x^(beta-1)) G (beta 1: den = Wt G).  The kernels multiply where
+ * the mask kernels select: a cell of weight 0 is dropped, V is not read there (NaN, Inf or a negative value there gives
+ * the bits a zero gives), and a weight of exactly 1 gives the bits of a mask.  Every call that follows a mask follows the
+ * weight: update_w, update_h, nmf_iterate, loss, nmf_loss_prefetch_w (= loss), raw_terms (2 x the factor's numel at every
+ * beta), w_apply, contract_only and target_minmax (the cells with w != 0), on the fp32 CUDA-core kernels
+ * (precision_for_beta reports NMFB200_PREC_F32, nmf_peer_supported 0).  Asynchronous. */
+int nmfb200_set_weight(nmfb200_ctx* ctx, const float* Wt, void* stream);
 
 /* ---- tile plans of the fp32 CUDA-core kernels (host only: no device work, no allocation) -------- */
 

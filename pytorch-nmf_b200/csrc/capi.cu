@@ -29,9 +29,10 @@ struct nmfb200_ctx {
   int vdtype = NMFB200_DTYPE_F32;
   int64_t ldv = 0;
   bool has_target = false;
-  // nmfb200_set_mask: the observed cells (uint8, V's shape, contiguous), borrowed; cleared by every set_target*.  While set,
-  // every pass runs the masked fp32 kernels and beta 1 takes its denominators from the contraction, not the column sums.
-  const uint8_t* mask = nullptr;
+  // nmfb200_set_mask / nmfb200_set_weight: the observed cells (uint8) or the cells' weights (fp32), V's shape, contiguous,
+  // borrowed; cleared by every set_target*.  While set, every pass runs the selecting fp32 kernels and beta 1 takes its
+  // denominators from the contraction, not the column sums.
+  CellSel sel;
   // chunked partial numerators / denominators of the CUDA-core path
   float* num = nullptr;
   float* den = nullptr;
@@ -52,6 +53,7 @@ struct nmfb200_ctx {
   float* sp_den = nullptr;        // max(N, C) x R: the reduced V-free denominator of an update at beta != 1, 2
   const int64_t *sp_crow = nullptr, *sp_col = nullptr, *sp_ccol = nullptr, *sp_row = nullptr;
   const float *sp_val = nullptr, *sp_val_t = nullptr;
+  const float *sp_wt = nullptr, *sp_wt_t = nullptr;     // observed cells: the entries' weights in CSR / CSC order, or none
   double sp_vnorm_kl = 0.0, sp_vnorm_eu = 0.0;
   float* sp_gram = nullptr;       // [2][R*R] (W^T W, H^T H) + per-block partials
   double* sp_loss_part = nullptr;
@@ -148,13 +150,13 @@ int alloc_workspace(nmfb200_ctx* c, int64_t pn_floats) {
   return 0;
 }
 
-// beta 1 without a mask: the denominator is the column sum of the other factor (nmf.py:122-131).  A masked fit takes it
-// from the second backward pass, M G, like every other beta.
-bool kl_colsum(const nmfb200_ctx* c, double beta) { return beta == 1.0 && !c->mask && !c->observed; }
+// beta 1 without a mask: the denominator is the column sum of the other factor (nmf.py:122-131).  A masked or weighted fit
+// takes it from the second backward pass, M G, like every other beta.
+bool kl_colsum(const nmfb200_ctx* c, double beta) { return beta == 1.0 && !c->sel && !c->observed; }
 
 // Whether the context's own tensor-core kernels (c->tc: NMF, c->tcd: NMFD / NMF2D / NMF3D) serve this beta.
 bool use_tc(const nmfb200_ctx* c, double beta) {
-  if (c->tc_off || c->mask) return false;
+  if (c->tc_off || c->sel) return false;
   if (c->tc) return tc_supports_beta(c->tc, beta);
   return c->tcd != nullptr && tc_nmfd_supported(c->d, beta);
 }
@@ -337,7 +339,7 @@ int nmfb200_nmf_set_target(nmfb200_ctx* ctx, const void* V, int64_t ldv, int dty
   if (int rc = check_target(V, dtype)) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   ctx->V = V; ctx->vdtype = dtype; ctx->ldv = ldv; ctx->has_target = true; ctx->sparse = false; ctx->sp_any_beta = false;
-  ctx->observed = false; ctx->mask = nullptr;
+  ctx->observed = false; ctx->sel = CellSel{};
   float* minmax = ctx->mm_scratch + kMmPartials;
   int rc = matrix_minmax(V, dtype, ctx->N, ctx->C, ldv, ctx->mm_scratch, minmax, st);
   if (rc) return rc;
@@ -385,9 +387,10 @@ int nmfb200_nmf_set_target_sparse(nmfb200_ctx* ctx, int64_t nnz, const int64_t* 
   ctx->sp_crow = crow; ctx->sp_col = col; ctx->sp_val = val; ctx->sp_ccol = ccol; ctx->sp_row = row; ctx->sp_val_t = val_t;
   ctx->sp_vnorm_kl = v_norm_kl; ctx->sp_vnorm_eu = v_norm_eu;
   ctx->sparse = true; ctx->has_target = true; ctx->V = nullptr; ctx->tc_off = true;      // the dense kernels are out of play
-  ctx->mask = nullptr;
+  ctx->sel = CellSel{};
   ctx->sp_any_beta = false;
   ctx->observed = false;
+  ctx->sp_wt = ctx->sp_wt_t = nullptr;
   return 0;
 }
 
@@ -417,6 +420,16 @@ int nmfb200_nmf_set_target_observed(nmfb200_ctx* ctx, int64_t nnz, const int64_t
   // target_minmax: the observed values (none: +inf / -inf)
   return matrix_minmax(val, NMFB200_DTYPE_F32, 1, nnz, nnz, ctx->mm_scratch, ctx->mm_scratch + kMmPartials,
                        (cudaStream_t)stream);
+}
+
+int nmfb200_nmf_set_target_observed_weighted(nmfb200_ctx* ctx, int64_t nnz, const int64_t* crow, const int64_t* col,
+                                             const float* val, const int64_t* ccol, const int64_t* row, const float* val_t,
+                                             const float* wt, const float* wt_t, void* stream) {
+  if (nnz > 0 && (!wt || !wt_t)) return fail(NMFB200_ERR_INVALID, "bad entry weights");
+  int rc = nmfb200_nmf_set_target_observed(ctx, nnz, crow, col, val, ccol, row, val_t, stream);
+  if (rc) return rc;
+  ctx->sp_wt = wt; ctx->sp_wt_t = wt_t;
+  return 0;
 }
 
 /* ---- NMFD ------------------------------------------------------------------------------------ */
@@ -499,7 +512,7 @@ int nmfb200_nmfnd_create(nmfb200_ctx** out, int device, int64_t B, int64_t C, in
 int nmfb200_nmfd_set_target(nmfb200_ctx* ctx, const void* V, int dtype, void* stream) {
   CTX_GUARD(ctx, 1);
   if (int rc = check_target(V, dtype)) return rc;
-  ctx->V = V; ctx->vdtype = dtype; ctx->has_target = true; ctx->mask = nullptr;
+  ctx->V = V; ctx->vdtype = dtype; ctx->has_target = true; ctx->sel = CellSel{};
   cudaStream_t st = (cudaStream_t)stream;
   const int64_t vin = ctx->d.v_inner();
   int rc = matrix_minmax(V, dtype, (int64_t)ctx->d.B * ctx->d.C, vin, vin, ctx->mm_scratch, ctx->mm_scratch + kMmPartials, st);
@@ -550,20 +563,34 @@ int nmfb200_nmfnd_tc_plan(int64_t B, int64_t C, int ndim, const int64_t* vdims, 
   return 0;
 }
 
-/* ---- both kinds: the mask, and the terms of one factor update that every CUDA-core path runs on ------------ */
+/* ---- both kinds: the mask or weights, and the terms of one factor update that every CUDA-core path runs on --- */
 
-int nmfb200_set_mask(nmfb200_ctx* ctx, const uint8_t* M, void* stream) {
+namespace {
+// set_mask / set_weight: one selector replaces the other
+int set_selector(nmfb200_ctx* ctx, CellSel sel, void* stream) {
   CTX_GUARD(ctx, kAnyKind);
   TARGET_GUARD(ctx);
-  if (ctx->sparse) return fail(NMFB200_ERR_INVALID, "a mask needs a dense target (set_target or nmfd_set_target)");
+  if (ctx->sparse)
+    return fail(NMFB200_ERR_INVALID, std::string(sel.kind == kSelWeight ? "a weight" : "a mask") +
+                                         " needs a dense target (set_target or nmfd_set_target)");
   cudaStream_t st = (cudaStream_t)stream;
-  ctx->mask = M;
-  // the tensor-core paths are bypassed while a mask is set: their operand copies are rebuilt on their next use
+  ctx->sel = sel.p ? sel : CellSel{};
+  // the tensor-core paths are bypassed while a selector is set: their operand copies are rebuilt on their next use
   mark_stale(ctx, true, true);
-  float* minmax = ctx->mm_scratch + kMmPartials;          // target_minmax: the observed cells only, or all of V again
-  if (ctx->kind == 0) return matrix_minmax(ctx->V, ctx->vdtype, ctx->N, ctx->C, ctx->ldv, ctx->mm_scratch, minmax, st, M);
+  float* minmax = ctx->mm_scratch + kMmPartials;          // target_minmax: the selected cells only, or all of V again
+  if (ctx->kind == 0)
+    return matrix_minmax(ctx->V, ctx->vdtype, ctx->N, ctx->C, ctx->ldv, ctx->mm_scratch, minmax, st, ctx->sel);
   const int64_t vin = ctx->d.v_inner();
-  return matrix_minmax(ctx->V, ctx->vdtype, (int64_t)ctx->d.B * ctx->d.C, vin, vin, ctx->mm_scratch, minmax, st, M);
+  return matrix_minmax(ctx->V, ctx->vdtype, (int64_t)ctx->d.B * ctx->d.C, vin, vin, ctx->mm_scratch, minmax, st, ctx->sel);
+}
+}  // namespace
+
+int nmfb200_set_mask(nmfb200_ctx* ctx, const uint8_t* M, void* stream) {
+  return set_selector(ctx, CellSel{M, kSelMask}, stream);
+}
+
+int nmfb200_set_weight(nmfb200_ctx* ctx, const float* Wt, void* stream) {
+  return set_selector(ctx, CellSel{Wt, kSelWeight}, stream);
 }
 
 namespace {
@@ -589,7 +616,8 @@ int sparse_terms(nmfb200_ctx* ctx, int which, const float* F, const float* other
   const int64_t* ptr = which == 0 ? ctx->sp_ccol : ctx->sp_crow;
   const int64_t* idx = which == 0 ? ctx->sp_row : ctx->sp_col;
   const float* val = which == 0 ? ctx->sp_val_t : ctx->sp_val;
-  if (ctx->observed) return observed_terms(ptr, idx, val, F, other, R, f.rows, beta, num, den, st);
+  if (ctx->observed)
+    return observed_terms(ptr, idx, val, F, other, R, f.rows, beta, num, den, st, which == 0 ? ctx->sp_wt_t : ctx->sp_wt);
   int rc = sparse_numerator(ptr, idx, val, F, other, R, f.rows, beta, num, st);
   if (rc) return rc;
   if (beta != 1.0 && beta != 2.0) {     // the V-free denominator on the dense fp32 plan, its chunks summed as the dense path does
@@ -609,12 +637,12 @@ int sparse_terms(nmfb200_ctx* ctx, int which, const float* F, const float* other
 
 // CUDA-core contraction of one NMF factor update (which = 0: W, 1: H) into c->num / c->den (chunked partials).
 int simt_contract(nmfb200_ctx* c, int which, const float* W, const float* H, double beta, cudaStream_t st) {
-  if (beta != 1.0 || c->mask) { int e = ensure_den(c); if (e) return e; }
+  if (beta != 1.0 || c->sel) { int e = ensure_den(c); if (e) return e; }
   // W update: F = W (C rows), G = H (N rows), Vm = V^T;  H update: F = H (N rows), G = W (C rows), Vm = V
   const float* fac[2] = {W, H};
   const FactorDims f = factor_dims(c, which);
   return simt_nmf_contract(c->V, c->vdtype, c->ldv, /*trans=*/which == 0, fac[which], fac[1 - which], f.rows, f.other_rows,
-                           (int)c->R, beta, c->nslab[which], c->num, c->den, c->R, f.rows * c->R, c->mask, c->C, st);
+                           (int)c->R, beta, c->nslab[which], c->num, c->den, c->R, f.rows * c->R, c->sel, c->C, st);
 }
 
 // The same for NMFD / NMF2D / NMF3D: the ratio tiles Pn (and Pp), then their backward passes (wgrad for W, dgrad for H) into
@@ -626,7 +654,7 @@ int nmfd_contract(nmfb200_ctx* c, int which, const float* W, const float* H, dou
     int e = ensure_den(c);
     if (e) return e;
   }
-  int rc = nmfd_recon_phi(c->d, c->V, c->vdtype, W, H, beta, c->Pn, c->Pp, nullptr, 0, nullptr, st, c->mask);
+  int rc = nmfd_recon_phi(c->d, c->V, c->vdtype, W, H, beta, c->Pn, c->Pp, nullptr, 0, nullptr, st, c->sel);
   auto grad = [&](const float* P, float* out) {
     return which == 0 ? nmfd_wgrad(c->d, P, H, out, c->nslab[0], st) : nmfd_dgrad(c->d, P, W, out, c->nslab[1], st);
   };
@@ -699,7 +727,8 @@ int sparse_loss_ctx(nmfb200_ctx* ctx, const float* W, const float* H, double bet
   if (int rc = check_sparse_beta(ctx, beta)) return rc;
   const int R = (int)ctx->R;
   if (ctx->observed)                    // every cell's term at the observed cells, nothing elsewhere
-    return observed_loss(ctx->sp_crow, ctx->sp_col, ctx->sp_val, H, W, R, ctx->N, beta, ctx->sp_loss_part, loss_dev, st);
+    return observed_loss(ctx->sp_crow, ctx->sp_col, ctx->sp_val, H, W, R, ctx->N, beta, ctx->sp_loss_part, loss_dev, st,
+                         ctx->sp_wt);
   if (beta != 1.0 && beta != 2.0) {     // pos = sum x^beta over every cell without V, then V_norm - neg at the non-zeros
     int npos = 0;
     int rc = simt_nmf_pow_sum(H, W, ctx->N, ctx->C, R, beta, ctx->loss_blocks, ctx->loss_max_blocks, &npos, st);
@@ -849,12 +878,12 @@ int nmfb200_loss(nmfb200_ctx* ctx, const float* W, const float* H, double beta, 
   if (ctx->kind == 1) {
     if (use_tc(ctx, beta)) return tc_nmfd_recon(ctx->tcd, ctx->V, ctx->vdtype, W, H, true, loss_dev, st);
     return nmfd_recon_phi(ctx->d, ctx->V, ctx->vdtype, W, H, beta, nullptr, nullptr, ctx->loss_blocks, ctx->loss_max_blocks,
-                          loss_dev, st, ctx->mask);
+                          loss_dev, st, ctx->sel);
   }
   if (ctx->sparse) return sparse_loss_ctx(ctx, W, H, beta, loss_dev, st);
   if (use_tc(ctx, beta)) return tc_loss(ctx->tc, W, H, beta, loss_dev, st);
   return simt_nmf_loss(ctx->V, ctx->vdtype, ctx->ldv, H, W, ctx->N, ctx->C, (int)ctx->R, beta, ctx->loss_blocks,
-                       ctx->loss_max_blocks, loss_dev, ctx->mask, ctx->C, st);
+                       ctx->loss_max_blocks, loss_dev, ctx->sel, ctx->C, st);
 }
 
 int64_t nmfb200_raw_terms_numel(const nmfb200_ctx* ctx, int which, double beta) {

@@ -34,6 +34,34 @@ int with_vtype(const void* V, int dtype, F&& f) {
   return f(static_cast<const float*>(V));
 }
 
+// Per-cell selector of a dense fit (nmfb200_set_mask / nmfb200_set_weight): none, a uint8 mask (the kernels select the
+// observed cells) or fp32 weights (the kernels multiply each cell's terms by its weight, and drop the cells of weight 0).
+// Kernels take the selector's element type as a template parameter SEL: NoSel, uint8_t or float.
+enum SelKind : int { kSelNone = 0, kSelMask = 1, kSelWeight = 2 };
+struct NoSel {};
+struct CellSel {
+  const void* p = nullptr;
+  int kind = kSelNone;
+  explicit operator bool() const { return p != nullptr; }
+};
+template <class P>
+using sel_t = std::remove_cv_t<std::remove_pointer_t<P>>;
+template <class SEL>
+constexpr bool kWeighted = std::is_same<SEL, float>::value;
+// whether cell i takes part in the fit: always without a selector, else where M is non-zero
+template <class SEL>
+__device__ __forceinline__ bool sel_set(const SEL* M, int64_t i) {
+  if constexpr (std::is_same<SEL, NoSel>::value) return true;
+  else return M[i] != 0;
+}
+// Host dispatch: f(p) with p = the selector as `const NoSel*` (null), `const uint8_t*` or `const float*`
+template <class F>
+int with_sel(CellSel s, F&& f) {
+  if (s.p && s.kind == kSelWeight) return f(static_cast<const float*>(s.p));
+  if (s.p) return f(static_cast<const uint8_t*>(s.p));
+  return f(static_cast<const NoSel*>(nullptr));
+}
+
 // beta-divergence branch of nmf.py:61-74 / metrics.py:60-96
 enum BetaMode : int { kKL = 0, kEU = 1, kIS = 2, kGeneric = 3 };
 inline BetaMode beta_mode(double beta) {
@@ -61,6 +89,17 @@ __device__ __forceinline__ float loss_term(float v, float s, float beta) {
     float bm = beta - 1.0f;
     return (powf(t, beta) + bm * powf(x, beta) - beta * t * powf(x, bm)) / (beta * bm);
   }
+}
+
+// w * loss_term, with w folded into the product the caller's accumulation fuses with at beta 2, so that w = 1 gives the
+// bits of the unweighted term's accumulation and w = 2^k exactly 2^k times them
+template <int MODE>
+__device__ __forceinline__ float loss_term_w(float v, float s, float beta, float w) {
+  if (MODE == kEU) {
+    float d = s - v;
+    return (0.5f * w * d) * d;
+  }
+  return w * loss_term<MODE>(v, s, beta);
 }
 
 void set_error(const std::string& msg);
@@ -107,16 +146,17 @@ static inline bool grid_fits(const Grid3& g) {
 //   num[ch][m][r] = sum_{c in chunk ch} Pn[m,c] G[c,r]          [nmf.py:77]
 //   den[ch][m][r] = sum_{c in chunk ch} Pp[m,c] G[c,r]          [nmf.py:82, beta != 1 only]
 // Vm[m,c] = V[m*ldv + c] (trans = 0) or V[c*ldv + m] (trans = 1), elements of type `vdtype` (VDtype).  Any rank R >= 1.
-// M (optional, uint8, read like V with pitch ldm): a fit on the observed cells only -- Pn = Pp = 0 where M is 0, V is not
-// read there, and den is always formed (beta 1: Pp = M).  M == nullptr runs the unmasked kernels.
+// M (optional selector, read like V with pitch ldm): a fit on the observed cells only -- Pn = Pp = 0 where M is 0, V is not
+// read there, and den is always formed (beta 1: Pp = M).  A weight selector multiplies Pn and Pp by the cell's weight
+// (beta 1: Pp = the weight).  An empty M runs the unmasked kernels.
 int simt_nmf_contract(const void* V, int vdtype, int64_t ldv, int trans, const float* F, const float* G,
                       int64_t Mr, int64_t Nc, int R, double beta, int nchunks,
-                      float* num, float* den, int64_t ldp, int64_t chunk_stride, const uint8_t* M, int64_t ldm,
+                      float* num, float* den, int64_t ldp, int64_t chunk_stride, CellSel M, int64_t ldm,
                       cudaStream_t st);
 // beta_div(F G^T, Vm) accumulated into block partials then *loss_dev (double); over the cells where M (optional, pitch
-// ldm, not transposed) is set.
+// ldm, not transposed) is non-zero, each term times the cell's weight for a weight selector.
 int simt_nmf_loss(const void* V, int vdtype, int64_t ldv, const float* F, const float* G, int64_t Mr, int64_t Nc,
-                  int R, double beta, double* block_partials, int max_blocks, double* loss_dev, const uint8_t* M,
+                  int R, double beta, double* block_partials, int max_blocks, double* loss_dev, CellSel M,
                   int64_t ldm, cudaStream_t st);
 int simt_nmf_max_blocks(int64_t Mr, int64_t Nc);
 // The V-free pieces of a sparse target's update and loss at beta != 1, 2 (nmf.py:621-636):
@@ -158,9 +198,9 @@ int factor_colsum(const float* x, int64_t outer, int R, int64_t inner, float* sc
                   float* sums, cudaStream_t st);
 int64_t colsum_scratch_floats(int64_t outer, int R, int64_t inner);
 // min / max of a strided matrix of `vdtype` elements (fit()'s validation), results in mm[0..1]; with M (optional, contiguous
-// rows x cols uint8) over the cells where M is set only (none: +inf / -inf)
+// rows x cols selector) over the cells where M is non-zero only (none: +inf / -inf)
 int matrix_minmax(const void* V, int vdtype, int64_t rows, int64_t cols, int64_t ld, float* scratch2048, float* mm,
-                  cudaStream_t st, const uint8_t* M = nullptr);
+                  cudaStream_t st, CellSel M = CellSel{});
 // *out = sum of n doubles in fixed order (single block)
 int sum_partials(const double* p, int n, double* out, cudaStream_t st);
 
@@ -188,11 +228,12 @@ int sparse_beta_loss(const int64_t* crow, const int64_t* col, const float* val, 
                      cudaStream_t st);
 // Observed cells of a masked fit (the stored entries, zeros included), every beta: both raw terms of one factor's update in one
 // gather per segment (num, den: nseg x R), and loss_dev = beta_div(WH[obs], V[obs]) over the CSR form (loss_part: one double
-// per gather block over the N rows)
+// per gather block over the N rows).  wt (optional): one weight per stored entry, in the order of val -- each entry's
+// terms and loss term are multiplied by it.
 int observed_terms(const int64_t* ptr, const int64_t* idx, const float* val, const float* Fself, const float* Fother, int R,
-                   int64_t nseg, double beta, float* num, float* den, cudaStream_t st);
+                   int64_t nseg, double beta, float* num, float* den, cudaStream_t st, const float* wt = nullptr);
 int observed_loss(const int64_t* crow, const int64_t* col, const float* val, const float* H, const float* W, int R, int64_t N,
-                  double beta, double* loss_part, double* loss_dev, cudaStream_t st);
+                  double beta, double* loss_part, double* loss_dev, cudaStream_t st, const float* wt = nullptr);
 // launch plans (host only): rank floats per lane; blocks over nseg segments / rows (the loss: N, its partials); Gram rows per
 // block and blocks over `rows` rows; Gram passes of 4096 pairs
 int sparse_rpl(int R);
@@ -214,11 +255,12 @@ struct NmfdShape {
   __host__ __device__ bool one_d() const { return X1 == 1 && X2 == 1 && T1 == 1 && T2 == 1; }
 };
 // WH = conv(H, W); writes Pn (and Pp when beta != 1) (B,C,L) or, when loss_blocks != nullptr,
-// reduces beta_div(WH, V) instead.  M (optional, uint8 in V's layout): Pn = Pp = 0 at the missing cells and V is not read
-// there, Pp is written at every beta (beta 1: Pp = M as 0 / 1), and the loss skips them.
+// reduces beta_div(WH, V) instead.  M (optional selector in V's layout): Pn = Pp = 0 at the missing cells and V is not read
+// there, Pp is written at every beta (beta 1: Pp = M as 0 / 1), and the loss skips them; a weight selector also multiplies
+// Pn, Pp and the loss term by the cell's weight (beta 1: Pp = the weight).
 int nmfd_recon_phi(const NmfdShape& s, const void* V, int vdtype, const float* W, const float* H, double beta,
                    float* Pn, float* Pp, double* loss_blocks, int max_blocks, double* loss_dev,
-                   cudaStream_t st, const uint8_t* M = nullptr);
+                   cudaStream_t st, CellSel M = CellSel{});
 // batch elements per launch of the kernels that put the batch on grid.z (fp32 recon / dgrad, tensor-core recon / dgrad)
 static inline int64_t nmfd_batch_slice(int64_t B) { return B < kMaxGridYZ ? B : kMaxGridYZ; }
 // loss partials of nmfd_recon_phi: one per block of all its launches

@@ -78,16 +78,19 @@ struct SlideArgs {
   int64_t sm, sk;            // strides of A over m and k (elements); the offset (t1, t2, t) is contiguous
   int nsplit;                // !FWD: splits of k
   const void* V; float beta; float* Pn; float* Pp; double* block_partials;      // FWD epilogue (V: TV elements)
-  const uint8_t* mask;       // FWD, MASK: the observed cells (V's layout)
+  const void* mask;          // FWD, SEL: the observed cells or the weights (SEL elements, V's layout)
   float* out;                // !FWD: [split][B][R][h_inner]
   int b0;                    // first batch element of this launch
 };
 
-// MASK (FWD only): a fit on the observed cells -- at a missing cell V is not read, Pn = Pp = 0 and the loss adds nothing;
-// Pp is written at every beta (beta 1: the mask as 0 / 1), so wgrad / dgrad of Pp give the denominators
-template <int MT, bool FWD, int MODE, bool LOSS, typename TV, bool MASK = false>
+// SEL (FWD only): a fit on the observed cells -- at a missing cell V is not read, Pn = Pp = 0 and the loss adds nothing;
+// Pp is written at every beta (beta 1: the mask as 0 / 1), so wgrad / dgrad of Pp give the denominators.  A weighted fit
+// treats the cells of weight 0 as missing and multiplies Pn, Pp and the loss term by the weight elsewhere (beta 1: Pp = w).
+template <int MT, bool FWD, int MODE, bool LOSS, typename TV, typename SEL = NoSel>
 __global__ void __launch_bounds__(256)
 nmfd_slide_kernel(NmfdShape s, SlideArgs a) {
+  constexpr bool MASK = !std::is_same<SEL, NoSel>::value;
+  constexpr bool WEIGHT = kWeighted<SEL>;
   using G = Geo<MT>;
   constexpr int WIN = kLT + kTK;                          // window pitch per line (kLT + kTK - 1 elements used)
   __shared__ __align__(16) float As[kTK * G::PAD];        // As[tt][m]
@@ -189,7 +192,24 @@ nmfd_slide_kernel(NmfdShape s, SlideArgs a) {
         const int l = l0 + 4 * lt + j;
         if (c < s.C && l < s.L && o < OUT) {
           const int64_t off = (((int64_t)b * s.C + c) * OUT + o) * s.L + l;
-          if (MASK && !a.mask[off]) {
+          if constexpr (WEIGHT) {
+            const float w = static_cast<const float*>(a.mask)[off];
+            if (w == 0.f) {
+              if (!LOSS) { a.Pn[off] = 0.f; a.Pp[off] = 0.f; }
+              continue;
+            }
+            const float v = to_f32(static_cast<const TV*>(a.V)[off]);
+            if (LOSS) {
+              local += MODE == kEU ? loss_term_w<kEU>(v, acc[i][j], a.beta, w) : w * loss_term_d<MODE>(v, acc[i][j], a.beta);
+            } else {
+              float pn, pp;
+              phi_d<MODE>(v, acc[i][j], bm2, bm1, pn, pp);
+              a.Pn[off] = pn * w;
+              a.Pp[off] = MODE != kKL ? pp * w : w;
+            }
+            continue;
+          }
+          if (MASK && !static_cast<const uint8_t*>(a.mask)[off]) {
             if (!LOSS) { a.Pn[off] = 0.f; a.Pp[off] = 0.f; }
             continue;
           }
@@ -359,49 +379,40 @@ dim3 dim3_of(const Grid3& g) { return dim3((unsigned)g.x, (unsigned)g.y, (unsign
 
 
 // TV: the target's element type (FWD only; the dgrad pass reads no V and always takes float)
-template <int MT, bool FWD, typename TV>
+template <int MT, bool FWD, typename TV, typename SEL>
 void launch_slide(const NmfdShape& s, const SlideArgs& a, int mode, bool loss, dim3 grid, cudaStream_t st) {
   if (!FWD) { nmfd_slide_kernel<MT, false, kKL, false, float><<<grid, 256, 0, st>>>(s, a); return; }
-#define NMFD_GO(M, MK)                                                                  \
-  if (loss) nmfd_slide_kernel<MT, true, M, true, TV, MK><<<grid, 256, 0, st>>>(s, a);   \
-  else nmfd_slide_kernel<MT, true, M, false, TV, MK><<<grid, 256, 0, st>>>(s, a);
-  if (a.mask) {
-    switch (mode) {
-      case kKL: NMFD_GO(kKL, true); break;
-      case kEU: NMFD_GO(kEU, true); break;
-      case kIS: NMFD_GO(kIS, true); break;
-      default: NMFD_GO(kGeneric, true); break;
-    }
-  } else {
-    switch (mode) {
-      case kKL: NMFD_GO(kKL, false); break;
-      case kEU: NMFD_GO(kEU, false); break;
-      case kIS: NMFD_GO(kIS, false); break;
-      default: NMFD_GO(kGeneric, false); break;
-    }
+#define NMFD_GO(M)                                                                       \
+  if (loss) nmfd_slide_kernel<MT, true, M, true, TV, SEL><<<grid, 256, 0, st>>>(s, a);   \
+  else nmfd_slide_kernel<MT, true, M, false, TV, SEL><<<grid, 256, 0, st>>>(s, a);
+  switch (mode) {
+    case kKL: NMFD_GO(kKL); break;
+    case kEU: NMFD_GO(kEU); break;
+    case kIS: NMFD_GO(kIS); break;
+    default: NMFD_GO(kGeneric); break;
   }
 #undef NMFD_GO
 }
 
-template <bool FWD, typename TV>
+template <bool FWD, typename TV, typename SEL>
 void dispatch_slide(int mt, const NmfdShape& s, const SlideArgs& a, int mode, bool loss, dim3 grid, cudaStream_t st) {
   switch (mt) {
-    case 4: launch_slide<4, FWD, TV>(s, a, mode, loss, grid, st); break;
-    case 8: launch_slide<8, FWD, TV>(s, a, mode, loss, grid, st); break;
-    case 16: launch_slide<16, FWD, TV>(s, a, mode, loss, grid, st); break;
-    case 32: launch_slide<32, FWD, TV>(s, a, mode, loss, grid, st); break;
-    default: launch_slide<64, FWD, TV>(s, a, mode, loss, grid, st); break;
+    case 4: launch_slide<4, FWD, TV, SEL>(s, a, mode, loss, grid, st); break;
+    case 8: launch_slide<8, FWD, TV, SEL>(s, a, mode, loss, grid, st); break;
+    case 16: launch_slide<16, FWD, TV, SEL>(s, a, mode, loss, grid, st); break;
+    case 32: launch_slide<32, FWD, TV, SEL>(s, a, mode, loss, grid, st); break;
+    default: launch_slide<64, FWD, TV, SEL>(s, a, mode, loss, grid, st); break;
   }
 }
 
 // one launch of the sliding kernel per slice of at most kMaxGridYZ batch elements
-template <bool FWD, typename TV = float>
+template <bool FWD, typename TV = float, typename SEL = NoSel>
 int launch_slices(int mt, const NmfdShape& s, SlideArgs a, int mode, bool loss, const Grid3& g, cudaStream_t st) {
   for (int64_t b0 = 0; b0 < s.B; b0 += g.z) {
     a.b0 = (int)b0;
     dim3 grid = dim3_of(g);
     grid.z = (unsigned)std::min<int64_t>(g.z, s.B - b0);
-    dispatch_slide<FWD, TV>(mt, s, a, mode, loss, grid, st);
+    dispatch_slide<FWD, TV, SEL>(mt, s, a, mode, loss, grid, st);
     NMF_LAUNCH_CHECK();
   }
   return 0;
@@ -415,7 +426,7 @@ int64_t nmfd_max_blocks(const NmfdShape& s) {
 }
 
 int nmfd_recon_phi(const NmfdShape& s, const void* V, int vdtype, const float* W, const float* H, double beta, float* Pn,
-                   float* Pp, double* loss_blocks, int max_blocks, double* loss_dev, cudaStream_t st, const uint8_t* M) {
+                   float* Pp, double* loss_blocks, int max_blocks, double* loss_dev, cudaStream_t st, CellSel M) {
   const int mt = row_tile(s.C);
   const Grid3 grid = slide_grid(s, true, mt, s.C, 1);
   const int nblocks = (int)nmfd_max_blocks(s);          // create bounds it (nmfd_shape_of)
@@ -423,9 +434,11 @@ int nmfd_recon_phi(const NmfdShape& s, const void* V, int vdtype, const float* W
   if (loss && nblocks > max_blocks) { set_error("nmfd loss: partial buffer too small"); return 1; }
   SlideArgs a{};
   a.A = W; a.X = H; a.M = s.C; a.K = s.R; a.sm = (int64_t)s.R * s.w_inner(); a.sk = s.w_inner(); a.nsplit = 1;
-  a.V = V; a.beta = (float)beta; a.Pn = Pn; a.Pp = Pp; a.block_partials = loss_blocks; a.out = nullptr; a.mask = M;
+  a.V = V; a.beta = (float)beta; a.Pn = Pn; a.Pp = Pp; a.block_partials = loss_blocks; a.out = nullptr; a.mask = M.p;
   if (int rc = with_vtype(V, vdtype, [&](auto Vt) {
-        return launch_slices<true, vtype_t<decltype(Vt)>>(mt, s, a, beta_mode(beta), loss, grid, st);
+        return with_sel(M, [&](auto Mk) {
+          return launch_slices<true, vtype_t<decltype(Vt)>, sel_t<decltype(Mk)>>(mt, s, a, beta_mode(beta), loss, grid, st);
+        });
       }))
     return rc;
   if (loss) return sum_partials(loss_blocks, nblocks, loss_dev, st);

@@ -13,10 +13,11 @@
 // blocks the contraction does (nb + 1) / 2 (KL) or (nb + 2) / 3 (two outputs) times the minimal FLOPs.  With one block
 // (R <= 256) the kernel is the single-chunk kernel it always was: grid z = 1, F loaded once per CTA.
 //
-// MASK (a fit on the observed cells of V only): the kernel loads the uint8 mask tile beside the V tile, through the same
-// (possibly transposed) tile load, reads V only where the mask is set, and selects pn = pp = 0 at the missing cells.  It always
-// forms both outputs: at beta 1 pp is the mask itself (den = M G, not the column sums of G).  The unmasked instantiations
-// take no branch on it.
+// SEL (common.cuh), a fit on the observed cells of V only: the kernel loads the uint8 mask tile beside the V tile, through the
+// same (possibly transposed) tile load, reads V only where the mask is set, and selects pn = pp = 0 at the missing cells.  It
+// always forms both outputs: at beta 1 pp is the mask itself (den = M G, not the column sums of G).  A weighted fit loads the
+// fp32 weight tile the same way, reads V only where the weight is non-zero, and multiplies where the mask selects: pn *= w,
+// pp *= w, and pp = w at beta 1.  The unmasked instantiations (NoSel) take no branch on it.
 //
 // kVFree (sparse targets at beta != 1, 2): the contraction forms only den += (S+eps)^(beta-1) G_tile and reads no V, with
 // kGeneric's plan, staging and arithmetic, so its den partials equal kGeneric's bit for bit whatever V holds; the loss sums
@@ -81,12 +82,14 @@ __device__ __forceinline__ void phi(float v, float s, float bm2, float bm1, floa
   }
 }
 
-template <int RB, bool TRANS, int MODE, typename TV, bool MASK = false>
+template <int RB, bool TRANS, int MODE, typename TV, typename SEL = NoSel>
 __global__ void __launch_bounds__(256)
 simt_contract_kernel(const TV* __restrict__ V, int64_t ldv, const float* __restrict__ F,
                      const float* __restrict__ G, int64_t Mr, int64_t Nc, int R, float bm2, float bm1,
                      int nchunks, float* __restrict__ num, float* __restrict__ den, int64_t ldp,
-                     int64_t chunk_stride, const uint8_t* __restrict__ Mk, int64_t ldm) {
+                     int64_t chunk_stride, const SEL* __restrict__ Mk, int64_t ldm) {
+  constexpr bool MASK = !std::is_same<SEL, NoSel>::value;
+  constexpr bool WEIGHT = kWeighted<SEL>;
   constexpr int Rp = 16 * RB;
   constexpr bool kDenOnly = (MODE == kVFree);
   constexpr bool kNum = !kDenOnly;
@@ -95,7 +98,7 @@ simt_contract_kernel(const TV* __restrict__ V, int64_t ldv, const float* __restr
   float* Fs = smem;                 // [Rp][kLd]  Fs[r][row]
   float* Gs = Fs + Rp * kLd;        // [Rp][kLd]  Gs[r][col]
   float* Ps = Gs + Rp * kLd;        // [64][kLd]  V tile, then Pn in place
-  float* Qs = kDenOnly ? Ps : Ps + kTile * kLd;     // [64][kLd]  Pp (kTwo only; kVFree: in Ps's place); MASK: the mask first
+  float* Qs = kDenOnly ? Ps : Ps + kTile * kLd;     // [64][kLd]  Pp (kTwo only; kVFree: in Ps's place); MASK: the selector first
 
   const int tid = threadIdx.x;
   const int tx = tid & 15, ty = tid >> 4;
@@ -141,8 +144,12 @@ simt_contract_kernel(const TV* __restrict__ V, int64_t ldv, const float* __restr
             col = a; row = b;
           }
           const bool in = m0 + row < Mr && c0 + col < Nc;
-          if (!MASK) {
+          if constexpr (!MASK) {
             if (in) val = to_f32(TRANS ? V[(c0 + col) * ldv + m0 + row] : V[(m0 + row) * ldv + c0 + col]);
+          } else if constexpr (WEIGHT) {
+            const float w = in ? (TRANS ? Mk[(c0 + col) * ldm + m0 + row] : Mk[(m0 + row) * ldm + c0 + col]) : 0.f;
+            if (w != 0.f) val = to_f32(TRANS ? V[(c0 + col) * ldv + m0 + row] : V[(m0 + row) * ldv + c0 + col]);
+            Qs[row * kLd + col] = w;
           } else {
             const bool seen = in && (TRANS ? Mk[(c0 + col) * ldm + m0 + row] : Mk[(m0 + row) * ldm + c0 + col]) != 0;
             if (seen) val = to_f32(TRANS ? V[(c0 + col) * ldv + m0 + row] : V[(m0 + row) * ldv + c0 + col]);
@@ -179,8 +186,13 @@ simt_contract_kernel(const TV* __restrict__ V, int64_t ldv, const float* __restr
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
           const bool seen = mv[j] != 0.f;
-          pn[j] = seen ? pn[j] : 0.f;
-          pp[j] = MODE == kKL ? mv[j] : (seen ? pp[j] : 0.f);
+          if constexpr (WEIGHT) {
+            pn[j] = seen ? pn[j] * mv[j] : 0.f;
+            pp[j] = MODE == kKL ? mv[j] : (seen ? pp[j] * mv[j] : 0.f);
+          } else {
+            pn[j] = seen ? pn[j] : 0.f;
+            pp[j] = MODE == kKL ? mv[j] : (seen ? pp[j] : 0.f);
+          }
         }
       }
       *reinterpret_cast<float4*>(&Ps[(4 * ty + i) * kLd + 4 * tx]) = make_float4(pn[0], pn[1], pn[2], pn[3]);
@@ -226,14 +238,14 @@ simt_contract_kernel(const TV* __restrict__ V, int64_t ldv, const float* __restr
   }
 }
 
-template <int RB, bool TRANS, typename TV, bool MASK>
+template <int RB, bool TRANS, typename TV, typename SEL>
 int launch_contract_mode(int mode, dim3 grid, size_t smem, cudaStream_t st, const TV* V, int64_t ldv,
                          const float* F, const float* G, int64_t Mr, int64_t Nc, int R, float bm2, float bm1,
-                         int nchunks, float* num, float* den, int64_t ldp, int64_t chunk_stride, const uint8_t* Mk,
+                         int nchunks, float* num, float* den, int64_t ldp, int64_t chunk_stride, const SEL* Mk,
                          int64_t ldm) {
 #define NMF_LAUNCH_MODE(M)                                                                              \
   {                                                                                                     \
-    auto kern = simt_contract_kernel<RB, TRANS, M, TV, MASK>;                                           \
+    auto kern = simt_contract_kernel<RB, TRANS, M, TV, SEL>;                                            \
     NMF_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
     kern<<<grid, 256, smem, st>>>(V, ldv, F, G, Mr, Nc, R, bm2, bm1, nchunks, num, den, ldp,            \
                                   chunk_stride, Mk, ldm);                                               \
@@ -249,18 +261,19 @@ int launch_contract_mode(int mode, dim3 grid, size_t smem, cudaStream_t st, cons
   return 0;
 }
 
-template <int RB, typename TV, bool MASK>
+template <int RB, typename TV, typename SEL>
 int launch_contract_rb(int trans, int mode, dim3 grid, cudaStream_t st, const TV* V, int64_t ldv,
                        const float* F, const float* G, int64_t Mr, int64_t Nc, int R, float bm2, float bm1,
-                       int nchunks, float* num, float* den, int64_t ldp, int64_t chunk_stride, const uint8_t* Mk,
+                       int nchunks, float* num, float* den, int64_t ldp, int64_t chunk_stride, const SEL* Mk,
                        int64_t ldm) {
   const int Rp = 16 * RB;
+  constexpr bool MASK = !std::is_same<SEL, NoSel>::value;
   size_t smem = (size_t)(2 * Rp + kTile * (mode == kKL && !MASK ? 1 : 2)) * kLd * sizeof(float);
   if (trans)
-    return launch_contract_mode<RB, true, TV, MASK>(mode, grid, smem, st, V, ldv, F, G, Mr, Nc, R, bm2, bm1, nchunks,
-                                                    num, den, ldp, chunk_stride, Mk, ldm);
-  return launch_contract_mode<RB, false, TV, MASK>(mode, grid, smem, st, V, ldv, F, G, Mr, Nc, R, bm2, bm1, nchunks, num,
-                                                   den, ldp, chunk_stride, Mk, ldm);
+    return launch_contract_mode<RB, true, TV, SEL>(mode, grid, smem, st, V, ldv, F, G, Mr, Nc, R, bm2, bm1, nchunks,
+                                                   num, den, ldp, chunk_stride, Mk, ldm);
+  return launch_contract_mode<RB, false, TV, SEL>(mode, grid, smem, st, V, ldv, F, G, Mr, Nc, R, bm2, bm1, nchunks, num,
+                                                  den, ldp, chunk_stride, Mk, ldm);
 }
 
 // ---- loss ------------------------------------------------------------------------------------
@@ -279,13 +292,13 @@ __device__ __forceinline__ double block_reduce_sum(double v, double* sh) {
   return t;   // valid in warp 0
 }
 
-// MASK: the sum runs over the observed cells only (the missing ones are dropped, not zeroed: at beta != 0, 1, 2 a zeroed
-// cell would still add eps^beta / beta)
-template <int MODE, typename TV, bool MASK = false>
+// SEL: the sum runs over the observed cells only (the missing ones are dropped, not zeroed: at beta != 0, 1, 2 a zeroed
+// cell would still add eps^beta / beta); a weighted fit adds w * term over the cells with w != 0
+template <int MODE, typename TV, typename SEL = NoSel>
 __global__ void __launch_bounds__(256)
 simt_loss_kernel(const TV* __restrict__ V, int64_t ldv, const float* __restrict__ F,
                  const float* __restrict__ G, int64_t Mr, int64_t Nc, int R, int Rp, float beta, int nchunks,
-                 double* __restrict__ block_partials, const uint8_t* __restrict__ Mk, int64_t ldm) {
+                 double* __restrict__ block_partials, const SEL* __restrict__ Mk, int64_t ldm) {
   extern __shared__ __align__(16) float smem[];
   float* Fs = smem;
   float* Gs = Fs + Rp * kLd;
@@ -323,7 +336,10 @@ simt_loss_kernel(const TV* __restrict__ V, int64_t ldv, const float* __restrict_
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
         int64_t col = c0 + 4 * tx + j;
-        if (row < Mr && col < Nc && (!MASK || Mk[row * ldm + col])) {
+        if constexpr (kWeighted<SEL>) {
+          const float w = row < Mr && col < Nc ? Mk[row * ldm + col] : 0.f;
+          if (w != 0.f) local += loss_term_w<MODE>(to_f32(V[row * ldv + col]), s[i][j], beta, w);
+        } else if (row < Mr && col < Nc && sel_set(Mk, row * ldm + col)) {
           if (MODE == kVFree) local += powf(s[i][j] + kEps, beta);       // nmf.py:635-636, before the division by beta
           else local += loss_term<MODE>(to_f32(V[row * ldv + col]), s[i][j], beta);
         }
@@ -372,7 +388,7 @@ int sum_partials(const double* p, int n, double* out, cudaStream_t st) {
 
 int simt_nmf_contract(const void* V, int vdtype, int64_t ldv, int trans, const float* F, const float* G, int64_t Mr,
                       int64_t Nc, int R, double beta, int nchunks, float* num, float* den, int64_t ldp,
-                      int64_t chunk_stride, const uint8_t* M, int64_t ldm, cudaStream_t st) {
+                      int64_t chunk_stride, CellSel M, int64_t ldm, cudaStream_t st) {
   if (R < 1) { set_error("simt_nmf_contract: rank must be positive"); return 1; }
   int mode = beta_mode(beta);
   float bm2 = (float)(beta - 2.0), bm1 = (float)(beta - 1.0);
@@ -380,24 +396,25 @@ int simt_nmf_contract(const void* V, int vdtype, int64_t ldv, int trans, const f
   const int rb = contract_rb(R);
   return with_vtype(V, vdtype, [&](auto Vt) {
     using TV = vtype_t<decltype(Vt)>;
-#define NMF_RB(RBV)                                                                                                  \
-  return M ? launch_contract_rb<RBV, TV, true>(trans, mode, grid, st, Vt, ldv, F, G, Mr, Nc, R, bm2, bm1, nchunks, num, \
-                                               den, ldp, chunk_stride, M, ldm)                                          \
-           : launch_contract_rb<RBV, TV, false>(trans, mode, grid, st, Vt, ldv, F, G, Mr, Nc, R, bm2, bm1, nchunks, num, \
-                                                den, ldp, chunk_stride, nullptr, 0)
-    switch (rb) {
-      case 1: NMF_RB(1);
-      case 2: NMF_RB(2);
-      case 4: NMF_RB(4);
-      case 8: NMF_RB(8);
-      default: NMF_RB(16);
-    }
+    return with_sel(M, [&](auto Mk) {
+      using SEL = sel_t<decltype(Mk)>;
+#define NMF_RB(RBV)                                                                                                     \
+  return launch_contract_rb<RBV, TV, SEL>(trans, mode, grid, st, Vt, ldv, F, G, Mr, Nc, R, bm2, bm1, nchunks, num, den, \
+                                          ldp, chunk_stride, Mk, M ? ldm : 0)
+      switch (rb) {
+        case 1: NMF_RB(1);
+        case 2: NMF_RB(2);
+        case 4: NMF_RB(4);
+        case 8: NMF_RB(8);
+        default: NMF_RB(16);
+      }
 #undef NMF_RB
+    });
   });
 }
 
 int simt_nmf_loss(const void* V, int vdtype, int64_t ldv, const float* F, const float* G, int64_t Mr, int64_t Nc, int R,
-                  double beta, double* block_partials, int max_blocks, double* loss_dev, const uint8_t* M, int64_t ldm,
+                  double beta, double* block_partials, int max_blocks, double* loss_dev, CellSel M, int64_t ldm,
                   cudaStream_t st) {
   if (R < 1) { set_error("simt_nmf_loss: rank must be positive"); return 1; }
   int nchunks = loss_chunks(Mr, Nc);
@@ -409,30 +426,24 @@ int simt_nmf_loss(const void* V, int vdtype, int64_t ldv, const float* F, const 
   int mode = beta_mode(beta);
   int rc = with_vtype(V, vdtype, [&](auto Vt) {
     using TV = vtype_t<decltype(Vt)>;
-#define NMF_LOSS(MD, MK)                                                                                          \
-  {                                                                                                               \
-    auto kern = simt_loss_kernel<MD, TV, MK>;                                                                     \
-    NMF_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));           \
-    kern<<<grid, 256, smem, st>>>(Vt, ldv, F, G, Mr, Nc, R, Rp, (float)beta, nchunks, block_partials, M, ldm);  \
+    return with_sel(M, [&](auto Mk) {
+      using SEL = sel_t<decltype(Mk)>;
+#define NMF_LOSS(MD)                                                                                                        \
+  {                                                                                                                         \
+    auto kern = simt_loss_kernel<MD, TV, SEL>;                                                                              \
+    NMF_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));                     \
+    kern<<<grid, 256, smem, st>>>(Vt, ldv, F, G, Mr, Nc, R, Rp, (float)beta, nchunks, block_partials, Mk, M ? ldm : 0);    \
   }
-    if (M) {
       switch (mode) {
-        case kKL: NMF_LOSS(kKL, true); break;
-        case kEU: NMF_LOSS(kEU, true); break;
-        case kIS: NMF_LOSS(kIS, true); break;
-        default: NMF_LOSS(kGeneric, true); break;
+        case kKL: NMF_LOSS(kKL); break;
+        case kEU: NMF_LOSS(kEU); break;
+        case kIS: NMF_LOSS(kIS); break;
+        default: NMF_LOSS(kGeneric); break;
       }
-    } else {
-      switch (mode) {
-        case kKL: NMF_LOSS(kKL, false); break;
-        case kEU: NMF_LOSS(kEU, false); break;
-        case kIS: NMF_LOSS(kIS, false); break;
-        default: NMF_LOSS(kGeneric, false); break;
-      }
-    }
 #undef NMF_LOSS
-    NMF_LAUNCH_CHECK();
-    return 0;
+      NMF_LAUNCH_CHECK();
+      return 0;
+    });
   });
   if (rc) return rc;
   return sum_partials(block_partials, nblocks, loss_dev, st);

@@ -22,7 +22,9 @@
 //   num[s,:] = sum_j v a(x) w_j      den[s,:] = sum_j b(x) w_j
 //   beta 2: a = 1, b = x;  beta 1: a = 1 / (x + eps), b = 1;  beta 0: a = 1 / (x + eps)^2, b = 1 / (x + eps);
 //   other:  b = (x + eps)^(beta - 1) from one powf, a = b / (x + eps)
-// and the loss gather sums metrics.beta_div's per-cell term (loss_term) at each stored entry, in double.
+// and the loss gather sums metrics.beta_div's per-cell term (loss_term) at each stored entry, in double.  A weighted fit
+// (nmfb200_nmf_set_target_observed_weighted) reads one weight w per entry beside its value, in the same order:
+//   num[s,:] = sum_j (w v) a(x) w_j      den[s,:] = sum_j (w b(x)) w_j      loss = sum_j w loss_term
 #include "common.cuh"
 
 namespace nmfb200 {
@@ -54,12 +56,14 @@ __device__ __forceinline__ void obs_phi(float x, float bm1, float& a, float& b) 
 }
 
 // pa, pb, ca, cb: the beta constants of kSpBeta / kSpBetaLoss (unused by the other modes); kSpObsTerms: pa = beta - 1,
-// den_out the denominator (nseg x R); kSpObsLoss: pa = beta.  BM: the beta mode of the two observed-cell modes.
-template <int RPL, int MODE, int BM = kKL>
+// den_out the denominator (nseg x R); kSpObsLoss: pa = beta.  BM: the beta mode of the two observed-cell modes; WT: they
+// read the entries' weights wt (in val's order).
+template <int RPL, int MODE, int BM = kKL, bool WT = false>
 __device__ __forceinline__ void
 sp_gather(const int64_t* __restrict__ ptr, const int64_t* __restrict__ idx, const float* __restrict__ val,
           const float* __restrict__ Fs, const float* __restrict__ Fo, int R, int64_t nseg, float* __restrict__ out,
-          float* __restrict__ den_out, double* __restrict__ loss_part, float pa, float pb, double ca, double cb) {
+          float* __restrict__ den_out, double* __restrict__ loss_part, float pa, float pb, double ca, double cb,
+          const float* __restrict__ wt = nullptr) {
   const int lane = threadIdx.x & 31;
   const int64_t seg = (int64_t)blockIdx.x * 8 + (threadIdx.x >> 5);
   double lacc = 0.0;
@@ -106,14 +110,22 @@ sp_gather(const int64_t* __restrict__ ptr, const int64_t* __restrict__ idx, cons
       } else if (MODE == kSpObsTerms) {
         float a, b;
         obs_phi<BM>(dot, pa, a, b);
-        const float ratio = v * a;
+        float ratio;
+        if constexpr (WT) {
+          const float we = wt[e];
+          ratio = (we * v) * a;
+          b = we * b;
+        } else {
+          ratio = v * a;
+        }
 #pragma unroll
         for (int k = 0; k < RPL; ++k) {
           acc[k] = fmaf(ratio, w[k], acc[k]);
           dacc[k] = fmaf(b, w[k], dacc[k]);
         }
       } else if (MODE == kSpObsLoss) {
-        lacc += (double)loss_term<BM>(v, dot, pa);                   // metrics.py:60-96 at this cell
+        if constexpr (WT) lacc += (double)(wt[e] * loss_term<BM>(v, dot, pa));
+        else lacc += (double)loss_term<BM>(v, dot, pa);              // metrics.py:60-96 at this cell
       } else if (MODE == kSpKLLoss) {
         lacc += (double)(v * logf(dot + kEps));                      // nmf.py:619
       } else {
@@ -158,13 +170,13 @@ sp_gather_beta_kernel(const int64_t* __restrict__ ptr, const int64_t* __restrict
   sp_gather<RPL, MODE>(ptr, idx, val, Fs, Fo, R, nseg, out, nullptr, loss_part, pa, pb, ca, cb);
 }
 
-// the observed-cell modes (kSpObsTerms, kSpObsLoss) at beta mode BM; pa as sp_gather's
-template <int RPL, int MODE, int BM>
+// the observed-cell modes (kSpObsTerms, kSpObsLoss) at beta mode BM; pa as sp_gather's; WT: with the entries' weights wt
+template <int RPL, int MODE, int BM, bool WT>
 __global__ void __launch_bounds__(256)
 sp_gather_obs_kernel(const int64_t* __restrict__ ptr, const int64_t* __restrict__ idx, const float* __restrict__ val,
                      const float* __restrict__ Fs, const float* __restrict__ Fo, int R, int64_t nseg, float* __restrict__ num,
-                     float* __restrict__ den, double* __restrict__ loss_part, float pa) {
-  sp_gather<RPL, MODE, BM>(ptr, idx, val, Fs, Fo, R, nseg, num, den, loss_part, pa, 0.f, 0.0, 0.0);
+                     float* __restrict__ den, double* __restrict__ loss_part, float pa, const float* __restrict__ wt) {
+  sp_gather<RPL, MODE, BM, WT>(ptr, idx, val, Fs, Fo, R, nseg, num, den, loss_part, pa, 0.f, 0.0, 0.0, wt);
 }
 
 // Gram matrix G = F^T F (R x R) of a (rows x R) factor: per-block slabs, then a fixed-order sum over the blocks
@@ -299,26 +311,35 @@ int launch_gather(const int64_t* ptr, const int64_t* idx, const float* val, cons
   return 0;
 }
 
-// The observed-cell gathers: MODE kSpObsTerms or kSpObsLoss, on the plan of launch_gather
+// The observed-cell gathers: MODE kSpObsTerms or kSpObsLoss, on the plan of launch_gather; wt (optional) the entries' weights
 template <int MODE>
 int launch_observed(const int64_t* ptr, const int64_t* idx, const float* val, const float* Fs, const float* Fo, int R,
-                    int64_t nseg, double beta, float* num, float* den, double* loss_part, cudaStream_t st) {
+                    int64_t nseg, double beta, float* num, float* den, double* loss_part, cudaStream_t st,
+                    const float* wt) {
   const unsigned grid = (unsigned)sparse_gather_blocks(nseg);
   const int rpl = sparse_rpl(R);
   const float pa = (float)(MODE == kSpObsTerms ? beta - 1.0 : beta);
-  auto go = [&](auto bm) {
+  auto go = [&](auto bm, auto weighted) {
     constexpr int BM = decltype(bm)::value;
-    if (rpl <= 1) sp_gather_obs_kernel<1, MODE, BM><<<grid, 256, 0, st>>>(ptr, idx, val, Fs, Fo, R, nseg, num, den, loss_part, pa);
-    else if (rpl <= 2) sp_gather_obs_kernel<2, MODE, BM><<<grid, 256, 0, st>>>(ptr, idx, val, Fs, Fo, R, nseg, num, den, loss_part, pa);
-    else if (rpl <= 4) sp_gather_obs_kernel<4, MODE, BM><<<grid, 256, 0, st>>>(ptr, idx, val, Fs, Fo, R, nseg, num, den, loss_part, pa);
-    else sp_gather_obs_kernel<8, MODE, BM><<<grid, 256, 0, st>>>(ptr, idx, val, Fs, Fo, R, nseg, num, den, loss_part, pa);
+    constexpr bool WT = decltype(weighted)::value;
+#define NMF_OBS(RPLV) \
+  sp_gather_obs_kernel<RPLV, MODE, BM, WT><<<grid, 256, 0, st>>>(ptr, idx, val, Fs, Fo, R, nseg, num, den, loss_part, pa, wt)
+    if (rpl <= 1) NMF_OBS(1);
+    else if (rpl <= 2) NMF_OBS(2);
+    else if (rpl <= 4) NMF_OBS(4);
+    else NMF_OBS(8);
+#undef NMF_OBS
   };
-  switch (beta_mode(beta)) {
-    case kKL: go(std::integral_constant<int, kKL>{}); break;
-    case kEU: go(std::integral_constant<int, kEU>{}); break;
-    case kIS: go(std::integral_constant<int, kIS>{}); break;
-    default: go(std::integral_constant<int, kGeneric>{}); break;
-  }
+  auto by_beta = [&](auto weighted) {
+    switch (beta_mode(beta)) {
+      case kKL: go(std::integral_constant<int, kKL>{}, weighted); break;
+      case kEU: go(std::integral_constant<int, kEU>{}, weighted); break;
+      case kIS: go(std::integral_constant<int, kIS>{}, weighted); break;
+      default: go(std::integral_constant<int, kGeneric>{}, weighted); break;
+    }
+  };
+  if (wt) by_beta(std::true_type{});
+  else by_beta(std::false_type{});
   NMF_LAUNCH_CHECK();
   return 0;
 }
@@ -385,15 +406,15 @@ int sparse_beta_loss(const int64_t* crow, const int64_t* col, const float* val, 
 // Observed cells: both raw terms of one factor's update (num, den: nseg x R) over the compressed form whose segments are that
 // factor's rows
 int observed_terms(const int64_t* ptr, const int64_t* idx, const float* val, const float* Fself, const float* Fother, int R,
-                   int64_t nseg, double beta, float* num, float* den, cudaStream_t st) {
-  return launch_observed<kSpObsTerms>(ptr, idx, val, Fself, Fother, R, nseg, beta, num, den, nullptr, st);
+                   int64_t nseg, double beta, float* num, float* den, cudaStream_t st, const float* wt) {
+  return launch_observed<kSpObsTerms>(ptr, idx, val, Fself, Fother, R, nseg, beta, num, den, nullptr, st, wt);
 }
 
 // Observed cells: loss_dev = sum over the stored entries of metrics.beta_div's term, one partial per block over the CSR rows,
 // then a fixed-order sum
 int observed_loss(const int64_t* crow, const int64_t* col, const float* val, const float* H, const float* W, int R, int64_t N,
-                  double beta, double* loss_part, double* loss_dev, cudaStream_t st) {
-  int rc = launch_observed<kSpObsLoss>(crow, col, val, H, W, R, N, beta, nullptr, nullptr, loss_part, st);
+                  double beta, double* loss_part, double* loss_dev, cudaStream_t st, const float* wt) {
+  int rc = launch_observed<kSpObsLoss>(crow, col, val, H, W, R, N, beta, nullptr, nullptr, loss_part, st, wt);
   if (rc) return rc;
   // no V-free part: npos = 0, and the divisor 1 leaves the gather's sum as it is (at every beta, 0 included)
   sp_beta_loss_final_kernel<<<1, 256, 0, st>>>(loss_part, (int)sparse_gather_blocks(N), nullptr, 0, 1.0, loss_dev);

@@ -123,16 +123,16 @@ __device__ __forceinline__ float nan_min(float a, float b) { return (a != a || b
 __device__ __forceinline__ float nan_max(float a, float b) { return (a != a || b != b) ? NAN : fmaxf(a, b); }
 
 // NaN-sticky min / max so that a NaN in V fails fit()'s non-negativity assertion like torch.all(V >= 0) does
-// MASK: the cells where M (contiguous rows x cols) is 0 are skipped, V is not read there
-template <typename TV, bool MASK = false>
+// SEL: the cells where M (contiguous rows x cols: a mask or weights) is 0 are skipped, V is not read there
+template <typename TV, typename SEL = NoSel>
 __global__ void __launch_bounds__(256)
 minmax_stage1(const TV* __restrict__ V, int64_t rows, int64_t cols, int64_t ld, float* __restrict__ scratch,
-              const uint8_t* __restrict__ M) {
+              const SEL* __restrict__ M) {
   __shared__ float smin[8], smax[8];
   float mn = INFINITY, mx = -INFINITY;
   const int64_t total = rows * cols;
   for (int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x; i < total; i += (int64_t)gridDim.x * 256) {
-    if (MASK && !M[i]) continue;
+    if (!sel_set(M, i)) continue;
     int64_t r = i / cols, c = i - r * cols;
     float v = to_f32(V[r * ld + c]);
     mn = nan_min(mn, v);
@@ -263,16 +263,17 @@ int factor_colsum(const float* x, int64_t outer, int R, int64_t inner, float* sc
 }
 
 int matrix_minmax(const void* V, int vdtype, int64_t rows, int64_t cols, int64_t ld, float* scratch2048, float* mm,
-                  cudaStream_t st, const uint8_t* M) {
+                  cudaStream_t st, CellSel M) {
   int64_t nb = ceil_div(rows * cols, 256 * 16);
   if (nb > 1024) nb = 1024;
   if (nb < 1) nb = 1;
   int rc = with_vtype(V, vdtype, [&](auto Vt) {
     using TV = vtype_t<decltype(Vt)>;
-    if (M) minmax_stage1<TV, true><<<(unsigned)nb, 256, 0, st>>>(Vt, rows, cols, ld, scratch2048, M);
-    else minmax_stage1<TV, false><<<(unsigned)nb, 256, 0, st>>>(Vt, rows, cols, ld, scratch2048, nullptr);
-    NMF_LAUNCH_CHECK();
-    return 0;
+    return with_sel(M, [&](auto Mk) {
+      minmax_stage1<TV, sel_t<decltype(Mk)>><<<(unsigned)nb, 256, 0, st>>>(Vt, rows, cols, ld, scratch2048, Mk);
+      NMF_LAUNCH_CHECK();
+      return 0;
+    });
   });
   if (rc) return rc;
   minmax_stage2<<<1, 32, 0, st>>>(scratch2048, (int)nb, mm);

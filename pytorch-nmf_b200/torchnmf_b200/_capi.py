@@ -42,6 +42,7 @@ SIGNATURES = {
     "nmfb200_nmf_set_target_sparse": (_int, [_vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _dbl, _dbl, _vp]),
     "nmfb200_nmf_set_target_sparse_any_beta": (_int, [_vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _dbl, _dbl, _vp]),
     "nmfb200_nmf_set_target_observed": (_int, [_vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "nmfb200_nmf_set_target_observed_weighted": (_int, [_vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "nmfb200_nmf_peer_supported": (_int, [_vp, _dbl]),
     "nmfb200_nmf_peer_alloc": (_int, [_vp, _vp]),
     "nmfb200_nmf_peer_connect": (_int, [_vp, _int, _int, _vp]),
@@ -58,6 +59,7 @@ SIGNATURES = {
     "nmfb200_raw_terms": (_int, [_vp, _vp, _vp, _int, _dbl, _vp, _vp]),
     "nmfb200_w_apply": (_int, [_vp, _vp, _vp, _dbl, _dbl, _dbl, _dbl, _vp]),
     "nmfb200_set_mask": (_int, [_vp, _vp, _vp]),
+    "nmfb200_set_weight": (_int, [_vp, _vp, _vp]),
     "nmfb200_hoyer_project": (_int, [_int, _vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp]),
     "nmfb200_nmf_plan": (_int, [_i64, _i64, _i64, _c.POINTER(_i64), _int]),
     "nmfb200_nmfd_plan": (_int, [_i64, _i64, _int, _c.POINTER(_i64), _i64, _c.POINTER(_i64), _c.POINTER(_i64), _int]),

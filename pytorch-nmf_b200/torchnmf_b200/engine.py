@@ -134,6 +134,7 @@ class _CudaEngine:
         self._key = None
         self._wbuf = None
         self._mask = None
+        self._weight = None
 
     def _acquire(self, key, create):
         """Take a cached context for `key` or create one with `create(ctx_ref)`."""
@@ -180,8 +181,21 @@ class _CudaEngine:
                 raise ValueError("the mask must be a contiguous bool tensor on the engine's device")
             if tuple(M.shape) != tuple(self.V.shape):
                 raise ValueError(f"the mask's shape {tuple(M.shape)} does not match V's {tuple(self.V.shape)}")
-        self._mask = M
+        self._mask, self._weight = M, None
         _capi.check(self._lib.nmfb200_set_mask(self._ctx, _ptr(M) if M is not None else None, _stream(self.device)))
+
+    def set_weight(self, Wt):
+        """Fit with per-cell weights from now on (include/nmf_b200.h: nmfb200_set_weight): Wt is a contiguous float32 tensor
+        of V's shape on the engine's device, read in place, every weight finite and >= 0 (fit() checks the values); None
+        clears it.  Replaces a mask, and a mask replaces it.  The engine keeps a reference to Wt while it is set.  minmax()
+        then covers the cells of non-zero weight only."""
+        if Wt is not None:
+            if Wt.dtype != torch.float32 or Wt.device != self.device or not Wt.is_contiguous():
+                raise ValueError("the weight must be a contiguous float32 tensor on the engine's device")
+            if tuple(Wt.shape) != tuple(self.V.shape):
+                raise ValueError(f"the weight's shape {tuple(Wt.shape)} does not match V's {tuple(self.V.shape)}")
+        self._mask, self._weight = None, Wt
+        _capi.check(self._lib.nmfb200_set_weight(self._ctx, _ptr(Wt) if Wt is not None else None, _stream(self.device)))
 
     def minmax(self):
         vmin, vmax = ctypes.c_float(), ctypes.c_float()
@@ -216,13 +230,13 @@ class _CudaEngine:
 
     def raw_terms(self, which, beta):
         """(numerator, denominator) of the update of W (which=0) or H (which=1) from the CURRENT factors, untouched: the
-        numerator in the factor's shape; the denominator (R,) for beta == 1 without a mask (the column sums of the other
-        factor), else in the factor's shape.  What BetaMu.step and PLCA.fit are built from (include/nmf_b200.h:
+        numerator in the factor's shape; the denominator (R,) for beta == 1 without a mask or weight (the column sums of the
+        other factor), else in the factor's shape.  What BetaMu.step and PLCA.fit are built from (include/nmf_b200.h:
         nmfb200_raw_terms)."""
         f = self.W if which == 0 else self.H
         buf = self._raw_terms_into(which, beta, None)
         num, den = buf[:f.numel()].view(f.shape), buf[f.numel():]
-        return num, (den if beta == 1 and self._mask is None else den.view(f.shape))
+        return num, (den if beta == 1 and self._mask is None and self._weight is None else den.view(f.shape))
 
     def _raw_terms_into(self, which, beta, buf):
         """nmfb200_raw_terms flat into `buf`, or into a new buffer when `buf` is None or of another size; returns it."""
@@ -327,9 +341,10 @@ class CudaNmfEngine(_CudaEngine):
                                                         l2_reg, _stream(self.device)))
 
 
-def _compressed_forms(V):
+def _compressed_forms(V, weights=None):
     """Both compressed forms of a coalesced sparse COO tensor V (N,C) on the device, built with torch (data-format plumbing):
-    (crow, col, val) = CSR, (ccol, row, val_t) = CSC, int64 indices and fp32 values, all contiguous."""
+    (crow, col, val) = CSR, (ccol, row, val_t) = CSC, int64 indices and fp32 values, all contiguous.  With `weights` (one
+    per stored entry, in V's order) also (wt, wt_t): the weights in CSR and in CSC order."""
     N, C = V.shape
     vals = V.values().to(torch.float32).contiguous()
     rows, cols = V.indices()[0].contiguous(), V.indices()[1].contiguous()          # coalesced: sorted by (row, col)
@@ -338,7 +353,11 @@ def _compressed_forms(V):
     order = torch.argsort(cols * N + rows)                                         # the same entries sorted by (col, row)
     ccol = torch.zeros(C + 1, dtype=torch.int64, device=vals.device)
     ccol[1:] = torch.cumsum(torch.bincount(cols, minlength=C), 0)
-    return crow, cols, vals, ccol, rows[order].contiguous(), vals[order].contiguous()
+    forms = (crow, cols, vals, ccol, rows[order].contiguous(), vals[order].contiguous())
+    if weights is None:
+        return forms
+    wt = weights.to(torch.float32).contiguous()
+    return forms + (wt, wt[order].contiguous())
 
 
 class CudaSparseNmfEngine(_CudaEngine):
@@ -401,10 +420,11 @@ class CudaObservedNmfEngine(_CudaEngine):
     """NMF on the observed cells of a masked fit (include/nmf_b200.h: nmfb200_nmf_set_target_observed), rank <= 256: O is a
     coalesced fp32 sparse COO tensor (N,C) on the device whose stored entries are exactly the observed cells, explicit zeros
     included, with V's values there.  The fit minimises beta_div(WH[obs], V[obs]) at every beta; every update and the loss
-    touch the observed cells only, O(observed x R) per update."""
+    touch the observed cells only, O(observed x R) per update.  `weights` (optional, one positive fp32 weight per stored entry
+    of O, in O's order): the fit minimises sum_obs w d_beta(v | WH) instead (nmfb200_nmf_set_target_observed_weighted)."""
     kind = "nmf"
 
-    def __init__(self, O, W, H, precision="auto"):
+    def __init__(self, O, W, H, precision="auto", weights=None):
         super().__init__()
         self.device = W.device
         for t, n in ((W, "W"), (H, "H")):
@@ -415,14 +435,22 @@ class CudaObservedNmfEngine(_CudaEngine):
         assert W.shape == (C, R) and H.shape == (N, R)
         self.W, self.H = W, H
         self.N, self.C, self.R = N, C, R
-        self._crow, self._col, self._val, self._ccol, self._row, self._val_t = _compressed_forms(O)
+        if weights is not None:
+            assert weights.shape == (O._nnz(),) and weights.device == W.device
+        forms = _compressed_forms(O, weights)
+        self._crow, self._col, self._val, self._ccol, self._row, self._val_t = forms[:6]
         dev_index = self.device.index if self.device.index is not None else torch.cuda.current_device()
         self._acquire(("nmf", dev_index, N, C, R, "f32"),
                       lambda ref: self._lib.nmfb200_nmf_create(ref, dev_index, N, C, R, _capi.PRECISIONS["f32"]))
         self._loss = torch.zeros(1, dtype=torch.float64, device=self.device)
-        _capi.check(self._lib.nmfb200_nmf_set_target_observed(
-            self._ctx, int(self._val.numel()), _ptr(self._crow), _ptr(self._col), _ptr(self._val), _ptr(self._ccol),
-            _ptr(self._row), _ptr(self._val_t), _stream(self.device)))
+        args = (self._ctx, int(self._val.numel()), _ptr(self._crow), _ptr(self._col), _ptr(self._val), _ptr(self._ccol),
+                _ptr(self._row), _ptr(self._val_t))
+        if weights is None:
+            _capi.check(self._lib.nmfb200_nmf_set_target_observed(*args, _stream(self.device)))
+        else:
+            self._wt, self._wt_t = forms[6:]
+            _capi.check(self._lib.nmfb200_nmf_set_target_observed_weighted(*args, _ptr(self._wt), _ptr(self._wt_t),
+                                                                           _stream(self.device)))
 
     def raw_terms(self, which, beta):
         """(numerator, denominator) of the update of W (which=0) or H (which=1), both in the factor's shape at every beta."""
@@ -498,6 +526,10 @@ class ShardedEngine:
         """This rank's shard of the mask (the rows / batch elements of its V shard)."""
         self.local.set_mask(M)
 
+    def set_weight(self, Wt):
+        """This rank's shard of the weight (the rows / batch elements of its V shard)."""
+        self.local.set_weight(Wt)
+
     def minmax(self):
         vmin, vmax = self.local.minmax()
         t = torch.tensor([-vmin, vmax], dtype=torch.float32, device=self._reduce_device())
@@ -510,6 +542,12 @@ class ShardedEngine:
     def _reduce_device(self):
         dev = getattr(self.local, "device", None)
         return dev if dev is not None else torch.device("cpu")
+
+    def all_ranks(self, flag):
+        """Collective: whether `flag` holds on every rank (one MIN all-reduce)."""
+        t = torch.tensor([int(bool(flag))], dtype=torch.int32, device=self._reduce_device())
+        self._dist.all_reduce(t, op=self._dist.ReduceOp.MIN, group=self.group)
+        return bool(t.item())
 
     def check_same_sizes(self, names, sizes):
         """Collective: raise ValueError on every rank unless every rank passed the same `sizes` (ints; `names` label them

@@ -94,6 +94,28 @@ def _observed_cells(V, M, device):
     M = M.to(device)
     idx, keep = M._indices(), M._values()                      # uncoalesced masks too: duplicates collapse in unique()
     lin = torch.unique(idx[0][keep] * C + idx[1][keep])        # sorted: the COO tensor is coalesced as built
+    return _cells_of(V, lin, device)
+
+
+def _weighted_cells(Wt, C, device):
+    """The observed set of a sparse weight Wt (N, C) on `device`: (sorted linear indices row * C + col, fp32 weights there)
+    of the cells whose weight is > 0, and whether every weight is valid (`_weight_values_ok` over every stored entry as
+    given, before duplicates are summed, and over the sums).  Duplicate coordinates add up, as in `Wt.to_dense()`; stored
+    zeros are dropped."""
+    Wt = Wt.to(device)
+    Wc = Wt.coalesce()
+    w = Wc.values().to(torch.float32)
+    ok = _weight_values_ok(torch.cat([Wt._values().to(torch.float32), w]))
+    keep = w > 0
+    idx = Wc.indices()
+    return idx[0][keep] * C + idx[1][keep], w[keep].contiguous(), ok
+
+
+def _cells_of(V, lin, device):
+    """A coalesced fp32 sparse COO tensor of V's shape storing V's value at the cells `lin` (sorted linear indices, each
+    once; explicit zeros kept): a dense V's element, gathered there only, or a sparse V's stored value (0 where V stores
+    nothing)."""
+    N, C = V.shape
     rows, cols = lin // C, lin % C
     if V.is_sparse:
         Vc = V.coalesce()
@@ -107,6 +129,16 @@ def _observed_cells(V, M, device):
     else:
         vals = V[rows.to(V.device), cols.to(V.device)].to(device, torch.float32)
     return torch.sparse_coo_tensor(torch.stack([rows, cols]), vals, (N, C), is_coalesced=True, check_invariants=False)
+
+
+def _weight_values_ok(w):
+    """One reduction over a weight's values (fp32, on its device): whether every weight is finite and >= 0.  No value (an
+    empty shard) is fine; a weight that is zero everywhere is refused by fit() after the (collective) min / max of V over
+    the weighted cells, as a mask with nothing observed is."""
+    if w.numel() == 0:
+        return True
+    lo, hi = torch.stack(torch.aminmax(w)).tolist()
+    return lo >= 0 and hi < math.inf                         # NaN fails both
 
 
 class _NullBar:
@@ -198,13 +230,17 @@ class BaseComponent(torch.nn.Module):
     _sparse_kernels = True        # a sparse target on the library's sparse kernels (False: densify)
     _strided_target = False       # the engine reads a row-strided (unit column stride) half-precision target as it is
 
-    def _open_engine(self, V, beta, precision, group, sparse_kernels, mask=None):
+    def _open_engine(self, V, beta, precision, group, sparse_kernels, mask=None, weight=None):
         """Shared entry of `fit` / `sparse_fit`: validation that needs no device pass, placement of V / W / H on the CUDA
         device (host buffers are copied there; a dense bf16 / fp16 target keeps its dtype, other target and factor dtypes are
         staged through fp32 device copies) and the engine for this target, with `mask` (validated by `_check_mask`) set on
-        it: moved to the engine's device and made contiguous, read there in place as one byte per cell.
+        it: moved to the engine's device and made contiguous, read there in place as one byte per cell.  A `weight`
+        (validated by `_check_weight`) is set the same way as one fp32 per cell (other dtypes staged through one fp32 copy),
+        after one reduction over its values (`_weight_values_ok`, agreed on by every rank with `group`, so that all of
+        them raise together); a sparse one takes the observed-cell kernels.
         Returns (engine, W, H, Wd, Hd, staged): W / H the Parameters, Wd / Hd the fp32 device tensors the engine updates."""
-        observed = mask is not None and mask.is_sparse       # a sparse mask: the observed-cell kernels (NMF, _check_mask)
+        wsparse = weight is not None and weight.is_sparse    # a sparse weight: the observed-cell kernels (NMF, _check_weight)
+        observed = (mask is not None and mask.is_sparse) or wsparse
         sparse_target = V.is_sparse and not observed
         if sparse_target and not self._sparse_targets:
             raise NotImplementedError                      # nmf.py:294-295: only NMF derives the sparse update
@@ -232,18 +268,29 @@ class BaseComponent(torch.nn.Module):
             f32 = torch.float32
             on_gpu = W.device.type == "cuda"
             dev = W.device if on_gpu else torch.device("cuda", torch.cuda.current_device())
+            wv = None
+            wok = True
             if observed:
                 # the observed cells up to rank 256 (sharded or not); above it, scattered into a dense fp32 V and a dense
-                # mask on the device, for the dense masked kernels
-                O = _observed_cells(V, mask, dev)
+                # mask (or weight) on the device, for the dense masked (weighted) kernels
+                if wsparse:
+                    lin, wv, wok = _weighted_cells(weight, V.shape[1], dev)
+                    O = _cells_of(V, lin, dev)
+                else:
+                    O = _observed_cells(V, mask, dev)
                 if W.shape[1] <= 256:
-                    Vd, sparse_cls, mask = O, _engine.CudaObservedNmfEngine, None
+                    Vd, sparse_cls, mask, weight = O, _engine.CudaObservedNmfEngine, None, None
                 else:
                     rows, cols = O.indices()
                     Vd = torch.zeros(O.shape, dtype=f32, device=dev)
                     Vd[rows, cols] = O.values()
-                    mask = torch.zeros(O.shape, dtype=torch.bool, device=dev)
-                    mask[rows, cols] = True
+                    if wsparse:
+                        weight = torch.zeros(O.shape, dtype=f32, device=dev)
+                        weight[rows, cols] = wv
+                        wv = None
+                    else:
+                        mask = torch.zeros(O.shape, dtype=torch.bool, device=dev)
+                        mask[rows, cols] = True
                     sparse_cls = None
             else:
                 Vd = V.to(dev, non_blocking=True)
@@ -265,13 +312,26 @@ class BaseComponent(torch.nn.Module):
                 Hd = H.data.to(dev, f32, non_blocking=True).contiguous()
             if not Wd.is_contiguous() or not Hd.is_contiguous():
                 raise ValueError("W and H must be contiguous")
-            eng = sparse_cls(Vd.coalesce(), Wd, Hd) if use_sparse_kernels else self._build_engine(Vd, Wd, Hd, precision)
+            if weight is not None and not wsparse:
+                weight = weight.to(dev, f32).contiguous()
+                wok = _weight_values_ok(weight)
+            if wv is not None:
+                eng = sparse_cls(Vd.coalesce(), Wd, Hd, weights=wv)
+            else:
+                eng = sparse_cls(Vd.coalesce(), Wd, Hd) if use_sparse_kernels else self._build_engine(Vd, Wd, Hd, precision)
             Md = mask.to(dev).contiguous() if mask is not None else None
         else:
             Wd, Hd = W.data, H.data
-            if observed:
+            wok = True
+            if wsparse:
+                lin, wv, wok = _weighted_cells(weight, V.shape[1], W.device)
+                eng, Md, weight = self._engine_factory(_cells_of(V, lin, W.device), Wd, Hd, weights=wv), None, None
+            elif observed:
                 eng, Md = self._engine_factory(_observed_cells(V, mask, W.device), Wd, Hd), None
             else:
+                if weight is not None:
+                    weight = weight.to(torch.float32).contiguous()
+                    wok = _weight_values_ok(weight)
                 eng = self._engine_factory(V.to_dense() if (sparse_target and not sparse_kernels) else V, Wd, Hd)
                 Md = mask
         if group is not None:
@@ -286,9 +346,17 @@ class BaseComponent(torch.nn.Module):
                 except ValueError:
                     eng.close()
                     raise
-        if Md is not None:
+            if wsparse or weight is not None:
+                wok = eng.all_ranks(wok)          # collective: a bad weight on any rank makes every rank raise
+        if not wok:
+            eng.close()
+            raise ValueError("weight: every weight must be finite and >= 0 (found a negative, NaN or Inf weight)")
+        if Md is not None or weight is not None:
             try:
-                eng.set_mask(Md)
+                if Md is not None:
+                    eng.set_mask(Md)
+                else:
+                    eng.set_weight(weight)
             except Exception:
                 eng.close()
                 raise
@@ -308,6 +376,22 @@ class BaseComponent(torch.nn.Module):
             raise ValueError(f"mask shape {tuple(mask.shape)} does not match the target's {tuple(V.shape)}")
         if precision in ("f16", "f16_split"):
             raise ValueError(f"mask: masked fits run on the fp32 kernels; precision must be 'auto' or 'f32' (got {precision!r})")
+
+    @classmethod
+    def _check_weight(cls, V, weight, precision):
+        """fit()'s checks of a weight that need no device pass (the values: `_weight_values_ok`)."""
+        if not isinstance(weight, Tensor) or not weight.dtype.is_floating_point:
+            raise ValueError(f"weight must be a floating-point tensor (got {getattr(weight, 'dtype', type(weight))})")
+        if weight.is_sparse:
+            if not cls._sparse_targets:
+                raise ValueError(f"weight: a sparse weight is supported by NMF only (got {cls.__name__}); pass a dense weight")
+        elif V.is_sparse:
+            raise ValueError("weight: a dense weight needs a dense target (pass a sparse weight for a sparse target)")
+        if tuple(weight.shape) != tuple(V.shape):
+            raise ValueError(f"weight shape {tuple(weight.shape)} does not match the target's {tuple(V.shape)}")
+        if precision in ("f16", "f16_split"):
+            raise ValueError(f"weight: weighted fits run on the fp32 kernels; precision must be 'auto' or 'f32' "
+                             f"(got {precision!r})")
 
     @torch.no_grad()
     def fit(self, V, beta=1, tol=1e-4, max_iter=200, verbose=False, alpha=0, l1_ratio=0, *,
@@ -355,19 +439,50 @@ class BaseComponent(torch.nn.Module):
                    run on the observed cells alone, O(observed x R) per update and O(observed + (N + C) R) memory, for
                    matrix completion where few cells are observed.  Above rank 256 the observed values and the mask are
                    densified on the device.  With `group`, each rank passes the row shards of V and of the mask.
+
+        weight:    (keyword-only, default None, through **options like `mask`; exclusive with it -- fold a mask into the
+                   weight) a floating-point tensor of V's shape holding one weight w >= 0 per cell: the fit minimises
+                   sum over the cells with w > 0 of w * d_beta(v | WH), with every update the reference's ratio
+                   (nmf.py:78-92) of the two backward passes of that loss (num = contraction of w V (WH + eps)^(beta-2),
+                   den = of w (WH + eps)^(beta-1); at beta 1 den is the weighted contraction, not the column sums).  The
+                   loss reported and used by the stop rule is sqrt(2 sum w d_beta), summed over ranks with `group`.
+                   Confidence weights, per-bin reliabilities or inverse noise variances are the usual uses; weights in
+                   {0, 1} give exactly the fit of the mask `weight > 0`.  Cells of weight 0 are dropped as missing cells
+                   are for a mask: V is never read there, and the non-negativity and beta <= 0 checks look at the cells
+                   with w > 0 only.  ValueError: a non-floating weight, a shape mismatch, any negative, NaN or Inf weight
+                   (one reduction at entry; a sparse weight's stored entries are checked before duplicates are summed),
+                   a weight that is zero everywhere, precision "f16" / "f16_split" ("auto" resolves to "f32").  A float32
+                   weight is read in place (NMF: contiguous N x C whatever V's stride); float16, bfloat16 and float64
+                   ones are staged through one fp32 copy on the device.  V is dense, of any
+                   dtype (NMF: any row stride).  NMF also takes a sparse COO float weight: the observed cells are its
+                   stored entries with w > 0 (duplicate coordinates add up, as in `weight.to_dense()`), V is dense or
+                   sparse COO (0 where it stores nothing), and up to rank 256 every update and the loss run on those
+                   cells alone, O(observed x R) per update; above rank 256 the weights and values are densified on the
+                   device.  A dense weight on a sparse V and a sparse weight on NMFD / NMF2D / NMF3D raise ValueError.
+                   With `group`, each rank passes the weight shard of its V shard; a shard may be zero everywhere (or,
+                   sparse, store nothing), and the value check is agreed on by all ranks, so every rank raises together.
         """
         mask = options.pop("mask", None)
+        weight = options.pop("weight", None)
         if options:
             raise TypeError(f"fit() got an unexpected keyword argument {next(iter(options))!r}")
+        if mask is not None and weight is not None:
+            raise ValueError("mask and weight are exclusive: fold the mask into the weight (weight * mask)")
         if mask is not None:
             self._check_mask(V, mask, precision)
             precision = "f32"
-        eng, W, H, Wd, Hd, staged = self._open_engine(V, beta, precision, group, sparse_kernels=True, mask=mask)
+        if weight is not None:
+            self._check_weight(V, weight, precision)
+            precision = "f32"
+        eng, W, H, Wd, Hd, staged = self._open_engine(V, beta, precision, group, sparse_kernels=True, mask=mask,
+                                                      weight=weight)
 
         try:
             vmin, vmax = eng.minmax()
             if mask is not None and vmin > vmax:                                           # +inf / -inf: nothing seen
                 raise ValueError("mask: no cell of the target is observed")
+            if weight is not None and vmin > vmax:                                         # on every rank of a group
+                raise ValueError("weight: every weight is zero")
             assert vmin >= 0., "Target should be non-negative."                            # nmf.py:329-330
             if vmin == 0 and beta <= 0:                                                    # nmf.py:332-336
                 raise ValueError("When beta <= 0 and V contains zeros, the training process may diverge. "
