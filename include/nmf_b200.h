@@ -116,6 +116,32 @@ int nmfb200_nmf_iterate(nmfb200_ctx* ctx, float* W, float* H, double beta, doubl
 int nmfb200_nmf_loss_prefetch_w(nmfb200_ctx* ctx, const float* W, const float* H, double beta,
                                 double* loss_dev, void* stream);
 
+/* ---- batched NMF: many independent problems of one shape in one context ---------------------------------- */
+
+/* A context for B independent NMF problems of one shape, on the fp32 CUDA-core kernels: problem b has the target V_b (N,C)
+ * and the factors W_b (C,R) = W + b C R and H_b (N,R) = H + b N R of the caller's (B,C,R) / (B,N,R) storages.  Every
+ * update, loss and column-sum launch runs all B problems at once, in the number of launches one problem takes, and each
+ * problem keeps the tile plan and summation order of a single-problem NMFB200_PREC_F32 context of (N, C, R): its factors
+ * and loss are, bit for bit, those of that context.  Workspace: B times the partial slabs, column sums and loss partials of
+ * one such context.  NMFB200_ERR_INVALID for B < 1, R > 256, or a batch too large for the launch grids.
+ * On a batched context: nmfb200_update_w / _update_h / nmfb200_nmf_iterate / nmfb200_sync_factors serve it;
+ * nmfb200_loss writes B doubles (loss_dev[b]); nmfb200_raw_terms returns [B N_f R numerators | B R column sums (beta 1) or
+ * B N_f R denominators] (N_f: the rows of the updated factor), and nmfb200_raw_terms_numel reports that length;
+ * nmfb200_target_minmax covers every problem; nmfb200_precision_for_beta reports NMFB200_PREC_F32.  nmfb200_set_mask,
+ * nmfb200_set_weight, nmfb200_w_apply, nmfb200_nmf_set_target and its sparse / observed forms, nmfb200_nmf_loss_prefetch_w,
+ * nmfb200_nmf_contract_only and the peer calls return NMFB200_ERR_INVALID.  The three calls below take batched contexts
+ * only (NMFB200_ERR_INVALID otherwise). */
+int nmfb200_nmf_batched_create(nmfb200_ctx** out, int device, int64_t B, int64_t N, int64_t C, int64_t R);
+/* Register the targets: problem b reads V + b batch_stride, rows ldv >= C elements apart, elements of type `dtype`.
+ * batch_stride 0: one V shared by every problem (restarts of one fit); otherwise batch_stride >= N ldv.  Alignment and dtype
+ * checks as nmfb200_nmf_set_target.  V stays borrowed.  Asynchronous. */
+int nmfb200_nmf_batched_set_target(nmfb200_ctx* ctx, const void* V, int64_t ldv, int64_t batch_stride, int dtype,
+                                   void* stream);
+/* Which problems run from now on: `active` is B device bytes, borrowed (read by every later launch), null = every problem.
+ * A problem flagged 0 is skipped by every update, loss and raw-terms launch: its factors, its loss_dev slot and its
+ * raw-terms slots are left as they are, at the cost of one flag read per block. */
+int nmfb200_nmf_batched_set_active(nmfb200_ctx* ctx, const uint8_t* active, void* stream);
+
 /* Sparse target for beta 1 and beta 2 (nmf.py:603-638 `_nmf_sp_recon_beta_pos_neg`, :95-119): registers V (N x C) in both
  * compressed forms -- CSR (crow[N+1], col[nnz], val[nnz]) and CSC = CSR of V^T (ccol[C+1], row[nnz], val_t[nnz]) -- int64
  * indices, fp32 values, device pointers borrowed until the next set_target*.  v_norm_kl / v_norm_eu: `_get_V_norm` nmf.py:161-170

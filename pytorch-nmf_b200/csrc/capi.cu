@@ -18,12 +18,16 @@ void count_launch() { g_launches.fetch_add(1, std::memory_order_relaxed); }
 using namespace nmfb200;
 
 struct nmfb200_ctx {
-  int kind = 0;            // 0 = NMF, 1 = NMFD
+  int kind = 0;            // 0 = NMF, 1 = NMFD, 2 = a batch of NMF problems (nmfb200_nmf_batched_create)
   int device = 0;
   int precision = NMFB200_PREC_F32;
   bool auto_mode = false;   // precision AUTO: the tensor-core path is used only where it is known to hold the parity bar
   bool tc_off = false;      // AUTO found the target outside the fp16 operand range: fp32 CUDA-core kernels instead
   int64_t N = 0, C = 0, R = 0;
+  // a batch (kind 2): nprob problems of the shape (N, C, R), their targets bstride elements apart (0: one shared target),
+  // factors and partial slabs back to back; `active` (borrowed, nprob device bytes, null: all) flags the problems that run
+  int64_t nprob = 1, bstride = 0;
+  const uint8_t* active = nullptr;
   NmfdShape d{};
   const void* V = nullptr;        // the dense target, borrowed: vdtype (NMFB200_DTYPE_*) elements
   int vdtype = NMFB200_DTYPE_F32;
@@ -87,11 +91,17 @@ struct DeviceGuard {
   DeviceGuard& operator=(const DeviceGuard&) = delete;
 };
 
-// want_kind: 0 = NMF, 1 = NMFD, kAnyKind for the calls that serve both
+// want_kind: 0 = NMF, 1 = NMFD, 2 = batched NMF, kAnyKind for the calls that serve every kind, kDenseNmf for those that
+// serve NMF and batched NMF
 constexpr int kAnyKind = -1;
+constexpr int kDenseNmf = -2;
+constexpr int kBatched = 2;
+inline bool kind_ok(const nmfb200_ctx* c, int want) {
+  return want == kAnyKind || c->kind == want || (want == kDenseNmf && (c->kind == 0 || c->kind == kBatched));
+}
 #define CTX_GUARD(ctx, want_kind)                                                   \
   if (!(ctx)) return fail(NMFB200_ERR_INVALID, "null context");                     \
-  if ((want_kind) != kAnyKind && (ctx)->kind != (want_kind))                        \
+  if (!kind_ok((ctx), (want_kind)))                                                 \
     return fail(NMFB200_ERR_INVALID, "wrong context kind");                         \
   DeviceGuard _dev_guard((ctx)->device);                                            \
   if (!_dev_guard.ok) return fail(NMFB200_ERR_CUDA, "cannot select the context's device");
@@ -138,7 +148,7 @@ void free_ctx(nmfb200_ctx* c) {
 // `pn_floats` for NMFD's ratio tile (0: none).  On failure frees `c` and returns the error.
 int alloc_workspace(nmfb200_ctx* c, int64_t pn_floats) {
   cudaError_t e = cudaMalloc(&c->num, c->part_floats * sizeof(float));
-  if (e == cudaSuccess) e = cudaMalloc(&c->colsum, 2 * c->R * sizeof(float));
+  if (e == cudaSuccess) e = cudaMalloc(&c->colsum, 2 * c->R * c->nprob * sizeof(float));
   if (e == cudaSuccess) e = cudaMalloc(&c->cs_scratch, c->cs_scratch_floats * sizeof(float));
   if (e == cudaSuccess) e = cudaMalloc(&c->loss_blocks, (size_t)c->loss_max_blocks * sizeof(double));
   if (e == cudaSuccess) e = cudaMalloc(&c->mm_scratch, kMmFloats * sizeof(float));
@@ -173,16 +183,18 @@ void mark_stale(nmfb200_ctx* c, bool w, bool h) {
 struct FactorDims { int64_t rows, inner, other_rows, other_inner; };
 FactorDims factor_dims(const nmfb200_ctx* c, int which) {
   const NmfdShape& d = c->d;
-  const FactorDims w = c->kind == 0 ? FactorDims{c->C, 1, c->N, 1} : FactorDims{d.C, d.w_inner(), d.B, d.h_inner()};
+  const FactorDims w = c->kind != 1 ? FactorDims{c->C, 1, c->N, 1} : FactorDims{d.C, d.w_inner(), d.B, d.h_inner()};
   return which == 0 ? w : FactorDims{w.other_rows, w.other_inner, w.rows, w.inner};
 }
 
 // The ratio stage's view of one factor's terms: its rows x R x inner elements, summed over `nchunks` slabs of that layout.
+// A batch: the problems' factors back to back, each slab holding every problem's partials in that order.
 ApplyArgs factor_view(const nmfb200_ctx* c, int which, int nchunks) {
   const FactorDims f = factor_dims(c, which);
   ApplyArgs a{};
   a.R = (int)c->R; a.inner = f.inner; a.rowlen = c->R * f.inner; a.ldp = a.rowlen;
-  a.numel = f.rows * a.rowlen; a.chunk_stride = a.numel; a.nchunks = nchunks;
+  a.numel = f.rows * a.rowlen * c->nprob; a.chunk_stride = a.numel; a.nchunks = nchunks;
+  if (c->kind == kBatched) { a.prob_numel = f.rows * a.rowlen; a.active = c->active; }
   return a;
 }
 
@@ -365,6 +377,56 @@ int nmfb200_nmf_set_target(nmfb200_ctx* ctx, const void* V, int64_t ldv, int dty
       }
     }
   }
+  return 0;
+}
+
+/* ---- batched NMF: B independent problems of one shape on the fp32 kernels ------------------------------------ */
+
+int nmfb200_nmf_batched_create(nmfb200_ctx** out, int device, int64_t B, int64_t N, int64_t C, int64_t R) {
+  if (!out) return fail(NMFB200_ERR_INVALID, "out is null");
+  *out = nullptr;
+  if (B < 1 || N < 1 || C < 1 || R < 1) return fail(NMFB200_ERR_INVALID, "B, N, C, R must be positive");
+  if (R > 256) return fail(NMFB200_ERR_INVALID, "batched fits support rank <= 256");
+  // the batch rides on grid x of every launch, the loss partials are counted in int
+  const int64_t rows = N > C ? N : C;
+  if (ceil_div(rows, 64) > kMaxGridX / B || (int64_t)simt_nmf_max_blocks(N, C) > INT32_MAX / B ||
+      ceil_div(R, 64) > kMaxGridX / B)
+    return fail(NMFB200_ERR_INVALID, "batch too large for the launch grids");
+  DeviceGuard guard(device);
+  if (!guard.ok) return fail(NMFB200_ERR_CUDA, "cannot select the requested device");
+  nmfb200_ctx* c = new (std::nothrow) nmfb200_ctx();
+  if (!c) return fail(NMFB200_ERR_INVALID, "out of host memory");
+  c->kind = kBatched; c->device = device; c->N = N; c->C = C; c->R = R; c->nprob = B;
+  c->precision = NMFB200_PREC_F32;
+  // each problem's plan is the single problem's: same chunks, loss blocks and column-sum blocks
+  c->nslab[0] = chunks_for(C, N, R);
+  c->nslab[1] = chunks_for(N, C, R);
+  int64_t pf = (int64_t)c->nslab[0] * C * R;
+  if ((int64_t)c->nslab[1] * N * R > pf) pf = (int64_t)c->nslab[1] * N * R;
+  c->part_floats = pf * B;
+  c->cs_scratch_floats = colsum_scratch_floats(rows, (int)R, 1) * B;
+  c->loss_max_blocks = (int)(simt_nmf_max_blocks(N, C) * B);
+  if (int rc = alloc_workspace(c, 0)) return rc;
+  *out = c;
+  return 0;
+}
+
+int nmfb200_nmf_batched_set_target(nmfb200_ctx* ctx, const void* V, int64_t ldv, int64_t batch_stride, int dtype,
+                                   void* stream) {
+  CTX_GUARD(ctx, kBatched);
+  if (!V || ldv < ctx->C) return fail(NMFB200_ERR_INVALID, "bad target pointer / leading dimension");
+  if (batch_stride != 0 && batch_stride < ctx->N * ldv)
+    return fail(NMFB200_ERR_INVALID, "batch stride must be 0 (one shared target) or at least N x ldv");
+  if (int rc = check_target(V, dtype)) return rc;
+  ctx->V = V; ctx->vdtype = dtype; ctx->ldv = ldv; ctx->bstride = batch_stride; ctx->has_target = true;
+  return matrix_minmax(V, dtype, ctx->N, ctx->C, ldv, ctx->mm_scratch, ctx->mm_scratch + kMmPartials, (cudaStream_t)stream,
+                       CellSel{}, batch_stride ? ctx->nprob : 1, batch_stride);
+}
+
+int nmfb200_nmf_batched_set_active(nmfb200_ctx* ctx, const uint8_t* active, void* stream) {
+  CTX_GUARD(ctx, kBatched);
+  (void)stream;
+  ctx->active = active;
   return 0;
 }
 
@@ -570,6 +632,7 @@ namespace {
 int set_selector(nmfb200_ctx* ctx, CellSel sel, void* stream) {
   CTX_GUARD(ctx, kAnyKind);
   TARGET_GUARD(ctx);
+  if (ctx->kind == kBatched) return fail(NMFB200_ERR_INVALID, "batched fits take no mask or weight");
   if (ctx->sparse)
     return fail(NMFB200_ERR_INVALID, std::string(sel.kind == kSelWeight ? "a weight" : "a mask") +
                                          " needs a dense target (set_target or nmfd_set_target)");
@@ -641,8 +704,12 @@ int simt_contract(nmfb200_ctx* c, int which, const float* W, const float* H, dou
   // W update: F = W (C rows), G = H (N rows), Vm = V^T;  H update: F = H (N rows), G = W (C rows), Vm = V
   const float* fac[2] = {W, H};
   const FactorDims f = factor_dims(c, which);
+  // a batch: problem b's target, factors and partials (slab layout [chunk][problem][rows][R]); one problem otherwise
+  Batch bt;
+  if (c->kind == kBatched) bt = Batch{c->nprob, c->bstride, f.rows * c->R, f.other_rows * c->R, f.rows * c->R, c->active};
   return simt_nmf_contract(c->V, c->vdtype, c->ldv, /*trans=*/which == 0, fac[which], fac[1 - which], f.rows, f.other_rows,
-                           (int)c->R, beta, c->nslab[which], c->num, c->den, c->R, f.rows * c->R, c->sel, c->C, st);
+                           (int)c->R, beta, c->nslab[which], c->num, c->den, c->R, f.rows * c->R * c->nprob, c->sel, c->C,
+                           st, bt);
 }
 
 // The same for NMFD / NMF2D / NMF3D: the ratio tiles Pn (and Pp), then their backward passes (wgrad for W, dgrad for H) into
@@ -679,7 +746,7 @@ int factor_terms(nmfb200_ctx* c, int which, const float* W, const float* H, doub
   if (c->sparse && beta == 2.0 && !out) { int e = ensure_den(c); if (e) return e; }
   float* num_out = out ? out : c->num;
   float* den_out = out ? out + a.numel
-                 : kl ? c->colsum + (1 - which) * c->R : (beta == 2.0 || c->observed) ? c->den : c->sp_den;
+                 : kl ? c->colsum + (1 - which) * c->R * c->nprob : (beta == 2.0 || c->observed) ? c->den : c->sp_den;
   *tc = c->tcd && use_tc(c, beta);
   if (*tc) {                  // NMFD beta 1: the recon pass also brings both column sums and kappa up to date
     int rc = tc_nmfd_recon(c->tcd, c->V, c->vdtype, W, H, false, nullptr, st);
@@ -697,14 +764,14 @@ int factor_terms(nmfb200_ctx* c, int which, const float* W, const float* H, doub
     else a.den = den_out;
     return sparse_terms(c, which, fac[which], fac[1 - which], beta, num_out, den_out, st);
   }
-  int rc = c->kind == 0 ? simt_contract(c, which, W, H, beta, st) : nmfd_contract(c, which, W, H, beta, st);
+  int rc = c->kind == 1 ? nmfd_contract(c, which, W, H, beta, st) : simt_contract(c, which, W, H, beta, st);
   if (rc) return rc;
   a.num = c->num; a.nchunks = c->nslab[which];
   if (!kl) { a.den = c->den; return 0; }
   a.kl_den = den_out;
   const FactorDims f = factor_dims(c, which);
   return factor_colsum(fac[1 - which], f.other_rows, (int)c->R, f.other_inner, c->cs_scratch, c->cs_scratch_floats, den_out,
-                       st);
+                       st, c->nprob, c->active);
 }
 
 // One factor update (which = 0: param = W, 1: param = H) on the kernels that serve this context and beta.  No device guard:
@@ -768,7 +835,7 @@ int nmfb200_target_minmax(nmfb200_ctx* ctx, float* vmin, float* vmax, void* stre
 
 int nmfb200_nmf_iterate(nmfb200_ctx* ctx, float* W, float* H, double beta, double gamma, double l1_reg,
                         double l2_reg, int n_iter, void* stream) {
-  CTX_GUARD(ctx, 0);
+  CTX_GUARD(ctx, kDenseNmf);
   TARGET_GUARD(ctx);
   if (!W || !H || n_iter < 0) return fail(NMFB200_ERR_INVALID, "bad argument");
   cudaStream_t st = (cudaStream_t)stream;
@@ -882,14 +949,16 @@ int nmfb200_loss(nmfb200_ctx* ctx, const float* W, const float* H, double beta, 
   }
   if (ctx->sparse) return sparse_loss_ctx(ctx, W, H, beta, loss_dev, st);
   if (use_tc(ctx, beta)) return tc_loss(ctx->tc, W, H, beta, loss_dev, st);
+  Batch bt;         // a batch: loss_dev[b] for every active problem b
+  if (ctx->kind == kBatched) bt = Batch{ctx->nprob, ctx->bstride, ctx->N * ctx->R, ctx->C * ctx->R, 0, ctx->active};
   return simt_nmf_loss(ctx->V, ctx->vdtype, ctx->ldv, H, W, ctx->N, ctx->C, (int)ctx->R, beta, ctx->loss_blocks,
-                       ctx->loss_max_blocks, loss_dev, ctx->sel, ctx->C, st);
+                       ctx->loss_max_blocks, loss_dev, ctx->sel, ctx->C, st, bt);
 }
 
 int64_t nmfb200_raw_terms_numel(const nmfb200_ctx* ctx, int which, double beta) {
   if (!ctx || (which != 0 && which != 1)) return -1;
   const int64_t n = factor_view(ctx, which, 1).numel;
-  return kl_colsum(ctx, beta) ? n + ctx->R : 2 * n;
+  return kl_colsum(ctx, beta) ? n + ctx->R * ctx->nprob : 2 * n;
 }
 
 // The raw terms of one factor's update (which = 0: W, 1: H) into `out`, nmfb200_raw_terms_numel floats: the partial slabs
@@ -917,6 +986,7 @@ int nmfb200_w_apply(nmfb200_ctx* ctx, float* W, const float* reduced, double bet
                     double l2_reg, void* stream) {
   CTX_GUARD(ctx, kAnyKind);
   TARGET_GUARD(ctx);
+  if (ctx->kind == kBatched) return fail(NMFB200_ERR_INVALID, "w_apply does not serve batched contexts");
   if (!W || !reduced) return fail(NMFB200_ERR_INVALID, "null pointer");
   cudaStream_t st = (cudaStream_t)stream;
   if (ctx->tc && use_tc(ctx, beta)) return tc_w_apply(ctx->tc, W, reduced, beta, gamma, l1_reg, l2_reg, st);

@@ -62,6 +62,19 @@ int with_sel(CellSel s, F&& f) {
   return f(static_cast<const NoSel*>(nullptr));
 }
 
+// A batch of independent NMF problems of one shape (nmfb200_nmf_batched_create).  The kernels that take it run every problem
+// in one launch, with the batch folded into grid x: problem b owns the blocks [b nbx, (b + 1) nbx) of the nbx blocks one
+// problem launches, and does in them exactly what a launch for that problem alone does.  Offsets between problems are in
+// elements of the pointer they apply to, int64.  The default is one problem (every single-problem call).
+struct Batch {
+  int64_t n = 1;                      // problems
+  int64_t v = 0;                      // target elements between problems (0: one target shared by every problem)
+  int64_t f = 0, g = 0;               // floats between problems' F / G factors of a contraction or loss
+  int64_t p = 0;                      // floats between problems' partial slabs (within one chunk)
+  const uint8_t* active = nullptr;    // n flags, 0 = skipped: the problem's blocks exit at once (null: every problem runs)
+};
+__device__ __forceinline__ bool batch_skips(const uint8_t* active, int64_t b) { return active && !active[b]; }
+
 // beta-divergence branch of nmf.py:61-74 / metrics.py:60-96
 enum BetaMode : int { kKL = 0, kEU = 1, kIS = 2, kGeneric = 3 };
 inline BetaMode beta_mode(double beta) {
@@ -149,15 +162,18 @@ static inline bool grid_fits(const Grid3& g) {
 // M (optional selector, read like V with pitch ldm): a fit on the observed cells only -- Pn = Pp = 0 where M is 0, V is not
 // read there, and den is always formed (beta 1: Pp = M).  A weight selector multiplies Pn and Pp by the cell's weight
 // (beta 1: Pp = the weight).  An empty M runs the unmasked kernels.
+// bt: bt.n problems in one launch (no selector then), problem b reading V + b bt.v, F + b bt.f, G + b bt.g and writing its
+// slabs at num / den + b bt.p.
 int simt_nmf_contract(const void* V, int vdtype, int64_t ldv, int trans, const float* F, const float* G,
                       int64_t Mr, int64_t Nc, int R, double beta, int nchunks,
                       float* num, float* den, int64_t ldp, int64_t chunk_stride, CellSel M, int64_t ldm,
-                      cudaStream_t st);
+                      cudaStream_t st, const Batch& bt = Batch{});
 // beta_div(F G^T, Vm) accumulated into block partials then *loss_dev (double); over the cells where M (optional, pitch
-// ldm, not transposed) is non-zero, each term times the cell's weight for a weight selector.
+// ldm, not transposed) is non-zero, each term times the cell's weight for a weight selector.  bt: loss_dev[b] for problem
+// b, from its own run of partials summed in the single problem's order; a skipped problem's slot is left as it is.
 int simt_nmf_loss(const void* V, int vdtype, int64_t ldv, const float* F, const float* G, int64_t Mr, int64_t Nc,
                   int R, double beta, double* block_partials, int max_blocks, double* loss_dev, CellSel M,
-                  int64_t ldm, cudaStream_t st);
+                  int64_t ldm, cudaStream_t st, const Batch& bt = Batch{});
 int simt_nmf_max_blocks(int64_t Mr, int64_t Nc);
 // The V-free pieces of a sparse target's update and loss at beta != 1, 2 (nmf.py:621-636):
 //   den[ch][m][r] = sum_{c in chunk ch} (S[m,c] + eps)^(beta-1) G[c,r]: simt_nmf_contract's denominator at this beta, bit for
@@ -187,22 +203,30 @@ struct ApplyArgs {
   unsigned int* absmax_bits;  // optional: atomicMax of the updated values (non-negative floats)
   const float* kappa;         // optional (with kappa_vec): the partials hold sum (P - kappa) G; num += *kappa * kappa_vec[r]
   const float* kappa_vec;     // [R]
+  // a batch of problems (Batch): every prob_numel consecutive elements are one problem's, which takes its kl_den at
+  // kl_den + b R; a problem whose active flag is 0 is left untouched (0: one problem)
+  int64_t prob_numel = 0;
+  const uint8_t* active = nullptr;
 };
 int apply_update(const ApplyArgs& a, cudaStream_t st);
 // whether apply_update takes its four-elements-per-thread kernel for this shape (16-byte aligned buffers provided)
 bool apply_update_vec4_shape(const ApplyArgs& a);
 // num_out[i] (and den_out[i] when a.den) = what the ratio stage would read for element i: summed partials + centring term
 int raw_sum(const ApplyArgs& a, float* num_out, float* den_out, cudaStream_t st);
-// sums[r] = sum over all other dims of x viewed as (outer, R, inner); deterministic two-stage.
+// sums[r] = sum over all other dims of x viewed as (outer, R, inner); deterministic two-stage.  nprob > 1 (inner 1 only):
+// sums[b R + r] for nprob consecutive (outer, R) problems, each summed in the single problem's order, skipping those whose
+// `active` flag is 0; scratch_floats then covers nprob x colsum_scratch_floats.
 int factor_colsum(const float* x, int64_t outer, int R, int64_t inner, float* scratch, int64_t scratch_floats,
-                  float* sums, cudaStream_t st);
+                  float* sums, cudaStream_t st, int64_t nprob = 1, const uint8_t* active = nullptr);
 int64_t colsum_scratch_floats(int64_t outer, int R, int64_t inner);
 // min / max of a strided matrix of `vdtype` elements (fit()'s validation), results in mm[0..1]; with M (optional, contiguous
-// rows x cols selector) over the cells where M is non-zero only (none: +inf / -inf)
+// rows x cols selector) over the cells where M is non-zero only (none: +inf / -inf).  nprob > 1: over nprob such matrices,
+// `bstride` elements apart (no selector).
 int matrix_minmax(const void* V, int vdtype, int64_t rows, int64_t cols, int64_t ld, float* scratch2048, float* mm,
-                  cudaStream_t st, CellSel M = CellSel{});
-// *out = sum of n doubles in fixed order (single block)
-int sum_partials(const double* p, int n, double* out, cudaStream_t st);
+                  cudaStream_t st, CellSel M = CellSel{}, int64_t nprob = 1, int64_t bstride = 0);
+// *out = sum of n doubles in fixed order (single block).  nprob > 1: out[b] = the sum of p[b n, (b + 1) n), one block per
+// problem, in the same order; a problem whose `active` flag is 0 keeps its out[b].
+int sum_partials(const double* p, int n, double* out, cudaStream_t st, int64_t nprob = 1, const uint8_t* active = nullptr);
 
 // project.cu -------------------------------------------------------------------------------
 // Hoyer's projection (nmf.py:21-49) of every slice x[:, j, :] of x viewed as (outer, D, inner) onto {v >= 0, |v|_1 = k1[j],

@@ -19,6 +19,10 @@
 // fp32 weight tile the same way, reads V only where the weight is non-zero, and multiplies where the mask selects: pn *= w,
 // pp *= w, and pp = w at beta 1.  The unmasked instantiations (NoSel) take no branch on it.
 //
+// Batch (common.cuh, batched NMF): grid x holds the row blocks of every problem, problem after problem; a CTA reads its
+// problem's V, F and G and writes its partials at the problem's offsets, and otherwise runs the single problem's plan and
+// arithmetic unchanged, so each problem's partials equal a single-problem launch's bit for bit.
+//
 // kVFree (sparse targets at beta != 1, 2): the contraction forms only den += (S+eps)^(beta-1) G_tile and reads no V, with
 // kGeneric's plan, staging and arithmetic, so its den partials equal kGeneric's bit for bit whatever V holds; the loss sums
 // (S+eps)^beta over every cell, again without V.
@@ -82,12 +86,12 @@ __device__ __forceinline__ void phi(float v, float s, float bm2, float bm1, floa
   }
 }
 
-template <int RB, bool TRANS, int MODE, typename TV, typename SEL = NoSel>
+template <int RB, bool TRANS, int MODE, typename TV, typename SEL = NoSel, bool BATCH = false>
 __global__ void __launch_bounds__(256)
 simt_contract_kernel(const TV* __restrict__ V, int64_t ldv, const float* __restrict__ F,
                      const float* __restrict__ G, int64_t Mr, int64_t Nc, int R, float bm2, float bm1,
                      int nchunks, float* __restrict__ num, float* __restrict__ den, int64_t ldp,
-                     int64_t chunk_stride, const SEL* __restrict__ Mk, int64_t ldm) {
+                     int64_t chunk_stride, const SEL* __restrict__ Mk, int64_t ldm, Batch bt) {
   constexpr bool MASK = !std::is_same<SEL, NoSel>::value;
   constexpr bool WEIGHT = kWeighted<SEL>;
   constexpr int Rp = 16 * RB;
@@ -100,9 +104,22 @@ simt_contract_kernel(const TV* __restrict__ V, int64_t ldv, const float* __restr
   float* Ps = Gs + Rp * kLd;        // [64][kLd]  V tile, then Pn in place
   float* Qs = kDenOnly ? Ps : Ps + kTile * kLd;     // [64][kLd]  Pp (kTwo only; kVFree: in Ps's place); MASK: the selector first
 
+  // BATCH (NoSel only): this block's problem and its row block within it; the problem's pointers.  The single-problem
+  // instantiations compile none of it.
+  int64_t bx = blockIdx.x;
+  if constexpr (BATCH) {
+    const int64_t nbx = (Mr + kTile - 1) / kTile;
+    const int64_t prob = bx / nbx;
+    if (batch_skips(bt.active, prob)) return;
+    bx -= prob * nbx;
+    V += prob * bt.v; F += prob * bt.f; G += prob * bt.g;
+    if (kNum) num += prob * bt.p;
+    if (kTwo) den += prob * bt.p;
+  }
+
   const int tid = threadIdx.x;
   const int tx = tid & 15, ty = tid >> 4;
-  const int64_t m0 = (int64_t)blockIdx.x * kTile;
+  const int64_t m0 = bx * kTile;
   const int chunk = blockIdx.y;
   const int64_t tiles_total = (Nc + kTile - 1) / kTile;
   const int64_t tpc = chunk_tiles(Nc, nchunks);
@@ -238,17 +255,17 @@ simt_contract_kernel(const TV* __restrict__ V, int64_t ldv, const float* __restr
   }
 }
 
-template <int RB, bool TRANS, typename TV, typename SEL>
+template <int RB, bool TRANS, typename TV, typename SEL, bool BATCH>
 int launch_contract_mode(int mode, dim3 grid, size_t smem, cudaStream_t st, const TV* V, int64_t ldv,
                          const float* F, const float* G, int64_t Mr, int64_t Nc, int R, float bm2, float bm1,
                          int nchunks, float* num, float* den, int64_t ldp, int64_t chunk_stride, const SEL* Mk,
-                         int64_t ldm) {
+                         int64_t ldm, const Batch& bt) {
 #define NMF_LAUNCH_MODE(M)                                                                              \
   {                                                                                                     \
-    auto kern = simt_contract_kernel<RB, TRANS, M, TV, SEL>;                                            \
+    auto kern = simt_contract_kernel<RB, TRANS, M, TV, SEL, BATCH>;                                     \
     NMF_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
     kern<<<grid, 256, smem, st>>>(V, ldv, F, G, Mr, Nc, R, bm2, bm1, nchunks, num, den, ldp,            \
-                                  chunk_stride, Mk, ldm);                                               \
+                                  chunk_stride, Mk, ldm, bt);                                           \
   }
   switch (mode) {
     case kKL: NMF_LAUNCH_MODE(kKL); break;
@@ -265,15 +282,25 @@ template <int RB, typename TV, typename SEL>
 int launch_contract_rb(int trans, int mode, dim3 grid, cudaStream_t st, const TV* V, int64_t ldv,
                        const float* F, const float* G, int64_t Mr, int64_t Nc, int R, float bm2, float bm1,
                        int nchunks, float* num, float* den, int64_t ldp, int64_t chunk_stride, const SEL* Mk,
-                       int64_t ldm) {
+                       int64_t ldm, const Batch& bt) {
   const int Rp = 16 * RB;
   constexpr bool MASK = !std::is_same<SEL, NoSel>::value;
   size_t smem = (size_t)(2 * Rp + kTile * (mode == kKL && !MASK ? 1 : 2)) * kLd * sizeof(float);
+  // a batch runs the BATCH instantiations (no selector); one problem the single-problem ones
+  if constexpr (std::is_same<SEL, NoSel>::value) {
+    if (bt.n > 1 || bt.active) {
+      if (trans)
+        return launch_contract_mode<RB, true, TV, SEL, true>(mode, grid, smem, st, V, ldv, F, G, Mr, Nc, R, bm2, bm1,
+                                                             nchunks, num, den, ldp, chunk_stride, Mk, ldm, bt);
+      return launch_contract_mode<RB, false, TV, SEL, true>(mode, grid, smem, st, V, ldv, F, G, Mr, Nc, R, bm2, bm1,
+                                                            nchunks, num, den, ldp, chunk_stride, Mk, ldm, bt);
+    }
+  }
   if (trans)
-    return launch_contract_mode<RB, true, TV, SEL>(mode, grid, smem, st, V, ldv, F, G, Mr, Nc, R, bm2, bm1, nchunks,
-                                                   num, den, ldp, chunk_stride, Mk, ldm);
-  return launch_contract_mode<RB, false, TV, SEL>(mode, grid, smem, st, V, ldv, F, G, Mr, Nc, R, bm2, bm1, nchunks, num,
-                                                  den, ldp, chunk_stride, Mk, ldm);
+    return launch_contract_mode<RB, true, TV, SEL, false>(mode, grid, smem, st, V, ldv, F, G, Mr, Nc, R, bm2, bm1, nchunks,
+                                                          num, den, ldp, chunk_stride, Mk, ldm, bt);
+  return launch_contract_mode<RB, false, TV, SEL, false>(mode, grid, smem, st, V, ldv, F, G, Mr, Nc, R, bm2, bm1, nchunks,
+                                                         num, den, ldp, chunk_stride, Mk, ldm, bt);
 }
 
 // ---- loss ------------------------------------------------------------------------------------
@@ -294,18 +321,29 @@ __device__ __forceinline__ double block_reduce_sum(double v, double* sh) {
 
 // SEL: the sum runs over the observed cells only (the missing ones are dropped, not zeroed: at beta != 0, 1, 2 a zeroed
 // cell would still add eps^beta / beta); a weighted fit adds w * term over the cells with w != 0
-template <int MODE, typename TV, typename SEL = NoSel>
+template <int MODE, typename TV, typename SEL = NoSel, bool BATCH = false>
 __global__ void __launch_bounds__(256)
 simt_loss_kernel(const TV* __restrict__ V, int64_t ldv, const float* __restrict__ F,
                  const float* __restrict__ G, int64_t Mr, int64_t Nc, int R, int Rp, float beta, int nchunks,
-                 double* __restrict__ block_partials, const SEL* __restrict__ Mk, int64_t ldm) {
+                 double* __restrict__ block_partials, const SEL* __restrict__ Mk, int64_t ldm, Batch bt) {
   extern __shared__ __align__(16) float smem[];
   float* Fs = smem;
   float* Gs = Fs + Rp * kLd;
   __shared__ double red[8];
+  // BATCH (NoSel only): problem `prob`'s blocks write its own run of gridDim.y x nbx partials, laid out as a single
+  // problem's
+  int64_t bx = blockIdx.x, part = 0;
+  if constexpr (BATCH) {
+    const int64_t nbx = (Mr + kTile - 1) / kTile;
+    const int64_t prob = bx / nbx;
+    if (batch_skips(bt.active, prob)) return;
+    bx -= prob * nbx;
+    part = (prob * gridDim.y + blockIdx.y) * nbx + bx;
+    V += prob * bt.v; F += prob * bt.f; G += prob * bt.g;
+  }
   const int tid = threadIdx.x;
   const int tx = tid & 15, ty = tid >> 4;
-  const int64_t m0 = (int64_t)blockIdx.x * kTile;
+  const int64_t m0 = bx * kTile;
   const int chunk = blockIdx.y;
   const int64_t tiles_total = (Nc + kTile - 1) / kTile;
   const int64_t tpc = chunk_tiles(Nc, nchunks);
@@ -348,15 +386,20 @@ simt_loss_kernel(const TV* __restrict__ V, int64_t ldv, const float* __restrict_
     acc += (double)local;
   }
   double tot = block_reduce_sum(acc, red);
-  if (tid == 0) block_partials[(int64_t)blockIdx.y * gridDim.x + blockIdx.x] = tot;
+  if (tid == 0) block_partials[BATCH ? part : (int64_t)blockIdx.y * gridDim.x + blockIdx.x] = tot;
 }
 
-__global__ void __launch_bounds__(256) sum_partials_kernel(const double* __restrict__ p, int n, double* out) {
+// one block per problem (grid x): out[b] = the sum of p[b n, (b + 1) n)
+__global__ void __launch_bounds__(256) sum_partials_kernel(const double* __restrict__ p, int n, double* out,
+                                                           const uint8_t* __restrict__ active) {
   __shared__ double red[8];
+  const int64_t b = blockIdx.x;
+  if (batch_skips(active, b)) return;
+  p += b * n;
   double acc = 0.0;
   for (int i = threadIdx.x; i < n; i += 256) acc += p[i];
   double tot = block_reduce_sum(acc, red);
-  if (threadIdx.x == 0) *out = tot;
+  if (threadIdx.x == 0) out[b] = tot;
 }
 
 int loss_chunks(int64_t Mr, int64_t Nc) {
@@ -380,19 +423,30 @@ void simt_nmf_plan(int64_t Mr, int64_t Nc, int R, int nchunks, SimtNmfPlan* p) {
   p->loss_tiles_per_chunk = chunk_tiles(Nc, p->loss_chunks);
 }
 
-int sum_partials(const double* p, int n, double* out, cudaStream_t st) {
-  sum_partials_kernel<<<1, 256, 0, st>>>(p, n, out);
+int sum_partials(const double* p, int n, double* out, cudaStream_t st, int64_t nprob, const uint8_t* active) {
+  if (nprob < 1 || nprob > kMaxGridX) { set_error("sum_partials: bad problem count"); return 1; }
+  sum_partials_kernel<<<(unsigned)nprob, 256, 0, st>>>(p, n, out, active);
   NMF_LAUNCH_CHECK();
+  return 0;
+}
+
+// grid x of a batched launch: nbx blocks per problem for bt.n problems
+static int batch_grid_x(int64_t nbx, const Batch& bt, const char* who, unsigned* x) {
+  if (bt.n < 1 || nbx > kMaxGridX / bt.n) { set_error(std::string(who) + ": batch x row blocks pass grid x"); return 1; }
+  *x = (unsigned)(nbx * bt.n);
   return 0;
 }
 
 int simt_nmf_contract(const void* V, int vdtype, int64_t ldv, int trans, const float* F, const float* G, int64_t Mr,
                       int64_t Nc, int R, double beta, int nchunks, float* num, float* den, int64_t ldp,
-                      int64_t chunk_stride, CellSel M, int64_t ldm, cudaStream_t st) {
+                      int64_t chunk_stride, CellSel M, int64_t ldm, cudaStream_t st, const Batch& bt) {
   if (R < 1) { set_error("simt_nmf_contract: rank must be positive"); return 1; }
+  if (bt.n > 1 && M) { set_error("simt_nmf_contract: a batch takes no selector"); return 1; }
   int mode = beta_mode(beta);
   float bm2 = (float)(beta - 2.0), bm1 = (float)(beta - 1.0);
-  dim3 grid((unsigned)ceil_div(Mr, kTile), (unsigned)nchunks, (unsigned)simt_rank_blocks(R));
+  unsigned gx;
+  if (batch_grid_x(ceil_div(Mr, kTile), bt, "simt_nmf_contract", &gx)) return 1;
+  dim3 grid(gx, (unsigned)nchunks, (unsigned)simt_rank_blocks(R));
   const int rb = contract_rb(R);
   return with_vtype(V, vdtype, [&](auto Vt) {
     using TV = vtype_t<decltype(Vt)>;
@@ -400,7 +454,7 @@ int simt_nmf_contract(const void* V, int vdtype, int64_t ldv, int trans, const f
       using SEL = sel_t<decltype(Mk)>;
 #define NMF_RB(RBV)                                                                                                     \
   return launch_contract_rb<RBV, TV, SEL>(trans, mode, grid, st, Vt, ldv, F, G, Mr, Nc, R, bm2, bm1, nchunks, num, den, \
-                                          ldp, chunk_stride, Mk, M ? ldm : 0)
+                                          ldp, chunk_stride, Mk, M ? ldm : 0, bt)
       switch (rb) {
         case 1: NMF_RB(1);
         case 2: NMF_RB(2);
@@ -415,24 +469,35 @@ int simt_nmf_contract(const void* V, int vdtype, int64_t ldv, int trans, const f
 
 int simt_nmf_loss(const void* V, int vdtype, int64_t ldv, const float* F, const float* G, int64_t Mr, int64_t Nc, int R,
                   double beta, double* block_partials, int max_blocks, double* loss_dev, CellSel M, int64_t ldm,
-                  cudaStream_t st) {
+                  cudaStream_t st, const Batch& bt) {
   if (R < 1) { set_error("simt_nmf_loss: rank must be positive"); return 1; }
+  if (bt.n > 1 && M) { set_error("simt_nmf_loss: a batch takes no selector"); return 1; }
   int nchunks = loss_chunks(Mr, Nc);
-  dim3 grid((unsigned)ceil_div(Mr, kTile), (unsigned)nchunks);
-  int nblocks = (int)(grid.x * grid.y);
-  if (nblocks > max_blocks) { set_error("simt_nmf_loss: partial buffer too small"); return 1; }
+  unsigned gx;
+  if (batch_grid_x(ceil_div(Mr, kTile), bt, "simt_nmf_loss", &gx)) return 1;
+  dim3 grid(gx, (unsigned)nchunks);
+  const int nblocks = (int)(ceil_div(Mr, kTile) * nchunks);          // per problem
+  if ((double)nblocks * (double)bt.n > (double)max_blocks) { set_error("simt_nmf_loss: partial buffer too small"); return 1; }
   int Rp = (int)round_up(R < 256 ? R : 256, 16);
   size_t smem = (size_t)2 * Rp * kLd * sizeof(float);
   int mode = beta_mode(beta);
+  const bool batched = bt.n > 1 || bt.active;
   int rc = with_vtype(V, vdtype, [&](auto Vt) {
     using TV = vtype_t<decltype(Vt)>;
     return with_sel(M, [&](auto Mk) {
       using SEL = sel_t<decltype(Mk)>;
+#define NMF_LOSS_B(MD, BATCH)                                                                                               \
+  {                                                                                                                         \
+    auto kern = simt_loss_kernel<MD, TV, SEL, BATCH>;                                                                       \
+    NMF_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));                     \
+    kern<<<grid, 256, smem, st>>>(Vt, ldv, F, G, Mr, Nc, R, Rp, (float)beta, nchunks, block_partials, Mk, M ? ldm : 0, bt);\
+  }
 #define NMF_LOSS(MD)                                                                                                        \
   {                                                                                                                         \
-    auto kern = simt_loss_kernel<MD, TV, SEL>;                                                                              \
-    NMF_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));                     \
-    kern<<<grid, 256, smem, st>>>(Vt, ldv, F, G, Mr, Nc, R, Rp, (float)beta, nchunks, block_partials, Mk, M ? ldm : 0);    \
+    if constexpr (std::is_same<SEL, NoSel>::value) {                                                                        \
+      if (batched) { NMF_LOSS_B(MD, true); break; }                                                                         \
+    }                                                                                                                       \
+    NMF_LOSS_B(MD, false);                                                                                                  \
   }
       switch (mode) {
         case kKL: NMF_LOSS(kKL); break;
@@ -441,12 +506,13 @@ int simt_nmf_loss(const void* V, int vdtype, int64_t ldv, const float* F, const 
         default: NMF_LOSS(kGeneric); break;
       }
 #undef NMF_LOSS
+#undef NMF_LOSS_B
       NMF_LAUNCH_CHECK();
       return 0;
     });
   });
   if (rc) return rc;
-  return sum_partials(block_partials, nblocks, loss_dev, st);
+  return sum_partials(block_partials, nblocks, loss_dev, st, bt.n, bt.active);
 }
 
 int simt_nmf_contract_den(const float* F, const float* G, int64_t Mr, int64_t Nc, int R, double beta, int nchunks,
@@ -461,7 +527,7 @@ int simt_nmf_contract_den(const float* F, const float* G, int64_t Mr, int64_t Nc
     auto kern = simt_contract_kernel<RBV, false, kVFree, float>;                                                     \
     NMF_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));              \
     kern<<<grid, 256, smem, st>>>(nullptr, 0, F, G, Mr, Nc, R, 0.f, bm1, nchunks, nullptr, den, ldp, chunk_stride,   \
-                                  nullptr, 0);                                                                       \
+                                  nullptr, 0, Batch{});                                                              \
   } break
   switch (contract_rb(R)) {
     case 1: NMF_DEN(1);
@@ -486,7 +552,7 @@ int simt_nmf_pow_sum(const float* F, const float* G, int64_t Mr, int64_t Nc, int
   const size_t smem = (size_t)2 * Rp * kLd * sizeof(float);
   auto kern = simt_loss_kernel<kVFree, float>;
   NMF_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  kern<<<grid, 256, smem, st>>>(nullptr, 0, F, G, Mr, Nc, R, Rp, (float)beta, nchunks, block_partials, nullptr, 0);
+  kern<<<grid, 256, smem, st>>>(nullptr, 0, F, G, Mr, Nc, R, Rp, (float)beta, nchunks, block_partials, nullptr, 0, Batch{});
   NMF_LAUNCH_CHECK();
   return 0;
 }

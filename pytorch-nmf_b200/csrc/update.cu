@@ -9,7 +9,8 @@ __global__ void __launch_bounds__(256)
 apply_update_kernel(ApplyArgs a) {
   const int64_t idx = (int64_t)blockIdx.x * 256 + threadIdx.x;
   float newv = 0.f;
-  if (idx < a.numel) {
+  const int64_t b = a.prob_numel ? idx / a.prob_numel : 0;      // Batch: the element's problem
+  if (idx < a.numel && !batch_skips(a.active, b)) {
     const int64_t row = idx / a.rowlen;
     const int64_t col = idx - row * a.rowlen;
     const int64_t off = row * a.ldp + col;
@@ -28,7 +29,7 @@ apply_update_kernel(ApplyArgs a) {
       den *= sc;
       pos = fmaxf(den, 0.f) + kEps;                          // nmf.py:83
     } else {
-      pos = a.kl_den[r];                                     // nmf.py:368-369 / :381-382 (no relu, no eps)
+      pos = a.kl_den[b * a.R + r];                           // nmf.py:368-369 / :381-382 (no relu, no eps)
     }
     if (a.l1 > 0.f) pos += a.l1;                             // nmf.py:85-86
     if (a.l2 > 0.f) pos = fmaf(a.l2, p, pos);                // nmf.py:87-88
@@ -54,7 +55,7 @@ apply_update_kernel(ApplyArgs a) {
 __global__ void __launch_bounds__(256)
 raw_sum_kernel(ApplyArgs a, float* __restrict__ num_out, float* __restrict__ den_out) {
   const int64_t idx = (int64_t)blockIdx.x * 256 + threadIdx.x;
-  if (idx >= a.numel) return;
+  if (idx >= a.numel || batch_skips(a.active, a.prob_numel ? idx / a.prob_numel : 0)) return;
   const int64_t row = idx / a.rowlen;
   const int64_t off = row * a.ldp + (idx - row * a.rowlen);
   const float sc = a.out_scale ? *a.out_scale : 1.0f;
@@ -71,16 +72,22 @@ raw_sum_kernel(ApplyArgs a, float* __restrict__ num_out, float* __restrict__ den
 }
 
 // stage 1 for inner == 1: x is (outer, R) row-major; block (b, y) sums a row slab of components [256 y, 256 y + 256).
+// Batch: nb blocks per problem along x, each problem's x and partials nprob-strided (outer R and nb R floats).
 __global__ void __launch_bounds__(256)
 colsum_rows_kernel(const float* __restrict__ x, int64_t outer, int R, int64_t rows_per_block,
-                   float* __restrict__ partial) {
+                   float* __restrict__ partial, int64_t nb, const uint8_t* __restrict__ active) {
   __shared__ float sh[256];
+  const int64_t prob = (int64_t)blockIdx.x / nb;
+  if (batch_skips(active, prob)) return;
+  x += prob * outer * R;
+  partial += prob * nb * R;
+  const int64_t bx = (int64_t)blockIdx.x - prob * nb;
   const int tid = threadIdx.x;
   const int r0 = blockIdx.y * 256;
   const int Rb = min(R - r0, 256);               // this block's components
   const int ng = 256 / Rb > 0 ? 256 / Rb : 1;    // row groups
   const int g = tid / Rb, r = tid - g * Rb;
-  const int64_t row0 = (int64_t)blockIdx.x * rows_per_block;
+  const int64_t row0 = bx * rows_per_block;
   const int64_t row1 = min(outer, row0 + rows_per_block);
   float acc = 0.f;
   if (g < ng)
@@ -90,7 +97,7 @@ colsum_rows_kernel(const float* __restrict__ x, int64_t outer, int R, int64_t ro
   if (tid < Rb) {
     float t = 0.f;
     for (int k = 0; k < ng; ++k) t += sh[k * Rb + tid];
-    partial[(int64_t)blockIdx.x * R + r0 + tid] = t;
+    partial[bx * R + r0 + tid] = t;
   }
 }
 
@@ -111,8 +118,15 @@ colsum_runs_kernel(const float* __restrict__ x, int64_t inner, float* __restrict
   }
 }
 
-__global__ void colsum_final_kernel(const float* __restrict__ partial, int64_t nb, int R, float* __restrict__ sums) {
-  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+// Batch: ceil(R / blockDim) blocks per problem along x
+__global__ void colsum_final_kernel(const float* __restrict__ partial, int64_t nb, int R, float* __restrict__ sums,
+                                    const uint8_t* __restrict__ active) {
+  const int64_t per = (R + blockDim.x - 1) / blockDim.x;
+  const int64_t prob = (int64_t)blockIdx.x / per;
+  if (batch_skips(active, prob)) return;
+  partial += prob * nb * R;
+  sums += prob * R;
+  const int r = (int)((int64_t)blockIdx.x - prob * per) * blockDim.x + threadIdx.x;
   if (r >= R) return;
   float t = 0.f;
   for (int64_t b = 0; b < nb; ++b) t += partial[b * R + r];
@@ -124,17 +138,20 @@ __device__ __forceinline__ float nan_max(float a, float b) { return (a != a || b
 
 // NaN-sticky min / max so that a NaN in V fails fit()'s non-negativity assertion like torch.all(V >= 0) does
 // SEL: the cells where M (contiguous rows x cols: a mask or weights) is 0 are skipped, V is not read there
+// Batch: nprob matrices of rows x cols, bstride elements apart
 template <typename TV, typename SEL = NoSel>
 __global__ void __launch_bounds__(256)
 minmax_stage1(const TV* __restrict__ V, int64_t rows, int64_t cols, int64_t ld, float* __restrict__ scratch,
-              const SEL* __restrict__ M) {
+              const SEL* __restrict__ M, int64_t nprob, int64_t bstride) {
   __shared__ float smin[8], smax[8];
   float mn = INFINITY, mx = -INFINITY;
-  const int64_t total = rows * cols;
+  const int64_t total = nprob * rows * cols;
   for (int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x; i < total; i += (int64_t)gridDim.x * 256) {
     if (!sel_set(M, i)) continue;
     int64_t r = i / cols, c = i - r * cols;
-    float v = to_f32(V[r * ld + c]);
+    const int64_t b = nprob > 1 ? r / rows : 0;
+    r -= b * rows;
+    float v = to_f32(V[b * bstride + r * ld + c]);
     mn = nan_min(mn, v);
     mx = nan_max(mx, v);
   }
@@ -167,7 +184,8 @@ __global__ void __launch_bounds__(256)
 apply_update_vec4_kernel(ApplyArgs a) {
   const int64_t idx = ((int64_t)blockIdx.x * 256 + threadIdx.x) * 4;
   float m = 0.f;
-  if (idx < a.numel) {
+  const int64_t b = a.prob_numel ? idx / a.prob_numel : 0;      // Batch: prob_numel is a multiple of 4 here
+  if (idx < a.numel && !batch_skips(a.active, b)) {
     const int64_t row = idx / a.rowlen;
     const int64_t off = row * a.ldp + (idx - row * a.rowlen);
     const int r = (int)((idx / a.inner) % a.R);
@@ -184,7 +202,7 @@ apply_update_vec4_kernel(ApplyArgs a) {
         den.x += t.x; den.y += t.y; den.z += t.z; den.w += t.w;
       }
     }
-    const float klden = a.den ? 0.f : a.kl_den[r];
+    const float klden = a.den ? 0.f : a.kl_den[b * a.R + r];
     float4 p = *reinterpret_cast<const float4*>(a.param + idx);
     auto one = [&](float pv, float n, float d) {
       n *= sc;
@@ -217,7 +235,7 @@ static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 
 
 bool apply_update_vec4_shape(const ApplyArgs& a) {
   return a.inner % 4 == 0 && a.rowlen % 4 == 0 && a.ldp % 4 == 0 && a.numel % 4 == 0 &&
-         (a.nchunks == 1 || a.chunk_stride % 4 == 0);
+         (a.nchunks == 1 || a.chunk_stride % 4 == 0) && a.prob_numel % 4 == 0;
 }
 
 int apply_update(const ApplyArgs& a, cudaStream_t st) {
@@ -247,30 +265,35 @@ static int64_t colsum_blocks(int64_t outer, int64_t inner) {
 int64_t colsum_scratch_floats(int64_t outer, int R, int64_t inner) { return colsum_blocks(outer, inner) * R; }
 
 int factor_colsum(const float* x, int64_t outer, int R, int64_t inner, float* scratch, int64_t scratch_floats,
-                  float* sums, cudaStream_t st) {
+                  float* sums, cudaStream_t st, int64_t nprob, const uint8_t* active) {
   const int64_t nb = colsum_blocks(outer, inner);
-  if (nb * R > scratch_floats) { set_error("factor_colsum: scratch too small"); return 1; }
+  if (nprob < 1 || (nprob > 1 && inner > 1)) { set_error("factor_colsum: a batch needs inner == 1"); return 1; }
+  if ((double)nb * R * nprob > (double)scratch_floats) { set_error("factor_colsum: scratch too small"); return 1; }
+  if (nb * nprob > kMaxGridX || ceil_div(R, 64) * nprob > kMaxGridX) { set_error("factor_colsum: batch passes grid x"); return 1; }
   if (inner > 1) {
     colsum_runs_kernel<<<(unsigned)(outer * R), 256, 0, st>>>(x, inner, scratch);
   } else {
     const int64_t rpb = ceil_div(outer, nb);
-    colsum_rows_kernel<<<dim3((unsigned)nb, (unsigned)ceil_div(R, 256)), 256, 0, st>>>(x, outer, R, rpb, scratch);
+    colsum_rows_kernel<<<dim3((unsigned)(nb * nprob), (unsigned)ceil_div(R, 256)), 256, 0, st>>>(x, outer, R, rpb, scratch,
+                                                                                                  nb, active);
   }
   NMF_LAUNCH_CHECK();
-  colsum_final_kernel<<<(unsigned)ceil_div(R, 64), 64, 0, st>>>(scratch, nb, R, sums);
+  colsum_final_kernel<<<(unsigned)(ceil_div(R, 64) * nprob), 64, 0, st>>>(scratch, nb, R, sums, active);
   NMF_LAUNCH_CHECK();
   return 0;
 }
 
 int matrix_minmax(const void* V, int vdtype, int64_t rows, int64_t cols, int64_t ld, float* scratch2048, float* mm,
-                  cudaStream_t st, CellSel M) {
-  int64_t nb = ceil_div(rows * cols, 256 * 16);
+                  cudaStream_t st, CellSel M, int64_t nprob, int64_t bstride) {
+  if (nprob < 1 || (nprob > 1 && M)) { set_error("matrix_minmax: a batch takes no selector"); return 1; }
+  int64_t nb = ceil_div(nprob * rows * cols, 256 * 16);
   if (nb > 1024) nb = 1024;
   if (nb < 1) nb = 1;
   int rc = with_vtype(V, vdtype, [&](auto Vt) {
     using TV = vtype_t<decltype(Vt)>;
     return with_sel(M, [&](auto Mk) {
-      minmax_stage1<TV, sel_t<decltype(Mk)>><<<(unsigned)nb, 256, 0, st>>>(Vt, rows, cols, ld, scratch2048, Mk);
+      minmax_stage1<TV, sel_t<decltype(Mk)>><<<(unsigned)nb, 256, 0, st>>>(Vt, rows, cols, ld, scratch2048, Mk, nprob,
+                                                                          bstride);
       NMF_LAUNCH_CHECK();
       return 0;
     });

@@ -66,6 +66,11 @@ def _workspace_bytes(key):
             p = _capi.nmf_plan(N, C, R)
             est += 8 * R * max(p["nch_w"] * C, p["nch_h"] * N)
         return est
+    if key[0] == "nmf_batched":           # ("nmf_batched", device, B, N, C, R): B x the fp32 context of one problem
+        _, _, B, N, C, R = key
+        p = _capi.nmf_plan(N, C, R)
+        return B * (8 * R * max(p["nch_w"] * C, p["nch_h"] * N) + 8 * R + 8 * p["loss_chunks"] * ((N + 63) // 64)
+                    + 4 * R * max(p["colsum_blocks_n"], p["colsum_blocks_c"])) + (1 << 14)
     if key[0] == "nmfd":                  # ("nmfd", device, B, C, X, R, K, precision): ratio tiles + shifted operand copies
         _, _, B, C, X, R, K = key[:7]
         nx, nk = 1, 1
@@ -339,6 +344,83 @@ class CudaNmfEngine(_CudaEngine):
     def update_w_peer(self, beta, gamma, l1_reg, l2_reg):
         _capi.check(self._lib.nmfb200_nmf_update_w_peer(self._ctx, _ptr(self.W), _ptr(self.H), beta, gamma, l1_reg,
                                                         l2_reg, _stream(self.device)))
+
+
+class CudaBatchedNmfEngine(_CudaEngine):
+    """B independent dense NMF problems of one shape on one GPU (include/nmf_b200.h: nmfb200_nmf_batched_create), on the
+    fp32 kernels: V (B,N,C) -- or (N,C), one target shared by every problem -- fp32, fp16 or bf16 with unit column stride,
+    rows and problems strided; W (B,C,R) and H (B,N,R) contiguous fp32, updated in place.  Every update and loss launch
+    runs all problems, and problem b's factors and loss are bit for bit those of CudaNmfEngine(V[b], W[b], H[b], "f32")."""
+    kind = "nmf_batched"
+
+    def __init__(self, V, W, H):
+        super().__init__()
+        self.device = W.device
+        if V.dim() == 2:
+            V = V.unsqueeze(0).expand(W.shape[0], *V.shape)              # one target: batch stride 0
+        if V.dtype not in _capi.DTYPES:
+            raise TypeError(f"V must be float32, float16 or bfloat16 (got {V.dtype})")
+        if V.device != self.device:
+            raise ValueError(f"V is on {V.device}, expected {self.device}")
+        for t, n in ((W, "W"), (H, "H")):
+            _check_f32_cuda(t, n, self.device)
+        B, N, C = V.shape
+        R = W.shape[2]
+        assert W.shape == (B, C, R) and H.shape == (B, N, R)
+        if not (V.stride(2) == 1 and V.stride(1) >= C and (V.stride(0) == 0 or V.stride(0) >= N * V.stride(1))):
+            raise ValueError("V must have unit column stride, rows at least C apart and problems at least N rows apart")
+        self.V, self.W, self.H = V, W, H
+        self.B, self.N, self.C, self.R = B, N, C, R
+        self._active = None
+        dev_index = self.device.index if self.device.index is not None else torch.cuda.current_device()
+        self._acquire(("nmf_batched", dev_index, B, N, C, R),
+                      lambda ref: self._lib.nmfb200_nmf_batched_create(ref, dev_index, B, N, C, R))
+        self._loss = torch.zeros(B, dtype=torch.float64, device=self.device)
+        _capi.check(self._lib.nmfb200_nmf_batched_set_target(self._ctx, _ptr(V), V.stride(1), V.stride(0),
+                                                             _capi.DTYPES[V.dtype], _stream(self.device)))
+        _capi.check(self._lib.nmfb200_nmf_batched_set_active(self._ctx, None, _stream(self.device)))
+        self.sync()
+
+    @property
+    def precision(self):
+        return "f32"
+
+    def precision_for(self, beta):
+        return "f32"
+
+    def set_active(self, active):
+        """Run only the problems whose flag is set from now on: `active` is a bool sequence or tensor of B flags (None: all).
+        The others keep their factors and their slot of losses()."""
+        if active is None:
+            self._active = None
+        else:
+            self._active = torch.as_tensor(active).to(device=self.device, dtype=torch.uint8).contiguous()
+            assert self._active.shape == (self.B,)
+        _capi.check(self._lib.nmfb200_nmf_batched_set_active(
+            self._ctx, _ptr(self._active) if self._active is not None else None, _stream(self.device)))
+
+    def iterate(self, n_iter, beta, gamma, l1_reg, l2_reg):
+        """n_iter x (update_w; update_h) of every active problem in one call."""
+        _capi.check(self._lib.nmfb200_nmf_iterate(self._ctx, _ptr(self.W), _ptr(self.H), beta, gamma, l1_reg, l2_reg,
+                                                  int(n_iter), _stream(self.device)))
+
+    def losses(self, beta):
+        """beta_div of every problem's reconstruction as B float64 values on the host (one synchronisation); an inactive
+        problem's value is the last one computed for it."""
+        val = self.loss_tensor(beta).cpu()
+        self.check_health()
+        return val
+
+    def loss(self, beta):
+        raise TypeError("a batched engine has one loss per problem: use losses()")
+
+    def raw_terms(self, which, beta):
+        """(numerator, denominator) of every problem's update of W (which=0) or H (which=1): the numerator in the factor's
+        shape (B, rows, R); the denominator (B, R) at beta 1 (the column sums of the other factor), else (B, rows, R)."""
+        f = self.W if which == 0 else self.H
+        buf = self._raw_terms_into(which, beta, None)
+        num, den = buf[:f.numel()].view(f.shape), buf[f.numel():]
+        return num, (den.view(self.B, self.R) if beta == 1 else den.view(f.shape))
 
 
 def _compressed_forms(V, weights=None):

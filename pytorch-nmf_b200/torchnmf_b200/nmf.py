@@ -36,7 +36,7 @@ try:
 except Exception:  # pragma: no cover
     _tqdm = None
 
-__all__ = ["BaseComponent", "NMF", "NMFD", "NMF2D", "NMF3D"]
+__all__ = ["BaseComponent", "NMF", "NMFD", "NMF2D", "NMF3D", "BatchedNMF"]
 
 
 def _gamma(beta):
@@ -683,6 +683,184 @@ class NMFD(BaseComponent):
         if not ok:
             raise RuntimeError(f"target shape {tuple(V.shape)} does not match H {tuple(self.H.shape)} / "
                                f"W {tuple(self.W.shape)}")
+
+
+class BatchedNMF(BaseComponent):
+    """B independent NMF problems of one shape:  V[b] (N,C) ~= H[b] (N,R) @ W[b] (C,R)^T,  W (B,C,R), H (B,N,R).
+
+    Args:
+        Vshape: (B, N, C); W and H are then drawn as `NMF` draws them, |randn| of (B, C, rank) and (B, N, rank)
+        rank: size of the hidden dimension (default: C); the last axis of W and H
+        W / H: a size (iterable of ints -> random non-negative init) or an initial non-negative Tensor
+        trainable_W / trainable_H: whether a *given tensor* is updated by `fit`
+    """
+
+    def __init__(self, Vshape=None, rank=None, *, W=None, H=None, trainable_W=True, trainable_H=True):
+        torch.nn.Module.__init__(self)
+        if isinstance(Vshape, _Iterable):
+            B, N, C = Vshape
+            rank = rank if rank else C
+            W = (B, C, rank) if W is None else W
+            H = (B, N, rank) if H is None else H
+        inferred = None
+        for name, spec, trainable in (("W", W, trainable_W), ("H", H, trainable_H)):
+            if isinstance(spec, Tensor):
+                assert torch.all(spec >= 0.), f"Tensor {name} should be non-negative."
+                p = Parameter(torch.empty(*spec.size()), requires_grad=trainable)
+                p.data.copy_(spec)
+            elif isinstance(spec, _Iterable):
+                p = Parameter(torch.randn(*tuple(spec)).abs())
+            else:
+                p = None
+            self.register_parameter(name, p)
+            if p is not None:
+                if p.dim() != 3:
+                    raise ValueError(f"{name} must have three axes (B, rows, rank); got shape {tuple(p.shape)}")
+                if inferred is not None and p.shape[2] != inferred:
+                    raise ValueError("Latent size of H does not match with W")
+                inferred = p.shape[2]
+        if inferred is None:
+            assert rank, "A rank should be given when W and H are not available!"
+        else:
+            rank = inferred
+        if self.W is not None and self.H is not None and self.W.shape[0] != self.H.shape[0]:
+            raise ValueError(f"W and H hold different numbers of problems ({self.W.shape[0]} and {self.H.shape[0]})")
+        if self.W is not None:
+            self.out_channels = self.W.shape[1]
+        self.rank = rank
+
+    @staticmethod
+    def reconstruct(H, W):
+        return H @ W.transpose(-1, -2)
+
+    def _check_target_shape(self, V):
+        B, N, _ = self.H.shape
+        C = self.W.shape[1]
+        if tuple(V.shape) not in ((B, N, C), (N, C)):
+            raise ValueError(f"target shape {tuple(V.shape)} does not match H {tuple(self.H.shape)} / W {tuple(self.W.shape)}: "
+                             f"expected ({B}, {N}, {C}) or ({N}, {C})")
+
+    def sparse_fit(self, *args, **kwargs):
+        raise NotImplementedError("BatchedNMF has no sparse_fit: fit each problem with NMF.sparse_fit")
+
+    @torch.no_grad()
+    def fit(self, V, beta=1, tol=1e-4, max_iter=200, verbose=False, alpha=0, l1_ratio=0, *, precision="auto"):
+        """Fit every problem by multiplicative updates, as `NMF.fit(V[b], ...)` fits one, all of them in the same launches.
+
+        V: (B, N, C), or (N, C) -- one target shared by every problem (random restarts of one fit).  Dense float32,
+        float16 or bfloat16, read in place if its columns have unit stride (rows and problems may be strided; an expanded
+        (N, C) tensor is read once); float64 and other layouts are staged through one fp32 (or same-dtype contiguous)
+        copy on the device.  A sparse V raises NotImplementedError.
+
+        Returns a torch.int64 tensor of B iteration counts.  Problem b follows the reference's stop rule (nmf.py:366-409) on
+        its own: its loss sqrt(2 d_b) at the start and every 10th iteration, and it stops at the first check where
+        (previous_b - loss_b) / init_b < tol; from then on every kernel leaves its factors untouched while the others run
+        on.  n_iter[b], W[b] and H[b] equal, bit for bit, those of `NMF(W=W0[b], H=H0[b]).fit(V[b], ..., precision="f32")`:
+        each problem keeps the single fit's tile plan and summation order.  The losses cost one synchronisation per 10
+        iterations for the whole batch.
+
+        Every beta, `alpha` / `l1_ratio` and frozen factors (trainable_W / trainable_H) are supported, for 1 <= R <= 256,
+        on the fp32 CUDA-core kernels: precision "auto" and "f32" run them (`last_fit_precision` is "f32"); "f16" and
+        "f16_split" raise ValueError, as do R > 256 and shape mismatches.  Validation is the reference's over every problem:
+        a negative V fails its assertion, and beta <= 0 with a zero anywhere in V raises ValueError.  `mask`, `weight` and
+        `group` are not parameters of this class (TypeError).  Host or half-precision modules are staged through fp32
+        device copies and written back, as by `NMF.fit`.
+
+        Workspace (device memory, kept between fits of the same shape like `NMF.fit`'s): B times that of one fp32 NMF
+        problem -- the chunked partial numerators and denominators, 8 R max(nch_w C, nch_h N) bytes with up to 32 chunks
+        per contraction (`_capi.nmf_plan(N, C, R)`), plus the column sums and loss partials -- so it grows linearly with B.
+        """
+        if precision not in ("auto", "f32"):
+            if precision in ("f16", "f16_split"):
+                raise ValueError(f"BatchedNMF runs on the fp32 kernels: precision must be 'auto' or 'f32' (got {precision!r})")
+            raise ValueError(f"unknown precision {precision!r}")
+        if V.is_sparse:
+            raise NotImplementedError("BatchedNMF takes dense targets only")
+        W, H = self.W, self.H
+        assert W is not None and H is not None, "fit() needs both W and H"
+        if W.shape[2] > 256:
+            raise ValueError(f"BatchedNMF supports rank <= 256 (got {W.shape[2]})")
+        self._check_target_shape(V)
+        B = W.shape[0]
+
+        staged = False
+        if self._engine_factory is None:
+            if not torch.cuda.is_available():
+                raise RuntimeError("torchnmf_b200.fit needs a CUDA device (sm_90a); there is no CPU fallback")
+            f32 = torch.float32
+            on_gpu = W.device.type == "cuda"
+            dev = W.device if on_gpu else torch.device("cuda", torch.cuda.current_device())
+            Vd = V.to(dev, non_blocking=True)
+            if Vd.dtype not in (torch.float32, torch.float16, torch.bfloat16):
+                Vd = Vd.to(f32)
+            n = Vd.dim()
+            rows_ok = Vd.stride(-1) == 1 and Vd.stride(-2) >= Vd.shape[-1]
+            if not (rows_ok and (n == 2 or Vd.stride(0) == 0 or Vd.stride(0) >= Vd.shape[1] * Vd.stride(1))):
+                Vd = Vd.contiguous()
+            if on_gpu and W.dtype == f32 and H.dtype == f32 and W.is_contiguous() and H.is_contiguous():
+                Wd, Hd = W.data, H.data
+            else:
+                staged = True
+                Wd = W.data.to(dev, f32, non_blocking=True).contiguous()
+                Hd = H.data.to(dev, f32, non_blocking=True).contiguous()
+            eng = _engine.CudaBatchedNmfEngine(Vd, Wd, Hd)
+        else:
+            Wd, Hd = W.data, H.data
+            eng = self._engine_factory(V, Wd, Hd)
+
+        try:
+            vmin, vmax = eng.minmax()
+            assert vmin >= 0., "Target should be non-negative."                            # nmf.py:329-330
+            if vmin == 0 and beta <= 0:                                                    # nmf.py:332-336
+                raise ValueError("When beta <= 0 and V contains zeros, the training process may diverge. "
+                                 "Please add small values to V, or use a positive beta value.")
+            gamma = _gamma(beta)
+            l1_reg = alpha * l1_ratio                                                      # nmf.py:348
+            l2_reg = alpha * (1 - l1_ratio)                                                # nmf.py:349
+
+            def fit_losses():
+                d = eng.losses(beta).to(torch.float64)
+                return torch.where(d >= 0, torch.sqrt(2.0 * d.clamp(min=0)), float("nan"))  # nmf.py:362,402
+
+            loss_init = fit_losses()
+            previous = loss_init.clone()
+            n_iter = torch.full((B,), max_iter, dtype=torch.int64)
+            active = torch.ones(B, dtype=torch.bool)
+            train_w, train_h = W.requires_grad, H.requires_grad
+            bar = _tqdm(total=max_iter, disable=not verbose) if _tqdm is not None else _NullBar()
+            it = -1
+            with bar as pbar:
+                while it + 1 < max_iter and bool(active.any()):
+                    k = min(10 - ((it + 1) % 10), max_iter - (it + 1))
+                    if train_w and train_h:
+                        eng.iterate(k, beta, gamma, l1_reg, l2_reg)                        # nmf.py:366-391, k times
+                    else:
+                        for _ in range(k):
+                            if train_w:
+                                eng.update_w(beta, gamma, l1_reg, l2_reg)                  # nmf.py:367-378
+                            if train_h:
+                                eng.update_h(beta, gamma, l1_reg, l2_reg)                  # nmf.py:380-391
+                    it += k
+                    if it % 10 == 9:                                                       # nmf.py:393
+                        loss = fit_losses()
+                        with torch.no_grad():
+                            stop = active & ((previous - loss) / loss_init < tol)          # nmf.py:405, per problem
+                        n_iter[stop] = it + 1
+                        previous = torch.where(active & ~stop, loss, previous)
+                        pbar.set_postfix(active=int((active & ~stop).sum()))
+                        pbar.update(10)
+                        if bool(stop.any()):
+                            active &= ~stop
+                            eng.set_active(active)
+            if hasattr(eng, "check_health"):
+                eng.check_health()
+            if staged:
+                W.data.copy_(Wd)
+                H.data.copy_(Hd)
+            self.last_fit_precision = "f32"
+        finally:
+            eng.close()
+        return n_iter
 
 
 def _ntuple(x, n):
