@@ -20,7 +20,8 @@
  *       NMFD: V (B,C,L) W (C,R,T) H (B,R,L-T+1)      V ~= conv1d(H, flip(W)) (nmf.py:743-750)
  *   - a context holds one model, NMF or NMFD (NMF2D / NMF3D included), fixed by its create call.  The nmfb200_nmf_* and
  *     nmfb200_nmfd_* calls take only contexts of their model (NMFB200_ERR_INVALID, "wrong context kind", otherwise); the
- *     calls without a model in their name serve both.
+ *     calls without a model in their name serve both.  A batched context (nmfb200_nmf_batched_create,
+ *     nmfb200_nmfnd_batched_create) holds many problems of one model; its own calls are named after their kind.
  *   - `stream` is a cudaStream_t passed as void* (0 = legacy default stream).  Every call is
  *     asynchronous on that stream unless documented as synchronising.
  *   - W / H are the caller's storages (the nn.Parameter .data of the reference); updates are
@@ -225,6 +226,36 @@ int nmfb200_nmfnd_create(nmfb200_ctx** out, int device, int64_t B, int64_t C, in
                          int64_t R, const int64_t* kdims, int precision);
 /* Register a contiguous target of element type `dtype` (NMFB200_DTYPE_*), with the checks of nmfb200_nmf_set_target. */
 int nmfb200_nmfd_set_target(nmfb200_ctx* ctx, const void* V, int dtype, void* stream);
+
+/* ---- batched NMFD / NMF2D / NMF3D: many independent problems of one shape in one context ---------------------------- */
+
+/* A context for P independent NMFD / NMF2D / NMF3D problems of one shape, on the fp32 CUDA-core kernels.  Each problem has
+ * the shape of nmfb200_nmfnd_create(B, C, ndim, vdims, R, kdims) (the same checks apply to it): problem p has the target
+ * V_p (B,C,*vdims) and the factors W_p = W + p C R prod(kdims) and H_p = H + p B R prod(vdims - kdims + 1) of the caller's
+ * (P,C,R,*kdims) / (P,B,R,*(vdims - kdims + 1)) storages; its B clips share W_p.  Every reconstruction, wgrad, dgrad,
+ * column-sum and ratio-stage launch runs all P problems at once (grid z of the sliding kernels holds P x B lines, problem
+ * after problem; grid z of wgrad P x its splits, in launches of at most 65535), and each problem keeps the plan and
+ * summation order of a single NMFB200_PREC_F32 context of its shape: the same wgrad / dgrad splits, tiles and loss blocks,
+ * so its factors and loss are, bit for bit, that context's.  Workspace: P times the fp32 NMFD context's -- the ratio tile Pn
+ * (and Pp at beta != 1) of V's size, the split partial slabs, the column sums and the loss partials.
+ * NMFB200_ERR_INVALID, naming the limit, for P < 1, P x B >= 2^31 (the kernels' line index), P x loss partials per problem
+ * >= 2^31, P x column-sum blocks past grid x, or P x B x C x prod(vdims) > 2^46.
+ * On a batched NMFD context: nmfb200_update_w / _update_h / nmfb200_sync_factors serve it; nmfb200_loss writes P doubles
+ * (loss_dev[p]); nmfb200_raw_terms returns [P x factor numerators | P R column sums (beta 1) or P x factor denominators],
+ * nmfb200_raw_terms_numel reports that length; nmfb200_target_minmax covers every problem; nmfb200_precision_for_beta
+ * reports NMFB200_PREC_F32.  nmfb200_set_mask, nmfb200_set_weight, nmfb200_w_apply, nmfb200_nmfd_set_target and every
+ * nmfb200_nmf_* call return NMFB200_ERR_INVALID.  The two calls below take batched NMFD contexts only. */
+int nmfb200_nmfnd_batched_create(nmfb200_ctx** out, int device, int64_t P, int64_t B, int64_t C, int ndim,
+                                 const int64_t* vdims, int64_t R, const int64_t* kdims);
+/* Register the targets: problem p reads the contiguous block V + p problem_stride of B C prod(vdims) elements of type
+ * `dtype`.  problem_stride 0: one V shared by every problem (restarts of one fit); otherwise problem_stride >=
+ * B C prod(vdims).  Checks as nmfb200_nmfd_set_target; the min / max run over every problem.  V stays borrowed.
+ * Asynchronous. */
+int nmfb200_nmfd_batched_set_target(nmfb200_ctx* ctx, const void* V, int64_t problem_stride, int dtype, void* stream);
+/* Which problems run from now on, with the contract of nmfb200_nmf_batched_set_active: `active` is P device bytes, borrowed,
+ * null = every problem; a problem flagged 0 is skipped by every launch (its factors, loss_dev slot and raw-terms slots are
+ * left as they are) at the cost of one flag read per block. */
+int nmfb200_nmfd_batched_set_active(nmfb200_ctx* ctx, const uint8_t* active, void* stream);
 
 /* ---- both models ------------------------------------------------------------------------- */
 

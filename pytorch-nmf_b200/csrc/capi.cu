@@ -18,14 +18,16 @@ void count_launch() { g_launches.fetch_add(1, std::memory_order_relaxed); }
 using namespace nmfb200;
 
 struct nmfb200_ctx {
-  int kind = 0;            // 0 = NMF, 1 = NMFD, 2 = a batch of NMF problems (nmfb200_nmf_batched_create)
+  int kind = 0;            // 0 = NMF, 1 = NMFD, 2 = a batch of NMF problems (nmfb200_nmf_batched_create), 3 = a batch of
+                           // NMFD / NMF2D / NMF3D problems (nmfb200_nmfnd_batched_create)
   int device = 0;
   int precision = NMFB200_PREC_F32;
   bool auto_mode = false;   // precision AUTO: the tensor-core path is used only where it is known to hold the parity bar
   bool tc_off = false;      // AUTO found the target outside the fp16 operand range: fp32 CUDA-core kernels instead
   int64_t N = 0, C = 0, R = 0;
-  // a batch (kind 2): nprob problems of the shape (N, C, R), their targets bstride elements apart (0: one shared target),
-  // factors and partial slabs back to back; `active` (borrowed, nprob device bytes, null: all) flags the problems that run
+  // a batch (kind 2 or 3): nprob problems of the shape (N, C, R) or d, their targets bstride elements apart (0: one shared
+  // target), factors and partial slabs back to back; `active` (borrowed, nprob device bytes, null: all) flags the problems
+  // that run
   int64_t nprob = 1, bstride = 0;
   const uint8_t* active = nullptr;
   NmfdShape d{};
@@ -91,11 +93,14 @@ struct DeviceGuard {
   DeviceGuard& operator=(const DeviceGuard&) = delete;
 };
 
-// want_kind: 0 = NMF, 1 = NMFD, 2 = batched NMF, kAnyKind for the calls that serve every kind, kDenseNmf for those that
-// serve NMF and batched NMF
+// want_kind: 0 = NMF, 1 = NMFD, 2 = batched NMF, 3 = batched NMFD, kAnyKind for the calls that serve every kind, kDenseNmf
+// for those that serve NMF and batched NMF
 constexpr int kAnyKind = -1;
 constexpr int kDenseNmf = -2;
 constexpr int kBatched = 2;
+constexpr int kBatchedNmfd = 3;
+inline bool is_nmfd(const nmfb200_ctx* c) { return c->kind == 1 || c->kind == kBatchedNmfd; }
+inline bool is_batch(const nmfb200_ctx* c) { return c->kind == kBatched || c->kind == kBatchedNmfd; }
 inline bool kind_ok(const nmfb200_ctx* c, int want) {
   return want == kAnyKind || c->kind == want || (want == kDenseNmf && (c->kind == 0 || c->kind == kBatched));
 }
@@ -183,7 +188,7 @@ void mark_stale(nmfb200_ctx* c, bool w, bool h) {
 struct FactorDims { int64_t rows, inner, other_rows, other_inner; };
 FactorDims factor_dims(const nmfb200_ctx* c, int which) {
   const NmfdShape& d = c->d;
-  const FactorDims w = c->kind != 1 ? FactorDims{c->C, 1, c->N, 1} : FactorDims{d.C, d.w_inner(), d.B, d.h_inner()};
+  const FactorDims w = !is_nmfd(c) ? FactorDims{c->C, 1, c->N, 1} : FactorDims{d.C, d.w_inner(), d.B, d.h_inner()};
   return which == 0 ? w : FactorDims{w.other_rows, w.other_inner, w.rows, w.inner};
 }
 
@@ -194,7 +199,7 @@ ApplyArgs factor_view(const nmfb200_ctx* c, int which, int nchunks) {
   ApplyArgs a{};
   a.R = (int)c->R; a.inner = f.inner; a.rowlen = c->R * f.inner; a.ldp = a.rowlen;
   a.numel = f.rows * a.rowlen * c->nprob; a.chunk_stride = a.numel; a.nchunks = nchunks;
-  if (c->kind == kBatched) { a.prob_numel = f.rows * a.rowlen; a.active = c->active; }
+  if (is_batch(c)) { a.prob_numel = f.rows * a.rowlen; a.active = c->active; }
   return a;
 }
 
@@ -591,6 +596,64 @@ int nmfb200_nmfd_set_target(nmfb200_ctx* ctx, const void* V, int dtype, void* st
   return 0;
 }
 
+/* ---- batched NMFD / NMF2D / NMF3D: P independent problems of one shape on the fp32 kernels ------------------------ */
+
+int nmfb200_nmfnd_batched_create(nmfb200_ctx** out, int device, int64_t P, int64_t B, int64_t C, int ndim,
+                                 const int64_t* vdims, int64_t R, const int64_t* kdims) {
+  if (!out) return fail(NMFB200_ERR_INVALID, "out is null");
+  *out = nullptr;
+  if (P < 1) return fail(NMFB200_ERR_INVALID, "P must be positive");
+  NmfdShape d;
+  if (int rc = nmfd_shape_of(B, C, ndim, vdims, R, kdims, &d)) return rc;
+  // the problems ride on grid z of the sliding kernels (int line index b0 + z) and of wgrad (sliced), on grid x of the
+  // column sums, and their loss partials are counted in int
+  const int64_t vol = B * C * d.v_inner();
+  if (P > INT32_MAX / B)
+    return fail(NMFB200_ERR_INVALID, "batched NMFD: P x B must be below 2^31 (the line index of the fp32 kernels)");
+  if (nmfd_max_blocks(d) > INT32_MAX / P)
+    return fail(NMFB200_ERR_INVALID, "batched NMFD: P x loss partials per problem must be below 2^31");
+  const int64_t cs_w = colsum_scratch_floats(C, (int)R, d.w_inner()), cs_h = colsum_scratch_floats(B, (int)R, d.h_inner());
+  if ((double)(d.w_inner() > 1 ? cs_w : cs_w / R) * P > (double)kMaxGridX ||
+      (double)(d.h_inner() > 1 ? cs_h : cs_h / R) * P > (double)kMaxGridX || ceil_div(R, 64) * P > kMaxGridX)
+    return fail(NMFB200_ERR_INVALID, "batched NMFD: P x column-sum blocks must be below 2^31 (grid x of the column sums)");
+  if ((double)vol * P > (double)((int64_t)1 << 46)) return fail(NMFB200_ERR_INVALID, "batched NMFD: targets too large");
+  DeviceGuard guard(device);
+  if (!guard.ok) return fail(NMFB200_ERR_CUDA, "cannot select the requested device");
+  nmfb200_ctx* c = new (std::nothrow) nmfb200_ctx();
+  if (!c) return fail(NMFB200_ERR_INVALID, "out of host memory");
+  c->kind = kBatchedNmfd; c->device = device; c->precision = NMFB200_PREC_F32; c->R = R; c->d = d; c->nprob = P;
+  // each problem's plan is the single problem's: same wgrad / dgrad splits, tiles, loss blocks and column-sum blocks
+  c->nslab[0] = nmfd_wgrad_nsplit(d);
+  c->nslab[1] = nmfd_dgrad_nsplit(d);
+  int64_t pf = (int64_t)c->nslab[0] * C * R * d.w_inner();
+  const int64_t hf = (int64_t)c->nslab[1] * B * R * d.h_inner();
+  if (hf > pf) pf = hf;
+  c->part_floats = pf * P;
+  c->cs_scratch_floats = (cs_w > cs_h ? cs_w : cs_h) * P;
+  c->loss_max_blocks = (int)(nmfd_max_blocks(d) * P);
+  if (int rc = alloc_workspace(c, vol * P)) return rc;
+  *out = c;
+  return 0;
+}
+
+int nmfb200_nmfd_batched_set_target(nmfb200_ctx* ctx, const void* V, int64_t problem_stride, int dtype, void* stream) {
+  CTX_GUARD(ctx, kBatchedNmfd);
+  if (int rc = check_target(V, dtype)) return rc;
+  const int64_t vin = ctx->d.v_inner(), rows = (int64_t)ctx->d.B * ctx->d.C;
+  if (problem_stride != 0 && problem_stride < rows * vin)
+    return fail(NMFB200_ERR_INVALID, "problem stride must be 0 (one shared target) or at least B x C x prod(X)");
+  ctx->V = V; ctx->vdtype = dtype; ctx->bstride = problem_stride; ctx->has_target = true;
+  return matrix_minmax(V, dtype, rows, vin, vin, ctx->mm_scratch, ctx->mm_scratch + kMmPartials, (cudaStream_t)stream,
+                       CellSel{}, problem_stride ? ctx->nprob : 1, problem_stride);
+}
+
+int nmfb200_nmfd_batched_set_active(nmfb200_ctx* ctx, const uint8_t* active, void* stream) {
+  CTX_GUARD(ctx, kBatchedNmfd);
+  (void)stream;
+  ctx->active = active;
+  return 0;
+}
+
 int nmfb200_nmfd_plan(int64_t B, int64_t C, int ndim, const int64_t* vdims, int64_t R, const int64_t* kdims, int64_t* out,
                       int n) {
   if (!out || n < NMFB200_NMFD_PLAN_LEN) return fail(NMFB200_ERR_INVALID, "plan buffer too small");
@@ -632,7 +695,7 @@ namespace {
 int set_selector(nmfb200_ctx* ctx, CellSel sel, void* stream) {
   CTX_GUARD(ctx, kAnyKind);
   TARGET_GUARD(ctx);
-  if (ctx->kind == kBatched) return fail(NMFB200_ERR_INVALID, "batched fits take no mask or weight");
+  if (is_batch(ctx)) return fail(NMFB200_ERR_INVALID, "batched fits take no mask or weight");
   if (ctx->sparse)
     return fail(NMFB200_ERR_INVALID, std::string(sel.kind == kSelWeight ? "a weight" : "a mask") +
                                          " needs a dense target (set_target or nmfd_set_target)");
@@ -717,13 +780,15 @@ int simt_contract(nmfb200_ctx* c, int which, const float* W, const float* H, dou
 int nmfd_contract(nmfb200_ctx* c, int which, const float* W, const float* H, double beta, cudaStream_t st) {
   const bool den = !kl_colsum(c, beta);
   if (den) {
-    if (!c->Pp) NMF_CUDA_CHECK(cudaMalloc(&c->Pp, (size_t)c->d.B * c->d.C * c->d.v_inner() * sizeof(float)));
+    if (!c->Pp) NMF_CUDA_CHECK(cudaMalloc(&c->Pp, (size_t)c->d.B * c->d.C * c->d.v_inner() * c->nprob * sizeof(float)));
     int e = ensure_den(c);
     if (e) return e;
   }
-  int rc = nmfd_recon_phi(c->d, c->V, c->vdtype, W, H, beta, c->Pn, c->Pp, nullptr, 0, nullptr, st, c->sel);
+  // a batch: every problem's tiles and split partials in the same launches (slab layout [split][problem][rows][R][inner])
+  const Batch bt{c->nprob, c->bstride, 0, 0, 0, c->active};
+  int rc = nmfd_recon_phi(c->d, c->V, c->vdtype, W, H, beta, c->Pn, c->Pp, nullptr, 0, nullptr, st, c->sel, bt);
   auto grad = [&](const float* P, float* out) {
-    return which == 0 ? nmfd_wgrad(c->d, P, H, out, c->nslab[0], st) : nmfd_dgrad(c->d, P, W, out, c->nslab[1], st);
+    return which == 0 ? nmfd_wgrad(c->d, P, H, out, c->nslab[0], st, bt) : nmfd_dgrad(c->d, P, W, out, c->nslab[1], st, bt);
   };
   if (rc == 0) rc = grad(c->Pn, c->num);
   if (rc == 0 && den) rc = grad(c->Pp, c->den);
@@ -764,7 +829,7 @@ int factor_terms(nmfb200_ctx* c, int which, const float* W, const float* H, doub
     else a.den = den_out;
     return sparse_terms(c, which, fac[which], fac[1 - which], beta, num_out, den_out, st);
   }
-  int rc = c->kind == 1 ? nmfd_contract(c, which, W, H, beta, st) : simt_contract(c, which, W, H, beta, st);
+  int rc = is_nmfd(c) ? nmfd_contract(c, which, W, H, beta, st) : simt_contract(c, which, W, H, beta, st);
   if (rc) return rc;
   a.num = c->num; a.nchunks = c->nslab[which];
   if (!kl) { a.den = c->den; return 0; }
@@ -942,10 +1007,10 @@ int nmfb200_loss(nmfb200_ctx* ctx, const float* W, const float* H, double beta, 
   TARGET_GUARD(ctx);
   if (!W || !H || !loss_dev) return fail(NMFB200_ERR_INVALID, "null pointer");
   cudaStream_t st = (cudaStream_t)stream;
-  if (ctx->kind == 1) {
+  if (is_nmfd(ctx)) {       // a batch: loss_dev[b] for every active problem b
     if (use_tc(ctx, beta)) return tc_nmfd_recon(ctx->tcd, ctx->V, ctx->vdtype, W, H, true, loss_dev, st);
     return nmfd_recon_phi(ctx->d, ctx->V, ctx->vdtype, W, H, beta, nullptr, nullptr, ctx->loss_blocks, ctx->loss_max_blocks,
-                          loss_dev, st, ctx->sel);
+                          loss_dev, st, ctx->sel, Batch{ctx->nprob, ctx->bstride, 0, 0, 0, ctx->active});
   }
   if (ctx->sparse) return sparse_loss_ctx(ctx, W, H, beta, loss_dev, st);
   if (use_tc(ctx, beta)) return tc_loss(ctx->tc, W, H, beta, loss_dev, st);
@@ -986,7 +1051,7 @@ int nmfb200_w_apply(nmfb200_ctx* ctx, float* W, const float* reduced, double bet
                     double l2_reg, void* stream) {
   CTX_GUARD(ctx, kAnyKind);
   TARGET_GUARD(ctx);
-  if (ctx->kind == kBatched) return fail(NMFB200_ERR_INVALID, "w_apply does not serve batched contexts");
+  if (is_batch(ctx)) return fail(NMFB200_ERR_INVALID, "w_apply does not serve batched contexts");
   if (!W || !reduced) return fail(NMFB200_ERR_INVALID, "null pointer");
   cudaStream_t st = (cudaStream_t)stream;
   if (ctx->tc && use_tc(ctx, beta)) return tc_w_apply(ctx->tc, W, reduced, beta, gamma, l1_reg, l2_reg, st);

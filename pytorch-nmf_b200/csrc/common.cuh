@@ -213,9 +213,9 @@ int apply_update(const ApplyArgs& a, cudaStream_t st);
 bool apply_update_vec4_shape(const ApplyArgs& a);
 // num_out[i] (and den_out[i] when a.den) = what the ratio stage would read for element i: summed partials + centring term
 int raw_sum(const ApplyArgs& a, float* num_out, float* den_out, cudaStream_t st);
-// sums[r] = sum over all other dims of x viewed as (outer, R, inner); deterministic two-stage.  nprob > 1 (inner 1 only):
-// sums[b R + r] for nprob consecutive (outer, R) problems, each summed in the single problem's order, skipping those whose
-// `active` flag is 0; scratch_floats then covers nprob x colsum_scratch_floats.
+// sums[r] = sum over all other dims of x viewed as (outer, R, inner); deterministic two-stage.  nprob > 1: sums[b R + r] for
+// nprob consecutive (outer, R, inner) problems, each summed in the single problem's order, skipping those whose `active`
+// flag is 0; scratch_floats then covers nprob x colsum_scratch_floats.
 int factor_colsum(const float* x, int64_t outer, int R, int64_t inner, float* scratch, int64_t scratch_floats,
                   float* sums, cudaStream_t st, int64_t nprob = 1, const uint8_t* active = nullptr);
 int64_t colsum_scratch_floats(int64_t outer, int R, int64_t inner);
@@ -282,18 +282,26 @@ struct NmfdShape {
 // reduces beta_div(WH, V) instead.  M (optional selector in V's layout): Pn = Pp = 0 at the missing cells and V is not read
 // there, Pp is written at every beta (beta 1: Pp = M as 0 / 1), and the loss skips them; a weight selector also multiplies
 // Pn, Pp and the loss term by the cell's weight (beta 1: Pp = the weight).
+// bt (no selector; nmfb200_nmfnd_batched_create): bt.n problems of shape s in the same launches, problem b with its target
+// at V + b bt.v (0: one shared target) and its W, H, Pn, Pp in the b-th block of (bt.n, ...) storages; loss_dev[b] from its
+// own run of partials summed in the single problem's order.  Problems whose bt.active flag is 0 are skipped: their factors'
+// terms and loss_dev slots are left as they are.  The kernels derive bt.f / bt.g / bt.p from s; the caller's are not read.
 int nmfd_recon_phi(const NmfdShape& s, const void* V, int vdtype, const float* W, const float* H, double beta,
                    float* Pn, float* Pp, double* loss_blocks, int max_blocks, double* loss_dev,
-                   cudaStream_t st, CellSel M = CellSel{});
+                   cudaStream_t st, CellSel M = CellSel{}, const Batch& bt = Batch{});
 // batch elements per launch of the kernels that put the batch on grid.z (fp32 recon / dgrad, tensor-core recon / dgrad)
 static inline int64_t nmfd_batch_slice(int64_t B) { return B < kMaxGridYZ ? B : kMaxGridYZ; }
 // loss partials of nmfd_recon_phi: one per block of all its launches
 int64_t nmfd_max_blocks(const NmfdShape& s);
 // out[c,r,t] = sum_{b,x} G[b,c,x] H[b,r,x-t]   (x, t multi-indices over up to three axes)
-int nmfd_wgrad(const NmfdShape& s, const float* G, const float* H, float* out, int nsplit, cudaStream_t st);   // out[split][C,R,T]
+// bt (as nmfd_recon_phi's): out[split][problem][C,R,T], each problem's lines in the single problem's splits
+int nmfd_wgrad(const NmfdShape& s, const float* G, const float* H, float* out, int nsplit, cudaStream_t st,
+               const Batch& bt = Batch{});   // out[split][C,R,T]
 int nmfd_wgrad_nsplit(const NmfdShape& s);
 // out[split][b,r,j] = sum_{c in split, t} W[c,r,t] G[b,c,j+t]   (j, t multi-indices)
-int nmfd_dgrad(const NmfdShape& s, const float* G, const float* W, float* out, int nsplit, cudaStream_t st);
+// bt (as nmfd_recon_phi's): out[split][problem][B,R,J]
+int nmfd_dgrad(const NmfdShape& s, const float* G, const float* W, float* out, int nsplit, cudaStream_t st,
+               const Batch& bt = Batch{});
 int nmfd_dgrad_nsplit(const NmfdShape& s);
 // wgrad's block plan (nmfd.cu): row tile MT of channels, TP = roundup(min(T, 64), 4) offsets of NR components for NO outer
 // kernel offsets per block; NTT x NRG x NOG column blocks

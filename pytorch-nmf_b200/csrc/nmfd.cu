@@ -71,6 +71,10 @@ struct Geo {
 //   !FWD: m = r, k = c in this block's split, X = G, shift +t; the epilogue writes the partial sums of this split
 // grid (line tiles * line groups, row tiles * nsplit, batch elements [b0, b0 + gridDim.z)), 256 threads: batches beyond the
 // 65535 of grid.z take several launches
+// BATCH (NoSel only, nmfb200_nmfnd_batched_create): the grid-z lines are bt.n problems of s.B lines each, problem after
+// problem.  A block of problem `prob` reads A + prob bt.f, X + prob bt.g and its target at V + prob bt.v, writes its Pn / Pp
+// (FWD) or its dgrad partials at + prob bt.p (the dgrad slab of one split holds every problem's) and its loss partials as
+// the contiguous run a single launch of that problem writes; otherwise it runs the single problem's plan and arithmetic.
 struct SlideArgs {
   const float* A;            // W
   const float* X;            // H (FWD) or G
@@ -86,9 +90,9 @@ struct SlideArgs {
 // SEL (FWD only): a fit on the observed cells -- at a missing cell V is not read, Pn = Pp = 0 and the loss adds nothing;
 // Pp is written at every beta (beta 1: the mask as 0 / 1), so wgrad / dgrad of Pp give the denominators.  A weighted fit
 // treats the cells of weight 0 as missing and multiplies Pn, Pp and the loss term by the weight elsewhere (beta 1: Pp = w).
-template <int MT, bool FWD, int MODE, bool LOSS, typename TV, typename SEL = NoSel>
+template <int MT, bool FWD, int MODE, bool LOSS, typename TV, typename SEL = NoSel, bool BATCH = false>
 __global__ void __launch_bounds__(256)
-nmfd_slide_kernel(NmfdShape s, SlideArgs a) {
+nmfd_slide_kernel(NmfdShape s, SlideArgs a, Batch bt) {
   constexpr bool MASK = !std::is_same<SEL, NoSel>::value;
   constexpr bool WEIGHT = kWeighted<SEL>;
   using G = Geo<MT>;
@@ -107,7 +111,20 @@ nmfd_slide_kernel(NmfdShape s, SlideArgs a) {
   const int mtiles = (a.M + MT - 1) / MT;
   const int split = blockIdx.y / mtiles;
   const int m0 = (blockIdx.y - split * mtiles) * MT;
-  const int b = a.b0 + blockIdx.z;
+  int b = a.b0 + blockIdx.z;
+  if constexpr (BATCH) {          // the single-problem instantiations compile none of this
+    const int prob = b / s.B;
+    if (batch_skips(bt.active, prob)) return;
+    b -= prob * s.B;
+    a.A += prob * bt.f; a.X += prob * bt.g;
+    if (FWD) {
+      a.V = static_cast<const TV*>(a.V) + prob * bt.v;
+      a.Pn += prob * bt.p; a.Pp += prob * bt.p;
+      if (LOSS) a.block_partials += (int64_t)prob * s.B * gridDim.y * gridDim.x;
+    } else {
+      a.out += prob * bt.p;
+    }
+  }
   const int kps = (a.K + a.nsplit - 1) / a.nsplit;
   const int kbeg = split * kps, kend = min(a.K, kbeg + kps);
   const int J1 = s.J1(), J2 = s.J2();
@@ -233,7 +250,7 @@ nmfd_slide_kernel(NmfdShape s, SlideArgs a) {
     }
   } else {
     const int64_t HI = s.h_inner();
-    float* out = a.out + (int64_t)split * s.B * s.R * HI;
+    float* out = a.out + (int64_t)split * (BATCH ? bt.n * bt.p : (int64_t)s.B * s.R * HI);
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
       const int r = m0 + 4 * ty + i;
@@ -251,11 +268,13 @@ nmfd_slide_kernel(NmfdShape s, SlideArgs a) {
 // A block owns MT channels x NCOL columns.  A column is (outer offset, component, offset t): TP = roundup(T, 4) <= 64 offsets
 // of NR components (their H windows are staged once per line) for each of NO outer offsets (each with its own G tile).
 // grid (t tiles * r groups * outer-offset groups, c tiles, nsplit), 256 threads.
+// BATCH: grid z is (problem, split) from z0 on, problem-major, over bt.n problems; problem `prob` reads Gm + prob bt.g and
+// H + prob bt.f and writes out[split][prob] (bt.p floats per problem), summing its own lines in the single problem's splits.
 
-template <int MT>
+template <int MT, bool BATCH = false>
 __global__ void __launch_bounds__(256)
 nmfd_wgrad_kernel(NmfdShape s, const float* __restrict__ Gm, const float* __restrict__ H, float* __restrict__ out,
-                  int nsplit, WgradPlan p) {
+                  int nsplit, WgradPlan p, Batch bt, int64_t z0) {
   using G = Geo<MT>;
   __shared__ __align__(16) float Gs[G::NTO * kTK * G::PAD];      // Gs[oo][ll][c]
   __shared__ float Hs[G::HS];
@@ -283,8 +302,16 @@ nmfd_wgrad_kernel(NmfdShape s, const float* __restrict__ Gm, const float* __rest
   // the lines are split over blockIdx.z: more blocks than the output tiles alone give, and shorter fp32 sums
   // 64-bit: create admits up to 2^31 - 1 lines, and the rounded-up split end may pass that
   const int64_t nlines = (int64_t)s.B * J1 * J2, lps = (nlines + nsplit - 1) / nsplit;
-  const int64_t line0 = blockIdx.z * lps, line1 = min(nlines, line0 + lps);
-  out += (int64_t)blockIdx.z * s.C * s.R * s.w_inner();
+  if constexpr (BATCH) {
+    const int64_t z = z0 + blockIdx.z, prob = z / nsplit, split = z - prob * nsplit;
+    if (batch_skips(bt.active, prob)) return;
+    Gm += prob * bt.g; H += prob * bt.f;
+    out += (split * bt.n + prob) * bt.p;
+    z0 = split;                 // from here on: this block's split
+  }
+  const int64_t zs = BATCH ? z0 : (int64_t)blockIdx.z;
+  const int64_t line0 = zs * lps, line1 = min(nlines, line0 + lps);
+  if (!BATCH) out += zs * s.C * s.R * s.w_inner();
   for (int64_t bo = line0; bo < line1; ++bo) {            // every H line (b, j1, j2) meets the G lines (b, j1 + t1, j2 + t2)
     const int b = (int)(bo / (J1 * J2)), jo = (int)(bo - (int64_t)b * (J1 * J2));
     const int j1 = jo / J2, j2 = jo - j1 * J2;
@@ -379,12 +406,12 @@ dim3 dim3_of(const Grid3& g) { return dim3((unsigned)g.x, (unsigned)g.y, (unsign
 
 
 // TV: the target's element type (FWD only; the dgrad pass reads no V and always takes float)
-template <int MT, bool FWD, typename TV, typename SEL>
-void launch_slide(const NmfdShape& s, const SlideArgs& a, int mode, bool loss, dim3 grid, cudaStream_t st) {
-  if (!FWD) { nmfd_slide_kernel<MT, false, kKL, false, float><<<grid, 256, 0, st>>>(s, a); return; }
-#define NMFD_GO(M)                                                                       \
-  if (loss) nmfd_slide_kernel<MT, true, M, true, TV, SEL><<<grid, 256, 0, st>>>(s, a);   \
-  else nmfd_slide_kernel<MT, true, M, false, TV, SEL><<<grid, 256, 0, st>>>(s, a);
+template <int MT, bool FWD, typename TV, typename SEL, bool BATCH>
+void launch_slide(const NmfdShape& s, const SlideArgs& a, const Batch& bt, int mode, bool loss, dim3 grid, cudaStream_t st) {
+  if (!FWD) { nmfd_slide_kernel<MT, false, kKL, false, float, NoSel, BATCH><<<grid, 256, 0, st>>>(s, a, bt); return; }
+#define NMFD_GO(M)                                                                                  \
+  if (loss) nmfd_slide_kernel<MT, true, M, true, TV, SEL, BATCH><<<grid, 256, 0, st>>>(s, a, bt);   \
+  else nmfd_slide_kernel<MT, true, M, false, TV, SEL, BATCH><<<grid, 256, 0, st>>>(s, a, bt);
   switch (mode) {
     case kKL: NMFD_GO(kKL); break;
     case kEU: NMFD_GO(kEU); break;
@@ -394,28 +421,49 @@ void launch_slide(const NmfdShape& s, const SlideArgs& a, int mode, bool loss, d
 #undef NMFD_GO
 }
 
-template <bool FWD, typename TV, typename SEL>
-void dispatch_slide(int mt, const NmfdShape& s, const SlideArgs& a, int mode, bool loss, dim3 grid, cudaStream_t st) {
+template <bool FWD, typename TV, typename SEL, bool BATCH>
+void dispatch_slide(int mt, const NmfdShape& s, const SlideArgs& a, const Batch& bt, int mode, bool loss, dim3 grid,
+                    cudaStream_t st) {
   switch (mt) {
-    case 4: launch_slide<4, FWD, TV, SEL>(s, a, mode, loss, grid, st); break;
-    case 8: launch_slide<8, FWD, TV, SEL>(s, a, mode, loss, grid, st); break;
-    case 16: launch_slide<16, FWD, TV, SEL>(s, a, mode, loss, grid, st); break;
-    case 32: launch_slide<32, FWD, TV, SEL>(s, a, mode, loss, grid, st); break;
-    default: launch_slide<64, FWD, TV, SEL>(s, a, mode, loss, grid, st); break;
+    case 4: launch_slide<4, FWD, TV, SEL, BATCH>(s, a, bt, mode, loss, grid, st); break;
+    case 8: launch_slide<8, FWD, TV, SEL, BATCH>(s, a, bt, mode, loss, grid, st); break;
+    case 16: launch_slide<16, FWD, TV, SEL, BATCH>(s, a, bt, mode, loss, grid, st); break;
+    case 32: launch_slide<32, FWD, TV, SEL, BATCH>(s, a, bt, mode, loss, grid, st); break;
+    default: launch_slide<64, FWD, TV, SEL, BATCH>(s, a, bt, mode, loss, grid, st); break;
   }
 }
 
-// one launch of the sliding kernel per slice of at most kMaxGridYZ batch elements
+// one launch of the sliding kernel per slice of at most kMaxGridYZ lines: s.B batch elements, or a batch's bt.n x s.B
 template <bool FWD, typename TV = float, typename SEL = NoSel>
-int launch_slices(int mt, const NmfdShape& s, SlideArgs a, int mode, bool loss, const Grid3& g, cudaStream_t st) {
-  for (int64_t b0 = 0; b0 < s.B; b0 += g.z) {
+int launch_slices(int mt, const NmfdShape& s, SlideArgs a, const Batch& bt, int mode, bool loss, cudaStream_t st) {
+  const int64_t lines = s.B * bt.n;
+  Grid3 g = slide_grid(s, FWD, mt, a.M, a.nsplit);
+  g.z = nmfd_batch_slice(lines);
+  for (int64_t b0 = 0; b0 < lines; b0 += g.z) {
     a.b0 = (int)b0;
     dim3 grid = dim3_of(g);
-    grid.z = (unsigned)std::min<int64_t>(g.z, s.B - b0);
-    dispatch_slide<FWD, TV, SEL>(mt, s, a, mode, loss, grid, st);
+    grid.z = (unsigned)std::min<int64_t>(g.z, lines - b0);
+    bool batched = false;                 // a batch runs the BATCH instantiations (no selector); one problem the others
+    if constexpr (std::is_same<SEL, NoSel>::value) batched = bt.n > 1 || bt.active;
+    if (batched) {
+      if constexpr (std::is_same<SEL, NoSel>::value) dispatch_slide<FWD, TV, SEL, true>(mt, s, a, bt, mode, loss, grid, st);
+    } else {
+      dispatch_slide<FWD, TV, SEL, false>(mt, s, a, bt, mode, loss, grid, st);
+    }
     NMF_LAUNCH_CHECK();
   }
   return 0;
+}
+
+// The per-problem offsets of a batch of problems of shape s from the caller's bt.n, bt.v and bt.active: A = W, X = H or G,
+// P = Pn / Pp (FWD) or the dgrad partials of one split
+Batch slide_batch(const NmfdShape& s, bool fwd, const Batch& bt) {
+  Batch b = bt;
+  b.f = (int64_t)s.C * s.R * s.w_inner();
+  const int64_t vol = (int64_t)s.B * s.C * s.v_inner(), hvol = (int64_t)s.B * s.R * s.h_inner();
+  b.g = fwd ? hvol : vol;
+  b.p = fwd ? vol : hvol;
+  return b;
 }
 
 }  // namespace
@@ -426,22 +474,27 @@ int64_t nmfd_max_blocks(const NmfdShape& s) {
 }
 
 int nmfd_recon_phi(const NmfdShape& s, const void* V, int vdtype, const float* W, const float* H, double beta, float* Pn,
-                   float* Pp, double* loss_blocks, int max_blocks, double* loss_dev, cudaStream_t st, CellSel M) {
+                   float* Pp, double* loss_blocks, int max_blocks, double* loss_dev, cudaStream_t st, CellSel M,
+                   const Batch& bt) {
   const int mt = row_tile(s.C);
-  const Grid3 grid = slide_grid(s, true, mt, s.C, 1);
-  const int nblocks = (int)nmfd_max_blocks(s);          // create bounds it (nmfd_shape_of)
+  const int nblocks = (int)nmfd_max_blocks(s);          // per problem; create bounds it (nmfd_shape_of)
   const bool loss = loss_blocks != nullptr;
-  if (loss && nblocks > max_blocks) { set_error("nmfd loss: partial buffer too small"); return 1; }
+  if (bt.n < 1 || (bt.n > 1 && M)) { set_error("nmfd_recon_phi: a batch takes no selector"); return 1; }
+  if (loss && (double)nblocks * (double)bt.n > (double)max_blocks) {
+    set_error("nmfd loss: partial buffer too small");
+    return 1;
+  }
   SlideArgs a{};
   a.A = W; a.X = H; a.M = s.C; a.K = s.R; a.sm = (int64_t)s.R * s.w_inner(); a.sk = s.w_inner(); a.nsplit = 1;
   a.V = V; a.beta = (float)beta; a.Pn = Pn; a.Pp = Pp; a.block_partials = loss_blocks; a.out = nullptr; a.mask = M.p;
   if (int rc = with_vtype(V, vdtype, [&](auto Vt) {
         return with_sel(M, [&](auto Mk) {
-          return launch_slices<true, vtype_t<decltype(Vt)>, sel_t<decltype(Mk)>>(mt, s, a, beta_mode(beta), loss, grid, st);
+          return launch_slices<true, vtype_t<decltype(Vt)>, sel_t<decltype(Mk)>>(mt, s, a, slide_batch(s, true, bt),
+                                                                                  beta_mode(beta), loss, st);
         });
       }))
     return rc;
-  if (loss) return sum_partials(loss_blocks, nblocks, loss_dev, st);
+  if (loss) return sum_partials(loss_blocks, nblocks, loss_dev, st, bt.n, bt.active);
   return 0;
 }
 
@@ -456,19 +509,31 @@ int nmfd_wgrad_nsplit(const NmfdShape& s) {
   return (int)ns;
 }
 
-int nmfd_wgrad(const NmfdShape& s, const float* G, const float* H, float* out, int nsplit, cudaStream_t st) {
+int nmfd_wgrad(const NmfdShape& s, const float* G, const float* H, float* out, int nsplit, cudaStream_t st, const Batch& bt) {
   const WgradPlan p = wgrad_plan(s);
   const int ncol = 4 * (256 / (p.mt / 4));
   if (p.nr * (p.tp + kTK) > (ncol / 4) * (4 + kTK)) { set_error("nmfd_wgrad: internal tile plan exceeds shared memory"); return 1; }
-  const dim3 grid = dim3_of(wgrad_grid(s, p, nsplit));
-  switch (p.mt) {
-    case 4: nmfd_wgrad_kernel<4><<<grid, 256, 0, st>>>(s, G, H, out, nsplit, p); break;
-    case 8: nmfd_wgrad_kernel<8><<<grid, 256, 0, st>>>(s, G, H, out, nsplit, p); break;
-    case 16: nmfd_wgrad_kernel<16><<<grid, 256, 0, st>>>(s, G, H, out, nsplit, p); break;
-    case 32: nmfd_wgrad_kernel<32><<<grid, 256, 0, st>>>(s, G, H, out, nsplit, p); break;
-    default: nmfd_wgrad_kernel<64><<<grid, 256, 0, st>>>(s, G, H, out, nsplit, p); break;
+  if (bt.n < 1) { set_error("nmfd_wgrad: bad problem count"); return 1; }
+  Grid3 g = wgrad_grid(s, p, nsplit);
+  const bool batched = bt.n > 1 || bt.active;
+  Batch b = bt;                           // a batch: problem after problem on grid z, sliced at kMaxGridYZ
+  b.f = (int64_t)s.B * s.R * s.h_inner(); b.g = (int64_t)s.B * s.C * s.v_inner(); b.p = (int64_t)s.C * s.R * s.w_inner();
+  const int64_t zall = g.z * bt.n;
+  for (int64_t z0 = 0; z0 < zall; z0 += kMaxGridYZ) {
+    dim3 grid = dim3_of(Grid3{g.x, g.y, std::min<int64_t>(zall - z0, kMaxGridYZ)});
+#define NMFD_WGRAD(MT)                                                                           \
+  if (batched) nmfd_wgrad_kernel<MT, true><<<grid, 256, 0, st>>>(s, G, H, out, nsplit, p, b, z0); \
+  else nmfd_wgrad_kernel<MT><<<grid, 256, 0, st>>>(s, G, H, out, nsplit, p, b, 0);
+    switch (p.mt) {
+      case 4: NMFD_WGRAD(4); break;
+      case 8: NMFD_WGRAD(8); break;
+      case 16: NMFD_WGRAD(16); break;
+      case 32: NMFD_WGRAD(32); break;
+      default: NMFD_WGRAD(64); break;
+    }
+#undef NMFD_WGRAD
+    NMF_LAUNCH_CHECK();
   }
-  NMF_LAUNCH_CHECK();
   return 0;
 }
 
@@ -497,14 +562,14 @@ void nmfd_plan(const NmfdShape& s, NmfdPlan* p) {
   p->wgrad_grid = wgrad_grid(s, p->wgrad, p->wgrad_nsplit);
 }
 
-int nmfd_dgrad(const NmfdShape& s, const float* G, const float* W, float* out, int nsplit, cudaStream_t st) {
+int nmfd_dgrad(const NmfdShape& s, const float* G, const float* W, float* out, int nsplit, cudaStream_t st, const Batch& bt) {
   if (s.R > 256) { set_error("nmfd_dgrad: rank must be <= 256"); return 1; }
+  if (bt.n < 1) { set_error("nmfd_dgrad: bad problem count"); return 1; }
   const int mt = row_tile(s.R);
-  const Grid3 grid = slide_grid(s, false, mt, s.R, nsplit);
   SlideArgs a{};
   a.A = W; a.X = G; a.M = s.R; a.K = s.C; a.sm = s.w_inner(); a.sk = (int64_t)s.R * s.w_inner(); a.nsplit = nsplit;
   a.out = out;
-  return launch_slices<false>(mt, s, a, 0, false, grid, st);
+  return launch_slices<false>(mt, s, a, slide_batch(s, false, bt), 0, false, st);
 }
 
 }  // namespace nmfb200

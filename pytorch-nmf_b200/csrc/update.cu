@@ -101,10 +101,16 @@ colsum_rows_kernel(const float* __restrict__ x, int64_t outer, int R, int64_t ro
   }
 }
 
-// stage 1 for inner > 1: one block per (o, r) run of `inner` contiguous elements.
+// stage 1 for inner > 1: one block per (o, r) run of `inner` contiguous elements.  BATCH: `runs` blocks per problem, problem
+// after problem (their runs and partials are contiguous); a problem whose `active` flag is 0 is skipped.
+template <bool BATCH = false>
 __global__ void __launch_bounds__(256)
-colsum_runs_kernel(const float* __restrict__ x, int64_t inner, float* __restrict__ partial) {
+colsum_runs_kernel(const float* __restrict__ x, int64_t inner, float* __restrict__ partial, int64_t runs,
+                   const uint8_t* __restrict__ active) {
   __shared__ float sh[8];
+  if constexpr (BATCH) {
+    if (batch_skips(active, (int64_t)blockIdx.x / runs)) return;
+  }
   const float* run = x + (int64_t)blockIdx.x * inner;
   float acc = 0.f;
   for (int64_t i = threadIdx.x; i < inner; i += 256) acc += run[i];
@@ -267,11 +273,16 @@ int64_t colsum_scratch_floats(int64_t outer, int R, int64_t inner) { return cols
 int factor_colsum(const float* x, int64_t outer, int R, int64_t inner, float* scratch, int64_t scratch_floats,
                   float* sums, cudaStream_t st, int64_t nprob, const uint8_t* active) {
   const int64_t nb = colsum_blocks(outer, inner);
-  if (nprob < 1 || (nprob > 1 && inner > 1)) { set_error("factor_colsum: a batch needs inner == 1"); return 1; }
+  if (nprob < 1) { set_error("factor_colsum: bad problem count"); return 1; }
   if ((double)nb * R * nprob > (double)scratch_floats) { set_error("factor_colsum: scratch too small"); return 1; }
-  if (nb * nprob > kMaxGridX || ceil_div(R, 64) * nprob > kMaxGridX) { set_error("factor_colsum: batch passes grid x"); return 1; }
+  if ((double)nb * (inner > 1 ? R : 1) * nprob > (double)kMaxGridX || ceil_div(R, 64) * nprob > kMaxGridX) {
+    set_error("factor_colsum: batch passes grid x");
+    return 1;
+  }
   if (inner > 1) {
-    colsum_runs_kernel<<<(unsigned)(outer * R), 256, 0, st>>>(x, inner, scratch);
+    const unsigned gx = (unsigned)(outer * R * nprob);
+    if (nprob > 1 || active) colsum_runs_kernel<true><<<gx, 256, 0, st>>>(x, inner, scratch, outer * R, active);
+    else colsum_runs_kernel<<<gx, 256, 0, st>>>(x, inner, scratch, outer * R, active);
   } else {
     const int64_t rpb = ceil_div(outer, nb);
     colsum_rows_kernel<<<dim3((unsigned)(nb * nprob), (unsigned)ceil_div(R, 256)), 256, 0, st>>>(x, outer, R, rpb, scratch,

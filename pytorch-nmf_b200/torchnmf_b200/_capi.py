@@ -54,6 +54,10 @@ SIGNATURES = {
     "nmfb200_nmf_update_w_peer": (_int, [_vp, _vp, _vp, _dbl, _dbl, _dbl, _dbl, _vp]),
     "nmfb200_nmfnd_create": (_int, [_c.POINTER(_vp), _int, _i64, _i64, _int, _c.POINTER(_i64), _i64, _c.POINTER(_i64), _int]),
     "nmfb200_nmfd_set_target": (_int, [_vp, _vp, _int, _vp]),
+    "nmfb200_nmfnd_batched_create": (_int, [_c.POINTER(_vp), _int, _i64, _i64, _i64, _int, _c.POINTER(_i64), _i64,
+                                            _c.POINTER(_i64)]),
+    "nmfb200_nmfd_batched_set_target": (_int, [_vp, _vp, _i64, _int, _vp]),
+    "nmfb200_nmfd_batched_set_active": (_int, [_vp, _vp, _vp]),
     "nmfb200_sync_factors": (_int, [_vp]),
     "nmfb200_update_w": (_int, [_vp, _vp, _vp, _dbl, _dbl, _dbl, _dbl, _vp]),
     "nmfb200_update_h": (_int, [_vp, _vp, _vp, _dbl, _dbl, _dbl, _dbl, _vp]),

@@ -71,6 +71,18 @@ def _workspace_bytes(key):
         p = _capi.nmf_plan(N, C, R)
         return B * (8 * R * max(p["nch_w"] * C, p["nch_h"] * N) + 8 * R + 8 * p["loss_chunks"] * ((N + 63) // 64)
                     + 4 * R * max(p["colsum_blocks_n"], p["colsum_blocks_c"])) + (1 << 14)
+    if key[0] == "nmfd_batched":          # ("nmfd_batched", device, P, B, C, X, R, K): P x the fp32 context of one problem
+        _, _, P, B, C, X, R, K = key
+        nx, nk, nh = 1, 1, 1
+        for x, k in zip(X, K):
+            nx, nk, nh = nx * x, nk * k, nh * (x - k + 1)
+        p = _capi.nmfd_plan(B, C, X, R, K)
+
+        def colsum_floats(outer, inner):      # update.cu: colsum_scratch_floats
+            return R * (outer if inner > 1 else min(1024, max(1, (outer + 63) // 64)))
+        loss_blocks = p["recon_grid"][0] * p["recon_grid"][1] * B
+        return P * (8 * B * C * nx + 8 * R * max(p["wgrad_nsplit"] * C * nk, p["dgrad_nsplit"] * B * nh) + 8 * R
+                    + 8 * loss_blocks + 4 * max(colsum_floats(C, nk), colsum_floats(B, nh))) + (1 << 14)
     if key[0] == "nmfd":                  # ("nmfd", device, B, C, X, R, K, precision): ratio tiles + shifted operand copies
         _, _, B, C, X, R, K = key[:7]
         nx, nk = 1, 1
@@ -346,12 +358,56 @@ class CudaNmfEngine(_CudaEngine):
                                                         l2_reg, _stream(self.device)))
 
 
-class CudaBatchedNmfEngine(_CudaEngine):
+class _BatchedEngine(_CudaEngine):
+    """What the batched engines share: the problems are the leading axis of W and H, every launch runs the active ones, and
+    the loss is one value per problem."""
+    _set_active = None                     # the C ABI's set_active call of this context kind
+
+    @property
+    def precision(self):
+        return "f32"
+
+    def precision_for(self, beta):
+        return "f32"
+
+    def set_active(self, active):
+        """Run only the problems whose flag is set from now on: `active` is a bool sequence or tensor of one flag per
+        problem (None: all).  The others keep their factors and their slot of losses()."""
+        if active is None:
+            self._active = None
+        else:
+            self._active = torch.as_tensor(active).to(device=self.device, dtype=torch.uint8).contiguous()
+            assert self._active.shape == (self.W.shape[0],)
+        _capi.check(getattr(self._lib, self._set_active)(
+            self._ctx, _ptr(self._active) if self._active is not None else None, _stream(self.device)))
+
+    def losses(self, beta):
+        """beta_div of every problem's reconstruction, one float64 value per problem, on the host (one synchronisation); an
+        inactive problem's value is the last one computed for it."""
+        val = self.loss_tensor(beta).cpu()
+        self.check_health()
+        return val
+
+    def loss(self, beta):
+        raise TypeError("a batched engine has one loss per problem: use losses()")
+
+    def raw_terms(self, which, beta):
+        """(numerator, denominator) of every problem's update of W (which=0) or H (which=1): the numerator in the factor's
+        shape (problems, rows, R, ...); the denominator (problems, R) at beta 1 (the column sums of the other factor), else
+        in the factor's shape."""
+        f = self.W if which == 0 else self.H
+        buf = self._raw_terms_into(which, beta, None)
+        num, den = buf[:f.numel()].view(f.shape), buf[f.numel():]
+        return num, (den.view(f.shape[0], f.shape[2]) if beta == 1 else den.view(f.shape))
+
+
+class CudaBatchedNmfEngine(_BatchedEngine):
     """B independent dense NMF problems of one shape on one GPU (include/nmf_b200.h: nmfb200_nmf_batched_create), on the
     fp32 kernels: V (B,N,C) -- or (N,C), one target shared by every problem -- fp32, fp16 or bf16 with unit column stride,
     rows and problems strided; W (B,C,R) and H (B,N,R) contiguous fp32, updated in place.  Every update and loss launch
     runs all problems, and problem b's factors and loss are bit for bit those of CudaNmfEngine(V[b], W[b], H[b], "f32")."""
     kind = "nmf_batched"
+    _set_active = "nmfb200_nmf_batched_set_active"
 
     def __init__(self, V, W, H):
         super().__init__()
@@ -381,46 +437,51 @@ class CudaBatchedNmfEngine(_CudaEngine):
         _capi.check(self._lib.nmfb200_nmf_batched_set_active(self._ctx, None, _stream(self.device)))
         self.sync()
 
-    @property
-    def precision(self):
-        return "f32"
-
-    def precision_for(self, beta):
-        return "f32"
-
-    def set_active(self, active):
-        """Run only the problems whose flag is set from now on: `active` is a bool sequence or tensor of B flags (None: all).
-        The others keep their factors and their slot of losses()."""
-        if active is None:
-            self._active = None
-        else:
-            self._active = torch.as_tensor(active).to(device=self.device, dtype=torch.uint8).contiguous()
-            assert self._active.shape == (self.B,)
-        _capi.check(self._lib.nmfb200_nmf_batched_set_active(
-            self._ctx, _ptr(self._active) if self._active is not None else None, _stream(self.device)))
-
     def iterate(self, n_iter, beta, gamma, l1_reg, l2_reg):
         """n_iter x (update_w; update_h) of every active problem in one call."""
         _capi.check(self._lib.nmfb200_nmf_iterate(self._ctx, _ptr(self.W), _ptr(self.H), beta, gamma, l1_reg, l2_reg,
                                                   int(n_iter), _stream(self.device)))
 
-    def losses(self, beta):
-        """beta_div of every problem's reconstruction as B float64 values on the host (one synchronisation); an inactive
-        problem's value is the last one computed for it."""
-        val = self.loss_tensor(beta).cpu()
-        self.check_health()
-        return val
 
-    def loss(self, beta):
-        raise TypeError("a batched engine has one loss per problem: use losses()")
+class CudaBatchedNmfdEngine(_BatchedEngine):
+    """P independent NMFD / NMF2D / NMF3D problems of one shape on one GPU (include/nmf_b200.h:
+    nmfb200_nmfnd_batched_create), on the fp32 kernels: V (P,B,C,*X) -- or (B,C,*X), one target shared by every problem --
+    fp32, fp16 or bf16, each problem's block contiguous and the blocks at least B C prod(X) elements apart; W (P,C,R,*K) and
+    H (P,B,R,*(X-K+1)) contiguous fp32, updated in place.  Every update and loss launch runs all problems, and problem p's
+    factors and loss are bit for bit those of CudaNmfdEngine(V[p], W[p], H[p], "f32").  No `iterate`: the fit loop calls
+    update_w / update_h, as for a single NMFD engine."""
+    kind = "nmfd_batched"
+    _set_active = "nmfb200_nmfd_batched_set_active"
 
-    def raw_terms(self, which, beta):
-        """(numerator, denominator) of every problem's update of W (which=0) or H (which=1): the numerator in the factor's
-        shape (B, rows, R); the denominator (B, R) at beta 1 (the column sums of the other factor), else (B, rows, R)."""
-        f = self.W if which == 0 else self.H
-        buf = self._raw_terms_into(which, beta, None)
-        num, den = buf[:f.numel()].view(f.shape), buf[f.numel():]
-        return num, (den.view(self.B, self.R) if beta == 1 else den.view(f.shape))
+    def __init__(self, V, W, H):
+        super().__init__()
+        self.device = W.device
+        P, C, R, *K = W.shape
+        nd = len(K)
+        if V.dim() == nd + 2:
+            V = V.unsqueeze(0).expand(P, *V.shape)                       # one target: problem stride 0
+        if V.dtype not in _capi.DTYPES:
+            raise TypeError(f"V must be float32, float16 or bfloat16 (got {V.dtype})")
+        if V.device != self.device:
+            raise ValueError(f"V is on {V.device}, expected {self.device}")
+        for t, n in ((W, "W"), (H, "H")):
+            _check_f32_cuda(t, n, self.device)
+        _, B, _, *X = V.shape
+        assert 1 <= nd <= 3 and len(X) == nd
+        assert W.shape == (P, C, R, *K) and H.shape == (P, B, R, *(x - k + 1 for x, k in zip(X, K)))
+        if not (V[0].is_contiguous() and (V.stride(0) == 0 or V.stride(0) >= V[0].numel())):
+            raise ValueError("every problem's block of V must be contiguous, the blocks 0 or at least B C prod(X) apart")
+        self.V, self.W, self.H = V, W, H
+        self._active = None
+        dev_index = self.device.index if self.device.index is not None else torch.cuda.current_device()
+        vd, kd = (ctypes.c_int64 * nd)(*X), (ctypes.c_int64 * nd)(*K)
+        self._acquire(("nmfd_batched", dev_index, P, B, C, tuple(X), R, tuple(K)),
+                      lambda ref: self._lib.nmfb200_nmfnd_batched_create(ref, dev_index, P, B, C, nd, vd, R, kd))
+        self._loss = torch.zeros(P, dtype=torch.float64, device=self.device)
+        _capi.check(self._lib.nmfb200_nmfd_batched_set_target(self._ctx, _ptr(V), V.stride(0), _capi.DTYPES[V.dtype],
+                                                              _stream(self.device)))
+        _capi.check(self._lib.nmfb200_nmfd_batched_set_active(self._ctx, None, _stream(self.device)))
+        self.sync()
 
 
 def _compressed_forms(V, weights=None):

@@ -36,7 +36,8 @@ try:
 except Exception:  # pragma: no cover
     _tqdm = None
 
-__all__ = ["BaseComponent", "NMF", "NMFD", "NMF2D", "NMF3D", "BatchedNMF"]
+__all__ = ["BaseComponent", "NMF", "NMFD", "NMF2D", "NMF3D", "BatchedNMF", "BatchedNMFD", "BatchedNMF2D",
+           "BatchedNMF3D"]
 
 
 def _gamma(beta):
@@ -685,23 +686,16 @@ class NMFD(BaseComponent):
                                f"W {tuple(self.W.shape)}")
 
 
-class BatchedNMF(BaseComponent):
-    """B independent NMF problems of one shape:  V[b] (N,C) ~= H[b] (N,R) @ W[b] (C,R)^T,  W (B,C,R), H (B,N,R).
+class _BatchedComponent(BaseComponent):
+    """Shared part of the batched classes: P independent problems of one model and one shape, fitted together.  W and H
+    hold the problems on their leading axis and the rank on axis 2; problem p's factors W[p] / H[p] are those of the
+    single model.  `fit` runs every problem on the fp32 CUDA-core kernels in the launches one problem takes, each with its
+    own stop rule."""
+    _ndim = 3                      # axes of W and of H
+    _axes = "three axes (B, rows, rank)"
 
-    Args:
-        Vshape: (B, N, C); W and H are then drawn as `NMF` draws them, |randn| of (B, C, rank) and (B, N, rank)
-        rank: size of the hidden dimension (default: C); the last axis of W and H
-        W / H: a size (iterable of ints -> random non-negative init) or an initial non-negative Tensor
-        trainable_W / trainable_H: whether a *given tensor* is updated by `fit`
-    """
-
-    def __init__(self, Vshape=None, rank=None, *, W=None, H=None, trainable_W=True, trainable_H=True):
+    def __init__(self, rank=None, W=None, H=None, trainable_W=True, trainable_H=True):
         torch.nn.Module.__init__(self)
-        if isinstance(Vshape, _Iterable):
-            B, N, C = Vshape
-            rank = rank if rank else C
-            W = (B, C, rank) if W is None else W
-            H = (B, N, rank) if H is None else H
         inferred = None
         for name, spec, trainable in (("W", W, trainable_W), ("H", H, trainable_H)):
             if isinstance(spec, Tensor):
@@ -714,8 +708,8 @@ class BatchedNMF(BaseComponent):
                 p = None
             self.register_parameter(name, p)
             if p is not None:
-                if p.dim() != 3:
-                    raise ValueError(f"{name} must have three axes (B, rows, rank); got shape {tuple(p.shape)}")
+                if p.dim() != self._ndim:
+                    raise ValueError(f"{name} must have {self._axes}; got shape {tuple(p.shape)}")
                 if inferred is not None and p.shape[2] != inferred:
                     raise ValueError("Latent size of H does not match with W")
                 inferred = p.shape[2]
@@ -729,57 +723,49 @@ class BatchedNMF(BaseComponent):
             self.out_channels = self.W.shape[1]
         self.rank = rank
 
-    @staticmethod
-    def reconstruct(H, W):
-        return H @ W.transpose(-1, -2)
-
-    def _check_target_shape(self, V):
-        B, N, _ = self.H.shape
-        C = self.W.shape[1]
-        if tuple(V.shape) not in ((B, N, C), (N, C)):
-            raise ValueError(f"target shape {tuple(V.shape)} does not match H {tuple(self.H.shape)} / W {tuple(self.W.shape)}: "
-                             f"expected ({B}, {N}, {C}) or ({N}, {C})")
+    def _readable_in_place(self, Vd):
+        """Whether the engine reads this device target (fp32, fp16 or bf16) as it is laid out."""
+        raise NotImplementedError
 
     def sparse_fit(self, *args, **kwargs):
-        raise NotImplementedError("BatchedNMF has no sparse_fit: fit each problem with NMF.sparse_fit")
+        raise NotImplementedError(f"{type(self).__name__} has no sparse_fit: fit each problem with the single model's sparse_fit")
 
     @torch.no_grad()
     def fit(self, V, beta=1, tol=1e-4, max_iter=200, verbose=False, alpha=0, l1_ratio=0, *, precision="auto"):
-        """Fit every problem by multiplicative updates, as `NMF.fit(V[b], ...)` fits one, all of them in the same launches.
+        """Fit every problem by multiplicative updates, as the single model's `fit(V[p], ...)` fits one, all of them in the
+        same launches.
 
-        V: (B, N, C), or (N, C) -- one target shared by every problem (random restarts of one fit).  Dense float32,
-        float16 or bfloat16, read in place if its columns have unit stride (rows and problems may be strided; an expanded
-        (N, C) tensor is read once); float64 and other layouts are staged through one fp32 (or same-dtype contiguous)
-        copy on the device.  A sparse V raises NotImplementedError.
+        V: the problems' targets stacked on a leading axis, or one target of the single model's shape shared by every
+        problem (random restarts of one fit).  Dense float32, float16 or bfloat16, read in place where the class's layout
+        allows it (an expanded shared target is read once); float64 and other layouts are staged through one fp32 (or
+        same-dtype contiguous) copy on the device.  A sparse V raises NotImplementedError.
 
-        Returns a torch.int64 tensor of B iteration counts.  Problem b follows the reference's stop rule (nmf.py:366-409) on
-        its own: its loss sqrt(2 d_b) at the start and every 10th iteration, and it stops at the first check where
-        (previous_b - loss_b) / init_b < tol; from then on every kernel leaves its factors untouched while the others run
-        on.  n_iter[b], W[b] and H[b] equal, bit for bit, those of `NMF(W=W0[b], H=H0[b]).fit(V[b], ..., precision="f32")`:
-        each problem keeps the single fit's tile plan and summation order.  The losses cost one synchronisation per 10
-        iterations for the whole batch.
+        Returns a torch.int64 tensor of P iteration counts.  Problem p follows the reference's stop rule (nmf.py:366-409) on
+        its own: its loss sqrt(2 d_p) at the start and every 10th iteration, and it stops at the first check where
+        (previous_p - loss_p) / init_p < tol; from then on every kernel leaves its factors untouched while the others run
+        on.  n_iter[p], W[p] and H[p] equal, bit for bit, those of the single model's
+        `fit(V[p], ..., precision="f32")` from W0[p] / H0[p]: each problem keeps the single fit's tile plan and summation
+        order.  The losses cost one synchronisation per 10 iterations for the whole batch.
 
         Every beta, `alpha` / `l1_ratio` and frozen factors (trainable_W / trainable_H) are supported, for 1 <= R <= 256,
         on the fp32 CUDA-core kernels: precision "auto" and "f32" run them (`last_fit_precision` is "f32"); "f16" and
         "f16_split" raise ValueError, as do R > 256 and shape mismatches.  Validation is the reference's over every problem:
         a negative V fails its assertion, and beta <= 0 with a zero anywhere in V raises ValueError.  `mask`, `weight` and
-        `group` are not parameters of this class (TypeError).  Host or half-precision modules are staged through fp32
-        device copies and written back, as by `NMF.fit`.
-
-        Workspace (device memory, kept between fits of the same shape like `NMF.fit`'s): B times that of one fp32 NMF
-        problem -- the chunked partial numerators and denominators, 8 R max(nch_w C, nch_h N) bytes with up to 32 chunks
-        per contraction (`_capi.nmf_plan(N, C, R)`), plus the column sums and loss partials -- so it grows linearly with B.
+        `group` are not parameters of this method (TypeError).  Host or half-precision modules are staged through fp32
+        device copies and written back, as by the single model's `fit`.  The workspace is P times one fp32 problem's (see
+        the class).
         """
+        name = type(self).__name__
         if precision not in ("auto", "f32"):
             if precision in ("f16", "f16_split"):
-                raise ValueError(f"BatchedNMF runs on the fp32 kernels: precision must be 'auto' or 'f32' (got {precision!r})")
+                raise ValueError(f"{name} runs on the fp32 kernels: precision must be 'auto' or 'f32' (got {precision!r})")
             raise ValueError(f"unknown precision {precision!r}")
         if V.is_sparse:
-            raise NotImplementedError("BatchedNMF takes dense targets only")
+            raise NotImplementedError(f"{name} takes dense targets only")
         W, H = self.W, self.H
         assert W is not None and H is not None, "fit() needs both W and H"
         if W.shape[2] > 256:
-            raise ValueError(f"BatchedNMF supports rank <= 256 (got {W.shape[2]})")
+            raise ValueError(f"{name} supports rank <= 256 (got {W.shape[2]})")
         self._check_target_shape(V)
         B = W.shape[0]
 
@@ -793,9 +779,7 @@ class BatchedNMF(BaseComponent):
             Vd = V.to(dev, non_blocking=True)
             if Vd.dtype not in (torch.float32, torch.float16, torch.bfloat16):
                 Vd = Vd.to(f32)
-            n = Vd.dim()
-            rows_ok = Vd.stride(-1) == 1 and Vd.stride(-2) >= Vd.shape[-1]
-            if not (rows_ok and (n == 2 or Vd.stride(0) == 0 or Vd.stride(0) >= Vd.shape[1] * Vd.stride(1))):
+            if not self._readable_in_place(Vd):
                 Vd = Vd.contiguous()
             if on_gpu and W.dtype == f32 and H.dtype == f32 and W.is_contiguous() and H.is_contiguous():
                 Wd, Hd = W.data, H.data
@@ -803,7 +787,7 @@ class BatchedNMF(BaseComponent):
                 staged = True
                 Wd = W.data.to(dev, f32, non_blocking=True).contiguous()
                 Hd = H.data.to(dev, f32, non_blocking=True).contiguous()
-            eng = _engine.CudaBatchedNmfEngine(Vd, Wd, Hd)
+            eng = self._engine_cls(Vd, Wd, Hd)
         else:
             Wd, Hd = W.data, H.data
             eng = self._engine_factory(V, Wd, Hd)
@@ -832,7 +816,7 @@ class BatchedNMF(BaseComponent):
             with bar as pbar:
                 while it + 1 < max_iter and bool(active.any()):
                     k = min(10 - ((it + 1) % 10), max_iter - (it + 1))
-                    if train_w and train_h:
+                    if train_w and train_h and hasattr(eng, "iterate"):
                         eng.iterate(k, beta, gamma, l1_reg, l2_reg)                        # nmf.py:366-391, k times
                     else:
                         for _ in range(k):
@@ -861,6 +845,197 @@ class BatchedNMF(BaseComponent):
         finally:
             eng.close()
         return n_iter
+
+
+class BatchedNMF(_BatchedComponent):
+    """B independent NMF problems of one shape:  V[b] (N,C) ~= H[b] (N,R) @ W[b] (C,R)^T,  W (B,C,R), H (B,N,R).
+
+    Args:
+        Vshape: (B, N, C); W and H are then drawn as `NMF` draws them, |randn| of (B, C, rank) and (B, N, rank)
+        rank: size of the hidden dimension (default: C); the last axis of W and H
+        W / H: a size (iterable of ints -> random non-negative init) or an initial non-negative Tensor
+        trainable_W / trainable_H: whether a *given tensor* is updated by `fit`
+
+    `fit(V, ...)` takes V as (B, N, C), or as one (N, C) target shared by every problem; its columns must have unit stride
+    to be read in place (rows and problems may be strided).  Each problem's fit is `NMF.fit(V[b], ..., precision="f32")`.
+    Workspace (device memory, kept between fits of the same shape like `NMF.fit`'s): B times that of one fp32 NMF problem
+    -- the chunked partial numerators and denominators, 8 R max(nch_w C, nch_h N) bytes with up to 32 chunks per
+    contraction (`_capi.nmf_plan(N, C, R)`), plus the column sums and loss partials -- so it grows linearly with B.
+    """
+    _engine_cls = _engine.CudaBatchedNmfEngine
+
+    def __init__(self, Vshape=None, rank=None, *, W=None, H=None, trainable_W=True, trainable_H=True):
+        if isinstance(Vshape, _Iterable):
+            B, N, C = Vshape
+            rank = rank if rank else C
+            W = (B, C, rank) if W is None else W
+            H = (B, N, rank) if H is None else H
+        super().__init__(rank, W, H, trainable_W, trainable_H)
+
+    @staticmethod
+    def reconstruct(H, W):
+        return H @ W.transpose(-1, -2)
+
+    def _check_target_shape(self, V):
+        B, N, _ = self.H.shape
+        C = self.W.shape[1]
+        if tuple(V.shape) not in ((B, N, C), (N, C)):
+            raise ValueError(f"target shape {tuple(V.shape)} does not match H {tuple(self.H.shape)} / W {tuple(self.W.shape)}: "
+                             f"expected ({B}, {N}, {C}) or ({N}, {C})")
+
+    def _readable_in_place(self, Vd):
+        rows_ok = Vd.stride(-1) == 1 and Vd.stride(-2) >= Vd.shape[-1]
+        return rows_ok and (Vd.dim() == 2 or Vd.stride(0) == 0 or Vd.stride(0) >= Vd.shape[1] * Vd.stride(1))
+
+
+def _batched_conv(H, W, conv):
+    """The reconstructions of P convolutive problems at once: problem p's H[p] (B,R,*J) convolved with its flipped W[p]
+    (C,R,*K), full padding, as one grouped convolution; (P,B,C,*X)."""
+    P, B, R = H.shape[:3]
+    C, K = W.shape[1], W.shape[3:]
+    x = H.transpose(0, 1).reshape(B, P * R, *H.shape[3:])
+    w = W.flip(tuple(range(3, W.dim()))).reshape(P * C, R, *K)
+    out = conv(x, w, padding=tuple(k - 1 for k in K), groups=P)
+    return out.reshape(B, P, C, *out.shape[2:]).transpose(0, 1)
+
+
+class _BatchedConvolutive(_BatchedComponent):
+    """Shared part of BatchedNMFD / BatchedNMF2D / BatchedNMF3D: P independent problems of the single model over `_nd`
+    convolved axes, V (P,B,C,*X), W (P,C,R,*K), H (P,B,R,*(X-K+1)); each problem's B clips share its W[p].
+
+    `fit(V, ...)` takes V as (P, B, C, *X), or as one (B, C, *X) target shared by every problem.  It is read in place when
+    every problem's block is contiguous and the blocks are at least B C prod(X) elements apart (or 0: an expanded shared
+    target).  Workspace (device memory, kept between fits of the same shape): P times that of one fp32 problem of the
+    single model -- the ratio tile of V's size (two at beta != 1), the wgrad / dgrad split partial slabs, 8 R max(nsw C
+    prod(K), nsd B prod(X-K+1)) bytes with the splits of `_capi.nmfd_plan`, plus the column sums and loss partials -- so
+    it grows linearly with P."""
+    _engine_cls = _engine.CudaBatchedNmfdEngine
+    _nd = 1
+    _conv = None
+
+    def __init__(self, rank, W, H, trainable_W, trainable_H):
+        super().__init__(rank, W, H, trainable_W, trainable_H)
+        if self.W is not None:
+            self.kernel_size = self.W.shape[3:]
+
+    @classmethod
+    def reconstruct(cls, H, W):
+        return _batched_conv(H, W, cls._conv)
+
+    def _check_target_shape(self, V):
+        P, B = self.H.shape[:2]
+        C, K, J = self.W.shape[1], self.W.shape[3:], self.H.shape[3:]
+        single = (B, C) + tuple(j + k - 1 for j, k in zip(J, K))
+        if tuple(V.shape) not in ((P,) + single, single):
+            raise ValueError(f"target shape {tuple(V.shape)} does not match H {tuple(self.H.shape)} / W {tuple(self.W.shape)}: "
+                             f"expected {(P,) + single} or {single}")
+
+    def _readable_in_place(self, Vd):
+        if Vd.dim() == self._nd + 2:
+            return Vd.is_contiguous()
+        return Vd[0].is_contiguous() and (Vd.stride(0) == 0 or Vd.stride(0) >= Vd[0].numel())
+
+
+class BatchedNMFD(_BatchedConvolutive):
+    """P independent NMFD problems of one shape:  V[p] (B,C,L) ~= sum_t W[p][:,:,t] @ shift_t(H[p]),  W (P,C,R,T),
+    H (P,B,R,L-T+1).  Problem p is `NMFD(W=W[p], H=H[p])`; its B clips share W[p].
+
+    Args:
+        Vshape: (P, B, C, L); W and H are then drawn as `NMFD` draws them, |randn| of (P, C, rank, T) and (P, B, rank, L-T+1)
+        rank: size of the hidden dimension (default: C)
+        T: the kernel's length (an int or a 1-tuple)
+        W / H: a size (iterable of ints -> random non-negative init) or an initial non-negative Tensor
+        trainable_W / trainable_H: whether a *given tensor* is updated by `fit`
+
+    `fit(V, ...)` takes V as (P, B, C, *X), or as one (B, C, *X) target shared by every problem.  It is read in place when
+    every problem's block is contiguous and the blocks are at least B C prod(X) elements apart (or 0: an expanded shared
+    target).  Workspace (device memory, kept between fits of the same shape): P times that of one fp32 problem of the
+    single model -- the ratio tile of V's size (two at beta != 1), the wgrad / dgrad split partial slabs, 8 R max(nsw C
+    prod(K), nsd B prod(X-K+1)) bytes with the splits of `_capi.nmfd_plan`, plus the column sums and loss partials -- so
+    it grows linearly with P.
+    """
+    _nd = 1
+    _ndim = 4
+    _axes = "four axes (P, rows, rank, T)"
+    _conv = staticmethod(F.conv1d)
+
+    def __init__(self, Vshape=None, rank=None, T=1, *, W=None, H=None, trainable_W=True, trainable_H=True):
+        if isinstance(Vshape, _Iterable):
+            if isinstance(T, _Iterable):
+                T, = T
+            P, B, C, L = Vshape
+            rank = rank if rank else C
+            W = (P, C, rank, T) if W is None else W
+            H = (P, B, rank, L - T + 1) if H is None else H
+        super().__init__(rank, W, H, trainable_W, trainable_H)
+
+
+class BatchedNMF2D(_BatchedConvolutive):
+    """P independent NMF2D problems of one shape:  V[p] (B,C,X1,X2) ~= conv2d(H[p], flipped W[p], full padding),
+    W (P,C,R,k1,k2), H (P,B,R,X1-k1+1,X2-k2+1).  Problem p is `NMF2D(W=W[p], H=H[p])`; its B clips share W[p].
+
+    Args:
+        Vshape: (P, B, C, X1, X2); W and H are then drawn as `NMF2D` draws them (rank defaults to X1, as there)
+        rank: size of the hidden dimension
+        kernel_size: (k1, k2), or one int for both
+        W / H: a size (iterable of ints -> random non-negative init) or an initial non-negative Tensor
+        trainable_W / trainable_H: whether a *given tensor* is updated by `fit`
+
+    `fit(V, ...)` takes V as (P, B, C, *X), or as one (B, C, *X) target shared by every problem.  It is read in place when
+    every problem's block is contiguous and the blocks are at least B C prod(X) elements apart (or 0: an expanded shared
+    target).  Workspace (device memory, kept between fits of the same shape): P times that of one fp32 problem of the
+    single model -- the ratio tile of V's size (two at beta != 1), the wgrad / dgrad split partial slabs, 8 R max(nsw C
+    prod(K), nsd B prod(X-K+1)) bytes with the splits of `_capi.nmfd_plan`, plus the column sums and loss partials -- so
+    it grows linearly with P.
+    """
+    _nd = 2
+    _ndim = 5
+    _axes = "five axes (P, rows, rank, k1, k2)"
+    _conv = staticmethod(F.conv2d)
+
+    def __init__(self, Vshape=None, rank=None, kernel_size=1, *, W=None, H=None, trainable_W=True, trainable_H=True):
+        if isinstance(Vshape, _Iterable):
+            kernel_size = _ntuple(kernel_size, 2)
+            k1, k2 = kernel_size
+            P, B, C, X1, X2 = Vshape
+            rank = rank if rank else X1
+            W = (P, C, rank) + kernel_size if W is None else W
+            H = (P, B, rank, X1 - k1 + 1, X2 - k2 + 1) if H is None else H
+        super().__init__(rank, W, H, trainable_W, trainable_H)
+
+
+class BatchedNMF3D(_BatchedConvolutive):
+    """P independent NMF3D problems of one shape:  V[p] (B,C,X1,X2,X3) ~= conv3d(H[p], flipped W[p], full padding),
+    W (P,C,R,k1,k2,k3), H (P,B,R,X1-k1+1,X2-k2+1,X3-k3+1).  Problem p is `NMF3D(W=W[p], H=H[p])`; its B clips share W[p].
+
+    Args:
+        Vshape: (P, B, C, X1, X2, X3); W and H are then drawn as `NMF3D` draws them (rank defaults to X2, as there)
+        rank: size of the hidden dimension
+        kernel_size: (k1, k2, k3), or one int for all three
+        W / H: a size (iterable of ints -> random non-negative init) or an initial non-negative Tensor
+        trainable_W / trainable_H: whether a *given tensor* is updated by `fit`
+
+    `fit(V, ...)` takes V as (P, B, C, *X), or as one (B, C, *X) target shared by every problem.  It is read in place when
+    every problem's block is contiguous and the blocks are at least B C prod(X) elements apart (or 0: an expanded shared
+    target).  Workspace (device memory, kept between fits of the same shape): P times that of one fp32 problem of the
+    single model -- the ratio tile of V's size (two at beta != 1), the wgrad / dgrad split partial slabs, 8 R max(nsw C
+    prod(K), nsd B prod(X-K+1)) bytes with the splits of `_capi.nmfd_plan`, plus the column sums and loss partials -- so
+    it grows linearly with P.
+    """
+    _nd = 3
+    _ndim = 6
+    _axes = "six axes (P, rows, rank, k1, k2, k3)"
+    _conv = staticmethod(F.conv3d)
+
+    def __init__(self, Vshape=None, rank=None, kernel_size=1, *, W=None, H=None, trainable_W=True, trainable_H=True):
+        if isinstance(Vshape, _Iterable):
+            kernel_size = _ntuple(kernel_size, 3)
+            k1, k2, k3 = kernel_size
+            P, B, C, X1, X2, X3 = Vshape
+            rank = rank if rank else X2
+            W = (P, C, rank) + kernel_size if W is None else W
+            H = (P, B, rank, X1 - k1 + 1, X2 - k2 + 1, X3 - k3 + 1) if H is None else H
+        super().__init__(rank, W, H, trainable_W, trainable_H)
 
 
 def _ntuple(x, n):
