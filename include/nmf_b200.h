@@ -257,6 +257,37 @@ int nmfb200_nmfd_batched_set_target(nmfb200_ctx* ctx, const void* V, int64_t pro
  * left as they are) at the cost of one flag read per block. */
 int nmfb200_nmfd_batched_set_active(nmfb200_ctx* ctx, const uint8_t* active, void* stream);
 
+/* ---- batched PLCA / SIPLCA / SIPLCA2 / SIPLCA3: the EM iteration on a batched NMF or NMFD context ------------------ */
+
+/* Each problem p of a batched NMF context (PLCA) or batched NMFD context (SIPLCA, SIPLCA2, SIPLCA3) is one PLCA problem on
+ * the normalised target V_p / sum(V_p): W (P,C,R,*kdims), H (P,N,R) or (P,B,R,*(vdims - kdims + 1)), Z (P,R) and
+ * Hz = H diag(Z) in H's shape, all contiguous fp32.  The context's factor pair is (W, Hz).  flags: which factors the EM step
+ * updates (a frozen Z takes W's column sums as the prior, and with W frozen too H's own). */
+#define NMFB200_PLCA_TRAIN_W 1
+#define NMFB200_PLCA_TRAIN_H 2
+#define NMFB200_PLCA_TRAIN_Z 4
+/* Floats of the caller's `work` buffer of nmfb200_plca_iterate on this context: the raw W and H numerators of every problem
+ * and the EM step's scratch.  -1 for a null or non-batched context. */
+int64_t nmfb200_plca_work_numel(const nmfb200_ctx* ctx);
+/* n_iter x (the raw W numerators dW, the raw H numerators dHz -- each bit for bit nmfb200_raw_terms' numerator at beta 1 --
+ * then the EM step of every active problem) with no return to the host.  The EM step is the reference's plca.py:252-289 on
+ * dW and dH = dHz Z (the Z from before the step): Z <- Z relu(sum H dHz), that product kept as the prior, then the alpha
+ * (Z + alpha - 1, thresholded at eps) and Z / sum(Z); W <- W relu(dW) / prior (or / its column sums when Z is frozen), then
+ * the alpha, threshold and renormalisation; H likewise; then Hz = H Z.  One launch per EM step, one block per problem: every
+ * sum runs in an order fixed by the problem's shape, independent of P and of which problems are active.  W_alpha, H_alpha,
+ * Z_alpha: null (alpha = 1) or device fp32 buffers of the factor's batched shape holding alpha.  A problem flagged inactive
+ * (nmfb200_nmf_batched_set_active / nmfb200_nmfd_batched_set_active) keeps W, H, Z and Hz.  `work`: device fp32,
+ * nmfb200_plca_work_numel floats.  NMFB200_ERR_INVALID for any other context kind, rank > 256 or unknown flags;
+ * NMFB200_ERR_STATE before set_target.  Asynchronous. */
+int nmfb200_plca_iterate(nmfb200_ctx* ctx, float* W, float* H, float* Z, float* Hz, float* work, int flags,
+                         const float* W_alpha, const float* H_alpha, const float* Z_alpha, int n_iter, void* stream);
+/* loss_dev[p] (double) = kl_div(norm_p X_p, norm_p V_p) for every active problem p, X_p the reconstruction from (W, Hz) and
+ * V_p the registered (normalised) target: the reference's de-normalised PLCA loss (plca.py:245,293), without materialising
+ * X.  norm_dev: P device floats.  The batched KL loss launch with each problem's target and reconstructed cell scaled by
+ * norm_p; an inactive problem's slot is left as it is.  Asynchronous. */
+int nmfb200_plca_loss(nmfb200_ctx* ctx, const float* W, const float* Hz, const float* norm_dev, double* loss_dev,
+                      void* stream);
+
 /* ---- both models ------------------------------------------------------------------------- */
 
 /* Every call below takes a context of either model and runs that model's kernels.  update_w, update_h, loss, raw_terms and

@@ -1067,6 +1067,78 @@ int nmfb200_w_apply(nmfb200_ctx* ctx, float* W, const float* reduced, double bet
   return 0;
 }
 
+/* ---- batched PLCA: the EM iteration on the raw terms of a batched NMF / NMFD context ---------------------------- */
+
+namespace {
+// The floats of plca_iterate's work buffer: [dW | dHz | the EM step's scratch]
+struct PlcaWork { int64_t wn, hn, buf; };
+PlcaWork plca_work(const nmfb200_ctx* c) {
+  const FactorDims w = factor_dims(c, 0);
+  return {w.rows * c->R * w.inner * c->nprob, w.other_rows * c->R * w.other_inner * c->nprob,
+          plca_em_buf_floats((int)c->R, w.inner, w.other_inner) * c->nprob};
+}
+
+// The raw numerator of one factor's update at beta 1 into `out`: the contraction and raw_sum of nmfb200_raw_terms, without
+// the column sums PLCA does not use
+int plca_numerator(nmfb200_ctx* c, int which, const float* W, const float* Hz, float* out, cudaStream_t st) {
+  int rc = is_nmfd(c) ? nmfd_contract(c, which, W, Hz, 1.0, st) : simt_contract(c, which, W, Hz, 1.0, st);
+  if (rc) return rc;
+  ApplyArgs a = factor_view(c, which, c->nslab[which]);
+  a.num = c->num;
+  return raw_sum(a, out, nullptr, st);
+}
+}  // namespace
+
+int64_t nmfb200_plca_work_numel(const nmfb200_ctx* ctx) {
+  if (!ctx || !is_batch(ctx)) return -1;
+  const PlcaWork w = plca_work(ctx);
+  return w.wn + w.hn + w.buf;
+}
+
+int nmfb200_plca_iterate(nmfb200_ctx* ctx, float* W, float* H, float* Z, float* Hz, float* work, int flags,
+                         const float* W_alpha, const float* H_alpha, const float* Z_alpha, int n_iter, void* stream) {
+  CTX_GUARD(ctx, kAnyKind);
+  if (!is_batch(ctx)) return fail(NMFB200_ERR_INVALID, "plca_iterate takes a batched NMF or NMFD context");
+  TARGET_GUARD(ctx);
+  if (!W || !H || !Z || !Hz || !work || n_iter < 0) return fail(NMFB200_ERR_INVALID, "bad argument");
+  if (flags & ~(NMFB200_PLCA_TRAIN_W | NMFB200_PLCA_TRAIN_H | NMFB200_PLCA_TRAIN_Z))
+    return fail(NMFB200_ERR_INVALID, "unknown plca_iterate flags");
+  if (ctx->R > 256) return fail(NMFB200_ERR_INVALID, "batched PLCA supports rank <= 256");
+  cudaStream_t st = (cudaStream_t)stream;
+  const PlcaWork pw = plca_work(ctx);
+  float* dW = work;
+  float* dHz = work + pw.wn;
+  float* buf = dHz + pw.hn;
+  const FactorDims w = factor_dims(ctx, 0);
+  for (int i = 0; i < n_iter; ++i) {
+    int rc = plca_numerator(ctx, 0, W, Hz, dW, st);
+    if (rc == 0) rc = plca_numerator(ctx, 1, W, Hz, dHz, st);
+    if (rc == 0) rc = plca_em(ctx->nprob, w.rows, w.inner, w.other_rows, w.other_inner, (int)ctx->R, W, H, Z, Hz, dW, dHz,
+                              W_alpha, H_alpha, Z_alpha, flags, buf, ctx->active, st);
+    if (rc) return rc;
+  }
+  return 0;
+}
+
+int nmfb200_plca_loss(nmfb200_ctx* ctx, const float* W, const float* Hz, const float* norm_dev, double* loss_dev,
+                      void* stream) {
+  CTX_GUARD(ctx, kAnyKind);
+  if (!is_batch(ctx)) return fail(NMFB200_ERR_INVALID, "plca_loss takes a batched NMF or NMFD context");
+  TARGET_GUARD(ctx);
+  if (!W || !Hz || !norm_dev || !loss_dev) return fail(NMFB200_ERR_INVALID, "null pointer");
+  cudaStream_t st = (cudaStream_t)stream;
+  if (is_nmfd(ctx)) {
+    Batch bt{ctx->nprob, ctx->bstride, 0, 0, 0, ctx->active};
+    bt.scale = norm_dev;
+    return nmfd_recon_phi(ctx->d, ctx->V, ctx->vdtype, W, Hz, 1.0, nullptr, nullptr, ctx->loss_blocks, ctx->loss_max_blocks,
+                          loss_dev, st, CellSel{}, bt);
+  }
+  Batch bt{ctx->nprob, ctx->bstride, ctx->N * ctx->R, ctx->C * ctx->R, 0, ctx->active};
+  bt.scale = norm_dev;
+  return simt_nmf_loss(ctx->V, ctx->vdtype, ctx->ldv, Hz, W, ctx->N, ctx->C, (int)ctx->R, 1.0, ctx->loss_blocks,
+                       ctx->loss_max_blocks, loss_dev, CellSel{}, ctx->C, st, bt);
+}
+
 int nmfb200_hoyer_project(int device, float* x, int64_t outer, int64_t D, int64_t inner, const float* k1, const float* k2,
                           void* zeroed_ws, void* stream) {
   if (!x || !k1 || !k2 || !zeroed_ws) return fail(NMFB200_ERR_INVALID, "null pointer");

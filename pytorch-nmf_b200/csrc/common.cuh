@@ -72,6 +72,9 @@ struct Batch {
   int64_t f = 0, g = 0;               // floats between problems' F / G factors of a contraction or loss
   int64_t p = 0;                      // floats between problems' partial slabs (within one chunk)
   const uint8_t* active = nullptr;    // n flags, 0 = skipped: the problem's blocks exit at once (null: every problem runs)
+  // KL loss only (batched PLCA): n floats, problem b's target and reconstruction are multiplied by scale[b] before the loss
+  // term (null: none)
+  const float* scale = nullptr;
 };
 __device__ __forceinline__ bool batch_skips(const uint8_t* active, int64_t b) { return active && !active[b]; }
 
@@ -264,6 +267,15 @@ int sparse_rpl(int R);
 int64_t sparse_gather_blocks(int64_t nseg);
 void sparse_gram_plan(int64_t rows, int64_t* rpb, int* nb);
 int sparse_gram_passes(int R);
+
+// plca_em.cu -------------------------------------------------------------------------------
+// The EM step of nprob PLCA problems (nmfb200_plca_iterate), one block per problem: W (wrows, R, winner) and H, Hz (hrows, R,
+// hinner) per problem back to back, Z (R) per problem; dW / dHz the raw numerators in the factors' shapes; aW / aH / aZ the
+// alphas in the factors' shapes (null: 1); `flags` NMFB200_PLCA_TRAIN_*; buf: nprob x plca_em_buf_floats of scratch.
+int plca_em(int64_t nprob, int64_t wrows, int64_t winner, int64_t hrows, int64_t hinner, int R, float* W, float* H, float* Z,
+            float* Hz, const float* dW, const float* dHz, const float* aW, const float* aH, const float* aZ, int flags,
+            float* buf, const uint8_t* active, cudaStream_t st);
+int64_t plca_em_buf_floats(int R, int64_t w_inner, int64_t h_inner);
 
 // nmfd.cu ----------------------------------------------------------------------------------
 // L, T, Lin are the sizes along the LAST (contiguous) axis; NMF2D / NMF3D (nmf.py:782-942) add up to two outer axes of the

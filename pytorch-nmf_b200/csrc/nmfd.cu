@@ -112,9 +112,11 @@ nmfd_slide_kernel(NmfdShape s, SlideArgs a, Batch bt) {
   const int split = blockIdx.y / mtiles;
   const int m0 = (blockIdx.y - split * mtiles) * MT;
   int b = a.b0 + blockIdx.z;
+  float sc = 1.f;                 // BATCH, KL loss: the problem's bt.scale
   if constexpr (BATCH) {          // the single-problem instantiations compile none of this
     const int prob = b / s.B;
     if (batch_skips(bt.active, prob)) return;
+    if (LOSS && MODE == kKL && bt.scale) sc = bt.scale[prob];
     b -= prob * s.B;
     a.A += prob * bt.f; a.X += prob * bt.g;
     if (FWD) {
@@ -232,7 +234,8 @@ nmfd_slide_kernel(NmfdShape s, SlideArgs a, Batch bt) {
           }
           const float v = to_f32(static_cast<const TV*>(a.V)[off]);
           if (LOSS) {
-            local += loss_term_d<MODE>(v, acc[i][j], a.beta);
+            if (BATCH && MODE == kKL) local += loss_term_d<MODE>(sc * v, sc * acc[i][j], a.beta);
+            else local += loss_term_d<MODE>(v, acc[i][j], a.beta);
           } else {
             float pn, pp;
             phi_d<MODE>(v, acc[i][j], bm2, bm1, pn, pp);
@@ -444,7 +447,7 @@ int launch_slices(int mt, const NmfdShape& s, SlideArgs a, const Batch& bt, int 
     dim3 grid = dim3_of(g);
     grid.z = (unsigned)std::min<int64_t>(g.z, lines - b0);
     bool batched = false;                 // a batch runs the BATCH instantiations (no selector); one problem the others
-    if constexpr (std::is_same<SEL, NoSel>::value) batched = bt.n > 1 || bt.active;
+    if constexpr (std::is_same<SEL, NoSel>::value) batched = bt.n > 1 || bt.active || bt.scale;
     if (batched) {
       if constexpr (std::is_same<SEL, NoSel>::value) dispatch_slide<FWD, TV, SEL, true>(mt, s, a, bt, mode, loss, grid, st);
     } else {

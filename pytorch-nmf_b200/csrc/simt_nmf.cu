@@ -333,6 +333,7 @@ simt_loss_kernel(const TV* __restrict__ V, int64_t ldv, const float* __restrict_
   // BATCH (NoSel only): problem `prob`'s blocks write its own run of gridDim.y x nbx partials, laid out as a single
   // problem's
   int64_t bx = blockIdx.x, part = 0;
+  float sc = 1.f;                    // BATCH, KL: the problem's bt.scale
   if constexpr (BATCH) {
     const int64_t nbx = (Mr + kTile - 1) / kTile;
     const int64_t prob = bx / nbx;
@@ -340,6 +341,7 @@ simt_loss_kernel(const TV* __restrict__ V, int64_t ldv, const float* __restrict_
     bx -= prob * nbx;
     part = (prob * gridDim.y + blockIdx.y) * nbx + bx;
     V += prob * bt.v; F += prob * bt.f; G += prob * bt.g;
+    if (MODE == kKL && bt.scale) sc = bt.scale[prob];
   }
   const int tid = threadIdx.x;
   const int tx = tid & 15, ty = tid >> 4;
@@ -379,6 +381,7 @@ simt_loss_kernel(const TV* __restrict__ V, int64_t ldv, const float* __restrict_
           if (w != 0.f) local += loss_term_w<MODE>(to_f32(V[row * ldv + col]), s[i][j], beta, w);
         } else if (row < Mr && col < Nc && sel_set(Mk, row * ldm + col)) {
           if (MODE == kVFree) local += powf(s[i][j] + kEps, beta);       // nmf.py:635-636, before the division by beta
+          else if (BATCH && MODE == kKL) local += loss_term<MODE>(sc * to_f32(V[row * ldv + col]), sc * s[i][j], beta);
           else local += loss_term<MODE>(to_f32(V[row * ldv + col]), s[i][j], beta);
         }
       }
@@ -481,7 +484,7 @@ int simt_nmf_loss(const void* V, int vdtype, int64_t ldv, const float* F, const 
   int Rp = (int)round_up(R < 256 ? R : 256, 16);
   size_t smem = (size_t)2 * Rp * kLd * sizeof(float);
   int mode = beta_mode(beta);
-  const bool batched = bt.n > 1 || bt.active;
+  const bool batched = bt.n > 1 || bt.active || bt.scale;
   int rc = with_vtype(V, vdtype, [&](auto Vt) {
     using TV = vtype_t<decltype(Vt)>;
     return with_sel(M, [&](auto Mk) {

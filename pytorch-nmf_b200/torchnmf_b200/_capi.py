@@ -58,6 +58,9 @@ SIGNATURES = {
                                             _c.POINTER(_i64)]),
     "nmfb200_nmfd_batched_set_target": (_int, [_vp, _vp, _i64, _int, _vp]),
     "nmfb200_nmfd_batched_set_active": (_int, [_vp, _vp, _vp]),
+    "nmfb200_plca_work_numel": (_i64, [_vp]),
+    "nmfb200_plca_iterate": (_int, [_vp, _vp, _vp, _vp, _vp, _vp, _int, _vp, _vp, _vp, _int, _vp]),
+    "nmfb200_plca_loss": (_int, [_vp, _vp, _vp, _vp, _vp, _vp]),
     "nmfb200_sync_factors": (_int, [_vp]),
     "nmfb200_update_w": (_int, [_vp, _vp, _vp, _dbl, _dbl, _dbl, _dbl, _vp]),
     "nmfb200_update_h": (_int, [_vp, _vp, _vp, _dbl, _dbl, _dbl, _dbl, _vp]),
@@ -74,6 +77,7 @@ SIGNATURES = {
     "nmfb200_nmfnd_tc_plan": (_int, [_i64, _i64, _int, _c.POINTER(_i64), _i64, _c.POINTER(_i64), _c.POINTER(_i64), _int]),
 }
 NMF_PLAN_LEN, NMFD_PLAN_LEN, SPARSE_PLAN_LEN, NMFND_TC_PLAN_LEN = 9, 19, 8, 31         # include/nmf_b200.h
+PLCA_TRAIN_W, PLCA_TRAIN_H, PLCA_TRAIN_Z = 1, 2, 4                                       # include/nmf_b200.h
 
 _lib = None
 

@@ -400,6 +400,31 @@ class _BatchedEngine(_CudaEngine):
         num, den = buf[:f.numel()].view(f.shape), buf[f.numel():]
         return num, (den.view(f.shape[0], f.shape[2]) if beta == 1 else den.view(f.shape))
 
+    # ---- batched PLCA (include/nmf_b200.h: nmfb200_plca_iterate): the engine's factor pair is (W, Hz = H diag(Z)) ----
+    def plca_iterate(self, n_iter, H, Z, train_w, train_h, train_z, W_alpha=None, H_alpha=None, Z_alpha=None):
+        """n_iter EM iterations of every active problem in one call: the two raw-terms passes and one EM-step launch each.
+        Updates self.W, H (H's shape), Z (P, R) and self.H (= H Z) in place; the alphas are None (1) or contiguous fp32
+        tensors of the batched factor's shape."""
+        if getattr(self, "_plca_work", None) is None:
+            n = int(self._lib.nmfb200_plca_work_numel(self._ctx))
+            self._plca_work = torch.empty(n, dtype=torch.float32, device=self.device)
+        flags = (_capi.PLCA_TRAIN_W if train_w else 0) | (_capi.PLCA_TRAIN_H if train_h else 0) | (
+            _capi.PLCA_TRAIN_Z if train_z else 0)
+        alphas = [_ptr(a) if a is not None else None for a in (W_alpha, H_alpha, Z_alpha)]
+        _capi.check(self._lib.nmfb200_plca_iterate(self._ctx, _ptr(self.W), _ptr(H), _ptr(Z), _ptr(self.H),
+                                                   _ptr(self._plca_work), flags, *alphas, int(n_iter),
+                                                   _stream(self.device)))
+
+    def plca_losses(self, norm):
+        """kl_div(norm[p] X_p, norm[p] V_p) of every problem (X_p from W and Hz, V_p the normalised target), one float64 value
+        per problem, on the host (one synchronisation); an inactive problem's value is the last one computed for it.
+        norm: (P,) fp32 on the engine's device."""
+        _capi.check(self._lib.nmfb200_plca_loss(self._ctx, _ptr(self.W), _ptr(self.H), _ptr(norm), _ptr(self._loss),
+                                                _stream(self.device)))
+        val = self._loss.cpu()
+        self.check_health()
+        return val
+
 
 class CudaBatchedNmfEngine(_BatchedEngine):
     """B independent dense NMF problems of one shape on one GPU (include/nmf_b200.h: nmfb200_nmf_batched_create), on the

@@ -33,7 +33,8 @@ try:
 except Exception:  # pragma: no cover
     _tqdm = None
 
-__all__ = ["PLCA", "SIPLCA", "SIPLCA2", "SIPLCA3", "BaseComponent"]
+__all__ = ["PLCA", "SIPLCA", "SIPLCA2", "SIPLCA3", "BaseComponent", "BatchedPLCA", "BatchedSIPLCA", "BatchedSIPLCA2",
+           "BatchedSIPLCA3"]
 
 
 @torch.no_grad()
@@ -315,3 +316,344 @@ class SIPLCA3(_ShiftInvariant):
     @staticmethod
     def reconstruct(H, W, Z):
         return _flip_conv(F.conv3d, H, W, Z)
+
+
+# ---- many independent problems in one fit ---------------------------------------------------------------------------------
+
+@torch.no_grad()
+def _batched_norm(x):
+    """get_norm of every problem of a batched factor (problems on axis 0, rank on axis 2), kept for broadcasting."""
+    return x.sum([d for d in range(x.dim()) if d not in (0, 2)], keepdim=True)
+
+
+def _alpha_buffer(alpha, like):
+    """None for the scalar 1 (no prior), else alpha as one contiguous fp32 buffer of the batched factor's shape: a scalar, or
+    a tensor that broadcasts to it (a single problem's alpha applies to every problem)."""
+    if _is_one(alpha):
+        return None
+    a = torch.as_tensor(alpha).to(like.device, torch.float32)
+    try:
+        return torch.broadcast_to(a, like.shape).contiguous()
+    except RuntimeError:
+        raise ValueError(f"alpha of shape {tuple(a.shape)} does not broadcast to the factor's {tuple(like.shape)}") from None
+
+
+class _BatchedPLCABase(BaseComponent):
+    """Shared part of the batched PLCA classes: P independent problems of one model and one shape, fitted together.  W and H
+    hold the problems on axis 0 and the rank on axis 2, Z is (P, R); problem p's W[p], H[p], Z[p] are those of the single
+    model.  `fit` runs every problem's EM iteration on the fp32 CUDA-core kernels in the launches one problem takes, each
+    with its own stop rule."""
+    _ndim = 3
+    _axes = "three axes (P, rows, rank)"
+    _engine_cls = None
+    _engine_factory = None
+
+    def __init__(self, rank=None, W=None, H=None, Z=None, trainable_W=True, trainable_H=True, trainable_Z=True):
+        torch.nn.Module.__init__(self)
+        inferred = P = None
+        for name, spec, trainable in (("W", W, trainable_W), ("H", H, trainable_H)):
+            if isinstance(spec, Tensor):
+                assert torch.all(spec >= 0.), f"Tensor {name} should be non-negative."
+                p = Parameter(torch.empty(*spec.size()), requires_grad=trainable)
+                p.data.copy_(spec)
+            elif isinstance(spec, _Iterable):
+                p = Parameter(torch.randn(*tuple(spec)).abs())
+            else:
+                p = None
+            self.register_parameter(name, p)
+            if p is not None:
+                if p.dim() != self._ndim:
+                    raise ValueError(f"{name} must have {self._axes}; got shape {tuple(p.shape)}")
+                if inferred is not None and p.shape[2] != inferred:
+                    raise ValueError("Latent size of H does not match with W")
+                if P is not None and p.shape[0] != P:
+                    raise ValueError(f"W and H hold different numbers of problems ({P} and {p.shape[0]})")
+                inferred, P = p.shape[2], p.shape[0]
+                p.data.div_(_batched_norm(p))
+        if isinstance(Z, Tensor):
+            if Z.dim() != 2:
+                raise ValueError(f"Z must have two axes (P, rank); got shape {tuple(Z.shape)}")
+            assert torch.all(Z >= 0.), "Tensor Z should be non-negative."
+            z = Parameter(torch.empty(*Z.size()), requires_grad=trainable_Z)
+            z.data.copy_(Z)
+        elif P is not None and (inferred or rank):
+            R = inferred or rank
+            z = Parameter(torch.ones(P, R) / R)
+        else:
+            z = None
+        self.register_parameter("Z", z)
+        if z is not None:
+            z.data.div_(z.data.sum(1, keepdim=True))
+            if inferred is not None and z.shape[1] != inferred:
+                raise ValueError("Latent size of Z does not match with others!")
+            if P is not None and z.shape[0] != P:
+                raise ValueError(f"Z holds {z.shape[0]} problems, W / H {P}")
+            inferred = z.shape[1]
+        if inferred is None:
+            assert rank, "A rank should be given when W, H and Z are not available!"
+        else:
+            rank = inferred
+        if self.W is not None:
+            self.out_channels = self.W.shape[1]
+            if self.W.dim() > 3:
+                self.kernel_size = self.W.shape[3:]
+        self.rank = rank
+
+    def forward(self, H=None, W=None, Z=None, norm=None):
+        """Every problem's reconstruction (P, *V's single shape), problem p scaled by norm[p] when `norm` is given."""
+        H = self.H if H is None else H
+        W = self.W if W is None else W
+        Z = self.Z if Z is None else Z
+        out = self.reconstruct(H, W, Z)
+        return out if norm is None else out * torch.as_tensor(norm).reshape(-1, *([1] * (out.dim() - 1)))
+
+    def _single_shape(self):
+        raise NotImplementedError
+
+    def _check_target_shape(self, V):
+        """Whether V is one target shared by every problem (else it is stacked); ValueError if it is neither."""
+        P = self.W.shape[0]
+        single = self._single_shape()
+        if tuple(V.shape) not in ((P,) + single, single):
+            raise ValueError(f"target shape {tuple(V.shape)} does not match H {tuple(self.H.shape)} / W {tuple(self.W.shape)}: "
+                             f"expected {(P,) + single} or {single}")
+        return tuple(V.shape) == single
+
+    @torch.no_grad()
+    def fit(self, V, tol=1e-4, max_iter=200, verbose=False, W_alpha=1., H_alpha=1., Z_alpha=1., *, precision="f32"):
+        """Fit every problem by EM, as the single model's `fit(V[p], ...)` fits one, all of them in the same launches.
+
+        V: the problems' targets stacked on a leading axis, or one target of the single model's shape shared by every
+        problem (random restarts of one fit), of any floating dtype.  Each problem's target is normalised by its sum into
+        one fp32 copy (a shared target once, read by every problem).  A sparse V raises NotImplementedError.
+
+        Returns `(n_iter, norm)`: n_iter a torch.int64 tensor of P values, each what the single `fit` returns for that
+        problem -- the loop index at its stop, or max_iter - 1 -- and norm the P sums V[p].sum() in V's dtype.  Problem p
+        follows the reference's stop rule (plca.py:245-302) on its own: its loss sqrt(2 kl_div(norm_p X_p, V_p)) at the start
+        and every 10th iteration, and it stops at the first check where (previous_p - loss_p) / init_p < tol; from then on
+        every launch leaves its W, H and Z untouched while the others run on.  Each problem's EM step sums in an order fixed
+        by its shape, so problem p's results do not depend on the other problems or on P.  The losses cost one
+        synchronisation per 10 iterations for the whole batch.
+
+        W_alpha / H_alpha / Z_alpha: the Dirichlet priors, each a scalar or a tensor broadcasting to the batched factor's
+        shape (a single problem's alpha applies to every problem).  Frozen factors (trainable_W / _H / _Z) take the
+        reference's branches.  precision: "f32" only ("f16" / "f16_split" and unknown strings raise ValueError), and so does
+        a rank above 256 or a shape mismatch; `last_fit_precision` is "f32".  `mask`, `weight` and `group` are not
+        parameters of this method (TypeError).  Host-resident and half or double modules are staged through fp32 device
+        copies and written back.
+        """
+        name = type(self).__name__
+        if precision != "f32":
+            if precision in ("f16", "f16_split"):
+                raise ValueError(f"{name} runs on the fp32 kernels: precision must be 'f32' (got {precision!r})")
+            raise ValueError(f"unknown precision {precision!r}")
+        if V.is_sparse:
+            raise NotImplementedError(f"{name} takes dense targets only")
+        W, H, Z = self.W, self.H, self.Z
+        assert W is not None and H is not None and Z is not None, "fit() needs W, H and Z"
+        P, R = W.shape[0], W.shape[2]
+        if R > 256:
+            raise ValueError(f"{name} supports rank <= 256 (got {R})")
+        shared = self._check_target_shape(V)
+        assert torch.all(V >= 0.), "Target should be non-negative."                         # plca.py:236
+        f32 = torch.float32
+        if self._engine_factory is None:
+            if not torch.cuda.is_available():
+                raise RuntimeError(f"torchnmf_b200.{name}.fit needs a CUDA device (sm_90a); there is no CPU fallback")
+            on_gpu = W.device.type == "cuda"
+            dev = W.device if on_gpu else torch.device("cuda", torch.cuda.current_device())
+        else:
+            on_gpu, dev = True, W.device
+        # every problem's norm as the single fit takes it (V[p].sum()), whatever P is
+        norm = V.sum().reshape(1).expand(P).clone() if shared else torch.stack([V[p].sum() for p in range(P)])
+        normd = norm.to(dev, f32)
+        Vd = V.to(dev, f32).contiguous()
+        Vn = (Vd / normd[0] if shared else Vd / normd.reshape(P, *([1] * (V.dim() - 1)))).contiguous()     # plca.py:241-242
+        stage = not (on_gpu and all(t.dtype == f32 and t.is_contiguous() for t in (W, H, Z)))
+        Wd, Hd, Zd = ((t.data.to(dev, f32).contiguous() if stage else t.data) for t in (W, H, Z))
+        Hz = (Hd * Zd.reshape(P, 1, R, *([1] * (Hd.dim() - 3)))).contiguous()
+        alphas = [_alpha_buffer(a, t) for a, t in ((W_alpha, Wd), (H_alpha, Hd), (Z_alpha, Zd))]
+        eng = (self._engine_cls if self._engine_factory is None else self._engine_factory)(Vn, Wd, Hz)
+        try:
+            def fit_losses():
+                d = eng.plca_losses(normd).to(torch.float64)
+                return torch.where(d >= 0, torch.sqrt(2.0 * d.clamp(min=0)), float("nan"))  # plca.py:245-246,293-294
+
+            loss_init = fit_losses()
+            previous = loss_init.clone()
+            n_iter = torch.full((P,), max_iter - 1, dtype=torch.int64)
+            active = torch.ones(P, dtype=torch.bool)
+            bar = _tqdm(total=max_iter, disable=not verbose) if _tqdm is not None else None
+            it = -1
+            while it + 1 < max_iter and bool(active.any()):
+                k = min(10 - ((it + 1) % 10), max_iter - (it + 1))
+                eng.plca_iterate(k, Hd, Zd, W.requires_grad, H.requires_grad, Z.requires_grad, *alphas)  # plca.py:247-289
+                it += k
+                if it % 10 == 9:                                                             # plca.py:290-302
+                    loss = fit_losses()
+                    stop = active & ((previous - loss) / loss_init < tol)
+                    n_iter[stop] = it
+                    previous = torch.where(active & ~stop, loss, previous)
+                    if bar is not None:
+                        bar.set_postfix(active=int((active & ~stop).sum()))
+                        bar.update(10)
+                    if bool(stop.any()):
+                        active &= ~stop
+                        eng.set_active(active)
+            eng.check_health()
+            self.last_fit_precision = "f32"
+            if bar is not None:
+                bar.close()
+        finally:
+            eng.close()
+        if stage:
+            W.data.copy_(Wd); H.data.copy_(Hd); Z.data.copy_(Zd)
+        return n_iter, norm
+
+
+class BatchedPLCA(_BatchedPLCABase):
+    """P independent PLCA problems of one shape:  V[p] / sum(V[p]) (N,C) ~= H[p] diag(Z[p]) W[p]^T,  W (P,C,R), H (P,N,R),
+    Z (P,R).  Problem p is `PLCA(W=W[p], H=H[p], Z=Z[p])`.
+
+    Args:
+        Vshape: (P, N, C); W and H are then drawn as `PLCA` draws them, |randn| of (P, C, rank) and (P, N, rank), and every
+            problem's factors normalised
+        rank: size of the hidden dimension (default: C)
+        W / H: a size (iterable of ints -> random non-negative init) or an initial non-negative Tensor
+        Z: an initial non-negative (P, rank) Tensor (default: ones(P, rank) / rank), each row normalised
+        trainable_W / trainable_H / trainable_Z: whether a *given tensor* is updated by `fit`
+
+    `fit(V, ...)` takes V as (P, N, C), or as one (N, C) target shared by every problem.  Each problem's fit is
+    `PLCA.fit(V[p], ..., precision="f32")`'s EM iteration.  Workspace (device memory, kept between fits of the same shape):
+    that of `BatchedNMF` at this shape, plus per fit the raw numerators of W and H (the factors' size) and the EM step's
+    scratch.
+    """
+    _engine_cls = _engine.CudaBatchedNmfEngine
+
+    def __init__(self, Vshape=None, rank=None, *, W=None, H=None, Z=None, trainable_W=True, trainable_H=True,
+                 trainable_Z=True):
+        if isinstance(Vshape, _Iterable):
+            P, N, C = Vshape
+            rank = rank if rank else C
+            W = (P, C, rank) if W is None else W
+            H = (P, N, rank) if H is None else H
+        super().__init__(rank, W, H, Z, trainable_W, trainable_H, trainable_Z)
+
+    @staticmethod
+    def reconstruct(H, W, Z):
+        return H @ (W * Z.unsqueeze(1)).transpose(-1, -2)
+
+    def _single_shape(self):
+        return (self.H.shape[1], self.W.shape[1])
+
+
+class _BatchedShiftInvariant(_BatchedPLCABase):
+    """Shared part of BatchedSIPLCA / BatchedSIPLCA2 / BatchedSIPLCA3: P independent problems of the single model over `_nd`
+    shifted axes, V (P,B,C,*X), W (P,C,R,*K), H (P,B,R,*(X-K+1)), Z (P,R); each problem's B clips share its W[p] and Z[p]."""
+    _engine_cls = _engine.CudaBatchedNmfdEngine
+    _conv = None
+
+    @classmethod
+    def reconstruct(cls, H, W, Z):
+        from .nmf import _batched_conv
+        return _batched_conv(H, W * Z.reshape(*Z.shape, *([1] * (W.dim() - 3))).unsqueeze(1), cls._conv)
+
+    def _single_shape(self):
+        B = self.H.shape[1]
+        C, K, J = self.W.shape[1], self.W.shape[3:], self.H.shape[3:]
+        return (B, C) + tuple(j + k - 1 for j, k in zip(J, K))
+
+
+class BatchedSIPLCA(_BatchedShiftInvariant):
+    """P independent SIPLCA problems of one shape: V[p] (B,C,L), W (P,C,R,T), H (P,B,R,L-T+1), Z (P,R).  Problem p is
+    `SIPLCA(W=W[p], H=H[p], Z=Z[p])`; its B clips share W[p] and Z[p].
+
+    Args:
+        Vshape: (P, B, C, L); W and H are then drawn as `SIPLCA` draws them, |randn| of (P, C, rank, T) and
+            (P, B, rank, L-T+1), and every problem's factors normalised
+        rank: size of the hidden dimension (default: C)
+        T: the kernel's length (an int or a 1-tuple)
+        W / H: a size (iterable of ints -> random non-negative init) or an initial non-negative Tensor
+        Z: an initial non-negative (P, rank) Tensor (default: ones(P, rank) / rank), each row normalised
+        trainable_W / trainable_H / trainable_Z: whether a *given tensor* is updated by `fit`
+
+    `fit(V, ...)` takes V as (P, B, C, L), or as one (B, C, L) target shared by every problem.  Workspace (device memory,
+    kept between fits of the same shape): that of `BatchedNMFD` at this shape, plus per fit the raw numerators of W and H
+    and the EM step's scratch.
+    """
+    _ndim = 4
+    _axes = "four axes (P, rows, rank, T)"
+    _conv = staticmethod(F.conv1d)
+
+    def __init__(self, Vshape=None, rank=None, T=1, *, W=None, H=None, Z=None, trainable_W=True, trainable_H=True,
+                 trainable_Z=True):
+        if isinstance(Vshape, _Iterable):
+            T, = _single(T)
+            P, B, C, L = Vshape
+            rank = rank if rank else C
+            W = (P, C, rank, T) if W is None else W
+            H = (P, B, rank, L - T + 1) if H is None else H
+        super().__init__(rank, W, H, Z, trainable_W, trainable_H, trainable_Z)
+
+
+class BatchedSIPLCA2(_BatchedShiftInvariant):
+    """P independent SIPLCA2 problems of one shape: V[p] (B,C,X1,X2), W (P,C,R,k1,k2), H (P,B,R,X1-k1+1,X2-k2+1), Z (P,R).
+    Problem p is `SIPLCA2(W=W[p], H=H[p], Z=Z[p])`; its B clips share W[p] and Z[p].
+
+    Args:
+        Vshape: (P, B, C, X1, X2); W and H are then drawn as `SIPLCA2` draws them (rank defaults to X1, as there)
+        rank: size of the hidden dimension
+        kernel_size: (k1, k2), or one int for both
+        W / H: a size (iterable of ints -> random non-negative init) or an initial non-negative Tensor
+        Z: an initial non-negative (P, rank) Tensor (default: ones(P, rank) / rank), each row normalised
+        trainable_W / trainable_H / trainable_Z: whether a *given tensor* is updated by `fit`
+
+    `fit(V, ...)` takes V as (P, B, C, X1, X2), or as one (B, C, X1, X2) target shared by every problem.  Workspace: that of
+    `BatchedNMF2D` at this shape, plus per fit the raw numerators of W and H and the EM step's scratch.
+    """
+    _ndim = 5
+    _axes = "five axes (P, rows, rank, k1, k2)"
+    _conv = staticmethod(F.conv2d)
+
+    def __init__(self, Vshape=None, rank=None, kernel_size=1, *, W=None, H=None, Z=None, trainable_W=True,
+                 trainable_H=True, trainable_Z=True):
+        if isinstance(Vshape, _Iterable):
+            kernel_size = _pair(kernel_size)
+            k1, k2 = kernel_size
+            P, B, C, X1, X2 = Vshape
+            rank = rank if rank else X1
+            W = (P, C, rank) + tuple(kernel_size) if W is None else W
+            H = (P, B, rank, X1 - k1 + 1, X2 - k2 + 1) if H is None else H
+        super().__init__(rank, W, H, Z, trainable_W, trainable_H, trainable_Z)
+
+
+class BatchedSIPLCA3(_BatchedShiftInvariant):
+    """P independent SIPLCA3 problems of one shape: V[p] (B,C,X1,X2,X3), W (P,C,R,k1,k2,k3),
+    H (P,B,R,X1-k1+1,X2-k2+1,X3-k3+1), Z (P,R).  Problem p is `SIPLCA3(W=W[p], H=H[p], Z=Z[p])`; its B clips share W[p]
+    and Z[p].
+
+    Args:
+        Vshape: (P, B, C, X1, X2, X3); W and H are then drawn as `SIPLCA3` draws them (rank defaults to X2, as there)
+        rank: size of the hidden dimension
+        kernel_size: (k1, k2, k3), or one int for all three
+        W / H: a size (iterable of ints -> random non-negative init) or an initial non-negative Tensor
+        Z: an initial non-negative (P, rank) Tensor (default: ones(P, rank) / rank), each row normalised
+        trainable_W / trainable_H / trainable_Z: whether a *given tensor* is updated by `fit`
+
+    `fit(V, ...)` takes V as (P, B, C, X1, X2, X3), or as one (B, C, X1, X2, X3) target shared by every problem.  Workspace:
+    that of `BatchedNMF3D` at this shape, plus per fit the raw numerators of W and H and the EM step's scratch.
+    """
+    _ndim = 6
+    _axes = "six axes (P, rows, rank, k1, k2, k3)"
+    _conv = staticmethod(F.conv3d)
+
+    def __init__(self, Vshape=None, rank=None, kernel_size=1, *, W=None, H=None, Z=None, trainable_W=True,
+                 trainable_H=True, trainable_Z=True):
+        if isinstance(Vshape, _Iterable):
+            kernel_size = _triple(kernel_size)
+            k1, k2, k3 = kernel_size
+            P, B, C, X1, X2, X3 = Vshape
+            rank = rank if rank else X2
+            W = (P, C, rank) + tuple(kernel_size) if W is None else W
+            H = (P, B, rank, X1 - k1 + 1, X2 - k2 + 1, X3 - k3 + 1) if H is None else H
+        super().__init__(rank, W, H, Z, trainable_W, trainable_H, trainable_Z)
