@@ -363,6 +363,30 @@ class _BatchedEngine(_CudaEngine):
     the loss is one value per problem."""
     _set_active = None                     # the C ABI's set_active call of this context kind
 
+    def __init__(self, V, W, H):
+        """V stacked on a leading problem axis, or one target of a single problem's shape shared by every problem (read at
+        problem stride 0), on W's device; W and H contiguous fp32.  Every problem starts active."""
+        super().__init__()
+        self.device = W.device
+        if V.dim() == W.dim() - 1:
+            V = V.unsqueeze(0).expand(W.shape[0], *V.shape)              # one target: problem stride 0
+        if V.dtype not in _capi.DTYPES:
+            raise TypeError(f"V must be float32, float16 or bfloat16 (got {V.dtype})")
+        if V.device != self.device:
+            raise ValueError(f"V is on {V.device}, expected {self.device}")
+        for t, n in ((W, "W"), (H, "H")):
+            _check_f32_cuda(t, n, self.device)
+        dev_index = self.device.index if self.device.index is not None else torch.cuda.current_device()
+        self._loss = torch.zeros(W.shape[0], dtype=torch.float64, device=self.device)
+        self._create(V, W, H, dev_index)
+        self.V, self.W, self.H = V, W, H
+        self.set_active(None)
+        self.sync()
+
+    def _create(self, V, W, H, dev_index):
+        """Check the shapes, take a context for them and set V (problems on axis 0) as its target."""
+        raise NotImplementedError
+
     @property
     def precision(self):
         return "f32"
@@ -434,33 +458,16 @@ class CudaBatchedNmfEngine(_BatchedEngine):
     kind = "nmf_batched"
     _set_active = "nmfb200_nmf_batched_set_active"
 
-    def __init__(self, V, W, H):
-        super().__init__()
-        self.device = W.device
-        if V.dim() == 2:
-            V = V.unsqueeze(0).expand(W.shape[0], *V.shape)              # one target: batch stride 0
-        if V.dtype not in _capi.DTYPES:
-            raise TypeError(f"V must be float32, float16 or bfloat16 (got {V.dtype})")
-        if V.device != self.device:
-            raise ValueError(f"V is on {V.device}, expected {self.device}")
-        for t, n in ((W, "W"), (H, "H")):
-            _check_f32_cuda(t, n, self.device)
+    def _create(self, V, W, H, dev_index):
         B, N, C = V.shape
         R = W.shape[2]
         assert W.shape == (B, C, R) and H.shape == (B, N, R)
         if not (V.stride(2) == 1 and V.stride(1) >= C and (V.stride(0) == 0 or V.stride(0) >= N * V.stride(1))):
             raise ValueError("V must have unit column stride, rows at least C apart and problems at least N rows apart")
-        self.V, self.W, self.H = V, W, H
-        self.B, self.N, self.C, self.R = B, N, C, R
-        self._active = None
-        dev_index = self.device.index if self.device.index is not None else torch.cuda.current_device()
         self._acquire(("nmf_batched", dev_index, B, N, C, R),
                       lambda ref: self._lib.nmfb200_nmf_batched_create(ref, dev_index, B, N, C, R))
-        self._loss = torch.zeros(B, dtype=torch.float64, device=self.device)
         _capi.check(self._lib.nmfb200_nmf_batched_set_target(self._ctx, _ptr(V), V.stride(1), V.stride(0),
                                                              _capi.DTYPES[V.dtype], _stream(self.device)))
-        _capi.check(self._lib.nmfb200_nmf_batched_set_active(self._ctx, None, _stream(self.device)))
-        self.sync()
 
     def iterate(self, n_iter, beta, gamma, l1_reg, l2_reg):
         """n_iter x (update_w; update_h) of every active problem in one call."""
@@ -478,35 +485,19 @@ class CudaBatchedNmfdEngine(_BatchedEngine):
     kind = "nmfd_batched"
     _set_active = "nmfb200_nmfd_batched_set_active"
 
-    def __init__(self, V, W, H):
-        super().__init__()
-        self.device = W.device
+    def _create(self, V, W, H, dev_index):
         P, C, R, *K = W.shape
-        nd = len(K)
-        if V.dim() == nd + 2:
-            V = V.unsqueeze(0).expand(P, *V.shape)                       # one target: problem stride 0
-        if V.dtype not in _capi.DTYPES:
-            raise TypeError(f"V must be float32, float16 or bfloat16 (got {V.dtype})")
-        if V.device != self.device:
-            raise ValueError(f"V is on {V.device}, expected {self.device}")
-        for t, n in ((W, "W"), (H, "H")):
-            _check_f32_cuda(t, n, self.device)
         _, B, _, *X = V.shape
+        nd = len(K)
         assert 1 <= nd <= 3 and len(X) == nd
         assert W.shape == (P, C, R, *K) and H.shape == (P, B, R, *(x - k + 1 for x, k in zip(X, K)))
         if not (V[0].is_contiguous() and (V.stride(0) == 0 or V.stride(0) >= V[0].numel())):
             raise ValueError("every problem's block of V must be contiguous, the blocks 0 or at least B C prod(X) apart")
-        self.V, self.W, self.H = V, W, H
-        self._active = None
-        dev_index = self.device.index if self.device.index is not None else torch.cuda.current_device()
         vd, kd = (ctypes.c_int64 * nd)(*X), (ctypes.c_int64 * nd)(*K)
         self._acquire(("nmfd_batched", dev_index, P, B, C, tuple(X), R, tuple(K)),
                       lambda ref: self._lib.nmfb200_nmfnd_batched_create(ref, dev_index, P, B, C, nd, vd, R, kd))
-        self._loss = torch.zeros(P, dtype=torch.float64, device=self.device)
         _capi.check(self._lib.nmfb200_nmfd_batched_set_target(self._ctx, _ptr(V), V.stride(0), _capi.DTYPES[V.dtype],
                                                               _stream(self.device)))
-        _capi.check(self._lib.nmfb200_nmfd_batched_set_active(self._ctx, None, _stream(self.device)))
-        self.sync()
 
 
 def _compressed_forms(V, weights=None):

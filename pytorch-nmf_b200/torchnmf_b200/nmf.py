@@ -19,6 +19,7 @@ device above that rank, for sharded fits and for `sparse_fit`).
 raw-terms launch, line-search losses from the fused loss launch, every component projected by ONE
 `nmfb200_hoyer_project` launch.  `trainer.BetaMu` / `SparsityProj` and `plca.*` live in their own modules.
 """
+import contextlib
 import math
 import weakref
 from collections.abc import Iterable as _Iterable
@@ -686,6 +687,97 @@ class NMFD(BaseComponent):
                                f"W {tuple(self.W.shape)}")
 
 
+# ---- many independent problems in one fit: what the batched NMF and PLCA classes share ------------------------------------
+
+def _register_batched_factors(module, W, H, trainable_W, trainable_H):
+    """Register W and H on a batched module (problems on axis 0, rank on axis 2): a Tensor is copied, an iterable of ints
+    draws |randn| of that size, None registers None.  A factor without the class's `_ndim` axes, or W and H disagreeing on
+    the rank or on the number of problems, raises ValueError.  Sets out_channels (and kernel_size, for a convolutive W)
+    from W.  Returns (rank, number of problems) of the factors, None for each when neither is given."""
+    rank = P = None
+    for name, spec, trainable in (("W", W, trainable_W), ("H", H, trainable_H)):
+        if isinstance(spec, Tensor):
+            assert torch.all(spec >= 0.), f"Tensor {name} should be non-negative."
+            p = Parameter(torch.empty(*spec.size()), requires_grad=trainable)
+            p.data.copy_(spec)
+        elif isinstance(spec, _Iterable):
+            p = Parameter(torch.randn(*tuple(spec)).abs())
+        else:
+            p = None
+        module.register_parameter(name, p)
+        if p is not None:
+            if p.dim() != module._ndim:
+                raise ValueError(f"{name} must have {module._axes}; got shape {tuple(p.shape)}")
+            if rank is not None and p.shape[2] != rank:
+                raise ValueError("Latent size of H does not match with W")
+            if P is not None and p.shape[0] != P:
+                raise ValueError(f"W and H hold different numbers of problems ({P} and {p.shape[0]})")
+            rank, P = p.shape[2], p.shape[0]
+    if module.W is not None:
+        module.out_channels = module.W.shape[1]
+        if module.W.dim() > 3:
+            module.kernel_size = module.W.shape[3:]
+    return rank, P
+
+
+@contextlib.contextmanager
+def _placed_factors(module, factors, no_cuda):
+    """Places a batched fit: yields (device, the fp32 contiguous tensors the engine updates, one per Parameter of
+    `factors`).  They are the Parameters' own storages when every factor is fp32 and contiguous on a CUDA device, else
+    device copies, written back into the Parameters when the block completes.  Without CUDA it raises
+    RuntimeError(no_cuda).  With the `_engine_factory` test hook the storages are taken where they are."""
+    f32 = torch.float32
+    if module._engine_factory is not None:
+        dev, staged = factors[0].device, False
+    else:
+        if not torch.cuda.is_available():
+            raise RuntimeError(no_cuda)
+        on_gpu = factors[0].device.type == "cuda"
+        dev = factors[0].device if on_gpu else torch.device("cuda", torch.cuda.current_device())
+        staged = not (on_gpu and all(t.dtype == f32 and t.is_contiguous() for t in factors))
+    placed = [t.data.to(dev, f32, non_blocking=True).contiguous() if staged else t.data for t in factors]
+    yield dev, placed
+    if staged:
+        for t, d in zip(factors, placed):
+            t.data.copy_(d)
+
+
+def _fit_problems(eng, P, max_iter, tol, verbose, losses, step):
+    """The reference's stop rule (nmf.py:366-409, plca.py:245-302) for each of P problems fitted together on `eng`: problem
+    p's loss sqrt(2 d_p) (NaN for d_p < 0) from `losses()`, the P raw divergences, at the start and every 10th iteration,
+    and it stops at the first check where (previous_p - loss_p) / init_p < tol; `eng.set_active` then freezes it while the
+    others run on.  `step(k)` runs k iterations of every active problem, at most 10 and never past a check.  Returns the
+    int64 iteration count of every problem: the iterations it ran, max_iter for one that never stopped."""
+    def fit_losses():
+        d = losses().to(torch.float64)
+        return torch.where(d >= 0, torch.sqrt(2.0 * d.clamp(min=0)), float("nan"))
+
+    loss_init = fit_losses()
+    previous = loss_init.clone()
+    n_iter = torch.full((P,), max_iter, dtype=torch.int64)
+    active = torch.ones(P, dtype=torch.bool)
+    bar = _tqdm(total=max_iter, disable=not verbose) if _tqdm is not None else _NullBar()
+    it = -1
+    with bar as pbar:
+        while it + 1 < max_iter and bool(active.any()):
+            k = min(10 - ((it + 1) % 10), max_iter - (it + 1))
+            step(k)
+            it += k
+            if it % 10 == 9:
+                loss = fit_losses()
+                stop = active & ((previous - loss) / loss_init < tol)
+                n_iter[stop] = it + 1
+                previous = torch.where(active & ~stop, loss, previous)
+                pbar.set_postfix(active=int((active & ~stop).sum()))
+                pbar.update(10)
+                if bool(stop.any()):
+                    active &= ~stop
+                    eng.set_active(active)
+    if hasattr(eng, "check_health"):
+        eng.check_health()
+    return n_iter
+
+
 class _BatchedComponent(BaseComponent):
     """Shared part of the batched classes: P independent problems of one model and one shape, fitted together.  W and H
     hold the problems on their leading axis and the rank on axis 2; problem p's factors W[p] / H[p] are those of the
@@ -696,31 +788,11 @@ class _BatchedComponent(BaseComponent):
 
     def __init__(self, rank=None, W=None, H=None, trainable_W=True, trainable_H=True):
         torch.nn.Module.__init__(self)
-        inferred = None
-        for name, spec, trainable in (("W", W, trainable_W), ("H", H, trainable_H)):
-            if isinstance(spec, Tensor):
-                assert torch.all(spec >= 0.), f"Tensor {name} should be non-negative."
-                p = Parameter(torch.empty(*spec.size()), requires_grad=trainable)
-                p.data.copy_(spec)
-            elif isinstance(spec, _Iterable):
-                p = Parameter(torch.randn(*tuple(spec)).abs())
-            else:
-                p = None
-            self.register_parameter(name, p)
-            if p is not None:
-                if p.dim() != self._ndim:
-                    raise ValueError(f"{name} must have {self._axes}; got shape {tuple(p.shape)}")
-                if inferred is not None and p.shape[2] != inferred:
-                    raise ValueError("Latent size of H does not match with W")
-                inferred = p.shape[2]
+        inferred, _ = _register_batched_factors(self, W, H, trainable_W, trainable_H)
         if inferred is None:
             assert rank, "A rank should be given when W and H are not available!"
         else:
             rank = inferred
-        if self.W is not None and self.H is not None and self.W.shape[0] != self.H.shape[0]:
-            raise ValueError(f"W and H hold different numbers of problems ({self.W.shape[0]} and {self.H.shape[0]})")
-        if self.W is not None:
-            self.out_channels = self.W.shape[1]
         self.rank = rank
 
     def _readable_in_place(self, Vd):
@@ -767,55 +839,30 @@ class _BatchedComponent(BaseComponent):
         if W.shape[2] > 256:
             raise ValueError(f"{name} supports rank <= 256 (got {W.shape[2]})")
         self._check_target_shape(V)
-        B = W.shape[0]
 
-        staged = False
-        if self._engine_factory is None:
-            if not torch.cuda.is_available():
-                raise RuntimeError("torchnmf_b200.fit needs a CUDA device (sm_90a); there is no CPU fallback")
-            f32 = torch.float32
-            on_gpu = W.device.type == "cuda"
-            dev = W.device if on_gpu else torch.device("cuda", torch.cuda.current_device())
-            Vd = V.to(dev, non_blocking=True)
-            if Vd.dtype not in (torch.float32, torch.float16, torch.bfloat16):
-                Vd = Vd.to(f32)
-            if not self._readable_in_place(Vd):
-                Vd = Vd.contiguous()
-            if on_gpu and W.dtype == f32 and H.dtype == f32 and W.is_contiguous() and H.is_contiguous():
-                Wd, Hd = W.data, H.data
+        no_cuda = "torchnmf_b200.fit needs a CUDA device (sm_90a); there is no CPU fallback"
+        with _placed_factors(self, (W, H), no_cuda) as (dev, (Wd, Hd)):
+            if self._engine_factory is None:
+                Vd = V.to(dev, non_blocking=True)
+                if Vd.dtype not in (torch.float32, torch.float16, torch.bfloat16):
+                    Vd = Vd.to(torch.float32)
+                if not self._readable_in_place(Vd):
+                    Vd = Vd.contiguous()
+                eng = self._engine_cls(Vd, Wd, Hd)
             else:
-                staged = True
-                Wd = W.data.to(dev, f32, non_blocking=True).contiguous()
-                Hd = H.data.to(dev, f32, non_blocking=True).contiguous()
-            eng = self._engine_cls(Vd, Wd, Hd)
-        else:
-            Wd, Hd = W.data, H.data
-            eng = self._engine_factory(V, Wd, Hd)
+                eng = self._engine_factory(V, Wd, Hd)
+            try:
+                vmin, vmax = eng.minmax()
+                assert vmin >= 0., "Target should be non-negative."                        # nmf.py:329-330
+                if vmin == 0 and beta <= 0:                                                # nmf.py:332-336
+                    raise ValueError("When beta <= 0 and V contains zeros, the training process may diverge. "
+                                     "Please add small values to V, or use a positive beta value.")
+                gamma = _gamma(beta)
+                l1_reg = alpha * l1_ratio                                                  # nmf.py:348
+                l2_reg = alpha * (1 - l1_ratio)                                            # nmf.py:349
+                train_w, train_h = W.requires_grad, H.requires_grad
 
-        try:
-            vmin, vmax = eng.minmax()
-            assert vmin >= 0., "Target should be non-negative."                            # nmf.py:329-330
-            if vmin == 0 and beta <= 0:                                                    # nmf.py:332-336
-                raise ValueError("When beta <= 0 and V contains zeros, the training process may diverge. "
-                                 "Please add small values to V, or use a positive beta value.")
-            gamma = _gamma(beta)
-            l1_reg = alpha * l1_ratio                                                      # nmf.py:348
-            l2_reg = alpha * (1 - l1_ratio)                                                # nmf.py:349
-
-            def fit_losses():
-                d = eng.losses(beta).to(torch.float64)
-                return torch.where(d >= 0, torch.sqrt(2.0 * d.clamp(min=0)), float("nan"))  # nmf.py:362,402
-
-            loss_init = fit_losses()
-            previous = loss_init.clone()
-            n_iter = torch.full((B,), max_iter, dtype=torch.int64)
-            active = torch.ones(B, dtype=torch.bool)
-            train_w, train_h = W.requires_grad, H.requires_grad
-            bar = _tqdm(total=max_iter, disable=not verbose) if _tqdm is not None else _NullBar()
-            it = -1
-            with bar as pbar:
-                while it + 1 < max_iter and bool(active.any()):
-                    k = min(10 - ((it + 1) % 10), max_iter - (it + 1))
+                def step(k):
                     if train_w and train_h and hasattr(eng, "iterate"):
                         eng.iterate(k, beta, gamma, l1_reg, l2_reg)                        # nmf.py:366-391, k times
                     else:
@@ -824,26 +871,11 @@ class _BatchedComponent(BaseComponent):
                                 eng.update_w(beta, gamma, l1_reg, l2_reg)                  # nmf.py:367-378
                             if train_h:
                                 eng.update_h(beta, gamma, l1_reg, l2_reg)                  # nmf.py:380-391
-                    it += k
-                    if it % 10 == 9:                                                       # nmf.py:393
-                        loss = fit_losses()
-                        with torch.no_grad():
-                            stop = active & ((previous - loss) / loss_init < tol)          # nmf.py:405, per problem
-                        n_iter[stop] = it + 1
-                        previous = torch.where(active & ~stop, loss, previous)
-                        pbar.set_postfix(active=int((active & ~stop).sum()))
-                        pbar.update(10)
-                        if bool(stop.any()):
-                            active &= ~stop
-                            eng.set_active(active)
-            if hasattr(eng, "check_health"):
-                eng.check_health()
-            if staged:
-                W.data.copy_(Wd)
-                H.data.copy_(Hd)
-            self.last_fit_precision = "f32"
-        finally:
-            eng.close()
+
+                n_iter = _fit_problems(eng, W.shape[0], max_iter, tol, verbose, lambda: eng.losses(beta), step)
+                self.last_fit_precision = "f32"
+            finally:
+                eng.close()
         return n_iter
 
 
@@ -912,11 +944,6 @@ class _BatchedConvolutive(_BatchedComponent):
     _engine_cls = _engine.CudaBatchedNmfdEngine
     _nd = 1
     _conv = None
-
-    def __init__(self, rank, W, H, trainable_W, trainable_H):
-        super().__init__(rank, W, H, trainable_W, trainable_H)
-        if self.W is not None:
-            self.kernel_size = self.W.shape[3:]
 
     @classmethod
     def reconstruct(cls, H, W):

@@ -25,6 +25,7 @@ from torch.nn import Parameter
 
 from .constants import eps
 from . import engine as _engine
+from .nmf import _batched_conv, _fit_problems, _placed_factors, _register_batched_factors
 
 from torch.nn.modules.utils import _single, _pair, _triple
 
@@ -350,25 +351,9 @@ class _BatchedPLCABase(BaseComponent):
 
     def __init__(self, rank=None, W=None, H=None, Z=None, trainable_W=True, trainable_H=True, trainable_Z=True):
         torch.nn.Module.__init__(self)
-        inferred = P = None
-        for name, spec, trainable in (("W", W, trainable_W), ("H", H, trainable_H)):
-            if isinstance(spec, Tensor):
-                assert torch.all(spec >= 0.), f"Tensor {name} should be non-negative."
-                p = Parameter(torch.empty(*spec.size()), requires_grad=trainable)
-                p.data.copy_(spec)
-            elif isinstance(spec, _Iterable):
-                p = Parameter(torch.randn(*tuple(spec)).abs())
-            else:
-                p = None
-            self.register_parameter(name, p)
+        inferred, P = _register_batched_factors(self, W, H, trainable_W, trainable_H)
+        for p in (self.W, self.H):
             if p is not None:
-                if p.dim() != self._ndim:
-                    raise ValueError(f"{name} must have {self._axes}; got shape {tuple(p.shape)}")
-                if inferred is not None and p.shape[2] != inferred:
-                    raise ValueError("Latent size of H does not match with W")
-                if P is not None and p.shape[0] != P:
-                    raise ValueError(f"W and H hold different numbers of problems ({P} and {p.shape[0]})")
-                inferred, P = p.shape[2], p.shape[0]
                 p.data.div_(_batched_norm(p))
         if isinstance(Z, Tensor):
             if Z.dim() != 2:
@@ -393,10 +378,6 @@ class _BatchedPLCABase(BaseComponent):
             assert rank, "A rank should be given when W, H and Z are not available!"
         else:
             rank = inferred
-        if self.W is not None:
-            self.out_channels = self.W.shape[1]
-            if self.W.dim() > 3:
-                self.kernel_size = self.W.shape[3:]
         self.rank = rank
 
     def forward(self, H=None, W=None, Z=None, norm=None):
@@ -457,57 +438,25 @@ class _BatchedPLCABase(BaseComponent):
         shared = self._check_target_shape(V)
         assert torch.all(V >= 0.), "Target should be non-negative."                         # plca.py:236
         f32 = torch.float32
-        if self._engine_factory is None:
-            if not torch.cuda.is_available():
-                raise RuntimeError(f"torchnmf_b200.{name}.fit needs a CUDA device (sm_90a); there is no CPU fallback")
-            on_gpu = W.device.type == "cuda"
-            dev = W.device if on_gpu else torch.device("cuda", torch.cuda.current_device())
-        else:
-            on_gpu, dev = True, W.device
-        # every problem's norm as the single fit takes it (V[p].sum()), whatever P is
-        norm = V.sum().reshape(1).expand(P).clone() if shared else torch.stack([V[p].sum() for p in range(P)])
-        normd = norm.to(dev, f32)
-        Vd = V.to(dev, f32).contiguous()
-        Vn = (Vd / normd[0] if shared else Vd / normd.reshape(P, *([1] * (V.dim() - 1)))).contiguous()     # plca.py:241-242
-        stage = not (on_gpu and all(t.dtype == f32 and t.is_contiguous() for t in (W, H, Z)))
-        Wd, Hd, Zd = ((t.data.to(dev, f32).contiguous() if stage else t.data) for t in (W, H, Z))
-        Hz = (Hd * Zd.reshape(P, 1, R, *([1] * (Hd.dim() - 3)))).contiguous()
-        alphas = [_alpha_buffer(a, t) for a, t in ((W_alpha, Wd), (H_alpha, Hd), (Z_alpha, Zd))]
-        eng = (self._engine_cls if self._engine_factory is None else self._engine_factory)(Vn, Wd, Hz)
-        try:
-            def fit_losses():
-                d = eng.plca_losses(normd).to(torch.float64)
-                return torch.where(d >= 0, torch.sqrt(2.0 * d.clamp(min=0)), float("nan"))  # plca.py:245-246,293-294
+        no_cuda = f"torchnmf_b200.{name}.fit needs a CUDA device (sm_90a); there is no CPU fallback"
+        with _placed_factors(self, (W, H, Z), no_cuda) as (dev, (Wd, Hd, Zd)):
+            # every problem's norm as the single fit takes it (V[p].sum()), whatever P is
+            norm = V.sum().reshape(1).expand(P).clone() if shared else torch.stack([V[p].sum() for p in range(P)])
+            normd = norm.to(dev, f32)
+            Vd = V.to(dev, f32).contiguous()
+            Vn = (Vd / normd[0] if shared else Vd / normd.reshape(P, *([1] * (V.dim() - 1)))).contiguous()  # plca.py:241-242
+            Hz = (Hd * Zd.reshape(P, 1, R, *([1] * (Hd.dim() - 3)))).contiguous()
+            alphas = [_alpha_buffer(a, t) for a, t in ((W_alpha, Wd), (H_alpha, Hd), (Z_alpha, Zd))]
+            eng = (self._engine_cls if self._engine_factory is None else self._engine_factory)(Vn, Wd, Hz)
+            try:
+                def step(k):                                                                 # plca.py:247-289, k times
+                    eng.plca_iterate(k, Hd, Zd, W.requires_grad, H.requires_grad, Z.requires_grad, *alphas)
 
-            loss_init = fit_losses()
-            previous = loss_init.clone()
-            n_iter = torch.full((P,), max_iter - 1, dtype=torch.int64)
-            active = torch.ones(P, dtype=torch.bool)
-            bar = _tqdm(total=max_iter, disable=not verbose) if _tqdm is not None else None
-            it = -1
-            while it + 1 < max_iter and bool(active.any()):
-                k = min(10 - ((it + 1) % 10), max_iter - (it + 1))
-                eng.plca_iterate(k, Hd, Zd, W.requires_grad, H.requires_grad, Z.requires_grad, *alphas)  # plca.py:247-289
-                it += k
-                if it % 10 == 9:                                                             # plca.py:290-302
-                    loss = fit_losses()
-                    stop = active & ((previous - loss) / loss_init < tol)
-                    n_iter[stop] = it
-                    previous = torch.where(active & ~stop, loss, previous)
-                    if bar is not None:
-                        bar.set_postfix(active=int((active & ~stop).sum()))
-                        bar.update(10)
-                    if bool(stop.any()):
-                        active &= ~stop
-                        eng.set_active(active)
-            eng.check_health()
-            self.last_fit_precision = "f32"
-            if bar is not None:
-                bar.close()
-        finally:
-            eng.close()
-        if stage:
-            W.data.copy_(Wd); H.data.copy_(Hd); Z.data.copy_(Zd)
+                # the single fit returns its loop index: one less than the iterations it ran (plca.py:304)
+                n_iter = _fit_problems(eng, P, max_iter, tol, verbose, lambda: eng.plca_losses(normd), step) - 1
+                self.last_fit_precision = "f32"
+            finally:
+                eng.close()
         return n_iter, norm
 
 
@@ -555,7 +504,6 @@ class _BatchedShiftInvariant(_BatchedPLCABase):
 
     @classmethod
     def reconstruct(cls, H, W, Z):
-        from .nmf import _batched_conv
         return _batched_conv(H, W * Z.reshape(*Z.shape, *([1] * (W.dim() - 3))).unsqueeze(1), cls._conv)
 
     def _single_shape(self):
