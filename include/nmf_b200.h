@@ -329,6 +329,21 @@ int nmfb200_loss(nmfb200_ctx* ctx, const float* W, const float* H, double beta, 
  * kernels above. */
 int64_t nmfb200_raw_terms_numel(const nmfb200_ctx* ctx, int which, double beta);
 int nmfb200_raw_terms(nmfb200_ctx* ctx, const float* W, const float* H, int which, double beta, float* out, void* stream);
+
+/* The gradient terms of one EM step of a PLCA / SIPLCA* fit on a partially observed target, from the current W and
+ * Hz = H Z without touching either.  The mask M (nmfb200_set_mask) holds the observed cells O; the registered target is
+ * Vn = V / sum_O V on O (its missing cells are never read); q = W Hz (NMF) or conv(Hz, W) (NMFD / NMF2D / NMF3D) the
+ * model, q_O = sum_O q.  The EM step's ratio on the completed target is q_O M Vn / (q + eps) + (1 - M) q / (q + eps), so
+ * the factor's gradient is q_O A + B with
+ *   A = the backward pass of M Vn / (q + eps)        (the masked beta-1 numerator),
+ *   B = the backward pass of (1 - M) q / (q + eps)   (the missing cells' fill term),
+ * and `out` receives [A | B], each the factor's numel (which = 0: W, 1: Hz), raw-summed as nmfb200_raw_terms' slabs.
+ * qobs_dev (optional device double): q_O, from one partial per block of the same pass summed in a fixed order.  One
+ * contraction pass over V and M per call, as nmfb200_raw_terms at beta 1.  fp32 CUDA-core kernels, fp32 V; NMFD / NMF2D /
+ * NMF3D up to rank 256.  NMFB200_ERR_STATE before set_target or without a mask; NMFB200_ERR_INVALID for a weight, a
+ * sparse, observed-cell or batched context, a non-fp32 target, or an NMFD rank above 256.  Asynchronous. */
+int nmfb200_plca_masked_terms(nmfb200_ctx* ctx, const float* W, const float* Hz, int which, float* out, double* qobs_dev,
+                              void* stream);
 int nmfb200_w_apply(nmfb200_ctx* ctx, float* W, const float* reduced, double beta, double gamma, double l1_reg,
                     double l2_reg, void* stream);
 

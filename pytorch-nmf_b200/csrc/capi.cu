@@ -66,6 +66,9 @@ struct nmfb200_ctx {
   // NMFD
   float* Pn = nullptr;
   float* Pp = nullptr;
+  // nmfb200_plca_masked_terms on NMF: one q_O partial per block of the fp32 contraction (grown on demand)
+  double* qobs_part = nullptr;
+  int64_t qobs_part_n = 0;
   // tensor-core path state (tc_nmf.cu / tc_nmfd.cu)
   TcState* tc = nullptr;
   TcNmfdState* tcd = nullptr;
@@ -145,7 +148,7 @@ void free_ctx(nmfb200_ctx* c) {
   if (c->tcd) tc_nmfd_destroy(c->tcd);
   cudaFree(c->num); cudaFree(c->den); cudaFree(c->colsum); cudaFree(c->cs_scratch);
   cudaFree(c->loss_blocks); cudaFree(c->mm_scratch); cudaFree(c->Pn); cudaFree(c->Pp);
-  cudaFree(c->sp_gram); cudaFree(c->sp_loss_part); cudaFree(c->sp_den);
+  cudaFree(c->sp_gram); cudaFree(c->sp_loss_part); cudaFree(c->sp_den); cudaFree(c->qobs_part);
   delete c;
 }
 
@@ -1065,6 +1068,55 @@ int nmfb200_w_apply(nmfb200_ctx* ctx, float* W, const float* reduced, double bet
   if (rc) return rc;
   if (!tc) mark_stale(ctx, true, false);
   return 0;
+}
+
+/* ---- masked PLCA: the two gradient terms of one EM step on a partially observed target ---------------------------- */
+
+int nmfb200_plca_masked_terms(nmfb200_ctx* ctx, const float* W, const float* Hz, int which, float* out, double* qobs_dev,
+                              void* stream) {
+  CTX_GUARD(ctx, kAnyKind);
+  if (is_batch(ctx)) return fail(NMFB200_ERR_INVALID, "plca_masked_terms does not serve batched contexts");
+  TARGET_GUARD(ctx);
+  if (ctx->sparse || ctx->observed) return fail(NMFB200_ERR_INVALID, "plca_masked_terms needs a dense target");
+  if (ctx->sel.kind == kSelWeight) return fail(NMFB200_ERR_INVALID, "plca_masked_terms takes a mask, not a weight");
+  if (!ctx->sel) return fail(NMFB200_ERR_STATE, "plca_masked_terms needs a mask (nmfb200_set_mask)");
+  if (ctx->vdtype != NMFB200_DTYPE_F32) return fail(NMFB200_ERR_INVALID, "plca_masked_terms needs an fp32 target");
+  if (is_nmfd(ctx) && ctx->R > 256) return fail(NMFB200_ERR_INVALID, "plca_masked_terms: NMFD rank must be <= 256");
+  if (!W || !Hz || !out || (which != 0 && which != 1)) return fail(NMFB200_ERR_INVALID, "bad argument");
+  cudaStream_t st = (cudaStream_t)stream;
+  if (int e = ensure_den(ctx)) return e;
+  const float* V = static_cast<const float*>(ctx->V);
+  const uint8_t* M = static_cast<const uint8_t*>(ctx->sel.p);
+  int rc;
+  if (is_nmfd(ctx)) {        // the fill-mode ratio tiles (and q_O), then their backward passes
+    if (!ctx->Pp) NMF_CUDA_CHECK(cudaMalloc(&ctx->Pp, (size_t)ctx->d.B * ctx->d.C * ctx->d.v_inner() * sizeof(float)));
+    rc = nmfd_plca_fill(ctx->d, V, W, Hz, ctx->Pn, ctx->Pp, M, ctx->loss_blocks, ctx->loss_max_blocks, qobs_dev, st);
+    auto grad = [&](const float* P, float* part) {
+      return which == 0 ? nmfd_wgrad(ctx->d, P, Hz, part, ctx->nslab[0], st)
+                        : nmfd_dgrad(ctx->d, P, W, part, ctx->nslab[1], st);
+    };
+    if (rc == 0) rc = grad(ctx->Pn, ctx->num);
+    if (rc == 0) rc = grad(ctx->Pp, ctx->den);
+  } else {                   // W: F = W, G = Hz over V^T;  H: F = Hz, G = W over V (simt_contract's roles)
+    const FactorDims f = factor_dims(ctx, which);
+    const int nch = ctx->nslab[which];
+    const int64_t nblocks = simt_plca_fill_blocks(f.rows, nch);
+    if (qobs_dev && ctx->qobs_part_n < nblocks) {
+      cudaFree(ctx->qobs_part);
+      ctx->qobs_part = nullptr; ctx->qobs_part_n = 0;
+      NMF_CUDA_CHECK(cudaMalloc(&ctx->qobs_part, (size_t)nblocks * sizeof(double)));
+      ctx->qobs_part_n = nblocks;
+    }
+    const float* fac[2] = {W, Hz};
+    rc = simt_plca_fill_contract(V, ctx->ldv, /*trans=*/which == 0, fac[which], fac[1 - which], f.rows, f.other_rows,
+                                 (int)ctx->R, nch, ctx->num, ctx->den, ctx->R, f.rows * ctx->R, M, ctx->C,
+                                 qobs_dev ? ctx->qobs_part : nullptr, st);
+    if (rc == 0 && qobs_dev) rc = sum_partials(ctx->qobs_part, (int)nblocks, qobs_dev, st);
+  }
+  if (rc) return rc;
+  ApplyArgs a = factor_view(ctx, which, ctx->nslab[which]);
+  a.num = ctx->num; a.den = ctx->den;
+  return raw_sum(a, out, out + a.numel, st);
 }
 
 /* ---- batched PLCA: the EM iteration on the raw terms of a batched NMF / NMFD context ---------------------------- */

@@ -80,6 +80,10 @@ __device__ __forceinline__ bool batch_skips(const uint8_t* active, int64_t b) { 
 
 // beta-divergence branch of nmf.py:61-74 / metrics.py:60-96
 enum BetaMode : int { kKL = 0, kEU = 1, kIS = 2, kGeneric = 3 };
+// The term mode of a masked PLCA fit (nmfb200_plca_masked_terms), beside BetaMode (and simt_nmf.cu's kVFree = 4): with the
+// uint8 mask, Pn = v / (s + eps) at an observed cell and 0 elsewhere, Pp = s / (s + eps) at a missing cell and 0 elsewhere,
+// and the pass sums s over the observed cells it covers into one double partial per block.  fp32 V, one problem.
+constexpr int kPlcaFill = 5;
 inline BetaMode beta_mode(double beta) {
   if (beta == 1.0) return kKL;
   if (beta == 2.0) return kEU;
@@ -178,6 +182,15 @@ int simt_nmf_loss(const void* V, int vdtype, int64_t ldv, const float* F, const 
                   int R, double beta, double* block_partials, int max_blocks, double* loss_dev, CellSel M,
                   int64_t ldm, cudaStream_t st, const Batch& bt = Batch{});
 int simt_nmf_max_blocks(int64_t Mr, int64_t Nc);
+// The terms of one factor of a masked PLCA fit on simt_nmf_contract's plan at beta 1 (kPlcaFill), fp32 V, uint8 mask M:
+//   num[ch][m][r] = sum_{c in chunk ch} M Vm[m,c] / (S[m,c] + eps) G[c,r]
+//   den[ch][m][r] = sum_{c in chunk ch} (1 - M) S[m,c] / (S[m,c] + eps) G[c,r]
+// and, when qobs_part is not null, qobs_part[ch * ceil(Mr / 64) + row block] = the sum of S over the observed cells of that
+// block's tiles (rank-blocked plans: output block 0 only), simt_plca_fill_blocks of them.
+int simt_plca_fill_contract(const float* V, int64_t ldv, int trans, const float* F, const float* G, int64_t Mr, int64_t Nc,
+                            int R, int nchunks, float* num, float* den, int64_t ldp, int64_t chunk_stride, const uint8_t* M,
+                            int64_t ldm, double* qobs_part, cudaStream_t st);
+int64_t simt_plca_fill_blocks(int64_t Mr, int nchunks);
 // The V-free pieces of a sparse target's update and loss at beta != 1, 2 (nmf.py:621-636):
 //   den[ch][m][r] = sum_{c in chunk ch} (S[m,c] + eps)^(beta-1) G[c,r]: simt_nmf_contract's denominator at this beta, bit for
 //   bit (same grid, chunks and arithmetic), without reading V; R <= 256.
@@ -301,6 +314,11 @@ struct NmfdShape {
 int nmfd_recon_phi(const NmfdShape& s, const void* V, int vdtype, const float* W, const float* H, double beta,
                    float* Pn, float* Pp, double* loss_blocks, int max_blocks, double* loss_dev,
                    cudaStream_t st, CellSel M = CellSel{}, const Batch& bt = Batch{});
+// The kPlcaFill mode of nmfd_recon_phi (one problem, fp32 V, uint8 mask M in V's layout, rank <= 256): Pn = M V / (WH + eps)
+// and Pp = (1 - M) WH / (WH + eps) in V's layout, and *qobs_dev = the sum of WH over the observed cells, from one double
+// partial per block of all its launches (nmfd_max_blocks, at most max_blocks) summed in a fixed order.
+int nmfd_plca_fill(const NmfdShape& s, const float* V, const float* W, const float* H, float* Pn, float* Pp,
+                   const uint8_t* M, double* part, int max_blocks, double* qobs_dev, cudaStream_t st);
 // batch elements per launch of the kernels that put the batch on grid.z (fp32 recon / dgrad, tensor-core recon / dgrad)
 static inline int64_t nmfd_batch_slice(int64_t B) { return B < kMaxGridYZ ? B : kMaxGridYZ; }
 // loss partials of nmfd_recon_phi: one per block of all its launches

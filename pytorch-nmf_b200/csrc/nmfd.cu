@@ -90,11 +90,17 @@ struct SlideArgs {
 // SEL (FWD only): a fit on the observed cells -- at a missing cell V is not read, Pn = Pp = 0 and the loss adds nothing;
 // Pp is written at every beta (beta 1: the mask as 0 / 1), so wgrad / dgrad of Pp give the denominators.  A weighted fit
 // treats the cells of weight 0 as missing and multiplies Pn, Pp and the loss term by the weight elsewhere (beta 1: Pp = w).
+// kPlcaFill (FWD, !LOSS, fp32 V, the uint8 mask, one problem; a masked PLCA fit): Pn = V / (WH + eps) and Pp = 0 at an
+// observed cell, Pn = 0 and Pp = WH / (WH + eps) at a missing one (V not read), and, when a.block_partials is set, each
+// block's sum of WH over its observed cells into the loss partial the LOSS pass of this launch would write.
 template <int MT, bool FWD, int MODE, bool LOSS, typename TV, typename SEL = NoSel, bool BATCH = false>
 __global__ void __launch_bounds__(256)
 nmfd_slide_kernel(NmfdShape s, SlideArgs a, Batch bt) {
   constexpr bool MASK = !std::is_same<SEL, NoSel>::value;
   constexpr bool WEIGHT = kWeighted<SEL>;
+  constexpr bool FILL = (MODE == kPlcaFill);
+  static_assert(!FILL || (FWD && !LOSS && std::is_same<SEL, uint8_t>::value && std::is_same<TV, float>::value && !BATCH),
+                "kPlcaFill: the FWD pass of one problem, fp32 V, the uint8 mask");
   using G = Geo<MT>;
   constexpr int WIN = kLT + kTK;                          // window pitch per line (kLT + kTK - 1 elements used)
   __shared__ __align__(16) float As[kTK * G::PAD];        // As[tt][m]
@@ -229,11 +235,16 @@ nmfd_slide_kernel(NmfdShape s, SlideArgs a, Batch bt) {
             continue;
           }
           if (MASK && !static_cast<const uint8_t*>(a.mask)[off]) {
-            if (!LOSS) { a.Pn[off] = 0.f; a.Pp[off] = 0.f; }
+            if (FILL) { a.Pn[off] = 0.f; a.Pp[off] = acc[i][j] / (acc[i][j] + kEps); }
+            else if (!LOSS) { a.Pn[off] = 0.f; a.Pp[off] = 0.f; }
             continue;
           }
           const float v = to_f32(static_cast<const TV*>(a.V)[off]);
-          if (LOSS) {
+          if (FILL) {
+            a.Pn[off] = v / (acc[i][j] + kEps);
+            a.Pp[off] = 0.f;
+            local += acc[i][j];
+          } else if (LOSS) {
             if (BATCH && MODE == kKL) local += loss_term_d<MODE>(sc * v, sc * acc[i][j], a.beta);
             else local += loss_term_d<MODE>(v, acc[i][j], a.beta);
           } else {
@@ -246,7 +257,7 @@ nmfd_slide_kernel(NmfdShape s, SlideArgs a, Batch bt) {
         }
       }
     }
-    if (LOSS) {
+    if (LOSS || (FILL && a.block_partials)) {
       const double tot = block_sum_d((double)local, red);
       if (tid == 0)
         a.block_partials[((int64_t)b * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x] = tot;
@@ -415,6 +426,9 @@ void launch_slide(const NmfdShape& s, const SlideArgs& a, const Batch& bt, int m
 #define NMFD_GO(M)                                                                                  \
   if (loss) nmfd_slide_kernel<MT, true, M, true, TV, SEL, BATCH><<<grid, 256, 0, st>>>(s, a, bt);   \
   else nmfd_slide_kernel<MT, true, M, false, TV, SEL, BATCH><<<grid, 256, 0, st>>>(s, a, bt);
+  if constexpr (std::is_same<TV, float>::value && std::is_same<SEL, uint8_t>::value && !BATCH) {
+    if (mode == kPlcaFill) { nmfd_slide_kernel<MT, true, kPlcaFill, false, TV, SEL, false><<<grid, 256, 0, st>>>(s, a, bt); return; }
+  }
   switch (mode) {
     case kKL: NMFD_GO(kKL); break;
     case kEU: NMFD_GO(kEU); break;
@@ -498,6 +512,20 @@ int nmfd_recon_phi(const NmfdShape& s, const void* V, int vdtype, const float* W
       }))
     return rc;
   if (loss) return sum_partials(loss_blocks, nblocks, loss_dev, st, bt.n, bt.active);
+  return 0;
+}
+
+int nmfd_plca_fill(const NmfdShape& s, const float* V, const float* W, const float* H, float* Pn, float* Pp,
+                   const uint8_t* M, double* part, int max_blocks, double* qobs_dev, cudaStream_t st) {
+  const int mt = row_tile(s.C);
+  const int nblocks = (int)nmfd_max_blocks(s);
+  if (!M) { set_error("nmfd_plca_fill: needs the mask"); return 1; }
+  if (qobs_dev && (!part || nblocks > max_blocks)) { set_error("nmfd_plca_fill: partial buffer too small"); return 1; }
+  SlideArgs a{};
+  a.A = W; a.X = H; a.M = s.C; a.K = s.R; a.sm = (int64_t)s.R * s.w_inner(); a.sk = s.w_inner(); a.nsplit = 1;
+  a.V = V; a.beta = 1.f; a.Pn = Pn; a.Pp = Pp; a.block_partials = qobs_dev ? part : nullptr; a.out = nullptr; a.mask = M;
+  if (int rc = launch_slices<true, float, uint8_t>(mt, s, a, slide_batch(s, true, Batch{}), kPlcaFill, false, st)) return rc;
+  if (qobs_dev) return sum_partials(part, nblocks, qobs_dev, st);
   return 0;
 }
 

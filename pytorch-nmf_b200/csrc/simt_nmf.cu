@@ -26,6 +26,11 @@
 // kVFree (sparse targets at beta != 1, 2): the contraction forms only den += (S+eps)^(beta-1) G_tile and reads no V, with
 // kGeneric's plan, staging and arithmetic, so its den partials equal kGeneric's bit for bit whatever V holds; the loss sums
 // (S+eps)^beta over every cell, again without V.
+//
+// kPlcaFill (common.cuh; a masked PLCA fit, fp32 V and the uint8 mask only): the masked KL numerator pn = v / (s+eps) at the
+// observed cells, and pp = s / (s+eps) at the missing ones -- the expected complete data of the EM there -- in place of the
+// mask.  The CTAs of output block 0 also sum s over their observed cells (fp32 per tile and thread, double across tiles,
+// then one fixed-order block reduction) into one partial each, so q_O comes out of the same pass.
 #include "common.cuh"
 
 namespace nmfb200 {
@@ -67,6 +72,20 @@ __device__ __forceinline__ void stage_chunk(float* Xs, const float* __restrict__
   }
 }
 
+__device__ __forceinline__ double block_reduce_sum(double v, double* sh) {
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  int w = threadIdx.x >> 5, l = threadIdx.x & 31;
+  if (l == 0) sh[w] = v;
+  __syncthreads();
+  double t = 0.0;
+  if (w == 0) {
+    int nw = (blockDim.x + 31) >> 5;
+    t = l < nw ? sh[l] : 0.0;
+    for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
+  }
+  return t;   // valid in warp 0
+}
+
 template <int MODE>
 __device__ __forceinline__ void phi(float v, float s, float bm2, float bm1, float& pn, float& pp) {
   if (MODE == kKL) {
@@ -91,9 +110,13 @@ __global__ void __launch_bounds__(256)
 simt_contract_kernel(const TV* __restrict__ V, int64_t ldv, const float* __restrict__ F,
                      const float* __restrict__ G, int64_t Mr, int64_t Nc, int R, float bm2, float bm1,
                      int nchunks, float* __restrict__ num, float* __restrict__ den, int64_t ldp,
-                     int64_t chunk_stride, const SEL* __restrict__ Mk, int64_t ldm, Batch bt) {
+                     int64_t chunk_stride, const SEL* __restrict__ Mk, int64_t ldm, Batch bt,
+                     double* __restrict__ qobs_part) {
   constexpr bool MASK = !std::is_same<SEL, NoSel>::value;
   constexpr bool WEIGHT = kWeighted<SEL>;
+  constexpr bool kFill = (MODE == kPlcaFill);
+  static_assert(!kFill || (std::is_same<SEL, uint8_t>::value && std::is_same<TV, float>::value && !BATCH),
+                "kPlcaFill: fp32 V, the uint8 mask, one problem");
   constexpr int Rp = 16 * RB;
   constexpr bool kDenOnly = (MODE == kVFree);
   constexpr bool kNum = !kDenOnly;
@@ -137,6 +160,7 @@ simt_contract_kernel(const TV* __restrict__ V, int64_t ldv, const float* __restr
   for (int i = 0; i < 4; ++i)
 #pragma unroll
     for (int k = 0; k < RB; ++k) { accn[i][k] = 0.f; accd[i][k] = 0.f; }
+  double qacc = 0.0;                // kFill: this thread's sum of s over its observed cells
 
   for (int64_t tile = tile_begin; tile < tile_end; ++tile) {
     const int64_t c0 = tile * kTile;
@@ -181,6 +205,7 @@ simt_contract_kernel(const TV* __restrict__ V, int64_t ldv, const float* __restr
       else
         gemm1(Fs, Gs, Rp, tx, ty, s);
     }
+    float qloc = 0.f;
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
       if (kDenOnly) {
@@ -195,8 +220,10 @@ simt_contract_kernel(const TV* __restrict__ V, int64_t ldv, const float* __restr
       }
       float4 v4 = *reinterpret_cast<const float4*>(&Ps[(4 * ty + i) * kLd + 4 * tx]);
       float vv[4] = {v4.x, v4.y, v4.z, v4.w}, pn[4], pp[4];
+      if constexpr (!kFill) {
 #pragma unroll
-      for (int j = 0; j < 4; ++j) phi<MODE>(vv[j], s[i][j], bm2, bm1, pn[j], pp[j]);
+        for (int j = 0; j < 4; ++j) phi<MODE>(vv[j], s[i][j], bm2, bm1, pn[j], pp[j]);
+      }
       if (MASK) {
         float4 m4 = *reinterpret_cast<const float4*>(&Qs[(4 * ty + i) * kLd + 4 * tx]);
         const float mv[4] = {m4.x, m4.y, m4.z, m4.w};
@@ -206,6 +233,12 @@ simt_contract_kernel(const TV* __restrict__ V, int64_t ldv, const float* __restr
           if constexpr (WEIGHT) {
             pn[j] = seen ? pn[j] * mv[j] : 0.f;
             pp[j] = MODE == kKL ? mv[j] : (seen ? pp[j] * mv[j] : 0.f);
+          } else if constexpr (kFill) {
+            // one division per cell: v / (s+eps) where observed (kKL's pn), s / (s+eps) where missing
+            const float r = (seen ? vv[j] : s[i][j]) / (s[i][j] + kEps);
+            pn[j] = seen ? r : 0.f;
+            pp[j] = seen ? 0.f : r;
+            if (seen) qloc += s[i][j];
           } else {
             pn[j] = seen ? pn[j] : 0.f;
             pp[j] = MODE == kKL ? mv[j] : (seen ? pp[j] : 0.f);
@@ -216,6 +249,7 @@ simt_contract_kernel(const TV* __restrict__ V, int64_t ldv, const float* __restr
       if (kTwo)
         *reinterpret_cast<float4*>(&Qs[(4 * ty + i) * kLd + 4 * tx]) = make_float4(pp[0], pp[1], pp[2], pp[3]);
     }
+    if (kFill) qacc += (double)qloc;
     __syncthreads();
 
 #pragma unroll 2
@@ -253,6 +287,14 @@ simt_contract_kernel(const TV* __restrict__ V, int64_t ldv, const float* __restr
       }
     }
   }
+  if constexpr (kFill) {
+    // every cell's s is the same in each output block: block 0 alone counts it.  (The row loop above exits no thread.)
+    if (qobs_part && ob == 0) {
+      __shared__ double red[8];
+      const double tot = block_reduce_sum(qacc, red);
+      if (tid == 0) qobs_part[(int64_t)chunk * gridDim.x + blockIdx.x] = tot;
+    }
+  }
 }
 
 template <int RB, bool TRANS, typename TV, typename SEL, bool BATCH>
@@ -265,7 +307,7 @@ int launch_contract_mode(int mode, dim3 grid, size_t smem, cudaStream_t st, cons
     auto kern = simt_contract_kernel<RB, TRANS, M, TV, SEL, BATCH>;                                     \
     NMF_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
     kern<<<grid, 256, smem, st>>>(V, ldv, F, G, Mr, Nc, R, bm2, bm1, nchunks, num, den, ldp,            \
-                                  chunk_stride, Mk, ldm, bt);                                           \
+                                  chunk_stride, Mk, ldm, bt, nullptr);                                  \
   }
   switch (mode) {
     case kKL: NMF_LAUNCH_MODE(kKL); break;
@@ -304,20 +346,6 @@ int launch_contract_rb(int trans, int mode, dim3 grid, cudaStream_t st, const TV
 }
 
 // ---- loss ------------------------------------------------------------------------------------
-
-__device__ __forceinline__ double block_reduce_sum(double v, double* sh) {
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  int w = threadIdx.x >> 5, l = threadIdx.x & 31;
-  if (l == 0) sh[w] = v;
-  __syncthreads();
-  double t = 0.0;
-  if (w == 0) {
-    int nw = (blockDim.x + 31) >> 5;
-    t = l < nw ? sh[l] : 0.0;
-    for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
-  }
-  return t;   // valid in warp 0
-}
 
 // SEL: the sum runs over the observed cells only (the missing ones are dropped, not zeroed: at beta != 0, 1, 2 a zeroed
 // cell would still add eps^beta / beta); a weighted fit adds w * term over the cells with w != 0
@@ -530,7 +558,7 @@ int simt_nmf_contract_den(const float* F, const float* G, int64_t Mr, int64_t Nc
     auto kern = simt_contract_kernel<RBV, false, kVFree, float>;                                                     \
     NMF_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));              \
     kern<<<grid, 256, smem, st>>>(nullptr, 0, F, G, Mr, Nc, R, 0.f, bm1, nchunks, nullptr, den, ldp, chunk_stride,   \
-                                  nullptr, 0, Batch{});                                                              \
+                                  nullptr, 0, Batch{}, nullptr);                                                     \
   } break
   switch (contract_rb(R)) {
     case 1: NMF_DEN(1);
@@ -540,6 +568,40 @@ int simt_nmf_contract_den(const float* F, const float* G, int64_t Mr, int64_t Nc
     default: NMF_DEN(16);
   }
 #undef NMF_DEN
+  NMF_LAUNCH_CHECK();
+  return 0;
+}
+
+int64_t simt_plca_fill_blocks(int64_t Mr, int nchunks) { return ceil_div(Mr, kTile) * nchunks; }
+
+int simt_plca_fill_contract(const float* V, int64_t ldv, int trans, const float* F, const float* G, int64_t Mr, int64_t Nc,
+                            int R, int nchunks, float* num, float* den, int64_t ldp, int64_t chunk_stride, const uint8_t* M,
+                            int64_t ldm, double* qobs_part, cudaStream_t st) {
+  if (R < 1) { set_error("simt_plca_fill_contract: rank must be positive"); return 1; }
+  if (!M) { set_error("simt_plca_fill_contract: needs the mask"); return 1; }
+  const dim3 grid((unsigned)ceil_div(Mr, kTile), (unsigned)nchunks, (unsigned)simt_rank_blocks(R));
+  const int Rp = 16 * contract_rb(R);
+  const size_t smem = (size_t)(2 * Rp + 2 * kTile) * kLd * sizeof(float);      // Fs, Gs, the V / Pn and mask / Pp tiles
+#define NMF_FILL(RBV, TR)                                                                                              \
+  {                                                                                                                    \
+    auto kern = simt_contract_kernel<RBV, TR, kPlcaFill, float, uint8_t>;                                              \
+    NMF_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));                \
+    kern<<<grid, 256, smem, st>>>(V, ldv, F, G, Mr, Nc, R, 0.f, 0.f, nchunks, num, den, ldp, chunk_stride, M, ldm,     \
+                                  Batch{}, qobs_part);                                                                 \
+  }
+#define NMF_FILL_RB(RBV)                  \
+  if (trans) NMF_FILL(RBV, true)          \
+  else NMF_FILL(RBV, false)               \
+  break
+  switch (contract_rb(R)) {
+    case 1: NMF_FILL_RB(1);
+    case 2: NMF_FILL_RB(2);
+    case 4: NMF_FILL_RB(4);
+    case 8: NMF_FILL_RB(8);
+    default: NMF_FILL_RB(16);
+  }
+#undef NMF_FILL_RB
+#undef NMF_FILL
   NMF_LAUNCH_CHECK();
   return 0;
 }

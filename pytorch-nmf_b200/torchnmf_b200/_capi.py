@@ -61,6 +61,7 @@ SIGNATURES = {
     "nmfb200_plca_work_numel": (_i64, [_vp]),
     "nmfb200_plca_iterate": (_int, [_vp, _vp, _vp, _vp, _vp, _vp, _int, _vp, _vp, _vp, _int, _vp]),
     "nmfb200_plca_loss": (_int, [_vp, _vp, _vp, _vp, _vp, _vp]),
+    "nmfb200_plca_masked_terms": (_int, [_vp, _vp, _vp, _int, _vp, _vp, _vp]),
     "nmfb200_sync_factors": (_int, [_vp]),
     "nmfb200_update_w": (_int, [_vp, _vp, _vp, _dbl, _dbl, _dbl, _dbl, _vp]),
     "nmfb200_update_h": (_int, [_vp, _vp, _vp, _dbl, _dbl, _dbl, _dbl, _vp]),

@@ -255,6 +255,18 @@ class _CudaEngine:
         num, den = buf[:f.numel()].view(f.shape), buf[f.numel():]
         return num, (den if beta == 1 and self._mask is None and self._weight is None else den.view(f.shape))
 
+    def plca_masked_terms(self, which, qobs=None):
+        """(A, B), each in the shape of W (which=0) or H (which=1), of one EM step of a PLCA fit on the observed cells of V
+        (set_mask), from the current factors: with W and H = H diag(Z) the model q, its mass q_O on the observed cells and
+        V the normalised observed target, the step's gradient of that factor is q_O A + B (include/nmf_b200.h:
+        nmfb200_plca_masked_terms).  `qobs`: an optional float64 device tensor of one element that receives q_O."""
+        f = self.W if which == 0 else self.H
+        n = f.numel()
+        buf = torch.empty(2 * n, dtype=torch.float32, device=self.device)
+        _capi.check(self._lib.nmfb200_plca_masked_terms(self._ctx, _ptr(self.W), _ptr(self.H), int(which), _ptr(buf),
+                                                        _ptr(qobs) if qobs is not None else None, _stream(self.device)))
+        return buf[:n].view(f.shape), buf[n:].view(f.shape)
+
     def _raw_terms_into(self, which, beta, buf):
         """nmfb200_raw_terms flat into `buf`, or into a new buffer when `buf` is None or of another size; returns it."""
         n = int(self._lib.nmfb200_raw_terms_numel(self._ctx, int(which), float(beta)))

@@ -120,7 +120,8 @@ class BaseComponent(torch.nn.Module):
         raise NotImplementedError
 
     @torch.no_grad()
-    def fit(self, V, tol=1e-4, max_iter=200, verbose=False, W_alpha=1., H_alpha=1., Z_alpha=1., *, precision="f32"):
+    def fit(self, V, tol=1e-4, max_iter=200, verbose=False, W_alpha=1., H_alpha=1., Z_alpha=1., *, precision="f32",
+            mask=None):
         """EM fit of the PLCA model (reference: plca.py:193-304; same arguments, stop rule and return value
         `(n_iter, norm)`).  Runs on the parameters' CUDA device; host-resident modules are staged like `NMF.fit`.
 
@@ -128,7 +129,21 @@ class BaseComponent(torch.nn.Module):
                    "f16" / "f16_split" (wgmma contraction: ~10x faster at large shapes; the EM recursion keeps the
                    fp16 operand rounding, measured 1.0-1.4e-3 relative after 30-50 iterations on the fixtures of
                    tests/golden/reference_next.npz -- outside the 1e-3 bar, hence opt-in).  SIPLCA2 / SIPLCA3 at "f16"
-                   run the tensor-core sliding GEMMs of NMFD with the outer axes (rank <= 256)."""
+                   run the tensor-core sliding GEMMs of NMFD with the outer axes (rank <= 256).
+        mask:      (keyword-only, default None) a dense torch.bool tensor of V's shape, True where V is observed: the fit
+                   maximises the observed-data log-likelihood sum_O Vn log(q / q_O) (plus the Dirichlet priors), with O the
+                   observed cells, q the model (summing to 1), q_O = sum_O q and Vn = V / sum_O V, by EM over the missing
+                   cells (Smaragdis, Raj and Shashanka's missing-data PLCA): every iteration is the reference's EM step on
+                   the completed target q_O Vn on O and q off O.  Zeroing the missing cells instead would fit them as
+                   observed zeros.  V is never read off O (NaN there is fine).  The loss and stop rule are the reference's
+                   on O, with the model rescaled to the observed mass: sqrt(2 kl_div(x[O], V[O])), x = q sum_O V / q_O.
+                   Returns `(n_iter, norm)` with norm = sum_O V / q_O at the final factors, so `model(norm=norm)`
+                   reconstructs V at its own scale and `model(norm=norm)[~mask]` is the imputation.  fp32 kernels only
+                   (precision "f32"); a dense V; rank <= 256 for the shift-invariant models.  ValueError for a mask that is
+                   not a dense torch.bool tensor of V's shape, a sparse V, another precision, no observed cell or
+                   sum_O V = 0."""
+        if mask is not None:
+            return self._fit_masked(V, mask, tol, max_iter, verbose, W_alpha, H_alpha, Z_alpha, precision)
         assert torch.all(V >= 0.), "Target should be non-negative."                         # plca.py:236
         W, H, Z = self.W, self.H, self.Z
         assert W is not None and H is not None and Z is not None, "fit() needs W, H and Z"
@@ -151,72 +166,168 @@ class BaseComponent(torch.nn.Module):
             d = float(_kl(WZH * normd, Vfull))
             return math.sqrt(2.0 * d) if d >= 0 else float("nan")                           # plca.py:245-246,293-294
 
-        def over(z, x):                               # a rank vector against the rank dimension (1) of a factor
-            return z[(slice(None),) + (None,) * (x.dim() - 2)]                               # plca.py:269-270,282-283
-
-        Hz = (Hd * over(Zd, Hd)).contiguous()         # the engine's activation factor: H diag(Z)
+        Hz = (Hd * _over(Zd, Hd)).contiguous()        # the engine's activation factor: H diag(Z)
         eng = self._engine(Vn, Wd, Hz, precision)
         try:
-            loss_init = previous_loss = loss_now()
-            bar = _tqdm(total=max_iter, disable=not verbose) if _tqdm is not None else None
-            n_iter = -1
-            for n_iter in range(max_iter):
-                torch.mul(Hd, over(Zd, Hd), out=Hz)
+            def step():
+                torch.mul(Hd, _over(Zd, Hd), out=Hz)
                 eng.sync()
                 dW, _ = eng.raw_terms(0, 1.0)         # P contracted with H Z  = W.grad   (plca.py:252-253)
                 dHz, _ = eng.raw_terms(1, 1.0)        # P contracted with W;  H.grad = dHz * Z,  Z.grad = sum H dHz
-                dH = dHz * over(Zd, Hd)
-                dZ = get_norm(Hd * dHz).reshape(-1)
-                Z_prior = None
-                if Z.requires_grad:                                                          # plca.py:256-262
-                    Zd.mul_(dZ.clamp_min(0))
-                    Z_prior = Zd.clone()
-                    if not _is_one(Z_alpha):
-                        Zd.add_(_as(Z_alpha, Zd) - 1)
-                        F.threshold(Zd, eps, eps, True)
-                    Zd.div_(Zd.sum())
-                if W.requires_grad:                                                          # plca.py:264-275
-                    Wd.mul_(dW.clamp_min(0))
-                    if Z_prior is None:
-                        W_div = get_norm(Wd)
-                        Z_prior = W_div.squeeze()
-                    else:
-                        W_div = over(Z_prior, Wd)
-                    Wd.div_(W_div)
-                    if not _is_one(W_alpha):
-                        Wd.add_(_as(W_alpha, Wd) - 1)
-                        F.threshold(Wd, eps, eps, True)
-                        Wd.div_(get_norm(Wd))
-                if H.requires_grad:                                                          # plca.py:277-288
-                    Hd.mul_(dH.clamp_min(0))
-                    H_div = get_norm(Hd) if Z_prior is None else over(Z_prior, Hd)
-                    Hd.div_(H_div)
-                    if not _is_one(H_alpha):
-                        Hd.add_(_as(H_alpha, Hd) - 1)
-                        F.threshold(Hd, eps, eps, True)
-                        Hd.div_(get_norm(Hd))
-                if n_iter % 10 == 9:                                                         # plca.py:290-302
-                    loss = loss_now()
-                    if bar is not None:
-                        bar.set_postfix(loss=loss)
-                        bar.update(10)
-                    if (previous_loss - loss) / loss_init < tol:
-                        break
-                    previous_loss = loss
-            eng.check_health()
+                self._em_update(Wd, Hd, Zd, dW, dHz, W_alpha, H_alpha, Z_alpha)
+
+            n_iter = _em_loop(step, loss_now, tol, max_iter, verbose, eng.check_health)
             self.last_fit_precision = eng.precision_for(1.0)
-            if bar is not None:
-                bar.close()
         finally:
             eng.close()
         if stage:
             W.data.copy_(Wd); H.data.copy_(Hd); Z.data.copy_(Zd)
         return n_iter, norm                                                                  # plca.py:304
 
+    def _em_update(self, Wd, Hd, Zd, dW, dHz, W_alpha, H_alpha, Z_alpha):
+        """The Z, W and H updates of one EM step (plca.py:256-288) from the raw gradients dW and dHz (= H.grad / Z),
+        in place on the working copies, each taken only where the module's factor is trainable."""
+        dH = dHz * _over(Zd, Hd)
+        dZ = get_norm(Hd * dHz).reshape(-1)
+        Z_prior = None
+        if self.Z.requires_grad:                                                             # plca.py:256-262
+            Zd.mul_(dZ.clamp_min(0))
+            Z_prior = Zd.clone()
+            if not _is_one(Z_alpha):
+                Zd.add_(_as(Z_alpha, Zd) - 1)
+                F.threshold(Zd, eps, eps, True)
+            Zd.div_(Zd.sum())
+        if self.W.requires_grad:                                                             # plca.py:264-275
+            Wd.mul_(dW.clamp_min(0))
+            if Z_prior is None:
+                W_div = get_norm(Wd)
+                Z_prior = W_div.squeeze()
+            else:
+                W_div = _over(Z_prior, Wd)
+            Wd.div_(W_div)
+            if not _is_one(W_alpha):
+                Wd.add_(_as(W_alpha, Wd) - 1)
+                F.threshold(Wd, eps, eps, True)
+                Wd.div_(get_norm(Wd))
+        if self.H.requires_grad:                                                             # plca.py:277-288
+            Hd.mul_(dH.clamp_min(0))
+            H_div = get_norm(Hd) if Z_prior is None else _over(Z_prior, Hd)
+            Hd.div_(H_div)
+            if not _is_one(H_alpha):
+                Hd.add_(_as(H_alpha, Hd) - 1)
+                F.threshold(Hd, eps, eps, True)
+                Hd.div_(get_norm(Hd))
+
+    def _check_mask(self, V, mask, precision):
+        """The masked fit's refusals, before any device work: (the mask on V's device, sum_O V in V's dtype)."""
+        if not isinstance(mask, Tensor) or mask.dtype != torch.bool:
+            raise ValueError(f"mask must be a torch.bool tensor (got {getattr(mask, 'dtype', type(mask))})")
+        if mask.is_sparse:
+            raise ValueError(f"mask: {type(self).__name__}.fit takes a dense mask only")
+        if tuple(mask.shape) != tuple(V.shape):
+            raise ValueError(f"mask shape {tuple(mask.shape)} does not match the target's {tuple(V.shape)}")
+        if V.is_sparse:
+            raise ValueError("mask: a masked fit needs a dense target")
+        if precision != "f32":
+            raise ValueError(f"mask: masked fits run on the fp32 kernels; precision must be 'f32' (got {precision!r})")
+        M = mask.to(V.device)
+        assert bool(torch.where(M, V >= 0., True).all()), "Target should be non-negative."   # plca.py:236, on O only
+        if not bool(M.any()):
+            raise ValueError("mask: no cell of the target is observed")
+        norm_o = torch.where(M, V, torch.zeros((), dtype=V.dtype, device=V.device)).sum()
+        if not bool(norm_o > 0):
+            raise ValueError("mask: the observed cells of the target sum to 0")
+        return M, norm_o
+
+    def _fit_masked(self, V, mask, tol, max_iter, verbose, W_alpha, H_alpha, Z_alpha, precision):
+        """fit(V, ..., mask=mask): EM with the missing cells latent (see fit)."""
+        M, norm_o = self._check_mask(V, mask, precision)
+        W, H, Z = self.W, self.H, self.Z
+        assert W is not None and H is not None and Z is not None, "fit() needs W, H and Z"
+        if not torch.cuda.is_available():
+            raise RuntimeError(f"torchnmf_b200.{type(self).__name__}.fit needs a CUDA device (sm_90a); there is no CPU "
+                               "fallback")
+        f32 = torch.float32
+        on_gpu = W.device.type == "cuda"
+        dev = W.device if on_gpu else torch.device("cuda", torch.cuda.current_device())
+        Md = M.to(dev).contiguous()
+        normd = norm_o.to(dev, f32)
+        # Vn on O and 0 off O: the kernels never meet what V holds at the missing cells
+        Vn = (torch.where(Md, V.to(dev, f32), torch.zeros((), dtype=f32, device=dev)) / normd).contiguous()
+        stage = not (on_gpu and all(t.dtype == f32 for t in (W, H, Z)))
+        Wd = W.data.to(dev, f32).contiguous() if stage else W.data
+        Hd = H.data.to(dev, f32).contiguous() if stage else H.data
+        Zd = Z.data.to(dev, f32).contiguous() if stage else Z.data
+        Vobs = Vn * normd
+
+        def q_obs():
+            q = self.reconstruct(Hd, Wd, Zd)
+            return q, torch.where(Md, q, 0.).sum()
+
+        def loss_now():
+            # kl_div(x[O], V[O]) with the model scaled to the observed mass, x = q sum_O V / q_O; Vobs is 0 off O
+            q, qo = q_obs()
+            x = q * (normd / qo)
+            d = float(Vobs.reshape(-1) @ (torch.log(Vobs + eps) - torch.log(x + eps)).reshape(-1) - Vobs.sum()
+                      + torch.where(Md, x, 0.).sum())
+            return math.sqrt(2.0 * d) if d >= 0 else float("nan")
+
+        Hz = (Hd * _over(Zd, Hd)).contiguous()
+        qobs = torch.zeros(1, dtype=torch.float64, device=dev)
+        eng = self._engine(Vn, Wd, Hz, precision)
+        try:
+            eng.set_mask(Md)
+
+            def step():
+                # the reference's EM step on the completed target q_O Vn (O) / q (off O): its gradients are q_O A + B
+                torch.mul(Hd, _over(Zd, Hd), out=Hz)
+                eng.sync()
+                aW, bW = eng.plca_masked_terms(0, qobs)
+                aH, bH = eng.plca_masked_terms(1)
+                q = qobs.to(f32)
+                self._em_update(Wd, Hd, Zd, torch.addcmul(bW, aW, q), torch.addcmul(bH, aH, q), W_alpha, H_alpha, Z_alpha)
+
+            n_iter = _em_loop(step, loss_now, tol, max_iter, verbose, eng.check_health)
+            self.last_fit_precision = "f32"
+        finally:
+            eng.close()
+        # the returned norm's q_O in float64 (the fp32 reconstruction may run on TF32 convolutions)
+        q = self.reconstruct(Hd.double(), Wd.double(), Zd.double())
+        qo = torch.where(Md, q, 0.).sum()
+        if stage:
+            W.data.copy_(Wd); H.data.copy_(Hd); Z.data.copy_(Zd)
+        return n_iter, (norm_o.double() / qo.to(norm_o.device)).to(norm_o.dtype)
 
     @staticmethod
     def _engine(Vn, W, Hz, precision):
         raise NotImplementedError
+
+
+def _over(z, x):
+    """A rank vector against the rank dimension (1) of a factor (plca.py:269-270,282-283)."""
+    return z[(slice(None),) + (None,) * (x.dim() - 2)]
+
+
+def _em_loop(step, loss_now, tol, max_iter, verbose, check_health):
+    """The reference's iteration loop (plca.py:247-302): `step()` max_iter times, the loss before the first and after every
+    10th, stopping at the first check where (previous - loss) / initial < tol.  Returns the last loop index."""
+    loss_init = previous_loss = loss_now()
+    bar = _tqdm(total=max_iter, disable=not verbose) if _tqdm is not None else None
+    n_iter = -1
+    for n_iter in range(max_iter):
+        step()
+        if n_iter % 10 == 9:                                                                 # plca.py:290-302
+            loss = loss_now()
+            if bar is not None:
+                bar.set_postfix(loss=loss)
+                bar.update(10)
+            if (previous_loss - loss) / loss_init < tol:
+                break
+            previous_loss = loss
+    check_health()
+    if bar is not None:
+        bar.close()
+    return n_iter
 
 
 def _is_one(a):
