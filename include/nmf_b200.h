@@ -213,6 +213,24 @@ int nmfb200_nmf_update_w_peer(nmfb200_ctx* ctx, float* W, const float* H,
 int nmfb200_nmf_contract_only(nmfb200_ctx* ctx, const float* W, const float* H, int which, double beta,
                               void* stream);
 
+/* Coordinate descent at beta 2 (HALS, sklearn's solver="cd"): one update of W (which = 0) or H (which = 1) in place, that
+ * minimises 1/2 |V - H W^T|^2 + l1_reg (sum W + sum H) + l2_reg / 2 (|W|^2 + |H|^2) over that factor by one sweep over its
+ * columns.  With X the updated factor, A = V^T H (W) or V W (H) and B = the other factor's Gram matrix, both formed once at
+ * the start of the update, for k = 0 .. R-1 in order and every row c:
+ *   X[c,k] <- max(0, X[c,k] + (A[c,k] - sum_j X[c,j] B[j,k] - l1_reg - l2_reg X[c,k]) / (B[k,k] + l2_reg)),
+ * X[c,j] already updated for j < k; a column with B[k,k] + l2_reg == 0 is left as it is.  The floor is exactly 0, and a
+ * later multiplicative update cannot move an entry that is exactly 0.  A is, bit for bit, nmfb200_raw_terms(which, 2.0)'s
+ * numerator: on a dense target the fp32 contraction without S = W H^T (any target dtype and row stride), on a sparse one
+ * (nmfb200_nmf_set_target_sparse / _sparse_any_beta) the gather at the stored entries.  B comes from the fixed-order Gram
+ * kernel of the sparse beta-2 path, and each row's sweep sums in an order fixed by R alone: the result is deterministic.
+ * Dense contexts of any precision run on these fp32 kernels and mark the tensor-core operand copies of X stale.  The Gram
+ * scratch (2 R^2 floats and the Gram kernel's block partials) is allocated at the first call on a dense context.
+ * NMFB200_ERR_INVALID for NMFD / NMF2D / NMF3D, batched and observed-cell contexts, a context with a mask or a weight, and
+ * R > 256; NMFB200_ERR_STATE before set_target.  Asynchronous. */
+int nmfb200_nmf_cd_update(nmfb200_ctx* ctx, float* W, float* H, int which, double l1_reg, double l2_reg, void* stream);
+/* n_iter x (nmfb200_nmf_cd_update of W; of H with the new W) in one host call; same contexts and refusals. */
+int nmfb200_nmf_cd_iterate(nmfb200_ctx* ctx, float* W, float* H, double l1_reg, double l2_reg, int n_iter, void* stream);
+
 /* ---- NMFD (1-D convolutive NMF), NMF2D, NMF3D ------------------------------------------------ */
 
 /* Sizes as NMFD.__init__ (nmf.py:762-774) with ndim = 1: V (B,C,L), W (C,R,T), H (B,R,L-T+1), vdims = {L}, kdims = {T}.

@@ -61,7 +61,7 @@ struct nmfb200_ctx {
   const float *sp_val = nullptr, *sp_val_t = nullptr;
   const float *sp_wt = nullptr, *sp_wt_t = nullptr;     // observed cells: the entries' weights in CSR / CSC order, or none
   double sp_vnorm_kl = 0.0, sp_vnorm_eu = 0.0;
-  float* sp_gram = nullptr;       // [2][R*R] (W^T W, H^T H) + per-block partials
+  float* sp_gram = nullptr;       // [2][R*R] (W^T W, H^T H) + per-block partials; also the Gram scratch of nmfb200_nmf_cd_*
   double* sp_loss_part = nullptr;
   // NMFD
   float* Pn = nullptr;
@@ -138,6 +138,13 @@ int chunks_for(int64_t rows, int64_t cols, int64_t R) {
 
 int ensure_den(nmfb200_ctx* c) {
   if (!c->den) NMF_CUDA_CHECK(cudaMalloc(&c->den, c->part_floats * sizeof(float)));
+  return 0;
+}
+
+// sp_gram: the two R x R Gram matrices and sparse_gram's block partials (R <= 256)
+int ensure_gram(nmfb200_ctx* c) {
+  const int64_t R = c->R;
+  if (!c->sp_gram) NMF_CUDA_CHECK(cudaMalloc(&c->sp_gram, (size_t)(2 * R * R + sparse_gram_part_floats((int)R)) * sizeof(float)));
   return 0;
 }
 
@@ -449,11 +456,9 @@ int nmfb200_nmf_set_target_sparse(nmfb200_ctx* ctx, int64_t nnz, const int64_t* 
     return fail(NMFB200_ERR_INVALID, "bad compressed sparse target");
   if (ctx->R > 256)
     return fail(NMFB200_ERR_INVALID, "rank > 256 is not supported by the sparse-target kernels (densify the target)");
-  if (!ctx->sp_gram) {
-    const int64_t R = ctx->R;
-    NMF_CUDA_CHECK(cudaMalloc(&ctx->sp_gram, (size_t)(2 * R * R + sparse_gram_part_floats((int)R)) * sizeof(float)));
+  if (int rc = ensure_gram(ctx)) return rc;
+  if (!ctx->sp_loss_part)
     NMF_CUDA_CHECK(cudaMalloc(&ctx->sp_loss_part, (size_t)sparse_gather_blocks(ctx->N) * sizeof(double)));
-  }
   ctx->sp_crow = crow; ctx->sp_col = col; ctx->sp_val = val; ctx->sp_ccol = ccol; ctx->sp_row = row; ctx->sp_val_t = val_t;
   ctx->sp_vnorm_kl = v_norm_kl; ctx->sp_vnorm_eu = v_norm_eu;
   ctx->sparse = true; ctx->has_target = true; ctx->V = nullptr; ctx->tc_off = true;      // the dense kernels are out of play
@@ -1117,6 +1122,69 @@ int nmfb200_plca_masked_terms(nmfb200_ctx* ctx, const float* W, const float* Hz,
   ApplyArgs a = factor_view(ctx, which, ctx->nslab[which]);
   a.num = ctx->num; a.den = ctx->den;
   return raw_sum(a, out, out + a.numel, st);
+}
+
+/* ---- coordinate descent at beta 2 (HALS): one sweep per factor update, dense or sparse NMF targets -------------------- */
+
+namespace {
+// What the cd calls serve: a single NMF context of rank <= 256 with a dense target and no selector, or a sparse one set by
+// set_target_sparse / set_target_sparse_any_beta.
+int cd_check(nmfb200_ctx* ctx) {
+  if (is_nmfd(ctx)) return fail(NMFB200_ERR_INVALID, "cd: NMFD / NMF2D / NMF3D contexts are not served (NMF only)");
+  if (is_batch(ctx)) return fail(NMFB200_ERR_INVALID, "cd: batched contexts are not served");
+  if (ctx->R > 256) return fail(NMFB200_ERR_INVALID, "cd: rank must be at most 256");
+  TARGET_GUARD(ctx);
+  if (ctx->observed) return fail(NMFB200_ERR_INVALID, "cd: observed-cell targets are not served");
+  if (ctx->sel) return fail(NMFB200_ERR_INVALID, "cd: contexts with a mask or a weight are not served");
+  return 0;
+}
+
+// One HALS sweep of W (which = 0) or H (which = 1) in place: A = the beta-2 numerator of that factor's update into c->num
+// (dense: the numerator-only contraction's chunk partials; sparse: the gather at the stored entries, in final form), B = the
+// other factor's Gram matrix, then the sweep.
+int cd_update_factor(nmfb200_ctx* c, int which, float* W, float* H, double l1_reg, double l2_reg, cudaStream_t st) {
+  const int R = (int)c->R;
+  const FactorDims f = factor_dims(c, which);
+  float* X = which == 0 ? W : H;
+  const float* other = which == 0 ? H : W;
+  int nch = 1;
+  int rc;
+  if (c->sparse) {            // the compressed form whose segments are X's rows (sparse_terms' choice)
+    rc = sparse_numerator(which == 0 ? c->sp_ccol : c->sp_crow, which == 0 ? c->sp_row : c->sp_col,
+                          which == 0 ? c->sp_val_t : c->sp_val, X, other, R, f.rows, 2.0, c->num, st);
+  } else {
+    if ((rc = ensure_gram(c))) return rc;
+    nch = c->nslab[which];
+    rc = simt_nmf_contract_num(c->V, c->vdtype, c->ldv, /*trans=*/which == 0, other, f.rows, f.other_rows, R, nch, c->num,
+                               f.rows * R, st);
+  }
+  if (rc) return rc;
+  float* G = c->sp_gram + (1 - which) * R * R;
+  if ((rc = sparse_gram(other, f.other_rows, R, c->sp_gram + 2 * R * R, G, st))) return rc;
+  if ((rc = cd_sweep(X, f.rows, R, c->num, nch, f.rows * R, G, (float)l1_reg, (float)l2_reg, st))) return rc;
+  if (!c->sparse) mark_stale(c, which == 0, which == 1);   // the tensor-core operand copies of X are out of date
+  return 0;
+}
+}  // namespace
+
+int nmfb200_nmf_cd_update(nmfb200_ctx* ctx, float* W, float* H, int which, double l1_reg, double l2_reg, void* stream) {
+  CTX_GUARD(ctx, kAnyKind);
+  if (int rc = cd_check(ctx)) return rc;
+  if (!W || !H || (which != 0 && which != 1)) return fail(NMFB200_ERR_INVALID, "bad argument");
+  return cd_update_factor(ctx, which, W, H, l1_reg, l2_reg, (cudaStream_t)stream);
+}
+
+int nmfb200_nmf_cd_iterate(nmfb200_ctx* ctx, float* W, float* H, double l1_reg, double l2_reg, int n_iter, void* stream) {
+  CTX_GUARD(ctx, kAnyKind);
+  if (int rc = cd_check(ctx)) return rc;
+  if (!W || !H || n_iter < 0) return fail(NMFB200_ERR_INVALID, "bad argument");
+  cudaStream_t st = (cudaStream_t)stream;
+  for (int i = 0; i < n_iter; ++i) {
+    int rc = cd_update_factor(ctx, 0, W, H, l1_reg, l2_reg, st);
+    if (rc == 0) rc = cd_update_factor(ctx, 1, W, H, l1_reg, l2_reg, st);
+    if (rc) return rc;
+  }
+  return 0;
 }
 
 /* ---- batched PLCA: the EM iteration on the raw terms of a batched NMF / NMFD context ---------------------------- */

@@ -1,0 +1,113 @@
+// Coordinate descent at beta 2 (HALS, Cichocki & Phan 2009): the sweep stage that takes the place of the ratio stage.
+//
+// One factor update of  1/2 |V - H W^T|^2 + l1 (sum W + sum H) + l2 / 2 (|W|^2 + |H|^2)  with the other factor fixed: for the
+// updated factor X (rows x R), A = the numerator (V^T H for W, V W for H) and B = the other factor's Gram matrix (R x R),
+//   for k = 0 .. R-1:  X[c,k] <- max(0, X[c,k] + (A[c,k] - sum_j X[c,j] B[j,k] - l1 - l2 X[c,k]) / (B[k,k] + l2))
+// with X[c,j] already updated for j < k.  Every row c is independent; the R column steps of a row are sequential.
+//
+// One warp owns ROWS rows.  Lane l holds components l, l + 32, ... (RPL of them) of each row's X and A in registers.  B is
+// staged through shared memory one panel of 32 columns at a time (every row j of them), so rank 256 needs 33 KB, not 256 KB.
+//
+// Summation orders (fixed by R alone, whatever the grid or the number of rows; the oracle tolerance rests on them):
+//   A[c,k]: 0 + the partial slabs in slab order, each added in fp32 -- raw_sum's order, so A equals nmfb200_raw_terms'
+//           numerator at beta 2 bit for bit (one slab: the sparse numerator as it is);
+//   sum_j X[c,j] B[j,k]: lane l accumulates j = l, l + 32, l + 64, ... in ascending order with fmaf from 0, then the 32 lane
+//           sums are added by an xor butterfly over lane distances 16, 8, 4, 2, 1 (every lane ends with the same bits).
+#include "common.cuh"
+
+namespace nmfb200 {
+
+namespace {
+
+constexpr int kPanel = 32;        // columns of B per shared-memory panel: one per lane
+constexpr int kPanelLd = 33;      // padded pitch: lane l reads row l + 32 m of a column conflict-free
+constexpr int kWarps = 8;
+
+template <int RPL, int ROWS>
+__global__ void __launch_bounds__(256)
+cd_sweep_kernel(float* __restrict__ X, int64_t rows, int R, const float* __restrict__ A, int nchunks,
+                int64_t chunk_stride, const float* __restrict__ B, float l1, float l2) {
+  __shared__ float Bp[kPanel * RPL * kPanelLd];        // Bp[j][kk] = B[j, 32 m + kk] of panel m, zero outside R x R
+  const int lane = threadIdx.x & 31;
+  const int64_t row0 = ((int64_t)blockIdx.x * kWarps + (threadIdx.x >> 5)) * ROWS;
+  float x[ROWS][RPL], a[ROWS][RPL];
+#pragma unroll
+  for (int q = 0; q < ROWS; ++q) {
+    const int64_t row = row0 + q;
+#pragma unroll
+    for (int m = 0; m < RPL; ++m) {
+      const int r = lane + 32 * m;
+      const bool in = row < rows && r < R;
+      float s = 0.f;
+      if (in)
+        for (int ch = 0; ch < nchunks; ++ch) s += A[ch * chunk_stride + row * R + r];
+      a[q][m] = s;
+      x[q][m] = in ? X[row * R + r] : 0.f;
+    }
+  }
+
+#pragma unroll
+  for (int m = 0; m < RPL; ++m) {        // panel m: columns k = 32 m + kk, owned by lane kk's slot m
+    __syncthreads();
+    for (int i = threadIdx.x; i < kPanel * RPL * kPanel; i += 256) {
+      const int j = i / kPanel, kk = i - j * kPanel, k = kPanel * m + kk;
+      Bp[j * kPanelLd + kk] = (j < R && k < R) ? B[(int64_t)j * R + k] : 0.f;
+    }
+    __syncthreads();
+    const int kend = min(kPanel, R - kPanel * m);
+    for (int kk = 0; kk < kend; ++kk) {
+      const float hess = Bp[(kPanel * m + kk) * kPanelLd + kk] + l2;
+      float dot[ROWS];
+#pragma unroll
+      for (int q = 0; q < ROWS; ++q) {
+        float p = 0.f;
+#pragma unroll
+        for (int m2 = 0; m2 < RPL; ++m2) p = fmaf(x[q][m2], Bp[(lane + 32 * m2) * kPanelLd + kk], p);
+        dot[q] = p;
+      }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1)
+#pragma unroll
+        for (int q = 0; q < ROWS; ++q) dot[q] += __shfl_xor_sync(0xffffffffu, dot[q], o);
+      if (hess != 0.f && lane == kk) {   // sklearn's `hess != 0` guard: a dead component keeps its column
+#pragma unroll
+        for (int q = 0; q < ROWS; ++q) {
+          const float v = x[q][m];
+          x[q][m] = fmaxf(0.f, v + (a[q][m] - dot[q] - l1 - l2 * v) / hess);
+        }
+      }
+    }
+  }
+
+#pragma unroll
+  for (int q = 0; q < ROWS; ++q) {
+    const int64_t row = row0 + q;
+#pragma unroll
+    for (int m = 0; m < RPL; ++m) {
+      const int r = lane + 32 * m;
+      if (row < rows && r < R) X[row * R + r] = x[q][m];
+    }
+  }
+}
+
+}  // namespace
+
+int cd_sweep(float* X, int64_t rows, int R, const float* A, int nchunks, int64_t chunk_stride, const float* B, float l1,
+             float l2, cudaStream_t st) {
+  if (R < 1 || R > 256) { set_error("cd_sweep: rank must be in [1, 256]"); return 1; }
+  if (rows < 1) return 0;
+  const int rpl = (R + 31) / 32;
+  constexpr int kRows = 4;
+  const int64_t blocks = ceil_div(rows, (int64_t)kWarps * kRows);
+  if (blocks > kMaxGridX) { set_error("cd_sweep: too many rows for grid x"); return 1; }
+#define NMF_CD(RPLV) cd_sweep_kernel<RPLV, kRows><<<(unsigned)blocks, 256, 0, st>>>(X, rows, R, A, nchunks, chunk_stride, B, l1, l2)
+  if (rpl <= 1) NMF_CD(1);
+  else if (rpl <= 2) NMF_CD(2);
+  else if (rpl <= 4) NMF_CD(4);
+  else NMF_CD(8);
+#undef NMF_CD
+  NMF_LAUNCH_CHECK();
+  return 0;
+}
+
+}  // namespace nmfb200

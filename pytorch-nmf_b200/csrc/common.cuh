@@ -199,12 +199,30 @@ int simt_nmf_contract_den(const float* F, const float* G, int64_t Mr, int64_t Nc
 //   block_partials[*nblocks] of sum over every cell of (S + eps)^beta (fp32 terms, double block sums), on simt_nmf_loss's plan.
 int simt_nmf_pow_sum(const float* F, const float* G, int64_t Mr, int64_t Nc, int R, double beta, double* block_partials,
                      int max_blocks, int* nblocks, cudaStream_t st);
+// The numerator alone of simt_nmf_contract at beta 2 (kNumOnly), one problem, no selector, R <= 256:
+//   num[ch][m][r] = sum_{c in chunk ch} Vm[m,c] G[c,r]     (row pitch R)
+// bit for bit simt_nmf_contract's num partials at beta 2 (same grid, chunks, staging and loop order), without S = F G^T.
+int simt_nmf_contract_num(const void* V, int vdtype, int64_t ldv, int trans, const float* G, int64_t Mr, int64_t Nc, int R,
+                          int nchunks, float* num, int64_t chunk_stride, cudaStream_t st);
 // Output blocks of 256 components of simt_nmf_contract (grid z): 1 up to rank 256, each block recomputes S over all ranks.
 int simt_rank_blocks(int R);
 // The tile plan of simt_nmf_contract (Mr rows, Nc contracted columns, `nchunks` chunks) and of simt_nmf_loss: the register
 // blocks RB of 16 components, the 64-column tiles per chunk (the last chunks may be short or empty) and the loss's chunks.
 struct SimtNmfPlan { int rb; int64_t tiles_per_chunk; int loss_chunks; int64_t loss_tiles_per_chunk; };
 void simt_nmf_plan(int64_t Mr, int64_t Nc, int R, int nchunks, SimtNmfPlan* p);
+
+// Gram matrix out = F^T F (R x R) of a (rows x R) fp32 factor, R <= 256: one partial per block (sparse_gram_part_floats(R)
+// floats of `part`), then a sum over the blocks in fixed order (sparse_nmf.cu; serves the sparse beta-2 path and cd.cu)
+int sparse_gram(const float* F, int64_t rows, int R, float* part, float* out, cudaStream_t st);
+int64_t sparse_gram_part_floats(int R);
+
+// cd.cu ------------------------------------------------------------------------------------
+// One HALS sweep of a (rows x R) factor X in place, R <= 256 (nmfb200_nmf_cd_update): with A = the sum over `nchunks` slabs
+// (chunk_stride apart, row pitch R) of the numerator partials, in raw_sum's order, and B (R x R), for k = 0 .. R-1 in order
+//   X[c,k] <- max(0, X[c,k] + (A[c,k] - sum_j X[c,j] B[j,k] - l1 - l2 X[c,k]) / (B[k,k] + l2))
+// on every row c, columns with B[k,k] + l2 == 0 left as they are.
+int cd_sweep(float* X, int64_t rows, int R, const float* A, int nchunks, int64_t chunk_stride, const float* B, float l1,
+             float l2, cudaStream_t st);
 
 // update.cu --------------------------------------------------------------------------------
 // nmf.py:78-92 on a flattened parameter of `numel` elements whose rank index is
@@ -255,8 +273,6 @@ int hoyer_project(float* x, int64_t outer, int D, int64_t inner, const float* k1
 // of any beta > 0; the denominators of beta 1 (factor_colsum) and 2 (Gram) are below, of other beta simt_nmf_contract_den.
 int sparse_numerator(const int64_t* ptr, const int64_t* idx, const float* val, const float* Fself, const float* Fother,
                      int R, int64_t nseg, double beta, float* out, cudaStream_t st);
-int sparse_gram(const float* F, int64_t rows, int R, float* part, float* out, cudaStream_t st);          // out = F^T F (R x R)
-int64_t sparse_gram_part_floats(int R);
 int sparse_rows_times_gram(const float* F, const float* G, int64_t rows, int R, float* out, cudaStream_t st);
 int sparse_loss(const int64_t* crow, const int64_t* col, const float* val, const float* H, const float* W, int R, int64_t N,
                 double beta, const float* pos_a, const float* pos_b, double v_norm, double* loss_part, double* loss_dev,

@@ -31,6 +31,10 @@
 // observed cells, and pp = s / (s+eps) at the missing ones -- the expected complete data of the EM there -- in place of the
 // mask.  The CTAs of output block 0 also sum s over their observed cells (fp32 per tile and thread, double across tiles,
 // then one fixed-order block reduction) into one partial each, so q_O comes out of the same pass.
+//
+// kNumOnly (the coordinate-descent solver, cd.cu): the contraction forms only num += V_tile G_tile, with kEU's plan, staging
+// and loop order, and skips GEMM-1 and phi -- at beta 2 phi leaves the V tile as it is -- so its num partials equal kEU's bit
+// for bit.  It stages no F (Gs starts the shared memory), and runs one problem without a selector, up to rank 256.
 #include "common.cuh"
 
 namespace nmfb200 {
@@ -39,6 +43,7 @@ namespace {
 
 constexpr int kTile = 64;   // rows per CTA and columns per tile
 constexpr int kVFree = 4;   // MODE of the V-free kernels, beside BetaMode's kKL ... kGeneric
+constexpr int kNumOnly = 6; // MODE of the numerator-only kernels (common.cuh's kPlcaFill is 5)
 constexpr int kLd = 68;     // padded shared-memory pitch (floats): float4-aligned, conflict-free
 
 // 64-column tiles per chunk of the contracted dimension; the last chunks may be short or hold no tile at all
@@ -119,11 +124,13 @@ simt_contract_kernel(const TV* __restrict__ V, int64_t ldv, const float* __restr
                 "kPlcaFill: fp32 V, the uint8 mask, one problem");
   constexpr int Rp = 16 * RB;
   constexpr bool kDenOnly = (MODE == kVFree);
+  constexpr bool kNumOnly_ = (MODE == kNumOnly);
+  static_assert(!kNumOnly_ || (!MASK && !BATCH), "kNumOnly: one problem, no selector");
   constexpr bool kNum = !kDenOnly;
-  constexpr bool kTwo = (MODE != kKL) || MASK;
+  constexpr bool kTwo = !kNumOnly_ && ((MODE != kKL) || MASK);
   extern __shared__ __align__(16) float smem[];
-  float* Fs = smem;                 // [Rp][kLd]  Fs[r][row]
-  float* Gs = Fs + Rp * kLd;        // [Rp][kLd]  Gs[r][col]
+  float* Fs = smem;                 // [Rp][kLd]  Fs[r][row] (kNumOnly: none)
+  float* Gs = Fs + (kNumOnly_ ? 0 : Rp * kLd);     // [Rp][kLd]  Gs[r][col]
   float* Ps = Gs + Rp * kLd;        // [64][kLd]  V tile, then Pn in place
   float* Qs = kDenOnly ? Ps : Ps + kTile * kLd;     // [64][kLd]  Pp (kTwo only; kVFree: in Ps's place); MASK: the selector first
 
@@ -153,7 +160,7 @@ simt_contract_kernel(const TV* __restrict__ V, int64_t ldv, const float* __restr
   const int ob = RB == 16 ? (int)blockIdx.z : 0;
   const bool multi = nb > 1;
 
-  if (!multi) stage_chunk(Fs, F, m0, Mr, R, 0, Rp, tid);
+  if (!multi && !kNumOnly_) stage_chunk(Fs, F, m0, Mr, R, 0, Rp, tid);
 
   float accn[4][RB], accd[4][RB];
 #pragma unroll
@@ -200,6 +207,7 @@ simt_contract_kernel(const TV* __restrict__ V, int64_t ldv, const float* __restr
         }
       }
       __syncthreads();
+      if (kNumOnly_) continue;
       if (multi)
         gemm1(Fs, Gs, min(Rp, (R - k0 + 15) & ~15), tx, ty, s);   // the chunk's components, zero-padded to 16
       else
@@ -208,6 +216,7 @@ simt_contract_kernel(const TV* __restrict__ V, int64_t ldv, const float* __restr
     float qloc = 0.f;
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
+      if (kNumOnly_) continue;         // num = V G: the V tile is GEMM-2's operand as it stands
       if (kDenOnly) {
         float pp[4];
 #pragma unroll
@@ -570,6 +579,39 @@ int simt_nmf_contract_den(const float* F, const float* G, int64_t Mr, int64_t Nc
 #undef NMF_DEN
   NMF_LAUNCH_CHECK();
   return 0;
+}
+
+int simt_nmf_contract_num(const void* V, int vdtype, int64_t ldv, int trans, const float* G, int64_t Mr, int64_t Nc, int R,
+                          int nchunks, float* num, int64_t chunk_stride, cudaStream_t st) {
+  if (R < 1 || R > 256) { set_error("simt_nmf_contract_num: rank must be in [1, 256]"); return 1; }
+  const dim3 grid((unsigned)ceil_div(Mr, kTile), (unsigned)nchunks, 1u);
+  const int Rp = 16 * contract_rb(R);
+  const size_t smem = (size_t)(Rp + kTile) * kLd * sizeof(float);           // Gs and the V tile
+  return with_vtype(V, vdtype, [&](auto Vt) {
+    using TV = vtype_t<decltype(Vt)>;
+#define NMF_NUM(RBV, TR)                                                                                             \
+  {                                                                                                                  \
+    auto kern = simt_contract_kernel<RBV, TR, kNumOnly, TV>;                                                         \
+    NMF_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));              \
+    kern<<<grid, 256, smem, st>>>(Vt, ldv, nullptr, G, Mr, Nc, R, 0.f, 0.f, nchunks, num, nullptr, R, chunk_stride,  \
+                                  nullptr, 0, Batch{}, nullptr);                                                     \
+  }
+#define NMF_NUM_RB(RBV)          \
+  if (trans) NMF_NUM(RBV, true)  \
+  else NMF_NUM(RBV, false)       \
+  break
+    switch (contract_rb(R)) {
+      case 1: NMF_NUM_RB(1);
+      case 2: NMF_NUM_RB(2);
+      case 4: NMF_NUM_RB(4);
+      case 8: NMF_NUM_RB(8);
+      default: NMF_NUM_RB(16);
+    }
+#undef NMF_NUM_RB
+#undef NMF_NUM
+    NMF_LAUNCH_CHECK();
+    return 0;
+  });
 }
 
 int64_t simt_plca_fill_blocks(int64_t Mr, int nchunks) { return ceil_div(Mr, kTile) * nchunks; }

@@ -332,6 +332,17 @@ class CudaNmfEngine(_CudaEngine):
         _capi.check(self._lib.nmfb200_nmf_iterate(self._ctx, _ptr(self.W), _ptr(self.H), beta, gamma, l1_reg, l2_reg,
                                                   int(n_iter), _stream(self.device)))
 
+    def cd_update(self, which, l1_reg, l2_reg):
+        """One coordinate-descent (HALS) update at beta 2 of W (which=0) or H (which=1) in place: one sweep over its columns
+        (include/nmf_b200.h: nmfb200_nmf_cd_update)."""
+        _capi.check(self._lib.nmfb200_nmf_cd_update(self._ctx, _ptr(self.W), _ptr(self.H), int(which), float(l1_reg),
+                                                    float(l2_reg), _stream(self.device)))
+
+    def cd_iterate(self, n_iter, l1_reg, l2_reg):
+        """n_iter x (cd_update(0); cd_update(1)) in one call."""
+        _capi.check(self._lib.nmfb200_nmf_cd_iterate(self._ctx, _ptr(self.W), _ptr(self.H), float(l1_reg), float(l2_reg),
+                                                     int(n_iter), _stream(self.device)))
+
     def loss_prefetch_w(self, beta):
         """The loss at the current factors, taken out of the NEXT W update's contraction pass where the library can fold it
         (beta 1 on the tensor-core path): that update then skips its contraction.  Same value as loss() (synchronises)."""
@@ -578,6 +589,8 @@ class CudaSparseNmfEngine(_CudaEngine):
         return (min(self._vmin, 0.0) if self._has_zeros else self._vmin), self._vmax
 
     iterate = CudaNmfEngine.iterate
+    cd_update = CudaNmfEngine.cd_update
+    cd_iterate = CudaNmfEngine.cd_iterate
 
 
 class CudaSparseAnyBetaEngine(CudaSparseNmfEngine):

@@ -231,6 +231,7 @@ class BaseComponent(torch.nn.Module):
     _sparse_targets = False       # NMF only (nmf.py:603-638); the convolutive models raise, as in the reference
     _sparse_kernels = True        # a sparse target on the library's sparse kernels (False: densify)
     _strided_target = False       # the engine reads a row-strided (unit column stride) half-precision target as it is
+    _cd_solver = False            # fit(..., solver="cd") at beta 2: NMF only
 
     def _open_engine(self, V, beta, precision, group, sparse_kernels, mask=None, weight=None):
         """Shared entry of `fit` / `sparse_fit`: validation that needs no device pass, placement of V / W / H on the CUDA
@@ -395,6 +396,22 @@ class BaseComponent(torch.nn.Module):
             raise ValueError(f"weight: weighted fits run on the fp32 kernels; precision must be 'auto' or 'f32' "
                              f"(got {precision!r})")
 
+    def _check_cd(self, beta, precision, group, mask, weight):
+        """fit(solver="cd")'s refusals, before any device work."""
+        if not self._cd_solver:
+            raise ValueError(f"solver='cd' is supported by NMF only (got {type(self).__name__})")
+        if beta != 2:
+            raise ValueError(f"solver='cd' minimises the beta = 2 objective; beta must be 2 (got {beta!r})")
+        if mask is not None or weight is not None:
+            raise ValueError("solver='cd' takes no mask or weight")
+        if group is not None:
+            raise ValueError("solver='cd' does not run sharded fits (group)")
+        if precision in ("f16", "f16_split"):
+            raise ValueError(f"solver='cd' runs on the fp32 kernels; precision must be 'auto' or 'f32' (got {precision!r})")
+        rank = self.W.shape[1] if self.W is not None else self.rank
+        if rank > 256:
+            raise ValueError(f"solver='cd' supports rank <= 256 (got {rank})")
+
     @torch.no_grad()
     def fit(self, V, beta=1, tol=1e-4, max_iter=200, verbose=False, alpha=0, l1_ratio=0, *,
             precision="auto", group=None, **options):
@@ -463,11 +480,34 @@ class BaseComponent(torch.nn.Module):
                    device.  A dense weight on a sparse V and a sparse weight on NMFD / NMF2D / NMF3D raise ValueError.
                    With `group`, each rank passes the weight shard of its V shard; a shard may be zero everywhere (or,
                    sparse, store nothing), and the value check is agreed on by all ranks, so every rank raises together.
+
+        solver:    (keyword-only, default "mu", through **options like `mask`) "mu" -- the multiplicative updates above -- or
+                   "cd": coordinate descent (HALS, sklearn's `solver="cd"`) at beta 2, which usually reaches a given loss
+                   in far fewer iterations.  It minimises 1/2 |V - H W^T|^2 + l1 (sum W + sum H) + l2 / 2 (|W|^2 + |H|^2),
+                   l1 = alpha * l1_ratio and l2 = alpha * (1 - l1_ratio) as for "mu".  Each iteration updates W, then H
+                   with the new W; each update is one sweep over the factor's columns k = 0 .. R-1 in order, every row c
+                   at once:  X[c,k] <- max(0, X[c,k] + (A[c,k] - sum_j X[c,j] B[j,k] - l1 - l2 X[c,k]) / (B[k,k] + l2)),
+                   with A = V^T H, B = H^T H for W and A = V W, B = W^T W for H, taken at the start of the update; a
+                   column with B[k,k] + l2 == 0 (a dead component) is left as it is.  The floor is exactly 0, so the
+                   objective never rises in exact arithmetic -- and a later "mu" fit cannot move an entry that is exactly
+                   0.  Loss, stop rule and return value are those of "mu".  NMF only, on the fp32 kernels: precision
+                   "auto" resolves to "f32" and `last_fit_precision` is "f32".  V dense (float32, float16 or bfloat16 read
+                   in place at any row stride; float64 staged) or sparse COO; `alpha`, `l1_ratio`, frozen factors and
+                   host or float64 modules work as for "mu".  ValueError, before any device work: beta != 2, `mask` or
+                   `weight`, `group`, precision "f16" / "f16_split", rank > 256, an unknown solver, and NMFD / NMF2D /
+                   NMF3D.
         """
         mask = options.pop("mask", None)
         weight = options.pop("weight", None)
+        solver = options.pop("solver", "mu")
         if options:
             raise TypeError(f"fit() got an unexpected keyword argument {next(iter(options))!r}")
+        if solver not in ("mu", "cd"):
+            raise ValueError(f"solver must be 'mu' or 'cd' (got {solver!r})")
+        cd = solver == "cd"
+        if cd:
+            self._check_cd(beta, precision, group, mask, weight)
+            precision = "f32"
         if mask is not None and weight is not None:
             raise ValueError("mask and weight are exclusive: fold the mask into the weight (weight * mask)")
         if mask is not None:
@@ -505,12 +545,15 @@ class BaseComponent(torch.nn.Module):
             train_w, train_h = W.requires_grad, H.requires_grad
             bar = _tqdm(total=max_iter, disable=not verbose) if _tqdm is not None else _NullBar()
             n_iter = -1
-            batched = train_w and train_h and group is None and hasattr(eng, "iterate")
+            batched = train_w and train_h and group is None and hasattr(eng, "cd_iterate" if cd else "iterate")
             with bar as pbar:
                 while batched and n_iter + 1 < max_iter:
                     # both factors trainable: run the iterations up to the next loss evaluation in one engine call
                     k = min(10 - ((n_iter + 1) % 10), max_iter - (n_iter + 1))
-                    eng.iterate(k, beta, gamma, l1_reg, l2_reg)                            # nmf.py:366-391, k times
+                    if cd:
+                        eng.cd_iterate(k, l1_reg, l2_reg)
+                    else:
+                        eng.iterate(k, beta, gamma, l1_reg, l2_reg)                        # nmf.py:366-391, k times
                     n_iter += k
                     if n_iter % 10 == 9:                                                   # nmf.py:393
                         loss = fit_loss(more=n_iter + 1 < max_iter)
@@ -521,9 +564,15 @@ class BaseComponent(torch.nn.Module):
                         previous_loss = loss
                 for n_iter in (range(max_iter) if not batched else ()):                    # nmf.py:366
                     if train_w:
-                        eng.update_w(beta, gamma, l1_reg, l2_reg)                          # nmf.py:367-378
+                        if cd:
+                            eng.cd_update(0, l1_reg, l2_reg)
+                        else:
+                            eng.update_w(beta, gamma, l1_reg, l2_reg)                      # nmf.py:367-378
                     if train_h:
-                        eng.update_h(beta, gamma, l1_reg, l2_reg)                          # nmf.py:380-391
+                        if cd:
+                            eng.cd_update(1, l1_reg, l2_reg)
+                        else:
+                            eng.update_h(beta, gamma, l1_reg, l2_reg)                      # nmf.py:380-391
                     if n_iter % 10 == 9:                                                   # nmf.py:393
                         loss = fit_loss(more=train_w and group is None and n_iter + 1 < max_iter)
                         pbar.set_postfix(loss=loss)
@@ -639,6 +688,7 @@ class NMF(BaseComponent):
     _engine_cls = _engine.CudaNmfEngine
     _sparse_targets = True
     _strided_target = True
+    _cd_solver = True
 
     def __init__(self, Vshape=None, rank=None, **kwargs):
         if isinstance(Vshape, _Iterable):
