@@ -130,8 +130,8 @@ int nmfb200_nmf_loss_prefetch_w(nmfb200_ctx* ctx, const float* W, const float* H
  * B N_f R denominators] (N_f: the rows of the updated factor), and nmfb200_raw_terms_numel reports that length;
  * nmfb200_target_minmax covers every problem; nmfb200_precision_for_beta reports NMFB200_PREC_F32.  nmfb200_set_mask,
  * nmfb200_set_weight, nmfb200_w_apply, nmfb200_nmf_set_target and its sparse / observed forms, nmfb200_nmf_loss_prefetch_w,
- * nmfb200_nmf_contract_only and the peer calls return NMFB200_ERR_INVALID.  The three calls below take batched contexts
- * only (NMFB200_ERR_INVALID otherwise). */
+ * nmfb200_nmf_contract_only, nmfb200_nmf_cd_update / _iterate and the peer calls return NMFB200_ERR_INVALID.  The three
+ * calls below and nmfb200_nmf_batched_cd_update / _iterate take batched contexts only (NMFB200_ERR_INVALID otherwise). */
 int nmfb200_nmf_batched_create(nmfb200_ctx** out, int device, int64_t B, int64_t N, int64_t C, int64_t R);
 /* Register the targets: problem b reads V + b batch_stride, rows ldv >= C elements apart, elements of type `dtype`.
  * batch_stride 0: one V shared by every problem (restarts of one fit); otherwise batch_stride >= N ldv.  Alignment and dtype
@@ -230,6 +230,21 @@ int nmfb200_nmf_contract_only(nmfb200_ctx* ctx, const float* W, const float* H, 
 int nmfb200_nmf_cd_update(nmfb200_ctx* ctx, float* W, float* H, int which, double l1_reg, double l2_reg, void* stream);
 /* n_iter x (nmfb200_nmf_cd_update of W; of H with the new W) in one host call; same contexts and refusals. */
 int nmfb200_nmf_cd_iterate(nmfb200_ctx* ctx, float* W, float* H, double l1_reg, double l2_reg, int n_iter, void* stream);
+/* The same update on a nmfb200_nmf_batched_create context, for every active problem (nmfb200_nmf_batched_set_active) in
+ * the launches one problem takes (four per factor update, whatever B): problem b's W_b / H_b (W + b C R, H + b N R) are,
+ * bit for bit, what nmfb200_nmf_cd_update gives on a single NMFB200_PREC_F32 context of (N, C, R) with target V_b -- each
+ * problem keeps that context's contraction chunks, Gram plan and summation orders.  An inactive problem's factors are not
+ * written.  Workspace: the A partials use the context's partial slabs; the Gram scratch, allocated at the first call, is
+ * B (2 R^2 + max(nb(N), nb(C)) R^2) floats, nb(rows) the Gram blocks of nmfb200_nmf_sparse_plan (at most 128).
+ * NMFB200_ERR_INVALID for any other context kind (a single dense or sparse NMF, an observed-cell, NMFD or batched NMFD
+ * context), a null context or pointer, which not 0 / 1, and for B x ceil(max(N, C) / 32) sweep blocks (or B x the Gram
+ * blocks) past grid x (2^31 - 1); NMFB200_ERR_STATE before nmfb200_nmf_batched_set_target.  Asynchronous. */
+int nmfb200_nmf_batched_cd_update(nmfb200_ctx* ctx, float* W, float* H, int which, double l1_reg, double l2_reg,
+                                  void* stream);
+/* n_iter x (nmfb200_nmf_batched_cd_update of W; of H with the new W) in one host call; n_iter < 0 and the refusals above
+ * return NMFB200_ERR_INVALID. */
+int nmfb200_nmf_batched_cd_iterate(nmfb200_ctx* ctx, float* W, float* H, double l1_reg, double l2_reg, int n_iter,
+                                   void* stream);
 
 /* ---- NMFD (1-D convolutive NMF), NMF2D, NMF3D ------------------------------------------------ */
 

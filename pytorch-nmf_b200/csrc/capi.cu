@@ -141,10 +141,20 @@ int ensure_den(nmfb200_ctx* c) {
   return 0;
 }
 
-// sp_gram: the two R x R Gram matrices and sparse_gram's block partials (R <= 256)
+// sp_gram: the two R x R Gram matrices and sparse_gram's block partials (R <= 256).  A batch of P problems: [2][P][R^2], then
+// each problem's partials on its own Gram plan, P x max(nb(N), nb(C)) R^2 (sparse_gram_plan), not P x the fixed 128 R^2.
 int ensure_gram(nmfb200_ctx* c) {
+  if (c->sp_gram) return 0;
   const int64_t R = c->R;
-  if (!c->sp_gram) NMF_CUDA_CHECK(cudaMalloc(&c->sp_gram, (size_t)(2 * R * R + sparse_gram_part_floats((int)R)) * sizeof(float)));
+  int64_t floats = 2 * R * R + sparse_gram_part_floats((int)R);
+  if (is_batch(c)) {
+    int64_t rpb;
+    int nb_n, nb_c;
+    sparse_gram_plan(c->N, &rpb, &nb_n);
+    sparse_gram_plan(c->C, &rpb, &nb_c);
+    floats = c->nprob * (2 + (int64_t)(nb_n > nb_c ? nb_n : nb_c)) * R * R;
+  }
+  NMF_CUDA_CHECK(cudaMalloc(&c->sp_gram, (size_t)floats * sizeof(float)));
   return 0;
 }
 
@@ -1139,14 +1149,35 @@ int cd_check(nmfb200_ctx* ctx) {
   return 0;
 }
 
+// What the batched cd calls serve: a nmfb200_nmf_batched_create context (CTX_GUARD) whose every launch fits grid x.  The
+// problems ride on grid x, and the sweep and Gram kernels take more blocks per problem than nmfb200_nmf_batched_create checks.
+int cd_batched_check(nmfb200_ctx* ctx) {
+  int64_t rpb;
+  int nb_n, nb_c;
+  sparse_gram_plan(ctx->N, &rpb, &nb_n);
+  sparse_gram_plan(ctx->C, &rpb, &nb_c);
+  const int64_t per_problem[] = {cd_sweep_blocks(ctx->N > ctx->C ? ctx->N : ctx->C), nb_n > nb_c ? nb_n : nb_c,
+                                 ceil_div(ctx->R * ctx->R, 256)};
+  for (int64_t blocks : per_problem)
+    if (blocks > kMaxGridX / ctx->nprob)
+      return fail(NMFB200_ERR_INVALID, "batched cd: B x ceil(max(N, C) / 32) sweep blocks (and B x the Gram blocks) must "
+                                       "fit grid x (2^31 - 1)");
+  TARGET_GUARD(ctx);
+  return 0;
+}
+
 // One HALS sweep of W (which = 0) or H (which = 1) in place: A = the beta-2 numerator of that factor's update into c->num
 // (dense: the numerator-only contraction's chunk partials; sparse: the gather at the stored entries, in final form), B = the
-// other factor's Gram matrix, then the sweep.
+// other factor's Gram matrix, then the sweep.  A batch runs every active problem in the same four launches, each on its single
+// context's plan: A's slabs [chunk][problem][rows][R] (simt_contract's layout), the Grams [2][problem][R^2].
 int cd_update_factor(nmfb200_ctx* c, int which, float* W, float* H, double l1_reg, double l2_reg, cudaStream_t st) {
   const int R = (int)c->R;
+  const int64_t P = c->nprob;
   const FactorDims f = factor_dims(c, which);
   float* X = which == 0 ? W : H;
   const float* other = which == 0 ? H : W;
+  Batch bt;               // X / A partials (f, p), the other factor (g) and its Gram (p of the Gram) of problem b
+  if (c->kind == kBatched) bt = Batch{P, c->bstride, f.rows * R, f.other_rows * R, f.rows * R, c->active};
   int nch = 1;
   int rc;
   if (c->sparse) {            // the compressed form whose segments are X's rows (sparse_terms' choice)
@@ -1156,13 +1187,26 @@ int cd_update_factor(nmfb200_ctx* c, int which, float* W, float* H, double l1_re
     if ((rc = ensure_gram(c))) return rc;
     nch = c->nslab[which];
     rc = simt_nmf_contract_num(c->V, c->vdtype, c->ldv, /*trans=*/which == 0, other, f.rows, f.other_rows, R, nch, c->num,
-                               f.rows * R, st);
+                               f.rows * R * P, st, bt);
   }
   if (rc) return rc;
-  float* G = c->sp_gram + (1 - which) * R * R;
-  if ((rc = sparse_gram(other, f.other_rows, R, c->sp_gram + 2 * R * R, G, st))) return rc;
-  if ((rc = cd_sweep(X, f.rows, R, c->num, nch, f.rows * R, G, (float)l1_reg, (float)l2_reg, st))) return rc;
+  float* G = c->sp_gram + (1 - which) * P * R * R;
+  Batch gbt = bt;
+  gbt.f = bt.g; gbt.p = (int64_t)R * R;
+  if ((rc = sparse_gram(other, f.other_rows, R, c->sp_gram + 2 * P * R * R, G, st, gbt))) return rc;
+  Batch sbt = bt;
+  sbt.g = (int64_t)R * R;
+  if ((rc = cd_sweep(X, f.rows, R, c->num, nch, f.rows * R * P, G, (float)l1_reg, (float)l2_reg, st, sbt))) return rc;
   if (!c->sparse) mark_stale(c, which == 0, which == 1);   // the tensor-core operand copies of X are out of date
+  return 0;
+}
+
+int cd_iterate(nmfb200_ctx* c, float* W, float* H, double l1_reg, double l2_reg, int n_iter, cudaStream_t st) {
+  for (int i = 0; i < n_iter; ++i) {
+    int rc = cd_update_factor(c, 0, W, H, l1_reg, l2_reg, st);
+    if (rc == 0) rc = cd_update_factor(c, 1, W, H, l1_reg, l2_reg, st);
+    if (rc) return rc;
+  }
   return 0;
 }
 }  // namespace
@@ -1178,13 +1222,23 @@ int nmfb200_nmf_cd_iterate(nmfb200_ctx* ctx, float* W, float* H, double l1_reg, 
   CTX_GUARD(ctx, kAnyKind);
   if (int rc = cd_check(ctx)) return rc;
   if (!W || !H || n_iter < 0) return fail(NMFB200_ERR_INVALID, "bad argument");
-  cudaStream_t st = (cudaStream_t)stream;
-  for (int i = 0; i < n_iter; ++i) {
-    int rc = cd_update_factor(ctx, 0, W, H, l1_reg, l2_reg, st);
-    if (rc == 0) rc = cd_update_factor(ctx, 1, W, H, l1_reg, l2_reg, st);
-    if (rc) return rc;
-  }
-  return 0;
+  return cd_iterate(ctx, W, H, l1_reg, l2_reg, n_iter, (cudaStream_t)stream);
+}
+
+int nmfb200_nmf_batched_cd_update(nmfb200_ctx* ctx, float* W, float* H, int which, double l1_reg, double l2_reg,
+                                  void* stream) {
+  CTX_GUARD(ctx, kBatched);
+  if (int rc = cd_batched_check(ctx)) return rc;
+  if (!W || !H || (which != 0 && which != 1)) return fail(NMFB200_ERR_INVALID, "bad argument");
+  return cd_update_factor(ctx, which, W, H, l1_reg, l2_reg, (cudaStream_t)stream);
+}
+
+int nmfb200_nmf_batched_cd_iterate(nmfb200_ctx* ctx, float* W, float* H, double l1_reg, double l2_reg, int n_iter,
+                                   void* stream) {
+  CTX_GUARD(ctx, kBatched);
+  if (int rc = cd_batched_check(ctx)) return rc;
+  if (!W || !H || n_iter < 0) return fail(NMFB200_ERR_INVALID, "bad argument");
+  return cd_iterate(ctx, W, H, l1_reg, l2_reg, n_iter, (cudaStream_t)stream);
 }
 
 /* ---- batched PLCA: the EM iteration on the raw terms of a batched NMF / NMFD context ---------------------------- */

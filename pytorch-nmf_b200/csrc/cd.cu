@@ -22,14 +22,26 @@ namespace {
 constexpr int kPanel = 32;        // columns of B per shared-memory panel: one per lane
 constexpr int kPanelLd = 33;      // padded pitch: lane l reads row l + 32 m of a column conflict-free
 constexpr int kWarps = 8;
+constexpr int kSweepRows = 4;     // rows per warp
 
-template <int RPL, int ROWS>
+// BATCH: bt.n problems, problem b on the single problem's blocks [b nbx, (b + 1) nbx) of grid x, with its X at X + b bt.f,
+// its A partials at A + b bt.p within each slab and its B at B + b bt.g; a problem whose bt.active flag is 0 exits at once.
+// The single-problem instantiations compile none of it.
+template <int RPL, int ROWS, bool BATCH>
 __global__ void __launch_bounds__(256)
 cd_sweep_kernel(float* __restrict__ X, int64_t rows, int R, const float* __restrict__ A, int nchunks,
-                int64_t chunk_stride, const float* __restrict__ B, float l1, float l2) {
+                int64_t chunk_stride, const float* __restrict__ B, float l1, float l2, Batch bt) {
   __shared__ float Bp[kPanel * RPL * kPanelLd];        // Bp[j][kk] = B[j, 32 m + kk] of panel m, zero outside R x R
   const int lane = threadIdx.x & 31;
-  const int64_t row0 = ((int64_t)blockIdx.x * kWarps + (threadIdx.x >> 5)) * ROWS;
+  int64_t bx = blockIdx.x;
+  if constexpr (BATCH) {
+    const int64_t nbx = (rows + kWarps * ROWS - 1) / (kWarps * ROWS);
+    const int64_t prob = bx / nbx;
+    if (batch_skips(bt.active, prob)) return;
+    bx -= prob * nbx;
+    X += prob * bt.f; A += prob * bt.p; B += prob * bt.g;
+  }
+  const int64_t row0 = (bx * kWarps + (threadIdx.x >> 5)) * ROWS;
   float x[ROWS][RPL], a[ROWS][RPL];
 #pragma unroll
   for (int q = 0; q < ROWS; ++q) {
@@ -92,20 +104,30 @@ cd_sweep_kernel(float* __restrict__ X, int64_t rows, int R, const float* __restr
 
 }  // namespace
 
+int64_t cd_sweep_blocks(int64_t rows) { return ceil_div(rows, (int64_t)kWarps * kSweepRows); }
+
 int cd_sweep(float* X, int64_t rows, int R, const float* A, int nchunks, int64_t chunk_stride, const float* B, float l1,
-             float l2, cudaStream_t st) {
+             float l2, cudaStream_t st, const Batch& bt) {
   if (R < 1 || R > 256) { set_error("cd_sweep: rank must be in [1, 256]"); return 1; }
   if (rows < 1) return 0;
   const int rpl = (R + 31) / 32;
-  constexpr int kRows = 4;
-  const int64_t blocks = ceil_div(rows, (int64_t)kWarps * kRows);
-  if (blocks > kMaxGridX) { set_error("cd_sweep: too many rows for grid x"); return 1; }
-#define NMF_CD(RPLV) cd_sweep_kernel<RPLV, kRows><<<(unsigned)blocks, 256, 0, st>>>(X, rows, R, A, nchunks, chunk_stride, B, l1, l2)
+  const int64_t blocks = cd_sweep_blocks(rows);
+  if (bt.n < 1 || blocks > kMaxGridX / bt.n) { set_error("cd_sweep: batch x row blocks pass grid x"); return 1; }
+  const unsigned gx = (unsigned)(blocks * bt.n);
+  const bool batched = bt.n > 1 || bt.active;
+#define NMF_CD_B(RPLV, BATCH) \
+  cd_sweep_kernel<RPLV, kSweepRows, BATCH><<<gx, 256, 0, st>>>(X, rows, R, A, nchunks, chunk_stride, B, l1, l2, bt)
+#define NMF_CD(RPLV)                 \
+  do {                               \
+    if (batched) NMF_CD_B(RPLV, true); \
+    else NMF_CD_B(RPLV, false);      \
+  } while (0)
   if (rpl <= 1) NMF_CD(1);
   else if (rpl <= 2) NMF_CD(2);
   else if (rpl <= 4) NMF_CD(4);
   else NMF_CD(8);
 #undef NMF_CD
+#undef NMF_CD_B
   NMF_LAUNCH_CHECK();
   return 0;
 }

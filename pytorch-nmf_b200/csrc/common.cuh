@@ -199,11 +199,12 @@ int simt_nmf_contract_den(const float* F, const float* G, int64_t Mr, int64_t Nc
 //   block_partials[*nblocks] of sum over every cell of (S + eps)^beta (fp32 terms, double block sums), on simt_nmf_loss's plan.
 int simt_nmf_pow_sum(const float* F, const float* G, int64_t Mr, int64_t Nc, int R, double beta, double* block_partials,
                      int max_blocks, int* nblocks, cudaStream_t st);
-// The numerator alone of simt_nmf_contract at beta 2 (kNumOnly), one problem, no selector, R <= 256:
+// The numerator alone of simt_nmf_contract at beta 2 (kNumOnly), no selector, R <= 256:
 //   num[ch][m][r] = sum_{c in chunk ch} Vm[m,c] G[c,r]     (row pitch R)
 // bit for bit simt_nmf_contract's num partials at beta 2 (same grid, chunks, staging and loop order), without S = F G^T.
+// bt: as simt_nmf_contract's (bt.f unused), problem b reading V + b bt.v, G + b bt.g and writing num + b bt.p.
 int simt_nmf_contract_num(const void* V, int vdtype, int64_t ldv, int trans, const float* G, int64_t Mr, int64_t Nc, int R,
-                          int nchunks, float* num, int64_t chunk_stride, cudaStream_t st);
+                          int nchunks, float* num, int64_t chunk_stride, cudaStream_t st, const Batch& bt = Batch{});
 // Output blocks of 256 components of simt_nmf_contract (grid z): 1 up to rank 256, each block recomputes S over all ranks.
 int simt_rank_blocks(int R);
 // The tile plan of simt_nmf_contract (Mr rows, Nc contracted columns, `nchunks` chunks) and of simt_nmf_loss: the register
@@ -212,17 +213,23 @@ struct SimtNmfPlan { int rb; int64_t tiles_per_chunk; int loss_chunks; int64_t l
 void simt_nmf_plan(int64_t Mr, int64_t Nc, int R, int nchunks, SimtNmfPlan* p);
 
 // Gram matrix out = F^T F (R x R) of a (rows x R) fp32 factor, R <= 256: one partial per block (sparse_gram_part_floats(R)
-// floats of `part`), then a sum over the blocks in fixed order (sparse_nmf.cu; serves the sparse beta-2 path and cd.cu)
-int sparse_gram(const float* F, int64_t rows, int R, float* part, float* out, cudaStream_t st);
+// floats of `part`), then a sum over the blocks in fixed order (sparse_nmf.cu; serves the sparse beta-2 path and cd.cu).
+// bt: bt.n problems in the same two launches, problem b's F at F + b bt.f and its Gram at out + b bt.p, each on the single
+// problem's sparse_gram_plan(rows) blocks and summation order; its nb R^2 partials are the b-th run of `part`.
+int sparse_gram(const float* F, int64_t rows, int R, float* part, float* out, cudaStream_t st, const Batch& bt = Batch{});
 int64_t sparse_gram_part_floats(int R);
 
 // cd.cu ------------------------------------------------------------------------------------
 // One HALS sweep of a (rows x R) factor X in place, R <= 256 (nmfb200_nmf_cd_update): with A = the sum over `nchunks` slabs
 // (chunk_stride apart, row pitch R) of the numerator partials, in raw_sum's order, and B (R x R), for k = 0 .. R-1 in order
 //   X[c,k] <- max(0, X[c,k] + (A[c,k] - sum_j X[c,j] B[j,k] - l1 - l2 X[c,k]) / (B[k,k] + l2))
-// on every row c, columns with B[k,k] + l2 == 0 left as they are.
+// on every row c, columns with B[k,k] + l2 == 0 left as they are.  bt: bt.n problems in one launch, problem b's X at
+// X + b bt.f, its A partials at A + b bt.p within each slab and its B at B + b bt.g, each summed in the single problem's
+// order; problems whose bt.active flag is 0 are left untouched.
 int cd_sweep(float* X, int64_t rows, int R, const float* A, int nchunks, int64_t chunk_stride, const float* B, float l1,
-             float l2, cudaStream_t st);
+             float l2, cudaStream_t st, const Batch& bt = Batch{});
+// blocks of one problem's sweep over `rows` rows (grid x: this times the problems of a batch)
+int64_t cd_sweep_blocks(int64_t rows);
 
 // update.cu --------------------------------------------------------------------------------
 // nmf.py:78-92 on a flattened parameter of `numel` elements whose rank index is

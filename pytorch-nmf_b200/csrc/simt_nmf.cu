@@ -34,7 +34,8 @@
 //
 // kNumOnly (the coordinate-descent solver, cd.cu): the contraction forms only num += V_tile G_tile, with kEU's plan, staging
 // and loop order, and skips GEMM-1 and phi -- at beta 2 phi leaves the V tile as it is -- so its num partials equal kEU's bit
-// for bit.  It stages no F (Gs starts the shared memory), and runs one problem without a selector, up to rank 256.
+// for bit.  It stages no F (Gs starts the shared memory), and runs without a selector, up to rank 256: one problem, or a
+// batch (BATCH) in which every problem runs the single problem's plan.
 #include "common.cuh"
 
 namespace nmfb200 {
@@ -125,7 +126,7 @@ simt_contract_kernel(const TV* __restrict__ V, int64_t ldv, const float* __restr
   constexpr int Rp = 16 * RB;
   constexpr bool kDenOnly = (MODE == kVFree);
   constexpr bool kNumOnly_ = (MODE == kNumOnly);
-  static_assert(!kNumOnly_ || (!MASK && !BATCH), "kNumOnly: one problem, no selector");
+  static_assert(!kNumOnly_ || !MASK, "kNumOnly: no selector");
   constexpr bool kNum = !kDenOnly;
   constexpr bool kTwo = !kNumOnly_ && ((MODE != kKL) || MASK);
   extern __shared__ __align__(16) float smem[];
@@ -582,19 +583,27 @@ int simt_nmf_contract_den(const float* F, const float* G, int64_t Mr, int64_t Nc
 }
 
 int simt_nmf_contract_num(const void* V, int vdtype, int64_t ldv, int trans, const float* G, int64_t Mr, int64_t Nc, int R,
-                          int nchunks, float* num, int64_t chunk_stride, cudaStream_t st) {
+                          int nchunks, float* num, int64_t chunk_stride, cudaStream_t st, const Batch& bt) {
   if (R < 1 || R > 256) { set_error("simt_nmf_contract_num: rank must be in [1, 256]"); return 1; }
-  const dim3 grid((unsigned)ceil_div(Mr, kTile), (unsigned)nchunks, 1u);
+  unsigned gx;
+  if (batch_grid_x(ceil_div(Mr, kTile), bt, "simt_nmf_contract_num", &gx)) return 1;
+  const dim3 grid(gx, (unsigned)nchunks, 1u);
   const int Rp = 16 * contract_rb(R);
   const size_t smem = (size_t)(Rp + kTile) * kLd * sizeof(float);           // Gs and the V tile
+  const bool batched = bt.n > 1 || bt.active;
   return with_vtype(V, vdtype, [&](auto Vt) {
     using TV = vtype_t<decltype(Vt)>;
-#define NMF_NUM(RBV, TR)                                                                                             \
+#define NMF_NUM_B(RBV, TR, BATCH)                                                                                    \
   {                                                                                                                  \
-    auto kern = simt_contract_kernel<RBV, TR, kNumOnly, TV>;                                                         \
+    auto kern = simt_contract_kernel<RBV, TR, kNumOnly, TV, NoSel, BATCH>;                                           \
     NMF_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));              \
     kern<<<grid, 256, smem, st>>>(Vt, ldv, nullptr, G, Mr, Nc, R, 0.f, 0.f, nchunks, num, nullptr, R, chunk_stride,  \
-                                  nullptr, 0, Batch{}, nullptr);                                                     \
+                                  nullptr, 0, bt, nullptr);                                                          \
+  }
+#define NMF_NUM(RBV, TR)                  \
+  {                                       \
+    if (batched) NMF_NUM_B(RBV, TR, true) \
+    else NMF_NUM_B(RBV, TR, false)        \
   }
 #define NMF_NUM_RB(RBV)          \
   if (trans) NMF_NUM(RBV, true)  \
@@ -609,6 +618,7 @@ int simt_nmf_contract_num(const void* V, int vdtype, int64_t ldv, int trans, con
     }
 #undef NMF_NUM_RB
 #undef NMF_NUM
+#undef NMF_NUM_B
     NMF_LAUNCH_CHECK();
     return 0;
   });

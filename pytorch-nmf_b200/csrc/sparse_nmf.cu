@@ -179,11 +179,22 @@ sp_gather_obs_kernel(const int64_t* __restrict__ ptr, const int64_t* __restrict_
   sp_gather<RPL, MODE, BM, WT>(ptr, idx, val, Fs, Fo, R, nseg, num, den, loss_part, pa, 0.f, 0.0, 0.0, wt);
 }
 
-// Gram matrix G = F^T F (R x R) of a (rows x R) factor: per-block slabs, then a fixed-order sum over the blocks
+// Gram matrix G = F^T F (R x R) of a (rows x R) factor: per-block slabs, then a fixed-order sum over the blocks.
+// BATCH: bt.n problems, problem b's F at F + b bt.f, on the single problem's nb blocks [b nb, (b + 1) nb) of grid x; the
+// slabs stay indexed by blockIdx.x, so problem b's are the b-th run of nb.  The single-problem instantiations compile none of it.
+template <bool BATCH>
 __global__ void __launch_bounds__(256)
-sp_gram_part_kernel(const float* __restrict__ F, int64_t rows, int R, int64_t rpb, float* __restrict__ part) {
+sp_gram_part_kernel(const float* __restrict__ F, int64_t rows, int R, int64_t rpb, float* __restrict__ part, Batch bt) {
   extern __shared__ float tile[];                     // [32][R]
-  const int64_t r0 = (int64_t)blockIdx.x * rpb, r1 = min(rows, r0 + rpb);
+  int64_t bx = blockIdx.x;
+  if constexpr (BATCH) {
+    const int64_t nb = gridDim.x / bt.n;
+    const int64_t prob = bx / nb;
+    if (batch_skips(bt.active, prob)) return;
+    bx -= prob * nb;
+    F += prob * bt.f;
+  }
+  const int64_t r0 = bx * rpb, r1 = min(rows, r0 + rpb);
   const int npairs = R * R;
   float acc[16];                                      // R <= 64: 4096 / 256; larger ranks loop below
   for (int base = 0; base < npairs; base += kSpGramPass) {
@@ -213,8 +224,20 @@ sp_gram_part_kernel(const float* __restrict__ F, int64_t rows, int R, int64_t rp
   }
 }
 
-__global__ void sp_gram_sum_kernel(const float* __restrict__ part, int nb, int n, float* __restrict__ out) {
-  const int p = blockIdx.x * 256 + threadIdx.x;
+// BATCH: problem b sums its own run of nb slabs into out + b bt.p, on the single problem's ceil(n / 256) blocks of grid x
+template <bool BATCH>
+__global__ void sp_gram_sum_kernel(const float* __restrict__ part, int nb, int n, float* __restrict__ out, Batch bt) {
+  int p;
+  if constexpr (BATCH) {
+    const int64_t nbx = (n + 255) / 256;
+    const int64_t prob = (int64_t)blockIdx.x / nbx;
+    if (batch_skips(bt.active, prob)) return;
+    p = (int)((int64_t)blockIdx.x - prob * nbx) * 256 + threadIdx.x;
+    part += prob * nb * (int64_t)n;
+    out += prob * bt.p;
+  } else {
+    p = blockIdx.x * 256 + threadIdx.x;
+  }
   if (p >= n) return;
   float s = 0.f;
   for (int b = 0; b < nb; ++b) s += part[(int64_t)b * n + p];
@@ -356,13 +379,25 @@ int sparse_numerator(const int64_t* ptr, const int64_t* idx, const float* val, c
   return launch_gather<kSpBeta>(ptr, idx, val, Fself, Fother, R, nseg, out, nullptr, st, (float)(beta - 2.0));
 }
 
-int sparse_gram(const float* F, int64_t rows, int R, float* part, float* out, cudaStream_t st) {
+int sparse_gram(const float* F, int64_t rows, int R, float* part, float* out, cudaStream_t st, const Batch& bt) {
   int64_t rpb;
   int nb;
   sparse_gram_plan(rows, &rpb, &nb);
-  sp_gram_part_kernel<<<nb, 256, 32 * R * sizeof(float), st>>>(F, rows, R, rpb, part);
-  NMF_LAUNCH_CHECK();
-  sp_gram_sum_kernel<<<(unsigned)ceil_div(R * R, 256), 256, 0, st>>>(part, nb, R * R, out);
+  const int64_t nsum = ceil_div((int64_t)R * R, 256);
+  if (bt.n < 1 || nb > kMaxGridX / bt.n || nsum > kMaxGridX / bt.n) {
+    set_error("sparse_gram: batch x blocks pass grid x");
+    return 1;
+  }
+  const size_t smem = 32 * R * sizeof(float);
+  if (bt.n > 1 || bt.active) {
+    sp_gram_part_kernel<true><<<(unsigned)(nb * bt.n), 256, smem, st>>>(F, rows, R, rpb, part, bt);
+    NMF_LAUNCH_CHECK();
+    sp_gram_sum_kernel<true><<<(unsigned)(nsum * bt.n), 256, 0, st>>>(part, nb, R * R, out, bt);
+  } else {
+    sp_gram_part_kernel<false><<<nb, 256, smem, st>>>(F, rows, R, rpb, part, bt);
+    NMF_LAUNCH_CHECK();
+    sp_gram_sum_kernel<false><<<(unsigned)nsum, 256, 0, st>>>(part, nb, R * R, out, bt);
+  }
   NMF_LAUNCH_CHECK();
   return 0;
 }

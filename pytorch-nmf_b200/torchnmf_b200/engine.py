@@ -497,6 +497,17 @@ class CudaBatchedNmfEngine(_BatchedEngine):
         _capi.check(self._lib.nmfb200_nmf_iterate(self._ctx, _ptr(self.W), _ptr(self.H), beta, gamma, l1_reg, l2_reg,
                                                   int(n_iter), _stream(self.device)))
 
+    def cd_update(self, which, l1_reg, l2_reg):
+        """One coordinate-descent (HALS) update at beta 2 of W (which=0) or H (which=1) of every active problem, in place
+        (include/nmf_b200.h: nmfb200_nmf_batched_cd_update)."""
+        _capi.check(self._lib.nmfb200_nmf_batched_cd_update(self._ctx, _ptr(self.W), _ptr(self.H), int(which),
+                                                            float(l1_reg), float(l2_reg), _stream(self.device)))
+
+    def cd_iterate(self, n_iter, l1_reg, l2_reg):
+        """n_iter x (cd_update(0); cd_update(1)) of every active problem in one call."""
+        _capi.check(self._lib.nmfb200_nmf_batched_cd_iterate(self._ctx, _ptr(self.W), _ptr(self.H), float(l1_reg),
+                                                             float(l2_reg), int(n_iter), _stream(self.device)))
+
 
 class CudaBatchedNmfdEngine(_BatchedEngine):
     """P independent NMFD / NMF2D / NMF3D problems of one shape on one GPU (include/nmf_b200.h:

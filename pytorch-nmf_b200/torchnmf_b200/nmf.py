@@ -853,7 +853,7 @@ class _BatchedComponent(BaseComponent):
         raise NotImplementedError(f"{type(self).__name__} has no sparse_fit: fit each problem with the single model's sparse_fit")
 
     @torch.no_grad()
-    def fit(self, V, beta=1, tol=1e-4, max_iter=200, verbose=False, alpha=0, l1_ratio=0, *, precision="auto"):
+    def fit(self, V, beta=1, tol=1e-4, max_iter=200, verbose=False, alpha=0, l1_ratio=0, *, precision="auto", solver="mu"):
         """Fit every problem by multiplicative updates, as the single model's `fit(V[p], ...)` fits one, all of them in the
         same launches.
 
@@ -876,8 +876,22 @@ class _BatchedComponent(BaseComponent):
         `group` are not parameters of this method (TypeError).  Host or half-precision modules are staged through fp32
         device copies and written back, as by the single model's `fit`.  The workspace is P times one fp32 problem's (see
         the class).
+
+        solver: "mu" (default) -- the multiplicative updates above -- or, BatchedNMF only, "cd": coordinate descent (HALS)
+        at beta 2, each problem fitted as `NMF.fit(V[p], 2, ..., precision="f32", solver="cd")` fits it (see `NMF.fit`),
+        bit for bit, with the same per-problem stop rule.  The iterations between two loss checks run in one call when both
+        factors train; a frozen factor leaves the other's updates one call each.  ValueError, before any device work: an
+        unknown solver, "cd" with beta != 2, and "cd" on the convolutive batched models.
         """
         name = type(self).__name__
+        if solver not in ("mu", "cd"):
+            raise ValueError(f"solver must be 'mu' or 'cd' (got {solver!r})")
+        cd = solver == "cd"
+        if cd:
+            if not self._cd_solver:
+                raise ValueError(f"solver='cd' is supported by BatchedNMF only (got {name})")
+            if beta != 2:
+                raise ValueError(f"solver='cd' minimises the beta = 2 objective; beta must be 2 (got {beta!r})")
         if precision not in ("auto", "f32"):
             if precision in ("f16", "f16_split"):
                 raise ValueError(f"{name} runs on the fp32 kernels: precision must be 'auto' or 'f32' (got {precision!r})")
@@ -913,7 +927,15 @@ class _BatchedComponent(BaseComponent):
                 train_w, train_h = W.requires_grad, H.requires_grad
 
                 def step(k):
-                    if train_w and train_h and hasattr(eng, "iterate"):
+                    if cd and train_w and train_h:
+                        eng.cd_iterate(k, l1_reg, l2_reg)
+                    elif cd:
+                        for _ in range(k):
+                            if train_w:
+                                eng.cd_update(0, l1_reg, l2_reg)
+                            if train_h:
+                                eng.cd_update(1, l1_reg, l2_reg)
+                    elif train_w and train_h and hasattr(eng, "iterate"):
                         eng.iterate(k, beta, gamma, l1_reg, l2_reg)                        # nmf.py:366-391, k times
                     else:
                         for _ in range(k):
@@ -943,8 +965,13 @@ class BatchedNMF(_BatchedComponent):
     Workspace (device memory, kept between fits of the same shape like `NMF.fit`'s): B times that of one fp32 NMF problem
     -- the chunked partial numerators and denominators, 8 R max(nch_w C, nch_h N) bytes with up to 32 chunks per
     contraction (`_capi.nmf_plan(N, C, R)`), plus the column sums and loss partials -- so it grows linearly with B.
+    `fit(..., solver="cd")` fits each problem by coordinate descent (HALS) at beta 2, as `NMF.fit(V[b], 2, ...,
+    precision="f32", solver="cd")`; it adds the Gram scratch, allocated at the first such fit, of 4 B (2 R^2 + max(nb(N),
+    nb(C)) R^2) bytes, nb(rows) = ceil(rows / rpb) <= 128 Gram blocks of rpb = roundup(ceil(rows / 128), 32) rows
+    (include/nmf_b200.h: nmfb200_nmf_sparse_plan).
     """
     _engine_cls = _engine.CudaBatchedNmfEngine
+    _cd_solver = True
 
     def __init__(self, Vshape=None, rank=None, *, W=None, H=None, trainable_W=True, trainable_H=True):
         if isinstance(Vshape, _Iterable):
