@@ -81,6 +81,15 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   if (!mbar_try_wait(bar, parity)) mbar_wait_slow(bar, parity);
 }
 
+// ---- named barriers (bar 0 is __syncthreads) -----------------------------------------------------------
+// Unbounded: every arrive must be matched by a sync of the same barrier before the threads that take part exit.
+__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
+__device__ __forceinline__ void named_bar_arrive(uint32_t id, uint32_t nthreads) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
+
 // ---- TMA ----------------------------------------------------------------------------------------
 __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* m) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(m)) : "memory");

@@ -14,6 +14,14 @@
 // so neither S = WH nor P = V/(WH) ever leaves the SM (nmf.py:376-378 materialises both in HBM).
 // F/G are fp16 copies of the factors scaled by a power of two; in split mode they carry hi|lo halves
 // (KW = 2*Rp) and S = Fhi Ghi + Flo Ghi + Fhi Glo, O = P Ghi + P Glo recovers ~22-bit factors.
+//
+// Schedule.  Within a warpgroup the three phases run one after the other (S, wait, ratio, O, wait): the ratio tile is read
+// from S's accumulators and the O-MMA reads its A operand from registers.  Between the two warpgroups a token passed on
+// two named barriers orders the MMA batches S_1, S_2, O_1, O_2, S_1, ... (FlashAttention-3's ping-pong), so one warpgroup's
+// ratio math (MUFU, ALU) runs while the other's MMAs hold the tensor cores instead of both fighting for the same unit at
+// the same time.  Neither warpgroup's instruction stream or accumulation order depends on the other's timing: the
+// partials are the same bit for bit whatever the interleaving.  Where the shared memory left over after the stages holds a
+// second F block (SmemLayout::NF), the producer loads the next item's F while the consumers still read the current one.
 #include "tc_nmf.cuh"
 
 #include <cooperative_groups.h>
@@ -33,6 +41,7 @@ namespace {
 constexpr int kTileM = 128;          // rows of the row factor per work item (two consumer warpgroups of 64 rows)
 constexpr int kStep = 64;            // columns of a tile per S / ratio / O step
 constexpr int kThreads = 384;        // warpgroup 0: TMA producer | warpgroups 1, 2: MMA + ratio stage
+constexpr uint32_t kBarTok = 2;      // named barriers 2, 3: MMA token of consumer warpgroups 1, 2 (0: __syncthreads, 1: loss)
 
 // Compile-time configuration of the fused kernel.
 //   RP    padded rank (64 or 128);  SPLIT  hi|lo fp16 factors (KW = 2 RP operand columns)
@@ -59,19 +68,23 @@ struct TcKernelParams {
   const float* kappa;         // device scalar: centring constant of the ratio tile (typical P), 0 = off
 };
 
-// shared memory: F block | NS stages of (G tile, V tile) | mbarriers | loss slots.  As many stages as fit in the 227 KB
-// a block may opt into: the V stream is the HBM-bound one and wants as many tiles in flight as possible.
+// shared memory: NF F blocks | NS stages of (G tile, V tile) | mbarriers | loss slots.  As many stages as fit in the 227 KB
+// a block may opt into: the V stream is the HBM-bound one and wants as many tiles in flight as possible.  A second F slot
+// (NF = 2) is taken only where the leftover after the stages holds it: the producer then loads item k+1's F and tiles
+// while the consumers finish item k, instead of letting the ring drain at every item boundary.
 template <int KW, int TN>
 struct SmemLayout {
   static constexpr int kFBytes = kTileM * KW * 2;
   static constexpr int kGBytes = TN * KW * 2;
   static constexpr int kVBytes = kTileM * TN * 2;
   static constexpr int kStageBytes = kGBytes + kVBytes;
-  static constexpr int NS = (232448 - 1024 - 256 - kFBytes) / kStageBytes;
+  static constexpr int stages(int nf) { return (232448 - 1024 - 256 - nf * kFBytes) / kStageBytes; }
+  static constexpr int NS = stages(1);
+  static constexpr int NF = stages(2) == NS ? 2 : 1;
   static constexpr int kF = 0;
-  static constexpr int kStage0 = kFBytes;
+  static constexpr int kStage0 = NF * kFBytes;
   static constexpr int kBar = kStage0 + NS * kStageBytes;
-  static constexpr int kNumBars = 2 + 2 * NS;
+  static constexpr int kNumBars = 2 * NF + 2 * NS;
   static constexpr int kLossSlots = kBar + 8 * kNumBars;
   static constexpr int kTotal = kLossSlots + 8 * 16;
 };
@@ -96,7 +109,7 @@ tc_contract_kernel(const __grid_constant__ CUtensorMap tmF, const __grid_constan
   constexpr bool TWO = BM != kBmKL && BM != kBmEU && !LOSS;     // LOSS kernels only need S, whatever the beta
   constexpr bool EU = BM == kBmEU;
   using L = SmemLayout<KW, TN>;
-  constexpr int NS = L::NS;
+  constexpr int NS = L::NS, NF = L::NF;
   static_assert(NS >= 2, "shared memory: at least two stages");
   static_assert(!TWO || (!SPLIT && RP == 64), "two-output kernels: fast mode, R <= 64");
   static_assert(TN == 64 || TN == 128, "tile width");
@@ -106,10 +119,10 @@ tc_contract_kernel(const __grid_constant__ CUtensorMap tmF, const __grid_constan
   const uint32_t raw32 = ptx::smem_u32(smem_raw);
   const uint32_t sbase = (raw32 + 1023u) & ~1023u;
   uint8_t* smem_al = smem_raw + (sbase - raw32);
-  const uint32_t sF = sbase + L::kF;
+  auto FSLOT = [&](uint32_t f) { return sbase + L::kF + f * (uint32_t)L::kFBytes; };
   auto STAGE = [&](uint32_t s) { return sbase + L::kStage0 + s * (uint32_t)L::kStageBytes; };
   auto BAR = [&](int i) { return sbase + L::kBar + 8u * i; };
-  constexpr int B_FFULL = 0, B_FEMPTY = 1, B_FULL = 2, B_EMPTY = 2 + NS;
+  constexpr int B_FFULL = 0, B_FEMPTY = NF, B_FULL = 2 * NF, B_EMPTY = 2 * NF + NS;     // F barriers: one pair per slot
   double* loss_slots = reinterpret_cast<double*>(smem_al + L::kLossSlots);      // [8 consumer warps][2]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -117,8 +130,10 @@ tc_contract_kernel(const __grid_constant__ CUtensorMap tmF, const __grid_constan
 
   if (threadIdx.x == 0) {
     ptx::prefetch_tmap(&tmF); ptx::prefetch_tmap(&tmG); ptx::prefetch_tmap(&tmV);
-    ptx::mbar_init(BAR(B_FFULL), 1);
-    ptx::mbar_init(BAR(B_FEMPTY), 8);               // one arrival per consumer warp
+    for (int f = 0; f < NF; ++f) {
+      ptx::mbar_init(BAR(B_FFULL + f), 1);
+      ptx::mbar_init(BAR(B_FEMPTY + f), 8);         // one arrival per consumer warp
+    }
     for (int i = 0; i < NS; ++i) { ptx::mbar_init(BAR(B_FULL + i), 1); ptx::mbar_init(BAR(B_EMPTY + i), 8); }
     ptx::fence_barrier_init();
     ptx::fence_proxy_async();
@@ -135,10 +150,11 @@ tc_contract_kernel(const __grid_constant__ CUtensorMap tmF, const __grid_constan
         const int rb = item % p.row_blocks, chunk = item / p.row_blocks;
         const int tb = chunk * p.tiles_per_chunk;
         const int te = min(p.tiles, tb + p.tiles_per_chunk);
-        ptx::mbar_wait(BAR(B_FEMPTY), (it & 1) ^ 1);                 // both consumer warpgroups are done with the last F
-        ptx::mbar_expect_tx(BAR(B_FFULL), L::kFBytes);
+        const uint32_t f = it % NF;
+        ptx::mbar_wait(BAR(B_FEMPTY + f), ((it / NF) & 1) ^ 1);      // both consumer warpgroups are done with this slot's F
+        ptx::mbar_expect_tx(BAR(B_FFULL + f), L::kFBytes);
         for (int kb = 0; kb < KW / 64; ++kb)
-          ptx::tma_load_2d(&tmF, BAR(B_FFULL), sF + kb * (kTileM * 128), kb * 64, rb * kTileM);
+          ptx::tma_load_2d(&tmF, BAR(B_FFULL + f), FSLOT(f) + kb * (kTileM * 128), kb * 64, rb * kTileM);
         for (int j = tb; j < te; ++j, ++t) {
           const uint32_t s = t % NS, ph = (t / NS) & 1;
           ptx::mbar_wait(BAR(B_EMPTY + s), ph ^ 1);
@@ -186,6 +202,12 @@ tc_contract_kernel(const __grid_constant__ CUtensorMap tmF, const __grid_constan
   constexpr int kTerms = SPLIT ? 3 : 1;
   constexpr int termF[3] = {0, 1, 0}, termG[3] = {0, 0, 1};
   double accA = 0.0, accB = 0.0;
+  // Ping-pong between the two consumer warpgroups: a warpgroup issues an MMA batch only while it holds the token (bar.sync on
+  // its own named barrier) and passes it on right after the commit (bar.arrive on the other's), so the tensor pipe sees
+  // S_1, S_2, O_1, O_2, S_1, ... and one warpgroup's ratio math runs under the other's MMAs.  Both warpgroups issue the
+  // same batches in the same number, and warpgroup 1 starts with the token.
+  const uint32_t tok_mine = kBarTok + cw, tok_next = kBarTok + (cw ^ 1);
+  if (cw == 1) ptx::named_bar_arrive(tok_next, 256);
   uint32_t it = 0, t = 0;
   for (int item = blockIdx.x; item < total_items; item += gridDim.x, ++it) {
     const int rb = item % p.row_blocks, chunk = item / p.row_blocks;
@@ -196,7 +218,8 @@ tc_contract_kernel(const __grid_constant__ CUtensorMap tmF, const __grid_constan
     for (int i = 0; i < RP / 2; ++i) o[i] = 0.f;
 #pragma unroll
     for (int i = 0; i < (TWO ? 32 : 1); ++i) o2[i] = 0.f;
-    ptx::mbar_wait(BAR(B_FFULL), it & 1);
+    const uint32_t fs = it % NF, sF = FSLOT(fs);
+    ptx::mbar_wait(BAR(B_FFULL + fs), (it / NF) & 1);
     for (int j = 0; j < n; ++j, ++t) {
       const uint32_t s = t % NS;
       ptx::mbar_wait(BAR(B_FULL + s), (t / NS) & 1);
@@ -205,6 +228,7 @@ tc_contract_kernel(const __grid_constant__ CUtensorMap tmF, const __grid_constan
       for (int st = 0; st < TN / kStep; ++st) {
         // ---- S = F G^T over the 64 columns of this step
         float sacc[32];
+        ptx::named_bar_sync(tok_mine, 256);
         ptx::wgmma_fence();
 #pragma unroll
         for (int term = 0; term < kTerms; ++term) {
@@ -217,6 +241,7 @@ tc_contract_kernel(const __grid_constant__ CUtensorMap tmF, const __grid_constan
           }
         }
         ptx::wgmma_commit();
+        ptx::named_bar_arrive(tok_next, 256);
         ptx::wgmma_wait<0>();
         ptx::fence_regs(sacc);
         // ---- ratio stage on the accumulator fragment; V~ pairs from the swizzled V tile: byte (row, 16-byte chunk k)
@@ -305,6 +330,7 @@ tc_contract_kernel(const __grid_constant__ CUtensorMap tmF, const __grid_constan
         if constexpr (!LOSS) {
           // ---- O += P G over the same 64 columns: B = G step as [K = 16 c-rows][N = RP] MN-major, 8-row groups 1024 B
           //      apart, 64-wide column blocks one sub-block (TN x 128 B) apart; split: hi and lo halves into the same O
+          ptx::named_bar_sync(tok_mine, 256);
           ptx::wgmma_fence();
 #pragma unroll
           for (int kk = 0; kk < kStep / 16; ++kk) {
@@ -323,6 +349,7 @@ tc_contract_kernel(const __grid_constant__ CUtensorMap tmF, const __grid_constan
             }
           }
           ptx::wgmma_commit();
+          ptx::named_bar_arrive(tok_next, 256);
           ptx::wgmma_wait<0>();
           ptx::fence_regs(o);
           ptx::fence_regs(o2);
@@ -333,7 +360,7 @@ tc_contract_kernel(const __grid_constant__ CUtensorMap tmF, const __grid_constan
       if (lane == 0) ptx::mbar_arrive(BAR(B_EMPTY + s));
     }
     __syncwarp();
-    if (lane == 0) ptx::mbar_arrive(BAR(B_FEMPTY));
+    if (lane == 0) ptx::mbar_arrive(BAR(B_FEMPTY + fs));
     if constexpr (!LOSS) {
       // ---- epilogue: the item's partial numerators (and denominators) of its 64 rows
 #pragma unroll
@@ -354,6 +381,7 @@ tc_contract_kernel(const __grid_constant__ CUtensorMap tmF, const __grid_constan
       }
     }
   }
+  if (cw == 0) ptx::named_bar_sync(tok_mine, 256);      // takes back the token warpgroup 2 passed on after its last batch
   if constexpr (LOSS || FOLD) {
     for (int off = 16; off > 0; off >>= 1) {
       accA += __shfl_xor_sync(0xffffffffu, accA, off);
@@ -1576,7 +1604,7 @@ int launch_contract_t(TcState* s, int which, double beta, cudaStream_t st) {
 }
 
 // Kernel configurations <RP, SPLIT, TN>; the stage count follows from the shared-memory budget (SmemLayout::NS).
-using CfgFast64 = Cfg<64, false, 128>;       // F 16 KB | 4 stages x (G 16 + V 32 KB)
+using CfgFast64 = Cfg<64, false, 128>;       // 2 x F 16 KB | 4 stages x (G 16 + V 32 KB)
 using CfgSplit64 = Cfg<64, true, 128>;       // F 32 KB | 3 stages x (G 32 + V 32 KB)
 using CfgFast128 = Cfg<128, false, 128>;     // F 32 KB | 3 stages x (G 32 + V 32 KB)
 using CfgSplit128 = Cfg<128, true, 64>;      // F 64 KB | 3 stages x (G 32 + V 16 KB)
