@@ -133,6 +133,20 @@ int nmfb200_nmf_loss_prefetch_w(nmfb200_ctx* ctx, const float* W, const float* H
  * nmfb200_nmf_contract_only, nmfb200_nmf_cd_update / _iterate and the peer calls return NMFB200_ERR_INVALID.  The three
  * calls below and nmfb200_nmf_batched_cd_update / _iterate take batched contexts only (NMFB200_ERR_INVALID otherwise). */
 int nmfb200_nmf_batched_create(nmfb200_ctx** out, int device, int64_t B, int64_t N, int64_t C, int64_t R);
+/* A batch of B problems of different row counts over one C: problem b has lengths[b] (1 <= lengths[b] <= N; `lengths` is B
+ * host int64, read during the call) rows, stored in the same padded layouts as a nmfb200_nmf_batched_create context's --
+ * V_b's first lengths[b] rows, W_b (C,R) = W + b C R, H_b's first lengths[b] rows of H + b N R.  Every call that serves a
+ * batched NMF context serves it, with these differences:
+ *   - problem b runs, bit for bit, the plan of a single NMFB200_PREC_F32 context of (lengths[b], C, R): its own contraction
+ *     chunks, loss chunks and column-sum blocks, each launch holding every problem's blocks on grid x;
+ *   - no call reads rows lengths[b].. of V_b or H_b, and no call writes them (nor those rows of nmfb200_raw_terms' output);
+ *   - nmfb200_target_minmax covers every problem's first lengths[b] rows (of a shared target too);
+ *   - nmfb200_nmf_batched_cd_update / _iterate, nmfb200_plca_iterate and nmfb200_plca_loss return NMFB200_ERR_INVALID.
+ * Workspace: the sum over the problems of a single context's partial slabs, column-sum and loss partials, not B times the
+ * largest.  NMFB200_ERR_INVALID, before any device work, for B < 1, R > 256, a null `lengths`, a length outside [1, N], and
+ * a launch whose problems' blocks together pass grid x (2^31 - 1) or whose loss partials pass 2^31. */
+int nmfb200_nmf_batched_create_ragged(nmfb200_ctx** out, int device, int64_t B, int64_t N, int64_t C, int64_t R,
+                                      const int64_t* lengths);
 /* Register the targets: problem b reads V + b batch_stride, rows ldv >= C elements apart, elements of type `dtype`.
  * batch_stride 0: one V shared by every problem (restarts of one fit); otherwise batch_stride >= N ldv.  Alignment and dtype
  * checks as nmfb200_nmf_set_target.  V stays borrowed.  Asynchronous. */

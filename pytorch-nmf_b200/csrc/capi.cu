@@ -1,8 +1,10 @@
 // C ABI of libnmf_b200 (see include/nmf_b200.h): context management and the per-update call graphs.
 #include "../../include/nmf_b200.h"
 
+#include <algorithm>
 #include <atomic>
 #include <new>
+#include <vector>
 
 #include "common.cuh"
 #include "tc_nmf.cuh"
@@ -30,6 +32,10 @@ struct nmfb200_ctx {
   // that run
   int64_t nprob = 1, bstride = 0;
   const uint8_t* active = nullptr;
+  // a ragged batch of NMF problems (nmfb200_nmf_batched_create_ragged; kind 2): each problem's plan (device, nprob of them)
+  // and the grid x of each RaggedLaunch, the sum of the problems' blocks
+  RaggedProblem* rag = nullptr;
+  int64_t rag_gx[4] = {0, 0, 0, 0};
   NmfdShape d{};
   const void* V = nullptr;        // the dense target, borrowed: vdtype (NMFB200_DTYPE_*) elements
   int vdtype = NMFB200_DTYPE_F32;
@@ -165,7 +171,7 @@ void free_ctx(nmfb200_ctx* c) {
   if (c->tcd) tc_nmfd_destroy(c->tcd);
   cudaFree(c->num); cudaFree(c->den); cudaFree(c->colsum); cudaFree(c->cs_scratch);
   cudaFree(c->loss_blocks); cudaFree(c->mm_scratch); cudaFree(c->Pn); cudaFree(c->Pp);
-  cudaFree(c->sp_gram); cudaFree(c->sp_loss_part); cudaFree(c->sp_den); cudaFree(c->qobs_part);
+  cudaFree(c->sp_gram); cudaFree(c->sp_loss_part); cudaFree(c->sp_den); cudaFree(c->qobs_part); cudaFree(c->rag);
   delete c;
 }
 
@@ -220,6 +226,7 @@ ApplyArgs factor_view(const nmfb200_ctx* c, int which, int nchunks) {
   a.R = (int)c->R; a.inner = f.inner; a.rowlen = c->R * f.inner; a.ldp = a.rowlen;
   a.numel = f.rows * a.rowlen * c->nprob; a.chunk_stride = a.numel; a.nchunks = nchunks;
   if (is_batch(c)) { a.prob_numel = f.rows * a.rowlen; a.active = c->active; }
+  if (c->rag) { a.rag = c->rag; a.rag_launch = which == 0 ? kRagW : kRagH; }
   return a;
 }
 
@@ -436,6 +443,69 @@ int nmfb200_nmf_batched_create(nmfb200_ctx** out, int device, int64_t B, int64_t
   return 0;
 }
 
+int nmfb200_nmf_batched_create_ragged(nmfb200_ctx** out, int device, int64_t B, int64_t N, int64_t C, int64_t R,
+                                      const int64_t* lengths) {
+  if (!out) return fail(NMFB200_ERR_INVALID, "out is null");
+  *out = nullptr;
+  if (B < 1 || N < 1 || C < 1 || R < 1) return fail(NMFB200_ERR_INVALID, "B, N, C, R must be positive");
+  if (R > 256) return fail(NMFB200_ERR_INVALID, "batched fits support rank <= 256");
+  if (!lengths) return fail(NMFB200_ERR_INVALID, "lengths is null");
+  if (B > kMaxGridX) return fail(NMFB200_ERR_INVALID, "ragged batch: B must be below 2^31 (one block per problem and launch)");
+  // each problem's single-problem plan, its blocks after the previous problems' on grid x and its workspace after theirs
+  std::vector<RaggedProblem> t(B);
+  int64_t gx[4] = {0, 0, 0, 0}, part = 0, loss = 0, cs = 0;
+  const int64_t w_blocks = ceil_div(C, 64);
+  for (int64_t b = 0; b < B; ++b) {
+    const int64_t L = lengths[b];
+    if (L < 1 || L > N)
+      return fail(NMFB200_ERR_INVALID, "lengths[" + std::to_string(b) + "] = " + std::to_string(L) + " is outside [1, N]");
+    RaggedProblem& p = t[b];
+    p.rows = L;
+    p.nch[0] = chunks_for(C, L, R);
+    p.nch[1] = chunks_for(L, C, R);
+    SimtNmfPlan sp;
+    simt_nmf_plan(L, C, (int)R, p.nch[1], &sp);
+    p.loss_chunks = sp.loss_chunks;
+    p.cs_blocks = (int)colsum_scratch_floats(L, 1, 1);
+    const int64_t blocks[4] = {w_blocks * p.nch[0], ceil_div(L, 64) * p.nch[1], ceil_div(L, 64) * p.loss_chunks, p.cs_blocks};
+    for (int k = 0; k < 4; ++k) { p.x0[k] = gx[k]; gx[k] += blocks[k]; }
+    p.part = part; p.loss_part = loss; p.cs_part = cs;
+    part += std::max((int64_t)p.nch[0] * C * R, (int64_t)p.nch[1] * L * R);
+    loss += blocks[2];
+    cs += p.cs_blocks * R;
+    // checked after every problem, so no sum can overflow int64 first
+    if (gx[0] > kMaxGridX || gx[1] > kMaxGridX || gx[2] > kMaxGridX || gx[3] > kMaxGridX)
+      return fail(NMFB200_ERR_INVALID, "ragged batch: the problems' blocks of one launch pass grid x (2^31 - 1)");
+    if (loss > INT32_MAX) return fail(NMFB200_ERR_INVALID, "ragged batch: loss partials must be below 2^31");
+  }
+  // the launches every problem shares the shape of: the column sums of W, their final stage, the ratio stage
+  const int64_t rows = N > C ? N : C;
+  if (colsum_scratch_floats(C, 1, 1) > kMaxGridX / B || ceil_div(R, 64) > kMaxGridX / B ||
+      ceil_div(rows * R, 256) > kMaxGridX / B)
+    return fail(NMFB200_ERR_INVALID, "batch too large for the launch grids");
+  DeviceGuard guard(device);
+  if (!guard.ok) return fail(NMFB200_ERR_CUDA, "cannot select the requested device");
+  nmfb200_ctx* c = new (std::nothrow) nmfb200_ctx();
+  if (!c) return fail(NMFB200_ERR_INVALID, "out of host memory");
+  c->kind = kBatched; c->device = device; c->N = N; c->C = C; c->R = R; c->nprob = B;
+  c->precision = NMFB200_PREC_F32;
+  c->nslab[0] = chunks_for(C, N, R);        // unused by the ragged launches: each problem's own counts are in its plan
+  c->nslab[1] = chunks_for(N, C, R);
+  c->part_floats = part;
+  c->cs_scratch_floats = std::max(cs, colsum_scratch_floats(C, (int)R, 1) * B);
+  c->loss_max_blocks = (int)loss;
+  for (int k = 0; k < 4; ++k) c->rag_gx[k] = gx[k];
+  if (int rc = alloc_workspace(c, 0)) return rc;
+  cudaError_t e = cudaMalloc(&c->rag, (size_t)B * sizeof(RaggedProblem));
+  if (e == cudaSuccess) e = cudaMemcpy(c->rag, t.data(), (size_t)B * sizeof(RaggedProblem), cudaMemcpyHostToDevice);
+  if (e != cudaSuccess) {
+    free_ctx(c);
+    return fail(NMFB200_ERR_CUDA, std::string("ragged batch plans: ") + cudaGetErrorString(e));
+  }
+  *out = c;
+  return 0;
+}
+
 int nmfb200_nmf_batched_set_target(nmfb200_ctx* ctx, const void* V, int64_t ldv, int64_t batch_stride, int dtype,
                                    void* stream) {
   CTX_GUARD(ctx, kBatched);
@@ -444,8 +514,9 @@ int nmfb200_nmf_batched_set_target(nmfb200_ctx* ctx, const void* V, int64_t ldv,
     return fail(NMFB200_ERR_INVALID, "batch stride must be 0 (one shared target) or at least N x ldv");
   if (int rc = check_target(V, dtype)) return rc;
   ctx->V = V; ctx->vdtype = dtype; ctx->ldv = ldv; ctx->bstride = batch_stride; ctx->has_target = true;
+  // a ragged batch: every problem's own rows, even of a shared target
   return matrix_minmax(V, dtype, ctx->N, ctx->C, ldv, ctx->mm_scratch, ctx->mm_scratch + kMmPartials, (cudaStream_t)stream,
-                       CellSel{}, batch_stride ? ctx->nprob : 1, batch_stride);
+                       CellSel{}, batch_stride || ctx->rag ? ctx->nprob : 1, batch_stride, ctx->rag);
 }
 
 int nmfb200_nmf_batched_set_active(nmfb200_ctx* ctx, const uint8_t* active, void* stream) {
@@ -788,6 +859,7 @@ int simt_contract(nmfb200_ctx* c, int which, const float* W, const float* H, dou
   // a batch: problem b's target, factors and partials (slab layout [chunk][problem][rows][R]); one problem otherwise
   Batch bt;
   if (c->kind == kBatched) bt = Batch{c->nprob, c->bstride, f.rows * c->R, f.other_rows * c->R, f.rows * c->R, c->active};
+  if (c->rag) { bt.rag = c->rag; bt.rag_launch = which == 0 ? kRagW : kRagH; bt.rag_gx = c->rag_gx[bt.rag_launch]; }
   return simt_nmf_contract(c->V, c->vdtype, c->ldv, /*trans=*/which == 0, fac[which], fac[1 - which], f.rows, f.other_rows,
                            (int)c->R, beta, c->nslab[which], c->num, c->den, c->R, f.rows * c->R * c->nprob, c->sel, c->C,
                            st, bt);
@@ -853,8 +925,9 @@ int factor_terms(nmfb200_ctx* c, int which, const float* W, const float* H, doub
   if (!kl) { a.den = c->den; return 0; }
   a.kl_den = den_out;
   const FactorDims f = factor_dims(c, which);
+  const bool rag_h = c->rag && which == 0;        // a ragged batch's H: each problem's own rows
   return factor_colsum(fac[1 - which], f.other_rows, (int)c->R, f.other_inner, c->cs_scratch, c->cs_scratch_floats, den_out,
-                       st, c->nprob, c->active);
+                       st, c->nprob, c->active, rag_h ? c->rag : nullptr, rag_h ? c->rag_gx[kRagColsum] : 0);
 }
 
 // One factor update (which = 0: param = W, 1: param = H) on the kernels that serve this context and beta.  No device guard:
@@ -1034,6 +1107,7 @@ int nmfb200_loss(nmfb200_ctx* ctx, const float* W, const float* H, double beta, 
   if (use_tc(ctx, beta)) return tc_loss(ctx->tc, W, H, beta, loss_dev, st);
   Batch bt;         // a batch: loss_dev[b] for every active problem b
   if (ctx->kind == kBatched) bt = Batch{ctx->nprob, ctx->bstride, ctx->N * ctx->R, ctx->C * ctx->R, 0, ctx->active};
+  if (ctx->rag) { bt.rag = ctx->rag; bt.rag_launch = kRagLoss; bt.rag_gx = ctx->rag_gx[kRagLoss]; }
   return simt_nmf_loss(ctx->V, ctx->vdtype, ctx->ldv, H, W, ctx->N, ctx->C, (int)ctx->R, beta, ctx->loss_blocks,
                        ctx->loss_max_blocks, loss_dev, ctx->sel, ctx->C, st, bt);
 }
@@ -1152,6 +1226,7 @@ int cd_check(nmfb200_ctx* ctx) {
 // What the batched cd calls serve: a nmfb200_nmf_batched_create context (CTX_GUARD) whose every launch fits grid x.  The
 // problems ride on grid x, and the sweep and Gram kernels take more blocks per problem than nmfb200_nmf_batched_create checks.
 int cd_batched_check(nmfb200_ctx* ctx) {
+  if (ctx->rag) return fail(NMFB200_ERR_INVALID, "batched cd: a ragged batch (nmfb200_nmf_batched_create_ragged) is not served");
   int64_t rpb;
   int nb_n, nb_c;
   sparse_gram_plan(ctx->N, &rpb, &nb_n);
@@ -1273,6 +1348,7 @@ int nmfb200_plca_iterate(nmfb200_ctx* ctx, float* W, float* H, float* Z, float* 
                          const float* W_alpha, const float* H_alpha, const float* Z_alpha, int n_iter, void* stream) {
   CTX_GUARD(ctx, kAnyKind);
   if (!is_batch(ctx)) return fail(NMFB200_ERR_INVALID, "plca_iterate takes a batched NMF or NMFD context");
+  if (ctx->rag) return fail(NMFB200_ERR_INVALID, "plca_iterate does not serve a ragged batch");
   TARGET_GUARD(ctx);
   if (!W || !H || !Z || !Hz || !work || n_iter < 0) return fail(NMFB200_ERR_INVALID, "bad argument");
   if (flags & ~(NMFB200_PLCA_TRAIN_W | NMFB200_PLCA_TRAIN_H | NMFB200_PLCA_TRAIN_Z))
@@ -1298,6 +1374,7 @@ int nmfb200_plca_loss(nmfb200_ctx* ctx, const float* W, const float* Hz, const f
                       void* stream) {
   CTX_GUARD(ctx, kAnyKind);
   if (!is_batch(ctx)) return fail(NMFB200_ERR_INVALID, "plca_loss takes a batched NMF or NMFD context");
+  if (ctx->rag) return fail(NMFB200_ERR_INVALID, "plca_loss does not serve a ragged batch");
   TARGET_GUARD(ctx);
   if (!W || !Hz || !norm_dev || !loss_dev) return fail(NMFB200_ERR_INVALID, "null pointer");
   cudaStream_t st = (cudaStream_t)stream;

@@ -62,10 +62,39 @@ int with_sel(CellSel s, F&& f) {
   return f(static_cast<const NoSel*>(nullptr));
 }
 
+// One problem of a ragged batch (nmfb200_nmf_batched_create_ragged): N_b <= N rows over the batch's C columns, stored in
+// the padded (B, N, ...) layouts of V and H.  It runs the plan of a single problem of N_b rows: its own chunk counts, loss
+// chunks and column-sum blocks, and its partials laid out as that problem's, at its own offsets in the shared buffers.  Its
+// blocks of each launch below start at x0[launch] on grid x and run up to the next problem's (x0 ascends with b).
+enum RaggedLaunch : int { kRagW = 0, kRagH = 1, kRagLoss = 2, kRagColsum = 3 };
+struct RaggedProblem {
+  int64_t rows;           // N_b
+  int64_t x0[4];          // first block on grid x of the W and H contractions, the loss and the column sums of H
+  int64_t part;           // floats before its partial slabs ([chunk][rows][R], rows = C for W and N_b for H)
+  int64_t loss_part;      // doubles before its loss partials ([chunk][row block])
+  int64_t cs_part;        // floats before its column-sum partials of H ([block][R])
+  int nch[2];             // contraction chunks of its W / H update
+  int loss_chunks;
+  int cs_blocks;          // column-sum blocks over its rows
+};
+// the problem of a ragged batch's n whose blocks of `launch` hold grid-x block bx: the last one with x0[launch] <= bx
+__device__ __forceinline__ int64_t ragged_problem(const RaggedProblem* t, int64_t n, int launch, int64_t bx) {
+  int64_t lo = 0, hi = n - 1;
+  while (lo < hi) {
+    const int64_t mid = (lo + hi + 1) >> 1;
+    if (t[mid].x0[launch] <= bx) lo = mid;
+    else hi = mid - 1;
+  }
+  return lo;
+}
+
 // A batch of independent NMF problems of one shape (nmfb200_nmf_batched_create).  The kernels that take it run every problem
 // in one launch, with the batch folded into grid x: problem b owns the blocks [b nbx, (b + 1) nbx) of the nbx blocks one
 // problem launches, and does in them exactly what a launch for that problem alone does.  Offsets between problems are in
 // elements of the pointer they apply to, int64.  The default is one problem (every single-problem call).
+// A ragged batch (rag set: n problems' plans in device memory) keeps v, f and g -- V and the factors stay padded -- and takes
+// each problem's rows, chunks, partial offsets and first block from rag[b] instead; the launch's grid x is rag_gx, its
+// grid y 1 (the chunks ride on grid x too).
 struct Batch {
   int64_t n = 1;                      // problems
   int64_t v = 0;                      // target elements between problems (0: one target shared by every problem)
@@ -75,6 +104,9 @@ struct Batch {
   // KL loss only (batched PLCA): n floats, problem b's target and reconstruction are multiplied by scale[b] before the loss
   // term (null: none)
   const float* scale = nullptr;
+  const RaggedProblem* rag = nullptr; // ragged batch: n per-problem plans (null: every problem has the launch's shape)
+  int rag_launch = 0;                 // RaggedLaunch of this launch
+  int64_t rag_gx = 0;                 // its grid x: the sum of the problems' blocks
 };
 __device__ __forceinline__ bool batch_skips(const uint8_t* active, int64_t b) { return active && !active[b]; }
 
@@ -248,6 +280,11 @@ struct ApplyArgs {
   // kl_den + b R; a problem whose active flag is 0 is left untouched (0: one problem)
   int64_t prob_numel = 0;
   const uint8_t* active = nullptr;
+  // a ragged batch (Batch::rag, with prob_numel): problem b's partials are its own nch[rag_launch] slabs at rag[b].part, of
+  // its rows (kRagH: rag[b].rows, kRagW: all prob_numel / rowlen) x ldp; nchunks and chunk_stride are not read.  The rows of
+  // H past rag[b].rows are padding: left untouched.
+  const RaggedProblem* rag = nullptr;
+  int rag_launch = 0;
 };
 int apply_update(const ApplyArgs& a, cudaStream_t st);
 // whether apply_update takes its four-elements-per-thread kernel for this shape (16-byte aligned buffers provided)
@@ -256,18 +293,24 @@ bool apply_update_vec4_shape(const ApplyArgs& a);
 int raw_sum(const ApplyArgs& a, float* num_out, float* den_out, cudaStream_t st);
 // sums[r] = sum over all other dims of x viewed as (outer, R, inner); deterministic two-stage.  nprob > 1: sums[b R + r] for
 // nprob consecutive (outer, R, inner) problems, each summed in the single problem's order, skipping those whose `active`
-// flag is 0; scratch_floats then covers nprob x colsum_scratch_floats.
+// flag is 0; scratch_floats then covers nprob x colsum_scratch_floats.  rag (inner 1; a ragged batch's table): problem b
+// sums its rag[b].rows rows of its (outer, R) block on its own rag[b].cs_blocks blocks, partials at rag[b].cs_part; rag_gx
+// is their sum.
 int factor_colsum(const float* x, int64_t outer, int R, int64_t inner, float* scratch, int64_t scratch_floats,
-                  float* sums, cudaStream_t st, int64_t nprob = 1, const uint8_t* active = nullptr);
+                  float* sums, cudaStream_t st, int64_t nprob = 1, const uint8_t* active = nullptr,
+                  const RaggedProblem* rag = nullptr, int64_t rag_gx = 0);
 int64_t colsum_scratch_floats(int64_t outer, int R, int64_t inner);
 // min / max of a strided matrix of `vdtype` elements (fit()'s validation), results in mm[0..1]; with M (optional, contiguous
 // rows x cols selector) over the cells where M is non-zero only (none: +inf / -inf).  nprob > 1: over nprob such matrices,
-// `bstride` elements apart (no selector).
+// `bstride` elements apart (no selector); rag (a ragged batch's table): matrix b's first rag[b].rows rows only.
 int matrix_minmax(const void* V, int vdtype, int64_t rows, int64_t cols, int64_t ld, float* scratch2048, float* mm,
-                  cudaStream_t st, CellSel M = CellSel{}, int64_t nprob = 1, int64_t bstride = 0);
+                  cudaStream_t st, CellSel M = CellSel{}, int64_t nprob = 1, int64_t bstride = 0,
+                  const RaggedProblem* rag = nullptr);
 // *out = sum of n doubles in fixed order (single block).  nprob > 1: out[b] = the sum of p[b n, (b + 1) n), one block per
-// problem, in the same order; a problem whose `active` flag is 0 keeps its out[b].
-int sum_partials(const double* p, int n, double* out, cudaStream_t st, int64_t nprob = 1, const uint8_t* active = nullptr);
+// problem, in the same order; a problem whose `active` flag is 0 keeps its out[b].  rag (a ragged batch's table): problem
+// b's run is its own simt_nmf_loss partials at rag[b].loss_part (n is not read).
+int sum_partials(const double* p, int n, double* out, cudaStream_t st, int64_t nprob = 1, const uint8_t* active = nullptr,
+                 const RaggedProblem* rag = nullptr);
 
 // project.cu -------------------------------------------------------------------------------
 // Hoyer's projection (nmf.py:21-49) of every slice x[:, j, :] of x viewed as (outer, D, inner) onto {v >= 0, |v|_1 = k1[j],

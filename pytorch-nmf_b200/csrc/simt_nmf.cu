@@ -21,7 +21,9 @@
 //
 // Batch (common.cuh, batched NMF): grid x holds the row blocks of every problem, problem after problem; a CTA reads its
 // problem's V, F and G and writes its partials at the problem's offsets, and otherwise runs the single problem's plan and
-// arithmetic unchanged, so each problem's partials equal a single-problem launch's bit for bit.
+// arithmetic unchanged, so each problem's partials equal a single-problem launch's bit for bit.  In a ragged batch
+// (Batch::rag) each problem's plan is that of its own row count: a CTA finds its problem by a binary search over the
+// problems' first blocks on grid x, which holds every problem's (chunk, row block) pairs; it reads no row past the problem's.
 //
 // kVFree (sparse targets at beta != 1, 2): the contraction forms only den += (S+eps)^(beta-1) G_tile and reads no V, with
 // kGeneric's plan, staging and arithmetic, so its den partials equal kGeneric's bit for bit whatever V holds; the loss sums
@@ -111,7 +113,7 @@ __device__ __forceinline__ void phi(float v, float s, float bm2, float bm1, floa
   }
 }
 
-template <int RB, bool TRANS, int MODE, typename TV, typename SEL = NoSel, bool BATCH = false>
+template <int RB, bool TRANS, int MODE, typename TV, typename SEL = NoSel, bool BATCH = false, bool RAGGED = false>
 __global__ void __launch_bounds__(256)
 simt_contract_kernel(const TV* __restrict__ V, int64_t ldv, const float* __restrict__ F,
                      const float* __restrict__ G, int64_t Mr, int64_t Nc, int R, float bm2, float bm1,
@@ -136,9 +138,28 @@ simt_contract_kernel(const TV* __restrict__ V, int64_t ldv, const float* __restr
   float* Qs = kDenOnly ? Ps : Ps + kTile * kLd;     // [64][kLd]  Pp (kTwo only; kVFree: in Ps's place); MASK: the selector first
 
   // BATCH (NoSel only): this block's problem and its row block within it; the problem's pointers.  The single-problem
-  // instantiations compile none of it.
+  // instantiations compile none of it.  RAGGED (a ragged batch, bt.rag) also takes the problem's rows (F's for the H update,
+  // the contracted ones for the W update), chunks and partial slabs from its plan, and its chunk from grid x; the uniform
+  // batch instantiations compile none of that.
+  static_assert(!RAGGED || (BATCH && !kNumOnly_), "RAGGED: a batch of MU contractions");
   int64_t bx = blockIdx.x;
-  if constexpr (BATCH) {
+  int chunk = blockIdx.y;
+  if constexpr (RAGGED) {
+    const int64_t prob = ragged_problem(bt.rag, bt.n, bt.rag_launch, bx);
+    if (batch_skips(bt.active, prob)) return;
+    const RaggedProblem& p = bt.rag[prob];
+    if (bt.rag_launch == kRagW) Nc = p.rows;
+    else Mr = p.rows;
+    nchunks = p.nch[bt.rag_launch];
+    const int64_t nbx = (Mr + kTile - 1) / kTile;
+    bx -= p.x0[bt.rag_launch];
+    chunk = (int)(bx / nbx);
+    bx -= chunk * nbx;
+    chunk_stride = Mr * ldp;
+    V += prob * bt.v; F += prob * bt.f; G += prob * bt.g;
+    if (kNum) num += p.part;
+    if (kTwo) den += p.part;
+  } else if constexpr (BATCH) {
     const int64_t nbx = (Mr + kTile - 1) / kTile;
     const int64_t prob = bx / nbx;
     if (batch_skips(bt.active, prob)) return;
@@ -151,7 +172,6 @@ simt_contract_kernel(const TV* __restrict__ V, int64_t ldv, const float* __restr
   const int tid = threadIdx.x;
   const int tx = tid & 15, ty = tid >> 4;
   const int64_t m0 = bx * kTile;
-  const int chunk = blockIdx.y;
   const int64_t tiles_total = (Nc + kTile - 1) / kTile;
   const int64_t tpc = chunk_tiles(Nc, nchunks);
   const int64_t tile_begin = chunk * tpc;
@@ -307,14 +327,14 @@ simt_contract_kernel(const TV* __restrict__ V, int64_t ldv, const float* __restr
   }
 }
 
-template <int RB, bool TRANS, typename TV, typename SEL, bool BATCH>
+template <int RB, bool TRANS, typename TV, typename SEL, bool BATCH, bool RAGGED = false>
 int launch_contract_mode(int mode, dim3 grid, size_t smem, cudaStream_t st, const TV* V, int64_t ldv,
                          const float* F, const float* G, int64_t Mr, int64_t Nc, int R, float bm2, float bm1,
                          int nchunks, float* num, float* den, int64_t ldp, int64_t chunk_stride, const SEL* Mk,
                          int64_t ldm, const Batch& bt) {
 #define NMF_LAUNCH_MODE(M)                                                                              \
   {                                                                                                     \
-    auto kern = simt_contract_kernel<RB, TRANS, M, TV, SEL, BATCH>;                                     \
+    auto kern = simt_contract_kernel<RB, TRANS, M, TV, SEL, BATCH, RAGGED>;                             \
     NMF_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
     kern<<<grid, 256, smem, st>>>(V, ldv, F, G, Mr, Nc, R, bm2, bm1, nchunks, num, den, ldp,            \
                                   chunk_stride, Mk, ldm, bt, nullptr);                                  \
@@ -338,8 +358,15 @@ int launch_contract_rb(int trans, int mode, dim3 grid, cudaStream_t st, const TV
   const int Rp = 16 * RB;
   constexpr bool MASK = !std::is_same<SEL, NoSel>::value;
   size_t smem = (size_t)(2 * Rp + kTile * (mode == kKL && !MASK ? 1 : 2)) * kLd * sizeof(float);
-  // a batch runs the BATCH instantiations (no selector); one problem the single-problem ones
+  // a batch runs the BATCH instantiations (no selector), a ragged one the RAGGED ones; one problem the single-problem ones
   if constexpr (std::is_same<SEL, NoSel>::value) {
+    if (bt.rag) {
+      if (trans)
+        return launch_contract_mode<RB, true, TV, SEL, true, true>(mode, grid, smem, st, V, ldv, F, G, Mr, Nc, R, bm2, bm1,
+                                                                   nchunks, num, den, ldp, chunk_stride, Mk, ldm, bt);
+      return launch_contract_mode<RB, false, TV, SEL, true, true>(mode, grid, smem, st, V, ldv, F, G, Mr, Nc, R, bm2, bm1,
+                                                                  nchunks, num, den, ldp, chunk_stride, Mk, ldm, bt);
+    }
     if (bt.n > 1 || bt.active) {
       if (trans)
         return launch_contract_mode<RB, true, TV, SEL, true>(mode, grid, smem, st, V, ldv, F, G, Mr, Nc, R, bm2, bm1,
@@ -359,7 +386,7 @@ int launch_contract_rb(int trans, int mode, dim3 grid, cudaStream_t st, const TV
 
 // SEL: the sum runs over the observed cells only (the missing ones are dropped, not zeroed: at beta != 0, 1, 2 a zeroed
 // cell would still add eps^beta / beta); a weighted fit adds w * term over the cells with w != 0
-template <int MODE, typename TV, typename SEL = NoSel, bool BATCH = false>
+template <int MODE, typename TV, typename SEL = NoSel, bool BATCH = false, bool RAGGED = false>
 __global__ void __launch_bounds__(256)
 simt_loss_kernel(const TV* __restrict__ V, int64_t ldv, const float* __restrict__ F,
                  const float* __restrict__ G, int64_t Mr, int64_t Nc, int R, int Rp, float beta, int nchunks,
@@ -369,10 +396,26 @@ simt_loss_kernel(const TV* __restrict__ V, int64_t ldv, const float* __restrict_
   float* Gs = Fs + Rp * kLd;
   __shared__ double red[8];
   // BATCH (NoSel only): problem `prob`'s blocks write its own run of gridDim.y x nbx partials, laid out as a single
-  // problem's
+  // problem's.  RAGGED (a ragged batch, bt.rag): the problem's rows and loss chunks from its plan, its chunk from grid x,
+  // its run of partials at its loss_part.
+  static_assert(!RAGGED || BATCH, "RAGGED: a batch");
   int64_t bx = blockIdx.x, part = 0;
+  int chunk = blockIdx.y;
   float sc = 1.f;                    // BATCH, KL: the problem's bt.scale
-  if constexpr (BATCH) {
+  if constexpr (RAGGED) {
+    const int64_t prob = ragged_problem(bt.rag, bt.n, kRagLoss, bx);
+    if (batch_skips(bt.active, prob)) return;
+    const RaggedProblem& p = bt.rag[prob];
+    Mr = p.rows;
+    nchunks = p.loss_chunks;
+    const int64_t nbx = (Mr + kTile - 1) / kTile;
+    bx -= p.x0[kRagLoss];
+    part = p.loss_part + bx;
+    chunk = (int)(bx / nbx);
+    bx -= chunk * nbx;
+    V += prob * bt.v; F += prob * bt.f; G += prob * bt.g;
+    if (MODE == kKL && bt.scale) sc = bt.scale[prob];
+  } else if constexpr (BATCH) {
     const int64_t nbx = (Mr + kTile - 1) / kTile;
     const int64_t prob = bx / nbx;
     if (batch_skips(bt.active, prob)) return;
@@ -384,7 +427,6 @@ simt_loss_kernel(const TV* __restrict__ V, int64_t ldv, const float* __restrict_
   const int tid = threadIdx.x;
   const int tx = tid & 15, ty = tid >> 4;
   const int64_t m0 = bx * kTile;
-  const int chunk = blockIdx.y;
   const int64_t tiles_total = (Nc + kTile - 1) / kTile;
   const int64_t tpc = chunk_tiles(Nc, nchunks);
   const int64_t tile_begin = chunk * tpc;
@@ -430,13 +472,20 @@ simt_loss_kernel(const TV* __restrict__ V, int64_t ldv, const float* __restrict_
   if (tid == 0) block_partials[BATCH ? part : (int64_t)blockIdx.y * gridDim.x + blockIdx.x] = tot;
 }
 
-// one block per problem (grid x): out[b] = the sum of p[b n, (b + 1) n)
+// one block per problem (grid x): out[b] = the sum of p[b n, (b + 1) n); RAGGED: of problem b's own loss partials
+template <bool RAGGED>
 __global__ void __launch_bounds__(256) sum_partials_kernel(const double* __restrict__ p, int n, double* out,
-                                                           const uint8_t* __restrict__ active) {
+                                                           const uint8_t* __restrict__ active,
+                                                           const RaggedProblem* __restrict__ rag) {
   __shared__ double red[8];
   const int64_t b = blockIdx.x;
   if (batch_skips(active, b)) return;
-  p += b * n;
+  if constexpr (RAGGED) {
+    p += rag[b].loss_part;
+    n = (int)((rag[b].rows + kTile - 1) / kTile * rag[b].loss_chunks);
+  } else {
+    p += b * n;
+  }
   double acc = 0.0;
   for (int i = threadIdx.x; i < n; i += 256) acc += p[i];
   double tot = block_reduce_sum(acc, red);
@@ -464,15 +513,22 @@ void simt_nmf_plan(int64_t Mr, int64_t Nc, int R, int nchunks, SimtNmfPlan* p) {
   p->loss_tiles_per_chunk = chunk_tiles(Nc, p->loss_chunks);
 }
 
-int sum_partials(const double* p, int n, double* out, cudaStream_t st, int64_t nprob, const uint8_t* active) {
+int sum_partials(const double* p, int n, double* out, cudaStream_t st, int64_t nprob, const uint8_t* active,
+                 const RaggedProblem* rag) {
   if (nprob < 1 || nprob > kMaxGridX) { set_error("sum_partials: bad problem count"); return 1; }
-  sum_partials_kernel<<<(unsigned)nprob, 256, 0, st>>>(p, n, out, active);
+  if (rag) sum_partials_kernel<true><<<(unsigned)nprob, 256, 0, st>>>(p, n, out, active, rag);
+  else sum_partials_kernel<false><<<(unsigned)nprob, 256, 0, st>>>(p, n, out, active, nullptr);
   NMF_LAUNCH_CHECK();
   return 0;
 }
 
-// grid x of a batched launch: nbx blocks per problem for bt.n problems
+// grid x of a batched launch: nbx blocks per problem for bt.n problems; a ragged batch's own sum of blocks
 static int batch_grid_x(int64_t nbx, const Batch& bt, const char* who, unsigned* x) {
+  if (bt.rag) {
+    if (bt.rag_gx < 1 || bt.rag_gx > kMaxGridX) { set_error(std::string(who) + ": ragged blocks pass grid x"); return 1; }
+    *x = (unsigned)bt.rag_gx;
+    return 0;
+  }
   if (bt.n < 1 || nbx > kMaxGridX / bt.n) { set_error(std::string(who) + ": batch x row blocks pass grid x"); return 1; }
   *x = (unsigned)(nbx * bt.n);
   return 0;
@@ -487,7 +543,8 @@ int simt_nmf_contract(const void* V, int vdtype, int64_t ldv, int trans, const f
   float bm2 = (float)(beta - 2.0), bm1 = (float)(beta - 1.0);
   unsigned gx;
   if (batch_grid_x(ceil_div(Mr, kTile), bt, "simt_nmf_contract", &gx)) return 1;
-  dim3 grid(gx, (unsigned)nchunks, (unsigned)simt_rank_blocks(R));
+  if (bt.rag && R > 256) { set_error("simt_nmf_contract: a ragged batch takes rank <= 256"); return 1; }
+  dim3 grid(gx, bt.rag ? 1u : (unsigned)nchunks, (unsigned)simt_rank_blocks(R));     // ragged: the chunks are on grid x
   const int rb = contract_rb(R);
   return with_vtype(V, vdtype, [&](auto Vt) {
     using TV = vtype_t<decltype(Vt)>;
@@ -516,9 +573,10 @@ int simt_nmf_loss(const void* V, int vdtype, int64_t ldv, const float* F, const 
   int nchunks = loss_chunks(Mr, Nc);
   unsigned gx;
   if (batch_grid_x(ceil_div(Mr, kTile), bt, "simt_nmf_loss", &gx)) return 1;
-  dim3 grid(gx, (unsigned)nchunks);
-  const int nblocks = (int)(ceil_div(Mr, kTile) * nchunks);          // per problem
-  if ((double)nblocks * (double)bt.n > (double)max_blocks) { set_error("simt_nmf_loss: partial buffer too small"); return 1; }
+  dim3 grid(gx, bt.rag ? 1u : (unsigned)nchunks);                    // ragged: the chunks are on grid x
+  const int nblocks = (int)(ceil_div(Mr, kTile) * nchunks);          // per problem (ragged: every problem's, below)
+  const double total = bt.rag ? (double)bt.rag_gx : (double)nblocks * (double)bt.n;
+  if (total > (double)max_blocks) { set_error("simt_nmf_loss: partial buffer too small"); return 1; }
   int Rp = (int)round_up(R < 256 ? R : 256, 16);
   size_t smem = (size_t)2 * Rp * kLd * sizeof(float);
   int mode = beta_mode(beta);
@@ -527,18 +585,19 @@ int simt_nmf_loss(const void* V, int vdtype, int64_t ldv, const float* F, const 
     using TV = vtype_t<decltype(Vt)>;
     return with_sel(M, [&](auto Mk) {
       using SEL = sel_t<decltype(Mk)>;
-#define NMF_LOSS_B(MD, BATCH)                                                                                               \
+#define NMF_LOSS_B(MD, BATCH, RAGGED)                                                                                       \
   {                                                                                                                         \
-    auto kern = simt_loss_kernel<MD, TV, SEL, BATCH>;                                                                       \
+    auto kern = simt_loss_kernel<MD, TV, SEL, BATCH, RAGGED>;                                                               \
     NMF_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));                     \
     kern<<<grid, 256, smem, st>>>(Vt, ldv, F, G, Mr, Nc, R, Rp, (float)beta, nchunks, block_partials, Mk, M ? ldm : 0, bt);\
   }
 #define NMF_LOSS(MD)                                                                                                        \
   {                                                                                                                         \
     if constexpr (std::is_same<SEL, NoSel>::value) {                                                                        \
-      if (batched) { NMF_LOSS_B(MD, true); break; }                                                                         \
+      if (bt.rag) { NMF_LOSS_B(MD, true, true); break; }                                                                    \
+      if (batched) { NMF_LOSS_B(MD, true, false); break; }                                                                  \
     }                                                                                                                       \
-    NMF_LOSS_B(MD, false);                                                                                                  \
+    NMF_LOSS_B(MD, false, false);                                                                                           \
   }
       switch (mode) {
         case kKL: NMF_LOSS(kKL); break;
@@ -553,7 +612,7 @@ int simt_nmf_loss(const void* V, int vdtype, int64_t ldv, const float* F, const 
     });
   });
   if (rc) return rc;
-  return sum_partials(block_partials, nblocks, loss_dev, st, bt.n, bt.active);
+  return sum_partials(block_partials, nblocks, loss_dev, st, bt.n, bt.active, bt.rag);
 }
 
 int simt_nmf_contract_den(const float* F, const float* G, int64_t Mr, int64_t Nc, int R, double beta, int nchunks,
@@ -585,6 +644,7 @@ int simt_nmf_contract_den(const float* F, const float* G, int64_t Mr, int64_t Nc
 int simt_nmf_contract_num(const void* V, int vdtype, int64_t ldv, int trans, const float* G, int64_t Mr, int64_t Nc, int R,
                           int nchunks, float* num, int64_t chunk_stride, cudaStream_t st, const Batch& bt) {
   if (R < 1 || R > 256) { set_error("simt_nmf_contract_num: rank must be in [1, 256]"); return 1; }
+  if (bt.rag) { set_error("simt_nmf_contract_num: a ragged batch is not served"); return 1; }
   unsigned gx;
   if (batch_grid_x(ceil_div(Mr, kTile), bt, "simt_nmf_contract_num", &gx)) return 1;
   const dim3 grid(gx, (unsigned)nchunks, 1u);

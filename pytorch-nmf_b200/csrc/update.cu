@@ -5,19 +5,39 @@ namespace nmfb200 {
 
 namespace {
 
+// Where the partials of element idx (of problem b) are: the offset in the first slab, the slab count and stride.  False for
+// a padding row of a ragged batch's H, which no kernel writes.  The kernels below take RAGGED (a.rag set) as a template flag,
+// so that their uniform instantiations run the code they always ran.
+struct PartialAt { int64_t off, stride; int nch; };
+template <bool RAGGED>
+__device__ __forceinline__ bool partial_at(const ApplyArgs& a, int64_t idx, int64_t b, PartialAt& p) {
+  if constexpr (RAGGED) {
+    const RaggedProblem& rp = a.rag[b];
+    const int64_t local = idx - b * a.prob_numel;
+    const int64_t row = local / a.rowlen;
+    const int64_t rows = a.rag_launch == kRagW ? a.prob_numel / a.rowlen : rp.rows;
+    if (row >= rows) return false;
+    p = PartialAt{rp.part + row * a.ldp + (local - row * a.rowlen), rows * a.ldp, rp.nch[a.rag_launch]};
+    return true;
+  }
+  const int64_t row = idx / a.rowlen;
+  p = PartialAt{row * a.ldp + (idx - row * a.rowlen), a.chunk_stride, a.nchunks};
+  return true;
+}
+
+template <bool RAGGED>
 __global__ void __launch_bounds__(256)
 apply_update_kernel(ApplyArgs a) {
   const int64_t idx = (int64_t)blockIdx.x * 256 + threadIdx.x;
   float newv = 0.f;
   const int64_t b = a.prob_numel ? idx / a.prob_numel : 0;      // Batch: the element's problem
-  if (idx < a.numel && !batch_skips(a.active, b)) {
-    const int64_t row = idx / a.rowlen;
-    const int64_t col = idx - row * a.rowlen;
-    const int64_t off = row * a.ldp + col;
+  PartialAt pa;
+  if (idx < a.numel && !batch_skips(a.active, b) && partial_at<RAGGED>(a, idx, b, pa)) {
+    const int64_t off = pa.off;
     const int r = (int)((idx / a.inner) % a.R);
     const float sc = a.out_scale ? *a.out_scale : 1.0f;
     float num = 0.f;
-    for (int ch = 0; ch < a.nchunks; ++ch) num += a.num[ch * a.chunk_stride + off];
+    for (int ch = 0; ch < pa.nch; ++ch) num += a.num[ch * pa.stride + off];
     num *= sc;
     if (a.kappa) num = fmaf(*a.kappa, a.kappa_vec[r], num);
     const float p = a.param[idx];
@@ -25,7 +45,7 @@ apply_update_kernel(ApplyArgs a) {
     float pos;
     if (a.den) {
       float den = 0.f;
-      for (int ch = 0; ch < a.nchunks; ++ch) den += a.den[ch * a.chunk_stride + off];
+      for (int ch = 0; ch < pa.nch; ++ch) den += a.den[ch * pa.stride + off];
       den *= sc;
       pos = fmaxf(den, 0.f) + kEps;                          // nmf.py:83
     } else {
@@ -52,36 +72,51 @@ apply_update_kernel(ApplyArgs a) {
 }
 
 // The ratio stage's inputs without the ratio stage: the summed partials (+ the centring term), nothing clamped.
+template <bool RAGGED>
 __global__ void __launch_bounds__(256)
 raw_sum_kernel(ApplyArgs a, float* __restrict__ num_out, float* __restrict__ den_out) {
   const int64_t idx = (int64_t)blockIdx.x * 256 + threadIdx.x;
-  if (idx >= a.numel || batch_skips(a.active, a.prob_numel ? idx / a.prob_numel : 0)) return;
-  const int64_t row = idx / a.rowlen;
-  const int64_t off = row * a.ldp + (idx - row * a.rowlen);
+  const int64_t b = a.prob_numel ? idx / a.prob_numel : 0;
+  PartialAt pa;
+  if (idx >= a.numel || batch_skips(a.active, b) || !partial_at<RAGGED>(a, idx, b, pa)) return;
+  const int64_t off = pa.off;
   const float sc = a.out_scale ? *a.out_scale : 1.0f;
   float num = 0.f;
-  for (int ch = 0; ch < a.nchunks; ++ch) num += a.num[ch * a.chunk_stride + off];
+  for (int ch = 0; ch < pa.nch; ++ch) num += a.num[ch * pa.stride + off];
   num *= sc;
   if (a.kappa) num = fmaf(*a.kappa, a.kappa_vec[(int)((idx / a.inner) % a.R)], num);
   num_out[idx] = num;
   if (den_out) {
     float den = 0.f;
-    for (int ch = 0; ch < a.nchunks; ++ch) den += a.den[ch * a.chunk_stride + off];
+    for (int ch = 0; ch < pa.nch; ++ch) den += a.den[ch * pa.stride + off];
     den_out[idx] = den * sc;
   }
 }
 
 // stage 1 for inner == 1: x is (outer, R) row-major; block (b, y) sums a row slab of components [256 y, 256 y + 256).
-// Batch: nb blocks per problem along x, each problem's x and partials nprob-strided (outer R and nb R floats).
+// Batch: nb blocks per problem along x, each problem's x and partials nprob-strided (outer R and nb R floats).  A ragged
+// batch (rag, nprob problems): problem b's own rows, blocks and partials from its plan.
+template <bool RAGGED>
 __global__ void __launch_bounds__(256)
 colsum_rows_kernel(const float* __restrict__ x, int64_t outer, int R, int64_t rows_per_block,
-                   float* __restrict__ partial, int64_t nb, const uint8_t* __restrict__ active) {
+                   float* __restrict__ partial, int64_t nb, const uint8_t* __restrict__ active,
+                   const RaggedProblem* __restrict__ rag, int64_t nprob) {
   __shared__ float sh[256];
-  const int64_t prob = (int64_t)blockIdx.x / nb;
+  int64_t prob, bx;
+  if constexpr (RAGGED) {
+    prob = ragged_problem(rag, nprob, kRagColsum, blockIdx.x);
+    x += prob * outer * R;
+    partial += rag[prob].cs_part;
+    bx = (int64_t)blockIdx.x - rag[prob].x0[kRagColsum];
+    outer = rag[prob].rows;
+    rows_per_block = (outer + rag[prob].cs_blocks - 1) / rag[prob].cs_blocks;
+  } else {
+    prob = (int64_t)blockIdx.x / nb;
+    x += prob * outer * R;
+    partial += prob * nb * R;
+    bx = (int64_t)blockIdx.x - prob * nb;
+  }
   if (batch_skips(active, prob)) return;
-  x += prob * outer * R;
-  partial += prob * nb * R;
-  const int64_t bx = (int64_t)blockIdx.x - prob * nb;
   const int tid = threadIdx.x;
   const int r0 = blockIdx.y * 256;
   const int Rb = min(R - r0, 256);               // this block's components
@@ -124,13 +159,19 @@ colsum_runs_kernel(const float* __restrict__ x, int64_t inner, float* __restrict
   }
 }
 
-// Batch: ceil(R / blockDim) blocks per problem along x
+// Batch: ceil(R / blockDim) blocks per problem along x; a ragged batch's problem b: its own partials and blocks
+template <bool RAGGED>
 __global__ void colsum_final_kernel(const float* __restrict__ partial, int64_t nb, int R, float* __restrict__ sums,
-                                    const uint8_t* __restrict__ active) {
+                                    const uint8_t* __restrict__ active, const RaggedProblem* __restrict__ rag) {
   const int64_t per = (R + blockDim.x - 1) / blockDim.x;
   const int64_t prob = (int64_t)blockIdx.x / per;
   if (batch_skips(active, prob)) return;
-  partial += prob * nb * R;
+  if constexpr (RAGGED) {
+    partial += rag[prob].cs_part;
+    nb = rag[prob].cs_blocks;
+  } else {
+    partial += prob * nb * R;
+  }
   sums += prob * R;
   const int r = (int)((int64_t)blockIdx.x - prob * per) * blockDim.x + threadIdx.x;
   if (r >= R) return;
@@ -144,11 +185,11 @@ __device__ __forceinline__ float nan_max(float a, float b) { return (a != a || b
 
 // NaN-sticky min / max so that a NaN in V fails fit()'s non-negativity assertion like torch.all(V >= 0) does
 // SEL: the cells where M (contiguous rows x cols: a mask or weights) is 0 are skipped, V is not read there
-// Batch: nprob matrices of rows x cols, bstride elements apart
+// Batch: nprob matrices of rows x cols, bstride elements apart (ragged, rag: matrix b's first rag[b].rows rows)
 template <typename TV, typename SEL = NoSel>
 __global__ void __launch_bounds__(256)
 minmax_stage1(const TV* __restrict__ V, int64_t rows, int64_t cols, int64_t ld, float* __restrict__ scratch,
-              const SEL* __restrict__ M, int64_t nprob, int64_t bstride) {
+              const SEL* __restrict__ M, int64_t nprob, int64_t bstride, const RaggedProblem* __restrict__ rag) {
   __shared__ float smin[8], smax[8];
   float mn = INFINITY, mx = -INFINITY;
   const int64_t total = nprob * rows * cols;
@@ -157,6 +198,7 @@ minmax_stage1(const TV* __restrict__ V, int64_t rows, int64_t cols, int64_t ld, 
     int64_t r = i / cols, c = i - r * cols;
     const int64_t b = nprob > 1 ? r / rows : 0;
     r -= b * rows;
+    if (rag && r >= rag[b].rows) continue;
     float v = to_f32(V[b * bstride + r * ld + c]);
     mn = nan_min(mn, v);
     mx = nan_max(mx, v);
@@ -186,25 +228,26 @@ __global__ void minmax_stage2(const float* __restrict__ scratch, int nb, float* 
 
 // Four consecutive elements per thread (same row, same component: inner % 4 == 0), 16-byte loads of the parameter and of every
 // partial slab.  Same arithmetic per element as apply_update_kernel.
+template <bool RAGGED>
 __global__ void __launch_bounds__(256)
 apply_update_vec4_kernel(ApplyArgs a) {
   const int64_t idx = ((int64_t)blockIdx.x * 256 + threadIdx.x) * 4;
   float m = 0.f;
   const int64_t b = a.prob_numel ? idx / a.prob_numel : 0;      // Batch: prob_numel is a multiple of 4 here
-  if (idx < a.numel && !batch_skips(a.active, b)) {
-    const int64_t row = idx / a.rowlen;
-    const int64_t off = row * a.ldp + (idx - row * a.rowlen);
+  PartialAt pa;      // the four elements share a row: a ragged batch's offsets and strides are multiples of R here
+  if (idx < a.numel && !batch_skips(a.active, b) && partial_at<RAGGED>(a, idx, b, pa)) {
+    const int64_t off = pa.off;
     const int r = (int)((idx / a.inner) % a.R);
     const float sc = a.out_scale ? *a.out_scale : 1.0f;
     float4 num = make_float4(0.f, 0.f, 0.f, 0.f);
-    for (int ch = 0; ch < a.nchunks; ++ch) {
-      const float4 t = *reinterpret_cast<const float4*>(a.num + ch * a.chunk_stride + off);
+    for (int ch = 0; ch < pa.nch; ++ch) {
+      const float4 t = *reinterpret_cast<const float4*>(a.num + ch * pa.stride + off);
       num.x += t.x; num.y += t.y; num.z += t.z; num.w += t.w;
     }
     float4 den = make_float4(0.f, 0.f, 0.f, 0.f);
     if (a.den) {
-      for (int ch = 0; ch < a.nchunks; ++ch) {
-        const float4 t = *reinterpret_cast<const float4*>(a.den + ch * a.chunk_stride + off);
+      for (int ch = 0; ch < pa.nch; ++ch) {
+        const float4 t = *reinterpret_cast<const float4*>(a.den + ch * pa.stride + off);
         den.x += t.x; den.y += t.y; den.z += t.z; den.w += t.w;
       }
     }
@@ -247,17 +290,20 @@ bool apply_update_vec4_shape(const ApplyArgs& a) {
 int apply_update(const ApplyArgs& a, cudaStream_t st) {
   if (a.numel <= 0) return 0;
   const bool vec4 = apply_update_vec4_shape(a) && aligned16(a.param) && aligned16(a.num) && (!a.den || aligned16(a.den));
-  if (vec4)
-    apply_update_vec4_kernel<<<(unsigned)ceil_div(a.numel / 4, 256), 256, 0, st>>>(a);
-  else
-    apply_update_kernel<<<(unsigned)ceil_div(a.numel, 256), 256, 0, st>>>(a);
+  const unsigned g4 = (unsigned)ceil_div(a.numel / 4, 256), g1 = (unsigned)ceil_div(a.numel, 256);
+  if (vec4 && a.rag) apply_update_vec4_kernel<true><<<g4, 256, 0, st>>>(a);
+  else if (vec4) apply_update_vec4_kernel<false><<<g4, 256, 0, st>>>(a);
+  else if (a.rag) apply_update_kernel<true><<<g1, 256, 0, st>>>(a);
+  else apply_update_kernel<false><<<g1, 256, 0, st>>>(a);
   NMF_LAUNCH_CHECK();
   return 0;
 }
 
 int raw_sum(const ApplyArgs& a, float* num_out, float* den_out, cudaStream_t st) {
   if (a.numel <= 0) return 0;
-  raw_sum_kernel<<<(unsigned)ceil_div(a.numel, 256), 256, 0, st>>>(a, num_out, a.den ? den_out : nullptr);
+  const unsigned g1 = (unsigned)ceil_div(a.numel, 256);
+  if (a.rag) raw_sum_kernel<true><<<g1, 256, 0, st>>>(a, num_out, a.den ? den_out : nullptr);
+  else raw_sum_kernel<false><<<g1, 256, 0, st>>>(a, num_out, a.den ? den_out : nullptr);
   NMF_LAUNCH_CHECK();
   return 0;
 }
@@ -271,9 +317,21 @@ static int64_t colsum_blocks(int64_t outer, int64_t inner) {
 int64_t colsum_scratch_floats(int64_t outer, int R, int64_t inner) { return colsum_blocks(outer, inner) * R; }
 
 int factor_colsum(const float* x, int64_t outer, int R, int64_t inner, float* scratch, int64_t scratch_floats,
-                  float* sums, cudaStream_t st, int64_t nprob, const uint8_t* active) {
+                  float* sums, cudaStream_t st, int64_t nprob, const uint8_t* active, const RaggedProblem* rag,
+                  int64_t rag_gx) {
   const int64_t nb = colsum_blocks(outer, inner);
   if (nprob < 1) { set_error("factor_colsum: bad problem count"); return 1; }
+  if (rag) {         // the scratch and grid were checked where the plans were made (nmfb200_nmf_batched_create_ragged)
+    if (inner != 1 || rag_gx < 1 || rag_gx > kMaxGridX || R > 256 || nprob > kMaxGridX / 4) {
+      set_error("factor_colsum: bad ragged batch");
+      return 1;
+    }
+    colsum_rows_kernel<true><<<(unsigned)rag_gx, 256, 0, st>>>(x, outer, R, 0, scratch, 0, active, rag, nprob);
+    NMF_LAUNCH_CHECK();
+    colsum_final_kernel<true><<<(unsigned)(ceil_div(R, 64) * nprob), 64, 0, st>>>(scratch, 0, R, sums, active, rag);
+    NMF_LAUNCH_CHECK();
+    return 0;
+  }
   if ((double)nb * R * nprob > (double)scratch_floats) { set_error("factor_colsum: scratch too small"); return 1; }
   if ((double)nb * (inner > 1 ? R : 1) * nprob > (double)kMaxGridX || ceil_div(R, 64) * nprob > kMaxGridX) {
     set_error("factor_colsum: batch passes grid x");
@@ -285,17 +343,17 @@ int factor_colsum(const float* x, int64_t outer, int R, int64_t inner, float* sc
     else colsum_runs_kernel<<<gx, 256, 0, st>>>(x, inner, scratch, outer * R, active);
   } else {
     const int64_t rpb = ceil_div(outer, nb);
-    colsum_rows_kernel<<<dim3((unsigned)(nb * nprob), (unsigned)ceil_div(R, 256)), 256, 0, st>>>(x, outer, R, rpb, scratch,
-                                                                                                  nb, active);
+    colsum_rows_kernel<false><<<dim3((unsigned)(nb * nprob), (unsigned)ceil_div(R, 256)), 256, 0, st>>>(
+        x, outer, R, rpb, scratch, nb, active, nullptr, nprob);
   }
   NMF_LAUNCH_CHECK();
-  colsum_final_kernel<<<(unsigned)(ceil_div(R, 64) * nprob), 64, 0, st>>>(scratch, nb, R, sums, active);
+  colsum_final_kernel<false><<<(unsigned)(ceil_div(R, 64) * nprob), 64, 0, st>>>(scratch, nb, R, sums, active, nullptr);
   NMF_LAUNCH_CHECK();
   return 0;
 }
 
 int matrix_minmax(const void* V, int vdtype, int64_t rows, int64_t cols, int64_t ld, float* scratch2048, float* mm,
-                  cudaStream_t st, CellSel M, int64_t nprob, int64_t bstride) {
+                  cudaStream_t st, CellSel M, int64_t nprob, int64_t bstride, const RaggedProblem* rag) {
   if (nprob < 1 || (nprob > 1 && M)) { set_error("matrix_minmax: a batch takes no selector"); return 1; }
   int64_t nb = ceil_div(nprob * rows * cols, 256 * 16);
   if (nb > 1024) nb = 1024;
@@ -304,7 +362,7 @@ int matrix_minmax(const void* V, int vdtype, int64_t rows, int64_t cols, int64_t
     using TV = vtype_t<decltype(Vt)>;
     return with_sel(M, [&](auto Mk) {
       minmax_stage1<TV, sel_t<decltype(Mk)>><<<(unsigned)nb, 256, 0, st>>>(Vt, rows, cols, ld, scratch2048, Mk, nprob,
-                                                                          bstride);
+                                                                          bstride, rag);
       NMF_LAUNCH_CHECK();
       return 0;
     });

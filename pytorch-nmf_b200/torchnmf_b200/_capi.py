@@ -42,6 +42,7 @@ SIGNATURES = {
     "nmfb200_nmf_cd_update": (_int, [_vp, _vp, _vp, _int, _dbl, _dbl, _vp]),
     "nmfb200_nmf_cd_iterate": (_int, [_vp, _vp, _vp, _dbl, _dbl, _int, _vp]),
     "nmfb200_nmf_batched_create": (_int, [_c.POINTER(_vp), _int, _i64, _i64, _i64, _i64]),
+    "nmfb200_nmf_batched_create_ragged": (_int, [_c.POINTER(_vp), _int, _i64, _i64, _i64, _i64, _c.POINTER(_i64)]),
     "nmfb200_nmf_batched_set_target": (_int, [_vp, _vp, _i64, _i64, _int, _vp]),
     "nmfb200_nmf_batched_set_active": (_int, [_vp, _vp, _vp]),
     "nmfb200_nmf_batched_cd_update": (_int, [_vp, _vp, _vp, _int, _dbl, _dbl, _vp]),

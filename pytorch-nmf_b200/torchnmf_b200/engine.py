@@ -66,11 +66,16 @@ def _workspace_bytes(key):
             p = _capi.nmf_plan(N, C, R)
             est += 8 * R * max(p["nch_w"] * C, p["nch_h"] * N)
         return est
-    if key[0] == "nmf_batched":           # ("nmf_batched", device, B, N, C, R): B x the fp32 context of one problem
-        _, _, B, N, C, R = key
-        p = _capi.nmf_plan(N, C, R)
-        return B * (8 * R * max(p["nch_w"] * C, p["nch_h"] * N) + 8 * R + 8 * p["loss_chunks"] * ((N + 63) // 64)
-                    + 4 * R * max(p["colsum_blocks_n"], p["colsum_blocks_c"])) + (1 << 14)
+    if key[0] == "nmf_batched":           # ("nmf_batched", device, B, N, C, R[, lengths]): B x the fp32 context of one problem
+        _, _, B, N, C, R = key[:6]        # with the lengths of a ragged batch: the sum of each problem's own context
+
+        def one(n):
+            p = _capi.nmf_plan(n, C, R)
+            return (8 * R * max(p["nch_w"] * C, p["nch_h"] * n) + 8 * R + 8 * p["loss_chunks"] * ((n + 63) // 64)
+                    + 4 * R * max(p["colsum_blocks_n"], p["colsum_blocks_c"]))
+        if len(key) > 6:
+            return sum(one(n) for n in key[6]) + 88 * B + (1 << 14)
+        return B * one(N) + (1 << 14)
     if key[0] == "nmfd_batched":          # ("nmfd_batched", device, P, B, C, X, R, K): P x the fp32 context of one problem
         _, _, P, B, C, X, R, K = key
         nx, nk, nh = 1, 1, 1
@@ -477,9 +482,17 @@ class CudaBatchedNmfEngine(_BatchedEngine):
     """B independent dense NMF problems of one shape on one GPU (include/nmf_b200.h: nmfb200_nmf_batched_create), on the
     fp32 kernels: V (B,N,C) -- or (N,C), one target shared by every problem -- fp32, fp16 or bf16 with unit column stride,
     rows and problems strided; W (B,C,R) and H (B,N,R) contiguous fp32, updated in place.  Every update and loss launch
-    runs all problems, and problem b's factors and loss are bit for bit those of CudaNmfEngine(V[b], W[b], H[b], "f32")."""
+    runs all problems, and problem b's factors and loss are bit for bit those of CudaNmfEngine(V[b], W[b], H[b], "f32").
+
+    `lengths` (B ints in [1, N], or None): a ragged batch (nmfb200_nmf_batched_create_ragged) -- problem b is the problem of
+    V[b, :lengths[b]], W[b] and H[b, :lengths[b]], bit for bit CudaNmfEngine(V[b, :L], W[b], H[b, :L], "f32"); the rows
+    past lengths[b] of V[b] are never read and those of H[b] never written.  No cd_update / cd_iterate then."""
     kind = "nmf_batched"
     _set_active = "nmfb200_nmf_batched_set_active"
+
+    def __init__(self, V, W, H, lengths=None):
+        self._lengths = None if lengths is None else tuple(int(n) for n in lengths)
+        super().__init__(V, W, H)
 
     def _create(self, V, W, H, dev_index):
         B, N, C = V.shape
@@ -487,8 +500,15 @@ class CudaBatchedNmfEngine(_BatchedEngine):
         assert W.shape == (B, C, R) and H.shape == (B, N, R)
         if not (V.stride(2) == 1 and V.stride(1) >= C and (V.stride(0) == 0 or V.stride(0) >= N * V.stride(1))):
             raise ValueError("V must have unit column stride, rows at least C apart and problems at least N rows apart")
-        self._acquire(("nmf_batched", dev_index, B, N, C, R),
-                      lambda ref: self._lib.nmfb200_nmf_batched_create(ref, dev_index, B, N, C, R))
+        if self._lengths is None:
+            self._acquire(("nmf_batched", dev_index, B, N, C, R),
+                          lambda ref: self._lib.nmfb200_nmf_batched_create(ref, dev_index, B, N, C, R))
+        else:
+            if len(self._lengths) != B:
+                raise ValueError(f"lengths holds {len(self._lengths)} values for {B} problems")
+            lens = (ctypes.c_int64 * B)(*self._lengths)
+            self._acquire(("nmf_batched", dev_index, B, N, C, R, self._lengths),
+                          lambda ref: self._lib.nmfb200_nmf_batched_create_ragged(ref, dev_index, B, N, C, R, lens))
         _capi.check(self._lib.nmfb200_nmf_batched_set_target(self._ctx, _ptr(V), V.stride(1), V.stride(0),
                                                              _capi.DTYPES[V.dtype], _stream(self.device)))
 

@@ -21,6 +21,7 @@ raw-terms launch, line-search losses from the fused loss launch, every component
 """
 import contextlib
 import math
+import numbers
 import weakref
 from collections.abc import Iterable as _Iterable
 
@@ -771,11 +772,13 @@ def _register_batched_factors(module, W, H, trainable_W, trainable_H):
 
 
 @contextlib.contextmanager
-def _placed_factors(module, factors, no_cuda):
+def _placed_factors(module, factors, no_cuda, rows=None):
     """Places a batched fit: yields (device, the fp32 contiguous tensors the engine updates, one per Parameter of
     `factors`).  They are the Parameters' own storages when every factor is fp32 and contiguous on a CUDA device, else
     device copies, written back into the Parameters when the block completes.  Without CUDA it raises
-    RuntimeError(no_cuda).  With the `_engine_factory` test hook the storages are taken where they are."""
+    RuntimeError(no_cuda).  With the `_engine_factory` test hook the storages are taken where they are.  `rows` (a bool
+    (problems, rows) tensor, or None): the rows of the second factor that are written back; the others are left as they
+    are (a ragged batch's padding)."""
     f32 = torch.float32
     if module._engine_factory is not None:
         dev, staged = factors[0].device, False
@@ -788,8 +791,11 @@ def _placed_factors(module, factors, no_cuda):
     placed = [t.data.to(dev, f32, non_blocking=True).contiguous() if staged else t.data for t in factors]
     yield dev, placed
     if staged:
-        for t, d in zip(factors, placed):
-            t.data.copy_(d)
+        for i, (t, d) in enumerate(zip(factors, placed)):
+            if i == 1 and rows is not None:
+                t.data[rows.to(t.device)] = d[rows.to(d.device)].to(t.device, t.dtype)
+            else:
+                t.data.copy_(d)
 
 
 def _fit_problems(eng, P, max_iter, tol, verbose, losses, step):
@@ -835,6 +841,7 @@ class _BatchedComponent(BaseComponent):
     own stop rule."""
     _ndim = 3                      # axes of W and of H
     _axes = "three axes (B, rows, rank)"
+    _ragged = False                # fit(..., lengths=L): BatchedNMF only
 
     def __init__(self, rank=None, W=None, H=None, trainable_W=True, trainable_H=True):
         torch.nn.Module.__init__(self)
@@ -852,8 +859,40 @@ class _BatchedComponent(BaseComponent):
     def sparse_fit(self, *args, **kwargs):
         raise NotImplementedError(f"{type(self).__name__} has no sparse_fit: fit each problem with the single model's sparse_fit")
 
+    def _check_lengths(self, V, lengths, cd):
+        """fit(..., lengths=L)'s checks, before any device work: the lengths as a list of B Python ints in [1, N]."""
+        name = type(self).__name__
+        if not self._ragged:
+            raise ValueError(f"lengths is supported by BatchedNMF only (got {name})")
+        if cd:
+            raise ValueError("lengths: solver='cd' does not fit ragged batches; use solver='mu'")
+        B, N = self.H.shape[:2]
+        if V.dim() != 3:
+            raise ValueError(f"lengths needs one target per problem, V of shape ({B}, N, C); a shared 2-D target has "
+                             f"one length")
+        if isinstance(lengths, Tensor):
+            if lengths.dtype.is_floating_point or lengths.dtype.is_complex or lengths.dtype == torch.bool:
+                raise ValueError(f"lengths must hold integers (got {lengths.dtype})")
+            if lengths.dim() != 1:
+                raise ValueError(f"lengths must be 1-D (got shape {tuple(lengths.shape)})")
+            lens = [int(n) for n in lengths.tolist()]
+        elif isinstance(lengths, _Iterable) and not isinstance(lengths, (str, bytes)):
+            lens = list(lengths)
+            if not all(isinstance(n, numbers.Integral) and not isinstance(n, bool) for n in lens):
+                raise ValueError("lengths must be a sequence of ints or an integer tensor")
+            lens = [int(n) for n in lens]
+        else:
+            raise ValueError(f"lengths must be a sequence of ints or an integer tensor (got {type(lengths).__name__})")
+        if len(lens) != B:
+            raise ValueError(f"lengths holds {len(lens)} values for {B} problems")
+        bad = [n for n in lens if not 1 <= n <= N]
+        if bad:
+            raise ValueError(f"every length must be in [1, N = {N}] (got {bad[0]})")
+        return lens
+
     @torch.no_grad()
-    def fit(self, V, beta=1, tol=1e-4, max_iter=200, verbose=False, alpha=0, l1_ratio=0, *, precision="auto", solver="mu"):
+    def fit(self, V, beta=1, tol=1e-4, max_iter=200, verbose=False, alpha=0, l1_ratio=0, *, precision="auto", solver="mu",
+            lengths=None):
         """Fit every problem by multiplicative updates, as the single model's `fit(V[p], ...)` fits one, all of them in the
         same launches.
 
@@ -882,11 +921,25 @@ class _BatchedComponent(BaseComponent):
         bit for bit, with the same per-problem stop rule.  The iterations between two loss checks run in one call when both
         factors train; a frozen factor leaves the other's updates one call each.  ValueError, before any device work: an
         unknown solver, "cd" with beta != 2, and "cd" on the convolutive batched models.
+
+        lengths: (BatchedNMF only, keyword-only, default None) B ints in [1, N], as a sequence or an integer tensor of shape
+        (B,) on any device: a ragged batch, problem b being the fit of V[b, :lengths[b]] with W[b] and H[b, :lengths[b]].
+        V (B, N, C) and H (B, N, R) stay padded.  n_iter[b], W[b] and H[b, :L_b] equal, bit for bit, those of
+        `NMF(W=W0[b], H=H0[b, :L_b]).fit(V[b, :L_b], ..., precision="f32")`, stop rule included: each problem runs the tile
+        plan of its own length.  Rows L_b: of H[b] are never written and rows L_b: of V[b] never read (NaN there does not
+        reach the fit); the non-negativity assertion and the beta <= 0 zero check look at the real rows only.  Every beta,
+        alpha / l1_ratio, frozen factors, fp16 / bf16 / strided targets and host or float64 modules work as without it;
+        lengths all equal to N give the bits of lengths=None.  The workspace is the sum of the problems' single-problem
+        workspaces.  ValueError, before any device work: the wrong number of lengths, a length outside [1, N], a
+        non-integer or non-1-D lengths, a shared 2-D target, solver="cd", and lengths on the convolutive batched models.
         """
         name = type(self).__name__
         if solver not in ("mu", "cd"):
             raise ValueError(f"solver must be 'mu' or 'cd' (got {solver!r})")
         cd = solver == "cd"
+        if lengths is not None:
+            assert self.W is not None and self.H is not None, "fit() needs both W and H"
+            lengths = self._check_lengths(V, lengths, cd)
         if cd:
             if not self._cd_solver:
                 raise ValueError(f"solver='cd' is supported by BatchedNMF only (got {name})")
@@ -905,16 +958,20 @@ class _BatchedComponent(BaseComponent):
         self._check_target_shape(V)
 
         no_cuda = "torchnmf_b200.fit needs a CUDA device (sm_90a); there is no CPU fallback"
-        with _placed_factors(self, (W, H), no_cuda) as (dev, (Wd, Hd)):
+        rows = None                # a ragged batch: the real rows of H, the only ones written back from a staged copy
+        if lengths is not None:
+            rows = torch.arange(H.shape[1]) < torch.tensor(lengths).unsqueeze(1)
+        ragged = {} if lengths is None else {"lengths": lengths}
+        with _placed_factors(self, (W, H), no_cuda, rows) as (dev, (Wd, Hd)):
             if self._engine_factory is None:
                 Vd = V.to(dev, non_blocking=True)
                 if Vd.dtype not in (torch.float32, torch.float16, torch.bfloat16):
                     Vd = Vd.to(torch.float32)
                 if not self._readable_in_place(Vd):
                     Vd = Vd.contiguous()
-                eng = self._engine_cls(Vd, Wd, Hd)
+                eng = self._engine_cls(Vd, Wd, Hd, **ragged)
             else:
-                eng = self._engine_factory(V, Wd, Hd)
+                eng = self._engine_factory(V, Wd, Hd, **ragged)
             try:
                 vmin, vmax = eng.minmax()
                 assert vmin >= 0., "Target should be non-negative."                        # nmf.py:329-330
@@ -965,6 +1022,9 @@ class BatchedNMF(_BatchedComponent):
     Workspace (device memory, kept between fits of the same shape like `NMF.fit`'s): B times that of one fp32 NMF problem
     -- the chunked partial numerators and denominators, 8 R max(nch_w C, nch_h N) bytes with up to 32 chunks per
     contraction (`_capi.nmf_plan(N, C, R)`), plus the column sums and loss partials -- so it grows linearly with B.
+    `fit(..., lengths=L)` fits a ragged batch: problem b is `NMF.fit(V[b, :L[b]], ..., precision="f32")` with W[b] and
+    H[b, :L[b]], V and H padded to N rows, each problem on the tile plan of its own length (see `fit`); its workspace is the
+    sum over the problems of one fp32 problem's of L[b] rows, not B times the largest.
     `fit(..., solver="cd")` fits each problem by coordinate descent (HALS) at beta 2, as `NMF.fit(V[b], 2, ...,
     precision="f32", solver="cd")`; it adds the Gram scratch, allocated at the first such fit, of 4 B (2 R^2 + max(nb(N),
     nb(C)) R^2) bytes, nb(rows) = ceil(rows / rpb) <= 128 Gram blocks of rpb = roundup(ceil(rows / 128), 32) rows
@@ -972,6 +1032,7 @@ class BatchedNMF(_BatchedComponent):
     """
     _engine_cls = _engine.CudaBatchedNmfEngine
     _cd_solver = True
+    _ragged = True
 
     def __init__(self, Vshape=None, rank=None, *, W=None, H=None, trainable_W=True, trainable_H=True):
         if isinstance(Vshape, _Iterable):
