@@ -463,6 +463,16 @@ int nmfb200_nmfd_plan(int64_t B, int64_t C, int ndim, const int64_t* vdims, int6
 #define NMFB200_NMFND_TC_PLAN_LEN 31
 int nmfb200_nmfnd_tc_plan(int64_t B, int64_t C, int ndim, const int64_t* vdims, int64_t R, const int64_t* kdims,
                           int64_t* out, int n);
+/* What the tensor-core contraction of a dense (N, C) rank-R NMF context (nmfb200_nmf_create) launches on a device with
+ * num_sms SMs, from the planner and the shared-memory layout those launches use; precision f16 or f16_split (auto plans as
+ * f16).  The kernel is persistent: grid CTAs, CTA b walks the work items b, b + grid, b + 2 grid, ... (item = chunk x
+ * row_blocks + row block).  NMFB200_ERR_INVALID for f32, sizes below 1, num_sms below 1, and shapes create refuses at f16.
+ * NMFB200_NMF_TC_PLAN_LEN values:
+ *   [0] TN, columns of V per tile   [1] NS, stages of the tile ring   [2] NF, F blocks (1 or 2) the producer loads ahead
+ *   [3..8] the W update (rows C, contracted over N): row blocks of 128, tiles, chunks, tiles per chunk (the last chunk
+ *   may be short), items, grid   [9..14] the same for the H update and the loss (rows N, contracted over C) */
+#define NMFB200_NMF_TC_PLAN_LEN 15
+int nmfb200_nmf_tc_plan(int64_t N, int64_t C, int64_t R, int precision, int num_sms, int64_t* out, int n);
 
 /* ---- sparseness-constrained NMF (Hoyer 2004) --------------------------------------------- */
 

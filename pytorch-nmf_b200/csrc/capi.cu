@@ -777,6 +777,18 @@ int nmfb200_nmfnd_tc_plan(int64_t B, int64_t C, int ndim, const int64_t* vdims, 
   return 0;
 }
 
+int nmfb200_nmf_tc_plan(int64_t N, int64_t C, int64_t R, int precision, int num_sms, int64_t* out, int n) {
+  if (!out || n < NMFB200_NMF_TC_PLAN_LEN) return fail(NMFB200_ERR_INVALID, "plan buffer too small");
+  if (N < 1 || C < 1 || R < 1) return fail(NMFB200_ERR_INVALID, "N, C, R must be positive");
+  if (num_sms < 1) return fail(NMFB200_ERR_INVALID, "num_sms must be positive");
+  if (precision != NMFB200_PREC_AUTO && precision != NMFB200_PREC_F16 && precision != NMFB200_PREC_F16_SPLIT)
+    return fail(NMFB200_ERR_INVALID, "the tensor-core plan needs precision f16, f16_split or auto");
+  if (!tc_shape_supported(N, C, R))
+    return fail(NMFB200_ERR_INVALID, "shape not supported by the tensor-core path (need R <= 128)");
+  tc_plan(N, C, R, precision == NMFB200_PREC_F16_SPLIT, num_sms, out);
+  return 0;
+}
+
 /* ---- both kinds: the mask or weights, and the terms of one factor update that every CUDA-core path runs on --- */
 
 namespace {

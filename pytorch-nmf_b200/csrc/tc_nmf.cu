@@ -1224,6 +1224,12 @@ Plan make_plan(int64_t Mr, int64_t Nc, int num_sms, int TN) {
   return pl;
 }
 
+// persistent CTAs of one contraction launch: one per SM, fewer when there are fewer items
+int plan_grid(const Plan& pl, int num_sms) {
+  const int items = pl.row_blocks * pl.nchunks;
+  return items < num_sms ? items : num_sms;
+}
+
 }  // namespace
 
 static PFN_cuTensorMapEncodeTiled_v12000 get_encode_fn() {
@@ -1593,8 +1599,7 @@ int launch_contract_t(TcState* s, int which, double beta, cudaStream_t st) {
   p.eg = which == 0 ? 2 : 1;
   p.loss_part = s->loss_part;
   p.kappa = s->kappa;
-  const int items = pl.row_blocks * pl.nchunks;
-  const int grid = items < s->num_sms ? items : s->num_sms;
+  const int grid = plan_grid(pl, s->num_sms);
   if (which == 0)
     kern<<<grid, kThreads, smem, st>>>(s->tmWf, s->tmHg, s->tmVt, p);
   else
@@ -1618,6 +1623,19 @@ int launch_contract_one(TcState* s, int which, double beta, cudaStream_t st) {
   }
   if (!s->split) return launch_contract_t<CfgFast128, BM, false>(s, which, beta, st);
   return launch_contract_t<CfgSplit128, BM, false>(s, which, beta, st);
+}
+
+// tc_plan for the configuration C: its layout, then each orientation's plan as launch_contract_t launches it
+template <class C>
+void tc_plan_cfg(int64_t N, int64_t Cols, int num_sms, int64_t* out) {
+  using L = SmemLayout<C::KW, C::TN>;
+  out[0] = C::TN; out[1] = L::NS; out[2] = L::NF;
+  const Plan pls[2] = {make_plan(Cols, N, num_sms, C::TN), make_plan(N, Cols, num_sms, C::TN)};
+  for (int k = 0; k < 2; ++k) {
+    int64_t* o = out + 3 + 6 * k;
+    o[0] = pls[k].row_blocks; o[1] = pls[k].tiles; o[2] = pls[k].nchunks; o[3] = pls[k].tpc;
+    o[4] = (int64_t)pls[k].row_blocks * pls[k].nchunks; o[5] = plan_grid(pls[k], num_sms);
+  }
 }
 
 // beta 1, W orientation, loss sums folded in (fast, non-split configurations)
@@ -1666,6 +1684,11 @@ int launch_contract(TcState* s, int which, double beta, cudaStream_t st) {
 }
 
 }  // namespace
+
+void tc_plan(int64_t N, int64_t C, int64_t R, bool split, int num_sms, int64_t* out) {
+  if (R <= 64) return split ? tc_plan_cfg<CfgSplit64>(N, C, num_sms, out) : tc_plan_cfg<CfgFast64>(N, C, num_sms, out);
+  return split ? tc_plan_cfg<CfgSplit128>(N, C, num_sms, out) : tc_plan_cfg<CfgFast128>(N, C, num_sms, out);
+}
 
 int tc_update(TcState* s, int which, float* param, const float* W, const float* H, double beta, double gamma, double l1,
               double l2, cudaStream_t st) {

@@ -8,6 +8,9 @@ struct TcState;
 
 // shapes the wgmma kernels accept (rank padded to 64 or 128 columns)
 bool tc_shape_supported(int64_t N, int64_t C, int64_t R);
+// host only: the contraction kernel's layout and launch plan of a supported (N, C, R) shape on num_sms SMs, the
+// NMFB200_NMF_TC_PLAN_LEN values of nmfb200_nmf_tc_plan
+void tc_plan(int64_t N, int64_t C, int64_t R, bool split, int num_sms, int64_t* out);
 int tc_create(TcState** out, int device, int64_t N, int64_t C, int64_t R, bool split);
 void tc_destroy(TcState* s);
 bool tc_supports_beta(const TcState* s, double beta);

@@ -81,8 +81,10 @@ SIGNATURES = {
     "nmfb200_nmfd_plan": (_int, [_i64, _i64, _int, _c.POINTER(_i64), _i64, _c.POINTER(_i64), _c.POINTER(_i64), _int]),
     "nmfb200_nmf_sparse_plan": (_int, [_i64, _i64, _i64, _c.POINTER(_i64), _int]),
     "nmfb200_nmfnd_tc_plan": (_int, [_i64, _i64, _int, _c.POINTER(_i64), _i64, _c.POINTER(_i64), _c.POINTER(_i64), _int]),
+    "nmfb200_nmf_tc_plan": (_int, [_i64, _i64, _i64, _int, _int, _c.POINTER(_i64), _int]),
 }
 NMF_PLAN_LEN, NMFD_PLAN_LEN, SPARSE_PLAN_LEN, NMFND_TC_PLAN_LEN = 9, 19, 8, 31         # include/nmf_b200.h
+NMF_TC_PLAN_LEN = 15                                                                    # include/nmf_b200.h
 PLCA_TRAIN_W, PLCA_TRAIN_H, PLCA_TRAIN_Z = 1, 2, 4                                       # include/nmf_b200.h
 
 _lib = None
@@ -167,3 +169,19 @@ def nmfnd_tc_plan(B, C, vdims, R, kdims):
             "dgrad": tuple(v[12:15]), "bslice": v[15], "slices": v[16], "dgrad_rblocks": v[17], "loss_blocks": v[18],
             "ws_w": v[19], "kbs_w": v[20], "ws_h": v[21], "kbs_h": v[22], "hslice": v[23], "hslices": v[24],
             "Tp": v[25], "padl": v[26], "Lp": v[27], "Lq": v[28], "Cpad": v[29], "nch": v[30]}
+
+
+def nmf_tc_plan(N, C, R, precision, num_sms):
+    """The tensor-core contraction's layout and launch plan of an (N, C) rank-R NMF context on a device with `num_sms` SMs
+    (nmfb200_nmf_tc_plan), as a dict; no device needed.  `tn`, `ns`, `nf`: tile width, ring stages, F slots; then per
+    orientation (`_w`: rows C over N, `_h`: rows N over C) `row_blocks`, `tiles`, `nchunks`, `tpc`, `items`, `grid`.
+    `precision` is a name of PRECISIONS or its value; raises NmfB200Error for f32 and for shapes the f16 path refuses."""
+    prec = PRECISIONS[precision] if isinstance(precision, str) else int(precision)
+    out = (_i64 * NMF_TC_PLAN_LEN)()
+    check(load().nmfb200_nmf_tc_plan(N, C, R, prec, num_sms, out, NMF_TC_PLAN_LEN))
+    v = list(out)
+    keys = ("row_blocks", "tiles", "nchunks", "tpc", "items", "grid")
+    plan = {"tn": v[0], "ns": v[1], "nf": v[2]}
+    plan.update({f"{k}_w": x for k, x in zip(keys, v[3:9])})
+    plan.update({f"{k}_h": x for k, x in zip(keys, v[9:15])})
+    return plan
