@@ -294,6 +294,24 @@ int nmfb200_nmfd_set_target(nmfb200_ctx* ctx, const void* V, int dtype, void* st
  * nmfb200_nmf_* call return NMFB200_ERR_INVALID.  The two calls below take batched NMFD contexts only. */
 int nmfb200_nmfnd_batched_create(nmfb200_ctx** out, int device, int64_t P, int64_t B, int64_t C, int ndim,
                                  const int64_t* vdims, int64_t R, const int64_t* kdims);
+/* A batch of P problems of different lengths along the LAST convolved axis (the sliding axis): problem p has lengths[p]
+ * (T <= lengths[p] <= L, T = kdims[ndim - 1] and L = vdims[ndim - 1]; `lengths` is P host int64, read during the call)
+ * positions there, stored in the same padded layouts as a nmfb200_nmfnd_batched_create context's of vdims -- V_p's first
+ * lengths[p] positions of every line of the last axis, W_p as there, and H_p's first lengths[p] - T + 1 positions of every
+ * line of its last axis (L - T + 1 long).  Every call that serves a batched NMFD context serves it, with these differences:
+ *   - problem p runs, bit for bit, the plan of a single NMFB200_PREC_F32 context of (B, C, vdims with the last size
+ *     lengths[p], R, kdims): its own reconstruction grid and loss blocks, dgrad splits and column-sum blocking, each launch
+ *     sized for the largest problem, a problem's surplus blocks exiting at once;
+ *   - no call reads positions lengths[p].. of V_p or lengths[p] - T + 1.. of H_p, and no call writes the latter (nor those
+ *     positions of nmfb200_raw_terms' output);
+ *   - nmfb200_target_minmax covers every problem's real positions (of a shared target too);
+ *   - nmfb200_plca_iterate and nmfb200_plca_loss return NMFB200_ERR_INVALID.
+ * Workspace: the sum over the problems of a single context's ratio tiles, split partial slabs, column-sum and loss
+ * partials, not P times the largest.  NMFB200_ERR_INVALID, before any device work, for whatever
+ * nmfb200_nmfnd_batched_create refuses at the padded shape, a null `lengths`, a length outside [T, L], and P x B x R
+ * past grid x (2^31 - 1). */
+int nmfb200_nmfnd_batched_create_ragged(nmfb200_ctx** out, int device, int64_t P, int64_t B, int64_t C, int ndim,
+                                        const int64_t* vdims, int64_t R, const int64_t* kdims, const int64_t* lengths);
 /* Register the targets: problem p reads the contiguous block V + p problem_stride of B C prod(vdims) elements of type
  * `dtype`.  problem_stride 0: one V shared by every problem (restarts of one fit); otherwise problem_stride >=
  * B C prod(vdims).  Checks as nmfb200_nmfd_set_target; the min / max run over every problem.  V stays borrowed.

@@ -69,9 +69,10 @@ struct nmfb200_ctx {
   double sp_vnorm_kl = 0.0, sp_vnorm_eu = 0.0;
   float* sp_gram = nullptr;       // [2][R*R] (W^T W, H^T H) + per-block partials; also the Gram scratch of nmfb200_nmf_cd_*
   double* sp_loss_part = nullptr;
-  // NMFD
+  // NMFD: the ratio tiles, pn_floats each (a batch: every problem's, back to back)
   float* Pn = nullptr;
   float* Pp = nullptr;
+  int64_t pn_floats = 0;
   // nmfb200_plca_masked_terms on NMF: one q_O partial per block of the fp32 contraction (grown on demand)
   double* qobs_part = nullptr;
   int64_t qobs_part_n = 0;
@@ -184,6 +185,7 @@ int alloc_workspace(nmfb200_ctx* c, int64_t pn_floats) {
   if (e == cudaSuccess) e = cudaMalloc(&c->loss_blocks, (size_t)c->loss_max_blocks * sizeof(double));
   if (e == cudaSuccess) e = cudaMalloc(&c->mm_scratch, kMmFloats * sizeof(float));
   if (e == cudaSuccess && pn_floats) e = cudaMalloc(&c->Pn, pn_floats * sizeof(float));
+  c->pn_floats = pn_floats;
   if (e != cudaSuccess) {
     free_ctx(c);
     return fail(NMFB200_ERR_CUDA, std::string("cudaMalloc: ") + cudaGetErrorString(e));
@@ -227,6 +229,7 @@ ApplyArgs factor_view(const nmfb200_ctx* c, int which, int nchunks) {
   a.numel = f.rows * a.rowlen * c->nprob; a.chunk_stride = a.numel; a.nchunks = nchunks;
   if (is_batch(c)) { a.prob_numel = f.rows * a.rowlen; a.active = c->active; }
   if (c->rag) { a.rag = c->rag; a.rag_launch = which == 0 ? kRagW : kRagH; }
+  if (c->rag && is_nmfd(c) && which == 1) a.line = c->d.Lin;      // a ragged NMFD batch's H: padding inside every line
   return a;
 }
 
@@ -469,7 +472,7 @@ int nmfb200_nmf_batched_create_ragged(nmfb200_ctx** out, int device, int64_t B, 
     p.cs_blocks = (int)colsum_scratch_floats(L, 1, 1);
     const int64_t blocks[4] = {w_blocks * p.nch[0], ceil_div(L, 64) * p.nch[1], ceil_div(L, 64) * p.loss_chunks, p.cs_blocks};
     for (int k = 0; k < 4; ++k) { p.x0[k] = gx[k]; gx[k] += blocks[k]; }
-    p.part = part; p.loss_part = loss; p.cs_part = cs;
+    p.part = part; p.loss_part = loss; p.cs_part = cs; p.loss_n = blocks[2];
     part += std::max((int64_t)p.nch[0] * C * R, (int64_t)p.nch[1] * L * R);
     loss += blocks[2];
     cs += p.cs_blocks * R;
@@ -687,10 +690,10 @@ int nmfb200_nmfd_set_target(nmfb200_ctx* ctx, const void* V, int dtype, void* st
 
 /* ---- batched NMFD / NMF2D / NMF3D: P independent problems of one shape on the fp32 kernels ------------------------ */
 
-int nmfb200_nmfnd_batched_create(nmfb200_ctx** out, int device, int64_t P, int64_t B, int64_t C, int ndim,
-                                 const int64_t* vdims, int64_t R, const int64_t* kdims) {
-  if (!out) return fail(NMFB200_ERR_INVALID, "out is null");
-  *out = nullptr;
+namespace {
+// The shape of a batch of P NMFD problems (validated): what every problem's launches and counts must fit.
+int batched_nmfd_shape_of(int64_t P, int64_t B, int64_t C, int ndim, const int64_t* vdims, int64_t R, const int64_t* kdims,
+                          NmfdShape* out) {
   if (P < 1) return fail(NMFB200_ERR_INVALID, "P must be positive");
   NmfdShape d;
   if (int rc = nmfd_shape_of(B, C, ndim, vdims, R, kdims, &d)) return rc;
@@ -706,6 +709,19 @@ int nmfb200_nmfnd_batched_create(nmfb200_ctx** out, int device, int64_t P, int64
       (double)(d.h_inner() > 1 ? cs_h : cs_h / R) * P > (double)kMaxGridX || ceil_div(R, 64) * P > kMaxGridX)
     return fail(NMFB200_ERR_INVALID, "batched NMFD: P x column-sum blocks must be below 2^31 (grid x of the column sums)");
   if ((double)vol * P > (double)((int64_t)1 << 46)) return fail(NMFB200_ERR_INVALID, "batched NMFD: targets too large");
+  *out = d;
+  return 0;
+}
+}  // namespace
+
+int nmfb200_nmfnd_batched_create(nmfb200_ctx** out, int device, int64_t P, int64_t B, int64_t C, int ndim,
+                                 const int64_t* vdims, int64_t R, const int64_t* kdims) {
+  if (!out) return fail(NMFB200_ERR_INVALID, "out is null");
+  *out = nullptr;
+  NmfdShape d;
+  if (int rc = batched_nmfd_shape_of(P, B, C, ndim, vdims, R, kdims, &d)) return rc;
+  const int64_t vol = B * C * d.v_inner();
+  const int64_t cs_w = colsum_scratch_floats(C, (int)R, d.w_inner()), cs_h = colsum_scratch_floats(B, (int)R, d.h_inner());
   DeviceGuard guard(device);
   if (!guard.ok) return fail(NMFB200_ERR_CUDA, "cannot select the requested device");
   nmfb200_ctx* c = new (std::nothrow) nmfb200_ctx();
@@ -725,6 +741,68 @@ int nmfb200_nmfnd_batched_create(nmfb200_ctx** out, int device, int64_t P, int64
   return 0;
 }
 
+int nmfb200_nmfnd_batched_create_ragged(nmfb200_ctx** out, int device, int64_t P, int64_t B, int64_t C, int ndim,
+                                        const int64_t* vdims, int64_t R, const int64_t* kdims, const int64_t* lengths) {
+  if (!out) return fail(NMFB200_ERR_INVALID, "out is null");
+  *out = nullptr;
+  NmfdShape d;
+  if (int rc = batched_nmfd_shape_of(P, B, C, ndim, vdims, R, kdims, &d)) return rc;
+  if (!lengths) return fail(NMFB200_ERR_INVALID, "lengths is null");
+  if ((double)B * R * P > (double)kMaxGridX)
+    return fail(NMFB200_ERR_INVALID, "ragged NMFD batch: P x B x R must be below 2^31 (grid x of the column sums of H)");
+  // each problem's single-problem plan along its own length, its workspace after the previous problems'.  Every count is
+  // at most the padded shape's, which the checks above bound for P problems.
+  std::vector<RaggedProblem> t(P);
+  const int64_t wpart = (int64_t)nmfd_wgrad_nsplit(d) * C * R * d.w_inner();
+  int64_t pn = 0, part = 0, loss = 0, cs = 0;
+  int dgrad_nsplit = 1;
+  for (int64_t p = 0; p < P; ++p) {
+    const int64_t L = lengths[p];
+    if (L < d.T || L > d.L)
+      return fail(NMFB200_ERR_INVALID, "lengths[" + std::to_string(p) + "] = " + std::to_string(L) + " is outside [" +
+                                           std::to_string(d.T) + ", " + std::to_string(d.L) + "] (the last kernel and target sizes)");
+    NmfdShape e = d;
+    e.L = (int)L; e.Lin = (int)(L - d.T + 1);
+    NmfdPlan plan;
+    nmfd_plan(e, &plan);
+    RaggedProblem& q = t[p];
+    q.rows = L; q.lin = e.Lin;
+    q.gx[0] = (int)plan.recon_grid.x; q.gx[1] = (int)plan.dgrad_grid.x;
+    q.nch[0] = plan.wgrad_nsplit; q.nch[1] = plan.dgrad_nsplit;
+    q.loss_n = nmfd_max_blocks(e);
+    // the column sums of H at beta 1 as its single fit forms them: one partial per (clip, component) run, or the rows
+    // blocking of a run of one element
+    q.cs_blocks = (int)(e.h_inner() > 1 ? B : colsum_scratch_floats(B, 1, 1));
+    q.pn = pn; q.part = part; q.loss_part = loss; q.cs_part = cs;
+    dgrad_nsplit = std::max(dgrad_nsplit, plan.dgrad_nsplit);
+    // every problem's tiles and slabs start 16-byte aligned: the ratio stage of W reads its slabs as float4 (update.cu:
+    // apply_update_vec4_kernel) wherever the shape allows, and a dgrad slab may hold any number of floats
+    pn += round_up(B * C * e.v_inner(), 4);
+    part += round_up(std::max(wpart, (int64_t)plan.dgrad_nsplit * B * R * e.h_inner()), 4);
+    loss += q.loss_n;
+    cs += B * R;
+  }
+  DeviceGuard guard(device);
+  if (!guard.ok) return fail(NMFB200_ERR_CUDA, "cannot select the requested device");
+  nmfb200_ctx* c = new (std::nothrow) nmfb200_ctx();
+  if (!c) return fail(NMFB200_ERR_INVALID, "out of host memory");
+  c->kind = kBatchedNmfd; c->device = device; c->precision = NMFB200_PREC_F32; c->R = R; c->d = d; c->nprob = P;
+  c->nslab[0] = nmfd_wgrad_nsplit(d);
+  c->nslab[1] = dgrad_nsplit;            // the dgrad launch's grid y; each problem runs its own splits
+  c->part_floats = part;
+  c->cs_scratch_floats = std::max(cs, colsum_scratch_floats(C, (int)R, d.w_inner()) * P);
+  c->loss_max_blocks = (int)loss;
+  if (int rc = alloc_workspace(c, pn)) return rc;
+  cudaError_t e = cudaMalloc(&c->rag, (size_t)P * sizeof(RaggedProblem));
+  if (e == cudaSuccess) e = cudaMemcpy(c->rag, t.data(), (size_t)P * sizeof(RaggedProblem), cudaMemcpyHostToDevice);
+  if (e != cudaSuccess) {
+    free_ctx(c);
+    return fail(NMFB200_ERR_CUDA, std::string("ragged batch plans: ") + cudaGetErrorString(e));
+  }
+  *out = c;
+  return 0;
+}
+
 int nmfb200_nmfd_batched_set_target(nmfb200_ctx* ctx, const void* V, int64_t problem_stride, int dtype, void* stream) {
   CTX_GUARD(ctx, kBatchedNmfd);
   if (int rc = check_target(V, dtype)) return rc;
@@ -732,6 +810,9 @@ int nmfb200_nmfd_batched_set_target(nmfb200_ctx* ctx, const void* V, int64_t pro
   if (problem_stride != 0 && problem_stride < rows * vin)
     return fail(NMFB200_ERR_INVALID, "problem stride must be 0 (one shared target) or at least B x C x prod(X)");
   ctx->V = V; ctx->vdtype = dtype; ctx->bstride = problem_stride; ctx->has_target = true;
+  if (ctx->rag)           // a ragged batch: every problem's real positions of each line, even of a shared target
+    return matrix_minmax(V, dtype, rows * (vin / ctx->d.L), ctx->d.L, ctx->d.L, ctx->mm_scratch, ctx->mm_scratch + kMmPartials,
+                         (cudaStream_t)stream, CellSel{}, ctx->nprob, problem_stride, ctx->rag, true);
   return matrix_minmax(V, dtype, rows, vin, vin, ctx->mm_scratch, ctx->mm_scratch + kMmPartials, (cudaStream_t)stream,
                        CellSel{}, problem_stride ? ctx->nprob : 1, problem_stride);
 }
@@ -882,12 +963,14 @@ int simt_contract(nmfb200_ctx* c, int which, const float* W, const float* H, dou
 int nmfd_contract(nmfb200_ctx* c, int which, const float* W, const float* H, double beta, cudaStream_t st) {
   const bool den = !kl_colsum(c, beta);
   if (den) {
-    if (!c->Pp) NMF_CUDA_CHECK(cudaMalloc(&c->Pp, (size_t)c->d.B * c->d.C * c->d.v_inner() * c->nprob * sizeof(float)));
+    if (!c->Pp) NMF_CUDA_CHECK(cudaMalloc(&c->Pp, (size_t)c->pn_floats * sizeof(float)));
     int e = ensure_den(c);
     if (e) return e;
   }
-  // a batch: every problem's tiles and split partials in the same launches (slab layout [split][problem][rows][R][inner])
-  const Batch bt{c->nprob, c->bstride, 0, 0, 0, c->active};
+  // a batch: every problem's tiles and split partials in the same launches (slab layout [split][problem][rows][R][inner]; a
+  // ragged batch: each problem's own [split][rows][R][inner] at its offset)
+  Batch bt{c->nprob, c->bstride, 0, 0, 0, c->active};
+  bt.rag = c->rag;
   int rc = nmfd_recon_phi(c->d, c->V, c->vdtype, W, H, beta, c->Pn, c->Pp, nullptr, 0, nullptr, st, c->sel, bt);
   auto grad = [&](const float* P, float* out) {
     return which == 0 ? nmfd_wgrad(c->d, P, H, out, c->nslab[0], st, bt) : nmfd_dgrad(c->d, P, W, out, c->nslab[1], st, bt);
@@ -937,9 +1020,10 @@ int factor_terms(nmfb200_ctx* c, int which, const float* W, const float* H, doub
   if (!kl) { a.den = c->den; return 0; }
   a.kl_den = den_out;
   const FactorDims f = factor_dims(c, which);
-  const bool rag_h = c->rag && which == 0;        // a ragged batch's H: each problem's own rows
+  const bool rag_h = c->rag && which == 0;        // a ragged batch's H: each problem's own rows (NMFD: line positions)
   return factor_colsum(fac[1 - which], f.other_rows, (int)c->R, f.other_inner, c->cs_scratch, c->cs_scratch_floats, den_out,
-                       st, c->nprob, c->active, rag_h ? c->rag : nullptr, rag_h ? c->rag_gx[kRagColsum] : 0);
+                       st, c->nprob, c->active, rag_h ? c->rag : nullptr, rag_h ? c->rag_gx[kRagColsum] : 0,
+                       rag_h && is_nmfd(c) ? c->d.Lin : 0);
 }
 
 // One factor update (which = 0: param = W, 1: param = H) on the kernels that serve this context and beta.  No device guard:
@@ -1112,8 +1196,10 @@ int nmfb200_loss(nmfb200_ctx* ctx, const float* W, const float* H, double beta, 
   cudaStream_t st = (cudaStream_t)stream;
   if (is_nmfd(ctx)) {       // a batch: loss_dev[b] for every active problem b
     if (use_tc(ctx, beta)) return tc_nmfd_recon(ctx->tcd, ctx->V, ctx->vdtype, W, H, true, loss_dev, st);
+    Batch bt{ctx->nprob, ctx->bstride, 0, 0, 0, ctx->active};
+    bt.rag = ctx->rag;
     return nmfd_recon_phi(ctx->d, ctx->V, ctx->vdtype, W, H, beta, nullptr, nullptr, ctx->loss_blocks, ctx->loss_max_blocks,
-                          loss_dev, st, ctx->sel, Batch{ctx->nprob, ctx->bstride, 0, 0, 0, ctx->active});
+                          loss_dev, st, ctx->sel, bt);
   }
   if (ctx->sparse) return sparse_loss_ctx(ctx, W, H, beta, loss_dev, st);
   if (use_tc(ctx, beta)) return tc_loss(ctx->tc, W, H, beta, loss_dev, st);

@@ -66,16 +66,26 @@ int with_sel(CellSel s, F&& f) {
 // the padded (B, N, ...) layouts of V and H.  It runs the plan of a single problem of N_b rows: its own chunk counts, loss
 // chunks and column-sum blocks, and its partials laid out as that problem's, at its own offsets in the shared buffers.  Its
 // blocks of each launch below start at x0[launch] on grid x and run up to the next problem's (x0 ascends with b).
+// A ragged batch of NMFD / NMF2D / NMF3D problems (nmfb200_nmfnd_batched_create_ragged) uses the same table: `rows` is then
+// L_p, the problem's length along the sliding axis of the padded (P, B, C, *X) target, and `lin` = L_p - T + 1 its
+// activation positions there.  Its launches put the problems' lines on grid z (no x0, no search): each sizes grid x / y for
+// the largest problem, and a problem's blocks past its own grid x (gx) or dgrad splits (nch[1]) exit at once.  Its ratio
+// tiles Pn / Pp are the single problem's (B, C, *X[:-1], L_p) at `pn`, its wgrad / dgrad split slabs ([split][C, R, K] /
+// [split][B, R, *J[:-1], lin]) at `part`, its loss partials at `loss_part` and its column-sum partials of H at `cs_part`.
 enum RaggedLaunch : int { kRagW = 0, kRagH = 1, kRagLoss = 2, kRagColsum = 3 };
 struct RaggedProblem {
-  int64_t rows;           // N_b
+  int64_t rows;           // N_b (NMFD: L_p)
   int64_t x0[4];          // first block on grid x of the W and H contractions, the loss and the column sums of H
   int64_t part;           // floats before its partial slabs ([chunk][rows][R], rows = C for W and N_b for H)
   int64_t loss_part;      // doubles before its loss partials ([chunk][row block])
   int64_t cs_part;        // floats before its column-sum partials of H ([block][R])
-  int nch[2];             // contraction chunks of its W / H update
+  int64_t loss_n;         // its loss partials
+  int nch[2];             // contraction chunks of its W / H update (NMFD: wgrad / dgrad splits)
   int loss_chunks;
   int cs_blocks;          // column-sum blocks over its rows
+  int64_t pn;             // NMFD: floats before its ratio tiles
+  int lin;                // NMFD: L_p - T + 1
+  int gx[2];              // NMFD: grid x of its recon (FWD) and dgrad slides
 };
 // the problem of a ragged batch's n whose blocks of `launch` hold grid-x block bx: the last one with x0[launch] <= bx
 __device__ __forceinline__ int64_t ragged_problem(const RaggedProblem* t, int64_t n, int launch, int64_t bx) {
@@ -285,6 +295,10 @@ struct ApplyArgs {
   // H past rag[b].rows are padding: left untouched.
   const RaggedProblem* rag = nullptr;
   int rag_launch = 0;
+  // a ragged NMFD batch's H (kRagH): the padded length of the sliding axis, the last of H's (R, *J) inner axes.  Element
+  // (line, j) of problem b is real for j < rag[b].lin, its partials at rag[b].part + line rag[b].lin + j in slabs of the
+  // problem's compact size; the others are padding, left untouched.  0: the layout above
+  int64_t line = 0;
 };
 int apply_update(const ApplyArgs& a, cudaStream_t st);
 // whether apply_update takes its four-elements-per-thread kernel for this shape (16-byte aligned buffers provided)
@@ -295,20 +309,23 @@ int raw_sum(const ApplyArgs& a, float* num_out, float* den_out, cudaStream_t st)
 // nprob consecutive (outer, R, inner) problems, each summed in the single problem's order, skipping those whose `active`
 // flag is 0; scratch_floats then covers nprob x colsum_scratch_floats.  rag (inner 1; a ragged batch's table): problem b
 // sums its rag[b].rows rows of its (outer, R) block on its own rag[b].cs_blocks blocks, partials at rag[b].cs_part; rag_gx
-// is their sum.
+// is their sum.  rag with rag_line (a ragged NMFD batch's H, inner > 1, its last axis rag_line long): problem b sums the
+// first rag[b].lin positions of every line, in the order and blocking of a single problem's inner = inner / rag_line
+// rag[b].lin (rows blocking when that is 1), partials at rag[b].cs_part.
 int factor_colsum(const float* x, int64_t outer, int R, int64_t inner, float* scratch, int64_t scratch_floats,
                   float* sums, cudaStream_t st, int64_t nprob = 1, const uint8_t* active = nullptr,
-                  const RaggedProblem* rag = nullptr, int64_t rag_gx = 0);
+                  const RaggedProblem* rag = nullptr, int64_t rag_gx = 0, int64_t rag_line = 0);
 int64_t colsum_scratch_floats(int64_t outer, int R, int64_t inner);
 // min / max of a strided matrix of `vdtype` elements (fit()'s validation), results in mm[0..1]; with M (optional, contiguous
 // rows x cols selector) over the cells where M is non-zero only (none: +inf / -inf).  nprob > 1: over nprob such matrices,
-// `bstride` elements apart (no selector); rag (a ragged batch's table): matrix b's first rag[b].rows rows only.
+// `bstride` elements apart (no selector); rag (a ragged batch's table): matrix b's first rag[b].rows rows only, or with
+// rag_cols its first rag[b].rows columns (a ragged NMFD batch: the real positions of every line of the sliding axis).
 int matrix_minmax(const void* V, int vdtype, int64_t rows, int64_t cols, int64_t ld, float* scratch2048, float* mm,
                   cudaStream_t st, CellSel M = CellSel{}, int64_t nprob = 1, int64_t bstride = 0,
-                  const RaggedProblem* rag = nullptr);
+                  const RaggedProblem* rag = nullptr, bool rag_cols = false);
 // *out = sum of n doubles in fixed order (single block).  nprob > 1: out[b] = the sum of p[b n, (b + 1) n), one block per
 // problem, in the same order; a problem whose `active` flag is 0 keeps its out[b].  rag (a ragged batch's table): problem
-// b's run is its own simt_nmf_loss partials at rag[b].loss_part (n is not read).
+// b's run is its own rag[b].loss_n loss partials at rag[b].loss_part (n is not read).
 int sum_partials(const double* p, int n, double* out, cudaStream_t st, int64_t nprob = 1, const uint8_t* active = nullptr,
                  const RaggedProblem* rag = nullptr);
 
@@ -377,6 +394,9 @@ struct NmfdShape {
 // at V + b bt.v (0: one shared target) and its W, H, Pn, Pp in the b-th block of (bt.n, ...) storages; loss_dev[b] from its
 // own run of partials summed in the single problem's order.  Problems whose bt.active flag is 0 are skipped: their factors'
 // terms and loss_dev slots are left as they are.  The kernels derive bt.f / bt.g / bt.p from s; the caller's are not read.
+// bt.rag (a ragged batch, s its padded shape): problem b runs the plan of its own length rag[b].rows along the sliding
+// axis, reads V and H in their padded layouts up to that length and writes its tiles and loss partials at its own offsets
+// (RaggedProblem); so do nmfd_wgrad and nmfd_dgrad, nsplit then the largest problem's.
 int nmfd_recon_phi(const NmfdShape& s, const void* V, int vdtype, const float* W, const float* H, double beta,
                    float* Pn, float* Pp, double* loss_blocks, int max_blocks, double* loss_dev,
                    cudaStream_t st, CellSel M = CellSel{}, const Batch& bt = Batch{});

@@ -75,6 +75,11 @@ struct Geo {
 // problem.  A block of problem `prob` reads A + prob bt.f, X + prob bt.g and its target at V + prob bt.v, writes its Pn / Pp
 // (FWD) or its dgrad partials at + prob bt.p (the dgrad slab of one split holds every problem's) and its loss partials as
 // the contiguous run a single launch of that problem writes; otherwise it runs the single problem's plan and arithmetic.
+// RAGGED (BATCH, bt.rag; s the padded shape): problem `prob` runs the plan of its own lengths rag[prob].rows / .lin along
+// the sliding axis.  It reads H (FWD) and V in their padded layouts up to those lengths, and the ratio tiles (!FWD) in its
+// own compact layout at + rag[prob].pn; it writes its Pn / Pp there, its dgrad partials at + rag[prob].part in the single
+// problem's [split][B][R][h_inner] layout and its loss partials at + rag[prob].loss_part.  Its blocks past its own grid x
+// (rag[prob].gx) or dgrad splits (rag[prob].nch[1]) exit at once.
 struct SlideArgs {
   const float* A;            // W
   const float* X;            // H (FWD) or G
@@ -93,7 +98,7 @@ struct SlideArgs {
 // kPlcaFill (FWD, !LOSS, fp32 V, the uint8 mask, one problem; a masked PLCA fit): Pn = V / (WH + eps) and Pp = 0 at an
 // observed cell, Pn = 0 and Pp = WH / (WH + eps) at a missing one (V not read), and, when a.block_partials is set, each
 // block's sum of WH over its observed cells into the loss partial the LOSS pass of this launch would write.
-template <int MT, bool FWD, int MODE, bool LOSS, typename TV, typename SEL = NoSel, bool BATCH = false>
+template <int MT, bool FWD, int MODE, bool LOSS, typename TV, typename SEL = NoSel, bool BATCH = false, bool RAGGED = false>
 __global__ void __launch_bounds__(256)
 nmfd_slide_kernel(NmfdShape s, SlideArgs a, Batch bt) {
   constexpr bool MASK = !std::is_same<SEL, NoSel>::value;
@@ -101,7 +106,20 @@ nmfd_slide_kernel(NmfdShape s, SlideArgs a, Batch bt) {
   constexpr bool FILL = (MODE == kPlcaFill);
   static_assert(!FILL || (FWD && !LOSS && std::is_same<SEL, uint8_t>::value && std::is_same<TV, float>::value && !BATCH),
                 "kPlcaFill: the FWD pass of one problem, fp32 V, the uint8 mask");
+  static_assert(!RAGGED || BATCH, "RAGGED: a batch");
   using G = Geo<MT>;
+  const int hpitch = s.Lin, vpitch = s.L;     // the padded pitches of H and V (RAGGED: s then holds the problem's lengths)
+  int gx = 0;                                 // RAGGED: the problem's grid x
+  if constexpr (RAGGED) {
+    const RaggedProblem& rp = bt.rag[(a.b0 + (int)blockIdx.z) / s.B];
+    s.L = (int)rp.rows; s.Lin = rp.lin;
+    gx = rp.gx[FWD ? 0 : 1];
+    if ((int)blockIdx.x >= gx) return;
+    if (!FWD) {
+      a.nsplit = rp.nch[1];
+      if ((int)blockIdx.y >= a.nsplit * ((a.M + MT - 1) / MT)) return;
+    }
+  }
   constexpr int WIN = kLT + kTK;                          // window pitch per line (kLT + kTK - 1 elements used)
   __shared__ __align__(16) float As[kTK * G::PAD];        // As[tt][m]
   __shared__ float Xs[G::XT * WIN];
@@ -124,13 +142,27 @@ nmfd_slide_kernel(NmfdShape s, SlideArgs a, Batch bt) {
     if (batch_skips(bt.active, prob)) return;
     if (LOSS && MODE == kKL && bt.scale) sc = bt.scale[prob];
     b -= prob * s.B;
-    a.A += prob * bt.f; a.X += prob * bt.g;
-    if (FWD) {
-      a.V = static_cast<const TV*>(a.V) + prob * bt.v;
-      a.Pn += prob * bt.p; a.Pp += prob * bt.p;
-      if (LOSS) a.block_partials += (int64_t)prob * s.B * gridDim.y * gridDim.x;
+    if constexpr (RAGGED) {
+      const RaggedProblem& rp = bt.rag[prob];
+      a.A += prob * bt.f;
+      if (FWD) {
+        a.X += prob * bt.g;
+        a.V = static_cast<const TV*>(a.V) + prob * bt.v;
+        a.Pn += rp.pn; a.Pp += rp.pn;
+        if (LOSS) a.block_partials += rp.loss_part;
+      } else {
+        a.X += rp.pn;
+        a.out += rp.part;
+      }
     } else {
-      a.out += prob * bt.p;
+      a.A += prob * bt.f; a.X += prob * bt.g;
+      if (FWD) {
+        a.V = static_cast<const TV*>(a.V) + prob * bt.v;
+        a.Pn += prob * bt.p; a.Pp += prob * bt.p;
+        if (LOSS) a.block_partials += (int64_t)prob * s.B * gridDim.y * gridDim.x;
+      } else {
+        a.out += prob * bt.p;
+      }
     }
   }
   const int kps = (a.K + a.nsplit - 1) / a.nsplit;
@@ -163,7 +195,7 @@ nmfd_slide_kernel(NmfdShape s, SlideArgs a, Batch bt) {
           if (FWD) {
             const int j1 = o1 - t1, j2 = o2 - t2, src = l0 - t0 - (kTK - 1) + i;      // window index of (lj, tt): lj - tt + kTK - 1
             if (j1 >= 0 && j1 < J1 && j2 >= 0 && j2 < J2 && src >= 0 && src < s.Lin)
-              x = a.X[((((int64_t)b * a.K + k) * J1 + j1) * J2 + j2) * s.Lin + src];
+              x = a.X[((((int64_t)b * a.K + k) * J1 + j1) * J2 + j2) * hpitch + src];
           } else {
             const int src = l0 + t0 + i;                                              // window index of (jj, tt): jj + tt
             if (src < s.L) x = a.X[((((int64_t)b * a.K + k) * s.X1 + (o1 + t1)) * s.X2 + (o2 + t2)) * s.L + src];
@@ -217,13 +249,14 @@ nmfd_slide_kernel(NmfdShape s, SlideArgs a, Batch bt) {
         const int l = l0 + 4 * lt + j;
         if (c < s.C && l < s.L && o < OUT) {
           const int64_t off = (((int64_t)b * s.C + c) * OUT + o) * s.L + l;
+          const int64_t voff = RAGGED ? (((int64_t)b * s.C + c) * OUT + o) * vpitch + l : off;     // V's padded layout
           if constexpr (WEIGHT) {
             const float w = static_cast<const float*>(a.mask)[off];
             if (w == 0.f) {
               if (!LOSS) { a.Pn[off] = 0.f; a.Pp[off] = 0.f; }
               continue;
             }
-            const float v = to_f32(static_cast<const TV*>(a.V)[off]);
+            const float v = to_f32(static_cast<const TV*>(a.V)[voff]);
             if (LOSS) {
               local += MODE == kEU ? loss_term_w<kEU>(v, acc[i][j], a.beta, w) : w * loss_term_d<MODE>(v, acc[i][j], a.beta);
             } else {
@@ -239,7 +272,7 @@ nmfd_slide_kernel(NmfdShape s, SlideArgs a, Batch bt) {
             else if (!LOSS) { a.Pn[off] = 0.f; a.Pp[off] = 0.f; }
             continue;
           }
-          const float v = to_f32(static_cast<const TV*>(a.V)[off]);
+          const float v = to_f32(static_cast<const TV*>(a.V)[voff]);
           if (FILL) {
             a.Pn[off] = v / (acc[i][j] + kEps);
             a.Pp[off] = 0.f;
@@ -260,11 +293,11 @@ nmfd_slide_kernel(NmfdShape s, SlideArgs a, Batch bt) {
     if (LOSS || (FILL && a.block_partials)) {
       const double tot = block_sum_d((double)local, red);
       if (tid == 0)
-        a.block_partials[((int64_t)b * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x] = tot;
+        a.block_partials[((int64_t)b * gridDim.y + blockIdx.y) * (RAGGED ? (unsigned)gx : gridDim.x) + blockIdx.x] = tot;
     }
   } else {
     const int64_t HI = s.h_inner();
-    float* out = a.out + (int64_t)split * (BATCH ? bt.n * bt.p : (int64_t)s.B * s.R * HI);
+    float* out = a.out + (int64_t)split * (BATCH && !RAGGED ? bt.n * bt.p : (int64_t)s.B * s.R * HI);
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
       const int r = m0 + 4 * ty + i;
@@ -284,12 +317,21 @@ nmfd_slide_kernel(NmfdShape s, SlideArgs a, Batch bt) {
 // grid (t tiles * r groups * outer-offset groups, c tiles, nsplit), 256 threads.
 // BATCH: grid z is (problem, split) from z0 on, problem-major, over bt.n problems; problem `prob` reads Gm + prob bt.g and
 // H + prob bt.f and writes out[split][prob] (bt.p floats per problem), summing its own lines in the single problem's splits.
+// RAGGED (BATCH, bt.rag; s the padded shape): problem `prob` reads its ratio tile in its own compact layout at Gm +
+// rag[prob].pn and H in its padded layout, up to its own lengths rag[prob].rows / .lin along the sliding axis, and writes
+// its split slabs at out + rag[prob].part, split after split (the plan and the splits do not depend on the length).
 
-template <int MT, bool BATCH = false>
+template <int MT, bool BATCH = false, bool RAGGED = false>
 __global__ void __launch_bounds__(256)
 nmfd_wgrad_kernel(NmfdShape s, const float* __restrict__ Gm, const float* __restrict__ H, float* __restrict__ out,
                   int nsplit, WgradPlan p, Batch bt, int64_t z0) {
+  static_assert(!RAGGED || BATCH, "RAGGED: a batch");
   using G = Geo<MT>;
+  const int hpitch = s.Lin;                   // H's padded pitch (RAGGED: s then holds the problem's lengths)
+  if constexpr (RAGGED) {
+    const RaggedProblem& rp = bt.rag[(z0 + blockIdx.z) / nsplit];
+    s.L = (int)rp.rows; s.Lin = rp.lin;
+  }
   __shared__ __align__(16) float Gs[G::NTO * kTK * G::PAD];      // Gs[oo][ll][c]
   __shared__ float Hs[G::HS];
   const int tid = threadIdx.x, tx = tid % G::TX, ty = tid / G::TX;
@@ -319,8 +361,14 @@ nmfd_wgrad_kernel(NmfdShape s, const float* __restrict__ Gm, const float* __rest
   if constexpr (BATCH) {
     const int64_t z = z0 + blockIdx.z, prob = z / nsplit, split = z - prob * nsplit;
     if (batch_skips(bt.active, prob)) return;
-    Gm += prob * bt.g; H += prob * bt.f;
-    out += (split * bt.n + prob) * bt.p;
+    H += prob * bt.f;
+    if constexpr (RAGGED) {
+      Gm += bt.rag[prob].pn;
+      out += bt.rag[prob].part + split * bt.p;
+    } else {
+      Gm += prob * bt.g;
+      out += (split * bt.n + prob) * bt.p;
+    }
     z0 = split;                 // from here on: this block's split
   }
   const int64_t zs = BATCH ? z0 : (int64_t)blockIdx.z;
@@ -329,7 +377,7 @@ nmfd_wgrad_kernel(NmfdShape s, const float* __restrict__ Gm, const float* __rest
   for (int64_t bo = line0; bo < line1; ++bo) {            // every H line (b, j1, j2) meets the G lines (b, j1 + t1, j2 + t2)
     const int b = (int)(bo / (J1 * J2)), jo = (int)(bo - (int64_t)b * (J1 * J2));
     const int j1 = jo / J2, j2 = jo - j1 * J2;
-    const float* Hb = H + ((int64_t)b * s.R * J1 * J2 + jo) * s.Lin;           // + r * J1 * J2 * Lin per component
+    const float* Hb = H + ((int64_t)b * s.R * J1 * J2 + jo) * hpitch;          // + r * J1 * J2 * hpitch per component
     const float* Gb = Gm + (int64_t)b * s.C * VI;
     for (int l0 = 0; l0 < s.L; l0 += kTK) {
       __syncthreads();
@@ -348,7 +396,7 @@ nmfd_wgrad_kernel(NmfdShape s, const float* __restrict__ Gm, const float* __rest
         const int rr = idx / (WIN - 1), i = idx - rr * (WIN - 1);
         const int src = l0 - t0 - (TP - 1) + i;           // window index of (ll, tj): ll - tj + TP - 1
         float h = 0.f;
-        if (rg * NR + rr < s.R && src >= 0 && src < s.Lin) h = Hb[(int64_t)(rg * NR + rr) * J1 * J2 * s.Lin + src];
+        if (rg * NR + rr < s.R && src >= 0 && src < s.Lin) h = Hb[(int64_t)(rg * NR + rr) * J1 * J2 * hpitch + src];
         Hs[rr * WIN + i] = h;
       }
       __syncthreads();
@@ -420,13 +468,16 @@ dim3 dim3_of(const Grid3& g) { return dim3((unsigned)g.x, (unsigned)g.y, (unsign
 
 
 // TV: the target's element type (FWD only; the dgrad pass reads no V and always takes float)
-template <int MT, bool FWD, typename TV, typename SEL, bool BATCH>
+template <int MT, bool FWD, typename TV, typename SEL, bool BATCH, bool RAGGED>
 void launch_slide(const NmfdShape& s, const SlideArgs& a, const Batch& bt, int mode, bool loss, dim3 grid, cudaStream_t st) {
-  if (!FWD) { nmfd_slide_kernel<MT, false, kKL, false, float, NoSel, BATCH><<<grid, 256, 0, st>>>(s, a, bt); return; }
-#define NMFD_GO(M)                                                                                  \
-  if (loss) nmfd_slide_kernel<MT, true, M, true, TV, SEL, BATCH><<<grid, 256, 0, st>>>(s, a, bt);   \
-  else nmfd_slide_kernel<MT, true, M, false, TV, SEL, BATCH><<<grid, 256, 0, st>>>(s, a, bt);
-  if constexpr (std::is_same<TV, float>::value && std::is_same<SEL, uint8_t>::value && !BATCH) {
+  if (!FWD) {
+    nmfd_slide_kernel<MT, false, kKL, false, float, NoSel, BATCH, RAGGED><<<grid, 256, 0, st>>>(s, a, bt);
+    return;
+  }
+#define NMFD_GO(M)                                                                                          \
+  if (loss) nmfd_slide_kernel<MT, true, M, true, TV, SEL, BATCH, RAGGED><<<grid, 256, 0, st>>>(s, a, bt);   \
+  else nmfd_slide_kernel<MT, true, M, false, TV, SEL, BATCH, RAGGED><<<grid, 256, 0, st>>>(s, a, bt);
+  if constexpr (std::is_same<TV, float>::value && std::is_same<SEL, uint8_t>::value && !BATCH && !RAGGED) {
     if (mode == kPlcaFill) { nmfd_slide_kernel<MT, true, kPlcaFill, false, TV, SEL, false><<<grid, 256, 0, st>>>(s, a, bt); return; }
   }
   switch (mode) {
@@ -438,19 +489,20 @@ void launch_slide(const NmfdShape& s, const SlideArgs& a, const Batch& bt, int m
 #undef NMFD_GO
 }
 
-template <bool FWD, typename TV, typename SEL, bool BATCH>
+template <bool FWD, typename TV, typename SEL, bool BATCH, bool RAGGED = false>
 void dispatch_slide(int mt, const NmfdShape& s, const SlideArgs& a, const Batch& bt, int mode, bool loss, dim3 grid,
                     cudaStream_t st) {
   switch (mt) {
-    case 4: launch_slide<4, FWD, TV, SEL, BATCH>(s, a, bt, mode, loss, grid, st); break;
-    case 8: launch_slide<8, FWD, TV, SEL, BATCH>(s, a, bt, mode, loss, grid, st); break;
-    case 16: launch_slide<16, FWD, TV, SEL, BATCH>(s, a, bt, mode, loss, grid, st); break;
-    case 32: launch_slide<32, FWD, TV, SEL, BATCH>(s, a, bt, mode, loss, grid, st); break;
-    default: launch_slide<64, FWD, TV, SEL, BATCH>(s, a, bt, mode, loss, grid, st); break;
+    case 4: launch_slide<4, FWD, TV, SEL, BATCH, RAGGED>(s, a, bt, mode, loss, grid, st); break;
+    case 8: launch_slide<8, FWD, TV, SEL, BATCH, RAGGED>(s, a, bt, mode, loss, grid, st); break;
+    case 16: launch_slide<16, FWD, TV, SEL, BATCH, RAGGED>(s, a, bt, mode, loss, grid, st); break;
+    case 32: launch_slide<32, FWD, TV, SEL, BATCH, RAGGED>(s, a, bt, mode, loss, grid, st); break;
+    default: launch_slide<64, FWD, TV, SEL, BATCH, RAGGED>(s, a, bt, mode, loss, grid, st); break;
   }
 }
 
-// one launch of the sliding kernel per slice of at most kMaxGridYZ lines: s.B batch elements, or a batch's bt.n x s.B
+// one launch of the sliding kernel per slice of at most kMaxGridYZ lines: s.B batch elements, or a batch's bt.n x s.B (a ragged
+// batch's grid sized for its padded shape, a.nsplit its largest dgrad split count)
 template <bool FWD, typename TV = float, typename SEL = NoSel>
 int launch_slices(int mt, const NmfdShape& s, SlideArgs a, const Batch& bt, int mode, bool loss, cudaStream_t st) {
   const int64_t lines = s.B * bt.n;
@@ -461,8 +513,10 @@ int launch_slices(int mt, const NmfdShape& s, SlideArgs a, const Batch& bt, int 
     dim3 grid = dim3_of(g);
     grid.z = (unsigned)std::min<int64_t>(g.z, lines - b0);
     bool batched = false;                 // a batch runs the BATCH instantiations (no selector); one problem the others
-    if constexpr (std::is_same<SEL, NoSel>::value) batched = bt.n > 1 || bt.active || bt.scale;
-    if (batched) {
+    if constexpr (std::is_same<SEL, NoSel>::value) batched = bt.n > 1 || bt.active || bt.scale || bt.rag;
+    if (batched && bt.rag) {
+      if constexpr (std::is_same<SEL, NoSel>::value) dispatch_slide<FWD, TV, SEL, true, true>(mt, s, a, bt, mode, loss, grid, st);
+    } else if (batched) {
       if constexpr (std::is_same<SEL, NoSel>::value) dispatch_slide<FWD, TV, SEL, true>(mt, s, a, bt, mode, loss, grid, st);
     } else {
       dispatch_slide<FWD, TV, SEL, false>(mt, s, a, bt, mode, loss, grid, st);
@@ -496,8 +550,10 @@ int nmfd_recon_phi(const NmfdShape& s, const void* V, int vdtype, const float* W
   const int mt = row_tile(s.C);
   const int nblocks = (int)nmfd_max_blocks(s);          // per problem; create bounds it (nmfd_shape_of)
   const bool loss = loss_blocks != nullptr;
-  if (bt.n < 1 || (bt.n > 1 && M)) { set_error("nmfd_recon_phi: a batch takes no selector"); return 1; }
-  if (loss && (double)nblocks * (double)bt.n > (double)max_blocks) {
+  if (bt.n < 1 || ((bt.n > 1 || bt.rag) && M)) { set_error("nmfd_recon_phi: a batch takes no selector"); return 1; }
+  if (bt.rag && bt.scale) { set_error("nmfd_recon_phi: a ragged batch takes no scale"); return 1; }
+  // a ragged batch's buffer holds its problems' own partials, as its create sized it
+  if (loss && !bt.rag && (double)nblocks * (double)bt.n > (double)max_blocks) {
     set_error("nmfd loss: partial buffer too small");
     return 1;
   }
@@ -511,7 +567,7 @@ int nmfd_recon_phi(const NmfdShape& s, const void* V, int vdtype, const float* W
         });
       }))
     return rc;
-  if (loss) return sum_partials(loss_blocks, nblocks, loss_dev, st, bt.n, bt.active);
+  if (loss) return sum_partials(loss_blocks, nblocks, loss_dev, st, bt.n, bt.active, bt.rag);
   return 0;
 }
 
@@ -546,14 +602,15 @@ int nmfd_wgrad(const NmfdShape& s, const float* G, const float* H, float* out, i
   if (p.nr * (p.tp + kTK) > (ncol / 4) * (4 + kTK)) { set_error("nmfd_wgrad: internal tile plan exceeds shared memory"); return 1; }
   if (bt.n < 1) { set_error("nmfd_wgrad: bad problem count"); return 1; }
   Grid3 g = wgrad_grid(s, p, nsplit);
-  const bool batched = bt.n > 1 || bt.active;
+  const bool batched = bt.n > 1 || bt.active || bt.rag;
   Batch b = bt;                           // a batch: problem after problem on grid z, sliced at kMaxGridYZ
   b.f = (int64_t)s.B * s.R * s.h_inner(); b.g = (int64_t)s.B * s.C * s.v_inner(); b.p = (int64_t)s.C * s.R * s.w_inner();
   const int64_t zall = g.z * bt.n;
   for (int64_t z0 = 0; z0 < zall; z0 += kMaxGridYZ) {
     dim3 grid = dim3_of(Grid3{g.x, g.y, std::min<int64_t>(zall - z0, kMaxGridYZ)});
 #define NMFD_WGRAD(MT)                                                                           \
-  if (batched) nmfd_wgrad_kernel<MT, true><<<grid, 256, 0, st>>>(s, G, H, out, nsplit, p, b, z0); \
+  if (bt.rag) nmfd_wgrad_kernel<MT, true, true><<<grid, 256, 0, st>>>(s, G, H, out, nsplit, p, b, z0); \
+  else if (batched) nmfd_wgrad_kernel<MT, true><<<grid, 256, 0, st>>>(s, G, H, out, nsplit, p, b, z0); \
   else nmfd_wgrad_kernel<MT><<<grid, 256, 0, st>>>(s, G, H, out, nsplit, p, b, 0);
     switch (p.mt) {
       case 4: NMFD_WGRAD(4); break;

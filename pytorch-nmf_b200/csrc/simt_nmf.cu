@@ -482,7 +482,7 @@ __global__ void __launch_bounds__(256) sum_partials_kernel(const double* __restr
   if (batch_skips(active, b)) return;
   if constexpr (RAGGED) {
     p += rag[b].loss_part;
-    n = (int)((rag[b].rows + kTile - 1) / kTile * rag[b].loss_chunks);
+    n = (int)rag[b].loss_n;
   } else {
     p += b * n;
   }

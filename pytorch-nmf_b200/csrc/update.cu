@@ -6,14 +6,21 @@ namespace nmfb200 {
 namespace {
 
 // Where the partials of element idx (of problem b) are: the offset in the first slab, the slab count and stride.  False for
-// a padding row of a ragged batch's H, which no kernel writes.  The kernels below take RAGGED (a.rag set) as a template flag,
-// so that their uniform instantiations run the code they always ran.
+// a padding row of a ragged batch's H, or (LINES) a padding position of a ragged NMFD batch's H lines, which no kernel
+// writes.  The kernels below take RAGGED (a.rag set) and LINES (a.line set as well) as template flags, so that their other
+// instantiations run the code they always ran.
 struct PartialAt { int64_t off, stride; int nch; };
-template <bool RAGGED>
+template <bool RAGGED, bool LINES = false>
 __device__ __forceinline__ bool partial_at(const ApplyArgs& a, int64_t idx, int64_t b, PartialAt& p) {
   if constexpr (RAGGED) {
     const RaggedProblem& rp = a.rag[b];
     const int64_t local = idx - b * a.prob_numel;
+    if constexpr (LINES) {                       // NMFD's H: the problem's compact [split][lines][lin] slabs
+      const int64_t ln = local / a.line, j = local - ln * a.line;
+      if (j >= rp.lin) return false;
+      p = PartialAt{rp.part + ln * rp.lin + j, a.prob_numel / a.line * rp.lin, rp.nch[1]};
+      return true;
+    }
     const int64_t row = local / a.rowlen;
     const int64_t rows = a.rag_launch == kRagW ? a.prob_numel / a.rowlen : rp.rows;
     if (row >= rows) return false;
@@ -25,14 +32,14 @@ __device__ __forceinline__ bool partial_at(const ApplyArgs& a, int64_t idx, int6
   return true;
 }
 
-template <bool RAGGED>
+template <bool RAGGED, bool LINES = false>
 __global__ void __launch_bounds__(256)
 apply_update_kernel(ApplyArgs a) {
   const int64_t idx = (int64_t)blockIdx.x * 256 + threadIdx.x;
   float newv = 0.f;
   const int64_t b = a.prob_numel ? idx / a.prob_numel : 0;      // Batch: the element's problem
   PartialAt pa;
-  if (idx < a.numel && !batch_skips(a.active, b) && partial_at<RAGGED>(a, idx, b, pa)) {
+  if (idx < a.numel && !batch_skips(a.active, b) && partial_at<RAGGED, LINES>(a, idx, b, pa)) {
     const int64_t off = pa.off;
     const int r = (int)((idx / a.inner) % a.R);
     const float sc = a.out_scale ? *a.out_scale : 1.0f;
@@ -72,13 +79,13 @@ apply_update_kernel(ApplyArgs a) {
 }
 
 // The ratio stage's inputs without the ratio stage: the summed partials (+ the centring term), nothing clamped.
-template <bool RAGGED>
+template <bool RAGGED, bool LINES = false>
 __global__ void __launch_bounds__(256)
 raw_sum_kernel(ApplyArgs a, float* __restrict__ num_out, float* __restrict__ den_out) {
   const int64_t idx = (int64_t)blockIdx.x * 256 + threadIdx.x;
   const int64_t b = a.prob_numel ? idx / a.prob_numel : 0;
   PartialAt pa;
-  if (idx >= a.numel || batch_skips(a.active, b) || !partial_at<RAGGED>(a, idx, b, pa)) return;
+  if (idx >= a.numel || batch_skips(a.active, b) || !partial_at<RAGGED, LINES>(a, idx, b, pa)) return;
   const int64_t off = pa.off;
   const float sc = a.out_scale ? *a.out_scale : 1.0f;
   float num = 0.f;
@@ -159,6 +166,51 @@ colsum_runs_kernel(const float* __restrict__ x, int64_t inner, float* __restrict
   }
 }
 
+// stage 1 of a ragged NMFD batch's H: x is nprob problems of (outer, R, inner) activations whose last axis is `line` long,
+// one block per (problem, o, r).  Problem b's run (o, r) is the first rag[b].lin positions of each of its inner / line lines,
+// summed as colsum_runs_kernel sums a single problem's run of that many elements, its partial at rag[b].cs_part + o R + r.
+// A problem whose run is one element (one line, lin 1) is summed as its single fit sums it, by colsum_rows_kernel: block
+// (o, r) for o < rag[b].cs_blocks forms that kernel's block-o partial of component r, in its order, in one thread.
+__global__ void __launch_bounds__(256)
+colsum_lines_kernel(const float* __restrict__ x, int64_t outer, int R, int64_t inner, int64_t line, float* __restrict__ partial,
+                    const uint8_t* __restrict__ active, const RaggedProblem* __restrict__ rag) {
+  __shared__ float sh[8];
+  const int64_t runs = outer * R, prob = (int64_t)blockIdx.x / runs, k = (int64_t)blockIdx.x - prob * runs;
+  if (batch_skips(active, prob)) return;
+  const RaggedProblem& rp = rag[prob];
+  const int64_t lin = rp.lin, n = inner / line * lin;
+  x += prob * runs * inner;
+  partial += rp.cs_part;
+  if (n == 1) {
+    const int64_t o = k / R, r = k - o * R;
+    if (o >= rp.cs_blocks || threadIdx.x != 0) return;
+    const int64_t rpb = (outer + rp.cs_blocks - 1) / rp.cs_blocks, row0 = o * rpb, row1 = min(outer, row0 + rpb);
+    const int ng = 256 / R;
+    float t = 0.f;
+    for (int g = 0; g < ng; ++g) {
+      float acc = 0.f;
+      for (int64_t row = row0 + g; row < row1; row += ng) acc += x[(row * R + r) * inner];
+      t += acc;
+    }
+    partial[o * R + r] = t;
+    return;
+  }
+  const float* run = x + k * inner;
+  float acc = 0.f;
+  for (int64_t i = threadIdx.x; i < n; i += 256) {
+    const int64_t ln = i / lin;
+    acc += run[ln * line + (i - ln * lin)];
+  }
+  for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+  if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = acc;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float t = 0.f;
+    for (int q = 0; q < 8; ++q) t += sh[q];
+    partial[k] = t;
+  }
+}
+
 // Batch: ceil(R / blockDim) blocks per problem along x; a ragged batch's problem b: its own partials and blocks
 template <bool RAGGED>
 __global__ void colsum_final_kernel(const float* __restrict__ partial, int64_t nb, int R, float* __restrict__ sums,
@@ -185,8 +237,9 @@ __device__ __forceinline__ float nan_max(float a, float b) { return (a != a || b
 
 // NaN-sticky min / max so that a NaN in V fails fit()'s non-negativity assertion like torch.all(V >= 0) does
 // SEL: the cells where M (contiguous rows x cols: a mask or weights) is 0 are skipped, V is not read there
-// Batch: nprob matrices of rows x cols, bstride elements apart (ragged, rag: matrix b's first rag[b].rows rows)
-template <typename TV, typename SEL = NoSel>
+// Batch: nprob matrices of rows x cols, bstride elements apart (ragged, rag: matrix b's first rag[b].rows rows, or with
+// COLS its first rag[b].rows columns)
+template <typename TV, typename SEL = NoSel, bool COLS = false>
 __global__ void __launch_bounds__(256)
 minmax_stage1(const TV* __restrict__ V, int64_t rows, int64_t cols, int64_t ld, float* __restrict__ scratch,
               const SEL* __restrict__ M, int64_t nprob, int64_t bstride, const RaggedProblem* __restrict__ rag) {
@@ -198,7 +251,7 @@ minmax_stage1(const TV* __restrict__ V, int64_t rows, int64_t cols, int64_t ld, 
     int64_t r = i / cols, c = i - r * cols;
     const int64_t b = nprob > 1 ? r / rows : 0;
     r -= b * rows;
-    if (rag && r >= rag[b].rows) continue;
+    if (rag && (COLS ? c : r) >= rag[b].rows) continue;
     float v = to_f32(V[b * bstride + r * ld + c]);
     mn = nan_min(mn, v);
     mx = nan_max(mx, v);
@@ -234,7 +287,7 @@ apply_update_vec4_kernel(ApplyArgs a) {
   const int64_t idx = ((int64_t)blockIdx.x * 256 + threadIdx.x) * 4;
   float m = 0.f;
   const int64_t b = a.prob_numel ? idx / a.prob_numel : 0;      // Batch: prob_numel is a multiple of 4 here
-  PartialAt pa;      // the four elements share a row: a ragged batch's offsets and strides are multiples of R here
+  PartialAt pa;      // the four elements share a row; a ragged batch's offsets and strides are multiples of 4 here
   if (idx < a.numel && !batch_skips(a.active, b) && partial_at<RAGGED>(a, idx, b, pa)) {
     const int64_t off = pa.off;
     const int r = (int)((idx / a.inner) % a.R);
@@ -284,7 +337,7 @@ static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 
 
 bool apply_update_vec4_shape(const ApplyArgs& a) {
   return a.inner % 4 == 0 && a.rowlen % 4 == 0 && a.ldp % 4 == 0 && a.numel % 4 == 0 &&
-         (a.nchunks == 1 || a.chunk_stride % 4 == 0) && a.prob_numel % 4 == 0;
+         (a.nchunks == 1 || a.chunk_stride % 4 == 0) && a.prob_numel % 4 == 0 && a.line == 0;
 }
 
 int apply_update(const ApplyArgs& a, cudaStream_t st) {
@@ -293,6 +346,7 @@ int apply_update(const ApplyArgs& a, cudaStream_t st) {
   const unsigned g4 = (unsigned)ceil_div(a.numel / 4, 256), g1 = (unsigned)ceil_div(a.numel, 256);
   if (vec4 && a.rag) apply_update_vec4_kernel<true><<<g4, 256, 0, st>>>(a);
   else if (vec4) apply_update_vec4_kernel<false><<<g4, 256, 0, st>>>(a);
+  else if (a.rag && a.line) apply_update_kernel<true, true><<<g1, 256, 0, st>>>(a);
   else if (a.rag) apply_update_kernel<true><<<g1, 256, 0, st>>>(a);
   else apply_update_kernel<false><<<g1, 256, 0, st>>>(a);
   NMF_LAUNCH_CHECK();
@@ -302,7 +356,8 @@ int apply_update(const ApplyArgs& a, cudaStream_t st) {
 int raw_sum(const ApplyArgs& a, float* num_out, float* den_out, cudaStream_t st) {
   if (a.numel <= 0) return 0;
   const unsigned g1 = (unsigned)ceil_div(a.numel, 256);
-  if (a.rag) raw_sum_kernel<true><<<g1, 256, 0, st>>>(a, num_out, a.den ? den_out : nullptr);
+  if (a.rag && a.line) raw_sum_kernel<true, true><<<g1, 256, 0, st>>>(a, num_out, a.den ? den_out : nullptr);
+  else if (a.rag) raw_sum_kernel<true><<<g1, 256, 0, st>>>(a, num_out, a.den ? den_out : nullptr);
   else raw_sum_kernel<false><<<g1, 256, 0, st>>>(a, num_out, a.den ? den_out : nullptr);
   NMF_LAUNCH_CHECK();
   return 0;
@@ -318,9 +373,20 @@ int64_t colsum_scratch_floats(int64_t outer, int R, int64_t inner) { return cols
 
 int factor_colsum(const float* x, int64_t outer, int R, int64_t inner, float* scratch, int64_t scratch_floats,
                   float* sums, cudaStream_t st, int64_t nprob, const uint8_t* active, const RaggedProblem* rag,
-                  int64_t rag_gx) {
+                  int64_t rag_gx, int64_t rag_line) {
   const int64_t nb = colsum_blocks(outer, inner);
   if (nprob < 1) { set_error("factor_colsum: bad problem count"); return 1; }
+  if (rag && rag_line) {   // the scratch was sized where the plans were made (nmfb200_nmfnd_batched_create_ragged)
+    if (inner % rag_line || R > 256 || (double)outer * R * nprob > (double)kMaxGridX || ceil_div(R, 64) * nprob > kMaxGridX) {
+      set_error("factor_colsum: bad ragged NMFD batch");
+      return 1;
+    }
+    colsum_lines_kernel<<<(unsigned)(outer * R * nprob), 256, 0, st>>>(x, outer, R, inner, rag_line, scratch, active, rag);
+    NMF_LAUNCH_CHECK();
+    colsum_final_kernel<true><<<(unsigned)(ceil_div(R, 64) * nprob), 64, 0, st>>>(scratch, 0, R, sums, active, rag);
+    NMF_LAUNCH_CHECK();
+    return 0;
+  }
   if (rag) {         // the scratch and grid were checked where the plans were made (nmfb200_nmf_batched_create_ragged)
     if (inner != 1 || rag_gx < 1 || rag_gx > kMaxGridX || R > 256 || nprob > kMaxGridX / 4) {
       set_error("factor_colsum: bad ragged batch");
@@ -353,7 +419,7 @@ int factor_colsum(const float* x, int64_t outer, int R, int64_t inner, float* sc
 }
 
 int matrix_minmax(const void* V, int vdtype, int64_t rows, int64_t cols, int64_t ld, float* scratch2048, float* mm,
-                  cudaStream_t st, CellSel M, int64_t nprob, int64_t bstride, const RaggedProblem* rag) {
+                  cudaStream_t st, CellSel M, int64_t nprob, int64_t bstride, const RaggedProblem* rag, bool rag_cols) {
   if (nprob < 1 || (nprob > 1 && M)) { set_error("matrix_minmax: a batch takes no selector"); return 1; }
   int64_t nb = ceil_div(nprob * rows * cols, 256 * 16);
   if (nb > 1024) nb = 1024;
@@ -361,8 +427,12 @@ int matrix_minmax(const void* V, int vdtype, int64_t rows, int64_t cols, int64_t
   int rc = with_vtype(V, vdtype, [&](auto Vt) {
     using TV = vtype_t<decltype(Vt)>;
     return with_sel(M, [&](auto Mk) {
-      minmax_stage1<TV, sel_t<decltype(Mk)>><<<(unsigned)nb, 256, 0, st>>>(Vt, rows, cols, ld, scratch2048, Mk, nprob,
-                                                                          bstride, rag);
+      if (rag_cols)
+        minmax_stage1<TV, sel_t<decltype(Mk)>, true><<<(unsigned)nb, 256, 0, st>>>(Vt, rows, cols, ld, scratch2048, Mk,
+                                                                                   nprob, bstride, rag);
+      else
+        minmax_stage1<TV, sel_t<decltype(Mk)>><<<(unsigned)nb, 256, 0, st>>>(Vt, rows, cols, ld, scratch2048, Mk, nprob,
+                                                                            bstride, rag);
       NMF_LAUNCH_CHECK();
       return 0;
     });

@@ -61,6 +61,8 @@ SIGNATURES = {
     "nmfb200_nmfd_set_target": (_int, [_vp, _vp, _int, _vp]),
     "nmfb200_nmfnd_batched_create": (_int, [_c.POINTER(_vp), _int, _i64, _i64, _i64, _int, _c.POINTER(_i64), _i64,
                                             _c.POINTER(_i64)]),
+    "nmfb200_nmfnd_batched_create_ragged": (_int, [_c.POINTER(_vp), _int, _i64, _i64, _i64, _int, _c.POINTER(_i64), _i64,
+                                                   _c.POINTER(_i64), _c.POINTER(_i64)]),
     "nmfb200_nmfd_batched_set_target": (_int, [_vp, _vp, _i64, _int, _vp]),
     "nmfb200_nmfd_batched_set_active": (_int, [_vp, _vp, _vp]),
     "nmfb200_plca_work_numel": (_i64, [_vp]),

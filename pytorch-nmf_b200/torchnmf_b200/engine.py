@@ -76,18 +76,23 @@ def _workspace_bytes(key):
         if len(key) > 6:
             return sum(one(n) for n in key[6]) + 88 * B + (1 << 14)
         return B * one(N) + (1 << 14)
-    if key[0] == "nmfd_batched":          # ("nmfd_batched", device, P, B, C, X, R, K): P x the fp32 context of one problem
-        _, _, P, B, C, X, R, K = key
-        nx, nk, nh = 1, 1, 1
-        for x, k in zip(X, K):
-            nx, nk, nh = nx * x, nk * k, nh * (x - k + 1)
-        p = _capi.nmfd_plan(B, C, X, R, K)
+    if key[0] == "nmfd_batched":          # ("nmfd_batched", device, P, B, C, X, R, K[, lengths]): P x the fp32 context of one
+        _, _, P, B, C, X, R, K = key[:8]  # problem; with the lengths of a ragged batch the sum of each problem's own context
 
         def colsum_floats(outer, inner):      # update.cu: colsum_scratch_floats
             return R * (outer if inner > 1 else min(1024, max(1, (outer + 63) // 64)))
-        loss_blocks = p["recon_grid"][0] * p["recon_grid"][1] * B
-        return P * (8 * B * C * nx + 8 * R * max(p["wgrad_nsplit"] * C * nk, p["dgrad_nsplit"] * B * nh) + 8 * R
-                    + 8 * loss_blocks + 4 * max(colsum_floats(C, nk), colsum_floats(B, nh))) + (1 << 14)
+
+        def one(X):
+            nx, nk, nh = 1, 1, 1
+            for x, k in zip(X, K):
+                nx, nk, nh = nx * x, nk * k, nh * (x - k + 1)
+            p = _capi.nmfd_plan(B, C, X, R, K)
+            loss_blocks = p["recon_grid"][0] * p["recon_grid"][1] * B
+            return (8 * B * C * nx + 8 * R * max(p["wgrad_nsplit"] * C * nk, p["dgrad_nsplit"] * B * nh) + 8 * R
+                    + 8 * loss_blocks + 4 * max(colsum_floats(C, nk), colsum_floats(B, nh)))
+        if len(key) > 8:
+            return sum(one(tuple(X[:-1]) + (n,)) for n in key[8]) + 96 * P + (1 << 14)
+        return P * one(X) + (1 << 14)
     if key[0] == "nmfd":                  # ("nmfd", device, B, C, X, R, K, precision): ratio tiles + shifted operand copies
         _, _, B, C, X, R, K = key[:7]
         nx, nk = 1, 1
@@ -535,9 +540,18 @@ class CudaBatchedNmfdEngine(_BatchedEngine):
     fp32, fp16 or bf16, each problem's block contiguous and the blocks at least B C prod(X) elements apart; W (P,C,R,*K) and
     H (P,B,R,*(X-K+1)) contiguous fp32, updated in place.  Every update and loss launch runs all problems, and problem p's
     factors and loss are bit for bit those of CudaNmfdEngine(V[p], W[p], H[p], "f32").  No `iterate`: the fit loop calls
-    update_w / update_h, as for a single NMFD engine."""
+    update_w / update_h, as for a single NMFD engine.
+
+    `lengths` (P ints in [K_last, X_last], or None): a ragged batch along the last axis
+    (nmfb200_nmfnd_batched_create_ragged) -- problem p is the problem of V[p, ..., :lengths[p]], W[p] and
+    H[p, ..., :lengths[p] - K_last + 1], bit for bit CudaNmfdEngine on those, "f32"; the positions past them of V[p] are
+    never read and those of H[p] never written."""
     kind = "nmfd_batched"
     _set_active = "nmfb200_nmfd_batched_set_active"
+
+    def __init__(self, V, W, H, lengths=None):
+        self._lengths = None if lengths is None else tuple(int(n) for n in lengths)
+        super().__init__(V, W, H)
 
     def _create(self, V, W, H, dev_index):
         P, C, R, *K = W.shape
@@ -548,8 +562,16 @@ class CudaBatchedNmfdEngine(_BatchedEngine):
         if not (V[0].is_contiguous() and (V.stride(0) == 0 or V.stride(0) >= V[0].numel())):
             raise ValueError("every problem's block of V must be contiguous, the blocks 0 or at least B C prod(X) apart")
         vd, kd = (ctypes.c_int64 * nd)(*X), (ctypes.c_int64 * nd)(*K)
-        self._acquire(("nmfd_batched", dev_index, P, B, C, tuple(X), R, tuple(K)),
-                      lambda ref: self._lib.nmfb200_nmfnd_batched_create(ref, dev_index, P, B, C, nd, vd, R, kd))
+        if self._lengths is None:
+            self._acquire(("nmfd_batched", dev_index, P, B, C, tuple(X), R, tuple(K)),
+                          lambda ref: self._lib.nmfb200_nmfnd_batched_create(ref, dev_index, P, B, C, nd, vd, R, kd))
+        else:
+            if len(self._lengths) != P:
+                raise ValueError(f"lengths holds {len(self._lengths)} values for {P} problems")
+            lens = (ctypes.c_int64 * P)(*self._lengths)
+            self._acquire(("nmfd_batched", dev_index, P, B, C, tuple(X), R, tuple(K), self._lengths),
+                          lambda ref: self._lib.nmfb200_nmfnd_batched_create_ragged(ref, dev_index, P, B, C, nd, vd, R, kd,
+                                                                                   lens))
         _capi.check(self._lib.nmfb200_nmfd_batched_set_target(self._ctx, _ptr(V), V.stride(0), _capi.DTYPES[V.dtype],
                                                               _stream(self.device)))
 

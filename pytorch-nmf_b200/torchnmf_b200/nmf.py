@@ -772,13 +772,14 @@ def _register_batched_factors(module, W, H, trainable_W, trainable_H):
 
 
 @contextlib.contextmanager
-def _placed_factors(module, factors, no_cuda, rows=None):
+def _placed_factors(module, factors, no_cuda, real=None):
     """Places a batched fit: yields (device, the fp32 contiguous tensors the engine updates, one per Parameter of
     `factors`).  They are the Parameters' own storages when every factor is fp32 and contiguous on a CUDA device, else
     device copies, written back into the Parameters when the block completes.  Without CUDA it raises
-    RuntimeError(no_cuda).  With the `_engine_factory` test hook the storages are taken where they are.  `rows` (a bool
-    (problems, rows) tensor, or None): the rows of the second factor that are written back; the others are left as they
-    are (a ragged batch's padding)."""
+    RuntimeError(no_cuda).  With the `_engine_factory` test hook the storages are taken where they are.  `real` (a bool
+    tensor over the leading axes of the second factor, or over all of them, or None): the cells of the second factor that
+    are written back -- the real rows of a ragged BatchedNMF's H, the real positions of a ragged convolutive batch's H along
+    its last axis; the others are left as they are (a ragged batch's padding)."""
     f32 = torch.float32
     if module._engine_factory is not None:
         dev, staged = factors[0].device, False
@@ -792,8 +793,8 @@ def _placed_factors(module, factors, no_cuda, rows=None):
     yield dev, placed
     if staged:
         for i, (t, d) in enumerate(zip(factors, placed)):
-            if i == 1 and rows is not None:
-                t.data[rows.to(t.device)] = d[rows.to(d.device)].to(t.device, t.dtype)
+            if i == 1 and real is not None:
+                t.data[real.to(t.device)] = d[real.to(d.device)].to(t.device, t.dtype)
             else:
                 t.data.copy_(d)
 
@@ -841,7 +842,7 @@ class _BatchedComponent(BaseComponent):
     own stop rule."""
     _ndim = 3                      # axes of W and of H
     _axes = "three axes (B, rows, rank)"
-    _ragged = False                # fit(..., lengths=L): BatchedNMF only
+    _ragged = False                # fit(..., lengths=L): BatchedNMF and the convolutive batched models
 
     def __init__(self, rank=None, W=None, H=None, trainable_W=True, trainable_H=True):
         torch.nn.Module.__init__(self)
@@ -859,17 +860,22 @@ class _BatchedComponent(BaseComponent):
     def sparse_fit(self, *args, **kwargs):
         raise NotImplementedError(f"{type(self).__name__} has no sparse_fit: fit each problem with the single model's sparse_fit")
 
+    def _length_range(self, V):
+        """(lo, hi, name of hi) of the lengths of a ragged fit: rows of H in [1, N]."""
+        return 1, self.H.shape[1], "N"
+
     def _check_lengths(self, V, lengths, cd):
-        """fit(..., lengths=L)'s checks, before any device work: the lengths as a list of B Python ints in [1, N]."""
+        """fit(..., lengths=L)'s checks, before any device work: the lengths as a list of P Python ints in
+        `_length_range`."""
         name = type(self).__name__
         if not self._ragged:
-            raise ValueError(f"lengths is supported by BatchedNMF only (got {name})")
+            raise ValueError(f"lengths is not supported by {name}")
         if cd:
             raise ValueError("lengths: solver='cd' does not fit ragged batches; use solver='mu'")
-        B, N = self.H.shape[:2]
-        if V.dim() != 3:
-            raise ValueError(f"lengths needs one target per problem, V of shape ({B}, N, C); a shared 2-D target has "
-                             f"one length")
+        B = self.H.shape[0]
+        if V.dim() != self.H.dim():
+            raise ValueError(f"lengths needs one target per problem, V with a leading axis of {B} problems; a shared "
+                             f"target of shape {tuple(V.shape)} has one length")
         if isinstance(lengths, Tensor):
             if lengths.dtype.is_floating_point or lengths.dtype.is_complex or lengths.dtype == torch.bool:
                 raise ValueError(f"lengths must hold integers (got {lengths.dtype})")
@@ -885,9 +891,10 @@ class _BatchedComponent(BaseComponent):
             raise ValueError(f"lengths must be a sequence of ints or an integer tensor (got {type(lengths).__name__})")
         if len(lens) != B:
             raise ValueError(f"lengths holds {len(lens)} values for {B} problems")
-        bad = [n for n in lens if not 1 <= n <= N]
+        lo, hi, hi_name = self._length_range(V)
+        bad = [n for n in lens if not lo <= n <= hi]
         if bad:
-            raise ValueError(f"every length must be in [1, N = {N}] (got {bad[0]})")
+            raise ValueError(f"every length must be in [{lo}, {hi_name} = {hi}] (got {bad[0]})")
         return lens
 
     @torch.no_grad()
@@ -922,16 +929,21 @@ class _BatchedComponent(BaseComponent):
         factors train; a frozen factor leaves the other's updates one call each.  ValueError, before any device work: an
         unknown solver, "cd" with beta != 2, and "cd" on the convolutive batched models.
 
-        lengths: (BatchedNMF only, keyword-only, default None) B ints in [1, N], as a sequence or an integer tensor of shape
-        (B,) on any device: a ragged batch, problem b being the fit of V[b, :lengths[b]] with W[b] and H[b, :lengths[b]].
-        V (B, N, C) and H (B, N, R) stay padded.  n_iter[b], W[b] and H[b, :L_b] equal, bit for bit, those of
-        `NMF(W=W0[b], H=H0[b, :L_b]).fit(V[b, :L_b], ..., precision="f32")`, stop rule included: each problem runs the tile
-        plan of its own length.  Rows L_b: of H[b] are never written and rows L_b: of V[b] never read (NaN there does not
-        reach the fit); the non-negativity assertion and the beta <= 0 zero check look at the real rows only.  Every beta,
-        alpha / l1_ratio, frozen factors, fp16 / bf16 / strided targets and host or float64 modules work as without it;
-        lengths all equal to N give the bits of lengths=None.  The workspace is the sum of the problems' single-problem
-        workspaces.  ValueError, before any device work: the wrong number of lengths, a length outside [1, N], a
-        non-integer or non-1-D lengths, a shared 2-D target, solver="cd", and lengths on the convolutive batched models.
+        lengths: (keyword-only, default None) one int per problem, as a sequence or an integer tensor of shape (P,) on
+        any device: a ragged batch.  BatchedNMF: B ints in [1, N], problem b being the fit of V[b, :lengths[b]] with W[b]
+        and H[b, :lengths[b]]; V (B, N, C) and H (B, N, R) stay padded, and n_iter[b], W[b] and H[b, :L_b] equal, bit for
+        bit, those of `NMF(W=W0[b], H=H0[b, :L_b]).fit(V[b, :L_b], ..., precision="f32")`.  BatchedNMFD / 2D / 3D: P ints
+        in [K_last, X_last] (W's and V's last sizes) along the last convolved axis, problem p being the fit of
+        V[p, ..., :L_p] with W[p] and H[p, ..., :L_p - K_last + 1]; V (P, B, C, *X) and H (P, B, R, *(X - K + 1)) stay
+        padded, and n_iter[p], W[p] and those positions of H[p] equal, bit for bit, those of the single model's
+        `(W=W0[p], H=H0[p, ..., :L_p - K_last + 1]).fit(V[p, ..., :L_p], ..., precision="f32")`; its B clips share W[p]
+        and L_p.  The stop rule is included: each problem runs the tile plan of its own length.  The padding of V is never
+        read (NaN there does not reach the fit) and that of H never written, even through a staged host or float64
+        module; the non-negativity assertion and the beta <= 0 zero check look at the real cells only.  Every beta,
+        alpha / l1_ratio, frozen factors, fp16 / bf16 (and, for BatchedNMF, strided) targets and host or float64 modules
+        work as without it; lengths all at their maximum give the bits of lengths=None.  The workspace is the sum of the
+        problems' single-problem workspaces.  ValueError, before any device work: the wrong number of lengths, a length
+        out of range, a non-integer, bool or non-1-D lengths, a shared target (no problem axis), and solver="cd".
         """
         name = type(self).__name__
         if solver not in ("mu", "cd"):
@@ -958,11 +970,11 @@ class _BatchedComponent(BaseComponent):
         self._check_target_shape(V)
 
         no_cuda = "torchnmf_b200.fit needs a CUDA device (sm_90a); there is no CPU fallback"
-        rows = None                # a ragged batch: the real rows of H, the only ones written back from a staged copy
+        real = None                # a ragged batch: the real cells of H, the only ones written back from a staged copy
         if lengths is not None:
-            rows = torch.arange(H.shape[1]) < torch.tensor(lengths).unsqueeze(1)
+            real = self._real_cells(lengths)
         ragged = {} if lengths is None else {"lengths": lengths}
-        with _placed_factors(self, (W, H), no_cuda, rows) as (dev, (Wd, Hd)):
+        with _placed_factors(self, (W, H), no_cuda, real) as (dev, (Wd, Hd)):
             if self._engine_factory is None:
                 Vd = V.to(dev, non_blocking=True)
                 if Vd.dtype not in (torch.float32, torch.float16, torch.bfloat16):
@@ -1057,6 +1069,10 @@ class BatchedNMF(_BatchedComponent):
         rows_ok = Vd.stride(-1) == 1 and Vd.stride(-2) >= Vd.shape[-1]
         return rows_ok and (Vd.dim() == 2 or Vd.stride(0) == 0 or Vd.stride(0) >= Vd.shape[1] * Vd.stride(1))
 
+    def _real_cells(self, lengths):
+        """The real rows of H, a bool (B, N) tensor."""
+        return torch.arange(self.H.shape[1]) < torch.tensor(lengths).unsqueeze(1)
+
 
 def _batched_conv(H, W, conv):
     """The reconstructions of P convolutive problems at once: problem p's H[p] (B,R,*J) convolved with its flipped W[p]
@@ -1078,8 +1094,12 @@ class _BatchedConvolutive(_BatchedComponent):
     target).  Workspace (device memory, kept between fits of the same shape): P times that of one fp32 problem of the
     single model -- the ratio tile of V's size (two at beta != 1), the wgrad / dgrad split partial slabs, 8 R max(nsw C
     prod(K), nsd B prod(X-K+1)) bytes with the splits of `_capi.nmfd_plan`, plus the column sums and loss partials -- so
-    it grows linearly with P."""
+    it grows linearly with P.  `fit(..., lengths=L)` fits a ragged batch along the last convolved axis: problem p is the
+    single model's `fit(V[p, ..., :L[p]], ..., precision="f32")` with W[p] and H[p, ..., :L[p] - K_last + 1], V and H
+    padded, each problem on the plan of its own length; its workspace is the sum of the problems' single-problem
+    workspaces, not P times the largest."""
     _engine_cls = _engine.CudaBatchedNmfdEngine
+    _ragged = True
     _nd = 1
     _conv = None
 
@@ -1100,6 +1120,18 @@ class _BatchedConvolutive(_BatchedComponent):
             return Vd.is_contiguous()
         return Vd[0].is_contiguous() and (Vd.stride(0) == 0 or Vd.stride(0) >= Vd[0].numel())
 
+    def _length_range(self, V):
+        """A ragged fit's lengths run along the last convolved axis, from W's last size to V's."""
+        return self.W.shape[-1], V.shape[-1], "X_last"
+
+    def _real_cells(self, lengths):
+        """The real cells of H (P, B, R, *J): positions below L_p - K_last + 1 of its last axis, a bool tensor of H's
+        shape."""
+        H = self.H
+        lin = torch.tensor(lengths) - self.W.shape[-1] + 1
+        real = torch.arange(H.shape[-1]) < lin.view(-1, *([1] * (H.dim() - 1)))
+        return real.expand(H.shape)
+
 
 class BatchedNMFD(_BatchedConvolutive):
     """P independent NMFD problems of one shape:  V[p] (B,C,L) ~= sum_t W[p][:,:,t] @ shift_t(H[p]),  W (P,C,R,T),
@@ -1117,7 +1149,8 @@ class BatchedNMFD(_BatchedConvolutive):
     target).  Workspace (device memory, kept between fits of the same shape): P times that of one fp32 problem of the
     single model -- the ratio tile of V's size (two at beta != 1), the wgrad / dgrad split partial slabs, 8 R max(nsw C
     prod(K), nsd B prod(X-K+1)) bytes with the splits of `_capi.nmfd_plan`, plus the column sums and loss partials -- so
-    it grows linearly with P.
+    it grows linearly with P.  `fit(..., lengths=L)` fits problems of different lengths along the clips' length L (the last axis),
+    each bit for bit its own single fit on its real positions (see `fit`).
     """
     _nd = 1
     _ndim = 4
@@ -1151,7 +1184,8 @@ class BatchedNMF2D(_BatchedConvolutive):
     target).  Workspace (device memory, kept between fits of the same shape): P times that of one fp32 problem of the
     single model -- the ratio tile of V's size (two at beta != 1), the wgrad / dgrad split partial slabs, 8 R max(nsw C
     prod(K), nsd B prod(X-K+1)) bytes with the splits of `_capi.nmfd_plan`, plus the column sums and loss partials -- so
-    it grows linearly with P.
+    it grows linearly with P.  `fit(..., lengths=L)` fits problems of different lengths along X2 (the last axis),
+    each bit for bit its own single fit on its real positions (see `fit`).
     """
     _nd = 2
     _ndim = 5
@@ -1185,7 +1219,8 @@ class BatchedNMF3D(_BatchedConvolutive):
     target).  Workspace (device memory, kept between fits of the same shape): P times that of one fp32 problem of the
     single model -- the ratio tile of V's size (two at beta != 1), the wgrad / dgrad split partial slabs, 8 R max(nsw C
     prod(K), nsd B prod(X-K+1)) bytes with the splits of `_capi.nmfd_plan`, plus the column sums and loss partials -- so
-    it grows linearly with P.
+    it grows linearly with P.  `fit(..., lengths=L)` fits problems of different lengths along X3 (the last axis),
+    each bit for bit its own single fit on its real positions (see `fit`).
     """
     _nd = 3
     _ndim = 6
