@@ -36,7 +36,13 @@ from . import engine as _engine
 try:
     from tqdm import tqdm as _tqdm
 except Exception:  # pragma: no cover
-    _tqdm = None
+    class _tqdm:
+        """The progress bar where tqdm is not installed: shows nothing."""
+        def __init__(self, *a, **k): pass
+        def __enter__(self): return self
+        def __exit__(self, *a): return False
+        def set_postfix(self, **k): pass
+        def update(self, n): pass
 
 __all__ = ["BaseComponent", "NMF", "NMFD", "NMF2D", "NMF3D", "BatchedNMF", "BatchedNMFD", "BatchedNMF2D",
            "BatchedNMF3D"]
@@ -144,12 +150,7 @@ def _weight_values_ok(w):
     return lo >= 0 and hi < math.inf                         # NaN fails both
 
 
-class _NullBar:
-    def __init__(self, *a, **k): pass
-    def __enter__(self): return self
-    def __exit__(self, *a): return False
-    def set_postfix(self, **k): pass
-    def update(self, n): pass
+_NO_CUDA = "torchnmf_b200.fit needs a CUDA device (sm_90a); there is no CPU fallback"
 
 
 class BaseComponent(torch.nn.Module):
@@ -220,9 +221,6 @@ class BaseComponent(torch.nn.Module):
     # ---- engine selection -------------------------------------------------------------------
     _engine_cls = None
 
-    def _build_engine(self, V, W, H, precision):
-        return self._engine_cls(V, W, H, precision)
-
     def _check_target_shape(self, V):
         raise NotImplementedError
 
@@ -234,17 +232,10 @@ class BaseComponent(torch.nn.Module):
     _strided_target = False       # the engine reads a row-strided (unit column stride) half-precision target as it is
     _cd_solver = False            # fit(..., solver="cd") at beta 2: NMF only
 
-    def _open_engine(self, V, beta, precision, group, sparse_kernels, mask=None, weight=None):
-        """Shared entry of `fit` / `sparse_fit`: validation that needs no device pass, placement of V / W / H on the CUDA
-        device (host buffers are copied there; a dense bf16 / fp16 target keeps its dtype, other target and factor dtypes are
-        staged through fp32 device copies) and the engine for this target, with `mask` (validated by `_check_mask`) set on
-        it: moved to the engine's device and made contiguous, read there in place as one byte per cell.  A `weight`
-        (validated by `_check_weight`) is set the same way as one fp32 per cell (other dtypes staged through one fp32 copy),
-        after one reduction over its values (`_weight_values_ok`, agreed on by every rank with `group`, so that all of
-        them raise together); a sparse one takes the observed-cell kernels.
-        Returns (engine, W, H, Wd, Hd, staged): W / H the Parameters, Wd / Hd the fp32 device tensors the engine updates."""
-        wsparse = weight is not None and weight.is_sparse    # a sparse weight: the observed-cell kernels (NMF, _check_weight)
-        observed = (mask is not None and mask.is_sparse) or wsparse
+    def _checked_target(self, V, beta, mask=None, weight=None):
+        """The checks of `fit` / `sparse_fit` that need no device pass, in the reference's order; returns the target, a
+        sparse one coalesced."""
+        observed = (mask is not None and mask.is_sparse) or (weight is not None and weight.is_sparse)
         sparse_target = V.is_sparse and not observed
         if sparse_target and not self._sparse_targets:
             raise NotImplementedError                      # nmf.py:294-295: only NMF derives the sparse update
@@ -260,20 +251,26 @@ class BaseComponent(torch.nn.Module):
             if beta <= 0:                                                                    # nmf.py:332-336
                 raise ValueError("When beta <= 0 and V contains zeros, the training process may diverge. "
                                  "Please add small values to V, or use a positive beta value.")
-        W, H = self.W, self.H
-        assert W is not None and H is not None, "fit() needs both W and H"
+        assert self.W is not None and self.H is not None, "fit() needs both W and H"
         self._check_target_shape(V)
+        return V
 
-        # ---- placement: run on the parameters' CUDA device, or stage host buffers through cuda ----
-        staged = False
+    def _open_engine(self, V, dev, Wd, Hd, beta, precision, group, sparse_kernels, mask=None, weight=None):
+        """The engine of `fit` / `sparse_fit` for the target V (`_checked_target`) on the device `dev`, updating the fp32
+        factors Wd / Hd (`_placed_factors`).  A dense bf16 / fp16 target keeps its dtype, other target dtypes are staged
+        through an fp32 device copy.  A `mask` (validated by `_check_mask`) is set on the engine: moved to its device and
+        made contiguous, read there in place as one byte per cell.  A `weight` (validated by `_check_weight`) is set the
+        same way as one fp32 per cell (other dtypes staged through one fp32 copy), after one reduction over its values
+        (`_weight_values_ok`, agreed on by every rank with `group`, so that all of them raise together); a sparse one takes
+        the observed-cell kernels."""
+        wsparse = weight is not None and weight.is_sparse    # a sparse weight: the observed-cell kernels (NMF, _check_weight)
+        observed = (mask is not None and mask.is_sparse) or wsparse
+        sparse_target = V.is_sparse and not observed
+        rank = Wd.shape[1]
+        wok = True
         if self._engine_factory is None:
-            if not torch.cuda.is_available():
-                raise RuntimeError("torchnmf_b200.fit needs a CUDA device (sm_90a); there is no CPU fallback")
             f32 = torch.float32
-            on_gpu = W.device.type == "cuda"
-            dev = W.device if on_gpu else torch.device("cuda", torch.cuda.current_device())
             wv = None
-            wok = True
             if observed:
                 # the observed cells up to rank 256 (sharded or not); above it, scattered into a dense fp32 V and a dense
                 # mask (or weight) on the device, for the dense masked (weighted) kernels
@@ -282,7 +279,7 @@ class BaseComponent(torch.nn.Module):
                     O = _cells_of(V, lin, dev)
                 else:
                     O = _observed_cells(V, mask, dev)
-                if W.shape[1] <= 256:
+                if rank <= 256:
                     Vd, sparse_cls, mask, weight = O, _engine.CudaObservedNmfEngine, None, None
                 else:
                     rows, cols = O.indices()
@@ -298,7 +295,7 @@ class BaseComponent(torch.nn.Module):
                     sparse_cls = None
             else:
                 Vd = V.to(dev, non_blocking=True)
-                sparse_cls = (_sparse_engine_cls(sparse_kernels and self._sparse_kernels, beta, W.shape[1], group)
+                sparse_cls = (_sparse_engine_cls(sparse_kernels and self._sparse_kernels, beta, rank, group)
                               if sparse_target else None)
                 if not sparse_target and Vd.dtype in (torch.float16, torch.bfloat16):
                     # the kernels convert each element exactly where they load it: the fit is bit for bit that of V.float(),
@@ -307,31 +304,22 @@ class BaseComponent(torch.nn.Module):
                         Vd = Vd.contiguous()
                 elif sparse_cls is None:
                     Vd = (Vd.to_dense() if sparse_target else Vd).to(f32).contiguous()
-            use_sparse_kernels = sparse_cls is not None
-            if on_gpu and W.dtype == f32 and H.dtype == f32:
-                Wd, Hd = W.data, H.data                       # updated in place, like param.data in the reference
-            else:
-                staged = True                                 # host buffers and / or another dtype: fp32 device copies
-                Wd = W.data.to(dev, f32, non_blocking=True).contiguous()
-                Hd = H.data.to(dev, f32, non_blocking=True).contiguous()
-            if not Wd.is_contiguous() or not Hd.is_contiguous():
-                raise ValueError("W and H must be contiguous")
             if weight is not None and not wsparse:
                 weight = weight.to(dev, f32).contiguous()
                 wok = _weight_values_ok(weight)
             if wv is not None:
                 eng = sparse_cls(Vd.coalesce(), Wd, Hd, weights=wv)
+            elif sparse_cls is not None:
+                eng = sparse_cls(Vd.coalesce(), Wd, Hd)
             else:
-                eng = sparse_cls(Vd.coalesce(), Wd, Hd) if use_sparse_kernels else self._build_engine(Vd, Wd, Hd, precision)
+                eng = self._engine_cls(Vd, Wd, Hd, precision)
             Md = mask.to(dev).contiguous() if mask is not None else None
         else:
-            Wd, Hd = W.data, H.data
-            wok = True
             if wsparse:
-                lin, wv, wok = _weighted_cells(weight, V.shape[1], W.device)
-                eng, Md, weight = self._engine_factory(_cells_of(V, lin, W.device), Wd, Hd, weights=wv), None, None
+                lin, wv, wok = _weighted_cells(weight, V.shape[1], dev)
+                eng, Md, weight = self._engine_factory(_cells_of(V, lin, dev), Wd, Hd, weights=wv), None, None
             elif observed:
-                eng, Md = self._engine_factory(_observed_cells(V, mask, W.device), Wd, Hd), None
+                eng, Md = self._engine_factory(_observed_cells(V, mask, dev), Wd, Hd), None
             else:
                 if weight is not None:
                     weight = weight.to(torch.float32).contiguous()
@@ -346,7 +334,7 @@ class BaseComponent(torch.nn.Module):
                 names = ["ndim", "C", "R"] + [f"kernel_size[{i}]" for i in range(3)] + [f"V.shape[{i + 2}]" for i in range(3)]
                 pad = [0] * (3 - nd)
                 try:
-                    eng.check_same_sizes(names, [nd, V.shape[1], W.shape[1], *W.shape[2:], *pad, *V.shape[2:], *pad])
+                    eng.check_same_sizes(names, [nd, V.shape[1], rank, *Wd.shape[2:], *pad, *V.shape[2:], *pad])
                 except ValueError:
                     eng.close()
                     raise
@@ -364,7 +352,7 @@ class BaseComponent(torch.nn.Module):
             except Exception:
                 eng.close()
                 raise
-        return eng, W, H, Wd, Hd, staged
+        return eng
 
     @classmethod
     def _check_mask(cls, V, mask, precision):
@@ -434,8 +422,8 @@ class BaseComponent(torch.nn.Module):
         dtype: the kernels keep fp32 master factors and fp32 accumulators.  The reference computes in the module's
         dtype (nmf.py:214-218).  Here a dense bfloat16 / float16 target is read as it is, with no fp32 copy (NMF also
         takes a row-strided view), and gives exactly the fit of `V.float()`; a float64 target is staged through an fp32
-        copy.  A float64 / half module is staged through fp32 copies and the result is written back into the same
-        Parameter storages in their own dtype.
+        copy.  A float64 / half module, or fp32 factors that are not contiguous, are staged through fp32 copies and the
+        result is written back into the same Parameter storages in their own dtype and layout.
 
         sparse V (NMF, a COO tensor): fitted without densifying it at every beta > 0 up to rank 256 -- the update terms at
         the stored entries only and, for beta != 1, 2, the denominators and the loss's sum (WH + eps)^beta from dense
@@ -517,79 +505,40 @@ class BaseComponent(torch.nn.Module):
         if weight is not None:
             self._check_weight(V, weight, precision)
             precision = "f32"
-        eng, W, H, Wd, Hd, staged = self._open_engine(V, beta, precision, group, sparse_kernels=True, mask=mask,
-                                                      weight=weight)
+        V = self._checked_target(V, beta, mask, weight)
+        W, H = self.W, self.H
+        with _placed_factors(self, (W, H), _NO_CUDA) as (dev, (Wd, Hd)):
+            eng = self._open_engine(V, dev, Wd, Hd, beta, precision, group, True, mask, weight)
+            try:
+                vmin, vmax = eng.minmax()
+                if mask is not None and vmin > vmax:                                       # +inf / -inf: nothing seen
+                    raise ValueError("mask: no cell of the target is observed")
+                if weight is not None and vmin > vmax:                                     # on every rank of a group
+                    raise ValueError("weight: every weight is zero")
+                assert vmin >= 0., "Target should be non-negative."                        # nmf.py:329-330
+                if vmin == 0 and beta <= 0:                                                # nmf.py:332-336
+                    raise ValueError("When beta <= 0 and V contains zeros, the training process may diverge. "
+                                     "Please add small values to V, or use a positive beta value.")
+                gamma = _gamma(beta)
+                l1_reg = alpha * l1_ratio                                                  # nmf.py:348
+                l2_reg = alpha * (1 - l1_ratio)                                            # nmf.py:349
+                train_w, train_h = W.requires_grad, H.requires_grad
 
-        try:
-            vmin, vmax = eng.minmax()
-            if mask is not None and vmin > vmax:                                           # +inf / -inf: nothing seen
-                raise ValueError("mask: no cell of the target is observed")
-            if weight is not None and vmin > vmax:                                         # on every rank of a group
-                raise ValueError("weight: every weight is zero")
-            assert vmin >= 0., "Target should be non-negative."                            # nmf.py:329-330
-            if vmin == 0 and beta <= 0:                                                    # nmf.py:332-336
-                raise ValueError("When beta <= 0 and V contains zeros, the training process may diverge. "
-                                 "Please add small values to V, or use a positive beta value.")
-            gamma = _gamma(beta)
-            l1_reg = alpha * l1_ratio                                                      # nmf.py:348
-            l2_reg = alpha * (1 - l1_ratio)                                                # nmf.py:349
+                def divergence(follows):
+                    # a W update follows on these very factors: the engine may take the loss out of that update's own
+                    # contraction pass (engine.loss_prefetch_w) instead of a pass over V of its own
+                    if follows and train_w and group is None and hasattr(eng, "loss_prefetch_w"):
+                        return eng.loss_prefetch_w(beta)
+                    return eng.loss(beta)
 
-            def fit_loss(more=False):
-                # `more`: a W update follows on these very factors -- the engine may take the loss out of that update's own
-                # contraction pass (engine.loss_prefetch_w) instead of a pass over V of its own
-                fold = more and hasattr(eng, "loss_prefetch_w")
-                d = eng.loss_prefetch_w(beta) if fold else eng.loss(beta)
-                return math.sqrt(2.0 * d) if d >= 0 else float("nan")                      # nmf.py:362,402
-
-            loss_init = fit_loss()
-            previous_loss = loss_init
-            train_w, train_h = W.requires_grad, H.requires_grad
-            bar = _tqdm(total=max_iter, disable=not verbose) if _tqdm is not None else _NullBar()
-            n_iter = -1
-            batched = train_w and train_h and group is None and hasattr(eng, "cd_iterate" if cd else "iterate")
-            with bar as pbar:
-                while batched and n_iter + 1 < max_iter:
-                    # both factors trainable: run the iterations up to the next loss evaluation in one engine call
-                    k = min(10 - ((n_iter + 1) % 10), max_iter - (n_iter + 1))
-                    if cd:
-                        eng.cd_iterate(k, l1_reg, l2_reg)
-                    else:
-                        eng.iterate(k, beta, gamma, l1_reg, l2_reg)                        # nmf.py:366-391, k times
-                    n_iter += k
-                    if n_iter % 10 == 9:                                                   # nmf.py:393
-                        loss = fit_loss(more=n_iter + 1 < max_iter)
-                        pbar.set_postfix(loss=loss)
-                        pbar.update(10)
-                        if (previous_loss - loss) / loss_init < tol:                       # nmf.py:405
-                            break
-                        previous_loss = loss
-                for n_iter in (range(max_iter) if not batched else ()):                    # nmf.py:366
-                    if train_w:
-                        if cd:
-                            eng.cd_update(0, l1_reg, l2_reg)
-                        else:
-                            eng.update_w(beta, gamma, l1_reg, l2_reg)                      # nmf.py:367-378
-                    if train_h:
-                        if cd:
-                            eng.cd_update(1, l1_reg, l2_reg)
-                        else:
-                            eng.update_h(beta, gamma, l1_reg, l2_reg)                      # nmf.py:380-391
-                    if n_iter % 10 == 9:                                                   # nmf.py:393
-                        loss = fit_loss(more=train_w and group is None and n_iter + 1 < max_iter)
-                        pbar.set_postfix(loss=loss)
-                        pbar.update(10)
-                        if (previous_loss - loss) / loss_init < tol:                       # nmf.py:405
-                            break
-                        previous_loss = loss
-            if hasattr(eng, "check_health"):
-                eng.check_health()
-            if staged:
-                W.data.copy_(Wd)
-                H.data.copy_(Hd)
-            self.last_fit_precision = eng.precision_for(beta) if hasattr(eng, "precision_for") else eng.precision
-            self.last_w_update_path = getattr(eng, "w_update_path", None)     # sharded fits: "peer" (NVLink P2P) or "nccl"
-        finally:
-            eng.close()
+                step = _update_step(eng, cd, train_w, train_h, beta, gamma, l1_reg, l2_reg)
+                n_iter = _fit_single(step, divergence, max_iter, tol, verbose)
+                if hasattr(eng, "check_health"):
+                    eng.check_health()
+                self.last_fit_precision = eng.precision_for(beta) if hasattr(eng, "precision_for") else eng.precision
+                self.last_w_update_path = getattr(eng, "w_update_path", None)  # sharded fits: "peer" (NVLink P2P) or "nccl"
+            finally:
+                eng.close()
         return n_iter + 1                                                                  # nmf.py:409
 
 
@@ -613,75 +562,75 @@ class BaseComponent(torch.nn.Module):
                        or (sH is not None and self.H is not None and self.H.requires_grad))
         if precision == "auto" and constrained:
             precision = "f32"
-        eng, W, H, Wd, Hd, staged = self._open_engine(V, beta, precision, None, sparse_kernels=False)
-        try:
-            vmin, vmax = eng.minmax()
-            assert vmin >= 0., "Target should be non-negative."                            # nmf.py:447-448
-            if vmin == 0 and beta <= 0:                                                    # nmf.py:450-454
-                raise ValueError("When beta <= 0 and V contains zeros, the training process may diverge. "
-                                 "Please add small values to V, or use a positive beta value.")
-            train_w, train_h = W.requires_grad, H.requires_grad
-            R = Wd.shape[1]
-            L1a = L1s = None
-            if sW is not None and train_w:                                                 # nmf.py:459-467
-                L1a = Wd[:, 0].numel() ** 0.5 * (1 - sW) + sW
-                eng.project(Wd, 1, [L1a] * R, [1.0] * R)
-            if sH is not None and train_h:                                                 # nmf.py:469-477
-                L1s = Hd[:, 0].numel() ** 0.5 * (1 - sH) + sH
-                eng.project(Hd, 1, [L1s] * R, [1.0] * R)
-            eng.sync()
-            gamma = _gamma(beta)                                                           # nmf.py:479-484
-            step = {0: 1.0, 1: 1.0}                                                        # nmf.py:490
-
-            def projected_step(which, L1):
-                """nmf.py:513-538 (W) / :559-586 (H): gradient step, projection of every component, halving line search."""
-                cur = Wd if which == 0 else Hd
-                loss = eng.loss(beta)
-                num, den = eng.raw_terms(which, beta)
-                if beta == 1:
-                    den = den.view((1, -1) + (1,) * (cur.dim() - 2))                       # colsum of the other factor
-                grad = den - num
-                for _ in range(10):
-                    new = cur - step[which] * grad
-                    norms = _get_norm(new)
-                    eng.project(new, 1, L1 * norms, norms * norms)
-                    new_loss = eng.loss_at(new if which == 0 else Wd, Hd if which == 0 else new, beta)
-                    if new_loss <= loss:
-                        break
-                    step[which] *= 0.5
-                step[which] *= 1.2
-                cur.copy_(new)
+        V = self._checked_target(V, beta)
+        W, H = self.W, self.H
+        with _placed_factors(self, (W, H), _NO_CUDA) as (dev, (Wd, Hd)):
+            eng = self._open_engine(V, dev, Wd, Hd, beta, precision, None, False)
+            try:
+                vmin, vmax = eng.minmax()
+                assert vmin >= 0., "Target should be non-negative."                        # nmf.py:447-448
+                if vmin == 0 and beta <= 0:                                                # nmf.py:450-454
+                    raise ValueError("When beta <= 0 and V contains zeros, the training process may diverge. "
+                                     "Please add small values to V, or use a positive beta value.")
+                train_w, train_h = W.requires_grad, H.requires_grad
+                R = Wd.shape[1]
+                L1a = L1s = None
+                if sW is not None and train_w:                                             # nmf.py:459-467
+                    L1a = Wd[:, 0].numel() ** 0.5 * (1 - sW) + sW
+                    eng.project(Wd, 1, [L1a] * R, [1.0] * R)
+                if sH is not None and train_h:                                             # nmf.py:469-477
+                    L1s = Hd[:, 0].numel() ** 0.5 * (1 - sH) + sH
+                    eng.project(Hd, 1, [L1s] * R, [1.0] * R)
                 eng.sync()
+                gamma = _gamma(beta)                                                       # nmf.py:479-484
+                step = {0: 1.0, 1: 1.0}                                                    # nmf.py:490
 
-            bar = _tqdm(total=max_iter, disable=not verbose) if _tqdm is not None else _NullBar()
-            n_iter = -1
-            with bar as pbar:
-                for n_iter in range(max_iter):
-                    if train_w:
-                        if L1a is None:
-                            eng.update_w(beta, gamma, 0.0, 0.0)                            # nmf.py:503-511
-                        else:
-                            projected_step(0, L1a)
-                    if train_h:
-                        if L1s is None:
-                            eng.update_h(beta, gamma, 0.0, 0.0)                            # nmf.py:549-557
-                        else:
-                            projected_step(1, L1s)
-                        _renorm(Wd, Hd, "H")                                               # nmf.py:588
-                        eng.sync()
-                    if n_iter % 10 == 9 and verbose:                                       # nmf.py:590-598 (display only)
-                        d = eng.loss(beta)
-                        pbar.set_postfix(loss=math.sqrt(2.0 * d) if d >= 0 else float("nan"))
-                        pbar.update(10)
-            if hasattr(eng, "check_health"):
-                eng.check_health()
-            if staged:
-                W.data.copy_(Wd)
-                H.data.copy_(Hd)
-            self.last_fit_precision = eng.precision_for(beta) if hasattr(eng, "precision_for") else eng.precision
-        finally:
-            eng.close()
-        return n_iter + 1                                                                  # nmf.py:599
+                def projected_step(which, L1):
+                    """nmf.py:513-538 (W) / :559-586 (H): gradient step, projection of every component, halving line
+                    search."""
+                    cur = Wd if which == 0 else Hd
+                    loss = eng.loss(beta)
+                    num, den = eng.raw_terms(which, beta)
+                    if beta == 1:
+                        den = den.view((1, -1) + (1,) * (cur.dim() - 2))                   # colsum of the other factor
+                    grad = den - num
+                    for _ in range(10):
+                        new = cur - step[which] * grad
+                        norms = _get_norm(new)
+                        eng.project(new, 1, L1 * norms, norms * norms)
+                        new_loss = eng.loss_at(new if which == 0 else Wd, Hd if which == 0 else new, beta)
+                        if new_loss <= loss:
+                            break
+                        step[which] *= 0.5
+                    step[which] *= 1.2
+                    cur.copy_(new)
+                    eng.sync()
+
+                n_iter = -1
+                with _tqdm(total=max_iter, disable=not verbose) as pbar:
+                    for n_iter in range(max_iter):
+                        if train_w:
+                            if L1a is None:
+                                eng.update_w(beta, gamma, 0.0, 0.0)                        # nmf.py:503-511
+                            else:
+                                projected_step(0, L1a)
+                        if train_h:
+                            if L1s is None:
+                                eng.update_h(beta, gamma, 0.0, 0.0)                        # nmf.py:549-557
+                            else:
+                                projected_step(1, L1s)
+                            _renorm(Wd, Hd, "H")                                           # nmf.py:588
+                            eng.sync()
+                        if n_iter % 10 == 9 and verbose:                                   # nmf.py:590-598 (display only)
+                            d = eng.loss(beta)
+                            pbar.set_postfix(loss=math.sqrt(2.0 * d) if d >= 0 else float("nan"))
+                            pbar.update(10)
+                if hasattr(eng, "check_health"):
+                    eng.check_health()
+                self.last_fit_precision = eng.precision_for(beta) if hasattr(eng, "precision_for") else eng.precision
+            finally:
+                eng.close()
+        return n_iter + 1                                                              # nmf.py:599
 
 
 class NMF(BaseComponent):
@@ -738,7 +687,7 @@ class NMFD(BaseComponent):
                                f"W {tuple(self.W.shape)}")
 
 
-# ---- many independent problems in one fit: what the batched NMF and PLCA classes share ------------------------------------
+# ---- what the fits share: factor registration (batched), placement, update step and stop rules -----------------------------
 
 def _register_batched_factors(module, W, H, trainable_W, trainable_H):
     """Register W and H on a batched module (problems on axis 0, rank on axis 2): a Tensor is copied, an iterable of ints
@@ -773,7 +722,7 @@ def _register_batched_factors(module, W, H, trainable_W, trainable_H):
 
 @contextlib.contextmanager
 def _placed_factors(module, factors, no_cuda, real=None):
-    """Places a batched fit: yields (device, the fp32 contiguous tensors the engine updates, one per Parameter of
+    """Places a fit: yields (device, the fp32 contiguous tensors the engine updates, one per Parameter of
     `factors`).  They are the Parameters' own storages when every factor is fp32 and contiguous on a CUDA device, else
     device copies, written back into the Parameters when the block completes.  Without CUDA it raises
     RuntimeError(no_cuda).  With the `_engine_factory` test hook the storages are taken where they are.  `real` (a bool
@@ -799,6 +748,58 @@ def _placed_factors(module, factors, no_cuda, real=None):
                 t.data.copy_(d)
 
 
+def _update_step(eng, cd, train_w, train_h, beta, gamma, l1_reg, l2_reg):
+    """step(k) of `fit`: k iterations of the multiplicative updates (`cd`: of coordinate descent) of the trainable factors,
+    W then H.  They run in one engine call when both factors train and the engine has it, else in one call per update."""
+    fused = train_w and train_h and hasattr(eng, "cd_iterate" if cd else "iterate")
+
+    def step(k):
+        if fused and cd:
+            eng.cd_iterate(k, l1_reg, l2_reg)
+        elif fused:
+            eng.iterate(k, beta, gamma, l1_reg, l2_reg)                                    # nmf.py:366-391, k times
+        else:
+            for _ in range(k):
+                if train_w:
+                    if cd:
+                        eng.cd_update(0, l1_reg, l2_reg)
+                    else:
+                        eng.update_w(beta, gamma, l1_reg, l2_reg)                          # nmf.py:367-378
+                if train_h:
+                    if cd:
+                        eng.cd_update(1, l1_reg, l2_reg)
+                    else:
+                        eng.update_h(beta, gamma, l1_reg, l2_reg)                          # nmf.py:380-391
+    return step
+
+
+def _fit_single(step, divergence, max_iter, tol, verbose):
+    """The reference's stop rule (nmf.py:366-409, plca.py:245-302) for one problem: the loss sqrt(2 d) (NaN for d < 0) of
+    the raw divergence d = `divergence(follows)` before the first iteration and after every 10th, stopping at the first
+    check where (previous - loss) / initial < tol.  `follows` says whether iterations follow the check (False for the
+    initial loss).  `step(k)` runs k iterations, at most 10 and never past a check.  Returns the last loop index: the
+    iterations run, minus one."""
+    def fit_loss(follows):
+        d = divergence(follows)
+        return math.sqrt(2.0 * d) if d >= 0 else float("nan")                              # nmf.py:362,402
+
+    loss_init = previous = fit_loss(False)
+    it = -1
+    with _tqdm(total=max_iter, disable=not verbose) as pbar:
+        while it + 1 < max_iter:
+            k = min(10 - ((it + 1) % 10), max_iter - (it + 1))
+            step(k)
+            it += k
+            if it % 10 == 9:                                                               # nmf.py:393
+                loss = fit_loss(it + 1 < max_iter)
+                pbar.set_postfix(loss=loss)
+                pbar.update(10)
+                if (previous - loss) / loss_init < tol:                                    # nmf.py:405
+                    break
+                previous = loss
+    return it
+
+
 def _fit_problems(eng, P, max_iter, tol, verbose, losses, step):
     """The reference's stop rule (nmf.py:366-409, plca.py:245-302) for each of P problems fitted together on `eng`: problem
     p's loss sqrt(2 d_p) (NaN for d_p < 0) from `losses()`, the P raw divergences, at the start and every 10th iteration,
@@ -813,9 +814,8 @@ def _fit_problems(eng, P, max_iter, tol, verbose, losses, step):
     previous = loss_init.clone()
     n_iter = torch.full((P,), max_iter, dtype=torch.int64)
     active = torch.ones(P, dtype=torch.bool)
-    bar = _tqdm(total=max_iter, disable=not verbose) if _tqdm is not None else _NullBar()
     it = -1
-    with bar as pbar:
+    with _tqdm(total=max_iter, disable=not verbose) as pbar:
         while it + 1 < max_iter and bool(active.any()):
             k = min(10 - ((it + 1) % 10), max_iter - (it + 1))
             step(k)
@@ -969,12 +969,11 @@ class _BatchedComponent(BaseComponent):
             raise ValueError(f"{name} supports rank <= 256 (got {W.shape[2]})")
         self._check_target_shape(V)
 
-        no_cuda = "torchnmf_b200.fit needs a CUDA device (sm_90a); there is no CPU fallback"
         real = None                # a ragged batch: the real cells of H, the only ones written back from a staged copy
         if lengths is not None:
             real = self._real_cells(lengths)
         ragged = {} if lengths is None else {"lengths": lengths}
-        with _placed_factors(self, (W, H), no_cuda, real) as (dev, (Wd, Hd)):
+        with _placed_factors(self, (W, H), _NO_CUDA, real) as (dev, (Wd, Hd)):
             if self._engine_factory is None:
                 Vd = V.to(dev, non_blocking=True)
                 if Vd.dtype not in (torch.float32, torch.float16, torch.bfloat16):
@@ -993,26 +992,7 @@ class _BatchedComponent(BaseComponent):
                 gamma = _gamma(beta)
                 l1_reg = alpha * l1_ratio                                                  # nmf.py:348
                 l2_reg = alpha * (1 - l1_ratio)                                            # nmf.py:349
-                train_w, train_h = W.requires_grad, H.requires_grad
-
-                def step(k):
-                    if cd and train_w and train_h:
-                        eng.cd_iterate(k, l1_reg, l2_reg)
-                    elif cd:
-                        for _ in range(k):
-                            if train_w:
-                                eng.cd_update(0, l1_reg, l2_reg)
-                            if train_h:
-                                eng.cd_update(1, l1_reg, l2_reg)
-                    elif train_w and train_h and hasattr(eng, "iterate"):
-                        eng.iterate(k, beta, gamma, l1_reg, l2_reg)                        # nmf.py:366-391, k times
-                    else:
-                        for _ in range(k):
-                            if train_w:
-                                eng.update_w(beta, gamma, l1_reg, l2_reg)                  # nmf.py:367-378
-                            if train_h:
-                                eng.update_h(beta, gamma, l1_reg, l2_reg)                  # nmf.py:380-391
-
+                step = _update_step(eng, cd, W.requires_grad, H.requires_grad, beta, gamma, l1_reg, l2_reg)
                 n_iter = _fit_problems(eng, W.shape[0], max_iter, tol, verbose, lambda: eng.losses(beta), step)
                 self.last_fit_precision = "f32"
             finally:

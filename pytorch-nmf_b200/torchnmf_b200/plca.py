@@ -15,7 +15,6 @@ The shift-invariant models (plca.py:376-625) are the same EM step around the con
 `sum_{r,t} W[c,r,t] Z[r] H[b,r,x-t]`: the factor pair handed to the library is (W, H Z) as well, and the two gradients are
 the sliding contractions of `nmfb200_raw_terms` (wgrad and dgrad of the ratio tile; csrc/nmfd.cu, csrc/tc_nmfd.cu).
 """
-import math
 from collections.abc import Iterable as _Iterable
 
 import torch
@@ -25,14 +24,9 @@ from torch.nn import Parameter
 
 from .constants import eps
 from . import engine as _engine
-from .nmf import _batched_conv, _fit_problems, _placed_factors, _register_batched_factors
+from .nmf import _batched_conv, _fit_problems, _fit_single, _placed_factors, _register_batched_factors
 
 from torch.nn.modules.utils import _single, _pair, _triple
-
-try:
-    from tqdm import tqdm as _tqdm
-except Exception:  # pragma: no cover
-    _tqdm = None
 
 __all__ = ["PLCA", "SIPLCA", "SIPLCA2", "SIPLCA3", "BaseComponent", "BatchedPLCA", "BatchedSIPLCA", "BatchedSIPLCA2",
            "BatchedSIPLCA3"]
@@ -147,41 +141,33 @@ class BaseComponent(torch.nn.Module):
         assert torch.all(V >= 0.), "Target should be non-negative."                         # plca.py:236
         W, H, Z = self.W, self.H, self.Z
         assert W is not None and H is not None and Z is not None, "fit() needs W, H and Z"
-        if not torch.cuda.is_available():
-            raise RuntimeError("torchnmf_b200.PLCA.fit needs a CUDA device (sm_90a); there is no CPU fallback")
-        f32 = torch.float32
-        on_gpu = W.device.type == "cuda"
-        dev = W.device if on_gpu else torch.device("cuda", torch.cuda.current_device())
-        norm = V.sum()
-        Vn = (V.to(dev, f32).contiguous() / norm.to(dev, f32)).contiguous()                  # plca.py:241-242
-        stage = not (on_gpu and all(t.dtype == f32 for t in (W, H, Z)))
-        Wd = W.data.to(dev, f32).contiguous() if stage else W.data
-        Hd = H.data.to(dev, f32).contiguous() if stage else H.data
-        Zd = Z.data.to(dev, f32).contiguous() if stage else Z.data
-        normd = norm.to(dev, f32)
-        Vfull = Vn * normd
+        no_cuda = "torchnmf_b200.PLCA.fit needs a CUDA device (sm_90a); there is no CPU fallback"
+        with _placed_factors(self, (W, H, Z), no_cuda) as (dev, (Wd, Hd, Zd)):
+            f32 = torch.float32
+            norm = V.sum()
+            Vn = (V.to(dev, f32).contiguous() / norm.to(dev, f32)).contiguous()              # plca.py:241-242
+            normd = norm.to(dev, f32)
+            Vfull = Vn * normd
 
-        def loss_now():
-            WZH = self.reconstruct(Hd, Wd, Zd)
-            d = float(_kl(WZH * normd, Vfull))
-            return math.sqrt(2.0 * d) if d >= 0 else float("nan")                           # plca.py:245-246,293-294
+            def divergence(follows):
+                return float(_kl(self.reconstruct(Hd, Wd, Zd) * normd, Vfull))            # plca.py:245-246,293-294
 
-        Hz = (Hd * _over(Zd, Hd)).contiguous()        # the engine's activation factor: H diag(Z)
-        eng = self._engine(Vn, Wd, Hz, precision)
-        try:
-            def step():
-                torch.mul(Hd, _over(Zd, Hd), out=Hz)
-                eng.sync()
-                dW, _ = eng.raw_terms(0, 1.0)         # P contracted with H Z  = W.grad   (plca.py:252-253)
-                dHz, _ = eng.raw_terms(1, 1.0)        # P contracted with W;  H.grad = dHz * Z,  Z.grad = sum H dHz
-                self._em_update(Wd, Hd, Zd, dW, dHz, W_alpha, H_alpha, Z_alpha)
+            Hz = (Hd * _over(Zd, Hd)).contiguous()        # the engine's activation factor: H diag(Z)
+            eng = self._engine(Vn, Wd, Hz, precision) if self._engine_factory is None else self._engine_factory(Vn, Wd, Hz)
+            try:
+                def step(k):
+                    for _ in range(k):
+                        torch.mul(Hd, _over(Zd, Hd), out=Hz)
+                        eng.sync()
+                        dW, _ = eng.raw_terms(0, 1.0)     # P contracted with H Z  = W.grad   (plca.py:252-253)
+                        dHz, _ = eng.raw_terms(1, 1.0)    # P contracted with W;  H.grad = dHz * Z,  Z.grad = sum H dHz
+                        self._em_update(Wd, Hd, Zd, dW, dHz, W_alpha, H_alpha, Z_alpha)
 
-            n_iter = _em_loop(step, loss_now, tol, max_iter, verbose, eng.check_health)
-            self.last_fit_precision = eng.precision_for(1.0)
-        finally:
-            eng.close()
-        if stage:
-            W.data.copy_(Wd); H.data.copy_(Hd); Z.data.copy_(Zd)
+                n_iter = _fit_single(step, divergence, max_iter, tol, verbose)
+                eng.check_health()
+                self.last_fit_precision = eng.precision_for(1.0)
+            finally:
+                eng.close()
         return n_iter, norm                                                                  # plca.py:304
 
     def _em_update(self, Wd, Hd, Zd, dW, dHz, W_alpha, H_alpha, Z_alpha):
@@ -244,59 +230,51 @@ class BaseComponent(torch.nn.Module):
         M, norm_o = self._check_mask(V, mask, precision)
         W, H, Z = self.W, self.H, self.Z
         assert W is not None and H is not None and Z is not None, "fit() needs W, H and Z"
-        if not torch.cuda.is_available():
-            raise RuntimeError(f"torchnmf_b200.{type(self).__name__}.fit needs a CUDA device (sm_90a); there is no CPU "
-                               "fallback")
-        f32 = torch.float32
-        on_gpu = W.device.type == "cuda"
-        dev = W.device if on_gpu else torch.device("cuda", torch.cuda.current_device())
-        Md = M.to(dev).contiguous()
-        normd = norm_o.to(dev, f32)
-        # Vn on O and 0 off O: the kernels never meet what V holds at the missing cells
-        Vn = (torch.where(Md, V.to(dev, f32), torch.zeros((), dtype=f32, device=dev)) / normd).contiguous()
-        stage = not (on_gpu and all(t.dtype == f32 for t in (W, H, Z)))
-        Wd = W.data.to(dev, f32).contiguous() if stage else W.data
-        Hd = H.data.to(dev, f32).contiguous() if stage else H.data
-        Zd = Z.data.to(dev, f32).contiguous() if stage else Z.data
-        Vobs = Vn * normd
+        no_cuda = f"torchnmf_b200.{type(self).__name__}.fit needs a CUDA device (sm_90a); there is no CPU fallback"
+        with _placed_factors(self, (W, H, Z), no_cuda) as (dev, (Wd, Hd, Zd)):
+            f32 = torch.float32
+            Md = M.to(dev).contiguous()
+            normd = norm_o.to(dev, f32)
+            # Vn on O and 0 off O: the kernels never meet what V holds at the missing cells
+            Vn = (torch.where(Md, V.to(dev, f32), torch.zeros((), dtype=f32, device=dev)) / normd).contiguous()
+            Vobs = Vn * normd
 
-        def q_obs():
-            q = self.reconstruct(Hd, Wd, Zd)
-            return q, torch.where(Md, q, 0.).sum()
+            def divergence(follows):
+                # kl_div(x[O], V[O]) with the model scaled to the observed mass, x = q sum_O V / q_O; Vobs is 0 off O
+                q = self.reconstruct(Hd, Wd, Zd)
+                x = q * (normd / torch.where(Md, q, 0.).sum())
+                return float(Vobs.reshape(-1) @ (torch.log(Vobs + eps) - torch.log(x + eps)).reshape(-1) - Vobs.sum()
+                             + torch.where(Md, x, 0.).sum())
 
-        def loss_now():
-            # kl_div(x[O], V[O]) with the model scaled to the observed mass, x = q sum_O V / q_O; Vobs is 0 off O
-            q, qo = q_obs()
-            x = q * (normd / qo)
-            d = float(Vobs.reshape(-1) @ (torch.log(Vobs + eps) - torch.log(x + eps)).reshape(-1) - Vobs.sum()
-                      + torch.where(Md, x, 0.).sum())
-            return math.sqrt(2.0 * d) if d >= 0 else float("nan")
+            Hz = (Hd * _over(Zd, Hd)).contiguous()
+            qobs = torch.zeros(1, dtype=torch.float64, device=dev)
+            eng = self._engine(Vn, Wd, Hz, precision) if self._engine_factory is None else self._engine_factory(Vn, Wd, Hz)
+            try:
+                eng.set_mask(Md)
 
-        Hz = (Hd * _over(Zd, Hd)).contiguous()
-        qobs = torch.zeros(1, dtype=torch.float64, device=dev)
-        eng = self._engine(Vn, Wd, Hz, precision)
-        try:
-            eng.set_mask(Md)
+                def step(k):
+                    # the reference's EM step on the completed target q_O Vn (O) / q (off O): its gradients are q_O A + B
+                    for _ in range(k):
+                        torch.mul(Hd, _over(Zd, Hd), out=Hz)
+                        eng.sync()
+                        aW, bW = eng.plca_masked_terms(0, qobs)
+                        aH, bH = eng.plca_masked_terms(1)
+                        q = qobs.to(f32)
+                        self._em_update(Wd, Hd, Zd, torch.addcmul(bW, aW, q), torch.addcmul(bH, aH, q), W_alpha, H_alpha,
+                                        Z_alpha)
 
-            def step():
-                # the reference's EM step on the completed target q_O Vn (O) / q (off O): its gradients are q_O A + B
-                torch.mul(Hd, _over(Zd, Hd), out=Hz)
-                eng.sync()
-                aW, bW = eng.plca_masked_terms(0, qobs)
-                aH, bH = eng.plca_masked_terms(1)
-                q = qobs.to(f32)
-                self._em_update(Wd, Hd, Zd, torch.addcmul(bW, aW, q), torch.addcmul(bH, aH, q), W_alpha, H_alpha, Z_alpha)
-
-            n_iter = _em_loop(step, loss_now, tol, max_iter, verbose, eng.check_health)
-            self.last_fit_precision = "f32"
-        finally:
-            eng.close()
-        # the returned norm's q_O in float64 (the fp32 reconstruction may run on TF32 convolutions)
-        q = self.reconstruct(Hd.double(), Wd.double(), Zd.double())
-        qo = torch.where(Md, q, 0.).sum()
-        if stage:
-            W.data.copy_(Wd); H.data.copy_(Hd); Z.data.copy_(Zd)
+                n_iter = _fit_single(step, divergence, max_iter, tol, verbose)
+                eng.check_health()
+                self.last_fit_precision = "f32"
+            finally:
+                eng.close()
+            # the returned norm's q_O in float64 (the fp32 reconstruction may run on TF32 convolutions)
+            q = self.reconstruct(Hd.double(), Wd.double(), Zd.double())
+            qo = torch.where(Md, q, 0.).sum()
         return n_iter, (norm_o.double() / qo.to(norm_o.device)).to(norm_o.dtype)
+
+    # test hook, as the NMF modules' (tests/test_plca.py): factory(Vn, W, Hz) stands in for `_engine`
+    _engine_factory = None
 
     @staticmethod
     def _engine(Vn, W, Hz, precision):
@@ -306,28 +284,6 @@ class BaseComponent(torch.nn.Module):
 def _over(z, x):
     """A rank vector against the rank dimension (1) of a factor (plca.py:269-270,282-283)."""
     return z[(slice(None),) + (None,) * (x.dim() - 2)]
-
-
-def _em_loop(step, loss_now, tol, max_iter, verbose, check_health):
-    """The reference's iteration loop (plca.py:247-302): `step()` max_iter times, the loss before the first and after every
-    10th, stopping at the first check where (previous - loss) / initial < tol.  Returns the last loop index."""
-    loss_init = previous_loss = loss_now()
-    bar = _tqdm(total=max_iter, disable=not verbose) if _tqdm is not None else None
-    n_iter = -1
-    for n_iter in range(max_iter):
-        step()
-        if n_iter % 10 == 9:                                                                 # plca.py:290-302
-            loss = loss_now()
-            if bar is not None:
-                bar.set_postfix(loss=loss)
-                bar.update(10)
-            if (previous_loss - loss) / loss_init < tol:
-                break
-            previous_loss = loss
-    check_health()
-    if bar is not None:
-        bar.close()
-    return n_iter
 
 
 def _is_one(a):
@@ -458,7 +414,6 @@ class _BatchedPLCABase(BaseComponent):
     _ndim = 3
     _axes = "three axes (P, rows, rank)"
     _engine_cls = None
-    _engine_factory = None
 
     def __init__(self, rank=None, W=None, H=None, Z=None, trainable_W=True, trainable_H=True, trainable_Z=True):
         torch.nn.Module.__init__(self)

@@ -83,3 +83,15 @@ class OracleNmfdEngine(_OracleEngine):
 
     def update_h(self, beta, gamma, l1, l2):
         self.H.copy_(orc.nmfd_update_h(self.V, self.W, self.H, beta, gamma, l1, l2))
+
+
+class OracleNmfndEngine(_OracleEngine):
+    """One NMF2D / NMF3D problem on the CPU oracle (oracle/mu_oracle.py: nmfnd_*)."""
+    kind = "nmfd"
+    _recon = staticmethod(orc.nmfnd_reconstruct)
+
+    def update_w(self, beta, gamma, l1, l2):
+        self.W.copy_(orc.nmfnd_update_w(self.V, self.W, self.H, beta, gamma, l1, l2))
+
+    def update_h(self, beta, gamma, l1, l2):
+        self.H.copy_(orc.nmfnd_update_h(self.V, self.W, self.H, beta, gamma, l1, l2))

@@ -9,68 +9,9 @@ import pytest
 import torch
 
 from conftest import GOLDEN
+from batched_oracle import BatchedOracleEngine
 from oracle_engine import OracleNmfEngine
 from torchnmf_b200 import NMF, BatchedNMF
-
-
-class BatchedOracleEngine:
-    """The batched engine interface (engine.CudaBatchedNmfEngine) over one oracle engine per problem.  Counts the updates
-    each problem receives, so a test can see that a stopped problem is never touched again."""
-    kind = "nmf_batched"
-    device = torch.device("cpu")
-    precision = "oracle"
-
-    def __init__(self, V, W, H):
-        B = W.shape[0]
-        if V.dim() == 2:
-            V = V.expand(B, *V.shape)
-        self.V = V.float()
-        self.W, self.H = W, H
-        self.engines = [OracleNmfEngine(self.V[b], W[b], H[b]) for b in range(B)]
-        self.active = [True] * B
-        self.updates_w = [0] * B
-        self.updates_h = [0] * B
-        self._last = torch.full((B,), float("nan"), dtype=torch.float64)
-
-    def close(self):
-        pass
-
-    def minmax(self):
-        return float(self.V.min()), float(self.V.max())
-
-    def set_active(self, active):
-        self.active = [bool(a) for a in active]
-
-    def update_w(self, beta, gamma, l1, l2):
-        for b, e in enumerate(self.engines):
-            if self.active[b]:
-                e.update_w(beta, gamma, l1, l2)
-                self.updates_w[b] += 1
-
-    def update_h(self, beta, gamma, l1, l2):
-        for b, e in enumerate(self.engines):
-            if self.active[b]:
-                e.update_h(beta, gamma, l1, l2)
-                self.updates_h[b] += 1
-
-    def iterate(self, k, beta, gamma, l1, l2):
-        for _ in range(k):
-            self.update_w(beta, gamma, l1, l2)
-            self.update_h(beta, gamma, l1, l2)
-
-    def losses(self, beta):
-        for b, e in enumerate(self.engines):
-            if self.active[b]:
-                self._last[b] = e.loss(beta)
-        return self._last.clone()
-
-    @classmethod
-    def factory(cls, log):
-        def make(V, W, H):
-            eng = cls(V, W, H)
-            log.append(eng)
-            return eng
-        return make
 
 
 def _single_oracle(V, W0, H0, **kw):
@@ -82,7 +23,7 @@ def _single_oracle(V, W0, H0, **kw):
 
 def _batched(V, W0, H0, trainable_W=True, trainable_H=True, log=None, **kw):
     m = BatchedNMF(W=W0, H=H0, trainable_W=trainable_W, trainable_H=trainable_H)
-    m._engine_factory = BatchedOracleEngine.factory([] if log is None else log)
+    m._engine_factory = BatchedOracleEngine.factory(OracleNmfEngine, [] if log is None else log)
     n = m.fit(V, **kw)
     return n, m.W.data.clone(), m.H.data.clone(), m
 
@@ -194,7 +135,7 @@ def test_constructor_shapes():
 def test_refusals():
     V, W0, H0 = _inputs()
     m = BatchedNMF(W=W0, H=H0)
-    m._engine_factory = BatchedOracleEngine.factory([])
+    m._engine_factory = BatchedOracleEngine.factory(OracleNmfEngine, [])
     for prec in ("f16", "f16_split", "bogus"):
         with pytest.raises(ValueError):
             m.fit(V, precision=prec)
@@ -213,7 +154,7 @@ def test_refusals():
     with pytest.raises(ValueError):
         m.fit(torch.cat([V[:, :1] * 0, V[:, 1:]], 1), beta=0)
     big = BatchedNMF(W=torch.rand(1, 4, 257), H=torch.rand(1, 3, 257))
-    big._engine_factory = BatchedOracleEngine.factory([])
+    big._engine_factory = BatchedOracleEngine.factory(OracleNmfEngine, [])
     with pytest.raises(ValueError):
         big.fit(torch.rand(1, 3, 4))
 

@@ -7,86 +7,11 @@ import os
 import pytest
 import torch
 
+from batched_oracle import BatchedOracleEngine
 from test_cd import CdOracleEngine
 from torchnmf_b200 import NMF, BatchedNMF, BatchedNMF2D, BatchedNMF3D, BatchedNMFD
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-class BatchedCdOracleEngine:
-    """The batched engine interface (engine.CudaBatchedNmfEngine) over one CdOracleEngine per problem.  Logs every call and
-    counts the factor updates each problem receives, so a test can see that a stopped problem is never touched again."""
-    kind = "nmf_batched"
-    device = torch.device("cpu")
-    precision = "oracle"
-
-    def __init__(self, V, W, H):
-        B = W.shape[0]
-        if V.dim() == 2:
-            V = V.expand(B, *V.shape)
-        self.V, self.W, self.H = V, W, H
-        self.engines = [CdOracleEngine(V[b], W[b], H[b]) for b in range(B)]
-        self.active = [True] * B
-        self.updates_w = [0] * B
-        self.updates_h = [0] * B
-        self.calls = []
-        self._last = torch.full((B,), float("nan"), dtype=torch.float64)
-
-    def close(self):
-        pass
-
-    def minmax(self):
-        return float(self.V.min()), float(self.V.max())
-
-    def set_active(self, active):
-        self.active = [bool(a) for a in active]
-
-    def _each(self, fn, which):
-        for b, e in enumerate(self.engines):
-            if self.active[b]:
-                fn(e)
-                if which == 0:
-                    self.updates_w[b] += 1
-                else:
-                    self.updates_h[b] += 1
-
-    def update_w(self, *a):
-        self.calls.append(("update_w",) + a)
-        self._each(lambda e: e.update_w(*a), 0)
-
-    def update_h(self, *a):
-        self.calls.append(("update_h",) + a)
-        self._each(lambda e: e.update_h(*a), 1)
-
-    def iterate(self, k, *a):
-        self.calls.append(("iterate", k) + a)
-        for _ in range(k):
-            self._each(lambda e: e.update_w(*a), 0)
-            self._each(lambda e: e.update_h(*a), 1)
-
-    def cd_update(self, which, l1, l2):
-        self.calls.append(("cd_update", which, l1, l2))
-        self._each(lambda e: e.cd_update(which, l1, l2), which)
-
-    def cd_iterate(self, k, l1, l2):
-        self.calls.append(("cd_iterate", k, l1, l2))
-        for _ in range(k):
-            self._each(lambda e: e.cd_update(0, l1, l2), 0)
-            self._each(lambda e: e.cd_update(1, l1, l2), 1)
-
-    def losses(self, beta):
-        for b, e in enumerate(self.engines):
-            if self.active[b]:
-                self._last[b] = e.loss(beta)
-        return self._last.clone()
-
-    @classmethod
-    def factory(cls, log):
-        def make(V, W, H):
-            eng = cls(V, W, H)
-            log.append(eng)
-            return eng
-        return make
 
 
 def _inputs(B=6, N=23, C=17, R=4, seed=0):
@@ -102,7 +27,7 @@ def _inputs(B=6, N=23, C=17, R=4, seed=0):
 def _batched(V, W0, H0, trainable_W=True, trainable_H=True, **kw):
     m = BatchedNMF(W=W0, H=H0, trainable_W=trainable_W, trainable_H=trainable_H).double()
     log = []
-    m._engine_factory = BatchedCdOracleEngine.factory(log)
+    m._engine_factory = BatchedOracleEngine.factory(CdOracleEngine, log)
     n = m.fit(V, **kw)
     eng, = log
     return n, m.W.data.clone(), m.H.data.clone(), eng, m

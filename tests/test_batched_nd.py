@@ -9,82 +9,14 @@ import pytest
 import torch
 
 from conftest import GOLDEN
-from oracle import mu_oracle as orc
-from oracle_engine import OracleNmfdEngine, _OracleEngine
+from batched_oracle import BatchedOracleEngine
+from oracle_engine import OracleNmfdEngine, OracleNmfndEngine
 from torchnmf_b200 import NMFD, NMF2D, NMF3D, BatchedNMF, BatchedNMFD, BatchedNMF2D, BatchedNMF3D
-
-
-class OracleNmfndEngine(_OracleEngine):
-    """One NMF2D / NMF3D problem on the CPU oracle (oracle/mu_oracle.py: nmfnd_*)."""
-    kind = "nmfd"
-    _recon = staticmethod(orc.nmfnd_reconstruct)
-
-    def update_w(self, beta, gamma, l1, l2):
-        self.W.copy_(orc.nmfnd_update_w(self.V, self.W, self.H, beta, gamma, l1, l2))
-
-    def update_h(self, beta, gamma, l1, l2):
-        self.H.copy_(orc.nmfnd_update_h(self.V, self.W, self.H, beta, gamma, l1, l2))
 
 
 SINGLE = {BatchedNMFD: (NMFD, OracleNmfdEngine), BatchedNMF2D: (NMF2D, OracleNmfndEngine),
           BatchedNMF3D: (NMF3D, OracleNmfndEngine)}
 CLASSES = {"nmfd": BatchedNMFD, "nmf2d": BatchedNMF2D, "nmf3d": BatchedNMF3D}
-
-
-class BatchedNdOracleEngine:
-    """The batched engine interface (engine.CudaBatchedNmfdEngine) over one oracle engine per problem: no `iterate`, as the
-    CUDA engine has none.  Counts the updates each problem receives, so a test can see that a stopped problem is never
-    touched again."""
-    kind = "nmfd_batched"
-    device = torch.device("cpu")
-    precision = "oracle"
-
-    def __init__(self, V, W, H, single):
-        P = W.shape[0]
-        if V.dim() == W.dim() - 1:
-            V = V.expand(P, *V.shape)
-        self.V = V.float()
-        self.W, self.H = W, H
-        self.engines = [single(self.V[p], W[p], H[p]) for p in range(P)]
-        self.active = [True] * P
-        self.updates_w = [0] * P
-        self.updates_h = [0] * P
-        self._last = torch.full((P,), float("nan"), dtype=torch.float64)
-
-    def close(self):
-        pass
-
-    def minmax(self):
-        return float(self.V.min()), float(self.V.max())
-
-    def set_active(self, active):
-        self.active = [bool(a) for a in active]
-
-    def update_w(self, beta, gamma, l1, l2):
-        for p, e in enumerate(self.engines):
-            if self.active[p]:
-                e.update_w(beta, gamma, l1, l2)
-                self.updates_w[p] += 1
-
-    def update_h(self, beta, gamma, l1, l2):
-        for p, e in enumerate(self.engines):
-            if self.active[p]:
-                e.update_h(beta, gamma, l1, l2)
-                self.updates_h[p] += 1
-
-    def losses(self, beta):
-        for p, e in enumerate(self.engines):
-            if self.active[p]:
-                self._last[p] = e.loss(beta)
-        return self._last.clone()
-
-    @classmethod
-    def factory(cls, single, log):
-        def make(V, W, H):
-            eng = cls(V, W, H, single)
-            log.append(eng)
-            return eng
-        return make
 
 
 def _single_oracle(cls, V, W0, H0, **kw):
@@ -97,7 +29,7 @@ def _single_oracle(cls, V, W0, H0, **kw):
 
 def _batched(cls, V, W0, H0, trainable_W=True, trainable_H=True, log=None, **kw):
     m = cls(W=W0, H=H0, trainable_W=trainable_W, trainable_H=trainable_H)
-    m._engine_factory = BatchedNdOracleEngine.factory(SINGLE[cls][1], [] if log is None else log)
+    m._engine_factory = BatchedOracleEngine.factory(SINGLE[cls][1], [] if log is None else log)
     n = m.fit(V, **kw)
     return n, m.W.data.clone(), m.H.data.clone(), m
 
@@ -244,7 +176,7 @@ def test_constructor_shapes():
 def test_refusals(cls):
     V, W0, H0 = _inputs(cls)
     m = cls(W=W0, H=H0)
-    m._engine_factory = BatchedNdOracleEngine.factory(SINGLE[cls][1], [])
+    m._engine_factory = BatchedOracleEngine.factory(SINGLE[cls][1], [])
     for prec in ("f16", "f16_split", "bogus"):
         with pytest.raises(ValueError):
             m.fit(V, precision=prec)
@@ -266,7 +198,7 @@ def test_refusals(cls):
         m.fit(zero, beta=0)
     X, K = SHAPES[cls]
     big = cls(W=torch.rand(1, 2, 257, *K), H=torch.rand(1, 1, 257, *(x - k + 1 for x, k in zip(X, K))))
-    big._engine_factory = BatchedNdOracleEngine.factory(SINGLE[cls][1], [])
+    big._engine_factory = BatchedOracleEngine.factory(SINGLE[cls][1], [])
     with pytest.raises(ValueError):
         big.fit(torch.rand(1, 1, 2, *X))
 
@@ -279,22 +211,15 @@ def test_last_fit_precision():
 
 def test_batched_nmf_keeps_its_iterate_path():
     """The shared loop takes `iterate` where the engine has it: BatchedNMF's engine gets one call per 10 iterations."""
-    calls = []
-
-    class Eng(BatchedNdOracleEngine):
-        def iterate(self, k, beta, gamma, l1, l2):
-            calls.append(k)
-            for _ in range(k):
-                self.update_w(beta, gamma, l1, l2)
-                self.update_h(beta, gamma, l1, l2)
-
     from oracle_engine import OracleNmfEngine
     g = torch.Generator().manual_seed(3)
     V, W0, H0 = torch.rand(2, 9, 7, generator=g) + 0.1, torch.rand(2, 7, 3, generator=g), torch.rand(2, 9, 3, generator=g)
     m = BatchedNMF(W=W0, H=H0)
-    m._engine_factory = Eng.factory(OracleNmfEngine, [])
+    log = []
+    m._engine_factory = BatchedOracleEngine.factory(OracleNmfEngine, log)
     n = m.fit(V, beta=2, tol=float("-inf"), max_iter=25)
-    assert n.tolist() == [25, 25] and calls == [10, 10, 5]
+    eng, = log
+    assert n.tolist() == [25, 25] and [c[:2] for c in eng.calls] == [("iterate", 10), ("iterate", 10), ("iterate", 5)]
 
 
 def test_public_classes_document_themselves_and_import_without_docstrings():

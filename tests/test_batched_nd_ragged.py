@@ -10,23 +10,11 @@ import pytest
 import torch
 
 from conftest import GOLDEN
-from oracle import mu_oracle as orc
-from oracle_engine import OracleNmfdEngine, _OracleEngine
+from batched_oracle import BatchedOracleEngine
+from oracle_engine import OracleNmfdEngine, OracleNmfndEngine
 from torchnmf_b200 import NMFD, NMF2D, NMF3D, BatchedNMFD, BatchedNMF2D, BatchedNMF3D
 
 SENTINEL = 5.0
-
-
-class OracleNmfndEngine(_OracleEngine):
-    """One NMF2D / NMF3D problem on the CPU oracle (oracle/mu_oracle.py: nmfnd_*)."""
-    kind = "nmfd"
-    _recon = staticmethod(orc.nmfnd_reconstruct)
-
-    def update_w(self, beta, gamma, l1, l2):
-        self.W.copy_(orc.nmfnd_update_w(self.V, self.W, self.H, beta, gamma, l1, l2))
-
-    def update_h(self, beta, gamma, l1, l2):
-        self.H.copy_(orc.nmfnd_update_h(self.V, self.W, self.H, beta, gamma, l1, l2))
 
 
 SINGLE = {BatchedNMFD: (NMFD, OracleNmfdEngine), BatchedNMF2D: (NMF2D, OracleNmfndEngine),
@@ -34,61 +22,12 @@ SINGLE = {BatchedNMFD: (NMFD, OracleNmfdEngine), BatchedNMF2D: (NMF2D, OracleNmf
 CLASSES = {"nmfd": BatchedNMFD, "nmf2d": BatchedNMF2D, "nmf3d": BatchedNMF3D}
 
 
-class RaggedNdOracleEngine:
-    """The batched engine interface over one oracle engine per problem, each built on the problem's real positions only:
-    V[p, ..., :L], W[p] and the copy of H[p, ..., :L - T + 1], written back into H after every update (so the padding of
-    H is never touched).  Records the lengths it was given and counts the updates."""
-    kind = "nmfd_batched"
-    device = torch.device("cpu")
-    precision = "oracle"
-
-    def __init__(self, V, W, H, lengths, single):
-        self.lengths = list(lengths)
-        self.V = V.float()
-        self.W, self.H = W, H
-        T = W.shape[-1]
-        self.lins = [L - T + 1 for L in self.lengths]
-        self.engines = [single(self.V[p, ..., :L].contiguous(), W[p], H[p, ..., :lin].contiguous())
-                        for p, (L, lin) in enumerate(zip(self.lengths, self.lins))]
-        self.active = [True] * len(self.lengths)
-        self.updates = [0] * len(self.lengths)
-        self._last = torch.full((len(self.lengths),), float("nan"), dtype=torch.float64)
-
-    def close(self):
-        pass
-
-    def minmax(self):
-        real = torch.cat([e.V.reshape(-1) for e in self.engines])
-        return float(real.min()), float(real.max())
-
-    def set_active(self, active):
-        self.active = [bool(a) for a in active]
-
-    def update_w(self, beta, gamma, l1, l2):
-        for p, e in enumerate(self.engines):
-            if self.active[p]:
-                e.update_w(beta, gamma, l1, l2)
-
-    def update_h(self, beta, gamma, l1, l2):
-        for p, e in enumerate(self.engines):
-            if self.active[p]:
-                e.update_h(beta, gamma, l1, l2)
-                self.H[p, ..., :self.lins[p]] = e.H
-                self.updates[p] += 1
-
-    def losses(self, beta):
-        for p, e in enumerate(self.engines):
-            if self.active[p]:
-                self._last[p] = e.loss(beta)
-        return self._last.clone()
-
-
 def _factory(cls, log):
     def make(V, W, H, **kw):
         log.append(kw)
         if "lengths" not in kw:
             raise AssertionError("a fit without lengths reached the ragged factory")
-        eng = RaggedNdOracleEngine(V, W, H, kw["lengths"], SINGLE[cls][1])
+        eng = BatchedOracleEngine(V, W, H, SINGLE[cls][1], kw["lengths"])
         log.append(eng)
         return eng
     return make
@@ -177,7 +116,7 @@ def test_ragged_fit_matches_reference_problem_by_problem(name):
         assert torch.allclose(H[p, ..., :lin], c["H"][p, ..., :lin], rtol=2e-5, atol=1e-7), p
         assert torch.equal(H[p, ..., lin:], c["H0"][p, ..., lin:])
     kw, eng = log
-    assert kw == {"lengths": c["lengths"]} and eng.updates == c["n_iter"]
+    assert kw == {"lengths": c["lengths"]} and eng.updates_h == c["n_iter"]
 
 
 def test_golden_ragged_problems_differ():
@@ -196,7 +135,7 @@ def test_each_problem_is_its_own_fit(cls, beta):
     log = []
     n, W, H, _ = _ragged(cls, V, W0, H0, LENGTHS, log=log, **kw)
     counts = _check(cls, V, W0, H0, LENGTHS, n, W, H, **kw)
-    assert log[1].updates == counts                                 # no update after a problem's stop
+    assert log[1].updates_h == counts                               # no update after a problem's stop
 
 
 @pytest.mark.parametrize("as_tensor", [False, True])
@@ -253,7 +192,7 @@ def test_checks_look_at_the_real_positions_only():
 def test_full_lengths_equal_the_uniform_fit():
     V, W0, H0 = _inputs(BatchedNMFD, lengths=[16, 16, 16], pad=0.0)
     ref = BatchedNMFD(W=W0, H=H0)
-    ref._engine_factory = lambda V, W, H: RaggedNdOracleEngine(V, W, H, [16] * 3, OracleNmfdEngine)
+    ref._engine_factory = lambda V, W, H: BatchedOracleEngine(V, W, H, OracleNmfdEngine, [16] * 3)
     n_ref = ref.fit(V, beta=1.5, tol=1e-3, max_iter=40)
     n, W, H, _ = _ragged(BatchedNMFD, V, W0, H0, [16] * 3, beta=1.5, tol=1e-3, max_iter=40)
     assert torch.equal(n, n_ref) and torch.equal(W, ref.W.data) and torch.equal(H, ref.H.data)
@@ -288,7 +227,7 @@ def test_default_keeps_the_three_argument_factory():
 
     def make(V, W, H):                                              # no lengths keyword: today's factories
         seen.append(True)
-        return RaggedNdOracleEngine(V, W, H, [16] * 4, OracleNmfdEngine)
+        return BatchedOracleEngine(V, W, H, OracleNmfdEngine, [16] * 4)
     m = BatchedNMFD(W=W0, H=H0)
     m._engine_factory = make
     m.fit(V, beta=1, max_iter=10)

@@ -9,57 +9,9 @@ import pytest
 import torch
 
 from conftest import GOLDEN
+from batched_oracle import BatchedOracleEngine
 from oracle_engine import OracleNmfEngine
 from torchnmf_b200 import NMF, BatchedNMF, BatchedNMFD, BatchedNMF2D, BatchedNMF3D
-
-
-class RaggedOracleEngine:
-    """The batched engine interface over one oracle engine per problem, each built on the problem's real rows only:
-    V[b, :L], W[b] and the view H[b, :L] (updated in place).  Records the lengths it was given and counts the updates."""
-    kind = "nmf_batched"
-    device = torch.device("cpu")
-    precision = "oracle"
-
-    def __init__(self, V, W, H, lengths):
-        self.lengths = list(lengths)
-        self.V = V.float()
-        self.W, self.H = W, H
-        self.engines = [OracleNmfEngine(self.V[b, :L], W[b], H[b, :L]) for b, L in enumerate(self.lengths)]
-        self.active = [True] * len(self.lengths)
-        self.updates = [0] * len(self.lengths)
-        self._last = torch.full((len(self.lengths),), float("nan"), dtype=torch.float64)
-
-    def close(self):
-        pass
-
-    def minmax(self):
-        real = torch.cat([e.V.reshape(-1) for e in self.engines])
-        return float(real.min()), float(real.max())
-
-    def set_active(self, active):
-        self.active = [bool(a) for a in active]
-
-    def update_w(self, beta, gamma, l1, l2):
-        for b, e in enumerate(self.engines):
-            if self.active[b]:
-                e.update_w(beta, gamma, l1, l2)
-
-    def update_h(self, beta, gamma, l1, l2):
-        for b, e in enumerate(self.engines):
-            if self.active[b]:
-                e.update_h(beta, gamma, l1, l2)
-                self.updates[b] += 1
-
-    def iterate(self, k, beta, gamma, l1, l2):
-        for _ in range(k):
-            self.update_w(beta, gamma, l1, l2)
-            self.update_h(beta, gamma, l1, l2)
-
-    def losses(self, beta):
-        for b, e in enumerate(self.engines):
-            if self.active[b]:
-                self._last[b] = e.loss(beta)
-        return self._last.clone()
 
 
 def _factory(log):
@@ -67,7 +19,7 @@ def _factory(log):
         log.append(kw)
         if "lengths" not in kw:
             raise AssertionError("a fit without lengths reached the ragged factory")
-        eng = RaggedOracleEngine(V, W, H, kw["lengths"])
+        eng = BatchedOracleEngine(V, W, H, OracleNmfEngine, kw["lengths"])
         log.append(eng)
         return eng
     return make
@@ -132,7 +84,7 @@ def test_ragged_fit_matches_reference_prefix_by_prefix(name):
         assert torch.allclose(H[b, :L], c["H"][b, :L], rtol=2e-5, atol=1e-7), (b, (H[b, :L] - c["H"][b, :L]).abs().max())
         assert torch.equal(H[b, L:], c["H0"][b, L:])              # the sentinel padding, untouched
     kw, eng = log
-    assert kw == {"lengths": c["lengths"]} and eng.updates == c["n_iter"]
+    assert kw == {"lengths": c["lengths"]} and eng.updates_h == c["n_iter"]
 
 
 def test_golden_ragged_problems_differ():
@@ -157,7 +109,7 @@ def test_each_problem_is_its_own_fit_on_its_rows(beta):
         assert int(n[b]) == nb
         assert torch.equal(W[b], Wb) and torch.equal(H[b, :L], Hb)
         assert torch.equal(H[b, L:], H0[b, L:])
-    assert log[1].updates == counts                                 # no update after a problem's stop
+    assert log[1].updates_h == counts                               # no update after a problem's stop
     if beta == 1:
         assert len(set(counts)) > 1, counts
 
@@ -205,7 +157,7 @@ def test_checks_look_at_the_real_rows_only():
 def test_all_lengths_n_equal_the_uniform_fit():
     V, W0, H0 = _inputs((20, 20, 20), pad=0.0)
     ref = BatchedNMF(W=W0, H=H0)
-    ref._engine_factory = lambda V, W, H: RaggedOracleEngine(V, W, H, [20, 20, 20])
+    ref._engine_factory = lambda V, W, H: BatchedOracleEngine(V, W, H, OracleNmfEngine, [20, 20, 20])
     n_ref = ref.fit(V, beta=1.5, tol=1e-3, max_iter=60)
     n, W, H, _ = _ragged(V, W0, H0, [20, 20, 20], beta=1.5, tol=1e-3, max_iter=60)
     assert torch.equal(n, n_ref) and torch.equal(W, ref.W.data) and torch.equal(H, ref.H.data)
@@ -245,7 +197,7 @@ def test_default_keeps_the_three_argument_factory():
 
     def make(V, W, H):                                              # no lengths keyword: today's factories
         seen.append(True)
-        return RaggedOracleEngine(V, W, H, [20] * 4)
+        return BatchedOracleEngine(V, W, H, OracleNmfEngine, [20] * 4)
     m = BatchedNMF(W=W0, H=H0)
     m._engine_factory = make
     m.fit(V, beta=1, max_iter=10)

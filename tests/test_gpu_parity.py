@@ -15,7 +15,7 @@ import torch
 
 from conftest import GOLDEN, load_golden
 from oracle import mu_oracle as orc
-from torchnmf_b200 import NMF, NMFD, _capi
+from torchnmf_b200 import NMF, NMFD, PLCA, _capi
 
 pytestmark = pytest.mark.gpu
 CASES = load_golden()
@@ -60,6 +60,36 @@ def test_host_buffer_mode_updates_cpu_parameters_in_place():
     assert n_iter == c["n_iter"] and m.W.device.type == "cpu"
     assert m.W.data_ptr() == w_ptr and m.H.data_ptr() == h_ptr
     assert _close(m.W.data, c["W"], 2e-4, 1e-6)[0] and _close(m.H.data, c["H"], 2e-4, 1e-6)[0]
+
+
+@pytest.mark.parametrize("fit", ["nmf", "sparse_fit", "plca", "plca_masked"])
+def test_non_contiguous_cuda_factors_are_staged_and_written_back(fit):
+    """fp32 CUDA factors that are not contiguous (here transposed storages) are staged through contiguous copies and
+    written back into the same storages: the fit equals the contiguous one bit for bit."""
+    g = torch.Generator().manual_seed(7)
+    N, C, R = 300, 200, 12
+    V = (torch.rand(N, C, generator=g) + 0.01).cuda()
+    M = (torch.rand(N, C, generator=g) > 0.3).cuda()
+    W0, H0 = torch.rand(C, R, generator=g) + 0.1, torch.rand(N, R, generator=g) + 0.1
+    runs = []
+    for strided in (False, True):
+        m = (PLCA(W=W0, H=H0, rank=R) if fit.startswith("plca") else NMF(W=W0, H=H0)).cuda()
+        if strided:
+            for p in (m.W, m.H):
+                p.data = p.data.t().contiguous().t()
+            assert not m.W.is_contiguous() and not m.H.is_contiguous()
+        ptrs = [p.data_ptr() for p in m.parameters()]
+        if fit == "nmf":
+            out = (m.fit(V, 1, 1e-4, 50, precision="f32"),)
+        elif fit == "sparse_fit":
+            out = (m.sparse_fit(V, 2, 20, sW=0.5, sH=0.5),)
+        else:
+            out = m.fit(V, 1e-4, 50, mask=M if fit == "plca_masked" else None)
+        assert [p.data_ptr() for p in m.parameters()] == ptrs
+        runs.append((out[0], out[1:], [p.data.cpu() for p in m.parameters()]))
+    (n1, norm1, f1), (n2, norm2, f2) = runs
+    assert n1 == n2 and all(torch.equal(a, b) for a, b in zip(norm1, norm2))
+    assert all(bool(torch.isfinite(a).all()) and torch.equal(a, b) for a, b in zip(f1, f2))
 
 
 @pytest.mark.parametrize("beta", [-1, 0, 0.5, 1, 1.5, 2, 3])

@@ -16,6 +16,7 @@ import torch
 
 from conftest import GOLDEN
 from oracle import plca_oracle
+from oracle_engine import OracleNmfEngine, OracleNmfdEngine
 from torchnmf_b200 import PLCA, SIPLCA, SIPLCA2, SIPLCA3, NMFD, NMF2D, NMF3D, BetaMu
 
 ZN = np.load(os.path.join(GOLDEN, "reference_next.npz"), allow_pickle=False)
@@ -62,6 +63,42 @@ def test_oracle_matches_reference(name):
     assert n_iter == int(c["n_iter"]) and abs(float(norm) - float(c["norm"])) <= 1e-6 * float(c["norm"])
     for nm, got in (("W", W), ("H", H), ("Z", Z)):
         assert _close(got, _t(c, nm), 1e-4), (name, nm, _worst(got, _t(c, nm)))
+
+
+class _PlcaOracleTerms:
+    """The rest of the PLCA engine interface over an oracle engine whose factors are (W, H diag(Z))."""
+
+    def check_health(self):
+        pass
+
+    def precision_for(self, beta):
+        return self.precision
+
+
+class PlcaOracleEngine(_PlcaOracleTerms, OracleNmfEngine):
+    pass
+
+
+class SiplcaOracleEngine(_PlcaOracleTerms, OracleNmfdEngine):
+    pass
+
+
+@pytest.mark.parametrize("name", [n for n in SMALL if int(_case(n)["cls"]) in (0, 1)])
+def test_fit_host_logic_matches_reference(name):
+    """PLCA / SIPLCA `fit` on the CPU through the `_engine_factory` hook: placement, the EM step around the raw terms, the
+    stop rule and the returned (n_iter, norm), with the oracle's raw terms standing in for the kernels."""
+    c = _case(name)
+    cls = CLS[int(c["cls"])]
+    m = cls(W=_t(c, "W0"), H=_t(c, "H0"), Z=_t(c, "Z0"), trainable_W=bool(int(c["trainable_W"])),
+            trainable_H=bool(int(c["trainable_H"])), trainable_Z=bool(int(c["trainable_Z"])))
+    m._engine_factory = PlcaOracleEngine if cls is PLCA else SiplcaOracleEngine
+    n_iter, norm = m.fit(_t(c, "V"), float(c["tol"]), int(c["iters"]), False,
+                         float(c["W_alpha"]), float(c["H_alpha"]), float(c["Z_alpha"]))
+    assert m.last_fit_precision == "oracle"
+    assert n_iter == int(c["n_iter"]) and abs(float(norm) - float(c["norm"])) <= 1e-6 * float(c["norm"])
+    for nm in ("W", "H", "Z"):
+        got, want = getattr(m, nm).data, _t(c, nm)
+        assert _close(got, want, 1e-4), (name, nm, _worst(got, want))
 
 
 def test_oracle_reconstruct_is_the_flipped_convolution():
