@@ -353,6 +353,43 @@ int nmfb200_plca_iterate(nmfb200_ctx* ctx, float* W, float* H, float* Z, float* 
 int nmfb200_plca_loss(nmfb200_ctx* ctx, const float* W, const float* Hz, const float* norm_dev, double* loss_dev,
                       void* stream);
 
+/* ---- sparse-target PLCA (PLSA): the EM step's gradients at the stored entries only ------------------------------------ */
+
+/* A context of its own kind for one PLCA problem on a sparse target V (N,C) with nnz stored entries, rank R
+ * (1 <= R <= 65535 x 256), with the factor pair W (C,R) and Hz = H diag(Z) (N,R).  Its device workspace is
+ * 4 nnz + 8 ceil(N / 8) + 8 R (nb(N) + nb(C)) bytes, nb(rows) = ceil(rows / max(256, ceil(rows / 1024))) <= 1024: the ratio
+ * of each stored entry, the loss partials of the row gather and the column sums' partials, nothing of size N x C
+ * (nmfb200_plca_sparse_device_bytes reports it).  Only the nmfb200_plca_sparse_* calls, nmfb200_destroy,
+ * nmfb200_ctx_check_health and nmfb200_precision* (NMFB200_PREC_F32) take it; every other call that takes a context returns
+ * NMFB200_ERR_INVALID ("wrong context kind").  NMFB200_ERR_INVALID for sizes below 1, nnz < 0, and ceil(max(N, C) / 8) past
+ * grid x (2^31 - 1). */
+int nmfb200_plca_sparse_create(nmfb200_ctx** out, int device, int64_t N, int64_t C, int64_t R, int64_t nnz);
+/* Register V / sum(V) in both compressed forms: CSR (crow[N+1], col[nnz], val[nnz]: the normalised fp32 values) and CSC
+ * (ccol[C+1], row[nnz]), int64 indices, each segment in ascending index order; perm[nnz] holds, for the e-th CSC entry, its
+ * position in the CSR form (the entry's value is val[perm[e]]).  Device pointers, borrowed until the next set_target or
+ * nmfb200_destroy.  NMFB200_ERR_INVALID for a null pointer (col, val, row and perm may be null when nnz is 0).  No device
+ * work. */
+int nmfb200_plca_sparse_set_target(nmfb200_ctx* ctx, const int64_t* crow, const int64_t* col, const float* val,
+                                   const int64_t* ccol, const int64_t* row, const int64_t* perm, void* stream);
+/* The raw gradients of one EM step (plca.py:252-253) at the current W and Hz, without touching either:
+ *   P[n,c] = val / (hz_n . w_c + eps) at each stored entry,   dW = P^T Hz (C,R),   dHz = P W (N,R),
+ * into `out` = [dW | dHz] (C R + N R floats), or nothing when `out` is null.  Rows and columns that store nothing get zero
+ * gradients.  One gather over the CSR rows (one warp per row) forms each entry's dot product and P once and, at R <= 256,
+ * accumulates dHz; one gather over the CSC columns reads P through perm and accumulates dW without a dot product.  At
+ * R <= 256, dW and dHz are bit for bit the beta-1 numerators of nmfb200_raw_terms on a nmfb200_nmf_set_target_sparse
+ * context holding the same values with the factor pair (W, Hz).  Above rank 256 the row gather takes the dot product over
+ * blocks of 256 components and writes P, and both gradients come from gathers of P, one block of 256 components per grid
+ * y.  loss_dev (optional device double): metrics.kl_div(norm q, norm V) of plca.py:245 with q = Hz W^T, without forming
+ * q:  sum_nnz [t (log(t + eps) - log(x + eps)) - t] + norm sum_r colsum(W)[r] colsum(Hz)[r],  t = val norm and
+ * x = norm (hz_n . w_c) in fp32 at each stored entry; the entries' terms come from the row gather's own pass (one double
+ * partial per block), the column sums from double partials over row blocks, and one block sums them in a fixed order.
+ * fp32 kernels; no atomics: every result is deterministic.  NMFB200_ERR_INVALID for another context kind, a null W or Hz,
+ * or `out` and `loss_dev` both null; NMFB200_ERR_STATE before set_target.  Asynchronous. */
+int nmfb200_plca_sparse_terms(nmfb200_ctx* ctx, const float* W, const float* Hz, float* out /* [dW | dHz] */, float norm,
+                              double* loss_dev /* nullable */, void* stream);
+/* Device bytes the context's workspace holds (the caller's buffers excluded); -1 for a null context or another kind. */
+int64_t nmfb200_plca_sparse_device_bytes(const nmfb200_ctx* ctx);
+
 /* ---- both models ------------------------------------------------------------------------- */
 
 /* Every call below takes a context of either model and runs that model's kernels.  update_w, update_h, loss, raw_terms and

@@ -21,7 +21,8 @@ using namespace nmfb200;
 
 struct nmfb200_ctx {
   int kind = 0;            // 0 = NMF, 1 = NMFD, 2 = a batch of NMF problems (nmfb200_nmf_batched_create), 3 = a batch of
-                           // NMFD / NMF2D / NMF3D problems (nmfb200_nmfnd_batched_create)
+                           // NMFD / NMF2D / NMF3D problems (nmfb200_nmfnd_batched_create), 4 = sparse-target PLCA
+                           // (nmfb200_plca_sparse_create)
   int device = 0;
   int precision = NMFB200_PREC_F32;
   bool auto_mode = false;   // precision AUTO: the tensor-core path is used only where it is known to hold the parity bar
@@ -79,6 +80,10 @@ struct nmfb200_ctx {
   // tensor-core path state (tc_nmf.cu / tc_nmfd.cu)
   TcState* tc = nullptr;
   TcNmfdState* tcd = nullptr;
+  // sparse-target PLCA (kind 4): the borrowed compressed forms, the workspace, its size in bytes and its nnz
+  SparsePlcaTarget spl;
+  SparsePlcaWork splw;
+  int64_t spl_nnz = 0, spl_bytes = 0;
 };
 
 namespace {
@@ -109,9 +114,11 @@ constexpr int kAnyKind = -1;
 constexpr int kDenseNmf = -2;
 constexpr int kBatched = 2;
 constexpr int kBatchedNmfd = 3;
+constexpr int kPlcaSparse = 4;            // served by its own calls only: kAnyKind does not take it
 inline bool is_nmfd(const nmfb200_ctx* c) { return c->kind == 1 || c->kind == kBatchedNmfd; }
 inline bool is_batch(const nmfb200_ctx* c) { return c->kind == kBatched || c->kind == kBatchedNmfd; }
 inline bool kind_ok(const nmfb200_ctx* c, int want) {
+  if (c->kind == kPlcaSparse || want == kPlcaSparse) return c->kind == want;
   return want == kAnyKind || c->kind == want || (want == kDenseNmf && (c->kind == 0 || c->kind == kBatched));
 }
 #define CTX_GUARD(ctx, want_kind)                                                   \
@@ -173,6 +180,7 @@ void free_ctx(nmfb200_ctx* c) {
   cudaFree(c->num); cudaFree(c->den); cudaFree(c->colsum); cudaFree(c->cs_scratch);
   cudaFree(c->loss_blocks); cudaFree(c->mm_scratch); cudaFree(c->Pn); cudaFree(c->Pp);
   cudaFree(c->sp_gram); cudaFree(c->sp_loss_part); cudaFree(c->sp_den); cudaFree(c->qobs_part); cudaFree(c->rag);
+  cudaFree(c->splw.P); cudaFree(c->splw.loss_part); cudaFree(c->splw.cs_part);
   delete c;
 }
 
@@ -1077,6 +1085,7 @@ int nmfb200_target_minmax(nmfb200_ctx* ctx, float* vmin, float* vmax, void* stre
   DeviceGuard guard(ctx->device);
   if (!guard.ok) return fail(NMFB200_ERR_CUDA, "cannot select the context's device");
   TARGET_GUARD(ctx);
+  if (!ctx->mm_scratch) return fail(NMFB200_ERR_INVALID, "wrong context kind");
   float mm[2];
   NMF_CUDA_CHECK(cudaMemcpyAsync(mm, ctx->mm_scratch + kMmPartials, sizeof(mm), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
   NMF_CUDA_CHECK(cudaStreamSynchronize((cudaStream_t)stream));
@@ -1486,6 +1495,63 @@ int nmfb200_plca_loss(nmfb200_ctx* ctx, const float* W, const float* Hz, const f
   bt.scale = norm_dev;
   return simt_nmf_loss(ctx->V, ctx->vdtype, ctx->ldv, Hz, W, ctx->N, ctx->C, (int)ctx->R, 1.0, ctx->loss_blocks,
                        ctx->loss_max_blocks, loss_dev, CellSel{}, ctx->C, st, bt);
+}
+
+/* ---- sparse-target PLCA: one ratio pass per EM step at the stored entries ------------------------------------------ */
+
+int nmfb200_plca_sparse_create(nmfb200_ctx** out, int device, int64_t N, int64_t C, int64_t R, int64_t nnz) {
+  if (!out) return fail(NMFB200_ERR_INVALID, "out is null");
+  *out = nullptr;
+  if (N < 1 || C < 1 || R < 1 || nnz < 0) return fail(NMFB200_ERR_INVALID, "N, C, R must be positive and nnz >= 0");
+  if (R > kMaxRank) return fail(NMFB200_ERR_INVALID, kMaxRankMsg);
+  if (sparse_gather_blocks(N > C ? N : C) > kMaxGridX)
+    return fail(NMFB200_ERR_INVALID, "sparse PLCA: ceil(max(N, C) / 8) gather blocks pass grid x (2^31 - 1)");
+  DeviceGuard guard(device);
+  if (!guard.ok) return fail(NMFB200_ERR_CUDA, "cannot select the requested device");
+  nmfb200_ctx* c = new (std::nothrow) nmfb200_ctx();
+  if (!c) return fail(NMFB200_ERR_INVALID, "out of host memory");
+  c->kind = kPlcaSparse; c->device = device; c->N = N; c->C = C; c->R = R;
+  c->spl_nnz = nnz;
+  const int64_t pb = nnz * (int64_t)sizeof(float), lb = sparse_plca_loss_parts(N) * (int64_t)sizeof(double);
+  const int64_t cb = (sparse_plca_colsum_parts(C, (int)R) + sparse_plca_colsum_parts(N, (int)R)) * (int64_t)sizeof(double);
+  cudaError_t e = cudaMalloc(&c->splw.P, (size_t)(pb > 0 ? pb : sizeof(float)));
+  if (e == cudaSuccess) e = cudaMalloc(&c->splw.loss_part, (size_t)lb);
+  if (e == cudaSuccess) e = cudaMalloc(&c->splw.cs_part, (size_t)cb);
+  if (e != cudaSuccess) {
+    free_ctx(c);
+    return fail(NMFB200_ERR_CUDA, std::string("cudaMalloc: ") + cudaGetErrorString(e));
+  }
+  c->spl_bytes = (pb > 0 ? pb : (int64_t)sizeof(float)) + lb + cb;
+  *out = c;
+  return 0;
+}
+
+int nmfb200_plca_sparse_set_target(nmfb200_ctx* ctx, const int64_t* crow, const int64_t* col, const float* val,
+                                   const int64_t* ccol, const int64_t* row, const int64_t* perm, void* stream) {
+  CTX_GUARD(ctx, kPlcaSparse);
+  (void)stream;
+  if (!crow || !ccol || (ctx->spl_nnz > 0 && (!col || !val || !row || !perm)))
+    return fail(NMFB200_ERR_INVALID, "bad compressed sparse target");
+  SparsePlcaTarget& t = ctx->spl;
+  t.crow = crow; t.col = col; t.val = val; t.ccol = ccol; t.row = row; t.perm = perm;
+  t.N = ctx->N; t.C = ctx->C; t.R = (int)ctx->R;
+  ctx->has_target = true;
+  return 0;
+}
+
+int nmfb200_plca_sparse_terms(nmfb200_ctx* ctx, const float* W, const float* Hz, float* out, float norm, double* loss_dev,
+                              void* stream) {
+  CTX_GUARD(ctx, kPlcaSparse);
+  TARGET_GUARD(ctx);
+  if (!W || !Hz || (!out && !loss_dev)) return fail(NMFB200_ERR_INVALID, "null pointer");
+  float* dW = out;
+  float* dHz = out ? out + ctx->C * ctx->R : nullptr;
+  return sparse_plca_terms(ctx->spl, ctx->splw, W, Hz, dW, dHz, norm, loss_dev, (cudaStream_t)stream);
+}
+
+int64_t nmfb200_plca_sparse_device_bytes(const nmfb200_ctx* ctx) {
+  if (!ctx || ctx->kind != kPlcaSparse) return -1;
+  return ctx->spl_bytes;
 }
 
 int nmfb200_hoyer_project(int device, float* x, int64_t outer, int64_t D, int64_t inner, const float* k1, const float* k2,

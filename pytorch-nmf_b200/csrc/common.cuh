@@ -364,6 +364,29 @@ int64_t sparse_gather_blocks(int64_t nseg);
 void sparse_gram_plan(int64_t rows, int64_t* rpb, int* nb);
 int sparse_gram_passes(int R);
 
+// sparse_plca.cu ---------------------------------------------------------------------------
+// Sparse-target PLCA (nmfb200_plca_sparse_*): V (N x C) in both compressed forms, borrowed -- CSR (crow, col, val: the
+// normalised values) and CSC (ccol, row) with perm[e] the CSR position of the e-th CSC entry.
+struct SparsePlcaTarget {
+  const int64_t *crow = nullptr, *col = nullptr, *ccol = nullptr, *row = nullptr, *perm = nullptr;
+  const float* val = nullptr;
+  int64_t N = 0, C = 0;
+  int R = 0;
+};
+// workspace: P (nnz floats), loss_part (sparse_plca_loss_parts doubles), cs_part (the two column sums' partials,
+// sparse_plca_colsum_parts(C, R) + sparse_plca_colsum_parts(N, R) doubles)
+struct SparsePlcaWork {
+  float* P = nullptr;
+  double* loss_part = nullptr;
+  double* cs_part = nullptr;
+};
+void sparse_plca_colsum_plan(int64_t rows, int64_t* rpb, int* nb);
+int64_t sparse_plca_loss_parts(int64_t N);
+int64_t sparse_plca_colsum_parts(int64_t rows, int R);
+// dW (C x R) and dHz (N x R) of one EM step at (W, Hz), each skipped when null; loss_dev (optional) the KL loss of norm q
+int sparse_plca_terms(const SparsePlcaTarget& t, const SparsePlcaWork& ws, const float* W, const float* Hz, float* dW,
+                      float* dHz, float norm, double* loss_dev, cudaStream_t st);
+
 // plca_em.cu -------------------------------------------------------------------------------
 // The EM step of nprob PLCA problems (nmfb200_plca_iterate), one block per problem: W (wrows, R, winner) and H, Hz (hrows, R,
 // hinner) per problem back to back, Z (R) per problem; dW / dHz the raw numerators in the factors' shapes; aW / aH / aZ the

@@ -69,6 +69,10 @@ SIGNATURES = {
     "nmfb200_plca_iterate": (_int, [_vp, _vp, _vp, _vp, _vp, _vp, _int, _vp, _vp, _vp, _int, _vp]),
     "nmfb200_plca_loss": (_int, [_vp, _vp, _vp, _vp, _vp, _vp]),
     "nmfb200_plca_masked_terms": (_int, [_vp, _vp, _vp, _int, _vp, _vp, _vp]),
+    "nmfb200_plca_sparse_create": (_int, [_c.POINTER(_vp), _int, _i64, _i64, _i64, _i64]),
+    "nmfb200_plca_sparse_set_target": (_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "nmfb200_plca_sparse_terms": (_int, [_vp, _vp, _vp, _vp, _c.c_float, _vp, _vp]),
+    "nmfb200_plca_sparse_device_bytes": (_i64, [_vp]),
     "nmfb200_sync_factors": (_int, [_vp]),
     "nmfb200_update_w": (_int, [_vp, _vp, _vp, _dbl, _dbl, _dbl, _dbl, _vp]),
     "nmfb200_update_h": (_int, [_vp, _vp, _vp, _dbl, _dbl, _dbl, _dbl, _vp]),

@@ -576,10 +576,11 @@ class CudaBatchedNmfdEngine(_BatchedEngine):
                                                               _stream(self.device)))
 
 
-def _compressed_forms(V, weights=None):
+def _compressed_forms(V, weights=None, with_order=False):
     """Both compressed forms of a coalesced sparse COO tensor V (N,C) on the device, built with torch (data-format plumbing):
     (crow, col, val) = CSR, (ccol, row, val_t) = CSC, int64 indices and fp32 values, all contiguous.  With `weights` (one
-    per stored entry, in V's order) also (wt, wt_t): the weights in CSR and in CSC order."""
+    per stored entry, in V's order) also (wt, wt_t): the weights in CSR and in CSC order.  With `with_order`, last, the CSR
+    position of each CSC entry (int64, contiguous)."""
     N, C = V.shape
     vals = V.values().to(torch.float32).contiguous()
     rows, cols = V.indices()[0].contiguous(), V.indices()[1].contiguous()          # coalesced: sorted by (row, col)
@@ -589,10 +590,10 @@ def _compressed_forms(V, weights=None):
     ccol = torch.zeros(C + 1, dtype=torch.int64, device=vals.device)
     ccol[1:] = torch.cumsum(torch.bincount(cols, minlength=C), 0)
     forms = (crow, cols, vals, ccol, rows[order].contiguous(), vals[order].contiguous())
-    if weights is None:
-        return forms
-    wt = weights.to(torch.float32).contiguous()
-    return forms + (wt, wt[order].contiguous())
+    if weights is not None:
+        wt = weights.to(torch.float32).contiguous()
+        forms += (wt, wt[order].contiguous())
+    return forms + (order.contiguous(),) if with_order else forms
 
 
 class CudaSparseNmfEngine(_CudaEngine):
@@ -651,6 +652,65 @@ class CudaSparseAnyBetaEngine(CudaSparseNmfEngine):
     nmfb200_nmf_set_target_sparse_any_beta): beta 1 and 2 as CudaSparseNmfEngine; any other beta takes its numerators at the
     non-zeros and its denominators and loss from V-free dense contractions, so the device holds O(nnz + (N + C) R)."""
     _set_target = "nmfb200_nmf_set_target_sparse_any_beta"
+
+
+class CudaSparsePlcaEngine(_CudaEngine):
+    """One EM step's gradients of a PLCA fit on a sparse target (include/nmf_b200.h: nmfb200_plca_sparse_*): Vn is a
+    coalesced sparse COO tensor (N,C) of V / sum(V) with fp32 values on the device, W (C,R) and Hz = H diag(Z) (N,R)
+    contiguous fp32 on the same device.  Its own context kind: the device holds O(nnz + (N + C) R), nothing of size N x C,
+    at every rank."""
+    kind = "plca_sparse"
+
+    def __init__(self, Vn, W, Hz):
+        super().__init__()
+        self.device = W.device
+        for t, n in ((W, "W"), (Hz, "Hz")):
+            _check_f32_cuda(t, n, self.device)
+        assert Vn.is_sparse and Vn.is_coalesced() and Vn.device == W.device
+        N, C = Vn.shape
+        R = W.shape[1]
+        assert W.shape == (C, R) and Hz.shape == (N, R)
+        self.W, self.H = W, Hz
+        self.N, self.C, self.R = N, C, R
+        crow, col, val, ccol, row, _, perm = _compressed_forms(Vn, with_order=True)
+        self._forms = (crow, col, val, ccol, row, perm)          # borrowed by the context: kept alive here
+        dev_index = self.device.index if self.device.index is not None else torch.cuda.current_device()
+        _capi.check(self._lib.nmfb200_plca_sparse_create(ctypes.byref(self._ctx), dev_index, N, C, R, int(val.numel())))
+        _capi.check(self._lib.nmfb200_plca_sparse_set_target(self._ctx, *(_ptr(t) for t in self._forms),
+                                                             _stream(self.device)))
+        self._out = torch.empty(C * R + N * R, dtype=torch.float32, device=self.device)
+        self._loss = torch.zeros(1, dtype=torch.float64, device=self.device)
+
+    @property
+    def precision(self):
+        return "f32"
+
+    def precision_for(self, beta):
+        return "f32"
+
+    def device_bytes(self):
+        """Device bytes of the context's workspace (the compressed forms and the gradient buffer are torch tensors)."""
+        return int(self._lib.nmfb200_plca_sparse_device_bytes(self._ctx))
+
+    def plca_terms(self, Hz, norm=None):
+        """(dW, dHz) of one EM step at self.W and Hz: P = Vn / (Hz W^T + eps) at the stored entries, dW = P^T Hz, dHz = P W,
+        in a buffer the next call overwrites.  With `norm` (a float: the fp32 value of sum(V)) also the loss
+        kl_div(norm q, norm Vn) from the same pass, as a float64 device tensor of one element: (dW, dHz, loss)."""
+        _capi.check(self._lib.nmfb200_plca_sparse_terms(self._ctx, _ptr(self.W), _ptr(Hz), _ptr(self._out),
+                                                        float(norm) if norm is not None else 0.0,
+                                                        _ptr(self._loss) if norm is not None else None,
+                                                        _stream(self.device)))
+        C, N, R = self.C, self.N, self.R
+        dW, dHz = self._out[:C * R].view(C, R), self._out[C * R:].view(N, R)
+        return (dW, dHz) if norm is None else (dW, dHz, self._loss)
+
+    def loss(self, norm):
+        """kl_div(norm q, norm Vn) at self.W and self.H (= Hz), on the host (synchronises): one row-gather launch."""
+        _capi.check(self._lib.nmfb200_plca_sparse_terms(self._ctx, _ptr(self.W), _ptr(self.H), None, float(norm),
+                                                        _ptr(self._loss), _stream(self.device)))
+        val = float(self._loss.item())
+        self.check_health()
+        return val
 
 
 class CudaObservedNmfEngine(_CudaEngine):

@@ -135,9 +135,22 @@ class BaseComponent(torch.nn.Module):
                    reconstructs V at its own scale and `model(norm=norm)[~mask]` is the imputation.  fp32 kernels only
                    (precision "f32"); a dense V; rank <= 256 for the shift-invariant models.  ValueError for a mask that is
                    not a dense torch.bool tensor of V's shape, a sparse V, another precision, no observed cell or
-                   sum_O V = 0."""
+                   sum_O V = 0.
+
+        A sparse V (PLCA only; PLSA on a count matrix): a sparse COO tensor (N, C) of any floating dtype, on the host or
+        the device, coalesced or not (duplicates sum, as in `coalesce()`), is fitted as `V.to_dense()` is -- same EM step,
+        priors, frozen factors, stop rule and `(n_iter, norm)`, norm = V.sum() in V's dtype -- without forming anything
+        of size N x C, at every rank: each EM step takes one ratio Vn / (q + eps) per stored entry in one gather over the
+        rows, which also yields H's gradient, and one gather over the columns reuses it for W's; the loss takes the stored
+        entries' terms from a gather over the rows and the model's mass from the factors' column sums.  The device holds
+        O(nnz + (N + C) R).  fp32 kernels only (`last_fit_precision` "f32"); the summation order differs from the dense
+        fit's, so the two agree to fp32 rounding, not bit for bit.  AssertionError for a negative stored value; ValueError
+        for a target storing nothing or summing to 0, a sparse layout other than COO, precision "f16" / "f16_split" or an
+        unknown precision, and a mask.  SIPLCA, SIPLCA2 and SIPLCA3 raise NotImplementedError for a sparse V."""
         if mask is not None:
             return self._fit_masked(V, mask, tol, max_iter, verbose, W_alpha, H_alpha, Z_alpha, precision)
+        if V.layout != torch.strided:
+            return self._fit_sparse(V, tol, max_iter, verbose, W_alpha, H_alpha, Z_alpha, precision)
         assert torch.all(V >= 0.), "Target should be non-negative."                         # plca.py:236
         W, H, Z = self.W, self.H, self.Z
         assert W is not None and H is not None and Z is not None, "fit() needs W, H and Z"
@@ -273,6 +286,9 @@ class BaseComponent(torch.nn.Module):
             qo = torch.where(Md, q, 0.).sum()
         return n_iter, (norm_o.double() / qo.to(norm_o.device)).to(norm_o.dtype)
 
+    def _fit_sparse(self, V, tol, max_iter, verbose, W_alpha, H_alpha, Z_alpha, precision):
+        raise NotImplementedError(f"{type(self).__name__}.fit takes dense targets only (PLCA fits sparse COO targets)")
+
     # test hook, as the NMF modules' (tests/test_plca.py): factory(Vn, W, Hz) stands in for `_engine`
     _engine_factory = None
 
@@ -313,6 +329,53 @@ class PLCA(BaseComponent):
     @staticmethod
     def _engine(Vn, W, Hz, precision):
         return _engine.CudaNmfEngine(Vn, W, Hz, precision)
+
+    def _fit_sparse(self, V, tol, max_iter, verbose, W_alpha, H_alpha, Z_alpha, precision):
+        """fit(V) for a sparse COO V: the EM fit of V.to_dense() without forming anything of size N x C (see `fit`)."""
+        if V.layout != torch.sparse_coo:
+            raise ValueError(f"PLCA.fit takes a dense or a sparse COO target (got layout {V.layout})")
+        if precision != "f32":
+            if precision in ("f16", "f16_split"):
+                raise ValueError(f"a sparse target runs on the fp32 kernels: precision must be 'f32' (got {precision!r})")
+            raise ValueError(f"unknown precision {precision!r}")
+        W, H, Z = self.W, self.H, self.Z
+        assert W is not None and H is not None and Z is not None, "fit() needs W, H and Z"
+        if V.dim() != 2 or tuple(V.shape) != (H.shape[0], W.shape[0]):
+            raise ValueError(f"target shape {tuple(V.shape)} does not match H {tuple(H.shape)} / W {tuple(W.shape)}")
+        Vc = V.coalesce()                                   # duplicates sum, as in V.to_dense()
+        vals = Vc.values()
+        assert bool((vals >= 0.).all()), "Target should be non-negative."                   # plca.py:236
+        if vals.numel() == 0:
+            raise ValueError("the sparse target stores no entry")
+        norm = vals.sum()                                                                    # V.sum(), in V's dtype
+        if not bool(norm > 0):
+            raise ValueError("the sparse target's values sum to 0")
+        no_cuda = "torchnmf_b200.PLCA.fit needs a CUDA device (sm_90a); there is no CPU fallback"
+        with _placed_factors(self, (W, H, Z), no_cuda) as (dev, (Wd, Hd, Zd)):
+            ft = Wd.dtype                                   # fp32 on the device; the test hook's factors as they are
+            normd = norm.to(dev, ft)
+            Vn = torch.sparse_coo_tensor(Vc.indices().to(dev), vals.to(dev, ft) / normd, V.shape,
+                                         is_coalesced=True)                                 # plca.py:241-242
+            normf = float(normd)
+            Hz = (Hd * _over(Zd, Hd)).contiguous()
+            eng = _engine.CudaSparsePlcaEngine(Vn, Wd, Hz) if self._engine_factory is None else self._engine_factory(Vn, Wd, Hz)
+            try:
+                def divergence(follows):
+                    torch.mul(Hd, _over(Zd, Hd), out=Hz)
+                    return eng.loss(normf)                  # kl_div(norm q, V) at the stored entries and the column sums
+
+                def step(k):
+                    for _ in range(k):
+                        torch.mul(Hd, _over(Zd, Hd), out=Hz)
+                        dW, dHz = eng.plca_terms(Hz)        # one ratio P per stored entry serves both gradients
+                        self._em_update(Wd, Hd, Zd, dW, dHz, W_alpha, H_alpha, Z_alpha)
+
+                n_iter = _fit_single(step, divergence, max_iter, tol, verbose)
+                eng.check_health()
+                self.last_fit_precision = eng.precision_for(1.0)
+            finally:
+                eng.close()
+        return n_iter, norm
 
 
 class _ShiftInvariant(BaseComponent):
