@@ -141,7 +141,10 @@ int nmfb200_nmf_batched_create(nmfb200_ctx** out, int device, int64_t B, int64_t
  *     chunks, loss chunks and column-sum blocks, each launch holding every problem's blocks on grid x;
  *   - no call reads rows lengths[b].. of V_b or H_b, and no call writes them (nor those rows of nmfb200_raw_terms' output);
  *   - nmfb200_target_minmax covers every problem's first lengths[b] rows (of a shared target too);
- *   - nmfb200_nmf_batched_cd_update / _iterate, nmfb200_plca_iterate and nmfb200_plca_loss return NMFB200_ERR_INVALID.
+ *   - nmfb200_plca_iterate and nmfb200_plca_loss serve it: problem b is the PLCA problem of V_b's first lengths[b] rows, W_b,
+ *     H_b's first lengths[b] rows and Z_b, bit for bit that of a nmfb200_nmf_batched_create context of (1, lengths[b], C, R);
+ *     rows lengths[b].. of H_b, Hz_b, H_alpha_b and of the raw H numerators in `work` are neither read nor written;
+ *   - nmfb200_nmf_batched_cd_update / _iterate return NMFB200_ERR_INVALID.
  * Workspace: the sum over the problems of a single context's partial slabs, column-sum and loss partials, not B times the
  * largest.  NMFB200_ERR_INVALID, before any device work, for B < 1, R > 256, a null `lengths`, a length outside [1, N], and
  * a launch whose problems' blocks together pass grid x (2^31 - 1) or whose loss partials pass 2^31. */
@@ -342,14 +345,19 @@ int64_t nmfb200_plca_work_numel(const nmfb200_ctx* ctx);
  * sum runs in an order fixed by the problem's shape, independent of P and of which problems are active.  W_alpha, H_alpha,
  * Z_alpha: null (alpha = 1) or device fp32 buffers of the factor's batched shape holding alpha.  A problem flagged inactive
  * (nmfb200_nmf_batched_set_active / nmfb200_nmfd_batched_set_active) keeps W, H, Z and Hz.  `work`: device fp32,
- * nmfb200_plca_work_numel floats.  NMFB200_ERR_INVALID for any other context kind, rank > 256 or unknown flags;
- * NMFB200_ERR_STATE before set_target.  Asynchronous. */
+ * nmfb200_plca_work_numel floats.  A ragged NMF batch (nmfb200_nmf_batched_create_ragged) is served: problem b's EM step
+ * runs over its first lengths[b] rows of H and Hz, every sum in the order of a batched context of (1, lengths[b], C, R), so
+ * its W, Z and those rows of H and Hz equal that context's bit for bit; the padding rows are neither read nor written.
+ * NMFB200_ERR_INVALID for a ragged NMFD batch (nmfb200_nmfnd_batched_create_ragged), any other context kind, rank > 256 or
+ * unknown flags; NMFB200_ERR_STATE before set_target.  Asynchronous. */
 int nmfb200_plca_iterate(nmfb200_ctx* ctx, float* W, float* H, float* Z, float* Hz, float* work, int flags,
                          const float* W_alpha, const float* H_alpha, const float* Z_alpha, int n_iter, void* stream);
 /* loss_dev[p] (double) = kl_div(norm_p X_p, norm_p V_p) for every active problem p, X_p the reconstruction from (W, Hz) and
  * V_p the registered (normalised) target: the reference's de-normalised PLCA loss (plca.py:245,293), without materialising
  * X.  norm_dev: P device floats.  The batched KL loss launch with each problem's target and reconstructed cell scaled by
- * norm_p; an inactive problem's slot is left as it is.  Asynchronous. */
+ * norm_p; an inactive problem's slot is left as it is.  A ragged NMF batch: problem b's loss over its first lengths[b] rows,
+ * on its own loss plan, bit for bit the value of a batched context of (1, lengths[b], C, R); a ragged NMFD batch returns
+ * NMFB200_ERR_INVALID.  Asynchronous. */
 int nmfb200_plca_loss(nmfb200_ctx* ctx, const float* W, const float* Hz, const float* norm_dev, double* loss_dev,
                       void* stream);
 

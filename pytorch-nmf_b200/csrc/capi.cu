@@ -1455,7 +1455,7 @@ int nmfb200_plca_iterate(nmfb200_ctx* ctx, float* W, float* H, float* Z, float* 
                          const float* W_alpha, const float* H_alpha, const float* Z_alpha, int n_iter, void* stream) {
   CTX_GUARD(ctx, kAnyKind);
   if (!is_batch(ctx)) return fail(NMFB200_ERR_INVALID, "plca_iterate takes a batched NMF or NMFD context");
-  if (ctx->rag) return fail(NMFB200_ERR_INVALID, "plca_iterate does not serve a ragged batch");
+  if (ctx->rag && is_nmfd(ctx)) return fail(NMFB200_ERR_INVALID, "plca_iterate does not serve a ragged NMFD batch");
   TARGET_GUARD(ctx);
   if (!W || !H || !Z || !Hz || !work || n_iter < 0) return fail(NMFB200_ERR_INVALID, "bad argument");
   if (flags & ~(NMFB200_PLCA_TRAIN_W | NMFB200_PLCA_TRAIN_H | NMFB200_PLCA_TRAIN_Z))
@@ -1471,7 +1471,7 @@ int nmfb200_plca_iterate(nmfb200_ctx* ctx, float* W, float* H, float* Z, float* 
     int rc = plca_numerator(ctx, 0, W, Hz, dW, st);
     if (rc == 0) rc = plca_numerator(ctx, 1, W, Hz, dHz, st);
     if (rc == 0) rc = plca_em(ctx->nprob, w.rows, w.inner, w.other_rows, w.other_inner, (int)ctx->R, W, H, Z, Hz, dW, dHz,
-                              W_alpha, H_alpha, Z_alpha, flags, buf, ctx->active, st);
+                              W_alpha, H_alpha, Z_alpha, flags, buf, ctx->active, ctx->rag, st);
     if (rc) return rc;
   }
   return 0;
@@ -1481,7 +1481,7 @@ int nmfb200_plca_loss(nmfb200_ctx* ctx, const float* W, const float* Hz, const f
                       void* stream) {
   CTX_GUARD(ctx, kAnyKind);
   if (!is_batch(ctx)) return fail(NMFB200_ERR_INVALID, "plca_loss takes a batched NMF or NMFD context");
-  if (ctx->rag) return fail(NMFB200_ERR_INVALID, "plca_loss does not serve a ragged batch");
+  if (ctx->rag && is_nmfd(ctx)) return fail(NMFB200_ERR_INVALID, "plca_loss does not serve a ragged NMFD batch");
   TARGET_GUARD(ctx);
   if (!W || !Hz || !norm_dev || !loss_dev) return fail(NMFB200_ERR_INVALID, "null pointer");
   cudaStream_t st = (cudaStream_t)stream;
@@ -1493,6 +1493,8 @@ int nmfb200_plca_loss(nmfb200_ctx* ctx, const float* W, const float* Hz, const f
   }
   Batch bt{ctx->nprob, ctx->bstride, ctx->N * ctx->R, ctx->C * ctx->R, 0, ctx->active};
   bt.scale = norm_dev;
+  // a ragged batch: problem b's rows, loss chunks and run of partials (loss_part, loss_n) from its plan, as nmfb200_loss
+  if (ctx->rag) { bt.rag = ctx->rag; bt.rag_launch = kRagLoss; bt.rag_gx = ctx->rag_gx[kRagLoss]; }
   return simt_nmf_loss(ctx->V, ctx->vdtype, ctx->ldv, Hz, W, ctx->N, ctx->C, (int)ctx->R, 1.0, ctx->loss_blocks,
                        ctx->loss_max_blocks, loss_dev, CellSel{}, ctx->C, st, bt);
 }

@@ -391,9 +391,11 @@ int sparse_plca_terms(const SparsePlcaTarget& t, const SparsePlcaWork& ws, const
 // The EM step of nprob PLCA problems (nmfb200_plca_iterate), one block per problem: W (wrows, R, winner) and H, Hz (hrows, R,
 // hinner) per problem back to back, Z (R) per problem; dW / dHz the raw numerators in the factors' shapes; aW / aH / aZ the
 // alphas in the factors' shapes (null: 1); `flags` NMFB200_PLCA_TRAIN_*; buf: nprob x plca_em_buf_floats of scratch.
+// rag (a ragged PLCA batch's table, hinner 1): problem p's H side -- H, Hz, dHz and aH -- is its first rag[p].rows of the
+// hrows rows, each step summed as a batch of that many rows sums it; the rows past them are neither read nor written.
 int plca_em(int64_t nprob, int64_t wrows, int64_t winner, int64_t hrows, int64_t hinner, int R, float* W, float* H, float* Z,
             float* Hz, const float* dW, const float* dHz, const float* aW, const float* aH, const float* aZ, int flags,
-            float* buf, const uint8_t* active, cudaStream_t st);
+            float* buf, const uint8_t* active, const RaggedProblem* rag, cudaStream_t st);
 int64_t plca_em_buf_floats(int R, int64_t w_inner, int64_t h_inner);
 
 // nmfd.cu ----------------------------------------------------------------------------------

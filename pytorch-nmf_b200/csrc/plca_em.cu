@@ -1,6 +1,8 @@
 // The EM step of a batch of PLCA / SIPLCA / SIPLCA2 / SIPLCA3 problems (nmfb200_plca_iterate), after the two raw-terms passes
 // of the batched NMF / NMFD contexts.  W and H are viewed as (P, outer, R, inner) -- PLCA: W (P, C, R, 1), H (P, N, R, 1); the
 // shift-invariant models flatten their kernel and activation axes into `inner` -- so one kernel serves every model and ndim.
+// A ragged batch of PLCA problems (nmfb200_nmf_batched_create_ragged) keeps H, Hz and dHz in the padded (P, N, R) layout and
+// runs problem p's H side over its own rag[p].rows rows, as a batch of that many rows does.
 #include "../../include/nmf_b200.h"
 #include "common.cuh"
 
@@ -20,6 +22,7 @@ struct EmArgs {
   int64_t wrows, winner, hrows, hinner; int R;
   int flags;                                             // NMFB200_PLCA_TRAIN_W / _H / _Z
   const uint8_t* active;
+  const RaggedProblem* rag;                              // a ragged PLCA batch: problem p's H rows are rag[p].rows
 };
 
 __device__ __forceinline__ float relu(float x) { return x < 0.f ? 0.f : x; }              // torch.clamp_min(x, 0): NaN stays
@@ -69,7 +72,10 @@ __device__ __forceinline__ void each(int64_t rows, int R, int64_t inner, F f) {
 }
 
 // One block per problem (grid x): plca.py's EM step (Z, then W, then H, then Hz = H Z) on that problem's raw terms, every sum
-// in comp_sums' order.  A problem whose active flag is 0 returns at once.
+// in comp_sums' order.  A problem whose active flag is 0 returns at once.  RAGGED (a.rag set): every sum over H and every
+// write of H and Hz runs over the problem's first rag[p].rows rows, in walk's order for that row count; the padding rows past
+// them are neither read nor written.  The problems' blocks stay the padded a.hrows rows apart (hn).
+template <bool RAGGED>
 __global__ void __launch_bounds__(kEmThreads) plca_em_kernel(EmArgs a) {
   __shared__ float Zold[256], Znew[256], prior[256], S[256];
   __shared__ float zsum;
@@ -77,6 +83,7 @@ __global__ void __launch_bounds__(kEmThreads) plca_em_kernel(EmArgs a) {
   if (batch_skips(a.active, p)) return;
   const int R = a.R, tid = threadIdx.x;
   const int64_t wn = a.wrows * R * a.winner, hn = a.hrows * R * a.hinner;
+  if constexpr (RAGGED) a.hrows = a.rag[p].rows;       // H's rows from here on; hn keeps the padded problem stride
   float* W = a.W + p * wn;
   float* H = a.H + p * hn;
   float* Hz = a.Hz + p * hn;
@@ -171,12 +178,13 @@ int64_t plca_em_buf_floats(int R, int64_t w_inner, int64_t h_inner) {
 
 int plca_em(int64_t nprob, int64_t wrows, int64_t winner, int64_t hrows, int64_t hinner, int R, float* W, float* H, float* Z,
             float* Hz, const float* dW, const float* dHz, const float* aW, const float* aH, const float* aZ, int flags,
-            float* buf, const uint8_t* active, cudaStream_t st) {
+            float* buf, const uint8_t* active, const RaggedProblem* rag, cudaStream_t st) {
   if (R < 1 || R > 256) { set_error("plca_em: rank must be in [1, 256]"); return 1; }
   if (nprob < 1 || nprob > kMaxGridX) { set_error("plca_em: bad problem count"); return 1; }
   const EmArgs a{W, H, Z, Hz, dW, dHz, aW, aH, aZ, buf, plca_em_buf_floats(R, winner, hinner),
-                 wrows, winner, hrows, hinner, R, flags, active};
-  plca_em_kernel<<<(unsigned)nprob, kEmThreads, 0, st>>>(a);
+                 wrows, winner, hrows, hinner, R, flags, active, rag};
+  if (rag) plca_em_kernel<true><<<(unsigned)nprob, kEmThreads, 0, st>>>(a);
+  else plca_em_kernel<false><<<(unsigned)nprob, kEmThreads, 0, st>>>(a);
   NMF_LAUNCH_CHECK();
   return 0;
 }

@@ -491,7 +491,9 @@ class CudaBatchedNmfEngine(_BatchedEngine):
 
     `lengths` (B ints in [1, N], or None): a ragged batch (nmfb200_nmf_batched_create_ragged) -- problem b is the problem of
     V[b, :lengths[b]], W[b] and H[b, :lengths[b]], bit for bit CudaNmfEngine(V[b, :L], W[b], H[b, :L], "f32"); the rows
-    past lengths[b] of V[b] are never read and those of H[b] never written.  No cd_update / cd_iterate then."""
+    past lengths[b] of V[b] are never read and those of H[b] never written.  plca_iterate / plca_losses serve it (problem b
+    is then the PLCA problem of those rows, the padding rows of H and Hz neither read nor written); cd_update / cd_iterate
+    do not."""
     kind = "nmf_batched"
     _set_active = "nmfb200_nmf_batched_set_active"
 

@@ -835,6 +835,42 @@ def _fit_problems(eng, P, max_iter, tol, verbose, losses, step):
     return n_iter
 
 
+def _check_lengths(module, V, lengths, cd=False):
+    """fit(..., lengths=L)'s checks for a batched module, before any device work: the lengths as a list of P Python ints in
+    the module's `_length_range(V)`.  ValueError for a class without ragged fits (`_ragged` False), for `cd`, for a shared
+    target (V without the problem axis), for lengths that are not a 1-D sequence or tensor of integers, and for a wrong
+    count or a length out of range."""
+    name = type(module).__name__
+    if not module._ragged:
+        raise ValueError(f"lengths is not supported by {name}")
+    if cd:
+        raise ValueError("lengths: solver='cd' does not fit ragged batches; use solver='mu'")
+    B = module.H.shape[0]
+    if V.dim() != module.H.dim():
+        raise ValueError(f"lengths needs one target per problem, V with a leading axis of {B} problems; a shared "
+                         f"target of shape {tuple(V.shape)} has one length")
+    if isinstance(lengths, Tensor):
+        if lengths.dtype.is_floating_point or lengths.dtype.is_complex or lengths.dtype == torch.bool:
+            raise ValueError(f"lengths must hold integers (got {lengths.dtype})")
+        if lengths.dim() != 1:
+            raise ValueError(f"lengths must be 1-D (got shape {tuple(lengths.shape)})")
+        lens = [int(n) for n in lengths.tolist()]
+    elif isinstance(lengths, _Iterable) and not isinstance(lengths, (str, bytes)):
+        lens = list(lengths)
+        if not all(isinstance(n, numbers.Integral) and not isinstance(n, bool) for n in lens):
+            raise ValueError("lengths must be a sequence of ints or an integer tensor")
+        lens = [int(n) for n in lens]
+    else:
+        raise ValueError(f"lengths must be a sequence of ints or an integer tensor (got {type(lengths).__name__})")
+    if len(lens) != B:
+        raise ValueError(f"lengths holds {len(lens)} values for {B} problems")
+    lo, hi, hi_name = module._length_range(V)
+    bad = [n for n in lens if not lo <= n <= hi]
+    if bad:
+        raise ValueError(f"every length must be in [{lo}, {hi_name} = {hi}] (got {bad[0]})")
+    return lens
+
+
 class _BatchedComponent(BaseComponent):
     """Shared part of the batched classes: P independent problems of one model and one shape, fitted together.  W and H
     hold the problems on their leading axis and the rank on axis 2; problem p's factors W[p] / H[p] are those of the
@@ -863,39 +899,6 @@ class _BatchedComponent(BaseComponent):
     def _length_range(self, V):
         """(lo, hi, name of hi) of the lengths of a ragged fit: rows of H in [1, N]."""
         return 1, self.H.shape[1], "N"
-
-    def _check_lengths(self, V, lengths, cd):
-        """fit(..., lengths=L)'s checks, before any device work: the lengths as a list of P Python ints in
-        `_length_range`."""
-        name = type(self).__name__
-        if not self._ragged:
-            raise ValueError(f"lengths is not supported by {name}")
-        if cd:
-            raise ValueError("lengths: solver='cd' does not fit ragged batches; use solver='mu'")
-        B = self.H.shape[0]
-        if V.dim() != self.H.dim():
-            raise ValueError(f"lengths needs one target per problem, V with a leading axis of {B} problems; a shared "
-                             f"target of shape {tuple(V.shape)} has one length")
-        if isinstance(lengths, Tensor):
-            if lengths.dtype.is_floating_point or lengths.dtype.is_complex or lengths.dtype == torch.bool:
-                raise ValueError(f"lengths must hold integers (got {lengths.dtype})")
-            if lengths.dim() != 1:
-                raise ValueError(f"lengths must be 1-D (got shape {tuple(lengths.shape)})")
-            lens = [int(n) for n in lengths.tolist()]
-        elif isinstance(lengths, _Iterable) and not isinstance(lengths, (str, bytes)):
-            lens = list(lengths)
-            if not all(isinstance(n, numbers.Integral) and not isinstance(n, bool) for n in lens):
-                raise ValueError("lengths must be a sequence of ints or an integer tensor")
-            lens = [int(n) for n in lens]
-        else:
-            raise ValueError(f"lengths must be a sequence of ints or an integer tensor (got {type(lengths).__name__})")
-        if len(lens) != B:
-            raise ValueError(f"lengths holds {len(lens)} values for {B} problems")
-        lo, hi, hi_name = self._length_range(V)
-        bad = [n for n in lens if not lo <= n <= hi]
-        if bad:
-            raise ValueError(f"every length must be in [{lo}, {hi_name} = {hi}] (got {bad[0]})")
-        return lens
 
     @torch.no_grad()
     def fit(self, V, beta=1, tol=1e-4, max_iter=200, verbose=False, alpha=0, l1_ratio=0, *, precision="auto", solver="mu",
@@ -951,7 +954,7 @@ class _BatchedComponent(BaseComponent):
         cd = solver == "cd"
         if lengths is not None:
             assert self.W is not None and self.H is not None, "fit() needs both W and H"
-            lengths = self._check_lengths(V, lengths, cd)
+            lengths = _check_lengths(self, V, lengths, cd)
         if cd:
             if not self._cd_solver:
                 raise ValueError(f"solver='cd' is supported by BatchedNMF only (got {name})")

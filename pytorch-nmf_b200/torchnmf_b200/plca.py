@@ -24,7 +24,8 @@ from torch.nn import Parameter
 
 from .constants import eps
 from . import engine as _engine
-from .nmf import _batched_conv, _fit_problems, _fit_single, _placed_factors, _register_batched_factors
+from .nmf import (_batched_conv, _check_lengths, _fit_problems, _fit_single, _placed_factors,
+                  _register_batched_factors)
 
 from torch.nn.modules.utils import _single, _pair, _triple
 
@@ -477,6 +478,7 @@ class _BatchedPLCABase(BaseComponent):
     _ndim = 3
     _axes = "three axes (P, rows, rank)"
     _engine_cls = None
+    _ragged = False                # fit(..., lengths=L): BatchedPLCA only
 
     def __init__(self, rank=None, W=None, H=None, Z=None, trainable_W=True, trainable_H=True, trainable_Z=True):
         torch.nn.Module.__init__(self)
@@ -529,8 +531,13 @@ class _BatchedPLCABase(BaseComponent):
                              f"expected {(P,) + single} or {single}")
         return tuple(V.shape) == single
 
+    def _length_range(self, V):
+        """(lo, hi, name of hi) of the lengths of a ragged fit: rows of H in [1, N]."""
+        return 1, self.H.shape[1], "N"
+
     @torch.no_grad()
-    def fit(self, V, tol=1e-4, max_iter=200, verbose=False, W_alpha=1., H_alpha=1., Z_alpha=1., *, precision="f32"):
+    def fit(self, V, tol=1e-4, max_iter=200, verbose=False, W_alpha=1., H_alpha=1., Z_alpha=1., *, precision="f32",
+            lengths=None):
         """Fit every problem by EM, as the single model's `fit(V[p], ...)` fits one, all of them in the same launches.
 
         V: the problems' targets stacked on a leading axis, or one target of the single model's shape shared by every
@@ -551,8 +558,25 @@ class _BatchedPLCABase(BaseComponent):
         a rank above 256 or a shape mismatch; `last_fit_precision` is "f32".  `mask`, `weight` and `group` are not
         parameters of this method (TypeError).  Host-resident and half or double modules are staged through fp32 device
         copies and written back.
+
+        lengths: (keyword-only, default None; BatchedPLCA only) P ints in [1, N], as a sequence or an integer tensor of shape
+        (P,) on any device: a ragged batch.  V (P, N, C) and H (P, N, R) stay padded, and problem p is the EM fit of
+        V[p, :L_p] with W[p], H[p, :L_p] and Z[p]: n_iter[p], norm[p] = V[p, :L_p].sum(), W[p], H[p, :L_p] and Z[p] equal, bit
+        for bit, those of this class's fit with P = 1 on V[p:p+1, :L_p] from W[p:p+1], H[p:p+1, :L_p] and Z[p:p+1], stop rule
+        included: each problem runs the plan and summation order of its own row count.  The padding rows of V are never read
+        by the fit (NaN there does not reach it), those of H are neither read nor written, even through a staged host, half
+        or float64 module, the padding of an H_alpha tensor is ignored, and the non-negativity assertion looks at the real
+        rows only.  The fit does not renormalise H: the constructor normalises H over all N rows, so pad H with zeros, or
+        set the factors after construction, for each problem to start from its own normalised H[p, :L_p].  forward()[p, :L_p]
+        is problem p's model (the rows of a PLCA model are independent).  Every alpha form, frozen factors and target dtype
+        work as without lengths, and lengths all equal to N give the bits of lengths=None.  ValueError, before any device
+        work: the wrong number of lengths, a length out of range, non-integer, bool or non-1-D lengths, a shared target, and
+        lengths on BatchedSIPLCA / BatchedSIPLCA2 / BatchedSIPLCA3.
         """
         name = type(self).__name__
+        if lengths is not None:
+            assert self.W is not None and self.H is not None and self.Z is not None, "fit() needs W, H and Z"
+            lengths = _check_lengths(self, V, lengths)
         if precision != "f32":
             if precision in ("f16", "f16_split"):
                 raise ValueError(f"{name} runs on the fp32 kernels: precision must be 'f32' (got {precision!r})")
@@ -565,18 +589,27 @@ class _BatchedPLCABase(BaseComponent):
         if R > 256:
             raise ValueError(f"{name} supports rank <= 256 (got {R})")
         shared = self._check_target_shape(V)
-        assert torch.all(V >= 0.), "Target should be non-negative."                         # plca.py:236
+        real = None                # a ragged batch: the real rows of V and H, (P, N)
+        if lengths is None:
+            assert torch.all(V >= 0.), "Target should be non-negative."                     # plca.py:236
+        else:
+            real = torch.arange(H.shape[1]) < torch.tensor(lengths).unsqueeze(1)
+            assert bool(torch.where(real.to(V.device).unsqueeze(2), V >= 0., True).all()), "Target should be non-negative."
         f32 = torch.float32
         no_cuda = f"torchnmf_b200.{name}.fit needs a CUDA device (sm_90a); there is no CPU fallback"
-        with _placed_factors(self, (W, H, Z), no_cuda) as (dev, (Wd, Hd, Zd)):
-            # every problem's norm as the single fit takes it (V[p].sum()), whatever P is
-            norm = V.sum().reshape(1).expand(P).clone() if shared else torch.stack([V[p].sum() for p in range(P)])
+        with _placed_factors(self, (W, H, Z), no_cuda, real) as (dev, (Wd, Hd, Zd)):
+            # every problem's norm as the single fit takes it (V[p].sum(), a ragged problem's V[p, :L_p].sum()), whatever P is
+            if lengths is not None:
+                norm = torch.stack([V[p, :n].sum() for p, n in enumerate(lengths)])
+            else:
+                norm = V.sum().reshape(1).expand(P).clone() if shared else torch.stack([V[p].sum() for p in range(P)])
             normd = norm.to(dev, f32)
             Vd = V.to(dev, f32).contiguous()
             Vn = (Vd / normd[0] if shared else Vd / normd.reshape(P, *([1] * (V.dim() - 1)))).contiguous()  # plca.py:241-242
             Hz = (Hd * Zd.reshape(P, 1, R, *([1] * (Hd.dim() - 3)))).contiguous()
             alphas = [_alpha_buffer(a, t) for a, t in ((W_alpha, Wd), (H_alpha, Hd), (Z_alpha, Zd))]
-            eng = (self._engine_cls if self._engine_factory is None else self._engine_factory)(Vn, Wd, Hz)
+            ragged = {} if lengths is None else {"lengths": lengths}
+            eng = (self._engine_cls if self._engine_factory is None else self._engine_factory)(Vn, Wd, Hz, **ragged)
             try:
                 def step(k):                                                                 # plca.py:247-289, k times
                     eng.plca_iterate(k, Hd, Zd, W.requires_grad, H.requires_grad, Z.requires_grad, *alphas)
@@ -604,9 +637,12 @@ class BatchedPLCA(_BatchedPLCABase):
     `fit(V, ...)` takes V as (P, N, C), or as one (N, C) target shared by every problem.  Each problem's fit is
     `PLCA.fit(V[p], ..., precision="f32")`'s EM iteration.  Workspace (device memory, kept between fits of the same shape):
     that of `BatchedNMF` at this shape, plus per fit the raw numerators of W and H (the factors' size) and the EM step's
-    scratch.
+    scratch.  `fit(..., lengths=L)` fits a ragged batch: problem p is the EM fit of V[p, :L[p]] with W[p], H[p, :L[p]] and
+    Z[p], V and H padded to N rows, each problem bit for bit its own fit with P = 1 (see `fit`); the workspace is then that
+    of a ragged `BatchedNMF` with the same lengths plus the same per-fit buffers.
     """
     _engine_cls = _engine.CudaBatchedNmfEngine
+    _ragged = True
 
     def __init__(self, Vshape=None, rank=None, *, W=None, H=None, Z=None, trainable_W=True, trainable_H=True,
                  trainable_Z=True):
