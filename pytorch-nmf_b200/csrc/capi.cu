@@ -19,21 +19,36 @@ void count_launch() { g_launches.fetch_add(1, std::memory_order_relaxed); }
 
 using namespace nmfb200;
 
+// NmfBatch / NmfdBatch: a batch of NMF / of NMFD, NMF2D, NMF3D problems; PlcaSparse: served by its own calls only
+enum class CtxKind { Nmf, Nmfd, NmfBatch, NmfdBatch, PlcaSparse };
+
+// What the last successful set_target* registered.  Observed: the compressed forms hold the observed cells of a masked fit,
+// and every beta fits beta_div(WH[obs], V[obs]) on the observed-cell gathers.
+enum class TargetForm { None, Dense, Sparse, SparseAnyBeta, Observed };
+
+// A sparse target, borrowed: CSR (rows of V) and CSC (= CSR of V^T) forms; an observed target's entry weights in CSR / CSC
+// order (none: unweighted); V_norm of nmf.py:161-170 (beta 1 / 2); sparse PLCA's CSR position of each CSC entry
+struct SparseTarget {            // members in the order of the set_target_sparse* arguments
+  const int64_t* crow = nullptr; const int64_t* col = nullptr; const float* val = nullptr;
+  const int64_t* ccol = nullptr; const int64_t* row = nullptr; const float* val_t = nullptr;
+  const float *wt = nullptr, *wt_t = nullptr;
+  double vnorm_kl = 0.0, vnorm_eu = 0.0;
+  const int64_t* perm = nullptr;
+};
+
 struct nmfb200_ctx {
-  int kind = 0;            // 0 = NMF, 1 = NMFD, 2 = a batch of NMF problems (nmfb200_nmf_batched_create), 3 = a batch of
-                           // NMFD / NMF2D / NMF3D problems (nmfb200_nmfnd_batched_create), 4 = sparse-target PLCA
-                           // (nmfb200_plca_sparse_create)
+  CtxKind kind = CtxKind::Nmf;
   int device = 0;
   int precision = NMFB200_PREC_F32;
   bool auto_mode = false;   // precision AUTO: the tensor-core path is used only where it is known to hold the parity bar
   bool tc_off = false;      // AUTO found the target outside the fp16 operand range: fp32 CUDA-core kernels instead
   int64_t N = 0, C = 0, R = 0;
-  // a batch (kind 2 or 3): nprob problems of the shape (N, C, R) or d, their targets bstride elements apart (0: one shared
+  // a batch: nprob problems of the shape (N, C, R) or d, their targets bstride elements apart (0: one shared
   // target), factors and partial slabs back to back; `active` (borrowed, nprob device bytes, null: all) flags the problems
   // that run
   int64_t nprob = 1, bstride = 0;
   const uint8_t* active = nullptr;
-  // a ragged batch of NMF problems (nmfb200_nmf_batched_create_ragged; kind 2): each problem's plan (device, nprob of them)
+  // a ragged batch of NMF problems (nmfb200_nmf_batched_create_ragged): each problem's plan (device, nprob of them)
   // and the grid x of each RaggedLaunch, the sum of the problems' blocks
   RaggedProblem* rag = nullptr;
   int64_t rag_gx[4] = {0, 0, 0, 0};
@@ -41,7 +56,8 @@ struct nmfb200_ctx {
   const void* V = nullptr;        // the dense target, borrowed: vdtype (NMFB200_DTYPE_*) elements
   int vdtype = NMFB200_DTYPE_F32;
   int64_t ldv = 0;
-  bool has_target = false;
+  TargetForm form = TargetForm::None;
+  SparseTarget sp;
   // nmfb200_set_mask / nmfb200_set_weight: the observed cells (uint8) or the cells' weights (fp32), V's shape, contiguous,
   // borrowed; cleared by every set_target*.  While set, every pass runs the selecting fp32 kernels and beta 1 takes its
   // denominators from the contraction, not the column sums.
@@ -57,17 +73,7 @@ struct nmfb200_ctx {
   double* loss_blocks = nullptr;
   int loss_max_blocks = 0;
   float* mm_scratch = nullptr;    // kMmFloats: matrix_minmax's partials, then the target's min / max
-  // sparse target (beta 1 / 2): borrowed CSR (rows of V) and CSC (= CSR of V^T) forms, V_norm of nmf.py:161-170
-  bool sparse = false;
-  bool sp_any_beta = false;       // set by nmfb200_nmf_set_target_sparse_any_beta, reset by every other set_target
-  // set by nmfb200_nmf_set_target_observed, reset by every other set_target: the compressed forms hold the observed cells of
-  // a masked fit, and every beta fits beta_div(WH[obs], V[obs]) on the observed-cell gathers
-  bool observed = false;
   float* sp_den = nullptr;        // max(N, C) x R: the reduced V-free denominator of an update at beta != 1, 2
-  const int64_t *sp_crow = nullptr, *sp_col = nullptr, *sp_ccol = nullptr, *sp_row = nullptr;
-  const float *sp_val = nullptr, *sp_val_t = nullptr;
-  const float *sp_wt = nullptr, *sp_wt_t = nullptr;     // observed cells: the entries' weights in CSR / CSC order, or none
-  double sp_vnorm_kl = 0.0, sp_vnorm_eu = 0.0;
   float* sp_gram = nullptr;       // [2][R*R] (W^T W, H^T H) + per-block partials; also the Gram scratch of nmfb200_nmf_cd_*
   double* sp_loss_part = nullptr;
   // NMFD: the ratio tiles, pn_floats each (a batch: every problem's, back to back)
@@ -80,8 +86,7 @@ struct nmfb200_ctx {
   // tensor-core path state (tc_nmf.cu / tc_nmfd.cu)
   TcState* tc = nullptr;
   TcNmfdState* tcd = nullptr;
-  // sparse-target PLCA (kind 4): the borrowed compressed forms, the workspace, its size in bytes and its nnz
-  SparsePlcaTarget spl;
+  // sparse-target PLCA: the workspace, its size in bytes and its nnz
   SparsePlcaWork splw;
   int64_t spl_nnz = 0, spl_bytes = 0;
 };
@@ -108,27 +113,24 @@ struct DeviceGuard {
   DeviceGuard& operator=(const DeviceGuard&) = delete;
 };
 
-// want_kind: 0 = NMF, 1 = NMFD, 2 = batched NMF, 3 = batched NMFD, kAnyKind for the calls that serve every kind, kDenseNmf
-// for those that serve NMF and batched NMF
-constexpr int kAnyKind = -1;
-constexpr int kDenseNmf = -2;
-constexpr int kBatched = 2;
-constexpr int kBatchedNmfd = 3;
-constexpr int kPlcaSparse = 4;            // served by its own calls only: kAnyKind does not take it
-inline bool is_nmfd(const nmfb200_ctx* c) { return c->kind == 1 || c->kind == kBatchedNmfd; }
-inline bool is_batch(const nmfb200_ctx* c) { return c->kind == kBatched || c->kind == kBatchedNmfd; }
-inline bool kind_ok(const nmfb200_ctx* c, int want) {
-  if (c->kind == kPlcaSparse || want == kPlcaSparse) return c->kind == want;
-  return want == kAnyKind || c->kind == want || (want == kDenseNmf && (c->kind == 0 || c->kind == kBatched));
-}
-#define CTX_GUARD(ctx, want_kind)                                                   \
+// A set of context kinds, one bit per kind: what an entry point serves
+template <class... K>
+constexpr unsigned kinds(K... k) { return ((1u << static_cast<int>(k)) | ...); }
+constexpr unsigned kDenseModels = kinds(CtxKind::Nmf, CtxKind::Nmfd, CtxKind::NmfBatch, CtxKind::NmfdBatch);
+constexpr unsigned kDenseNmf = kinds(CtxKind::Nmf, CtxKind::NmfBatch);
+inline bool is_nmfd(const nmfb200_ctx* c) { return c->kind == CtxKind::Nmfd || c->kind == CtxKind::NmfdBatch; }
+inline bool is_batch(const nmfb200_ctx* c) { return c->kind == CtxKind::NmfBatch || c->kind == CtxKind::NmfdBatch; }
+inline bool has_target(const nmfb200_ctx* c) { return c->form != TargetForm::None; }
+// a compressed target (c->sp): the dense kernels are out of play
+inline bool is_sparse(const nmfb200_ctx* c) { return has_target(c) && c->form != TargetForm::Dense; }
+#define CTX_GUARD(ctx, kind_set)                                                    \
   if (!(ctx)) return fail(NMFB200_ERR_INVALID, "null context");                     \
-  if (!kind_ok((ctx), (want_kind)))                                                 \
+  if (!((kind_set) & kinds((ctx)->kind)))                                           \
     return fail(NMFB200_ERR_INVALID, "wrong context kind");                         \
   DeviceGuard _dev_guard((ctx)->device);                                            \
   if (!_dev_guard.ok) return fail(NMFB200_ERR_CUDA, "cannot select the context's device");
 #define TARGET_GUARD(ctx) \
-  if (!(ctx)->has_target) return fail(NMFB200_ERR_STATE, "set_target has not been called");
+  if (!has_target(ctx)) return fail(NMFB200_ERR_STATE, "set_target has not been called");
 
 // mm_scratch: kMmPartials per-block partials of matrix_minmax, then the target's min / max
 constexpr int kMmPartials = 2048;
@@ -203,7 +205,7 @@ int alloc_workspace(nmfb200_ctx* c, int64_t pn_floats) {
 
 // beta 1 without a mask: the denominator is the column sum of the other factor (nmf.py:122-131).  A masked or weighted fit
 // takes it from the second backward pass, M G, like every other beta.
-bool kl_colsum(const nmfb200_ctx* c, double beta) { return beta == 1.0 && !c->sel && !c->observed; }
+bool kl_colsum(const nmfb200_ctx* c, double beta) { return beta == 1.0 && !c->sel && c->form != TargetForm::Observed; }
 
 // Whether the context's own tensor-core kernels (c->tc: NMF, c->tcd: NMFD / NMF2D / NMF3D) serve this beta.
 bool use_tc(const nmfb200_ctx* c, double beta) {
@@ -254,6 +256,15 @@ int check_target(const void* V, int dtype) {
   return 0;
 }
 
+// The one place a set_target* changes the target, once its checks and allocations have passed: a call refused before it
+// leaves the context as it was.  A new target drops the mask or weight; a sparse one takes the tensor cores out of play.
+void commit_target(nmfb200_ctx* c, TargetForm form, const void* V, int vdtype, int64_t ldv, int64_t bstride,
+                   const SparseTarget& sp = SparseTarget{}) {
+  c->form = form; c->V = V; c->vdtype = vdtype; c->ldv = ldv; c->bstride = bstride; c->sp = sp;
+  c->sel = CellSel{};
+  c->tc_off = form != TargetForm::Dense;
+}
+
 // AUTO keeps heavy-tailed targets (max / mean > 64: spectrogram-like, lognormal, ...) off the tensor cores.  Measured on the
 // lognormal fixtures of tests/golden/reference_r2.npz (30 iterations, tolerance rtol 1e-3): f16 34x, f16_split 2x, f32 0.1x
 // of the tolerance -- MU on such targets converges slowly and keeps the per-update operand rounding instead of averaging it
@@ -277,6 +288,26 @@ int check_health(void* stream) {
   return 0;
 }
 
+// What the four sparse set_target calls of an NMF context share: the checks and the workspace of `form`, then the commit
+int set_sparse_target(nmfb200_ctx* ctx, TargetForm form, int64_t nnz, const SparseTarget& sp, void* stream) {
+  CTX_GUARD(ctx, kinds(CtxKind::Nmf));
+  if (nnz < 0 || !sp.crow || !sp.ccol || (nnz > 0 && (!sp.col || !sp.val || !sp.row || !sp.val_t)))
+    return fail(NMFB200_ERR_INVALID, "bad compressed sparse target");
+  if (ctx->R > 256)
+    return fail(NMFB200_ERR_INVALID, "rank > 256 is not supported by the sparse-target kernels (densify the target)");
+  if (int rc = ensure_gram(ctx)) return rc;
+  if (!ctx->sp_loss_part)
+    NMF_CUDA_CHECK(cudaMalloc(&ctx->sp_loss_part, (size_t)sparse_gather_blocks(ctx->N) * sizeof(double)));
+  if (form != TargetForm::Sparse)                          // the denominator of an update outside raw_terms
+    if (int rc = ensure_den(ctx)) return rc;
+  if (form == TargetForm::SparseAnyBeta && !ctx->sp_den)
+    NMF_CUDA_CHECK(cudaMalloc(&ctx->sp_den, (size_t)(ctx->N > ctx->C ? ctx->N : ctx->C) * ctx->R * sizeof(float)));
+  commit_target(ctx, form, nullptr, NMFB200_DTYPE_F32, 0, 0, sp);
+  if (form != TargetForm::Observed) return 0;
+  // target_minmax: the observed values (none: +inf / -inf)
+  return matrix_minmax(sp.val, NMFB200_DTYPE_F32, 1, nnz, nnz, ctx->mm_scratch, ctx->mm_scratch + kMmPartials,
+                       (cudaStream_t)stream);
+}
 }  // namespace
 
 extern "C" {
@@ -318,7 +349,7 @@ int nmfb200_nmf_create(nmfb200_ctx** out, int device, int64_t N, int64_t C, int6
   if (!guard.ok) return fail(NMFB200_ERR_CUDA, "cannot select the requested device");
   nmfb200_ctx* c = new (std::nothrow) nmfb200_ctx();
   if (!c) return fail(NMFB200_ERR_INVALID, "out of host memory");
-  c->kind = 0; c->device = device; c->N = N; c->C = C; c->R = R;
+  c->kind = CtxKind::Nmf; c->device = device; c->N = N; c->C = C; c->R = R;
   int resolved = precision;
   // AUTO: single-rounded fp16 operands hold the north-star parity (rtol 1e-3) once the ratio tile is kappa-centred;
   // the parity tests check it against the reference at the configuration shapes
@@ -389,16 +420,14 @@ int nmfb200_nmf_sparse_plan(int64_t N, int64_t C, int64_t R, int64_t* out, int n
 }
 
 int nmfb200_nmf_set_target(nmfb200_ctx* ctx, const void* V, int64_t ldv, int dtype, void* stream) {
-  CTX_GUARD(ctx, 0);
+  CTX_GUARD(ctx, kinds(CtxKind::Nmf));
   if (!V || ldv < ctx->C) return fail(NMFB200_ERR_INVALID, "bad target pointer / leading dimension");
   if (int rc = check_target(V, dtype)) return rc;
   cudaStream_t st = (cudaStream_t)stream;
-  ctx->V = V; ctx->vdtype = dtype; ctx->ldv = ldv; ctx->has_target = true; ctx->sparse = false; ctx->sp_any_beta = false;
-  ctx->observed = false; ctx->sel = CellSel{};
+  commit_target(ctx, TargetForm::Dense, V, dtype, ldv, 0);
   float* minmax = ctx->mm_scratch + kMmPartials;
   int rc = matrix_minmax(V, dtype, ctx->N, ctx->C, ldv, ctx->mm_scratch, minmax, st);
   if (rc) return rc;
-  ctx->tc_off = false;
   if (ctx->tc) {
     rc = tc_set_target(ctx->tc, V, dtype, ldv, minmax, st);
     if (rc) return rc;
@@ -439,7 +468,7 @@ int nmfb200_nmf_batched_create(nmfb200_ctx** out, int device, int64_t B, int64_t
   if (!guard.ok) return fail(NMFB200_ERR_CUDA, "cannot select the requested device");
   nmfb200_ctx* c = new (std::nothrow) nmfb200_ctx();
   if (!c) return fail(NMFB200_ERR_INVALID, "out of host memory");
-  c->kind = kBatched; c->device = device; c->N = N; c->C = C; c->R = R; c->nprob = B;
+  c->kind = CtxKind::NmfBatch; c->device = device; c->N = N; c->C = C; c->R = R; c->nprob = B;
   c->precision = NMFB200_PREC_F32;
   // each problem's plan is the single problem's: same chunks, loss blocks and column-sum blocks
   c->nslab[0] = chunks_for(C, N, R);
@@ -498,7 +527,7 @@ int nmfb200_nmf_batched_create_ragged(nmfb200_ctx** out, int device, int64_t B, 
   if (!guard.ok) return fail(NMFB200_ERR_CUDA, "cannot select the requested device");
   nmfb200_ctx* c = new (std::nothrow) nmfb200_ctx();
   if (!c) return fail(NMFB200_ERR_INVALID, "out of host memory");
-  c->kind = kBatched; c->device = device; c->N = N; c->C = C; c->R = R; c->nprob = B;
+  c->kind = CtxKind::NmfBatch; c->device = device; c->N = N; c->C = C; c->R = R; c->nprob = B;
   c->precision = NMFB200_PREC_F32;
   c->nslab[0] = chunks_for(C, N, R);        // unused by the ragged launches: each problem's own counts are in its plan
   c->nslab[1] = chunks_for(N, C, R);
@@ -519,19 +548,19 @@ int nmfb200_nmf_batched_create_ragged(nmfb200_ctx** out, int device, int64_t B, 
 
 int nmfb200_nmf_batched_set_target(nmfb200_ctx* ctx, const void* V, int64_t ldv, int64_t batch_stride, int dtype,
                                    void* stream) {
-  CTX_GUARD(ctx, kBatched);
+  CTX_GUARD(ctx, kinds(CtxKind::NmfBatch));
   if (!V || ldv < ctx->C) return fail(NMFB200_ERR_INVALID, "bad target pointer / leading dimension");
   if (batch_stride != 0 && batch_stride < ctx->N * ldv)
     return fail(NMFB200_ERR_INVALID, "batch stride must be 0 (one shared target) or at least N x ldv");
   if (int rc = check_target(V, dtype)) return rc;
-  ctx->V = V; ctx->vdtype = dtype; ctx->ldv = ldv; ctx->bstride = batch_stride; ctx->has_target = true;
+  commit_target(ctx, TargetForm::Dense, V, dtype, ldv, batch_stride);
   // a ragged batch: every problem's own rows, even of a shared target
   return matrix_minmax(V, dtype, ctx->N, ctx->C, ldv, ctx->mm_scratch, ctx->mm_scratch + kMmPartials, (cudaStream_t)stream,
                        CellSel{}, batch_stride || ctx->rag ? ctx->nprob : 1, batch_stride, ctx->rag);
 }
 
 int nmfb200_nmf_batched_set_active(nmfb200_ctx* ctx, const uint8_t* active, void* stream) {
-  CTX_GUARD(ctx, kBatched);
+  CTX_GUARD(ctx, kinds(CtxKind::NmfBatch));
   (void)stream;
   ctx->active = active;
   return 0;
@@ -542,61 +571,28 @@ int nmfb200_nmf_batched_set_active(nmfb200_ctx* ctx, const uint8_t* active, void
 int nmfb200_nmf_set_target_sparse(nmfb200_ctx* ctx, int64_t nnz, const int64_t* crow, const int64_t* col, const float* val,
                                   const int64_t* ccol, const int64_t* row, const float* val_t, double v_norm_kl,
                                   double v_norm_eu, void* stream) {
-  CTX_GUARD(ctx, 0);
-  (void)stream;
-  if (nnz < 0 || !crow || !ccol || (nnz > 0 && (!col || !val || !row || !val_t)))
-    return fail(NMFB200_ERR_INVALID, "bad compressed sparse target");
-  if (ctx->R > 256)
-    return fail(NMFB200_ERR_INVALID, "rank > 256 is not supported by the sparse-target kernels (densify the target)");
-  if (int rc = ensure_gram(ctx)) return rc;
-  if (!ctx->sp_loss_part)
-    NMF_CUDA_CHECK(cudaMalloc(&ctx->sp_loss_part, (size_t)sparse_gather_blocks(ctx->N) * sizeof(double)));
-  ctx->sp_crow = crow; ctx->sp_col = col; ctx->sp_val = val; ctx->sp_ccol = ccol; ctx->sp_row = row; ctx->sp_val_t = val_t;
-  ctx->sp_vnorm_kl = v_norm_kl; ctx->sp_vnorm_eu = v_norm_eu;
-  ctx->sparse = true; ctx->has_target = true; ctx->V = nullptr; ctx->tc_off = true;      // the dense kernels are out of play
-  ctx->sel = CellSel{};
-  ctx->sp_any_beta = false;
-  ctx->observed = false;
-  ctx->sp_wt = ctx->sp_wt_t = nullptr;
-  return 0;
+  return set_sparse_target(ctx, TargetForm::Sparse, nnz,
+                           SparseTarget{crow, col, val, ccol, row, val_t, nullptr, nullptr, v_norm_kl, v_norm_eu}, stream);
 }
 
 int nmfb200_nmf_set_target_sparse_any_beta(nmfb200_ctx* ctx, int64_t nnz, const int64_t* crow, const int64_t* col,
                                            const float* val, const int64_t* ccol, const int64_t* row, const float* val_t,
                                            double v_norm_kl, double v_norm_eu, void* stream) {
-  int rc = nmfb200_nmf_set_target_sparse(ctx, nnz, crow, col, val, ccol, row, val_t, v_norm_kl, v_norm_eu, stream);
-  if (rc) return rc;
-  DeviceGuard guard(ctx->device);
-  if (!guard.ok) return fail(NMFB200_ERR_CUDA, "cannot select the context's device");
-  if ((rc = ensure_den(ctx))) return rc;
-  if (!ctx->sp_den)
-    NMF_CUDA_CHECK(cudaMalloc(&ctx->sp_den, (size_t)(ctx->N > ctx->C ? ctx->N : ctx->C) * ctx->R * sizeof(float)));
-  ctx->sp_any_beta = true;
-  return 0;
+  return set_sparse_target(ctx, TargetForm::SparseAnyBeta, nnz,
+                           SparseTarget{crow, col, val, ccol, row, val_t, nullptr, nullptr, v_norm_kl, v_norm_eu}, stream);
 }
 
 int nmfb200_nmf_set_target_observed(nmfb200_ctx* ctx, int64_t nnz, const int64_t* crow, const int64_t* col,
                                     const float* val, const int64_t* ccol, const int64_t* row, const float* val_t,
                                     void* stream) {
-  int rc = nmfb200_nmf_set_target_sparse(ctx, nnz, crow, col, val, ccol, row, val_t, 0.0, 0.0, stream);
-  if (rc) return rc;
-  DeviceGuard guard(ctx->device);
-  if (!guard.ok) return fail(NMFB200_ERR_CUDA, "cannot select the context's device");
-  if ((rc = ensure_den(ctx))) return rc;                  // the denominator of an update outside raw_terms
-  ctx->observed = true;
-  // target_minmax: the observed values (none: +inf / -inf)
-  return matrix_minmax(val, NMFB200_DTYPE_F32, 1, nnz, nnz, ctx->mm_scratch, ctx->mm_scratch + kMmPartials,
-                       (cudaStream_t)stream);
+  return set_sparse_target(ctx, TargetForm::Observed, nnz, SparseTarget{crow, col, val, ccol, row, val_t}, stream);
 }
 
 int nmfb200_nmf_set_target_observed_weighted(nmfb200_ctx* ctx, int64_t nnz, const int64_t* crow, const int64_t* col,
                                              const float* val, const int64_t* ccol, const int64_t* row, const float* val_t,
                                              const float* wt, const float* wt_t, void* stream) {
   if (nnz > 0 && (!wt || !wt_t)) return fail(NMFB200_ERR_INVALID, "bad entry weights");
-  int rc = nmfb200_nmf_set_target_observed(ctx, nnz, crow, col, val, ccol, row, val_t, stream);
-  if (rc) return rc;
-  ctx->sp_wt = wt; ctx->sp_wt_t = wt_t;
-  return 0;
+  return set_sparse_target(ctx, TargetForm::Observed, nnz, SparseTarget{crow, col, val, ccol, row, val_t, wt, wt_t}, stream);
 }
 
 /* ---- NMFD ------------------------------------------------------------------------------------ */
@@ -649,8 +645,8 @@ int nmfb200_nmfnd_create(nmfb200_ctx** out, int device, int64_t B, int64_t C, in
   if (!guard.ok) return fail(NMFB200_ERR_CUDA, "cannot select the requested device");
   nmfb200_ctx* c = new (std::nothrow) nmfb200_ctx();
   if (!c) return fail(NMFB200_ERR_INVALID, "out of host memory");
-  c->kind = 1; c->device = device; c->precision = precision == NMFB200_PREC_F32 ? NMFB200_PREC_F32 : NMFB200_PREC_F16; c->R = R;
-  c->auto_mode = precision == NMFB200_PREC_AUTO;
+  c->kind = CtxKind::Nmfd; c->device = device; c->precision = precision == NMFB200_PREC_F32 ? NMFB200_PREC_F32 : NMFB200_PREC_F16;
+  c->R = R; c->auto_mode = precision == NMFB200_PREC_AUTO;
   c->d = shape;
   c->nslab[0] = nmfd_wgrad_nsplit(c->d);
   c->nslab[1] = nmfd_dgrad_nsplit(c->d);
@@ -677,14 +673,13 @@ int nmfb200_nmfnd_create(nmfb200_ctx** out, int device, int64_t B, int64_t C, in
 }
 
 int nmfb200_nmfd_set_target(nmfb200_ctx* ctx, const void* V, int dtype, void* stream) {
-  CTX_GUARD(ctx, 1);
+  CTX_GUARD(ctx, kinds(CtxKind::Nmfd));
   if (int rc = check_target(V, dtype)) return rc;
-  ctx->V = V; ctx->vdtype = dtype; ctx->has_target = true; ctx->sel = CellSel{};
+  commit_target(ctx, TargetForm::Dense, V, dtype, 0, 0);
   cudaStream_t st = (cudaStream_t)stream;
   const int64_t vin = ctx->d.v_inner();
   int rc = matrix_minmax(V, dtype, (int64_t)ctx->d.B * ctx->d.C, vin, vin, ctx->mm_scratch, ctx->mm_scratch + kMmPartials, st);
   if (rc) return rc;
-  ctx->tc_off = false;
   if (ctx->tcd) {
     double vsum = 0.0;
     rc = tc_nmfd_set_target(ctx->tcd, V, dtype, &vsum, st);       // synchronises: sum(V) for kappa
@@ -734,7 +729,7 @@ int nmfb200_nmfnd_batched_create(nmfb200_ctx** out, int device, int64_t P, int64
   if (!guard.ok) return fail(NMFB200_ERR_CUDA, "cannot select the requested device");
   nmfb200_ctx* c = new (std::nothrow) nmfb200_ctx();
   if (!c) return fail(NMFB200_ERR_INVALID, "out of host memory");
-  c->kind = kBatchedNmfd; c->device = device; c->precision = NMFB200_PREC_F32; c->R = R; c->d = d; c->nprob = P;
+  c->kind = CtxKind::NmfdBatch; c->device = device; c->precision = NMFB200_PREC_F32; c->R = R; c->d = d; c->nprob = P;
   // each problem's plan is the single problem's: same wgrad / dgrad splits, tiles, loss blocks and column-sum blocks
   c->nslab[0] = nmfd_wgrad_nsplit(d);
   c->nslab[1] = nmfd_dgrad_nsplit(d);
@@ -794,7 +789,7 @@ int nmfb200_nmfnd_batched_create_ragged(nmfb200_ctx** out, int device, int64_t P
   if (!guard.ok) return fail(NMFB200_ERR_CUDA, "cannot select the requested device");
   nmfb200_ctx* c = new (std::nothrow) nmfb200_ctx();
   if (!c) return fail(NMFB200_ERR_INVALID, "out of host memory");
-  c->kind = kBatchedNmfd; c->device = device; c->precision = NMFB200_PREC_F32; c->R = R; c->d = d; c->nprob = P;
+  c->kind = CtxKind::NmfdBatch; c->device = device; c->precision = NMFB200_PREC_F32; c->R = R; c->d = d; c->nprob = P;
   c->nslab[0] = nmfd_wgrad_nsplit(d);
   c->nslab[1] = dgrad_nsplit;            // the dgrad launch's grid y; each problem runs its own splits
   c->part_floats = part;
@@ -812,12 +807,12 @@ int nmfb200_nmfnd_batched_create_ragged(nmfb200_ctx** out, int device, int64_t P
 }
 
 int nmfb200_nmfd_batched_set_target(nmfb200_ctx* ctx, const void* V, int64_t problem_stride, int dtype, void* stream) {
-  CTX_GUARD(ctx, kBatchedNmfd);
+  CTX_GUARD(ctx, kinds(CtxKind::NmfdBatch));
   if (int rc = check_target(V, dtype)) return rc;
   const int64_t vin = ctx->d.v_inner(), rows = (int64_t)ctx->d.B * ctx->d.C;
   if (problem_stride != 0 && problem_stride < rows * vin)
     return fail(NMFB200_ERR_INVALID, "problem stride must be 0 (one shared target) or at least B x C x prod(X)");
-  ctx->V = V; ctx->vdtype = dtype; ctx->bstride = problem_stride; ctx->has_target = true;
+  commit_target(ctx, TargetForm::Dense, V, dtype, 0, problem_stride);
   if (ctx->rag)           // a ragged batch: every problem's real positions of each line, even of a shared target
     return matrix_minmax(V, dtype, rows * (vin / ctx->d.L), ctx->d.L, ctx->d.L, ctx->mm_scratch, ctx->mm_scratch + kMmPartials,
                          (cudaStream_t)stream, CellSel{}, ctx->nprob, problem_stride, ctx->rag, true);
@@ -826,7 +821,7 @@ int nmfb200_nmfd_batched_set_target(nmfb200_ctx* ctx, const void* V, int64_t pro
 }
 
 int nmfb200_nmfd_batched_set_active(nmfb200_ctx* ctx, const uint8_t* active, void* stream) {
-  CTX_GUARD(ctx, kBatchedNmfd);
+  CTX_GUARD(ctx, kinds(CtxKind::NmfdBatch));
   (void)stream;
   ctx->active = active;
   return 0;
@@ -841,7 +836,7 @@ int nmfb200_nmfd_plan(int64_t B, int64_t C, int ndim, const int64_t* vdims, int6
   nmfd_plan(d, &p);
   const WgradPlan& w = p.wgrad;
   nmfb200_ctx c;                      // the shape alone, for the ratio stage's views of W and H
-  c.kind = 1; c.R = R; c.d = d;
+  c.kind = CtxKind::Nmfd; c.R = R; c.d = d;
   const int64_t v[NMFB200_NMFD_PLAN_LEN] = {
       p.recon_mt, p.recon_grid.x, p.recon_grid.y, p.recon_grid.z,
       p.dgrad_mt, p.dgrad_nsplit, p.dgrad_grid.x, p.dgrad_grid.y, p.dgrad_grid.z,
@@ -883,10 +878,10 @@ int nmfb200_nmf_tc_plan(int64_t N, int64_t C, int64_t R, int precision, int num_
 namespace {
 // set_mask / set_weight: one selector replaces the other
 int set_selector(nmfb200_ctx* ctx, CellSel sel, void* stream) {
-  CTX_GUARD(ctx, kAnyKind);
+  CTX_GUARD(ctx, kDenseModels);
   TARGET_GUARD(ctx);
   if (is_batch(ctx)) return fail(NMFB200_ERR_INVALID, "batched fits take no mask or weight");
-  if (ctx->sparse)
+  if (is_sparse(ctx))
     return fail(NMFB200_ERR_INVALID, std::string(sel.kind == kSelWeight ? "a weight" : "a mask") +
                                          " needs a dense target (set_target or nmfd_set_target)");
   cudaStream_t st = (cudaStream_t)stream;
@@ -894,7 +889,7 @@ int set_selector(nmfb200_ctx* ctx, CellSel sel, void* stream) {
   // the tensor-core paths are bypassed while a selector is set: their operand copies are rebuilt on their next use
   mark_stale(ctx, true, true);
   float* minmax = ctx->mm_scratch + kMmPartials;          // target_minmax: the selected cells only, or all of V again
-  if (ctx->kind == 0)
+  if (ctx->kind == CtxKind::Nmf)
     return matrix_minmax(ctx->V, ctx->vdtype, ctx->N, ctx->C, ctx->ldv, ctx->mm_scratch, minmax, st, ctx->sel);
   const int64_t vin = ctx->d.v_inner();
   return matrix_minmax(ctx->V, ctx->vdtype, (int64_t)ctx->d.B * ctx->d.C, vin, vin, ctx->mm_scratch, minmax, st, ctx->sel);
@@ -913,8 +908,8 @@ namespace {
 // beta 1 and 2 run on every sparse context; any other beta > 0 only on one set by nmfb200_nmf_set_target_sparse_any_beta,
 // every beta on one set by nmfb200_nmf_set_target_observed
 int check_sparse_beta(const nmfb200_ctx* ctx, double beta) {
-  if (beta == 1.0 || beta == 2.0 || ctx->observed) return 0;
-  if (!ctx->sp_any_beta)
+  if (beta == 1.0 || beta == 2.0 || ctx->form == TargetForm::Observed) return 0;
+  if (ctx->form != TargetForm::SparseAnyBeta)
     return fail(NMFB200_ERR_INVALID, "sparse targets: beta must be 1 or 2 (densify the target for other beta)");
   if (!(beta > 0.0)) return fail(NMFB200_ERR_INVALID, "sparse targets: beta must be positive");
   return 0;
@@ -929,11 +924,11 @@ int sparse_terms(nmfb200_ctx* ctx, int which, const float* F, const float* other
   if (int rc = check_sparse_beta(ctx, beta)) return rc;
   const int R = (int)ctx->R;
   const FactorDims f = factor_dims(ctx, which);
-  const int64_t* ptr = which == 0 ? ctx->sp_ccol : ctx->sp_crow;
-  const int64_t* idx = which == 0 ? ctx->sp_row : ctx->sp_col;
-  const float* val = which == 0 ? ctx->sp_val_t : ctx->sp_val;
-  if (ctx->observed)
-    return observed_terms(ptr, idx, val, F, other, R, f.rows, beta, num, den, st, which == 0 ? ctx->sp_wt_t : ctx->sp_wt);
+  const int64_t* ptr = which == 0 ? ctx->sp.ccol : ctx->sp.crow;
+  const int64_t* idx = which == 0 ? ctx->sp.row : ctx->sp.col;
+  const float* val = which == 0 ? ctx->sp.val_t : ctx->sp.val;
+  if (ctx->form == TargetForm::Observed)
+    return observed_terms(ptr, idx, val, F, other, R, f.rows, beta, num, den, st, which == 0 ? ctx->sp.wt_t : ctx->sp.wt);
   int rc = sparse_numerator(ptr, idx, val, F, other, R, f.rows, beta, num, st);
   if (rc) return rc;
   if (beta != 1.0 && beta != 2.0) {     // the V-free denominator on the dense fp32 plan, its chunks summed as the dense path does
@@ -959,7 +954,7 @@ int simt_contract(nmfb200_ctx* c, int which, const float* W, const float* H, dou
   const FactorDims f = factor_dims(c, which);
   // a batch: problem b's target, factors and partials (slab layout [chunk][problem][rows][R]); one problem otherwise
   Batch bt;
-  if (c->kind == kBatched) bt = Batch{c->nprob, c->bstride, f.rows * c->R, f.other_rows * c->R, f.rows * c->R, c->active};
+  if (is_batch(c)) bt = Batch{c->nprob, c->bstride, f.rows * c->R, f.other_rows * c->R, f.rows * c->R, c->active};
   if (c->rag) { bt.rag = c->rag; bt.rag_launch = which == 0 ? kRagW : kRagH; bt.rag_gx = c->rag_gx[bt.rag_launch]; }
   return simt_nmf_contract(c->V, c->vdtype, c->ldv, /*trans=*/which == 0, fac[which], fac[1 - which], f.rows, f.other_rows,
                            (int)c->R, beta, c->nslab[which], c->num, c->den, c->R, f.rows * c->R * c->nprob, c->sel, c->C,
@@ -1001,10 +996,10 @@ int factor_terms(nmfb200_ctx* c, int which, const float* W, const float* H, doub
   const bool kl = kl_colsum(c, beta);
   // where the final-form terms go without `out`: c->colsum is [colsum(W) | colsum(H)], the sparse raw denominator lives in
   // c->den at beta 2 and on observed cells, and in c->sp_den at other beta (whose c->den holds the chunks)
-  if (c->sparse && beta == 2.0 && !out) { int e = ensure_den(c); if (e) return e; }
+  if (is_sparse(c) && beta == 2.0 && !out) { int e = ensure_den(c); if (e) return e; }
   float* num_out = out ? out : c->num;
-  float* den_out = out ? out + a.numel
-                 : kl ? c->colsum + (1 - which) * c->R * c->nprob : (beta == 2.0 || c->observed) ? c->den : c->sp_den;
+  float* den_out = out ? out + a.numel : kl ? c->colsum + (1 - which) * c->R * c->nprob
+                 : (beta == 2.0 || c->form == TargetForm::Observed) ? c->den : c->sp_den;
   *tc = c->tcd && use_tc(c, beta);
   if (*tc) {                  // NMFD beta 1: the recon pass also brings both column sums and kappa up to date
     int rc = tc_nmfd_recon(c->tcd, c->V, c->vdtype, W, H, false, nullptr, st);
@@ -1016,7 +1011,7 @@ int factor_terms(nmfb200_ctx* c, int which, const float* W, const float* H, doub
     a.num = part; a.nchunks = nsplit; a.kl_den = cs; a.kappa = tc_nmfd_kappa(c->tcd); a.kappa_vec = cs;
     return 0;
   }
-  if (c->sparse) {
+  if (is_sparse(c)) {
     a.num = num_out;
     if (kl) a.kl_den = den_out;
     else a.den = den_out;
@@ -1053,14 +1048,14 @@ int update_factor(nmfb200_ctx* ctx, int which, float* param, const float* W, con
 int sparse_loss_ctx(nmfb200_ctx* ctx, const float* W, const float* H, double beta, double* loss_dev, cudaStream_t st) {
   if (int rc = check_sparse_beta(ctx, beta)) return rc;
   const int R = (int)ctx->R;
-  if (ctx->observed)                    // every cell's term at the observed cells, nothing elsewhere
-    return observed_loss(ctx->sp_crow, ctx->sp_col, ctx->sp_val, H, W, R, ctx->N, beta, ctx->sp_loss_part, loss_dev, st,
-                         ctx->sp_wt);
+  if (ctx->form == TargetForm::Observed)      // every cell's term at the observed cells, nothing elsewhere
+    return observed_loss(ctx->sp.crow, ctx->sp.col, ctx->sp.val, H, W, R, ctx->N, beta, ctx->sp_loss_part, loss_dev, st,
+                         ctx->sp.wt);
   if (beta != 1.0 && beta != 2.0) {     // pos = sum x^beta over every cell without V, then V_norm - neg at the non-zeros
     int npos = 0;
     int rc = simt_nmf_pow_sum(H, W, ctx->N, ctx->C, R, beta, ctx->loss_blocks, ctx->loss_max_blocks, &npos, st);
     if (rc) return rc;
-    return sparse_beta_loss(ctx->sp_crow, ctx->sp_col, ctx->sp_val, H, W, R, ctx->N, beta, ctx->loss_blocks, npos,
+    return sparse_beta_loss(ctx->sp.crow, ctx->sp.col, ctx->sp.val, H, W, R, ctx->N, beta, ctx->loss_blocks, npos,
                             ctx->sp_loss_part, loss_dev, st);
   }
   const float *pa, *pb;
@@ -1075,8 +1070,8 @@ int sparse_loss_ctx(nmfb200_ctx* ctx, const float* W, const float* H, double bet
     pa = ctx->sp_gram; pb = ctx->sp_gram + R * R;
   }
   if (rc) return rc;
-  return sparse_loss(ctx->sp_crow, ctx->sp_col, ctx->sp_val, H, W, R, ctx->N, beta, pa, pb,
-                     beta == 1.0 ? ctx->sp_vnorm_kl : ctx->sp_vnorm_eu, ctx->sp_loss_part, loss_dev, st);
+  return sparse_loss(ctx->sp.crow, ctx->sp.col, ctx->sp.val, H, W, R, ctx->N, beta, pa, pb,
+                     beta == 1.0 ? ctx->sp.vnorm_kl : ctx->sp.vnorm_eu, ctx->sp_loss_part, loss_dev, st);
 }
 }  // namespace
 
@@ -1085,7 +1080,7 @@ int nmfb200_target_minmax(nmfb200_ctx* ctx, float* vmin, float* vmax, void* stre
   DeviceGuard guard(ctx->device);
   if (!guard.ok) return fail(NMFB200_ERR_CUDA, "cannot select the context's device");
   TARGET_GUARD(ctx);
-  if (!ctx->mm_scratch) return fail(NMFB200_ERR_INVALID, "wrong context kind");
+  if (ctx->kind == CtxKind::PlcaSparse) return fail(NMFB200_ERR_INVALID, "wrong context kind");
   float mm[2];
   NMF_CUDA_CHECK(cudaMemcpyAsync(mm, ctx->mm_scratch + kMmPartials, sizeof(mm), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
   NMF_CUDA_CHECK(cudaStreamSynchronize((cudaStream_t)stream));
@@ -1111,10 +1106,10 @@ int nmfb200_nmf_iterate(nmfb200_ctx* ctx, float* W, float* H, double beta, doubl
 
 int nmfb200_nmf_loss_prefetch_w(nmfb200_ctx* ctx, const float* W, const float* H, double beta, double* loss_dev,
                                 void* stream) {
-  CTX_GUARD(ctx, 0);
+  CTX_GUARD(ctx, kinds(CtxKind::Nmf));
   TARGET_GUARD(ctx);
   if (!W || !H || !loss_dev) return fail(NMFB200_ERR_INVALID, "null pointer");
-  if (!ctx->sparse && use_tc(ctx, beta))
+  if (!is_sparse(ctx) && use_tc(ctx, beta))
     return tc_loss_prefetch_w(ctx->tc, W, H, beta, loss_dev, (cudaStream_t)stream);
   return nmfb200_loss(ctx, W, H, beta, loss_dev, stream);
 }
@@ -1122,37 +1117,37 @@ int nmfb200_nmf_loss_prefetch_w(nmfb200_ctx* ctx, const float* W, const float* H
 /* ---- row-sharded W update over peer memory (NVLink, one process per GPU) ---------------------- */
 
 int nmfb200_nmf_peer_supported(const nmfb200_ctx* ctx, double beta) {
-  if (!ctx || ctx->kind != 0 || !ctx->has_target || !use_tc(ctx, beta)) return 0;
+  if (!ctx || ctx->kind != CtxKind::Nmf || !has_target(ctx) || !use_tc(ctx, beta)) return 0;
   return tc_peer_supported(ctx->tc, beta) ? 1 : 0;
 }
 
 int nmfb200_nmf_peer_alloc(nmfb200_ctx* ctx, void* ipc_handle_out) {
-  CTX_GUARD(ctx, 0);
+  CTX_GUARD(ctx, kinds(CtxKind::Nmf));
   if (!ctx->tc) return fail(NMFB200_ERR_STATE, "the peer-memory W update needs the tensor-core path");
   if (!ipc_handle_out) return fail(NMFB200_ERR_INVALID, "null pointer");
   return tc_peer_alloc(ctx->tc, ipc_handle_out);
 }
 
 int nmfb200_nmf_peer_connect(nmfb200_ctx* ctx, int world, int rank, const void* ipc_handles) {
-  CTX_GUARD(ctx, 0);
+  CTX_GUARD(ctx, kinds(CtxKind::Nmf));
   if (!ctx->tc) return fail(NMFB200_ERR_STATE, "the peer-memory W update needs the tensor-core path");
   if (!ipc_handles) return fail(NMFB200_ERR_INVALID, "null pointer");
   return tc_peer_connect(ctx->tc, world, rank, ipc_handles);
 }
 
 int nmfb200_nmf_peer_world(const nmfb200_ctx* ctx) {
-  return (ctx && ctx->kind == 0 && ctx->tc) ? tc_peer_world(ctx->tc) : 0;
+  return (ctx && ctx->kind == CtxKind::Nmf && ctx->tc) ? tc_peer_world(ctx->tc) : 0;
 }
 
 int nmfb200_nmf_peer_release(nmfb200_ctx* ctx) {
-  CTX_GUARD(ctx, 0);
+  CTX_GUARD(ctx, kinds(CtxKind::Nmf));
   if (ctx->tc) tc_peer_release(ctx->tc);
   return 0;
 }
 
 int nmfb200_nmf_update_w_peer(nmfb200_ctx* ctx, float* W, const float* H, double beta, double gamma, double l1_reg,
                               double l2_reg, void* stream) {
-  CTX_GUARD(ctx, 0);
+  CTX_GUARD(ctx, kinds(CtxKind::Nmf));
   TARGET_GUARD(ctx);
   if (!W || !H) return fail(NMFB200_ERR_INVALID, "null factor pointer");
   if (!nmfb200_nmf_peer_supported(ctx, beta)) return fail(NMFB200_ERR_STATE, "peer-memory W update is not available for this context / beta");
@@ -1161,9 +1156,9 @@ int nmfb200_nmf_update_w_peer(nmfb200_ctx* ctx, float* W, const float* H, double
 
 int nmfb200_nmf_contract_only(nmfb200_ctx* ctx, const float* W, const float* H, int which, double beta,
                               void* stream) {
-  CTX_GUARD(ctx, 0);
+  CTX_GUARD(ctx, kinds(CtxKind::Nmf));
   TARGET_GUARD(ctx);
-  if (ctx->sparse) return fail(NMFB200_ERR_STATE, "not available for a sparse target");
+  if (is_sparse(ctx)) return fail(NMFB200_ERR_STATE, "not available for a sparse target");
   if (!W || !H) return fail(NMFB200_ERR_INVALID, "null factor pointer");
   cudaStream_t st = (cudaStream_t)stream;
   if (use_tc(ctx, beta)) return tc_contract_only(ctx->tc, W, H, which, beta, st);
@@ -1173,7 +1168,7 @@ int nmfb200_nmf_contract_only(nmfb200_ctx* ctx, const float* W, const float* H, 
 /* ---- both kinds: the arguments are checked once, then the context's own kernels run ------------------------ */
 
 int nmfb200_sync_factors(nmfb200_ctx* ctx) {
-  CTX_GUARD(ctx, kAnyKind);
+  CTX_GUARD(ctx, kDenseModels);
   // operand copies are rebuilt lazily; the CUDA-core paths read the fp32 factors directly
   mark_stale(ctx, true, true);
   return 0;
@@ -1182,7 +1177,7 @@ int nmfb200_sync_factors(nmfb200_ctx* ctx) {
 // update_w / update_h: one factor update (which = 0: param = W, 1: param = H)
 static int checked_update(nmfb200_ctx* ctx, int which, float* param, const float* W, const float* H, double beta,
                           double gamma, double l1_reg, double l2_reg, void* stream) {
-  CTX_GUARD(ctx, kAnyKind);
+  CTX_GUARD(ctx, kDenseModels);
   TARGET_GUARD(ctx);
   if (!W || !H) return fail(NMFB200_ERR_INVALID, "null factor pointer");
   return update_factor(ctx, which, param, W, H, beta, gamma, l1_reg, l2_reg, (cudaStream_t)stream);
@@ -1199,7 +1194,7 @@ int nmfb200_update_h(nmfb200_ctx* ctx, const float* W, float* H, double beta, do
 }
 
 int nmfb200_loss(nmfb200_ctx* ctx, const float* W, const float* H, double beta, double* loss_dev, void* stream) {
-  CTX_GUARD(ctx, kAnyKind);
+  CTX_GUARD(ctx, kDenseModels);
   TARGET_GUARD(ctx);
   if (!W || !H || !loss_dev) return fail(NMFB200_ERR_INVALID, "null pointer");
   cudaStream_t st = (cudaStream_t)stream;
@@ -1210,10 +1205,10 @@ int nmfb200_loss(nmfb200_ctx* ctx, const float* W, const float* H, double beta, 
     return nmfd_recon_phi(ctx->d, ctx->V, ctx->vdtype, W, H, beta, nullptr, nullptr, ctx->loss_blocks, ctx->loss_max_blocks,
                           loss_dev, st, ctx->sel, bt);
   }
-  if (ctx->sparse) return sparse_loss_ctx(ctx, W, H, beta, loss_dev, st);
+  if (is_sparse(ctx)) return sparse_loss_ctx(ctx, W, H, beta, loss_dev, st);
   if (use_tc(ctx, beta)) return tc_loss(ctx->tc, W, H, beta, loss_dev, st);
   Batch bt;         // a batch: loss_dev[b] for every active problem b
-  if (ctx->kind == kBatched) bt = Batch{ctx->nprob, ctx->bstride, ctx->N * ctx->R, ctx->C * ctx->R, 0, ctx->active};
+  if (is_batch(ctx)) bt = Batch{ctx->nprob, ctx->bstride, ctx->N * ctx->R, ctx->C * ctx->R, 0, ctx->active};
   if (ctx->rag) { bt.rag = ctx->rag; bt.rag_launch = kRagLoss; bt.rag_gx = ctx->rag_gx[kRagLoss]; }
   return simt_nmf_loss(ctx->V, ctx->vdtype, ctx->ldv, H, W, ctx->N, ctx->C, (int)ctx->R, beta, ctx->loss_blocks,
                        ctx->loss_max_blocks, loss_dev, ctx->sel, ctx->C, st, bt);
@@ -1228,7 +1223,7 @@ int64_t nmfb200_raw_terms_numel(const nmfb200_ctx* ctx, int which, double beta) 
 // The raw terms of one factor's update (which = 0: W, 1: H) into `out`, nmfb200_raw_terms_numel floats: the partial slabs
 // summed with the centring term folded in (raw_sum), then the KL column sums at beta 1.
 int nmfb200_raw_terms(nmfb200_ctx* ctx, const float* W, const float* H, int which, double beta, float* out, void* stream) {
-  CTX_GUARD(ctx, kAnyKind);
+  CTX_GUARD(ctx, kDenseModels);
   TARGET_GUARD(ctx);
   if (!W || !H || !out || (which != 0 && which != 1)) return fail(NMFB200_ERR_INVALID, "bad argument");
   cudaStream_t st = (cudaStream_t)stream;
@@ -1248,7 +1243,7 @@ int nmfb200_raw_terms(nmfb200_ctx* ctx, const float* W, const float* H, int whic
 // The update's ratio stage on summed raw W terms: one slab, leaving the tensor-core state as update_w does
 int nmfb200_w_apply(nmfb200_ctx* ctx, float* W, const float* reduced, double beta, double gamma, double l1_reg,
                     double l2_reg, void* stream) {
-  CTX_GUARD(ctx, kAnyKind);
+  CTX_GUARD(ctx, kDenseModels);
   TARGET_GUARD(ctx);
   if (is_batch(ctx)) return fail(NMFB200_ERR_INVALID, "w_apply does not serve batched contexts");
   if (!W || !reduced) return fail(NMFB200_ERR_INVALID, "null pointer");
@@ -1270,10 +1265,10 @@ int nmfb200_w_apply(nmfb200_ctx* ctx, float* W, const float* reduced, double bet
 
 int nmfb200_plca_masked_terms(nmfb200_ctx* ctx, const float* W, const float* Hz, int which, float* out, double* qobs_dev,
                               void* stream) {
-  CTX_GUARD(ctx, kAnyKind);
+  CTX_GUARD(ctx, kDenseModels);
   if (is_batch(ctx)) return fail(NMFB200_ERR_INVALID, "plca_masked_terms does not serve batched contexts");
   TARGET_GUARD(ctx);
-  if (ctx->sparse || ctx->observed) return fail(NMFB200_ERR_INVALID, "plca_masked_terms needs a dense target");
+  if (is_sparse(ctx)) return fail(NMFB200_ERR_INVALID, "plca_masked_terms needs a dense target");
   if (ctx->sel.kind == kSelWeight) return fail(NMFB200_ERR_INVALID, "plca_masked_terms takes a mask, not a weight");
   if (!ctx->sel) return fail(NMFB200_ERR_STATE, "plca_masked_terms needs a mask (nmfb200_set_mask)");
   if (ctx->vdtype != NMFB200_DTYPE_F32) return fail(NMFB200_ERR_INVALID, "plca_masked_terms needs an fp32 target");
@@ -1325,7 +1320,7 @@ int cd_check(nmfb200_ctx* ctx) {
   if (is_batch(ctx)) return fail(NMFB200_ERR_INVALID, "cd: batched contexts are not served");
   if (ctx->R > 256) return fail(NMFB200_ERR_INVALID, "cd: rank must be at most 256");
   TARGET_GUARD(ctx);
-  if (ctx->observed) return fail(NMFB200_ERR_INVALID, "cd: observed-cell targets are not served");
+  if (ctx->form == TargetForm::Observed) return fail(NMFB200_ERR_INVALID, "cd: observed-cell targets are not served");
   if (ctx->sel) return fail(NMFB200_ERR_INVALID, "cd: contexts with a mask or a weight are not served");
   return 0;
 }
@@ -1359,12 +1354,12 @@ int cd_update_factor(nmfb200_ctx* c, int which, float* W, float* H, double l1_re
   float* X = which == 0 ? W : H;
   const float* other = which == 0 ? H : W;
   Batch bt;               // X / A partials (f, p), the other factor (g) and its Gram (p of the Gram) of problem b
-  if (c->kind == kBatched) bt = Batch{P, c->bstride, f.rows * R, f.other_rows * R, f.rows * R, c->active};
+  if (is_batch(c)) bt = Batch{P, c->bstride, f.rows * R, f.other_rows * R, f.rows * R, c->active};
   int nch = 1;
   int rc;
-  if (c->sparse) {            // the compressed form whose segments are X's rows (sparse_terms' choice)
-    rc = sparse_numerator(which == 0 ? c->sp_ccol : c->sp_crow, which == 0 ? c->sp_row : c->sp_col,
-                          which == 0 ? c->sp_val_t : c->sp_val, X, other, R, f.rows, 2.0, c->num, st);
+  if (is_sparse(c)) {         // the compressed form whose segments are X's rows (sparse_terms' choice)
+    rc = sparse_numerator(which == 0 ? c->sp.ccol : c->sp.crow, which == 0 ? c->sp.row : c->sp.col,
+                          which == 0 ? c->sp.val_t : c->sp.val, X, other, R, f.rows, 2.0, c->num, st);
   } else {
     if ((rc = ensure_gram(c))) return rc;
     nch = c->nslab[which];
@@ -1379,7 +1374,7 @@ int cd_update_factor(nmfb200_ctx* c, int which, float* W, float* H, double l1_re
   Batch sbt = bt;
   sbt.g = (int64_t)R * R;
   if ((rc = cd_sweep(X, f.rows, R, c->num, nch, f.rows * R * P, G, (float)l1_reg, (float)l2_reg, st, sbt))) return rc;
-  if (!c->sparse) mark_stale(c, which == 0, which == 1);   // the tensor-core operand copies of X are out of date
+  if (!is_sparse(c)) mark_stale(c, which == 0, which == 1);   // the tensor-core operand copies of X are out of date
   return 0;
 }
 
@@ -1394,14 +1389,14 @@ int cd_iterate(nmfb200_ctx* c, float* W, float* H, double l1_reg, double l2_reg,
 }  // namespace
 
 int nmfb200_nmf_cd_update(nmfb200_ctx* ctx, float* W, float* H, int which, double l1_reg, double l2_reg, void* stream) {
-  CTX_GUARD(ctx, kAnyKind);
+  CTX_GUARD(ctx, kDenseModels);
   if (int rc = cd_check(ctx)) return rc;
   if (!W || !H || (which != 0 && which != 1)) return fail(NMFB200_ERR_INVALID, "bad argument");
   return cd_update_factor(ctx, which, W, H, l1_reg, l2_reg, (cudaStream_t)stream);
 }
 
 int nmfb200_nmf_cd_iterate(nmfb200_ctx* ctx, float* W, float* H, double l1_reg, double l2_reg, int n_iter, void* stream) {
-  CTX_GUARD(ctx, kAnyKind);
+  CTX_GUARD(ctx, kDenseModels);
   if (int rc = cd_check(ctx)) return rc;
   if (!W || !H || n_iter < 0) return fail(NMFB200_ERR_INVALID, "bad argument");
   return cd_iterate(ctx, W, H, l1_reg, l2_reg, n_iter, (cudaStream_t)stream);
@@ -1409,7 +1404,7 @@ int nmfb200_nmf_cd_iterate(nmfb200_ctx* ctx, float* W, float* H, double l1_reg, 
 
 int nmfb200_nmf_batched_cd_update(nmfb200_ctx* ctx, float* W, float* H, int which, double l1_reg, double l2_reg,
                                   void* stream) {
-  CTX_GUARD(ctx, kBatched);
+  CTX_GUARD(ctx, kinds(CtxKind::NmfBatch));
   if (int rc = cd_batched_check(ctx)) return rc;
   if (!W || !H || (which != 0 && which != 1)) return fail(NMFB200_ERR_INVALID, "bad argument");
   return cd_update_factor(ctx, which, W, H, l1_reg, l2_reg, (cudaStream_t)stream);
@@ -1417,7 +1412,7 @@ int nmfb200_nmf_batched_cd_update(nmfb200_ctx* ctx, float* W, float* H, int whic
 
 int nmfb200_nmf_batched_cd_iterate(nmfb200_ctx* ctx, float* W, float* H, double l1_reg, double l2_reg, int n_iter,
                                    void* stream) {
-  CTX_GUARD(ctx, kBatched);
+  CTX_GUARD(ctx, kinds(CtxKind::NmfBatch));
   if (int rc = cd_batched_check(ctx)) return rc;
   if (!W || !H || n_iter < 0) return fail(NMFB200_ERR_INVALID, "bad argument");
   return cd_iterate(ctx, W, H, l1_reg, l2_reg, n_iter, (cudaStream_t)stream);
@@ -1453,7 +1448,7 @@ int64_t nmfb200_plca_work_numel(const nmfb200_ctx* ctx) {
 
 int nmfb200_plca_iterate(nmfb200_ctx* ctx, float* W, float* H, float* Z, float* Hz, float* work, int flags,
                          const float* W_alpha, const float* H_alpha, const float* Z_alpha, int n_iter, void* stream) {
-  CTX_GUARD(ctx, kAnyKind);
+  CTX_GUARD(ctx, kDenseModels);
   if (!is_batch(ctx)) return fail(NMFB200_ERR_INVALID, "plca_iterate takes a batched NMF or NMFD context");
   if (ctx->rag && is_nmfd(ctx)) return fail(NMFB200_ERR_INVALID, "plca_iterate does not serve a ragged NMFD batch");
   TARGET_GUARD(ctx);
@@ -1479,7 +1474,7 @@ int nmfb200_plca_iterate(nmfb200_ctx* ctx, float* W, float* H, float* Z, float* 
 
 int nmfb200_plca_loss(nmfb200_ctx* ctx, const float* W, const float* Hz, const float* norm_dev, double* loss_dev,
                       void* stream) {
-  CTX_GUARD(ctx, kAnyKind);
+  CTX_GUARD(ctx, kDenseModels);
   if (!is_batch(ctx)) return fail(NMFB200_ERR_INVALID, "plca_loss takes a batched NMF or NMFD context");
   if (ctx->rag && is_nmfd(ctx)) return fail(NMFB200_ERR_INVALID, "plca_loss does not serve a ragged NMFD batch");
   TARGET_GUARD(ctx);
@@ -1512,7 +1507,7 @@ int nmfb200_plca_sparse_create(nmfb200_ctx** out, int device, int64_t N, int64_t
   if (!guard.ok) return fail(NMFB200_ERR_CUDA, "cannot select the requested device");
   nmfb200_ctx* c = new (std::nothrow) nmfb200_ctx();
   if (!c) return fail(NMFB200_ERR_INVALID, "out of host memory");
-  c->kind = kPlcaSparse; c->device = device; c->N = N; c->C = C; c->R = R;
+  c->kind = CtxKind::PlcaSparse; c->device = device; c->N = N; c->C = C; c->R = R;
   c->spl_nnz = nnz;
   const int64_t pb = nnz * (int64_t)sizeof(float), lb = sparse_plca_loss_parts(N) * (int64_t)sizeof(double);
   const int64_t cb = (sparse_plca_colsum_parts(C, (int)R) + sparse_plca_colsum_parts(N, (int)R)) * (int64_t)sizeof(double);
@@ -1530,29 +1525,30 @@ int nmfb200_plca_sparse_create(nmfb200_ctx** out, int device, int64_t N, int64_t
 
 int nmfb200_plca_sparse_set_target(nmfb200_ctx* ctx, const int64_t* crow, const int64_t* col, const float* val,
                                    const int64_t* ccol, const int64_t* row, const int64_t* perm, void* stream) {
-  CTX_GUARD(ctx, kPlcaSparse);
+  CTX_GUARD(ctx, kinds(CtxKind::PlcaSparse));
   (void)stream;
   if (!crow || !ccol || (ctx->spl_nnz > 0 && (!col || !val || !row || !perm)))
     return fail(NMFB200_ERR_INVALID, "bad compressed sparse target");
-  SparsePlcaTarget& t = ctx->spl;
-  t.crow = crow; t.col = col; t.val = val; t.ccol = ccol; t.row = row; t.perm = perm;
-  t.N = ctx->N; t.C = ctx->C; t.R = (int)ctx->R;
-  ctx->has_target = true;
+  SparseTarget sp{crow, col, val, ccol, row};
+  sp.perm = perm;
+  commit_target(ctx, TargetForm::Sparse, nullptr, NMFB200_DTYPE_F32, 0, 0, sp);
   return 0;
 }
 
 int nmfb200_plca_sparse_terms(nmfb200_ctx* ctx, const float* W, const float* Hz, float* out, float norm, double* loss_dev,
                               void* stream) {
-  CTX_GUARD(ctx, kPlcaSparse);
+  CTX_GUARD(ctx, kinds(CtxKind::PlcaSparse));
   TARGET_GUARD(ctx);
   if (!W || !Hz || (!out && !loss_dev)) return fail(NMFB200_ERR_INVALID, "null pointer");
   float* dW = out;
   float* dHz = out ? out + ctx->C * ctx->R : nullptr;
-  return sparse_plca_terms(ctx->spl, ctx->splw, W, Hz, dW, dHz, norm, loss_dev, (cudaStream_t)stream);
+  const SparseTarget& s = ctx->sp;
+  const SparsePlcaTarget t{s.crow, s.col, s.ccol, s.row, s.perm, s.val, ctx->N, ctx->C, (int)ctx->R};
+  return sparse_plca_terms(t, ctx->splw, W, Hz, dW, dHz, norm, loss_dev, (cudaStream_t)stream);
 }
 
 int64_t nmfb200_plca_sparse_device_bytes(const nmfb200_ctx* ctx) {
-  if (!ctx || ctx->kind != kPlcaSparse) return -1;
+  if (!ctx || ctx->kind != CtxKind::PlcaSparse) return -1;
   return ctx->spl_bytes;
 }
 

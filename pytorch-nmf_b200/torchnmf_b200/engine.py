@@ -26,6 +26,11 @@ def _stream(device):
     return ctypes.c_void_p(torch.cuda.current_stream(device).cuda_stream)
 
 
+def _device_index(device):
+    """The CUDA ordinal the library is given for `device` (a bare "cuda": the current device)."""
+    return device.index if device.index is not None else torch.cuda.current_device()
+
+
 def _check_f32_cuda(t, name, device):
     if t.dtype != torch.float32:
         raise TypeError(f"{name} must be float32 (got {t.dtype}); the engine mirrors the reference's default dtype")
@@ -138,8 +143,8 @@ def hoyer_project_(x, dim, k1, k2):
     assert k1.numel() == D and k2.numel() == D
     zeroed = torch.empty(x.numel(), dtype=torch.uint8, device=x.device)
     lib = _capi.load()
-    _capi.check(lib.nmfb200_hoyer_project(x.device.index if x.device.index is not None else torch.cuda.current_device(),
-                                          _ptr(x), outer, D, inner, _ptr(k1), _ptr(k2), _ptr(zeroed), _stream(x.device)))
+    _capi.check(lib.nmfb200_hoyer_project(_device_index(x.device), _ptr(x), outer, D, inner, _ptr(k1), _ptr(k2), _ptr(zeroed),
+                                          _stream(x.device)))
     return x
 
 
@@ -329,7 +334,7 @@ class CudaNmfEngine(_CudaEngine):
         assert W.shape == (C, R) and H.shape == (N, R)
         self.V, self.W, self.H = V, W, H
         self.N, self.C, self.R = N, C, R
-        dev_index = self.device.index if self.device.index is not None else torch.cuda.current_device()
+        dev_index = _device_index(self.device)
         self._acquire(("nmf", dev_index, N, C, R, precision),
                       lambda ref: self._lib.nmfb200_nmf_create(ref, dev_index, N, C, R, _capi.PRECISIONS[precision]))
         self._loss = torch.zeros(1, dtype=torch.float64, device=self.device)
@@ -391,7 +396,18 @@ class CudaNmfEngine(_CudaEngine):
                                                         l2_reg, _stream(self.device)))
 
 
-class _BatchedEngine(_CudaEngine):
+class _F32Engine(_CudaEngine):
+    """An engine whose context runs the fp32 kernels only."""
+
+    @property
+    def precision(self):
+        return "f32"
+
+    def precision_for(self, beta):
+        return "f32"
+
+
+class _BatchedEngine(_F32Engine):
     """What the batched engines share: the problems are the leading axis of W and H, every launch runs the active ones, and
     the loss is one value per problem."""
     _set_active = None                     # the C ABI's set_active call of this context kind
@@ -409,9 +425,8 @@ class _BatchedEngine(_CudaEngine):
             raise ValueError(f"V is on {V.device}, expected {self.device}")
         for t, n in ((W, "W"), (H, "H")):
             _check_f32_cuda(t, n, self.device)
-        dev_index = self.device.index if self.device.index is not None else torch.cuda.current_device()
         self._loss = torch.zeros(W.shape[0], dtype=torch.float64, device=self.device)
-        self._create(V, W, H, dev_index)
+        self._create(V, W, H, _device_index(self.device))
         self.V, self.W, self.H = V, W, H
         self.set_active(None)
         self.sync()
@@ -419,13 +434,6 @@ class _BatchedEngine(_CudaEngine):
     def _create(self, V, W, H, dev_index):
         """Check the shapes, take a context for them and set V (problems on axis 0) as its target."""
         raise NotImplementedError
-
-    @property
-    def precision(self):
-        return "f32"
-
-    def precision_for(self, beta):
-        return "f32"
 
     def set_active(self, active):
         """Run only the problems whose flag is set from now on: `active` is a bool sequence or tensor of one flag per
@@ -598,17 +606,16 @@ def _compressed_forms(V, weights=None, with_order=False):
     return forms + (order.contiguous(),) if with_order else forms
 
 
-class CudaSparseNmfEngine(_CudaEngine):
-    """NMF on a sparse target, beta 1 or 2 (reference: nmf.py:603-638): V is a coalesced sparse COO tensor (N,C) on the device;
-    its CSR and CSC forms are built here with torch (data-format plumbing) and the update terms are evaluated at the non-zeros
-    only by the library (include/nmf_b200.h: nmfb200_nmf_set_target_sparse)."""
+class _SparseEngine(_F32Engine):
+    """What the engines on a sparse target share: V is a coalesced sparse COO tensor (N,C) on the device of W (C,R) and
+    H (N,R), both contiguous fp32.  The target's compressed forms (_compressed_forms of V, `weights` and `with_order`) are
+    built here with torch (data-format plumbing) and kept alive for the context, which borrows them."""
     kind = "nmf"
-    _set_target = "nmfb200_nmf_set_target_sparse"
 
-    def __init__(self, V, W, H, precision="auto"):
+    def __init__(self, V, W, H, h_name="H", weights=None, with_order=False):
         super().__init__()
         self.device = W.device
-        for t, n in ((W, "W"), (H, "H")):
+        for t, n in ((W, "W"), (H, h_name)):
             _check_f32_cuda(t, n, self.device)
         assert V.is_sparse and V.is_coalesced() and V.device == W.device
         N, C = V.shape
@@ -616,30 +623,37 @@ class CudaSparseNmfEngine(_CudaEngine):
         assert W.shape == (C, R) and H.shape == (N, R)
         self.W, self.H = W, H
         self.N, self.C, self.R = N, C, R
-        self._crow, self._col, self._val, self._ccol, self._row, self._val_t = _compressed_forms(V)
-        vals = self._val
+        if weights is not None:
+            assert weights.shape == (V._nnz(),) and weights.device == W.device
+        self._forms = _compressed_forms(V, weights, with_order)
+        self._loss = torch.zeros(1, dtype=torch.float64, device=self.device)
+
+    def _acquire_nmf(self):
+        """Take a cached or new fp32 NMF context of the engine's shape: the sparse and observed-cell NMF targets run on it."""
+        dev_index, N, C, R = _device_index(self.device), self.N, self.C, self.R
+        self._acquire(("nmf", dev_index, N, C, R, "f32"),
+                      lambda ref: self._lib.nmfb200_nmf_create(ref, dev_index, N, C, R, _capi.PRECISIONS["f32"]))
+
+
+class CudaSparseNmfEngine(_SparseEngine):
+    """NMF on a sparse target, beta 1 or 2 (reference: nmf.py:603-638): the update terms are evaluated at the non-zeros
+    only by the library (include/nmf_b200.h: nmfb200_nmf_set_target_sparse)."""
+    _set_target = "nmfb200_nmf_set_target_sparse"
+
+    def __init__(self, V, W, H, precision="auto"):
+        super().__init__(V, W, H)
+        vals = self._forms[2]
         nnz = int(vals.numel())
         v64 = vals.double()
         pos = v64[v64 > 0]
-        self._vnorm_kl = float((pos * pos.log()).sum() - v64.sum())                # nmf.py:166-167 (0 log 0 = 0)
-        self._vnorm_eu = float((v64 * v64).sum() * 0.5)                            # nmf.py:164-165
+        vnorm_kl = float((pos * pos.log()).sum() - v64.sum())                # nmf.py:166-167 (0 log 0 = 0)
+        vnorm_eu = float((v64 * v64).sum() * 0.5)                            # nmf.py:164-165
         self._vmin = float(vals.min()) if nnz else 0.0
         self._vmax = float(vals.max()) if nnz else 0.0
-        self._has_zeros = nnz < N * C
-        dev_index = self.device.index if self.device.index is not None else torch.cuda.current_device()
-        self._acquire(("nmf", dev_index, N, C, R, "f32"),
-                      lambda ref: self._lib.nmfb200_nmf_create(ref, dev_index, N, C, R, _capi.PRECISIONS["f32"]))
-        self._loss = torch.zeros(1, dtype=torch.float64, device=self.device)
-        _capi.check(getattr(self._lib, self._set_target)(
-            self._ctx, nnz, _ptr(self._crow), _ptr(self._col), _ptr(self._val), _ptr(self._ccol), _ptr(self._row),
-            _ptr(self._val_t), self._vnorm_kl, self._vnorm_eu, _stream(self.device)))
-
-    @property
-    def precision(self):
-        return "f32"
-
-    def precision_for(self, beta):
-        return "f32"
+        self._has_zeros = nnz < self.N * self.C
+        self._acquire_nmf()
+        _capi.check(getattr(self._lib, self._set_target)(self._ctx, nnz, *(_ptr(t) for t in self._forms), vnorm_kl,
+                                                          vnorm_eu, _stream(self.device)))
 
     def minmax(self):
         return (min(self._vmin, 0.0) if self._has_zeros else self._vmin), self._vmax
@@ -656,7 +670,7 @@ class CudaSparseAnyBetaEngine(CudaSparseNmfEngine):
     _set_target = "nmfb200_nmf_set_target_sparse_any_beta"
 
 
-class CudaSparsePlcaEngine(_CudaEngine):
+class CudaSparsePlcaEngine(_SparseEngine):
     """One EM step's gradients of a PLCA fit on a sparse target (include/nmf_b200.h: nmfb200_plca_sparse_*): Vn is a
     coalesced sparse COO tensor (N,C) of V / sum(V) with fp32 values on the device, W (C,R) and Hz = H diag(Z) (N,R)
     contiguous fp32 on the same device.  Its own context kind: the device holds O(nnz + (N + C) R), nothing of size N x C,
@@ -664,31 +678,15 @@ class CudaSparsePlcaEngine(_CudaEngine):
     kind = "plca_sparse"
 
     def __init__(self, Vn, W, Hz):
-        super().__init__()
-        self.device = W.device
-        for t, n in ((W, "W"), (Hz, "Hz")):
-            _check_f32_cuda(t, n, self.device)
-        assert Vn.is_sparse and Vn.is_coalesced() and Vn.device == W.device
-        N, C = Vn.shape
-        R = W.shape[1]
-        assert W.shape == (C, R) and Hz.shape == (N, R)
-        self.W, self.H = W, Hz
-        self.N, self.C, self.R = N, C, R
-        crow, col, val, ccol, row, _, perm = _compressed_forms(Vn, with_order=True)
-        self._forms = (crow, col, val, ccol, row, perm)          # borrowed by the context: kept alive here
-        dev_index = self.device.index if self.device.index is not None else torch.cuda.current_device()
-        _capi.check(self._lib.nmfb200_plca_sparse_create(ctypes.byref(self._ctx), dev_index, N, C, R, int(val.numel())))
+        super().__init__(Vn, W, Hz, h_name="Hz", with_order=True)
+        crow, col, val, ccol, row, _, perm = self._forms
+        self._forms = (crow, col, val, ccol, row, perm)          # the CSC values are not read: not kept
+        N, C, R = self.N, self.C, self.R
+        _capi.check(self._lib.nmfb200_plca_sparse_create(ctypes.byref(self._ctx), _device_index(self.device), N, C, R,
+                                                         int(val.numel())))
         _capi.check(self._lib.nmfb200_plca_sparse_set_target(self._ctx, *(_ptr(t) for t in self._forms),
                                                              _stream(self.device)))
         self._out = torch.empty(C * R + N * R, dtype=torch.float32, device=self.device)
-        self._loss = torch.zeros(1, dtype=torch.float64, device=self.device)
-
-    @property
-    def precision(self):
-        return "f32"
-
-    def precision_for(self, beta):
-        return "f32"
 
     def device_bytes(self):
         """Device bytes of the context's workspace (the compressed forms and the gradient buffer are torch tensors)."""
@@ -715,41 +713,20 @@ class CudaSparsePlcaEngine(_CudaEngine):
         return val
 
 
-class CudaObservedNmfEngine(_CudaEngine):
+class CudaObservedNmfEngine(_SparseEngine):
     """NMF on the observed cells of a masked fit (include/nmf_b200.h: nmfb200_nmf_set_target_observed), rank <= 256: O is a
     coalesced fp32 sparse COO tensor (N,C) on the device whose stored entries are exactly the observed cells, explicit zeros
     included, with V's values there.  The fit minimises beta_div(WH[obs], V[obs]) at every beta; every update and the loss
     touch the observed cells only, O(observed x R) per update.  `weights` (optional, one positive fp32 weight per stored entry
     of O, in O's order): the fit minimises sum_obs w d_beta(v | WH) instead (nmfb200_nmf_set_target_observed_weighted)."""
-    kind = "nmf"
 
     def __init__(self, O, W, H, precision="auto", weights=None):
-        super().__init__()
-        self.device = W.device
-        for t, n in ((W, "W"), (H, "H")):
-            _check_f32_cuda(t, n, self.device)
-        assert O.is_sparse and O.is_coalesced() and O.device == W.device
-        N, C = O.shape
-        R = W.shape[1]
-        assert W.shape == (C, R) and H.shape == (N, R)
-        self.W, self.H = W, H
-        self.N, self.C, self.R = N, C, R
-        if weights is not None:
-            assert weights.shape == (O._nnz(),) and weights.device == W.device
-        forms = _compressed_forms(O, weights)
-        self._crow, self._col, self._val, self._ccol, self._row, self._val_t = forms[:6]
-        dev_index = self.device.index if self.device.index is not None else torch.cuda.current_device()
-        self._acquire(("nmf", dev_index, N, C, R, "f32"),
-                      lambda ref: self._lib.nmfb200_nmf_create(ref, dev_index, N, C, R, _capi.PRECISIONS["f32"]))
-        self._loss = torch.zeros(1, dtype=torch.float64, device=self.device)
-        args = (self._ctx, int(self._val.numel()), _ptr(self._crow), _ptr(self._col), _ptr(self._val), _ptr(self._ccol),
-                _ptr(self._row), _ptr(self._val_t))
-        if weights is None:
-            _capi.check(self._lib.nmfb200_nmf_set_target_observed(*args, _stream(self.device)))
-        else:
-            self._wt, self._wt_t = forms[6:]
-            _capi.check(self._lib.nmfb200_nmf_set_target_observed_weighted(*args, _ptr(self._wt), _ptr(self._wt_t),
-                                                                           _stream(self.device)))
+        super().__init__(O, W, H, weights=weights)
+        self._acquire_nmf()
+        set_target = (self._lib.nmfb200_nmf_set_target_observed if weights is None
+                      else self._lib.nmfb200_nmf_set_target_observed_weighted)
+        _capi.check(set_target(self._ctx, int(self._forms[2].numel()), *(_ptr(t) for t in self._forms),
+                               _stream(self.device)))
 
     def raw_terms(self, which, beta):
         """(numerator, denominator) of the update of W (which=0) or H (which=1), both in the factor's shape at every beta."""
@@ -777,7 +754,7 @@ class CudaNmfdEngine(_CudaEngine):
         assert 1 <= nd <= 3 and len(K) == nd
         assert W.shape == (C, R, *K) and H.shape == (B, R, *(x - k + 1 for x, k in zip(X, K)))
         self.V, self.W, self.H = V, W, H
-        dev_index = self.device.index if self.device.index is not None else torch.cuda.current_device()
+        dev_index = _device_index(self.device)
         # "f16": beta 1 on the tensor-core sliding GEMMs; "auto" stays on the fp32 kernels for NMF2D / NMF3D
         vd, kd = (ctypes.c_int64 * nd)(*X), (ctypes.c_int64 * nd)(*K)
         self._acquire(("nmfd", dev_index, B, C, tuple(X), R, tuple(K), precision),
