@@ -3,6 +3,7 @@
 
 #include <algorithm>
 #include <atomic>
+#include <functional>
 #include <new>
 #include <vector>
 
@@ -36,6 +37,26 @@ struct SparseTarget {            // members in the order of the set_target_spars
   const int64_t* perm = nullptr;
 };
 
+// A device buffer a context owns: `n` elements of T, freed with the context (an empty one makes no CUDA call)
+template <class T>
+struct DevBuf {
+  T* p = nullptr;
+  int64_t n = 0;
+  DevBuf() = default;
+  DevBuf(const DevBuf&) = delete;
+  DevBuf& operator=(const DevBuf&) = delete;
+  ~DevBuf() { if (p) cudaFree(p); }
+  operator T*() const { return p; }
+  // at least `count` elements: allocated on first need, or grown (dropping the contents)
+  cudaError_t ensure(int64_t count) {
+    if (p && n >= count) return cudaSuccess;
+    if (p) { cudaFree(p); p = nullptr; n = 0; }
+    const cudaError_t e = cudaMalloc(&p, (size_t)count * sizeof(T));
+    if (e == cudaSuccess) n = count;
+    return e;
+  }
+};
+
 struct nmfb200_ctx {
   CtxKind kind = CtxKind::Nmf;
   int device = 0;
@@ -50,7 +71,7 @@ struct nmfb200_ctx {
   const uint8_t* active = nullptr;
   // a ragged batch of NMF problems (nmfb200_nmf_batched_create_ragged): each problem's plan (device, nprob of them)
   // and the grid x of each RaggedLaunch, the sum of the problems' blocks
-  RaggedProblem* rag = nullptr;
+  DevBuf<RaggedProblem> rag;
   int64_t rag_gx[4] = {0, 0, 0, 0};
   NmfdShape d{};
   const void* V = nullptr;        // the dense target, borrowed: vdtype (NMFB200_DTYPE_*) elements
@@ -62,33 +83,27 @@ struct nmfb200_ctx {
   // borrowed; cleared by every set_target*.  While set, every pass runs the selecting fp32 kernels and beta 1 takes its
   // denominators from the contraction, not the column sums.
   CellSel sel;
-  // chunked partial numerators / denominators of the CUDA-core path
-  float* num = nullptr;
-  float* den = nullptr;
-  int64_t part_floats = 0;
+  // chunked partial numerators / denominators of the CUDA-core path; den (lazy) is sized like num
+  DevBuf<float> num, den;
   int nslab[2] = {1, 1};          // partial slabs of the W / H terms: contraction chunks (NMF), wgrad / dgrad splits (NMFD)
-  float* colsum = nullptr;        // [2][R]: 0 = colsum(W), 1 = colsum(H)
-  float* cs_scratch = nullptr;
-  int64_t cs_scratch_floats = 0;
-  double* loss_blocks = nullptr;
-  int loss_max_blocks = 0;
-  float* mm_scratch = nullptr;    // kMmFloats: matrix_minmax's partials, then the target's min / max
-  float* sp_den = nullptr;        // max(N, C) x R: the reduced V-free denominator of an update at beta != 1, 2
-  float* sp_gram = nullptr;       // [2][R*R] (W^T W, H^T H) + per-block partials; also the Gram scratch of nmfb200_nmf_cd_*
-  double* sp_loss_part = nullptr;
-  // NMFD: the ratio tiles, pn_floats each (a batch: every problem's, back to back)
-  float* Pn = nullptr;
-  float* Pp = nullptr;
-  int64_t pn_floats = 0;
+  DevBuf<float> colsum;           // [2][R]: 0 = colsum(W), 1 = colsum(H)
+  DevBuf<float> cs_scratch;
+  DevBuf<double> loss_blocks;
+  DevBuf<float> mm_scratch;       // kMmFloats: matrix_minmax's partials, then the target's min / max
+  DevBuf<float> sp_den;           // max(N, C) x R: the reduced V-free denominator of an update at beta != 1, 2
+  DevBuf<float> sp_gram;          // [2][R*R] (W^T W, H^T H) + per-block partials; also the Gram scratch of nmfb200_nmf_cd_*
+  DevBuf<double> sp_loss_part;
+  // NMFD: the ratio tiles, Pp (lazy) sized like Pn (a batch: every problem's, back to back)
+  DevBuf<float> Pn, Pp;
   // nmfb200_plca_masked_terms on NMF: one q_O partial per block of the fp32 contraction (grown on demand)
-  double* qobs_part = nullptr;
-  int64_t qobs_part_n = 0;
+  DevBuf<double> qobs_part;
   // tensor-core path state (tc_nmf.cu / tc_nmfd.cu)
   TcState* tc = nullptr;
   TcNmfdState* tcd = nullptr;
-  // sparse-target PLCA: the workspace, its size in bytes and its nnz
-  SparsePlcaWork splw;
-  int64_t spl_nnz = 0, spl_bytes = 0;
+  // sparse-target PLCA: the workspace of SparsePlcaWork and its nnz
+  DevBuf<float> spl_P;
+  DevBuf<double> spl_loss_part, spl_cs_part;
+  int64_t spl_nnz = 0;
 };
 
 namespace {
@@ -152,26 +167,17 @@ int chunks_for(int64_t rows, int64_t cols, int64_t R) {
   return (int)want;
 }
 
-int ensure_den(nmfb200_ctx* c) {
-  if (!c->den) NMF_CUDA_CHECK(cudaMalloc(&c->den, c->part_floats * sizeof(float)));
-  return 0;
-}
-
-// sp_gram: the two R x R Gram matrices and sparse_gram's block partials (R <= 256).  A batch of P problems: [2][P][R^2], then
-// each problem's partials on its own Gram plan, P x max(nb(N), nb(C)) R^2 (sparse_gram_plan), not P x the fixed 128 R^2.
-int ensure_gram(nmfb200_ctx* c) {
-  if (c->sp_gram) return 0;
+// sp_gram's floats: the two R x R Gram matrices and sparse_gram's block partials (R <= 256).  A batch of P problems:
+// [2][P][R^2], then each problem's partials on its own Gram plan, P x max(nb(N), nb(C)) R^2 (sparse_gram_plan), not P x the
+// fixed 128 R^2.
+int64_t gram_floats(const nmfb200_ctx* c) {
   const int64_t R = c->R;
-  int64_t floats = 2 * R * R + sparse_gram_part_floats((int)R);
-  if (is_batch(c)) {
-    int64_t rpb;
-    int nb_n, nb_c;
-    sparse_gram_plan(c->N, &rpb, &nb_n);
-    sparse_gram_plan(c->C, &rpb, &nb_c);
-    floats = c->nprob * (2 + (int64_t)(nb_n > nb_c ? nb_n : nb_c)) * R * R;
-  }
-  NMF_CUDA_CHECK(cudaMalloc(&c->sp_gram, (size_t)floats * sizeof(float)));
-  return 0;
+  if (!is_batch(c)) return 2 * R * R + sparse_gram_part_floats((int)R);
+  int64_t rpb;
+  int nb_n, nb_c;
+  sparse_gram_plan(c->N, &rpb, &nb_n);
+  sparse_gram_plan(c->C, &rpb, &nb_c);
+  return c->nprob * (2 + (int64_t)(nb_n > nb_c ? nb_n : nb_c)) * R * R;
 }
 
 void free_ctx(nmfb200_ctx* c) {
@@ -179,27 +185,170 @@ void free_ctx(nmfb200_ctx* c) {
   DeviceGuard guard(c->device);
   if (c->tc) tc_destroy(c->tc);
   if (c->tcd) tc_nmfd_destroy(c->tcd);
-  cudaFree(c->num); cudaFree(c->den); cudaFree(c->colsum); cudaFree(c->cs_scratch);
-  cudaFree(c->loss_blocks); cudaFree(c->mm_scratch); cudaFree(c->Pn); cudaFree(c->Pp);
-  cudaFree(c->sp_gram); cudaFree(c->sp_loss_part); cudaFree(c->sp_den); cudaFree(c->qobs_part); cudaFree(c->rag);
-  cudaFree(c->splw.P); cudaFree(c->splw.loss_part); cudaFree(c->splw.cs_part);
   delete c;
 }
 
-// The create-time workspace of both kinds, sized from c->part_floats, R, cs_scratch_floats and loss_max_blocks, plus
-// `pn_floats` for NMFD's ratio tile (0: none).  On failure frees `c` and returns the error.
-int alloc_workspace(nmfb200_ctx* c, int64_t pn_floats) {
-  cudaError_t e = cudaMalloc(&c->num, c->part_floats * sizeof(float));
-  if (e == cudaSuccess) e = cudaMalloc(&c->colsum, 2 * c->R * c->nprob * sizeof(float));
-  if (e == cudaSuccess) e = cudaMalloc(&c->cs_scratch, c->cs_scratch_floats * sizeof(float));
-  if (e == cudaSuccess) e = cudaMalloc(&c->loss_blocks, (size_t)c->loss_max_blocks * sizeof(double));
-  if (e == cudaSuccess) e = cudaMalloc(&c->mm_scratch, kMmFloats * sizeof(float));
-  if (e == cudaSuccess && pn_floats) e = cudaMalloc(&c->Pn, pn_floats * sizeof(float));
-  c->pn_floats = pn_floats;
-  if (e != cudaSuccess) {
-    free_ctx(c);
-    return fail(NMFB200_ERR_CUDA, std::string("cudaMalloc: ") + cudaGetErrorString(e));
+// A context's shape and what it allocates at create: the partial slabs (num), the column-sum scratch, the loss partials and
+// NMFD's ratio tile Pn (0: none); a ragged batch's per-problem plans and the grid x of each RaggedLaunch.  nslab: the partial
+// slabs of the W / H terms (contraction chunks of NMF, wgrad / dgrad splits of NMFD).
+struct CtxPlan {
+  int64_t N = 0, C = 0, R = 0, nprob = 1;
+  NmfdShape d{};
+  int nslab[2] = {1, 1};
+  int64_t part_floats = 0, cs_scratch_floats = 0, loss_blocks = 0, pn_floats = 0;
+  std::vector<RaggedProblem> rag;
+  int64_t rag_gx[4] = {0, 0, 0, 0};
+};
+
+// P NMF problems of one shape: each problem's plan is the single problem's (P = 1), its workspace after the previous ones'
+CtxPlan plan_nmf(int64_t N, int64_t C, int64_t R, int64_t P) {
+  CtxPlan p{N, C, R, P};
+  p.nslab[0] = chunks_for(C, N, R);
+  p.nslab[1] = chunks_for(N, C, R);
+  p.part_floats = std::max((int64_t)p.nslab[0] * C * R, (int64_t)p.nslab[1] * N * R) * P;
+  p.cs_scratch_floats = colsum_scratch_floats(std::max(N, C), (int)R, 1) * P;
+  p.loss_blocks = simt_nmf_max_blocks(N, C) * P;
+  return p;
+}
+
+// A ragged batch of B NMF problems: each problem's single-problem plan along its own length, its blocks after the previous
+// problems' on grid x and its workspace after theirs
+int plan_nmf_ragged(int64_t B, int64_t N, int64_t C, int64_t R, const int64_t* lengths, CtxPlan* out) {
+  CtxPlan plan{N, C, R, B};
+  plan.rag.resize(B);
+  int64_t* gx = plan.rag_gx;
+  int64_t cs = 0;
+  const int64_t w_blocks = ceil_div(C, 64);
+  for (int64_t b = 0; b < B; ++b) {
+    const int64_t L = lengths[b];
+    if (L < 1 || L > N)
+      return fail(NMFB200_ERR_INVALID, "lengths[" + std::to_string(b) + "] = " + std::to_string(L) + " is outside [1, N]");
+    RaggedProblem& p = plan.rag[b];
+    p.rows = L;
+    p.nch[0] = chunks_for(C, L, R);
+    p.nch[1] = chunks_for(L, C, R);
+    SimtNmfPlan sp;
+    simt_nmf_plan(L, C, (int)R, p.nch[1], &sp);
+    p.loss_chunks = sp.loss_chunks;
+    p.cs_blocks = (int)colsum_scratch_floats(L, 1, 1);
+    const int64_t blocks[4] = {w_blocks * p.nch[0], ceil_div(L, 64) * p.nch[1], ceil_div(L, 64) * p.loss_chunks, p.cs_blocks};
+    for (int k = 0; k < 4; ++k) { p.x0[k] = gx[k]; gx[k] += blocks[k]; }
+    p.part = plan.part_floats; p.loss_part = plan.loss_blocks; p.cs_part = cs; p.loss_n = blocks[2];
+    plan.part_floats += std::max((int64_t)p.nch[0] * C * R, (int64_t)p.nch[1] * L * R);
+    plan.loss_blocks += blocks[2];
+    cs += p.cs_blocks * R;
+    // checked after every problem, so no sum can overflow int64 first
+    if (gx[0] > kMaxGridX || gx[1] > kMaxGridX || gx[2] > kMaxGridX || gx[3] > kMaxGridX)
+      return fail(NMFB200_ERR_INVALID, "ragged batch: the problems' blocks of one launch pass grid x (2^31 - 1)");
+    if (plan.loss_blocks > INT32_MAX) return fail(NMFB200_ERR_INVALID, "ragged batch: loss partials must be below 2^31");
   }
+  // the launches every problem shares the shape of: the column sums of W, their final stage, the ratio stage
+  if (colsum_scratch_floats(C, 1, 1) > kMaxGridX / B || ceil_div(R, 64) > kMaxGridX / B ||
+      ceil_div(std::max(N, C) * R, 256) > kMaxGridX / B)
+    return fail(NMFB200_ERR_INVALID, "batch too large for the launch grids");
+  plan.nslab[0] = chunks_for(C, N, R);      // unused by the ragged launches: each problem's own counts are in its plan
+  plan.nslab[1] = chunks_for(N, C, R);
+  plan.cs_scratch_floats = std::max(cs, colsum_scratch_floats(C, (int)R, 1) * B);
+  *out = std::move(plan);
+  return 0;
+}
+
+// P NMFD / NMF2D / NMF3D problems of shape d: each problem's plan is the single problem's (P = 1), its workspace after the
+// previous ones'
+CtxPlan plan_nmfd(const NmfdShape& d, int64_t P) {
+  const int64_t B = d.B, C = d.C, R = d.R;
+  CtxPlan p{0, 0, R, P, d};
+  p.nslab[0] = nmfd_wgrad_nsplit(d);
+  p.nslab[1] = nmfd_dgrad_nsplit(d);
+  p.part_floats = std::max((int64_t)p.nslab[0] * C * R * d.w_inner(), (int64_t)p.nslab[1] * B * R * d.h_inner()) * P;
+  p.cs_scratch_floats =
+      std::max(colsum_scratch_floats(C, (int)R, d.w_inner()), colsum_scratch_floats(B, (int)R, d.h_inner())) * P;
+  p.loss_blocks = nmfd_max_blocks(d) * P;
+  p.pn_floats = B * C * d.v_inner() * P;
+  return p;
+}
+
+// A ragged batch of P NMFD / NMF2D / NMF3D problems of padded shape d: each problem's single-problem plan along its own
+// length, its workspace after the previous problems'.  Every count is at most the padded shape's, which the batch's shape
+// checks bound for P problems.
+int plan_nmfd_ragged(const NmfdShape& d, int64_t P, const int64_t* lengths, CtxPlan* out) {
+  const int64_t B = d.B, C = d.C, R = d.R;
+  CtxPlan plan{0, 0, R, P, d};
+  plan.rag.resize(P);
+  plan.nslab[0] = nmfd_wgrad_nsplit(d);
+  const int64_t wpart = (int64_t)plan.nslab[0] * C * R * d.w_inner();
+  int64_t cs = 0;
+  for (int64_t p = 0; p < P; ++p) {
+    const int64_t L = lengths[p];
+    if (L < d.T || L > d.L)
+      return fail(NMFB200_ERR_INVALID, "lengths[" + std::to_string(p) + "] = " + std::to_string(L) + " is outside [" +
+                                           std::to_string(d.T) + ", " + std::to_string(d.L) + "] (the last kernel and target sizes)");
+    NmfdShape e = d;
+    e.L = (int)L; e.Lin = (int)(L - d.T + 1);
+    NmfdPlan np;
+    nmfd_plan(e, &np);
+    RaggedProblem& q = plan.rag[p];
+    q.rows = L; q.lin = e.Lin;
+    q.gx[0] = (int)np.recon_grid.x; q.gx[1] = (int)np.dgrad_grid.x;
+    q.nch[0] = np.wgrad_nsplit; q.nch[1] = np.dgrad_nsplit;
+    q.loss_n = nmfd_max_blocks(e);
+    // the column sums of H at beta 1 as its single fit forms them: one partial per (clip, component) run, or the rows
+    // blocking of a run of one element
+    q.cs_blocks = (int)(e.h_inner() > 1 ? B : colsum_scratch_floats(B, 1, 1));
+    q.pn = plan.pn_floats; q.part = plan.part_floats; q.loss_part = plan.loss_blocks; q.cs_part = cs;
+    plan.nslab[1] = std::max(plan.nslab[1], np.dgrad_nsplit);    // the dgrad launch's grid y; each problem runs its own splits
+    // every problem's tiles and slabs start 16-byte aligned: the ratio stage of W reads its slabs as float4 (update.cu:
+    // apply_update_vec4_kernel) wherever the shape allows, and a dgrad slab may hold any number of floats
+    plan.pn_floats += round_up(B * C * e.v_inner(), 4);
+    plan.part_floats += round_up(std::max(wpart, (int64_t)np.dgrad_nsplit * B * R * e.h_inner()), 4);
+    plan.loss_blocks += q.loss_n;
+    cs += B * R;
+  }
+  plan.cs_scratch_floats = std::max(cs, colsum_scratch_floats(C, (int)R, d.w_inner()) * P);
+  *out = std::move(plan);
+  return 0;
+}
+
+// A refused create leaves *out null
+int check_out(nmfb200_ctx** out) {
+  if (!out) return fail(NMFB200_ERR_INVALID, "out is null");
+  *out = nullptr;
+  return 0;
+}
+
+// The one constructor of every context kind, once the create's own checks have passed: selects `device`, allocates a
+// context of `kind` and plan's shape, lets `init` (if any) set or refuse the rest of it, allocates what the plan asks for and
+// uploads a ragged batch's plans, then runs `finish` (if any: the kind's tensor-core state or workspace) under the same
+// device guard.  On any failure it frees everything and leaves *out null.
+using CtxStep = std::function<int(nmfb200_ctx*)>;
+int create_ctx(nmfb200_ctx** out, int device, CtxKind kind, const CtxPlan& plan, const CtxStep& init = nullptr,
+               const CtxStep& finish = nullptr) {
+  DeviceGuard guard(device);
+  if (!guard.ok) return fail(NMFB200_ERR_CUDA, "cannot select the requested device");
+  nmfb200_ctx* c = new (std::nothrow) nmfb200_ctx();
+  if (!c) return fail(NMFB200_ERR_INVALID, "out of host memory");
+  c->kind = kind; c->device = device; c->N = plan.N; c->C = plan.C; c->R = plan.R; c->nprob = plan.nprob; c->d = plan.d;
+  c->nslab[0] = plan.nslab[0]; c->nslab[1] = plan.nslab[1];
+  for (int k = 0; k < 4; ++k) c->rag_gx[k] = plan.rag_gx[k];
+  int rc = init ? init(c) : 0;
+  if (rc == 0 && plan.part_floats) {                  // the dense models' workspace
+    cudaError_t e = c->num.ensure(plan.part_floats);
+    if (e == cudaSuccess) e = c->colsum.ensure(2 * c->R * c->nprob);
+    if (e == cudaSuccess) e = c->cs_scratch.ensure(plan.cs_scratch_floats);
+    if (e == cudaSuccess) e = c->loss_blocks.ensure(plan.loss_blocks);
+    if (e == cudaSuccess) e = c->mm_scratch.ensure(kMmFloats);
+    if (e == cudaSuccess && plan.pn_floats) e = c->Pn.ensure(plan.pn_floats);
+    if (e != cudaSuccess) rc = fail(NMFB200_ERR_CUDA, std::string("cudaMalloc: ") + cudaGetErrorString(e));
+  }
+  if (rc == 0 && !plan.rag.empty()) {
+    cudaError_t e = c->rag.ensure((int64_t)plan.rag.size());
+    if (e == cudaSuccess)
+      e = cudaMemcpy(c->rag, plan.rag.data(), plan.rag.size() * sizeof(RaggedProblem), cudaMemcpyHostToDevice);
+    if (e != cudaSuccess) rc = fail(NMFB200_ERR_CUDA, std::string("ragged batch plans: ") + cudaGetErrorString(e));
+  }
+  if (rc == 0 && finish) rc = finish(c);
+  if (rc) { free_ctx(c); return rc; }
+  *out = c;
   return 0;
 }
 
@@ -241,6 +390,23 @@ ApplyArgs factor_view(const nmfb200_ctx* c, int which, int nchunks) {
   if (c->rag) { a.rag = c->rag; a.rag_launch = which == 0 ? kRagW : kRagH; }
   if (c->rag && is_nmfd(c) && which == 1) a.line = c->d.Lin;      // a ragged NMFD batch's H: padding inside every line
   return a;
+}
+
+// The problems of one launch (kRagW / kRagH: the contraction of W / H, kRagLoss: the loss): the NMFD kernels take their
+// strides from the shape; an NMF batch's F / G factors and partial slabs of problem b (slab layout [chunk][problem][rows][R],
+// the loss: F = H, no slabs), and a ragged batch's launch and grid x.  One NMF problem: Batch{}, the single-problem kernels.
+Batch launch_batch(const nmfb200_ctx* c, RaggedLaunch launch) {
+  Batch bt;
+  if (is_nmfd(c)) {
+    bt = Batch{c->nprob, c->bstride, 0, 0, 0, c->active};
+    bt.rag = c->rag;
+    return bt;
+  }
+  if (!is_batch(c)) return bt;
+  const FactorDims f = factor_dims(c, launch == kRagW ? 0 : 1);
+  bt = Batch{c->nprob, c->bstride, f.rows * c->R, f.other_rows * c->R, launch == kRagLoss ? 0 : f.rows * c->R, c->active};
+  if (c->rag) { bt.rag = c->rag; bt.rag_launch = launch; bt.rag_gx = c->rag_gx[launch]; }
+  return bt;
 }
 
 // What every dense set_target checks of the target's element type and pointer (the kernels load single elements: element
@@ -295,13 +461,11 @@ int set_sparse_target(nmfb200_ctx* ctx, TargetForm form, int64_t nnz, const Spar
     return fail(NMFB200_ERR_INVALID, "bad compressed sparse target");
   if (ctx->R > 256)
     return fail(NMFB200_ERR_INVALID, "rank > 256 is not supported by the sparse-target kernels (densify the target)");
-  if (int rc = ensure_gram(ctx)) return rc;
-  if (!ctx->sp_loss_part)
-    NMF_CUDA_CHECK(cudaMalloc(&ctx->sp_loss_part, (size_t)sparse_gather_blocks(ctx->N) * sizeof(double)));
+  NMF_CUDA_CHECK(ctx->sp_gram.ensure(gram_floats(ctx)));
+  NMF_CUDA_CHECK(ctx->sp_loss_part.ensure(sparse_gather_blocks(ctx->N)));
   if (form != TargetForm::Sparse)                          // the denominator of an update outside raw_terms
-    if (int rc = ensure_den(ctx)) return rc;
-  if (form == TargetForm::SparseAnyBeta && !ctx->sp_den)
-    NMF_CUDA_CHECK(cudaMalloc(&ctx->sp_den, (size_t)(ctx->N > ctx->C ? ctx->N : ctx->C) * ctx->R * sizeof(float)));
+    NMF_CUDA_CHECK(ctx->den.ensure(ctx->num.n));
+  if (form == TargetForm::SparseAnyBeta) NMF_CUDA_CHECK(ctx->sp_den.ensure(std::max(ctx->N, ctx->C) * ctx->R));
   commit_target(ctx, form, nullptr, NMFB200_DTYPE_F32, 0, 0, sp);
   if (form != TargetForm::Observed) return 0;
   // target_minmax: the observed values (none: +inf / -inf)
@@ -339,41 +503,27 @@ int nmfb200_ctx_check_health(nmfb200_ctx* ctx, void* stream) {
 }
 
 int nmfb200_nmf_create(nmfb200_ctx** out, int device, int64_t N, int64_t C, int64_t R, int precision) {
-  if (!out) return fail(NMFB200_ERR_INVALID, "out is null");
-  *out = nullptr;
+  if (int rc = check_out(out)) return rc;
   if (N < 1 || C < 1 || R < 1) return fail(NMFB200_ERR_INVALID, "N, C, R must be positive");
   if (R > kMaxRank) return fail(NMFB200_ERR_INVALID, kMaxRankMsg);
   if (precision < NMFB200_PREC_AUTO || precision > NMFB200_PREC_F16_SPLIT)
     return fail(NMFB200_ERR_INVALID, "unknown precision mode");
-  DeviceGuard guard(device);
-  if (!guard.ok) return fail(NMFB200_ERR_CUDA, "cannot select the requested device");
-  nmfb200_ctx* c = new (std::nothrow) nmfb200_ctx();
-  if (!c) return fail(NMFB200_ERR_INVALID, "out of host memory");
-  c->kind = CtxKind::Nmf; c->device = device; c->N = N; c->C = C; c->R = R;
-  int resolved = precision;
-  // AUTO: single-rounded fp16 operands hold the north-star parity (rtol 1e-3) once the ratio tile is kappa-centred;
-  // the parity tests check it against the reference at the configuration shapes
-  if (precision == NMFB200_PREC_AUTO) resolved = tc_shape_supported(N, C, R) ? NMFB200_PREC_F16 : NMFB200_PREC_F32;
-  if (resolved != NMFB200_PREC_F32 && !tc_shape_supported(N, C, R)) {
-    delete c;
-    return fail(NMFB200_ERR_INVALID, "shape not supported by the tensor-core path (need R <= 128)");
-  }
-  c->precision = resolved;
-  c->auto_mode = precision == NMFB200_PREC_AUTO;
-  c->nslab[0] = chunks_for(C, N, R);
-  c->nslab[1] = chunks_for(N, C, R);
-  int64_t pf = (int64_t)c->nslab[0] * C * R;
-  if ((int64_t)c->nslab[1] * N * R > pf) pf = (int64_t)c->nslab[1] * N * R;
-  c->part_floats = pf;
-  c->cs_scratch_floats = colsum_scratch_floats(N > C ? N : C, (int)R, 1);
-  c->loss_max_blocks = simt_nmf_max_blocks(N, C);
-  if (int rc = alloc_workspace(c, 0)) return rc;
-  if (resolved != NMFB200_PREC_F32) {
-    int rc = tc_create(&c->tc, device, N, C, R, resolved == NMFB200_PREC_F16_SPLIT);
-    if (rc) { free_ctx(c); return rc; }
-  }
-  *out = c;
-  return 0;
+  auto init = [&](nmfb200_ctx* c) {
+    int resolved = precision;
+    // AUTO: single-rounded fp16 operands hold the north-star parity (rtol 1e-3) once the ratio tile is kappa-centred;
+    // the parity tests check it against the reference at the configuration shapes
+    if (precision == NMFB200_PREC_AUTO) resolved = tc_shape_supported(N, C, R) ? NMFB200_PREC_F16 : NMFB200_PREC_F32;
+    if (resolved != NMFB200_PREC_F32 && !tc_shape_supported(N, C, R))
+      return fail(NMFB200_ERR_INVALID, "shape not supported by the tensor-core path (need R <= 128)");
+    c->precision = resolved;
+    c->auto_mode = precision == NMFB200_PREC_AUTO;
+    return 0;
+  };
+  auto finish = [&](nmfb200_ctx* c) {
+    if (c->precision == NMFB200_PREC_F32) return 0;
+    return tc_create(&c->tc, device, N, C, R, c->precision == NMFB200_PREC_F16_SPLIT);
+  };
+  return create_ctx(out, device, CtxKind::Nmf, plan_nmf(N, C, R, 1), init, finish);
 }
 
 void nmfb200_destroy(nmfb200_ctx* ctx) { free_ctx(ctx); }
@@ -455,95 +605,26 @@ int nmfb200_nmf_set_target(nmfb200_ctx* ctx, const void* V, int64_t ldv, int dty
 /* ---- batched NMF: B independent problems of one shape on the fp32 kernels ------------------------------------ */
 
 int nmfb200_nmf_batched_create(nmfb200_ctx** out, int device, int64_t B, int64_t N, int64_t C, int64_t R) {
-  if (!out) return fail(NMFB200_ERR_INVALID, "out is null");
-  *out = nullptr;
+  if (int rc = check_out(out)) return rc;
   if (B < 1 || N < 1 || C < 1 || R < 1) return fail(NMFB200_ERR_INVALID, "B, N, C, R must be positive");
   if (R > 256) return fail(NMFB200_ERR_INVALID, "batched fits support rank <= 256");
   // the batch rides on grid x of every launch, the loss partials are counted in int
-  const int64_t rows = N > C ? N : C;
-  if (ceil_div(rows, 64) > kMaxGridX / B || (int64_t)simt_nmf_max_blocks(N, C) > INT32_MAX / B ||
+  if (ceil_div(std::max(N, C), 64) > kMaxGridX / B || (int64_t)simt_nmf_max_blocks(N, C) > INT32_MAX / B ||
       ceil_div(R, 64) > kMaxGridX / B)
     return fail(NMFB200_ERR_INVALID, "batch too large for the launch grids");
-  DeviceGuard guard(device);
-  if (!guard.ok) return fail(NMFB200_ERR_CUDA, "cannot select the requested device");
-  nmfb200_ctx* c = new (std::nothrow) nmfb200_ctx();
-  if (!c) return fail(NMFB200_ERR_INVALID, "out of host memory");
-  c->kind = CtxKind::NmfBatch; c->device = device; c->N = N; c->C = C; c->R = R; c->nprob = B;
-  c->precision = NMFB200_PREC_F32;
-  // each problem's plan is the single problem's: same chunks, loss blocks and column-sum blocks
-  c->nslab[0] = chunks_for(C, N, R);
-  c->nslab[1] = chunks_for(N, C, R);
-  int64_t pf = (int64_t)c->nslab[0] * C * R;
-  if ((int64_t)c->nslab[1] * N * R > pf) pf = (int64_t)c->nslab[1] * N * R;
-  c->part_floats = pf * B;
-  c->cs_scratch_floats = colsum_scratch_floats(rows, (int)R, 1) * B;
-  c->loss_max_blocks = (int)(simt_nmf_max_blocks(N, C) * B);
-  if (int rc = alloc_workspace(c, 0)) return rc;
-  *out = c;
-  return 0;
+  return create_ctx(out, device, CtxKind::NmfBatch, plan_nmf(N, C, R, B));
 }
 
 int nmfb200_nmf_batched_create_ragged(nmfb200_ctx** out, int device, int64_t B, int64_t N, int64_t C, int64_t R,
                                       const int64_t* lengths) {
-  if (!out) return fail(NMFB200_ERR_INVALID, "out is null");
-  *out = nullptr;
+  if (int rc = check_out(out)) return rc;
   if (B < 1 || N < 1 || C < 1 || R < 1) return fail(NMFB200_ERR_INVALID, "B, N, C, R must be positive");
   if (R > 256) return fail(NMFB200_ERR_INVALID, "batched fits support rank <= 256");
   if (!lengths) return fail(NMFB200_ERR_INVALID, "lengths is null");
   if (B > kMaxGridX) return fail(NMFB200_ERR_INVALID, "ragged batch: B must be below 2^31 (one block per problem and launch)");
-  // each problem's single-problem plan, its blocks after the previous problems' on grid x and its workspace after theirs
-  std::vector<RaggedProblem> t(B);
-  int64_t gx[4] = {0, 0, 0, 0}, part = 0, loss = 0, cs = 0;
-  const int64_t w_blocks = ceil_div(C, 64);
-  for (int64_t b = 0; b < B; ++b) {
-    const int64_t L = lengths[b];
-    if (L < 1 || L > N)
-      return fail(NMFB200_ERR_INVALID, "lengths[" + std::to_string(b) + "] = " + std::to_string(L) + " is outside [1, N]");
-    RaggedProblem& p = t[b];
-    p.rows = L;
-    p.nch[0] = chunks_for(C, L, R);
-    p.nch[1] = chunks_for(L, C, R);
-    SimtNmfPlan sp;
-    simt_nmf_plan(L, C, (int)R, p.nch[1], &sp);
-    p.loss_chunks = sp.loss_chunks;
-    p.cs_blocks = (int)colsum_scratch_floats(L, 1, 1);
-    const int64_t blocks[4] = {w_blocks * p.nch[0], ceil_div(L, 64) * p.nch[1], ceil_div(L, 64) * p.loss_chunks, p.cs_blocks};
-    for (int k = 0; k < 4; ++k) { p.x0[k] = gx[k]; gx[k] += blocks[k]; }
-    p.part = part; p.loss_part = loss; p.cs_part = cs; p.loss_n = blocks[2];
-    part += std::max((int64_t)p.nch[0] * C * R, (int64_t)p.nch[1] * L * R);
-    loss += blocks[2];
-    cs += p.cs_blocks * R;
-    // checked after every problem, so no sum can overflow int64 first
-    if (gx[0] > kMaxGridX || gx[1] > kMaxGridX || gx[2] > kMaxGridX || gx[3] > kMaxGridX)
-      return fail(NMFB200_ERR_INVALID, "ragged batch: the problems' blocks of one launch pass grid x (2^31 - 1)");
-    if (loss > INT32_MAX) return fail(NMFB200_ERR_INVALID, "ragged batch: loss partials must be below 2^31");
-  }
-  // the launches every problem shares the shape of: the column sums of W, their final stage, the ratio stage
-  const int64_t rows = N > C ? N : C;
-  if (colsum_scratch_floats(C, 1, 1) > kMaxGridX / B || ceil_div(R, 64) > kMaxGridX / B ||
-      ceil_div(rows * R, 256) > kMaxGridX / B)
-    return fail(NMFB200_ERR_INVALID, "batch too large for the launch grids");
-  DeviceGuard guard(device);
-  if (!guard.ok) return fail(NMFB200_ERR_CUDA, "cannot select the requested device");
-  nmfb200_ctx* c = new (std::nothrow) nmfb200_ctx();
-  if (!c) return fail(NMFB200_ERR_INVALID, "out of host memory");
-  c->kind = CtxKind::NmfBatch; c->device = device; c->N = N; c->C = C; c->R = R; c->nprob = B;
-  c->precision = NMFB200_PREC_F32;
-  c->nslab[0] = chunks_for(C, N, R);        // unused by the ragged launches: each problem's own counts are in its plan
-  c->nslab[1] = chunks_for(N, C, R);
-  c->part_floats = part;
-  c->cs_scratch_floats = std::max(cs, colsum_scratch_floats(C, (int)R, 1) * B);
-  c->loss_max_blocks = (int)loss;
-  for (int k = 0; k < 4; ++k) c->rag_gx[k] = gx[k];
-  if (int rc = alloc_workspace(c, 0)) return rc;
-  cudaError_t e = cudaMalloc(&c->rag, (size_t)B * sizeof(RaggedProblem));
-  if (e == cudaSuccess) e = cudaMemcpy(c->rag, t.data(), (size_t)B * sizeof(RaggedProblem), cudaMemcpyHostToDevice);
-  if (e != cudaSuccess) {
-    free_ctx(c);
-    return fail(NMFB200_ERR_CUDA, std::string("ragged batch plans: ") + cudaGetErrorString(e));
-  }
-  *out = c;
-  return 0;
+  CtxPlan plan;
+  if (int rc = plan_nmf_ragged(B, N, C, R, lengths, &plan)) return rc;
+  return create_ctx(out, device, CtxKind::NmfBatch, plan);
 }
 
 int nmfb200_nmf_batched_set_target(nmfb200_ctx* ctx, const void* V, int64_t ldv, int64_t batch_stride, int dtype,
@@ -559,11 +640,18 @@ int nmfb200_nmf_batched_set_target(nmfb200_ctx* ctx, const void* V, int64_t ldv,
                        CellSel{}, batch_stride || ctx->rag ? ctx->nprob : 1, batch_stride, ctx->rag);
 }
 
-int nmfb200_nmf_batched_set_active(nmfb200_ctx* ctx, const uint8_t* active, void* stream) {
-  CTX_GUARD(ctx, kinds(CtxKind::NmfBatch));
-  (void)stream;
+namespace {
+// nmfb200_nmf_batched_set_active / nmfb200_nmfd_batched_set_active on a batch of `kind`
+int set_active(nmfb200_ctx* ctx, CtxKind kind, const uint8_t* active) {
+  CTX_GUARD(ctx, kinds(kind));
   ctx->active = active;
   return 0;
+}
+}  // namespace
+
+int nmfb200_nmf_batched_set_active(nmfb200_ctx* ctx, const uint8_t* active, void* stream) {
+  (void)stream;
+  return set_active(ctx, CtxKind::NmfBatch, active);
 }
 
 /* ---- sparse targets (beta 1 and 2): nmf.py:603-638 without the dense product ------------------------------ */
@@ -630,8 +718,7 @@ static int nmfd_shape_of(int64_t B, int64_t C, int ndim, const int64_t* vdims, i
 
 int nmfb200_nmfnd_create(nmfb200_ctx** out, int device, int64_t B, int64_t C, int ndim, const int64_t* vdims,
                          int64_t R, const int64_t* kdims, int precision) {
-  if (!out) return fail(NMFB200_ERR_INVALID, "out is null");
-  *out = nullptr;
+  if (int rc = check_out(out)) return rc;
   NmfdShape shape;
   if (int rc = nmfd_shape_of(B, C, ndim, vdims, R, kdims, &shape)) return rc;
   if (precision != NMFB200_PREC_AUTO && precision != NMFB200_PREC_F32 && precision != NMFB200_PREC_F16)
@@ -641,35 +728,17 @@ int nmfb200_nmfnd_create(nmfb200_ctx** out, int device, int64_t B, int64_t C, in
   TcNmfdPlan tc_plan;
   const char* tc_limit = (one_d || precision == NMFB200_PREC_F16) ? tc_nmfd_plan(shape, &tc_plan) : "";
   if (precision == NMFB200_PREC_F16 && tc_limit) return fail(NMFB200_ERR_INVALID, tc_limit);
-  DeviceGuard guard(device);
-  if (!guard.ok) return fail(NMFB200_ERR_CUDA, "cannot select the requested device");
-  nmfb200_ctx* c = new (std::nothrow) nmfb200_ctx();
-  if (!c) return fail(NMFB200_ERR_INVALID, "out of host memory");
-  c->kind = CtxKind::Nmfd; c->device = device; c->precision = precision == NMFB200_PREC_F32 ? NMFB200_PREC_F32 : NMFB200_PREC_F16;
-  c->R = R; c->auto_mode = precision == NMFB200_PREC_AUTO;
-  c->d = shape;
-  c->nslab[0] = nmfd_wgrad_nsplit(c->d);
-  c->nslab[1] = nmfd_dgrad_nsplit(c->d);
-  int64_t pf = (int64_t)c->nslab[0] * C * R * c->d.w_inner();
-  int64_t hf = (int64_t)c->nslab[1] * B * R * c->d.h_inner();
-  if (hf > pf) pf = hf;
-  c->part_floats = pf;
-  int64_t cs1 = colsum_scratch_floats(C, (int)R, c->d.w_inner()), cs2 = colsum_scratch_floats(B, (int)R, c->d.h_inner());
-  c->cs_scratch_floats = cs1 > cs2 ? cs1 : cs2;
-  c->loss_max_blocks = (int)nmfd_max_blocks(c->d);         // bounded by nmfd_shape_of
-  if (int rc = alloc_workspace(c, B * C * c->d.v_inner())) return rc;
-  if (c->precision != NMFB200_PREC_F32 && !tc_limit) {    // NMFD at auto / f16, NMF2D / NMF3D at f16
+  auto finish = [&](nmfb200_ctx* c) {
+    c->precision = precision == NMFB200_PREC_F32 ? NMFB200_PREC_F32 : NMFB200_PREC_F16;
+    c->auto_mode = precision == NMFB200_PREC_AUTO;
+    if (c->precision == NMFB200_PREC_F32 || tc_limit) return 0;    // NMFD at auto / f16, NMF2D / NMF3D at f16
     cudaDeviceProp prop;
-    if (cudaGetDeviceProperties(&prop, device) == cudaSuccess && prop.major == 9) {
-      int rc = tc_nmfd_create(&c->tcd, c->d);          // beta = 1 runs as wgmma sliding GEMMs (tc_nmfd.cu)
-      if (rc) { free_ctx(c); return rc; }
-    } else if (precision == NMFB200_PREC_F16) {
-      free_ctx(c);
-      return fail(NMFB200_ERR_INVALID, "the tensor-core NMFD path needs an sm_90 device");
-    }
-  }
-  *out = c;
-  return 0;
+    if (cudaGetDeviceProperties(&prop, device) == cudaSuccess && prop.major == 9)
+      return tc_nmfd_create(&c->tcd, c->d);            // beta = 1 runs as wgmma sliding GEMMs (tc_nmfd.cu)
+    if (precision == NMFB200_PREC_F16) return fail(NMFB200_ERR_INVALID, "the tensor-core NMFD path needs an sm_90 device");
+    return 0;
+  };
+  return create_ctx(out, device, CtxKind::Nmfd, plan_nmfd(shape, 1), nullptr, finish);  // loss partials: nmfd_shape_of
 }
 
 int nmfb200_nmfd_set_target(nmfb200_ctx* ctx, const void* V, int dtype, void* stream) {
@@ -719,91 +788,23 @@ int batched_nmfd_shape_of(int64_t P, int64_t B, int64_t C, int ndim, const int64
 
 int nmfb200_nmfnd_batched_create(nmfb200_ctx** out, int device, int64_t P, int64_t B, int64_t C, int ndim,
                                  const int64_t* vdims, int64_t R, const int64_t* kdims) {
-  if (!out) return fail(NMFB200_ERR_INVALID, "out is null");
-  *out = nullptr;
+  if (int rc = check_out(out)) return rc;
   NmfdShape d;
   if (int rc = batched_nmfd_shape_of(P, B, C, ndim, vdims, R, kdims, &d)) return rc;
-  const int64_t vol = B * C * d.v_inner();
-  const int64_t cs_w = colsum_scratch_floats(C, (int)R, d.w_inner()), cs_h = colsum_scratch_floats(B, (int)R, d.h_inner());
-  DeviceGuard guard(device);
-  if (!guard.ok) return fail(NMFB200_ERR_CUDA, "cannot select the requested device");
-  nmfb200_ctx* c = new (std::nothrow) nmfb200_ctx();
-  if (!c) return fail(NMFB200_ERR_INVALID, "out of host memory");
-  c->kind = CtxKind::NmfdBatch; c->device = device; c->precision = NMFB200_PREC_F32; c->R = R; c->d = d; c->nprob = P;
-  // each problem's plan is the single problem's: same wgrad / dgrad splits, tiles, loss blocks and column-sum blocks
-  c->nslab[0] = nmfd_wgrad_nsplit(d);
-  c->nslab[1] = nmfd_dgrad_nsplit(d);
-  int64_t pf = (int64_t)c->nslab[0] * C * R * d.w_inner();
-  const int64_t hf = (int64_t)c->nslab[1] * B * R * d.h_inner();
-  if (hf > pf) pf = hf;
-  c->part_floats = pf * P;
-  c->cs_scratch_floats = (cs_w > cs_h ? cs_w : cs_h) * P;
-  c->loss_max_blocks = (int)(nmfd_max_blocks(d) * P);
-  if (int rc = alloc_workspace(c, vol * P)) return rc;
-  *out = c;
-  return 0;
+  return create_ctx(out, device, CtxKind::NmfdBatch, plan_nmfd(d, P));
 }
 
 int nmfb200_nmfnd_batched_create_ragged(nmfb200_ctx** out, int device, int64_t P, int64_t B, int64_t C, int ndim,
                                         const int64_t* vdims, int64_t R, const int64_t* kdims, const int64_t* lengths) {
-  if (!out) return fail(NMFB200_ERR_INVALID, "out is null");
-  *out = nullptr;
+  if (int rc = check_out(out)) return rc;
   NmfdShape d;
   if (int rc = batched_nmfd_shape_of(P, B, C, ndim, vdims, R, kdims, &d)) return rc;
   if (!lengths) return fail(NMFB200_ERR_INVALID, "lengths is null");
   if ((double)B * R * P > (double)kMaxGridX)
     return fail(NMFB200_ERR_INVALID, "ragged NMFD batch: P x B x R must be below 2^31 (grid x of the column sums of H)");
-  // each problem's single-problem plan along its own length, its workspace after the previous problems'.  Every count is
-  // at most the padded shape's, which the checks above bound for P problems.
-  std::vector<RaggedProblem> t(P);
-  const int64_t wpart = (int64_t)nmfd_wgrad_nsplit(d) * C * R * d.w_inner();
-  int64_t pn = 0, part = 0, loss = 0, cs = 0;
-  int dgrad_nsplit = 1;
-  for (int64_t p = 0; p < P; ++p) {
-    const int64_t L = lengths[p];
-    if (L < d.T || L > d.L)
-      return fail(NMFB200_ERR_INVALID, "lengths[" + std::to_string(p) + "] = " + std::to_string(L) + " is outside [" +
-                                           std::to_string(d.T) + ", " + std::to_string(d.L) + "] (the last kernel and target sizes)");
-    NmfdShape e = d;
-    e.L = (int)L; e.Lin = (int)(L - d.T + 1);
-    NmfdPlan plan;
-    nmfd_plan(e, &plan);
-    RaggedProblem& q = t[p];
-    q.rows = L; q.lin = e.Lin;
-    q.gx[0] = (int)plan.recon_grid.x; q.gx[1] = (int)plan.dgrad_grid.x;
-    q.nch[0] = plan.wgrad_nsplit; q.nch[1] = plan.dgrad_nsplit;
-    q.loss_n = nmfd_max_blocks(e);
-    // the column sums of H at beta 1 as its single fit forms them: one partial per (clip, component) run, or the rows
-    // blocking of a run of one element
-    q.cs_blocks = (int)(e.h_inner() > 1 ? B : colsum_scratch_floats(B, 1, 1));
-    q.pn = pn; q.part = part; q.loss_part = loss; q.cs_part = cs;
-    dgrad_nsplit = std::max(dgrad_nsplit, plan.dgrad_nsplit);
-    // every problem's tiles and slabs start 16-byte aligned: the ratio stage of W reads its slabs as float4 (update.cu:
-    // apply_update_vec4_kernel) wherever the shape allows, and a dgrad slab may hold any number of floats
-    pn += round_up(B * C * e.v_inner(), 4);
-    part += round_up(std::max(wpart, (int64_t)plan.dgrad_nsplit * B * R * e.h_inner()), 4);
-    loss += q.loss_n;
-    cs += B * R;
-  }
-  DeviceGuard guard(device);
-  if (!guard.ok) return fail(NMFB200_ERR_CUDA, "cannot select the requested device");
-  nmfb200_ctx* c = new (std::nothrow) nmfb200_ctx();
-  if (!c) return fail(NMFB200_ERR_INVALID, "out of host memory");
-  c->kind = CtxKind::NmfdBatch; c->device = device; c->precision = NMFB200_PREC_F32; c->R = R; c->d = d; c->nprob = P;
-  c->nslab[0] = nmfd_wgrad_nsplit(d);
-  c->nslab[1] = dgrad_nsplit;            // the dgrad launch's grid y; each problem runs its own splits
-  c->part_floats = part;
-  c->cs_scratch_floats = std::max(cs, colsum_scratch_floats(C, (int)R, d.w_inner()) * P);
-  c->loss_max_blocks = (int)loss;
-  if (int rc = alloc_workspace(c, pn)) return rc;
-  cudaError_t e = cudaMalloc(&c->rag, (size_t)P * sizeof(RaggedProblem));
-  if (e == cudaSuccess) e = cudaMemcpy(c->rag, t.data(), (size_t)P * sizeof(RaggedProblem), cudaMemcpyHostToDevice);
-  if (e != cudaSuccess) {
-    free_ctx(c);
-    return fail(NMFB200_ERR_CUDA, std::string("ragged batch plans: ") + cudaGetErrorString(e));
-  }
-  *out = c;
-  return 0;
+  CtxPlan plan;
+  if (int rc = plan_nmfd_ragged(d, P, lengths, &plan)) return rc;
+  return create_ctx(out, device, CtxKind::NmfdBatch, plan);
 }
 
 int nmfb200_nmfd_batched_set_target(nmfb200_ctx* ctx, const void* V, int64_t problem_stride, int dtype, void* stream) {
@@ -821,10 +822,8 @@ int nmfb200_nmfd_batched_set_target(nmfb200_ctx* ctx, const void* V, int64_t pro
 }
 
 int nmfb200_nmfd_batched_set_active(nmfb200_ctx* ctx, const uint8_t* active, void* stream) {
-  CTX_GUARD(ctx, kinds(CtxKind::NmfdBatch));
   (void)stream;
-  ctx->active = active;
-  return 0;
+  return set_active(ctx, CtxKind::NmfdBatch, active);
 }
 
 int nmfb200_nmfd_plan(int64_t B, int64_t C, int ndim, const int64_t* vdims, int64_t R, const int64_t* kdims, int64_t* out,
@@ -939,7 +938,7 @@ int sparse_terms(nmfb200_ctx* ctx, int which, const float* F, const float* other
     return raw_sum(chunks, den, nullptr, st);
   }
   if (beta == 1.0)                                             // colsum of the OTHER factor, nmf.py:122-131
-    return factor_colsum(other, f.other_rows, R, 1, ctx->cs_scratch, ctx->cs_scratch_floats, den, st);
+    return factor_colsum(other, f.other_rows, R, 1, ctx->cs_scratch, ctx->cs_scratch.n, den, st);
   float* G = ctx->sp_gram + (1 - which) * R * R;               // Gram matrix of the other factor
   rc = sparse_gram(other, f.other_rows, R, ctx->sp_gram + 2 * R * R, G, st);
   if (rc) return rc;
@@ -948,17 +947,13 @@ int sparse_terms(nmfb200_ctx* ctx, int which, const float* F, const float* other
 
 // CUDA-core contraction of one NMF factor update (which = 0: W, 1: H) into c->num / c->den (chunked partials).
 int simt_contract(nmfb200_ctx* c, int which, const float* W, const float* H, double beta, cudaStream_t st) {
-  if (beta != 1.0 || c->sel) { int e = ensure_den(c); if (e) return e; }
+  if (beta != 1.0 || c->sel) NMF_CUDA_CHECK(c->den.ensure(c->num.n));
   // W update: F = W (C rows), G = H (N rows), Vm = V^T;  H update: F = H (N rows), G = W (C rows), Vm = V
   const float* fac[2] = {W, H};
   const FactorDims f = factor_dims(c, which);
-  // a batch: problem b's target, factors and partials (slab layout [chunk][problem][rows][R]); one problem otherwise
-  Batch bt;
-  if (is_batch(c)) bt = Batch{c->nprob, c->bstride, f.rows * c->R, f.other_rows * c->R, f.rows * c->R, c->active};
-  if (c->rag) { bt.rag = c->rag; bt.rag_launch = which == 0 ? kRagW : kRagH; bt.rag_gx = c->rag_gx[bt.rag_launch]; }
   return simt_nmf_contract(c->V, c->vdtype, c->ldv, /*trans=*/which == 0, fac[which], fac[1 - which], f.rows, f.other_rows,
                            (int)c->R, beta, c->nslab[which], c->num, c->den, c->R, f.rows * c->R * c->nprob, c->sel, c->C,
-                           st, bt);
+                           st, launch_batch(c, which == 0 ? kRagW : kRagH));
 }
 
 // The same for NMFD / NMF2D / NMF3D: the ratio tiles Pn (and Pp), then their backward passes (wgrad for W, dgrad for H) into
@@ -966,14 +961,12 @@ int simt_contract(nmfb200_ctx* c, int which, const float* W, const float* H, dou
 int nmfd_contract(nmfb200_ctx* c, int which, const float* W, const float* H, double beta, cudaStream_t st) {
   const bool den = !kl_colsum(c, beta);
   if (den) {
-    if (!c->Pp) NMF_CUDA_CHECK(cudaMalloc(&c->Pp, (size_t)c->pn_floats * sizeof(float)));
-    int e = ensure_den(c);
-    if (e) return e;
+    NMF_CUDA_CHECK(c->Pp.ensure(c->Pn.n));
+    NMF_CUDA_CHECK(c->den.ensure(c->num.n));
   }
   // a batch: every problem's tiles and split partials in the same launches (slab layout [split][problem][rows][R][inner]; a
   // ragged batch: each problem's own [split][rows][R][inner] at its offset)
-  Batch bt{c->nprob, c->bstride, 0, 0, 0, c->active};
-  bt.rag = c->rag;
+  const Batch bt = launch_batch(c, which == 0 ? kRagW : kRagH);
   int rc = nmfd_recon_phi(c->d, c->V, c->vdtype, W, H, beta, c->Pn, c->Pp, nullptr, 0, nullptr, st, c->sel, bt);
   auto grad = [&](const float* P, float* out) {
     return which == 0 ? nmfd_wgrad(c->d, P, H, out, c->nslab[0], st, bt) : nmfd_dgrad(c->d, P, W, out, c->nslab[1], st, bt);
@@ -996,7 +989,7 @@ int factor_terms(nmfb200_ctx* c, int which, const float* W, const float* H, doub
   const bool kl = kl_colsum(c, beta);
   // where the final-form terms go without `out`: c->colsum is [colsum(W) | colsum(H)], the sparse raw denominator lives in
   // c->den at beta 2 and on observed cells, and in c->sp_den at other beta (whose c->den holds the chunks)
-  if (is_sparse(c) && beta == 2.0 && !out) { int e = ensure_den(c); if (e) return e; }
+  if (is_sparse(c) && beta == 2.0 && !out) NMF_CUDA_CHECK(c->den.ensure(c->num.n));
   float* num_out = out ? out : c->num;
   float* den_out = out ? out + a.numel : kl ? c->colsum + (1 - which) * c->R * c->nprob
                  : (beta == 2.0 || c->form == TargetForm::Observed) ? c->den : c->sp_den;
@@ -1024,8 +1017,8 @@ int factor_terms(nmfb200_ctx* c, int which, const float* W, const float* H, doub
   a.kl_den = den_out;
   const FactorDims f = factor_dims(c, which);
   const bool rag_h = c->rag && which == 0;        // a ragged batch's H: each problem's own rows (NMFD: line positions)
-  return factor_colsum(fac[1 - which], f.other_rows, (int)c->R, f.other_inner, c->cs_scratch, c->cs_scratch_floats, den_out,
-                       st, c->nprob, c->active, rag_h ? c->rag : nullptr, rag_h ? c->rag_gx[kRagColsum] : 0,
+  return factor_colsum(fac[1 - which], f.other_rows, (int)c->R, f.other_inner, c->cs_scratch, c->cs_scratch.n, den_out,
+                       st, c->nprob, c->active, rag_h ? c->rag.p : nullptr, rag_h ? c->rag_gx[kRagColsum] : 0,
                        rag_h && is_nmfd(c) ? c->d.Lin : 0);
 }
 
@@ -1053,7 +1046,7 @@ int sparse_loss_ctx(nmfb200_ctx* ctx, const float* W, const float* H, double bet
                          ctx->sp.wt);
   if (beta != 1.0 && beta != 2.0) {     // pos = sum x^beta over every cell without V, then V_norm - neg at the non-zeros
     int npos = 0;
-    int rc = simt_nmf_pow_sum(H, W, ctx->N, ctx->C, R, beta, ctx->loss_blocks, ctx->loss_max_blocks, &npos, st);
+    int rc = simt_nmf_pow_sum(H, W, ctx->N, ctx->C, R, beta, ctx->loss_blocks, (int)ctx->loss_blocks.n, &npos, st);
     if (rc) return rc;
     return sparse_beta_loss(ctx->sp.crow, ctx->sp.col, ctx->sp.val, H, W, R, ctx->N, beta, ctx->loss_blocks, npos,
                             ctx->sp_loss_part, loss_dev, st);
@@ -1061,8 +1054,8 @@ int sparse_loss_ctx(nmfb200_ctx* ctx, const float* W, const float* H, double bet
   const float *pa, *pb;
   int rc;
   if (beta == 1.0) {
-    rc = factor_colsum(W, ctx->C, R, 1, ctx->cs_scratch, ctx->cs_scratch_floats, ctx->colsum, st);
-    if (rc == 0) rc = factor_colsum(H, ctx->N, R, 1, ctx->cs_scratch, ctx->cs_scratch_floats, ctx->colsum + R, st);
+    rc = factor_colsum(W, ctx->C, R, 1, ctx->cs_scratch, ctx->cs_scratch.n, ctx->colsum, st);
+    if (rc == 0) rc = factor_colsum(H, ctx->N, R, 1, ctx->cs_scratch, ctx->cs_scratch.n, ctx->colsum + R, st);
     pa = ctx->colsum; pb = ctx->colsum + R;
   } else {
     rc = sparse_gram(W, ctx->C, R, ctx->sp_gram + 2 * R * R, ctx->sp_gram, st);
@@ -1198,20 +1191,16 @@ int nmfb200_loss(nmfb200_ctx* ctx, const float* W, const float* H, double beta, 
   TARGET_GUARD(ctx);
   if (!W || !H || !loss_dev) return fail(NMFB200_ERR_INVALID, "null pointer");
   cudaStream_t st = (cudaStream_t)stream;
-  if (is_nmfd(ctx)) {       // a batch: loss_dev[b] for every active problem b
+  // a batch: loss_dev[b] for every active problem b
+  if (is_nmfd(ctx)) {
     if (use_tc(ctx, beta)) return tc_nmfd_recon(ctx->tcd, ctx->V, ctx->vdtype, W, H, true, loss_dev, st);
-    Batch bt{ctx->nprob, ctx->bstride, 0, 0, 0, ctx->active};
-    bt.rag = ctx->rag;
-    return nmfd_recon_phi(ctx->d, ctx->V, ctx->vdtype, W, H, beta, nullptr, nullptr, ctx->loss_blocks, ctx->loss_max_blocks,
-                          loss_dev, st, ctx->sel, bt);
+    return nmfd_recon_phi(ctx->d, ctx->V, ctx->vdtype, W, H, beta, nullptr, nullptr, ctx->loss_blocks, (int)ctx->loss_blocks.n,
+                          loss_dev, st, ctx->sel, launch_batch(ctx, kRagLoss));
   }
   if (is_sparse(ctx)) return sparse_loss_ctx(ctx, W, H, beta, loss_dev, st);
   if (use_tc(ctx, beta)) return tc_loss(ctx->tc, W, H, beta, loss_dev, st);
-  Batch bt;         // a batch: loss_dev[b] for every active problem b
-  if (is_batch(ctx)) bt = Batch{ctx->nprob, ctx->bstride, ctx->N * ctx->R, ctx->C * ctx->R, 0, ctx->active};
-  if (ctx->rag) { bt.rag = ctx->rag; bt.rag_launch = kRagLoss; bt.rag_gx = ctx->rag_gx[kRagLoss]; }
   return simt_nmf_loss(ctx->V, ctx->vdtype, ctx->ldv, H, W, ctx->N, ctx->C, (int)ctx->R, beta, ctx->loss_blocks,
-                       ctx->loss_max_blocks, loss_dev, ctx->sel, ctx->C, st, bt);
+                       (int)ctx->loss_blocks.n, loss_dev, ctx->sel, ctx->C, st, launch_batch(ctx, kRagLoss));
 }
 
 int64_t nmfb200_raw_terms_numel(const nmfb200_ctx* ctx, int which, double beta) {
@@ -1275,13 +1264,13 @@ int nmfb200_plca_masked_terms(nmfb200_ctx* ctx, const float* W, const float* Hz,
   if (is_nmfd(ctx) && ctx->R > 256) return fail(NMFB200_ERR_INVALID, "plca_masked_terms: NMFD rank must be <= 256");
   if (!W || !Hz || !out || (which != 0 && which != 1)) return fail(NMFB200_ERR_INVALID, "bad argument");
   cudaStream_t st = (cudaStream_t)stream;
-  if (int e = ensure_den(ctx)) return e;
+  NMF_CUDA_CHECK(ctx->den.ensure(ctx->num.n));
   const float* V = static_cast<const float*>(ctx->V);
   const uint8_t* M = static_cast<const uint8_t*>(ctx->sel.p);
   int rc;
   if (is_nmfd(ctx)) {        // the fill-mode ratio tiles (and q_O), then their backward passes
-    if (!ctx->Pp) NMF_CUDA_CHECK(cudaMalloc(&ctx->Pp, (size_t)ctx->d.B * ctx->d.C * ctx->d.v_inner() * sizeof(float)));
-    rc = nmfd_plca_fill(ctx->d, V, W, Hz, ctx->Pn, ctx->Pp, M, ctx->loss_blocks, ctx->loss_max_blocks, qobs_dev, st);
+    NMF_CUDA_CHECK(ctx->Pp.ensure(ctx->Pn.n));
+    rc = nmfd_plca_fill(ctx->d, V, W, Hz, ctx->Pn, ctx->Pp, M, ctx->loss_blocks, (int)ctx->loss_blocks.n, qobs_dev, st);
     auto grad = [&](const float* P, float* part) {
       return which == 0 ? nmfd_wgrad(ctx->d, P, Hz, part, ctx->nslab[0], st)
                         : nmfd_dgrad(ctx->d, P, W, part, ctx->nslab[1], st);
@@ -1292,16 +1281,11 @@ int nmfb200_plca_masked_terms(nmfb200_ctx* ctx, const float* W, const float* Hz,
     const FactorDims f = factor_dims(ctx, which);
     const int nch = ctx->nslab[which];
     const int64_t nblocks = simt_plca_fill_blocks(f.rows, nch);
-    if (qobs_dev && ctx->qobs_part_n < nblocks) {
-      cudaFree(ctx->qobs_part);
-      ctx->qobs_part = nullptr; ctx->qobs_part_n = 0;
-      NMF_CUDA_CHECK(cudaMalloc(&ctx->qobs_part, (size_t)nblocks * sizeof(double)));
-      ctx->qobs_part_n = nblocks;
-    }
+    if (qobs_dev) NMF_CUDA_CHECK(ctx->qobs_part.ensure(nblocks));
     const float* fac[2] = {W, Hz};
     rc = simt_plca_fill_contract(V, ctx->ldv, /*trans=*/which == 0, fac[which], fac[1 - which], f.rows, f.other_rows,
                                  (int)ctx->R, nch, ctx->num, ctx->den, ctx->R, f.rows * ctx->R, M, ctx->C,
-                                 qobs_dev ? ctx->qobs_part : nullptr, st);
+                                 qobs_dev ? ctx->qobs_part.p : nullptr, st);
     if (rc == 0 && qobs_dev) rc = sum_partials(ctx->qobs_part, (int)nblocks, qobs_dev, st);
   }
   if (rc) return rc;
@@ -1353,15 +1337,15 @@ int cd_update_factor(nmfb200_ctx* c, int which, float* W, float* H, double l1_re
   const FactorDims f = factor_dims(c, which);
   float* X = which == 0 ? W : H;
   const float* other = which == 0 ? H : W;
-  Batch bt;               // X / A partials (f, p), the other factor (g) and its Gram (p of the Gram) of problem b
-  if (is_batch(c)) bt = Batch{P, c->bstride, f.rows * R, f.other_rows * R, f.rows * R, c->active};
+  // X / A partials (f, p), the other factor (g) and its Gram (p of the Gram) of problem b
+  const Batch bt = launch_batch(c, which == 0 ? kRagW : kRagH);
   int nch = 1;
   int rc;
   if (is_sparse(c)) {         // the compressed form whose segments are X's rows (sparse_terms' choice)
     rc = sparse_numerator(which == 0 ? c->sp.ccol : c->sp.crow, which == 0 ? c->sp.row : c->sp.col,
                           which == 0 ? c->sp.val_t : c->sp.val, X, other, R, f.rows, 2.0, c->num, st);
   } else {
-    if ((rc = ensure_gram(c))) return rc;
+    NMF_CUDA_CHECK(c->sp_gram.ensure(gram_floats(c)));
     nch = c->nslab[which];
     rc = simt_nmf_contract_num(c->V, c->vdtype, c->ldv, /*trans=*/which == 0, other, f.rows, f.other_rows, R, nch, c->num,
                                f.rows * R * P, st, bt);
@@ -1480,47 +1464,35 @@ int nmfb200_plca_loss(nmfb200_ctx* ctx, const float* W, const float* Hz, const f
   TARGET_GUARD(ctx);
   if (!W || !Hz || !norm_dev || !loss_dev) return fail(NMFB200_ERR_INVALID, "null pointer");
   cudaStream_t st = (cudaStream_t)stream;
-  if (is_nmfd(ctx)) {
-    Batch bt{ctx->nprob, ctx->bstride, 0, 0, 0, ctx->active};
-    bt.scale = norm_dev;
-    return nmfd_recon_phi(ctx->d, ctx->V, ctx->vdtype, W, Hz, 1.0, nullptr, nullptr, ctx->loss_blocks, ctx->loss_max_blocks,
-                          loss_dev, st, CellSel{}, bt);
-  }
-  Batch bt{ctx->nprob, ctx->bstride, ctx->N * ctx->R, ctx->C * ctx->R, 0, ctx->active};
-  bt.scale = norm_dev;
   // a ragged batch: problem b's rows, loss chunks and run of partials (loss_part, loss_n) from its plan, as nmfb200_loss
-  if (ctx->rag) { bt.rag = ctx->rag; bt.rag_launch = kRagLoss; bt.rag_gx = ctx->rag_gx[kRagLoss]; }
+  Batch bt = launch_batch(ctx, kRagLoss);
+  bt.scale = norm_dev;
+  if (is_nmfd(ctx))
+    return nmfd_recon_phi(ctx->d, ctx->V, ctx->vdtype, W, Hz, 1.0, nullptr, nullptr, ctx->loss_blocks, (int)ctx->loss_blocks.n,
+                          loss_dev, st, CellSel{}, bt);
   return simt_nmf_loss(ctx->V, ctx->vdtype, ctx->ldv, Hz, W, ctx->N, ctx->C, (int)ctx->R, 1.0, ctx->loss_blocks,
-                       ctx->loss_max_blocks, loss_dev, CellSel{}, ctx->C, st, bt);
+                       (int)ctx->loss_blocks.n, loss_dev, CellSel{}, ctx->C, st, bt);
 }
 
 /* ---- sparse-target PLCA: one ratio pass per EM step at the stored entries ------------------------------------------ */
 
 int nmfb200_plca_sparse_create(nmfb200_ctx** out, int device, int64_t N, int64_t C, int64_t R, int64_t nnz) {
-  if (!out) return fail(NMFB200_ERR_INVALID, "out is null");
-  *out = nullptr;
+  if (int rc = check_out(out)) return rc;
   if (N < 1 || C < 1 || R < 1 || nnz < 0) return fail(NMFB200_ERR_INVALID, "N, C, R must be positive and nnz >= 0");
   if (R > kMaxRank) return fail(NMFB200_ERR_INVALID, kMaxRankMsg);
   if (sparse_gather_blocks(N > C ? N : C) > kMaxGridX)
     return fail(NMFB200_ERR_INVALID, "sparse PLCA: ceil(max(N, C) / 8) gather blocks pass grid x (2^31 - 1)");
-  DeviceGuard guard(device);
-  if (!guard.ok) return fail(NMFB200_ERR_CUDA, "cannot select the requested device");
-  nmfb200_ctx* c = new (std::nothrow) nmfb200_ctx();
-  if (!c) return fail(NMFB200_ERR_INVALID, "out of host memory");
-  c->kind = CtxKind::PlcaSparse; c->device = device; c->N = N; c->C = C; c->R = R;
-  c->spl_nnz = nnz;
-  const int64_t pb = nnz * (int64_t)sizeof(float), lb = sparse_plca_loss_parts(N) * (int64_t)sizeof(double);
-  const int64_t cb = (sparse_plca_colsum_parts(C, (int)R) + sparse_plca_colsum_parts(N, (int)R)) * (int64_t)sizeof(double);
-  cudaError_t e = cudaMalloc(&c->splw.P, (size_t)(pb > 0 ? pb : sizeof(float)));
-  if (e == cudaSuccess) e = cudaMalloc(&c->splw.loss_part, (size_t)lb);
-  if (e == cudaSuccess) e = cudaMalloc(&c->splw.cs_part, (size_t)cb);
-  if (e != cudaSuccess) {
-    free_ctx(c);
-    return fail(NMFB200_ERR_CUDA, std::string("cudaMalloc: ") + cudaGetErrorString(e));
-  }
-  c->spl_bytes = (pb > 0 ? pb : (int64_t)sizeof(float)) + lb + cb;
-  *out = c;
-  return 0;
+  // none of the dense models' workspace: the ratios at the stored entries (at least one float), the loss partials and the
+  // two column sums' partials
+  auto finish = [&](nmfb200_ctx* c) {
+    c->spl_nnz = nnz;
+    cudaError_t e = c->spl_P.ensure(std::max(nnz, (int64_t)1));
+    if (e == cudaSuccess) e = c->spl_loss_part.ensure(sparse_plca_loss_parts(N));
+    if (e == cudaSuccess) e = c->spl_cs_part.ensure(sparse_plca_colsum_parts(C, (int)R) + sparse_plca_colsum_parts(N, (int)R));
+    if (e != cudaSuccess) return fail(NMFB200_ERR_CUDA, std::string("cudaMalloc: ") + cudaGetErrorString(e));
+    return 0;
+  };
+  return create_ctx(out, device, CtxKind::PlcaSparse, CtxPlan{N, C, R}, nullptr, finish);
 }
 
 int nmfb200_plca_sparse_set_target(nmfb200_ctx* ctx, const int64_t* crow, const int64_t* col, const float* val,
@@ -1544,12 +1516,13 @@ int nmfb200_plca_sparse_terms(nmfb200_ctx* ctx, const float* W, const float* Hz,
   float* dHz = out ? out + ctx->C * ctx->R : nullptr;
   const SparseTarget& s = ctx->sp;
   const SparsePlcaTarget t{s.crow, s.col, s.ccol, s.row, s.perm, s.val, ctx->N, ctx->C, (int)ctx->R};
-  return sparse_plca_terms(t, ctx->splw, W, Hz, dW, dHz, norm, loss_dev, (cudaStream_t)stream);
+  const SparsePlcaWork ws{ctx->spl_P, ctx->spl_loss_part, ctx->spl_cs_part};
+  return sparse_plca_terms(t, ws, W, Hz, dW, dHz, norm, loss_dev, (cudaStream_t)stream);
 }
 
 int64_t nmfb200_plca_sparse_device_bytes(const nmfb200_ctx* ctx) {
   if (!ctx || ctx->kind != CtxKind::PlcaSparse) return -1;
-  return ctx->spl_bytes;
+  return ctx->spl_P.n * (int64_t)sizeof(float) + (ctx->spl_loss_part.n + ctx->spl_cs_part.n) * (int64_t)sizeof(double);
 }
 
 int nmfb200_hoyer_project(int device, float* x, int64_t outer, int64_t D, int64_t inner, const float* k1, const float* k2,
