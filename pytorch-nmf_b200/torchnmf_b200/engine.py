@@ -8,7 +8,8 @@ needs from its loop body:
     loss(beta) -> float            metrics.beta_div of the current reconstruction, nmf.py:360-361,:400-401
 
 `ShardedEngine` wraps any engine that also offers ``w_partial`` / ``w_apply`` / ``loss_tensor`` and
-inserts the one collective per iteration that the row-sharded layout needs.
+inserts the one collective per iteration that the row-sharded layout needs.  Its base, `Collectives`, holds the
+collectives themselves; the sharded PLCA fits (plca.py) call them around unwrapped engines.
 """
 import ctypes
 import os
@@ -764,7 +765,48 @@ class CudaNmfdEngine(_CudaEngine):
         _capi.check(self._lib.nmfb200_nmfd_set_target(self._ctx, _ptr(V), _capi.DTYPES[V.dtype], _stream(self.device)))
 
 
-class ShardedEngine:
+class Collectives:
+    """The collectives of a sharded fit's host code over a process group (None: the default group), on small tensors on
+    `device` (a CUDA device for NCCL): a sum in place, agreement on a flag and agreement on sizes.  Every rank calls them
+    in the same order."""
+
+    def __init__(self, group, device):
+        import torch.distributed as dist
+        self._dist = dist
+        self.group = group
+        self.device = device
+        self.world = dist.get_world_size(group)
+
+    def _reduce_device(self):
+        return self.device
+
+    def all_reduce_(self, t):
+        """Collective: `t` summed over the ranks, in place (one SUM all-reduce); returns t."""
+        self._dist.all_reduce(t, op=self._dist.ReduceOp.SUM, group=self.group)
+        return t
+
+    def all_ranks(self, flag):
+        """Collective: whether `flag` holds on every rank (one MIN all-reduce)."""
+        t = torch.tensor([int(bool(flag))], dtype=torch.int32, device=self._reduce_device())
+        self._dist.all_reduce(t, op=self._dist.ReduceOp.MIN, group=self.group)
+        return bool(t.item())
+
+    def check_same_sizes(self, names, sizes):
+        """Collective: raise ValueError on every rank unless every rank passed the same `sizes` (ints; `names` label them
+        in the message), so the W all-reduce never sums buffers of different lengths.  One MIN and one MAX all-reduce."""
+        lo = torch.tensor(sizes, dtype=torch.int64, device=self._reduce_device())
+        hi = lo.clone()
+        self._dist.all_reduce(lo, op=self._dist.ReduceOp.MIN, group=self.group)
+        self._dist.all_reduce(hi, op=self._dist.ReduceOp.MAX, group=self.group)
+        lo, hi = lo.tolist(), hi.tolist()
+        if lo != hi:
+            differ = ", ".join(f"{n} from {a} to {b}" for n, a, b in zip(names, lo, hi) if a != b)
+            mine = ", ".join(f"{n}={s}" for n, s in zip(names, sizes))
+            raise ValueError(f"sharded fit: every rank must have the same sizes past the batch axis, but across ranks {differ} "
+                             f"(this rank: {mine})")
+
+
+class ShardedEngine(Collectives):
     """Sharded fit over a process group: every rank holds a shard of V and H and a replica of W -- NMF shards the rows
     (V[n_g,:], H[n_g,:]), NMFD / NMF2D / NMF3D the batch axis (V[b_g], H[b_g]).
 
@@ -776,12 +818,10 @@ class ShardedEngine:
     """
 
     def __init__(self, local, group=None):
-        import torch.distributed as dist
-        self._dist = dist
+        dev = getattr(local, "device", None)
+        super().__init__(group, dev if dev is not None else torch.device("cpu"))
         self.local = local
-        self.group = group
         self.kind = local.kind
-        self.world = dist.get_world_size(group)
         self._peer = {}                      # beta -> does the W update run over peer memory
         self.w_update_path = "nccl"
 
@@ -814,30 +854,6 @@ class ShardedEngine:
         self._dist.all_reduce(t, op=self._dist.ReduceOp.MAX, group=self.group)
         t = t.cpu()
         return -float(t[0]), float(t[1])
-
-    def _reduce_device(self):
-        dev = getattr(self.local, "device", None)
-        return dev if dev is not None else torch.device("cpu")
-
-    def all_ranks(self, flag):
-        """Collective: whether `flag` holds on every rank (one MIN all-reduce)."""
-        t = torch.tensor([int(bool(flag))], dtype=torch.int32, device=self._reduce_device())
-        self._dist.all_reduce(t, op=self._dist.ReduceOp.MIN, group=self.group)
-        return bool(t.item())
-
-    def check_same_sizes(self, names, sizes):
-        """Collective: raise ValueError on every rank unless every rank passed the same `sizes` (ints; `names` label them
-        in the message), so the W all-reduce never sums buffers of different lengths.  One MIN and one MAX all-reduce."""
-        lo = torch.tensor(sizes, dtype=torch.int64, device=self._reduce_device())
-        hi = lo.clone()
-        self._dist.all_reduce(lo, op=self._dist.ReduceOp.MIN, group=self.group)
-        self._dist.all_reduce(hi, op=self._dist.ReduceOp.MAX, group=self.group)
-        lo, hi = lo.tolist(), hi.tolist()
-        if lo != hi:
-            differ = ", ".join(f"{n} from {a} to {b}" for n, a, b in zip(names, lo, hi) if a != b)
-            mine = ", ".join(f"{n}={s}" for n, s in zip(names, sizes))
-            raise ValueError(f"sharded fit: every rank must have the same sizes past the batch axis, but across ranks {differ} "
-                             f"(this rank: {mine})")
 
     def _peer_ready(self, beta):
         """Collective, once per (engine, beta): may the W update run over peer memory?  Every rank must answer the same, so

@@ -116,7 +116,7 @@ class BaseComponent(torch.nn.Module):
 
     @torch.no_grad()
     def fit(self, V, tol=1e-4, max_iter=200, verbose=False, W_alpha=1., H_alpha=1., Z_alpha=1., *, precision="f32",
-            mask=None):
+            mask=None, group=None):
         """EM fit of the PLCA model (reference: plca.py:193-304; same arguments, stop rule and return value
         `(n_iter, norm)`).  Runs on the parameters' CUDA device; host-resident modules are staged like `NMF.fit`.
 
@@ -147,26 +147,57 @@ class BaseComponent(torch.nn.Module):
         O(nnz + (N + C) R).  fp32 kernels only (`last_fit_precision` "f32"); the summation order differs from the dense
         fit's, so the two agree to fp32 rounding, not bit for bit.  AssertionError for a negative stored value; ValueError
         for a target storing nothing or summing to 0, a sparse layout other than COO, precision "f16" / "f16_split" or an
-        unknown precision, and a mask.  SIPLCA, SIPLCA2 and SIPLCA3 raise NotImplementedError for a sparse V."""
+        unknown precision, and a mask.  SIPLCA, SIPLCA2 and SIPLCA3 raise NotImplementedError for a sparse V.
+
+        group:     (keyword-only, default None) a torch.distributed process group: a sharded fit, for a corpus or a set of
+                   recordings that does not fit one GPU.  PLCA shards the rows: each rank passes its rows V[n_g, :] (dense or
+                   sparse COO) and its module holds H[n_g, :]; SIPLCA / SIPLCA2 / SIPLCA3 shard the batch axis: V[b_g] and
+                   H[b_g].  W and Z are replicated and must be identical on every rank at entry; an H_alpha tensor is this
+                   rank's shard.  Shards may be uneven, but every size past the shard axis -- C, R and for the
+                   shift-invariant models the kernel size and V's sizes past C -- must agree across ranks.  Each EM step
+                   runs this rank's contractions on its own shard (the same kernels as the unsharded fit, at the same
+                   precision) and sums W's and Z's gradients over the ranks in one all-reduce of C R prod(K) + R floats;
+                   the Z and W updates then compute the same bits on every rank, so the replicas stay identical.  H's
+                   update is local, apart from one R-float all-reduce of H's column sums where the update divides by
+                   them (W and Z both frozen, or H_alpha != 1).  The loss is every shard's divergence summed in float64
+                   by one scalar all-reduce every 10th iteration, so every rank takes the same stop decision.  Returns
+                   `(n_iter, norm)` on every rank, norm = the sum of every shard's V.sum(), in V's dtype, by which each
+                   rank normalises its shard.  A one-rank group gives the unsharded fit bit for bit.  V and H data never
+                   move between ranks.  The checks that can fail on one rank only -- a shard that does not match the
+                   module's H / W, a negative value (AssertionError), an empty shard (no row or clip; a sparse one storing no
+                   entry) -- and the sizes
+                   are agreed by every rank before any raises, so they raise on every rank together; so does a sparse
+                   target whose shards all sum to 0.  ValueError for `mask` with `group`.  Not covered: masked fits,
+                   the batched classes (which take no `group`), a peer-memory (NVLink) exchange, and (NMF) sharded
+                   sparse targets without densifying.
+        """
         if mask is not None:
+            if group is not None:
+                raise ValueError(f"group: {type(self).__name__}.fit does not run masked fits sharded (mask with group)")
             return self._fit_masked(V, mask, tol, max_iter, verbose, W_alpha, H_alpha, Z_alpha, precision)
         if V.layout != torch.strided:
-            return self._fit_sparse(V, tol, max_iter, verbose, W_alpha, H_alpha, Z_alpha, precision)
-        assert torch.all(V >= 0.), "Target should be non-negative."                         # plca.py:236
+            return self._fit_sparse(V, tol, max_iter, verbose, W_alpha, H_alpha, Z_alpha, precision, group)
+        if group is None:
+            assert torch.all(V >= 0.), "Target should be non-negative."                     # plca.py:236
         W, H, Z = self.W, self.H, self.Z
         assert W is not None and H is not None and Z is not None, "fit() needs W, H and Z"
         no_cuda = "torchnmf_b200.PLCA.fit needs a CUDA device (sm_90a); there is no CPU fallback"
         with _placed_factors(self, (W, H, Z), no_cuda) as (dev, (Wd, Hd, Zd)):
             f32 = torch.float32
             norm = V.sum()
+            ops = None
+            if group is not None:
+                ops = _engine.Collectives(group, dev)
+                norm = self._agree_on_shards(ops, V, self._shape_mismatch(V), bool(torch.all(V >= 0.)), V.numel() > 0, norm)
             Vn = (V.to(dev, f32).contiguous() / norm.to(dev, f32)).contiguous()              # plca.py:241-242
             normd = norm.to(dev, f32)
             Vfull = Vn * normd
 
             def divergence(follows):
-                return float(_kl(self.reconstruct(Hd, Wd, Zd) * normd, Vfull))            # plca.py:245-246,293-294
+                return _total(ops, _kl(self.reconstruct(Hd, Wd, Zd) * normd, Vfull))      # plca.py:245-246,293-294
 
             Hz = (Hd * _over(Zd, Hd)).contiguous()        # the engine's activation factor: H diag(Z)
+            buf = _terms_buffer(ops, Wd)
             eng = self._engine(Vn, Wd, Hz, precision) if self._engine_factory is None else self._engine_factory(Vn, Wd, Hz)
             try:
                 def step(k):
@@ -175,7 +206,8 @@ class BaseComponent(torch.nn.Module):
                         eng.sync()
                         dW, _ = eng.raw_terms(0, 1.0)     # P contracted with H Z  = W.grad   (plca.py:252-253)
                         dHz, _ = eng.raw_terms(1, 1.0)    # P contracted with W;  H.grad = dHz * Z,  Z.grad = sum H dHz
-                        self._em_update(Wd, Hd, Zd, dW, dHz, W_alpha, H_alpha, Z_alpha)
+                        dW, dZ = _em_terms(ops, Hd, dW, dHz, buf)
+                        self._em_update(Wd, Hd, Zd, dW, dHz, dZ, W_alpha, H_alpha, Z_alpha, ops)
 
                 n_iter = _fit_single(step, divergence, max_iter, tol, verbose)
                 eng.check_health()
@@ -184,11 +216,46 @@ class BaseComponent(torch.nn.Module):
                 eng.close()
         return n_iter, norm                                                                  # plca.py:304
 
-    def _em_update(self, Wd, Hd, Zd, dW, dHz, W_alpha, H_alpha, Z_alpha):
-        """The Z, W and H updates of one EM step (plca.py:256-288) from the raw gradients dW and dHz (= H.grad / Z),
-        in place on the working copies, each taken only where the module's factor is trainable."""
+    def _target_shape(self):
+        """The target's shape the factors model: (N, C) for PLCA, (B, C, *(J + K - 1)) for the shift-invariant models."""
+        H, W = self.H, self.W
+        return (H.shape[0], W.shape[0]) + tuple(j + k - 1 for j, k in zip(H.shape[2:], W.shape[2:]))
+
+    def _shape_mismatch(self, V):
+        """None when V has the shape the factors model, else the message of the mismatch."""
+        if tuple(V.shape) == self._target_shape():
+            return None
+        return f"target shape {tuple(V.shape)} does not match H {tuple(self.H.shape)} / W {tuple(self.W.shape)}"
+
+    def _agree_on_shards(self, ops, V, mismatch, nonneg, stored, norm):
+        """A sharded fit's entry over the Collectives `ops`: this rank's checks -- `mismatch` (None or the message of a
+        shard that does not match H / W), `nonneg` (no negative value) and `stored` (the shard holds a row or clip; a
+        sparse one stores an entry) --
+        agreed by every rank before any raises, so that no rank waits in a collective the others never reach; then the
+        sizes past the shard axis, equal on every rank.  Returns the global norm, the sum of every shard's `norm`
+        (float64 across ranks), in norm's dtype and on its device."""
+        if not ops.all_ranks(mismatch is None):
+            raise ValueError(mismatch or "sharded fit: the target shard of another rank does not match its H / W")
+        nonneg = ops.all_ranks(nonneg)
+        assert nonneg, "Target should be non-negative."                                     # plca.py:236, on any rank
+        if not ops.all_ranks(stored):
+            if stored:
+                raise ValueError("sharded fit: the target shard of another rank is empty")
+            raise ValueError("the sparse target stores no entry" if V.is_sparse
+                             else f"sharded fit: this rank's target shard {tuple(V.shape)} is empty")
+        K, X = tuple(self.W.shape[2:]), tuple(V.shape[2:])
+        ops.check_same_sizes(["C", "R"] + [f"kernel_size[{i}]" for i in range(len(K))]
+                             + [f"V.shape[{i + 2}]" for i in range(len(X))], [*self.W.shape[:2], *K, *X])
+        total = ops.all_reduce_(norm.to(ops.device, torch.float64).reshape(1))
+        return total[0].to(norm.device, norm.dtype)
+
+    def _em_update(self, Wd, Hd, Zd, dW, dHz, dZ, W_alpha, H_alpha, Z_alpha, ops=None):
+        """The Z, W and H updates of one EM step (plca.py:256-288) from the raw gradients dW, dHz (= H.grad / Z) and
+        dZ (= Z.grad, `_em_terms`), in place on the working copies, each taken only where the module's factor is
+        trainable.  With `ops` (a sharded fit's Collectives: dW and dZ already summed over the ranks) the two divisions
+        by H's column sums take them over every rank's rows, one R-float all-reduce each."""
+        h_norm = get_norm if ops is None else (lambda x: ops.all_reduce_(get_norm(x)))
         dH = dHz * _over(Zd, Hd)
-        dZ = get_norm(Hd * dHz).reshape(-1)
         Z_prior = None
         if self.Z.requires_grad:                                                             # plca.py:256-262
             Zd.mul_(dZ.clamp_min(0))
@@ -211,12 +278,12 @@ class BaseComponent(torch.nn.Module):
                 Wd.div_(get_norm(Wd))
         if self.H.requires_grad:                                                             # plca.py:277-288
             Hd.mul_(dH.clamp_min(0))
-            H_div = get_norm(Hd) if Z_prior is None else _over(Z_prior, Hd)
+            H_div = h_norm(Hd) if Z_prior is None else _over(Z_prior, Hd)
             Hd.div_(H_div)
             if not _is_one(H_alpha):
                 Hd.add_(_as(H_alpha, Hd) - 1)
                 F.threshold(Hd, eps, eps, True)
-                Hd.div_(get_norm(Hd))
+                Hd.div_(h_norm(Hd))
 
     def _check_mask(self, V, mask, precision):
         """The masked fit's refusals, before any device work: (the mask on V's device, sum_O V in V's dtype)."""
@@ -274,8 +341,9 @@ class BaseComponent(torch.nn.Module):
                         aW, bW = eng.plca_masked_terms(0, qobs)
                         aH, bH = eng.plca_masked_terms(1)
                         q = qobs.to(f32)
-                        self._em_update(Wd, Hd, Zd, torch.addcmul(bW, aW, q), torch.addcmul(bH, aH, q), W_alpha, H_alpha,
-                                        Z_alpha)
+                        dHz = torch.addcmul(bH, aH, q)
+                        dW, dZ = _em_terms(None, Hd, torch.addcmul(bW, aW, q), dHz)
+                        self._em_update(Wd, Hd, Zd, dW, dHz, dZ, W_alpha, H_alpha, Z_alpha)
 
                 n_iter = _fit_single(step, divergence, max_iter, tol, verbose)
                 eng.check_health()
@@ -287,7 +355,7 @@ class BaseComponent(torch.nn.Module):
             qo = torch.where(Md, q, 0.).sum()
         return n_iter, (norm_o.double() / qo.to(norm_o.device)).to(norm_o.dtype)
 
-    def _fit_sparse(self, V, tol, max_iter, verbose, W_alpha, H_alpha, Z_alpha, precision):
+    def _fit_sparse(self, V, tol, max_iter, verbose, W_alpha, H_alpha, Z_alpha, precision, group):
         raise NotImplementedError(f"{type(self).__name__}.fit takes dense targets only (PLCA fits sparse COO targets)")
 
     # test hook, as the NMF modules' (tests/test_plca.py): factory(Vn, W, Hz) stands in for `_engine`
@@ -301,6 +369,31 @@ class BaseComponent(torch.nn.Module):
 def _over(z, x):
     """A rank vector against the rank dimension (1) of a factor (plca.py:269-270,282-283)."""
     return z[(slice(None),) + (None,) * (x.dim() - 2)]
+
+
+def _terms_buffer(ops, Wd):
+    """A sharded fit's flat [dW | dZ] buffer, W's size + R elements, allocated once per fit (None without `ops`)."""
+    return None if ops is None else torch.empty(Wd.numel() + Wd.shape[1], dtype=Wd.dtype, device=Wd.device)
+
+
+def _em_terms(ops, Hd, dW, dHz, buf=None):
+    """(dW, dZ) of one EM step: Z's gradient dZ = sum H dHz beside W's dW; with `ops` (a sharded fit's Collectives) both
+    copied into `buf` (`_terms_buffer`) and summed over the ranks in one all-reduce of it, returned as views of it."""
+    dZ = get_norm(Hd * dHz).reshape(-1)
+    if ops is None:
+        return dW, dZ
+    n = dW.numel()
+    buf[:n].view(dW.shape).copy_(dW)
+    buf[n:].copy_(dZ)
+    ops.all_reduce_(buf)
+    return buf[:n].view(dW.shape), buf[n:]
+
+
+def _total(ops, d):
+    """A divergence as a float: as it is without `ops`, else every rank's summed in float64 (one scalar all-reduce)."""
+    if ops is None:
+        return float(d)
+    return float(ops.all_reduce_(torch.as_tensor(d, dtype=torch.float64).reshape(1).to(ops.device)))
 
 
 def _is_one(a):
@@ -331,7 +424,7 @@ class PLCA(BaseComponent):
     def _engine(Vn, W, Hz, precision):
         return _engine.CudaNmfEngine(Vn, W, Hz, precision)
 
-    def _fit_sparse(self, V, tol, max_iter, verbose, W_alpha, H_alpha, Z_alpha, precision):
+    def _fit_sparse(self, V, tol, max_iter, verbose, W_alpha, H_alpha, Z_alpha, precision, group):
         """fit(V) for a sparse COO V: the EM fit of V.to_dense() without forming anything of size N x C (see `fit`)."""
         if V.layout != torch.sparse_coo:
             raise ValueError(f"PLCA.fit takes a dense or a sparse COO target (got layout {V.layout})")
@@ -341,35 +434,46 @@ class PLCA(BaseComponent):
             raise ValueError(f"unknown precision {precision!r}")
         W, H, Z = self.W, self.H, self.Z
         assert W is not None and H is not None and Z is not None, "fit() needs W, H and Z"
-        if V.dim() != 2 or tuple(V.shape) != (H.shape[0], W.shape[0]):
-            raise ValueError(f"target shape {tuple(V.shape)} does not match H {tuple(H.shape)} / W {tuple(W.shape)}")
+        mismatch = self._shape_mismatch(V)
+        if mismatch is not None and group is None:
+            raise ValueError(mismatch)
         Vc = V.coalesce()                                   # duplicates sum, as in V.to_dense()
         vals = Vc.values()
-        assert bool((vals >= 0.).all()), "Target should be non-negative."                   # plca.py:236
-        if vals.numel() == 0:
-            raise ValueError("the sparse target stores no entry")
+        nonneg = bool((vals >= 0.).all())
+        if group is None:
+            assert nonneg, "Target should be non-negative."                                 # plca.py:236
+            if vals.numel() == 0:
+                raise ValueError("the sparse target stores no entry")
         norm = vals.sum()                                                                    # V.sum(), in V's dtype
-        if not bool(norm > 0):
+        if group is None and not bool(norm > 0):
             raise ValueError("the sparse target's values sum to 0")
         no_cuda = "torchnmf_b200.PLCA.fit needs a CUDA device (sm_90a); there is no CPU fallback"
         with _placed_factors(self, (W, H, Z), no_cuda) as (dev, (Wd, Hd, Zd)):
+            ops = None
+            if group is not None:
+                ops = _engine.Collectives(group, dev)
+                norm = self._agree_on_shards(ops, V, mismatch, nonneg, vals.numel() > 0, norm)
+                if not bool(norm > 0):                      # the same global norm on every rank
+                    raise ValueError("the sparse target's values sum to 0")
             ft = Wd.dtype                                   # fp32 on the device; the test hook's factors as they are
             normd = norm.to(dev, ft)
             Vn = torch.sparse_coo_tensor(Vc.indices().to(dev), vals.to(dev, ft) / normd, V.shape,
                                          is_coalesced=True)                                 # plca.py:241-242
             normf = float(normd)
             Hz = (Hd * _over(Zd, Hd)).contiguous()
+            buf = _terms_buffer(ops, Wd)
             eng = _engine.CudaSparsePlcaEngine(Vn, Wd, Hz) if self._engine_factory is None else self._engine_factory(Vn, Wd, Hz)
             try:
                 def divergence(follows):
                     torch.mul(Hd, _over(Zd, Hd), out=Hz)
-                    return eng.loss(normf)                  # kl_div(norm q, V) at the stored entries and the column sums
+                    return _total(ops, eng.loss(normf))     # kl_div(norm q, V) at the stored entries and the column sums
 
                 def step(k):
                     for _ in range(k):
                         torch.mul(Hd, _over(Zd, Hd), out=Hz)
                         dW, dHz = eng.plca_terms(Hz)        # one ratio P per stored entry serves both gradients
-                        self._em_update(Wd, Hd, Zd, dW, dHz, W_alpha, H_alpha, Z_alpha)
+                        dW, dZ = _em_terms(ops, Hd, dW, dHz, buf)
+                        self._em_update(Wd, Hd, Zd, dW, dHz, dZ, W_alpha, H_alpha, Z_alpha, ops)
 
                 n_iter = _fit_single(step, divergence, max_iter, tol, verbose)
                 eng.check_health()
