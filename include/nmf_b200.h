@@ -262,6 +262,28 @@ int nmfb200_nmf_batched_cd_update(nmfb200_ctx* ctx, float* W, float* H, int whic
  * return NMFB200_ERR_INVALID. */
 int nmfb200_nmf_batched_cd_iterate(nmfb200_ctx* ctx, float* W, float* H, double l1_reg, double l2_reg, int n_iter,
                                    void* stream);
+/* Coordinate descent at beta 2 on the observed cells (CCD++, Yu et al. 2012, made non-negative), on a context whose target
+ * was set by nmfb200_nmf_set_target_observed or _observed_weighted.  One update of W (which = 0) or H (which = 1) in place
+ * minimises  1/2 sum_{(n,c) observed} w (v - h_n . w_c)^2 + l1_reg (sum W + sum H) + l2_reg / 2 (|W|^2 + |H|^2)  over that
+ * factor (w = 1 without weights) by one exact sweep over its columns.  Every row s of the updated factor X runs on its own,
+ * over the observed cells O_s of its segment (a column of V for W, a row for H), with f_j the other factor's row of cell j
+ * and r = v - f_j . x_s at the current x_s; for k = 0 .. R-1 in order:
+ *   num = sum_{j in O_s} w_j r_j f_{j,k},  hess = sum_{j in O_s} w_j f_{j,k}^2 + l2_reg,
+ *   if hess != 0:  x_{s,k} <- max(0, x_{s,k} + (num - l1_reg - l2_reg x_{s,k}) / hess),
+ * entries j < k already updated.  The floor is exactly 0; a row with no observed cell and l2_reg = 0 is left as it is.
+ * With every cell observed and unit weights this is nmfb200_nmf_cd_update's update in exact arithmetic.  One warp per
+ * segment sums in the segment's stored order: no atomics, the result is deterministic.  O(observed x R) work per update,
+ * in ceil(R / 32) passes over the observed entries; above rank 32 a residual workspace of one float per observed entry is
+ * allocated at the first call.  These are separate calls: nmfb200_nmf_cd_update / _iterate still refuse observed-cell
+ * contexts.  NMFB200_ERR_STATE before any set_target*; NMFB200_ERR_INVALID for any other target form (dense, with or
+ * without a mask or weight, or sparse), NMFD / NMF2D / NMF3D and batched contexts, a null context or pointer, and which
+ * not 0 / 1.  Asynchronous. */
+int nmfb200_nmf_observed_cd_update(nmfb200_ctx* ctx, float* W, float* H, int which, double l1_reg, double l2_reg,
+                                   void* stream);
+/* n_iter x (nmfb200_nmf_observed_cd_update of W; of H with the new W) in one host call; n_iter < 0 and the refusals above
+ * return NMFB200_ERR_INVALID. */
+int nmfb200_nmf_observed_cd_iterate(nmfb200_ctx* ctx, float* W, float* H, double l1_reg, double l2_reg, int n_iter,
+                                    void* stream);
 
 /* ---- NMFD (1-D convolutive NMF), NMF2D, NMF3D ------------------------------------------------ */
 

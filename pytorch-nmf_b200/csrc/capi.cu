@@ -28,13 +28,15 @@ enum class CtxKind { Nmf, Nmfd, NmfBatch, NmfdBatch, PlcaSparse };
 enum class TargetForm { None, Dense, Sparse, SparseAnyBeta, Observed };
 
 // A sparse target, borrowed: CSR (rows of V) and CSC (= CSR of V^T) forms; an observed target's entry weights in CSR / CSC
-// order (none: unweighted); V_norm of nmf.py:161-170 (beta 1 / 2); sparse PLCA's CSR position of each CSC entry
+// order (none: unweighted); V_norm of nmf.py:161-170 (beta 1 / 2); sparse PLCA's CSR position of each CSC entry; the
+// stored entries' count (set by set_sparse_target)
 struct SparseTarget {            // members in the order of the set_target_sparse* arguments
   const int64_t* crow = nullptr; const int64_t* col = nullptr; const float* val = nullptr;
   const int64_t* ccol = nullptr; const int64_t* row = nullptr; const float* val_t = nullptr;
   const float *wt = nullptr, *wt_t = nullptr;
   double vnorm_kl = 0.0, vnorm_eu = 0.0;
   const int64_t* perm = nullptr;
+  int64_t nnz = 0;
 };
 
 // A device buffer a context owns: `n` elements of T, freed with the context (an empty one makes no CUDA call)
@@ -92,6 +94,7 @@ struct nmfb200_ctx {
   DevBuf<float> mm_scratch;       // kMmFloats: matrix_minmax's partials, then the target's min / max
   DevBuf<float> sp_den;           // max(N, C) x R: the reduced V-free denominator of an update at beta != 1, 2
   DevBuf<float> sp_gram;          // [2][R*R] (W^T W, H^T H) + per-block partials; also the Gram scratch of nmfb200_nmf_cd_*
+  DevBuf<float> obs_r;            // nmfb200_nmf_observed_cd_*: one residual per observed entry (R > 32 only)
   DevBuf<double> sp_loss_part;
   // NMFD: the ratio tiles, Pp (lazy) sized like Pn (a batch: every problem's, back to back)
   DevBuf<float> Pn, Pp;
@@ -466,7 +469,9 @@ int set_sparse_target(nmfb200_ctx* ctx, TargetForm form, int64_t nnz, const Spar
   if (form != TargetForm::Sparse)                          // the denominator of an update outside raw_terms
     NMF_CUDA_CHECK(ctx->den.ensure(ctx->num.n));
   if (form == TargetForm::SparseAnyBeta) NMF_CUDA_CHECK(ctx->sp_den.ensure(std::max(ctx->N, ctx->C) * ctx->R));
-  commit_target(ctx, form, nullptr, NMFB200_DTYPE_F32, 0, 0, sp);
+  SparseTarget t = sp;
+  t.nnz = nnz;
+  commit_target(ctx, form, nullptr, NMFB200_DTYPE_F32, 0, 0, t);
   if (form != TargetForm::Observed) return 0;
   // target_minmax: the observed values (none: +inf / -inf)
   return matrix_minmax(sp.val, NMFB200_DTYPE_F32, 1, nnz, nnz, ctx->mm_scratch, ctx->mm_scratch + kMmPartials,
@@ -1400,6 +1405,55 @@ int nmfb200_nmf_batched_cd_iterate(nmfb200_ctx* ctx, float* W, float* H, double 
   if (int rc = cd_batched_check(ctx)) return rc;
   if (!W || !H || n_iter < 0) return fail(NMFB200_ERR_INVALID, "bad argument");
   return cd_iterate(ctx, W, H, l1_reg, l2_reg, n_iter, (cudaStream_t)stream);
+}
+
+/* ---- coordinate descent at beta 2 on the observed cells of a target (observed_cd.cu) ------------------------------ */
+
+namespace {
+// What the observed cd calls serve: a single NMF context whose target was set by set_target_observed / _weighted
+// (so R <= 256 and no mask or weight).  nmfb200_nmf_cd_* keeps its own refusal of these contexts.
+int observed_cd_check(nmfb200_ctx* ctx) {
+  if (is_nmfd(ctx)) return fail(NMFB200_ERR_INVALID, "observed cd: NMFD / NMF2D / NMF3D contexts are not served (NMF only)");
+  if (is_batch(ctx)) return fail(NMFB200_ERR_INVALID, "observed cd: batched contexts are not served");
+  if (ctx->R > 256) return fail(NMFB200_ERR_INVALID, "observed cd: rank must be at most 256");
+  TARGET_GUARD(ctx);
+  if (ctx->form != TargetForm::Observed)
+    return fail(NMFB200_ERR_INVALID, "observed cd: only targets set by nmfb200_nmf_set_target_observed / _weighted are "
+                                     "served (nmfb200_nmf_cd_update serves dense and sparse targets)");
+  return 0;
+}
+
+// One update of W (which = 0, over the CSC form) or H (which = 1, over the CSR form) in place.
+int observed_cd_update_factor(nmfb200_ctx* c, int which, float* W, float* H, double l1_reg, double l2_reg,
+                              cudaStream_t st) {
+  const int R = (int)c->R;
+  if (const int64_t nr = observed_cd_workspace_floats(R, c->sp.nnz)) NMF_CUDA_CHECK(c->obs_r.ensure(nr));
+  const SparseTarget& s = c->sp;
+  if (which == 0)
+    return observed_cd(s.ccol, s.row, s.val_t, s.wt_t, W, H, R, c->C, c->obs_r, (float)l1_reg, (float)l2_reg, st);
+  return observed_cd(s.crow, s.col, s.val, s.wt, H, W, R, c->N, c->obs_r, (float)l1_reg, (float)l2_reg, st);
+}
+}  // namespace
+
+int nmfb200_nmf_observed_cd_update(nmfb200_ctx* ctx, float* W, float* H, int which, double l1_reg, double l2_reg,
+                                   void* stream) {
+  CTX_GUARD(ctx, kDenseModels);
+  if (int rc = observed_cd_check(ctx)) return rc;
+  if (!W || !H || (which != 0 && which != 1)) return fail(NMFB200_ERR_INVALID, "bad argument");
+  return observed_cd_update_factor(ctx, which, W, H, l1_reg, l2_reg, (cudaStream_t)stream);
+}
+
+int nmfb200_nmf_observed_cd_iterate(nmfb200_ctx* ctx, float* W, float* H, double l1_reg, double l2_reg, int n_iter,
+                                    void* stream) {
+  CTX_GUARD(ctx, kDenseModels);
+  if (int rc = observed_cd_check(ctx)) return rc;
+  if (!W || !H || n_iter < 0) return fail(NMFB200_ERR_INVALID, "bad argument");
+  for (int i = 0; i < n_iter; ++i) {
+    int rc = observed_cd_update_factor(ctx, 0, W, H, l1_reg, l2_reg, (cudaStream_t)stream);
+    if (rc == 0) rc = observed_cd_update_factor(ctx, 1, W, H, l1_reg, l2_reg, (cudaStream_t)stream);
+    if (rc) return rc;
+  }
+  return 0;
 }
 
 /* ---- batched PLCA: the EM iteration on the raw terms of a batched NMF / NMFD context ---------------------------- */

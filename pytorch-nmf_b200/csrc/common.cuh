@@ -273,6 +273,14 @@ int cd_sweep(float* X, int64_t rows, int R, const float* A, int nchunks, int64_t
 // blocks of one problem's sweep over `rows` rows (grid x: this times the problems of a batch)
 int64_t cd_sweep_blocks(int64_t rows);
 
+// observed_cd.cu ---------------------------------------------------------------------------
+// One coordinate-descent update of a (nseg x R) factor X in place on the observed cells, R <= 256
+// (nmfb200_nmf_observed_cd_update): ptr / idx / val (and the entries' weights wt, null: unweighted) the compressed form whose
+// segments are X's rows, F the other factor.  rbuf: observed_cd_workspace_floats(R, nnz) floats (none for R <= 32).
+int observed_cd(const int64_t* ptr, const int64_t* idx, const float* val, const float* wt, float* X, const float* F, int R,
+                int64_t nseg, float* rbuf, float l1, float l2, cudaStream_t st);
+int64_t observed_cd_workspace_floats(int R, int64_t nnz);
+
 // update.cu --------------------------------------------------------------------------------
 // nmf.py:78-92 on a flattened parameter of `numel` elements whose rank index is
 // r = (idx / inner) % R.   num/den are sums over `nchunks` partial slabs (stride chunk_stride,

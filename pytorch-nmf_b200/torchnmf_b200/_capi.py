@@ -47,6 +47,8 @@ SIGNATURES = {
     "nmfb200_nmf_batched_set_active": (_int, [_vp, _vp, _vp]),
     "nmfb200_nmf_batched_cd_update": (_int, [_vp, _vp, _vp, _int, _dbl, _dbl, _vp]),
     "nmfb200_nmf_batched_cd_iterate": (_int, [_vp, _vp, _vp, _dbl, _dbl, _int, _vp]),
+    "nmfb200_nmf_observed_cd_update": (_int, [_vp, _vp, _vp, _int, _dbl, _dbl, _vp]),
+    "nmfb200_nmf_observed_cd_iterate": (_int, [_vp, _vp, _vp, _dbl, _dbl, _int, _vp]),
     "nmfb200_nmf_set_target_sparse": (_int, [_vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _dbl, _dbl, _vp]),
     "nmfb200_nmf_set_target_sparse_any_beta": (_int, [_vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _dbl, _dbl, _vp]),
     "nmfb200_nmf_set_target_observed": (_int, [_vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),

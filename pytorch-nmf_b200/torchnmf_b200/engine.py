@@ -735,6 +735,17 @@ class CudaObservedNmfEngine(_SparseEngine):
         buf = self._raw_terms_into(which, beta, None)
         return buf[:f.numel()].view(f.shape), buf[f.numel():].view(f.shape)
 
+    def cd_update(self, which, l1_reg, l2_reg):
+        """One coordinate-descent update at beta 2 of W (which=0) or H (which=1) in place on the observed cells: one exact
+        sweep over its columns (include/nmf_b200.h: nmfb200_nmf_observed_cd_update)."""
+        _capi.check(self._lib.nmfb200_nmf_observed_cd_update(self._ctx, _ptr(self.W), _ptr(self.H), int(which),
+                                                             float(l1_reg), float(l2_reg), _stream(self.device)))
+
+    def cd_iterate(self, n_iter, l1_reg, l2_reg):
+        """n_iter x (cd_update(0); cd_update(1)) in one call."""
+        _capi.check(self._lib.nmfb200_nmf_observed_cd_iterate(self._ctx, _ptr(self.W), _ptr(self.H), float(l1_reg),
+                                                              float(l2_reg), int(n_iter), _stream(self.device)))
+
     iterate = CudaNmfEngine.iterate
 
 

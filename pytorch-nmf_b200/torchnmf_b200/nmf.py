@@ -391,8 +391,10 @@ class BaseComponent(torch.nn.Module):
             raise ValueError(f"solver='cd' is supported by NMF only (got {type(self).__name__})")
         if beta != 2:
             raise ValueError(f"solver='cd' minimises the beta = 2 objective; beta must be 2 (got {beta!r})")
-        if mask is not None or weight is not None:
-            raise ValueError("solver='cd' takes no mask or weight")
+        for name, sel in (("mask", mask), ("weight", weight)):
+            if isinstance(sel, Tensor) and not sel.is_sparse:
+                raise ValueError(f"solver='cd' takes a sparse {name} only, fitted on its observed cells; pass "
+                                 f"{name}.to_sparse()")
         if group is not None:
             raise ValueError("solver='cd' does not run sharded fits (group)")
         if precision in ("f16", "f16_split"):
@@ -446,7 +448,8 @@ class BaseComponent(torch.nn.Module):
                    -- is read at those cells only.  The objective is the same; up to rank 256 every update and the loss
                    run on the observed cells alone, O(observed x R) per update and O(observed + (N + C) R) memory, for
                    matrix completion where few cells are observed.  Above rank 256 the observed values and the mask are
-                   densified on the device.  With `group`, each rank passes the row shards of V and of the mask.
+                   densified on the device.  With `group`, each rank passes the row shards of V and of the mask.  A
+                   sparse mask also takes solver="cd" at beta 2 (see `solver`); a dense one does not.
 
         weight:    (keyword-only, default None, through **options like `mask`; exclusive with it -- fold a mask into the
                    weight) a floating-point tensor of V's shape holding one weight w >= 0 per cell: the fit minimises
@@ -467,6 +470,7 @@ class BaseComponent(torch.nn.Module):
                    sparse COO (0 where it stores nothing), and up to rank 256 every update and the loss run on those
                    cells alone, O(observed x R) per update; above rank 256 the weights and values are densified on the
                    device.  A dense weight on a sparse V and a sparse weight on NMFD / NMF2D / NMF3D raise ValueError.
+                   A sparse weight also takes solver="cd" at beta 2 (see `solver`); a dense one does not.
                    With `group`, each rank passes the weight shard of its V shard; a shard may be zero everywhere (or,
                    sparse, store nothing), and the value check is agreed on by all ranks, so every rank raises together.
 
@@ -482,8 +486,18 @@ class BaseComponent(torch.nn.Module):
                    0.  Loss, stop rule and return value are those of "mu".  NMF only, on the fp32 kernels: precision
                    "auto" resolves to "f32" and `last_fit_precision` is "f32".  V dense (float32, float16 or bfloat16 read
                    in place at any row stride; float64 staged) or sparse COO; `alpha`, `l1_ratio`, frozen factors and
-                   host or float64 modules work as for "mu".  ValueError, before any device work: beta != 2, `mask` or
-                   `weight`, `group`, precision "f16" / "f16_split", rank > 256, an unknown solver, and NMFD / NMF2D /
+                   host or float64 modules work as for "mu".
+                   With a sparse `mask` or `weight` (NMF, rank <= 256), "cd" fits the observed cells O alone:
+                   1/2 sum_O w (v - h_n . w_c)^2 + the same penalties (w = 1 for a mask), by coordinate descent on O
+                   (CCD++, Yu et al. 2012, made non-negative).  Each update is one exact sweep per row s of the factor
+                   over the observed cells O_s of its segment (a column of V for W, a row for H): with f_j the other
+                   factor's row of cell j and r = v - f_j . x_s at the current x_s, for k = 0 .. R-1 in order,
+                   num = sum_{O_s} w r f_{j,k}, hess = sum_{O_s} w f_{j,k}^2 + l2, and if hess != 0,
+                   x_{s,k} <- max(0, x_{s,k} + (num - l1 - l2 x_{s,k}) / hess).  O(observed x R) per update, device
+                   memory O(observed + (N + C) R); the loss is the observed-cell loss "mu" reports.  Every cell observed
+                   with unit weights gives the update above in exact arithmetic.  ValueError, before any device work:
+                   beta != 2, a dense `mask` or `weight` (pass `mask.to_sparse()`: a dense one would need a Gram matrix
+                   per row), `group`, precision "f16" / "f16_split", rank > 256, an unknown solver, and NMFD / NMF2D /
                    NMF3D.
         """
         mask = options.pop("mask", None)
