@@ -505,6 +505,18 @@ int nmfb200_set_mask(nmfb200_ctx* ctx, const uint8_t* M, void* stream);
  * (precision_for_beta reports NMFB200_PREC_F32, nmf_peer_supported 0).  Asynchronous. */
 int nmfb200_set_weight(nmfb200_ctx* ctx, const float* Wt, void* stream);
 
+/* Hold chosen components of W at their values (semi-supervised fits: a dictionary learned beforehand stays fixed while the
+ * other components learn the rest of the target).  fixed: a DEVICE array of R uint8, non-zero for a fixed component k
+ * (W[:, k] for NMF, W[:, k, ...] for NMFD / NMF2D / NMF3D), borrowed like a mask.  Valid on a single NMF or NMFD context
+ * after any set_target* (NMFB200_ERR_STATE before); NMFB200_ERR_INVALID on batched and sparse-PLCA contexts.  A null fixed,
+ * or any later set_target*, clears it.  While it is set, every call that writes W -- update_w, nmf_iterate, w_apply,
+ * nmf_cd_update / _iterate and nmf_observed_cd_update / _iterate, on every kernel family -- leaves the fixed components
+ * unstored: the free ones take exactly the update they take without it (the reconstruction formed from all R components,
+ * the penalties on the free ones only), and a fixed component still enters the tensor-core operand scale, column sums and
+ * loss as it is.  The coordinate-descent sweeps skip each fixed k: no step, and later components see its unchanged value.
+ * H updates are unaffected, and nmf_peer_supported reports 0 while it is set.  Queues nothing. */
+int nmfb200_set_fixed_w(nmfb200_ctx* ctx, const uint8_t* fixed, void* stream);
+
 /* ---- tile plans of the fp32 CUDA-core kernels (host only: no device work, no allocation) -------- */
 
 /* What a context of these sizes runs on the fp32 kernels, from the library's own planners.  `out` receives

@@ -85,6 +85,9 @@ struct nmfb200_ctx {
   // borrowed; cleared by every set_target*.  While set, every pass runs the selecting fp32 kernels and beta 1 takes its
   // denominators from the contraction, not the column sums.
   CellSel sel;
+  // nmfb200_set_fixed_w: R bytes, non-zero for a component of W held at its value, borrowed; cleared by every set_target*.
+  // While set, every call that writes W leaves those components unstored.
+  const uint8_t* fixed_w = nullptr;
   // chunked partial numerators / denominators of the CUDA-core path; den (lazy) is sized like num
   DevBuf<float> num, den;
   int nslab[2] = {1, 1};          // partial slabs of the W / H terms: contraction chunks (NMF), wgrad / dgrad splits (NMFD)
@@ -426,11 +429,13 @@ int check_target(const void* V, int dtype) {
 }
 
 // The one place a set_target* changes the target, once its checks and allocations have passed: a call refused before it
-// leaves the context as it was.  A new target drops the mask or weight; a sparse one takes the tensor cores out of play.
+// leaves the context as it was.  A new target drops the mask or weight and the fixed components of W; a sparse one takes
+// the tensor cores out of play.
 void commit_target(nmfb200_ctx* c, TargetForm form, const void* V, int vdtype, int64_t ldv, int64_t bstride,
                    const SparseTarget& sp = SparseTarget{}) {
   c->form = form; c->V = V; c->vdtype = vdtype; c->ldv = ldv; c->bstride = bstride; c->sp = sp;
   c->sel = CellSel{};
+  c->fixed_w = nullptr;
   c->tc_off = form != TargetForm::Dense;
 }
 
@@ -908,6 +913,17 @@ int nmfb200_set_weight(nmfb200_ctx* ctx, const float* Wt, void* stream) {
   return set_selector(ctx, CellSel{Wt, kSelWeight}, stream);
 }
 
+int nmfb200_set_fixed_w(nmfb200_ctx* ctx, const uint8_t* fixed, void* stream) {
+  (void)stream;              // nothing is queued: the flags are read by the kernels of later W updates
+  CTX_GUARD(ctx, kDenseModels | kinds(CtxKind::PlcaSparse));
+  if (is_batch(ctx)) return fail(NMFB200_ERR_INVALID, "batched fits take no fixed components of W");
+  if (ctx->kind == CtxKind::PlcaSparse)
+    return fail(NMFB200_ERR_INVALID, "sparse PLCA contexts do not update W (its EM step is the caller's)");
+  TARGET_GUARD(ctx);
+  ctx->fixed_w = fixed;
+  return 0;
+}
+
 namespace {
 // beta 1 and 2 run on every sparse context; any other beta > 0 only on one set by nmfb200_nmf_set_target_sparse_any_beta,
 // every beta on one set by nmfb200_nmf_set_target_observed
@@ -1031,13 +1047,14 @@ int factor_terms(nmfb200_ctx* c, int which, const float* W, const float* H, doub
 // the entry points select the context's device.
 int update_factor(nmfb200_ctx* ctx, int which, float* param, const float* W, const float* H, double beta, double gamma,
                   double l1_reg, double l2_reg, cudaStream_t st) {
-  if (ctx->tc && use_tc(ctx, beta)) return tc_update(ctx->tc, which, param, W, H, beta, gamma, l1_reg, l2_reg, st);
+  const uint8_t* fixed = which == 0 ? ctx->fixed_w : nullptr;
+  if (ctx->tc && use_tc(ctx, beta)) return tc_update(ctx->tc, which, param, W, H, beta, gamma, l1_reg, l2_reg, st, fixed);
   ApplyArgs a; bool tc;
   int rc = factor_terms(ctx, which, W, H, beta, nullptr, a, &tc, st);
   if (rc) return rc;
   a.param = param; a.gamma = (float)gamma; a.l1 = (float)l1_reg; a.l2 = (float)l2_reg;
   if (tc) a.absmax_bits = tc_nmfd_begin_update(ctx->tcd, which, st);
-  rc = apply_update(a, st);
+  rc = apply_update(a, st, fixed);
   if (rc) return rc;
   if (!tc) mark_stale(ctx, which == 0, which == 1);
   return 0;
@@ -1115,7 +1132,7 @@ int nmfb200_nmf_loss_prefetch_w(nmfb200_ctx* ctx, const float* W, const float* H
 /* ---- row-sharded W update over peer memory (NVLink, one process per GPU) ---------------------- */
 
 int nmfb200_nmf_peer_supported(const nmfb200_ctx* ctx, double beta) {
-  if (!ctx || ctx->kind != CtxKind::Nmf || !has_target(ctx) || !use_tc(ctx, beta)) return 0;
+  if (!ctx || ctx->kind != CtxKind::Nmf || !has_target(ctx) || ctx->fixed_w || !use_tc(ctx, beta)) return 0;
   return tc_peer_supported(ctx->tc, beta) ? 1 : 0;
 }
 
@@ -1242,14 +1259,14 @@ int nmfb200_w_apply(nmfb200_ctx* ctx, float* W, const float* reduced, double bet
   if (is_batch(ctx)) return fail(NMFB200_ERR_INVALID, "w_apply does not serve batched contexts");
   if (!W || !reduced) return fail(NMFB200_ERR_INVALID, "null pointer");
   cudaStream_t st = (cudaStream_t)stream;
-  if (ctx->tc && use_tc(ctx, beta)) return tc_w_apply(ctx->tc, W, reduced, beta, gamma, l1_reg, l2_reg, st);
+  if (ctx->tc && use_tc(ctx, beta)) return tc_w_apply(ctx->tc, W, reduced, beta, gamma, l1_reg, l2_reg, st, ctx->fixed_w);
   ApplyArgs a = factor_view(ctx, 0, 1);     // an NMFD centring term is already folded in by raw_sum
   a.param = W; a.num = reduced; a.gamma = (float)gamma; a.l1 = (float)l1_reg; a.l2 = (float)l2_reg;
   if (kl_colsum(ctx, beta)) a.kl_den = reduced + a.numel;
   else a.den = reduced + a.numel;
   const bool tc = use_tc(ctx, beta);        // here: the NMFD tensor cores
   if (tc) a.absmax_bits = tc_nmfd_begin_update(ctx->tcd, 0, st);
-  int rc = apply_update(a, st);
+  int rc = apply_update(a, st, ctx->fixed_w);
   if (rc) return rc;
   if (!tc) mark_stale(ctx, true, false);
   return 0;
@@ -1362,7 +1379,9 @@ int cd_update_factor(nmfb200_ctx* c, int which, float* W, float* H, double l1_re
   if ((rc = sparse_gram(other, f.other_rows, R, c->sp_gram + 2 * P * R * R, G, st, gbt))) return rc;
   Batch sbt = bt;
   sbt.g = (int64_t)R * R;
-  if ((rc = cd_sweep(X, f.rows, R, c->num, nch, f.rows * R * P, G, (float)l1_reg, (float)l2_reg, st, sbt))) return rc;
+  if ((rc = cd_sweep(X, f.rows, R, c->num, nch, f.rows * R * P, G, (float)l1_reg, (float)l2_reg, st, sbt,
+                     which == 0 ? c->fixed_w : nullptr)))
+    return rc;
   if (!is_sparse(c)) mark_stale(c, which == 0, which == 1);   // the tensor-core operand copies of X are out of date
   return 0;
 }
@@ -1430,7 +1449,8 @@ int observed_cd_update_factor(nmfb200_ctx* c, int which, float* W, float* H, dou
   if (const int64_t nr = observed_cd_workspace_floats(R, c->sp.nnz)) NMF_CUDA_CHECK(c->obs_r.ensure(nr));
   const SparseTarget& s = c->sp;
   if (which == 0)
-    return observed_cd(s.ccol, s.row, s.val_t, s.wt_t, W, H, R, c->C, c->obs_r, (float)l1_reg, (float)l2_reg, st);
+    return observed_cd(s.ccol, s.row, s.val_t, s.wt_t, W, H, R, c->C, c->obs_r, (float)l1_reg, (float)l2_reg, st,
+                       c->fixed_w);
   return observed_cd(s.crow, s.col, s.val, s.wt, H, W, R, c->N, c->obs_r, (float)l1_reg, (float)l2_reg, st);
 }
 }  // namespace

@@ -26,11 +26,12 @@ constexpr int kSweepRows = 4;     // rows per warp
 
 // BATCH: bt.n problems, problem b on the single problem's blocks [b nbx, (b + 1) nbx) of grid x, with its X at X + b bt.f,
 // its A partials at A + b bt.p within each slab and its B at B + b bt.g; a problem whose bt.active flag is 0 exits at once.
-// The single-problem instantiations compile none of it.
-template <int RPL, int ROWS, bool BATCH>
+// The single-problem instantiations compile none of it.  FIXED: the columns k with fixed[k] != 0 take no step.
+template <int RPL, int ROWS, bool BATCH, bool FIXED = false>
 __global__ void __launch_bounds__(256)
 cd_sweep_kernel(float* __restrict__ X, int64_t rows, int R, const float* __restrict__ A, int nchunks,
-                int64_t chunk_stride, const float* __restrict__ B, float l1, float l2, Batch bt) {
+                int64_t chunk_stride, const float* __restrict__ B, float l1, float l2, Batch bt,
+                const uint8_t* __restrict__ fixed) {
   __shared__ float Bp[kPanel * RPL * kPanelLd];        // Bp[j][kk] = B[j, 32 m + kk] of panel m, zero outside R x R
   const int lane = threadIdx.x & 31;
   int64_t bx = blockIdx.x;
@@ -81,7 +82,8 @@ cd_sweep_kernel(float* __restrict__ X, int64_t rows, int R, const float* __restr
       for (int o = 16; o > 0; o >>= 1)
 #pragma unroll
         for (int q = 0; q < ROWS; ++q) dot[q] += __shfl_xor_sync(0xffffffffu, dot[q], o);
-      if (hess != 0.f && lane == kk) {   // sklearn's `hess != 0` guard: a dead component keeps its column
+      // sklearn's `hess != 0` guard: a dead component keeps its column; so does a fixed one
+      if (hess != 0.f && lane == kk && !(FIXED && fixed[kPanel * m + kk])) {
 #pragma unroll
         for (int q = 0; q < ROWS; ++q) {
           const float v = x[q][m];
@@ -107,7 +109,7 @@ cd_sweep_kernel(float* __restrict__ X, int64_t rows, int R, const float* __restr
 int64_t cd_sweep_blocks(int64_t rows) { return ceil_div(rows, (int64_t)kWarps * kSweepRows); }
 
 int cd_sweep(float* X, int64_t rows, int R, const float* A, int nchunks, int64_t chunk_stride, const float* B, float l1,
-             float l2, cudaStream_t st, const Batch& bt) {
+             float l2, cudaStream_t st, const Batch& bt, const uint8_t* fixed) {
   if (R < 1 || R > 256) { set_error("cd_sweep: rank must be in [1, 256]"); return 1; }
   if (rows < 1) return 0;
   const int rpl = (R + 31) / 32;
@@ -115,12 +117,15 @@ int cd_sweep(float* X, int64_t rows, int R, const float* A, int nchunks, int64_t
   if (bt.n < 1 || blocks > kMaxGridX / bt.n) { set_error("cd_sweep: batch x row blocks pass grid x"); return 1; }
   const unsigned gx = (unsigned)(blocks * bt.n);
   const bool batched = bt.n > 1 || bt.active;
-#define NMF_CD_B(RPLV, BATCH) \
-  cd_sweep_kernel<RPLV, kSweepRows, BATCH><<<gx, 256, 0, st>>>(X, rows, R, A, nchunks, chunk_stride, B, l1, l2, bt)
-#define NMF_CD(RPLV)                 \
-  do {                               \
-    if (batched) NMF_CD_B(RPLV, true); \
-    else NMF_CD_B(RPLV, false);      \
+  if (fixed && batched) { set_error("cd_sweep: fixed components need a single problem"); return 1; }
+#define NMF_CD_B(RPLV, BATCH, FIXED)                                                                                  \
+  cd_sweep_kernel<RPLV, kSweepRows, BATCH, FIXED><<<gx, 256, 0, st>>>(X, rows, R, A, nchunks, chunk_stride, B, l1, l2, bt, \
+                                                                     fixed)
+#define NMF_CD(RPLV)                          \
+  do {                                        \
+    if (fixed) NMF_CD_B(RPLV, false, true);   \
+    else if (batched) NMF_CD_B(RPLV, true, false); \
+    else NMF_CD_B(RPLV, false, false);        \
   } while (0)
   if (rpl <= 1) NMF_CD(1);
   else if (rpl <= 2) NMF_CD(2);

@@ -267,9 +267,10 @@ int64_t sparse_gram_part_floats(int R);
 //   X[c,k] <- max(0, X[c,k] + (A[c,k] - sum_j X[c,j] B[j,k] - l1 - l2 X[c,k]) / (B[k,k] + l2))
 // on every row c, columns with B[k,k] + l2 == 0 left as they are.  bt: bt.n problems in one launch, problem b's X at
 // X + b bt.f, its A partials at A + b bt.p within each slab and its B at B + b bt.g, each summed in the single problem's
-// order; problems whose bt.active flag is 0 are left untouched.
+// order; problems whose bt.active flag is 0 are left untouched.  fixed (R bytes, one problem only; null: none): the sweep
+// skips every column k with fixed[k] != 0, which keeps its value, and later columns see that value.
 int cd_sweep(float* X, int64_t rows, int R, const float* A, int nchunks, int64_t chunk_stride, const float* B, float l1,
-             float l2, cudaStream_t st, const Batch& bt = Batch{});
+             float l2, cudaStream_t st, const Batch& bt = Batch{}, const uint8_t* fixed = nullptr);
 // blocks of one problem's sweep over `rows` rows (grid x: this times the problems of a batch)
 int64_t cd_sweep_blocks(int64_t rows);
 
@@ -277,8 +278,9 @@ int64_t cd_sweep_blocks(int64_t rows);
 // One coordinate-descent update of a (nseg x R) factor X in place on the observed cells, R <= 256
 // (nmfb200_nmf_observed_cd_update): ptr / idx / val (and the entries' weights wt, null: unweighted) the compressed form whose
 // segments are X's rows, F the other factor.  rbuf: observed_cd_workspace_floats(R, nnz) floats (none for R <= 32).
+// fixed (R bytes; null: none): the sweep skips every component k with fixed[k] != 0 -- no step, no residual update.
 int observed_cd(const int64_t* ptr, const int64_t* idx, const float* val, const float* wt, float* X, const float* F, int R,
-                int64_t nseg, float* rbuf, float l1, float l2, cudaStream_t st);
+                int64_t nseg, float* rbuf, float l1, float l2, cudaStream_t st, const uint8_t* fixed = nullptr);
 int64_t observed_cd_workspace_floats(int R, int64_t nnz);
 
 // update.cu --------------------------------------------------------------------------------
@@ -308,7 +310,9 @@ struct ApplyArgs {
   // problem's compact size; the others are padding, left untouched.  0: the layout above
   int64_t line = 0;
 };
-int apply_update(const ApplyArgs& a, cudaStream_t st);
+// fixed (R bytes, one problem only; null: none): the elements of every component r with fixed[r] != 0 are not stored
+// (they keep their value, which is what an absmax_bits update takes for them)
+int apply_update(const ApplyArgs& a, cudaStream_t st, const uint8_t* fixed = nullptr);
 // whether apply_update takes its four-elements-per-thread kernel for this shape (16-byte aligned buffers provided)
 bool apply_update_vec4_shape(const ApplyArgs& a);
 // num_out[i] (and den_out[i] when a.den) = what the ratio stage would read for element i: summed partials + centring term

@@ -45,12 +45,13 @@ __device__ __forceinline__ float warp_sum(float p) {
 }
 
 // RPL: rank floats per lane (R <= 32 RPL); WT: the entries carry weights wt (in val's order).  ptr / idx / val: the
-// compressed form whose segments are X's rows; X (nseg x R) is updated in place, F (rows of idx x R) is read.
-template <int RPL, bool WT>
+// compressed form whose segments are X's rows; X (nseg x R) is updated in place, F (rows of idx x R) is read.  FIXED: the
+// components k with fixed[k] != 0 take no step (delta 0), so the residual the later components see is unchanged.
+template <int RPL, bool WT, bool FIXED = false>
 __global__ void __launch_bounds__(256)
 observed_cd_kernel(const int64_t* __restrict__ ptr, const int64_t* __restrict__ idx, const float* __restrict__ val,
                    const float* __restrict__ wt, float* __restrict__ X, const float* __restrict__ F, int R, int64_t nseg,
-                   float* __restrict__ rbuf, float l1, float l2) {
+                   float* __restrict__ rbuf, float l1, float l2, const uint8_t* __restrict__ fixed) {
   const int lane = threadIdx.x & 31;
   const int64_t seg = (int64_t)blockIdx.x * kSegsPerBlock + (threadIdx.x >> 5);
   if (seg >= nseg) return;                       // the whole warp leaves together
@@ -113,7 +114,7 @@ observed_cd_kernel(const int64_t* __restrict__ ptr, const int64_t* __restrict__ 
           float d = 0.f;
           if (lane == k) {
             const float hess = G[k] + l2;
-            if (hess != 0.f) {                   // a dead component keeps its value, as in cd.cu
+            if (hess != 0.f && !(FIXED && fixed[32 * g + k])) {   // a dead or fixed component keeps its value, as in cd.cu
               const float xo = x[g];
               const float xn = fmaxf(0.f, xo + (a - corr - l1 - l2 * xo) / hess);
               x[g] = xn;
@@ -141,25 +142,27 @@ observed_cd_kernel(const int64_t* __restrict__ ptr, const int64_t* __restrict__ 
 int64_t observed_cd_workspace_floats(int R, int64_t nnz) { return R > 32 ? nnz : 0; }
 
 int observed_cd(const int64_t* ptr, const int64_t* idx, const float* val, const float* wt, float* X, const float* F, int R,
-                int64_t nseg, float* rbuf, float l1, float l2, cudaStream_t st) {
+                int64_t nseg, float* rbuf, float l1, float l2, cudaStream_t st, const uint8_t* fixed) {
   if (R < 1 || R > 256) { set_error("observed_cd: rank must be in [1, 256]"); return 1; }
   if (nseg < 1) return 0;
   const int64_t blocks = ceil_div(nseg, (int64_t)kSegsPerBlock);
   if (blocks > kMaxGridX) { set_error("observed_cd: segment blocks pass grid x"); return 1; }
   const unsigned grid = (unsigned)blocks;
   const int rpl = sparse_rpl(R);
-  auto go = [&](auto weighted) {
-    constexpr bool WT = decltype(weighted)::value;
+  auto go = [&](auto weighted, auto with_fixed) {
+    constexpr bool WT = decltype(weighted)::value, FIXED = decltype(with_fixed)::value;
 #define NMF_OCD(RPLV) \
-  observed_cd_kernel<RPLV, WT><<<grid, 256, 0, st>>>(ptr, idx, val, wt, X, F, R, nseg, rbuf, l1, l2)
+  observed_cd_kernel<RPLV, WT, FIXED><<<grid, 256, 0, st>>>(ptr, idx, val, wt, X, F, R, nseg, rbuf, l1, l2, fixed)
     if (rpl <= 1) NMF_OCD(1);
     else if (rpl <= 2) NMF_OCD(2);
     else if (rpl <= 4) NMF_OCD(4);
     else NMF_OCD(8);
 #undef NMF_OCD
   };
-  if (wt) go(std::true_type{});
-  else go(std::false_type{});
+  if (fixed && wt) go(std::true_type{}, std::true_type{});
+  else if (fixed) go(std::false_type{}, std::true_type{});
+  else if (wt) go(std::true_type{}, std::false_type{});
+  else go(std::false_type{}, std::false_type{});
   NMF_LAUNCH_CHECK();
   return 0;
 }

@@ -536,8 +536,11 @@ struct TcApplyArgs {
   const float* peers[kMaxPeers]; int npeers; const unsigned int* flags; unsigned int flag_target; unsigned int* peer_err;
 };
 
+// FIXED (and in the two kernels below): the components r with fixed[r] != 0 are not stored; they keep their value, which
+// enters the column sums and the max as it is.  The instantiations without it compile none of this.
+template <bool FIXED = false>
 __global__ void __launch_bounds__(256)
-tc_apply_kernel(TcApplyArgs a) {
+tc_apply_kernel(TcApplyArgs a, const uint8_t* __restrict__ fixed) {
   __shared__ float sh[2][128];
   const int r = threadIdx.x & 127, rg = threadIdx.x >> 7;
   const int64_t row0 = (int64_t)blockIdx.x * a.rpb;
@@ -546,10 +549,11 @@ tc_apply_kernel(TcApplyArgs a) {
   if (r < a.R) {
     const float klden = (a.apply && !a.den) ? a.kl_den[r] : 1.f;
     const float kap = (a.apply && !a.den) ? *a.kappa : 0.f;
+    const bool upd = a.apply && !(FIXED && fixed[r]);
     for (int64_t row = row0 + rg; row < row1; row += 2) {
       const int64_t idx = row * a.R + r;
       float v = a.param[idx];
-      if (a.apply) {
+      if (upd) {
         float num = 0.f;
         for (int ch = 0; ch < a.nchunks; ++ch) num += a.num[ch * a.chunk_stride + row * a.Rp + r];
         float pos;
@@ -673,9 +677,9 @@ gram_sum_kernel(const float* __restrict__ part, int nb, int nout, float* __restr
 // Row tiles of 64: thread (ty, tx) owns rows 4 ty .. 4 ty + 3 and components TR tx .. TR tx + TR - 1 of the tile.  The tile's
 // old values are staged before anything is overwritten (pitch RP + 1: the four rows of a thread and the two row groups of a
 // warp fall into different banks), the Gram matrix once per block.  Dynamic shared memory: gram RP x RP | tile 64 x (RP + 1).
-template <int TR>
+template <int TR, bool FIXED = false>
 __global__ void __launch_bounds__(256, TR == 4 ? 3 : 1)
-tc_apply_eu_kernel(TcApplyArgs a, const float* __restrict__ gram) {
+tc_apply_eu_kernel(TcApplyArgs a, const float* __restrict__ gram, const uint8_t* __restrict__ fixed) {
   constexpr int RP = 16 * TR, FP = RP + 1;
   extern __shared__ __align__(16) float eu_smem[];
   float* gs = eu_smem;                           // [RP][RP], zero-padded
@@ -774,8 +778,10 @@ tc_apply_eu_kernel(TcApplyArgs a, const float* __restrict__ gram) {
         if (a.l2 > 0.f) pos = fmaf(a.l2, v, pos);                 // nmf.py:87-88
         float mult = neg / pos;                                   // nmf.py:89
         if (a.gamma != 1.0f) mult = powf(mult, a.gamma);          // nmf.py:90-91 (gamma == 1 for beta 2)
-        v *= mult;                                                // nmf.py:92
-        a.param[row * R + r] = v;
+        if (!(FIXED && fixed[r])) {
+          v *= mult;                                              // nmf.py:92
+          a.param[row * R + r] = v;
+        }
         cs[j] += v;
         mx = fmaxf(mx, v);
       }
@@ -953,9 +959,9 @@ __device__ __forceinline__ void wait_peer_flags(const unsigned int* flags, int n
   __syncthreads();
 }
 
-template <bool SPLIT>
+template <bool SPLIT, bool FIXED = false>
 __global__ void __launch_bounds__(256)
-tc_apply_finish_kernel(TcApplyArgs a, TcFinishArgs f) {
+tc_apply_finish_kernel(TcApplyArgs a, TcFinishArgs f, const uint8_t* __restrict__ fixed) {
   __shared__ float4 sh[256];
   const int lanes = a.R >> 2;                    // threads per row
   const int rows_per_pass = 256 / lanes;
@@ -973,6 +979,11 @@ tc_apply_finish_kernel(TcApplyArgs a, TcFinishArgs f) {
     if (a.apply && !a.den) {
       kd = peer ? sum_peers4(a.peers, a.npeers, RR + 4 * q) : *reinterpret_cast<const float4*>(a.kl_den + 4 * q);
       kap = *a.kappa;
+    }
+    bool fx[4] = {false, false, false, false};               // this thread's four components: fixed ones are not stored
+    if constexpr (FIXED) {
+#pragma unroll
+      for (int i = 0; i < 4; ++i) fx[i] = fixed[4 * q + i] != 0;
     }
     for (int64_t row = row0 + rl; row < row1; row += rows_per_pass) {
       float4* pp = reinterpret_cast<float4*>(a.param + row * a.R) + q;
@@ -994,10 +1005,16 @@ tc_apply_finish_kernel(TcApplyArgs a, TcFinishArgs f) {
           if (a.l2 > 0.f) pos = fmaf(a.l2, vv[i], pos);             // nmf.py:87-88
           float mult = neg / pos;                                   // nmf.py:89
           if (a.gamma != 1.0f) mult = powf(mult, a.gamma);          // nmf.py:90-91
-          vv[i] *= mult;                                            // nmf.py:92
+          if (!fx[i]) vv[i] *= mult;                                // nmf.py:92
         }
         v = make_float4(vv[0], vv[1], vv[2], vv[3]);
-        *pp = v;
+        if constexpr (FIXED) {
+#pragma unroll
+          for (int i = 0; i < 4; ++i)
+            if (!fx[i]) a.param[row * a.R + 4 * q + i] = vv[i];
+        } else {
+          *pp = v;
+        }
       }
       cs.x += v.x; cs.y += v.y; cs.z += v.z; cs.w += v.w;
       mx = fmaxf(fmaxf(mx, fmaxf(v.x, v.y)), fmaxf(v.z, v.w));
@@ -1310,6 +1327,7 @@ struct TcState {
   double exps_beta = 1.0;           // the beta exps[4] / exps[5] were last published for
   float* zero = nullptr;           // device scalar 0 (kappa of an already complete numerator)
   int coop_blocks = 0;              // co-resident blocks of the fused tail kernel (cooperative launch), 0 = unavailable
+  int coop_blocks_fixed = 0;        // the same for its instantiation with fixed components (its own register count)
 };
 
 bool tc_shape_supported(int64_t N, int64_t C, int64_t R) {
@@ -1350,14 +1368,17 @@ int tc_create(TcState** out, int device, int64_t N, int64_t C, int64_t R, bool s
   s->num_sms = prop.multiProcessorCount;
   if (prop.major != 9) { delete s; set_error("the tensor-core path needs an sm_90 device"); return 1; }
   {
-    int coop = 0, per_sm = 0;
+    int coop = 0;
     cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, device);
-    const void* fn = split ? (const void*)tc_apply_finish_kernel<true> : (const void*)tc_apply_finish_kernel<false>;
-    if (coop && cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, 256, 0) == cudaSuccess && per_sm > 0) {
+    auto coop_blocks = [&](const void* fn) {
+      int per_sm = 0;
+      if (!coop || cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, 256, 0) != cudaSuccess || per_sm < 1) return 0;
       if (per_sm > 4) per_sm = 4;                            // enough loads in flight to stream the partials
-      s->coop_blocks = per_sm * s->num_sms;
-      if (s->coop_blocks > 1024) s->coop_blocks = 1024;      // cs_part capacity
-    }
+      return std::min(per_sm * s->num_sms, 1024);            // cs_part capacity
+    };
+    s->coop_blocks = coop_blocks(split ? (const void*)tc_apply_finish_kernel<true> : (const void*)tc_apply_finish_kernel<false>);
+    s->coop_blocks_fixed = coop_blocks(split ? (const void*)tc_apply_finish_kernel<true, true>
+                                             : (const void*)tc_apply_finish_kernel<false, true>);
   }
   s->plan_w = make_plan(C, N, s->num_sms, s->TN);
   s->plan_h = make_plan(N, C, s->num_sms, s->TN);
@@ -1464,7 +1485,8 @@ namespace {
 // buffer [rows*R num | R colsum or rows*R den] instead of this rank's chunked partials.
 int apply_and_finish(TcState* s, int which, float* param, bool apply, const Plan* pl, double beta, double gamma,
                      double l1, double l2, cudaStream_t st, const float* reduced = nullptr,
-                     const float* other = nullptr, bool peer = false) {
+                     const float* other = nullptr, bool peer = false, const uint8_t* fixed = nullptr) {
+  if (fixed && (!apply || peer)) { set_error("internal: fixed components need a local ratio stage"); return 1; }
   const int64_t rows = which == 0 ? s->C : s->N;
   int rpb = (int)round_up(ceil_div(rows, 1024), 4);
   if (rpb < 64) rpb = 64;
@@ -1494,11 +1516,12 @@ int apply_and_finish(TcState* s, int which, float* param, bool apply, const Plan
     a.flag_target = s->peer_iter; a.peer_err = s->peer_err;
   }
   s->exps_beta = beta;                 // both branches below end in publish_scales at this beta
-  if ((s->R & 3) == 0 && s->coop_blocks > 0 && !(apply && beta == 2.0 && !reduced)) {
+  const int coop_blocks = fixed ? s->coop_blocks_fixed : s->coop_blocks;
+  if ((s->R & 3) == 0 && coop_blocks > 0 && !(apply && beta == 2.0 && !reduced)) {
     // one cooperative launch: ratio stage, grid barrier, operand copy + scalars
     const int lanes = (int)s->R >> 2, rows_per_pass = 256 / lanes;
     int64_t g = ceil_div(rows, rows_per_pass);
-    if (g > s->coop_blocks) g = s->coop_blocks;
+    if (g > coop_blocks) g = coop_blocks;
     a.rpb = (int)round_up(ceil_div(rows, g), rows_per_pass);
     const int gblocks = (int)ceil_div(rows, a.rpb);
     TcFinishArgs f{};
@@ -1506,8 +1529,10 @@ int apply_and_finish(TcState* s, int which, float* param, bool apply, const Plan
     f.exps = s->exps; f.which = which; f.colsum = s->colsum; f.vconst = s->vconst; f.kappa = s->kappa;
     f.bm1 = (float)(beta - 1.0); f.bm2 = (float)(beta - 2.0);
     f.cells = (double)s->N * (double)s->C;
-    void* args[2] = {&a, &f};
-    const void* fn = s->split ? (const void*)tc_apply_finish_kernel<true> : (const void*)tc_apply_finish_kernel<false>;
+    void* args[3] = {&a, &f, &fixed};
+    const void* fn = fixed ? (s->split ? (const void*)tc_apply_finish_kernel<true, true>
+                                       : (const void*)tc_apply_finish_kernel<false, true>)
+                           : (s->split ? (const void*)tc_apply_finish_kernel<true> : (const void*)tc_apply_finish_kernel<false>);
     NMF_CUDA_CHECK(cudaLaunchCooperativeKernel(fn, dim3(gblocks), dim3(256), args, 0, st));
     count_launch();
     return 0;
@@ -1532,17 +1557,23 @@ int apply_and_finish(TcState* s, int which, float* param, bool apply, const Plan
     const int RPk = s->Rp == 64 ? 64 : 128;
     const int eu_smem = (RPk * RPk + 64 * (RPk + 1)) * (int)sizeof(float);
     if (RPk == 64) {
-      tc_apply_eu_kernel<4><<<blocks, 256, eu_smem, st>>>(a, s->gram);
+      if (fixed) tc_apply_eu_kernel<4, true><<<blocks, 256, eu_smem, st>>>(a, s->gram, fixed);
+      else tc_apply_eu_kernel<4><<<blocks, 256, eu_smem, st>>>(a, s->gram, nullptr);
     } else {
-      static unsigned long long eu_attr_mask = 0;                    // > 48 KB of dynamic shared memory: opt in once per device
-      if (!((eu_attr_mask >> (s->device & 63)) & 1ull)) {
-        NMF_CUDA_CHECK(cudaFuncSetAttribute(tc_apply_eu_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, eu_smem));
-        eu_attr_mask |= 1ull << (s->device & 63);
+      // > 48 KB of dynamic shared memory: opt in once per device and instantiation
+      static unsigned long long eu_attr_mask[2] = {0, 0};
+      const auto kern = fixed ? tc_apply_eu_kernel<8, true> : tc_apply_eu_kernel<8>;
+      unsigned long long& mask = eu_attr_mask[fixed ? 1 : 0];
+      if (!((mask >> (s->device & 63)) & 1ull)) {
+        NMF_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, eu_smem));
+        mask |= 1ull << (s->device & 63);
       }
-      tc_apply_eu_kernel<8><<<blocks, 256, eu_smem, st>>>(a, s->gram);
+      kern<<<blocks, 256, eu_smem, st>>>(a, s->gram, fixed);
     }
+  } else if (fixed) {
+    tc_apply_kernel<true><<<blocks, 256, 0, st>>>(a, fixed);
   } else {
-    tc_apply_kernel<<<blocks, 256, 0, st>>>(a);
+    tc_apply_kernel<<<blocks, 256, 0, st>>>(a, nullptr);
   }
   NMF_LAUNCH_CHECK();
   __half* out = which == 0 ? s->W16 : s->H16;
@@ -1691,7 +1722,7 @@ void tc_plan(int64_t N, int64_t C, int64_t R, bool split, int num_sms, int64_t* 
 }
 
 int tc_update(TcState* s, int which, float* param, const float* W, const float* H, double beta, double gamma, double l1,
-              double l2, cudaStream_t st) {
+              double l2, cudaStream_t st, const uint8_t* fixed) {
   // tc_loss_prefetch_w already ran the W contraction on these very factors (its numerators are still in `part`)
   const bool reuse = which == 0 && s->w_pending && !s->dirty_w && !s->dirty_h && beta == 1.0;
   s->w_pending = false;
@@ -1702,7 +1733,7 @@ int tc_update(TcState* s, int which, float* param, const float* W, const float* 
     if (rc) return rc;
   }
   return apply_and_finish(s, which, param, true, which == 0 ? &s->plan_w : &s->plan_h, beta, gamma, l1, l2, st, nullptr,
-                          which == 0 ? H : W);
+                          which == 0 ? H : W, false, fixed);
 }
 
 // Raw update terms of one factor (which = 0: W, 1: H) in one dense buffer: numerator (rows x R; chunk sums, + kappa
@@ -1727,9 +1758,9 @@ int tc_raw_terms(TcState* s, int which, const float* W, const float* H, double b
 // Sharded W update, second half: nmf.py:78-92 on the all-reduced buffer with the tensor-core path's own ratio-stage
 // kernels, which also rebuild W16 / colsum(W) / exponents (no separate resync pass).
 int tc_w_apply(TcState* s, float* W, const float* reduced, double beta, double gamma, double l1, double l2,
-               cudaStream_t st) {
+               cudaStream_t st, const uint8_t* fixed) {
   if (!s->has_target) { set_error("tensor-core path: set_target has not been called"); return 3; }
-  int rc = apply_and_finish(s, 0, W, true, nullptr, beta, gamma, l1, l2, st, reduced);
+  int rc = apply_and_finish(s, 0, W, true, nullptr, beta, gamma, l1, l2, st, reduced, nullptr, false, fixed);
   if (rc == 0) s->dirty_w = false;
   return rc;
 }

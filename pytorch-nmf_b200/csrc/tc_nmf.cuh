@@ -25,13 +25,14 @@ int tc_target_lossy(TcState* s, unsigned long long* count, cudaStream_t st);
 int tc_target_sum(TcState* s, double* vsum, cudaStream_t st);
 // the fp32 factor changed outside the tensor-core path: operand copies must be rebuilt before use
 void tc_mark_dirty(TcState* s, bool w, bool h);
-// one factor update in place (which = 0: param = W, 1: param = H)
+// one factor update in place (which = 0: param = W, 1: param = H).  fixed (R bytes; null: none): the ratio stage does not
+// store the components with fixed[r] != 0, which keep their value and enter the operand copy, column sums and scale as such.
 int tc_update(TcState* s, int which, float* param, const float* W, const float* H, double beta, double gamma, double l1,
-              double l2, cudaStream_t st);
+              double l2, cudaStream_t st, const uint8_t* fixed = nullptr);
 // raw terms of either factor's update (which = 0: W, 1: H): [numerator rows x R | colsum(other) R (beta 1) or denominator rows x R]
 int tc_raw_terms(TcState* s, int which, const float* W, const float* H, double beta, float* out, cudaStream_t st);
 int tc_w_apply(TcState* s, float* W, const float* reduced, double beta, double gamma, double l1, double l2,
-               cudaStream_t st);
+               cudaStream_t st, const uint8_t* fixed = nullptr);
 // row-sharded W update over peer memory (one NVLink domain, 2 to 8 ranks): allocate this rank's exchange block and export its
 // 64-byte CUDA IPC handle; open the other ranks' blocks (`handles`: world x 64 bytes, in rank order); then every rank calls
 // tc_update_w_peer for every W update (collective).  tc_peer_check: > 0 if a kernel gave up waiting for a rank.

@@ -8,7 +8,8 @@ namespace {
 // Where the partials of element idx (of problem b) are: the offset in the first slab, the slab count and stride.  False for
 // a padding row of a ragged batch's H, or (LINES) a padding position of a ragged NMFD batch's H lines, which no kernel
 // writes.  The kernels below take RAGGED (a.rag set) and LINES (a.line set as well) as template flags, so that their other
-// instantiations run the code they always ran.
+// instantiations run the code they always ran.  The ratio-stage kernels take FIXED the same way: `fixed` (R bytes, non-zero
+// for a component held at its value, nmfb200_set_fixed_w) predicates the final store of each element on its component.
 struct PartialAt { int64_t off, stride; int nch; };
 template <bool RAGGED, bool LINES = false>
 __device__ __forceinline__ bool partial_at(const ApplyArgs& a, int64_t idx, int64_t b, PartialAt& p) {
@@ -32,9 +33,9 @@ __device__ __forceinline__ bool partial_at(const ApplyArgs& a, int64_t idx, int6
   return true;
 }
 
-template <bool RAGGED, bool LINES = false>
+template <bool RAGGED, bool LINES = false, bool FIXED = false>
 __global__ void __launch_bounds__(256)
-apply_update_kernel(ApplyArgs a) {
+apply_update_kernel(ApplyArgs a, const uint8_t* __restrict__ fixed) {
   const int64_t idx = (int64_t)blockIdx.x * 256 + threadIdx.x;
   float newv = 0.f;
   const int64_t b = a.prob_numel ? idx / a.prob_numel : 0;      // Batch: the element's problem
@@ -63,7 +64,8 @@ apply_update_kernel(ApplyArgs a) {
     float mult = neg / pos;                                  // nmf.py:89
     if (a.gamma != 1.0f) mult = powf(mult, a.gamma);         // nmf.py:90-91
     newv = p * mult;                                         // nmf.py:92
-    a.param[idx] = newv;
+    if (FIXED && fixed[r]) newv = p;                         // a fixed component keeps its value and still enters absmax
+    else a.param[idx] = newv;
   }
   if (a.absmax_bits) {          // one atomic per block: tens of thousands of same-address atomics serialise in L2
     __shared__ float wmax[8];
@@ -281,9 +283,9 @@ __global__ void minmax_stage2(const float* __restrict__ scratch, int nb, float* 
 
 // Four consecutive elements per thread (same row, same component: inner % 4 == 0), 16-byte loads of the parameter and of every
 // partial slab.  Same arithmetic per element as apply_update_kernel.
-template <bool RAGGED>
+template <bool RAGGED, bool FIXED = false>
 __global__ void __launch_bounds__(256)
-apply_update_vec4_kernel(ApplyArgs a) {
+apply_update_vec4_kernel(ApplyArgs a, const uint8_t* __restrict__ fixed) {
   const int64_t idx = ((int64_t)blockIdx.x * 256 + threadIdx.x) * 4;
   float m = 0.f;
   const int64_t b = a.prob_numel ? idx / a.prob_numel : 0;      // Batch: prob_numel is a multiple of 4 here
@@ -317,8 +319,10 @@ apply_update_vec4_kernel(ApplyArgs a) {
       if (a.gamma != 1.0f) mult = powf(mult, a.gamma);         // nmf.py:90-91
       return pv * mult;                                        // nmf.py:92
     };
-    p.x = one(p.x, num.x, den.x); p.y = one(p.y, num.y, den.y); p.z = one(p.z, num.z, den.z); p.w = one(p.w, num.w, den.w);
-    *reinterpret_cast<float4*>(a.param + idx) = p;
+    if (!(FIXED && fixed[r])) {                                // the four elements share component r
+      p.x = one(p.x, num.x, den.x); p.y = one(p.y, num.y, den.y); p.z = one(p.z, num.z, den.z); p.w = one(p.w, num.w, den.w);
+      *reinterpret_cast<float4*>(a.param + idx) = p;
+    }
     m = fmaxf(fmaxf(p.x, p.y), fmaxf(p.z, p.w));
   }
   if (a.absmax_bits) {
@@ -340,15 +344,18 @@ bool apply_update_vec4_shape(const ApplyArgs& a) {
          (a.nchunks == 1 || a.chunk_stride % 4 == 0) && a.prob_numel % 4 == 0 && a.line == 0;
 }
 
-int apply_update(const ApplyArgs& a, cudaStream_t st) {
+int apply_update(const ApplyArgs& a, cudaStream_t st, const uint8_t* fixed) {
   if (a.numel <= 0) return 0;
+  if (fixed && (a.rag || a.prob_numel)) { set_error("apply_update: fixed components need a single problem"); return 1; }
   const bool vec4 = apply_update_vec4_shape(a) && aligned16(a.param) && aligned16(a.num) && (!a.den || aligned16(a.den));
   const unsigned g4 = (unsigned)ceil_div(a.numel / 4, 256), g1 = (unsigned)ceil_div(a.numel, 256);
-  if (vec4 && a.rag) apply_update_vec4_kernel<true><<<g4, 256, 0, st>>>(a);
-  else if (vec4) apply_update_vec4_kernel<false><<<g4, 256, 0, st>>>(a);
-  else if (a.rag && a.line) apply_update_kernel<true, true><<<g1, 256, 0, st>>>(a);
-  else if (a.rag) apply_update_kernel<true><<<g1, 256, 0, st>>>(a);
-  else apply_update_kernel<false><<<g1, 256, 0, st>>>(a);
+  if (fixed && vec4) apply_update_vec4_kernel<false, true><<<g4, 256, 0, st>>>(a, fixed);
+  else if (fixed) apply_update_kernel<false, false, true><<<g1, 256, 0, st>>>(a, fixed);
+  else if (vec4 && a.rag) apply_update_vec4_kernel<true><<<g4, 256, 0, st>>>(a, nullptr);
+  else if (vec4) apply_update_vec4_kernel<false><<<g4, 256, 0, st>>>(a, nullptr);
+  else if (a.rag && a.line) apply_update_kernel<true, true><<<g1, 256, 0, st>>>(a, nullptr);
+  else if (a.rag) apply_update_kernel<true><<<g1, 256, 0, st>>>(a, nullptr);
+  else apply_update_kernel<false><<<g1, 256, 0, st>>>(a, nullptr);
   NMF_LAUNCH_CHECK();
   return 0;
 }

@@ -230,6 +230,19 @@ class _CudaEngine:
         self._mask, self._weight = None, Wt
         _capi.check(self._lib.nmfb200_set_weight(self._ctx, _ptr(Wt) if Wt is not None else None, _stream(self.device)))
 
+    def set_fixed_w(self, fixed):
+        """Hold the components k of W with fixed[k] != 0 at their values from now on (include/nmf_b200.h:
+        nmfb200_set_fixed_w): fixed is a contiguous uint8 tensor of R elements on the engine's device, read in place by every
+        later W update; None clears it.  The engine keeps a reference to it while it is set."""
+        if fixed is not None:
+            if fixed.dtype != torch.uint8 or fixed.device != self.device or not fixed.is_contiguous():
+                raise ValueError("fixed must be a contiguous uint8 tensor on the engine's device")
+            if fixed.numel() != self.W.shape[1]:
+                raise ValueError(f"fixed has {fixed.numel()} elements for W's {self.W.shape[1]} components")
+        self._fixed_w = fixed
+        _capi.check(self._lib.nmfb200_set_fixed_w(self._ctx, _ptr(fixed) if fixed is not None else None,
+                                                  _stream(self.device)))
+
     def minmax(self):
         vmin, vmax = ctypes.c_float(), ctypes.c_float()
         _capi.check(self._lib.nmfb200_target_minmax(self._ctx, ctypes.byref(vmin), ctypes.byref(vmax),

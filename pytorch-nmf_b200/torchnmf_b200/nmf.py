@@ -153,6 +153,24 @@ def _weight_values_ok(w):
 _NO_CUDA = "torchnmf_b200.fit needs a CUDA device (sm_90a); there is no CPU fallback"
 
 
+def _checked_fixed_w(W, fixed_W, group):
+    """The checks of a `fit(..., fixed_W=F)` argument for the module's W, before any device work: ValueError for a
+    `fixed_W` that is not a dense torch.bool tensor of one flag per component, for a W that is not trainable and for
+    `group`.  Returns None when no component is fixed (the plain fit), else `fixed_W` itself."""
+    if fixed_W is None or W is None:                # no W: fit()'s own assertion reports it
+        return None
+    R = W.shape[1]
+    if not isinstance(fixed_W, Tensor) or fixed_W.dtype != torch.bool or fixed_W.layout != torch.strided:
+        raise ValueError(f"fixed_W must be a dense torch.bool tensor (got {getattr(fixed_W, 'dtype', type(fixed_W))})")
+    if tuple(fixed_W.shape) != (R,):
+        raise ValueError(f"fixed_W must hold one flag per component of W: shape ({R},) (got {tuple(fixed_W.shape)})")
+    if not W.requires_grad:
+        raise ValueError("fixed_W: W is not trainable (trainable_W=False); every component is already fixed")
+    if group is not None:
+        raise ValueError("fixed_W does not run sharded fits (group)")
+    return fixed_W if bool(fixed_W.any()) else None
+
+
 class BaseComponent(torch.nn.Module):
     """Base class of the NMF modules (reference: nmf.py:173-292).
 
@@ -499,12 +517,26 @@ class BaseComponent(torch.nn.Module):
                    beta != 2, a dense `mask` or `weight` (pass `mask.to_sparse()`: a dense one would need a Gram matrix
                    per row), `group`, precision "f16" / "f16_split", rank > 256, an unknown solver, and NMFD / NMF2D /
                    NMF3D.
+
+        fixed_W:   (keyword-only, default None, through **options like `mask`) a torch.bool tensor of R elements, on any
+                   device: the components k where it is True keep W[:, k] (W[:, k, ...] for NMFD / NMF2D / NMF3D) at its
+                   value, for semi-supervised separation (Mysore and Smaragdis 2011): a dictionary learned for a known
+                   source stays fixed while the free components learn the rest of the target.  The free components take
+                   exactly the update they take without it, with the reconstruction formed from all R components: the
+                   multiplicative ratio (`alpha` / `l1_ratio` penalise the free components only, since the fixed ones are
+                   not updated), or with solver="cd" the sweep over k = 0 .. R-1 that skips each fixed k, so later columns
+                   see its unchanged value (block coordinate descent on the free components).  H is learned for every
+                   component.  Every component fixed is the fit of trainable_W=False, bit for bit; none fixed is the plain
+                   fit.  Every target form, precision and solver above is covered.  ValueError, before any device work: a
+                   `fixed_W` that is not a dense torch.bool tensor of shape (R,), a W that is not trainable, and `group`.
         """
         mask = options.pop("mask", None)
         weight = options.pop("weight", None)
         solver = options.pop("solver", "mu")
+        fixed_W = options.pop("fixed_W", None)
         if options:
             raise TypeError(f"fit() got an unexpected keyword argument {next(iter(options))!r}")
+        fixed_W = _checked_fixed_w(self.W, fixed_W, group)
         if solver not in ("mu", "cd"):
             raise ValueError(f"solver must be 'mu' or 'cd' (got {solver!r})")
         cd = solver == "cd"
@@ -537,6 +569,10 @@ class BaseComponent(torch.nn.Module):
                 l1_reg = alpha * l1_ratio                                                  # nmf.py:348
                 l2_reg = alpha * (1 - l1_ratio)                                            # nmf.py:349
                 train_w, train_h = W.requires_grad, H.requires_grad
+                if fixed_W is not None and bool(fixed_W.all()):
+                    train_w = False                     # every component fixed: the fit of trainable_W=False
+                elif fixed_W is not None:
+                    eng.set_fixed_w(fixed_W.to(dev, torch.uint8).contiguous())
 
                 def divergence(follows):
                     # a W update follows on these very factors: the engine may take the loss out of that update's own

@@ -24,7 +24,7 @@ from torch.nn import Parameter
 
 from .constants import eps
 from . import engine as _engine
-from .nmf import (_batched_conv, _check_lengths, _fit_problems, _fit_single, _placed_factors,
+from .nmf import (_batched_conv, _check_lengths, _checked_fixed_w, _fit_problems, _fit_single, _placed_factors,
                   _register_batched_factors)
 
 from torch.nn.modules.utils import _single, _pair, _triple
@@ -116,7 +116,7 @@ class BaseComponent(torch.nn.Module):
 
     @torch.no_grad()
     def fit(self, V, tol=1e-4, max_iter=200, verbose=False, W_alpha=1., H_alpha=1., Z_alpha=1., *, precision="f32",
-            mask=None, group=None):
+            mask=None, group=None, fixed_W=None):
         """EM fit of the PLCA model (reference: plca.py:193-304; same arguments, stop rule and return value
         `(n_iter, norm)`).  Runs on the parameters' CUDA device; host-resident modules are staged like `NMF.fit`.
 
@@ -170,13 +170,24 @@ class BaseComponent(torch.nn.Module):
                    target whose shards all sum to 0.  ValueError for `mask` with `group`.  Not covered: masked fits,
                    the batched classes (which take no `group`), a peer-memory (NVLink) exchange, and (NMF) sharded
                    sparse targets without densifying.
+
+        fixed_W:   (keyword-only, default None) a torch.bool tensor of R elements, on any device: the components k where it
+                   is True keep W[:, k] (W[:, k, ...] for the shift-invariant models) at its value, for semi-supervised
+                   separation (Smaragdis, Raj and Shashanka 2007): a dictionary learned for a known source stays fixed while
+                   the free components learn the rest of the target.  Each EM step applies W's update -- the
+                   multiplicative step, its normalisation and W_alpha's prior -- to the free components only, with the
+                   same bits as without `fixed_W`; H and Z are learned for every component, Z from the gradient over all of
+                   them.  Every component fixed is the fit of trainable_W=False; none fixed is the plain fit.  Dense,
+                   sparse and masked targets alike.  ValueError, before any device work: a `fixed_W` that is not a dense
+                   torch.bool tensor of shape (R,), a W that is not trainable, and `group`.
         """
+        fixed_W = _checked_fixed_w(self.W, fixed_W, group)
         if mask is not None:
             if group is not None:
                 raise ValueError(f"group: {type(self).__name__}.fit does not run masked fits sharded (mask with group)")
-            return self._fit_masked(V, mask, tol, max_iter, verbose, W_alpha, H_alpha, Z_alpha, precision)
+            return self._fit_masked(V, mask, tol, max_iter, verbose, W_alpha, H_alpha, Z_alpha, precision, fixed_W)
         if V.layout != torch.strided:
-            return self._fit_sparse(V, tol, max_iter, verbose, W_alpha, H_alpha, Z_alpha, precision, group)
+            return self._fit_sparse(V, tol, max_iter, verbose, W_alpha, H_alpha, Z_alpha, precision, group, fixed_W)
         if group is None:
             assert torch.all(V >= 0.), "Target should be non-negative."                     # plca.py:236
         W, H, Z = self.W, self.H, self.Z
@@ -198,6 +209,7 @@ class BaseComponent(torch.nn.Module):
 
             Hz = (Hd * _over(Zd, Hd)).contiguous()        # the engine's activation factor: H diag(Z)
             buf = _terms_buffer(ops, Wd)
+            wfix = _w_fixing(self.W, fixed_W, dev)
             eng = self._engine(Vn, Wd, Hz, precision) if self._engine_factory is None else self._engine_factory(Vn, Wd, Hz)
             try:
                 def step(k):
@@ -207,7 +219,7 @@ class BaseComponent(torch.nn.Module):
                         dW, _ = eng.raw_terms(0, 1.0)     # P contracted with H Z  = W.grad   (plca.py:252-253)
                         dHz, _ = eng.raw_terms(1, 1.0)    # P contracted with W;  H.grad = dHz * Z,  Z.grad = sum H dHz
                         dW, dZ = _em_terms(ops, Hd, dW, dHz, buf)
-                        self._em_update(Wd, Hd, Zd, dW, dHz, dZ, W_alpha, H_alpha, Z_alpha, ops)
+                        self._em_update(Wd, Hd, Zd, dW, dHz, dZ, W_alpha, H_alpha, Z_alpha, ops, *wfix)
 
                 n_iter = _fit_single(step, divergence, max_iter, tol, verbose)
                 eng.check_health()
@@ -249,11 +261,16 @@ class BaseComponent(torch.nn.Module):
         total = ops.all_reduce_(norm.to(ops.device, torch.float64).reshape(1))
         return total[0].to(norm.device, norm.dtype)
 
-    def _em_update(self, Wd, Hd, Zd, dW, dHz, dZ, W_alpha, H_alpha, Z_alpha, ops=None):
+    def _em_update(self, Wd, Hd, Zd, dW, dHz, dZ, W_alpha, H_alpha, Z_alpha, ops=None, train_w=None, fixed=None):
         """The Z, W and H updates of one EM step (plca.py:256-288) from the raw gradients dW, dHz (= H.grad / Z) and
         dZ (= Z.grad, `_em_terms`), in place on the working copies, each taken only where the module's factor is
-        trainable.  With `ops` (a sharded fit's Collectives: dW and dZ already summed over the ranks) the two divisions
-        by H's column sums take them over every rank's rows, one R-float all-reduce each."""
+        trainable (`train_w`, when given, in place of W's flag).  With `ops` (a sharded fit's Collectives: dW and dZ
+        already summed over the ranks) the two divisions by H's column sums take them over every rank's rows, one R-float
+        all-reduce each.  `fixed` (the indices of W's fixed components, on its device): those components keep their
+        values; every step of W's update acts on each component alone, so the free ones take the bits they take without
+        it, and the column masses H divides by with Z frozen are those of the whole step, as W's gradient gives them."""
+        if train_w is None:
+            train_w = self.W.requires_grad
         h_norm = get_norm if ops is None else (lambda x: ops.all_reduce_(get_norm(x)))
         dH = dHz * _over(Zd, Hd)
         Z_prior = None
@@ -264,7 +281,8 @@ class BaseComponent(torch.nn.Module):
                 Zd.add_(_as(Z_alpha, Zd) - 1)
                 F.threshold(Zd, eps, eps, True)
             Zd.div_(Zd.sum())
-        if self.W.requires_grad:                                                             # plca.py:264-275
+        if train_w:                                                                          # plca.py:264-275
+            kept = Wd.index_select(1, fixed) if fixed is not None else None
             Wd.mul_(dW.clamp_min(0))
             if Z_prior is None:
                 W_div = get_norm(Wd)
@@ -276,6 +294,8 @@ class BaseComponent(torch.nn.Module):
                 Wd.add_(_as(W_alpha, Wd) - 1)
                 F.threshold(Wd, eps, eps, True)
                 Wd.div_(get_norm(Wd))
+            if fixed is not None:
+                Wd.index_copy_(1, fixed, kept)
         if self.H.requires_grad:                                                             # plca.py:277-288
             Hd.mul_(dH.clamp_min(0))
             H_div = h_norm(Hd) if Z_prior is None else _over(Z_prior, Hd)
@@ -306,7 +326,7 @@ class BaseComponent(torch.nn.Module):
             raise ValueError("mask: the observed cells of the target sum to 0")
         return M, norm_o
 
-    def _fit_masked(self, V, mask, tol, max_iter, verbose, W_alpha, H_alpha, Z_alpha, precision):
+    def _fit_masked(self, V, mask, tol, max_iter, verbose, W_alpha, H_alpha, Z_alpha, precision, fixed_W=None):
         """fit(V, ..., mask=mask): EM with the missing cells latent (see fit)."""
         M, norm_o = self._check_mask(V, mask, precision)
         W, H, Z = self.W, self.H, self.Z
@@ -329,6 +349,7 @@ class BaseComponent(torch.nn.Module):
 
             Hz = (Hd * _over(Zd, Hd)).contiguous()
             qobs = torch.zeros(1, dtype=torch.float64, device=dev)
+            wfix = _w_fixing(self.W, fixed_W, dev)
             eng = self._engine(Vn, Wd, Hz, precision) if self._engine_factory is None else self._engine_factory(Vn, Wd, Hz)
             try:
                 eng.set_mask(Md)
@@ -343,7 +364,7 @@ class BaseComponent(torch.nn.Module):
                         q = qobs.to(f32)
                         dHz = torch.addcmul(bH, aH, q)
                         dW, dZ = _em_terms(None, Hd, torch.addcmul(bW, aW, q), dHz)
-                        self._em_update(Wd, Hd, Zd, dW, dHz, dZ, W_alpha, H_alpha, Z_alpha)
+                        self._em_update(Wd, Hd, Zd, dW, dHz, dZ, W_alpha, H_alpha, Z_alpha, None, *wfix)
 
                 n_iter = _fit_single(step, divergence, max_iter, tol, verbose)
                 eng.check_health()
@@ -355,7 +376,7 @@ class BaseComponent(torch.nn.Module):
             qo = torch.where(Md, q, 0.).sum()
         return n_iter, (norm_o.double() / qo.to(norm_o.device)).to(norm_o.dtype)
 
-    def _fit_sparse(self, V, tol, max_iter, verbose, W_alpha, H_alpha, Z_alpha, precision, group):
+    def _fit_sparse(self, V, tol, max_iter, verbose, W_alpha, H_alpha, Z_alpha, precision, group, fixed_W=None):
         raise NotImplementedError(f"{type(self).__name__}.fit takes dense targets only (PLCA fits sparse COO targets)")
 
     # test hook, as the NMF modules' (tests/test_plca.py): factory(Vn, W, Hz) stands in for `_engine`
@@ -364,6 +385,17 @@ class BaseComponent(torch.nn.Module):
     @staticmethod
     def _engine(Vn, W, Hz, precision):
         raise NotImplementedError
+
+
+def _w_fixing(W, fixed_W, dev):
+    """`_em_update`'s (train_w, fixed) for a fit's checked `fixed_W` (`_checked_fixed_w`): W's own flag and no fixed
+    component; False when every component is fixed (the fit of trainable_W=False); else the indices of the fixed components
+    on the device `dev`, found once per fit (indexing by the flags would synchronise with the host at every step)."""
+    if fixed_W is None:
+        return W.requires_grad, None
+    if bool(fixed_W.all()):
+        return False, None
+    return True, fixed_W.nonzero().reshape(-1).to(dev)
 
 
 def _over(z, x):
@@ -424,7 +456,7 @@ class PLCA(BaseComponent):
     def _engine(Vn, W, Hz, precision):
         return _engine.CudaNmfEngine(Vn, W, Hz, precision)
 
-    def _fit_sparse(self, V, tol, max_iter, verbose, W_alpha, H_alpha, Z_alpha, precision, group):
+    def _fit_sparse(self, V, tol, max_iter, verbose, W_alpha, H_alpha, Z_alpha, precision, group, fixed_W=None):
         """fit(V) for a sparse COO V: the EM fit of V.to_dense() without forming anything of size N x C (see `fit`)."""
         if V.layout != torch.sparse_coo:
             raise ValueError(f"PLCA.fit takes a dense or a sparse COO target (got layout {V.layout})")
@@ -462,6 +494,7 @@ class PLCA(BaseComponent):
             normf = float(normd)
             Hz = (Hd * _over(Zd, Hd)).contiguous()
             buf = _terms_buffer(ops, Wd)
+            wfix = _w_fixing(self.W, fixed_W, dev)
             eng = _engine.CudaSparsePlcaEngine(Vn, Wd, Hz) if self._engine_factory is None else self._engine_factory(Vn, Wd, Hz)
             try:
                 def divergence(follows):
@@ -473,7 +506,7 @@ class PLCA(BaseComponent):
                         torch.mul(Hd, _over(Zd, Hd), out=Hz)
                         dW, dHz = eng.plca_terms(Hz)        # one ratio P per stored entry serves both gradients
                         dW, dZ = _em_terms(ops, Hd, dW, dHz, buf)
-                        self._em_update(Wd, Hd, Zd, dW, dHz, dZ, W_alpha, H_alpha, Z_alpha, ops)
+                        self._em_update(Wd, Hd, Zd, dW, dHz, dZ, W_alpha, H_alpha, Z_alpha, ops, *wfix)
 
                 n_iter = _fit_single(step, divergence, max_iter, tol, verbose)
                 eng.check_health()
