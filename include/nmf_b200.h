@@ -517,6 +517,30 @@ int nmfb200_set_weight(nmfb200_ctx* ctx, const float* Wt, void* stream);
  * H updates are unaffected, and nmf_peer_supported reports 0 while it is set.  Queues nothing. */
 int nmfb200_set_fixed_w(nmfb200_ctx* ctx, const uint8_t* fixed, void* stream);
 
+/* Automatic relevance determination with the l1 prior (Tan and Fevotte, TPAMI 2013): component k has a relevance lambda_k,
+ * and every W and H update adds pen_k = phi / lambda_k to the denominator of component k's elements, with the fp32 add of the
+ * scalar l1_reg (pass l1_reg = l2_reg = 0 for the ARD objective).  Registration: W and H are the factors the fit starts
+ * from (read here, not kept); b, c and phi (finite, > 0) the prior's scale, c = n_W + n_H + a + 1 and the dispersion.  It
+ * sets lambda_k = (sum W[:, k] + sum H[:, k] + b) / c, pen_k = phi / lambda_k and the change to 0 (the sums over every entry
+ * of component k, W[:, k, ...] and H[:, k, ...] for NMFD / NMF2D / NMF3D; fixed-order fp32 column sums, the rest in double,
+ * lambda and pen stored as fp32).  The context owns lambda, pen and the change.  W and H both null clear the registration,
+ * and so does any later set_target*.  Valid on a single NMF or NMFD context after any set_target* (NMFB200_ERR_STATE
+ * before); NMFB200_ERR_INVALID on batched and sparse-PLCA contexts and while nmfb200_set_fixed_w holds components (and
+ * set_fixed_w refuses the same way while ARD is registered).  While it is registered: update_w, update_h and nmf_iterate
+ * add pen on every kernel family; nmf_iterate runs, each iteration, the W update, the H update, then nmfb200_ard_update;
+ * loss_prefetch_w stays valid (the lambda update moves no factor); nmf_peer_supported reports 0, and nmf_update_w_peer,
+ * w_apply, nmf_cd_* and nmf_observed_cd_* return NMFB200_ERR_INVALID.  Asynchronous. */
+int nmfb200_set_ard(nmfb200_ctx* ctx, const float* W, const float* H, double b, double c, double phi, void* stream);
+
+/* The lambda update from the current W and H: lambda_k as at registration, pen_k = phi / lambda_k, and the change
+ * max_k |lambda_k - previous lambda_k| / previous lambda_k.  Deterministic: no float atomics.  NMFB200_ERR_STATE without
+ * a registration.  Asynchronous. */
+int nmfb200_ard_update(nmfb200_ctx* ctx, const float* W, const float* H, void* stream);
+
+/* Copies lambda (R floats), pen (R floats) and the change (one float) to the non-null pointers among lambda / pen /
+ * change, host or device memory, then synchronises `stream`.  NMFB200_ERR_STATE without a registration. */
+int nmfb200_ard_read(nmfb200_ctx* ctx, float* lambda, float* pen, float* change, void* stream);
+
 /* ---- tile plans of the fp32 CUDA-core kernels (host only: no device work, no allocation) -------- */
 
 /* What a context of these sizes runs on the fp32 kernels, from the library's own planners.  `out` receives

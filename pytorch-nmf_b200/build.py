@@ -14,7 +14,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libnmf_b200.so")
 SOURCES = ["capi.cu", "simt_nmf.cu", "update.cu", "nmfd.cu", "tc_nmf.cu", "tc_nmfd.cu", "sparse_nmf.cu", "project.cu", "plca_em.cu", "cd.cu",
-           "sparse_plca.cu", "observed_cd.cu"]
+           "sparse_plca.cu", "observed_cd.cu", "ard.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr",

@@ -2,6 +2,7 @@
 #include "../../include/nmf_b200.h"
 
 #include <algorithm>
+#include <cmath>
 #include <atomic>
 #include <functional>
 #include <new>
@@ -88,6 +89,13 @@ struct nmfb200_ctx {
   // nmfb200_set_fixed_w: R bytes, non-zero for a component of W held at its value, borrowed; cleared by every set_target*.
   // While set, every call that writes W leaves those components unstored.
   const uint8_t* fixed_w = nullptr;
+  // nmfb200_set_ard: automatic relevance determination is registered (`ard`), with its prior's b, c = n_W + n_H + a + 1 and
+  // the dispersion phi; cleared by every set_target*.  ard_state (kept across registrations): ard_state_floats(R) floats,
+  // [sW R | sH R | lambda R | pen R | change 1].  While set, every W and H update adds pen[k] to the denominators of
+  // component k, and nmf_iterate runs the lambda update after each H update.
+  bool ard = false;
+  double ard_b = 0.0, ard_c = 0.0, ard_phi = 0.0;
+  DevBuf<float> ard_state;
   // chunked partial numerators / denominators of the CUDA-core path; den (lazy) is sized like num
   DevBuf<float> num, den;
   int nslab[2] = {1, 1};          // partial slabs of the W / H terms: contraction chunks (NMF), wgrad / dgrad splits (NMFD)
@@ -429,13 +437,14 @@ int check_target(const void* V, int dtype) {
 }
 
 // The one place a set_target* changes the target, once its checks and allocations have passed: a call refused before it
-// leaves the context as it was.  A new target drops the mask or weight and the fixed components of W; a sparse one takes
-// the tensor cores out of play.
+// leaves the context as it was.  A new target drops the mask or weight, the fixed components of W and the ARD registration;
+// a sparse one takes the tensor cores out of play.
 void commit_target(nmfb200_ctx* c, TargetForm form, const void* V, int vdtype, int64_t ldv, int64_t bstride,
                    const SparseTarget& sp = SparseTarget{}) {
   c->form = form; c->V = V; c->vdtype = vdtype; c->ldv = ldv; c->bstride = bstride; c->sp = sp;
   c->sel = CellSel{};
   c->fixed_w = nullptr;
+  c->ard = false;
   c->tc_off = form != TargetForm::Dense;
 }
 
@@ -920,7 +929,61 @@ int nmfb200_set_fixed_w(nmfb200_ctx* ctx, const uint8_t* fixed, void* stream) {
   if (ctx->kind == CtxKind::PlcaSparse)
     return fail(NMFB200_ERR_INVALID, "sparse PLCA contexts do not update W (its EM step is the caller's)");
   TARGET_GUARD(ctx);
+  if (fixed && ctx->ard) return fail(NMFB200_ERR_INVALID, "fixed components of W do not combine with ARD (nmfb200_set_ard)");
   ctx->fixed_w = fixed;
+  return 0;
+}
+
+namespace {
+// The ARD lambda update from W and H (first: the registration's initial lambda, change 0)
+int ard_lambda(nmfb200_ctx* c, const float* W, const float* H, bool first, cudaStream_t st) {
+  const FactorDims w = factor_dims(c, 0), h = factor_dims(c, 1);
+  return ard_update(W, w.rows, w.inner, H, h.rows, h.inner, (int)c->R, c->ard_b, c->ard_c, c->ard_phi, first,
+                    c->cs_scratch, c->cs_scratch.n, c->ard_state, st);
+}
+
+// What the ARD calls serve: a single NMF or NMFD / NMF2D / NMF3D context (CTX_GUARD) with a target
+int ard_check(nmfb200_ctx* ctx) {
+  if (is_batch(ctx)) return fail(NMFB200_ERR_INVALID, "batched fits take no ARD");
+  TARGET_GUARD(ctx);
+  return 0;
+}
+}  // namespace
+
+int nmfb200_set_ard(nmfb200_ctx* ctx, const float* W, const float* H, double b, double c, double phi, void* stream) {
+  CTX_GUARD(ctx, kDenseModels);
+  if (int rc = ard_check(ctx)) return rc;
+  if (!W && !H) { ctx->ard = false; return 0; }
+  if (!W || !H) return fail(NMFB200_ERR_INVALID, "set_ard: W and H must both be given (both null clears ARD)");
+  auto positive = [](double x) { return std::isfinite(x) && x > 0.0; };
+  if (!positive(b) || !positive(c) || !positive(phi)) return fail(NMFB200_ERR_INVALID, "set_ard: b, c and phi must be finite and > 0");
+  if (ctx->fixed_w) return fail(NMFB200_ERR_INVALID, "ARD does not combine with fixed components of W (nmfb200_set_fixed_w)");
+  NMF_CUDA_CHECK(ctx->ard_state.ensure(ard_state_floats((int)ctx->R)));
+  ctx->ard_b = b; ctx->ard_c = c; ctx->ard_phi = phi;
+  int rc = ard_lambda(ctx, W, H, true, (cudaStream_t)stream);
+  ctx->ard = rc == 0;
+  return rc;
+}
+
+int nmfb200_ard_update(nmfb200_ctx* ctx, const float* W, const float* H, void* stream) {
+  CTX_GUARD(ctx, kDenseModels);
+  if (int rc = ard_check(ctx)) return rc;
+  if (!ctx->ard) return fail(NMFB200_ERR_STATE, "ard_update: ARD is not registered (nmfb200_set_ard)");
+  if (!W || !H) return fail(NMFB200_ERR_INVALID, "null factor pointer");
+  return ard_lambda(ctx, W, H, false, (cudaStream_t)stream);
+}
+
+int nmfb200_ard_read(nmfb200_ctx* ctx, float* lambda, float* pen, float* change, void* stream) {
+  CTX_GUARD(ctx, kDenseModels);
+  if (int rc = ard_check(ctx)) return rc;
+  if (!ctx->ard) return fail(NMFB200_ERR_STATE, "ard_read: ARD is not registered (nmfb200_set_ard)");
+  cudaStream_t st = (cudaStream_t)stream;
+  const size_t R = (size_t)ctx->R;
+  const float* state = ctx->ard_state;
+  if (lambda) NMF_CUDA_CHECK(cudaMemcpyAsync(lambda, state + 2 * R, R * sizeof(float), cudaMemcpyDefault, st));
+  if (pen) NMF_CUDA_CHECK(cudaMemcpyAsync(pen, state + 3 * R, R * sizeof(float), cudaMemcpyDefault, st));
+  if (change) NMF_CUDA_CHECK(cudaMemcpyAsync(change, state + 4 * R, sizeof(float), cudaMemcpyDefault, st));
+  NMF_CUDA_CHECK(cudaStreamSynchronize(st));
   return 0;
 }
 
@@ -1048,13 +1111,15 @@ int factor_terms(nmfb200_ctx* c, int which, const float* W, const float* H, doub
 int update_factor(nmfb200_ctx* ctx, int which, float* param, const float* W, const float* H, double beta, double gamma,
                   double l1_reg, double l2_reg, cudaStream_t st) {
   const uint8_t* fixed = which == 0 ? ctx->fixed_w : nullptr;
-  if (ctx->tc && use_tc(ctx, beta)) return tc_update(ctx->tc, which, param, W, H, beta, gamma, l1_reg, l2_reg, st, fixed);
+  const float* pen = ctx->ard ? ctx->ard_state + 3 * ctx->R : nullptr;       // ARD: both factors
+  if (ctx->tc && use_tc(ctx, beta))
+    return tc_update(ctx->tc, which, param, W, H, beta, gamma, l1_reg, l2_reg, st, fixed, pen);
   ApplyArgs a; bool tc;
   int rc = factor_terms(ctx, which, W, H, beta, nullptr, a, &tc, st);
   if (rc) return rc;
   a.param = param; a.gamma = (float)gamma; a.l1 = (float)l1_reg; a.l2 = (float)l2_reg;
   if (tc) a.absmax_bits = tc_nmfd_begin_update(ctx->tcd, which, st);
-  rc = apply_update(a, st, fixed);
+  rc = apply_update(a, st, fixed, pen);
   if (rc) return rc;
   if (!tc) mark_stale(ctx, which == 0, which == 1);
   return 0;
@@ -1114,6 +1179,7 @@ int nmfb200_nmf_iterate(nmfb200_ctx* ctx, float* W, float* H, double beta, doubl
     int rc = update_factor(ctx, 0, W, W, H, beta, gamma, l1_reg, l2_reg, st);
     if (rc) return rc;
     rc = update_factor(ctx, 1, H, W, H, beta, gamma, l1_reg, l2_reg, st);
+    if (rc == 0 && ctx->ard) rc = ard_lambda(ctx, W, H, false, st);
     if (rc) return rc;
   }
   return 0;
@@ -1132,7 +1198,7 @@ int nmfb200_nmf_loss_prefetch_w(nmfb200_ctx* ctx, const float* W, const float* H
 /* ---- row-sharded W update over peer memory (NVLink, one process per GPU) ---------------------- */
 
 int nmfb200_nmf_peer_supported(const nmfb200_ctx* ctx, double beta) {
-  if (!ctx || ctx->kind != CtxKind::Nmf || !has_target(ctx) || ctx->fixed_w || !use_tc(ctx, beta)) return 0;
+  if (!ctx || ctx->kind != CtxKind::Nmf || !has_target(ctx) || ctx->fixed_w || ctx->ard || !use_tc(ctx, beta)) return 0;
   return tc_peer_supported(ctx->tc, beta) ? 1 : 0;
 }
 
@@ -1165,6 +1231,7 @@ int nmfb200_nmf_update_w_peer(nmfb200_ctx* ctx, float* W, const float* H, double
   CTX_GUARD(ctx, kinds(CtxKind::Nmf));
   TARGET_GUARD(ctx);
   if (!W || !H) return fail(NMFB200_ERR_INVALID, "null factor pointer");
+  if (ctx->ard) return fail(NMFB200_ERR_INVALID, "ARD fits are not sharded (nmfb200_set_ard)");
   if (!nmfb200_nmf_peer_supported(ctx, beta)) return fail(NMFB200_ERR_STATE, "peer-memory W update is not available for this context / beta");
   return tc_update_w_peer(ctx->tc, W, H, beta, gamma, l1_reg, l2_reg, (cudaStream_t)stream);
 }
@@ -1257,6 +1324,7 @@ int nmfb200_w_apply(nmfb200_ctx* ctx, float* W, const float* reduced, double bet
   CTX_GUARD(ctx, kDenseModels);
   TARGET_GUARD(ctx);
   if (is_batch(ctx)) return fail(NMFB200_ERR_INVALID, "w_apply does not serve batched contexts");
+  if (ctx->ard) return fail(NMFB200_ERR_INVALID, "ARD fits are not sharded (nmfb200_set_ard)");
   if (!W || !reduced) return fail(NMFB200_ERR_INVALID, "null pointer");
   cudaStream_t st = (cudaStream_t)stream;
   if (ctx->tc && use_tc(ctx, beta)) return tc_w_apply(ctx->tc, W, reduced, beta, gamma, l1_reg, l2_reg, st, ctx->fixed_w);
@@ -1328,6 +1396,7 @@ int cd_check(nmfb200_ctx* ctx) {
   TARGET_GUARD(ctx);
   if (ctx->form == TargetForm::Observed) return fail(NMFB200_ERR_INVALID, "cd: observed-cell targets are not served");
   if (ctx->sel) return fail(NMFB200_ERR_INVALID, "cd: contexts with a mask or a weight are not served");
+  if (ctx->ard) return fail(NMFB200_ERR_INVALID, "cd: ARD takes the multiplicative updates (nmfb200_set_ard)");
   return 0;
 }
 
@@ -1439,6 +1508,7 @@ int observed_cd_check(nmfb200_ctx* ctx) {
   if (ctx->form != TargetForm::Observed)
     return fail(NMFB200_ERR_INVALID, "observed cd: only targets set by nmfb200_nmf_set_target_observed / _weighted are "
                                      "served (nmfb200_nmf_cd_update serves dense and sparse targets)");
+  if (ctx->ard) return fail(NMFB200_ERR_INVALID, "observed cd: ARD takes the multiplicative updates (nmfb200_set_ard)");
   return 0;
 }
 

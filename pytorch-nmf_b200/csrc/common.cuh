@@ -311,8 +311,9 @@ struct ApplyArgs {
   int64_t line = 0;
 };
 // fixed (R bytes, one problem only; null: none): the elements of every component r with fixed[r] != 0 are not stored
-// (they keep their value, which is what an absmax_bits update takes for them)
-int apply_update(const ApplyArgs& a, cudaStream_t st, const uint8_t* fixed = nullptr);
+// (they keep their value, which is what an absmax_bits update takes for them).  pen (R floats, one problem only, exclusive
+// with fixed; null: none): the ARD penalties, pen[r] added to the denominator of every element of component r after a.l1.
+int apply_update(const ApplyArgs& a, cudaStream_t st, const uint8_t* fixed = nullptr, const float* pen = nullptr);
 // whether apply_update takes its four-elements-per-thread kernel for this shape (16-byte aligned buffers provided)
 bool apply_update_vec4_shape(const ApplyArgs& a);
 // num_out[i] (and den_out[i] when a.den) = what the ratio stage would read for element i: summed partials + centring term
@@ -340,6 +341,17 @@ int matrix_minmax(const void* V, int vdtype, int64_t rows, int64_t cols, int64_t
 // b's run is its own rag[b].loss_n loss partials at rag[b].loss_part (n is not read).
 int sum_partials(const double* p, int n, double* out, cudaStream_t st, int64_t nprob = 1, const uint8_t* active = nullptr,
                  const RaggedProblem* rag = nullptr);
+
+// ard.cu -----------------------------------------------------------------------------------
+// The relevance update of an l1-ARD fit (Tan and Fevotte 2013): with sW[k] and sH[k] the sums of component k of W (rows_w
+// x R x inner_w) and H (rows_h x R x inner_h), each by factor_colsum in its fixed order (through `scratch`),
+//   lambda[k] = (sW[k] + sH[k] + b) / c  (in double, stored as fp32),  pen[k] = phi / lambda[k]  (double, stored as fp32),
+// and, unless `first`, *change = max_k |lambda[k] - old lambda[k]| / old lambda[k] (0 when `first`).  state: the ARD
+// buffer, ard_state_floats(R) floats laid out [sW R | sH R | lambda R | pen R | change 1].  No float atomics: deterministic.
+int64_t ard_state_floats(int R);
+int ard_update(const float* W, int64_t rows_w, int64_t inner_w, const float* H, int64_t rows_h, int64_t inner_h, int R,
+               double b, double c, double phi, bool first, float* scratch, int64_t scratch_floats, float* state,
+               cudaStream_t st);
 
 // project.cu -------------------------------------------------------------------------------
 // Hoyer's projection (nmf.py:21-49) of every slice x[:, j, :] of x viewed as (outer, D, inner) onto {v >= 0, |v|_1 = k1[j],

@@ -537,10 +537,14 @@ struct TcApplyArgs {
 };
 
 // FIXED (and in the two kernels below): the components r with fixed[r] != 0 are not stored; they keep their value, which
-// enters the column sums and the max as it is.  The instantiations without it compile none of this.
-template <bool FIXED = false>
+// enters the column sums and the max as it is.  PEN (likewise): pen[r], the ARD penalty of component r (nmfb200_set_ard), is
+// added to the denominator after a.l1 with the same fp32 add.  The instantiations without them compile none of this.  This
+// kernel takes both through its one per-component pointer `comp` (the flags exclude each other): R bytes `fixed` or R
+// floats `pen`.  A second pointer parameter alone changed its register allocation; this way the instantiations that ran
+// before compile to the same SASS.
+template <bool FIXED = false, bool PEN = false>
 __global__ void __launch_bounds__(256)
-tc_apply_kernel(TcApplyArgs a, const uint8_t* __restrict__ fixed) {
+tc_apply_kernel(TcApplyArgs a, const uint8_t* __restrict__ comp) {
   __shared__ float sh[2][128];
   const int r = threadIdx.x & 127, rg = threadIdx.x >> 7;
   const int64_t row0 = (int64_t)blockIdx.x * a.rpb;
@@ -549,7 +553,7 @@ tc_apply_kernel(TcApplyArgs a, const uint8_t* __restrict__ fixed) {
   if (r < a.R) {
     const float klden = (a.apply && !a.den) ? a.kl_den[r] : 1.f;
     const float kap = (a.apply && !a.den) ? *a.kappa : 0.f;
-    const bool upd = a.apply && !(FIXED && fixed[r]);
+    const bool upd = a.apply && !(FIXED && comp[r]);
     for (int64_t row = row0 + rg; row < row1; row += 2) {
       const int64_t idx = row * a.R + r;
       float v = a.param[idx];
@@ -567,6 +571,7 @@ tc_apply_kernel(TcApplyArgs a, const uint8_t* __restrict__ fixed) {
         }
         const float neg = fmaxf(num, 0.f) + kEps;              // nmf.py:78
         if (a.l1 > 0.f) pos += a.l1;                            // nmf.py:85-86
+        if constexpr (PEN) pos += reinterpret_cast<const float*>(comp)[r];   // ARD: l1 of component r
         if (a.l2 > 0.f) pos = fmaf(a.l2, v, pos);               // nmf.py:87-88
         float mult = neg / pos;                                 // nmf.py:89
         if (a.gamma != 1.0f) mult = powf(mult, a.gamma);        // nmf.py:90-91
@@ -677,9 +682,10 @@ gram_sum_kernel(const float* __restrict__ part, int nb, int nout, float* __restr
 // Row tiles of 64: thread (ty, tx) owns rows 4 ty .. 4 ty + 3 and components TR tx .. TR tx + TR - 1 of the tile.  The tile's
 // old values are staged before anything is overwritten (pitch RP + 1: the four rows of a thread and the two row groups of a
 // warp fall into different banks), the Gram matrix once per block.  Dynamic shared memory: gram RP x RP | tile 64 x (RP + 1).
-template <int TR, bool FIXED = false>
+template <int TR, bool FIXED = false, bool PEN = false>
 __global__ void __launch_bounds__(256, TR == 4 ? 3 : 1)
-tc_apply_eu_kernel(TcApplyArgs a, const float* __restrict__ gram, const uint8_t* __restrict__ fixed) {
+tc_apply_eu_kernel(TcApplyArgs a, const float* __restrict__ gram, const uint8_t* __restrict__ fixed,
+                   const float* __restrict__ pen) {
   constexpr int RP = 16 * TR, FP = RP + 1;
   extern __shared__ __align__(16) float eu_smem[];
   float* gs = eu_smem;                           // [RP][RP], zero-padded
@@ -775,6 +781,7 @@ tc_apply_eu_kernel(TcApplyArgs a, const float* __restrict__ gram, const uint8_t*
         const float neg = fmaxf(num, 0.f) + kEps;                // nmf.py:78
         float pos = fmaxf(den, 0.f) + kEps;                      // nmf.py:83
         if (a.l1 > 0.f) pos += a.l1;                              // nmf.py:85-86
+        if constexpr (PEN) pos += pen[r];                         // ARD: l1 of component r
         if (a.l2 > 0.f) pos = fmaf(a.l2, v, pos);                 // nmf.py:87-88
         float mult = neg / pos;                                   // nmf.py:89
         if (a.gamma != 1.0f) mult = powf(mult, a.gamma);          // nmf.py:90-91 (gamma == 1 for beta 2)
@@ -959,9 +966,9 @@ __device__ __forceinline__ void wait_peer_flags(const unsigned int* flags, int n
   __syncthreads();
 }
 
-template <bool SPLIT, bool FIXED = false>
+template <bool SPLIT, bool FIXED = false, bool PEN = false>
 __global__ void __launch_bounds__(256)
-tc_apply_finish_kernel(TcApplyArgs a, TcFinishArgs f, const uint8_t* __restrict__ fixed) {
+tc_apply_finish_kernel(TcApplyArgs a, TcFinishArgs f, const uint8_t* __restrict__ fixed, const float* __restrict__ pen) {
   __shared__ float4 sh[256];
   const int lanes = a.R >> 2;                    // threads per row
   const int rows_per_pass = 256 / lanes;
@@ -985,6 +992,11 @@ tc_apply_finish_kernel(TcApplyArgs a, TcFinishArgs f, const uint8_t* __restrict_
 #pragma unroll
       for (int i = 0; i < 4; ++i) fx[i] = fixed[4 * q + i] != 0;
     }
+    float pr[4] = {0.f, 0.f, 0.f, 0.f};                      // this thread's four ARD penalties
+    if constexpr (PEN) {
+#pragma unroll
+      for (int i = 0; i < 4; ++i) pr[i] = pen[4 * q + i];
+    }
     for (int64_t row = row0 + rl; row < row1; row += rows_per_pass) {
       float4* pp = reinterpret_cast<float4*>(a.param + row * a.R) + q;
       float4 v = *pp;
@@ -1002,6 +1014,7 @@ tc_apply_finish_kernel(TcApplyArgs a, TcFinishArgs f, const uint8_t* __restrict_
           const float neg = fmaxf(n, 0.f) + kEps;                   // nmf.py:78
           float pos = a.den ? fmaxf(ds[i], 0.f) + kEps : dd[i];     // nmf.py:83 | nmf.py:368-369 / :381-382
           if (a.l1 > 0.f) pos += a.l1;                              // nmf.py:85-86
+          if constexpr (PEN) pos += pr[i];                          // ARD: l1 of component 4 q + i
           if (a.l2 > 0.f) pos = fmaf(a.l2, vv[i], pos);             // nmf.py:87-88
           float mult = neg / pos;                                   // nmf.py:89
           if (a.gamma != 1.0f) mult = powf(mult, a.gamma);          // nmf.py:90-91
@@ -1328,6 +1341,7 @@ struct TcState {
   float* zero = nullptr;           // device scalar 0 (kappa of an already complete numerator)
   int coop_blocks = 0;              // co-resident blocks of the fused tail kernel (cooperative launch), 0 = unavailable
   int coop_blocks_fixed = 0;        // the same for its instantiation with fixed components (its own register count)
+  int coop_blocks_pen = 0;          // and for its instantiation with ARD penalties
 };
 
 bool tc_shape_supported(int64_t N, int64_t C, int64_t R) {
@@ -1379,6 +1393,8 @@ int tc_create(TcState** out, int device, int64_t N, int64_t C, int64_t R, bool s
     s->coop_blocks = coop_blocks(split ? (const void*)tc_apply_finish_kernel<true> : (const void*)tc_apply_finish_kernel<false>);
     s->coop_blocks_fixed = coop_blocks(split ? (const void*)tc_apply_finish_kernel<true, true>
                                              : (const void*)tc_apply_finish_kernel<false, true>);
+    s->coop_blocks_pen = coop_blocks(split ? (const void*)tc_apply_finish_kernel<true, false, true>
+                                           : (const void*)tc_apply_finish_kernel<false, false, true>);
   }
   s->plan_w = make_plan(C, N, s->num_sms, s->TN);
   s->plan_h = make_plan(N, C, s->num_sms, s->TN);
@@ -1485,8 +1501,10 @@ namespace {
 // buffer [rows*R num | R colsum or rows*R den] instead of this rank's chunked partials.
 int apply_and_finish(TcState* s, int which, float* param, bool apply, const Plan* pl, double beta, double gamma,
                      double l1, double l2, cudaStream_t st, const float* reduced = nullptr,
-                     const float* other = nullptr, bool peer = false, const uint8_t* fixed = nullptr) {
+                     const float* other = nullptr, bool peer = false, const uint8_t* fixed = nullptr,
+                     const float* pen = nullptr) {
   if (fixed && (!apply || peer)) { set_error("internal: fixed components need a local ratio stage"); return 1; }
+  if (pen && (!apply || peer || fixed)) { set_error("internal: ARD penalties need a local ratio stage, nothing fixed"); return 1; }
   const int64_t rows = which == 0 ? s->C : s->N;
   int rpb = (int)round_up(ceil_div(rows, 1024), 4);
   if (rpb < 64) rpb = 64;
@@ -1516,7 +1534,7 @@ int apply_and_finish(TcState* s, int which, float* param, bool apply, const Plan
     a.flag_target = s->peer_iter; a.peer_err = s->peer_err;
   }
   s->exps_beta = beta;                 // both branches below end in publish_scales at this beta
-  const int coop_blocks = fixed ? s->coop_blocks_fixed : s->coop_blocks;
+  const int coop_blocks = fixed ? s->coop_blocks_fixed : pen ? s->coop_blocks_pen : s->coop_blocks;
   if ((s->R & 3) == 0 && coop_blocks > 0 && !(apply && beta == 2.0 && !reduced)) {
     // one cooperative launch: ratio stage, grid barrier, operand copy + scalars
     const int lanes = (int)s->R >> 2, rows_per_pass = 256 / lanes;
@@ -1529,9 +1547,11 @@ int apply_and_finish(TcState* s, int which, float* param, bool apply, const Plan
     f.exps = s->exps; f.which = which; f.colsum = s->colsum; f.vconst = s->vconst; f.kappa = s->kappa;
     f.bm1 = (float)(beta - 1.0); f.bm2 = (float)(beta - 2.0);
     f.cells = (double)s->N * (double)s->C;
-    void* args[3] = {&a, &f, &fixed};
+    void* args[4] = {&a, &f, &fixed, &pen};
     const void* fn = fixed ? (s->split ? (const void*)tc_apply_finish_kernel<true, true>
                                        : (const void*)tc_apply_finish_kernel<false, true>)
+                   : pen   ? (s->split ? (const void*)tc_apply_finish_kernel<true, false, true>
+                                       : (const void*)tc_apply_finish_kernel<false, false, true>)
                            : (s->split ? (const void*)tc_apply_finish_kernel<true> : (const void*)tc_apply_finish_kernel<false>);
     NMF_CUDA_CHECK(cudaLaunchCooperativeKernel(fn, dim3(gblocks), dim3(256), args, 0, st));
     count_launch();
@@ -1557,21 +1577,24 @@ int apply_and_finish(TcState* s, int which, float* param, bool apply, const Plan
     const int RPk = s->Rp == 64 ? 64 : 128;
     const int eu_smem = (RPk * RPk + 64 * (RPk + 1)) * (int)sizeof(float);
     if (RPk == 64) {
-      if (fixed) tc_apply_eu_kernel<4, true><<<blocks, 256, eu_smem, st>>>(a, s->gram, fixed);
-      else tc_apply_eu_kernel<4><<<blocks, 256, eu_smem, st>>>(a, s->gram, nullptr);
+      if (fixed) tc_apply_eu_kernel<4, true><<<blocks, 256, eu_smem, st>>>(a, s->gram, fixed, nullptr);
+      else if (pen) tc_apply_eu_kernel<4, false, true><<<blocks, 256, eu_smem, st>>>(a, s->gram, nullptr, pen);
+      else tc_apply_eu_kernel<4><<<blocks, 256, eu_smem, st>>>(a, s->gram, nullptr, nullptr);
     } else {
       // > 48 KB of dynamic shared memory: opt in once per device and instantiation
-      static unsigned long long eu_attr_mask[2] = {0, 0};
-      const auto kern = fixed ? tc_apply_eu_kernel<8, true> : tc_apply_eu_kernel<8>;
-      unsigned long long& mask = eu_attr_mask[fixed ? 1 : 0];
+      static unsigned long long eu_attr_mask[3] = {0, 0, 0};
+      const auto kern = fixed ? tc_apply_eu_kernel<8, true> : pen ? tc_apply_eu_kernel<8, false, true> : tc_apply_eu_kernel<8>;
+      unsigned long long& mask = eu_attr_mask[fixed ? 1 : pen ? 2 : 0];
       if (!((mask >> (s->device & 63)) & 1ull)) {
         NMF_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, eu_smem));
         mask |= 1ull << (s->device & 63);
       }
-      kern<<<blocks, 256, eu_smem, st>>>(a, s->gram, fixed);
+      kern<<<blocks, 256, eu_smem, st>>>(a, s->gram, fixed, pen);
     }
   } else if (fixed) {
     tc_apply_kernel<true><<<blocks, 256, 0, st>>>(a, fixed);
+  } else if (pen) {
+    tc_apply_kernel<false, true><<<blocks, 256, 0, st>>>(a, reinterpret_cast<const uint8_t*>(pen));
   } else {
     tc_apply_kernel<<<blocks, 256, 0, st>>>(a, nullptr);
   }
@@ -1722,7 +1745,7 @@ void tc_plan(int64_t N, int64_t C, int64_t R, bool split, int num_sms, int64_t* 
 }
 
 int tc_update(TcState* s, int which, float* param, const float* W, const float* H, double beta, double gamma, double l1,
-              double l2, cudaStream_t st, const uint8_t* fixed) {
+              double l2, cudaStream_t st, const uint8_t* fixed, const float* pen) {
   // tc_loss_prefetch_w already ran the W contraction on these very factors (its numerators are still in `part`)
   const bool reuse = which == 0 && s->w_pending && !s->dirty_w && !s->dirty_h && beta == 1.0;
   s->w_pending = false;
@@ -1733,7 +1756,7 @@ int tc_update(TcState* s, int which, float* param, const float* W, const float* 
     if (rc) return rc;
   }
   return apply_and_finish(s, which, param, true, which == 0 ? &s->plan_w : &s->plan_h, beta, gamma, l1, l2, st, nullptr,
-                          which == 0 ? H : W, false, fixed);
+                          which == 0 ? H : W, false, fixed, pen);
 }
 
 // Raw update terms of one factor (which = 0: W, 1: H) in one dense buffer: numerator (rows x R; chunk sums, + kappa

@@ -27,8 +27,9 @@ int tc_target_sum(TcState* s, double* vsum, cudaStream_t st);
 void tc_mark_dirty(TcState* s, bool w, bool h);
 // one factor update in place (which = 0: param = W, 1: param = H).  fixed (R bytes; null: none): the ratio stage does not
 // store the components with fixed[r] != 0, which keep their value and enter the operand copy, column sums and scale as such.
+// pen (R floats, exclusive with fixed; null: none): the ARD penalties, pen[r] added to the denominator of component r.
 int tc_update(TcState* s, int which, float* param, const float* W, const float* H, double beta, double gamma, double l1,
-              double l2, cudaStream_t st, const uint8_t* fixed = nullptr);
+              double l2, cudaStream_t st, const uint8_t* fixed = nullptr, const float* pen = nullptr);
 // raw terms of either factor's update (which = 0: W, 1: H): [numerator rows x R | colsum(other) R (beta 1) or denominator rows x R]
 int tc_raw_terms(TcState* s, int which, const float* W, const float* H, double beta, float* out, cudaStream_t st);
 int tc_w_apply(TcState* s, float* W, const float* reduced, double beta, double gamma, double l1, double l2,

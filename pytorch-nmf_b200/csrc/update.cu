@@ -9,7 +9,9 @@ namespace {
 // a padding row of a ragged batch's H, or (LINES) a padding position of a ragged NMFD batch's H lines, which no kernel
 // writes.  The kernels below take RAGGED (a.rag set) and LINES (a.line set as well) as template flags, so that their other
 // instantiations run the code they always ran.  The ratio-stage kernels take FIXED the same way: `fixed` (R bytes, non-zero
-// for a component held at its value, nmfb200_set_fixed_w) predicates the final store of each element on its component.
+// for a component held at its value, nmfb200_set_fixed_w) predicates the final store of each element on its component.  And
+// PEN: `pen` (R floats, the ARD penalties of nmfb200_set_ard) adds pen[r] to the denominator of every element of component r,
+// with the fp32 add the scalar l1 takes.
 struct PartialAt { int64_t off, stride; int nch; };
 template <bool RAGGED, bool LINES = false>
 __device__ __forceinline__ bool partial_at(const ApplyArgs& a, int64_t idx, int64_t b, PartialAt& p) {
@@ -33,9 +35,9 @@ __device__ __forceinline__ bool partial_at(const ApplyArgs& a, int64_t idx, int6
   return true;
 }
 
-template <bool RAGGED, bool LINES = false, bool FIXED = false>
+template <bool RAGGED, bool LINES = false, bool FIXED = false, bool PEN = false>
 __global__ void __launch_bounds__(256)
-apply_update_kernel(ApplyArgs a, const uint8_t* __restrict__ fixed) {
+apply_update_kernel(ApplyArgs a, const uint8_t* __restrict__ fixed, const float* __restrict__ pen) {
   const int64_t idx = (int64_t)blockIdx.x * 256 + threadIdx.x;
   float newv = 0.f;
   const int64_t b = a.prob_numel ? idx / a.prob_numel : 0;      // Batch: the element's problem
@@ -60,6 +62,7 @@ apply_update_kernel(ApplyArgs a, const uint8_t* __restrict__ fixed) {
       pos = a.kl_den[b * a.R + r];                           // nmf.py:368-369 / :381-382 (no relu, no eps)
     }
     if (a.l1 > 0.f) pos += a.l1;                             // nmf.py:85-86
+    if constexpr (PEN) pos += pen[r];                        // ARD: l1 of component r
     if (a.l2 > 0.f) pos = fmaf(a.l2, p, pos);                // nmf.py:87-88
     float mult = neg / pos;                                  // nmf.py:89
     if (a.gamma != 1.0f) mult = powf(mult, a.gamma);         // nmf.py:90-91
@@ -283,9 +286,9 @@ __global__ void minmax_stage2(const float* __restrict__ scratch, int nb, float* 
 
 // Four consecutive elements per thread (same row, same component: inner % 4 == 0), 16-byte loads of the parameter and of every
 // partial slab.  Same arithmetic per element as apply_update_kernel.
-template <bool RAGGED, bool FIXED = false>
+template <bool RAGGED, bool FIXED = false, bool PEN = false>
 __global__ void __launch_bounds__(256)
-apply_update_vec4_kernel(ApplyArgs a, const uint8_t* __restrict__ fixed) {
+apply_update_vec4_kernel(ApplyArgs a, const uint8_t* __restrict__ fixed, const float* __restrict__ pen) {
   const int64_t idx = ((int64_t)blockIdx.x * 256 + threadIdx.x) * 4;
   float m = 0.f;
   const int64_t b = a.prob_numel ? idx / a.prob_numel : 0;      // Batch: prob_numel is a multiple of 4 here
@@ -307,6 +310,8 @@ apply_update_vec4_kernel(ApplyArgs a, const uint8_t* __restrict__ fixed) {
       }
     }
     const float klden = a.den ? 0.f : a.kl_den[b * a.R + r];
+    float pr = 0.f;
+    if constexpr (PEN) pr = pen[r];
     float4 p = *reinterpret_cast<const float4*>(a.param + idx);
     auto one = [&](float pv, float n, float d) {
       n *= sc;
@@ -314,6 +319,7 @@ apply_update_vec4_kernel(ApplyArgs a, const uint8_t* __restrict__ fixed) {
       const float neg = fmaxf(n, 0.f) + kEps;                  // nmf.py:78
       float pos = a.den ? fmaxf(d * sc, 0.f) + kEps : klden;   // nmf.py:83 / :368-369
       if (a.l1 > 0.f) pos += a.l1;                             // nmf.py:85-86
+      if constexpr (PEN) pos += pr;                            // ARD: l1 of component r
       if (a.l2 > 0.f) pos = fmaf(a.l2, pv, pos);               // nmf.py:87-88
       float mult = neg / pos;                                  // nmf.py:89
       if (a.gamma != 1.0f) mult = powf(mult, a.gamma);         // nmf.py:90-91
@@ -344,18 +350,21 @@ bool apply_update_vec4_shape(const ApplyArgs& a) {
          (a.nchunks == 1 || a.chunk_stride % 4 == 0) && a.prob_numel % 4 == 0 && a.line == 0;
 }
 
-int apply_update(const ApplyArgs& a, cudaStream_t st, const uint8_t* fixed) {
+int apply_update(const ApplyArgs& a, cudaStream_t st, const uint8_t* fixed, const float* pen) {
   if (a.numel <= 0) return 0;
   if (fixed && (a.rag || a.prob_numel)) { set_error("apply_update: fixed components need a single problem"); return 1; }
+  if (pen && (a.rag || a.prob_numel || fixed)) { set_error("apply_update: ARD penalties need a single problem, nothing fixed"); return 1; }
   const bool vec4 = apply_update_vec4_shape(a) && aligned16(a.param) && aligned16(a.num) && (!a.den || aligned16(a.den));
   const unsigned g4 = (unsigned)ceil_div(a.numel / 4, 256), g1 = (unsigned)ceil_div(a.numel, 256);
-  if (fixed && vec4) apply_update_vec4_kernel<false, true><<<g4, 256, 0, st>>>(a, fixed);
-  else if (fixed) apply_update_kernel<false, false, true><<<g1, 256, 0, st>>>(a, fixed);
-  else if (vec4 && a.rag) apply_update_vec4_kernel<true><<<g4, 256, 0, st>>>(a, nullptr);
-  else if (vec4) apply_update_vec4_kernel<false><<<g4, 256, 0, st>>>(a, nullptr);
-  else if (a.rag && a.line) apply_update_kernel<true, true><<<g1, 256, 0, st>>>(a, nullptr);
-  else if (a.rag) apply_update_kernel<true><<<g1, 256, 0, st>>>(a, nullptr);
-  else apply_update_kernel<false><<<g1, 256, 0, st>>>(a, nullptr);
+  if (pen && vec4) apply_update_vec4_kernel<false, false, true><<<g4, 256, 0, st>>>(a, nullptr, pen);
+  else if (pen) apply_update_kernel<false, false, false, true><<<g1, 256, 0, st>>>(a, nullptr, pen);
+  else if (fixed && vec4) apply_update_vec4_kernel<false, true><<<g4, 256, 0, st>>>(a, fixed, nullptr);
+  else if (fixed) apply_update_kernel<false, false, true><<<g1, 256, 0, st>>>(a, fixed, nullptr);
+  else if (vec4 && a.rag) apply_update_vec4_kernel<true><<<g4, 256, 0, st>>>(a, nullptr, nullptr);
+  else if (vec4) apply_update_vec4_kernel<false><<<g4, 256, 0, st>>>(a, nullptr, nullptr);
+  else if (a.rag && a.line) apply_update_kernel<true, true><<<g1, 256, 0, st>>>(a, nullptr, nullptr);
+  else if (a.rag) apply_update_kernel<true><<<g1, 256, 0, st>>>(a, nullptr, nullptr);
+  else apply_update_kernel<false><<<g1, 256, 0, st>>>(a, nullptr, nullptr);
   NMF_LAUNCH_CHECK();
   return 0;
 }

@@ -85,6 +85,9 @@ SIGNATURES = {
     "nmfb200_set_mask": (_int, [_vp, _vp, _vp]),
     "nmfb200_set_weight": (_int, [_vp, _vp, _vp]),
     "nmfb200_set_fixed_w": (_int, [_vp, _vp, _vp]),
+    "nmfb200_set_ard": (_int, [_vp, _vp, _vp, _dbl, _dbl, _dbl, _vp]),
+    "nmfb200_ard_update": (_int, [_vp, _vp, _vp, _vp]),
+    "nmfb200_ard_read": (_int, [_vp, _vp, _vp, _vp, _vp]),
     "nmfb200_hoyer_project": (_int, [_int, _vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp]),
     "nmfb200_nmf_plan": (_int, [_i64, _i64, _i64, _c.POINTER(_i64), _int]),
     "nmfb200_nmfd_plan": (_int, [_i64, _i64, _int, _c.POINTER(_i64), _i64, _c.POINTER(_i64), _c.POINTER(_i64), _int]),

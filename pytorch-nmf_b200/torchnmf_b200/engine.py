@@ -243,6 +243,36 @@ class _CudaEngine:
         _capi.check(self._lib.nmfb200_set_fixed_w(self._ctx, _ptr(fixed) if fixed is not None else None,
                                                   _stream(self.device)))
 
+    def set_ard(self, b, c, phi):
+        """Register automatic relevance determination on the current factors (include/nmf_b200.h: nmfb200_set_ard): the
+        relevances lambda_k = (sum W[:, k] + sum H[:, k] + b) / c and the penalties phi / lambda_k that every later W and H
+        update adds to component k's denominators; `iterate` then runs the lambda update after each H update.  b=None
+        clears it."""
+        if b is None:
+            _capi.check(self._lib.nmfb200_set_ard(self._ctx, None, None, 0.0, 0.0, 0.0, _stream(self.device)))
+            return
+        _capi.check(self._lib.nmfb200_set_ard(self._ctx, _ptr(self.W), _ptr(self.H), float(b), float(c), float(phi),
+                                              _stream(self.device)))
+
+    def ard_update(self):
+        """The lambda update from the current factors (include/nmf_b200.h: nmfb200_ard_update)."""
+        _capi.check(self._lib.nmfb200_ard_update(self._ctx, _ptr(self.W), _ptr(self.H), _stream(self.device)))
+
+    def ard_state(self):
+        """(lambda, pen) as float32 device tensors of R elements and the last lambda update's largest relative change, a
+        float (include/nmf_b200.h: nmfb200_ard_read; synchronises)."""
+        R = self.W.shape[1]
+        buf = torch.empty(2 * R + 1, dtype=torch.float32, device=self.device)
+        _capi.check(self._lib.nmfb200_ard_read(self._ctx, _ptr(buf), _ptr(buf[R:]), _ptr(buf[2 * R:]),
+                                               _stream(self.device)))
+        return buf[:R], buf[R:2 * R], float(buf[2 * R])
+
+    def ard_change(self):
+        """The last lambda update's largest relative change, max_k |lambda_k - previous| / previous (synchronises)."""
+        change = ctypes.c_float()
+        _capi.check(self._lib.nmfb200_ard_read(self._ctx, None, None, ctypes.byref(change), _stream(self.device)))
+        return change.value
+
     def minmax(self):
         vmin, vmax = ctypes.c_float(), ctypes.c_float()
         _capi.check(self._lib.nmfb200_target_minmax(self._ctx, ctypes.byref(vmin), ctypes.byref(vmax),

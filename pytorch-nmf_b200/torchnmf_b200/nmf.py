@@ -20,6 +20,7 @@ raw-terms launch, line-search losses from the fused loss launch, every component
 `nmfb200_hoyer_project` launch.  `trainer.BetaMu` / `SparsityProj` and `plca.*` live in their own modules.
 """
 import contextlib
+import dataclasses
 import math
 import numbers
 import weakref
@@ -45,7 +46,7 @@ except Exception:  # pragma: no cover
         def update(self, n): pass
 
 __all__ = ["BaseComponent", "NMF", "NMFD", "NMF2D", "NMF3D", "BatchedNMF", "BatchedNMFD", "BatchedNMF2D",
-           "BatchedNMF3D"]
+           "BatchedNMF3D", "ARD"]
 
 
 def _gamma(beta):
@@ -169,6 +170,87 @@ def _checked_fixed_w(W, fixed_W, group):
     if group is not None:
         raise ValueError("fixed_W does not run sharded fits (group)")
     return fixed_W if bool(fixed_W.any()) else None
+
+
+@dataclasses.dataclass(frozen=True)
+class ARD:
+    """Automatic relevance determination with the l1 prior (V. Y. F. Tan and C. Fevotte, "Automatic relevance determination
+    in nonnegative matrix factorization with the beta-divergence", IEEE TPAMI 35(7), 2013): `fit(V, ..., ard=ARD())`.
+
+    a:   shape of the inverse-gamma prior on each relevance lambda_k (default 5.0; must be > 2 when b is None).
+    b:   its scale; None sets it by moment matching, b = sqrt((a - 1)(a - 2) mean(V) / (R prod(K))), with mean(V) over the
+         cells the fit reads and prod(K) = 1 for NMF.
+    phi: the dispersion: 1 for KL (Poisson), the noise variance at beta 2.
+    """
+    a: float = 5.0
+    b: float = None
+    phi: float = 1.0
+
+
+def _finite_positive(x):
+    return isinstance(x, numbers.Real) and not isinstance(x, bool) and math.isfinite(x) and x > 0
+
+
+def _checked_ard(ard, W, H, alpha, solver, group, fixed_W):
+    """The checks of a `fit(..., ard=...)` argument, before any device work: ValueError for anything that is not an `ARD`,
+    a non-finite or non-positive a, b or phi, a <= 2 without b, and for alpha, solver="cd", group, fixed_W and a frozen
+    factor, which ARD does not combine with.  Returns `ard` (None: the plain fit)."""
+    if ard is None:
+        return None
+    if not isinstance(ard, ARD):
+        raise ValueError(f"ard must be an ARD instance (got {type(ard).__name__})")
+    for name in ("a", "phi") + (("b",) if ard.b is not None else ()):
+        if not _finite_positive(getattr(ard, name)):
+            raise ValueError(f"ARD.{name} must be finite and > 0 (got {getattr(ard, name)!r})")
+    if ard.b is None and not ard.a > 2:
+        raise ValueError(f"ARD.a must be > 2 to set b by moment matching (got {ard.a!r}); pass b")
+    if alpha != 0:
+        raise ValueError("ard: ARD replaces the alpha / l1_ratio penalty; alpha must be 0")
+    if solver == "cd":
+        raise ValueError("ard: ARD runs the multiplicative updates; solver='cd' is not supported")
+    if group is not None:
+        raise ValueError("ard does not run sharded fits (group)")
+    if fixed_W is not None:
+        raise ValueError("ard does not combine with fixed_W")
+    if W is not None and H is not None and not (W.requires_grad and H.requires_grad):
+        raise ValueError("ard: W and H must both be trainable")
+    return ard
+
+
+def _ard_mean(V, mask=None, weight=None):
+    """mean(V) over the cells a fit reads, in float64: every cell of a dense target; the observed cells of a mask (NaN at the
+    missing cells never enters); the cells of weight > 0, unweighted; the stored values of a sparse COO target over N x C."""
+    f64 = torch.float64
+    if weight is not None and weight.is_sparse:
+        lin, _, _ = _weighted_cells(weight, V.shape[1], weight.device)
+        vals = _cells_of(V, lin, weight.device).values()
+        return float(vals.sum(dtype=f64)) / max(vals.numel(), 1)
+    if mask is not None and mask.is_sparse:
+        vals = _observed_cells(V, mask, mask.device).values()
+        return float(vals.sum(dtype=f64)) / max(vals.numel(), 1)
+    if weight is not None or mask is not None:
+        on = (weight > 0) if weight is not None else mask
+        on = on.to(V.device)
+        total = torch.where(on, V, torch.zeros((), dtype=V.dtype, device=V.device)).sum(dtype=f64)
+        return float(total) / max(int(on.sum()), 1)
+    if V.is_sparse:
+        return float(V._values().sum(dtype=f64)) / V.shape[0] / V.shape[1]
+    return float(V.sum(dtype=f64)) / V.numel()
+
+
+def _ard_constants(ard, V, W, H, mask=None, weight=None):
+    """(b, c) of an ARD fit: c = n_W + n_H + a + 1, n_W and n_H the entries of one component of W and of H; b as given or
+    by moment matching (`ARD`).  ValueError when that b is not positive (a target of mean 0)."""
+    R = W.shape[1]
+    n_w, n_h = W.numel() // R, H.numel() // R
+    c = n_w + n_h + ard.a + 1.0
+    b = ard.b
+    if b is None:
+        prod_k = math.prod(W.shape[2:])
+        b = math.sqrt((ard.a - 1.0) * (ard.a - 2.0) * _ard_mean(V, mask, weight) / (R * prod_k))
+        if not _finite_positive(b):
+            raise ValueError(f"ard: moment matching gives b = {b!r} (the target's mean is not positive); pass ARD(b=...)")
+    return float(b), float(c)
 
 
 class BaseComponent(torch.nn.Module):
@@ -529,13 +611,34 @@ class BaseComponent(torch.nn.Module):
                    component.  Every component fixed is the fit of trainable_W=False, bit for bit; none fixed is the plain
                    fit.  Every target form, precision and solver above is covered.  ValueError, before any device work: a
                    `fixed_W` that is not a dense torch.bool tensor of shape (R,), a W that is not trainable, and `group`.
+
+        ard:       (keyword-only, default None, through **options like `mask`) an `ARD(a=5.0, b=None, phi=1.0)`: choose the
+                   rank during the fit by automatic relevance determination with the l1 prior (Tan and Fevotte, TPAMI
+                   2013).  Fit with a generous R; component k gets a relevance lambda_k and the fit minimises
+                     J = D / phi + sum_k [(sum W[:, k] + sum H[:, k] + b) / lambda_k + c log lambda_k],
+                   c = n_W + n_H + a + 1 (n_W, n_H: the entries of one component of W and of H), D the divergence this fit
+                   minimises without it (masked or weighted as given).  lambda starts at (sum W0[:, k] + sum H0[:, k] +
+                   b) / c; each iteration updates W, then H, each by the multiplicative update with l1_reg = phi /
+                   lambda_k on component k (the same exponent gamma(beta)), then sets lambda_k the same way from the new
+                   factors.  J never increases in exact arithmetic; a component the data does not support shrinks to zero
+                   and its lambda_k settles at the bound b / c.  b=None sets b by moment matching (`ARD`).  Stop rule: at
+                   every 10th iteration, stop when max_k |lambda_k - its previous value| / its previous value < tol.
+                   Afterwards `ard_lambda` holds lambda (float32, shape (R,), on the factors' device) and `ard_bound`
+                   b / c.  The fit removes no component; keep the relevant ones with, for example,
+                     keep = m.ard_lambda > m.ard_bound * (1 + 1e-3)
+                     W, H = m.W.data[:, keep], m.H.data[:, keep]
+                   NMF, NMFD, NMF2D and NMF3D on every target form and precision above.  ValueError, before any device
+                   work: an `ard` that is not an `ARD`, a, b or phi not finite and > 0, a <= 2 with b=None, alpha != 0,
+                   solver="cd", `group`, `fixed_W`, and a W or H that is not trainable.
         """
         mask = options.pop("mask", None)
         weight = options.pop("weight", None)
         solver = options.pop("solver", "mu")
         fixed_W = options.pop("fixed_W", None)
+        ard = options.pop("ard", None)
         if options:
             raise TypeError(f"fit() got an unexpected keyword argument {next(iter(options))!r}")
+        ard = _checked_ard(ard, self.W, self.H, alpha, solver, group, fixed_W)
         fixed_W = _checked_fixed_w(self.W, fixed_W, group)
         if solver not in ("mu", "cd"):
             raise ValueError(f"solver must be 'mu' or 'cd' (got {solver!r})")
@@ -581,8 +684,15 @@ class BaseComponent(torch.nn.Module):
                         return eng.loss_prefetch_w(beta)
                     return eng.loss(beta)
 
-                step = _update_step(eng, cd, train_w, train_h, beta, gamma, l1_reg, l2_reg)
-                n_iter = _fit_single(step, divergence, max_iter, tol, verbose)
+                if ard is not None:
+                    b, c = _ard_constants(ard, V, W, H, mask, weight)
+                    eng.set_ard(b, c, ard.phi)
+                    n_iter = _fit_ard(eng, beta, gamma, divergence, max_iter, tol, verbose)
+                    self.ard_lambda = eng.ard_state()[0].to(W.device, copy=True)
+                    self.ard_bound = b / c
+                else:
+                    step = _update_step(eng, cd, train_w, train_h, beta, gamma, l1_reg, l2_reg)
+                    n_iter = _fit_single(step, divergence, max_iter, tol, verbose)
                 if hasattr(eng, "check_health"):
                     eng.check_health()
                 self.last_fit_precision = eng.precision_for(beta) if hasattr(eng, "precision_for") else eng.precision
@@ -847,6 +957,39 @@ def _fit_single(step, divergence, max_iter, tol, verbose):
                 if (previous - loss) / loss_init < tol:                                    # nmf.py:405
                     break
                 previous = loss
+    return it
+
+
+def _fit_ard(eng, beta, gamma, divergence, max_iter, tol, verbose):
+    """The loop of an ARD fit on `eng` (ARD registered): each iteration updates W, then H (the engine adds the penalties),
+    then lambda -- one `iterate` call per run of iterations where the engine has it.  At every 10th iteration it stops when
+    the largest relative change of lambda in that iteration is < tol (Tan and Fevotte's criterion), read from the engine
+    there only.  With `verbose`, the progress bar shows the loss sqrt(2 d) of `divergence` at each check.  Returns the last
+    loop index: the iterations run, minus one (`_fit_single`'s convention)."""
+    fused = hasattr(eng, "iterate")
+
+    def step(k):
+        if fused:
+            eng.iterate(k, beta, gamma, 0.0, 0.0)
+            return
+        for _ in range(k):
+            eng.update_w(beta, gamma, 0.0, 0.0)
+            eng.update_h(beta, gamma, 0.0, 0.0)
+            eng.ard_update()
+
+    it = -1
+    with _tqdm(total=max_iter, disable=not verbose) as pbar:
+        while it + 1 < max_iter:
+            k = min(10 - ((it + 1) % 10), max_iter - (it + 1))
+            step(k)
+            it += k
+            if it % 10 == 9:
+                if verbose:
+                    d = divergence(it + 1 < max_iter)
+                    pbar.set_postfix(loss=math.sqrt(2.0 * d) if d >= 0 else float("nan"))
+                pbar.update(10)
+                if eng.ard_change() < tol:
+                    break
     return it
 
 
